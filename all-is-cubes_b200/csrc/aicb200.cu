@@ -675,8 +675,8 @@ aicb_status aicb_ctx_create(int device_id, aicb_ctx **out) {
     CU(cudaSetDevice(device_id));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device_id));
-    if (prop.major < 10)
-        return fail(AICB_ERR_CUDA, "device is not sm_100-class; this library is built for sm_100a only");
+    if (prop.major != 9 || prop.minor != 0)   // sm_90a code loads on compute capability 9.0 only
+        return fail(AICB_ERR_CUDA, "device is not compute capability 9.0; this library is built for sm_90a only");
     aicb_ctx *c = new aicb_ctx();
     c->device = device_id;
     c->num_sms = prop.multiProcessorCount;

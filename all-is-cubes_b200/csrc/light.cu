@@ -19,7 +19,7 @@ using namespace aicb_light;
 // ---------------------------------------------------------------------------------------------
 namespace {
 
-constexpr int CHAIN_WALK_BLOCKS_PER_SM = 6;   // 4 warps, 80 registers, 26 KB of shared memory each (8 blocks of 64 registers: -15 %)
+constexpr int CHAIN_WALK_BLOCKS_PER_SM = 6;   // 4 warps, 80 registers, 26 KB of shared memory each
 
 struct TreeNode {
     int8_t cube[3];
@@ -354,14 +354,14 @@ __global__ void __launch_bounds__(256) k_gather(const LightParams P, uint32_t n_
 }
 
 // 8 CTAs of 4 warps per SM (64 registers; the records requested ahead spill to L1-resident local memory): the walk is
-// latency bound, and 32 resident warps measured +14 % over the 20 that 94 registers allow (6 / 10 CTAs: +2 % / -30 %).
+// latency bound, so 32 resident warps serve it better than the 20 that 94 registers would allow.
 #ifndef AICB_LIGHT_MIN_BLOCKS
 #define AICB_LIGHT_MIN_BLOCKS 8
 #endif
 // How many consecutive list entries (neighbouring cubes) one warp walks for together.  The walk is a chain of dependent
-// loads per node; a lone warp takes ~1250 cycles per node whatever the number of its lanes that take part.  32 cubes
+// loads per node; a lone warp takes as long per node whatever the number of its lanes that take part.  32 cubes
 // share the most node records, but a round of a few ten thousand cubes then occupies a fraction of the resident
-// warps and lasts as long as its slowest warp (a 32-cube union of ~20 K nodes = 14 ms).  Narrower batches make more,
+// warps and lasts as long as its slowest warp (a 32-cube union of ~20 K nodes).  Narrower batches make more,
 // shorter walks: the width is the largest power of two that still yields `P.batches_per_warp` batches per resident warp.
 __device__ __forceinline__ uint32_t batch_width(const LightParams &P, uint32_t n, uint32_t n_warps) {
     if (P.batch_width) return P.batch_width;
@@ -709,8 +709,8 @@ aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, ui
     LightParams P = make_params(s);
     P.epsilon_priority = (uint32_t)epsilon / 2 + 1;
     {
-        // Cubes within 16 priority levels of the round's maximum are relaxed together: 3.5x the throughput of
-        // strict level-by-level rounds (few cubes per round leave the GPU idle) for 8 % more updates; the parity
+        // Cubes within 16 priority levels of the round's maximum are relaxed together: far fewer rounds than strict
+        // level-by-level relaxation (few cubes per round leave the GPU idle) for 8 % more updates; the parity
         // contract (tests/test_gpu_light.py) holds for every band, 0 = one level per round, 255 = all pending cubes.
         const char *e = getenv("AICB_LIGHT_BAND");
         P.priority_band = e ? (uint32_t)atoi(e) : 16u;

@@ -225,9 +225,8 @@ __device__ __forceinline__ unsigned gmask_of_lane() {
 // cubes of a warp in lockstep (see the header).  Warp-collective: every lane calls it; `active` = this lane has a
 // cube.  The lockstep unit is a group of LIGHT_GROUP lanes (default: the whole warp).  A group visits the union of
 // its cubes' node sets; with the whole warp 5 of 32 lanes take part in an average node.  Smaller groups have smaller
-// unions, but the groups of a warp then read different node records and cells in the same instruction, and measured
-// on the 128^3 bench scene that costs more than it saves (groups of 4 / 8 / 16 / 32 lanes: 1.31 / 1.44 / 1.61 / 1.87 M
-// cube updates per second): the walk is bound by its memory transactions, not by issue slots.  MARK as in compute_light.  Per-lane state of the walk: `ld`, the depth of the lane's deepest live frame
+// unions, but the groups of a warp then read different node records and cells in the same instruction, and that costs
+// more than it saves: the walk is bound by its memory transactions, not by issue slots.  MARK as in compute_light.  Per-lane state of the walk: `ld`, the depth of the lane's deepest live frame
 // (-1: only the call of the root is pending; -2: the lane does not walk), and its frames (alpha after traverse(),
 // ray_bundle_weight, the children's weight so far, light_ahead_cache) indexed by depth — the depth is warp-uniform,
 // so these local-memory accesses are coalesced.

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — Mrays/s of the B200-native voxel raytracer on BASELINE.json's workload.
+"""bench.py — Mrays/s of the H100-native voxel raytracer on BASELINE.json's workload.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload c2|c0|c1|c3|c4]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload c2|c0|c1|c3|c4] [--dump-outputs DIR]
 
 Default workload (the one BASELINE.json's metric is quoted on): a "step" is one full frame (1920x1080 primary
 rays) of the 256^3 mixed-transparent Space (BASELINE.json configs[2], SURVEY.md §8(d) C2) traced through the C ABI
@@ -16,6 +16,10 @@ Prints ONE JSON line (rank 0).  `value` = rays / device time with inputs residen
 region); `roofline` = algorithmic bytes / kernel time vs the measured HBM peak;
 `cpu_baseline` = the oracle (CPU restatement of the reference, all host threads) on a bounded
 sample of the same frame.  `--impl reference` times only that CPU path.
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed (the arrays its caller receives)
+as DIR/<name>.npy in float32 / float64, at most DUMP_BYTES in all.  The inputs are seeded, so two builds of the project
+run with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -33,6 +37,7 @@ sys.path.insert(0, os.path.join(ROOT, "all-is-cubes_b200"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 STRIP_ROWS = 16
+DUMP_BYTES = 60_000_000   # --dump-outputs: bytes of .npy files per run
 
 
 def parse_args():
@@ -49,7 +54,31 @@ def parse_args():
                    help="N>1: 'p2p' = the encode kernel stores its strips straight into rank 0's frame over NVLink "
                         "(CUDA IPC mapped peer memory) and an arrival counter in that memory replaces the collective; "
                         "'p2p-barrier' = the same stores + an NCCL barrier; 'nccl' = packed strips + NCCL gather + reassembly")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64)")
+    args = p.parse_args()
+    if args.steps < 1:
+        p.error("--steps must be at least 1")
+    return args
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each (name, array, dtype) as out_dir/<name>.npy, rows along the first axis, in order, within DUMP_BYTES in
+    all.  An array that does not fit whole is replaced by a seeded sample of its rows (the same rows in every run with
+    the same arguments) and the sampled row indices are written as <name>_rows.npy (float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    left = DUMP_BYTES
+    for name, a, dtype in arrays:
+        a = np.asarray(a).astype(dtype)
+        if a.nbytes + 256 > left:
+            per_row = a[0].nbytes + 8
+            k = max(0, min(a.shape[0], (left - 512) // per_row))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=k, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_rows.npy"), rows.astype(np.float64))
+            left -= rows.nbytes + 256
+            a = a[rows]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+        left -= a.nbytes + 256
 
 
 def make_workload(name):
@@ -129,10 +158,8 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    import __graft_entry__ as g
-    g.build_oracle()
     import aicb200
-    import orc
+    import orc   # oracle/liborc.so, built by __graft_entry__.build()
     # This arm never loads libaicb200.so: the scene is numpy, and the camera matrices come from the oracle library
     # (the same host source compiled under orc_* names, oracle/Makefile).
     aicb200.use_camera_library(orc.lib(), "orc_")
@@ -149,16 +176,19 @@ def run_reference(args):
 
     def one_step():
         t0 = time.perf_counter()
-        orc.render_rowlist(oscene, cam, opts, rows, n_threads=threads)
-        return w * len(rows), time.perf_counter() - t0
+        out = orc.render_rowlist(oscene, cam, opts, rows, n_threads=threads)
+        return w * len(rows), time.perf_counter() - t0, out
 
     for _ in range(args.warmup):
         one_step()
     tot_rays, tot_t = 0, 0.0
     for _ in range(args.steps):
-        r, t = one_step()
+        r, t, out = one_step()
         tot_rays += r
         tot_t += t
+    if args.dump_outputs:   # (the rows depend on the calibration, so they are written too)
+        dump_outputs(args.dump_outputs, [("srgb8", out["srgb8"], np.float32),
+                                         ("srgb8_frame_rows", np.asarray(rows), np.float64)])
     value = tot_rays / tot_t / 1e6
     line = {
         "impl": "reference", "metric": "Mrays/s", "value": value, "unit": "Mrays/s", "n_gpus": args.gpus,
@@ -210,12 +240,14 @@ def run_reference_light(args):
         v0 = int(orc.lib().orc_light_node_visits(ol.handle))
         t0 = time.perf_counter()
         ol.set_cubes(cubes, ids)
-        u, _ = ol.evaluate_threaded(1, threads)
+        u, md = ol.evaluate_threaded(1, threads)
         dt = time.perf_counter() - t0
         if step >= args.warmup:
             tot_u += u
             tot_t += dt
             tot_v += int(orc.lib().orc_light_node_visits(ol.handle)) - v0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, [("light_result", [u, md], np.float64)])
     value = tot_u / max(tot_t, 1e-9)
     sample = (f"{n}^3 Space of the same recipe, {n_edits} edits per step (the same edit density), {args.steps} steps, "
               f"{tot_u} cube updates in {tot_t:.1f} s, {threads} threads (the reference's threaded update_light_from_queue: "
@@ -244,10 +276,7 @@ def run_light(args):
         return
     if not torch.cuda.is_available():
         raise SystemExit("bench.py: no CUDA device — libaicb200 has no CPU fallback (use --impl reference for the CPU path)")
-    import __graft_entry__ as g
-    g.build_library()
-    g.build_oracle()
-    import aicb200
+    import aicb200   # built in the tree by __graft_entry__.build(); this script compiles nothing
     from aicb200 import scenes
     n = args.light_n
     space = scenes.config_c4(n)
@@ -271,7 +300,7 @@ def run_light(args):
         u, md = rt.light_edit_and_propagate(cubes, ids, 1)   # H2D: the edit list; blocks until the propagation is done
         st = rt.light_stats()
         img = r.draw() if render else None                   # D2H: the frame
-        return u, st, time.perf_counter() - t0, img
+        return u, md, st, time.perf_counter() - t0, img
 
     for k in range(max(3, args.warmup)):
         step(k, True)
@@ -281,7 +310,7 @@ def run_light(args):
     render_ms = []
     launches = 0
     for k in range(args.steps):
-        u, st, wall, img = step(max(3, args.warmup) + k, True)
+        u, md, st, wall, img = step(max(3, args.warmup) + k, True)
         tot_u += u
         tot_v += st["chart_node_visits"]
         dev_s += st["device_seconds"]
@@ -289,13 +318,17 @@ def run_light(args):
         render_ms.append(img.info.kernel_ms)
         launches += 2 + 7 * st["rounds"] + 4   # edits + tile rebuild; 7 kernels per relaxation round; the 4 kernels of the re-render
     clocks = sampler.stop()
+    if args.dump_outputs:   # the last step's propagation result, its re-rendered frame and the light field it left
+        dump_outputs(args.dump_outputs, [("light_result", [u, md], np.float64),
+                                         ("frame_srgb8", img.data.reshape(-1, 4), np.float32),
+                                         ("light_texels", rt.light_download().reshape(-1, 4), np.float32)])
     value = tot_u / dev_s
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     achieved = light_bytes(tot_u, tot_v) / dev_s / 1e9
     line = {
         "metric": "cube-updates/s", "value": value, "unit": "cube-updates/s", "n_gpus": world, "steps": args.steps,
@@ -309,7 +342,7 @@ def run_light(args):
                    "l2": "every step edits and relaxes different cubes of a 256^3 volume (scene + light + queue: 0.2 GB > L2)",
                    "sharding": "none (light propagation runs on one GPU; SURVEY 8(e) replicas only)"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else PEAK_SOURCE_DATASHEET,
                      "kernel": "k_walk_chains<compute> + k_walk_chains<mark> (chart walk, one warp per cube)", "kernel_ms": 1e3 * dev_s / args.steps,
                      "algorithmic_bytes_per_step": int(light_bytes(tot_u, tot_v) / args.steps),
                      "formula": "50 B per chart node visited + 4 B per cube update (SURVEY 8(d), per-hit term not counted)"},
@@ -333,6 +366,11 @@ def run_light(args):
                                       f"{threads} threads (the reference's threaded update_light_from_queue: batches of 32 "
                                       f"computed in parallel, applied serially)"}
     print(json.dumps(line))
+
+
+# HBM3 bandwidth of the H100 SXM from NVIDIA's data sheet: the roofline denominator when no measured peak is at hand
+H100_HBM_GBS = 3350.0
+PEAK_SOURCE_DATASHEET = "H100 SXM data sheet 3350 GB/s (not measured)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -409,13 +447,7 @@ def run_ours(args):
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
 
-    import __graft_entry__ as g
-    if rank == 0:
-        g.build_library()
-        g.build_oracle()
-    if world > 1:
-        dist.barrier()
-    import aicb200
+    import aicb200   # built in the tree by __graft_entry__.build(); this script compiles nothing
     from aicb200 import abi, scenes
     lib = aicb200.load_library()
 
@@ -431,7 +463,7 @@ def run_ours(args):
     d_out = torch.empty((n_max, 4), dtype=torch.uint8, device="cuda")
     gather_scratch = [torch.empty_like(d_out) for _ in range(world)] if (world > 1 and rank == 0) else None
     frame = torch.empty((h, w, 4), dtype=torch.uint8, device="cuda") if rank == 0 else None
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > the 50 MB L2 of an H100
     # a dedicated (non-default) stream: its handle is what the library launches on, and what the
     # CUDA events below are recorded on
     stream = torch.cuda.Stream()
@@ -532,6 +564,17 @@ def run_ours(args):
     sampler.mark()
     check(lib.aicb_ctx_stage_timing(ctx.handle, 0))   # the timed frames carry no per-kernel event records
     total_ms = timed(device_step, args.steps)
+    if args.dump_outputs:   # the sRGB8 pixels of the last timed frame: this rank's, or with N > 1 the frame rank 0 received
+        if world == 1:
+            dump_outputs(args.dump_outputs, [("srgb8", d_out[:n_local].cpu().numpy(), np.float32)])
+        elif rank == 0:
+            got = torch.empty((h * w, 4), dtype=torch.uint8).pin_memory()
+            if gather_mode == "p2p":
+                peer.read(got, stream.cuda_stream)
+                torch.cuda.synchronize()
+            else:
+                got.copy_(frame.view(h * w, 4))
+            dump_outputs(args.dump_outputs, [("srgb8", got.numpy(), np.float32)])
     # kernel-only duration of the last frame from the library's own events (same stream); a frame that overflowed its
     # hit stream inside the timed region would make this call fail (AICB_ERR_RETRY) and with it the run
     check(lib.aicb_render_finish(rt.handle, C.byref(info)))
@@ -586,20 +629,13 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except OSError:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     # the dominant kernel is the marching kernel: cells / voxels it steps over (2 B each), the palette entry of each
     # surface whose transmittance it applies (32 B) and the descriptor of each block it enters (32 B); the light
     # texels belong to the shading kernel and the pixels to the encode kernel (SURVEY 8(d) counts them per frame)
     march_bytes = 2 * ai.counters[0] + 2 * ai.counters[1] + 32 * ai.counters[2] + 32 * ai.counters[4]
     march_ms = stage_avg_ms[1]
     achieved = march_bytes / (march_ms * 1e-3) / 1e9
-    traffic = None   # DRAM bytes of the marching kernel per launch from the committed ncu --set full capture
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-        if tr.get("workload") == args.workload and world == 1:
-            traffic = int(tr["traffic_bytes_per_launch"])
-    except (OSError, ValueError, KeyError):
-        pass
     frame_achieved = alg_bytes / (kernel_avg_ms * 1e-3) / 1e9
 
     # ---- e2e: host buffers through the public API ------------------------------------------------------
@@ -687,7 +723,7 @@ def run_ours(args):
                        "l2": "256 MiB buffer rewritten between timed steps", "scene_device_bytes": rt.device_bytes,
                        "cubes_traced_per_frame_this_rank": int(ai.cubes_traced)},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)",
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else PEAK_SOURCE_DATASHEET,
                          "kernel": "trace_kernel (marching)", "kernel_ms": march_ms,
                          "algorithmic_bytes_per_launch": int(march_bytes),
                          "frame": {"kernels": ["gen_kernel", "trace_kernel", "shade_kernel", "encode_kernel"],

@@ -52,7 +52,7 @@ unsafe impl Send for B200Context {}
 unsafe impl Sync for B200Context {}
 
 impl B200Context {
-    /// Fails with `AICB_ERR_CUDA` when there is no sm_100 GPU: there is no CPU fallback.
+    /// Fails with `AICB_ERR_CUDA` when there is no H100 (sm_90) GPU: there is no CPU fallback.
     pub fn new(device_id: i32) -> Result<Arc<Self>, B200Error> {
         let mut ctx = core::ptr::null_mut();
         check(unsafe { sys::aicb_ctx_create(device_id, &mut ctx) })?;

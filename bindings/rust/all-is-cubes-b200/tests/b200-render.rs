@@ -1,4 +1,4 @@
-//! The reference's renderer-agnostic image suite (test-renderers) against the B200 path: the third target next to
+//! The reference's renderer-agnostic image suite (test-renderers) against the H100 path: the third target next to
 //! test-renderers/tests/ray-render.rs:6-19 and wgpu-render.rs.  The `-ray` / `-all` expectations apply: same
 //! algorithm, same pixels (RendererId::Raytracer).
 
@@ -28,7 +28,7 @@ impl RendererFactory for Factory {
 async fn main() -> test_renderers_runner::HarnessResult {
     let args = test_renderers_runner::HarnessArgs::parse();
     test_renderers_runner::initialize_logging(&args);
-    let factory = Factory(B200Factory::new().expect("no sm_100 GPU: libaicb200 has no CPU fallback"));
+    let factory = Factory(B200Factory::new().expect("no H100 (sm_90) GPU: libaicb200 has no CPU fallback"));
     test_renderers_runner::harness_main(
         &args,
         RendererId::Raytracer,

@@ -1,5 +1,5 @@
 /*
- * aicb200.h — C ABI of libaicb200.so: the B200-native (sm_100a) replacement for the
+ * aicb200.h — C ABI of libaicb200.so: the H100-native (sm_90a) replacement for the
  * per-pixel voxel raytracer of kpreid/all-is-cubes, behind the reference's own
  * HeadlessRenderer / Camera / SpaceRaytracer surface.
  *
@@ -10,7 +10,7 @@
  * plus aicb_last_error().
  *
  * There is NO CPU fallback.  Every compute entry point fails with AICB_ERR_CUDA when no
- * sm_100-class device is available.
+ * compute capability 9.0 device (H100) is available.
  */
 #ifndef AICB200_H
 #define AICB200_H

@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (compute capability 9.0; run with -m gpu)")
 
 
 @pytest.fixture(scope="session", autouse=True)

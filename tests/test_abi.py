@@ -39,12 +39,12 @@ def test_struct_layouts_match_c_header(tmp_path):
     assert sizes == [C.sizeof(m) for m in mirror]
 
 
-def test_library_was_built_for_sm_100a_only():
+def test_library_was_built_for_sm_90a_only():
     out = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-lelf", aicb200.LIB_PATH], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
     archs = set(re.findall(r"sm_(\d+a?)", out.stdout))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 @pytest.mark.skipif(has_gpu(), reason="this check is for the GPU-less build container")

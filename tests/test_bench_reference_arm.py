@@ -33,3 +33,18 @@ def test_reference_arm_line():
 
 def test_reference_arm_other_ranks_stay_silent():
     assert run({"RANK": "1", "WORLD_SIZE": "2", "LOCAL_RANK": "1"}) == ""
+
+
+def test_reference_arm_dump_outputs(tmp_path):
+    """--dump-outputs writes the last timed step's pixels as float32 .npy files, with the frame rows they belong to."""
+    import numpy as np
+    out = tmp_path / "out"
+    run_args = [sys.executable, os.path.join(ROOT, "bench.py"), "--impl", "reference", "--workload", "c0", "--steps", "1",
+                "--warmup", "0", "--cpu-seconds", "1", "--dump-outputs", str(out)]
+    r = subprocess.run(run_args, capture_output=True, text=True, timeout=300)
+    assert r.returncode == 0, r.stderr[-2000:]
+    srgb, rows = np.load(out / "srgb8.npy"), np.load(out / "srgb8_frame_rows.npy")
+    assert srgb.dtype == np.float32 and rows.dtype == np.float64
+    assert srgb.shape == (256 * len(rows), 4) and srgb.min() >= 0 and srgb.max() <= 255
+    assert (srgb[:, 3] == 255).all()
+    assert sum(f.stat().st_size for f in out.iterdir()) <= 64 * 10**6

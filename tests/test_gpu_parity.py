@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on a B200): the CUDA path, called through the C ABI,
+"""GPU parity tests (run with `-m gpu` on an H100): the CUDA path, called through the C ABI,
 against the oracle on identical Space / Camera / options.
 
 Bar (BASELINE.json north_star: +-1 ULP per f32 channel, hit indices bit-exact).  What is asserted here is
@@ -732,3 +732,28 @@ def test_bounce_voxel_blocks():
     compare(gpu, ref, "voxel blocks")
     same_srgb8(img, ref)
     assert gpu["info"].cubes_traced == ref["cubes_traced"]
+
+
+def test_bench_dump_outputs_is_the_timed_frame(tmp_path):
+    """bench.py --dump-outputs writes the sRGB8 frame of the last timed step: the frame a plain render of the same
+    workload gives, and the same in two runs."""
+    import subprocess
+    import sys
+    root = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
+    sys.path.insert(0, root)
+    import bench
+    outs = []
+    for k in range(2):
+        out = tmp_path / f"run{k}"
+        r = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--workload", "c0", "--steps", str(2 + k),
+                            "--warmup", "1", "--cpu-seconds", "0.5", "--dump-outputs", str(out)],
+                           capture_output=True, text=True, timeout=600)
+        assert r.returncode == 0, r.stderr[-2000:]
+        assert json.loads(r.stdout.strip().splitlines()[-1])["steps"] == 2 + k
+        outs.append(np.load(out / "srgb8.npy"))
+    assert outs[0].dtype == np.float32
+    assert np.array_equal(outs[0], outs[1])
+    space, opts, w, h, _ = bench.make_workload("c0")
+    r = RtRenderer(scenes.standard_camera(space, opts, w, h))
+    r.update(space)
+    assert np.array_equal(outs[0], r.draw().data.reshape(-1, 4).astype(np.float32))
