@@ -549,7 +549,9 @@ class RenderInfo:
     counters: tuple
     kernel_ms: float
     flaws: int
-    stage_ms: tuple = (0.0, 0.0, 0.0, 0.0)   # ray generation, marching, shading, encode (first chunk)
+    # first chunk: ray generation, marching, shading, encode; where shading and encode ran as one kernel
+    # (resolve_kernel: None / Flat lighting, most frames) [2] is its time and [3] is 0
+    stage_ms: tuple = (0.0, 0.0, 0.0, 0.0)
 
     @staticmethod
     def from_abi(i: abi.RenderInfo) -> "RenderInfo":

@@ -421,15 +421,24 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     sc->pending_rays = pixels * (P.antialias ? 4 : 1);
     sc->pending_out_bytes_per_pixel = out.srgb8 ? 4 : (out.rgba16f ? 8 : 16);
 
-    // ---- the four kernels of a frame, chunked so the per-frame streams stay bounded ---------------------------
+    // ---- the kernels of a frame, chunked so the per-frame streams stay bounded ----------------------------------
     P.n_samples = P.antialias ? 4 : 1;
+    // gen -> march -> resolve (shading and encode in one kernel) with None / Flat lighting, unless the context's last
+    // frame met 3/4 of a visible surface per ray or more; otherwise gen -> march -> shade -> encode.  resolve_kernel
+    // saves the ShadedHit round trip, the scan of the dead slots and a kernel drain, but its warps also list and
+    // composite, so fewer of them shade at once: where a warp has several 32-slot shading rounds the separate
+    // shade_kernel is faster.  Measured on one H100 SXM at 700 W: the opaque bench frames (C0, C1, C3: 0.3-0.5 visible
+    // surfaces per ray) 7-17 % faster fused; the C2 frame (1.0 per ray) 7 % slower with None and 11 % with Flat
+    // lighting, and 1.8x slower in shade + encode with interpolated lighting, which therefore never takes this path.
+    const bool fused = (opt->lighting_display == AICB_LIGHT_NONE || opt->lighting_display == AICB_LIGHT_FLAT) &&
+                       !ctx->deep_frames;
     const uint64_t total_tasks = (uint64_t)P.n_tasks * P.n_samples;
     // Tasks per chunk (a multiple of 32 * n_samples): at most 4 M (0.6 GB of ray records); fewer when the hit stream
     // has been enlarged after an overflow, so that the per-frame streams stay within ~8 GB however deep the scene is.
     uint64_t CHUNK = (uint64_t)4 << 20;
     {
         const uint64_t per_task = sizeof(RayRecord) + sizeof(TaskOut) + 4 * N_BINS +
-                                  (uint64_t)ctx->hits_per_task * (sizeof(HitRecord) + sizeof(ShadedHit));
+                                  (uint64_t)ctx->hits_per_task * (sizeof(HitRecord) + (fused ? 0 : sizeof(ShadedHit)));
         uint64_t fit = ((uint64_t)8 << 30) / per_task;
         if (fit < (1u << 17)) fit = 1u << 17;
         if (fit < CHUNK) CHUNK = fit & ~(uint64_t)127;
@@ -447,15 +456,18 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         P.hit_capacity = (uint32_t)cap;
         st = ensure(&ctx->d_hits, &ctx->d_hits_bytes, cap * sizeof(HitRecord) + 64);
         if (st != AICB_OK) return st;
-        st = ensure(&ctx->d_contrib, &ctx->d_contrib_bytes, cap * sizeof(ShadedHit) + 64);
-        if (st != AICB_OK) return st;
+        if (!fused) {
+            st = ensure(&ctx->d_contrib, &ctx->d_contrib_bytes, cap * sizeof(ShadedHit) + 64);
+            if (st != AICB_OK) return st;
+        }
         st = ensure(&ctx->d_bin_list, &ctx->d_bin_list_bytes, (size_t)N_BINS * chunk_cap * 4 + 64);
         if (st != AICB_OK) return st;
     }
     P.ray_records = (RayRecord *)ctx->d_rays;
     P.task_out = (TaskOut *)ctx->d_task_cb;
     P.hits = (HitRecord *)ctx->d_hits;
-    P.shaded = (ShadedHit *)ctx->d_contrib;
+    P.shaded = fused ? nullptr : (ShadedHit *)ctx->d_contrib;
+    sc->pending_fused = fused;
     P.hit_counter = ctx->d_tile_counter + 1;
     P.bin_count = ctx->d_tile_counter + 4;
     P.bin_list = (uint32_t *)ctx->d_bin_list;
@@ -550,13 +562,23 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             CU(launch_after(overlap, k, (unsigned)grid, WARPS_PER_BLOCK * 32, stream, P, n));
             P.debug_warp_times = nullptr;
             if (stage) cudaEventRecord(ctx->ev_k[2], stream);
-            switch (lc) {
-                case LC_NONE: CU(launch_after(overlap, shade_kernel<LC_NONE>, ctx->num_sms * 8, 128, stream, P)); break;
-                case LC_FLAT: CU(launch_after(overlap, shade_kernel<LC_FLAT>, ctx->num_sms * 8, 128, stream, P)); break;
-                case LC_BOUNCE: CU(launch_after(overlap, shade_kernel<LC_BOUNCE>, ctx->num_sms * 8, 128, stream, P)); break;
-                default: CU(launch_after(overlap, shade_kernel<LC_INTERP>, ctx->num_sms * 8, 128, stream, P)); break;
-            }
-            if (bounce) {
+            if (fused) {
+                const unsigned rb = (n + 127) / 128;   // one warp per 32 tasks
+                if (lc == LC_NONE) CU(launch_after(overlap, resolve_kernel<LC_NONE>, rb, 128, stream, P, n));
+                else CU(launch_after(overlap, resolve_kernel<LC_FLAT>, rb, 128, stream, P, n));
+                if (stage) cudaEventRecord(ctx->ev_k[3], stream);
+            } else if (!bounce) {
+                switch (lc) {
+                    case LC_NONE: CU(launch_after(overlap, shade_kernel<LC_NONE>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
+                    case LC_FLAT: CU(launch_after(overlap, shade_kernel<LC_FLAT>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
+                    default: CU(launch_after(overlap, shade_kernel<LC_INTERP>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
+                }
+                if (stage) cudaEventRecord(ctx->ev_k[3], stream);
+                const uint32_t n_pixels = n / P.n_samples;
+                CU(launch_after(overlap, encode_kernel, (n_pixels + 127) / 128, 128, stream, P, n));
+                if (stage) cudaEventRecord(ctx->ev_k[4], stream);
+            } else {
+                shade_kernel<LC_BOUNCE><<<ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, 0, stream>>>(P);
                 const unsigned tb = (n + 127) / 128;
                 bounce_select_kernel<<<tb, 128, 0, stream>>>(P, n);
                 Q.n_rays = n;
@@ -568,15 +590,15 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                     bounce_gen_kernel<<<tb, 128, 0, stream>>>(P, n);
                     gen_kernel<<<tb, 128, 0, stream>>>(Q, n);
                     k<<<(unsigned)grid, WARPS_PER_BLOCK * 32, 0, stream>>>(Q, n);
-                    shade_kernel<LC_FLAT><<<ctx->num_sms * 8, 128, 0, stream>>>(Q);
+                    shade_kernel<LC_FLAT><<<ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, 0, stream>>>(Q);
                     encode_kernel<<<tb, 128, 0, stream>>>(Q, n);
                 }
                 bounce_resolve_kernel<<<tb, 128, 0, stream>>>(P, n);
+                if (stage) cudaEventRecord(ctx->ev_k[3], stream);
+                const uint32_t n_pixels = n / P.n_samples;
+                encode_kernel<<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
+                if (stage) cudaEventRecord(ctx->ev_k[4], stream);
             }
-            if (stage) cudaEventRecord(ctx->ev_k[3], stream);
-            const uint32_t n_pixels = n / P.n_samples;
-            CU(launch_after(overlap, encode_kernel, (n_pixels + 127) / 128, 128, stream, P, n));
-            if (stage) cudaEventRecord(ctx->ev_k[4], stream);
         }
         CU(cudaGetLastError());
     }
@@ -595,7 +617,7 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
     sc->pending = false;
     if (ctx->profile_kernels && sc->pending_rays) {  // AICB_PROFILE_KERNELS=1: per-kernel times of the first chunk
         float t[4] = {0, 0, 0, 0};
-        for (int i = 0; i < 4; i++) cudaEventElapsedTime(&t[i], ctx->ev_k[i], ctx->ev_k[i + 1]);
+        for (int i = 0; i < (sc->pending_fused ? 3 : 4); i++) cudaEventElapsedTime(&t[i], ctx->ev_k[i], ctx->ev_k[i + 1]);
         if (ctx->d_debug && ctx->debug_warps) {
             std::vector<unsigned long long> w(4 * (size_t)ctx->debug_warps);
             cudaMemcpy(w.data(), ctx->d_debug, w.size() * 8, cudaMemcpyDeviceToHost);
@@ -608,9 +630,14 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
             fprintf(stderr, "[aicb200] march warps %u: end times ms min %.3f p10 %.3f p50 %.3f p90 %.3f p99 %.3f max %.3f; passes/warp %.0f rays %llu\n",
                     ctx->debug_warps, q(0), q(0.1), q(0.5), q(0.9), q(0.99), q(1.0), (double)passes / ctx->debug_warps, rays);
         }
-        fprintf(stderr, "[aicb200] gen %.3f ms  march %.3f ms  shade %.3f ms  encode %.3f ms  (hits %llu)\n", t[0], t[1], t[2],
-                t[3], c[3]);
+        if (sc->pending_fused)
+            fprintf(stderr, "[aicb200] gen %.3f ms  march %.3f ms  resolve (shade + encode) %.3f ms  (hits %llu)\n", t[0], t[1],
+                    t[2], c[3]);
+        else
+            fprintf(stderr, "[aicb200] gen %.3f ms  march %.3f ms  shade %.3f ms  encode %.3f ms  (hits %llu)\n", t[0], t[1], t[2],
+                    t[3], c[3]);
     }
+    if (sc->pending_rays) ctx->deep_frames = c[3] * 4 >= sc->pending_rays * 3;   // visible surfaces per ray >= 3/4
     if (c[7]) {  // the hit stream of some chunk overflowed: the frame is incomplete
         if (ctx->hits_per_task >= 2048)
             return fail(AICB_ERR_OOM, "hit stream overflowed at its largest capacity (2048 hit records per ray)");
@@ -637,8 +664,9 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
         float ms = 0.0f;
         CU(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
         info->kernel_ms = ms;
-        if (sc->pending_rays && ctx->stage_timing)
-            for (int i = 0; i < 4; i++) cudaEventElapsedTime(&info->stage_ms[i], ctx->ev_k[i], ctx->ev_k[i + 1]);
+        if (sc->pending_rays && ctx->stage_timing)   // a fused frame: [2] is resolve_kernel, [3] stays 0
+            for (int i = 0; i < (sc->pending_fused ? 3 : 4); i++)
+                cudaEventElapsedTime(&info->stage_ms[i], ctx->ev_k[i], ctx->ev_k[i + 1]);
         info->cubes_traced = c[0];
         info->rays = sc->pending_rays;
         for (int i = 0; i < 5; i++) info->counters[i] = c[1 + i];
@@ -1228,7 +1256,7 @@ aicb_status aicb_render_srgb8_device_frame(aicb_scene *s, const aicb_camera *cam
 // ---- full-frame buffers shared between ranks (CUDA IPC) ------------------------------------------
 // Behind the pixels of a shared frame sits a small control block in the same allocation (so it travels with the IPC
 // handle): two monotonic counters that replace the collective of the delivery step.
-//   arrived   += 1 by every rank once its strips of a frame are stored (aicb_frame_signal, after the rank's encode_kernel
+//   arrived   += 1 by every rank once its strips of a frame are stored (aicb_frame_signal, after the rank's last kernel
 //                in stream order; system-scope fence + atomic, so the pixels are visible before the count);
 //   consumed  := k by the owner once it is through with frame k (aicb_frame_release);
 // aicb_frame_wait_arrived / aicb_frame_wait_consumed are one-thread kernels that spin on them in stream order.  A wait

@@ -2,7 +2,7 @@
 // not Python (the reference's Rust process owns all its threads; a Rust `impl HeadlessRenderer` cannot call
 // torch.distributed).  An aicb_group is one aicb_ctx per device; an aicb_group_scene is the scene replicated on each of
 // them.  aicb_group_render_srgb8 cuts the frame into interleaved 16-row strips (strip s -> device s mod n), every
-// device's encode_kernel stores its pixels straight into device 0's frame over NVLink (peer access), device 0's stream
+// device's last kernel stores its pixels straight into device 0's frame over NVLink (peer access), device 0's stream
 // waits for the others' completion events and copies the frame to the caller: compute and delivery are one kernel
 // chain per device, there is no collective and no host thread per GPU.
 // Replaces the Rayon rows x pixels dispatch of trace_scene_to_image_impl (renderer.rs:516-556) across devices.

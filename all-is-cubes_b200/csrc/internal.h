@@ -43,14 +43,14 @@ struct aicb_ctx {
     size_t d_out_bytes = 0;
     void *d_aux = nullptr;
     size_t d_aux_bytes = 0;
-    // per-task streams between gen -> trace -> encode (trace_kernel.cuh)
+    // per-task streams between gen -> trace -> resolve, or -> shade -> encode (trace_kernel.cuh)
     void *d_rays = nullptr;
     size_t d_rays_bytes = 0;
     void *d_task_cb = nullptr;   // TaskOut per task
     size_t d_task_cb_bytes = 0;
-    void *d_hits = nullptr;      // HitRecord stream (march -> shade -> encode)
+    void *d_hits = nullptr;      // HitRecord stream (march -> resolve, or march -> shade -> encode)
     size_t d_hits_bytes = 0;
-    void *d_contrib = nullptr;   // ShadedHit per hit (shade -> encode)
+    void *d_contrib = nullptr;   // ShadedHit per hit (shade -> encode): not used by frames that run resolve_kernel
     size_t d_contrib_bytes = 0;
     void *d_bin_list = nullptr;  // task ids of the rays that enter the space, per chord-length bin
     size_t d_bin_list_bytes = 0;
@@ -61,6 +61,7 @@ struct aicb_ctx {
     size_t d_bounce_bytes = 0;
     uint32_t hits_per_task = 8;  // capacity of the hit stream per ray; raised x4 when a frame overflows it,
     uint32_t shallow_frames = 0; //   lowered again after 16 frames in a row that needed a small fraction of it
+    bool deep_frames = false;    // the last frame met >= 3/4 visible surfaces per ray: no resolve_kernel (launch_trace)
     void *h_stage = nullptr;     // pinned staging of frames whose destination is pageable host memory
     size_t h_stage_bytes = 0;
     // the frame whose per-frame scratch (streams, counters, events) is in use
@@ -101,6 +102,7 @@ struct aicb_scene {
     uint64_t pending_rays = 0;
     uint64_t pending_pixels = 0;
     uint32_t pending_out_bytes_per_pixel = 0;
+    bool pending_fused = false;    // shading and encode ran as one kernel (resolve_kernel)
     // ---- light propagation state (light.cu) ----
     std::vector<uint16_t> h_ids;            // host mirror of Space::contents (edits are applied in order on the host)
     std::vector<uint32_t> h_block_light;    // per block: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission

@@ -1,7 +1,7 @@
 // trace_kernel.cuh — the device code of libaicb200's raytracer: a from-scratch sm_90a implementation of
 // all-is-cubes' SpaceRaytracer::trace_ray (sr.rs:135-238) and its pixel dispatch (renderer.rs:424-451, 516-556).
 //
-// Design (GPU-first, not a translation).  One frame = four kernels on one stream:
+// Design (GPU-first, not a translation).  One frame = three or four kernels on one stream:
 //  * gen_kernel (one thread per ray, convergent): pixel -> world ray, Raycaster::new().within(space bounds); rays that
 //    miss the space are finished here, the others are listed by chord length (longest first);
 //  * trace_kernel (persistent warps): every lane owns one ray at a time and takes the next one from the list when it
@@ -13,13 +13,16 @@
 //    warp serves parked lanes together once enough of them wait.  The kernel evaluates no colour: of the transmittance
 //    it keeps only an upper bound, in the log domain (one multiply-add per span), to know when the ray is certainly
 //    opaque;
-//  * shade_kernel (one thread per hit record, convergent): cube / voxel coordinates and the intersection point from
-//    the recorded caster state, apply_transmittance (f64 pow), fog (f64 exp), the invisibility test and
+//  * shading (shade_hit), one thread per hit record, convergent: cube / voxel coordinates and the intersection point
+//    from the recorded caster state, apply_transmittance (f64 pow), fog (f64 exp), the invisibility test and
 //    compute_illumination;
-//  * encode_kernel (one thread per pixel): the exact transmittance chain in ray order, the opacity cut, sky, tone
-//    mapping, sRGB8.
+//  * compositing, one thread per ray: the exact transmittance chain in ray order, the opacity cut; then per pixel the
+//    sky, tone mapping, sRGB8 (finish_pixel).
+//  With None / Flat lighting both happen in resolve_kernel (one warp per 8x4 tile of rays, the shaded hits in shared
+//  memory) unless the previous frame was deep (launch_trace); otherwise in shade_kernel, then encode_kernel, through a
+//  ShadedHit stream.
 //  The kernels of a frame follow each other with programmatic dependent launch (grid_dependency_sync).  A frame with
-//  LightingOption::Bounce runs the same kernels a second time per sample for the secondary rays (see the bounce_*
+//  LightingOption::Bounce runs shade + encode a second time per sample for the secondary rays (see the bounce_*
 //  kernels).
 //  The two-level grid (Space cubes -> block id; block -> N^3 brick of palette indices) is walked by ONE unified DDA;
 //  entering a recursive block pushes the outer state (shared memory) and re-initialises the same DDA on the brick.
@@ -95,12 +98,12 @@ struct __align__(16) RayRecord {
 };
 static_assert(sizeof(RayRecord) == 144, "RayRecord must be 144 bytes");
 
-// One surface of one ray, emitted by the marching kernel and lit by the shade kernel: 64 bytes = 4 x 16-byte stores.
+// One surface of one ray, emitted by the marching kernel and lit by shade_hit: 64 bytes = 4 x 16-byte stores.
 // It is the caster's state at the surface, not a derived geometry: cube / voxel coordinates, the intersection point
-// (raycast.rs:409-439) and the palette entry are recovered from it by shade_kernel, convergently.  The marcher
+// (raycast.rs:409-439) and the palette entry are recovered from it by shade_hit, convergently.  The marcher
 // evaluates no colour or transmittance: apply_transmittance (f64 pow), the fog amount (f64 exp), the invisibility
-// test and the illumination all happen in shade_kernel, and the transmittance chain of the ray is multiplied up in
-// order by encode_kernel.
+// test and the illumination all happen in shade_hit, and the transmittance chain of the ray is multiplied up in
+// order by resolve_kernel or encode_kernel.
 struct __align__(16) HitRecord {
     double tmx, tmy, tmz;   // State::t_max of the level the surface is on (unscaled)
     double last_t;          // State::last_t_distance of that level: Hit::t_distance = last_t / resolution
@@ -111,14 +114,14 @@ struct __align__(16) HitRecord {
     float thickness;        // Volumetric: length of the span inside the surface's material (world units), written when
                             // the span is closed; Surface / Threshold: 0; < 0: the surface was never shaded
     uint32_t steps;         // the ray's step counter when the surface was shaded (the reference stops at the first
-                            // counted step after the hit that brings the transmittance under 1/256; encode_kernel
+                            // counted step after the hit that brings the transmittance under 1/256; compositing
                             // needs the counter to restore that when the marcher's bound let the ray run on)
     uint32_t task;          // the ray: index of its RayRecord in the chunk
     uint32_t next;          // in the last slot of a chunk: where the ray's hits continue (the first slot of another chunk)
 };
 static_assert(sizeof(HitRecord) == 64, "HitRecord must be 64 bytes");
 
-// What shade_kernel leaves per hit for encode_kernel: one 32-byte sector.
+// What shading yields per hit; shade_kernel leaves it in global memory for encode_kernel (one 32-byte sector).
 struct __align__(32) ShadedHit {
     float r, g, b;       // outgoing light of the surface
     float factor;        // what it multiplies the ray's transmittance by (< 0: surface invisible / never shaded, skip)
@@ -128,7 +131,7 @@ struct __align__(32) ShadedHit {
 };
 static_assert(sizeof(ShadedHit) == 32, "ShadedHit must be 32 bytes");
 
-// What the marching kernel hands to the encode kernel per ray (16 bytes).
+// What the marching kernel hands to the resolve / encode kernel per ray (16 bytes).
 struct __align__(16) TaskOut {
     uint32_t first_hit;  // index of the first HitRecord or 0xffffffff
     uint32_t steps;      // steps counted by the marcher (>= the reference's; see HitRecord::steps)
@@ -163,11 +166,11 @@ struct TraceParams {
     uint32_t out_full_frame;    // 1: outputs are indexed by framebuffer position (full-frame buffer, possibly peer memory)
     uint32_t n_samples;         // rays per pixel task: 4 with AntialiasingOption::Always, else 1
     uint32_t task_base;         // first task of the chunk being processed (tasks = pixel_task * n_samples + sample)
-    // per-task streams between the three kernels of a frame (HBM)
+    // per-task streams between the kernels of a frame (HBM)
     RayRecord *ray_records;     // gen -> march
-    TaskOut *task_out;          // march -> encode
-    HitRecord *hits;            // march -> shade
-    ShadedHit *shaded;          // shade -> encode
+    TaskOut *task_out;          // march -> resolve / encode
+    HitRecord *hits;            // march -> resolve / shade
+    ShadedHit *shaded;          // shade -> encode (nullptr in a frame that runs resolve_kernel)
     unsigned int *hit_counter;  // hit slots handed out in this chunk (in chunks of HIT_CHUNK per lane)
     uint32_t *bin_list;         // gen -> march: task ids of the rays that enter the space, binned by chord length
     unsigned int *bin_count;    // [N_BINS] entries of each bin
@@ -959,9 +962,9 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     int face = 0;                        // Face7 through which the current cube was entered
     uint32_t sbits = 0;                  // (sx+1) | (sy+1)<<2 | (sz+1)<<4
     bool valid = false, inner = false, need_advance = false, have_pending = false;
-    // Upper bound of log2 of the ColorBuf transmittance (never below the exact value the encode kernel computes).
+    // Upper bound of log2 of the ColorBuf transmittance (never below the exact value the compositing computes).
     // Once it is under -8 the ray is certainly finished (sr.rs:648-652); in the rare case that only the exact value is
-    // under 1/256 the marcher runs on and the encode kernel cuts the ray's hits and steps back (HitRecord::steps).
+    // under 1/256 the marcher runs on and the compositing cuts the ray's hits and steps back (HitRecord::steps).
     // count_step_should_stop is then ONE compare per step: steps > step_limit, with step_limit = 1000 (sr.rs:639-643)
     // until the bound says "opaque", 0 from then on.
     float L = 0.0f;
@@ -972,7 +975,7 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     AuxState<AUX> aux{};
     bool list_exhausted = false;         // warp-uniform: the ray list has run out (tail of the frame)
 
-    // log-domain bound of one transmittance factor.  Exact factor (shade_kernel): 1 - clamp(1 - (f32)pow(u, th)) with
+    // log-domain bound of one transmittance factor.  Exact factor (shade_hit): 1 - clamp(1 - (f32)pow(u, th)) with
     // u = 1 - alpha, i.e. <= u^th (1 + 2^-23) + 2^-24; with u^th >= 2^-8.5 that is <= u^th * 2^(3.3e-5).  l2a >= log2(u)
     // (host, rounded up); the f32 product and sum add < 2e-6.  A factor under 2^-8.5 makes the ray opaque by itself.
     auto bound_factor = [&](float p) {
@@ -1131,7 +1134,7 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
 
     for (;;) {
         dbg_passes++;
-        // =========================== FINALIZE: hand the ray's result to the encode kernel ================
+        // =========================== FINALIZE: hand the ray's result to the compositing ==================
         if (st == ST_DONE) {
             dbg_rays++;
             TaskOut o;
@@ -1365,12 +1368,13 @@ AICB_DEV void decode_hit(const DeviceScene &S, const HitRecord &h, HitGeom &g) {
     g.pal = h.pal;
 }
 
-// One hit record -> one ShadedHit.  `illum_override` (LC_BOUNCE only): the illumination gathered by the hit's secondary
-// rays; without it a Bounce frame lights the surface like Flat (surface.rs:171-176) and marks fully opaque surfaces
-// (the only ones the bounce RNG is handed to, surface.rs:85-88) for bounce_select_kernel.
+// One hit record -> its ShadedHit (returned, not stored: resolve_kernel keeps it in shared memory, shade_kernel and
+// bounce_resolve_kernel store it).  `illum_override` (LC_BOUNCE only): the illumination gathered by the hit's
+// secondary rays; without it a Bounce frame lights the surface like Flat (surface.rs:171-176) and marks fully opaque
+// surfaces (the only ones the bounce RNG is handed to, surface.rs:85-88) for bounce_select_kernel.
 template <int LC>
-AICB_DEV void shade_hit(const TraceParams &P, const float *s_lut, const uint32_t i, const float *illum_override,
-                        unsigned long long &texels) {
+AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uint32_t i, const float *illum_override,
+                             unsigned long long &texels) {
     const DeviceScene &S = P.scene;
     const bool volumetric = P.transparency == AICB_TRANSPARENCY_VOLUMETRIC;
     const bool have_fog = (P.fog != AICB_FOG_NONE) && P.include_sky;
@@ -1401,7 +1405,7 @@ AICB_DEV void shade_hit(const TraceParams &P, const float *s_lut, const uint32_t
     out.next = h.next;
     out.steps = h.steps;
     out._pad[0] = out._pad[1] = 0;
-    uint4 *outp = reinterpret_cast<uint4 *>(P.shaded + i);
+    if (h.thickness < 0.0f) return out;   // never shaded (its ray stopped before the span closed): skipped
     HitGeom g;
     decode_hit(S, h, g);
     float ca = col.w;
@@ -1430,11 +1434,7 @@ AICB_DEV void shade_hit(const TraceParams &P, const float *s_lut, const uint32_t
     if (P.transparency == AICB_TRANSPARENCY_THRESHOLD) {  // limit_alpha (graphics_options.rs:496-507)
         if (ca > P.threshold) { ca = 1.0f; } else { zeroed = true; ca = 0.0f; }
     }
-    if (ca == 0.0f && er == 0.0f && eg == 0.0f && eb == 0.0f) {   // nothing to see: the ray is not touched
-        outp[0] = reinterpret_cast<const uint4 *>(&out)[0];
-        outp[1] = reinterpret_cast<const uint4 *>(&out)[1];
-        return;
-    }
+    if (ca == 0.0f && er == 0.0f && eg == 0.0f && eb == 0.0f) return out;   // nothing to see: the ray is not touched
     const double t_scale = recip_pow2(g.res);
     float tr = 1.0f - ca;
     float fa = -1.0f;
@@ -1502,12 +1502,18 @@ AICB_DEV void shade_hit(const TraceParams &P, const float *s_lut, const uint32_t
         ob = ps_mul(ob, comp) + ps_mul(S.sky_colors[k][2], fa);
     }
     out.r = orr; out.g = og; out.b = ob; out.factor = tr;
-    outp[0] = reinterpret_cast<const uint4 *>(&out)[0];
-    outp[1] = reinterpret_cast<const uint4 *>(&out)[1];
+    return out;
+}
+
+AICB_DEV void store_shaded(const TraceParams &P, const uint32_t i, const ShadedHit &s) {
+    uint4 *outp = reinterpret_cast<uint4 *>(P.shaded + i);
+    outp[0] = reinterpret_cast<const uint4 *>(&s)[0];
+    outp[1] = reinterpret_cast<const uint4 *>(&s)[1];
 }
 
 // ======================================================================================================
-// Kernel 3 — shading: one thread per HitRecord, fully convergent.  Everything about a surface that does not depend
+// Kernel 3 of a frame that does not run resolve_kernel — shading: one thread per HitRecord, fully convergent, into
+// the ShadedHit stream.  Everything about a surface that does not depend
 // on the surfaces in front of it: its position (cube, voxel, face) and intersection point (raycast.rs:409-439,
 // surface.rs:406-407) from the recorded caster state, apply_transmittance (sr.rs:720-740,
 // raytracer_components.rs:215-258; Volumetric only), limit_alpha (graphics_options.rs:496-507), the invisibility
@@ -1516,8 +1522,12 @@ AICB_DEV void shade_hit(const TraceParams &P, const float *s_lut, const uint32_t
 // factor by which the surface multiplies the ray's transmittance (add_color_internal,
 // raytracer_components.rs:87-92), or "skip".
 // ======================================================================================================
+// One wave of persistent blocks: 6 per SM (80 registers, no spills).  Measured on the C2 bench frame (H100 SXM, 400 W
+// power limit): 0.236 ms against 0.27 ms for 8 blocks per SM at 90 registers, of which 5 were resident and 3 ran as a
+// second wave.
+constexpr int SHADE_BLOCKS_PER_SM = 6;
 template <int LC>
-__global__ void __launch_bounds__(128) shade_kernel(const __grid_constant__ TraceParams P) {
+__global__ void __launch_bounds__(128, SHADE_BLOCKS_PER_SM) shade_kernel(const __grid_constant__ TraceParams P) {
     __shared__ float s_lut[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lut[i] = P.scene.tables[i];
     grid_dependency_sync();
@@ -1526,7 +1536,7 @@ __global__ void __launch_bounds__(128) shade_kernel(const __grid_constant__ Trac
     uint32_t n = *P.hit_counter;
     if (n > P.hit_capacity) n = P.hit_capacity;
     unsigned long long texels = 0;
-    auto shade_one = [&](const uint32_t i) { shade_hit<LC>(P, s_lut, i, nullptr, texels); };
+    auto shade_one = [&](const uint32_t i) { store_shaded(P, i, shade_hit<LC>(P, s_lut, i, nullptr, texels)); };
 
     // The hit stream holds slots that were never shaded (the unused tail of each lane's last chunk, surfaces whose ray
     // stopped before their span closed: a quarter of the slots of the bench frame).  Each warp scans its slots 32 at
@@ -1550,9 +1560,7 @@ __global__ void __launch_bounds__(128) shade_kernel(const __grid_constant__ Trac
                     out.next = P.hits[slot].next;
                     out.steps = 0;
                     out._pad[0] = out._pad[1] = 0;
-                    uint4 *outp = reinterpret_cast<uint4 *>(P.shaded + slot);
-                    outp[0] = reinterpret_cast<const uint4 *>(&out)[0];
-                    outp[1] = reinterpret_cast<const uint4 *>(&out)[1];
+                    store_shaded(P, slot, out);
                 }
             }
             const unsigned m = __ballot_sync(0xffffffffu, live);
@@ -1734,177 +1742,146 @@ static __global__ void __launch_bounds__(128) bounce_resolve_kernel(const __grid
     const float recip = ps_clamped(1.0f / (float)P.bounce_samples);   // Rgb * f32 clamps the scalar (color.rs:912-927)
     const float illum[3] = {ps_mul(sum.x, recip), ps_mul(sum.y, recip), ps_mul(sum.z, recip)};
     unsigned long long texels = 0;
-    shade_hit<LC_BOUNCE>(P, s_lut, req, illum, texels);
+    store_shaded(P, req, shade_hit<LC_BOUNCE>(P, s_lut, req, illum, texels));
 }
 
 // ======================================================================================================
-// Kernel 4 — per pixel: the ray's transmittance chain and add_color_internal over its hits in order
-// (raytracer_components.rs:87-92), count_step_should_stop's opacity cut (sr.rs:648-652) applied to the chain,
-// finish (sr.rs:658-693: the sky; debug_pixel_cost), ColorBuf::mean of the 4 sub-samples
-// (raytracer_components.rs:97-102), the encoder of draw_rgba (renderer.rs:287-291) and the stores.
+// Per pixel, once the transmittance chain of each of its samples is known: finish (sr.rs:658-693: the sky;
+// debug_pixel_cost), ColorBuf::mean of the 4 sub-samples in sample order (raytracer_components.rs:97-102), the
+// encoder of draw_rgba (renderer.rs:287-291) and the stores.  `chain(k, o, lr, lg, lb, T, steps, sample_first)`
+// yields sample k's accumulator after its hits (add_color_internal, raytracer_components.rs:87-92, with
+// count_step_should_stop's opacity cut, sr.rs:648-652), its step count and the slot of its first visible surface.
+// Returns the pixel's cubes_traced.
 // ======================================================================================================
-static __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
-    __shared__ float s_thr[256];
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) s_thr[i] = P.scene.tables[256 + i];
-    grid_dependency_sync();
-    __syncthreads();
+template <class Chain>
+AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const uint32_t i, const size_t out_index,
+                               Chain &&chain) {
     const DeviceScene &S = P.scene;
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;   // pixel task within the chunk
-    const uint32_t n_pixels = n_chunk_tasks / P.n_samples;
-    uint32_t px = 0, py = 0;
-    size_t out_index = 0;
-    const bool active = i < n_pixels && task_pixel(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
-    unsigned long long cubes_traced = 0, n_hits = 0;
-    if (active) {
-        const uint32_t t0 = i * P.n_samples;
-        float a0 = 0.f, a1 = 0.f, a2 = 0.f, aT = 0.f;
-        uint32_t steps_total = 0;
-        double depth = D_INF;          // DepthBuf::mean = min over the sub-samples (accum.rs:284-297)
-        uint32_t first_valid = 0xffffffffu;   // Position of the first surface hit: first sub-sample that has one
-        int32_t text = AICB_TEXT_EMPTY;       // CharacterBuf of the pixel (text.rs:100-113 reduces the sub-samples)
-        for (uint32_t k = 0; k < P.n_samples; k++) {
-            TaskOut o;
-            *reinterpret_cast<uint4 *>(&o) = *reinterpret_cast<const uint4 *>(P.task_out + t0 + k);
-            float lr = 0.f, lg = 0.f, lb = 0.f, T = 1.0f;
-            if (P.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
-                const float4 a = P.in_accum[P.task_base + t0 + k];
-                lr = a.x; lg = a.y; lb = a.z; T = a.w;
+    const uint32_t t0 = i * P.n_samples;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, aT = 0.f;
+    uint32_t steps_total = 0;
+    double depth = D_INF;          // DepthBuf::mean = min over the sub-samples (accum.rs:284-297)
+    uint32_t first_valid = 0xffffffffu;   // Position of the first surface hit: first sub-sample that has one
+    int32_t text = AICB_TEXT_EMPTY;       // CharacterBuf of the pixel (text.rs:100-113 reduces the sub-samples)
+    for (uint32_t k = 0; k < P.n_samples; k++) {
+        TaskOut o;
+        *reinterpret_cast<uint4 *>(&o) = *reinterpret_cast<const uint4 *>(P.task_out + t0 + k);
+        float lr, lg, lb, T;
+        uint32_t steps, sample_first;
+        chain(k, o, lr, lg, lb, T, steps, sample_first);
+        if (sample_first != 0xffffffffu && (P.out_depth || P.out_hit)) {
+            const HitRecord *hr = P.hits + sample_first;   // Hit::t_distance = last_t / resolution (surface.rs:385-386)
+            depth = fmin(depth, hr->last_t * recip_pow2(1 << ((hr->flags >> 4) & 15u)));
+            if (first_valid == 0xffffffffu) first_valid = sample_first;
+        }
+        if (P.out_text) {
+            // CharacterBuf::add (text.rs:84-98): the first hit of a block names it; Exception::Incomplete without one
+            // is "X"; a ray that counted a step entered the space (sr.rs:628-637)
+            int32_t tk = o.steps > 0 ? AICB_TEXT_ENTERED_SPACE : AICB_TEXT_EMPTY;
+            if (sample_first != 0xffffffffu) {
+                const uint32_t cell = P.hits[sample_first].cell;
+                tk = S.wide_cells ? (int32_t)(__ldg((const uint32_t *)S.cells + cell) & 0xffffu)
+                                  : (int32_t)((uint32_t)__ldg((const uint16_t *)S.cells + cell) & 0x3fffu);
+            } else if (o.steps > 1000u) {
+                tk = AICB_TEXT_INCOMPLETE;
             }
-            uint32_t steps = o.steps;
-            uint32_t sample_first = 0xffffffffu;
-            uint32_t hi = o.first_hit;
-            for (uint32_t hk = 0; hk < o.n_hits; hk++) {
-                ShadedHit c;
-                {
-                    const uint4 *src = reinterpret_cast<const uint4 *>(P.shaded + hi);
-                    reinterpret_cast<uint4 *>(&c)[0] = src[0];
-                    reinterpret_cast<uint4 *>(&c)[1] = src[1];
-                }
-                if (c.factor >= 0.0f) {   // (a skipped surface leaves the ray untouched)
-                    lr = lr + c.r * T; lg = lg + c.g * T; lb = lb + c.b * T;
-                    T = T * c.factor;
-                    n_hits++;
-                    if (sample_first == 0xffffffffu) sample_first = hi;
-                    if (T < (1.0f / 256.0f)) {
-                        // the reference stops at the first step it counts after this hit; the marcher, which only
-                        // had an upper bound of T, may have gone further
-                        if (steps > c.steps) steps = c.steps + 1;
-                        break;
-                    }
-                }
-                hi = ((hi + 1u) & (HIT_CHUNK - 1u)) ? hi + 1u : c.next;   // consecutive slots; chunks are linked
-            }
-            if (sample_first != 0xffffffffu && (P.out_depth || P.out_hit)) {
-                const HitRecord *hr = P.hits + sample_first;   // Hit::t_distance = last_t / resolution (surface.rs:385-386)
-                depth = fmin(depth, hr->last_t * recip_pow2(1 << ((hr->flags >> 4) & 15u)));
-                if (first_valid == 0xffffffffu) first_valid = sample_first;
-            }
-            if (P.out_text) {
-                // CharacterBuf::add (text.rs:84-98): the first hit of a block names it; Exception::Incomplete without one
-                // is "X"; a ray that counted a step entered the space (sr.rs:628-637)
-                int32_t tk = o.steps > 0 ? AICB_TEXT_ENTERED_SPACE : AICB_TEXT_EMPTY;
-                if (sample_first != 0xffffffffu) {
-                    const uint32_t cell = P.hits[sample_first].cell;
-                    tk = S.wide_cells ? (int32_t)(__ldg((const uint32_t *)S.cells + cell) & 0xffffu)
-                                      : (int32_t)((uint32_t)__ldg((const uint16_t *)S.cells + cell) & 0x3fffu);
-                } else if (o.steps > 1000u) {
-                    tk = AICB_TEXT_INCOMPLETE;
-                }
-                // CharacterBuf::mean (text.rs:100-113): the first sample that hit wins; entered only if all entered
-                const bool ah = text >= 0 || text <= AICB_TEXT_INCOMPLETE, bh = tk >= 0 || tk <= AICB_TEXT_INCOMPLETE;
-                if (k == 0) text = tk;
-                else if (ah) {}
-                else if (bh) text = tk;
-                else if (text == AICB_TEXT_ENTERED_SPACE && tk == AICB_TEXT_ENTERED_SPACE) text = AICB_TEXT_ENTERED_SPACE;
-                else text = AICB_TEXT_EMPTY;
-            }
-            if (P.include_sky) {  // the sky is an opaque hit at t = inf
-                const int so = S.sky_kind ? (int)(o.flags & 7u) : 0;
-                lr = lr + (S.sky_colors[so][0] * 1.0f) * T;
-                lg = lg + (S.sky_colors[so][1] * 1.0f) * T;
-                lb = lb + (S.sky_colors[so][2] * 1.0f) * T;
-                T = T * (1.0f - 1.0f);
-            }
-            if (P.debug_pixel_cost) {  // ColorBuf::add for Exception::DebugOverrideRg (accum.rs:228-234)
-                float kk = ps_clamped((float)steps);
-                float red = ps_clamped(ps_mul(0.02f, kk) * 1.0f);
-                float green = ps_clamped(ps_mul(0.002f, kk) * 1.0f);
+            // CharacterBuf::mean (text.rs:100-113): the first sample that hit wins; entered only if all entered
+            const bool ah = text >= 0 || text <= AICB_TEXT_INCOMPLETE, bh = tk >= 0 || tk <= AICB_TEXT_INCOMPLETE;
+            if (k == 0) text = tk;
+            else if (ah) {}
+            else if (bh) text = tk;
+            else if (text == AICB_TEXT_ENTERED_SPACE && tk == AICB_TEXT_ENTERED_SPACE) text = AICB_TEXT_ENTERED_SPACE;
+            else text = AICB_TEXT_EMPTY;
+        }
+        if (P.include_sky) {  // the sky is an opaque hit at t = inf
+            const int so = S.sky_kind ? (int)(o.flags & 7u) : 0;
+            lr = lr + (S.sky_colors[so][0] * 1.0f) * T;
+            lg = lg + (S.sky_colors[so][1] * 1.0f) * T;
+            lb = lb + (S.sky_colors[so][2] * 1.0f) * T;
+            T = T * (1.0f - 1.0f);
+        }
+        if (P.debug_pixel_cost) {  // ColorBuf::add for Exception::DebugOverrideRg (accum.rs:228-234)
+            float kk = ps_clamped((float)steps);
+            float red = ps_clamped(ps_mul(0.02f, kk) * 1.0f);
+            float green = ps_clamped(ps_mul(0.002f, kk) * 1.0f);
+            float rgba[4];
+            colorbuf_to_rgba(lr, lg, lb, T, rgba);
+            float lum = rgba[1] * 0.7152f + (rgba[0] * 0.2126f + rgba[2] * 0.0722f);
+            lr = red; lg = green; lb = ps_clamped(lum * 0.2f);
+            T = 0.0f;
+        }
+        if (P.has_backdrop) {   // Exception::Backdrop between the UI and the world (renderer.rs:458-466)
+            lr = lr + P.backdrop[0] * T; lg = lg + P.backdrop[1] * T; lb = lb + P.backdrop[2] * T;
+            T = T * P.backdrop[3];
+        }
+        if (P.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint(NO_WORLD_TO_SHOW) replaces it (renderer.rs:474-477)
+            lr = P.no_world[0]; lg = P.no_world[1]; lb = P.no_world[2]; T = P.no_world[3];
+        }
+        if (P.out_accum) P.out_accum[P.task_base + t0 + k] = make_float4(lr, lg, lb, T);
+        if (P.bounce_mode == BOUNCE_SECONDARY) {
+            // Rgba::from(light_accum_buf.inner).to_rgb() added to the surface's multi_ray_accum (surface.rs:158-160)
+            if (P.bounce_req[t0 + k] != HIT_NONE) {
                 float rgba[4];
                 colorbuf_to_rgba(lr, lg, lb, T, rgba);
-                float lum = rgba[1] * 0.7152f + (rgba[0] * 0.2126f + rgba[2] * 0.0722f);
-                lr = red; lg = green; lb = ps_clamped(lum * 0.2f);
-                T = 0.0f;
+                float4 acc = P.bounce_sum[t0 + k];
+                acc.x = acc.x + rgba[0]; acc.y = acc.y + rgba[1]; acc.z = acc.z + rgba[2];
+                acc.w = __uint_as_float(__float_as_uint(acc.w) + steps);
+                P.bounce_sum[t0 + k] = acc;
             }
-            if (P.has_backdrop) {   // Exception::Backdrop between the UI and the world (renderer.rs:458-466)
-                lr = lr + P.backdrop[0] * T; lg = lg + P.backdrop[1] * T; lb = lb + P.backdrop[2] * T;
-                T = T * P.backdrop[3];
-            }
-            if (P.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint(NO_WORLD_TO_SHOW) replaces it (renderer.rs:474-477)
-                lr = P.no_world[0]; lg = P.no_world[1]; lb = P.no_world[2]; T = P.no_world[3];
-            }
-            if (P.out_accum) P.out_accum[P.task_base + t0 + k] = make_float4(lr, lg, lb, T);
-            if (P.bounce_mode == BOUNCE_SECONDARY) {
-                // Rgba::from(light_accum_buf.inner).to_rgb() added to the surface's multi_ray_accum (surface.rs:158-160)
-                if (P.bounce_req[t0 + k] != HIT_NONE) {
-                    float rgba[4];
-                    colorbuf_to_rgba(lr, lg, lb, T, rgba);
-                    float4 acc = P.bounce_sum[t0 + k];
-                    acc.x = acc.x + rgba[0]; acc.y = acc.y + rgba[1]; acc.z = acc.z + rgba[2];
-                    acc.w = __uint_as_float(__float_as_uint(acc.w) + steps);
-                    P.bounce_sum[t0 + k] = acc;
-                }
-                steps = 0;   // counted by the primary ray (RaytraceInfo + secondary_info, sr.rs:689-692)
-            } else if (P.bounce_mode == BOUNCE_PRIMARY) {
-                if (P.bounce_req[t0 + k] != HIT_NONE) steps += __float_as_uint(P.bounce_sum[t0 + k].w);
-            }
-            steps_total += steps;
-            a0 = a0 + lr; a1 = a1 + lg; a2 = a2 + lb; aT = aT + T;
+            steps = 0;   // counted by the primary ray (RaytraceInfo + secondary_info, sr.rs:689-692)
+        } else if (P.bounce_mode == BOUNCE_PRIMARY) {
+            if (P.bounce_req[t0 + k] != HIT_NONE) steps += __float_as_uint(P.bounce_sum[t0 + k].w);
         }
-        cubes_traced = steps_total;
-        if (P.out_text) P.out_text[out_index] = text;
-        float l0 = a0, l1 = a1, l2 = a2, tT = aT;
-        if (P.n_samples == 4) { l0 = a0 / 4.0f; l1 = a1 / 4.0f; l2 = a2 / 4.0f; tT = aT / 4.0f; }
-        if (P.out_srgb8) P.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
-        if (P.out_colorbuf) P.out_colorbuf[out_index] = make_float4(l0, l1, l2, tT);
-        if (P.out_rgba16f) {
-            // ColorBuf::into_premultiplied_rgba (raytracer_components.rs:70-77) scaled by the exposure and rounded to
-            // f16 as half::f16::from_f32 does (round to nearest even, overflow to infinity)
-            float a = 1.0f - tT;
-            a = a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a);   // clamp(0, 1): NaN passes through
-            const __half2 rg = __floats2half2_rn(l0 * P.exposure, l1 * P.exposure);
-            const __half2 ba = __floats2half2_rn(l2 * P.exposure, a);
-            uint2 packed;
-            packed.x = *reinterpret_cast<const uint32_t *>(&rg);
-            packed.y = *reinterpret_cast<const uint32_t *>(&ba);
-            P.out_rgba16f[out_index] = packed;
-        }
-        if (P.out_depth) P.out_depth[out_index] = depth;
-        if (P.out_steps) P.out_steps[out_index] = steps_total;
-        if (P.out_hit) {
-            aicb_hit hh;
-            if (first_valid != 0xffffffffu) {
-                HitRecord hr;
-                {
-                    const uint4 *src = reinterpret_cast<const uint4 *>(P.hits + first_valid);
-#pragma unroll
-                    for (int q = 0; q < 4; q++) reinterpret_cast<uint4 *>(&hr)[q] = src[q];
-                }
-                HitGeom g;
-                decode_hit(S, hr, g);
-                hh.cube[0] = g.cube[0]; hh.cube[1] = g.cube[1]; hh.cube[2] = g.cube[2];
-                hh.voxel[0] = g.voxel[0]; hh.voxel[1] = g.voxel[1]; hh.voxel[2] = g.voxel[2];
-                hh.resolution = g.res;
-                hh.face = g.face;
-            } else {
-                hh.cube[0] = hh.cube[1] = hh.cube[2] = -1;
-                hh.voxel[0] = hh.voxel[1] = hh.voxel[2] = -1;
-                hh.resolution = -1;
-                hh.face = -1;
-            }
-            P.out_hit[out_index] = hh;
-        }
+        steps_total += steps;
+        a0 = a0 + lr; a1 = a1 + lg; a2 = a2 + lb; aT = aT + T;
     }
-    // RaytraceInfo sum (renderer.rs:555) and the surface-hit counter: warp-reduce, one atomic per warp
+    if (P.out_text) P.out_text[out_index] = text;
+    float l0 = a0, l1 = a1, l2 = a2, tT = aT;
+    if (P.n_samples == 4) { l0 = a0 / 4.0f; l1 = a1 / 4.0f; l2 = a2 / 4.0f; tT = aT / 4.0f; }
+    if (P.out_srgb8) P.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
+    if (P.out_colorbuf) P.out_colorbuf[out_index] = make_float4(l0, l1, l2, tT);
+    if (P.out_rgba16f) {
+        // ColorBuf::into_premultiplied_rgba (raytracer_components.rs:70-77) scaled by the exposure and rounded to
+        // f16 as half::f16::from_f32 does (round to nearest even, overflow to infinity)
+        float a = 1.0f - tT;
+        a = a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a);   // clamp(0, 1): NaN passes through
+        const __half2 rg = __floats2half2_rn(l0 * P.exposure, l1 * P.exposure);
+        const __half2 ba = __floats2half2_rn(l2 * P.exposure, a);
+        uint2 packed;
+        packed.x = *reinterpret_cast<const uint32_t *>(&rg);
+        packed.y = *reinterpret_cast<const uint32_t *>(&ba);
+        P.out_rgba16f[out_index] = packed;
+    }
+    if (P.out_depth) P.out_depth[out_index] = depth;
+    if (P.out_steps) P.out_steps[out_index] = steps_total;
+    if (P.out_hit) {
+        aicb_hit hh;
+        if (first_valid != 0xffffffffu) {
+            HitRecord hr;
+            {
+                const uint4 *src = reinterpret_cast<const uint4 *>(P.hits + first_valid);
+#pragma unroll
+                for (int q = 0; q < 4; q++) reinterpret_cast<uint4 *>(&hr)[q] = src[q];
+            }
+            HitGeom g;
+            decode_hit(S, hr, g);
+            hh.cube[0] = g.cube[0]; hh.cube[1] = g.cube[1]; hh.cube[2] = g.cube[2];
+            hh.voxel[0] = g.voxel[0]; hh.voxel[1] = g.voxel[1]; hh.voxel[2] = g.voxel[2];
+            hh.resolution = g.res;
+            hh.face = g.face;
+        } else {
+            hh.cube[0] = hh.cube[1] = hh.cube[2] = -1;
+            hh.voxel[0] = hh.voxel[1] = hh.voxel[2] = -1;
+            hh.resolution = -1;
+            hh.face = -1;
+        }
+        P.out_hit[out_index] = hh;
+    }
+    return steps_total;
+}
+
+// RaytraceInfo sum (renderer.rs:555) and the surface-hit counter: warp-reduce, one atomic per warp
+AICB_DEV void count_pixels(const TraceParams &P, unsigned long long cubes_traced, unsigned long long n_hits) {
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) {
         cubes_traced += __shfl_down_sync(0xffffffffu, cubes_traced, off);
@@ -1914,6 +1891,206 @@ static __global__ void __launch_bounds__(128) encode_kernel(const __grid_constan
         if (cubes_traced) atomicAdd(P.counters + 0, cubes_traced);
         if (n_hits) atomicAdd(P.counters + 3, n_hits);
     }
+}
+
+// ======================================================================================================
+// Kernel 4 of a frame that does not run resolve_kernel — per pixel: the ray's transmittance chain over the ShadedHits
+// that shade_kernel left, then finish_pixel.
+// ======================================================================================================
+constexpr uint32_t ENCODE_RUN = 4;
+static __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
+    __shared__ float s_thr[256];
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) s_thr[i] = P.scene.tables[256 + i];
+    grid_dependency_sync();
+    __syncthreads();
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;   // pixel task within the chunk
+    const uint32_t n_pixels = n_chunk_tasks / P.n_samples;
+    uint32_t px = 0, py = 0;
+    size_t out_index = 0;
+    const bool active = i < n_pixels && task_pixel(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
+    unsigned long long cubes_traced = 0, n_hits = 0;
+    if (active) {
+        const uint32_t t0 = i * P.n_samples;
+        cubes_traced = finish_pixel(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
+                                                               float &T, uint32_t &steps, uint32_t &sample_first) {
+            lr = 0.f; lg = 0.f; lb = 0.f; T = 1.0f;
+            if (P.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
+                const float4 a = P.in_accum[P.task_base + t0 + k];
+                lr = a.x; lg = a.y; lb = a.z; T = a.w;
+            }
+            steps = o.steps;
+            sample_first = 0xffffffffu;
+            uint32_t hi = o.first_hit;
+            // the ray's consecutive slots, up to ENCODE_RUN at a time within a chunk: their colour and factor are
+            // requested together (and the chunk's link with them), so a deep ray waits once per run, not once per hit
+            for (uint32_t left = o.n_hits; left > 0u;) {
+                const uint32_t chunk_last = hi | (HIT_CHUNK - 1u);
+                const uint32_t run = min(left, min(ENCODE_RUN, chunk_last - hi + 1u));
+                float4 f[ENCODE_RUN];
+#pragma unroll
+                for (uint32_t j = 0; j < ENCODE_RUN; j++)
+                    if (j < run) f[j] = *reinterpret_cast<const float4 *>(P.shaded + hi + j);
+                const bool to_end = hi + run > chunk_last;
+                const uint32_t link = to_end ? P.shaded[chunk_last].next : HIT_NONE;
+                bool cut = false;
+#pragma unroll
+                for (uint32_t j = 0; j < ENCODE_RUN; j++) {
+                    if (j < run && !cut) {
+                        const float4 c = f[j];
+                        if (c.w >= 0.0f) {   // (a skipped surface leaves the ray untouched)
+                            lr = lr + c.x * T; lg = lg + c.y * T; lb = lb + c.z * T;
+                            T = T * c.w;
+                            n_hits++;
+                            if (sample_first == 0xffffffffu) sample_first = hi + j;
+                            if (T < (1.0f / 256.0f)) {
+                                // the reference stops at the first step it counts after this hit; the marcher, which
+                                // only had an upper bound of T, may have gone further
+                                const uint32_t cs = P.shaded[hi + j].steps;
+                                if (steps > cs) steps = cs + 1;
+                                cut = true;
+                            }
+                        }
+                    }
+                }
+                if (cut) break;
+                left -= run;
+                hi = to_end ? link : hi + run;
+            }
+        });
+    }
+    count_pixels(P, cubes_traced, n_hits);
+}
+
+// ======================================================================================================
+// Kernels 3+4 with None / Flat lighting (when the previous frame was shallow, launch_trace) — shading and compositing
+// in one pass, tile by tile.
+// One warp owns 32 consecutive tasks: one 8x4 tile of pixels, or with AntialiasingOption::Always 8 pixels x 4
+// samples.  Neighbouring rays mostly meet the same or adjacent cubes, so shading their hits together turns the ray,
+// palette, cell and light-texel loads into L1 hits, and no ShadedHit goes through global memory.  The warp works
+// through its rays' hit lists in windows of RESOLVE_WINDOW slots held in shared memory:
+//   list       an exclusive warp scan of the hits each lane has left places every lane's next slots in the window, in
+//              ray order (the chunk links followed as encode_kernel does);
+//   shade      the window's slots, 32 at a time, convergently (shade_hit; dead slots are skipped);
+//   composite  every lane runs its own slots in order: light += c T, T *= factor, the cut at T < 1/256 and the step
+//              restore.  A cut ray lists no more slots (its later surfaces cannot change the pixel).
+// Then finish_pixel, one lane per pixel (with 4 samples the pixel's first lane reads its samples' accumulators back
+// from shared memory, so the mean adds them in sample order as encode_kernel does).
+// ======================================================================================================
+constexpr uint32_t RESOLVE_WINDOW = 128;
+// 4 resident blocks of 128 threads per SM = 128 registers per thread at most (the kernel needs about 80)
+constexpr int RESOLVE_MIN_BLOCKS = 4;
+
+template <int LC>
+__global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const __grid_constant__ TraceParams P,
+                                                                          uint32_t n_chunk_tasks) {
+    static_assert(LC == LC_NONE || LC == LC_FLAT, "interpolated and Bounce lighting shade in shade_kernel");
+    __shared__ float s_lut[256], s_thr[256];
+    __shared__ float4 s_shaded[WARPS_PER_BLOCK][RESOLVE_WINDOW];   // r, g, b, factor (< 0: skip) of each window slot
+    __shared__ uint32_t s_slot[WARPS_PER_BLOCK][RESOLVE_WINDOW];   // hit slot, later the lanes' first surface
+    __shared__ uint32_t s_steps[WARPS_PER_BLOCK][RESOLVE_WINDOW];  // HitRecord::steps, later the lanes' step counts
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+        s_lut[i] = P.scene.tables[i];
+        s_thr[i] = P.scene.tables[256 + i];
+    }
+    grid_dependency_sync();
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    float4 *shaded = s_shaded[warp];
+    uint32_t *slots = s_slot[warp], *hsteps = s_steps[warp];
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;   // task within the chunk
+    const uint32_t i = t / P.n_samples;                          // its pixel task
+    uint32_t px = 0, py = 0;
+    size_t out_index = 0;
+    const bool active = t < n_chunk_tasks && task_pixel(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
+    float lr = 0.f, lg = 0.f, lb = 0.f, T = 1.0f;
+    uint32_t steps = 0, sample_first = 0xffffffffu, hi = HIT_NONE, left = 0;
+    if (active) {
+        TaskOut o;
+        *reinterpret_cast<uint4 *>(&o) = *reinterpret_cast<const uint4 *>(P.task_out + t);
+        if (P.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
+            const float4 a = P.in_accum[P.task_base + t];
+            lr = a.x; lg = a.y; lb = a.z; T = a.w;
+        }
+        steps = o.steps;
+        hi = o.first_hit;
+        left = o.n_hits;
+    }
+    unsigned long long texels = 0, n_hits = 0;
+    for (;;) {
+        // list: this lane's slots go to [first, first + take) of the window
+        uint32_t incl = left;
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xffffffffu, incl, off);
+            if ((int)lane >= off) incl += v;
+        }
+        const uint32_t total = __shfl_sync(0xffffffffu, incl, 31);
+        if (total == 0u) break;
+        const uint32_t first = incl - left;
+        const uint32_t take = first >= RESOLVE_WINDOW ? 0u : min(left, RESOLVE_WINDOW - first);
+        const uint32_t listed = min(total, RESOLVE_WINDOW);
+        // consecutive slots up to the end of the chunk (chunks are HIT_CHUNK-aligned), then the chunk's link: one
+        // dependent load per chunk, requested before the run's stores
+        for (uint32_t j = 0; j < take;) {
+            const uint32_t chunk_last = hi | (HIT_CHUNK - 1u);
+            const uint32_t run = min(take - j, chunk_last - hi + 1u);
+            const bool to_end = hi + run > chunk_last;
+            const uint32_t link = to_end ? __ldg(&P.hits[chunk_last].next) : HIT_NONE;
+            for (uint32_t q = 0; q < run; q++) slots[first + j + q] = hi + q;
+            j += run;
+            hi = to_end ? link : hi + run;
+        }
+        left -= take;
+        __syncwarp();
+        // shade
+        for (uint32_t b = 0; b < listed; b += 32u) {
+            const uint32_t j = b + lane;
+            if (j < listed) {
+                const ShadedHit c = shade_hit<LC>(P, s_lut, slots[j], nullptr, texels);
+                shaded[j] = make_float4(c.r, c.g, c.b, c.factor);
+                hsteps[j] = c.steps;
+            }
+        }
+        __syncwarp();
+        // composite
+        for (uint32_t j = first; j < first + take; j++) {
+            const float4 c = shaded[j];
+            if (c.w >= 0.0f) {   // (a skipped surface leaves the ray untouched)
+                lr = lr + c.x * T; lg = lg + c.y * T; lb = lb + c.z * T;
+                T = T * c.w;
+                n_hits++;
+                if (sample_first == 0xffffffffu) sample_first = slots[j];
+                if (T < (1.0f / 256.0f)) {
+                    // the reference stops at the first step it counts after this hit; the marcher, which only had an
+                    // upper bound of T, may have gone further
+                    if (steps > hsteps[j]) steps = hsteps[j] + 1;
+                    left = 0;
+                    break;
+                }
+            }
+        }
+        __syncwarp();
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) texels += __shfl_down_sync(0xffffffffu, texels, off);
+    if (lane == 0 && texels) atomicAdd(P.counters + 4, texels);
+
+    // finish: the accumulators of the warp's tasks through shared memory to their pixel's first lane
+    shaded[lane] = make_float4(lr, lg, lb, T);
+    hsteps[lane] = steps;
+    slots[lane] = sample_first;
+    __syncwarp();
+    unsigned long long cubes_traced = 0;
+    if (active && t % P.n_samples == 0u) {
+        cubes_traced = finish_pixel(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &, float &r, float &g, float &b,
+                                                               float &tr, uint32_t &st, uint32_t &sf) {
+            const float4 a = shaded[lane + k];
+            r = a.x; g = a.y; b = a.z; tr = a.w;
+            st = hsteps[lane + k];
+            sf = slots[lane + k];
+        });
+    }
+    count_pixels(P, cubes_traced, n_hits);
 }
 
 #endif  // __CUDACC__

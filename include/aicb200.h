@@ -154,7 +154,9 @@ typedef struct aicb_render_info {
     float kernel_ms;               /* CUDA-event duration of the whole frame (all kernels) on its stream */
     uint16_t flaws;                /* Flaws bits (flaws.rs:20-91) */
     uint16_t _pad;
-    float stage_ms[4];             /* the frame's kernels (first chunk): ray generation, marching, shading, encode */
+    float stage_ms[4];             /* the frame's kernels (first chunk): ray generation, marching, shading, encode;
+                                      where shading and encode ran as one kernel (LightingOption::None / Flat, most
+                                      frames) [2] is its time and [3] is 0 */
 } aicb_render_info;
 
 /* CharacterBuf states (raytracer/text.rs:52-123) of aicb_render_text: a value >= 0 is the block index (Space palette
@@ -182,7 +184,7 @@ uint32_t aicb_abi_version(void);
 /* device_id < 0 selects the current device. Fails with AICB_ERR_CUDA if there is no GPU. */
 aicb_status aicb_ctx_create(int device_id, aicb_ctx **out);
 void aicb_ctx_destroy(aicb_ctx *);
-/* aicb_render_info::stage_ms needs five event records per frame; on by default, off for callers that only want frames. */
+/* aicb_render_info::stage_ms needs up to five event records per frame; on by default, off for callers that only want frames. */
 aicb_status aicb_ctx_stage_timing(aicb_ctx *, int enable);
 /* Thread-local message for the last failing call on this thread. Never NULL. */
 const char *aicb_last_error(void);
@@ -307,7 +309,7 @@ aicb_status aicb_frame_timed_out(aicb_ctx *, void *d_frame, size_t n_pixels, uin
  * Several GPUs from ONE process (csrc/group.cu): replaces the Rayon rows x pixels dispatch of
  * trace_scene_to_image_impl (renderer.rs:516-556) across devices for hosts that own their process (the Rust
  * `impl HeadlessRenderer`, INTEGRATION.md).  The scene is replicated on every device of the group; a frame is cut into
- * interleaved 16-row strips (strip s -> device s mod n); every device's encode kernel stores its pixels straight into
+ * interleaved 16-row strips (strip s -> device s mod n); every device's last kernel stores its pixels straight into
  * device 0's frame over NVLink (peer access) and device 0 copies the frame to the caller once the other devices'
  * completion events have fired: no collective, no host thread per GPU.  The same device may be named more than once
  * (tests).  aicb_render_info: counters summed over the devices, times = the slowest device's.

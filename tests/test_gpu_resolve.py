@@ -1,0 +1,84 @@
+"""resolve_kernel (None / Flat lighting: shading and compositing in one pass, one warp per 32 rays, hit lists in
+shared-memory windows of 128 slots): frames in which a warp's hit lists span many windows, against the oracle, the
+choice between it and shade_kernel + encode_kernel, and the stage times a frame reports."""
+import numpy as np
+import pytest
+
+import orc
+from aicb200 import (LIGHT_BOUNCE, LIGHT_FLAT, LIGHT_LINEAR, LIGHT_NONE, TRANSPARENCY_SURFACE, TRANSPARENCY_VOLUMETRIC,
+                     Block, Context, GraphicsOptions, RtRenderer, Space, scenes)
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.fixture(autouse=True, scope="module")
+def _oracle_rounds_once():
+    prev = orc.get_libm()
+    orc.set_libm(orc.LIBM_CR)
+    yield
+    orc.set_libm(prev)
+
+
+def faint_slab():
+    """40 x 24 x 24 cubes of two faint transparent blocks (alpha 0.03 / 0.02), seen end on from close by: every ray
+    meets 19 to 65 surfaces and none becomes opaque, so a warp lists about a thousand slots and most lanes' lists
+    straddle a window boundary."""
+    n, m = 40, 24
+    x, y, z = np.meshgrid(np.arange(n), np.arange(m), np.arange(m), indexing="ij")
+    ids = (1 + (x + y + z) % 2).astype(np.uint16)
+    return Space((0, 0, 0), ids, [Block.air(), Block(color=(0.9, 0.5, 0.2, 0.03)), Block(color=(0.2, 0.4, 0.9, 0.02))])
+
+
+@pytest.mark.parametrize("antialias", [False, True])
+@pytest.mark.parametrize("transparency", [TRANSPARENCY_SURFACE, TRANSPARENCY_VOLUMETRIC])
+@pytest.mark.parametrize("lighting", [LIGHT_NONE, LIGHT_FLAT])
+def test_hit_lists_longer_than_a_window(lighting, transparency, antialias):
+    """A frame after a shallow one runs resolve_kernel; having met many surfaces per ray, the next one runs
+    shade_kernel + encode_kernel.  Both equal the oracle."""
+    space = faint_slab()
+    opts = GraphicsOptions(lighting_display=lighting, transparency=transparency, antialiasing_always=antialias,
+                           view_distance=200.0)
+    cam = scenes.standard_camera(space, opts, 64, 32, direction=(1.0, 0.04, 0.03), distance_scale=0.5)
+    ref = orc.OracleScene(space).render(cam, opts)
+    assert ref["steps"].min() >= 19
+    ctx = Context()
+    try:
+        r = RtRenderer(cam, ctx)
+        r.update(space)
+        r.draw_colorbuf()   # overflows the hit stream once (the library re-issues it with a larger one)
+        empty = RtRenderer(cam, ctx)
+        empty.update(Space((0, 0, 0), np.zeros((4, 4, 4), dtype=np.uint16), [Block.air()]))
+        empty.draw_colorbuf()   # no surfaces: the next frame is fused
+        empty.rt.close()
+        for fused in (True, False):
+            gpu = r.draw_colorbuf()
+            assert (gpu["info"].stage_ms[3] == 0.0) == fused
+            assert gpu["info"].counters[2] > 16 * gpu["info"].rays   # surface hits: many windows per warp
+            assert np.array_equal(gpu["hit"], ref["hit"])
+            assert np.array_equal(gpu["steps"], ref["steps"])
+            assert np.array_equal(gpu["depth"], ref["depth"])
+            assert orc.max_ulp_diff(gpu["colorbuf"], ref["colorbuf"]) == 0
+            assert gpu["info"].cubes_traced == ref["cubes_traced"]
+        r.rt.close()
+    finally:
+        ctx.close()
+
+
+def test_stage_times_of_fused_and_split_frames():
+    """With None / Flat lighting the first frame of a context runs gen -> march -> resolve: stage_ms[2] is the resolve
+    kernel and stage_ms[3] is 0.  Interpolated and Bounce lighting keep a separate encode kernel in stage_ms[3]."""
+    space = scenes.small_mixed_scene(n=12, seed=7)
+    for lighting, fused in ((LIGHT_NONE, True), (LIGHT_FLAT, True), (LIGHT_LINEAR, False), (LIGHT_BOUNCE, False)):
+        opts = GraphicsOptions(lighting_display=lighting, view_distance=40.0)
+        cam = scenes.standard_camera(space, opts, 64, 48)
+        ctx = Context()
+        try:
+            r = RtRenderer(cam, ctx)
+            r.update(space)
+            img = r.draw()
+            stage = img.info.stage_ms
+            assert all(v > 0.0 for v in stage[:3]), stage
+            assert (stage[3] == 0.0) == fused, stage
+            r.rt.close()
+        finally:
+            ctx.close()
