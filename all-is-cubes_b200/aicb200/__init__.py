@@ -104,6 +104,9 @@ def load_library() -> C.CDLL:
                                      C.POINTER(abi.RenderInfo)]
     lib.aicb_render_layers_srgb8.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_size_t, C.POINTER(abi.RenderInfo)]
+    lib.aicb_render_layers_texture.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p,
+                                               C.POINTER(C.c_double), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                               C.POINTER(abi.RenderInfo)]
     lib.aicb_ortho_image_size.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     lib.aicb_render_orthographic.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_create.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_void_p)]
@@ -267,6 +270,43 @@ class Camera:
         out = (C.c_double * 6)()
         _cam("camera_project_ndc")(C.byref(self.data), x, y, out)
         return np.array(out[:], dtype=np.float64)
+
+    NEAR_PLANE_DISTANCE = 1.0 / 32.0   # camera_struct.rs:202-205
+
+    def projection_matrix(self) -> np.ndarray:
+        """Camera::projection_matrix (camera_struct.rs:387-416): m11..m44 as a [4, 4] array, row-vector convention,
+        built as host/camera.cpp builds it."""
+        o = self.options
+        fov_cot = 1.0 / math.tan((o.fov_y / 2.0) * (math.pi / 180.0))
+        w, h = (float(v) for v in self.viewport.nominal_size)
+        aspect = w / h if h != 0.0 else math.inf
+        if not math.isfinite(aspect):
+            aspect = 1.0
+        near, far = self.NEAR_PLANE_DISTANCE, min(max(o.view_distance, 1.0), 10000.0)
+        m = np.zeros((4, 4), dtype=np.float64)
+        m[0, 0] = fov_cot / aspect
+        m[1, 1] = fov_cot
+        m[2, 2] = far / (near - far)
+        m[2, 3] = -1.0
+        m[3, 2] = (far * near) / (near - far)
+        return m
+
+    def depth_transform(self) -> np.ndarray:
+        """The matrix RaytraceToTexture maps a ray's depth with (raytrace_to_texture.rs:613-618):
+        projection_matrix().pre_translate((0, 0, -near)).pre_scale(0, 0, -(view_distance - near)), composed as euclid
+        0.22 defines pre_translate (Transform3D::translation(v).then(self)) and pre_scale (rows 1-3 scaled), in f64 and
+        in euclid's term order.  Returns m11..m44 as a [4, 4] array."""
+        p = [[float(v) for v in row] for row in self.projection_matrix()]
+        near = self.NEAR_PLANE_DISTANCE
+        far = min(max(self.options.view_distance, 1.0), 10000.0)
+        t = [[1.0, 0.0, 0.0, 0.0], [0.0, 1.0, 0.0, 0.0], [0.0, 0.0, 1.0, 0.0], [0.0, 0.0, -near, 1.0]]
+        # Transform3D::then: self.mi1 * other.m1j + self.mi2 * other.m2j + self.mi3 * other.m3j + self.mi4 * other.m4j
+        m = [[t[i][0] * p[0][j] + t[i][1] * p[1][j] + t[i][2] * p[2][j] + t[i][3] * p[3][j] for j in range(4)]
+             for i in range(4)]
+        scale = (0.0, 0.0, -(far - near))
+        for i in range(3):
+            m[i] = [v * scale[i] for v in m[i]]
+        return np.array(m, dtype=np.float64)
 
     @property
     def inverse_projection_view(self) -> np.ndarray:
@@ -699,6 +739,75 @@ def render_layers(world=None, ui=None, backdrop=None, no_world=None) -> "Renderi
                                                    nw.ctypes.data if nw is not None else None, out.ctypes.data, w * h,
                                                    C.byref(info)))
     return Rendering((w, h), out, int(info.flaws), RenderInfo.from_abi(info))
+
+
+def render_layers_texture(world=None, ui=None, backdrop=None, no_world=None, depth_transform=None, pixels=None):
+    """RaytraceToTexture::do_some_tracing's trace_one (raytrace_to_texture.rs:591-683) for a batch of pixels, through
+    every layer as render_layers traces them.  world / ui = (SpaceRaytracer, Camera, GraphicsOptions) or None;
+    depth_transform: [4, 4] (Camera.depth_transform() of the world camera); pixels: linear framebuffer indices
+    y * width + x (any order, repeats allowed) or None for the whole texture in row-major order.
+    Returns (rgba16f bits uint16 [n, 4], depth float32 [n], RenderInfo); the depth's sign is the pixel's layer (+ world,
+    - UI or neither)."""
+    lead = world if world else ui
+    cam = lead[1]
+    w, h = cam.data.fb_width, cam.data.fb_height
+    keep = []
+
+    def layer(l):
+        if not l:
+            return None
+        o = l[2].to_abi(True)
+        keep.append(o)
+        s = abi.Layer(l[0].handle, C.pointer(l[1].data), C.pointer(o))
+        keep.append(s)
+        return C.byref(s)
+
+    m = np.ascontiguousarray(depth_transform, dtype=np.float64).reshape(16)
+    if pixels is None:
+        n, plist = w * h, None
+    else:
+        plist = np.ascontiguousarray(pixels, dtype=np.uint32).reshape(-1)
+        n = plist.size
+    rgba = np.zeros((n, 4), dtype=np.uint16)
+    depth = np.zeros(n, dtype=np.float32)
+    info = abi.RenderInfo()
+    b = np.array(backdrop, dtype=np.float32) if backdrop is not None else None
+    nw = np.array(no_world, dtype=np.float32) if no_world is not None else None
+    _check(load_library().aicb_render_layers_texture(
+        layer(world), layer(ui), b.ctypes.data if b is not None else None, nw.ctypes.data if nw is not None else None,
+        m.ctypes.data_as(C.POINTER(C.c_double)), plist.ctypes.data if plist is not None else None, n,
+        rgba.ctypes.data, depth.ctypes.data, C.byref(info)))
+    return rgba, depth, RenderInfo.from_abi(info)
+
+
+CENTRAL_PIXEL_LIMIT = 60000   # raytrace_to_texture.rs:877
+
+
+def pixel_picker_order(width: int, height: int, count: Optional[int] = None) -> np.ndarray:
+    """The pixels RaytraceToTexture's PixelPicker yields (raytrace_to_texture.rs:856-918), as linear indices
+    y * width + x: the pixels stably sorted by square radius from the centre plus a 4-level dither, then the first
+    min(60000, n / 4) of that order (the centre) cycled interleaved with the rest.  `count` picks (default: one
+    cycle_length, after which every pixel has been picked at least once)."""
+    n = int(width) * int(height)
+    idx = np.arange(n, dtype=np.int64)
+    x, y = idx % width, idx // width
+    cx, cy = width / 2.0 - 0.5, height / 2.0 - 0.5
+    blend = ((x ^ y) % 4 * 2).astype(np.float64)
+    square_radius = np.maximum(np.abs(x.astype(np.float64) - cx), np.abs(y.astype(np.float64) - cy))
+    key = (square_radius + blend).astype(np.int64)   # `as i64` truncates; the values are >= 0
+    sorted_pixels = np.argsort(key, kind="stable")
+    central = min(CENTRAL_PIXEL_LIMIT, n // 4)
+    inner, outer = central, n - central
+    cycle_length = max(inner, outer) * 2
+    if count is None:
+        count = cycle_length
+    if inner == 0 or outer == 0:   # Interleave goes on with the other iterator alone
+        length = inner or outer
+        lin = (np.arange(count) % length) + (0 if inner else central) if length else np.zeros(0, dtype=np.int64)
+    else:
+        k = np.arange(count)
+        lin = np.where(k % 2 == 0, (k // 2) % inner, central + (k // 2) % outer)
+    return sorted_pixels[lin].astype(np.uint32)
 
 
 def render_orthographic(rt: "SpaceRaytracer", resolution: int = 32) -> "Rendering":

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -128,6 +128,7 @@ EXPORTED_SYMBOLS = [
     "aicb_render_colorbuf",
     "aicb_render_text",
     "aicb_render_layers_srgb8",
+    "aicb_render_layers_texture",
     "aicb_ortho_image_size",
     "aicb_render_orthographic",
     "aicb_render_srgb8_device",

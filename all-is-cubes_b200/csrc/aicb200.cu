@@ -336,6 +336,16 @@ struct Outputs {
     const float *backdrop = nullptr;    // premultiplied light rgb + transmittance
     const float *no_world = nullptr;    // ColorBuf (light rgb, transmittance)
     int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
+    // RaytraceToTexture's targets (aicb_render_layers_texture): the TEX kernels; rgba16f takes the colour texels
+    bool texture = false;
+    const uint32_t *pixel_list = nullptr;   // device: the pixel tasks (y * fb_width + x), or nullptr for every pixel
+    uint32_t n_list = 0;
+    float *tex_depth = nullptr;
+    const double *in_depth = nullptr;
+    double *out_task_depth = nullptr;
+    uint32_t tex_layer = TEX_WORLD;
+    float tex_exposure[2] = {1.0f, 1.0f};
+    double depth_m[8] = {0, 0, 0, 0, 0, 0, 0, 0};
 };
 
 // Launches the trace kernel on `stream`. Camera rays when cam != NULL, explicit rays otherwise.
@@ -367,6 +377,14 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         if ((uint64_t)P.tiles_x * P.tiles_y * 32 > 0xffffffffull) return fail(AICB_ERR_INVALID, "frame too large");
         P.n_tasks = P.tiles_x * P.tiles_y * 32;
         pixels = (uint64_t)P.fb_width * P.local_rows;
+        if (out.pixel_list) {   // one pixel task per listed pixel, 32 consecutive entries per warp
+            P.pixel_list = out.pixel_list;
+            P.n_list = out.n_list;
+            P.tiles_x = (out.n_list + 31) / 32;
+            P.tiles_y = 1;
+            P.n_tasks = out.n_list;
+            pixels = out.n_list;
+        }
     } else {
         P.exposure = 1.0f;
         P.rays = d_rays;
@@ -402,6 +420,16 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     P.out_accum = out.out_accum;
     if (out.backdrop) { std::memcpy(P.backdrop, out.backdrop, 16); P.has_backdrop = 1; }
     if (out.no_world) { std::memcpy(P.no_world, out.no_world, 16); P.has_no_world = 1; }
+    const bool tex = out.texture;
+    if (tex) {
+        P.tex_layer = out.tex_layer;
+        P.tex_exposure[0] = out.tex_exposure[0];
+        P.tex_exposure[1] = out.tex_exposure[1];
+        std::memcpy(P.depth_m, out.depth_m, sizeof P.depth_m);
+        P.in_depth = out.in_depth;
+        P.out_task_depth = out.out_task_depth;
+        P.out_tex_depth = out.tex_depth;
+    }
     P.counters = ctx->d_counters;
     P.task_counter = ctx->d_tile_counter;
     {
@@ -419,7 +447,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     sc->pending = true;
     sc->pending_pixels = pixels;
     sc->pending_rays = pixels * (P.antialias ? 4 : 1);
-    sc->pending_out_bytes_per_pixel = out.srgb8 ? 4 : (out.rgba16f ? 8 : 16);
+    sc->pending_out_bytes_per_pixel = out.srgb8 ? 4 : (tex ? 12 : (out.rgba16f ? 8 : 16));
 
     // ---- the kernels of a frame, chunked so the per-frame streams stay bounded ----------------------------------
     P.n_samples = P.antialias ? 4 : 1;
@@ -521,6 +549,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.out_srgb8 = nullptr; Q.out_colorbuf = nullptr; Q.out_rgba16f = nullptr; Q.out_depth = nullptr;
             Q.out_hit = nullptr; Q.out_steps = nullptr; Q.out_text = nullptr;
             Q.in_accum = nullptr; Q.out_accum = nullptr; Q.has_backdrop = 0; Q.has_no_world = 0;
+            Q.pixel_list = nullptr; Q.in_depth = nullptr; Q.out_task_depth = nullptr; Q.out_tex_depth = nullptr;
             Q.ray_records = (RayRecord *)ctx->d_rays2;
             Q.task_out = (TaskOut *)ctx->d_task_cb2;
             Q.hits = (HitRecord *)ctx->d_hits2;
@@ -564,8 +593,13 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             if (stage) cudaEventRecord(ctx->ev_k[2], stream);
             if (fused) {
                 const unsigned rb = (n + 127) / 128;   // one warp per 32 tasks
-                if (lc == LC_NONE) CU(launch_after(overlap, resolve_kernel<LC_NONE>, rb, 128, stream, P, n));
-                else CU(launch_after(overlap, resolve_kernel<LC_FLAT>, rb, 128, stream, P, n));
+                if (tex) {
+                    if (lc == LC_NONE) CU(launch_after(overlap, resolve_kernel<LC_NONE, true>, rb, 128, stream, P, n));
+                    else CU(launch_after(overlap, resolve_kernel<LC_FLAT, true>, rb, 128, stream, P, n));
+                } else {
+                    if (lc == LC_NONE) CU(launch_after(overlap, resolve_kernel<LC_NONE, false>, rb, 128, stream, P, n));
+                    else CU(launch_after(overlap, resolve_kernel<LC_FLAT, false>, rb, 128, stream, P, n));
+                }
                 if (stage) cudaEventRecord(ctx->ev_k[3], stream);
             } else if (!bounce) {
                 switch (lc) {
@@ -575,7 +609,8 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                 }
                 if (stage) cudaEventRecord(ctx->ev_k[3], stream);
                 const uint32_t n_pixels = n / P.n_samples;
-                CU(launch_after(overlap, encode_kernel, (n_pixels + 127) / 128, 128, stream, P, n));
+                if (tex) CU(launch_after(overlap, encode_kernel<true>, (n_pixels + 127) / 128, 128, stream, P, n));
+                else CU(launch_after(overlap, encode_kernel<false>, (n_pixels + 127) / 128, 128, stream, P, n));
                 if (stage) cudaEventRecord(ctx->ev_k[4], stream);
             } else {
                 shade_kernel<LC_BOUNCE><<<ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, 0, stream>>>(P);
@@ -591,12 +626,13 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                     gen_kernel<<<tb, 128, 0, stream>>>(Q, n);
                     k<<<(unsigned)grid, WARPS_PER_BLOCK * 32, 0, stream>>>(Q, n);
                     shade_kernel<LC_FLAT><<<ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, 0, stream>>>(Q);
-                    encode_kernel<<<tb, 128, 0, stream>>>(Q, n);
+                    encode_kernel<false><<<tb, 128, 0, stream>>>(Q, n);
                 }
                 bounce_resolve_kernel<<<tb, 128, 0, stream>>>(P, n);
                 if (stage) cudaEventRecord(ctx->ev_k[3], stream);
                 const uint32_t n_pixels = n / P.n_samples;
-                encode_kernel<<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
+                if (tex) encode_kernel<true><<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
+                else encode_kernel<false><<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
                 if (stage) cudaEventRecord(ctx->ev_k[4], stream);
             }
         }
@@ -757,6 +793,7 @@ void aicb_ctx_destroy(aicb_ctx *c) {
     if (c->d_delta) cudaFree(c->d_delta);
     if (c->ev_delta) cudaEventDestroy(c->ev_delta);
     if (c->d_task_aux) cudaFree(c->d_task_aux);
+    if (c->d_task_depth) cudaFree(c->d_task_depth);
     aicb_light_ctx_free(c);
     if (c->d_lut) cudaFree(c->d_lut);
     if (c->d_counters) cudaFree(c->d_counters);
@@ -1417,14 +1454,10 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
     return AICB_OK;
 }
 
-// == RtScene::trace_ray_through_layers for every pixel + the encoder of draw_rgba (renderer.rs:454-478, 287-291):
-// the UI layer's Space is traced first (its own camera, no sky), the backdrop colour is added, the world layer
-// continues in the same accumulator (its rays start opaque where the UI covered the pixel), and a pixel that is not
-// opaque in the end — there is no world — is painted NO_WORLD_TO_SHOW.  The world layer's options choose the sample
-// points (antialiasing) and the post-processing.
-aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *ui, const float backdrop_rgba[4],
-                                     const float no_world_rgba[4], uint8_t (*out)[4], size_t out_len,
-                                     aicb_render_info *info) {
+// Arguments shared by the layered entry points: at least one layer (or the paint colour), complete layers, one context
+// and one framebuffer size.  `lead` is the layer whose options choose the sample points.
+static aicb_status check_layers(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba, size_t out_len,
+                                const aicb_layer **lead_out) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
     if (!have_world && !have_ui && !no_world_rgba) return fail(AICB_ERR_INVALID, "no layer to draw");
     const aicb_layer *lead = have_world ? world : ui;
@@ -1441,13 +1474,28 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
         st = validate_options(ui->options);
         if (st != AICB_OK) return st;
     }
-    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
+    *lead_out = lead;
+    return AICB_OK;
+}
+
+// RtScene::trace_ray_through_layers for every pixel task of `target` (renderer.rs:454-478): the UI layer's Space is
+// traced first (its own camera, no sky), the backdrop colour is added, the world layer continues in the same
+// accumulator (its rays start opaque where the UI covered the pixel), and a pixel that is not opaque in the end — there
+// is no world — is painted NO_WORLD_TO_SHOW.  The last pass writes `target`'s outputs; with texture targets the UI pass
+// hands its DepthBuf on next to its ColorBuf.  Each pass is re-issued until its hit stream did not overflow; `total`
+// sums their RenderInfo.  The caller holds the context's lock.
+static aicb_status trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
+                                const float *no_world_rgba, const Outputs &target, aicb_render_info *total) {
+    const bool have_world = world && world->scene, have_ui = ui && ui->scene;
+    const aicb_layer *lead = have_world ? world : ui;
     aicb_ctx *ctx = lead->scene->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 4 + 16);
-    if (st != AICB_OK) return st;
+    aicb_status st = AICB_OK;
     const int aa = lead->options->antialiasing_always ? 1 : 0;
+    // per-task buffers between the passes: one entry per ray of the frame's task layout (launch_trace)
+    const size_t n_tasks = (target.pixel_list ? (size_t)target.n_list
+                                              : (((size_t)lead->camera->fb_width + TILE_W - 1) / TILE_W) *
+                                                    (((size_t)lead->camera->fb_height + TILE_H - 1) / TILE_H) * 32) *
+                           (aa ? 4 : 1);
     // Rgba -> ColorBuf (raytracer_components.rs:111-120): premultiplied light, transmittance = 1 - alpha
     float backdrop[4] = {0, 0, 0, 1}, no_world[4] = {0, 0, 0, 0};
     const bool have_backdrop = backdrop_rgba && !(backdrop_rgba[0] == 0.0f && backdrop_rgba[1] == 0.0f &&
@@ -1460,16 +1508,15 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
         for (int i = 0; i < 3; i++) no_world[i] = no_world_rgba[i] * no_world_rgba[3];
         no_world[3] = 1.0f - no_world_rgba[3];
     }
-    aicb_render_info total;
-    std::memset(&total, 0, sizeof total);
+    std::memset(total, 0, sizeof *total);
     auto add_info = [&](const aicb_render_info &one) {
-        total.cubes_traced += one.cubes_traced;
-        total.rays += one.rays;
-        total.algorithmic_bytes += one.algorithmic_bytes;
-        for (int k = 0; k < 6; k++) total.counters[k] += one.counters[k];
-        total.kernel_ms += one.kernel_ms;
-        for (int k = 0; k < 4; k++) total.stage_ms[k] += one.stage_ms[k];
-        total.flaws |= one.flaws;
+        total->cubes_traced += one.cubes_traced;
+        total->rays += one.rays;
+        total->algorithmic_bytes += one.algorithmic_bytes;
+        for (int k = 0; k < 6; k++) total->counters[k] += one.counters[k];
+        total->kernel_ms += one.kernel_ms;
+        for (int k = 0; k < 4; k++) total->stage_ms[k] += one.stage_ms[k];
+        total->flaws |= one.flaws;
     };
     auto run = [&](aicb_scene *sc, const aicb_camera *cam, const aicb_options *opt, const Outputs &o) -> aicb_status {
         for (;;) {
@@ -1483,13 +1530,23 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
             return r;
         }
     };
+    // the pass that writes no pixel (the UI pass in front of a world) keeps the task layout and the texture mode only
+    Outputs front;
+    front.texture = target.texture;
+    front.pixel_list = target.pixel_list;
+    front.n_list = target.n_list;
+    front.tex_layer = TEX_UI;
     if (have_ui && have_world) {
-        const size_t n_tasks = (((size_t)ui->camera->fb_width + TILE_W - 1) / TILE_W) * (((size_t)ui->camera->fb_height + TILE_H - 1) / TILE_H) * 32 * (aa ? 4 : 1);
         st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n_tasks * sizeof(float4) + 16);
         if (st != AICB_OK) return st;
+        if (target.texture) {   // the UI pass's DepthBuf, only when there is a UI layer
+            st = ensure(&ctx->d_task_depth, &ctx->d_task_depth_bytes, n_tasks * sizeof(double) + 16);
+            if (st != AICB_OK) return st;
+            front.out_task_depth = (double *)ctx->d_task_depth;
+        }
         aicb_options ui_opt = *ui->options;
         ui_opt.include_sky = 0;   // ui.trace_ray(.., false)
-        Outputs o1;
+        Outputs o1 = front;
         o1.out_accum = (float4 *)ctx->d_task_aux;
         o1.backdrop = have_backdrop ? backdrop : nullptr;
         o1.force_antialias = aa;
@@ -1497,19 +1554,19 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
         if (st != AICB_OK) return st;
         aicb_options w_opt = *world->options;
         w_opt.include_sky = 1;    // world.trace_ray(.., true)
-        Outputs o2;
-        o2.srgb8 = (uchar4 *)ctx->d_out;
+        Outputs o2 = target;
         o2.in_accum = (const float4 *)ctx->d_task_aux;
+        if (target.texture) o2.in_depth = (const double *)ctx->d_task_depth;
+        o2.tex_layer = TEX_WORLD;
         o2.no_world = no_world_rgba ? no_world : nullptr;
         st = run(world->scene, world->camera, &w_opt, o2);
     } else if (have_world) {
         aicb_options w_opt = *world->options;
         w_opt.include_sky = 1;
-        Outputs o;
-        o.srgb8 = (uchar4 *)ctx->d_out;
+        Outputs o = target;
+        o.tex_layer = TEX_WORLD;
         // without a UI Space the backdrop is still added in front of the world: as the accumulator's starting value
         if (have_backdrop) {
-            const size_t n_tasks = (((size_t)world->camera->fb_width + TILE_W - 1) / TILE_W) * (((size_t)world->camera->fb_height + TILE_H - 1) / TILE_H) * 32 * (aa ? 4 : 1);
             st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n_tasks * sizeof(float4) + 16);
             if (st != AICB_OK) return st;
             std::vector<float4> init(n_tasks, make_float4(backdrop[0] * 1.0f, backdrop[1] * 1.0f, backdrop[2] * 1.0f, 1.0f * backdrop[3]));
@@ -1521,14 +1578,92 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
     } else {
         aicb_options ui_opt = *ui->options;
         ui_opt.include_sky = 0;
-        Outputs o;
-        o.srgb8 = (uchar4 *)ctx->d_out;
+        Outputs o = target;
+        o.tex_layer = TEX_UI;
         o.backdrop = have_backdrop ? backdrop : nullptr;
         o.no_world = no_world_rgba ? no_world : nullptr;
         st = run(ui->scene, ui->camera, &ui_opt, o);
     }
+    return st;
+}
+
+// == RtScene::trace_ray_through_layers for every pixel + the encoder of draw_rgba (renderer.rs:454-478, 287-291).
+// The world layer's options choose the sample points (antialiasing) and the post-processing.
+aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *ui, const float backdrop_rgba[4],
+                                     const float no_world_rgba[4], uint8_t (*out)[4], size_t out_len,
+                                     aicb_render_info *info) {
+    const aicb_layer *lead = nullptr;
+    aicb_status st = check_layers(world, ui, no_world_rgba, out_len, &lead);
+    if (st != AICB_OK) return st;
+    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
+    aicb_ctx *ctx = lead->scene->ctx;
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    CU(cudaSetDevice(ctx->device));
+    st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 4 + 16);
+    if (st != AICB_OK) return st;
+    Outputs target;
+    target.srgb8 = (uchar4 *)ctx->d_out;
+    aicb_render_info total;
+    st = trace_layers(world, ui, backdrop_rgba, no_world_rgba, target, &total);
     if (st != AICB_OK) return st;
     if (out_len) CU(cudaMemcpy(out, ctx->d_out, out_len * 4, cudaMemcpyDeviceToHost));
+    if (info) *info = total;
+    return AICB_OK;
+}
+
+// == RaytraceToTexture::do_some_tracing's trace_one over a batch of pixels (raytrace_to_texture.rs:591-683): the
+// layers as aicb_render_layers_srgb8 traces them, accumulated in a Split (:922-977), stored as the colour and depth
+// texels.  Outputs are packed in list order; without a list they are the whole texture, row-major.
+aicb_status aicb_render_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float backdrop_rgba[4],
+                                       const float no_world_rgba[4], const double depth_transform[16],
+                                       const uint32_t *pixels, size_t n_pixels, uint16_t (*out_rgba16f)[4],
+                                       float *out_depth, aicb_render_info *info) {
+    const bool have_world = world && world->scene, have_ui = ui && ui->scene;
+    const aicb_layer *lead0 = have_world ? world : ui;
+    if (!lead0 || !lead0->camera) return fail(AICB_ERR_INVALID, "a layer needs its camera and options");
+    const size_t fb_pixels = (size_t)lead0->camera->fb_width * lead0->camera->fb_height;
+    const aicb_layer *lead = nullptr;
+    aicb_status st = check_layers(world, ui, no_world_rgba, fb_pixels, &lead);
+    if (st != AICB_OK) return st;
+    if (!depth_transform) return fail(AICB_ERR_INVALID, "depth_transform is NULL");
+    if (!pixels && n_pixels != fb_pixels && n_pixels != 0)
+        return fail(AICB_ERR_INVALID, "without a pixel list n_pixels must be fb_width * fb_height");
+    if (n_pixels > 0xffffffffull / 4) return fail(AICB_ERR_INVALID, "too many pixels");
+    if (n_pixels && (!out_rgba16f || !out_depth)) return fail(AICB_ERR_INVALID, "an output is NULL");
+    if (pixels)
+        for (size_t i = 0; i < n_pixels; i++)
+            if (pixels[i] >= fb_pixels) return fail(AICB_ERR_INVALID, "pixel index >= fb_width * fb_height");
+    if (info) std::memset(info, 0, sizeof *info);
+    if (n_pixels == 0) return AICB_OK;
+    aicb_ctx *ctx = lead->scene->ctx;
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    CU(cudaSetDevice(ctx->device));
+    // d_out: colour texels (8 B), depth texels (4 B), then the pixel list (4 B), each 256-byte aligned
+    const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
+    const size_t off_list = off_depth + ((n_pixels * 4 + 255) & ~(size_t)255);
+    st = ensure(&ctx->d_out, &ctx->d_out_bytes, off_list + (pixels ? n_pixels * 4 : 0) + 16);
+    if (st != AICB_OK) return st;
+    char *base = (char *)ctx->d_out;
+    Outputs target;
+    target.full_frame = true;
+    target.texture = true;
+    target.rgba16f = (uint2 *)base;
+    target.tex_depth = (float *)(base + off_depth);
+    if (pixels) {
+        CU(cudaMemcpy(base + off_list, pixels, n_pixels * 4, cudaMemcpyHostToDevice));
+        target.pixel_list = (const uint32_t *)(base + off_list);
+        target.n_list = (uint32_t)n_pixels;
+    }
+    // the exposure of each layer's camera (:603-605); a missing layer's is never used
+    target.tex_exposure[0] = have_world ? world->camera->exposure : 1.0f;
+    target.tex_exposure[1] = have_ui ? ui->camera->exposure : 1.0f;
+    const int cols[8] = {2, 6, 10, 14, 3, 7, 11, 15};   // m13 m23 m33 m43, m14 m24 m34 m44 (row-major m11..m44)
+    for (int k = 0; k < 8; k++) target.depth_m[k] = depth_transform[cols[k]];
+    aicb_render_info total;
+    st = trace_layers(world, ui, backdrop_rgba, no_world_rgba, target, &total);
+    if (st != AICB_OK) return st;
+    CU(cudaMemcpy(out_rgba16f, base, n_pixels * 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(out_depth, base + off_depth, n_pixels * 4, cudaMemcpyDeviceToHost));
     if (info) *info = total;
     return AICB_OK;
 }

@@ -70,6 +70,8 @@ struct aicb_ctx {
     struct aicb_scene *last_scene = nullptr;
     void *d_task_aux = nullptr;
     size_t d_task_aux_bytes = 0;
+    void *d_task_depth = nullptr;   // per task: the UI pass's DepthBuf for the world pass (aicb_render_layers_texture)
+    size_t d_task_depth_bytes = 0;
     // light propagation: the static ray chart (space/light/chart), built and uploaded on first use
     LightChartNode *d_chart = nullptr;
     LightNodePre *d_chart_pre = nullptr;   // the same chart in depth-first preorder (the lockstep walk)

@@ -197,6 +197,16 @@ struct TraceParams {
     uint32_t has_backdrop;
     float no_world[4];          // ColorBuf the accumulator is replaced by if it is not opaque in the end
     uint32_t has_no_world;
+    // RaytraceToTexture's colour and depth targets (raytrace_to_texture.rs:591-683): read only by the TEX
+    // instantiations of resolve_kernel / encode_kernel, and (the pixel list) by gen_kernel
+    const uint32_t *pixel_list; // pixel task i is the framebuffer pixel pixel_list[i] = y * fb_width + x, or nullptr
+    uint32_t n_list;
+    uint32_t tex_layer;         // InLayer of this pass's hits: TEX_WORLD or TEX_UI
+    float tex_exposure[2];      // exposure of the world and of the UI camera
+    double depth_m[8];          // m13 m23 m33 m43 m14 m24 m34 m44 of the depth transform
+    const double *in_depth;     // per task (global index): DepthBuf the layer in front left, or nullptr
+    double *out_task_depth;     // per task: the ray's DepthBuf, handed on next to out_accum, or nullptr
+    float *out_tex_depth;       // per pixel: the depth texel
     // LightingOption::Bounce (surface.rs:113-166): the frame's primary pass and its secondary passes share these
     uint32_t bounce_mode;       // BOUNCE_OFF / BOUNCE_PRIMARY / BOUNCE_SECONDARY
     uint32_t bounce_samples;    // LightingOption::Bounce { samples }
@@ -766,12 +776,23 @@ struct AuxState<true> {
 enum LaneState : int { ST_IDLE = 0, ST_MARCH = 1, ST_ENTER = 2, ST_POP = 3, ST_DONE = 4, ST_EXHAUSTED = 5 };
 
 // task -> pixel mapping shared by the three kernels: pixel tasks are tile-ordered (32 consecutive
-// pixel tasks = one 8x4 tile); returns false for the padding pixels of edge tiles.
+// pixel tasks = one 8x4 tile); returns false for the padding pixels of edge tiles.  With a pixel list (LIST
+// instantiations only, so that the kernels of other frames do not carry the branch) pixel task i is the listed pixel
+// and its outputs go to position i; a warp then takes 32 consecutive list entries.
+template <bool LIST>
 AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px, uint32_t *py, size_t *out_index) {
     if (P.rays) {
         *px = *py = 0;
         *out_index = pixel_task;
         return pixel_task < P.n_rays;
+    }
+    if (LIST && P.pixel_list) {
+        if (pixel_task >= P.n_list) return false;
+        const uint32_t v = __ldg(P.pixel_list + pixel_task);
+        *px = v % P.fb_width;
+        *py = v / P.fb_width;
+        *out_index = pixel_task;
+        return true;
     }
     const uint32_t tile = pixel_task >> 5, in_tile = pixel_task & 31;
     const uint32_t tx = tile % P.tiles_x, ty = tile / P.tiles_x;
@@ -802,7 +823,7 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
     RayRecord rec;
     uint32_t px, py;
     size_t out_index;
-    bool active = in_range && task_pixel(P, pixel_task, &px, &py, &out_index);
+    bool active = in_range && task_pixel<true>(P, pixel_task, &px, &py, &out_index);
     if (P.bounce_mode == BOUNCE_SECONDARY && active) active = P.bounce_req[i] != HIT_NONE;   // no surface to light
     rec.flags = 0;
     bool running = false;
@@ -1752,14 +1773,30 @@ static __global__ void __launch_bounds__(128) bounce_resolve_kernel(const __grid
 // yields sample k's accumulator after its hits (add_color_internal, raytracer_components.rs:87-92, with
 // count_step_should_stop's opacity cut, sr.rs:648-652), its step count and the slot of its first visible surface.
 // Returns the pixel's cubes_traced.
+//
+// TEX: the accumulator is RaytraceToTexture's Split (raytrace_to_texture.rs:922-977): ColorBuf, DepthBuf and the
+// layer the pixel belongs to, stored as the colour and depth texels of trace_one (:622-683).  Split::add sets the layer
+// of the first hit after which the ColorBuf is not OpacityCategory::Invisible (transmittance != 1).  Every hit
+// multiplies the transmittance by a factor in [0, 1] (or sets it to 0: DebugOverrideRg), so once it is not 1 it
+// never is again, and the first such hit can be found from the transmittance at the layer boundaries: the layer is Ui
+// if the accumulator the world pass starts from (UI hits + backdrop, whose block data is the UI layer's,
+// renderer.rs:242-252) has T != 1; otherwise this pass's layer if T != 1 after its hits; otherwise none.  P::paint
+// (accum.rs:135-151) starts a fresh Split: depth +inf, layer World if the paint colour has T != 1.  The oracle
+// (oracle_texture/aic_texture.cpp) applies the rule after each add it makes itself and after each layer's trace, and
+// counts every layer whose trace raised the transmittance, so a case that broke the argument would show in the tests.
 // ======================================================================================================
-template <class Chain>
+constexpr uint32_t TEX_NONE = 0, TEX_WORLD = 1, TEX_UI = 2;
+template <bool TEX, class Chain>
 AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const uint32_t i, const size_t out_index,
                                Chain &&chain) {
     const DeviceScene &S = P.scene;
     const uint32_t t0 = i * P.n_samples;
     float a0 = 0.f, a1 = 0.f, a2 = 0.f, aT = 0.f;
     uint32_t steps_total = 0;
+    // Split::mean: the sub-samples' DepthBuf reduced by f64::min (a NaN start is what reduce() without an initial value
+    // gives), the layer of the first sub-sample that has one
+    double tex_depth = __longlong_as_double(0x7ff8000000000000ll);
+    uint32_t tex_layer = TEX_NONE;
     double depth = D_INF;          // DepthBuf::mean = min over the sub-samples (accum.rs:284-297)
     uint32_t first_valid = 0xffffffffu;   // Position of the first surface hit: first sub-sample that has one
     int32_t text = AICB_TEXT_EMPTY;       // CharacterBuf of the pixel (text.rs:100-113 reduces the sub-samples)
@@ -1814,6 +1851,23 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
             lr = lr + P.backdrop[0] * T; lg = lg + P.backdrop[1] * T; lb = lb + P.backdrop[2] * T;
             T = T * P.backdrop[3];
         }
+        if constexpr (TEX) {
+            // DepthBuf::add (accum.rs:275-282): f64::min of the layer in front's depth and this layer's first surface
+            double d = P.in_depth ? P.in_depth[P.task_base + t0 + k] : D_INF;
+            if (sample_first != 0xffffffffu) {
+                const HitRecord *hr = P.hits + sample_first;
+                d = fmin(d, hr->last_t * recip_pow2(1 << ((hr->flags >> 4) & 15u)));
+            }
+            const float t_in = P.in_accum ? P.in_accum[P.task_base + t0 + k].w : 1.0f;
+            uint32_t layer = t_in != 1.0f ? TEX_UI : (T != 1.0f ? P.tex_layer : TEX_NONE);
+            if (P.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint: a fresh Split with the paint hit alone
+                d = D_INF;
+                layer = P.no_world[3] != 1.0f ? TEX_WORLD : TEX_NONE;
+            }
+            if (P.out_task_depth) P.out_task_depth[P.task_base + t0 + k] = d;
+            tex_depth = fmin(tex_depth, d);
+            if (tex_layer == TEX_NONE) tex_layer = layer;
+        }
         if (P.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint(NO_WORLD_TO_SHOW) replaces it (renderer.rs:474-477)
             lr = P.no_world[0]; lg = P.no_world[1]; lb = P.no_world[2]; T = P.no_world[3];
         }
@@ -1840,7 +1894,30 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
     if (P.n_samples == 4) { l0 = a0 / 4.0f; l1 = a1 / 4.0f; l2 = a2 / 4.0f; tT = aT / 4.0f; }
     if (P.out_srgb8) P.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
     if (P.out_colorbuf) P.out_colorbuf[out_index] = make_float4(l0, l1, l2, tT);
-    if (P.out_rgba16f) {
+    if constexpr (TEX) {
+        if (P.out_rgba16f) {   // trace_one's colour (raytrace_to_texture.rs:643-661): the exposure of the pixel's layer
+            const float e = tex_layer == TEX_UI ? P.tex_exposure[1] : (tex_layer == TEX_WORLD ? P.tex_exposure[0] : 1.0f);
+            float a = 1.0f - tT;
+            a = a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a);
+            const __half2 rg = __floats2half2_rn(l0 * e, l1 * e);
+            const __half2 ba = __floats2half2_rn(l2 * e, a);
+            uint2 packed;
+            packed.x = *reinterpret_cast<const uint32_t *>(&rg);
+            packed.y = *reinterpret_cast<const uint32_t *>(&ba);
+            P.out_rgba16f[out_index] = packed;
+        }
+        if (P.out_tex_depth) {
+            // trace_one's depth (:663-674): clamp(0, 1) (NaN passes), depth_transform.transform_point3d_homogeneous
+            // (0, 0, d) in euclid's term order, z / w as f32, the layer's sign (World +1, Ui or none -1)
+            double d = tex_depth;
+            if (d < 0.0) d = 0.0;
+            if (d > 1.0) d = 1.0;
+            const double *m = P.depth_m;
+            const double z = ((0.0 * m[0] + 0.0 * m[1]) + d * m[2]) + m[3];
+            const double w = ((0.0 * m[4] + 0.0 * m[5]) + d * m[6]) + m[7];
+            P.out_tex_depth[out_index] = (float)(z / w) * (tex_layer == TEX_WORLD ? 1.0f : -1.0f);
+        }
+    } else if (P.out_rgba16f) {
         // ColorBuf::into_premultiplied_rgba (raytracer_components.rs:70-77) scaled by the exposure and rounded to
         // f16 as half::f16::from_f32 does (round to nearest even, overflow to infinity)
         float a = 1.0f - tT;
@@ -1897,8 +1974,11 @@ AICB_DEV void count_pixels(const TraceParams &P, unsigned long long cubes_traced
 // Kernel 4 of a frame that does not run resolve_kernel — per pixel: the ray's transmittance chain over the ShadedHits
 // that shade_kernel left, then finish_pixel.
 // ======================================================================================================
+// TEX: the texture targets of aicb_render_layers_texture (finish_pixel); the instantiation other frames use does not
+// carry them.
 constexpr uint32_t ENCODE_RUN = 4;
-static __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
+template <bool TEX>
+__global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     __shared__ float s_thr[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_thr[i] = P.scene.tables[256 + i];
     grid_dependency_sync();
@@ -1907,11 +1987,11 @@ static __global__ void __launch_bounds__(128) encode_kernel(const __grid_constan
     const uint32_t n_pixels = n_chunk_tasks / P.n_samples;
     uint32_t px = 0, py = 0;
     size_t out_index = 0;
-    const bool active = i < n_pixels && task_pixel(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
+    const bool active = i < n_pixels && task_pixel<TEX>(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
     unsigned long long cubes_traced = 0, n_hits = 0;
     if (active) {
         const uint32_t t0 = i * P.n_samples;
-        cubes_traced = finish_pixel(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
+        cubes_traced = finish_pixel<TEX>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
                                                                float &T, uint32_t &steps, uint32_t &sample_first) {
             lr = 0.f; lg = 0.f; lb = 0.f; T = 1.0f;
             if (P.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
@@ -1980,7 +2060,7 @@ constexpr uint32_t RESOLVE_WINDOW = 128;
 // 4 resident blocks of 128 threads per SM = 128 registers per thread at most (the kernel needs about 80)
 constexpr int RESOLVE_MIN_BLOCKS = 4;
 
-template <int LC>
+template <int LC, bool TEX>
 __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const __grid_constant__ TraceParams P,
                                                                           uint32_t n_chunk_tasks) {
     static_assert(LC == LC_NONE || LC == LC_FLAT, "interpolated and Bounce lighting shade in shade_kernel");
@@ -2001,7 +2081,7 @@ __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const 
     const uint32_t i = t / P.n_samples;                          // its pixel task
     uint32_t px = 0, py = 0;
     size_t out_index = 0;
-    const bool active = t < n_chunk_tasks && task_pixel(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
+    const bool active = t < n_chunk_tasks && task_pixel<TEX>(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
     float lr = 0.f, lg = 0.f, lb = 0.f, T = 1.0f;
     uint32_t steps = 0, sample_first = 0xffffffffu, hi = HIT_NONE, left = 0;
     if (active) {
@@ -2082,7 +2162,7 @@ __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const 
     __syncwarp();
     unsigned long long cubes_traced = 0;
     if (active && t % P.n_samples == 0u) {
-        cubes_traced = finish_pixel(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &, float &r, float &g, float &b,
+        cubes_traced = finish_pixel<TEX>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &, float &r, float &g, float &b,
                                                                float &tr, uint32_t &st, uint32_t &sf) {
             const float4 a = shaded[lane + k];
             r = a.x; g = a.y; b = a.z; tr = a.w;

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 2 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 3 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -189,6 +189,10 @@ unsafe extern "C" {
     pub fn aicb_render_layers_srgb8(world: *const aicb_layer, ui: *const aicb_layer, backdrop_rgba: *const [f32; 4],
                                     no_world_rgba: *const [f32; 4], out: *mut [u8; 4], out_len: usize,
                                     info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_render_layers_texture(world: *const aicb_layer, ui: *const aicb_layer, backdrop_rgba: *const [f32; 4],
+                                      no_world_rgba: *const [f32; 4], depth_transform: *const [f64; 16],
+                                      pixels: *const u32, n_pixels: usize, out_rgba16f: *mut [u16; 4],
+                                      out_depth: *mut f32, info: *mut aicb_render_info) -> aicb_status;
     pub fn aicb_ortho_image_size(s: *const aicb_scene, resolution: u32, width: *mut u32, height: *mut u32) -> aicb_status;
     pub fn aicb_render_orthographic(s: *mut aicb_scene, resolution: u32, out: *mut [u8; 4], out_len: usize,
                                     info: *mut aicb_render_info) -> aicb_status;

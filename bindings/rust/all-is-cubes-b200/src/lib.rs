@@ -8,6 +8,8 @@
 //!   `UpdatingSpaceRaytracer` would apply (updating.rs:107-172 → `aicb_scene_update_blocks` / `_update_cubes`).
 //! * `draw()` = `RtRenderer::draw_rgba` (renderer.rs:282-308) with `trace_ray_through_layers` (renderer.rs:454-478)
 //!   → `aicb_render_layers_srgb8`; the info text is drawn here over the returned pixels like renderer.rs:659-683.
+//! * `trace_texture_batch()` = the tracing of `RaytraceToTexture::do_some_tracing` (raytrace_to_texture.rs:591-683)
+//!   for a batch of pixels → `aicb_render_layers_texture`.
 //!
 //! Not compiled in the repository this file ships in (no Rust toolchain there); see ../README.md.
 
@@ -209,6 +211,59 @@ impl B200Renderer {
     /// == `RtRenderer::new(cameras, size_policy = identity, custom_options = ())` (renderer.rs:65-81)
     pub fn new(ctx: Arc<B200Context>, cameras: StandardCameras) -> Self {
         Self { ctx, cameras, layers: Layers { world: None, ui: None }, had_cursor: false }
+    }
+
+    /// The body of `RaytraceToTexture::do_some_tracing` (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) for one
+    /// batch: `trace_one` for each pixel of `pixels` (linear indices `y * width + x`, e.g. what `PixelPicker` yields;
+    /// `None` = the whole texture, row-major), through the layers this renderer holds, on the GPU.  `cams` are the
+    /// cameras of the caller's `RtScene` (with its size policy applied).  `color[i]` receives the `Rgba16Float` texel
+    /// as raw f16 bits and `depth[i]` the `R32Float` texel of the i-th pixel; the caller stores them with
+    /// `set_pixel` as `store_one` does.
+    pub fn trace_texture_batch(
+        &self,
+        cams: &Layers<Camera>,
+        pixels: Option<&[u32]>,
+        color: &mut [[u16; 4]],
+        depth: &mut [f32],
+    ) -> Result<sys::aicb_render_info, B200Error> {
+        let camera = &cams.world;
+        // :613-618, composed by euclid exactly as the reference composes it
+        let depth_scale = -(camera.view_distance().into_inner() - camera.near_plane_distance().into_inner());
+        let depth_bias = -camera.near_plane_distance().into_inner();
+        let depth_transform = camera
+            .projection_matrix()
+            .pre_translate(euclid::vec3(0., 0., depth_bias))
+            .pre_scale(0., 0., depth_scale)
+            .to_array();
+
+        let world_cam = camera_of(&cams.world);
+        let world_opt = options_of(cams.world.options());
+        let ui_cam = camera_of(&cams.ui);
+        let ui_opt = options_of(cams.ui.options());
+        let world = self.layers.world.as_ref().map(|f| sys::aicb_layer { scene: f.scene, camera: &world_cam, options: &world_opt });
+        let ui = self.layers.ui.as_ref().map(|f| sys::aicb_layer { scene: f.scene, camera: &ui_cam, options: &ui_opt });
+        let backdrop: Rgba = self.cameras.ui_view_state().backdrop;
+        let backdrop_arr: [f32; 4] = backdrop.into();
+        let no_world: [f32; 4] = palette::NO_WORLD_TO_SHOW.into();
+        let n = pixels.map_or(color.len(), <[u32]>::len);
+        assert!(color.len() >= n && depth.len() >= n, "output slices shorter than the batch");
+
+        let mut info = sys::aicb_render_info::default();
+        check(unsafe {
+            sys::aicb_render_layers_texture(
+                world.as_ref().map_or(core::ptr::null(), |l| l),
+                ui.as_ref().map_or(core::ptr::null(), |l| l),
+                if backdrop == Rgba::TRANSPARENT { core::ptr::null() } else { &backdrop_arr },
+                &no_world,
+                &depth_transform,
+                pixels.map_or(core::ptr::null(), <[u32]>::as_ptr),
+                n,
+                color.as_mut_ptr(),
+                depth.as_mut_ptr(),
+                &mut info,
+            )
+        })?;
+        Ok(info)
     }
 
     fn sync_layer(

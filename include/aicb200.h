@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 2
+#define AICB_ABI_VERSION 3
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -259,6 +259,29 @@ typedef struct aicb_layer {
 aicb_status aicb_render_layers_srgb8(const aicb_layer *world_or_null, const aicb_layer *ui_or_null,
                                      const float backdrop_rgba[4], const float no_world_rgba[4],
                                      uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
+
+/* == RaytraceToTexture::do_some_tracing's trace_one for a batch (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683):
+ * the layers traced as aicb_render_layers_srgb8 traces them, into the Split accumulator (:922-977), stored as the two
+ * texels of a pixel.
+ *   out_rgba16f: ColorBuf::into_premultiplied_rgba with r, g, b scaled by the exposure (aicb_camera::exposure) of the
+ *                layer the pixel belongs to (1 for neither), as raw IEEE binary16 bits (half::f16::from_f32).
+ *   out_depth:   DepthBuf::depth().clamp(0, 1) through depth_transform (euclid's transform_point3d_homogeneous of
+ *                (0, 0, d), z / w in f64), as f32, times +1 for the world layer and -1 for the UI layer or neither.
+ * A pixel belongs to the layer of its first hit after which the accumulator is not fully transparent; the backdrop
+ * belongs to the UI layer and NO_WORLD_TO_SHOW to the world.  With antialiasing the four samples are reduced by
+ * Split::mean: ColorBuf mean, least depth, the first sample's layer that has one.
+ * depth_transform: m11..m44 (row-vector convention), as the caller builds it from the world camera
+ * (projection_matrix().pre_translate((0, 0, -near)).pre_scale(0, 0, -(view_distance - near)), :613-618).
+ * pixels_or_null: linear framebuffer indices y * fb_width + x, any order, repeats allowed; outputs are packed in list
+ * order.  With NULL, n_pixels must be fb_width * fb_height and the outputs are the whole texture, row-major.
+ * n_pixels == 0 does nothing.  AICB_ERR_INVALID: an index >= fb_width * fb_height, a length mismatch, or what
+ * aicb_render_layers_srgb8 rejects.  The lead layer's antialiasing option chooses the sample points. */
+aicb_status aicb_render_layers_texture(const aicb_layer *world_or_null, const aicb_layer *ui_or_null,
+                                       const float backdrop_rgba[4], const float no_world_rgba[4],
+                                       const double depth_transform[16],
+                                       const uint32_t *pixels_or_null, size_t n_pixels,
+                                       uint16_t (*out_rgba16f)[4], float *out_depth,
+                                       aicb_render_info *info_or_null);
 
 /* == render_orthographic (raytracer/ortho.rs:30-84): the five axis-aligned views of MultiOrthoCamera (:143-199) in one
  * image at `resolution` pixels per cube (the reference uses 32), UNALTERED_COLORS, sRGB8 without post-processing,
