@@ -119,6 +119,13 @@ def load_library() -> C.CDLL:
     lib.aicb_group_scene_update_cubes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_group_render_srgb8.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p,
                                             C.c_size_t, C.POINTER(abi.RenderInfo)]
+    lib.aicb_group_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_group_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_group_render_layers_srgb8.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
+    lib.aicb_group_render_layers_texture.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
+                                                     C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_size_t,
+                                                     C.c_void_p, C.c_void_p, C.POINTER(abi.RenderInfo)]
     lib.aicb_light_chart.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_light_chart.restype = C.c_uint32
     lib.aicb_light_fast_evaluate.argtypes = [C.c_void_p]
@@ -714,31 +721,35 @@ class SpaceRaytracer:
 NO_WORLD_TO_SHOW_SRGB8 = (0xBC, 0xBC, 0xBC, 0xFF)   # content/palette.rs:76
 
 
-def render_layers(world=None, ui=None, backdrop=None, no_world=None) -> "Rendering":
-    """RtRenderer::draw_rgba through every layer (renderer.rs:282-308, 454-478).
-    world / ui = (SpaceRaytracer, Camera, GraphicsOptions) or None; backdrop / no_world = linear RGBA or None."""
+def _layer_arg(l, keep, cls):
+    """(scene, Camera, GraphicsOptions) or None -> a pointer to an aicb_layer / aicb_group_layer (`cls`), kept alive by
+    `keep`."""
+    if not l:
+        return None
+    o = l[2].to_abi(True)
+    s = cls(l[0].handle, C.pointer(l[1].data), C.pointer(o))
+    keep += [o, s]
+    return C.byref(s)
+
+
+def _layers_srgb8(fn, cls, world, ui, backdrop, no_world) -> "Rendering":
     lead = world if world else ui
     cam = lead[1]
     w, h = cam.data.fb_width, cam.data.fb_height
     keep = []
-
-    def layer(l):
-        if not l:
-            return None
-        o = l[2].to_abi(True)
-        keep.append(o)
-        s = abi.Layer(l[0].handle, C.pointer(l[1].data), C.pointer(o))
-        keep.append(s)
-        return C.byref(s)
-
     out = np.zeros((h, w, 4), dtype=np.uint8)
     info = abi.RenderInfo()
     b = np.array(backdrop, dtype=np.float32) if backdrop is not None else None
     nw = np.array(no_world, dtype=np.float32) if no_world is not None else None
-    _check(load_library().aicb_render_layers_srgb8(layer(world), layer(ui), b.ctypes.data if b is not None else None,
-                                                   nw.ctypes.data if nw is not None else None, out.ctypes.data, w * h,
-                                                   C.byref(info)))
+    _check(fn(_layer_arg(world, keep, cls), _layer_arg(ui, keep, cls), b.ctypes.data if b is not None else None,
+              nw.ctypes.data if nw is not None else None, out.ctypes.data, w * h, C.byref(info)))
     return Rendering((w, h), out, int(info.flaws), RenderInfo.from_abi(info))
+
+
+def render_layers(world=None, ui=None, backdrop=None, no_world=None) -> "Rendering":
+    """RtRenderer::draw_rgba through every layer (renderer.rs:282-308, 454-478).
+    world / ui = (SpaceRaytracer, Camera, GraphicsOptions) or None; backdrop / no_world = linear RGBA or None."""
+    return _layers_srgb8(load_library().aicb_render_layers_srgb8, abi.Layer, world, ui, backdrop, no_world)
 
 
 def render_layers_texture(world=None, ui=None, backdrop=None, no_world=None, depth_transform=None, pixels=None):
@@ -748,20 +759,15 @@ def render_layers_texture(world=None, ui=None, backdrop=None, no_world=None, dep
     y * width + x (any order, repeats allowed) or None for the whole texture in row-major order.
     Returns (rgba16f bits uint16 [n, 4], depth float32 [n], RenderInfo); the depth's sign is the pixel's layer (+ world,
     - UI or neither)."""
+    return _layers_texture(load_library().aicb_render_layers_texture, abi.Layer, world, ui, backdrop, no_world,
+                           depth_transform, pixels)
+
+
+def _layers_texture(fn, cls, world, ui, backdrop, no_world, depth_transform, pixels):
     lead = world if world else ui
     cam = lead[1]
     w, h = cam.data.fb_width, cam.data.fb_height
     keep = []
-
-    def layer(l):
-        if not l:
-            return None
-        o = l[2].to_abi(True)
-        keep.append(o)
-        s = abi.Layer(l[0].handle, C.pointer(l[1].data), C.pointer(o))
-        keep.append(s)
-        return C.byref(s)
-
     m = np.ascontiguousarray(depth_transform, dtype=np.float64).reshape(16)
     if pixels is None:
         n, plist = w * h, None
@@ -773,10 +779,9 @@ def render_layers_texture(world=None, ui=None, backdrop=None, no_world=None, dep
     info = abi.RenderInfo()
     b = np.array(backdrop, dtype=np.float32) if backdrop is not None else None
     nw = np.array(no_world, dtype=np.float32) if no_world is not None else None
-    _check(load_library().aicb_render_layers_texture(
-        layer(world), layer(ui), b.ctypes.data if b is not None else None, nw.ctypes.data if nw is not None else None,
-        m.ctypes.data_as(C.POINTER(C.c_double)), plist.ctypes.data if plist is not None else None, n,
-        rgba.ctypes.data, depth.ctypes.data, C.byref(info)))
+    _check(fn(_layer_arg(world, keep, cls), _layer_arg(ui, keep, cls), b.ctypes.data if b is not None else None,
+              nw.ctypes.data if nw is not None else None, m.ctypes.data_as(C.POINTER(C.c_double)),
+              plist.ctypes.data if plist is not None else None, n, rgba.ctypes.data, depth.ctypes.data, C.byref(info)))
     return rgba, depth, RenderInfo.from_abi(info)
 
 
@@ -835,9 +840,50 @@ def print_space(space: "Space", direction, block_chars: dict, rt: "SpaceRaytrace
     return ["".join(special[v] if v < 0 else block_chars[int(v)] for v in out[r * 80:(r + 1) * 80]) for r in range(40)]
 
 
+class GroupScene:
+    """A Space replicated on every device of a DeviceGroup (aicb_group_scene): what a SpaceRaytracer is to one context,
+    kept current by the same updates, applied to every replica."""
+
+    def __init__(self, group: "DeviceGroup", space: "Space"):
+        self.group = group
+        self.space = space
+        desc, keep = space.to_desc()
+        self.handle = C.c_void_p()
+        _check(load_library().aicb_group_scene_create(group.handle, C.byref(desc), C.byref(self.handle)))
+        del keep
+
+    def update_cubes(self, cubes: np.ndarray, block_ids: np.ndarray, light: Optional[np.ndarray] = None):
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
+        lt = None if light is None else np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
+        _check(load_library().aicb_group_scene_update_cubes(self.handle, c.ctypes.data, ids.ctypes.data,
+                                                            lt.ctypes.data if lt is not None else None, c.shape[0]))
+
+    def update_blocks(self, indices, blocks):
+        """SpaceChange::BlockEvaluation / BlockIndex on every replica; a rejected update changes none."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint16)
+        arr = (abi.BlockDesc * len(blocks))()
+        for i, b in enumerate(blocks):
+            fill_block_desc(arr[i], b)
+        _check(load_library().aicb_group_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
+
+    def upload_light(self, light: np.ndarray):
+        lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
+        _check(load_library().aicb_group_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
+
+    def close(self):
+        if self.handle:
+            load_library().aicb_group_scene_destroy(self.handle)
+            self.handle = C.c_void_p()
+
+
 class DeviceGroup:
     """Several GPUs driven from this one process through the C ABI (csrc/group.cu): scene replicated, frame cut into
-    interleaved row strips, pixels stored straight into device 0's frame over NVLink."""
+    interleaved row strips, pixels stored straight into device 0's frame over NVLink.
+
+    update() / draw(): one world-only scene.  add_scene() / render_layers() / render_layers_texture(): any number of
+    replicated scenes (GroupScene) drawn through the layers as the module's render_layers / render_layers_texture draw
+    them on one context."""
 
     def __init__(self, device_ids):
         ids = (C.c_int * len(device_ids))(*[int(d) for d in device_ids])
@@ -845,6 +891,23 @@ class DeviceGroup:
         _check(load_library().aicb_group_create(ids, len(device_ids), C.byref(h)))
         self.handle = h
         self.scene = None
+        self.scenes = []
+
+    def add_scene(self, space: "Space") -> GroupScene:
+        s = GroupScene(self, space)
+        self.scenes.append(s)
+        return s
+
+    def render_layers(self, world=None, ui=None, backdrop=None, no_world=None) -> "Rendering":
+        """render_layers with GroupScenes of this group: world / ui = (GroupScene, Camera, GraphicsOptions) or None."""
+        return _layers_srgb8(load_library().aicb_group_render_layers_srgb8, abi.GroupLayer, world, ui, backdrop,
+                             no_world)
+
+    def render_layers_texture(self, world=None, ui=None, backdrop=None, no_world=None, depth_transform=None,
+                              pixels=None):
+        """render_layers_texture with GroupScenes of this group (same arguments and results)."""
+        return _layers_texture(load_library().aicb_group_render_layers_texture, abi.GroupLayer, world, ui, backdrop,
+                               no_world, depth_transform, pixels)
 
     def update(self, space: "Space"):
         if self.scene:
@@ -869,6 +932,9 @@ class DeviceGroup:
         if self.scene:
             load_library().aicb_group_scene_destroy(self.scene)
             self.scene = None
+        for s in self.scenes:
+            s.close()
+        self.scenes = []
         if self.handle:
             load_library().aicb_group_destroy(self.handle)
             self.handle = None

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -108,6 +108,10 @@ class Layer(C.Structure):
     _fields_ = [("scene", C.c_void_p), ("camera", C.POINTER(CameraData)), ("options", C.POINTER(Options))]
 
 
+class GroupLayer(C.Structure):
+    _fields_ = [("scene", C.c_void_p), ("camera", C.POINTER(CameraData)), ("options", C.POINTER(Options))]
+
+
 TEXT_ENTERED_SPACE, TEXT_EMPTY, TEXT_INCOMPLETE = -1, -2, -3
 
 EXPORTED_SYMBOLS = [
@@ -163,4 +167,8 @@ EXPORTED_SYMBOLS = [
     "aicb_group_scene_destroy",
     "aicb_group_scene_update_cubes",
     "aicb_group_render_srgb8",
+    "aicb_group_scene_update_blocks",
+    "aicb_group_scene_upload_light",
+    "aicb_group_render_layers_srgb8",
+    "aicb_group_render_layers_texture",
 ]

@@ -321,32 +321,7 @@ static aicb_status ensure(void **p, size_t *cur, size_t want) {
     return AICB_OK;
 }
 
-struct Outputs {
-    bool full_frame = false;
-    uchar4 *srgb8 = nullptr;
-    float4 *colorbuf = nullptr;
-    uint2 *rgba16f = nullptr;
-    double *depth = nullptr;
-    aicb_hit *hit = nullptr;
-    uint32_t *steps = nullptr;
-    int32_t *text = nullptr;
-    // layers (renderer.rs:454-478)
-    const float4 *in_accum = nullptr;
-    float4 *out_accum = nullptr;
-    const float *backdrop = nullptr;    // premultiplied light rgb + transmittance
-    const float *no_world = nullptr;    // ColorBuf (light rgb, transmittance)
-    int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
-    // RaytraceToTexture's targets (aicb_render_layers_texture): the TEX kernels; rgba16f takes the colour texels
-    bool texture = false;
-    const uint32_t *pixel_list = nullptr;   // device: the pixel tasks (y * fb_width + x), or nullptr for every pixel
-    uint32_t n_list = 0;
-    float *tex_depth = nullptr;
-    const double *in_depth = nullptr;
-    double *out_task_depth = nullptr;
-    uint32_t tex_layer = TEX_WORLD;
-    float tex_exposure[2] = {1.0f, 1.0f};
-    double depth_m[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-};
+aicb_status aicb_ensure_device(void **p, size_t *cur, size_t want) { return ensure(p, cur, want); }
 
 // Launches the trace kernel on `stream`. Camera rays when cam != NULL, explicit rays otherwise.
 static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const aicb_options *opt,
@@ -1004,6 +979,38 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
 // existing block indices.  New voxel data is appended to the brick pool and the palette (the replaced ranges are
 // reclaimed by the next aicb_scene_create); cubes that hold a block whose classification changed are re-encoded.
 // Does not queue light updates: call aicb_light_evaluate afterwards if the change affects light.
+// Validates and flattens the new definitions of aicb_scene_update_blocks without touching the scene.
+static aicb_status flatten_update(const aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n,
+                                  std::vector<BlockRec> &recs, std::vector<uint8_t> &kinds, std::vector<uint16_t> &bricks,
+                                  std::vector<float4> &palette, std::vector<float2> &pal_tab, bool *any_kind_changed) {
+    const size_t n_blocks = s->block_kind.size();
+    recs.resize(n);
+    kinds.resize(n);
+    for (size_t i = 0; i < n; i++) {
+        if (indices[i] >= n_blocks) return fail(AICB_ERR_INVALID, "block index out of range (new indices need a new scene)");
+        aicb_status fst = flatten_block(descs[i], recs[i], kinds[i], bricks, palette, pal_tab);
+        if (fst != AICB_OK) return fst;
+    }
+    if (s->n_bricks + bricks.size() > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
+    *any_kind_changed = false;
+    for (size_t i = 0; i < n; i++) *any_kind_changed |= s->block_kind[indices[i]] != kinds[i];
+    if (*any_kind_changed && s->h_ids.size() != s->volume)
+        return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
+    return AICB_OK;
+}
+
+aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
+    if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    std::vector<BlockRec> recs;
+    std::vector<uint8_t> kinds;
+    std::vector<uint16_t> bricks;
+    std::vector<float4> palette;
+    std::vector<float2> pal_tab;
+    bool any_kind_changed = false;
+    return flatten_update(s, indices, descs, n, recs, kinds, bricks, palette, pal_tab, &any_kind_changed);
+}
+
 aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
     if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
     aicb_ctx *ctx = s->ctx;
@@ -1011,22 +1018,15 @@ aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, con
     CU(cudaSetDevice(ctx->device));
     if (n == 0) return AICB_OK;
     const size_t n_blocks = s->block_kind.size();
-    std::vector<BlockRec> recs(n);
-    std::vector<uint8_t> kinds(n);
+    std::vector<BlockRec> recs;
+    std::vector<uint8_t> kinds;
     std::vector<uint16_t> bricks;
     std::vector<float4> palette;
     std::vector<float2> pal_tab;
-    // validate and flatten everything before touching any state
-    for (size_t i = 0; i < n; i++) {
-        if (indices[i] >= n_blocks) return fail(AICB_ERR_INVALID, "block index out of range (new indices need a new scene)");
-        aicb_status fst = flatten_block(descs[i], recs[i], kinds[i], bricks, palette, pal_tab);
-        if (fst != AICB_OK) return fst;
-    }
-    if (s->n_bricks + bricks.size() > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
     bool any_kind_changed = false;
-    for (size_t i = 0; i < n; i++) any_kind_changed |= s->block_kind[indices[i]] != kinds[i];
-    if (any_kind_changed && s->h_ids.size() != s->volume)
-        return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
+    // validate and flatten everything before touching any state
+    aicb_status vst = flatten_update(s, indices, descs, n, recs, kinds, bricks, palette, pal_tab, &any_kind_changed);
+    if (vst != AICB_OK) return vst;
     CU(cudaDeviceSynchronize());   // nothing (on any stream) may still be reading the arrays that are replaced
 
     // ---- grow the pools: the new arrays are complete before any pointer of the scene changes ----------------
@@ -1456,8 +1456,8 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
 
 // Arguments shared by the layered entry points: at least one layer (or the paint colour), complete layers, one context
 // and one framebuffer size.  `lead` is the layer whose options choose the sample points.
-static aicb_status check_layers(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba, size_t out_len,
-                                const aicb_layer **lead_out) {
+aicb_status aicb_check_layers(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba, size_t out_len,
+                              const aicb_layer **lead_out) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
     if (!have_world && !have_ui && !no_world_rgba) return fail(AICB_ERR_INVALID, "no layer to draw");
     const aicb_layer *lead = have_world ? world : ui;
@@ -1478,24 +1478,28 @@ static aicb_status check_layers(const aicb_layer *world, const aicb_layer *ui, c
     return AICB_OK;
 }
 
-// RtScene::trace_ray_through_layers for every pixel task of `target` (renderer.rs:454-478): the UI layer's Space is
+// RtScene::trace_ray_through_layers for every pixel task of every part (renderer.rs:454-478): the UI layer's Space is
 // traced first (its own camera, no sky), the backdrop colour is added, the world layer continues in the same
 // accumulator (its rays start opaque where the UI covered the pixel), and a pixel that is not opaque in the end — there
-// is no world — is painted NO_WORLD_TO_SHOW.  The last pass writes `target`'s outputs; with texture targets the UI pass
-// hands its DepthBuf on next to its ColorBuf.  Each pass is re-issued until its hit stream did not overflow; `total`
-// sums their RenderInfo.  The caller holds the context's lock.
-static aicb_status trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
-                                const float *no_world_rgba, const Outputs &target, aicb_render_info *total) {
+// is no world — is painted NO_WORLD_TO_SHOW.  The last pass writes each part's target; with texture targets the UI pass
+// hands its DepthBuf on next to its ColorBuf.
+// A pass is issued on every part before any part's pass is finished, so that the devices of a group overlap; a context
+// tracks one frame (finish), so its next pass waits until this one is finished.  A part whose hit stream overflowed
+// (finish has raised that context's capacity) is re-issued alone, that pass only.  A part's info sums its passes;
+// `total` sums the parts' counters and takes the slowest part's times.  The caller holds the parts' contexts' locks.
+aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
+                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
     const aicb_layer *lead = have_world ? world : ui;
-    aicb_ctx *ctx = lead->scene->ctx;
     aicb_status st = AICB_OK;
     const int aa = lead->options->antialiasing_always ? 1 : 0;
-    // per-task buffers between the passes: one entry per ray of the frame's task layout (launch_trace)
-    const size_t n_tasks = (target.pixel_list ? (size_t)target.n_list
-                                              : (((size_t)lead->camera->fb_width + TILE_W - 1) / TILE_W) *
-                                                    (((size_t)lead->camera->fb_height + TILE_H - 1) / TILE_H) * 32) *
-                           (aa ? 4 : 1);
+    // per-task buffers between the passes: one entry per ray of the part's task layout (launch_trace)
+    auto n_tasks = [&](const LayerPart &p) -> size_t {
+        return (p.target.pixel_list ? (size_t)p.target.n_list
+                                    : (((size_t)lead->camera->fb_width + TILE_W - 1) / TILE_W) *
+                                          ((shard_rows(lead->camera->fb_height, &p.shard) + TILE_H - 1) / TILE_H) * 32) *
+               (aa ? 4 : 1);
+    };
     // Rgba -> ColorBuf (raytracer_components.rs:111-120): premultiplied light, transmittance = 1 - alpha
     float backdrop[4] = {0, 0, 0, 1}, no_world[4] = {0, 0, 0, 0};
     const bool have_backdrop = backdrop_rgba && !(backdrop_rgba[0] == 0.0f && backdrop_rgba[1] == 0.0f &&
@@ -1508,83 +1512,166 @@ static aicb_status trace_layers(const aicb_layer *world, const aicb_layer *ui, c
         for (int i = 0; i < 3; i++) no_world[i] = no_world_rgba[i] * no_world_rgba[3];
         no_world[3] = 1.0f - no_world_rgba[3];
     }
+    auto add_info = [](aicb_render_info &sum, const aicb_render_info &one) {
+        sum.cubes_traced += one.cubes_traced;
+        sum.rays += one.rays;
+        sum.algorithmic_bytes += one.algorithmic_bytes;
+        for (int k = 0; k < 6; k++) sum.counters[k] += one.counters[k];
+        sum.kernel_ms += one.kernel_ms;
+        for (int k = 0; k < 4; k++) sum.stage_ms[k] += one.stage_ms[k];
+        sum.flaws |= one.flaws;
+    };
+    // one pass of the frame on every part: `layer` picks the part's scene, `outputs(part, ctx)` its Outputs
+    auto pass = [&](aicb_scene *LayerPart::*layer, const aicb_camera *cam, const aicb_options *opt,
+                    auto outputs) -> aicb_status {
+        std::vector<size_t> todo(n_parts), again;
+        for (size_t i = 0; i < n_parts; i++) todo[i] = i;
+        while (!todo.empty()) {
+            for (size_t i : todo) {
+                aicb_scene *sc = parts[i].*layer;
+                CU(cudaSetDevice(sc->ctx->device));
+                aicb_status r = launch_trace(sc, cam, opt, &parts[i].shard, nullptr, 0, outputs(parts[i], sc->ctx), false,
+                                             sc->ctx->stream);
+                if (r != AICB_OK) return r;
+            }
+            again.clear();
+            for (size_t i : todo) {
+                aicb_scene *sc = parts[i].*layer;
+                CU(cudaSetDevice(sc->ctx->device));
+                CU(cudaStreamSynchronize(sc->ctx->stream));
+                aicb_render_info one;
+                aicb_status r = finish(sc, &one);
+                if (r == AICB_ERR_RETRY) { again.push_back(i); continue; }   // (x4 per retry, AICB_ERR_OOM at the cap)
+                if (r != AICB_OK) return r;
+                add_info(parts[i].info, one);
+            }
+            todo.swap(again);
+        }
+        return AICB_OK;
+    };
+    for (size_t i = 0; i < n_parts; i++) std::memset(&parts[i].info, 0, sizeof parts[i].info);
+    if (have_ui && have_world) {
+        for (size_t i = 0; i < n_parts; i++) {
+            aicb_ctx *ctx = parts[i].world->ctx;
+            CU(cudaSetDevice(ctx->device));
+            st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n_tasks(parts[i]) * sizeof(float4) + 16);
+            if (st != AICB_OK) return st;
+            if (parts[i].target.texture) {   // the UI pass's DepthBuf, only when there is a UI layer
+                st = ensure(&ctx->d_task_depth, &ctx->d_task_depth_bytes, n_tasks(parts[i]) * sizeof(double) + 16);
+                if (st != AICB_OK) return st;
+            }
+        }
+        aicb_options ui_opt = *ui->options;
+        ui_opt.include_sky = 0;   // ui.trace_ray(.., false)
+        st = pass(&LayerPart::ui, ui->camera, &ui_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
+            // the pass that writes no pixel keeps the task layout and the texture mode only
+            Outputs o;
+            o.texture = p.target.texture;
+            o.pixel_list = p.target.pixel_list;
+            o.n_list = p.target.n_list;
+            o.tex_layer = TEX_UI;
+            if (p.target.texture) o.out_task_depth = (double *)ctx->d_task_depth;
+            o.out_accum = (float4 *)ctx->d_task_aux;
+            o.backdrop = have_backdrop ? backdrop : nullptr;
+            o.force_antialias = aa;
+            return o;
+        });
+        if (st != AICB_OK) return st;
+        aicb_options w_opt = *world->options;
+        w_opt.include_sky = 1;    // world.trace_ray(.., true)
+        st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
+            Outputs o = p.target;
+            o.in_accum = (const float4 *)ctx->d_task_aux;   // a re-issued world pass starts from the same accumulator
+            if (p.target.texture) o.in_depth = (const double *)ctx->d_task_depth;
+            o.tex_layer = TEX_WORLD;
+            o.no_world = no_world_rgba ? no_world : nullptr;
+            return o;
+        });
+    } else if (have_world) {
+        aicb_options w_opt = *world->options;
+        w_opt.include_sky = 1;
+        // without a UI Space the backdrop is still added in front of the world: as the accumulator's starting value
+        if (have_backdrop) {
+            for (size_t i = 0; i < n_parts; i++) {
+                aicb_ctx *ctx = parts[i].world->ctx;
+                const size_t n = n_tasks(parts[i]);
+                CU(cudaSetDevice(ctx->device));
+                st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n * sizeof(float4) + 16);
+                if (st != AICB_OK) return st;
+                std::vector<float4> init(n, make_float4(backdrop[0] * 1.0f, backdrop[1] * 1.0f, backdrop[2] * 1.0f, 1.0f * backdrop[3]));
+                CU(cudaMemcpy(ctx->d_task_aux, init.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
+            }
+        }
+        st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
+            Outputs o = p.target;
+            o.tex_layer = TEX_WORLD;
+            if (have_backdrop) o.in_accum = (const float4 *)ctx->d_task_aux;
+            o.no_world = no_world_rgba ? no_world : nullptr;
+            return o;
+        });
+    } else {
+        aicb_options ui_opt = *ui->options;
+        ui_opt.include_sky = 0;
+        st = pass(&LayerPart::ui, ui->camera, &ui_opt, [&](const LayerPart &p, aicb_ctx *) {
+            Outputs o = p.target;
+            o.tex_layer = TEX_UI;
+            o.backdrop = have_backdrop ? backdrop : nullptr;
+            o.no_world = no_world_rgba ? no_world : nullptr;
+            return o;
+        });
+    }
+    if (st != AICB_OK) return st;
+    // RaytraceInfo: summed over the parts (renderer.rs:555); the frame took as long as its slowest part
     std::memset(total, 0, sizeof *total);
-    auto add_info = [&](const aicb_render_info &one) {
+    for (size_t i = 0; i < n_parts; i++) {
+        const aicb_render_info &one = parts[i].info;
         total->cubes_traced += one.cubes_traced;
         total->rays += one.rays;
         total->algorithmic_bytes += one.algorithmic_bytes;
         for (int k = 0; k < 6; k++) total->counters[k] += one.counters[k];
-        total->kernel_ms += one.kernel_ms;
-        for (int k = 0; k < 4; k++) total->stage_ms[k] += one.stage_ms[k];
+        total->kernel_ms = std::max(total->kernel_ms, one.kernel_ms);
+        for (int k = 0; k < 4; k++) total->stage_ms[k] = std::max(total->stage_ms[k], one.stage_ms[k]);
         total->flaws |= one.flaws;
-    };
-    auto run = [&](aicb_scene *sc, const aicb_camera *cam, const aicb_options *opt, const Outputs &o) -> aicb_status {
-        for (;;) {
-            aicb_status r = launch_trace(sc, cam, opt, nullptr, nullptr, 0, o, false, ctx->stream);
-            if (r != AICB_OK) return r;
-            CU(cudaStreamSynchronize(ctx->stream));
-            aicb_render_info one;
-            r = finish(sc, &one);
-            if (r == AICB_ERR_RETRY) continue;
-            if (r == AICB_OK) add_info(one);
-            return r;
-        }
-    };
-    // the pass that writes no pixel (the UI pass in front of a world) keeps the task layout and the texture mode only
-    Outputs front;
-    front.texture = target.texture;
-    front.pixel_list = target.pixel_list;
-    front.n_list = target.n_list;
-    front.tex_layer = TEX_UI;
-    if (have_ui && have_world) {
-        st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n_tasks * sizeof(float4) + 16);
-        if (st != AICB_OK) return st;
-        if (target.texture) {   // the UI pass's DepthBuf, only when there is a UI layer
-            st = ensure(&ctx->d_task_depth, &ctx->d_task_depth_bytes, n_tasks * sizeof(double) + 16);
-            if (st != AICB_OK) return st;
-            front.out_task_depth = (double *)ctx->d_task_depth;
-        }
-        aicb_options ui_opt = *ui->options;
-        ui_opt.include_sky = 0;   // ui.trace_ray(.., false)
-        Outputs o1 = front;
-        o1.out_accum = (float4 *)ctx->d_task_aux;
-        o1.backdrop = have_backdrop ? backdrop : nullptr;
-        o1.force_antialias = aa;
-        st = run(ui->scene, ui->camera, &ui_opt, o1);
-        if (st != AICB_OK) return st;
-        aicb_options w_opt = *world->options;
-        w_opt.include_sky = 1;    // world.trace_ray(.., true)
-        Outputs o2 = target;
-        o2.in_accum = (const float4 *)ctx->d_task_aux;
-        if (target.texture) o2.in_depth = (const double *)ctx->d_task_depth;
-        o2.tex_layer = TEX_WORLD;
-        o2.no_world = no_world_rgba ? no_world : nullptr;
-        st = run(world->scene, world->camera, &w_opt, o2);
-    } else if (have_world) {
-        aicb_options w_opt = *world->options;
-        w_opt.include_sky = 1;
-        Outputs o = target;
-        o.tex_layer = TEX_WORLD;
-        // without a UI Space the backdrop is still added in front of the world: as the accumulator's starting value
-        if (have_backdrop) {
-            st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n_tasks * sizeof(float4) + 16);
-            if (st != AICB_OK) return st;
-            std::vector<float4> init(n_tasks, make_float4(backdrop[0] * 1.0f, backdrop[1] * 1.0f, backdrop[2] * 1.0f, 1.0f * backdrop[3]));
-            CU(cudaMemcpy(ctx->d_task_aux, init.data(), n_tasks * sizeof(float4), cudaMemcpyHostToDevice));
-            o.in_accum = (const float4 *)ctx->d_task_aux;
-        }
-        o.no_world = no_world_rgba ? no_world : nullptr;
-        st = run(world->scene, world->camera, &w_opt, o);
-    } else {
-        aicb_options ui_opt = *ui->options;
-        ui_opt.include_sky = 0;
-        Outputs o = target;
-        o.tex_layer = TEX_UI;
-        o.backdrop = have_backdrop ? backdrop : nullptr;
-        o.no_world = no_world_rgba ? no_world : nullptr;
-        st = run(ui->scene, ui->camera, &ui_opt, o);
     }
-    return st;
+    return AICB_OK;
+}
+
+// The single-context layered calls draw with one part: the layers' own scenes, every row.
+static LayerPart single_part(const aicb_layer *world, const aicb_layer *ui) {
+    LayerPart p;
+    p.world = world ? world->scene : nullptr;
+    p.ui = ui ? ui->scene : nullptr;
+    return p;
+}
+
+aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba,
+                                      const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
+                                      const void *out_rgba16f, const float *out_depth, const aicb_layer **lead_out) {
+    const bool have_world = world && world->scene;
+    const aicb_layer *lead0 = have_world ? world : ui;
+    if (!lead0 || !lead0->camera) return fail(AICB_ERR_INVALID, "a layer needs its camera and options");
+    const size_t fb_pixels = (size_t)lead0->camera->fb_width * lead0->camera->fb_height;
+    aicb_status st = aicb_check_layers(world, ui, no_world_rgba, fb_pixels, lead_out);
+    if (st != AICB_OK) return st;
+    if (!depth_transform) return fail(AICB_ERR_INVALID, "depth_transform is NULL");
+    if (!pixels && n_pixels != fb_pixels && n_pixels != 0)
+        return fail(AICB_ERR_INVALID, "without a pixel list n_pixels must be fb_width * fb_height");
+    if (n_pixels > 0xffffffffull / 4) return fail(AICB_ERR_INVALID, "too many pixels");
+    if (n_pixels && (!out_rgba16f || !out_depth)) return fail(AICB_ERR_INVALID, "an output is NULL");
+    if (pixels)
+        for (size_t i = 0; i < n_pixels; i++)
+            if (pixels[i] >= fb_pixels) return fail(AICB_ERR_INVALID, "pixel index >= fb_width * fb_height");
+    return AICB_OK;
+}
+
+void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *target) {
+    target->full_frame = true;
+    target->texture = true;
+    // the exposure of each layer's camera (:603-605); a missing layer's is never used
+    target->tex_exposure[0] = (world && world->scene) ? world->camera->exposure : 1.0f;
+    target->tex_exposure[1] = (ui && ui->scene) ? ui->camera->exposure : 1.0f;
+    const int cols[8] = {2, 6, 10, 14, 3, 7, 11, 15};   // m13 m23 m33 m43, m14 m24 m34 m44 (row-major m11..m44)
+    for (int k = 0; k < 8; k++) target->depth_m[k] = depth_transform[cols[k]];
 }
 
 // == RtScene::trace_ray_through_layers for every pixel + the encoder of draw_rgba (renderer.rs:454-478, 287-291).
@@ -1593,7 +1680,7 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
                                      const float no_world_rgba[4], uint8_t (*out)[4], size_t out_len,
                                      aicb_render_info *info) {
     const aicb_layer *lead = nullptr;
-    aicb_status st = check_layers(world, ui, no_world_rgba, out_len, &lead);
+    aicb_status st = aicb_check_layers(world, ui, no_world_rgba, out_len, &lead);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
     aicb_ctx *ctx = lead->scene->ctx;
@@ -1601,10 +1688,10 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
     CU(cudaSetDevice(ctx->device));
     st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 4 + 16);
     if (st != AICB_OK) return st;
-    Outputs target;
-    target.srgb8 = (uchar4 *)ctx->d_out;
+    LayerPart part = single_part(world, ui);
+    part.target.srgb8 = (uchar4 *)ctx->d_out;
     aicb_render_info total;
-    st = trace_layers(world, ui, backdrop_rgba, no_world_rgba, target, &total);
+    st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
     if (st != AICB_OK) return st;
     if (out_len) CU(cudaMemcpy(out, ctx->d_out, out_len * 4, cudaMemcpyDeviceToHost));
     if (info) *info = total;
@@ -1618,21 +1705,10 @@ aicb_status aicb_render_layers_texture(const aicb_layer *world, const aicb_layer
                                        const float no_world_rgba[4], const double depth_transform[16],
                                        const uint32_t *pixels, size_t n_pixels, uint16_t (*out_rgba16f)[4],
                                        float *out_depth, aicb_render_info *info) {
-    const bool have_world = world && world->scene, have_ui = ui && ui->scene;
-    const aicb_layer *lead0 = have_world ? world : ui;
-    if (!lead0 || !lead0->camera) return fail(AICB_ERR_INVALID, "a layer needs its camera and options");
-    const size_t fb_pixels = (size_t)lead0->camera->fb_width * lead0->camera->fb_height;
     const aicb_layer *lead = nullptr;
-    aicb_status st = check_layers(world, ui, no_world_rgba, fb_pixels, &lead);
+    aicb_status st = aicb_check_layers_texture(world, ui, no_world_rgba, depth_transform, pixels, n_pixels, out_rgba16f,
+                                               out_depth, &lead);
     if (st != AICB_OK) return st;
-    if (!depth_transform) return fail(AICB_ERR_INVALID, "depth_transform is NULL");
-    if (!pixels && n_pixels != fb_pixels && n_pixels != 0)
-        return fail(AICB_ERR_INVALID, "without a pixel list n_pixels must be fb_width * fb_height");
-    if (n_pixels > 0xffffffffull / 4) return fail(AICB_ERR_INVALID, "too many pixels");
-    if (n_pixels && (!out_rgba16f || !out_depth)) return fail(AICB_ERR_INVALID, "an output is NULL");
-    if (pixels)
-        for (size_t i = 0; i < n_pixels; i++)
-            if (pixels[i] >= fb_pixels) return fail(AICB_ERR_INVALID, "pixel index >= fb_width * fb_height");
     if (info) std::memset(info, 0, sizeof *info);
     if (n_pixels == 0) return AICB_OK;
     aicb_ctx *ctx = lead->scene->ctx;
@@ -1644,9 +1720,9 @@ aicb_status aicb_render_layers_texture(const aicb_layer *world, const aicb_layer
     st = ensure(&ctx->d_out, &ctx->d_out_bytes, off_list + (pixels ? n_pixels * 4 : 0) + 16);
     if (st != AICB_OK) return st;
     char *base = (char *)ctx->d_out;
-    Outputs target;
-    target.full_frame = true;
-    target.texture = true;
+    LayerPart part = single_part(world, ui);
+    Outputs &target = part.target;
+    aicb_texture_target(world, ui, depth_transform, &target);
     target.rgba16f = (uint2 *)base;
     target.tex_depth = (float *)(base + off_depth);
     if (pixels) {
@@ -1654,13 +1730,8 @@ aicb_status aicb_render_layers_texture(const aicb_layer *world, const aicb_layer
         target.pixel_list = (const uint32_t *)(base + off_list);
         target.n_list = (uint32_t)n_pixels;
     }
-    // the exposure of each layer's camera (:603-605); a missing layer's is never used
-    target.tex_exposure[0] = have_world ? world->camera->exposure : 1.0f;
-    target.tex_exposure[1] = have_ui ? ui->camera->exposure : 1.0f;
-    const int cols[8] = {2, 6, 10, 14, 3, 7, 11, 15};   // m13 m23 m33 m43, m14 m24 m34 m44 (row-major m11..m44)
-    for (int k = 0; k < 8; k++) target.depth_m[k] = depth_transform[cols[k]];
     aicb_render_info total;
-    st = trace_layers(world, ui, backdrop_rgba, no_world_rgba, target, &total);
+    st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
     if (st != AICB_OK) return st;
     CU(cudaMemcpy(out_rgba16f, base, n_pixels * 8, cudaMemcpyDeviceToHost));
     CU(cudaMemcpy(out_depth, base + off_depth, n_pixels * 4, cudaMemcpyDeviceToHost));

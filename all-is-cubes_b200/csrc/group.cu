@@ -6,7 +6,12 @@
 // waits for the others' completion events and copies the frame to the caller: compute and delivery are one kernel
 // chain per device, there is no collective and no host thread per GPU.
 // Replaces the Rayon rows x pixels dispatch of trace_scene_to_image_impl (renderer.rs:516-556) across devices.
+// Layered frames and texture targets (aicb_group_render_layers_*) cut the work the same way, or a pixel list into
+// ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu), which issues each pass on every device
+// before it waits for any.
+#include <algorithm>
 #include <cstring>
+#include <mutex>
 #include <vector>
 
 #include "internal.h"
@@ -16,6 +21,8 @@ struct aicb_group {
     std::vector<cudaEvent_t> done;   // per device: its strips of the current frame are in device 0's frame
     void *d_frame = nullptr;         // on device 0
     size_t frame_pixels = 0;
+    void *d_tex = nullptr;           // on device 0: the colour and depth texels of aicb_group_render_layers_texture
+    size_t d_tex_bytes = 0;
     void *h_stage = nullptr;         // pinned staging for pageable destinations
     size_t h_stage_bytes = 0;
 };
@@ -27,6 +34,70 @@ struct aicb_group_scene {
 
 static const uint32_t GROUP_STRIP_ROWS = 16;
 
+static aicb_status ensure_frame(aicb_group *g, size_t pixels) {   // device 0's sRGB8 frame; the root device is current
+    if (g->frame_pixels < pixels) {
+        if (g->d_frame) cudaFree(g->d_frame);
+        g->d_frame = nullptr;
+        g->frame_pixels = 0;
+        CU(cudaMalloc(&g->d_frame, pixels * 4 + 16));
+        g->frame_pixels = pixels;
+    }
+    return AICB_OK;
+}
+
+// ---- layered frames and texture targets -------------------------------------------------------------------------------
+// The layers of a group call as device i sees them: its replicas, the same cameras and options.
+static aicb_layer replica(const aicb_group_layer *l, size_t i) {
+    aicb_layer r;
+    r.scene = (l && l->scene) ? l->scene->scene[i] : nullptr;
+    r.camera = l ? l->camera : nullptr;
+    r.options = l ? l->options : nullptr;
+    return r;
+}
+
+// The group of the layers' scenes (nullptr if there is no scene: validation then rejects the call).
+static aicb_status group_of(const aicb_group_layer *world, const aicb_group_layer *ui, aicb_group **g) {
+    const bool have_world = world && world->scene, have_ui = ui && ui->scene;
+    if (have_world && have_ui && world->scene->group != ui->scene->group)
+        return aicb_fail(AICB_ERR_INVALID, "the layers must be scenes of the same group");
+    *g = have_world ? world->scene->group : (have_ui ? ui->scene->group : nullptr);
+    return AICB_OK;
+}
+
+// Every device's part of a whole frame or texture: interleaved 16-row strips, outputs at their framebuffer positions in
+// device 0's buffers (`target`).
+static std::vector<LayerPart> strip_parts(aicb_group *g, const aicb_group_layer *world, const aicb_group_layer *ui,
+                                          const Outputs &target) {
+    const uint32_t n = (uint32_t)g->ctx.size();
+    std::vector<LayerPart> parts(n);
+    for (uint32_t i = 0; i < n; i++) {
+        parts[i].world = replica(world, i).scene;
+        parts[i].ui = replica(ui, i).scene;
+        parts[i].shard = {GROUP_STRIP_ROWS, i, n};
+        parts[i].target = target;
+    }
+    return parts;
+}
+
+// Delivery: device 0's stream waits for the completion events of the devices that drew a part.
+static aicb_status join(aicb_group *g, size_t n_parts) {
+    for (size_t i = 1; i < n_parts; i++) {
+        CU(cudaSetDevice(g->ctx[i]->device));
+        CU(cudaEventRecord(g->done[i], g->ctx[i]->stream));
+    }
+    CU(cudaSetDevice(g->ctx[0]->device));
+    for (size_t i = 1; i < n_parts; i++) CU(cudaStreamWaitEvent(g->ctx[0]->stream, g->done[i], 0));
+    return AICB_OK;
+}
+
+// The contexts' locks, for the whole of a layered call (its passes run on every context).
+struct GroupLock {
+    std::vector<std::unique_lock<std::mutex>> locks;
+    explicit GroupLock(aicb_group *g) {
+        for (aicb_ctx *c : g->ctx) locks.emplace_back(c->mu);
+    }
+};
+
 extern "C" {
 
 void aicb_group_destroy(aicb_group *g) {
@@ -34,6 +105,7 @@ void aicb_group_destroy(aicb_group *g) {
     if (!g->ctx.empty()) {
         cudaSetDevice(g->ctx[0]->device);
         if (g->d_frame) cudaFree(g->d_frame);
+        if (g->d_tex) cudaFree(g->d_tex);
         if (g->h_stage) cudaFreeHost(g->h_stage);
     }
     for (size_t i = 0; i < g->ctx.size(); i++) {
@@ -134,13 +206,8 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
     const uint32_t n = (uint32_t)g->ctx.size();
     aicb_ctx *root = g->ctx[0];
     CU(cudaSetDevice(root->device));
-    if (g->frame_pixels < pixels) {
-        if (g->d_frame) cudaFree(g->d_frame);
-        g->d_frame = nullptr;
-        g->frame_pixels = 0;
-        CU(cudaMalloc(&g->d_frame, pixels * 4 + 16));
-        g->frame_pixels = pixels;
-    }
+    aicb_status fst = ensure_frame(g, pixels);
+    if (fst != AICB_OK) return fst;
     for (int attempt = 0;; attempt++) {
         // every device renders its strips into the root's frame; nothing here waits for a GPU
         for (uint32_t i = 0; i < n; i++) {
@@ -180,6 +247,126 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
         }
         if (attempt >= 5) return aicb_fail(AICB_ERR_OOM, "hit stream capacity exhausted");
     }
+}
+
+aicb_status aicb_group_scene_update_blocks(aicb_group_scene *gs, const uint16_t *indices, const aicb_block_desc *descs,
+                                           size_t n) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    // the replicas hold the same block table: what replica 0 accepts every replica accepts, and a rejected update
+    // leaves them all as they were
+    aicb_status st = aicb_scene_check_blocks(gs->scene[0], indices, descs, n);
+    if (st != AICB_OK) return st;
+    for (aicb_scene *s : gs->scene) {
+        st = aicb_scene_update_blocks(s, indices, descs, n);
+        if (st != AICB_OK) return st;
+    }
+    return AICB_OK;
+}
+
+aicb_status aicb_group_scene_upload_light(aicb_group_scene *gs, const uint8_t (*light)[4], size_t n_texels) {
+    if (!gs || !light) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n_texels != gs->scene[0]->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
+    for (aicb_scene *s : gs->scene) {
+        aicb_status st = aicb_scene_upload_light(s, light, n_texels);
+        if (st != AICB_OK) return st;
+    }
+    return AICB_OK;
+}
+
+aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world, const aicb_group_layer *ui,
+                                           const float backdrop_rgba[4], const float no_world_rgba[4], uint8_t (*out)[4],
+                                           size_t out_len, aicb_render_info *info) {
+    aicb_group *g = nullptr;
+    aicb_status st = group_of(world, ui, &g);
+    if (st != AICB_OK) return st;
+    aicb_layer w0 = replica(world, 0), u0 = replica(ui, 0);
+    const aicb_layer *w = world ? &w0 : nullptr, *u = ui ? &u0 : nullptr, *lead = nullptr;
+    st = aicb_check_layers(w, u, no_world_rgba, out_len, &lead);
+    if (st != AICB_OK) return st;
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    GroupLock lock(g);
+    aicb_ctx *root = g->ctx[0];
+    CU(cudaSetDevice(root->device));
+    st = ensure_frame(g, out_len);
+    if (st != AICB_OK) return st;
+    Outputs target;
+    target.full_frame = true;
+    target.srgb8 = (uchar4 *)g->d_frame;
+    std::vector<LayerPart> parts = strip_parts(g, world, ui, target);
+    aicb_render_info total;
+    st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
+    if (st != AICB_OK) return st;
+    st = join(g, parts.size());
+    if (st != AICB_OK) return st;
+    if (out_len) CU(cudaMemcpyAsync(out, g->d_frame, out_len * 4, cudaMemcpyDeviceToHost, root->stream));
+    CU(cudaStreamSynchronize(root->stream));
+    if (info) *info = total;
+    return AICB_OK;
+}
+
+aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world, const aicb_group_layer *ui,
+                                             const float backdrop_rgba[4], const float no_world_rgba[4],
+                                             const double depth_transform[16], const uint32_t *pixels, size_t n_pixels,
+                                             uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info) {
+    aicb_group *g = nullptr;
+    aicb_status st = group_of(world, ui, &g);
+    if (st != AICB_OK) return st;
+    aicb_layer w0 = replica(world, 0), u0 = replica(ui, 0);
+    const aicb_layer *w = world ? &w0 : nullptr, *u = ui ? &u0 : nullptr, *lead = nullptr;
+    st = aicb_check_layers_texture(w, u, no_world_rgba, depth_transform, pixels, n_pixels, out_rgba16f, out_depth, &lead);
+    if (st != AICB_OK) return st;
+    if (info) std::memset(info, 0, sizeof *info);
+    if (n_pixels == 0) return AICB_OK;
+    GroupLock lock(g);
+    aicb_ctx *root = g->ctx[0];
+    CU(cudaSetDevice(root->device));
+    // device 0: colour texels (8 B), then depth texels (4 B), 256-byte aligned
+    const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
+    st = aicb_ensure_device(&g->d_tex, &g->d_tex_bytes, off_depth + n_pixels * 4 + 16);
+    if (st != AICB_OK) return st;
+    char *base = (char *)g->d_tex;
+    Outputs target;
+    aicb_texture_target(w, u, depth_transform, &target);
+    target.rgba16f = (uint2 *)base;
+    target.tex_depth = (float *)(base + off_depth);
+    std::vector<LayerPart> parts;
+    if (!pixels) {
+        parts = strip_parts(g, world, ui, target);
+    } else {
+        // Contiguous ranges of whole warps (a warp takes 32 consecutive list entries), as even as whole warps allow.
+        // Device i traces its range from its own copy of it and stores at the range's offset: list order is kept.
+        const size_t warps = (n_pixels + 31) / 32;
+        const size_t used = std::min(g->ctx.size(), warps);
+        size_t begin = 0;
+        for (size_t i = 0; i < used; i++) {
+            const size_t count = std::min(32 * (warps / used + (i < warps % used ? 1 : 0)), n_pixels - begin);
+            aicb_ctx *c = g->ctx[i];
+            CU(cudaSetDevice(c->device));
+            st = aicb_ensure_device(&c->d_out, &c->d_out_bytes, count * 4 + 16);
+            if (st != AICB_OK) return st;
+            CU(cudaMemcpy(c->d_out, pixels + begin, count * 4, cudaMemcpyHostToDevice));
+            LayerPart p;
+            p.world = replica(world, i).scene;
+            p.ui = replica(ui, i).scene;
+            p.target = target;
+            p.target.pixel_list = (const uint32_t *)c->d_out;
+            p.target.n_list = (uint32_t)count;
+            p.target.rgba16f = target.rgba16f + begin;
+            p.target.tex_depth = target.tex_depth + begin;
+            parts.push_back(p);
+            begin += count;
+        }
+    }
+    aicb_render_info total;
+    st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
+    if (st != AICB_OK) return st;
+    st = join(g, parts.size());
+    if (st != AICB_OK) return st;
+    CU(cudaMemcpyAsync(out_rgba16f, base, n_pixels * 8, cudaMemcpyDeviceToHost, root->stream));
+    CU(cudaMemcpyAsync(out_depth, base + off_depth, n_pixels * 4, cudaMemcpyDeviceToHost, root->stream));
+    CU(cudaStreamSynchronize(root->stream));
+    if (info) *info = total;
+    return AICB_OK;
 }
 
 }  // extern "C"

@@ -120,3 +120,59 @@ struct aicb_scene {
     uint32_t light_max_distance = 0;
     uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
 };
+
+// Where a frame's kernels store their outputs, and what the layers hand on between passes (launch_trace).
+struct Outputs {
+    bool full_frame = false;
+    uchar4 *srgb8 = nullptr;
+    float4 *colorbuf = nullptr;
+    uint2 *rgba16f = nullptr;
+    double *depth = nullptr;
+    aicb_hit *hit = nullptr;
+    uint32_t *steps = nullptr;
+    int32_t *text = nullptr;
+    // layers (renderer.rs:454-478)
+    const float4 *in_accum = nullptr;
+    float4 *out_accum = nullptr;
+    const float *backdrop = nullptr;    // premultiplied light rgb + transmittance
+    const float *no_world = nullptr;    // ColorBuf (light rgb, transmittance)
+    int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
+    // RaytraceToTexture's targets (aicb_render_layers_texture): the TEX kernels; rgba16f takes the colour texels
+    bool texture = false;
+    const uint32_t *pixel_list = nullptr;   // device: the pixel tasks (y * fb_width + x), or nullptr for every pixel
+    uint32_t n_list = 0;
+    float *tex_depth = nullptr;
+    const double *in_depth = nullptr;
+    double *out_task_depth = nullptr;
+    uint32_t tex_layer = aicb::TEX_WORLD;
+    float tex_exposure[2] = {1.0f, 1.0f};
+    double depth_m[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+};
+
+// One device's share of a layered frame or texture (aicb_trace_layers): that device's scenes of the layers (nullptr for
+// an absent layer; both on one context), its row strips of a whole frame or its range of a pixel list
+// (target.pixel_list), and where it stores its outputs.  A single context draws with one part and no strips.
+struct LayerPart {
+    aicb_scene *world = nullptr, *ui = nullptr;
+    aicb_shard shard = {1, 0, 1};
+    Outputs target;
+    aicb_render_info info{};   // this part's passes, summed
+};
+
+// aicb200.cu: the layer rules shared by aicb_render_layers_* and aicb_group_render_layers_*.  The layers give the
+// cameras and options (their scenes only say which layers exist).  Validation of the arguments of the single-context
+// calls; the texture target's exposures and depth transform; the passes of a frame over every part.  aicb_trace_layers
+// needs the locks of the parts' contexts.  (C linkage: aicb200.cu defines them among the entry points of the C ABI.)
+extern "C" {
+aicb_status aicb_check_layers(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba, size_t out_len,
+                              const aicb_layer **lead_out);
+aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba,
+                                      const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
+                                      const void *out_rgba16f, const float *out_depth, const aicb_layer **lead_out);
+void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *target);
+aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
+                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total);
+aicb_status aicb_ensure_device(void **p, size_t *cur, size_t want);
+// aicb_scene_update_blocks' validation alone: AICB_OK if that call would accept the update (changes nothing)
+aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
+}

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 3 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 4 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -163,6 +163,15 @@ pub struct aicb_layer {
     pub options: *const aicb_options,
 }
 
+/// one layer of a layered frame on a device group: a replicated scene
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct aicb_group_layer {
+    pub scene: *mut aicb_group_scene,
+    pub camera: *const aicb_camera,
+    pub options: *const aicb_options,
+}
+
 unsafe extern "C" {
     pub fn aicb_abi_version() -> u32;
     pub fn aicb_ctx_create(device_id: c_int, out: *mut *mut aicb_ctx) -> aicb_status;
@@ -223,6 +232,19 @@ unsafe extern "C" {
                                          light: *const [u8; 4], n: usize) -> aicb_status;
     pub fn aicb_group_render_srgb8(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
                                    out: *mut [u8; 4], out_len: usize, info: *mut aicb_render_info) -> aicb_status;
+    // every replica; validated against replica 0 first, so a rejected call changes none
+    pub fn aicb_group_scene_update_blocks(gs: *mut aicb_group_scene, indices: *const u16, descs: *const aicb_block_desc,
+                                          n: usize) -> aicb_status;
+    pub fn aicb_group_scene_upload_light(gs: *mut aicb_group_scene, light: *const [u8; 4], n_texels: usize) -> aicb_status;
+    // aicb_render_layers_* on a group: both layers must be scenes of the same group
+    pub fn aicb_group_render_layers_srgb8(world: *const aicb_group_layer, ui: *const aicb_group_layer,
+                                          backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],
+                                          out: *mut [u8; 4], out_len: usize, info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_layers_texture(world: *const aicb_group_layer, ui: *const aicb_group_layer,
+                                            backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],
+                                            depth_transform: *const [f64; 16], pixels: *const u32, n_pixels: usize,
+                                            out_rgba16f: *mut [u16; 4], out_depth: *mut f32,
+                                            info: *mut aicb_render_info) -> aicb_status;
 
     pub fn aicb_trace_rays(s: *mut aicb_scene, origin_dir: *const [f64; 6], n: usize, opt: *const aicb_options,
                            out_colorbuf: *mut [f32; 4], depth: *mut f64, hit: *mut aicb_hit, steps: *mut u32,

@@ -10,6 +10,9 @@
 //!   → `aicb_render_layers_srgb8`; the info text is drawn here over the returned pixels like renderer.rs:659-683.
 //! * `trace_texture_batch()` = the tracing of `RaytraceToTexture::do_some_tracing` (raytrace_to_texture.rs:591-683)
 //!   for a batch of pixels → `aicb_render_layers_texture`.
+//! * `B200Renderer::on_devices()` / `on_group()`: the same renderer on several devices (`aicb_group_*`): scenes
+//!   replicated and kept current by the same deltas, `draw()` → `aicb_group_render_layers_srgb8`,
+//!   `trace_texture_batch()` → `aicb_group_render_layers_texture`.
 //!
 //! Not compiled in the repository this file ships in (no Rust toolchain there); see ../README.md.
 
@@ -67,6 +70,100 @@ impl Drop for B200Context {
     }
 }
 
+/// Several devices driven from this process (`aicb_group`): scenes replicated on each, frames cut into row strips,
+/// texture batches into ranges of the pixel list, every device storing into device 0's buffers.
+#[derive(Debug)]
+pub struct B200Group(*mut sys::aicb_group);
+// SAFETY: as B200Context: the library holds every context's lock for the whole of a group call.
+unsafe impl Send for B200Group {}
+unsafe impl Sync for B200Group {}
+
+impl B200Group {
+    /// `device_ids` may name a device more than once.  Fails if a device cannot reach device 0's memory (peer access).
+    pub fn new(device_ids: &[i32]) -> Result<Arc<Self>, B200Error> {
+        let mut group = core::ptr::null_mut();
+        check(unsafe { sys::aicb_group_create(device_ids.as_ptr(), device_ids.len() as i32, &mut group) })?;
+        Ok(Arc::new(Self(group)))
+    }
+}
+impl Drop for B200Group {
+    fn drop(&mut self) {
+        unsafe { sys::aicb_group_destroy(self.0) }
+    }
+}
+
+/// Where a renderer's scenes live.
+#[derive(Clone, Debug)]
+enum Backend {
+    Context(Arc<B200Context>),
+    Group(Arc<B200Group>),
+}
+
+/// One layer's device-resident scene: on one context, or replicated on a group.
+#[derive(Clone, Copy, Debug)]
+enum SceneHandle {
+    Single(*mut sys::aicb_scene),
+    Group(*mut sys::aicb_group_scene),
+}
+
+impl SceneHandle {
+    fn create(backend: &Backend, desc: &sys::aicb_scene_desc) -> Result<Self, B200Error> {
+        match backend {
+            Backend::Context(ctx) => {
+                let mut s = core::ptr::null_mut();
+                check(unsafe { sys::aicb_scene_create(ctx.0, desc, &mut s) })?;
+                Ok(Self::Single(s))
+            }
+            Backend::Group(group) => {
+                let mut s = core::ptr::null_mut();
+                check(unsafe { sys::aicb_group_scene_create(group.0, desc, &mut s) })?;
+                Ok(Self::Group(s))
+            }
+        }
+    }
+
+    fn update_blocks(self, indices: &[u16], descs: &[sys::aicb_block_desc]) -> Result<(), B200Error> {
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_scene_update_blocks(s, indices.as_ptr(), descs.as_ptr(), indices.len()),
+                Self::Group(s) => sys::aicb_group_scene_update_blocks(s, indices.as_ptr(), descs.as_ptr(), indices.len()),
+            }
+        })
+    }
+
+    fn update_cubes(self, cubes: &[[i32; 3]], ids: &[u16], light: &[[u8; 4]]) -> Result<(), B200Error> {
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_scene_update_cubes(s, cubes.as_ptr(), ids.as_ptr(), light.as_ptr(), cubes.len()),
+                Self::Group(s) => {
+                    sys::aicb_group_scene_update_cubes(s, cubes.as_ptr(), ids.as_ptr(), light.as_ptr(), cubes.len())
+                }
+            }
+        })
+    }
+
+    fn destroy(self) {
+        match self {
+            Self::Single(s) => unsafe { sys::aicb_scene_destroy(s) },
+            Self::Group(s) => unsafe { sys::aicb_group_scene_destroy(s) },
+        }
+    }
+
+    // A renderer's scenes all live on its backend.
+    fn single(self) -> *mut sys::aicb_scene {
+        match self {
+            Self::Single(s) => s,
+            Self::Group(_) => unreachable!("a group scene on a single-context renderer"),
+        }
+    }
+    fn grouped(self) -> *mut sys::aicb_group_scene {
+        match self {
+            Self::Group(s) => s,
+            Self::Single(_) => unreachable!("a single-context scene on a group renderer"),
+        }
+    }
+}
+
 /// The `SpaceChange` buckets of `SrtTodo` (updating.rs:176-219).
 #[derive(Debug, Default)]
 struct Todo {
@@ -100,7 +197,7 @@ impl listen::Store<SpaceChange> for Todo {
 /// the counterpart of `UpdatingSpaceRaytracer` (updating.rs:19-172).
 struct SceneFollower {
     space: Handle<Space>,
-    scene: *mut sys::aicb_scene,
+    scene: Option<SceneHandle>,
     todo: listen::StoreLock<Todo>,
 }
 // SAFETY: see B200Context.
@@ -110,12 +207,12 @@ impl SceneFollower {
     fn new(space: Handle<Space>) -> Self {
         Self {
             space,
-            scene: core::ptr::null_mut(),
+            scene: None,
             todo: listen::StoreLock::new(Todo { listener: true, everything: true, ..Todo::default() }),
         }
     }
 
-    fn update(&mut self, ctx: &B200Context, read_ticket: ReadTicket<'_>) -> Result<bool, RenderError> {
+    fn update(&mut self, backend: &Backend, read_ticket: ReadTicket<'_>) -> Result<bool, RenderError> {
         let todo = {
             let mut guard = self.todo.lock();
             if !guard.listener && !guard.everything && guard.blocks.is_empty() && guard.cubes.is_empty() {
@@ -127,7 +224,7 @@ impl SceneFollower {
         if todo.listener {
             space.listen(self.todo.listener());
         }
-        if self.scene.is_null() || todo.everything {
+        if self.scene.is_none() || todo.everything {
             // SpaceRaytracer::new (sr.rs:64-88): bounds, extract() of (block index, light texel), block_data(), sky
             let bounds = space.bounds();
             let cubes = space.extract(bounds, |e| (e.block_index(), e.light().as_texel())); // space.rs:740-761, Z-major
@@ -147,21 +244,19 @@ impl SceneFollower {
                 light_max_distance: convert::light_max_distance_of(&physics.light),
                 _pad: [0; 7],
             };
-            let mut fresh = core::ptr::null_mut();
-            check(unsafe { sys::aicb_scene_create(ctx.0, &desc, &mut fresh) }).map_err(to_render_error)?;
-            if !self.scene.is_null() {
-                unsafe { sys::aicb_scene_destroy(self.scene) };
+            let fresh = SceneHandle::create(backend, &desc).map_err(to_render_error)?;
+            if let Some(old) = self.scene.replace(fresh) {
+                old.destroy();
             }
-            self.scene = fresh;
-        } else {
-            // SpaceChange::BlockIndex / BlockEvaluation: re-run TracingBlock::from_block for those indices (updating.rs:128-150)
+        } else if let Some(scene) = self.scene {
+            // SpaceChange::BlockIndex / BlockEvaluation: re-run TracingBlock::from_block for those indices (updating.rs:128-150);
+            // on a group every replica takes them (aicb_group_scene_update_blocks), no rebuild
             if !todo.blocks.is_empty() {
                 let idx: Vec<u16> = todo.blocks.iter().copied().collect();
                 let owned: Vec<OwnedBlockDesc> =
                     idx.iter().map(|&i| block_desc_of(&space.block_data()[usize::from(i)])).collect();
                 let descs: Vec<sys::aicb_block_desc> = owned.iter().map(OwnedBlockDesc::as_ffi).collect();
-                check(unsafe { sys::aicb_scene_update_blocks(self.scene, idx.as_ptr(), descs.as_ptr(), idx.len()) })
-                    .map_err(to_render_error)?;
+                scene.update_blocks(&idx, &descs).map_err(to_render_error)?;
             }
             // SpaceChange::CubeBlock / CubeLight (updating.rs:151-166)
             if !todo.cubes.is_empty() {
@@ -175,10 +270,7 @@ impl SceneFollower {
                         light.push(space.get_lighting(cube).as_texel());
                     }
                 }
-                check(unsafe {
-                    sys::aicb_scene_update_cubes(self.scene, cubes.as_ptr(), ids.as_ptr(), light.as_ptr(), cubes.len())
-                })
-                .map_err(to_render_error)?;
+                scene.update_cubes(&cubes, &ids, &light).map_err(to_render_error)?;
             }
         }
         Ok(true)
@@ -186,8 +278,8 @@ impl SceneFollower {
 }
 impl Drop for SceneFollower {
     fn drop(&mut self) {
-        if !self.scene.is_null() {
-            unsafe { sys::aicb_scene_destroy(self.scene) };
+        if let Some(scene) = self.scene.take() {
+            scene.destroy();
         }
     }
 }
@@ -201,7 +293,7 @@ fn to_render_error(e: B200Error) -> RenderError {
 
 /// Drop-in for `RtRenderer<()>`.
 pub struct B200Renderer {
-    ctx: Arc<B200Context>,
+    backend: Backend,
     cameras: StandardCameras,
     layers: Layers<Option<SceneFollower>>,
     had_cursor: bool,
@@ -210,7 +302,51 @@ pub struct B200Renderer {
 impl B200Renderer {
     /// == `RtRenderer::new(cameras, size_policy = identity, custom_options = ())` (renderer.rs:65-81)
     pub fn new(ctx: Arc<B200Context>, cameras: StandardCameras) -> Self {
-        Self { ctx, cameras, layers: Layers { world: None, ui: None }, had_cursor: false }
+        Self::with_backend(Backend::Context(ctx), cameras)
+    }
+
+    /// The same renderer on a device group: each layer's Space is replicated on every device, kept current by the
+    /// same deltas, and every frame or texture batch is shared between the devices (`aicb_group_render_layers_*`).
+    /// The pixels are those `new` draws, bit for bit.
+    pub fn on_group(group: Arc<B200Group>, cameras: StandardCameras) -> Self {
+        Self::with_backend(Backend::Group(group), cameras)
+    }
+
+    /// `on_group` with a group of its own over `device_ids`.
+    pub fn on_devices(device_ids: &[i32], cameras: StandardCameras) -> Result<Self, B200Error> {
+        Ok(Self::on_group(B200Group::new(device_ids)?, cameras))
+    }
+
+    fn with_backend(backend: Backend, cameras: StandardCameras) -> Self {
+        Self { backend, cameras, layers: Layers { world: None, ui: None }, had_cursor: false }
+    }
+
+    /// Calls `single` with the layers this renderer holds as `aicb_layer`s, or on a group `group` with them as
+    /// `aicb_group_layer`s (NULL for an absent layer).
+    fn with_layers<R>(
+        &self,
+        cams: &Layers<Camera>,
+        single: impl FnOnce(*const sys::aicb_layer, *const sys::aicb_layer) -> R,
+        group: impl FnOnce(*const sys::aicb_group_layer, *const sys::aicb_group_layer) -> R,
+    ) -> R {
+        let world_cam = camera_of(&cams.world);
+        let world_opt = options_of(cams.world.options());
+        let ui_cam = camera_of(&cams.ui);
+        let ui_opt = options_of(cams.ui.options());
+        let w = self.layers.world.as_ref().and_then(|f| f.scene);
+        let u = self.layers.ui.as_ref().and_then(|f| f.scene);
+        match self.backend {
+            Backend::Context(_) => {
+                let world = w.map(|s| sys::aicb_layer { scene: s.single(), camera: &world_cam, options: &world_opt });
+                let ui = u.map(|s| sys::aicb_layer { scene: s.single(), camera: &ui_cam, options: &ui_opt });
+                single(world.as_ref().map_or(core::ptr::null(), |l| l), ui.as_ref().map_or(core::ptr::null(), |l| l))
+            }
+            Backend::Group(_) => {
+                let world = w.map(|s| sys::aicb_group_layer { scene: s.grouped(), camera: &world_cam, options: &world_opt });
+                let ui = u.map(|s| sys::aicb_group_layer { scene: s.grouped(), camera: &ui_cam, options: &ui_opt });
+                group(world.as_ref().map_or(core::ptr::null(), |l| l), ui.as_ref().map_or(core::ptr::null(), |l| l))
+            }
+        }
     }
 
     /// The body of `RaytraceToTexture::do_some_tracing` (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) for one
@@ -236,38 +372,33 @@ impl B200Renderer {
             .pre_scale(0., 0., depth_scale)
             .to_array();
 
-        let world_cam = camera_of(&cams.world);
-        let world_opt = options_of(cams.world.options());
-        let ui_cam = camera_of(&cams.ui);
-        let ui_opt = options_of(cams.ui.options());
-        let world = self.layers.world.as_ref().map(|f| sys::aicb_layer { scene: f.scene, camera: &world_cam, options: &world_opt });
-        let ui = self.layers.ui.as_ref().map(|f| sys::aicb_layer { scene: f.scene, camera: &ui_cam, options: &ui_opt });
         let backdrop: Rgba = self.cameras.ui_view_state().backdrop;
         let backdrop_arr: [f32; 4] = backdrop.into();
+        let backdrop_ptr: *const [f32; 4] = if backdrop == Rgba::TRANSPARENT { core::ptr::null() } else { &backdrop_arr };
         let no_world: [f32; 4] = palette::NO_WORLD_TO_SHOW.into();
         let n = pixels.map_or(color.len(), <[u32]>::len);
         assert!(color.len() >= n && depth.len() >= n, "output slices shorter than the batch");
+        let list = pixels.map_or(core::ptr::null(), <[u32]>::as_ptr);
+        let (color, depth) = (color.as_mut_ptr(), depth.as_mut_ptr());
 
         let mut info = sys::aicb_render_info::default();
-        check(unsafe {
-            sys::aicb_render_layers_texture(
-                world.as_ref().map_or(core::ptr::null(), |l| l),
-                ui.as_ref().map_or(core::ptr::null(), |l| l),
-                if backdrop == Rgba::TRANSPARENT { core::ptr::null() } else { &backdrop_arr },
-                &no_world,
-                &depth_transform,
-                pixels.map_or(core::ptr::null(), <[u32]>::as_ptr),
-                n,
-                color.as_mut_ptr(),
-                depth.as_mut_ptr(),
-                &mut info,
-            )
-        })?;
+        let info_ptr: *mut sys::aicb_render_info = &mut info;
+        check(self.with_layers(
+            cams,
+            |world, ui| unsafe {
+                sys::aicb_render_layers_texture(world, ui, backdrop_ptr, &no_world, &depth_transform, list, n, color, depth,
+                                                info_ptr)
+            },
+            |world, ui| unsafe {
+                sys::aicb_group_render_layers_texture(world, ui, backdrop_ptr, &no_world, &depth_transform, list, n, color,
+                                                      depth, info_ptr)
+            },
+        ))?;
         Ok(info)
     }
 
     fn sync_layer(
-        ctx: &B200Context,
+        backend: &Backend,
         slot: &mut Option<SceneFollower>,
         space: Option<&Handle<Space>>,
         ticket: ReadTicket<'_>,
@@ -279,7 +410,7 @@ impl B200Renderer {
             (None, slot) => *slot = None,
         }
         match slot {
-            Some(follower) => follower.update(ctx, ticket),
+            Some(follower) => follower.update(backend, ticket),
             None => Ok(false),
         }
     }
@@ -290,8 +421,8 @@ impl HeadlessRenderer for B200Renderer {
         self.had_cursor = cursor.is_some(); // the raytracer does not draw the cursor either (renderer.rs:104-105)
         self.cameras.update(read_tickets);
         let world_space = self.cameras.world_space().get();
-        Self::sync_layer(&self.ctx, &mut self.layers.world, Option::as_ref(&world_space), read_tickets.world)?;
-        Self::sync_layer(&self.ctx, &mut self.layers.ui, self.cameras.ui_space(), read_tickets.ui)?;
+        Self::sync_layer(&self.backend, &mut self.layers.world, Option::as_ref(&world_space), read_tickets.world)?;
+        Self::sync_layer(&self.backend, &mut self.layers.ui, self.cameras.ui_space(), read_tickets.ui)?;
         Ok(())
     }
 
@@ -301,31 +432,26 @@ impl HeadlessRenderer for B200Renderer {
             let size = cams.world.viewport().framebuffer_size;
             let mut data = vec![[0u8; 4]; (size.width as usize) * (size.height as usize)];
 
-            let world_cam = camera_of(&cams.world);
-            let world_opt = options_of(cams.world.options());
-            let ui_cam = camera_of(&cams.ui);
-            let ui_opt = options_of(cams.ui.options());
-            let world = self.layers.world.as_ref().map(|f| sys::aicb_layer { scene: f.scene, camera: &world_cam, options: &world_opt });
-            let ui = self.layers.ui.as_ref().map(|f| sys::aicb_layer { scene: f.scene, camera: &ui_cam, options: &ui_opt });
-
             // StandardCameras' UiViewState::backdrop (renderer.rs:235-252) and palette::NO_WORLD_TO_SHOW (:474-477)
             let backdrop: Rgba = self.cameras.ui_view_state().backdrop;
             let backdrop_arr: [f32; 4] = backdrop.into();
+            let backdrop_ptr: *const [f32; 4] = if backdrop == Rgba::TRANSPARENT { core::ptr::null() } else { &backdrop_arr };
             let no_world: [f32; 4] = palette::NO_WORLD_TO_SHOW.into();
 
             let mut info = sys::aicb_render_info::default();
-            if world.is_some() || ui.is_some() {
-                check(unsafe {
-                    sys::aicb_render_layers_srgb8(
-                        world.as_ref().map_or(core::ptr::null(), |l| l),
-                        ui.as_ref().map_or(core::ptr::null(), |l| l),
-                        if backdrop == Rgba::TRANSPARENT { core::ptr::null() } else { &backdrop_arr },
-                        &no_world,
-                        data.as_mut_ptr(),
-                        data.len(),
-                        &mut info,
-                    )
-                })
+            if self.layers.world.is_some() || self.layers.ui.is_some() {
+                let (out, out_len) = (data.as_mut_ptr(), data.len());
+                let info_ptr: *mut sys::aicb_render_info = &mut info;
+                // on a group: aicb_group_render_layers_srgb8, the same pixels from every device
+                check(self.with_layers(
+                    cams,
+                    |world, ui| unsafe {
+                        sys::aicb_render_layers_srgb8(world, ui, backdrop_ptr, &no_world, out, out_len, info_ptr)
+                    },
+                    |world, ui| unsafe {
+                        sys::aicb_group_render_layers_srgb8(world, ui, backdrop_ptr, &no_world, out, out_len, info_ptr)
+                    },
+                ))
                 .map_err(to_render_error)?;
             } else {
                 // no Space at all: every accumulator is painted NO_WORLD_TO_SHOW (renderer.rs:474-477)

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 3
+#define AICB_ABI_VERSION 4
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -349,6 +349,35 @@ aicb_status aicb_group_scene_update_cubes(aicb_group_scene *, const int32_t (*cu
 /* == draw_rgba on the whole group: out_len must be fb_width * fb_height. */
 aicb_status aicb_group_render_srgb8(aicb_group_scene *, const aicb_camera *, const aicb_options *,
                                     uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
+/* aicb_scene_update_blocks (SpaceChange::BlockEvaluation / BlockIndex, updating.rs:128-150) and aicb_scene_upload_light
+ * on every replica.  The update is validated against replica 0 first: a rejected call changes no replica. */
+aicb_status aicb_group_scene_update_blocks(aicb_group_scene *, const uint16_t *indices, const aicb_block_desc *descs,
+                                           size_t n);
+aicb_status aicb_group_scene_upload_light(aicb_group_scene *, const uint8_t (*light)[4], size_t n_texels);
+
+/* == RtScene::trace_ray_through_layers + draw_rgba (renderer.rs:454-478, 282-308) and RaytraceToTexture::do_some_tracing's
+ * trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) on the whole group: the arguments, the validation and
+ * the outputs of aicb_render_layers_srgb8 / aicb_render_layers_texture, bit for bit, with group scenes in place of
+ * scenes; both layers must be scenes of the same group (AICB_ERR_INVALID otherwise).  A whole frame or texture is cut
+ * into interleaved 16-row strips as aicb_group_render_srgb8 cuts it; a pixel list into contiguous ranges of whole
+ * 32-entry warps, one per device (a list of fewer than 32 x devices entries uses fewer devices).  Every device stores
+ * its outputs straight into device 0's buffers, in framebuffer or list order.  Each pass (UI, then world) is issued on
+ * every device before any device's pass is waited for; a pass whose hit stream overflowed is re-issued on that device
+ * alone.  aicb_render_info: counters summed over the devices, times = the slowest device's, its passes summed. */
+typedef struct aicb_group_layer {
+    aicb_group_scene *scene;
+    const aicb_camera *camera;
+    const aicb_options *options;
+} aicb_group_layer;
+aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world_or_null, const aicb_group_layer *ui_or_null,
+                                           const float backdrop_rgba[4], const float no_world_rgba[4],
+                                           uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
+aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world_or_null, const aicb_group_layer *ui_or_null,
+                                             const float backdrop_rgba[4], const float no_world_rgba[4],
+                                             const double depth_transform[16],
+                                             const uint32_t *pixels_or_null, size_t n_pixels,
+                                             uint16_t (*out_rgba16f)[4], float *out_depth,
+                                             aicb_render_info *info_or_null);
 
 /* == SpaceRaytracer::trace_ray (sr.rs:113-120) for a batch of explicit rays:
  * origin_dir[i] = {ox,oy,oz,dx,dy,dz}. Output as aicb_render_colorbuf. */
