@@ -911,30 +911,24 @@ class DeviceGroup:
 
     def update(self, space: "Space"):
         if self.scene:
-            load_library().aicb_group_scene_destroy(self.scene)
-            self.scene = None
-        desc, keep = space.to_desc()
-        h = C.c_void_p()
-        _check(load_library().aicb_group_scene_create(self.handle, C.byref(desc), C.byref(h)))
-        del keep
-        self.scene = h
+            self.scene.close()
+            self.scenes.remove(self.scene)
+        self.scene = self.add_scene(space)
 
     def draw(self, camera: "Camera", options: "GraphicsOptions") -> "Rendering":
         w, h = camera.data.fb_width, camera.data.fb_height
         out = np.zeros((h, w, 4), dtype=np.uint8)
         info = abi.RenderInfo()
         o = options.to_abi(True)
-        _check(load_library().aicb_group_render_srgb8(self.scene, C.byref(camera.data), C.byref(o), out.ctypes.data, w * h,
-                                                     C.byref(info)))
+        _check(load_library().aicb_group_render_srgb8(self.scene.handle if self.scene else None, C.byref(camera.data),
+                                                     C.byref(o), out.ctypes.data, w * h, C.byref(info)))
         return Rendering((w, h), out, int(info.flaws), RenderInfo.from_abi(info))
 
     def close(self):
-        if self.scene:
-            load_library().aicb_group_scene_destroy(self.scene)
-            self.scene = None
         for s in self.scenes:
             s.close()
         self.scenes = []
+        self.scene = None
         if self.handle:
             load_library().aicb_group_destroy(self.handle)
             self.handle = None

@@ -323,10 +323,9 @@ static aicb_status ensure(void **p, size_t *cur, size_t want) {
 
 aicb_status aicb_ensure_device(void **p, size_t *cur, size_t want) { return ensure(p, cur, want); }
 
-// Launches the trace kernel on `stream`. Camera rays when cam != NULL, explicit rays otherwise.
+// Launches the trace kernel on `stream`. Camera rays when cam != NULL, the explicit rays of `out` otherwise.
 static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const aicb_options *opt,
-                                const aicb_shard *shard, const double *d_rays, uint64_t n_rays, const Outputs &out,
-                                bool aux, cudaStream_t stream) {
+                                const aicb_shard *shard, const Outputs &out, cudaStream_t stream) {
     aicb_ctx *ctx = sc->ctx;
     TraceParams P;
     std::memset(&P, 0, sizeof P);
@@ -362,15 +361,15 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         }
     } else {
         P.exposure = 1.0f;
-        P.rays = d_rays;
-        P.n_rays = n_rays;
-        if (n_rays > 0xffffffffull) return fail(AICB_ERR_INVALID, "too many rays");
-        P.tiles_x = (uint32_t)((n_rays + 31) / 32);
+        P.rays = out.rays;
+        P.n_rays = out.n_rays;
+        if (out.n_rays > 0xffffffffull) return fail(AICB_ERR_INVALID, "too many rays");
+        P.tiles_x = (uint32_t)((out.n_rays + 31) / 32);
         P.tiles_y = 1;
-        P.n_tasks = (uint32_t)n_rays;
+        P.n_tasks = (uint32_t)out.n_rays;
         P.shard_count = 1;
         P.strip_rows = 1;
-        pixels = n_rays;
+        pixels = out.n_rays;
     }
     P.fog = opt->fog;
     P.lighting = opt->lighting_display;
@@ -535,7 +534,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.bin_count = Q.task_counter + 4;
             Q.debug_warp_times = nullptr;
         }
-        kernel_fn k = select_kernel(volumetric, sc->ds.wide_cells != 0, aux);
+        kernel_fn k = select_kernel(volumetric, sc->ds.wide_cells != 0, out.aux);
         int blocks_per_sm = 0;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k, WARPS_PER_BLOCK * 32, 0));
         if (blocks_per_sm < 1) blocks_per_sm = 1;
@@ -1143,8 +1142,8 @@ size_t aicb_shard_pixel_count(const aicb_camera *cam, const aicb_shard *shard) {
     return (size_t)cam->fb_width * shard_rows(cam->fb_height, shard);
 }
 
-static aicb_status check_render_args(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
-                                     const aicb_shard *shard, size_t out_len) {
+aicb_status aicb_check_render_args(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
+                                   const aicb_shard *shard, size_t out_len) {
     if (!s || !cam) return fail(AICB_ERR_INVALID, "NULL argument");
     aicb_status st = validate_options(opt);
     if (st != AICB_OK) return st;
@@ -1156,7 +1155,7 @@ static aicb_status check_render_args(aicb_scene *s, const aicb_camera *cam, cons
 
 aicb_status aicb_render_srgb8(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
                               uint8_t (*out)[4], size_t out_len, aicb_render_info *info) {
-    aicb_status st = check_render_args(s, cam, opt, shard, out_len);
+    aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
     aicb_ctx *ctx = s->ctx;
@@ -1164,8 +1163,8 @@ aicb_status aicb_render_srgb8(aicb_scene *s, const aicb_camera *cam, const aicb_
     CU(cudaSetDevice(ctx->device));
     st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 4 + 16);
     if (st != AICB_OK) return st;
-    Outputs o;
-    o.srgb8 = (uchar4 *)ctx->d_out;
+    FramePart part{s, shard};
+    part.out.srgb8 = (uchar4 *)ctx->d_out;
     // A pageable destination (a Rust Vec<[u8; 4]>, a numpy array) cannot take an asynchronous DMA: the frame goes to a
     // pinned staging buffer of the library's and is copied out by the host.  Pinned / registered memory is written directly.
     bool staged = false;
@@ -1182,23 +1181,20 @@ aicb_status aicb_render_srgb8(aicb_scene *s, const aicb_camera *cam, const aicb_
             ctx->h_stage_bytes = out_len * 4;
         }
     }
-    void *dst = staged ? ctx->h_stage : (void *)out;
-    for (int attempt = 0;; attempt++) {
-        st = launch_trace(s, cam, opt, shard, nullptr, 0, o, false, ctx->stream);
-        if (st != AICB_OK) return st;
-        // the copy is queued behind the frame: one host synchronisation per call
-        if (out_len) CU(cudaMemcpyAsync(dst, ctx->d_out, out_len * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        st = finish(s, info);
-        if (st != AICB_ERR_RETRY) break;   // (the capacity grows x4 per retry and ends in AICB_ERR_OOM at its cap)
-    }
-    if (st == AICB_OK && staged && out_len) std::memcpy(out, ctx->h_stage, out_len * 4);
-    return st;
+    // the copy is queued behind the frame: one host synchronisation per call
+    part.copy_to = staged ? ctx->h_stage : (void *)out;
+    part.copy_from = ctx->d_out;
+    part.copy_bytes = out_len * 4;
+    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
+    if (st != AICB_OK) return st;
+    if (staged && out_len) std::memcpy(out, ctx->h_stage, out_len * 4);
+    if (info) *info = part.info;
+    return AICB_OK;
 }
 
 aicb_status aicb_render_rgba16f(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
                                 uint16_t (*out)[4], size_t out_len, aicb_render_info *info) {
-    aicb_status st = check_render_args(s, cam, opt, shard, out_len);
+    aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
     aicb_ctx *ctx = s->ctx;
@@ -1206,17 +1202,15 @@ aicb_status aicb_render_rgba16f(aicb_scene *s, const aicb_camera *cam, const aic
     CU(cudaSetDevice(ctx->device));
     st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 8 + 16);
     if (st != AICB_OK) return st;
-    Outputs o;
-    o.rgba16f = (uint2 *)ctx->d_out;
-    for (int attempt = 0;; attempt++) {
-        st = launch_trace(s, cam, opt, shard, nullptr, 0, o, false, ctx->stream);
-        if (st != AICB_OK) return st;
-        if (out_len) CU(cudaMemcpyAsync(out, ctx->d_out, out_len * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        st = finish(s, info);
-        if (st != AICB_ERR_RETRY) break;
-    }
-    return st;
+    FramePart part{s, shard};
+    part.out.rgba16f = (uint2 *)ctx->d_out;
+    part.copy_to = out;
+    part.copy_from = ctx->d_out;
+    part.copy_bytes = out_len * 8;
+    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
+    if (st != AICB_OK) return st;
+    if (info) *info = part.info;
+    return AICB_OK;
 }
 
 static aicb_status render_aux(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
@@ -1229,19 +1223,18 @@ static aicb_status render_aux(aicb_scene *s, const aicb_camera *cam, const aicb_
     aicb_status st = ensure(&ctx->d_aux, &ctx->d_aux_bytes, total);
     if (st != AICB_OK) return st;
     char *base = (char *)ctx->d_aux;
-    Outputs o;
+    FramePart part{s, shard};
+    Outputs &o = part.out;
     o.colorbuf = (float4 *)(base + off_cb);
     o.depth = (double *)(base + off_depth);
     o.hit = (aicb_hit *)(base + off_hit);
     o.steps = (uint32_t *)(base + off_steps);
-    for (int attempt = 0;; attempt++) {
-        st = launch_trace(s, cam, opt, shard, d_rays, n_rays, o, true, ctx->stream);
-        if (st != AICB_OK) return st;
-        CU(cudaStreamSynchronize(ctx->stream));
-        st = finish(s, info);
-        if (st != AICB_ERR_RETRY) break;
-    }
+    o.rays = d_rays;
+    o.n_rays = n_rays;
+    o.aux = true;
+    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
     if (st != AICB_OK) return st;
+    if (info) *info = part.info;
     if (n) {
         if (out_cb) CU(cudaMemcpyAsync(out_cb, o.colorbuf, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
         if (depth) CU(cudaMemcpyAsync(depth, o.depth, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1255,7 +1248,7 @@ static aicb_status render_aux(aicb_scene *s, const aicb_camera *cam, const aicb_
 aicb_status aicb_render_colorbuf(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
                                  const aicb_shard *shard, float (*out_cb)[4], double *depth, aicb_hit *hit,
                                  uint32_t *steps, size_t out_len, aicb_render_info *info) {
-    aicb_status st = check_render_args(s, cam, opt, shard, out_len);
+    aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
@@ -1264,20 +1257,20 @@ aicb_status aicb_render_colorbuf(aicb_scene *s, const aicb_camera *cam, const ai
 
 aicb_status aicb_render_srgb8_device(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
                                      const aicb_shard *shard, void *d_out, size_t out_len, void *stream) {
-    aicb_status st = check_render_args(s, cam, opt, shard, out_len);
+    aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !d_out) return fail(AICB_ERR_INVALID, "d_out is NULL");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     Outputs o;
     o.srgb8 = (uchar4 *)d_out;
-    return launch_trace(s, cam, opt, shard, nullptr, 0, o, false, stream ? (cudaStream_t)stream : s->ctx->stream);
+    return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream);
 }
 
 aicb_status aicb_render_srgb8_device_frame(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
                                            const aicb_shard *shard, void *d_frame, size_t frame_len, void *stream) {
     if (!s || !cam) return fail(AICB_ERR_INVALID, "NULL argument");
-    aicb_status st = check_render_args(s, cam, opt, shard, aicb_shard_pixel_count(cam, shard));
+    aicb_status st = aicb_check_render_args(s, cam, opt, shard, aicb_shard_pixel_count(cam, shard));
     if (st != AICB_OK) return st;
     if (frame_len != (size_t)cam->fb_width * cam->fb_height)
         return fail(AICB_ERR_INVALID, "Viewport size does not match frame buffer length");
@@ -1287,7 +1280,7 @@ aicb_status aicb_render_srgb8_device_frame(aicb_scene *s, const aicb_camera *cam
     Outputs o;
     o.full_frame = true;
     o.srgb8 = (uchar4 *)d_frame;
-    return launch_trace(s, cam, opt, shard, nullptr, 0, o, false, stream ? (cudaStream_t)stream : s->ctx->stream);
+    return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream);
 }
 
 // ---- full-frame buffers shared between ranks (CUDA IPC) ------------------------------------------
@@ -1432,7 +1425,7 @@ aicb_status aicb_frame_read(aicb_ctx *ctx, const void *d_frame, uint8_t (*out)[4
 // == print_space's per-pixel CharacterBuf (raytracer/text.rs:52-123, 139-180): which block each pixel shows.
 aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, int32_t *out, size_t out_len,
                              aicb_render_info *info) {
-    aicb_status st = check_render_args(s, cam, opt, nullptr, out_len);
+    aicb_status st = aicb_check_render_args(s, cam, opt, nullptr, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
     aicb_ctx *ctx = s->ctx;
@@ -1440,16 +1433,11 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
     CU(cudaSetDevice(ctx->device));
     st = ensure(&ctx->d_aux, &ctx->d_aux_bytes, out_len * 4 + 16);
     if (st != AICB_OK) return st;
-    Outputs o;
-    o.text = (int32_t *)ctx->d_aux;
-    for (;;) {
-        st = launch_trace(s, cam, opt, nullptr, nullptr, 0, o, false, ctx->stream);
-        if (st != AICB_OK) return st;
-        CU(cudaStreamSynchronize(ctx->stream));
-        st = finish(s, info);
-        if (st != AICB_ERR_RETRY) break;
-    }
+    FramePart part{s};
+    part.out.text = (int32_t *)ctx->d_aux;
+    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
     if (st != AICB_OK) return st;
+    if (info) *info = part.info;
     if (out_len) CU(cudaMemcpy(out, ctx->d_aux, out_len * 4, cudaMemcpyDeviceToHost));
     return AICB_OK;
 }
@@ -1468,7 +1456,7 @@ aicb_status aicb_check_layers(const aicb_layer *world, const aicb_layer *ui, con
         if (world->camera->fb_width != ui->camera->fb_width || world->camera->fb_height != ui->camera->fb_height)
             return fail(AICB_ERR_INVALID, "the layers' cameras must share the framebuffer size");
     }
-    aicb_status st = check_render_args(lead->scene, lead->camera, lead->options, nullptr, out_len);
+    aicb_status st = aicb_check_render_args(lead->scene, lead->camera, lead->options, nullptr, out_len);
     if (st != AICB_OK) return st;
     if (have_ui && have_world) {
         st = validate_options(ui->options);
@@ -1478,15 +1466,60 @@ aicb_status aicb_check_layers(const aicb_layer *world, const aicb_layer *ui, con
     return AICB_OK;
 }
 
+// RaytraceInfo of several passes (renderer.rs:555): counters add up.  Times add up over the passes of one part, which
+// run one after another; over the parts of a frame, which run side by side, the frame took as long as its slowest part.
+void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part) {
+    auto time = [same_part](float t, float u) { return same_part ? t + u : std::max(t, u); };
+    sum->cubes_traced += one->cubes_traced;
+    sum->rays += one->rays;
+    sum->algorithmic_bytes += one->algorithmic_bytes;
+    for (int k = 0; k < 6; k++) sum->counters[k] += one->counters[k];
+    sum->kernel_ms = time(sum->kernel_ms, one->kernel_ms);
+    for (int k = 0; k < 4; k++) sum->stage_ms[k] = time(sum->stage_ms[k], one->stage_ms[k]);
+    sum->flaws |= one->flaws;
+}
+
+// A pass is issued on every part before any part's pass is finished, so that the devices of a group overlap; a context
+// tracks one frame (finish), so its next pass waits until this one is finished.  finish decides whether a part's hit
+// stream overflowed and raises that context's capacity (x4 per retry, AICB_ERR_OOM at the cap); such a part is
+// re-issued alone.  With want_info, each finished pass is added to its part's info; without, finish skips its event
+// queries, as a caller that passes no aicb_render_info expects.  The caller holds the parts' contexts' locks.
+aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
+                            bool want_info) {
+    std::vector<size_t> todo(n_parts), again;
+    for (size_t i = 0; i < n_parts; i++) todo[i] = i;
+    while (!todo.empty()) {
+        for (size_t i : todo) {
+            const FramePart &p = parts[i];
+            aicb_ctx *ctx = p.scene->ctx;
+            CU(cudaSetDevice(ctx->device));
+            aicb_status r = launch_trace(p.scene, cam, opt, p.shard, p.out, ctx->stream);
+            if (r != AICB_OK) return r;
+            if (p.copy_bytes)
+                CU(cudaMemcpyAsync(p.copy_to, p.copy_from, p.copy_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        }
+        again.clear();
+        for (size_t i : todo) {
+            aicb_scene *sc = parts[i].scene;
+            CU(cudaSetDevice(sc->ctx->device));
+            CU(cudaStreamSynchronize(sc->ctx->stream));
+            aicb_render_info one{};
+            aicb_status r = finish(sc, want_info ? &one : nullptr);
+            if (r == AICB_ERR_RETRY) { again.push_back(i); continue; }
+            if (r != AICB_OK) return r;
+            aicb_merge_info(&parts[i].info, &one, true);
+        }
+        todo.swap(again);
+    }
+    return AICB_OK;
+}
+
 // RtScene::trace_ray_through_layers for every pixel task of every part (renderer.rs:454-478): the UI layer's Space is
 // traced first (its own camera, no sky), the backdrop colour is added, the world layer continues in the same
 // accumulator (its rays start opaque where the UI covered the pixel), and a pixel that is not opaque in the end — there
 // is no world — is painted NO_WORLD_TO_SHOW.  The last pass writes each part's target; with texture targets the UI pass
-// hands its DepthBuf on next to its ColorBuf.
-// A pass is issued on every part before any part's pass is finished, so that the devices of a group overlap; a context
-// tracks one frame (finish), so its next pass waits until this one is finished.  A part whose hit stream overflowed
-// (finish has raised that context's capacity) is re-issued alone, that pass only.  A part's info sums its passes;
-// `total` sums the parts' counters and takes the slowest part's times.  The caller holds the parts' contexts' locks.
+// hands its DepthBuf on next to its ColorBuf.  Each pass runs on every part through aicb_trace_pass (a re-issued world
+// pass starts from the same accumulator).  The caller holds the parts' contexts' locks.
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
                               const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
@@ -1512,44 +1545,18 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         for (int i = 0; i < 3; i++) no_world[i] = no_world_rgba[i] * no_world_rgba[3];
         no_world[3] = 1.0f - no_world_rgba[3];
     }
-    auto add_info = [](aicb_render_info &sum, const aicb_render_info &one) {
-        sum.cubes_traced += one.cubes_traced;
-        sum.rays += one.rays;
-        sum.algorithmic_bytes += one.algorithmic_bytes;
-        for (int k = 0; k < 6; k++) sum.counters[k] += one.counters[k];
-        sum.kernel_ms += one.kernel_ms;
-        for (int k = 0; k < 4; k++) sum.stage_ms[k] += one.stage_ms[k];
-        sum.flaws |= one.flaws;
-    };
-    // one pass of the frame on every part: `layer` picks the part's scene, `outputs(part, ctx)` its Outputs
+    // one pass of the frame on every part: `layer` picks the part's scene, `outputs(part, ctx)` its Outputs; each
+    // part's info sums its passes
+    std::vector<FramePart> pass_parts(n_parts);
     auto pass = [&](aicb_scene *LayerPart::*layer, const aicb_camera *cam, const aicb_options *opt,
                     auto outputs) -> aicb_status {
-        std::vector<size_t> todo(n_parts), again;
-        for (size_t i = 0; i < n_parts; i++) todo[i] = i;
-        while (!todo.empty()) {
-            for (size_t i : todo) {
-                aicb_scene *sc = parts[i].*layer;
-                CU(cudaSetDevice(sc->ctx->device));
-                aicb_status r = launch_trace(sc, cam, opt, &parts[i].shard, nullptr, 0, outputs(parts[i], sc->ctx), false,
-                                             sc->ctx->stream);
-                if (r != AICB_OK) return r;
-            }
-            again.clear();
-            for (size_t i : todo) {
-                aicb_scene *sc = parts[i].*layer;
-                CU(cudaSetDevice(sc->ctx->device));
-                CU(cudaStreamSynchronize(sc->ctx->stream));
-                aicb_render_info one;
-                aicb_status r = finish(sc, &one);
-                if (r == AICB_ERR_RETRY) { again.push_back(i); continue; }   // (x4 per retry, AICB_ERR_OOM at the cap)
-                if (r != AICB_OK) return r;
-                add_info(parts[i].info, one);
-            }
-            todo.swap(again);
+        for (size_t i = 0; i < n_parts; i++) {
+            pass_parts[i].scene = parts[i].*layer;
+            pass_parts[i].shard = &parts[i].shard;
+            pass_parts[i].out = outputs(parts[i], pass_parts[i].scene->ctx);
         }
-        return AICB_OK;
+        return aicb_trace_pass(pass_parts.data(), n_parts, cam, opt, true);
     };
-    for (size_t i = 0; i < n_parts; i++) std::memset(&parts[i].info, 0, sizeof parts[i].info);
     if (have_ui && have_world) {
         for (size_t i = 0; i < n_parts; i++) {
             aicb_ctx *ctx = parts[i].world->ctx;
@@ -1621,18 +1628,8 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         });
     }
     if (st != AICB_OK) return st;
-    // RaytraceInfo: summed over the parts (renderer.rs:555); the frame took as long as its slowest part
     std::memset(total, 0, sizeof *total);
-    for (size_t i = 0; i < n_parts; i++) {
-        const aicb_render_info &one = parts[i].info;
-        total->cubes_traced += one.cubes_traced;
-        total->rays += one.rays;
-        total->algorithmic_bytes += one.algorithmic_bytes;
-        for (int k = 0; k < 6; k++) total->counters[k] += one.counters[k];
-        total->kernel_ms = std::max(total->kernel_ms, one.kernel_ms);
-        for (int k = 0; k < 4; k++) total->stage_ms[k] = std::max(total->stage_ms[k], one.stage_ms[k]);
-        total->flaws |= one.flaws;
-    }
+    for (const FramePart &p : pass_parts) aicb_merge_info(total, &p.info, false);
     return AICB_OK;
 }
 
@@ -1831,17 +1828,15 @@ aicb_status aicb_render_orthographic(aicb_scene *s, uint32_t resolution, uint8_t
                 opt.maximum_intensity = INFINITY;
                 opt.view_distance = 200.0;
                 opt.include_sky = 1;
-                Outputs o;
-                o.srgb8 = (uchar4 *)ctx->d_out;
-                for (;;) {
-                    st = launch_trace(s, nullptr, &opt, nullptr, d_rays, n, o, false, ctx->stream);
-                    if (st != AICB_OK) break;
-                    e = cudaStreamSynchronize(ctx->stream);
-                    if (e != cudaSuccess) break;
-                    st = finish(s, info);
-                    if (st != AICB_ERR_RETRY) break;
+                FramePart part{s};
+                part.out.srgb8 = (uchar4 *)ctx->d_out;
+                part.out.rays = d_rays;
+                part.out.n_rays = n;
+                st = aicb_trace_pass(&part, 1, nullptr, &opt, info != nullptr);
+                if (st == AICB_OK) {
+                    if (info) *info = part.info;
+                    e = cudaMemcpy(px.data(), ctx->d_out, n * 4, cudaMemcpyDeviceToHost);
                 }
-                if (st == AICB_OK && e == cudaSuccess) e = cudaMemcpy(px.data(), ctx->d_out, n * 4, cudaMemcpyDeviceToHost);
             }
         }
         cudaFree(d_rays);

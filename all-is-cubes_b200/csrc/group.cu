@@ -7,8 +7,8 @@
 // chain per device, there is no collective and no host thread per GPU.
 // Replaces the Rayon rows x pixels dispatch of trace_scene_to_image_impl (renderer.rs:516-556) across devices.
 // Layered frames and texture targets (aicb_group_render_layers_*) cut the work the same way, or a pixel list into
-// ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu), which issues each pass on every device
-// before it waits for any.
+// ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu).  Every call issues a pass on every
+// device before it waits for any, and re-issues it on a device whose hit stream overflowed (aicb_trace_pass).
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -90,7 +90,7 @@ static aicb_status join(aicb_group *g, size_t n_parts) {
     return AICB_OK;
 }
 
-// The contexts' locks, for the whole of a layered call (its passes run on every context).
+// The contexts' locks, for the whole of a frame (its passes run on every context).
 struct GroupLock {
     std::vector<std::unique_lock<std::mutex>> locks;
     explicit GroupLock(aicb_group *g) {
@@ -203,50 +203,32 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
     const size_t pixels = (size_t)cam->fb_width * cam->fb_height;
     if (out_len != pixels) return aicb_fail(AICB_ERR_INVALID, "Viewport size does not match output buffer length");
     if (pixels && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
-    const uint32_t n = (uint32_t)g->ctx.size();
+    aicb_status st = aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len);
+    if (st != AICB_OK) return st;
+    GroupLock lock(g);
     aicb_ctx *root = g->ctx[0];
     CU(cudaSetDevice(root->device));
-    aicb_status fst = ensure_frame(g, pixels);
-    if (fst != AICB_OK) return fst;
-    for (int attempt = 0;; attempt++) {
-        // every device renders its strips into the root's frame; nothing here waits for a GPU
-        for (uint32_t i = 0; i < n; i++) {
-            aicb_shard sh;
-            sh.strip_rows = GROUP_STRIP_ROWS;
-            sh.index = i;
-            sh.count = n;
-            aicb_status st = aicb_render_srgb8_device_frame(gs->scene[i], cam, opt, &sh, g->d_frame, pixels, nullptr);
-            if (st != AICB_OK) return st;
-            CU(cudaSetDevice(g->ctx[i]->device));
-            CU(cudaEventRecord(g->done[i], g->ctx[i]->stream));
-        }
-        CU(cudaSetDevice(root->device));
-        for (uint32_t i = 1; i < n; i++) CU(cudaStreamWaitEvent(root->stream, g->done[i], 0));
-        if (pixels) CU(cudaMemcpyAsync(out, g->d_frame, pixels * 4, cudaMemcpyDeviceToHost, root->stream));
-        CU(cudaStreamSynchronize(root->stream));
-        // RaytraceInfo: summed over the shards (renderer.rs:555); the frame took as long as its slowest device
-        aicb_render_info total;
-        std::memset(&total, 0, sizeof total);
-        bool retry = false;
-        for (uint32_t i = 0; i < n; i++) {
-            aicb_render_info one;
-            aicb_status st = aicb_render_finish(gs->scene[i], &one);
-            if (st == AICB_ERR_RETRY) { retry = true; continue; }
-            if (st != AICB_OK) return st;
-            total.cubes_traced += one.cubes_traced;
-            total.rays += one.rays;
-            total.algorithmic_bytes += one.algorithmic_bytes;
-            for (int k = 0; k < 6; k++) total.counters[k] += one.counters[k];
-            total.kernel_ms = one.kernel_ms > total.kernel_ms ? one.kernel_ms : total.kernel_ms;
-            for (int k = 0; k < 4; k++) total.stage_ms[k] = one.stage_ms[k] > total.stage_ms[k] ? one.stage_ms[k] : total.stage_ms[k];
-            total.flaws |= one.flaws;
-        }
-        if (!retry) {
-            if (info) *info = total;
-            return AICB_OK;
-        }
-        if (attempt >= 5) return aicb_fail(AICB_ERR_OOM, "hit stream capacity exhausted");
+    st = ensure_frame(g, pixels);
+    if (st != AICB_OK) return st;
+    Outputs target;
+    target.full_frame = true;
+    target.srgb8 = (uchar4 *)g->d_frame;
+    // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
+    const aicb_group_layer world = {gs, cam, opt};
+    const std::vector<LayerPart> strips = strip_parts(g, &world, nullptr, target);
+    std::vector<FramePart> parts;
+    for (const LayerPart &p : strips) parts.push_back({p.world, &p.shard, p.target});
+    st = aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr);
+    if (st != AICB_OK) return st;
+    st = join(g, parts.size());
+    if (st != AICB_OK) return st;
+    if (pixels) CU(cudaMemcpyAsync(out, g->d_frame, pixels * 4, cudaMemcpyDeviceToHost, root->stream));
+    CU(cudaStreamSynchronize(root->stream));
+    if (info) {
+        std::memset(info, 0, sizeof *info);
+        for (const FramePart &p : parts) aicb_merge_info(info, &p.info, false);
     }
+    return AICB_OK;
 }
 
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *gs, const uint16_t *indices, const aicb_block_desc *descs,

@@ -141,6 +141,9 @@ struct Outputs {
     bool texture = false;
     const uint32_t *pixel_list = nullptr;   // device: the pixel tasks (y * fb_width + x), or nullptr for every pixel
     uint32_t n_list = 0;
+    const double *rays = nullptr;           // device: the tasks of a frame without a camera (origin, direction per ray)
+    uint64_t n_rays = 0;
+    bool aux = false;                       // the marching kernel that also counts steps and blocks (render_aux)
     float *tex_depth = nullptr;
     const double *in_depth = nullptr;
     double *out_task_depth = nullptr;
@@ -156,14 +159,28 @@ struct LayerPart {
     aicb_scene *world = nullptr, *ui = nullptr;
     aicb_shard shard = {1, 0, 1};
     Outputs target;
-    aicb_render_info info{};   // this part's passes, summed
+};
+
+// One context's share of one pass of a frame (aicb_trace_pass): the scene it traces, its row strips, where it stores,
+// a device-to-host copy queued behind every issue (if copy_bytes), and its finished passes' info, summed.
+struct FramePart {
+    aicb_scene *scene = nullptr;
+    const aicb_shard *shard = nullptr;   // nullptr: every row
+    Outputs out;
+    void *copy_to = nullptr;
+    const void *copy_from = nullptr;
+    size_t copy_bytes = 0;
+    aicb_render_info info{};
 };
 
 // aicb200.cu: the layer rules shared by aicb_render_layers_* and aicb_group_render_layers_*.  The layers give the
 // cameras and options (their scenes only say which layers exist).  Validation of the arguments of the single-context
-// calls; the texture target's exposures and depth transform; the passes of a frame over every part.  aicb_trace_layers
-// needs the locks of the parts' contexts.  (C linkage: aicb200.cu defines them among the entry points of the C ABI.)
+// calls; the texture target's exposures and depth transform; the passes of a frame over every part, and the one loop
+// that re-issues a pass whose hit stream overflowed (aicb_trace_pass); the one merge of aicb_render_info.  The passes
+// need the locks of the parts' contexts.  (C linkage: aicb200.cu defines them among the entry points of the C ABI.)
 extern "C" {
+aicb_status aicb_check_render_args(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
+                                   const aicb_shard *shard, size_t out_len);
 aicb_status aicb_check_layers(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba, size_t out_len,
                               const aicb_layer **lead_out);
 aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba,
@@ -172,6 +189,9 @@ aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer 
 void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *target);
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
                               const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total);
+aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
+                            bool want_info);
+void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part);
 aicb_status aicb_ensure_device(void **p, size_t *cur, size_t want);
 // aicb_scene_update_blocks' validation alone: AICB_OK if that call would accept the update (changes nothing)
 aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);

@@ -346,7 +346,9 @@ aicb_status aicb_group_scene_create(aicb_group *, const aicb_scene_desc *, aicb_
 void aicb_group_scene_destroy(aicb_group_scene *);
 aicb_status aicb_group_scene_update_cubes(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *block_ids,
                                           const uint8_t (*light)[4], size_t n);
-/* == draw_rgba on the whole group: out_len must be fb_width * fb_height. */
+/* == draw_rgba on the whole group: out_len must be fb_width * fb_height; the options apply as given (include_sky too).
+ * The frame is issued on every device before any is waited for; a device whose hit stream overflowed is re-issued
+ * alone.  The call holds every context of the group until it returns. */
 aicb_status aicb_group_render_srgb8(aicb_group_scene *, const aicb_camera *, const aicb_options *,
                                     uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
 /* aicb_scene_update_blocks (SpaceChange::BlockEvaluation / BlockIndex, updating.rs:128-150) and aicb_scene_upload_light

@@ -1,12 +1,16 @@
 """resolve_kernel (None / Flat lighting: shading and compositing in one pass, one warp per 32 rays, hit lists in
 shared-memory windows of 128 slots): frames in which a warp's hit lists span many windows, against the oracle, the
-choice between it and shade_kernel + encode_kernel, and the stage times a frame reports."""
+choice between it and shade_kernel + encode_kernel, and the stage times a frame reports.  Also: every blocking entry
+point re-issues a frame that overflowed the hit stream and returns what the warmed context returns."""
+import ctypes as C
+
 import numpy as np
 import pytest
 
+import aicb200
 import orc
 from aicb200 import (LIGHT_BOUNCE, LIGHT_FLAT, LIGHT_LINEAR, LIGHT_NONE, TRANSPARENCY_SURFACE, TRANSPARENCY_VOLUMETRIC,
-                     Block, Context, GraphicsOptions, RtRenderer, Space, scenes)
+                     Block, Context, DeviceGroup, GraphicsOptions, RenderInfo, RtRenderer, Space, abi, scenes)
 
 pytestmark = pytest.mark.gpu
 
@@ -27,6 +31,73 @@ def faint_slab():
     x, y, z = np.meshgrid(np.arange(n), np.arange(m), np.arange(m), indexing="ij")
     ids = (1 + (x + y + z) % 2).astype(np.uint16)
     return Space((0, 0, 0), ids, [Block.air(), Block(color=(0.9, 0.5, 0.2, 0.03)), Block(color=(0.2, 0.4, 0.9, 0.02))])
+
+
+def _slab_rays(n=128):
+    """n x n explicit rays along the faint slab's length: each crosses its 40 cubes."""
+    y, z = np.meshgrid(np.linspace(0.25, 21.75, n), np.linspace(0.25, 21.75, n), indexing="ij")
+    d = np.array([1.0, 0.04, 0.03]) / np.linalg.norm([1.0, 0.04, 0.03])
+    return np.column_stack([np.full(n * n, -1.0), y.ravel(), z.ravel(), np.tile(d, (n * n, 1))])
+
+
+def _blocking_call(call, r, group, cam, opts):
+    """One blocking entry point on the faint slab: (its outputs, its RenderInfo)."""
+    if call == "draw":
+        img = r.draw()
+    elif call == "draw_shard":
+        img = r.draw(shard=(16, 1, 2))
+    elif call == "orthographic":
+        img = aicb200.render_orthographic(r.rt, 2)
+    elif call == "group":
+        img = group.draw(cam, opts)
+    elif call == "draw_colorbuf" or call == "trace_rays":
+        d = r.draw_colorbuf() if call == "draw_colorbuf" else r.rt.trace_rays(_slab_rays(), want_depth=True,
+                                                                                want_hit=True, want_steps=True)
+        return [d["colorbuf"], d["depth"], d["hit"], d["steps"]], d["info"]
+    else:   # aicb_render_rgba16f and aicb_render_text (print_space's entry point): their wrappers drop the info
+        lib, info, o, n = aicb200.load_library(), abi.RenderInfo(), r.rt.graphics_options.to_abi(True), r.pixel_count()
+        if call == "draw_rgba16f":
+            out = np.empty((n, 4), dtype=np.float16)
+            st = lib.aicb_render_rgba16f(r.rt.handle, C.byref(cam.data), C.byref(o), None, out.ctypes.data, n,
+                                         C.byref(info))
+        else:
+            out = np.empty(n, dtype=np.int32)
+            st = lib.aicb_render_text(r.rt.handle, C.byref(cam.data), C.byref(o), out.ctypes.data, n, C.byref(info))
+        assert st == abi.OK
+        return [out], RenderInfo.from_abi(info)
+    return [img.data], img.info
+
+
+@pytest.mark.parametrize("call", ["draw", "draw_shard", "draw_rgba16f", "draw_colorbuf", "trace_rays", "orthographic",
+                                  "text", "group"])
+def test_blocking_call_reissues_an_overflowed_frame(call):
+    """Every ray meets 19 to 65 surfaces of the faint slab, more than the 8 hit slots per ray (at least 65536 in all) of
+    a fresh context's hit stream: the first frame overflows it, and the blocking call issues the frame again with a
+    larger stream before it returns.  What it returns must equal the same call's on the warmed context.  `group` is
+    the world-only frame of a two-context DeviceGroup on one device."""
+    space = faint_slab()
+    opts = GraphicsOptions(lighting_display=LIGHT_NONE, transparency=TRANSPARENCY_VOLUMETRIC, view_distance=200.0)
+    cam = scenes.standard_camera(space, opts, 256, 192, direction=(1.0, 0.04, 0.03), distance_scale=0.5)
+    ctx = Context()
+    group = DeviceGroup([0, 0]) if call == "group" else None
+    try:
+        r = RtRenderer(cam, ctx)
+        if group:
+            group.update(space)
+        else:
+            r.update(space)
+        first, info = _blocking_call(call, r, group, cam, opts)
+        assert info.counters[2] > max(8 * info.rays, 1 << 16), info   # surface hits: more than the first stream held
+        again, warm = _blocking_call(call, r, group, cam, opts)
+        for a, b in zip(first, again):
+            assert np.array_equal(a.view(np.uint8), b.view(np.uint8)), call
+        assert (info.cubes_traced, info.rays, info.counters) == (warm.cubes_traced, warm.rays, warm.counters), call
+        if r.rt:
+            r.rt.close()
+    finally:
+        if group:
+            group.close()
+        ctx.close()
 
 
 @pytest.mark.parametrize("antialias", [False, True])
