@@ -107,6 +107,8 @@ def load_library() -> C.CDLL:
     lib.aicb_render_layers_texture.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p,
                                                C.POINTER(C.c_double), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                                C.POINTER(abi.RenderInfo)]
+    lib.aicb_render_layers_terminal.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_ortho_image_size.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
     lib.aicb_render_orthographic.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_create.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_void_p)]
@@ -126,6 +128,8 @@ def load_library() -> C.CDLL:
     lib.aicb_group_render_layers_texture.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
                                                      C.c_void_p, C.POINTER(C.c_double), C.c_void_p, C.c_size_t,
                                                      C.c_void_p, C.c_void_p, C.POINTER(abi.RenderInfo)]
+    lib.aicb_group_render_layers_terminal.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
+                                                      C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_light_chart.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_light_chart.restype = C.c_uint32
     lib.aicb_light_fast_evaluate.argtypes = [C.c_void_p]
@@ -785,6 +789,31 @@ def _layers_texture(fn, cls, world, ui, backdrop, no_world, depth_transform, pix
     return rgba, depth, RenderInfo.from_abi(info)
 
 
+def render_layers_terminal(world=None, ui=None, backdrop=None, no_world=None) -> dict:
+    """The desktop app's terminal frame (all-is-cubes-desktop/src/terminal.rs:114-142): draw::<ColorCharacterBuf>
+    through every layer as render_layers traces them, and ColorCharacterBuf::output per pixel.  Same arguments as
+    render_layers.  Returns a dict: text (int32 [H, W]: block index, or abi.TEXT_*), layer (int32 [H, W]: the layer
+    whose Space a block index belongs to, abi.LAYER_*), rgba (float32 [H, W, 4]: post_process_color(Rgba::from(ColorBuf)),
+    linear) and info (RenderInfo)."""
+    return _layers_terminal(load_library().aicb_render_layers_terminal, abi.Layer, world, ui, backdrop, no_world)
+
+
+def _layers_terminal(fn, cls, world, ui, backdrop, no_world) -> dict:
+    lead = world if world else ui
+    cam = lead[1]
+    w, h = cam.data.fb_width, cam.data.fb_height
+    keep = []
+    out = np.empty((h, w), dtype=[("rgba", np.float32, 4), ("text", np.int32), ("layer", np.int32)])
+    assert out.itemsize == C.sizeof(abi.TerminalPixel)
+    info = abi.RenderInfo()
+    b = np.array(backdrop, dtype=np.float32) if backdrop is not None else None
+    nw = np.array(no_world, dtype=np.float32) if no_world is not None else None
+    _check(fn(_layer_arg(world, keep, cls), _layer_arg(ui, keep, cls), b.ctypes.data if b is not None else None,
+              nw.ctypes.data if nw is not None else None, out.ctypes.data, w * h, C.byref(info)))
+    # views of the pixels as the call stored them (aicb_terminal_pixel, 24 bytes each)
+    return {"text": out["text"], "layer": out["layer"], "rgba": out["rgba"], "info": RenderInfo.from_abi(info)}
+
+
 CENTRAL_PIXEL_LIMIT = 60000   # raytrace_to_texture.rs:877
 
 
@@ -881,9 +910,9 @@ class DeviceGroup:
     """Several GPUs driven from this one process through the C ABI (csrc/group.cu): scene replicated, frame cut into
     interleaved row strips, pixels stored straight into device 0's frame over NVLink.
 
-    update() / draw(): one world-only scene.  add_scene() / render_layers() / render_layers_texture(): any number of
-    replicated scenes (GroupScene) drawn through the layers as the module's render_layers / render_layers_texture draw
-    them on one context."""
+    update() / draw(): one world-only scene.  add_scene() / render_layers() / render_layers_texture() /
+    render_layers_terminal(): any number of replicated scenes (GroupScene) drawn through the layers as the module's
+    functions of the same names draw them on one context."""
 
     def __init__(self, device_ids):
         ids = (C.c_int * len(device_ids))(*[int(d) for d in device_ids])
@@ -908,6 +937,11 @@ class DeviceGroup:
         """render_layers_texture with GroupScenes of this group (same arguments and results)."""
         return _layers_texture(load_library().aicb_group_render_layers_texture, abi.GroupLayer, world, ui, backdrop,
                                no_world, depth_transform, pixels)
+
+    def render_layers_terminal(self, world=None, ui=None, backdrop=None, no_world=None) -> dict:
+        """render_layers_terminal with GroupScenes of this group (same arguments and results)."""
+        return _layers_terminal(load_library().aicb_group_render_layers_terminal, abi.GroupLayer, world, ui, backdrop,
+                                no_world)
 
     def update(self, space: "Space"):
         if self.scene:

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -112,7 +112,13 @@ class GroupLayer(C.Structure):
     _fields_ = [("scene", C.c_void_p), ("camera", C.POINTER(CameraData)), ("options", C.POINTER(Options))]
 
 
-TEXT_ENTERED_SPACE, TEXT_EMPTY, TEXT_INCOMPLETE = -1, -2, -3
+TEXT_ENTERED_SPACE, TEXT_EMPTY, TEXT_INCOMPLETE, TEXT_BLANK = -1, -2, -3, -4
+LAYER_NONE, LAYER_WORLD, LAYER_UI = 0, 1, 2
+
+
+class TerminalPixel(C.Structure):
+    _fields_ = [("rgba", C.c_float * 4), ("text", C.c_int32), ("layer", C.c_int32)]
+
 
 EXPORTED_SYMBOLS = [
     "aicb_abi_version",
@@ -133,6 +139,7 @@ EXPORTED_SYMBOLS = [
     "aicb_render_text",
     "aicb_render_layers_srgb8",
     "aicb_render_layers_texture",
+    "aicb_render_layers_terminal",
     "aicb_ortho_image_size",
     "aicb_render_orthographic",
     "aicb_render_srgb8_device",
@@ -171,4 +178,5 @@ EXPORTED_SYMBOLS = [
     "aicb_group_scene_upload_light",
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",
+    "aicb_group_render_layers_terminal",
 ]

@@ -323,6 +323,19 @@ static aicb_status ensure(void **p, size_t *cur, size_t want) {
 
 aicb_status aicb_ensure_device(void **p, size_t *cur, size_t want) { return ensure(p, cur, want); }
 
+// The compositing kernels of a frame's target (TGT_*): resolve_kernel with None / Flat lighting, encode_kernel after
+// shade_kernel.
+static kernel_fn resolve_for(int lc, int tgt) {
+    switch (tgt) {
+        case TGT_TEX: return lc == LC_NONE ? resolve_kernel<LC_NONE, TGT_TEX> : resolve_kernel<LC_FLAT, TGT_TEX>;
+        case TGT_TERM: return lc == LC_NONE ? resolve_kernel<LC_NONE, TGT_TERM> : resolve_kernel<LC_FLAT, TGT_TERM>;
+        default: return lc == LC_NONE ? resolve_kernel<LC_NONE, TGT_FRAME> : resolve_kernel<LC_FLAT, TGT_FRAME>;
+    }
+}
+static kernel_fn encode_for(int tgt) {
+    return tgt == TGT_TEX ? encode_kernel<TGT_TEX> : (tgt == TGT_TERM ? encode_kernel<TGT_TERM> : encode_kernel<TGT_FRAME>);
+}
+
 // Launches the trace kernel on `stream`. Camera rays when cam != NULL, the explicit rays of `out` otherwise.
 static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const aicb_options *opt,
                                 const aicb_shard *shard, const Outputs &out, cudaStream_t stream) {
@@ -404,6 +417,15 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         P.out_task_depth = out.out_task_depth;
         P.out_tex_depth = out.tex_depth;
     }
+    const bool term = out.terminal;
+    if (term) {
+        P.tex_layer = out.tex_layer;
+        P.out_term = out.term;
+        P.in_text = out.in_text;
+        P.out_task_text = out.out_task_text;
+        P.text_start = out.text_start;
+    }
+    const int tgt = tex ? TGT_TEX : (term ? TGT_TERM : TGT_FRAME);
     P.counters = ctx->d_counters;
     P.task_counter = ctx->d_tile_counter;
     {
@@ -421,7 +443,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     sc->pending = true;
     sc->pending_pixels = pixels;
     sc->pending_rays = pixels * (P.antialias ? 4 : 1);
-    sc->pending_out_bytes_per_pixel = out.srgb8 ? 4 : (tex ? 12 : (out.rgba16f ? 8 : 16));
+    sc->pending_out_bytes_per_pixel = out.srgb8 ? 4 : (tex ? 12 : (term ? 24 : (out.rgba16f ? 8 : 16)));
 
     // ---- the kernels of a frame, chunked so the per-frame streams stay bounded ----------------------------------
     P.n_samples = P.antialias ? 4 : 1;
@@ -524,6 +546,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.out_hit = nullptr; Q.out_steps = nullptr; Q.out_text = nullptr;
             Q.in_accum = nullptr; Q.out_accum = nullptr; Q.has_backdrop = 0; Q.has_no_world = 0;
             Q.pixel_list = nullptr; Q.in_depth = nullptr; Q.out_task_depth = nullptr; Q.out_tex_depth = nullptr;
+            Q.out_term = nullptr; Q.in_text = nullptr; Q.out_task_text = nullptr;
             Q.ray_records = (RayRecord *)ctx->d_rays2;
             Q.task_out = (TaskOut *)ctx->d_task_cb2;
             Q.hits = (HitRecord *)ctx->d_hits2;
@@ -567,13 +590,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             if (stage) cudaEventRecord(ctx->ev_k[2], stream);
             if (fused) {
                 const unsigned rb = (n + 127) / 128;   // one warp per 32 tasks
-                if (tex) {
-                    if (lc == LC_NONE) CU(launch_after(overlap, resolve_kernel<LC_NONE, true>, rb, 128, stream, P, n));
-                    else CU(launch_after(overlap, resolve_kernel<LC_FLAT, true>, rb, 128, stream, P, n));
-                } else {
-                    if (lc == LC_NONE) CU(launch_after(overlap, resolve_kernel<LC_NONE, false>, rb, 128, stream, P, n));
-                    else CU(launch_after(overlap, resolve_kernel<LC_FLAT, false>, rb, 128, stream, P, n));
-                }
+                CU(launch_after(overlap, resolve_for(lc, tgt), rb, 128, stream, P, n));
                 if (stage) cudaEventRecord(ctx->ev_k[3], stream);
             } else if (!bounce) {
                 switch (lc) {
@@ -583,8 +600,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                 }
                 if (stage) cudaEventRecord(ctx->ev_k[3], stream);
                 const uint32_t n_pixels = n / P.n_samples;
-                if (tex) CU(launch_after(overlap, encode_kernel<true>, (n_pixels + 127) / 128, 128, stream, P, n));
-                else CU(launch_after(overlap, encode_kernel<false>, (n_pixels + 127) / 128, 128, stream, P, n));
+                CU(launch_after(overlap, encode_for(tgt), (n_pixels + 127) / 128, 128, stream, P, n));
                 if (stage) cudaEventRecord(ctx->ev_k[4], stream);
             } else {
                 shade_kernel<LC_BOUNCE><<<ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, 0, stream>>>(P);
@@ -600,13 +616,12 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                     gen_kernel<<<tb, 128, 0, stream>>>(Q, n);
                     k<<<(unsigned)grid, WARPS_PER_BLOCK * 32, 0, stream>>>(Q, n);
                     shade_kernel<LC_FLAT><<<ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, 0, stream>>>(Q);
-                    encode_kernel<false><<<tb, 128, 0, stream>>>(Q, n);
+                    encode_kernel<TGT_FRAME><<<tb, 128, 0, stream>>>(Q, n);
                 }
                 bounce_resolve_kernel<<<tb, 128, 0, stream>>>(P, n);
                 if (stage) cudaEventRecord(ctx->ev_k[3], stream);
                 const uint32_t n_pixels = n / P.n_samples;
-                if (tex) encode_kernel<true><<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
-                else encode_kernel<false><<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
+                encode_for(tgt)<<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
                 if (stage) cudaEventRecord(ctx->ev_k[4], stream);
             }
         }
@@ -768,6 +783,7 @@ void aicb_ctx_destroy(aicb_ctx *c) {
     if (c->ev_delta) cudaEventDestroy(c->ev_delta);
     if (c->d_task_aux) cudaFree(c->d_task_aux);
     if (c->d_task_depth) cudaFree(c->d_task_depth);
+    if (c->d_task_text) cudaFree(c->d_task_text);
     aicb_light_ctx_free(c);
     if (c->d_lut) cudaFree(c->d_lut);
     if (c->d_counters) cudaFree(c->d_counters);
@@ -1518,8 +1534,9 @@ aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera 
 // traced first (its own camera, no sky), the backdrop colour is added, the world layer continues in the same
 // accumulator (its rays start opaque where the UI covered the pixel), and a pixel that is not opaque in the end — there
 // is no world — is painted NO_WORLD_TO_SHOW.  The last pass writes each part's target; with texture targets the UI pass
-// hands its DepthBuf on next to its ColorBuf.  Each pass runs on every part through aicb_trace_pass (a re-issued world
-// pass starts from the same accumulator).  The caller holds the parts' contexts' locks.
+// hands its DepthBuf on next to its ColorBuf, with terminal targets its CharacterBuf.  Each pass runs on every part
+// through aicb_trace_pass (a re-issued world pass starts from the same accumulator).  The caller holds the parts'
+// contexts' locks.
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
                               const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
@@ -1567,17 +1584,23 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
                 st = ensure(&ctx->d_task_depth, &ctx->d_task_depth_bytes, n_tasks(parts[i]) * sizeof(double) + 16);
                 if (st != AICB_OK) return st;
             }
+            if (parts[i].target.terminal) {   // the UI pass's CharacterBuf, only when there is a UI layer
+                st = ensure(&ctx->d_task_text, &ctx->d_task_text_bytes, n_tasks(parts[i]) * sizeof(int2) + 16);
+                if (st != AICB_OK) return st;
+            }
         }
         aicb_options ui_opt = *ui->options;
         ui_opt.include_sky = 0;   // ui.trace_ray(.., false)
         st = pass(&LayerPart::ui, ui->camera, &ui_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
-            // the pass that writes no pixel keeps the task layout and the texture mode only
+            // the pass that writes no pixel keeps the task layout and the texture or terminal mode only
             Outputs o;
             o.texture = p.target.texture;
+            o.terminal = p.target.terminal;
             o.pixel_list = p.target.pixel_list;
             o.n_list = p.target.n_list;
             o.tex_layer = TEX_UI;
             if (p.target.texture) o.out_task_depth = (double *)ctx->d_task_depth;
+            if (p.target.terminal) o.out_task_text = (int2 *)ctx->d_task_text;
             o.out_accum = (float4 *)ctx->d_task_aux;
             o.backdrop = have_backdrop ? backdrop : nullptr;
             o.force_antialias = aa;
@@ -1590,6 +1613,7 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
             Outputs o = p.target;
             o.in_accum = (const float4 *)ctx->d_task_aux;   // a re-issued world pass starts from the same accumulator
             if (p.target.texture) o.in_depth = (const double *)ctx->d_task_depth;
+            if (p.target.terminal) o.in_text = (const int2 *)ctx->d_task_text;
             o.tex_layer = TEX_WORLD;
             o.no_world = no_world_rgba ? no_world : nullptr;
             return o;
@@ -1612,7 +1636,10 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
             Outputs o = p.target;
             o.tex_layer = TEX_WORLD;
-            if (have_backdrop) o.in_accum = (const float4 *)ctx->d_task_aux;
+            if (have_backdrop) {
+                o.in_accum = (const float4 *)ctx->d_task_aux;
+                o.text_start = AICB_TEXT_BLANK;   // the backdrop's hit names no block
+            }
             o.no_world = no_world_rgba ? no_world : nullptr;
             return o;
         });
@@ -1691,6 +1718,31 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
     st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
     if (st != AICB_OK) return st;
     if (out_len) CU(cudaMemcpy(out, ctx->d_out, out_len * 4, cudaMemcpyDeviceToHost));
+    if (info) *info = total;
+    return AICB_OK;
+}
+
+// == the desktop terminal's frame (terminal.rs:114-142): RtScene::trace_ray_through_layers into ColorCharacterBuf
+// (:341-394) for every pixel and ColorCharacterBuf::output: post-processed linear RGBA, text and the text's layer.
+aicb_status aicb_render_layers_terminal(const aicb_layer *world, const aicb_layer *ui, const float backdrop_rgba[4],
+                                        const float no_world_rgba[4], aicb_terminal_pixel *out, size_t out_len,
+                                        aicb_render_info *info) {
+    const aicb_layer *lead = nullptr;
+    aicb_status st = aicb_check_layers(world, ui, no_world_rgba, out_len, &lead);
+    if (st != AICB_OK) return st;
+    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
+    aicb_ctx *ctx = lead->scene->ctx;
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    CU(cudaSetDevice(ctx->device));
+    st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * sizeof(aicb_terminal_pixel) + 16);
+    if (st != AICB_OK) return st;
+    LayerPart part = single_part(world, ui);
+    part.target.terminal = true;
+    part.target.term = (aicb_terminal_pixel *)ctx->d_out;
+    aicb_render_info total;
+    st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
+    if (st != AICB_OK) return st;
+    if (out_len) CU(cudaMemcpy(out, ctx->d_out, out_len * sizeof(aicb_terminal_pixel), cudaMemcpyDeviceToHost));
     if (info) *info = total;
     return AICB_OK;
 }

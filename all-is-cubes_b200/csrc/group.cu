@@ -6,7 +6,7 @@
 // waits for the others' completion events and copies the frame to the caller: compute and delivery are one kernel
 // chain per device, there is no collective and no host thread per GPU.
 // Replaces the Rayon rows x pixels dispatch of trace_scene_to_image_impl (renderer.rs:516-556) across devices.
-// Layered frames and texture targets (aicb_group_render_layers_*) cut the work the same way, or a pixel list into
+// Layered frames, terminal frames and texture targets (aicb_group_render_layers_*) cut the work the same way, or a pixel list into
 // ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu).  Every call issues a pass on every
 // device before it waits for any, and re-issues it on a device whose hit stream overflowed (aicb_trace_pass).
 #include <algorithm>
@@ -21,7 +21,8 @@ struct aicb_group {
     std::vector<cudaEvent_t> done;   // per device: its strips of the current frame are in device 0's frame
     void *d_frame = nullptr;         // on device 0
     size_t frame_pixels = 0;
-    void *d_tex = nullptr;           // on device 0: the colour and depth texels of aicb_group_render_layers_texture
+    void *d_tex = nullptr;           // on device 0: the texels of aicb_group_render_layers_texture, or the pixels of
+                                     // aicb_group_render_layers_terminal
     size_t d_tex_bytes = 0;
     void *h_stage = nullptr;         // pinned staging for pageable destinations
     size_t h_stage_bytes = 0;
@@ -281,6 +282,39 @@ aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world, const 
     st = join(g, parts.size());
     if (st != AICB_OK) return st;
     if (out_len) CU(cudaMemcpyAsync(out, g->d_frame, out_len * 4, cudaMemcpyDeviceToHost, root->stream));
+    CU(cudaStreamSynchronize(root->stream));
+    if (info) *info = total;
+    return AICB_OK;
+}
+
+aicb_status aicb_group_render_layers_terminal(const aicb_group_layer *world, const aicb_group_layer *ui,
+                                              const float backdrop_rgba[4], const float no_world_rgba[4],
+                                              aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info) {
+    aicb_group *g = nullptr;
+    aicb_status st = group_of(world, ui, &g);
+    if (st != AICB_OK) return st;
+    aicb_layer w0 = replica(world, 0), u0 = replica(ui, 0);
+    const aicb_layer *w = world ? &w0 : nullptr, *u = ui ? &u0 : nullptr, *lead = nullptr;
+    st = aicb_check_layers(w, u, no_world_rgba, out_len, &lead);
+    if (st != AICB_OK) return st;
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    GroupLock lock(g);
+    aicb_ctx *root = g->ctx[0];
+    CU(cudaSetDevice(root->device));
+    const size_t bytes = out_len * sizeof(aicb_terminal_pixel);
+    st = aicb_ensure_device(&g->d_tex, &g->d_tex_bytes, bytes + 16);
+    if (st != AICB_OK) return st;
+    Outputs target;
+    target.full_frame = true;
+    target.terminal = true;
+    target.term = (aicb_terminal_pixel *)g->d_tex;
+    std::vector<LayerPart> parts = strip_parts(g, world, ui, target);
+    aicb_render_info total;
+    st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
+    if (st != AICB_OK) return st;
+    st = join(g, parts.size());
+    if (st != AICB_OK) return st;
+    if (out_len) CU(cudaMemcpyAsync(out, g->d_tex, bytes, cudaMemcpyDeviceToHost, root->stream));
     CU(cudaStreamSynchronize(root->stream));
     if (info) *info = total;
     return AICB_OK;

@@ -72,6 +72,8 @@ struct aicb_ctx {
     size_t d_task_aux_bytes = 0;
     void *d_task_depth = nullptr;   // per task: the UI pass's DepthBuf for the world pass (aicb_render_layers_texture)
     size_t d_task_depth_bytes = 0;
+    void *d_task_text = nullptr;    // per task: the UI pass's CharacterBuf for the world pass (aicb_render_layers_terminal)
+    size_t d_task_text_bytes = 0;
     // light propagation: the static ray chart (space/light/chart), built and uploaded on first use
     LightChartNode *d_chart = nullptr;
     LightNodePre *d_chart_pre = nullptr;   // the same chart in depth-first preorder (the lockstep walk)
@@ -150,6 +152,12 @@ struct Outputs {
     uint32_t tex_layer = aicb::TEX_WORLD;
     float tex_exposure[2] = {1.0f, 1.0f};
     double depth_m[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    // the terminal's ColorCharacterBuf (aicb_render_layers_terminal): the TERM kernels; tex_layer names the pass's layer
+    bool terminal = false;
+    aicb_terminal_pixel *term = nullptr;
+    const int2 *in_text = nullptr;
+    int2 *out_task_text = nullptr;
+    int32_t text_start = AICB_TEXT_EMPTY;
 };
 
 // One device's share of a layered frame or texture (aicb_trace_layers): that device's scenes of the layers (nullptr for

@@ -197,16 +197,32 @@ struct TraceParams {
     uint32_t has_backdrop;
     float no_world[4];          // ColorBuf the accumulator is replaced by if it is not opaque in the end
     uint32_t has_no_world;
-    // RaytraceToTexture's colour and depth targets (raytrace_to_texture.rs:591-683): read only by the TEX
+    // RaytraceToTexture's colour and depth targets (raytrace_to_texture.rs:591-683): read only by the TGT_TEX
     // instantiations of resolve_kernel / encode_kernel, and (the pixel list) by gen_kernel
     const uint32_t *pixel_list; // pixel task i is the framebuffer pixel pixel_list[i] = y * fb_width + x, or nullptr
     uint32_t n_list;
-    uint32_t tex_layer;         // InLayer of this pass's hits: TEX_WORLD or TEX_UI
-    float tex_exposure[2];      // exposure of the world and of the UI camera
-    double depth_m[8];          // m13 m23 m33 m43 m14 m24 m34 m44 of the depth transform
-    const double *in_depth;     // per task (global index): DepthBuf the layer in front left, or nullptr
-    double *out_task_depth;     // per task: the ray's DepthBuf, handed on next to out_accum, or nullptr
-    float *out_tex_depth;       // per pixel: the depth texel
+    uint32_t tex_layer;         // InLayer of this pass's hits: TEX_WORLD or TEX_UI (also the TGT_TERM text's layer)
+    // A frame has one target, so the fields of the other target share the space: the parameter block, and with it
+    // the code of the kernels that read neither, keeps its size.
+    union {
+        struct {
+            float tex_exposure[2];      // exposure of the world and of the UI camera
+            double depth_m[8];          // m13 m23 m33 m43 m14 m24 m34 m44 of the depth transform
+            const double *in_depth;     // per task (global index): DepthBuf the layer in front left, or nullptr
+            double *out_task_depth;     // per task: the ray's DepthBuf, handed on next to out_accum, or nullptr
+            float *out_tex_depth;       // per pixel: the depth texel
+        };
+        // The terminal's ColorCharacterBuf (aicb_render_layers_terminal): read only by the TGT_TERM instantiations.
+        // A CharacterBuf is (text, layer): an AICB_TEXT_* state or block index, and the tex_layer of the pass whose
+        // Space the index belongs to.
+        struct {
+            aicb_terminal_pixel *out_term;  // per pixel: post-processed colour, text, layer
+            const int2 *in_text;            // per task (global index): CharacterBuf the layer in front left, or nullptr
+            int2 *out_task_text;            // per task: the ray's CharacterBuf, handed on next to out_accum, or nullptr
+            int32_t text_start;             // CharacterBuf of a ray without in_text: Empty, or Hit(" ") behind a lone
+                                            // backdrop
+        };
+    };
     // LightingOption::Bounce (surface.rs:113-166): the frame's primary pass and its secondary passes share these
     uint32_t bounce_mode;       // BOUNCE_OFF / BOUNCE_PRIMARY / BOUNCE_SECONDARY
     uint32_t bounce_samples;    // LightingOption::Bounce { samples }
@@ -672,11 +688,9 @@ AICB_DEV unsigned char component_to_srgb8(const float *thr, float c) {
     return (unsigned char)lo;
 }
 
-// Camera::post_process_color + to_srgb8 (camera_struct.rs:376-382, graphics_options.rs:352-368, color.rs:669-676)
-AICB_DEV uchar4 encode_srgb8(const TraceParams &P, const float *thr, float l0, float l1, float l2, float tr) {
-    float rgba[4];
-    colorbuf_to_rgba(l0, l1, l2, tr, rgba);
-    float c[3] = {ps_mul(rgba[0], P.exposure), ps_mul(rgba[1], P.exposure), ps_mul(rgba[2], P.exposure)};
+// Camera::post_process_color (camera_struct.rs:376-382, graphics_options.rs:352-368) of rgba's colour; alpha is kept
+AICB_DEV void post_process_color(const TraceParams &P, const float rgba[4], float c[3]) {
+    c[0] = ps_mul(rgba[0], P.exposure); c[1] = ps_mul(rgba[1], P.exposure); c[2] = ps_mul(rgba[2], P.exposure);
     if (isfinite(P.maximum_intensity)) {
         if (P.tone_mapping == AICB_TONE_CLAMP) {
 #pragma unroll
@@ -688,6 +702,14 @@ AICB_DEV uchar4 encode_srgb8(const TraceParams &P, const float *thr, float l0, f
             for (int i = 0; i < 3; i++) c[i] = ps_mul(c[i], s);
         }
     }
+}
+
+// Camera::post_process_color + to_srgb8 (camera_struct.rs:376-382, color.rs:669-676)
+AICB_DEV uchar4 encode_srgb8(const TraceParams &P, const float *thr, float l0, float l1, float l2, float tr) {
+    float rgba[4];
+    colorbuf_to_rgba(l0, l1, l2, tr, rgba);
+    float c[3];
+    post_process_color(P, rgba, c);
     return make_uchar4(component_to_srgb8(thr, c[0]), component_to_srgb8(thr, c[1]), component_to_srgb8(thr, c[2]),
                        sat_u8(roundf(rgba[3] * 255.0f)));
 }
@@ -1784,9 +1806,30 @@ static __global__ void __launch_bounds__(128) bounce_resolve_kernel(const __grid
 // (accum.rs:135-151) starts a fresh Split: depth +inf, layer World if the paint colour has T != 1.  The oracle
 // (oracle_texture/aic_texture.cpp) applies the rule after each add it makes itself and after each layer's trace, and
 // counts every layer whose trace raised the transmittance, so a case that broke the argument would show in the tests.
+//
+// TERM: the accumulator is the terminal's ColorCharacterBuf (all-is-cubes-desktop/src/terminal.rs:341-394): the
+// ColorBuf, which alone decides opacity, and a CharacterBuf (text.rs:52-123) that every hit the colour gets is also
+// added to.  CharacterBuf::add keeps the first Hit it is given, so per layer only the first hit that is a Hit matters:
+// the first visible surface (its block), else Exception::Incomplete ("X"), else debug_pixel_cost's DebugOverrideRg
+// (" "); the sky is ignored.  Without any of them a ray that counted a step (EnterSpace, sr.rs:629-637) has entered the
+// space.  The backdrop adds " " after the UI layer's hits, and P::paint replaces the whole accumulator: text " ".  The
+// UI pass hands the CharacterBuf on next to the ColorBuf (out_task_text); CharacterBuf::mean reduces the samples.
 // ======================================================================================================
 constexpr uint32_t TEX_NONE = 0, TEX_WORLD = 1, TEX_UI = 2;
-template <bool TEX, class Chain>
+// the target of a pixel-writing kernel (template): frames, aicb_render_layers_texture's texels, the terminal's pixels
+constexpr int TGT_FRAME = 0, TGT_TEX = 1, TGT_TERM = 2;
+
+// the Space block index of the cube a hit is in (the cell word's block field)
+AICB_DEV int32_t hit_block(const TraceParams &P, uint32_t slot) {
+    const DeviceScene &S = P.scene;
+    const uint32_t cell = P.hits[slot].cell;
+    return S.wide_cells ? (int32_t)(__ldg((const uint32_t *)S.cells + cell) & 0xffffu)
+                        : (int32_t)((uint32_t)__ldg((const uint16_t *)S.cells + cell) & 0x3fffu);
+}
+
+AICB_DEV bool text_is_hit(int32_t t) { return t >= 0 || t <= AICB_TEXT_INCOMPLETE; }   // CharacterBuf State::Hit
+
+template <bool TEX, bool TERM, class Chain>
 AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const uint32_t i, const size_t out_index,
                                Chain &&chain) {
     const DeviceScene &S = P.scene;
@@ -1800,6 +1843,7 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
     double depth = D_INF;          // DepthBuf::mean = min over the sub-samples (accum.rs:284-297)
     uint32_t first_valid = 0xffffffffu;   // Position of the first surface hit: first sub-sample that has one
     int32_t text = AICB_TEXT_EMPTY;       // CharacterBuf of the pixel (text.rs:100-113 reduces the sub-samples)
+    int2 term;                            // TERM: the pixel's CharacterBuf (text, layer), set by sample 0
     for (uint32_t k = 0; k < P.n_samples; k++) {
         TaskOut o;
         *reinterpret_cast<uint4 *>(&o) = *reinterpret_cast<const uint4 *>(P.task_out + t0 + k);
@@ -1816,9 +1860,7 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
             // is "X"; a ray that counted a step entered the space (sr.rs:628-637)
             int32_t tk = o.steps > 0 ? AICB_TEXT_ENTERED_SPACE : AICB_TEXT_EMPTY;
             if (sample_first != 0xffffffffu) {
-                const uint32_t cell = P.hits[sample_first].cell;
-                tk = S.wide_cells ? (int32_t)(__ldg((const uint32_t *)S.cells + cell) & 0xffffu)
-                                  : (int32_t)((uint32_t)__ldg((const uint16_t *)S.cells + cell) & 0x3fffu);
+                tk = hit_block(P, sample_first);
             } else if (o.steps > 1000u) {
                 tk = AICB_TEXT_INCOMPLETE;
             }
@@ -1868,6 +1910,22 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
             tex_depth = fmin(tex_depth, d);
             if (tex_layer == TEX_NONE) tex_layer = layer;
         }
+        if constexpr (TERM) {
+            int2 c = P.in_text ? P.in_text[P.task_base + t0 + k] : make_int2(P.text_start, (int)TEX_NONE);
+            if (!text_is_hit(c.x)) {   // CharacterBuf::add of this layer's hits, then the backdrop's
+                if (sample_first != 0xffffffffu) c = make_int2(hit_block(P, sample_first), (int)P.tex_layer);
+                else if (o.steps > 1000u) c.x = AICB_TEXT_INCOMPLETE;
+                else if (P.debug_pixel_cost || P.has_backdrop) c.x = AICB_TEXT_BLANK;
+                else if (o.steps > 0) c.x = AICB_TEXT_ENTERED_SPACE;
+            }
+            if (P.has_no_world && !(T < (1.0f / 256.0f))) c = make_int2(AICB_TEXT_BLANK, (int)TEX_NONE);   // P::paint
+            if (P.out_task_text) P.out_task_text[P.task_base + t0 + k] = c;
+            // CharacterBuf::mean (text.rs:96-108): the first sample that holds a Hit; EnteredSpace only if all entered
+            if (k == 0 || (!text_is_hit(term.x) && text_is_hit(c.x))) term = c;
+            else if (!text_is_hit(term.x))
+                term.x = (term.x == AICB_TEXT_ENTERED_SPACE && c.x == AICB_TEXT_ENTERED_SPACE) ? AICB_TEXT_ENTERED_SPACE
+                                                                                             : AICB_TEXT_EMPTY;
+        }
         if (P.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint(NO_WORLD_TO_SHOW) replaces it (renderer.rs:474-477)
             lr = P.no_world[0]; lg = P.no_world[1]; lb = P.no_world[2]; T = P.no_world[3];
         }
@@ -1894,6 +1952,17 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
     if (P.n_samples == 4) { l0 = a0 / 4.0f; l1 = a1 / 4.0f; l2 = a2 / 4.0f; tT = aT / 4.0f; }
     if (P.out_srgb8) P.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
     if (P.out_colorbuf) P.out_colorbuf[out_index] = make_float4(l0, l1, l2, tT);
+    if constexpr (TERM) {
+        if (P.out_term) {   // ColorCharacterBuf::output (terminal.rs:355-366): post_process_color(Rgba::from(ColorBuf))
+            float rgba[4], c[3];
+            colorbuf_to_rgba(l0, l1, l2, tT, rgba);
+            post_process_color(P, rgba, c);
+            float2 *dst = reinterpret_cast<float2 *>(P.out_term + out_index);   // 24-byte pixels: 8-byte stores
+            dst[0] = make_float2(c[0], c[1]);
+            dst[1] = make_float2(c[2], rgba[3]);
+            reinterpret_cast<int2 *>(dst)[2] = term;
+        }
+    }
     if constexpr (TEX) {
         if (P.out_rgba16f) {   // trace_one's colour (raytrace_to_texture.rs:643-661): the exposure of the pixel's layer
             const float e = tex_layer == TEX_UI ? P.tex_exposure[1] : (tex_layer == TEX_WORLD ? P.tex_exposure[0] : 1.0f);
@@ -1974,11 +2043,12 @@ AICB_DEV void count_pixels(const TraceParams &P, unsigned long long cubes_traced
 // Kernel 4 of a frame that does not run resolve_kernel — per pixel: the ray's transmittance chain over the ShadedHits
 // that shade_kernel left, then finish_pixel.
 // ======================================================================================================
-// TEX: the texture targets of aicb_render_layers_texture (finish_pixel); the instantiation other frames use does not
-// carry them.
+// TGT: the texture targets of aicb_render_layers_texture or the terminal pixels of aicb_render_layers_terminal
+// (finish_pixel); the instantiation other frames use (TGT_FRAME) carries neither.
 constexpr uint32_t ENCODE_RUN = 4;
-template <bool TEX>
+template <int TGT>
 __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
+    constexpr bool TEX = TGT == TGT_TEX, TERM = TGT == TGT_TERM;
     __shared__ float s_thr[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_thr[i] = P.scene.tables[256 + i];
     grid_dependency_sync();
@@ -1991,7 +2061,7 @@ __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ Tra
     unsigned long long cubes_traced = 0, n_hits = 0;
     if (active) {
         const uint32_t t0 = i * P.n_samples;
-        cubes_traced = finish_pixel<TEX>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
+        cubes_traced = finish_pixel<TEX, TERM>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
                                                                float &T, uint32_t &steps, uint32_t &sample_first) {
             lr = 0.f; lg = 0.f; lb = 0.f; T = 1.0f;
             if (P.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
@@ -2060,7 +2130,7 @@ constexpr uint32_t RESOLVE_WINDOW = 128;
 // 4 resident blocks of 128 threads per SM = 128 registers per thread at most (the kernel needs about 80)
 constexpr int RESOLVE_MIN_BLOCKS = 4;
 
-template <int LC, bool TEX>
+template <int LC, int TGT>
 __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const __grid_constant__ TraceParams P,
                                                                           uint32_t n_chunk_tasks) {
     static_assert(LC == LC_NONE || LC == LC_FLAT, "interpolated and Bounce lighting shade in shade_kernel");
@@ -2081,7 +2151,8 @@ __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const 
     const uint32_t i = t / P.n_samples;                          // its pixel task
     uint32_t px = 0, py = 0;
     size_t out_index = 0;
-    const bool active = t < n_chunk_tasks && task_pixel<TEX>(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
+    const bool active = t < n_chunk_tasks &&
+                        task_pixel<TGT == TGT_TEX>(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
     float lr = 0.f, lg = 0.f, lb = 0.f, T = 1.0f;
     uint32_t steps = 0, sample_first = 0xffffffffu, hi = HIT_NONE, left = 0;
     if (active) {
@@ -2162,8 +2233,9 @@ __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const 
     __syncwarp();
     unsigned long long cubes_traced = 0;
     if (active && t % P.n_samples == 0u) {
-        cubes_traced = finish_pixel<TEX>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &, float &r, float &g, float &b,
-                                                               float &tr, uint32_t &st, uint32_t &sf) {
+        cubes_traced = finish_pixel<TGT == TGT_TEX, TGT == TGT_TERM>(
+            P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &, float &r, float &g, float &b, float &tr,
+                                        uint32_t &st, uint32_t &sf) {
             const float4 a = shaded[lane + k];
             r = a.x; g = a.y; b = a.z; tr = a.w;
             st = hsteps[lane + k];

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 4 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 5 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -17,6 +17,11 @@ pub const AICB_ERR_RETRY: aicb_status = 6;
 pub const AICB_TEXT_ENTERED_SPACE: i32 = -1;
 pub const AICB_TEXT_EMPTY: i32 = -2;
 pub const AICB_TEXT_INCOMPLETE: i32 = -3;
+pub const AICB_TEXT_BLANK: i32 = -4;
+
+pub const AICB_LAYER_NONE: i32 = 0;
+pub const AICB_LAYER_WORLD: i32 = 1;
+pub const AICB_LAYER_UI: i32 = 2;
 
 /// `GridAab` (all-is-cubes-base/src/math/grid_aab.rs)
 #[repr(C)]
@@ -137,6 +142,15 @@ pub struct aicb_hit {
     pub face: i32,
 }
 
+/// one pixel of the terminal's frame: `ColorCharacterBuf::output` (all-is-cubes-desktop/src/terminal.rs:355-366)
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_terminal_pixel {
+    pub rgba: [f32; 4],
+    pub text: i32,
+    pub layer: i32,
+}
+
 #[repr(C)]
 pub struct aicb_ctx {
     _opaque: [u8; 0],
@@ -202,6 +216,9 @@ unsafe extern "C" {
                                       no_world_rgba: *const [f32; 4], depth_transform: *const [f64; 16],
                                       pixels: *const u32, n_pixels: usize, out_rgba16f: *mut [u16; 4],
                                       out_depth: *mut f32, info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_render_layers_terminal(world: *const aicb_layer, ui: *const aicb_layer, backdrop_rgba: *const [f32; 4],
+                                       no_world_rgba: *const [f32; 4], out: *mut aicb_terminal_pixel, out_len: usize,
+                                       info: *mut aicb_render_info) -> aicb_status;
     pub fn aicb_ortho_image_size(s: *const aicb_scene, resolution: u32, width: *mut u32, height: *mut u32) -> aicb_status;
     pub fn aicb_render_orthographic(s: *mut aicb_scene, resolution: u32, out: *mut [u8; 4], out_len: usize,
                                     info: *mut aicb_render_info) -> aicb_status;
@@ -245,6 +262,10 @@ unsafe extern "C" {
                                             depth_transform: *const [f64; 16], pixels: *const u32, n_pixels: usize,
                                             out_rgba16f: *mut [u16; 4], out_depth: *mut f32,
                                             info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_layers_terminal(world: *const aicb_group_layer, ui: *const aicb_group_layer,
+                                             backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],
+                                             out: *mut aicb_terminal_pixel, out_len: usize,
+                                             info: *mut aicb_render_info) -> aicb_status;
 
     pub fn aicb_trace_rays(s: *mut aicb_scene, origin_dir: *const [f64; 6], n: usize, opt: *const aicb_options,
                            out_colorbuf: *mut [f32; 4], depth: *mut f64, hit: *mut aicb_hit, steps: *mut u32,

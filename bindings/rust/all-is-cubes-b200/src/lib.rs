@@ -10,9 +10,13 @@
 //!   → `aicb_render_layers_srgb8`; the info text is drawn here over the returned pixels like renderer.rs:659-683.
 //! * `trace_texture_batch()` = the tracing of `RaytraceToTexture::do_some_tracing` (raytrace_to_texture.rs:591-683)
 //!   for a batch of pixels → `aicb_render_layers_texture`.
+//! * `draw_terminal()` = the desktop terminal's `RtRenderer<CharacterRtData>::draw::<ColorCharacterBuf>`
+//!   (all-is-cubes-desktop/src/terminal.rs:114-142, 341-394) → `aicb_render_layers_terminal`; the block indices it
+//!   returns are mapped to `CharacterRtData` strings from one table per layer, kept current with the scenes.
 //! * `B200Renderer::on_devices()` / `on_group()`: the same renderer on several devices (`aicb_group_*`): scenes
 //!   replicated and kept current by the same deltas, `draw()` → `aicb_group_render_layers_srgb8`,
-//!   `trace_texture_batch()` → `aicb_group_render_layers_texture`.
+//!   `trace_texture_batch()` → `aicb_group_render_layers_texture`, `draw_terminal()` →
+//!   `aicb_group_render_layers_terminal`.
 //!
 //! Not compiled in the repository this file ships in (no Rust toolchain there); see ../README.md.
 
@@ -30,6 +34,8 @@ use all_is_cubes::util::maybe_sync::BoxFuture;
 use all_is_cubes_b200_sys as sys;
 use all_is_cubes_render::camera::{Camera, Layers, StandardCameras};
 use all_is_cubes_render::{Flaws, HeadlessRenderer, RenderError, Rendering};
+
+use unicode_segmentation::UnicodeSegmentation as _;
 
 pub use convert::{block_desc_of, camera_of, options_of, sky_of, OwnedBlockDesc};
 
@@ -199,6 +205,14 @@ struct SceneFollower {
     space: Handle<Space>,
     scene: Option<SceneHandle>,
     todo: listen::StoreLock<Todo>,
+    /// `CharacterRtData` of every block index (the terminal's text), current with `scene`
+    chars: Vec<String>,
+}
+
+/// `CharacterRtData::from_block` (raytracer/text.rs:30-38): the first grapheme of the block's display name, or "#".
+fn character_of(data: &space::SpaceBlockData) -> String {
+    let name: &str = &data.evaluated().attributes().display_name;
+    name.graphemes(true).next().unwrap_or("#").to_owned()
 }
 // SAFETY: see B200Context.
 unsafe impl Send for SceneFollower {}
@@ -209,6 +223,7 @@ impl SceneFollower {
             space,
             scene: None,
             todo: listen::StoreLock::new(Todo { listener: true, everything: true, ..Todo::default() }),
+            chars: Vec::new(),
         }
     }
 
@@ -248,6 +263,7 @@ impl SceneFollower {
             if let Some(old) = self.scene.replace(fresh) {
                 old.destroy();
             }
+            self.chars = space.block_data().iter().map(character_of).collect();
         } else if let Some(scene) = self.scene {
             // SpaceChange::BlockIndex / BlockEvaluation: re-run TracingBlock::from_block for those indices (updating.rs:128-150);
             // on a group every replica takes them (aicb_group_scene_update_blocks), no rebuild
@@ -257,6 +273,13 @@ impl SceneFollower {
                     idx.iter().map(|&i| block_desc_of(&space.block_data()[usize::from(i)])).collect();
                 let descs: Vec<sys::aicb_block_desc> = owned.iter().map(OwnedBlockDesc::as_ffi).collect();
                 scene.update_blocks(&idx, &descs).map_err(to_render_error)?;
+                for &i in &idx {
+                    let i = usize::from(i);
+                    if i >= self.chars.len() {
+                        self.chars.resize(i + 1, String::new());
+                    }
+                    self.chars[i] = character_of(&space.block_data()[i]);
+                }
             }
             // SpaceChange::CubeBlock / CubeLight (updating.rs:151-166)
             if !todo.cubes.is_empty() {
@@ -395,6 +418,56 @@ impl B200Renderer {
             },
         ))?;
         Ok(info)
+    }
+
+    /// The desktop terminal's frame (all-is-cubes-desktop/src/terminal.rs:114-142), in place of
+    /// `scene.draw::<ColorCharacterBuf, _, _, _>(|_| String::new(), |b| b.output(camera), &mut image)`: per pixel of
+    /// the world camera's framebuffer, row-major, the `CharacterBuf` string and
+    /// `Some(camera.post_process_color(Rgba::from(ColorBuf)))` (ColorCharacterBuf::output, :355-366), through the
+    /// layers this renderer holds, and the image's info.  The info text is empty, as the terminal draws it.
+    pub fn draw_terminal(&self) -> Result<(Vec<(String, Option<Rgba>)>, sys::aicb_render_info), B200Error> {
+        let cams: &Layers<Camera> = self.cameras.cameras();
+        let size = cams.world.viewport().framebuffer_size;
+        let mut pixels = vec![sys::aicb_terminal_pixel::default(); (size.width as usize) * (size.height as usize)];
+        let backdrop: Rgba = self.cameras.ui_view_state().backdrop;
+        let backdrop_arr: [f32; 4] = backdrop.into();
+        let backdrop_ptr: *const [f32; 4] = if backdrop == Rgba::TRANSPARENT { core::ptr::null() } else { &backdrop_arr };
+        let no_world: [f32; 4] = palette::NO_WORLD_TO_SHOW.into();
+        let mut info = sys::aicb_render_info::default();
+        if self.layers.world.is_none() && self.layers.ui.is_none() {
+            // no Space at all: every accumulator is P::paint(NO_WORLD_TO_SHOW) (renderer.rs:474-477)
+            let c = cams.world.post_process_color(palette::NO_WORLD_TO_SHOW);
+            return Ok((vec![(" ".to_owned(), Some(c)); pixels.len()], info));
+        }
+        let (out, out_len) = (pixels.as_mut_ptr(), pixels.len());
+        let info_ptr: *mut sys::aicb_render_info = &mut info;
+        check(self.with_layers(
+            cams,
+            |world, ui| unsafe {
+                sys::aicb_render_layers_terminal(world, ui, backdrop_ptr, &no_world, out, out_len, info_ptr)
+            },
+            |world, ui| unsafe {
+                sys::aicb_group_render_layers_terminal(world, ui, backdrop_ptr, &no_world, out, out_len, info_ptr)
+            },
+        ))?;
+        let table = |layer: i32| -> &[String] {
+            let slot = if layer == sys::AICB_LAYER_UI { &self.layers.ui } else { &self.layers.world };
+            slot.as_ref().map_or(&[], |f| f.chars.as_slice())
+        };
+        let image = pixels
+            .iter()
+            .map(|p| {
+                // From<CharacterBuf> for Substr (text.rs:111-119)
+                let text = match p.text {
+                    sys::AICB_TEXT_EMPTY => ".".to_owned(),
+                    sys::AICB_TEXT_INCOMPLETE => "X".to_owned(),
+                    sys::AICB_TEXT_ENTERED_SPACE | sys::AICB_TEXT_BLANK => " ".to_owned(),
+                    i => table(p.layer).get(i as usize).cloned().unwrap_or_else(|| "#".to_owned()),
+                };
+                (text, Some(Rgba::new(p.rgba[0], p.rgba[1], p.rgba[2], p.rgba[3])))
+            })
+            .collect();
+        Ok((image, info))
     }
 
     fn sync_layer(

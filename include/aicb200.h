@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 4
+#define AICB_ABI_VERSION 5
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -159,11 +159,13 @@ typedef struct aicb_render_info {
                                       frames) [2] is its time and [3] is 0 */
 } aicb_render_info;
 
-/* CharacterBuf states (raytracer/text.rs:52-123) of aicb_render_text: a value >= 0 is the block index (Space palette
- * index) of the first block hit; the caller maps it to that block's string like TracingBlock's D::from_block does. */
+/* CharacterBuf states (raytracer/text.rs:52-123) of aicb_render_text and aicb_render_layers_terminal: a value >= 0 is
+ * the block index (Space palette index) of the first block hit; the caller maps it to that block's string like
+ * TracingBlock's D::from_block does.  AICB_TEXT_BLANK comes from aicb_render_layers_terminal only. */
 #define AICB_TEXT_ENTERED_SPACE (-1) /* the ray entered the Space's bounds but hit nothing: " " */
 #define AICB_TEXT_EMPTY (-2)         /* the ray never entered the Space: "." */
 #define AICB_TEXT_INCOMPLETE (-3)    /* Exception::Incomplete (step cap) before any hit: "X" */
+#define AICB_TEXT_BLANK (-4)         /* a hit that names no block (backdrop, NO_WORLD_TO_SHOW paint, debug_pixel_cost): " " */
 
 /* Per-pixel hit record: Position of the first non-exception Hit (hit.rs:92-101):
  * cube xyz, voxel xyz, resolution, face; all -1 when the ray hit nothing. */
@@ -283,6 +285,29 @@ aicb_status aicb_render_layers_texture(const aicb_layer *world_or_null, const ai
                                        uint16_t (*out_rgba16f)[4], float *out_depth,
                                        aicb_render_info *info_or_null);
 
+/* == the desktop app's terminal frame (all-is-cubes-desktop/src/terminal.rs:114-142): RtRenderer<CharacterRtData>::draw
+ * into ColorCharacterBuf (:341-394) and ColorCharacterBuf::output (:355-366) per pixel, the layers traced as
+ * aicb_render_layers_srgb8 traces them.  The accumulator stops where that call's does (its ColorBuf's opacity), so the
+ * hits, step counts and cubes_traced are that call's; CharacterBuf (raytracer/text.rs:52-123) follows every hit the
+ * colour gets: the first surface names its block, Exception::Incomplete before one is "X", the backdrop, debug_pixel_cost
+ * and NO_WORLD_TO_SHOW (which replaces the whole accumulator) are " " (AICB_TEXT_BLANK), and a ray that counted a step
+ * entered the space.  The four antialiasing samples are reduced by ColorBuf::mean and CharacterBuf::mean (the first
+ * sample with a hit gives the text; EnteredSpace only if every sample entered).
+ *   rgba:  Camera::post_process_color(Rgba::from(ColorBuf)) of the world layer's camera and options (the UI layer's
+ *          without a world): exposure, then tone mapping, linear f32, the value aicb_render_layers_srgb8 encodes.
+ *   text:  the block index (>= 0) the caller maps with CharacterRtData::from_block, or AICB_TEXT_*.
+ *   layer: the layer whose Space the block index belongs to (AICB_LAYER_WORLD / _UI); AICB_LAYER_NONE for text < 0.
+ * Arguments, validation and options are aicb_render_layers_srgb8's; out_len pixels, row-major. */
+enum { AICB_LAYER_NONE = 0, AICB_LAYER_WORLD = 1, AICB_LAYER_UI = 2 };
+typedef struct aicb_terminal_pixel {
+    float rgba[4];
+    int32_t text;
+    int32_t layer;
+} aicb_terminal_pixel;
+aicb_status aicb_render_layers_terminal(const aicb_layer *world_or_null, const aicb_layer *ui_or_null,
+                                        const float backdrop_rgba[4], const float no_world_rgba[4],
+                                        aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info_or_null);
+
 /* == render_orthographic (raytracer/ortho.rs:30-84): the five axis-aligned views of MultiOrthoCamera (:143-199) in one
  * image at `resolution` pixels per cube (the reference uses 32), UNALTERED_COLORS, sRGB8 without post-processing,
  * transparent between the views.  aicb_ortho_image_size gives the image size for a scene. */
@@ -380,6 +405,13 @@ aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world_or_nu
                                              const uint32_t *pixels_or_null, size_t n_pixels,
                                              uint16_t (*out_rgba16f)[4], float *out_depth,
                                              aicb_render_info *info_or_null);
+
+/* == aicb_render_layers_terminal on the whole group, bit for bit: its arguments with group scenes (both of the same
+ * group), the frame cut into interleaved 16-row strips as aicb_group_render_layers_srgb8 cuts it, every device storing
+ * into device 0's buffer. */
+aicb_status aicb_group_render_layers_terminal(const aicb_group_layer *world_or_null, const aicb_group_layer *ui_or_null,
+                                              const float backdrop_rgba[4], const float no_world_rgba[4],
+                                              aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info_or_null);
 
 /* == SpaceRaytracer::trace_ray (sr.rs:113-120) for a batch of explicit rays:
  * origin_dir[i] = {ox,oy,oz,dx,dy,dz}. Output as aicb_render_colorbuf. */
