@@ -348,6 +348,8 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         std::memcpy(P.m, cam->inverse_projection_view, sizeof P.m);
         P.fb_width = cam->fb_width;
         P.fb_height = cam->fb_height;
+        P.inv_width = 1.0 / (double)cam->fb_width;
+        P.inv_height = 1.0 / (double)cam->fb_height;
         P.exposure = cam->exposure;
         P.local_rows = shard_rows(cam->fb_height, shard);
         if (shard && shard->count > 1) {
@@ -461,7 +463,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     // has been enlarged after an overflow, so that the per-frame streams stay within ~8 GB however deep the scene is.
     uint64_t CHUNK = (uint64_t)4 << 20;
     {
-        const uint64_t per_task = sizeof(RayRecord) + sizeof(TaskOut) + 4 * N_BINS +
+        const uint64_t per_task = sizeof(RayRecordA) + sizeof(RayRecordB) + sizeof(TaskOut) + 4 * N_BINS +
                                   (uint64_t)ctx->hits_per_task * (sizeof(HitRecord) + (fused ? 0 : sizeof(ShadedHit)));
         uint64_t fit = ((uint64_t)8 << 30) / per_task;
         if (fit < (1u << 17)) fit = 1u << 17;
@@ -469,7 +471,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     }
     const uint64_t chunk_cap = total_tasks < CHUNK ? total_tasks : CHUNK;
     {
-        aicb_status st = ensure(&ctx->d_rays, &ctx->d_rays_bytes, chunk_cap * sizeof(RayRecord) + 16);
+        aicb_status st = ensure(&ctx->d_rays, &ctx->d_rays_bytes, chunk_cap * (sizeof(RayRecordA) + sizeof(RayRecordB)) + 16);
         if (st != AICB_OK) return st;
         st = ensure(&ctx->d_task_cb, &ctx->d_task_cb_bytes, chunk_cap * sizeof(TaskOut) + 16);
         if (st != AICB_OK) return st;
@@ -487,7 +489,10 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         st = ensure(&ctx->d_bin_list, &ctx->d_bin_list_bytes, (size_t)N_BINS * chunk_cap * 4 + 64);
         if (st != AICB_OK) return st;
     }
-    P.ray_records = (RayRecord *)ctx->d_rays;
+    // the listed rays' records: array A (64-byte aligned: cudaMalloc aligns to 256 bytes), then array B
+    P.rays_a = (RayRecordA *)ctx->d_rays;
+    P.rays_b = (RayRecordB *)((char *)ctx->d_rays + chunk_cap * sizeof(RayRecordA));
+    P.ray_counter = ctx->d_tile_counter + 2;
     P.task_out = (TaskOut *)ctx->d_task_cb;
     P.hits = (HitRecord *)ctx->d_hits;
     P.shaded = fused ? nullptr : (ShadedHit *)ctx->d_contrib;
@@ -515,13 +520,13 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         TraceParams Q;
         const bool bounce = lc == LC_BOUNCE;
         if (bounce) {
-            aicb_status st = ensure(&ctx->d_rays2, &ctx->d_rays2_bytes, chunk_cap * sizeof(RayRecord) + 16);
+            aicb_status st = ensure(&ctx->d_rays2, &ctx->d_rays2_bytes, chunk_cap * (sizeof(RayRecordA) + sizeof(RayRecordB)) + 16);
             if (st == AICB_OK) st = ensure(&ctx->d_task_cb2, &ctx->d_task_cb2_bytes, chunk_cap * sizeof(TaskOut) + 16);
             if (st == AICB_OK) st = ensure(&ctx->d_hits2, &ctx->d_hits2_bytes, (size_t)P.hit_capacity * sizeof(HitRecord) + 64);
             if (st == AICB_OK) st = ensure(&ctx->d_contrib2, &ctx->d_contrib2_bytes, (size_t)P.hit_capacity * sizeof(ShadedHit) + 64);
             if (st == AICB_OK) st = ensure(&ctx->d_bin_list2, &ctx->d_bin_list2_bytes, (size_t)N_BINS * chunk_cap * 4 + 64);
-            // per task: request (4) + RNG state (32) + Rgb sum and steps (16) + the secondary ray (48)
-            if (st == AICB_OK) st = ensure(&ctx->d_bounce, &ctx->d_bounce_bytes, chunk_cap * 100 + 256);
+            // per task: request (4) + RNG state (32) + Rgb sum and steps (16) + the secondary ray (48) + record index (4)
+            if (st == AICB_OK) st = ensure(&ctx->d_bounce, &ctx->d_bounce_bytes, chunk_cap * 104 + 256);
             if (st != AICB_OK) return st;
             char *b = (char *)ctx->d_bounce;
             P.bounce_mode = BOUNCE_PRIMARY;
@@ -530,7 +535,9 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             P.bounce_rng = (unsigned long long *)(b + chunk_cap * 48);     // 32 B
             P.bounce_sum = (float4 *)(b + chunk_cap * 80);                 // 16 B
             P.bounce_req = (uint32_t *)(b + chunk_cap * 96);               // 4 B
+            P.ray_index = (uint32_t *)(b + chunk_cap * 100);               // 4 B
             Q = P;
+            Q.ray_index = nullptr;
             Q.bounce_mode = BOUNCE_SECONDARY;
             Q.rays = P.bounce_rays;
             Q.tiles_y = 1;
@@ -547,13 +554,15 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.in_accum = nullptr; Q.out_accum = nullptr; Q.has_backdrop = 0; Q.has_no_world = 0;
             Q.pixel_list = nullptr; Q.in_depth = nullptr; Q.out_task_depth = nullptr; Q.out_tex_depth = nullptr;
             Q.out_term = nullptr; Q.in_text = nullptr; Q.out_task_text = nullptr;
-            Q.ray_records = (RayRecord *)ctx->d_rays2;
+            Q.rays_a = (RayRecordA *)ctx->d_rays2;
+            Q.rays_b = (RayRecordB *)((char *)ctx->d_rays2 + chunk_cap * sizeof(RayRecordA));
             Q.task_out = (TaskOut *)ctx->d_task_cb2;
             Q.hits = (HitRecord *)ctx->d_hits2;
             Q.shaded = (ShadedHit *)ctx->d_contrib2;
             Q.bin_list = (uint32_t *)ctx->d_bin_list2;
             Q.task_counter = ctx->d_tile_counter + (4 + N_BINS);
             Q.hit_counter = Q.task_counter + 1;
+            Q.ray_counter = Q.task_counter + 2;
             Q.bin_count = Q.task_counter + 4;
             Q.debug_warp_times = nullptr;
         }

@@ -82,21 +82,27 @@ struct DeviceScene {
     uint32_t wide_cells;        // 0: u16 cells, 1: u32 cells
 };
 
-// One primary ray after trace_ray_impl's prologue (sr.rs:135-180) and Raycaster::new().within()
-// (raycast.rs:196-230): everything the marching kernel needs, 144 bytes = 9 x 16-byte loads.
-struct __align__(16) RayRecord {
+// One primary ray that enters the Space, after trace_ray_impl's prologue (sr.rs:135-180) and Raycaster::new().within()
+// (raycast.rs:196-230): everything the marching kernel needs, in two arrays split by reader.  gen_kernel gives the
+// rays it lists consecutive record indices (one atomic per warp), so a warp writes whole lines of both arrays.  The
+// binned ray list and the hit records (HitRecord::task) hold the record index; the ray's task is in RayRecordB.
+// A: what shading reads of a ray, one aligned half-line (4 x 16-byte loads); the marcher reads it too.
+struct __align__(64) RayRecordA {
     double ox, oy, oz, dx, dy, dz;   // ray (direction already zeroed if |d| >= 1e100, raycast.rs:760-764)
     float t_to_view;                 // sr.rs:149-151
     uint32_t flags;                  // face | running<<3 | valid<<4 | active<<5 | (sx+1)<<6 | (sy+1)<<8 | (sz+1)<<10 | sky octant<<12
-                                     // (the first 64 bytes are what the shading kernel reads of a ray)
+    double t_to_abs;                 // |d| of the original direction (sr.rs:146)
+};
+static_assert(sizeof(RayRecordA) == 64, "RayRecordA must be 64 bytes");
+// B: what only the marcher reads, 5 x 16-byte loads.
+struct __align__(16) RayRecordB {
     double tdx, tdy, tdz;            // t_delta
     double half_over_len;
     double tmx, tmy, tmz, last_t;    // outer caster at its first in-bounds cube
-    double t_to_abs;                 // |d| of the original direction (sr.rs:146)
-    int rx, ry, rz;
-    uint32_t idx;
+    int rx, ry, rz;                  // ... relative to the Space's lower corner (its index is (rx * ny + ry) * nz + rz)
+    uint32_t task;                   // the ray's task in the chunk
 };
-static_assert(sizeof(RayRecord) == 144, "RayRecord must be 144 bytes");
+static_assert(sizeof(RayRecordB) == 80, "RayRecordB must be 80 bytes");
 
 // One surface of one ray, emitted by the marching kernel and lit by shade_hit: 64 bytes = 4 x 16-byte stores.
 // It is the caster's state at the surface, not a derived geometry: cube / voxel coordinates, the intersection point
@@ -116,7 +122,7 @@ struct __align__(16) HitRecord {
     uint32_t steps;         // the ray's step counter when the surface was shaded (the reference stops at the first
                             // counted step after the hit that brings the transmittance under 1/256; compositing
                             // needs the counter to restore that when the marcher's bound let the ray run on)
-    uint32_t task;          // the ray: index of its RayRecord in the chunk
+    uint32_t task;          // the ray: index of its RayRecordA / RayRecordB
     uint32_t next;          // in the last slot of a chunk: where the ray's hits continue (the first slot of another chunk)
 };
 static_assert(sizeof(HitRecord) == 64, "HitRecord must be 64 bytes");
@@ -144,6 +150,7 @@ struct TraceParams {
     // camera
     double m[16];               // inverse_projection_view, row-major m11..m44
     uint32_t fb_width, fb_height;
+    double inv_width, inv_height;   // RN(1 / fb_width), RN(1 / fb_height): the pixel quotients by div_known_recip
     float exposure;
     // options
     uint32_t fog;
@@ -167,12 +174,15 @@ struct TraceParams {
     uint32_t n_samples;         // rays per pixel task: 4 with AntialiasingOption::Always, else 1
     uint32_t task_base;         // first task of the chunk being processed (tasks = pixel_task * n_samples + sample)
     // per-task streams between the kernels of a frame (HBM)
-    RayRecord *ray_records;     // gen -> march
+    RayRecordA *rays_a;         // gen -> march, shade (by record index)
+    RayRecordB *rays_b;         // gen -> march
+    unsigned int *ray_counter;  // records handed out in this chunk
+    uint32_t *ray_index;        // per task: its record index (written for listed rays when non-null; the bounce kernels)
     TaskOut *task_out;          // march -> resolve / encode
     HitRecord *hits;            // march -> resolve / shade
     ShadedHit *shaded;          // shade -> encode (nullptr in a frame that runs resolve_kernel)
     unsigned int *hit_counter;  // hit slots handed out in this chunk (in chunks of HIT_CHUNK per lane)
-    uint32_t *bin_list;         // gen -> march: task ids of the rays that enter the space, binned by chord length
+    uint32_t *bin_list;         // gen -> march: record indices of the rays that enter the space, binned by chord length
     unsigned int *bin_count;    // [N_BINS] entries of each bin
     uint32_t bin_stride;        // capacity of one bin's list
     unsigned int *overflow_flag; // set when a chunk produced more hits than hit_capacity (frame must be re-run)
@@ -729,13 +739,15 @@ AICB_DEV void project_ndc(const TraceParams &P, double x, double y, double z, do
     }
 }
 
-// viewport.rs:104-113 + renderer.rs:424-451,489-491
+// viewport.rs:104-113 + renderer.rs:424-451,489-491.  The four quotients by the framebuffer size are correctly rounded
+// from the host's RN(1 / W) and RN(1 / H) (pixel coordinates and sizes are integers < 2^32, well inside
+// div_known_recip's exponent window), so they equal the divisions bit for bit.
 AICB_DEV void pixel_ray(const TraceParams &P, uint32_t xch, uint32_t ych, int sample, double o[3], double d[3]) {
     const double W = (double)P.fb_width, H = (double)P.fb_height;
-    const double x0 = (double)xch / W * 2.0 - 1.0;
-    const double x1 = (double)(xch + 1) / W * 2.0 - 1.0;
-    const double y0 = -((double)ych / H * 2.0 - 1.0);
-    const double y1 = -((double)(ych + 1) / H * 2.0 - 1.0);
+    const double x0 = div_known_recip((double)xch, W, P.inv_width) * 2.0 - 1.0;
+    const double x1 = div_known_recip((double)(xch + 1), W, P.inv_width) * 2.0 - 1.0;
+    const double y0 = -(div_known_recip((double)ych, H, P.inv_height) * 2.0 - 1.0);
+    const double y1 = -(div_known_recip((double)(ych + 1), H, P.inv_height) * 2.0 - 1.0);
     double px, py;
     if (sample < 0) {
         px = (x0 + x1) / 2.0;
@@ -842,7 +854,8 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
     const bool in_range = i < n_chunk_tasks;
     const uint32_t task = P.task_base + i;
     const uint32_t pixel_task = task / P.n_samples, sample = task % P.n_samples;
-    RayRecord rec;
+    RayRecordA rec;
+    RayRecordB rb;
     uint32_t px, py;
     size_t out_index;
     bool active = in_range && task_pixel<true>(P, pixel_task, &px, &py, &out_index);
@@ -886,11 +899,11 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
         bool valid;
         running = caster_begin(c, r, o[0], o[1], o[2], lv, &valid);
         rec.ox = r.ox; rec.oy = r.oy; rec.oz = r.oz; rec.dx = r.dx; rec.dy = r.dy; rec.dz = r.dz;
-        rec.tdx = r.tdx; rec.tdy = r.tdy; rec.tdz = r.tdz;
-        rec.half_over_len = r.half_over_len;
-        rec.tmx = c.tmx; rec.tmy = c.tmy; rec.tmz = c.tmz; rec.last_t = c.last_t;
-        rec.rx = c.rx; rec.ry = c.ry; rec.rz = c.rz;
-        rec.idx = c.idx;
+        rb.tdx = r.tdx; rb.tdy = r.tdy; rb.tdz = r.tdz;
+        rb.half_over_len = r.half_over_len;
+        rb.tmx = c.tmx; rb.tmy = c.tmy; rb.tmz = c.tmz; rb.last_t = c.last_t;
+        rb.rx = c.rx; rb.ry = c.ry; rb.rz = c.rz;
+        rb.task = i;
         rec.flags = ((uint32_t)c.face & 7u) | (running ? 8u : 0u) | (valid ? 16u : 0u) | 32u | ((uint32_t)(r.sx + 1) << 6) |
                     ((uint32_t)(r.sy + 1) << 8) | ((uint32_t)(r.sz + 1) << 10) | (octant << 12);
         if (running) {
@@ -919,20 +932,33 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
     }   // (!certainly_misses)
     }
     // Rays that enter the space go to the marching kernel through the binned list (warp-aggregated append); all
-    // others are complete already: nothing hit, transmittance 1, no steps.
+    // others are complete already: nothing hit, transmittance 1, no steps.  The listed rays of a warp take
+    // consecutive record indices, so that their records are whole lines (a record at the task index would leave the
+    // ~1/3 of the lanes that write spread over 32 records, every line and sector written in pieces).
     const unsigned listed = __ballot_sync(0xffffffffu, running);
     if (running) {
+        const int lane = (int)(threadIdx.x & 31);
+        const unsigned below = listed & ((1u << lane) - 1u);
+        uint32_t rbase = 0;
+        if (below == 0) rbase = atomicAdd(P.ray_counter, (unsigned)__popc(listed));
+        rbase = __shfl_sync(listed, rbase, __ffs(listed) - 1);
+        const uint32_t r = rbase + __popc(below);
         const unsigned peers = __match_any_sync(listed, bin);
         const int leader = __ffs(peers) - 1;
         uint32_t base = 0;
-        if ((int)(threadIdx.x & 31) == leader) base = atomicAdd(P.bin_count + bin, (unsigned)__popc(peers));
+        if (lane == leader) base = atomicAdd(P.bin_count + bin, (unsigned)__popc(peers));
         base = __shfl_sync(peers, base, leader);
-        const uint32_t slot = base + __popc(peers & ((1u << (threadIdx.x & 31)) - 1u));
-        P.bin_list[(size_t)bin * P.bin_stride + slot] = i;
+        const uint32_t slot = base + __popc(peers & ((1u << lane) - 1u));
+        P.bin_list[(size_t)bin * P.bin_stride + slot] = r;
+        if (P.ray_index) P.ray_index[i] = r;
         const uint4 *src = reinterpret_cast<const uint4 *>(&rec);
-        uint4 *dst = reinterpret_cast<uint4 *>(P.ray_records + i);
+        uint4 *dst = reinterpret_cast<uint4 *>(P.rays_a + r);
 #pragma unroll
-        for (int k = 0; k < 9; k++) st_stream(dst + k, src[k]);
+        for (int k = 0; k < 4; k++) st_stream(dst + k, src[k]);
+        src = reinterpret_cast<const uint4 *>(&rb);
+        dst = reinterpret_cast<uint4 *>(P.rays_b + r);
+#pragma unroll
+        for (int k = 0; k < 5; k++) st_stream(dst + k, src[k]);
     } else if (in_range) {
         TaskOut o;
         o.first_hit = 0xffffffffu;
@@ -971,14 +997,15 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     // Cold per-ray state lives in shared memory, one column per thread, so that the registers of the marching loop
     // hold only what a DDA step touches; the level switches read what they need into short-lived locals.
     __shared__ double sh_d[13][WARPS_PER_BLOCK * 32];
-    __shared__ uint32_t sh_w[13][WARPS_PER_BLOCK * 32];
+    __shared__ uint32_t sh_w[14][WARPS_PER_BLOCK * 32];
     const int tid = threadIdx.x;
 #define COLD_D(k) sh_d[k][tid]
 #define COLD_W(k) sh_w[k][tid]
     // doubles: 0-2 origin, 3-5 direction, 6 half_over_len, 7 t_to_abs, 8-10 outer t_max while inside a block, 11 outer last_t
     // words:   0 outer index (= the Space cube of the entered block), 1-3 outer step counters, 4 outer face, 5 outer valid,
-    //          6 task, 7 first hit, 8 sky octant, 9 palette offset of the entered block, 10 log2(resolution) of it,
-    //          11 pending surface's slot, 12 its log2(1 - alpha) bound;  double 12: its entry t
+    //          6 record index (HitRecord::task), 7 first hit, 8 sky octant, 9 palette offset of the entered block,
+    //          10 log2(resolution) of it, 11 pending surface's slot, 12 its log2(1 - alpha) bound, 13 task;
+    //          double 12: the pending surface's entry t
     unsigned long long dbg_t0 = 0, dbg_passes = 0, dbg_rays = 0;
     if (P.debug_warp_times) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(dbg_t0));
 
@@ -1185,7 +1212,7 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
             o.steps = steps;
             o.flags = COLD_W(8);
             o.n_hits = n_hits;
-            *reinterpret_cast<uint4 *>(P.task_out + COLD_W(6)) = *reinterpret_cast<const uint4 *>(&o);
+            *reinterpret_cast<uint4 *>(P.task_out + COLD_W(13)) = *reinterpret_cast<const uint4 *>(&o);
             if constexpr (AUX) { n_outer += aux.n_outer; n_inner += aux.n_inner; n_blocks += aux.n_blocks; }
             st = ST_IDLE;
         }
@@ -1205,33 +1232,41 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
                     } else {
                         int b = 0;
                         while (k >= s_bin_start[b + 1]) b++;
-                        const uint32_t task = __ldg(P.bin_list + (size_t)b * P.bin_stride + (k - s_bin_start[b]));
-                        RayRecord rec;
+                        const uint32_t ri = __ldg(P.bin_list + (size_t)b * P.bin_stride + (k - s_bin_start[b]));
+                        RayRecordA rec;
+                        RayRecordB rb;
                         {
-                            const uint4 *src = reinterpret_cast<const uint4 *>(P.ray_records + task);
+                            // A stays in L2 for the shading of the ray's hits; B is not read again (evict-first)
+                            const uint4 *src = reinterpret_cast<const uint4 *>(P.rays_a + ri);
                             uint4 *dst = reinterpret_cast<uint4 *>(&rec);
 #pragma unroll
-                            for (int q = 0; q < 9; q++) dst[q] = ld_stream(src + q);
+                            for (int q = 0; q < 4; q++) dst[q] = ld_stream(src + q);
+                            src = reinterpret_cast<const uint4 *>(P.rays_b + ri);
+                            dst = reinterpret_cast<uint4 *>(&rb);
+#pragma unroll
+                            for (int q = 0; q < 5; q++) dst[q] = __ldcs(src + q);
                         }
-                        COLD_W(6) = task;
+                        const uint32_t task = rb.task;
+                        COLD_W(6) = ri;
+                        COLD_W(13) = task;
                         COLD_D(0) = rec.ox; COLD_D(1) = rec.oy; COLD_D(2) = rec.oz;
                         COLD_D(3) = rec.dx; COLD_D(4) = rec.dy; COLD_D(5) = rec.dz;
-                        COLD_D(6) = rec.half_over_len;
+                        COLD_D(6) = rb.half_over_len;
                         COLD_D(7) = rec.t_to_abs;
                         COLD_W(7) = HIT_NONE;
                         COLD_W(8) = (rec.flags >> 12) & 7u;
-                        tdx = rec.tdx; tdy = rec.tdy; tdz = rec.tdz;
-                        tmx = rec.tmx; tmy = rec.tmy; tmz = rec.tmz; last_t = rec.last_t;
+                        tdx = rb.tdx; tdy = rb.tdy; tdz = rb.tdz;
+                        tmx = rb.tmx; tmy = rb.tmy; tmz = rb.tmz; last_t = rb.last_t;
                         sbits = (rec.flags >> 6) & 0x3fu;
                         const int sx = (int)(sbits & 3u) - 1, sy = (int)((sbits >> 2) & 3u) - 1, sz = (int)((sbits >> 4) & 3u) - 1;
                         fcx = sx > 0 ? AICB_FACE_NX : AICB_FACE_PX;
                         fcy = sy > 0 ? AICB_FACE_NY : AICB_FACE_PY;
                         fcz = sz > 0 ? AICB_FACE_NZ : AICB_FACE_PZ;
                         stx = sx * (S.size[1] * S.size[2]); sty = sy * S.size[2]; stz = sz;
-                        cx = sx > 0 ? S.size[0] - 1 - rec.rx : (sx < 0 ? rec.rx : COUNTER_STATIC);
-                        cy = sy > 0 ? S.size[1] - 1 - rec.ry : (sy < 0 ? rec.ry : COUNTER_STATIC);
-                        cz = sz > 0 ? S.size[2] - 1 - rec.rz : (sz < 0 ? rec.rz : COUNTER_STATIC);
-                        idx = rec.idx;
+                        cx = sx > 0 ? S.size[0] - 1 - rb.rx : (sx < 0 ? rb.rx : COUNTER_STATIC);
+                        cy = sy > 0 ? S.size[1] - 1 - rb.ry : (sy < 0 ? rb.ry : COUNTER_STATIC);
+                        cz = sz > 0 ? S.size[2] - 1 - rb.rz : (sz < 0 ? rb.rz : COUNTER_STATIC);
+                        idx = (uint32_t)((rb.rx * S.size[1] + rb.ry) * S.size[2] + rb.rz);   // as caster_begin
                         face = (int)(rec.flags & 7u);
                         valid = (rec.flags & 16u) != 0;
                         L = 0.0f;
@@ -1430,7 +1465,7 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
         for (int k = 0; k < 4; k++) dst[k] = ld_stream(src + k);
     }
     // everything the shading reads through the record is requested now, before any of it is needed
-    const RayRecord *rp = P.ray_records + h.task;
+    const RayRecordA *rp = P.rays_a + h.task;
     const float4 col = __ldg(S.palette + 2 * (size_t)h.pal);
     const float4 emi = __ldg(S.palette + 2 * (size_t)h.pal + 1);
     const uint2 rmeta = __ldg(reinterpret_cast<const uint2 *>(&rp->t_to_view));   // t_to_view, flags
@@ -1693,7 +1728,7 @@ static __global__ void __launch_bounds__(128) bounce_select_kernel(const __grid_
     P.bounce_req[i] = req;
     P.bounce_sum[i] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(0u));
     if (req != HIT_NONE) {
-        const RayRecord *rp = P.ray_records + i;
+        const RayRecordA *rp = P.rays_a + P.ray_index[i];   // (a ray with a hit was listed)
         const unsigned long long seed = (unsigned long long)__double_as_longlong(rp->dx) +
                                         (unsigned long long)__double_as_longlong(rp->dy) +
                                         (unsigned long long)__double_as_longlong(rp->dz);
@@ -1721,7 +1756,7 @@ static __global__ void __launch_bounds__(128) bounce_gen_kernel(const __grid_con
 #pragma unroll
         for (int k = 0; k < 4; k++) dst[k] = src[k];
     }
-    const RayRecord *rp = P.ray_records + i;
+    const RayRecordA *rp = P.rays_a + P.ray_index[i];
     Ray rr;
     rr.ox = rp->ox; rr.oy = rp->oy; rr.oz = rp->oz; rr.dx = rp->dx; rr.dy = rp->dy; rr.dz = rp->dz;
     const uint32_t rflags = rp->flags;
