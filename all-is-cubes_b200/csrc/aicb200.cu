@@ -430,17 +430,9 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     const int tgt = tex ? TGT_TEX : (term ? TGT_TERM : TGT_FRAME);
     P.counters = ctx->d_counters;
     P.task_counter = ctx->d_tile_counter;
-    {
-        const char *e = getenv("AICB_REFILL_THRESHOLD");
-        int v = e ? atoi(e) : 4;
-        P.refill_threshold = (uint32_t)(v < 1 ? 1 : (v > 32 ? 32 : v));
-        const char *e3 = getenv("AICB_TAIL_DIVISOR");
-        int v3 = e3 ? atoi(e3) : 2;
-        P.tail_divisor = (uint32_t)(v3 < 1 ? 1 : (v3 > 32 ? 32 : v3));
-        const char *e2 = getenv("AICB_EVENT_THRESHOLD");
-        int v2 = e2 ? atoi(e2) : 24;
-        P.event_threshold = (uint32_t)(v2 < 1 ? 1 : (v2 > 32 ? 32 : v2));
-    }
+    P.refill_threshold = REFILL_THRESHOLD;
+    P.tail_divisor = TAIL_DIVISOR;
+    P.event_threshold = EVENT_THRESHOLD;
 
     sc->pending = true;
     sc->pending_pixels = pixels;
@@ -570,10 +562,6 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         int blocks_per_sm = 0;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k, WARPS_PER_BLOCK * 32, 0));
         if (blocks_per_sm < 1) blocks_per_sm = 1;
-        if (const char *e = getenv("AICB_BLOCKS_PER_SM")) {  // experiments: cap the resident marching blocks
-            int v = atoi(e);
-            if (v >= 1 && v < blocks_per_sm) blocks_per_sm = v;
-        }
         for (uint64_t base = 0; base < total_tasks; base += CHUNK) {
             const uint32_t n = (uint32_t)(total_tasks - base < CHUNK ? total_tasks - base : CHUNK);
             P.task_base = (uint32_t)base;
@@ -593,7 +581,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                 ctx->debug_warps = (uint32_t)grid * WARPS_PER_BLOCK;
             }
             // the frame's kernels follow each other with programmatic dependent launch (no events between them)
-            const bool overlap = ctx->dependent_launch && !stage && !prof && !bounce;
+            const bool overlap = !stage && !prof && !bounce;
             CU(launch_after(overlap, k, (unsigned)grid, WARPS_PER_BLOCK * 32, stream, P, n));
             P.debug_warp_times = nullptr;
             if (stage) cudaEventRecord(ctx->ev_k[2], stream);
@@ -746,7 +734,6 @@ aicb_status aicb_ctx_create(int device_id, aicb_ctx **out) {
     CU(cudaEventCreate(&c->ev0));
     CU(cudaEventCreate(&c->ev1));
     c->profile_kernels = getenv("AICB_PROFILE_KERNELS") != nullptr;
-    if (const char *e = getenv("AICB_PDL")) c->dependent_launch = atoi(e) != 0;
     for (int i = 0; i < 5; i++) CU(cudaEventCreate(&c->ev_k[i]));
     CU(cudaEventCreateWithFlags(&c->ev_delta, cudaEventDisableTiming));
     // the frame counters (8 x u64) and the per-chunk counters (4 + N_BINS x u32) share one allocation: one memset per frame

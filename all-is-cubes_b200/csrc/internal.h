@@ -16,7 +16,6 @@ aicb_status aicb_cuda_fail(cudaError_t e, const char *what);
         if (e__ != cudaSuccess) return aicb_cuda_fail(e__, #call); \
     } while (0)
 
-struct LightChartNode;  // light_kernel.cuh
 struct LightNodePre;    // light_kernel.cuh
 struct LightChain;      // light_kernel.cuh
 struct LightBlockDev;   // light_kernel.cuh
@@ -28,7 +27,6 @@ struct aicb_ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaEvent_t ev_k[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // AICB_PROFILE_KERNELS
     bool profile_kernels = false;
-    bool dependent_launch = true; // programmatic dependent launch between the kernels of a frame (AICB_PDL=0 disables)
     bool stage_timing = true;    // record the per-kernel events of a frame (aicb_render_info::stage_ms)
     void *h_delta = nullptr, *d_delta = nullptr;  // staging of aicb_scene_update_cubes batches (pinned / device)
     size_t h_delta_bytes = 0;
@@ -75,8 +73,7 @@ struct aicb_ctx {
     void *d_task_text = nullptr;    // per task: the UI pass's CharacterBuf for the world pass (aicb_render_layers_terminal)
     size_t d_task_text_bytes = 0;
     // light propagation: the static ray chart (space/light/chart), built and uploaded on first use
-    LightChartNode *d_chart = nullptr;
-    LightNodePre *d_chart_pre = nullptr;   // the same chart in depth-first preorder (the lockstep walk)
+    LightNodePre *d_chart_pre = nullptr;   // the chart in depth-first preorder (the lockstep walk)
     uint32_t chart_nodes = 0;
     LightChain *d_chains = nullptr;         // the chart as chains, the per-node cube offsets, the Euler tour of the chain tree
     uchar4 *d_node_rel = nullptr;

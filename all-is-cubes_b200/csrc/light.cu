@@ -3,7 +3,6 @@
 // replacing LightStorage::update_light_from_queue / apply_light_update / fast_evaluate_light /
 // modified_cube_needs_update (space/light/updater.rs) and Mutation::evaluate_light (space.rs:1496-1527).
 #include <cmath>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <unordered_map>
@@ -20,6 +19,9 @@ using namespace aicb_light;
 namespace {
 
 constexpr int CHAIN_WALK_BLOCKS_PER_SM = 6;   // 4 warps, 80 registers, 26 KB of shared memory each
+// Cubes within 16 priority levels of the round's maximum are relaxed together: far fewer rounds than strict
+// level-by-level relaxation (few cubes per round leave the GPU idle) for 8 % more updates.
+constexpr uint32_t PRIORITY_BAND = 16;
 
 struct TreeNode {
     int8_t cube[3];
@@ -204,8 +206,8 @@ const ChainTables &chain_tables_host() {
 }
 
 void free_chart(aicb_ctx *c) {
-    void **ptrs[] = {(void **)&c->d_chart, (void **)&c->d_chart_pre, (void **)&c->d_chains, (void **)&c->d_node_rel,
-                     (void **)&c->d_euler, (void **)&c->d_term_scratch};
+    void **ptrs[] = {(void **)&c->d_chart_pre, (void **)&c->d_chains, (void **)&c->d_node_rel, (void **)&c->d_euler,
+                     (void **)&c->d_term_scratch};
     for (void **p : ptrs) {
         if (*p) cudaFree(*p);
         *p = nullptr;
@@ -229,26 +231,18 @@ aicb_status upload_chart(aicb_ctx *ctx) {
         ctx->n_chains = (uint32_t)t.chains.size();
         ctx->n_euler = (uint32_t)t.euler.size();
         // one set of term slots per resident warp of the chain walk
-        int per_sm = CHAIN_WALK_BLOCKS_PER_SM;
-        if (const char *e = getenv("AICB_LIGHT_CTAS")) {   // experiments: fewer resident blocks
-            const int v = atoi(e);
-            if (v >= 1 && v < per_sm) per_sm = v;
-        }
-        ctx->chain_walk_blocks = (uint32_t)ctx->num_sms * (uint32_t)per_sm;
+        ctx->chain_walk_blocks = (uint32_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM;
         CU(cudaMalloc(&ctx->d_term_scratch, (size_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM * 4 * LIGHT_WARP_SCRATCH_F4 * sizeof(float4)));
     }
-    std::vector<LightChartNode> chart = build_chart();
     const std::vector<LightNodePre> &pre = chart_preorder_host();
     CU(cudaMalloc(&ctx->d_chart_pre, pre.size() * sizeof(LightNodePre)));
     CU(cudaMemcpy(ctx->d_chart_pre, pre.data(), pre.size() * sizeof(LightNodePre), cudaMemcpyHostToDevice));
-    CU(cudaMalloc(&ctx->d_chart, chart.size() * sizeof(LightChartNode)));
-    CU(cudaMemcpy(ctx->d_chart, chart.data(), chart.size() * sizeof(LightChartNode), cudaMemcpyHostToDevice));
-    ctx->chart_nodes = (uint32_t)chart.size();
+    ctx->chart_nodes = (uint32_t)pre.size();
     return AICB_OK;
 }
 
 aicb_status ensure_chart(aicb_ctx *ctx) {
-    if (ctx->d_chart) return AICB_OK;   // (d_chart is the last allocation of upload_chart)
+    if (ctx->d_chart_pre) return AICB_OK;   // (d_chart_pre is the last allocation of upload_chart)
     const aicb_status st = upload_chart(ctx);
     if (st != AICB_OK) free_chart(ctx);   // a later call starts over instead of leaking the tables that did fit
     return st;
@@ -312,14 +306,14 @@ __global__ void __launch_bounds__(256) k_gather(const LightParams P, uint32_t n_
     }
     for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const uint32_t tm = P.tile_max[tile];
-        if (tm <= P.epsilon_priority || tm + P.priority_band < prio) continue;   // (block-uniform)
+        if (tm <= P.epsilon_priority || tm + PRIORITY_BAND < prio) continue;   // (block-uniform)
         const uint32_t w = tile * (LIGHT_TILE / 4) + wl;
         uint32_t v = w < n_words ? ((uint32_t *)P.pending)[w] : 0u;
         uint32_t sel = 0, cnt = 0;
 #pragma unroll
         for (uint32_t k = 0; k < 4; k++) {
             const uint32_t p = (v >> (8 * k)) & 255u;
-            if (p > P.epsilon_priority && p + P.priority_band >= prio && w * 4 + k < P.volume) { sel |= 1u << k; cnt++; }
+            if (p > P.epsilon_priority && p + PRIORITY_BAND >= prio && w * 4 + k < P.volume) { sel |= 1u << k; cnt++; }
         }
         // exclusive scan of cnt over the block
         uint32_t inc = cnt;
@@ -353,68 +347,10 @@ __global__ void __launch_bounds__(256) k_gather(const LightParams P, uint32_t n_
     }
 }
 
-// 8 CTAs of 4 warps per SM (64 registers; the records requested ahead spill to L1-resident local memory): the walk is
-// latency bound, so 32 resident warps serve it better than the 20 that 94 registers would allow.
-#ifndef AICB_LIGHT_MIN_BLOCKS
-#define AICB_LIGHT_MIN_BLOCKS 8
-#endif
-// How many consecutive list entries (neighbouring cubes) one warp walks for together.  The walk is a chain of dependent
-// loads per node; a lone warp takes as long per node whatever the number of its lanes that take part.  32 cubes
-// share the most node records, but a round of a few ten thousand cubes then occupies a fraction of the resident
-// warps and lasts as long as its slowest warp (a 32-cube union of ~20 K nodes).  Narrower batches make more,
-// shorter walks: the width is the largest power of two that still yields `P.batches_per_warp` batches per resident warp.
-__device__ __forceinline__ uint32_t batch_width(const LightParams &P, uint32_t n, uint32_t n_warps) {
-    if (P.batch_width) return P.batch_width;
-    uint32_t w = 32;
-    while (w > P.min_batch_width && (uint64_t)n < (uint64_t)n_warps * P.batches_per_warp * w) w >>= 1;
-    return w;
-}
-
-__global__ void __launch_bounds__(128, AICB_LIGHT_MIN_BLOCKS) k_compute(const LightParams P, uint32_t n, const int32_t *explicit_cubes) {
-    __shared__ float s_lut[256];
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lut[i] = P.scene.tables[i];
-    __syncthreads();
-    if (!explicit_cubes) n = P.scalars[0];   // the round's list
-    unsigned long long total_visits = 0;
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t n_warps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t width = batch_width(P, n, n_warps);
-    // batches of `width` consecutive list entries, handed out by a counter: a warp whose cubes see open air walks
-    // ten times the nodes of one whose cubes are enclosed
-    for (;;) {
-        uint32_t batch = 0;
-        if (explicit_cubes) {
-            batch = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // (one batch per warp: the grid covers n)
-        } else {
-            if (lane == 0) batch = atomicAdd(P.scalars + 7, 1u);
-            batch = __shfl_sync(0xffffffffu, batch, 0);
-        }
-        const uint32_t base = batch * (explicit_cubes ? 32u : width);
-        if (base >= n) break;
-        const uint32_t i = base + lane;
-        const bool active = i < n && (explicit_cubes || lane < width);
-        int x = 0, y = 0, z = 0;
-        if (active) {
-            if (explicit_cubes) {
-                x = explicit_cubes[3 * i]; y = explicit_cubes[3 * i + 1]; z = explicit_cubes[3 * i + 2];
-            } else {
-                cube_of(P.scene, P.list[i], x, y, z);
-            }
-        }
-        uint32_t visits = 0;
-        const uint32_t nv = compute_light_lockstep<false>(P, s_lut, active, x, y, z, 0, &visits);
-        if (active) P.new_light[i] = nv;
-        total_visits += visits;
-        if (explicit_cubes) break;
-    }
-    for (int off = 16; off > 0; off >>= 1) total_visits += __shfl_down_sync(0xffffffffu, total_visits, off);
-    if (lane == 0 && total_visits) atomicAdd(reinterpret_cast<unsigned long long *>(P.scalars + 4), total_visits);
-}
-
 // compute_light / the dependency re-queue with the chain walk (light_kernel.cuh: compute_light_chains): one warp per
 // cube, cubes handed out by a counter.  k_walk_chains<false> writes new_light for the round's list (or explicit
 // cubes); a cube one of whose chains needs more than LIGHT_CHAIN_K terms goes to the overflow list and is computed by
-// the lockstep walk (k_compute_overflow).  k_walk_chains<true> is k_mark for the entries of `changed`.
+// the lockstep walk (k_compute_overflow).  k_walk_chains<true> re-queues the dependencies of the entries of `changed`.
 template <bool MARK>
 __global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(const LightParams P, uint32_t n, const int32_t *explicit_cubes) {
     __shared__ float s_lut[256];
@@ -448,8 +384,12 @@ __global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(c
     if (!MARK && lane == 0 && total_visits) atomicAdd(reinterpret_cast<unsigned long long *>(P.scalars + 4), total_visits);
 }
 
+// 8 CTAs of 4 warps per SM (64 registers; the records requested ahead spill to L1-resident local memory): the walk is
+// latency bound, so 32 resident warps serve it better than the 20 that 94 registers would allow.
+constexpr int LOCKSTEP_MIN_BLOCKS = 8;
+
 // the cubes the chain walk could not hold (scalars[9] entries of `overflow`), by the lockstep walk
-__global__ void __launch_bounds__(128, AICB_LIGHT_MIN_BLOCKS) k_compute_overflow(const LightParams P, const int32_t *explicit_cubes) {
+__global__ void __launch_bounds__(128, LOCKSTEP_MIN_BLOCKS) k_compute_overflow(const LightParams P, const int32_t *explicit_cubes) {
     __shared__ float s_lut[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lut[i] = P.scene.tables[i];
     __syncthreads();
@@ -466,7 +406,7 @@ __global__ void __launch_bounds__(128, AICB_LIGHT_MIN_BLOCKS) k_compute_overflow
             else cube_of(P.scene, P.list[i], x, y, z);
         }
         uint32_t visits = 0;
-        const uint32_t nv = compute_light_lockstep<false>(P, s_lut, active, x, y, z, 0, &visits);
+        const uint32_t nv = compute_light_lockstep(P, s_lut, active, x, y, z, &visits);
         if (active) P.new_light[i] = nv;
         total_visits += visits;
     }
@@ -474,7 +414,7 @@ __global__ void __launch_bounds__(128, AICB_LIGHT_MIN_BLOCKS) k_compute_overflow
     if (lane == 0 && total_visits) atomicAdd(reinterpret_cast<unsigned long long *>(P.scalars + 4), total_visits);
 }
 
-// apply_light_update (updater.rs:295-363) minus the dependency re-queue (k_mark)
+// apply_light_update (updater.rs:295-363) minus the dependency re-queue (k_walk_chains<true>)
 __global__ void k_apply(const LightParams P) {
     const uint32_t n = P.scalars[0];
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -508,8 +448,8 @@ __global__ void k_apply(const LightParams P) {
 }
 
 // apply_light_update re-queues a cube's dependencies only when its packed difference exceeds 1 (updater.rs:355-360).
-// The entries of the round's list that did are compacted (in list order within a block of 256) so that the warps of
-// k_mark walk the chart for 32 cubes that all need it.
+// The entries of the round's list that did are compacted (in list order within a block of 256) so that
+// k_walk_chains<true> walks the chart only for cubes that need it.
 __global__ void __launch_bounds__(256) k_compact_changed(const LightParams P) {
     __shared__ uint32_t s_part[8], s_base;
     const uint32_t n = P.scalars[0];
@@ -532,28 +472,6 @@ __global__ void __launch_bounds__(256) k_compact_changed(const LightParams P) {
         __syncthreads();
         if (keep) P.changed[s_base + s_part[wid] + inc - 1] = i;
         __syncthreads();
-    }
-}
-
-// the dependency re-queue of apply_light_update (updater.rs:355-360): re-walk the chart, raising the
-// queue priority of every cube whose light was read
-__global__ void __launch_bounds__(128, AICB_LIGHT_MIN_BLOCKS) k_mark(const LightParams P) {
-    const uint32_t n = P.scalars[6];   // entries of the round's list that changed by more than one unit
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t n_warps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t width = batch_width(P, n, n_warps);
-    for (;;) {
-        uint32_t batch = 0;
-        if (lane == 0) batch = atomicAdd(P.scalars + 8, 1u);
-        batch = __shfl_sync(0xffffffffu, batch, 0);
-        const uint32_t base = batch * width;
-        if (base >= n) break;
-        const bool active = base + lane < n && lane < width;
-        const uint32_t i = active ? P.changed[base + lane] : 0u;
-        const int d = active ? (int)P.diff[i] : 0;
-        int x = 0, y = 0, z = 0;
-        if (active) cube_of(P.scene, P.list[i], x, y, z);
-        compute_light_lockstep<true>(P, P.scene.tables, active, x, y, z, (uint32_t)(d / 2 + 1), nullptr);
     }
 }
 
@@ -618,7 +536,6 @@ LightParams make_params(aicb_scene *s) {
     std::memset(&P, 0, sizeof P);
     P.scene = s->ds;
     P.blocks = s->d_light_blocks;
-    P.chart = s->ctx->d_chart;
     P.chart_pre = s->ctx->d_chart_pre;
     P.sky_term = s->d_sky_term;
     P.chains = s->ctx->d_chains;
@@ -627,7 +544,7 @@ LightParams make_params(aicb_scene *s) {
     P.n_chains = s->ctx->n_chains;
     P.n_euler = s->ctx->n_euler;
     P.term_scratch = s->ctx->d_term_scratch;
-    P.overflow = s->d_changed;   // (k_compute's overflow list and k_mark's work list are never live together)
+    P.overflow = s->d_changed;   // (k_walk_chains<false>'s overflow list and k_walk_chains<true>'s work list are never live together)
     P.chart_nodes = s->ctx->chart_nodes;
     P.tile_max = s->d_tile_max;
     P.changed = s->d_changed;
@@ -696,36 +613,14 @@ aicb_status ensure_light_state(aicb_scene *s) {
     return AICB_OK;
 }
 
-// AICB_LIGHT_WALK=lockstep selects the previous walk (32 cubes per warp in lockstep) for comparisons
-bool use_chain_walk() {
-    const char *e = getenv("AICB_LIGHT_WALK");
-    return !(e && std::strcmp(e, "lockstep") == 0);
-}
-
 // evaluate_light (space.rs:1496-1527): rounds until the highest queued priority is <= from_difference(epsilon)
 aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits) {
     aicb_ctx *ctx = s->ctx;
     cudaStream_t st = ctx->stream;
     LightParams P = make_params(s);
     P.epsilon_priority = (uint32_t)epsilon / 2 + 1;
-    {
-        // Cubes within 16 priority levels of the round's maximum are relaxed together: far fewer rounds than strict
-        // level-by-level relaxation (few cubes per round leave the GPU idle) for 8 % more updates; the parity
-        // contract (tests/test_gpu_light.py) holds for every band, 0 = one level per round, 255 = all pending cubes.
-        const char *e = getenv("AICB_LIGHT_BAND");
-        P.priority_band = e ? (uint32_t)atoi(e) : 16u;
-        const char *w = getenv("AICB_LIGHT_WIDTH");        // experiments: a fixed batch width (1..32)
-        P.batch_width = w ? (uint32_t)atoi(w) : 0u;
-        const char *b = getenv("AICB_LIGHT_BATCHES_PER_WARP");
-        P.batches_per_warp = b ? (uint32_t)atoi(b) : 2u;
-        const char *m = getenv("AICB_LIGHT_MIN_WIDTH");
-        P.min_batch_width = m ? (uint32_t)atoi(m) : 4u;
-        if (P.batch_width > 32) P.batch_width = 32;
-        if (P.batches_per_warp < 1) P.batches_per_warp = 1;
-        if (P.min_batch_width < 1) P.min_batch_width = 1;
-    }
     const int blocks = ctx->num_sms * 8;
-    const int wide = ctx->num_sms * 8;    // 128-thread blocks of the lockstep kernels (one warp per 32 list entries, grid-stride)
+    const int wide = ctx->num_sms * 8;    // 128-thread blocks of k_compute_overflow and k_apply (grid-stride)
     const uint32_t n_tiles = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
     uint64_t total = 0, visits = 0, rounds = 0;
     uint32_t maxd = 0;
@@ -733,30 +628,22 @@ aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, ui
     CU(cudaMemsetAsync(s->d_scalars, 0, 16 * 4, st));
     k_tile_rebuild<<<blocks, 256, 0, st>>>(P, n_tiles);   // (fast_evaluate / edits write the priority bytes directly)
     const int ROUNDS_PER_SYNC = 8;
-    const bool chains = use_chain_walk();
     for (int batch = 0; batch < 100000; batch++) {
         for (int round = 0; round < ROUNDS_PER_SYNC; round++) {
             CU(cudaMemsetAsync(s->d_scalars, 0, 2 * 4, st));   // this round's count and priority
             CU(cudaMemsetAsync(s->d_scalars + 6, 0, 4 * 4, st));   // ... its count of changed cubes, the two work counters, the overflow count
             k_find_max<<<16, 256, 0, st>>>(P, n_tiles);
             k_gather<<<blocks, 256, 0, st>>>(P, n_tiles);
-            if (chains) {
-                k_walk_chains<false><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
-                k_compute_overflow<<<wide, 128, 0, st>>>(P, nullptr);
-            } else {
-                k_compute<<<wide, 128, 0, st>>>(P, 0, nullptr);
-            }
+            k_walk_chains<false><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
+            k_compute_overflow<<<wide, 128, 0, st>>>(P, nullptr);
             k_apply<<<wide, 128, 0, st>>>(P);
             k_compact_changed<<<blocks, 256, 0, st>>>(P);
-            if (chains) k_walk_chains<true><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
-            else k_mark<<<wide, 128, 0, st>>>(P);
+            k_walk_chains<true><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
         }
         uint32_t h[8];
         CU(cudaMemcpyAsync(h, s->d_scalars, 8 * 4, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         CU(cudaGetLastError());
-        if (getenv("AICB_LIGHT_TRACE"))
-            fprintf(stderr, "[aicb200 light] batch %d: last round %u cubes at priority %u; %u updates so far\n", batch, h[0], h[1], h[3]);
         total = h[3];
         visits = (uint64_t)h[4] | ((uint64_t)h[5] << 32);
         maxd = h[2];
@@ -900,12 +787,8 @@ aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t 
     CU(cudaMalloc(&d_cubes, n * 12));
     CU(cudaMemcpy(d_cubes, cubes, n * 12, cudaMemcpyHostToDevice));
     cudaMemsetAsync(s->d_scalars, 0, 16 * 4, s->ctx->stream);
-    if (use_chain_walk()) {
-        k_walk_chains<false><<<s->ctx->chain_walk_blocks, 128, 0, s->ctx->stream>>>(P, (uint32_t)n, d_cubes);
-        k_compute_overflow<<<s->ctx->num_sms * 8, 128, 0, s->ctx->stream>>>(P, d_cubes);
-    } else {
-        k_compute<<<(unsigned)((n + 127) / 128), 128, 0, s->ctx->stream>>>(P, (uint32_t)n, d_cubes);
-    }
+    k_walk_chains<false><<<s->ctx->chain_walk_blocks, 128, 0, s->ctx->stream>>>(P, (uint32_t)n, d_cubes);
+    k_compute_overflow<<<s->ctx->num_sms * 8, 128, 0, s->ctx->stream>>>(P, d_cubes);
     uint32_t h[16];
     cudaError_t e = cudaMemcpyAsync(out, s->d_new_light, n * 4, cudaMemcpyDeviceToHost, s->ctx->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(h, s->d_scalars, sizeof h, cudaMemcpyDeviceToHost, s->ctx->stream);

@@ -256,21 +256,16 @@ constexpr uint32_t BOUNCE_OFF = 0, BOUNCE_PRIMARY = 1, BOUNCE_SECONDARY = 2;  //
 constexpr int TILE_W = 8, TILE_H = 4;
 constexpr int WARPS_PER_BLOCK = 4;
 constexpr int N_BINS = 8;            // chord-length classes of the ray list (longest first)
-#ifndef AICB_HIT_CHUNK
-#define AICB_HIT_CHUNK 8
-#endif
-constexpr uint32_t HIT_CHUNK = AICB_HIT_CHUNK;   // hit slots a lane takes from the stream at a time (one atomic per chunk)
+constexpr uint32_t HIT_CHUNK = 8;   // hit slots a lane takes from the stream at a time (one atomic per chunk)
 constexpr uint32_t HIT_NONE = 0xffffffffu;
 // Resident marching blocks per SM the register budget is sized for (65536 registers / (128 threads x 5) = 96 registers).
 // For sm_90a the Volumetric kernels then spill a few dozen bytes to L1-resident local memory; 4 blocks (no spills) were
 // measured on an H100 SXM (700 W) 2.5 % faster on the C2 bench frame but 3-4 % slower on C1 and C3, so 5 stays.
-#ifndef AICB_MIN_BLOCKS
-#define AICB_MIN_BLOCKS 5
-#endif
-#ifndef AICB_STREAM_HINTS
-#define AICB_STREAM_HINTS 0
-#endif
-constexpr int MIN_BLOCKS_PER_SM = AICB_MIN_BLOCKS;
+constexpr int MIN_BLOCKS_PER_SM = 5;
+// The marching loop's exits (TraceParams::event_threshold, tail_divisor, refill_threshold; launch_trace sets them):
+// leave the loop once 24 lanes wait; once the ray list is exhausted, once half of the lanes that still have a ray
+// wait; and run the lean per-lane loop once at most 4 lanes of a warp still march.
+constexpr uint32_t EVENT_THRESHOLD = 24, TAIL_DIVISOR = 2, REFILL_THRESHOLD = 4;
 
 
 constexpr double D_INF = __builtin_huge_val();
@@ -309,22 +304,8 @@ struct Level {
     uint32_t base;
 };
 
-// The per-ray / per-hit streams are written once and read once: with AICB_STREAM_HINTS they bypass the
-// usual L2 retention (evict-first) so that the cell / brick volumes stay resident.
-AICB_DEV uint4 ld_stream(const uint4 *p) {
-#if AICB_STREAM_HINTS
-    return __ldcs(p);
-#else
-    return __ldg(p);
-#endif
-}
-AICB_DEV void st_stream(uint4 *p, uint4 v) {
-#if AICB_STREAM_HINTS
-    __stcs(p, v);
-#else
-    *p = v;
-#endif
-}
+AICB_DEV uint4 ld_stream(const uint4 *p) { return __ldg(p); }
+AICB_DEV void st_stream(uint4 *p, uint4 v) { *p = v; }
 
 AICB_DEV int signum_101(double x) { return (x == 0.0 || x != x) ? 0 : (x < 0.0 ? -1 : 1); }
 

@@ -16,8 +16,6 @@ cam = scenes.standard_camera(space, opts, w, h)
 r = aicb200.RtRenderer(cam)
 r.update(space)
 for shard in (None, (16, 2, 8)):
-    for thr in (sys.argv[2].split(",") if len(sys.argv) > 2 else ["24"]):
-        os.environ["AICB_EVENT_THRESHOLD"] = thr
-        print("shard", shard, "thr", thr, flush=True)
-        for i in range(3):
-            r.draw(shard=shard)
+    print("shard", shard, flush=True)
+    for i in range(3):
+        r.draw(shard=shard)
