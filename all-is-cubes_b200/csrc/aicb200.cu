@@ -38,8 +38,6 @@ static aicb_status cuda_fail(cudaError_t e, const char *what) { return aicb_cuda
 void aicb_light_scene_init(aicb_scene *s, const aicb_scene_desc *d);   // light.cu
 aicb_status aicb_light_scene_upload(aicb_scene *s, const aicb_scene_desc *d);
 aicb_status aicb_light_blocks_update(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
-void aicb_light_scene_free(aicb_scene *s);
-void aicb_light_ctx_free(aicb_ctx *c);
 
 // PackedLight::some -> scalar_in (light/data.rs:213-217)
 static uint8_t scalar_in(float v) {
@@ -311,18 +309,6 @@ static uint32_t shard_rows(uint32_t fb_height, const aicb_shard *sh) {
     return rows;
 }
 
-static aicb_status ensure(void **p, size_t *cur, size_t want) {
-    if (*cur >= want) return AICB_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cur = 0;
-    CU(cudaMalloc(p, want));
-    *cur = want;
-    return AICB_OK;
-}
-
-aicb_status aicb_ensure_device(void **p, size_t *cur, size_t want) { return ensure(p, cur, want); }
-
 // The compositing kernels of a frame's target (TGT_*): resolve_kernel with None / Flat lighting, encode_kernel after
 // shade_kernel.
 static kernel_fn resolve_for(int lc, int tgt) {
@@ -428,7 +414,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         P.text_start = out.text_start;
     }
     const int tgt = tex ? TGT_TEX : (term ? TGT_TERM : TGT_FRAME);
-    P.counters = ctx->d_counters;
+    P.counters = ctx->d_counters.get<unsigned long long>();
     P.task_counter = ctx->d_tile_counter;
     P.refill_threshold = REFILL_THRESHOLD;
     P.tail_divisor = TAIL_DIVISOR;
@@ -462,47 +448,28 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         if (fit < CHUNK) CHUNK = fit & ~(uint64_t)127;
     }
     const uint64_t chunk_cap = total_tasks < CHUNK ? total_tasks : CHUNK;
-    {
-        aicb_status st = ensure(&ctx->d_rays, &ctx->d_rays_bytes, chunk_cap * (sizeof(RayRecordA) + sizeof(RayRecordB)) + 16);
-        if (st != AICB_OK) return st;
-        st = ensure(&ctx->d_task_cb, &ctx->d_task_cb_bytes, chunk_cap * sizeof(TaskOut) + 16);
-        if (st != AICB_OK) return st;
-        uint64_t cap = chunk_cap * ctx->hits_per_task;
-        if (cap < (1u << 16)) cap = 1u << 16;
-        if (cap > 0xfffffff0ull) cap = 0xfffffff0ull;
-        cap &= ~(uint64_t)(HIT_CHUNK - 1);  // lanes take whole chunks of the stream
-        P.hit_capacity = (uint32_t)cap;
-        st = ensure(&ctx->d_hits, &ctx->d_hits_bytes, cap * sizeof(HitRecord) + 64);
-        if (st != AICB_OK) return st;
-        if (!fused) {
-            st = ensure(&ctx->d_contrib, &ctx->d_contrib_bytes, cap * sizeof(ShadedHit) + 64);
-            if (st != AICB_OK) return st;
-        }
-        st = ensure(&ctx->d_bin_list, &ctx->d_bin_list_bytes, (size_t)N_BINS * chunk_cap * 4 + 64);
-        if (st != AICB_OK) return st;
-    }
-    // the listed rays' records: array A (64-byte aligned: cudaMalloc aligns to 256 bytes), then array B
-    P.rays_a = (RayRecordA *)ctx->d_rays;
-    P.rays_b = (RayRecordB *)((char *)ctx->d_rays + chunk_cap * sizeof(RayRecordA));
+    uint64_t cap = chunk_cap * ctx->hits_per_task;
+    if (cap < (1u << 16)) cap = 1u << 16;
+    if (cap > 0xfffffff0ull) cap = 0xfffffff0ull;
+    cap &= ~(uint64_t)(HIT_CHUNK - 1);  // lanes take whole chunks of the stream
+    P.hit_capacity = (uint32_t)cap;
+    TRY(ctx->primary.size(chunk_cap, P.hit_capacity, !fused));
+    ctx->primary.bind(P, chunk_cap, !fused);
     P.ray_counter = ctx->d_tile_counter + 2;
-    P.task_out = (TaskOut *)ctx->d_task_cb;
-    P.hits = (HitRecord *)ctx->d_hits;
-    P.shaded = fused ? nullptr : (ShadedHit *)ctx->d_contrib;
     sc->pending_fused = fused;
     P.hit_counter = ctx->d_tile_counter + 1;
     P.bin_count = ctx->d_tile_counter + 4;
-    P.bin_list = (uint32_t *)ctx->d_bin_list;
     P.bin_stride = (uint32_t)chunk_cap;
-    P.overflow_flag = (unsigned int *)(ctx->d_counters + 7);
-    if (stream != ctx->stream) CU(cudaStreamWaitEvent(stream, ctx->ev_delta, 0));  // pending cube edits
+    P.overflow_flag = (unsigned int *)(P.counters + 7);
+    if (stream != ctx->stream.get()) CU(cudaStreamWaitEvent(stream, ctx->ev_delta.get(), 0));  // pending cube edits
     // The per-frame streams, counters and events belong to the context: a frame issued on another stream than the
     // previous one must not start before that one is through with them.
-    if (ctx->frame_in_flight && ctx->last_stream != stream) CU(cudaStreamWaitEvent(stream, ctx->ev1, 0));
+    if (ctx->frame_in_flight && ctx->last_stream != stream) CU(cudaStreamWaitEvent(stream, ctx->ev1.get(), 0));
     ctx->frame_in_flight = true;
     ctx->last_stream = stream;
     ctx->last_scene = sc;
-    CU(cudaMemsetAsync(ctx->d_counters, 0, 8 * sizeof(unsigned long long) + 2 * (4 + N_BINS) * sizeof(unsigned int), stream));
-    CU(cudaEventRecord(ctx->ev0, stream));
+    CU(cudaMemsetAsync(P.counters, 0, 8 * sizeof(unsigned long long) + 2 * (4 + N_BINS) * sizeof(unsigned int), stream));
+    CU(cudaEventRecord(ctx->ev0.get(), stream));
     if (total_tasks > 0) {
         const bool volumetric = opt->transparency == AICB_TRANSPARENCY_VOLUMETRIC;
         const int lc = opt->lighting_display == AICB_LIGHT_NONE ? LC_NONE
@@ -512,15 +479,10 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         TraceParams Q;
         const bool bounce = lc == LC_BOUNCE;
         if (bounce) {
-            aicb_status st = ensure(&ctx->d_rays2, &ctx->d_rays2_bytes, chunk_cap * (sizeof(RayRecordA) + sizeof(RayRecordB)) + 16);
-            if (st == AICB_OK) st = ensure(&ctx->d_task_cb2, &ctx->d_task_cb2_bytes, chunk_cap * sizeof(TaskOut) + 16);
-            if (st == AICB_OK) st = ensure(&ctx->d_hits2, &ctx->d_hits2_bytes, (size_t)P.hit_capacity * sizeof(HitRecord) + 64);
-            if (st == AICB_OK) st = ensure(&ctx->d_contrib2, &ctx->d_contrib2_bytes, (size_t)P.hit_capacity * sizeof(ShadedHit) + 64);
-            if (st == AICB_OK) st = ensure(&ctx->d_bin_list2, &ctx->d_bin_list2_bytes, (size_t)N_BINS * chunk_cap * 4 + 64);
+            TRY(ctx->secondary.size(chunk_cap, P.hit_capacity, true));
             // per task: request (4) + RNG state (32) + Rgb sum and steps (16) + the secondary ray (48) + record index (4)
-            if (st == AICB_OK) st = ensure(&ctx->d_bounce, &ctx->d_bounce_bytes, chunk_cap * 104 + 256);
-            if (st != AICB_OK) return st;
-            char *b = (char *)ctx->d_bounce;
+            TRY(ctx->d_bounce.ensure(chunk_cap * 104 + 256));
+            char *b = ctx->d_bounce.get<char>();
             P.bounce_mode = BOUNCE_PRIMARY;
             P.bounce_samples = opt->bounce_samples;
             P.bounce_rays = (double *)b;                                   // 48 B per task, 16-aligned
@@ -546,12 +508,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.in_accum = nullptr; Q.out_accum = nullptr; Q.has_backdrop = 0; Q.has_no_world = 0;
             Q.pixel_list = nullptr; Q.in_depth = nullptr; Q.out_task_depth = nullptr; Q.out_tex_depth = nullptr;
             Q.out_term = nullptr; Q.in_text = nullptr; Q.out_task_text = nullptr;
-            Q.rays_a = (RayRecordA *)ctx->d_rays2;
-            Q.rays_b = (RayRecordB *)((char *)ctx->d_rays2 + chunk_cap * sizeof(RayRecordA));
-            Q.task_out = (TaskOut *)ctx->d_task_cb2;
-            Q.hits = (HitRecord *)ctx->d_hits2;
-            Q.shaded = (ShadedHit *)ctx->d_contrib2;
-            Q.bin_list = (uint32_t *)ctx->d_bin_list2;
+            ctx->secondary.bind(Q, chunk_cap, true);
             Q.task_counter = ctx->d_tile_counter + (4 + N_BINS);
             Q.hit_counter = Q.task_counter + 1;
             Q.ray_counter = Q.task_counter + 2;
@@ -569,36 +526,36 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             if (!first) CU(cudaMemsetAsync(ctx->d_tile_counter, 0, (4 + N_BINS) * sizeof(unsigned int), stream));
             const bool prof = ctx->profile_kernels && first;
             const bool stage = first && ctx->stage_timing;
-            if (stage) cudaEventRecord(ctx->ev_k[0], stream);
+            if (stage) cudaEventRecord(ctx->ev_k[0].get(), stream);
             gen_kernel<<<(n + 127) / 128, 128, 0, stream>>>(P, n);
-            if (stage) cudaEventRecord(ctx->ev_k[1], stream);
+            if (stage) cudaEventRecord(ctx->ev_k[1].get(), stream);
             uint64_t want = ((uint64_t)n + WARPS_PER_BLOCK * 32 - 1) / (WARPS_PER_BLOCK * 32);
             uint64_t grid = (uint64_t)ctx->num_sms * blocks_per_sm;  // persistent: a multiple of the SM count
             if (grid > want) grid = want;
             if (prof) {
-                if (!ctx->d_debug) cudaMalloc(&ctx->d_debug, 4 * 8 * (size_t)ctx->num_sms * 64 * WARPS_PER_BLOCK);
-                P.debug_warp_times = (unsigned long long *)ctx->d_debug;
+                TRY(ctx->d_debug.ensure(4 * 8 * (size_t)ctx->num_sms * 64 * WARPS_PER_BLOCK));
+                P.debug_warp_times = ctx->d_debug.get<unsigned long long>();
                 ctx->debug_warps = (uint32_t)grid * WARPS_PER_BLOCK;
             }
             // the frame's kernels follow each other with programmatic dependent launch (no events between them)
             const bool overlap = !stage && !prof && !bounce;
             CU(launch_after(overlap, k, (unsigned)grid, WARPS_PER_BLOCK * 32, stream, P, n));
             P.debug_warp_times = nullptr;
-            if (stage) cudaEventRecord(ctx->ev_k[2], stream);
+            if (stage) cudaEventRecord(ctx->ev_k[2].get(), stream);
             if (fused) {
                 const unsigned rb = (n + 127) / 128;   // one warp per 32 tasks
                 CU(launch_after(overlap, resolve_for(lc, tgt), rb, 128, stream, P, n));
-                if (stage) cudaEventRecord(ctx->ev_k[3], stream);
+                if (stage) cudaEventRecord(ctx->ev_k[3].get(), stream);
             } else if (!bounce) {
                 switch (lc) {
                     case LC_NONE: CU(launch_after(overlap, shade_kernel<LC_NONE>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
                     case LC_FLAT: CU(launch_after(overlap, shade_kernel<LC_FLAT>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
                     default: CU(launch_after(overlap, shade_kernel<LC_INTERP>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
                 }
-                if (stage) cudaEventRecord(ctx->ev_k[3], stream);
+                if (stage) cudaEventRecord(ctx->ev_k[3].get(), stream);
                 const uint32_t n_pixels = n / P.n_samples;
                 CU(launch_after(overlap, encode_for(tgt), (n_pixels + 127) / 128, 128, stream, P, n));
-                if (stage) cudaEventRecord(ctx->ev_k[4], stream);
+                if (stage) cudaEventRecord(ctx->ev_k[4].get(), stream);
             } else {
                 shade_kernel<LC_BOUNCE><<<ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, 0, stream>>>(P);
                 const unsigned tb = (n + 127) / 128;
@@ -616,15 +573,15 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                     encode_kernel<TGT_FRAME><<<tb, 128, 0, stream>>>(Q, n);
                 }
                 bounce_resolve_kernel<<<tb, 128, 0, stream>>>(P, n);
-                if (stage) cudaEventRecord(ctx->ev_k[3], stream);
+                if (stage) cudaEventRecord(ctx->ev_k[3].get(), stream);
                 const uint32_t n_pixels = n / P.n_samples;
                 encode_for(tgt)<<<(n_pixels + 127) / 128, 128, 0, stream>>>(P, n);
-                if (stage) cudaEventRecord(ctx->ev_k[4], stream);
+                if (stage) cudaEventRecord(ctx->ev_k[4].get(), stream);
             }
         }
         CU(cudaGetLastError());
     }
-    CU(cudaEventRecord(ctx->ev1, stream));
+    CU(cudaEventRecord(ctx->ev1.get(), stream));
     return AICB_OK;
 }
 
@@ -632,17 +589,17 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
     aicb_ctx *ctx = sc->ctx;
     if (ctx->last_scene != sc)
         return fail(AICB_ERR_BUSY, "the context's last frame belongs to another scene (one frame per context is tracked)");
-    CU(cudaEventSynchronize(ctx->ev1));
+    CU(cudaEventSynchronize(ctx->ev1.get()));
     ctx->frame_in_flight = false;
     unsigned long long c[8];
-    CU(cudaMemcpy(c, ctx->d_counters, sizeof c, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(c, ctx->d_counters.get(), sizeof c, cudaMemcpyDeviceToHost));
     sc->pending = false;
     if (ctx->profile_kernels && sc->pending_rays) {  // AICB_PROFILE_KERNELS=1: per-kernel times of the first chunk
         float t[4] = {0, 0, 0, 0};
-        for (int i = 0; i < (sc->pending_fused ? 3 : 4); i++) cudaEventElapsedTime(&t[i], ctx->ev_k[i], ctx->ev_k[i + 1]);
+        for (int i = 0; i < (sc->pending_fused ? 3 : 4); i++) cudaEventElapsedTime(&t[i], ctx->ev_k[i].get(), ctx->ev_k[i + 1].get());
         if (ctx->d_debug && ctx->debug_warps) {
             std::vector<unsigned long long> w(4 * (size_t)ctx->debug_warps);
-            cudaMemcpy(w.data(), ctx->d_debug, w.size() * 8, cudaMemcpyDeviceToHost);
+            cudaMemcpy(w.data(), ctx->d_debug.get(), w.size() * 8, cudaMemcpyDeviceToHost);
             unsigned long long t0 = ~0ull, t1 = 0, passes = 0, rays = 0;
             for (uint32_t i = 0; i < ctx->debug_warps; i++) { t0 = std::min(t0, w[4 * i]); t1 = std::max(t1, w[4 * i + 1]); passes += w[4 * i + 2]; rays += w[4 * i + 3]; }
             std::vector<double> ends;
@@ -673,10 +630,8 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
         if (++ctx->shallow_frames >= 16) {
             ctx->hits_per_task /= 4;
             ctx->shallow_frames = 0;
-            if (ctx->d_hits) { cudaFree(ctx->d_hits); ctx->d_hits = nullptr; ctx->d_hits_bytes = 0; }
-            if (ctx->d_contrib) { cudaFree(ctx->d_contrib); ctx->d_contrib = nullptr; ctx->d_contrib_bytes = 0; }
-            if (ctx->d_hits2) { cudaFree(ctx->d_hits2); ctx->d_hits2 = nullptr; ctx->d_hits2_bytes = 0; }
-            if (ctx->d_contrib2) { cudaFree(ctx->d_contrib2); ctx->d_contrib2 = nullptr; ctx->d_contrib2_bytes = 0; }
+            ctx->primary.release_hits();
+            ctx->secondary.release_hits();
         }
     } else {
         ctx->shallow_frames = 0;
@@ -684,11 +639,11 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
     if (info) {
         std::memset(info, 0, sizeof *info);
         float ms = 0.0f;
-        CU(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
+        CU(cudaEventElapsedTime(&ms, ctx->ev0.get(), ctx->ev1.get()));
         info->kernel_ms = ms;
         if (sc->pending_rays && ctx->stage_timing)   // a fused frame: [2] is resolve_kernel, [3] stays 0
             for (int i = 0; i < (sc->pending_fused ? 3 : 4); i++)
-                cudaEventElapsedTime(&info->stage_ms[i], ctx->ev_k[i], ctx->ev_k[i + 1]);
+                cudaEventElapsedTime(&info->stage_ms[i], ctx->ev_k[i].get(), ctx->ev_k[i + 1].get());
         info->cubes_traced = c[0];
         info->rays = sc->pending_rays;
         for (int i = 0; i < 5; i++) info->counters[i] = c[1 + i];
@@ -727,27 +682,28 @@ aicb_status aicb_ctx_create(int device_id, aicb_ctx **out) {
     CU(cudaGetDeviceProperties(&prop, device_id));
     if (prop.major != 9 || prop.minor != 0)   // sm_90a code loads on compute capability 9.0 only
         return fail(AICB_ERR_CUDA, "device is not compute capability 9.0; this library is built for sm_90a only");
-    aicb_ctx *c = new aicb_ctx();
+    // the context is the caller's once every step has succeeded; until then a failure frees what was created
+    std::unique_ptr<aicb_ctx> c(new aicb_ctx());
     c->device = device_id;
     c->num_sms = prop.multiProcessorCount;
-    CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CU(cudaEventCreate(&c->ev0));
-    CU(cudaEventCreate(&c->ev1));
+    cudaStream_t stream = nullptr;
+    CU(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+    c->stream.reset(stream);
+    TRY(create_event(c->ev0, cudaEventDefault));
+    TRY(create_event(c->ev1, cudaEventDefault));
     c->profile_kernels = getenv("AICB_PROFILE_KERNELS") != nullptr;
-    for (int i = 0; i < 5; i++) CU(cudaEventCreate(&c->ev_k[i]));
-    CU(cudaEventCreateWithFlags(&c->ev_delta, cudaEventDisableTiming));
-    // the frame counters (8 x u64) and the per-chunk counters (4 + N_BINS x u32) share one allocation: one memset per frame
-    CU(cudaMalloc(&c->d_counters, 8 * sizeof(unsigned long long) + 2 * (4 + N_BINS) * sizeof(unsigned int)));  // + the secondary (Bounce) pass's block
-    c->d_tile_counter = (unsigned int *)(c->d_counters + 8);
+    for (int i = 0; i < 5; i++) TRY(create_event(c->ev_k[i], cudaEventDefault));
+    TRY(create_event(c->ev_delta, cudaEventDisableTiming));
+    TRY(c->d_counters.ensure(8 * sizeof(unsigned long long) + 2 * (4 + N_BINS) * sizeof(unsigned int)));
+    c->d_tile_counter = (unsigned int *)(c->d_counters.get<unsigned long long>() + 8);
     // PackedLight decode table (light/data.rs:232-243 scalar_out_arithmetic; table :301-354)
     float lut[768];
     lut[0] = 0.0f;
     for (int i = 1; i < 256; i++) lut[i] = (float)std::exp2((double)(((float)i - 144.0f) / 10.0f));
     build_srgb_thresholds(lut + 256);
     build_light_thresholds(lut + 512);
-    CU(cudaMalloc(&c->d_lut, sizeof lut));
-    CU(cudaMemcpy(c->d_lut, lut, sizeof lut, cudaMemcpyHostToDevice));
-    *out = c;
+    TRY(c->d_lut.upload(lut, sizeof lut));
+    *out = c.release();
     return AICB_OK;
 }
 
@@ -763,30 +719,6 @@ aicb_status aicb_ctx_stage_timing(aicb_ctx *c, int enable) {
 void aicb_ctx_destroy(aicb_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    if (c->d_out) cudaFree(c->d_out);
-    if (c->d_aux) cudaFree(c->d_aux);
-    if (c->d_rays) cudaFree(c->d_rays);
-    if (c->d_task_cb) cudaFree(c->d_task_cb);
-    if (c->d_hits) cudaFree(c->d_hits);
-    if (c->d_contrib) cudaFree(c->d_contrib);
-    if (c->d_bin_list) cudaFree(c->d_bin_list);
-    for (void *q : {c->d_rays2, c->d_task_cb2, c->d_hits2, c->d_contrib2, c->d_bin_list2, c->d_bounce})
-        if (q) cudaFree(q);
-    if (c->d_debug) cudaFree(c->d_debug);
-    if (c->h_delta) cudaFreeHost(c->h_delta);
-    if (c->h_stage) cudaFreeHost(c->h_stage);
-    if (c->d_delta) cudaFree(c->d_delta);
-    if (c->ev_delta) cudaEventDestroy(c->ev_delta);
-    if (c->d_task_aux) cudaFree(c->d_task_aux);
-    if (c->d_task_depth) cudaFree(c->d_task_depth);
-    if (c->d_task_text) cudaFree(c->d_task_text);
-    aicb_light_ctx_free(c);
-    if (c->d_lut) cudaFree(c->d_lut);
-    if (c->d_counters) cudaFree(c->d_counters);
-    if (c->ev0) cudaEventDestroy(c->ev0);
-    if (c->ev1) cudaEventDestroy(c->ev1);
-    for (int i = 0; i < 5; i++) if (c->ev_k[i]) cudaEventDestroy(c->ev_k[i]);
-    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
 
@@ -821,7 +753,8 @@ aicb_status aicb_scene_create(aicb_ctx *ctx, const aicb_scene_desc *d, aicb_scen
         blk_tab[i] = block_entry(kinds[i], recs[i].pal_off, pal_tab, 0);
     }
 
-    aicb_scene *s = new aicb_scene();
+    // the scene is the caller's once every step has succeeded; until then a failure frees what was uploaded
+    std::unique_ptr<aicb_scene> s(new aicb_scene());
     s->ctx = ctx;
     s->volume = (size_t)volume;
     s->block_kind = kinds;
@@ -832,80 +765,57 @@ aicb_status aicb_scene_create(aicb_ctx *ctx, const aicb_scene_desc *d, aicb_scen
     }
     ds.wide_cells = d->n_blocks > 16384 ? 1 : 0;
 
-    auto cleanup = [&](aicb_status st) {
-        aicb_scene_destroy(s);
-        return st;
-    };
-#define CUS(call)                                                        \
-    do {                                                                 \
-        cudaError_t e__ = (call);                                        \
-        if (e__ != cudaSuccess) return cleanup(cuda_fail(e__, #call));   \
-    } while (0)
-
     // ---- cells: block id with its kind in the top bits ------------------------------------------
     if (volume) {
         for (size_t i = 0; i < volume; i++)
-            if (d->block_ids[i] >= d->n_blocks) return cleanup(fail(AICB_ERR_INVALID, "block id out of range"));
+            if (d->block_ids[i] >= d->n_blocks) return fail(AICB_ERR_INVALID, "block id out of range");
         if (ds.wide_cells) {
             std::vector<uint32_t> cells(volume);
-            for (size_t i = 0; i < volume; i++) cells[i] = d->block_ids[i] | ((uint32_t)kinds[d->block_ids[i]] << 16);
-            CUS(cudaMalloc(&s->d_cells, volume * 4));
-            CUS(cudaMemcpy(s->d_cells, cells.data(), volume * 4, cudaMemcpyHostToDevice));
+            for (size_t i = 0; i < volume; i++) cells[i] = cell_word(d->block_ids[i], kinds[d->block_ids[i]], true);
+            TRY(s->d_cells.upload(cells));
             s->device_bytes += volume * 4;
         } else {
             std::vector<uint16_t> cells(volume);
-            for (size_t i = 0; i < volume; i++)
-                cells[i] = (uint16_t)(d->block_ids[i] | ((uint32_t)kinds[d->block_ids[i]] << 14));
-            CUS(cudaMalloc(&s->d_cells, volume * 2));
-            CUS(cudaMemcpy(s->d_cells, cells.data(), volume * 2, cudaMemcpyHostToDevice));
+            for (size_t i = 0; i < volume; i++) cells[i] = (uint16_t)cell_word(d->block_ids[i], kinds[d->block_ids[i]], false);
+            TRY(s->d_cells.upload(cells));
             s->device_bytes += volume * 2;
         }
         if (d->light) {
-            CUS(cudaMalloc(&s->d_light, volume * 4));
-            CUS(cudaMemcpy(s->d_light, d->light, volume * 4, cudaMemcpyHostToDevice));
+            TRY(s->d_light.upload(d->light, volume * 4));
             s->device_bytes += volume * 4;
         }
     }
     if (!recs.empty()) {
-        CUS(cudaMalloc(&s->d_blocks, recs.size() * sizeof(BlockRec)));
-        CUS(cudaMemcpy(s->d_blocks, recs.data(), recs.size() * sizeof(BlockRec), cudaMemcpyHostToDevice));
+        TRY(s->d_blocks.upload(recs));
         s->device_bytes += recs.size() * sizeof(BlockRec);
     }
     s->n_bricks = bricks.size();
     s->n_palette = palette.size();
     if (!bricks.empty()) {
-        CUS(cudaMalloc(&s->d_bricks, bricks.size() * 2));
-        CUS(cudaMemcpy(s->d_bricks, bricks.data(), bricks.size() * 2, cudaMemcpyHostToDevice));
+        TRY(s->d_bricks.upload(bricks));
         s->device_bytes += bricks.size() * 2;
     }
     if (!palette.empty()) {
-        CUS(cudaMalloc(&s->d_palette, palette.size() * sizeof(float4)));
-        CUS(cudaMemcpy(s->d_palette, palette.data(), palette.size() * sizeof(float4), cudaMemcpyHostToDevice));
+        TRY(s->d_palette.upload(palette));
         s->device_bytes += palette.size() * sizeof(float4);
-        CUS(cudaMalloc(&s->d_pal_tab, pal_tab.size() * sizeof(float2)));
-        CUS(cudaMemcpy(s->d_pal_tab, pal_tab.data(), pal_tab.size() * sizeof(float2), cudaMemcpyHostToDevice));
+        TRY(s->d_pal_tab.upload(pal_tab));
         s->device_bytes += pal_tab.size() * sizeof(float2);
     }
     if (!blk_tab.empty()) {
-        CUS(cudaMalloc(&s->d_blk_tab, blk_tab.size() * sizeof(float4)));
-        CUS(cudaMemcpy(s->d_blk_tab, blk_tab.data(), blk_tab.size() * sizeof(float4), cudaMemcpyHostToDevice));
+        TRY(s->d_blk_tab.upload(blk_tab));
         s->device_bytes += blk_tab.size() * sizeof(float4);
     }
-#undef CUS
-    ds.cells = s->d_cells;
-    ds.light = s->d_light;
-    ds.blocks = s->d_blocks;
-    ds.bricks = s->d_bricks;
-    ds.palette = s->d_palette;
-    ds.blk_tab = s->d_blk_tab;
-    ds.pal_tab = s->d_pal_tab;
-    ds.tables = ctx->d_lut;
+    ds.cells = s->d_cells.get();
+    ds.light = s->d_light.get<uint32_t>();
+    ds.blocks = s->d_blocks.get<BlockRec>();
+    ds.bricks = s->d_bricks.get<uint16_t>();
+    ds.palette = s->d_palette.get<float4>();
+    ds.blk_tab = s->d_blk_tab.get<float4>();
+    ds.pal_tab = s->d_pal_tab.get<float2>();
+    ds.tables = ctx->d_lut.get<float>();
     build_block_sky(d->sky, &ds);
-    {
-        aicb_status lst = aicb_light_scene_upload(s, d);
-        if (lst != AICB_OK) return cleanup(lst);
-    }
-    *out = s;
+    TRY(aicb_light_scene_upload(s.get(), d));
+    *out = s.release();
     return AICB_OK;
 }
 
@@ -913,18 +823,10 @@ void aicb_scene_destroy(aicb_scene *s) {
     if (!s) return;
     cudaSetDevice(s->ctx->device);
     if (s->ctx->last_scene == s) {   // its frame (if any) must be through with the scene's arrays
-        if (s->ctx->frame_in_flight) cudaEventSynchronize(s->ctx->ev1);
+        if (s->ctx->frame_in_flight) cudaEventSynchronize(s->ctx->ev1.get());
         s->ctx->last_scene = nullptr;
         s->ctx->frame_in_flight = false;
     }
-    if (s->d_cells) cudaFree(s->d_cells);
-    if (s->d_light) cudaFree(s->d_light);
-    if (s->d_blocks) cudaFree(s->d_blocks);
-    if (s->d_bricks) cudaFree(s->d_bricks);
-    if (s->d_palette) cudaFree(s->d_palette);
-    if (s->d_pal_tab) cudaFree(s->d_pal_tab);
-    if (s->d_blk_tab) cudaFree(s->d_blk_tab);
-    aicb_light_scene_free(s);
     delete s;
 }
 
@@ -949,16 +851,16 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
     // one pinned staging buffer, one H2D copy, one scatter kernel per batch; a cube named twice keeps its
     // last value (the scatter is parallel, so duplicates are resolved here)
     const size_t need = n * sizeof(CubeDelta);
-    if (ctx->h_delta_bytes < need) {
-        if (ctx->h_delta) { cudaEventSynchronize(ctx->ev_delta); cudaFreeHost(ctx->h_delta); cudaFree(ctx->d_delta); }
-        ctx->h_delta = nullptr; ctx->d_delta = nullptr; ctx->h_delta_bytes = 0;
-        size_t cap = need < 65536 ? 65536 : need * 2;
-        CU(cudaMallocHost(&ctx->h_delta, cap));
-        CU(cudaMalloc(&ctx->d_delta, cap));
-        ctx->h_delta_bytes = cap;
+    if (std::min(ctx->h_delta.bytes(), ctx->d_delta.bytes()) < need) {
+        if (ctx->h_delta) cudaEventSynchronize(ctx->ev_delta.get());   // the previous batch's copy may still read it
+        ctx->h_delta.reset();
+        ctx->d_delta.reset();
+        const size_t cap = need < 65536 ? 65536 : need * 2;
+        TRY(ctx->h_delta.ensure(cap));
+        TRY(ctx->d_delta.ensure(cap));
     }
-    CU(cudaEventSynchronize(ctx->ev_delta));  // the previous batch has left the staging buffer
-    CubeDelta *ops = (CubeDelta *)ctx->h_delta;
+    CU(cudaEventSynchronize(ctx->ev_delta.get()));  // the previous batch has left the staging buffer
+    CubeDelta *ops = ctx->h_delta.get<CubeDelta>();
     std::unordered_map<uint32_t, uint32_t> seen;
     seen.reserve(n * 2);
     uint32_t m = 0;
@@ -969,19 +871,18 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
         if (!s->h_ids.empty()) s->h_ids[idx] = ids[i];
         CubeDelta op;
         op.idx = (uint32_t)idx;
-        op.cell = ds.wide_cells ? (ids[i] | ((uint32_t)s->block_kind[ids[i]] << 16))
-                                : (ids[i] | ((uint32_t)s->block_kind[ids[i]] << 14));
+        op.cell = cell_word(ids[i], s->block_kind[ids[i]], ds.wide_cells);
         op.has_light = (light && s->d_light) ? 1u : 0u;
         op.light = 0;
         if (op.has_light) std::memcpy(&op.light, light[i], 4);
         auto it = seen.find(op.idx);
         if (it == seen.end()) { seen.emplace(op.idx, m); ops[m++] = op; } else { ops[it->second] = op; }
     }
-    CU(cudaMemcpyAsync(ctx->d_delta, ops, (size_t)m * sizeof(CubeDelta), cudaMemcpyHostToDevice, ctx->stream));
-    scatter_cubes_kernel<<<(m + 127) / 128, 128, 0, ctx->stream>>>((const CubeDelta *)ctx->d_delta, m, ds.wide_cells, s->d_cells,
-                                                                   s->d_light);
+    CU(cudaMemcpyAsync(ctx->d_delta.get(), ops, (size_t)m * sizeof(CubeDelta), cudaMemcpyHostToDevice, ctx->stream.get()));
+    scatter_cubes_kernel<<<(m + 127) / 128, 128, 0, ctx->stream.get()>>>(ctx->d_delta.get<const CubeDelta>(), m, ds.wide_cells,
+                                                                         s->d_cells.get(), s->d_light.get<uint32_t>());
     CU(cudaGetLastError());
-    CU(cudaEventRecord(ctx->ev_delta, ctx->stream));  // renders on other streams wait for it (launch_trace)
+    CU(cudaEventRecord(ctx->ev_delta.get(), ctx->stream.get()));  // renders on other streams wait for it (launch_trace)
     return AICB_OK;  // stream-ordered before any later render of this context
 }
 
@@ -1022,6 +923,14 @@ aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, cons
     return flatten_update(s, indices, descs, n, recs, kinds, bricks, palette, pal_tab, &any_kind_changed);
 }
 
+// A new buffer `out`: the first `old_bytes` of `old`, then `add_bytes` from the host.
+static aicb_status appended(DeviceBuffer &out, const DeviceBuffer &old, size_t old_bytes, const void *add, size_t add_bytes) {
+    TRY(out.ensure(old_bytes + add_bytes));
+    if (old_bytes) CU(cudaMemcpy(out.get(), old.get(), old_bytes, cudaMemcpyDeviceToDevice));
+    CU(cudaMemcpy(out.get<char>() + old_bytes, add, add_bytes, cudaMemcpyHostToDevice));
+    return AICB_OK;
+}
+
 aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
     if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
     aicb_ctx *ctx = s->ctx;
@@ -1042,48 +951,22 @@ aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, con
 
     // ---- grow the pools: the new arrays are complete before any pointer of the scene changes ----------------
     const size_t n_pal_old = s->n_palette / 2;   // palette entries (2 x float4 each)
-    uint16_t *nb = nullptr;
-    float4 *np = nullptr;
-    float2 *nt = nullptr;
-    auto grow = [&]() -> cudaError_t {
-        cudaError_t e;
-        if (!bricks.empty()) {
-            if ((e = cudaMalloc(&nb, (s->n_bricks + bricks.size()) * 2)) != cudaSuccess) return e;
-            if (s->n_bricks && (e = cudaMemcpy(nb, s->d_bricks, s->n_bricks * 2, cudaMemcpyDeviceToDevice)) != cudaSuccess) return e;
-            if ((e = cudaMemcpy(nb + s->n_bricks, bricks.data(), bricks.size() * 2, cudaMemcpyHostToDevice)) != cudaSuccess) return e;
-        }
-        if (!palette.empty()) {
-            if ((e = cudaMalloc(&np, (s->n_palette + palette.size()) * sizeof(float4))) != cudaSuccess) return e;
-            if (s->n_palette && (e = cudaMemcpy(np, s->d_palette, s->n_palette * sizeof(float4), cudaMemcpyDeviceToDevice)) != cudaSuccess) return e;
-            if ((e = cudaMemcpy(np + s->n_palette, palette.data(), palette.size() * sizeof(float4), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
-            if ((e = cudaMalloc(&nt, (n_pal_old + pal_tab.size()) * sizeof(float2))) != cudaSuccess) return e;
-            if (n_pal_old && (e = cudaMemcpy(nt, s->d_pal_tab, n_pal_old * sizeof(float2), cudaMemcpyDeviceToDevice)) != cudaSuccess) return e;
-            if ((e = cudaMemcpy(nt + n_pal_old, pal_tab.data(), pal_tab.size() * sizeof(float2), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
-        }
-        return cudaSuccess;
-    };
-    {
-        const cudaError_t e = grow();
-        if (e != cudaSuccess) {
-            if (nb) cudaFree(nb);
-            if (np) cudaFree(np);
-            if (nt) cudaFree(nt);
-            return cuda_fail(e, "growing the brick pool / palette");
-        }
+    DeviceBuffer nb, np, nt;
+    if (!bricks.empty()) TRY(appended(nb, s->d_bricks, s->n_bricks * 2, bricks.data(), bricks.size() * 2));
+    if (!palette.empty()) {
+        TRY(appended(np, s->d_palette, s->n_palette * sizeof(float4), palette.data(), palette.size() * sizeof(float4)));
+        TRY(appended(nt, s->d_pal_tab, n_pal_old * sizeof(float2), pal_tab.data(), pal_tab.size() * sizeof(float2)));
     }
     if (nb) {
-        if (s->d_bricks) cudaFree(s->d_bricks);
-        s->d_bricks = nb;
-        s->ds.bricks = nb;
+        s->d_bricks = std::move(nb);
+        s->ds.bricks = s->d_bricks.get<uint16_t>();
         s->device_bytes += bricks.size() * 2;
     }
     if (np) {
-        if (s->d_palette) cudaFree(s->d_palette);
-        if (s->d_pal_tab) cudaFree(s->d_pal_tab);
-        s->d_palette = np;
-        s->ds.palette = np;
-        s->d_pal_tab = nt;
-        s->ds.pal_tab = nt;
+        s->d_palette = std::move(np);
+        s->ds.palette = s->d_palette.get<float4>();
+        s->d_pal_tab = std::move(nt);
+        s->ds.pal_tab = s->d_pal_tab.get<float2>();
         s->device_bytes += palette.size() * sizeof(float4) + pal_tab.size() * sizeof(float2);
     }
     // ---- patch the block table ------------------------------------------------------------------------------
@@ -1093,8 +976,8 @@ aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, con
         const float4 bt = block_entry(kinds[i], r.pal_off, pal_tab, (uint32_t)n_pal_old);
         if (kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)s->n_bricks;
         if (kinds[i] != KIND_INVISIBLE || !descs[i].is_air) r.pal_off += (uint32_t)n_pal_old;
-        CU(cudaMemcpy(s->d_blocks + indices[i], &r, sizeof r, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(s->d_blk_tab + indices[i], &bt, sizeof bt, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(s->d_blocks.get<BlockRec>() + indices[i], &r, sizeof r, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(s->d_blk_tab.get<float4>() + indices[i], &bt, sizeof bt, cudaMemcpyHostToDevice));
         if (s->block_kind[indices[i]] != kinds[i]) {
             kind_changed[indices[i]] = 1;
             s->block_kind[indices[i]] = kinds[i];
@@ -1110,22 +993,17 @@ aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, con
             if (!kind_changed[id]) continue;
             CubeDelta op;
             op.idx = (uint32_t)idx;
-            op.cell = s->ds.wide_cells ? (id | ((uint32_t)s->block_kind[id] << 16)) : (id | ((uint32_t)s->block_kind[id] << 14));
+            op.cell = cell_word(id, s->block_kind[id], s->ds.wide_cells);
             op.light = 0;
             op.has_light = 0;
             ops.push_back(op);
         }
         if (!ops.empty()) {
-            CubeDelta *d_ops = nullptr;
-            CU(cudaMalloc(&d_ops, ops.size() * sizeof(CubeDelta)));
-            cudaError_t e = cudaMemcpy(d_ops, ops.data(), ops.size() * sizeof(CubeDelta), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) {
-                scatter_cubes_kernel<<<(unsigned)((ops.size() + 127) / 128), 128, 0, ctx->stream>>>(d_ops, (uint32_t)ops.size(),
-                                                                                              s->ds.wide_cells, s->d_cells, s->d_light);
-                e = cudaStreamSynchronize(ctx->stream);
-            }
-            cudaFree(d_ops);
-            if (e != cudaSuccess) return cuda_fail(e, "re-encoding cells");
+            DeviceBuffer d_ops;
+            TRY(d_ops.upload(ops));
+            scatter_cubes_kernel<<<(unsigned)((ops.size() + 127) / 128), 128, 0, ctx->stream.get()>>>(
+                d_ops.get<const CubeDelta>(), (uint32_t)ops.size(), s->ds.wide_cells, s->d_cells.get(), s->d_light.get<uint32_t>());
+            CU(cudaStreamSynchronize(ctx->stream.get()));
         }
     }
     return aicb_light_blocks_update(s, indices, descs, n);
@@ -1137,14 +1015,14 @@ aicb_status aicb_scene_upload_light(aicb_scene *s, const uint8_t (*light)[4], si
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     if (!s->d_light && s->volume) {
-        CU(cudaMalloc(&s->d_light, s->volume * 4));
+        TRY(s->d_light.ensure(s->volume * 4));
         s->device_bytes += s->volume * 4;
-        s->ds.light = s->d_light;
+        s->ds.light = s->d_light.get<uint32_t>();
     }
     if (s->volume) {   // ordered behind queued cube deltas; renders on other streams wait for ev_delta (launch_trace)
-        CU(cudaMemcpyAsync(s->d_light, light, s->volume * 4, cudaMemcpyHostToDevice, s->ctx->stream));
-        CU(cudaEventRecord(s->ctx->ev_delta, s->ctx->stream));
-        CU(cudaStreamSynchronize(s->ctx->stream));
+        CU(cudaMemcpyAsync(s->d_light.get(), light, s->volume * 4, cudaMemcpyHostToDevice, s->ctx->stream.get()));
+        CU(cudaEventRecord(s->ctx->ev_delta.get(), s->ctx->stream.get()));
+        CU(cudaStreamSynchronize(s->ctx->stream.get()));
     }
     return AICB_OK;
 }
@@ -1173,10 +1051,9 @@ aicb_status aicb_render_srgb8(aicb_scene *s, const aicb_camera *cam, const aicb_
     aicb_ctx *ctx = s->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
     CU(cudaSetDevice(ctx->device));
-    st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 4 + 16);
-    if (st != AICB_OK) return st;
+    TRY(ctx->d_out.ensure(out_len * 4 + 16));
     FramePart part{s, shard};
-    part.out.srgb8 = (uchar4 *)ctx->d_out;
+    part.out.srgb8 = ctx->d_out.get<uchar4>();
     // A pageable destination (a Rust Vec<[u8; 4]>, a numpy array) cannot take an asynchronous DMA: the frame goes to a
     // pinned staging buffer of the library's and is copied out by the host.  Pinned / registered memory is written directly.
     bool staged = false;
@@ -1185,21 +1062,15 @@ aicb_status aicb_render_srgb8(aicb_scene *s, const aicb_camera *cam, const aicb_
         const cudaError_t pe = cudaPointerGetAttributes(&attr, out);
         if (pe != cudaSuccess) cudaGetLastError();
         staged = pe != cudaSuccess || attr.type == cudaMemoryTypeUnregistered;
-        if (staged && ctx->h_stage_bytes < out_len * 4) {
-            if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-            ctx->h_stage = nullptr;
-            ctx->h_stage_bytes = 0;
-            CU(cudaMallocHost(&ctx->h_stage, out_len * 4));
-            ctx->h_stage_bytes = out_len * 4;
-        }
+        if (staged) TRY(ctx->h_stage.ensure(out_len * 4));
     }
     // the copy is queued behind the frame: one host synchronisation per call
-    part.copy_to = staged ? ctx->h_stage : (void *)out;
-    part.copy_from = ctx->d_out;
+    part.copy_to = staged ? ctx->h_stage.get() : (void *)out;
+    part.copy_from = ctx->d_out.get();
     part.copy_bytes = out_len * 4;
     st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
     if (st != AICB_OK) return st;
-    if (staged && out_len) std::memcpy(out, ctx->h_stage, out_len * 4);
+    if (staged && out_len) std::memcpy(out, ctx->h_stage.get(), out_len * 4);
     if (info) *info = part.info;
     return AICB_OK;
 }
@@ -1212,12 +1083,11 @@ aicb_status aicb_render_rgba16f(aicb_scene *s, const aicb_camera *cam, const aic
     aicb_ctx *ctx = s->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
     CU(cudaSetDevice(ctx->device));
-    st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 8 + 16);
-    if (st != AICB_OK) return st;
+    TRY(ctx->d_out.ensure(out_len * 8 + 16));
     FramePart part{s, shard};
-    part.out.rgba16f = (uint2 *)ctx->d_out;
+    part.out.rgba16f = ctx->d_out.get<uint2>();
     part.copy_to = out;
-    part.copy_from = ctx->d_out;
+    part.copy_from = ctx->d_out.get();
     part.copy_bytes = out_len * 8;
     st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
     if (st != AICB_OK) return st;
@@ -1232,9 +1102,8 @@ static aicb_status render_aux(aicb_scene *s, const aicb_camera *cam, const aicb_
     // layout of the aux staging buffer: colorbuf | depth | hit | steps
     size_t off_cb = 0, off_depth = off_cb + n * 16, off_hit = off_depth + n * 8, off_steps = off_hit + n * sizeof(aicb_hit);
     size_t total = off_steps + n * 4 + 16;
-    aicb_status st = ensure(&ctx->d_aux, &ctx->d_aux_bytes, total);
-    if (st != AICB_OK) return st;
-    char *base = (char *)ctx->d_aux;
+    TRY(ctx->d_aux.ensure(total));
+    char *base = ctx->d_aux.get<char>();
     FramePart part{s, shard};
     Outputs &o = part.out;
     o.colorbuf = (float4 *)(base + off_cb);
@@ -1244,16 +1113,15 @@ static aicb_status render_aux(aicb_scene *s, const aicb_camera *cam, const aicb_
     o.rays = d_rays;
     o.n_rays = n_rays;
     o.aux = true;
-    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
-    if (st != AICB_OK) return st;
+    TRY(aicb_trace_pass(&part, 1, cam, opt, info != nullptr));
     if (info) *info = part.info;
     if (n) {
-        if (out_cb) CU(cudaMemcpyAsync(out_cb, o.colorbuf, n * 16, cudaMemcpyDeviceToHost, ctx->stream));
-        if (depth) CU(cudaMemcpyAsync(depth, o.depth, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        if (hit) CU(cudaMemcpyAsync(hit, o.hit, n * sizeof(aicb_hit), cudaMemcpyDeviceToHost, ctx->stream));
-        if (steps) CU(cudaMemcpyAsync(steps, o.steps, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        if (out_cb) CU(cudaMemcpyAsync(out_cb, o.colorbuf, n * 16, cudaMemcpyDeviceToHost, ctx->stream.get()));
+        if (depth) CU(cudaMemcpyAsync(depth, o.depth, n * 8, cudaMemcpyDeviceToHost, ctx->stream.get()));
+        if (hit) CU(cudaMemcpyAsync(hit, o.hit, n * sizeof(aicb_hit), cudaMemcpyDeviceToHost, ctx->stream.get()));
+        if (steps) CU(cudaMemcpyAsync(steps, o.steps, n * 4, cudaMemcpyDeviceToHost, ctx->stream.get()));
     }
-    CU(cudaStreamSynchronize(ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream.get()));
     return AICB_OK;
 }
 
@@ -1276,7 +1144,7 @@ aicb_status aicb_render_srgb8_device(aicb_scene *s, const aicb_camera *cam, cons
     CU(cudaSetDevice(s->ctx->device));
     Outputs o;
     o.srgb8 = (uchar4 *)d_out;
-    return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream);
+    return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream.get());
 }
 
 aicb_status aicb_render_srgb8_device_frame(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
@@ -1292,7 +1160,7 @@ aicb_status aicb_render_srgb8_device_frame(aicb_scene *s, const aicb_camera *cam
     Outputs o;
     o.full_frame = true;
     o.srgb8 = (uchar4 *)d_frame;
-    return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream);
+    return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream.get());
 }
 
 // ---- full-frame buffers shared between ranks (CUDA IPC) ------------------------------------------
@@ -1356,7 +1224,7 @@ aicb_status aicb_frame_create(aicb_ctx *ctx, size_t n_pixels, void **d_frame, ui
 static aicb_status frame_ctl(aicb_ctx *ctx, void *d_frame, size_t n_pixels, void *stream, cudaStream_t *st, FrameControl **c) {
     if (!ctx || !d_frame) return fail(AICB_ERR_INVALID, "NULL argument");
     CU(cudaSetDevice(ctx->device));
-    *st = stream ? (cudaStream_t)stream : ctx->stream;
+    *st = stream ? (cudaStream_t)stream : ctx->stream.get();
     *c = (FrameControl *)((char *)d_frame + frame_control_offset(n_pixels));
     return AICB_OK;
 }
@@ -1428,7 +1296,7 @@ aicb_status aicb_frame_close(aicb_ctx *ctx, void *d_frame, int opened) {
 aicb_status aicb_frame_read(aicb_ctx *ctx, const void *d_frame, uint8_t (*out)[4], size_t n_pixels, void *stream) {
     if (!ctx || !d_frame || !out) return fail(AICB_ERR_INVALID, "NULL argument");
     CU(cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream.get();
     CU(cudaMemcpyAsync(out, d_frame, n_pixels * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     return AICB_OK;
@@ -1443,14 +1311,13 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
     aicb_ctx *ctx = s->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
     CU(cudaSetDevice(ctx->device));
-    st = ensure(&ctx->d_aux, &ctx->d_aux_bytes, out_len * 4 + 16);
-    if (st != AICB_OK) return st;
+    TRY(ctx->d_aux.ensure(out_len * 4 + 16));
     FramePart part{s};
-    part.out.text = (int32_t *)ctx->d_aux;
+    part.out.text = ctx->d_aux.get<int32_t>();
     st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
     if (st != AICB_OK) return st;
     if (info) *info = part.info;
-    if (out_len) CU(cudaMemcpy(out, ctx->d_aux, out_len * 4, cudaMemcpyDeviceToHost));
+    if (out_len) CU(cudaMemcpy(out, ctx->d_aux.get(), out_len * 4, cudaMemcpyDeviceToHost));
     return AICB_OK;
 }
 
@@ -1505,16 +1372,16 @@ aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera 
             const FramePart &p = parts[i];
             aicb_ctx *ctx = p.scene->ctx;
             CU(cudaSetDevice(ctx->device));
-            aicb_status r = launch_trace(p.scene, cam, opt, p.shard, p.out, ctx->stream);
+            aicb_status r = launch_trace(p.scene, cam, opt, p.shard, p.out, ctx->stream.get());
             if (r != AICB_OK) return r;
             if (p.copy_bytes)
-                CU(cudaMemcpyAsync(p.copy_to, p.copy_from, p.copy_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+                CU(cudaMemcpyAsync(p.copy_to, p.copy_from, p.copy_bytes, cudaMemcpyDeviceToHost, ctx->stream.get()));
         }
         again.clear();
         for (size_t i : todo) {
             aicb_scene *sc = parts[i].scene;
             CU(cudaSetDevice(sc->ctx->device));
-            CU(cudaStreamSynchronize(sc->ctx->stream));
+            CU(cudaStreamSynchronize(sc->ctx->stream.get()));
             aicb_render_info one{};
             aicb_status r = finish(sc, want_info ? &one : nullptr);
             if (r == AICB_ERR_RETRY) { again.push_back(i); continue; }
@@ -1574,15 +1441,12 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         for (size_t i = 0; i < n_parts; i++) {
             aicb_ctx *ctx = parts[i].world->ctx;
             CU(cudaSetDevice(ctx->device));
-            st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n_tasks(parts[i]) * sizeof(float4) + 16);
-            if (st != AICB_OK) return st;
+            TRY(ctx->d_task_aux.ensure(n_tasks(parts[i]) * sizeof(float4) + 16));
             if (parts[i].target.texture) {   // the UI pass's DepthBuf, only when there is a UI layer
-                st = ensure(&ctx->d_task_depth, &ctx->d_task_depth_bytes, n_tasks(parts[i]) * sizeof(double) + 16);
-                if (st != AICB_OK) return st;
+                TRY(ctx->d_task_depth.ensure(n_tasks(parts[i]) * sizeof(double) + 16));
             }
             if (parts[i].target.terminal) {   // the UI pass's CharacterBuf, only when there is a UI layer
-                st = ensure(&ctx->d_task_text, &ctx->d_task_text_bytes, n_tasks(parts[i]) * sizeof(int2) + 16);
-                if (st != AICB_OK) return st;
+                TRY(ctx->d_task_text.ensure(n_tasks(parts[i]) * sizeof(int2) + 16));
             }
         }
         aicb_options ui_opt = *ui->options;
@@ -1595,9 +1459,9 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
             o.pixel_list = p.target.pixel_list;
             o.n_list = p.target.n_list;
             o.tex_layer = TEX_UI;
-            if (p.target.texture) o.out_task_depth = (double *)ctx->d_task_depth;
-            if (p.target.terminal) o.out_task_text = (int2 *)ctx->d_task_text;
-            o.out_accum = (float4 *)ctx->d_task_aux;
+            if (p.target.texture) o.out_task_depth = ctx->d_task_depth.get<double>();
+            if (p.target.terminal) o.out_task_text = ctx->d_task_text.get<int2>();
+            o.out_accum = ctx->d_task_aux.get<float4>();
             o.backdrop = have_backdrop ? backdrop : nullptr;
             o.force_antialias = aa;
             return o;
@@ -1607,9 +1471,9 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         w_opt.include_sky = 1;    // world.trace_ray(.., true)
         st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
             Outputs o = p.target;
-            o.in_accum = (const float4 *)ctx->d_task_aux;   // a re-issued world pass starts from the same accumulator
-            if (p.target.texture) o.in_depth = (const double *)ctx->d_task_depth;
-            if (p.target.terminal) o.in_text = (const int2 *)ctx->d_task_text;
+            o.in_accum = ctx->d_task_aux.get<const float4>();   // a re-issued world pass starts from the same accumulator
+            if (p.target.texture) o.in_depth = ctx->d_task_depth.get<const double>();
+            if (p.target.terminal) o.in_text = ctx->d_task_text.get<const int2>();
             o.tex_layer = TEX_WORLD;
             o.no_world = no_world_rgba ? no_world : nullptr;
             return o;
@@ -1623,17 +1487,16 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
                 aicb_ctx *ctx = parts[i].world->ctx;
                 const size_t n = n_tasks(parts[i]);
                 CU(cudaSetDevice(ctx->device));
-                st = ensure(&ctx->d_task_aux, &ctx->d_task_aux_bytes, n * sizeof(float4) + 16);
-                if (st != AICB_OK) return st;
+                TRY(ctx->d_task_aux.ensure(n * sizeof(float4) + 16));
                 std::vector<float4> init(n, make_float4(backdrop[0] * 1.0f, backdrop[1] * 1.0f, backdrop[2] * 1.0f, 1.0f * backdrop[3]));
-                CU(cudaMemcpy(ctx->d_task_aux, init.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
+                CU(cudaMemcpy(ctx->d_task_aux.get(), init.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
             }
         }
         st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
             Outputs o = p.target;
             o.tex_layer = TEX_WORLD;
             if (have_backdrop) {
-                o.in_accum = (const float4 *)ctx->d_task_aux;
+                o.in_accum = ctx->d_task_aux.get<const float4>();
                 o.text_start = AICB_TEXT_BLANK;   // the backdrop's hit names no block
             }
             o.no_world = no_world_rgba ? no_world : nullptr;
@@ -1706,14 +1569,13 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
     aicb_ctx *ctx = lead->scene->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
     CU(cudaSetDevice(ctx->device));
-    st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * 4 + 16);
-    if (st != AICB_OK) return st;
+    TRY(ctx->d_out.ensure(out_len * 4 + 16));
     LayerPart part = single_part(world, ui);
-    part.target.srgb8 = (uchar4 *)ctx->d_out;
+    part.target.srgb8 = ctx->d_out.get<uchar4>();
     aicb_render_info total;
     st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
     if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpy(out, ctx->d_out, out_len * 4, cudaMemcpyDeviceToHost));
+    if (out_len) CU(cudaMemcpy(out, ctx->d_out.get(), out_len * 4, cudaMemcpyDeviceToHost));
     if (info) *info = total;
     return AICB_OK;
 }
@@ -1730,15 +1592,14 @@ aicb_status aicb_render_layers_terminal(const aicb_layer *world, const aicb_laye
     aicb_ctx *ctx = lead->scene->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
     CU(cudaSetDevice(ctx->device));
-    st = ensure(&ctx->d_out, &ctx->d_out_bytes, out_len * sizeof(aicb_terminal_pixel) + 16);
-    if (st != AICB_OK) return st;
+    TRY(ctx->d_out.ensure(out_len * sizeof(aicb_terminal_pixel) + 16));
     LayerPart part = single_part(world, ui);
     part.target.terminal = true;
-    part.target.term = (aicb_terminal_pixel *)ctx->d_out;
+    part.target.term = ctx->d_out.get<aicb_terminal_pixel>();
     aicb_render_info total;
     st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
     if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpy(out, ctx->d_out, out_len * sizeof(aicb_terminal_pixel), cudaMemcpyDeviceToHost));
+    if (out_len) CU(cudaMemcpy(out, ctx->d_out.get(), out_len * sizeof(aicb_terminal_pixel), cudaMemcpyDeviceToHost));
     if (info) *info = total;
     return AICB_OK;
 }
@@ -1762,9 +1623,8 @@ aicb_status aicb_render_layers_texture(const aicb_layer *world, const aicb_layer
     // d_out: colour texels (8 B), depth texels (4 B), then the pixel list (4 B), each 256-byte aligned
     const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
     const size_t off_list = off_depth + ((n_pixels * 4 + 255) & ~(size_t)255);
-    st = ensure(&ctx->d_out, &ctx->d_out_bytes, off_list + (pixels ? n_pixels * 4 : 0) + 16);
-    if (st != AICB_OK) return st;
-    char *base = (char *)ctx->d_out;
+    TRY(ctx->d_out.ensure(off_list + (pixels ? n_pixels * 4 : 0) + 16));
+    char *base = ctx->d_out.get<char>();
     LayerPart part = single_part(world, ui);
     Outputs &target = part.target;
     aicb_texture_target(world, ui, depth_transform, &target);
@@ -1861,35 +1721,25 @@ aicb_status aicb_render_orthographic(aicb_scene *s, uint32_t resolution, uint8_t
     const size_t n = where.size();
     std::vector<uchar4> px(n);
     if (n) {
-        double *d_rays = nullptr;
-        CU(cudaMalloc(&d_rays, n * 48 + 16));
-        cudaError_t e = cudaMemcpy(d_rays, rays.data(), n * 48, cudaMemcpyHostToDevice);
-        if (e == cudaSuccess) {
-            st = ensure(&ctx->d_out, &ctx->d_out_bytes, n * 4 + 16);
-            if (st == AICB_OK) {
-                aicb_options opt;   // GraphicsOptions::UNALTERED_COLORS (graphics_options.rs:168)
-                std::memset(&opt, 0, sizeof opt);
-                opt.fog = AICB_FOG_NONE;
-                opt.lighting_display = AICB_LIGHT_NONE;
-                opt.transparency = AICB_TRANSPARENCY_VOLUMETRIC;
-                opt.tone_mapping = AICB_TONE_CLAMP;
-                opt.maximum_intensity = INFINITY;
-                opt.view_distance = 200.0;
-                opt.include_sky = 1;
-                FramePart part{s};
-                part.out.srgb8 = (uchar4 *)ctx->d_out;
-                part.out.rays = d_rays;
-                part.out.n_rays = n;
-                st = aicb_trace_pass(&part, 1, nullptr, &opt, info != nullptr);
-                if (st == AICB_OK) {
-                    if (info) *info = part.info;
-                    e = cudaMemcpy(px.data(), ctx->d_out, n * 4, cudaMemcpyDeviceToHost);
-                }
-            }
-        }
-        cudaFree(d_rays);
-        if (e != cudaSuccess) return cuda_fail(e, "orthographic render");
-        if (st != AICB_OK) return st;
+        DeviceBuffer d_rays;
+        TRY(d_rays.upload(rays.data(), n * 48, 16));
+        TRY(ctx->d_out.ensure(n * 4 + 16));
+        aicb_options opt;   // GraphicsOptions::UNALTERED_COLORS (graphics_options.rs:168)
+        std::memset(&opt, 0, sizeof opt);
+        opt.fog = AICB_FOG_NONE;
+        opt.lighting_display = AICB_LIGHT_NONE;
+        opt.transparency = AICB_TRANSPARENCY_VOLUMETRIC;
+        opt.tone_mapping = AICB_TONE_CLAMP;
+        opt.maximum_intensity = INFINITY;
+        opt.view_distance = 200.0;
+        opt.include_sky = 1;
+        FramePart part{s};
+        part.out.srgb8 = ctx->d_out.get<uchar4>();
+        part.out.rays = d_rays.get<double>();
+        part.out.n_rays = n;
+        TRY(aicb_trace_pass(&part, 1, nullptr, &opt, info != nullptr));
+        if (info) *info = part.info;
+        CU(cudaMemcpy(px.data(), ctx->d_out.get(), n * 4, cudaMemcpyDeviceToHost));
     }
     std::memset(out, 0, out_len * 4);   // Rgba::TRANSPARENT between the views
     for (size_t i = 0; i < n; i++) std::memcpy(out[where[i]], &px[i], 4);
@@ -1912,16 +1762,9 @@ aicb_status aicb_trace_rays(aicb_scene *s, const double (*origin_dir)[6], size_t
     aicb_ctx *ctx = s->ctx;
     std::lock_guard<std::mutex> lock(ctx->mu);
     CU(cudaSetDevice(ctx->device));
-    double *d_rays = nullptr;
-    CU(cudaMalloc(&d_rays, n * 48 + 16));
-    cudaError_t e = cudaMemcpy(d_rays, origin_dir, n * 48, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-        cudaFree(d_rays);
-        return cuda_fail(e, "cudaMemcpy rays");
-    }
-    st = render_aux(s, nullptr, opt, nullptr, d_rays, n, out_cb, depth, hit, steps, n, info);
-    cudaFree(d_rays);
-    return st;
+    DeviceBuffer d_rays;
+    TRY(d_rays.upload(origin_dir, n * 48, 16));
+    return render_aux(s, nullptr, opt, nullptr, d_rays.get<double>(), n, out_cb, depth, hit, steps, n, info);
 }
 
 }

@@ -16,16 +16,22 @@
 
 #include "internal.h"
 
+// Destroyed with device 0 current (aicb_group_destroy): its own buffers first, then each device's event and context.
 struct aicb_group {
     std::vector<aicb_ctx *> ctx;
-    std::vector<cudaEvent_t> done;   // per device: its strips of the current frame are in device 0's frame
-    void *d_frame = nullptr;         // on device 0
-    size_t frame_pixels = 0;
-    void *d_tex = nullptr;           // on device 0: the texels of aicb_group_render_layers_texture, or the pixels of
-                                     // aicb_group_render_layers_terminal
-    size_t d_tex_bytes = 0;
-    void *h_stage = nullptr;         // pinned staging for pageable destinations
-    size_t h_stage_bytes = 0;
+    std::vector<Event> done;   // per device: its strips of the current frame are in device 0's frame
+    DeviceBuffer d_frame;      // on device 0
+    DeviceBuffer d_tex;        // on device 0: the texels of aicb_group_render_layers_texture, or the pixels of
+                               // aicb_group_render_layers_terminal
+    ~aicb_group() {
+        d_frame.reset();
+        d_tex.reset();
+        for (size_t i = 0; i < ctx.size(); i++) {
+            cudaSetDevice(ctx[i]->device);
+            done[i].reset();
+            aicb_ctx_destroy(ctx[i]);
+        }
+    }
 };
 
 struct aicb_group_scene {
@@ -34,17 +40,6 @@ struct aicb_group_scene {
 };
 
 static const uint32_t GROUP_STRIP_ROWS = 16;
-
-static aicb_status ensure_frame(aicb_group *g, size_t pixels) {   // device 0's sRGB8 frame; the root device is current
-    if (g->frame_pixels < pixels) {
-        if (g->d_frame) cudaFree(g->d_frame);
-        g->d_frame = nullptr;
-        g->frame_pixels = 0;
-        CU(cudaMalloc(&g->d_frame, pixels * 4 + 16));
-        g->frame_pixels = pixels;
-    }
-    return AICB_OK;
-}
 
 // ---- layered frames and texture targets -------------------------------------------------------------------------------
 // The layers of a group call as device i sees them: its replicas, the same cameras and options.
@@ -84,10 +79,10 @@ static std::vector<LayerPart> strip_parts(aicb_group *g, const aicb_group_layer 
 static aicb_status join(aicb_group *g, size_t n_parts) {
     for (size_t i = 1; i < n_parts; i++) {
         CU(cudaSetDevice(g->ctx[i]->device));
-        CU(cudaEventRecord(g->done[i], g->ctx[i]->stream));
+        CU(cudaEventRecord(g->done[i].get(), g->ctx[i]->stream.get()));
     }
     CU(cudaSetDevice(g->ctx[0]->device));
-    for (size_t i = 1; i < n_parts; i++) CU(cudaStreamWaitEvent(g->ctx[0]->stream, g->done[i], 0));
+    for (size_t i = 1; i < n_parts; i++) CU(cudaStreamWaitEvent(g->ctx[0]->stream.get(), g->done[i].get(), 0));
     return AICB_OK;
 }
 
@@ -103,19 +98,7 @@ extern "C" {
 
 void aicb_group_destroy(aicb_group *g) {
     if (!g) return;
-    if (!g->ctx.empty()) {
-        cudaSetDevice(g->ctx[0]->device);
-        if (g->d_frame) cudaFree(g->d_frame);
-        if (g->d_tex) cudaFree(g->d_tex);
-        if (g->h_stage) cudaFreeHost(g->h_stage);
-    }
-    for (size_t i = 0; i < g->ctx.size(); i++) {
-        if (g->done[i]) {
-            cudaSetDevice(g->ctx[i]->device);
-            cudaEventDestroy(g->done[i]);
-        }
-        aicb_ctx_destroy(g->ctx[i]);
-    }
+    if (!g->ctx.empty()) cudaSetDevice(g->ctx[0]->device);
     delete g;
 }
 
@@ -131,11 +114,11 @@ aicb_status aicb_group_create(const int *device_ids, int n_devices, aicb_group *
             return st;
         }
         g->ctx.push_back(c);
-        g->done.push_back(nullptr);
-        cudaError_t e = cudaEventCreateWithFlags(&g->done[i], cudaEventDisableTiming);
-        if (e != cudaSuccess) {
+        g->done.emplace_back();
+        st = create_event(g->done[i], cudaEventDisableTiming);
+        if (st != AICB_OK) {
             aicb_group_destroy(g);
-            return aicb_cuda_fail(e, "cudaEventCreate");
+            return st;
         }
     }
     // every device stores into device 0's frame
@@ -209,11 +192,10 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
     GroupLock lock(g);
     aicb_ctx *root = g->ctx[0];
     CU(cudaSetDevice(root->device));
-    st = ensure_frame(g, pixels);
-    if (st != AICB_OK) return st;
+    TRY(g->d_frame.ensure(pixels * 4 + 16));
     Outputs target;
     target.full_frame = true;
-    target.srgb8 = (uchar4 *)g->d_frame;
+    target.srgb8 = g->d_frame.get<uchar4>();
     // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
     const aicb_group_layer world = {gs, cam, opt};
     const std::vector<LayerPart> strips = strip_parts(g, &world, nullptr, target);
@@ -223,8 +205,8 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
     if (st != AICB_OK) return st;
     st = join(g, parts.size());
     if (st != AICB_OK) return st;
-    if (pixels) CU(cudaMemcpyAsync(out, g->d_frame, pixels * 4, cudaMemcpyDeviceToHost, root->stream));
-    CU(cudaStreamSynchronize(root->stream));
+    if (pixels) CU(cudaMemcpyAsync(out, g->d_frame.get(), pixels * 4, cudaMemcpyDeviceToHost, root->stream.get()));
+    CU(cudaStreamSynchronize(root->stream.get()));
     if (info) {
         std::memset(info, 0, sizeof *info);
         for (const FramePart &p : parts) aicb_merge_info(info, &p.info, false);
@@ -270,19 +252,18 @@ aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world, const 
     GroupLock lock(g);
     aicb_ctx *root = g->ctx[0];
     CU(cudaSetDevice(root->device));
-    st = ensure_frame(g, out_len);
-    if (st != AICB_OK) return st;
+    TRY(g->d_frame.ensure(out_len * 4 + 16));
     Outputs target;
     target.full_frame = true;
-    target.srgb8 = (uchar4 *)g->d_frame;
+    target.srgb8 = g->d_frame.get<uchar4>();
     std::vector<LayerPart> parts = strip_parts(g, world, ui, target);
     aicb_render_info total;
     st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
     if (st != AICB_OK) return st;
     st = join(g, parts.size());
     if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpyAsync(out, g->d_frame, out_len * 4, cudaMemcpyDeviceToHost, root->stream));
-    CU(cudaStreamSynchronize(root->stream));
+    if (out_len) CU(cudaMemcpyAsync(out, g->d_frame.get(), out_len * 4, cudaMemcpyDeviceToHost, root->stream.get()));
+    CU(cudaStreamSynchronize(root->stream.get()));
     if (info) *info = total;
     return AICB_OK;
 }
@@ -302,20 +283,19 @@ aicb_status aicb_group_render_layers_terminal(const aicb_group_layer *world, con
     aicb_ctx *root = g->ctx[0];
     CU(cudaSetDevice(root->device));
     const size_t bytes = out_len * sizeof(aicb_terminal_pixel);
-    st = aicb_ensure_device(&g->d_tex, &g->d_tex_bytes, bytes + 16);
-    if (st != AICB_OK) return st;
+    TRY(g->d_tex.ensure(bytes + 16));
     Outputs target;
     target.full_frame = true;
     target.terminal = true;
-    target.term = (aicb_terminal_pixel *)g->d_tex;
+    target.term = g->d_tex.get<aicb_terminal_pixel>();
     std::vector<LayerPart> parts = strip_parts(g, world, ui, target);
     aicb_render_info total;
     st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
     if (st != AICB_OK) return st;
     st = join(g, parts.size());
     if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpyAsync(out, g->d_tex, bytes, cudaMemcpyDeviceToHost, root->stream));
-    CU(cudaStreamSynchronize(root->stream));
+    if (out_len) CU(cudaMemcpyAsync(out, g->d_tex.get(), bytes, cudaMemcpyDeviceToHost, root->stream.get()));
+    CU(cudaStreamSynchronize(root->stream.get()));
     if (info) *info = total;
     return AICB_OK;
 }
@@ -338,9 +318,8 @@ aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world, cons
     CU(cudaSetDevice(root->device));
     // device 0: colour texels (8 B), then depth texels (4 B), 256-byte aligned
     const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
-    st = aicb_ensure_device(&g->d_tex, &g->d_tex_bytes, off_depth + n_pixels * 4 + 16);
-    if (st != AICB_OK) return st;
-    char *base = (char *)g->d_tex;
+    TRY(g->d_tex.ensure(off_depth + n_pixels * 4 + 16));
+    char *base = g->d_tex.get<char>();
     Outputs target;
     aicb_texture_target(w, u, depth_transform, &target);
     target.rgba16f = (uint2 *)base;
@@ -358,14 +337,13 @@ aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world, cons
             const size_t count = std::min(32 * (warps / used + (i < warps % used ? 1 : 0)), n_pixels - begin);
             aicb_ctx *c = g->ctx[i];
             CU(cudaSetDevice(c->device));
-            st = aicb_ensure_device(&c->d_out, &c->d_out_bytes, count * 4 + 16);
-            if (st != AICB_OK) return st;
-            CU(cudaMemcpy(c->d_out, pixels + begin, count * 4, cudaMemcpyHostToDevice));
+            TRY(c->d_out.ensure(count * 4 + 16));
+            CU(cudaMemcpy(c->d_out.get(), pixels + begin, count * 4, cudaMemcpyHostToDevice));
             LayerPart p;
             p.world = replica(world, i).scene;
             p.ui = replica(ui, i).scene;
             p.target = target;
-            p.target.pixel_list = (const uint32_t *)c->d_out;
+            p.target.pixel_list = c->d_out.get<const uint32_t>();
             p.target.n_list = (uint32_t)count;
             p.target.rgba16f = target.rgba16f + begin;
             p.target.tex_depth = target.tex_depth + begin;
@@ -378,9 +356,9 @@ aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world, cons
     if (st != AICB_OK) return st;
     st = join(g, parts.size());
     if (st != AICB_OK) return st;
-    CU(cudaMemcpyAsync(out_rgba16f, base, n_pixels * 8, cudaMemcpyDeviceToHost, root->stream));
-    CU(cudaMemcpyAsync(out_depth, base + off_depth, n_pixels * 4, cudaMemcpyDeviceToHost, root->stream));
-    CU(cudaStreamSynchronize(root->stream));
+    CU(cudaMemcpyAsync(out_rgba16f, base, n_pixels * 8, cudaMemcpyDeviceToHost, root->stream.get()));
+    CU(cudaMemcpyAsync(out_depth, base + off_depth, n_pixels * 4, cudaMemcpyDeviceToHost, root->stream.get()));
+    CU(cudaStreamSynchronize(root->stream.get()));
     if (info) *info = total;
     return AICB_OK;
 }

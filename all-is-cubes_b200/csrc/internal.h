@@ -1,7 +1,9 @@
 // internal.h — objects behind the opaque handles of include/aicb200.h (shared by aicb200.cu and light.cu).
 #pragma once
+#include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -15,71 +17,168 @@ aicb_status aicb_cuda_fail(cudaError_t e, const char *what);
         cudaError_t e__ = (call);                                  \
         if (e__ != cudaSuccess) return aicb_cuda_fail(e__, #call); \
     } while (0)
+#define TRY(call)                                  \
+    do {                                           \
+        aicb_status st__ = (call);                 \
+        if (st__ != AICB_OK) return st__;          \
+    } while (0)
 
-struct LightNodePre;    // light_kernel.cuh
-struct LightChain;      // light_kernel.cuh
-struct LightBlockDev;   // light_kernel.cuh
+// ---- owners of the library's CUDA resources -----------------------------------------------------------------------
+// Each frees what it holds when it is destroyed or replaced, on the current device: whoever destroys an object that
+// holds them sets its device first.
+struct DeviceMemory {
+    static cudaError_t alloc(void **p, size_t bytes) { return cudaMalloc(p, bytes); }
+    static void release(void *p) { cudaFree(p); }
+};
+struct PinnedMemory {
+    static cudaError_t alloc(void **p, size_t bytes) { return cudaMallocHost(p, bytes); }
+    static void release(void *p) { cudaFreeHost(p); }
+};
 
+template <typename Memory>
+class Buffer {
+public:
+    Buffer() = default;
+    Buffer(Buffer &&o) noexcept : p_(std::exchange(o.p_, nullptr)), bytes_(std::exchange(o.bytes_, 0)) {}
+    Buffer &operator=(Buffer &&o) noexcept {
+        if (this != &o) {
+            reset();
+            p_ = std::exchange(o.p_, nullptr);
+            bytes_ = std::exchange(o.bytes_, 0);
+        }
+        return *this;
+    }
+    ~Buffer() { reset(); }
+
+    // At least `bytes`, contents not kept: a smaller buffer is freed first, and stays empty if the allocation fails.
+    aicb_status ensure(size_t bytes) {
+        if (bytes_ >= bytes) return AICB_OK;
+        reset();
+        void *p = nullptr;
+        CU(Memory::alloc(&p, bytes));
+        p_ = p;
+        bytes_ = bytes;
+        return AICB_OK;
+    }
+    // Exactly `bytes + pad` bytes, the first `bytes` copied from the host; the buffer changes only if both steps succeed.
+    aicb_status upload(const void *src, size_t bytes, size_t pad = 0) {
+        Buffer b;
+        TRY(b.ensure(bytes + pad));
+        CU(cudaMemcpy(b.p_, src, bytes, cudaMemcpyHostToDevice));
+        *this = std::move(b);
+        return AICB_OK;
+    }
+    template <typename T>
+    aicb_status upload(const std::vector<T> &v) { return upload(v.data(), v.size() * sizeof(T)); }
+    void reset() {
+        if (p_) Memory::release(p_);
+        p_ = nullptr;
+        bytes_ = 0;
+    }
+
+    template <typename T = void>
+    T *get() const { return static_cast<T *>(p_); }
+    size_t bytes() const { return bytes_; }
+    explicit operator bool() const { return p_ != nullptr; }
+
+private:
+    void *p_ = nullptr;
+    size_t bytes_ = 0;
+};
+using DeviceBuffer = Buffer<DeviceMemory>;
+using PinnedBuffer = Buffer<PinnedMemory>;
+
+struct EventDestroy {
+    void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+struct StreamDestroy {
+    void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+};
+using Event = std::unique_ptr<CUevent_st, EventDestroy>;
+using Stream = std::unique_ptr<CUstream_st, StreamDestroy>;
+
+inline aicb_status create_event(Event &e, unsigned int flags) {
+    cudaEvent_t raw = nullptr;
+    CU(cudaEventCreateWithFlags(&raw, flags));
+    e.reset(raw);
+    return AICB_OK;
+}
+
+// A cube's cell word: its block id with the block's kind in the top bits (16-bit cells up to 16384 block ids).
+inline uint32_t cell_word(uint32_t id, uint8_t kind, bool wide) { return id | ((uint32_t)kind << (wide ? 16 : 14)); }
+
+// One chunk's streams between the kernels of a frame (trace_kernel.cuh): the listed rays' records (array A, then
+// array B), a TaskOut per task, the HitRecord stream (march -> resolve, or march -> shade -> encode), a ShadedHit per
+// hit (shade -> encode: not used by frames that run resolve_kernel) and the task ids of the rays that enter the space,
+// per chord-length bin.
+struct ChunkStreams {
+    DeviceBuffer rays, task_out, hits, shaded, bin_list;
+
+    aicb_status size(uint64_t chunk_cap, uint32_t hit_capacity, bool shade) {
+        TRY(rays.ensure(chunk_cap * (sizeof(aicb::RayRecordA) + sizeof(aicb::RayRecordB)) + 16));
+        TRY(task_out.ensure(chunk_cap * sizeof(aicb::TaskOut) + 16));
+        TRY(hits.ensure((size_t)hit_capacity * sizeof(aicb::HitRecord) + 64));
+        if (shade) TRY(shaded.ensure((size_t)hit_capacity * sizeof(aicb::ShadedHit) + 64));
+        return bin_list.ensure((size_t)aicb::N_BINS * chunk_cap * 4 + 64);
+    }
+    void bind(aicb::TraceParams &P, uint64_t chunk_cap, bool shade) const {
+        P.rays_a = rays.get<aicb::RayRecordA>();   // 64-byte aligned: cudaMalloc aligns to 256 bytes
+        P.rays_b = (aicb::RayRecordB *)(rays.get<char>() + chunk_cap * sizeof(aicb::RayRecordA));
+        P.task_out = task_out.get<aicb::TaskOut>();
+        P.hits = hits.get<aicb::HitRecord>();
+        P.shaded = shade ? shaded.get<aicb::ShadedHit>() : nullptr;
+        P.bin_list = bin_list.get<uint32_t>();
+    }
+    void release_hits() {
+        hits.reset();
+        shaded.reset();
+    }
+};
+
+// Members are destroyed in reverse order of declaration: the stream and events go after the buffers.
 struct aicb_ctx {
     int device = 0;
     int num_sms = 0;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    cudaEvent_t ev_k[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // AICB_PROFILE_KERNELS
+    Stream stream;
+    Event ev0, ev1;
+    Event ev_k[5];               // AICB_PROFILE_KERNELS
     bool profile_kernels = false;
     bool stage_timing = true;    // record the per-kernel events of a frame (aicb_render_info::stage_ms)
-    void *h_delta = nullptr, *d_delta = nullptr;  // staging of aicb_scene_update_cubes batches (pinned / device)
-    size_t h_delta_bytes = 0;
-    cudaEvent_t ev_delta = nullptr;
-    void *d_debug = nullptr;
+    PinnedBuffer h_delta;        // staging of aicb_scene_update_cubes batches (pinned / device)
+    DeviceBuffer d_delta;
+    Event ev_delta;
+    DeviceBuffer d_debug;
     uint32_t debug_warps = 0;
-    unsigned int *d_tile_counter = nullptr;
-    unsigned long long *d_counters = nullptr;
-    float *d_lut = nullptr;
+    // the frame counters (8 x u64), then the per-chunk counters (4 + N_BINS x u32) of the primary and the secondary
+    // (Bounce) pass: one memset per frame
+    DeviceBuffer d_counters;
+    unsigned int *d_tile_counter = nullptr;   // the per-chunk counters in d_counters
+    DeviceBuffer d_lut;
     // staging output buffers (grown on demand)
-    void *d_out = nullptr;
-    size_t d_out_bytes = 0;
-    void *d_aux = nullptr;
-    size_t d_aux_bytes = 0;
-    // per-task streams between gen -> trace -> resolve, or -> shade -> encode (trace_kernel.cuh)
-    void *d_rays = nullptr;
-    size_t d_rays_bytes = 0;
-    void *d_task_cb = nullptr;   // TaskOut per task
-    size_t d_task_cb_bytes = 0;
-    void *d_hits = nullptr;      // HitRecord stream (march -> resolve, or march -> shade -> encode)
-    size_t d_hits_bytes = 0;
-    void *d_contrib = nullptr;   // ShadedHit per hit (shade -> encode): not used by frames that run resolve_kernel
-    size_t d_contrib_bytes = 0;
-    void *d_bin_list = nullptr;  // task ids of the rays that enter the space, per chord-length bin
-    size_t d_bin_list_bytes = 0;
-    // LightingOption::Bounce: the same streams for the secondary rays of a chunk, and the per-task bounce state
-    void *d_rays2 = nullptr, *d_task_cb2 = nullptr, *d_hits2 = nullptr, *d_contrib2 = nullptr, *d_bin_list2 = nullptr;
-    size_t d_rays2_bytes = 0, d_task_cb2_bytes = 0, d_hits2_bytes = 0, d_contrib2_bytes = 0, d_bin_list2_bytes = 0;
-    void *d_bounce = nullptr;    // per task: secondary ray (48 B), RNG state (32 B), Rgb sum + steps (16 B), request (4 B)
-    size_t d_bounce_bytes = 0;
+    DeviceBuffer d_out, d_aux;
+    // the per-chunk streams of a frame, and with LightingOption::Bounce the same for the secondary rays of a chunk
+    // and the per-task bounce state: secondary ray (48 B), RNG state (32 B), Rgb sum + steps (16 B), request (4 B)
+    ChunkStreams primary, secondary;
+    DeviceBuffer d_bounce;
     uint32_t hits_per_task = 8;  // capacity of the hit stream per ray; raised x4 when a frame overflows it,
     uint32_t shallow_frames = 0; //   lowered again after 16 frames in a row that needed a small fraction of it
     bool deep_frames = false;    // the last frame met >= 3/4 visible surfaces per ray: no resolve_kernel (launch_trace)
-    void *h_stage = nullptr;     // pinned staging of frames whose destination is pageable host memory
-    size_t h_stage_bytes = 0;
+    PinnedBuffer h_stage;        // pinned staging of frames whose destination is pageable host memory
     // the frame whose per-frame scratch (streams, counters, events) is in use
     bool frame_in_flight = false;
     cudaStream_t last_stream = nullptr;
     struct aicb_scene *last_scene = nullptr;
-    void *d_task_aux = nullptr;
-    size_t d_task_aux_bytes = 0;
-    void *d_task_depth = nullptr;   // per task: the UI pass's DepthBuf for the world pass (aicb_render_layers_texture)
-    size_t d_task_depth_bytes = 0;
-    void *d_task_text = nullptr;    // per task: the UI pass's CharacterBuf for the world pass (aicb_render_layers_terminal)
-    size_t d_task_text_bytes = 0;
+    DeviceBuffer d_task_aux;
+    DeviceBuffer d_task_depth;   // per task: the UI pass's DepthBuf for the world pass (aicb_render_layers_texture)
+    DeviceBuffer d_task_text;    // per task: the UI pass's CharacterBuf for the world pass (aicb_render_layers_terminal)
     // light propagation: the static ray chart (space/light/chart), built and uploaded on first use
-    LightNodePre *d_chart_pre = nullptr;   // the chart in depth-first preorder (the lockstep walk)
+    DeviceBuffer d_chart_pre;    // LightNodePre: the chart in depth-first preorder (the lockstep walk)
     uint32_t chart_nodes = 0;
-    LightChain *d_chains = nullptr;         // the chart as chains, the per-node cube offsets, the Euler tour of the chain tree
-    uchar4 *d_node_rel = nullptr;
-    uint16_t *d_euler = nullptr;
+    DeviceBuffer d_chains;       // the chart as chains, the per-node cube offsets, the Euler tour of the chain tree
+    DeviceBuffer d_node_rel;
+    DeviceBuffer d_euler;
     uint32_t n_chains = 0, n_euler = 0;
-    float4 *d_term_scratch = nullptr;       // term slots of the chain walk, one set per resident warp
+    DeviceBuffer d_term_scratch; // term slots of the chain walk, one set per resident warp
     uint32_t chain_walk_blocks = 0;
     std::mutex mu;
 };
@@ -90,13 +189,13 @@ struct aicb_scene {
     std::vector<uint8_t> block_kind;   // host copy, for update_cubes
     size_t volume = 0;
     uint64_t device_bytes = 0;
-    void *d_cells = nullptr;
-    uint32_t *d_light = nullptr;
-    aicb::BlockRec *d_blocks = nullptr;
-    uint16_t *d_bricks = nullptr;
-    float4 *d_palette = nullptr;
-    float2 *d_pal_tab = nullptr;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
-    float4 *d_blk_tab = nullptr;   // per block id: that pair and the palette entry of single-voxel blocks
+    DeviceBuffer d_cells;
+    DeviceBuffer d_light;
+    DeviceBuffer d_blocks;
+    DeviceBuffer d_bricks;
+    DeviceBuffer d_palette;
+    DeviceBuffer d_pal_tab;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
+    DeviceBuffer d_blk_tab;   // per block id: that pair and the palette entry of single-voxel blocks
     size_t n_bricks = 0, n_palette = 0;   // elements in d_bricks / d_palette (aicb_scene_update_blocks appends)
     // state of the last asynchronous render
     bool pending = false;
@@ -107,15 +206,15 @@ struct aicb_scene {
     // ---- light propagation state (light.cu) ----
     std::vector<uint16_t> h_ids;            // host mirror of Space::contents (edits are applied in order on the host)
     std::vector<uint32_t> h_block_light;    // per block: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission
-    LightBlockDev *d_light_blocks = nullptr;
-    uint8_t *d_pending = nullptr;           // per cube: queued priority (0 = not queued) — LightUpdateQueue
-    uint32_t *d_list = nullptr;             // work list of one round (cube indices)
-    uint32_t *d_new_light = nullptr;        // computed texels of one round
-    uint8_t *d_diff = nullptr;              // difference_priority of one round
-    uint32_t *d_scalars = nullptr;          // [0] list length, [1] max priority, [2] max diff, [3] updates
-    float4 *d_sky_term = nullptr;           // per chart node: the sky light its bundle collects (end_of_ray), for this scene's sky
-    uint32_t *d_changed = nullptr;          // list positions whose cube changed by more than one unit this round
-    uint32_t *d_tile_max = nullptr;         // per LIGHT_TILE cubes: upper bound of the queued priorities
+    DeviceBuffer d_light_blocks;            // LightBlockDev per block
+    DeviceBuffer d_pending;                 // per cube: queued priority (0 = not queued) — LightUpdateQueue
+    DeviceBuffer d_list;                    // work list of one round (cube indices)
+    DeviceBuffer d_new_light;               // computed texels of one round
+    DeviceBuffer d_diff;                    // difference_priority of one round
+    DeviceBuffer d_scalars;                 // [0] list length, [1] max priority, [2] max diff, [3] updates
+    DeviceBuffer d_sky_term;                // per chart node: the sky light its bundle collects (end_of_ray), for this scene's sky
+    DeviceBuffer d_changed;                 // list positions whose cube changed by more than one unit this round
+    DeviceBuffer d_tile_max;                // per LIGHT_TILE cubes: upper bound of the queued priorities
     uint32_t light_max_distance = 0;
     uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
 };
@@ -197,7 +296,6 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
 aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
                             bool want_info);
 void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part);
-aicb_status aicb_ensure_device(void **p, size_t *cur, size_t want);
 // aicb_scene_update_blocks' validation alone: AICB_OK if that call would accept the update (changes nothing)
 aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
 }

@@ -205,47 +205,33 @@ const ChainTables &chain_tables_host() {
     return tables;
 }
 
-void free_chart(aicb_ctx *c) {
-    void **ptrs[] = {(void **)&c->d_chart_pre, (void **)&c->d_chains, (void **)&c->d_node_rel, (void **)&c->d_euler,
-                     (void **)&c->d_term_scratch};
-    for (void **p : ptrs) {
-        if (*p) cudaFree(*p);
-        *p = nullptr;
-    }
-}
-
-aicb_status upload_chart(aicb_ctx *ctx) {
-    {
-        const ChainTables &t = chain_tables_host();
-        if (t.chains.size() > (size_t)LIGHT_MAX_CHAINS || t.chains.size() >= 0x8000u)
-            return aicb_fail(AICB_ERR_INVALID, "light chart has more chains than the walk's shared arrays hold");
-        size_t branches = 0;
-        for (const LightChain &c : t.chains) branches += c.n_children ? 1 : 0;
-        if (branches > (size_t)LIGHT_MAX_BRANCHES) return aicb_fail(AICB_ERR_INVALID, "light chart has more branching chains than expected");
-        CU(cudaMalloc(&ctx->d_chains, t.chains.size() * sizeof(LightChain)));
-        CU(cudaMemcpy(ctx->d_chains, t.chains.data(), t.chains.size() * sizeof(LightChain), cudaMemcpyHostToDevice));
-        CU(cudaMalloc(&ctx->d_node_rel, t.node_rel.size() * sizeof(uchar4)));
-        CU(cudaMemcpy(ctx->d_node_rel, t.node_rel.data(), t.node_rel.size() * sizeof(uchar4), cudaMemcpyHostToDevice));
-        CU(cudaMalloc(&ctx->d_euler, t.euler.size() * sizeof(uint16_t)));
-        CU(cudaMemcpy(ctx->d_euler, t.euler.data(), t.euler.size() * sizeof(uint16_t), cudaMemcpyHostToDevice));
-        ctx->n_chains = (uint32_t)t.chains.size();
-        ctx->n_euler = (uint32_t)t.euler.size();
-        // one set of term slots per resident warp of the chain walk
-        ctx->chain_walk_blocks = (uint32_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM;
-        CU(cudaMalloc(&ctx->d_term_scratch, (size_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM * 4 * LIGHT_WARP_SCRATCH_F4 * sizeof(float4)));
-    }
+// The chart's tables on the context's device; the context takes them once every one is uploaded.
+aicb_status ensure_chart(aicb_ctx *ctx) {
+    if (ctx->d_chart_pre) return AICB_OK;
+    const ChainTables &t = chain_tables_host();
+    if (t.chains.size() > (size_t)LIGHT_MAX_CHAINS || t.chains.size() >= 0x8000u)
+        return aicb_fail(AICB_ERR_INVALID, "light chart has more chains than the walk's shared arrays hold");
+    size_t branches = 0;
+    for (const LightChain &c : t.chains) branches += c.n_children ? 1 : 0;
+    if (branches > (size_t)LIGHT_MAX_BRANCHES) return aicb_fail(AICB_ERR_INVALID, "light chart has more branching chains than expected");
+    DeviceBuffer chains, node_rel, euler, term_scratch, chart_pre;
+    TRY(chains.upload(t.chains));
+    TRY(node_rel.upload(t.node_rel));
+    TRY(euler.upload(t.euler));
+    // one set of term slots per resident warp of the chain walk
+    TRY(term_scratch.ensure((size_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM * 4 * LIGHT_WARP_SCRATCH_F4 * sizeof(float4)));
     const std::vector<LightNodePre> &pre = chart_preorder_host();
-    CU(cudaMalloc(&ctx->d_chart_pre, pre.size() * sizeof(LightNodePre)));
-    CU(cudaMemcpy(ctx->d_chart_pre, pre.data(), pre.size() * sizeof(LightNodePre), cudaMemcpyHostToDevice));
+    TRY(chart_pre.upload(pre));
+    ctx->d_chains = std::move(chains);
+    ctx->d_node_rel = std::move(node_rel);
+    ctx->d_euler = std::move(euler);
+    ctx->d_term_scratch = std::move(term_scratch);
+    ctx->d_chart_pre = std::move(chart_pre);
+    ctx->n_chains = (uint32_t)t.chains.size();
+    ctx->n_euler = (uint32_t)t.euler.size();
+    ctx->chain_walk_blocks = (uint32_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM;
     ctx->chart_nodes = (uint32_t)pre.size();
     return AICB_OK;
-}
-
-aicb_status ensure_chart(aicb_ctx *ctx) {
-    if (ctx->d_chart_pre) return AICB_OK;   // (d_chart_pre is the last allocation of upload_chart)
-    const aicb_status st = upload_chart(ctx);
-    if (st != AICB_OK) free_chart(ctx);   // a later call starts over instead of leaking the tables that did fit
-    return st;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -535,39 +521,37 @@ LightParams make_params(aicb_scene *s) {
     LightParams P;
     std::memset(&P, 0, sizeof P);
     P.scene = s->ds;
-    P.blocks = s->d_light_blocks;
-    P.chart_pre = s->ctx->d_chart_pre;
-    P.sky_term = s->d_sky_term;
-    P.chains = s->ctx->d_chains;
-    P.node_rel = s->ctx->d_node_rel;
-    P.euler = s->ctx->d_euler;
+    P.blocks = s->d_light_blocks.get<LightBlockDev>();
+    P.chart_pre = s->ctx->d_chart_pre.get<LightNodePre>();
+    P.sky_term = s->d_sky_term.get<float4>();
+    P.chains = s->ctx->d_chains.get<LightChain>();
+    P.node_rel = s->ctx->d_node_rel.get<uchar4>();
+    P.euler = s->ctx->d_euler.get<uint16_t>();
     P.n_chains = s->ctx->n_chains;
     P.n_euler = s->ctx->n_euler;
-    P.term_scratch = s->ctx->d_term_scratch;
-    P.overflow = s->d_changed;   // (k_walk_chains<false>'s overflow list and k_walk_chains<true>'s work list are never live together)
+    P.term_scratch = s->ctx->d_term_scratch.get<float4>();
+    P.overflow = s->d_changed.get<uint32_t>();   // (k_walk_chains<false>'s overflow list and k_walk_chains<true>'s work list are never live together)
     P.chart_nodes = s->ctx->chart_nodes;
-    P.tile_max = s->d_tile_max;
-    P.changed = s->d_changed;
-    P.pending = s->d_pending;
-    P.list = s->d_list;
-    P.new_light = s->d_new_light;
-    P.diff = s->d_diff;
-    P.scalars = s->d_scalars;
+    P.tile_max = s->d_tile_max.get<uint32_t>();
+    P.changed = s->d_changed.get<uint32_t>();
+    P.pending = s->d_pending.get<uint8_t>();
+    P.list = s->d_list.get<uint32_t>();
+    P.new_light = s->d_new_light.get<uint32_t>();
+    P.diff = s->d_diff.get<uint8_t>();
+    P.scalars = s->d_scalars.get<uint32_t>();
     P.volume = (uint32_t)s->volume;
     P.max_distance = s->light_max_distance;
     return P;
 }
 
+// The scene's light state, built in locals: the scene takes them once every step has succeeded.
 aicb_status ensure_light_state(aicb_scene *s) {
     if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
-    aicb_status st = ensure_chart(s->ctx);
-    if (st != AICB_OK) return st;
+    TRY(ensure_chart(s->ctx));
+    DeviceBuffer light, sky_term, pending, list, new_light, diff, scalars, tile_max, changed;
     if (!s->d_light) {  // a scene created without a light volume starts all NO_RAYS (initialize_light, updater.rs:628-656)
-        std::vector<uint32_t> init(s->volume, TX_NO_RAYS);
-        CU(cudaMalloc(&s->d_light, s->volume * 4 + 16));
-        CU(cudaMemcpy(s->d_light, init.data(), s->volume * 4, cudaMemcpyHostToDevice));
-        s->ds.light = s->d_light;
-        s->device_bytes += s->volume * 4;
+        const std::vector<uint32_t> init(s->volume, TX_NO_RAYS);
+        TRY(light.upload(init.data(), s->volume * 4, 16));
     }
     if (!s->d_sky_term) {
         // end_of_ray (updater.rs:889-924) without the lane's alpha and bundle weight: per chart node, the sky light
@@ -594,19 +578,36 @@ aicb_status ensure_light_state(aicb_scene *s) {
             for (int i = 0; i < 3; i++) c[i] = psm((t[0][i] + t[3][i]) + (t[1][i] + t[4][i]) + (t[2][i] + t[5][i]), kr);
             sky[k] = make_float4(c[0], c[1], c[2], 0.0f);
         }
-        CU(cudaMalloc(&s->d_sky_term, sky.size() * sizeof(float4)));
-        CU(cudaMemcpy(s->d_sky_term, sky.data(), sky.size() * sizeof(float4), cudaMemcpyHostToDevice));
-        s->device_bytes += sky.size() * sizeof(float4);
+        TRY(sky_term.upload(sky));
     }
-    if (!s->d_pending) {
-        CU(cudaMalloc(&s->d_pending, s->volume + 16));
-        CU(cudaMemset(s->d_pending, 0, s->volume + 16));
-        CU(cudaMalloc(&s->d_list, s->volume * 4 + 16));
-        CU(cudaMalloc(&s->d_new_light, s->volume * 4 + 16));
-        CU(cudaMalloc(&s->d_diff, s->volume + 16));
-        CU(cudaMalloc(&s->d_scalars, 16 * 4));
-        CU(cudaMalloc(&s->d_tile_max, ((s->volume + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
-        CU(cudaMalloc(&s->d_changed, s->volume * 4 + 16));
+    const bool work = !s->d_pending;
+    if (work) {
+        TRY(pending.ensure(s->volume + 16));
+        CU(cudaMemset(pending.get(), 0, s->volume + 16));
+        TRY(list.ensure(s->volume * 4 + 16));
+        TRY(new_light.ensure(s->volume * 4 + 16));
+        TRY(diff.ensure(s->volume + 16));
+        TRY(scalars.ensure(16 * 4));
+        TRY(tile_max.ensure(((s->volume + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
+        TRY(changed.ensure(s->volume * 4 + 16));
+    }
+    if (light) {
+        s->d_light = std::move(light);
+        s->ds.light = s->d_light.get<uint32_t>();
+        s->device_bytes += s->volume * 4;
+    }
+    if (sky_term) {
+        s->d_sky_term = std::move(sky_term);
+        s->device_bytes += chart_preorder_host().size() * sizeof(float4);
+    }
+    if (work) {
+        s->d_pending = std::move(pending);
+        s->d_list = std::move(list);
+        s->d_new_light = std::move(new_light);
+        s->d_diff = std::move(diff);
+        s->d_scalars = std::move(scalars);
+        s->d_tile_max = std::move(tile_max);
+        s->d_changed = std::move(changed);
         s->device_bytes += s->volume * 4;
         s->device_bytes += s->volume * 10;
     }
@@ -616,7 +617,7 @@ aicb_status ensure_light_state(aicb_scene *s) {
 // evaluate_light (space.rs:1496-1527): rounds until the highest queued priority is <= from_difference(epsilon)
 aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits) {
     aicb_ctx *ctx = s->ctx;
-    cudaStream_t st = ctx->stream;
+    cudaStream_t st = ctx->stream.get();
     LightParams P = make_params(s);
     P.epsilon_priority = (uint32_t)epsilon / 2 + 1;
     const int blocks = ctx->num_sms * 8;
@@ -624,14 +625,14 @@ aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, ui
     const uint32_t n_tiles = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
     uint64_t total = 0, visits = 0, rounds = 0;
     uint32_t maxd = 0;
-    CU(cudaEventRecord(ctx->ev0, st));
-    CU(cudaMemsetAsync(s->d_scalars, 0, 16 * 4, st));
+    CU(cudaEventRecord(ctx->ev0.get(), st));
+    CU(cudaMemsetAsync(P.scalars, 0, 16 * 4, st));
     k_tile_rebuild<<<blocks, 256, 0, st>>>(P, n_tiles);   // (fast_evaluate / edits write the priority bytes directly)
     const int ROUNDS_PER_SYNC = 8;
     for (int batch = 0; batch < 100000; batch++) {
         for (int round = 0; round < ROUNDS_PER_SYNC; round++) {
-            CU(cudaMemsetAsync(s->d_scalars, 0, 2 * 4, st));   // this round's count and priority
-            CU(cudaMemsetAsync(s->d_scalars + 6, 0, 4 * 4, st));   // ... its count of changed cubes, the two work counters, the overflow count
+            CU(cudaMemsetAsync(P.scalars, 0, 2 * 4, st));   // this round's count and priority
+            CU(cudaMemsetAsync(P.scalars + 6, 0, 4 * 4, st));   // ... its count of changed cubes, the two work counters, the overflow count
             k_find_max<<<16, 256, 0, st>>>(P, n_tiles);
             k_gather<<<blocks, 256, 0, st>>>(P, n_tiles);
             k_walk_chains<false><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
@@ -641,7 +642,7 @@ aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, ui
             k_walk_chains<true><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
         }
         uint32_t h[8];
-        CU(cudaMemcpyAsync(h, s->d_scalars, 8 * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(h, P.scalars, 8 * 4, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         CU(cudaGetLastError());
         total = h[3];
@@ -650,10 +651,10 @@ aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, ui
         rounds += ROUNDS_PER_SYNC;
         if (h[1] <= P.epsilon_priority) break;   // the batch's last round found nothing above epsilon
     }
-    CU(cudaEventRecord(ctx->ev1, st));
-    CU(cudaEventSynchronize(ctx->ev1));
+    CU(cudaEventRecord(ctx->ev1.get(), st));
+    CU(cudaEventSynchronize(ctx->ev1.get()));
     float ms = 0.0f;
-    CU(cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1));
+    CU(cudaEventElapsedTime(&ms, ctx->ev0.get(), ctx->ev1.get()));
     s->light_stats[0] = total;
     s->light_stats[1] = visits;
     s->light_stats[2] = rounds;
@@ -662,6 +663,21 @@ aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, ui
     if (max_diff) *max_diff = (uint8_t)maxd;
     if (node_visits) *node_visits = visits;
     return AICB_OK;
+}
+
+// The light-side record of a block definition: its face colours, emission and flags (which h_block_light mirrors).
+LightBlockDev light_block(const aicb_block_desc &b) {
+    LightBlockDev o;
+    std::memset(&o, 0, sizeof o);
+    std::memcpy(o.face_color[0], b.light_color, 16);
+    for (int f = 0; f < 6; f++) std::memcpy(o.face_color[f + 1], b.light_face_colors[f], 16);
+    std::memcpy(o.emission, b.light_emission, 12);
+    uint32_t fl = b.light_opaque_faces & 0x3f;
+    if (fl == 0x3f) fl |= LB_ALL_OPAQUE;
+    if (b.light_visible) fl |= LB_VISIBLE;
+    if (!(b.light_emission[0] == 0.0f && b.light_emission[1] == 0.0f && b.light_emission[2] == 0.0f)) fl |= LB_EMISSIVE;
+    o.flags = fl;
+    return o;
 }
 
 }  // namespace
@@ -675,21 +691,11 @@ aicb_status aicb_light_scene_upload(aicb_scene *s, const aicb_scene_desc *d) {
     std::vector<LightBlockDev> lb(d->n_blocks);
     s->h_block_light.resize(d->n_blocks);
     for (size_t i = 0; i < d->n_blocks; i++) {
-        const aicb_block_desc &b = d->blocks[i];
-        LightBlockDev &o = lb[i];
-        std::memcpy(o.face_color[0], b.light_color, 16);
-        for (int f = 0; f < 6; f++) std::memcpy(o.face_color[f + 1], b.light_face_colors[f], 16);
-        std::memcpy(o.emission, b.light_emission, 12);
-        uint32_t fl = b.light_opaque_faces & 0x3f;
-        if (fl == 0x3f) fl |= LB_ALL_OPAQUE;
-        if (b.light_visible) fl |= LB_VISIBLE;
-        if (!(b.light_emission[0] == 0.0f && b.light_emission[1] == 0.0f && b.light_emission[2] == 0.0f)) fl |= LB_EMISSIVE;
-        o.flags = fl;
-        s->h_block_light[i] = fl;
+        lb[i] = light_block(d->blocks[i]);
+        s->h_block_light[i] = lb[i].flags;
     }
     if (!lb.empty()) {
-        CU(cudaMalloc(&s->d_light_blocks, lb.size() * sizeof(LightBlockDev)));
-        CU(cudaMemcpy(s->d_light_blocks, lb.data(), lb.size() * sizeof(LightBlockDev), cudaMemcpyHostToDevice));
+        TRY(s->d_light_blocks.upload(lb));
         s->device_bytes += lb.size() * sizeof(LightBlockDev);
     }
     return AICB_OK;
@@ -698,36 +704,13 @@ aicb_status aicb_light_scene_upload(aicb_scene *s, const aicb_scene_desc *d) {
 // the light-side records of replaced block definitions (aicb_scene_update_blocks)
 aicb_status aicb_light_blocks_update(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
     for (size_t i = 0; i < n; i++) {
-        const aicb_block_desc &b = descs[i];
-        LightBlockDev o;
-        std::memset(&o, 0, sizeof o);
-        std::memcpy(o.face_color[0], b.light_color, 16);
-        for (int f = 0; f < 6; f++) std::memcpy(o.face_color[f + 1], b.light_face_colors[f], 16);
-        std::memcpy(o.emission, b.light_emission, 12);
-        uint32_t fl = b.light_opaque_faces & 0x3f;
-        if (fl == 0x3f) fl |= LB_ALL_OPAQUE;
-        if (b.light_visible) fl |= LB_VISIBLE;
-        if (!(b.light_emission[0] == 0.0f && b.light_emission[1] == 0.0f && b.light_emission[2] == 0.0f)) fl |= LB_EMISSIVE;
-        o.flags = fl;
-        if (indices[i] < s->h_block_light.size()) s->h_block_light[indices[i]] = fl;
-        if (s->d_light_blocks) CU(cudaMemcpy(s->d_light_blocks + indices[i], &o, sizeof o, cudaMemcpyHostToDevice));
+        const LightBlockDev o = light_block(descs[i]);
+        if (indices[i] < s->h_block_light.size()) s->h_block_light[indices[i]] = o.flags;
+        if (s->d_light_blocks)
+            CU(cudaMemcpy(s->d_light_blocks.get<LightBlockDev>() + indices[i], &o, sizeof o, cudaMemcpyHostToDevice));
     }
     return AICB_OK;
 }
-
-void aicb_light_scene_free(aicb_scene *s) {
-    if (s->d_light_blocks) cudaFree(s->d_light_blocks);
-    if (s->d_pending) cudaFree(s->d_pending);
-    if (s->d_list) cudaFree(s->d_list);
-    if (s->d_new_light) cudaFree(s->d_new_light);
-    if (s->d_diff) cudaFree(s->d_diff);
-    if (s->d_scalars) cudaFree(s->d_scalars);
-    if (s->d_tile_max) cudaFree(s->d_tile_max);
-    if (s->d_changed) cudaFree(s->d_changed);
-    if (s->d_sky_term) cudaFree(s->d_sky_term);
-}
-
-void aicb_light_ctx_free(aicb_ctx *c) { free_chart(c); }
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
@@ -768,9 +751,9 @@ aicb_status aicb_light_fast_evaluate(aicb_scene *s) {
     if (st != AICB_OK) return st;
     LightParams P = make_params(s);
     const uint32_t cols = (uint32_t)s->ds.size[0] * (uint32_t)s->ds.size[2];
-    if (cols) k_fast_evaluate<<<(cols + 127) / 128, 128, 0, s->ctx->stream>>>(P);
+    if (cols) k_fast_evaluate<<<(cols + 127) / 128, 128, 0, s->ctx->stream.get()>>>(P);
     CU(cudaGetLastError());
-    CU(cudaStreamSynchronize(s->ctx->stream));
+    CU(cudaStreamSynchronize(s->ctx->stream.get()));
     return AICB_OK;
 }
 
@@ -783,24 +766,20 @@ aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t 
     if (st != AICB_OK) return st;
     if (!n) return AICB_OK;
     LightParams P = make_params(s);
-    int32_t *d_cubes = nullptr;
-    CU(cudaMalloc(&d_cubes, n * 12));
-    CU(cudaMemcpy(d_cubes, cubes, n * 12, cudaMemcpyHostToDevice));
-    cudaMemsetAsync(s->d_scalars, 0, 16 * 4, s->ctx->stream);
-    k_walk_chains<false><<<s->ctx->chain_walk_blocks, 128, 0, s->ctx->stream>>>(P, (uint32_t)n, d_cubes);
-    k_compute_overflow<<<s->ctx->num_sms * 8, 128, 0, s->ctx->stream>>>(P, d_cubes);
+    cudaStream_t stream = s->ctx->stream.get();
+    DeviceBuffer d_cubes;
+    TRY(d_cubes.upload(cubes, n * 12));
+    cudaMemsetAsync(P.scalars, 0, 16 * 4, stream);
+    k_walk_chains<false><<<s->ctx->chain_walk_blocks, 128, 0, stream>>>(P, (uint32_t)n, d_cubes.get<int32_t>());
+    k_compute_overflow<<<s->ctx->num_sms * 8, 128, 0, stream>>>(P, d_cubes.get<int32_t>());
     uint32_t h[16];
-    cudaError_t e = cudaMemcpyAsync(out, s->d_new_light, n * 4, cudaMemcpyDeviceToHost, s->ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h, s->d_scalars, sizeof h, cudaMemcpyDeviceToHost, s->ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s->ctx->stream);
-    if (e == cudaSuccess) {
-        s->light_stats[0] = n;
-        s->light_stats[1] = (uint64_t)h[4] | ((uint64_t)h[5] << 32);
-        s->light_stats[2] = h[9];   // cubes that took the lockstep walk (a chain with more terms than its slots)
-        s->light_stats[3] = 0;
-    }
-    cudaFree(d_cubes);
-    if (e != cudaSuccess) return aicb_cuda_fail(e, "light compute");
+    CU(cudaMemcpyAsync(out, P.new_light, n * 4, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(h, P.scalars, sizeof h, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    s->light_stats[0] = n;
+    s->light_stats[1] = (uint64_t)h[4] | ((uint64_t)h[5] << 32);
+    s->light_stats[2] = h[9];   // cubes that took the lockstep walk (a chain with more terms than its slots)
+    s->light_stats[3] = 0;
     return AICB_OK;
 }
 
@@ -854,8 +833,7 @@ aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[
         if (s->h_ids[idx] == new_ids[i]) continue;  // Mutation::set of the same block changes nothing
         s->h_ids[idx] = new_ids[i];
         EditOp &o = op_of(idx);
-        o.cell = ds.wide_cells ? (new_ids[i] | ((uint32_t)s->block_kind[new_ids[i]] << 16))
-                               : (new_ids[i] | ((uint32_t)s->block_kind[new_ids[i]] << 14));
+        o.cell = cell_word(new_ids[i], s->block_kind[new_ids[i]], ds.wide_cells);
         const uint32_t fl = s->h_block_light[new_ids[i]];
         if ((fl & LB_ALL_OPAQUE) && !(fl & LB_EMISSIVE)) {  // opaque_for_light_computation
             o.set_opaque = 1;
@@ -876,14 +854,13 @@ aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[
         std::vector<EditOp> flat;
         flat.reserve(ops.size());
         for (auto &kv : ops) flat.push_back(kv.second);
-        EditOp *d_ops = nullptr;
-        CU(cudaMalloc(&d_ops, flat.size() * sizeof(EditOp)));
-        CU(cudaMemcpyAsync(d_ops, flat.data(), flat.size() * sizeof(EditOp), cudaMemcpyHostToDevice, s->ctx->stream));
+        cudaStream_t stream = s->ctx->stream.get();
+        DeviceBuffer d_ops;
+        TRY(d_ops.ensure(flat.size() * sizeof(EditOp)));
+        CU(cudaMemcpyAsync(d_ops.get(), flat.data(), flat.size() * sizeof(EditOp), cudaMemcpyHostToDevice, stream));
         LightParams P = make_params(s);
-        k_edits<<<(unsigned)((flat.size() + 127) / 128), 128, 0, s->ctx->stream>>>(P, d_ops, (uint32_t)flat.size(), ds.wide_cells);
-        cudaError_t e = cudaStreamSynchronize(s->ctx->stream);
-        cudaFree(d_ops);
-        if (e != cudaSuccess) return aicb_cuda_fail(e, "light edits");
+        k_edits<<<(unsigned)((flat.size() + 127) / 128), 128, 0, stream>>>(P, d_ops.get<EditOp>(), (uint32_t)flat.size(), ds.wide_cells);
+        CU(cudaStreamSynchronize(stream));
     }
     return propagate(s, epsilon, updates_done, max_diff, nullptr);
 }
@@ -895,8 +872,8 @@ aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texel
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     // ordered behind everything queued on the context's stream (cube deltas, propagation)
-    CU(cudaMemcpyAsync(out, s->d_light, s->volume * 4, cudaMemcpyDeviceToHost, s->ctx->stream));
-    CU(cudaStreamSynchronize(s->ctx->stream));
+    CU(cudaMemcpyAsync(out, s->d_light.get(), s->volume * 4, cudaMemcpyDeviceToHost, s->ctx->stream.get()));
+    CU(cudaStreamSynchronize(s->ctx->stream.get()));
     return AICB_OK;
 }
 

@@ -1,7 +1,8 @@
 """resolve_kernel (None / Flat lighting: shading and compositing in one pass, one warp per 32 rays, hit lists in
 shared-memory windows of 128 slots): frames in which a warp's hit lists span many windows, against the oracle, the
 choice between it and shade_kernel + encode_kernel, and the stage times a frame reports.  Also: every blocking entry
-point re-issues a frame that overflowed the hit stream and returns what the warmed context returns."""
+point re-issues a frame that overflowed the hit stream and returns what the warmed context returns, and a context
+gives an enlarged hit stream back after a run of shallow frames."""
 import ctypes as C
 
 import numpy as np
@@ -98,6 +99,44 @@ def test_blocking_call_reissues_an_overflowed_frame(call):
         if group:
             group.close()
         ctx.close()
+
+
+@pytest.mark.parametrize("lighting", [LIGHT_FLAT, LIGHT_BOUNCE])
+def test_enlarged_hit_stream_is_given_back(lighting):
+    """A faint-slab frame overflows a fresh context's hit stream and is re-issued with a larger one; after 16 shallow
+    frames in a row the context gives the large hit and ShadedHit buffers back (with Bounce, those of the secondary rays'
+    streams too) and lowers the capacity again.  Every shallow frame equals the same frame on a fresh context, and the
+    faint-slab frame drawn once more, which overflows the lowered capacity and is re-issued, equals the first.  The
+    shallow scene's blocks are opaque: at most one surface per primary ray and one per secondary ray, well under a
+    sixteenth of the enlarged capacity per ray."""
+    slab, mixed = faint_slab(), scenes.config_c0(n=16)
+    opts = GraphicsOptions(lighting_display=lighting, transparency=TRANSPARENCY_VOLUMETRIC, view_distance=200.0)
+    slab_cam = scenes.standard_camera(slab, opts, 128, 96, direction=(1.0, 0.04, 0.03), distance_scale=0.5)
+    mixed_cam = scenes.standard_camera(mixed, opts, 64, 48)
+    ctx, fresh = Context(), Context()
+    renderers = []
+    try:
+        deep, shallow, ref = RtRenderer(slab_cam, ctx), RtRenderer(mixed_cam, ctx), RtRenderer(mixed_cam, fresh)
+        renderers = [deep, shallow, ref]
+        deep.update(slab)
+        shallow.update(mixed)
+        ref.update(mixed)
+        first = deep.draw()
+        assert first.info.counters[2] > max(8 * first.info.rays, 1 << 16), first.info   # it overflowed a fresh stream
+        want = ref.draw()
+        for _ in range(16):
+            img = shallow.draw()
+            assert np.array_equal(img.data, want.data)
+            assert (img.info.cubes_traced, img.info.counters) == (want.info.cubes_traced, want.info.counters)
+        again = deep.draw()
+        assert np.array_equal(again.data, first.data)
+        assert (again.info.cubes_traced, again.info.counters) == (first.info.cubes_traced, first.info.counters)
+    finally:
+        for r in renderers:
+            if r.rt:
+                r.rt.close()
+        ctx.close()
+        fresh.close()
 
 
 @pytest.mark.parametrize("antialias", [False, True])
