@@ -136,6 +136,14 @@ def load_library() -> C.CDLL:
     lib.aicb_light_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     lib.aicb_light_evaluate.argtypes = [C.c_void_p, C.c_uint8, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
                                         C.POINTER(C.c_uint64)]
+    lib.aicb_group_light_fast_evaluate.argtypes = [C.c_void_p]
+    lib.aicb_group_light_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.aicb_group_light_evaluate.argtypes = [C.c_void_p, C.c_uint8, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
+                                              C.POINTER(C.c_uint64)]
+    lib.aicb_group_light_edit_and_propagate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8,
+                                                        C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
+    lib.aicb_group_light_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
+    lib.aicb_group_light_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     if lib.aicb_abi_version() != abi.ABI_VERSION:
         raise RuntimeError("libaicb200.so ABI version mismatch")
     _lib = lib
@@ -871,7 +879,8 @@ def print_space(space: "Space", direction, block_chars: dict, rt: "SpaceRaytrace
 
 class GroupScene:
     """A Space replicated on every device of a DeviceGroup (aicb_group_scene): what a SpaceRaytracer is to one context,
-    kept current by the same updates, applied to every replica."""
+    kept current by the same updates, applied to every replica, and lit by the same light calls, whose rounds every
+    device shares."""
 
     def __init__(self, group: "DeviceGroup", space: "Space"):
         self.group = group
@@ -899,6 +908,48 @@ class GroupScene:
     def upload_light(self, light: np.ndarray):
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
         _check(load_library().aicb_group_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
+
+    # ---- light propagation on every device of the group (SpaceRaytracer's light_* methods, same results) ----
+    def light_fast_evaluate(self):
+        """LightStorage::fast_evaluate_light (updater.rs:537-582) on device 0, copied to every replica"""
+        _check(load_library().aicb_group_light_fast_evaluate(self.handle))
+
+    def light_compute(self, cubes: np.ndarray) -> np.ndarray:
+        """LightStorage::compute_light (updater.rs:368-418) for explicit cubes, split across the devices; returns
+        texels [n,4] in input order."""
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        out = np.zeros((c.shape[0], 4), dtype=np.uint8)
+        _check(load_library().aicb_group_light_compute(self.handle, c.ctypes.data, c.shape[0], out.ctypes.data))
+        return out
+
+    def light_evaluate(self, epsilon: int = 0):
+        """Mutation::evaluate_light (space.rs:1496-1527) -> (updates, max_difference, chart_node_visits)"""
+        n, md, nv = C.c_uint64(0), C.c_uint8(0), C.c_uint64(0)
+        _check(load_library().aicb_group_light_evaluate(self.handle, epsilon, C.byref(n), C.byref(md), C.byref(nv)))
+        return int(n.value), int(md.value), int(nv.value)
+
+    def light_edit_and_propagate(self, cubes: np.ndarray, block_ids: np.ndarray, epsilon: int = 0):
+        """Mutation::set x n + evaluate_light(epsilon) -> (updates, max_difference)"""
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
+        n, md = C.c_uint64(0), C.c_uint8(0)
+        _check(load_library().aicb_group_light_edit_and_propagate(self.handle, c.ctypes.data, ids.ctypes.data, c.shape[0],
+                                                                  epsilon, C.byref(n), C.byref(md)))
+        return int(n.value), int(md.value)
+
+    def light_stats(self) -> dict:
+        """Counters of the last light call, summed over the devices; device seconds are device 0's (it waits for every
+        device in every round)."""
+        out = (C.c_uint64 * 4)()
+        _check(load_library().aicb_group_light_stats(self.handle, out))
+        return {"cube_updates": int(out[0]), "chart_node_visits": int(out[1]), "rounds": int(out[2]),
+                "device_seconds": int(out[3]) * 1e-6}
+
+    def light_download(self, replica: int = 0) -> np.ndarray:
+        """The light volume of one replica (they are identical after every light call)."""
+        out = np.zeros(self.space.size + (4,), dtype=np.uint8)
+        _check(load_library().aicb_group_light_download(self.handle, replica, out.ctypes.data, out.size // 4))
+        return out
 
     def close(self):
         if self.handle:

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -179,4 +179,10 @@ EXPORTED_SYMBOLS = [
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",
     "aicb_group_render_layers_terminal",
+    "aicb_group_light_fast_evaluate",
+    "aicb_group_light_compute",
+    "aicb_group_light_evaluate",
+    "aicb_group_light_edit_and_propagate",
+    "aicb_group_light_download",
+    "aicb_group_light_stats",
 ]

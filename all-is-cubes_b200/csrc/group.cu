@@ -9,6 +9,7 @@
 // Layered frames, terminal frames and texture targets (aicb_group_render_layers_*) cut the work the same way, or a pixel list into
 // ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu).  Every call issues a pass on every
 // device before it waits for any, and re-issues it on a device whose hit stream overflowed (aicb_trace_pass).
+// Light propagation (aicb_group_light_*) hands the replicas to light.cu, which runs one context's rounds over them.
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -23,6 +24,7 @@ struct aicb_group {
     DeviceBuffer d_frame;      // on device 0
     DeviceBuffer d_tex;        // on device 0: the texels of aicb_group_render_layers_texture, or the pixels of
                                // aicb_group_render_layers_terminal
+    bool light_peers = false;  // device 0 reaches every device too, and the devices have native peer atomics
     ~aicb_group() {
         d_frame.reset();
         d_tex.reset();
@@ -93,6 +95,36 @@ struct GroupLock {
         for (aicb_ctx *c : g->ctx) locks.emplace_back(c->mu);
     }
 };
+
+// ---- light propagation ------------------------------------------------------------------------------------------------
+// Light needs more than frames: device 0 stores into every device's light volume (the push of a round), and every
+// device's walks raise priorities in device 0's queue with atomics.  Checked and enabled at the first light call.
+static aicb_status ensure_light_peers(aicb_group *g) {
+    if (g->light_peers) return AICB_OK;
+    const int root = g->ctx[0]->device;
+    for (size_t i = 1; i < g->ctx.size(); i++) {
+        const int dev = g->ctx[i]->device;
+        if (dev == root) continue;
+        int can = 0, atomics = 0;
+        CU(cudaDeviceCanAccessPeer(&can, root, dev));
+        if (!can) return aicb_fail(AICB_ERR_UNSUPPORTED, "the root device cannot access a device's memory (no P2P / NVLink path)");
+        CU(cudaDeviceGetP2PAttribute(&atomics, cudaDevP2PAttrNativeAtomicSupported, dev, root));
+        if (!atomics) return aicb_fail(AICB_ERR_UNSUPPORTED, "a device has no native atomics on the root device's memory");
+        CU(cudaSetDevice(root));
+        cudaError_t e = cudaDeviceEnablePeerAccess(dev, 0);
+        if (e == cudaErrorPeerAccessAlreadyEnabled) { cudaGetLastError(); e = cudaSuccess; }
+        if (e != cudaSuccess) return aicb_cuda_fail(e, "cudaDeviceEnablePeerAccess");
+    }
+    g->light_peers = true;
+    return AICB_OK;
+}
+
+// The group's replicas for light.cu, after the group's locks are held and its peers are ready.
+static aicb_status light_replicas(aicb_group_scene *gs, LightReplicas *r) {
+    TRY(ensure_light_peers(gs->group));
+    *r = {gs->scene.data(), gs->scene.size()};
+    return AICB_OK;
+}
 
 extern "C" {
 
@@ -361,6 +393,55 @@ aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world, cons
     CU(cudaStreamSynchronize(root->stream.get()));
     if (info) *info = total;
     return AICB_OK;
+}
+
+// ---- light propagation: the single-context calls' arguments, validation and results (light.cu) --------------------
+aicb_status aicb_group_light_fast_evaluate(aicb_group_scene *gs) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    GroupLock lock(gs->group);
+    LightReplicas r;
+    TRY(light_replicas(gs, &r));
+    return light_fast_evaluate(r);
+}
+
+aicb_status aicb_group_light_compute(aicb_group_scene *gs, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
+    if (!gs || (n && (!cubes || !out))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n > gs->scene[0]->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
+    GroupLock lock(gs->group);
+    LightReplicas r;
+    TRY(light_replicas(gs, &r));
+    return light_compute(r, cubes, n, out);
+}
+
+aicb_status aicb_group_light_evaluate(aicb_group_scene *gs, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
+                                      uint64_t *node_visits) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    GroupLock lock(gs->group);
+    LightReplicas r;
+    TRY(light_replicas(gs, &r));
+    return light_evaluate(r, epsilon, updates_done, max_diff, node_visits);
+}
+
+aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *new_ids,
+                                                size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
+                                                uint8_t *max_diff) {
+    if (!gs || (n_edits && (!cubes || !new_ids))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    GroupLock lock(gs->group);
+    LightReplicas r;
+    TRY(light_replicas(gs, &r));
+    return light_edit_and_propagate(r, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+}
+
+aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t (*out)[4], size_t n_texels) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (replica < 0 || (size_t)replica >= gs->scene.size()) return aicb_fail(AICB_ERR_INVALID, "no such replica");
+    GroupLock lock(gs->group);
+    return light_download(gs->scene[replica], out, n_texels);
+}
+
+aicb_status aicb_group_light_stats(const aicb_group_scene *gs, uint64_t out[4]) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    return aicb_light_stats(gs->scene[0], out);   // device 0's counters are the group's (light.cu)
 }
 
 }  // extern "C"

@@ -141,6 +141,7 @@ struct aicb_ctx {
     int num_sms = 0;
     Stream stream;
     Event ev0, ev1;
+    Event ev_light;              // light propagation on a device group: this context's stream reached a step of a round
     Event ev_k[5];               // AICB_PROFILE_KERNELS
     bool profile_kernels = false;
     bool stage_timing = true;    // record the per-kernel events of a frame (aicb_render_info::stage_ms)
@@ -215,6 +216,9 @@ struct aicb_scene {
     DeviceBuffer d_sky_term;                // per chart node: the sky light its bundle collects (end_of_ray), for this scene's sky
     DeviceBuffer d_changed;                 // list positions whose cube changed by more than one unit this round
     DeviceBuffer d_tile_max;                // per LIGHT_TILE cubes: upper bound of the queued priorities
+    // replica 0 of a group scene: the light volume's segments written this round, and the other replicas' volumes
+    DeviceBuffer d_dirty;
+    DeviceBuffer d_push_targets;
     uint32_t light_max_distance = 0;
     uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
 };
@@ -299,3 +303,19 @@ void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool sa
 // aicb_scene_update_blocks' validation alone: AICB_OK if that call would accept the update (changes nothing)
 aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
 }
+
+// light.cu: the light calls over the replicas of one scene, device 0's first; a single context is the one-replica case.
+// Validation is against replica 0, before anything changes.  The caller holds every replica's context lock; on a group,
+// device 0 has peer access to every other device and they to device 0, with native atomics.  After every call the
+// replicas' light volumes are identical.
+struct LightReplicas {
+    aicb_scene *const *scene;
+    size_t n;
+};
+aicb_status light_fast_evaluate(LightReplicas r);
+aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]);
+aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
+                           uint64_t *node_visits);
+aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
+                                     uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
+aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels);

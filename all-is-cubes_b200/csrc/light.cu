@@ -362,7 +362,7 @@ __global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(c
         bool overflowed = false;
         const uint32_t nv = compute_light_chains<MARK>(P, s_lut, sh, terms, x, y, z, prio, &visits, &overflowed);
         if (!MARK && lane == 0) {
-            if (overflowed) P.overflow[atomicAdd(P.scalars + 9, 1u)] = i;
+            if (overflowed) P.overflow[atomicAdd(P.overflow_count, 1u)] = i;
             else P.new_light[i] = nv;
         }
         total_visits += visits;
@@ -374,12 +374,12 @@ __global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(c
 // latency bound, so 32 resident warps serve it better than the 20 that 94 registers would allow.
 constexpr int LOCKSTEP_MIN_BLOCKS = 8;
 
-// the cubes the chain walk could not hold (scalars[9] entries of `overflow`), by the lockstep walk
+// the cubes the chain walk could not hold (*overflow_count entries of `overflow`), by the lockstep walk
 __global__ void __launch_bounds__(128, LOCKSTEP_MIN_BLOCKS) k_compute_overflow(const LightParams P, const int32_t *explicit_cubes) {
     __shared__ float s_lut[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lut[i] = P.scene.tables[i];
     __syncthreads();
-    const uint32_t n = P.scalars[9];
+    const uint32_t n = *P.overflow_count;
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = (gridDim.x * blockDim.x) >> 5;
     unsigned long long total_visits = 0;
@@ -400,7 +400,14 @@ __global__ void __launch_bounds__(128, LOCKSTEP_MIN_BLOCKS) k_compute_overflow(c
     if (lane == 0 && total_visits) atomicAdd(reinterpret_cast<unsigned long long *>(P.scalars + 4), total_visits);
 }
 
-// apply_light_update (updater.rs:295-363) minus the dependency re-queue (k_walk_chains<true>)
+// A texel of device 0's light volume was written: its 32-cube segment goes to the other replicas (k_push).
+__device__ __forceinline__ void mark_dirty(const LightParams &P, uint32_t idx) {
+    atomicOr(P.dirty + idx / 1024u, 1u << ((idx / 32u) & 31u));
+}
+
+// apply_light_update (updater.rs:295-363) minus the dependency re-queue (k_walk_chains<true>).  GROUP: device 0 of a
+// group marks every texel it writes dirty.
+template <bool GROUP>
 __global__ void k_apply(const LightParams P) {
     const uint32_t n = P.scalars[0];
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -412,6 +419,7 @@ __global__ void k_apply(const LightParams P) {
     atomicAdd(P.scalars + 3, 1u);
     if (d > 0) {
         light[idx] = nv;
+        if (GROUP) mark_dirty(P, idx);
         atomicMax(P.scalars + 2, (uint32_t)d);
         int x, y, z;
         cube_of(P.scene, idx, x, y, z);
@@ -427,9 +435,32 @@ __global__ void k_apply(const LightParams P) {
             if (__ldg(&P.blocks[block_id_at(P.scene, nidx)].flags) & LB_ALL_OPAQUE) continue;
             // PackedLight::guess(new.value()): re-quantise the decoded value, status Uninitialized
             const uint32_t g = scalar_in_t(lut, lut[nv & 255]) | (scalar_in_t(lut, lut[(nv >> 8) & 255]) << 8) | (scalar_in_t(lut, lut[(nv >> 16) & 255]) << 16);
-            atomicCAS(&light[nidx], nl, g);
+            const uint32_t prev = atomicCAS(&light[nidx], nl, g);
+            if (GROUP && prev == nl) mark_dirty(P, nidx);
         }
     }
+    }
+}
+
+// The push of a group's round: every 32-cube segment of device 0's light volume that k_apply wrote (one 128-byte
+// line) is stored into the other replicas' volumes over NVLink, and its dirty bit cleared.  It runs after k_apply, so
+// it stores the final values even where two guesses raced for one neighbour.  One warp per word of dirty bits.
+__global__ void __launch_bounds__(256) k_push(const LightParams P, uint32_t *const *targets, uint32_t n_targets) {
+    const uint32_t n_words = (P.volume + 1023u) / 1024u;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t w = warp; w < n_words; w += n_warps) {
+        uint32_t bits = __shfl_sync(0xffffffffu, lane == 0 ? P.dirty[w] : 0u, 0);
+        if (!bits) continue;
+        if (lane == 0) P.dirty[w] = 0u;
+        while (bits) {
+            const uint32_t idx = (w * 32u + (uint32_t)(__ffs(bits) - 1)) * 32u + lane;
+            bits &= bits - 1u;
+            if (idx < P.volume) {
+                const uint32_t v = P.scene.light[idx];
+                for (uint32_t t = 0; t < n_targets; t++) targets[t][idx] = v;
+            }
+        }
     }
 }
 
@@ -504,7 +535,8 @@ struct EditOp {
     uint8_t _pad[2];
 };
 
-__global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint32_t wide) {
+// queue: apply the pending_op too (device 0 of a group holds the queue, the other replicas take cells and light only)
+__global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint32_t wide, uint32_t queue) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const EditOp op = ops[i];
@@ -513,6 +545,7 @@ __global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint
         else ((uint16_t *)P.scene.cells)[op.idx] = (uint16_t)op.cell;
     }
     if (op.set_opaque) const_cast<uint32_t *>(P.scene.light)[op.idx] = TX_OPAQUE;
+    if (!queue) return;
     if (op.pending_op == 1) P.pending[op.idx] = 0;
     else if (op.pending_op == 2) P.pending[op.idx] = PRIO_NEWLY_VISIBLE;
 }
@@ -539,13 +572,37 @@ LightParams make_params(aicb_scene *s) {
     P.new_light = s->d_new_light.get<uint32_t>();
     P.diff = s->d_diff.get<uint8_t>();
     P.scalars = s->d_scalars.get<uint32_t>();
+    P.overflow_count = P.scalars + 9;
+    P.dirty = s->d_dirty.get<uint32_t>();
     P.volume = (uint32_t)s->volume;
     P.max_distance = s->light_max_distance;
     return P;
 }
 
-// The scene's light state, built in locals: the scene takes them once every step has succeeded.
-aicb_status ensure_light_state(aicb_scene *s) {
+// Every replica's parameters: its own field, blocks, chart, term slots and overflow list; device 0's queue, round list,
+// results and counters (peer pointers).
+std::vector<LightParams> replica_params(LightReplicas r) {
+    std::vector<LightParams> P;
+    for (size_t i = 0; i < r.n; i++) {
+        LightParams p = make_params(r.scene[i]);
+        if (i > 0) {
+            const LightParams &p0 = P[0];
+            p.tile_max = p0.tile_max;
+            p.changed = p0.changed;
+            p.pending = p0.pending;
+            p.list = p0.list;
+            p.new_light = p0.new_light;
+            p.diff = p0.diff;
+            p.scalars = p0.scalars;
+        }
+        P.push_back(p);
+    }
+    return P;
+}
+
+// The scene's light state, built in locals: the scene takes them once every step has succeeded.  `queue`: the
+// priority queue and a round's lists, which only replica 0 of a group holds.
+aicb_status ensure_light_state(aicb_scene *s, bool queue = true) {
     if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     TRY(ensure_chart(s->ctx));
     DeviceBuffer light, sky_term, pending, list, new_light, diff, scalars, tile_max, changed;
@@ -580,17 +637,18 @@ aicb_status ensure_light_state(aicb_scene *s) {
         }
         TRY(sky_term.upload(sky));
     }
-    const bool work = !s->d_pending;
+    const bool work = queue && !s->d_pending;
+    const bool overflow = !s->d_changed;   // the overflow list and the scalars: every replica's
     if (work) {
         TRY(pending.ensure(s->volume + 16));
         CU(cudaMemset(pending.get(), 0, s->volume + 16));
         TRY(list.ensure(s->volume * 4 + 16));
         TRY(new_light.ensure(s->volume * 4 + 16));
         TRY(diff.ensure(s->volume + 16));
-        TRY(scalars.ensure(16 * 4));
-        TRY(tile_max.ensure(((s->volume + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
-        TRY(changed.ensure(s->volume * 4 + 16));
     }
+    if (overflow) TRY(scalars.ensure(16 * 4));
+    if (work) TRY(tile_max.ensure(((s->volume + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
+    if (overflow) TRY(changed.ensure(s->volume * 4 + 16));
     if (light) {
         s->d_light = std::move(light);
         s->ds.light = s->d_light.get<uint32_t>();
@@ -605,26 +663,111 @@ aicb_status ensure_light_state(aicb_scene *s) {
         s->d_list = std::move(list);
         s->d_new_light = std::move(new_light);
         s->d_diff = std::move(diff);
-        s->d_scalars = std::move(scalars);
         s->d_tile_max = std::move(tile_max);
+        s->device_bytes += s->volume * 10;
+    }
+    if (overflow) {
+        s->d_scalars = std::move(scalars);
         s->d_changed = std::move(changed);
         s->device_bytes += s->volume * 4;
-        s->device_bytes += s->volume * 10;
     }
     return AICB_OK;
 }
 
-// evaluate_light (space.rs:1496-1527): rounds until the highest queued priority is <= from_difference(epsilon)
-aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits) {
+// The order between a group's streams: every other replica's stream waits until device 0's has reached this point
+// (fan_out), or device 0's until every other one's has (fan_in).
+aicb_status fan_out(LightReplicas r) {
+    aicb_ctx *c0 = r.scene[0]->ctx;
+    CU(cudaSetDevice(c0->device));
+    CU(cudaEventRecord(c0->ev_light.get(), c0->stream.get()));
+    for (size_t i = 1; i < r.n; i++) {
+        aicb_ctx *c = r.scene[i]->ctx;
+        CU(cudaSetDevice(c->device));
+        CU(cudaStreamWaitEvent(c->stream.get(), c0->ev_light.get(), 0));
+    }
+    return AICB_OK;
+}
+aicb_status fan_in(LightReplicas r) {
+    for (size_t i = 1; i < r.n; i++) {
+        aicb_ctx *c = r.scene[i]->ctx;
+        CU(cudaSetDevice(c->device));
+        CU(cudaEventRecord(c->ev_light.get(), c->stream.get()));
+    }
+    aicb_ctx *c0 = r.scene[0]->ctx;
+    CU(cudaSetDevice(c0->device));
+    for (size_t i = 1; i < r.n; i++) CU(cudaStreamWaitEvent(c0->stream.get(), r.scene[i]->ctx->ev_light.get(), 0));
+    return AICB_OK;
+}
+
+// Every replica's light state (the queue on replica 0 only) and, on a group, what a round needs beyond one context's:
+// each context's event, replica 0's dirty bits, and the other replicas' light volumes as push targets.
+aicb_status ensure_replicas(LightReplicas r) {
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.scene[i]->ctx->device));
+        TRY(ensure_light_state(r.scene[i], i == 0));
+    }
+    if (r.n == 1) return AICB_OK;
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_ctx *c = r.scene[i]->ctx;
+        if (c->ev_light) continue;
+        CU(cudaSetDevice(c->device));
+        TRY(create_event(c->ev_light, cudaEventDisableTiming));
+    }
+    aicb_scene *s = r.scene[0];
+    CU(cudaSetDevice(s->ctx->device));
+    if (!s->d_dirty) {
+        const size_t bytes = (s->volume + 1023) / 1024 * 4 + 16;
+        DeviceBuffer dirty;
+        TRY(dirty.ensure(bytes));
+        CU(cudaMemset(dirty.get(), 0, bytes));
+        s->d_dirty = std::move(dirty);
+        s->device_bytes += bytes;
+    }
+    std::vector<uint32_t *> targets;
+    for (size_t i = 1; i < r.n; i++) targets.push_back(const_cast<uint32_t *>(r.scene[i]->ds.light));
+    TRY(s->d_push_targets.ensure(targets.size() * sizeof(uint32_t *)));
+    CU(cudaMemcpy(s->d_push_targets.get(), targets.data(), targets.size() * sizeof(uint32_t *), cudaMemcpyHostToDevice));
+    // device 0 writes the other replicas' volumes: after what their streams hold (aicb_scene_update_cubes is queued)
+    return fan_in(r);
+}
+
+// evaluate_light (space.rs:1496-1527): rounds until the highest queued priority is <= from_difference(epsilon).
+// A round: device 0 gathers the cubes of the round's band from its queue; every replica walks a share of them against
+// its own field (compute form + the overflow it met), taking cubes from device 0's counter and writing device 0's
+// results; device 0 applies them; on a group it pushes the segments it wrote to the other replicas; every replica
+// then walks a share of the changed cubes (mark form), raising priorities in device 0's queue.  Compute is Jacobi
+// within a round and marks merge by max, so a group performs one context's operations.  One context issues no event
+// and no push.
+aicb_status propagate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits) {
+    aicb_scene *s = r.scene[0];
     aicb_ctx *ctx = s->ctx;
     cudaStream_t st = ctx->stream.get();
-    LightParams P = make_params(s);
-    P.epsilon_priority = (uint32_t)epsilon / 2 + 1;
+    const bool group = r.n > 1;
+    std::vector<LightParams> RP = replica_params(r);
+    for (LightParams &p : RP) p.epsilon_priority = (uint32_t)epsilon / 2 + 1;
+    const LightParams &P = RP[0];
     const int blocks = ctx->num_sms * 8;
     const int wide = ctx->num_sms * 8;    // 128-thread blocks of k_compute_overflow and k_apply (grid-stride)
     const uint32_t n_tiles = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
     uint64_t total = 0, visits = 0, rounds = 0;
     uint32_t maxd = 0;
+    // every replica's walk of one form: replica i against its own field, on its own context
+    auto walk = [&](bool mark) -> aicb_status {
+        for (size_t i = 0; i < r.n; i++) {
+            aicb_ctx *c = r.scene[i]->ctx;
+            cudaStream_t cs = c->stream.get();
+            if (group) CU(cudaSetDevice(c->device));
+            if (mark) {
+                k_walk_chains<true><<<c->chain_walk_blocks, 128, 0, cs>>>(RP[i], 0, nullptr);
+                continue;
+            }
+            if (i > 0) CU(cudaMemsetAsync(RP[i].overflow_count, 0, 4, cs));   // (device 0's: with the round's counters)
+            k_walk_chains<false><<<c->chain_walk_blocks, 128, 0, cs>>>(RP[i], 0, nullptr);
+            k_compute_overflow<<<c->num_sms * 8, 128, 0, cs>>>(RP[i], nullptr);
+        }
+        if (group) CU(cudaSetDevice(ctx->device));
+        return AICB_OK;
+    };
     CU(cudaEventRecord(ctx->ev0.get(), st));
     CU(cudaMemsetAsync(P.scalars, 0, 16 * 4, st));
     k_tile_rebuild<<<blocks, 256, 0, st>>>(P, n_tiles);   // (fast_evaluate / edits write the priority bytes directly)
@@ -635,11 +778,18 @@ aicb_status propagate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, ui
             CU(cudaMemsetAsync(P.scalars + 6, 0, 4 * 4, st));   // ... its count of changed cubes, the two work counters, the overflow count
             k_find_max<<<16, 256, 0, st>>>(P, n_tiles);
             k_gather<<<blocks, 256, 0, st>>>(P, n_tiles);
-            k_walk_chains<false><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
-            k_compute_overflow<<<wide, 128, 0, st>>>(P, nullptr);
-            k_apply<<<wide, 128, 0, st>>>(P);
+            if (group) TRY(fan_out(r));
+            TRY(walk(false));
+            if (group) TRY(fan_in(r));
+            if (group) k_apply<true><<<wide, 128, 0, st>>>(P);
+            else k_apply<false><<<wide, 128, 0, st>>>(P);
             k_compact_changed<<<blocks, 256, 0, st>>>(P);
-            k_walk_chains<true><<<ctx->chain_walk_blocks, 128, 0, st>>>(P, 0, nullptr);
+            if (group) {
+                k_push<<<blocks, 256, 0, st>>>(P, s->d_push_targets.get<uint32_t *const>(), (uint32_t)(r.n - 1));
+                TRY(fan_out(r));
+            }
+            TRY(walk(true));
+            if (group) TRY(fan_in(r));   // (the next round's queue holds every replica's marks)
         }
         uint32_t h[8];
         CU(cudaMemcpyAsync(h, P.scalars, 8 * 4, cudaMemcpyDeviceToHost, st));
@@ -713,95 +863,77 @@ aicb_status aicb_light_blocks_update(aicb_scene *s, const uint16_t *indices, con
 }
 
 // ---------------------------------------------------------------------------------------------
-// C ABI
+// the light calls over a scene's replicas (internal.h): one context's entry points below, a group's in group.cu
 // ---------------------------------------------------------------------------------------------
-extern "C" {
-
-uint32_t aicb_light_chart_chains(uint32_t *preorder, uint32_t (*chains)[6], uint16_t *euler) {
-    const ChainTables &t = chain_tables_host();
-    if (preorder) {
-        std::vector<uint32_t> order;
-        build_chart_preorder(build_chart(), &order);
-        std::memcpy(preorder, order.data(), order.size() * sizeof(uint32_t));
-    }
-    if (chains)
-        for (size_t c = 0; c < t.chains.size(); c++) {
-            const LightChain &ch = t.chains[c];
-            chains[c][0] = ch.first_node; chains[c][1] = ch.length; chains[c][2] = ch.n_children;
-            chains[c][3] = ch.first_child; chains[c][4] = ch.parent_branch; chains[c][5] = ch.branch;
-        }
-    if (euler) std::memcpy(euler, t.euler.data(), t.euler.size() * sizeof(uint16_t));
-    return (uint32_t)t.chains.size();
-}
-
-uint32_t aicb_light_chart(float *weights, uint32_t *children) {
-    static const std::vector<LightChartNode> chart = build_chart();
-    for (size_t i = 0; i < chart.size(); i++) {
-        if (weights) std::memcpy(weights + 6 * i, chart[i].w, 24);
-        if (children) std::memcpy(children + 6 * i, chart[i].child, 24);
-    }
-    return (uint32_t)chart.size();
-}
-
-aicb_status aicb_light_fast_evaluate(aicb_scene *s) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    CU(cudaSetDevice(s->ctx->device));
-    aicb_status st = ensure_light_state(s);
-    if (st != AICB_OK) return st;
+aicb_status light_fast_evaluate(LightReplicas r) {
+    TRY(ensure_replicas(r));
+    aicb_scene *s = r.scene[0];
+    cudaStream_t stream = s->ctx->stream.get();
     LightParams P = make_params(s);
     const uint32_t cols = (uint32_t)s->ds.size[0] * (uint32_t)s->ds.size[2];
-    if (cols) k_fast_evaluate<<<(cols + 127) / 128, 128, 0, s->ctx->stream.get()>>>(P);
+    if (cols) k_fast_evaluate<<<(cols + 127) / 128, 128, 0, stream>>>(P);
     CU(cudaGetLastError());
-    CU(cudaStreamSynchronize(s->ctx->stream.get()));
+    // the other replicas take the whole volume once (peer copies)
+    for (size_t i = 1; i < r.n; i++)
+        CU(cudaMemcpyAsync(r.scene[i]->d_light.get(), s->d_light.get(), s->volume * 4, cudaMemcpyDefault, stream));
+    CU(cudaStreamSynchronize(stream));
     return AICB_OK;
 }
 
-aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
-    if (!s || (n && (!cubes || !out))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    CU(cudaSetDevice(s->ctx->device));
-    aicb_status st = ensure_light_state(s);
-    if (st != AICB_OK) return st;
+// The cubes are split across the replicas by device 0's work counter; every replica computes the overflow of its own
+// walks; the outputs are device 0's, in input order.
+aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
+    TRY(ensure_replicas(r));
     if (!n) return AICB_OK;
-    LightParams P = make_params(s);
+    aicb_scene *s = r.scene[0];
+    const bool group = r.n > 1;
+    const std::vector<LightParams> RP = replica_params(r);
+    const LightParams &P = RP[0];
     cudaStream_t stream = s->ctx->stream.get();
-    DeviceBuffer d_cubes;
+    DeviceBuffer d_cubes;   // on device 0; the other replicas read it over peer access
     TRY(d_cubes.upload(cubes, n * 12));
-    cudaMemsetAsync(P.scalars, 0, 16 * 4, stream);
-    k_walk_chains<false><<<s->ctx->chain_walk_blocks, 128, 0, stream>>>(P, (uint32_t)n, d_cubes.get<int32_t>());
-    k_compute_overflow<<<s->ctx->num_sms * 8, 128, 0, stream>>>(P, d_cubes.get<int32_t>());
+    const int32_t *explicit_cubes = d_cubes.get<int32_t>();
+    CU(cudaMemsetAsync(P.scalars, 0, 16 * 4, stream));
+    if (group) TRY(fan_out(r));
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_ctx *c = r.scene[i]->ctx;
+        cudaStream_t cs = c->stream.get();
+        if (group) CU(cudaSetDevice(c->device));
+        if (i > 0) CU(cudaMemsetAsync(RP[i].overflow_count, 0, 4, cs));
+        k_walk_chains<false><<<c->chain_walk_blocks, 128, 0, cs>>>(RP[i], (uint32_t)n, explicit_cubes);
+        k_compute_overflow<<<c->num_sms * 8, 128, 0, cs>>>(RP[i], explicit_cubes);
+    }
+    if (group) TRY(fan_in(r));
     uint32_t h[16];
     CU(cudaMemcpyAsync(out, P.new_light, n * 4, cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(h, P.scalars, sizeof h, cudaMemcpyDeviceToHost, stream));
     CU(cudaStreamSynchronize(stream));
+    uint64_t overflowed = h[9];
+    for (size_t i = 1; i < r.n; i++) {   // (every replica's stream is done: device 0's waited for them)
+        uint32_t c = 0;
+        CU(cudaMemcpy(&c, RP[i].overflow_count, 4, cudaMemcpyDeviceToHost));
+        overflowed += c;
+    }
     s->light_stats[0] = n;
     s->light_stats[1] = (uint64_t)h[4] | ((uint64_t)h[5] << 32);
-    s->light_stats[2] = h[9];   // cubes that took the lockstep walk (a chain with more terms than its slots)
+    s->light_stats[2] = overflowed;   // cubes that took the lockstep walk (a chain with more terms than its slots)
     s->light_stats[3] = 0;
     return AICB_OK;
 }
 
-aicb_status aicb_light_evaluate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
-                                uint64_t *node_visits) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    CU(cudaSetDevice(s->ctx->device));
-    aicb_status st = ensure_light_state(s);
-    if (st != AICB_OK) return st;
-    return propagate(s, epsilon, updates_done, max_diff, node_visits);
+aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
+                           uint64_t *node_visits) {
+    TRY(ensure_replicas(r));
+    return propagate(r, epsilon, updates_done, max_diff, node_visits);
 }
 
 // Mutation::set x n (space.rs:1346-1352 -> side_effects_of_set -> modified_cube_needs_update,
-// updater.rs:135-173) applied in order on the host mirror, then evaluate_light(epsilon).
-aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
-                                          uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
-    if (!s || (n_edits && (!cubes || !new_ids))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    CU(cudaSetDevice(s->ctx->device));
-    aicb_status st = ensure_light_state(s);
-    if (st != AICB_OK) return st;
+// updater.rs:135-173) applied in order on the host mirror, then evaluate_light(epsilon).  Every replica takes the
+// mirror's, the cells' and the light's changes; only replica 0 holds the queue.
+aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
+                                     uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
+    TRY(ensure_replicas(r));
+    aicb_scene *s = r.scene[0];
     const DeviceScene &ds = s->ds;
     auto index_of = [&](int x, int y, int z, uint32_t *idx) {
         uint32_t dx = (uint32_t)(x - ds.lo[0]), dy = (uint32_t)(y - ds.lo[1]), dz = (uint32_t)(z - ds.lo[2]);
@@ -854,27 +986,99 @@ aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[
         std::vector<EditOp> flat;
         flat.reserve(ops.size());
         for (auto &kv : ops) flat.push_back(kv.second);
-        cudaStream_t stream = s->ctx->stream.get();
-        DeviceBuffer d_ops;
-        TRY(d_ops.ensure(flat.size() * sizeof(EditOp)));
-        CU(cudaMemcpyAsync(d_ops.get(), flat.data(), flat.size() * sizeof(EditOp), cudaMemcpyHostToDevice, stream));
-        LightParams P = make_params(s);
-        k_edits<<<(unsigned)((flat.size() + 127) / 128), 128, 0, stream>>>(P, d_ops.get<EditOp>(), (uint32_t)flat.size(), ds.wide_cells);
-        CU(cudaStreamSynchronize(stream));
+        for (size_t i = 0; i < r.n; i++) {
+            aicb_scene *ri = r.scene[i];
+            if (i > 0)
+                for (const EditOp &o : flat)
+                    if (o.cell != 0xffffffffu) ri->h_ids[o.idx] = s->h_ids[o.idx];
+            CU(cudaSetDevice(ri->ctx->device));
+            cudaStream_t stream = ri->ctx->stream.get();
+            DeviceBuffer d_ops;
+            TRY(d_ops.ensure(flat.size() * sizeof(EditOp)));
+            CU(cudaMemcpyAsync(d_ops.get(), flat.data(), flat.size() * sizeof(EditOp), cudaMemcpyHostToDevice, stream));
+            LightParams P = make_params(ri);
+            k_edits<<<(unsigned)((flat.size() + 127) / 128), 128, 0, stream>>>(P, d_ops.get<EditOp>(), (uint32_t)flat.size(),
+                                                                               ds.wide_cells, i == 0);
+            CU(cudaStreamSynchronize(stream));
+        }
+        CU(cudaSetDevice(s->ctx->device));
     }
-    return propagate(s, epsilon, updates_done, max_diff, nullptr);
+    return propagate(r, epsilon, updates_done, max_diff, nullptr);
 }
 
-aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
+aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     if (!s || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n_texels != s->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
     if (!s->d_light) return aicb_fail(AICB_ERR_INVALID, "scene has no light volume (LightPhysics::None)");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     // ordered behind everything queued on the context's stream (cube deltas, propagation)
     CU(cudaMemcpyAsync(out, s->d_light.get(), s->volume * 4, cudaMemcpyDeviceToHost, s->ctx->stream.get()));
     CU(cudaStreamSynchronize(s->ctx->stream.get()));
     return AICB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// C ABI
+// ---------------------------------------------------------------------------------------------
+extern "C" {
+
+uint32_t aicb_light_chart_chains(uint32_t *preorder, uint32_t (*chains)[6], uint16_t *euler) {
+    const ChainTables &t = chain_tables_host();
+    if (preorder) {
+        std::vector<uint32_t> order;
+        build_chart_preorder(build_chart(), &order);
+        std::memcpy(preorder, order.data(), order.size() * sizeof(uint32_t));
+    }
+    if (chains)
+        for (size_t c = 0; c < t.chains.size(); c++) {
+            const LightChain &ch = t.chains[c];
+            chains[c][0] = ch.first_node; chains[c][1] = ch.length; chains[c][2] = ch.n_children;
+            chains[c][3] = ch.first_child; chains[c][4] = ch.parent_branch; chains[c][5] = ch.branch;
+        }
+    if (euler) std::memcpy(euler, t.euler.data(), t.euler.size() * sizeof(uint16_t));
+    return (uint32_t)t.chains.size();
+}
+
+uint32_t aicb_light_chart(float *weights, uint32_t *children) {
+    static const std::vector<LightChartNode> chart = build_chart();
+    for (size_t i = 0; i < chart.size(); i++) {
+        if (weights) std::memcpy(weights + 6 * i, chart[i].w, 24);
+        if (children) std::memcpy(children + 6 * i, chart[i].child, 24);
+    }
+    return (uint32_t)chart.size();
+}
+
+aicb_status aicb_light_fast_evaluate(aicb_scene *s) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_fast_evaluate({&s, 1});
+}
+
+aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
+    if (!s || (n && (!cubes || !out))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_compute({&s, 1}, cubes, n, out);
+}
+
+aicb_status aicb_light_evaluate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
+                                uint64_t *node_visits) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_evaluate({&s, 1}, epsilon, updates_done, max_diff, node_visits);
+}
+
+aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
+                                          uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
+    if (!s || (n_edits && (!cubes || !new_ids))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_edit_and_propagate({&s, 1}, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+}
+
+aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_download(s, out, n_texels);
 }
 
 aicb_status aicb_light_stats(const aicb_scene *s, uint64_t out[4]) {

@@ -88,7 +88,11 @@ struct LightParams {
     const uint16_t *euler;          // the Euler tour of the chain tree: chain | (0: its entry terms, 1: its pop term) << 15
     uint32_t n_chains, n_euler;
     float4 *term_scratch;           // per resident warp: LIGHT_MAX_CHAINS * LIGHT_CHAIN_SLOTS terms
-    uint32_t *overflow;             // list entries whose walk needs more than LIGHT_CHAIN_K terms in one chain ([9] counts them)
+    uint32_t *overflow;             // list entries whose walk needs more than LIGHT_CHAIN_K terms in one chain
+    uint32_t *overflow_count;       // ... and their count (scalars + 9 of the replica's own scalars: every device of a
+                                    // group computes the overflow of its own walks)
+    uint32_t *dirty;                // device 0 of a group: one bit per 32-cube segment of the light volume written this
+                                    // round, for the push to the other replicas (nullptr on one context)
     const float4 *sky_term;         // per preorder node: the sky light its bundle collects at the end of a ray (end_of_ray)
     uint32_t chart_nodes;
     uint32_t *tile_max;             // per LIGHT_TILE cubes: an upper bound of the tile's highest queued priority
@@ -99,7 +103,8 @@ struct LightParams {
     uint32_t *changed;              // positions in the round's list whose cube changed by more than one unit (the mark walk's work)
     uint32_t *scalars;              // [0] list length, [1] max priority, [2] max diff, [3] updates, [4..5] node visits, [6] changed,
                                     // [7] / [8] cubes handed out by the chain walk's compute / mark form this round,
-                                    // [9] overflow list length
+                                    // [9] overflow list length.  On a group every replica's kernels use device 0's
+                                    // scalars, except [9], which is each replica's own (overflow_count).
     uint32_t volume;
     uint32_t max_distance;
     uint32_t priority;              // the round's priority level

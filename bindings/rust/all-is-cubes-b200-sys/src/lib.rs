@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 5 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 6 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -290,4 +290,14 @@ unsafe extern "C" {
                                          epsilon: u8, updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
     pub fn aicb_light_download(s: *mut aicb_scene, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_light_stats(s: *const aicb_scene, out: *mut [u64; 4]) -> aicb_status;
+
+    pub fn aicb_group_light_fast_evaluate(gs: *mut aicb_group_scene) -> aicb_status;
+    pub fn aicb_group_light_compute(gs: *mut aicb_group_scene, cubes: *const [i32; 3], n: usize, out: *mut [u8; 4]) -> aicb_status;
+    pub fn aicb_group_light_evaluate(gs: *mut aicb_group_scene, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8,
+                                     chart_node_visits: *mut u64) -> aicb_status;
+    pub fn aicb_group_light_edit_and_propagate(gs: *mut aicb_group_scene, cubes: *const [i32; 3], new_ids: *const u16,
+                                               n_edits: usize, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8)
+                                               -> aicb_status;
+    pub fn aicb_group_light_download(gs: *mut aicb_group_scene, replica: c_int, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
+    pub fn aicb_group_light_stats(gs: *const aicb_group_scene, out: *mut [u64; 4]) -> aicb_status;
 }

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 5
+#define AICB_ABI_VERSION 6
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -472,6 +472,31 @@ aicb_status aicb_light_download(aicb_scene *, uint8_t (*out)[4], size_t n_texels
  * After aicb_light_compute: out[0] cubes computed, out[1] chart nodes visited, out[2] cubes whose walk needed more
  * term slots than the chain walk holds and took the lockstep walk instead, out[3] 0. */
 aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
+
+/* The light calls above on a device group (csrc/group.cu, csrc/light.cu), with their arguments, validation, errors and
+ * results: LightStorage::fast_evaluate_light / compute_light / Mutation::set x n + evaluate_light
+ * (space/light/updater.rs:537-582, 368-418, 135-363; space.rs:1346-1352, 1496-1527).  Validation is against replica 0
+ * before anything changes: a rejected call changes no replica.  A scene with LightPhysics::None is AICB_ERR_INVALID.
+ * The first light call of a group enables device 0's peer access to every other device and checks native peer
+ * atomics (AICB_ERR_UNSUPPORTED without them); a device named more than once needs neither.  Each call holds every
+ * context of the group until it returns, and leaves the replicas' light volumes identical.
+ * A relaxation round: device 0 gathers the round's cubes from its queue; every device computes a share of them against
+ * its own replica (cubes handed out one at a time by device 0's counter); device 0 applies the results and stores the
+ * 32-cube segments it wrote into every other replica (NVLink); every device re-queues the dependencies of a share of
+ * the changed cubes in device 0's queue.  The group performs one context's operations, so its results meet the same
+ * contract.  aicb_group_light_compute splits the cubes across the devices the same way; outputs in input order. */
+aicb_status aicb_group_light_fast_evaluate(aicb_group_scene *);
+aicb_status aicb_group_light_compute(aicb_group_scene *, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]);
+aicb_status aicb_group_light_evaluate(aicb_group_scene *, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
+                                      uint64_t *chart_node_visits_or_null);
+aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
+                                                size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
+                                                uint8_t *max_diff);
+/* Replica `replica` (0 .. group size - 1) of the light volume. */
+aicb_status aicb_group_light_download(aicb_group_scene *, int replica, uint8_t (*out)[4], size_t n_texels);
+/* aicb_light_stats of the group's last light call: counters summed over the devices; out[3] is device 0's device time
+ * of the whole propagation (device 0 waits for every device in every round). */
+aicb_status aicb_group_light_stats(const aicb_group_scene *, uint64_t out[4]);
 
 #ifdef __cplusplus
 }
