@@ -144,6 +144,10 @@ def load_library() -> C.CDLL:
                                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
     lib.aicb_group_light_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
     lib.aicb_group_light_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+    for prefix in ("aicb_light", "aicb_group_light"):
+        getattr(lib, prefix + "_changes_count").argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
+        getattr(lib, prefix + "_take_changes").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                           C.POINTER(C.c_size_t)]
     if lib.aicb_abi_version() != abi.ABI_VERSION:
         raise RuntimeError("libaicb200.so ABI version mismatch")
     _lib = lib
@@ -725,9 +729,41 @@ class SpaceRaytracer:
         _check(load_library().aicb_light_download(self.handle, out.ctypes.data, out.size // 4))
         return out
 
+    def light_changes_count(self) -> int:
+        """The number of cubes whose light texel the light calls wrote since the set was last taken
+        (SpaceChange::CubeLight, space.rs:1079-1083)."""
+        return _light_changes_count(load_library().aicb_light_changes_count, self.handle)
+
+    def light_take_changes(self, discard: bool = False):
+        """Take the set of changed cubes -> (indices uint32[n], texels uint8[n, 4]): Z-major linear indices in increasing
+        order and each cube's texel as it is now.  discard=True empties the set without copying (both arrays empty)."""
+        return _light_take_changes(load_library().aicb_light_changes_count, load_library().aicb_light_take_changes,
+                                   self.handle, discard)
+
     def upload_light(self, light: np.ndarray):
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
         _check(load_library().aicb_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
+
+
+def _light_changes_count(count_fn, handle) -> int:
+    n = C.c_size_t(0)
+    _check(count_fn(handle, C.byref(n)))
+    return int(n.value)
+
+
+def _light_take_changes(count_fn, take_fn, handle, discard: bool):
+    indices = np.zeros(0, dtype=np.uint32)
+    texels = np.zeros((0, 4), dtype=np.uint8)
+    got = C.c_size_t(0)
+    if discard:
+        _check(take_fn(handle, None, None, 0, C.byref(got)))
+        return indices, texels
+    n = _light_changes_count(count_fn, handle)
+    if n:
+        indices = np.zeros(n, dtype=np.uint32)
+        texels = np.zeros((n, 4), dtype=np.uint8)
+        _check(take_fn(handle, indices.ctypes.data, texels.ctypes.data, n, C.byref(got)))
+    return indices, texels
 
 
 NO_WORLD_TO_SHOW_SRGB8 = (0xBC, 0xBC, 0xBC, 0xFF)   # content/palette.rs:76
@@ -950,6 +986,16 @@ class GroupScene:
         out = np.zeros(self.space.size + (4,), dtype=np.uint8)
         _check(load_library().aicb_group_light_download(self.handle, replica, out.ctypes.data, out.size // 4))
         return out
+
+    def light_changes_count(self) -> int:
+        """SpaceRaytracer.light_changes_count of the group: the set is device 0's, and every replica's texels are
+        identical."""
+        return _light_changes_count(load_library().aicb_group_light_changes_count, self.handle)
+
+    def light_take_changes(self, discard: bool = False):
+        """SpaceRaytracer.light_take_changes of the group -> (indices uint32[n], texels uint8[n, 4])."""
+        return _light_take_changes(load_library().aicb_group_light_changes_count,
+                                   load_library().aicb_group_light_take_changes, self.handle, discard)
 
     def close(self):
         if self.handle:

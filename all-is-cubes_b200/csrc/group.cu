@@ -439,6 +439,21 @@ aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t
     return light_download(gs->scene[replica], out, n_texels);
 }
 
+// The set of changed cubes is device 0's: device 0 applies every round and the push keeps the replicas identical, so its
+// indices and texels are every replica's.
+aicb_status aicb_group_light_changes_count(const aicb_group_scene *gs, size_t *n_changed) {
+    if (!gs || !n_changed) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    GroupLock lock(gs->group);
+    return light_changes_count(gs->scene[0], n_changed);
+}
+
+aicb_status aicb_group_light_take_changes(aicb_group_scene *gs, uint32_t *indices, uint8_t (*texels)[4], size_t capacity,
+                                          size_t *n_taken) {
+    if (!gs || !n_taken) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    GroupLock lock(gs->group);
+    return light_take_changes(gs->scene[0], indices, texels, capacity, n_taken);
+}
+
 aicb_status aicb_group_light_stats(const aicb_group_scene *gs, uint64_t out[4]) {
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     return aicb_light_stats(gs->scene[0], out);   // device 0's counters are the group's (light.cu)

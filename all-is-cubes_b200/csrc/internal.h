@@ -216,6 +216,8 @@ struct aicb_scene {
     DeviceBuffer d_sky_term;                // per chart node: the sky light its bundle collects (end_of_ray), for this scene's sky
     DeviceBuffer d_changed;                 // list positions whose cube changed by more than one unit this round
     DeviceBuffer d_tile_max;                // per LIGHT_TILE cubes: upper bound of the queued priorities
+    DeviceBuffer d_changes;                 // one bit per cube: the set of changed cubes (SpaceChange::CubeLight), kept
+                                            // across calls until the host takes it; replica 0 of a group holds it
     // replica 0 of a group scene: the light volume's segments written this round, and the other replicas' volumes
     DeviceBuffer d_dirty;
     DeviceBuffer d_push_targets;
@@ -319,3 +321,6 @@ aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_d
 aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels);
+// The set of changed cubes of replica 0 (the other replicas' texels are identical); the caller holds the locks.
+aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed);
+aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity, size_t *n_taken);

@@ -405,8 +405,14 @@ __device__ __forceinline__ void mark_dirty(const LightParams &P, uint32_t idx) {
     atomicOr(P.dirty + idx / 1024u, 1u << ((idx / 32u) & 31u));
 }
 
-// apply_light_update (updater.rs:295-363) minus the dependency re-queue (k_walk_chains<true>).  GROUP: device 0 of a
-// group marks every texel it writes dirty.
+// A light call wrote the cube's texel: it enters the set of changed cubes (SpaceChange::CubeLight).
+__device__ __forceinline__ void mark_changed(const LightParams &P, uint32_t idx) {
+    atomicOr(P.changes + idx / 32u, 1u << (idx & 31u));
+}
+
+// apply_light_update (updater.rs:295-363) minus the dependency re-queue (k_walk_chains<true>).  Every stored value and
+// every guess written into an Uninitialized neighbour enters the set of changed cubes (updater.rs:313-317, 335-338).
+// GROUP: device 0 of a group also marks every texel it writes dirty.
 template <bool GROUP>
 __global__ void k_apply(const LightParams P) {
     const uint32_t n = P.scalars[0];
@@ -419,6 +425,7 @@ __global__ void k_apply(const LightParams P) {
     atomicAdd(P.scalars + 3, 1u);
     if (d > 0) {
         light[idx] = nv;
+        mark_changed(P, idx);
         if (GROUP) mark_dirty(P, idx);
         atomicMax(P.scalars + 2, (uint32_t)d);
         int x, y, z;
@@ -436,7 +443,10 @@ __global__ void k_apply(const LightParams P) {
             // PackedLight::guess(new.value()): re-quantise the decoded value, status Uninitialized
             const uint32_t g = scalar_in_t(lut, lut[nv & 255]) | (scalar_in_t(lut, lut[(nv >> 8) & 255]) << 8) | (scalar_in_t(lut, lut[(nv >> 16) & 255]) << 16);
             const uint32_t prev = atomicCAS(&light[nidx], nl, g);
-            if (GROUP && prev == nl) mark_dirty(P, nidx);
+            if (prev == nl) {
+                mark_changed(P, nidx);
+                if (GROUP) mark_dirty(P, nidx);
+            }
         }
     }
     }
@@ -492,7 +502,8 @@ __global__ void __launch_bounds__(256) k_compact_changed(const LightParams P) {
     }
 }
 
-// fast_evaluate_light (updater.rs:537-582): one thread per (x, z) column, top down
+// fast_evaluate_light (updater.rs:537-582): one thread per (x, z) column, top down.  The reference announces none of
+// these writes (its TODO for EveryBlock); a texel whose value changes enters the set of changed cubes all the same.
 __global__ void k_fast_evaluate(const LightParams P) {
     const DeviceScene &S = P.scene;
     const uint32_t col = blockIdx.x * blockDim.x + threadIdx.x;
@@ -522,6 +533,7 @@ __global__ void k_fast_evaluate(const LightParams P) {
                 value = TX_NO_RAYS;
             }
         }
+        if (light[idx] != value) mark_changed(P, idx);
         light[idx] = value;
         P.pending[idx] = pend;
     }
@@ -535,7 +547,9 @@ struct EditOp {
     uint8_t _pad[2];
 };
 
-// queue: apply the pending_op too (device 0 of a group holds the queue, the other replicas take cells and light only)
+// queue: apply the pending_op too and mark the cubes set to OPAQUE changed (device 0 of a group holds the queue and the
+// set, the other replicas take cells and light only).  A cube set to OPAQUE is changed even if it already was
+// (modified_cube_needs_update, updater.rs:153-161).
 __global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint32_t wide, uint32_t queue) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -544,10 +558,100 @@ __global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint
         if (wide) ((uint32_t *)P.scene.cells)[op.idx] = op.cell;
         else ((uint16_t *)P.scene.cells)[op.idx] = (uint16_t)op.cell;
     }
-    if (op.set_opaque) const_cast<uint32_t *>(P.scene.light)[op.idx] = TX_OPAQUE;
+    if (op.set_opaque) {
+        const_cast<uint32_t *>(P.scene.light)[op.idx] = TX_OPAQUE;
+        if (queue) mark_changed(P, op.idx);
+    }
     if (!queue) return;
     if (op.pending_op == 1) P.pending[op.idx] = 0;
     else if (op.pending_op == 2) P.pending[op.idx] = PRIO_NEWLY_VISIBLE;
+}
+
+// Taking the set of changed cubes: an ordered stream compaction of the bitmap.  A chunk is the CHANGES_CHUNK_WORDS
+// words of bits (32 768 cubes) one 256-thread block reads, four consecutive words per thread.
+constexpr uint32_t CHANGES_CHUNK_WORDS = 1024;
+
+// The exclusive prefix of `v` over the block's 256 threads, in thread order; the block's total in *total.
+__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t *total) {
+    __shared__ uint32_t s_part[8];
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint32_t inc = v;
+    for (int off = 1; off < 32; off <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, inc, off);
+        if ((int)lane >= off) inc += t;
+    }
+    if (lane == 31) s_part[wid] = inc;
+    __syncthreads();
+    uint32_t before = 0, sum = 0;
+    for (uint32_t k = 0; k < 8; k++) {
+        if (k < wid) before += s_part[k];
+        sum += s_part[k];
+    }
+    *total = sum;
+    return before + inc - v;
+}
+
+// 1. the number of changed cubes in each chunk
+__global__ void __launch_bounds__(256) k_changes_count(const uint32_t *bits, uint32_t n_words, uint32_t *chunk_sums) {
+    const uint32_t w0 = blockIdx.x * CHANGES_CHUNK_WORDS + threadIdx.x * 4u;
+    uint32_t c = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) c += w0 + k < n_words ? __popc(bits[w0 + k]) : 0u;
+    uint32_t total;
+    block_exclusive_scan(c, &total);
+    if (threadIdx.x == 0) chunk_sums[blockIdx.x] = total;
+}
+
+// 2. one block of 1024 threads: the chunk sums become each chunk's first output position, in place, and
+// chunk_sums[n_chunks] the size of the set
+__global__ void __launch_bounds__(1024) k_changes_scan(uint32_t *chunk_sums, uint32_t n_chunks) {
+    __shared__ uint32_t s_part[32];
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t per = (n_chunks + 1023u) / 1024u, c0 = threadIdx.x * per;
+    uint32_t run = 0;
+    for (uint32_t c = c0; c < c0 + per && c < n_chunks; c++) run += chunk_sums[c];
+    uint32_t inc = run;
+    for (int off = 1; off < 32; off <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, inc, off);
+        if ((int)lane >= off) inc += t;
+    }
+    if (lane == 31) s_part[wid] = inc;
+    __syncthreads();
+    uint32_t at = inc - run;
+    for (uint32_t k = 0; k < wid; k++) at += s_part[k];
+    for (uint32_t c = c0; c < c0 + per && c < n_chunks; c++) {
+        const uint32_t v = chunk_sums[c];
+        chunk_sums[c] = at;
+        at += v;
+    }
+    if (threadIdx.x == 1023) chunk_sums[n_chunks] = at;
+}
+
+// 3. every changed cube's index, in increasing order, and its texel as it is now; the words read are cleared
+__global__ void __launch_bounds__(256) k_changes_emit(uint32_t *bits, uint32_t n_words, const uint32_t *chunk_starts,
+                                                       const uint32_t *light, uint32_t *out_indices, uint32_t *out_texels) {
+    const uint32_t w0 = blockIdx.x * CHANGES_CHUNK_WORDS + threadIdx.x * 4u;
+    uint32_t word[4], c = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) {
+        word[k] = w0 + k < n_words ? bits[w0 + k] : 0u;
+        c += __popc(word[k]);
+    }
+    uint32_t total;
+    uint32_t at = chunk_starts[blockIdx.x] + block_exclusive_scan(c, &total);
+#pragma unroll
+    for (uint32_t k = 0; k < 4; k++) {
+        uint32_t b = word[k];
+        if (!b) continue;
+        bits[w0 + k] = 0u;
+        while (b) {
+            const uint32_t idx = (w0 + k) * 32u + (uint32_t)(__ffs(b) - 1);
+            b &= b - 1u;
+            out_indices[at] = idx;
+            out_texels[at] = light[idx];
+            at++;
+        }
+    }
 }
 
 LightParams make_params(aicb_scene *s) {
@@ -574,6 +678,7 @@ LightParams make_params(aicb_scene *s) {
     P.scalars = s->d_scalars.get<uint32_t>();
     P.overflow_count = P.scalars + 9;
     P.dirty = s->d_dirty.get<uint32_t>();
+    P.changes = s->d_changes.get<uint32_t>();
     P.volume = (uint32_t)s->volume;
     P.max_distance = s->light_max_distance;
     return P;
@@ -601,11 +706,12 @@ std::vector<LightParams> replica_params(LightReplicas r) {
 }
 
 // The scene's light state, built in locals: the scene takes them once every step has succeeded.  `queue`: the
-// priority queue and a round's lists, which only replica 0 of a group holds.
+// priority queue, a round's lists and the set of changed cubes, which only replica 0 of a group holds.
 aicb_status ensure_light_state(aicb_scene *s, bool queue = true) {
     if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     TRY(ensure_chart(s->ctx));
-    DeviceBuffer light, sky_term, pending, list, new_light, diff, scalars, tile_max, changed;
+    DeviceBuffer light, sky_term, pending, list, new_light, diff, scalars, tile_max, changed, changes;
+    const size_t change_bytes = (s->volume + 31) / 32 * 4;
     if (!s->d_light) {  // a scene created without a light volume starts all NO_RAYS (initialize_light, updater.rs:628-656)
         const std::vector<uint32_t> init(s->volume, TX_NO_RAYS);
         TRY(light.upload(init.data(), s->volume * 4, 16));
@@ -645,6 +751,8 @@ aicb_status ensure_light_state(aicb_scene *s, bool queue = true) {
         TRY(list.ensure(s->volume * 4 + 16));
         TRY(new_light.ensure(s->volume * 4 + 16));
         TRY(diff.ensure(s->volume + 16));
+        TRY(changes.ensure(change_bytes));
+        CU(cudaMemset(changes.get(), 0, change_bytes));
     }
     if (overflow) TRY(scalars.ensure(16 * 4));
     if (work) TRY(tile_max.ensure(((s->volume + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
@@ -664,7 +772,8 @@ aicb_status ensure_light_state(aicb_scene *s, bool queue = true) {
         s->d_new_light = std::move(new_light);
         s->d_diff = std::move(diff);
         s->d_tile_max = std::move(tile_max);
-        s->device_bytes += s->volume * 10;
+        s->d_changes = std::move(changes);
+        s->device_bytes += s->volume * 10 + change_bytes;
     }
     if (overflow) {
         s->d_scalars = std::move(scalars);
@@ -1017,6 +1126,66 @@ aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     return AICB_OK;
 }
 
+// The size of the set of changed cubes (kernels 1 and 2 of the take), behind everything queued on the context's stream.
+// The chunks' output positions stay in the round's `diff` buffer, which no light call keeps anything in between calls.
+static aicb_status count_changes(const aicb_scene *s, uint32_t *n) {
+    const uint32_t n_words = (uint32_t)((s->volume + 31) / 32);
+    const uint32_t n_chunks = (n_words + CHANGES_CHUNK_WORDS - 1) / CHANGES_CHUNK_WORDS;
+    cudaStream_t st = s->ctx->stream.get();
+    uint32_t *chunk_sums = s->d_diff.get<uint32_t>();   // (n_chunks + 1) * 4 <= volume / 8192 + 8 bytes of its volume + 16
+    k_changes_count<<<n_chunks, 256, 0, st>>>(s->d_changes.get<uint32_t>(), n_words, chunk_sums);
+    k_changes_scan<<<1, 1024, 0, st>>>(chunk_sums, n_chunks);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(n, chunk_sums + n_chunks, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return AICB_OK;
+}
+
+aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed) {
+    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    *n_changed = 0;
+    if (!s->d_changes) return AICB_OK;   // no light call yet
+    CU(cudaSetDevice(s->ctx->device));
+    uint32_t n = 0;
+    TRY(count_changes(s, &n));
+    *n_changed = n;
+    return AICB_OK;
+}
+
+// Both outputs: the set, in increasing index order, and the texels as they are now, then the set is empty.  Neither:
+// the set is emptied without a copy.  The indices and texels are compacted into the round's `list` and `new_light`
+// buffers (idle between light calls) and copied to the caller behind everything queued on the context's stream.
+aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity, size_t *n_taken) {
+    if (!indices != !texels) return aicb_fail(AICB_ERR_INVALID, "give both outputs, or neither to discard the set");
+    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    *n_taken = 0;
+    if (!s->d_changes) return AICB_OK;
+    CU(cudaSetDevice(s->ctx->device));
+    cudaStream_t st = s->ctx->stream.get();
+    uint32_t n = 0;
+    TRY(count_changes(s, &n));
+    if (indices && capacity < n) {
+        *n_taken = n;
+        return aicb_fail(AICB_ERR_INVALID, "capacity is smaller than the set of changed cubes (aicb_light_changes_count)");
+    }
+    if (n) {
+        const uint32_t n_words = (uint32_t)((s->volume + 31) / 32);
+        if (indices) {
+            const uint32_t n_chunks = (n_words + CHANGES_CHUNK_WORDS - 1) / CHANGES_CHUNK_WORDS;
+            k_changes_emit<<<n_chunks, 256, 0, st>>>(s->d_changes.get<uint32_t>(), n_words, s->d_diff.get<uint32_t>(),
+                                                      s->ds.light, s->d_list.get<uint32_t>(), s->d_new_light.get<uint32_t>());
+            CU(cudaMemcpyAsync(indices, s->d_list.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(texels, s->d_new_light.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+        } else {
+            CU(cudaMemsetAsync(s->d_changes.get(), 0, (size_t)n_words * 4, st));
+        }
+        CU(cudaStreamSynchronize(st));
+        CU(cudaGetLastError());
+    }
+    *n_taken = n;
+    return AICB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------------------------
@@ -1079,6 +1248,19 @@ aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texel
     if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return light_download(s, out, n_texels);
+}
+
+aicb_status aicb_light_changes_count(const aicb_scene *s, size_t *n_changed) {
+    if (!s || !n_changed) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_changes_count(s, n_changed);
+}
+
+aicb_status aicb_light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity,
+                                    size_t *n_taken) {
+    if (!s || !n_taken) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_take_changes(s, indices, texels, capacity, n_taken);
 }
 
 aicb_status aicb_light_stats(const aicb_scene *s, uint64_t out[4]) {

@@ -93,6 +93,8 @@ struct LightParams {
                                     // group computes the overflow of its own walks)
     uint32_t *dirty;                // device 0 of a group: one bit per 32-cube segment of the light volume written this
                                     // round, for the push to the other replicas (nullptr on one context)
+    uint32_t *changes;              // replica 0: one bit per cube whose texel a light call wrote since the host last took
+                                    // the set (SpaceChange::CubeLight, space.rs:1079-1083); nullptr on the others
     const float4 *sky_term;         // per preorder node: the sky light its bundle collects at the end of a ray (end_of_ray)
     uint32_t chart_nodes;
     uint32_t *tile_max;             // per LIGHT_TILE cubes: an upper bound of the tile's highest queued priority

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 6 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 7 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -290,6 +290,9 @@ unsafe extern "C" {
                                          epsilon: u8, updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
     pub fn aicb_light_download(s: *mut aicb_scene, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_light_stats(s: *const aicb_scene, out: *mut [u64; 4]) -> aicb_status;
+    pub fn aicb_light_changes_count(s: *const aicb_scene, n_changed: *mut usize) -> aicb_status;
+    pub fn aicb_light_take_changes(s: *mut aicb_scene, indices: *mut u32, texels: *mut [u8; 4], capacity: usize,
+                                   n_taken: *mut usize) -> aicb_status;
 
     pub fn aicb_group_light_fast_evaluate(gs: *mut aicb_group_scene) -> aicb_status;
     pub fn aicb_group_light_compute(gs: *mut aicb_group_scene, cubes: *const [i32; 3], n: usize, out: *mut [u8; 4]) -> aicb_status;
@@ -300,4 +303,7 @@ unsafe extern "C" {
                                                -> aicb_status;
     pub fn aicb_group_light_download(gs: *mut aicb_group_scene, replica: c_int, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_group_light_stats(gs: *const aicb_group_scene, out: *mut [u64; 4]) -> aicb_status;
+    pub fn aicb_group_light_changes_count(gs: *const aicb_group_scene, n_changed: *mut usize) -> aicb_status;
+    pub fn aicb_group_light_take_changes(gs: *mut aicb_group_scene, indices: *mut u32, texels: *mut [u8; 4],
+                                         capacity: usize, n_taken: *mut usize) -> aicb_status;
 }

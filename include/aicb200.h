@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 6
+#define AICB_ABI_VERSION 7
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -472,6 +472,27 @@ aicb_status aicb_light_download(aicb_scene *, uint8_t (*out)[4], size_t n_texels
  * After aicb_light_compute: out[0] cubes computed, out[1] chart nodes visited, out[2] cubes whose walk needed more
  * term slots than the chain walk holds and took the lockstep walk instead, out[3] 0. */
 aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
+/* SpaceChange::CubeLight (space.rs:1079-1083): the set of cubes whose light texel the light calls wrote.  A cube enters
+ * it when
+ *   - aicb_light_edit_and_propagate sets it to a different block that is opaque for light, which stores OPAQUE even
+ *     over OPAQUE (modified_cube_needs_update, space/light/updater.rs:153-161);
+ *   - a relaxation round stores a value with difference_priority > 0 (apply_light_update, updater.rs:313-317);
+ *   - a round writes a guess into an Uninitialized neighbour (updater.rs:335-338);
+ *   - aicb_light_fast_evaluate changes its texel.  The reference announces nothing there (fast_evaluate_light has a
+ *     TODO for EveryBlock); a host following the light needs the cubes all the same.
+ * Nothing else adds to it: not aicb_light_compute, aicb_scene_update_cubes, aicb_scene_upload_light (texels the host
+ * supplied), frames, or a rejected call.  The set accumulates across calls until it is taken; a scene with no light
+ * call yet has none.  LightPhysics::None is AICB_ERR_INVALID.
+ * aicb_light_take_changes with both outputs and capacity >= the set's size writes each cube once, as its Z-major
+ * linear index (the index into aicb_scene_desc::block_ids and light), in increasing order, with its texel as it is now
+ * (aicb_light_download's format), empties the set and sets *n_taken to its size.  With both outputs NULL it empties
+ * the set without copying and sets *n_taken to the number discarded: for a host that downloads the whole volume
+ * instead, which is cheaper once the set exceeds half of it.  capacity < size: AICB_ERR_INVALID, *n_taken = size and
+ * the set is unchanged.  Exactly one output NULL: AICB_ERR_INVALID.  Both hold the context lock; the copy is ordered
+ * behind all work queued on the context. */
+aicb_status aicb_light_changes_count(const aicb_scene *, size_t *n_changed);
+aicb_status aicb_light_take_changes(aicb_scene *, uint32_t *indices_or_null, uint8_t (*texels_or_null)[4],
+                                    size_t capacity, size_t *n_taken);
 
 /* The light calls above on a device group (csrc/group.cu, csrc/light.cu), with their arguments, validation, errors and
  * results: LightStorage::fast_evaluate_light / compute_light / Mutation::set x n + evaluate_light
@@ -497,6 +518,12 @@ aicb_status aicb_group_light_download(aicb_group_scene *, int replica, uint8_t (
 /* aicb_light_stats of the group's last light call: counters summed over the devices; out[3] is device 0's device time
  * of the whole propagation (device 0 waits for every device in every round). */
 aicb_status aicb_group_light_stats(const aicb_group_scene *, uint64_t out[4]);
+/* aicb_light_changes_count / aicb_light_take_changes of the group: the set is device 0's.  Device 0 applies every round
+ * and the push keeps the replicas identical, so the indices and texels are those of every replica.  Each call holds
+ * every context lock of the group. */
+aicb_status aicb_group_light_changes_count(const aicb_group_scene *, size_t *n_changed);
+aicb_status aicb_group_light_take_changes(aicb_group_scene *, uint32_t *indices_or_null, uint8_t (*texels_or_null)[4],
+                                          size_t capacity, size_t *n_taken);
 
 #ifdef __cplusplus
 }
