@@ -352,13 +352,11 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         if ((uint64_t)P.tiles_x * P.tiles_y * 32 > 0xffffffffull) return fail(AICB_ERR_INVALID, "frame too large");
         P.n_tasks = P.tiles_x * P.tiles_y * 32;
         pixels = (uint64_t)P.fb_width * P.local_rows;
-        if (out.pixel_list) {   // one pixel task per listed pixel, 32 consecutive entries per warp
-            P.pixel_list = out.pixel_list;
-            P.n_list = out.n_list;
-            P.tiles_x = (out.n_list + 31) / 32;
+        if (out.target.pixel_list) {   // one pixel task per listed pixel, 32 consecutive entries per warp
+            P.tiles_x = (out.target.n_list + 31) / 32;
             P.tiles_y = 1;
-            P.n_tasks = out.n_list;
-            pixels = out.n_list;
+            P.n_tasks = out.target.n_list;
+            pixels = out.target.n_list;
         }
     } else {
         P.exposure = 1.0f;
@@ -384,36 +382,8 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     P.debug_pixel_cost = opt->debug_pixel_cost;
     P.include_sky = opt->include_sky;
     P.out_full_frame = out.full_frame ? 1 : 0;
-    P.out_srgb8 = out.srgb8;
-    P.out_colorbuf = out.colorbuf;
-    P.out_rgba16f = out.rgba16f;
-    P.out_depth = out.depth;
-    P.out_hit = out.hit;
-    P.out_steps = out.steps;
-    P.out_text = out.text;
-    P.in_accum = out.in_accum;
-    P.out_accum = out.out_accum;
-    if (out.backdrop) { std::memcpy(P.backdrop, out.backdrop, 16); P.has_backdrop = 1; }
-    if (out.no_world) { std::memcpy(P.no_world, out.no_world, 16); P.has_no_world = 1; }
-    const bool tex = out.texture;
-    if (tex) {
-        P.tex_layer = out.tex_layer;
-        P.tex_exposure[0] = out.tex_exposure[0];
-        P.tex_exposure[1] = out.tex_exposure[1];
-        std::memcpy(P.depth_m, out.depth_m, sizeof P.depth_m);
-        P.in_depth = out.in_depth;
-        P.out_task_depth = out.out_task_depth;
-        P.out_tex_depth = out.tex_depth;
-    }
-    const bool term = out.terminal;
-    if (term) {
-        P.tex_layer = out.tex_layer;
-        P.out_term = out.term;
-        P.in_text = out.in_text;
-        P.out_task_text = out.out_task_text;
-        P.text_start = out.text_start;
-    }
-    const int tgt = tex ? TGT_TEX : (term ? TGT_TERM : TGT_FRAME);
+    P.target = out.target;
+    const int tgt = out.kind;
     P.counters = ctx->d_counters.get<unsigned long long>();
     P.task_counter = ctx->d_tile_counter;
     P.refill_threshold = REFILL_THRESHOLD;
@@ -423,7 +393,8 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     sc->pending = true;
     sc->pending_pixels = pixels;
     sc->pending_rays = pixels * (P.antialias ? 4 : 1);
-    sc->pending_out_bytes_per_pixel = out.srgb8 ? 4 : (tex ? 12 : (term ? 24 : (out.rgba16f ? 8 : 16)));
+    sc->pending_out_bytes_per_pixel =
+        P.target.out_srgb8 ? 4 : (tgt == TGT_TEX ? 12 : (tgt == TGT_TERM ? 24 : (P.target.out_rgba16f ? 8 : 16)));
 
     // ---- the kernels of a frame, chunked so the per-frame streams stay bounded ----------------------------------
     P.n_samples = P.antialias ? 4 : 1;
@@ -503,11 +474,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.include_sky = 1;                 // surface.rs:159
             Q.exposure = 1.0f;
             Q.out_full_frame = 0;
-            Q.out_srgb8 = nullptr; Q.out_colorbuf = nullptr; Q.out_rgba16f = nullptr; Q.out_depth = nullptr;
-            Q.out_hit = nullptr; Q.out_steps = nullptr; Q.out_text = nullptr;
-            Q.in_accum = nullptr; Q.out_accum = nullptr; Q.has_backdrop = 0; Q.has_no_world = 0;
-            Q.pixel_list = nullptr; Q.in_depth = nullptr; Q.out_task_depth = nullptr; Q.out_tex_depth = nullptr;
-            Q.out_term = nullptr; Q.in_text = nullptr; Q.out_task_text = nullptr;
+            Q.target = {};   // the secondary rays store nothing of the frame's
             ctx->secondary.bind(Q, chunk_cap, true);
             Q.task_counter = ctx->d_tile_counter + (4 + N_BINS);
             Q.hit_counter = Q.task_counter + 1;
@@ -694,6 +661,7 @@ aicb_status aicb_ctx_create(int device_id, aicb_ctx **out) {
     c->profile_kernels = getenv("AICB_PROFILE_KERNELS") != nullptr;
     for (int i = 0; i < 5; i++) TRY(create_event(c->ev_k[i], cudaEventDefault));
     TRY(create_event(c->ev_delta, cudaEventDisableTiming));
+    TRY(create_event(c->ev_join, cudaEventDisableTiming));
     TRY(c->d_counters.ensure(8 * sizeof(unsigned long long) + 2 * (4 + N_BINS) * sizeof(unsigned int)));
     c->d_tile_counter = (unsigned int *)(c->d_counters.get<unsigned long long>() + 8);
     // PackedLight decode table (light/data.rs:232-243 scalar_out_arithmetic; table :301-354)
@@ -1053,7 +1021,7 @@ aicb_status aicb_render_srgb8(aicb_scene *s, const aicb_camera *cam, const aicb_
     CU(cudaSetDevice(ctx->device));
     TRY(ctx->d_out.ensure(out_len * 4 + 16));
     FramePart part{s, shard};
-    part.out.srgb8 = ctx->d_out.get<uchar4>();
+    part.out.target.out_srgb8 = ctx->d_out.get<uchar4>();
     // A pageable destination (a Rust Vec<[u8; 4]>, a numpy array) cannot take an asynchronous DMA: the frame goes to a
     // pinned staging buffer of the library's and is copied out by the host.  Pinned / registered memory is written directly.
     bool staged = false;
@@ -1085,7 +1053,7 @@ aicb_status aicb_render_rgba16f(aicb_scene *s, const aicb_camera *cam, const aic
     CU(cudaSetDevice(ctx->device));
     TRY(ctx->d_out.ensure(out_len * 8 + 16));
     FramePart part{s, shard};
-    part.out.rgba16f = ctx->d_out.get<uint2>();
+    part.out.target.out_rgba16f = ctx->d_out.get<uint2>();
     part.copy_to = out;
     part.copy_from = ctx->d_out.get();
     part.copy_bytes = out_len * 8;
@@ -1106,20 +1074,21 @@ static aicb_status render_aux(aicb_scene *s, const aicb_camera *cam, const aicb_
     char *base = ctx->d_aux.get<char>();
     FramePart part{s, shard};
     Outputs &o = part.out;
-    o.colorbuf = (float4 *)(base + off_cb);
-    o.depth = (double *)(base + off_depth);
-    o.hit = (aicb_hit *)(base + off_hit);
-    o.steps = (uint32_t *)(base + off_steps);
+    o.target.out_colorbuf = (float4 *)(base + off_cb);
+    o.target.out_depth = (double *)(base + off_depth);
+    o.target.out_hit = (aicb_hit *)(base + off_hit);
+    o.target.out_steps = (uint32_t *)(base + off_steps);
     o.rays = d_rays;
     o.n_rays = n_rays;
     o.aux = true;
     TRY(aicb_trace_pass(&part, 1, cam, opt, info != nullptr));
     if (info) *info = part.info;
     if (n) {
-        if (out_cb) CU(cudaMemcpyAsync(out_cb, o.colorbuf, n * 16, cudaMemcpyDeviceToHost, ctx->stream.get()));
-        if (depth) CU(cudaMemcpyAsync(depth, o.depth, n * 8, cudaMemcpyDeviceToHost, ctx->stream.get()));
-        if (hit) CU(cudaMemcpyAsync(hit, o.hit, n * sizeof(aicb_hit), cudaMemcpyDeviceToHost, ctx->stream.get()));
-        if (steps) CU(cudaMemcpyAsync(steps, o.steps, n * 4, cudaMemcpyDeviceToHost, ctx->stream.get()));
+        const TargetParams &t = o.target;
+        if (out_cb) CU(cudaMemcpyAsync(out_cb, t.out_colorbuf, n * 16, cudaMemcpyDeviceToHost, ctx->stream.get()));
+        if (depth) CU(cudaMemcpyAsync(depth, t.out_depth, n * 8, cudaMemcpyDeviceToHost, ctx->stream.get()));
+        if (hit) CU(cudaMemcpyAsync(hit, t.out_hit, n * sizeof(aicb_hit), cudaMemcpyDeviceToHost, ctx->stream.get()));
+        if (steps) CU(cudaMemcpyAsync(steps, t.out_steps, n * 4, cudaMemcpyDeviceToHost, ctx->stream.get()));
     }
     CU(cudaStreamSynchronize(ctx->stream.get()));
     return AICB_OK;
@@ -1143,7 +1112,7 @@ aicb_status aicb_render_srgb8_device(aicb_scene *s, const aicb_camera *cam, cons
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     Outputs o;
-    o.srgb8 = (uchar4 *)d_out;
+    o.target.out_srgb8 = (uchar4 *)d_out;
     return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream.get());
 }
 
@@ -1159,7 +1128,7 @@ aicb_status aicb_render_srgb8_device_frame(aicb_scene *s, const aicb_camera *cam
     CU(cudaSetDevice(s->ctx->device));
     Outputs o;
     o.full_frame = true;
-    o.srgb8 = (uchar4 *)d_frame;
+    o.target.out_srgb8 = (uchar4 *)d_frame;
     return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream.get());
 }
 
@@ -1313,7 +1282,7 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
     CU(cudaSetDevice(ctx->device));
     TRY(ctx->d_aux.ensure(out_len * 4 + 16));
     FramePart part{s};
-    part.out.text = ctx->d_aux.get<int32_t>();
+    part.out.target.out_text = ctx->d_aux.get<int32_t>();
     st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
     if (st != AICB_OK) return st;
     if (info) *info = part.info;
@@ -1408,9 +1377,9 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
     const int aa = lead->options->antialiasing_always ? 1 : 0;
     // per-task buffers between the passes: one entry per ray of the part's task layout (launch_trace)
     auto n_tasks = [&](const LayerPart &p) -> size_t {
-        return (p.target.pixel_list ? (size_t)p.target.n_list
-                                    : (((size_t)lead->camera->fb_width + TILE_W - 1) / TILE_W) *
-                                          ((shard_rows(lead->camera->fb_height, &p.shard) + TILE_H - 1) / TILE_H) * 32) *
+        return (p.out.target.pixel_list ? (size_t)p.out.target.n_list
+                                        : (((size_t)lead->camera->fb_width + TILE_W - 1) / TILE_W) *
+                                              ((shard_rows(lead->camera->fb_height, &p.shard) + TILE_H - 1) / TILE_H) * 32) *
                (aa ? 4 : 1);
     };
     // Rgba -> ColorBuf (raytracer_components.rs:111-120): premultiplied light, transmittance = 1 - alpha
@@ -1425,6 +1394,16 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         for (int i = 0; i < 3; i++) no_world[i] = no_world_rgba[i] * no_world_rgba[3];
         no_world[3] = 1.0f - no_world_rgba[3];
     }
+    auto add_backdrop = [&](Outputs &o) {
+        if (!have_backdrop) return;
+        std::memcpy(o.target.backdrop, backdrop, 16);
+        o.target.has_backdrop = 1;
+    };
+    auto add_no_world = [&](Outputs &o) {
+        if (!no_world_rgba) return;
+        std::memcpy(o.target.no_world, no_world, 16);
+        o.target.has_no_world = 1;
+    };
     // one pass of the frame on every part: `layer` picks the part's scene, `outputs(part, ctx)` its Outputs; each
     // part's info sums its passes
     std::vector<FramePart> pass_parts(n_parts);
@@ -1442,27 +1421,29 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
             aicb_ctx *ctx = parts[i].world->ctx;
             CU(cudaSetDevice(ctx->device));
             TRY(ctx->d_task_aux.ensure(n_tasks(parts[i]) * sizeof(float4) + 16));
-            if (parts[i].target.texture) {   // the UI pass's DepthBuf, only when there is a UI layer
+            if (parts[i].out.kind == TGT_TEX) {   // the UI pass's DepthBuf, only when there is a UI layer
                 TRY(ctx->d_task_depth.ensure(n_tasks(parts[i]) * sizeof(double) + 16));
             }
-            if (parts[i].target.terminal) {   // the UI pass's CharacterBuf, only when there is a UI layer
+            if (parts[i].out.kind == TGT_TERM) {   // the UI pass's CharacterBuf, only when there is a UI layer
                 TRY(ctx->d_task_text.ensure(n_tasks(parts[i]) * sizeof(int2) + 16));
             }
         }
         aicb_options ui_opt = *ui->options;
         ui_opt.include_sky = 0;   // ui.trace_ray(.., false)
         st = pass(&LayerPart::ui, ui->camera, &ui_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
-            // the pass that writes no pixel keeps the task layout and the texture or terminal mode only
+            // the pass that writes no pixel keeps the task layout and the target kind only
             Outputs o;
-            o.texture = p.target.texture;
-            o.terminal = p.target.terminal;
-            o.pixel_list = p.target.pixel_list;
-            o.n_list = p.target.n_list;
-            o.tex_layer = TEX_UI;
-            if (p.target.texture) o.out_task_depth = ctx->d_task_depth.get<double>();
-            if (p.target.terminal) o.out_task_text = ctx->d_task_text.get<int2>();
-            o.out_accum = ctx->d_task_aux.get<float4>();
-            o.backdrop = have_backdrop ? backdrop : nullptr;
+            o.kind = p.out.kind;
+            o.target.pixel_list = p.out.target.pixel_list;
+            o.target.n_list = p.out.target.n_list;
+            o.target.tex_layer = TEX_UI;
+            if (o.kind == TGT_TEX) o.target.out_task_depth = ctx->d_task_depth.get<double>();
+            if (o.kind == TGT_TERM) {
+                o.target.out_task_text = ctx->d_task_text.get<int2>();
+                o.target.text_start = AICB_TEXT_EMPTY;
+            }
+            o.target.out_accum = ctx->d_task_aux.get<float4>();
+            add_backdrop(o);
             o.force_antialias = aa;
             return o;
         });
@@ -1470,12 +1451,13 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         aicb_options w_opt = *world->options;
         w_opt.include_sky = 1;    // world.trace_ray(.., true)
         st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
-            Outputs o = p.target;
-            o.in_accum = ctx->d_task_aux.get<const float4>();   // a re-issued world pass starts from the same accumulator
-            if (p.target.texture) o.in_depth = ctx->d_task_depth.get<const double>();
-            if (p.target.terminal) o.in_text = ctx->d_task_text.get<const int2>();
-            o.tex_layer = TEX_WORLD;
-            o.no_world = no_world_rgba ? no_world : nullptr;
+            Outputs o = p.out;
+            // a re-issued world pass starts from the same accumulator
+            o.target.in_accum = ctx->d_task_aux.get<const float4>();
+            if (o.kind == TGT_TEX) o.target.in_depth = ctx->d_task_depth.get<const double>();
+            if (o.kind == TGT_TERM) o.target.in_text = ctx->d_task_text.get<const int2>();
+            o.target.tex_layer = TEX_WORLD;
+            add_no_world(o);
             return o;
         });
     } else if (have_world) {
@@ -1493,23 +1475,23 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
             }
         }
         st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
-            Outputs o = p.target;
-            o.tex_layer = TEX_WORLD;
+            Outputs o = p.out;
+            o.target.tex_layer = TEX_WORLD;
             if (have_backdrop) {
-                o.in_accum = ctx->d_task_aux.get<const float4>();
-                o.text_start = AICB_TEXT_BLANK;   // the backdrop's hit names no block
+                o.target.in_accum = ctx->d_task_aux.get<const float4>();
+                if (o.kind == TGT_TERM) o.target.text_start = AICB_TEXT_BLANK;   // the backdrop's hit names no block
             }
-            o.no_world = no_world_rgba ? no_world : nullptr;
+            add_no_world(o);
             return o;
         });
     } else {
         aicb_options ui_opt = *ui->options;
         ui_opt.include_sky = 0;
         st = pass(&LayerPart::ui, ui->camera, &ui_opt, [&](const LayerPart &p, aicb_ctx *) {
-            Outputs o = p.target;
-            o.tex_layer = TEX_UI;
-            o.backdrop = have_backdrop ? backdrop : nullptr;
-            o.no_world = no_world_rgba ? no_world : nullptr;
+            Outputs o = p.out;
+            o.target.tex_layer = TEX_UI;
+            add_backdrop(o);
+            add_no_world(o);
             return o;
         });
     }
@@ -1517,14 +1499,6 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
     std::memset(total, 0, sizeof *total);
     for (const FramePart &p : pass_parts) aicb_merge_info(total, &p.info, false);
     return AICB_OK;
-}
-
-// The single-context layered calls draw with one part: the layers' own scenes, every row.
-static LayerPart single_part(const aicb_layer *world, const aicb_layer *ui) {
-    LayerPart p;
-    p.world = world ? world->scene : nullptr;
-    p.ui = ui ? ui->scene : nullptr;
-    return p;
 }
 
 aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba,
@@ -1547,14 +1521,20 @@ aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer 
     return AICB_OK;
 }
 
-void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *target) {
-    target->full_frame = true;
-    target->texture = true;
+void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out) {
+    out->full_frame = true;
+    out->kind = TGT_TEX;
     // the exposure of each layer's camera (:603-605); a missing layer's is never used
-    target->tex_exposure[0] = (world && world->scene) ? world->camera->exposure : 1.0f;
-    target->tex_exposure[1] = (ui && ui->scene) ? ui->camera->exposure : 1.0f;
+    out->target.tex_exposure[0] = (world && world->scene) ? world->camera->exposure : 1.0f;
+    out->target.tex_exposure[1] = (ui && ui->scene) ? ui->camera->exposure : 1.0f;
     const int cols[8] = {2, 6, 10, 14, 3, 7, 11, 15};   // m13 m23 m33 m43, m14 m24 m34 m44 (row-major m11..m44)
-    for (int k = 0; k < 8; k++) target->depth_m[k] = depth_transform[cols[k]];
+    for (int k = 0; k < 8; k++) out->target.depth_m[k] = depth_transform[cols[k]];
+}
+
+// The layered calls on one context: its scenes of the layers (group.cu draws them).
+static LayeredCall one_context(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
+                               const float *no_world_rgba) {
+    return {world, ui, world ? &world->scene : nullptr, ui ? &ui->scene : nullptr, 1, backdrop_rgba, no_world_rgba};
 }
 
 // == RtScene::trace_ray_through_layers for every pixel + the encoder of draw_rgba (renderer.rs:454-478, 287-291).
@@ -1562,22 +1542,7 @@ void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const do
 aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *ui, const float backdrop_rgba[4],
                                      const float no_world_rgba[4], uint8_t (*out)[4], size_t out_len,
                                      aicb_render_info *info) {
-    const aicb_layer *lead = nullptr;
-    aicb_status st = aicb_check_layers(world, ui, no_world_rgba, out_len, &lead);
-    if (st != AICB_OK) return st;
-    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
-    aicb_ctx *ctx = lead->scene->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    TRY(ctx->d_out.ensure(out_len * 4 + 16));
-    LayerPart part = single_part(world, ui);
-    part.target.srgb8 = ctx->d_out.get<uchar4>();
-    aicb_render_info total;
-    st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
-    if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpy(out, ctx->d_out.get(), out_len * 4, cudaMemcpyDeviceToHost));
-    if (info) *info = total;
-    return AICB_OK;
+    return layers_srgb8(one_context(world, ui, backdrop_rgba, no_world_rgba), out, out_len, info);
 }
 
 // == the desktop terminal's frame (terminal.rs:114-142): RtScene::trace_ray_through_layers into ColorCharacterBuf
@@ -1585,23 +1550,7 @@ aicb_status aicb_render_layers_srgb8(const aicb_layer *world, const aicb_layer *
 aicb_status aicb_render_layers_terminal(const aicb_layer *world, const aicb_layer *ui, const float backdrop_rgba[4],
                                         const float no_world_rgba[4], aicb_terminal_pixel *out, size_t out_len,
                                         aicb_render_info *info) {
-    const aicb_layer *lead = nullptr;
-    aicb_status st = aicb_check_layers(world, ui, no_world_rgba, out_len, &lead);
-    if (st != AICB_OK) return st;
-    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
-    aicb_ctx *ctx = lead->scene->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    TRY(ctx->d_out.ensure(out_len * sizeof(aicb_terminal_pixel) + 16));
-    LayerPart part = single_part(world, ui);
-    part.target.terminal = true;
-    part.target.term = ctx->d_out.get<aicb_terminal_pixel>();
-    aicb_render_info total;
-    st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
-    if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpy(out, ctx->d_out.get(), out_len * sizeof(aicb_terminal_pixel), cudaMemcpyDeviceToHost));
-    if (info) *info = total;
-    return AICB_OK;
+    return layers_terminal(one_context(world, ui, backdrop_rgba, no_world_rgba), out, out_len, info);
 }
 
 // == RaytraceToTexture::do_some_tracing's trace_one over a batch of pixels (raytrace_to_texture.rs:591-683): the
@@ -1611,37 +1560,8 @@ aicb_status aicb_render_layers_texture(const aicb_layer *world, const aicb_layer
                                        const float no_world_rgba[4], const double depth_transform[16],
                                        const uint32_t *pixels, size_t n_pixels, uint16_t (*out_rgba16f)[4],
                                        float *out_depth, aicb_render_info *info) {
-    const aicb_layer *lead = nullptr;
-    aicb_status st = aicb_check_layers_texture(world, ui, no_world_rgba, depth_transform, pixels, n_pixels, out_rgba16f,
-                                               out_depth, &lead);
-    if (st != AICB_OK) return st;
-    if (info) std::memset(info, 0, sizeof *info);
-    if (n_pixels == 0) return AICB_OK;
-    aicb_ctx *ctx = lead->scene->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    // d_out: colour texels (8 B), depth texels (4 B), then the pixel list (4 B), each 256-byte aligned
-    const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
-    const size_t off_list = off_depth + ((n_pixels * 4 + 255) & ~(size_t)255);
-    TRY(ctx->d_out.ensure(off_list + (pixels ? n_pixels * 4 : 0) + 16));
-    char *base = ctx->d_out.get<char>();
-    LayerPart part = single_part(world, ui);
-    Outputs &target = part.target;
-    aicb_texture_target(world, ui, depth_transform, &target);
-    target.rgba16f = (uint2 *)base;
-    target.tex_depth = (float *)(base + off_depth);
-    if (pixels) {
-        CU(cudaMemcpy(base + off_list, pixels, n_pixels * 4, cudaMemcpyHostToDevice));
-        target.pixel_list = (const uint32_t *)(base + off_list);
-        target.n_list = (uint32_t)n_pixels;
-    }
-    aicb_render_info total;
-    st = aicb_trace_layers(world, ui, backdrop_rgba, no_world_rgba, &part, 1, &total);
-    if (st != AICB_OK) return st;
-    CU(cudaMemcpy(out_rgba16f, base, n_pixels * 8, cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(out_depth, base + off_depth, n_pixels * 4, cudaMemcpyDeviceToHost));
-    if (info) *info = total;
-    return AICB_OK;
+    return layers_texture(one_context(world, ui, backdrop_rgba, no_world_rgba), depth_transform, pixels, n_pixels,
+                          out_rgba16f, out_depth, info);
 }
 
 // == render_orthographic (raytracer/ortho.rs:30-84) with MultiOrthoCamera (:143-199) / OrthoCamera (:209-297): five
@@ -1734,7 +1654,7 @@ aicb_status aicb_render_orthographic(aicb_scene *s, uint32_t resolution, uint8_t
         opt.view_distance = 200.0;
         opt.include_sky = 1;
         FramePart part{s};
-        part.out.srgb8 = ctx->d_out.get<uchar4>();
+        part.out.target.out_srgb8 = ctx->d_out.get<uchar4>();
         part.out.rays = d_rays.get<double>();
         part.out.n_rays = n;
         TRY(aicb_trace_pass(&part, 1, nullptr, &opt, info != nullptr));

@@ -6,9 +6,10 @@
 // waits for the others' completion events and copies the frame to the caller: compute and delivery are one kernel
 // chain per device, there is no collective and no host thread per GPU.
 // Replaces the Rayon rows x pixels dispatch of trace_scene_to_image_impl (renderer.rs:516-556) across devices.
-// Layered frames, terminal frames and texture targets (aicb_group_render_layers_*) cut the work the same way, or a pixel list into
-// ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu).  Every call issues a pass on every
-// device before it waits for any, and re-issues it on a device whose hit stream overflowed (aicb_trace_pass).
+// Layered frames, terminal frames and texture targets (layers_srgb8 / _terminal / _texture, which serve
+// aicb_render_layers_* on one context and aicb_group_render_layers_* on a group) cut the work the same way, or a pixel
+// list into ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu).  Every call issues a pass on
+// every device before it waits for any, and re-issues it on a device whose hit stream overflowed (aicb_trace_pass).
 // Light propagation (aicb_group_light_*) hands the replicas to light.cu, which runs one context's rounds over them.
 #include <algorithm>
 #include <cstring>
@@ -17,22 +18,11 @@
 
 #include "internal.h"
 
-// Destroyed with device 0 current (aicb_group_destroy): its own buffers first, then each device's event and context.
 struct aicb_group {
     std::vector<aicb_ctx *> ctx;
-    std::vector<Event> done;   // per device: its strips of the current frame are in device 0's frame
-    DeviceBuffer d_frame;      // on device 0
-    DeviceBuffer d_tex;        // on device 0: the texels of aicb_group_render_layers_texture, or the pixels of
-                               // aicb_group_render_layers_terminal
     bool light_peers = false;  // device 0 reaches every device too, and the devices have native peer atomics
     ~aicb_group() {
-        d_frame.reset();
-        d_tex.reset();
-        for (size_t i = 0; i < ctx.size(); i++) {
-            cudaSetDevice(ctx[i]->device);
-            done[i].reset();
-            aicb_ctx_destroy(ctx[i]);
-        }
+        for (aicb_ctx *c : ctx) aicb_ctx_destroy(c);
     }
 };
 
@@ -43,58 +33,181 @@ struct aicb_group_scene {
 
 static const uint32_t GROUP_STRIP_ROWS = 16;
 
+aicb_status fan_out(aicb_ctx *const *ctx, size_t n) {
+    CU(cudaSetDevice(ctx[0]->device));
+    CU(cudaEventRecord(ctx[0]->ev_join.get(), ctx[0]->stream.get()));
+    for (size_t i = 1; i < n; i++) {
+        CU(cudaSetDevice(ctx[i]->device));
+        CU(cudaStreamWaitEvent(ctx[i]->stream.get(), ctx[0]->ev_join.get(), 0));
+    }
+    return AICB_OK;
+}
+
+aicb_status fan_in(aicb_ctx *const *ctx, size_t n) {
+    for (size_t i = 1; i < n; i++) {
+        CU(cudaSetDevice(ctx[i]->device));
+        CU(cudaEventRecord(ctx[i]->ev_join.get(), ctx[i]->stream.get()));
+    }
+    CU(cudaSetDevice(ctx[0]->device));
+    for (size_t i = 1; i < n; i++) CU(cudaStreamWaitEvent(ctx[0]->stream.get(), ctx[i]->ev_join.get(), 0));
+    return AICB_OK;
+}
+
 // ---- layered frames and texture targets -------------------------------------------------------------------------------
-// The layers of a group call as device i sees them: its replicas, the same cameras and options.
-static aicb_layer replica(const aicb_group_layer *l, size_t i) {
+// Every context's part of a layered call.  A whole frame or texture: interleaved 16-row strips, outputs at their
+// framebuffer positions in device 0's buffers (`target`).  A pixel list: contiguous ranges of whole warps (a warp
+// takes 32 consecutive list entries), as even as whole warps allow; context i traces its range from its own copy of
+// it (its d_aux) and stores at the range's offset, so list order is kept.  One context: one part, every row or the
+// whole list.
+static aicb_status layer_parts(const LayeredCall &c, aicb_ctx *const *ctx, const Outputs &target,
+                               const uint32_t *pixels, size_t n_pixels, std::vector<LayerPart> *parts) {
+    auto part = [&](size_t i) {
+        LayerPart p;
+        p.world = c.world_scenes ? c.world_scenes[i] : nullptr;
+        p.ui = c.ui_scenes ? c.ui_scenes[i] : nullptr;
+        p.out = target;
+        return p;
+    };
+    if (!pixels) {
+        for (size_t i = 0; i < c.n; i++) {
+            parts->push_back(part(i));
+            parts->back().shard = {GROUP_STRIP_ROWS, (uint32_t)i, (uint32_t)c.n};
+        }
+        return AICB_OK;
+    }
+    const size_t warps = (n_pixels + 31) / 32;
+    const size_t used = std::min(c.n, warps);
+    size_t begin = 0;
+    for (size_t i = 0; i < used; i++) {
+        const size_t count = std::min(32 * (warps / used + (i < warps % used ? 1 : 0)), n_pixels - begin);
+        CU(cudaSetDevice(ctx[i]->device));
+        TRY(ctx[i]->d_aux.ensure(count * 4 + 16));
+        CU(cudaMemcpy(ctx[i]->d_aux.get(), pixels + begin, count * 4, cudaMemcpyHostToDevice));
+        LayerPart p = part(i);
+        p.out.target.pixel_list = ctx[i]->d_aux.get<const uint32_t>();
+        p.out.target.n_list = (uint32_t)count;
+        p.out.target.out_rgba16f = target.target.out_rgba16f + begin;
+        p.out.target.out_tex_depth = target.target.out_tex_depth + begin;
+        parts->push_back(p);
+        begin += count;
+    }
+    return AICB_OK;
+}
+
+// A copy of device 0's outputs to the caller.
+struct Delivery {
+    void *to;
+    const void *from;
+    size_t bytes;
+};
+
+// Device 0's stream waits for the streams of the contexts that drew a part, then copies the outputs to the caller.
+static aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, std::initializer_list<Delivery> copies) {
+    TRY(fan_in(ctx, n_parts));
+    cudaStream_t stream = ctx[0]->stream.get();
+    for (const Delivery &d : copies)
+        if (d.bytes) CU(cudaMemcpyAsync(d.to, d.from, d.bytes, cudaMemcpyDeviceToHost, stream));
+    CU(cudaStreamSynchronize(stream));
+    return AICB_OK;
+}
+
+// The contexts of a validated layered call: those of its lead layer's replicas.
+static std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *lead) {
+    aicb_scene *const *scenes = lead == c.world ? c.world_scenes : c.ui_scenes;
+    std::vector<aicb_ctx *> ctx;
+    for (size_t i = 0; i < c.n; i++) ctx.push_back(scenes[i]->ctx);
+    return ctx;
+}
+
+// The rest of a layered call once device 0's outputs are in `target`: the parts, the layers, the delivery.
+static aicb_status draw_layers(const LayeredCall &c, const std::vector<aicb_ctx *> &ctx, const Outputs &target,
+                               const uint32_t *pixels, size_t n_pixels, std::initializer_list<Delivery> copies,
+                               aicb_render_info *info) {
+    std::vector<LayerPart> parts;
+    TRY(layer_parts(c, ctx.data(), target, pixels, n_pixels, &parts));
+    aicb_render_info total;
+    TRY(aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), &total));
+    TRY(deliver(ctx.data(), parts.size(), copies));
+    if (info) *info = total;
+    return AICB_OK;
+}
+
+aicb_status layers_srgb8(const LayeredCall &c, uint8_t (*out)[4], size_t out_len, aicb_render_info *info) {
+    const aicb_layer *lead = nullptr;
+    TRY(aicb_check_layers(c.world, c.ui, c.no_world_rgba, out_len, &lead));
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
+    ContextLocks lock(ctx);
+    CU(cudaSetDevice(ctx[0]->device));
+    TRY(ctx[0]->d_out.ensure(out_len * 4 + 16));
+    Outputs target;
+    target.full_frame = true;
+    target.target.out_srgb8 = ctx[0]->d_out.get<uchar4>();
+    return draw_layers(c, ctx, target, nullptr, 0, {{out, ctx[0]->d_out.get(), out_len * 4}}, info);
+}
+
+aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info) {
+    const aicb_layer *lead = nullptr;
+    TRY(aicb_check_layers(c.world, c.ui, c.no_world_rgba, out_len, &lead));
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
+    ContextLocks lock(ctx);
+    CU(cudaSetDevice(ctx[0]->device));
+    const size_t bytes = out_len * sizeof(aicb_terminal_pixel);
+    TRY(ctx[0]->d_out.ensure(bytes + 16));
+    Outputs target;
+    target.full_frame = true;
+    target.kind = aicb::TGT_TERM;
+    target.target.out_term = ctx[0]->d_out.get<aicb_terminal_pixel>();
+    target.target.text_start = AICB_TEXT_EMPTY;
+    return draw_layers(c, ctx, target, nullptr, 0, {{out, ctx[0]->d_out.get(), bytes}}, info);
+}
+
+aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
+                           uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info) {
+    const aicb_layer *lead = nullptr;
+    TRY(aicb_check_layers_texture(c.world, c.ui, c.no_world_rgba, depth_transform, pixels, n_pixels, out_rgba16f,
+                                  out_depth, &lead));
+    if (info) std::memset(info, 0, sizeof *info);
+    if (n_pixels == 0) return AICB_OK;
+    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
+    ContextLocks lock(ctx);
+    CU(cudaSetDevice(ctx[0]->device));
+    // device 0's d_out: colour texels (8 B), then depth texels (4 B), 256-byte aligned
+    const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
+    TRY(ctx[0]->d_out.ensure(off_depth + n_pixels * 4 + 16));
+    char *base = ctx[0]->d_out.get<char>();
+    Outputs target;
+    aicb_texture_target(c.world, c.ui, depth_transform, &target);
+    target.target.out_rgba16f = (uint2 *)base;
+    target.target.out_tex_depth = (float *)(base + off_depth);
+    return draw_layers(c, ctx, target, pixels, n_pixels,
+                       {{out_rgba16f, base, n_pixels * 8}, {out_depth, base + off_depth, n_pixels * 4}}, info);
+}
+
+// The layers of a group call as device 0 sees them (its replicas, the cameras and options), and every replica of each.
+static aicb_layer on_device0(const aicb_group_layer *l) {
     aicb_layer r;
-    r.scene = (l && l->scene) ? l->scene->scene[i] : nullptr;
+    r.scene = (l && l->scene) ? l->scene->scene[0] : nullptr;
     r.camera = l ? l->camera : nullptr;
     r.options = l ? l->options : nullptr;
     return r;
 }
 
-// The group of the layers' scenes (nullptr if there is no scene: validation then rejects the call).
-static aicb_status group_of(const aicb_group_layer *world, const aicb_group_layer *ui, aicb_group **g) {
+static aicb_status group_call(const aicb_group_layer *world, const aicb_group_layer *ui, const float *backdrop_rgba,
+                              const float *no_world_rgba, aicb_layer views[2], LayeredCall *c) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
     if (have_world && have_ui && world->scene->group != ui->scene->group)
         return aicb_fail(AICB_ERR_INVALID, "the layers must be scenes of the same group");
-    *g = have_world ? world->scene->group : (have_ui ? ui->scene->group : nullptr);
+    // (no scene at all: validation rejects the call)
+    const aicb_group *g = have_world ? world->scene->group : (have_ui ? ui->scene->group : nullptr);
+    views[0] = on_device0(world);
+    views[1] = on_device0(ui);
+    *c = {world ? &views[0] : nullptr, ui ? &views[1] : nullptr,
+          have_world ? world->scene->scene.data() : nullptr, have_ui ? ui->scene->scene.data() : nullptr,
+          g ? g->ctx.size() : 0, backdrop_rgba, no_world_rgba};
     return AICB_OK;
 }
-
-// Every device's part of a whole frame or texture: interleaved 16-row strips, outputs at their framebuffer positions in
-// device 0's buffers (`target`).
-static std::vector<LayerPart> strip_parts(aicb_group *g, const aicb_group_layer *world, const aicb_group_layer *ui,
-                                          const Outputs &target) {
-    const uint32_t n = (uint32_t)g->ctx.size();
-    std::vector<LayerPart> parts(n);
-    for (uint32_t i = 0; i < n; i++) {
-        parts[i].world = replica(world, i).scene;
-        parts[i].ui = replica(ui, i).scene;
-        parts[i].shard = {GROUP_STRIP_ROWS, i, n};
-        parts[i].target = target;
-    }
-    return parts;
-}
-
-// Delivery: device 0's stream waits for the completion events of the devices that drew a part.
-static aicb_status join(aicb_group *g, size_t n_parts) {
-    for (size_t i = 1; i < n_parts; i++) {
-        CU(cudaSetDevice(g->ctx[i]->device));
-        CU(cudaEventRecord(g->done[i].get(), g->ctx[i]->stream.get()));
-    }
-    CU(cudaSetDevice(g->ctx[0]->device));
-    for (size_t i = 1; i < n_parts; i++) CU(cudaStreamWaitEvent(g->ctx[0]->stream.get(), g->done[i].get(), 0));
-    return AICB_OK;
-}
-
-// The contexts' locks, for the whole of a frame (its passes run on every context).
-struct GroupLock {
-    std::vector<std::unique_lock<std::mutex>> locks;
-    explicit GroupLock(aicb_group *g) {
-        for (aicb_ctx *c : g->ctx) locks.emplace_back(c->mu);
-    }
-};
 
 // ---- light propagation ------------------------------------------------------------------------------------------------
 // Light needs more than frames: device 0 stores into every device's light volume (the push of a round), and every
@@ -122,17 +235,13 @@ static aicb_status ensure_light_peers(aicb_group *g) {
 // The group's replicas for light.cu, after the group's locks are held and its peers are ready.
 static aicb_status light_replicas(aicb_group_scene *gs, LightReplicas *r) {
     TRY(ensure_light_peers(gs->group));
-    *r = {gs->scene.data(), gs->scene.size()};
+    *r = {gs->scene.data(), gs->group->ctx.data(), gs->scene.size()};
     return AICB_OK;
 }
 
 extern "C" {
 
-void aicb_group_destroy(aicb_group *g) {
-    if (!g) return;
-    if (!g->ctx.empty()) cudaSetDevice(g->ctx[0]->device);
-    delete g;
-}
+void aicb_group_destroy(aicb_group *g) { delete g; }
 
 aicb_status aicb_group_create(const int *device_ids, int n_devices, aicb_group **out) {
     if (!device_ids || n_devices < 1 || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument or no devices");
@@ -146,12 +255,6 @@ aicb_status aicb_group_create(const int *device_ids, int n_devices, aicb_group *
             return st;
         }
         g->ctx.push_back(c);
-        g->done.emplace_back();
-        st = create_event(g->done[i], cudaEventDisableTiming);
-        if (st != AICB_OK) {
-            aicb_group_destroy(g);
-            return st;
-        }
     }
     // every device stores into device 0's frame
     const int root = g->ctx[0]->device;
@@ -221,24 +324,22 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
     if (pixels && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
     aicb_status st = aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len);
     if (st != AICB_OK) return st;
-    GroupLock lock(g);
+    ContextLocks lock(g->ctx);
     aicb_ctx *root = g->ctx[0];
     CU(cudaSetDevice(root->device));
-    TRY(g->d_frame.ensure(pixels * 4 + 16));
+    TRY(root->d_out.ensure(pixels * 4 + 16));
     Outputs target;
     target.full_frame = true;
-    target.srgb8 = g->d_frame.get<uchar4>();
+    target.target.out_srgb8 = root->d_out.get<uchar4>();
     // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
-    const aicb_group_layer world = {gs, cam, opt};
-    const std::vector<LayerPart> strips = strip_parts(g, &world, nullptr, target);
+    const aicb_layer w0 = {gs->scene[0], cam, opt};
+    const LayeredCall world = {&w0, nullptr, gs->scene.data(), nullptr, g->ctx.size(), nullptr, nullptr};
+    std::vector<LayerPart> strips;
+    TRY(layer_parts(world, g->ctx.data(), target, nullptr, 0, &strips));
     std::vector<FramePart> parts;
-    for (const LayerPart &p : strips) parts.push_back({p.world, &p.shard, p.target});
-    st = aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr);
-    if (st != AICB_OK) return st;
-    st = join(g, parts.size());
-    if (st != AICB_OK) return st;
-    if (pixels) CU(cudaMemcpyAsync(out, g->d_frame.get(), pixels * 4, cudaMemcpyDeviceToHost, root->stream.get()));
-    CU(cudaStreamSynchronize(root->stream.get()));
+    for (const LayerPart &p : strips) parts.push_back({p.world, &p.shard, p.out});
+    TRY(aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr));
+    TRY(deliver(g->ctx.data(), parts.size(), {{out, root->d_out.get(), pixels * 4}}));
     if (info) {
         std::memset(info, 0, sizeof *info);
         for (const FramePart &p : parts) aicb_merge_info(info, &p.info, false);
@@ -273,132 +374,35 @@ aicb_status aicb_group_scene_upload_light(aicb_group_scene *gs, const uint8_t (*
 aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world, const aicb_group_layer *ui,
                                            const float backdrop_rgba[4], const float no_world_rgba[4], uint8_t (*out)[4],
                                            size_t out_len, aicb_render_info *info) {
-    aicb_group *g = nullptr;
-    aicb_status st = group_of(world, ui, &g);
-    if (st != AICB_OK) return st;
-    aicb_layer w0 = replica(world, 0), u0 = replica(ui, 0);
-    const aicb_layer *w = world ? &w0 : nullptr, *u = ui ? &u0 : nullptr, *lead = nullptr;
-    st = aicb_check_layers(w, u, no_world_rgba, out_len, &lead);
-    if (st != AICB_OK) return st;
-    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
-    GroupLock lock(g);
-    aicb_ctx *root = g->ctx[0];
-    CU(cudaSetDevice(root->device));
-    TRY(g->d_frame.ensure(out_len * 4 + 16));
-    Outputs target;
-    target.full_frame = true;
-    target.srgb8 = g->d_frame.get<uchar4>();
-    std::vector<LayerPart> parts = strip_parts(g, world, ui, target);
-    aicb_render_info total;
-    st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
-    if (st != AICB_OK) return st;
-    st = join(g, parts.size());
-    if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpyAsync(out, g->d_frame.get(), out_len * 4, cudaMemcpyDeviceToHost, root->stream.get()));
-    CU(cudaStreamSynchronize(root->stream.get()));
-    if (info) *info = total;
-    return AICB_OK;
+    aicb_layer views[2];
+    LayeredCall c;
+    TRY(group_call(world, ui, backdrop_rgba, no_world_rgba, views, &c));
+    return layers_srgb8(c, out, out_len, info);
 }
 
 aicb_status aicb_group_render_layers_terminal(const aicb_group_layer *world, const aicb_group_layer *ui,
                                               const float backdrop_rgba[4], const float no_world_rgba[4],
                                               aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info) {
-    aicb_group *g = nullptr;
-    aicb_status st = group_of(world, ui, &g);
-    if (st != AICB_OK) return st;
-    aicb_layer w0 = replica(world, 0), u0 = replica(ui, 0);
-    const aicb_layer *w = world ? &w0 : nullptr, *u = ui ? &u0 : nullptr, *lead = nullptr;
-    st = aicb_check_layers(w, u, no_world_rgba, out_len, &lead);
-    if (st != AICB_OK) return st;
-    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
-    GroupLock lock(g);
-    aicb_ctx *root = g->ctx[0];
-    CU(cudaSetDevice(root->device));
-    const size_t bytes = out_len * sizeof(aicb_terminal_pixel);
-    TRY(g->d_tex.ensure(bytes + 16));
-    Outputs target;
-    target.full_frame = true;
-    target.terminal = true;
-    target.term = g->d_tex.get<aicb_terminal_pixel>();
-    std::vector<LayerPart> parts = strip_parts(g, world, ui, target);
-    aicb_render_info total;
-    st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
-    if (st != AICB_OK) return st;
-    st = join(g, parts.size());
-    if (st != AICB_OK) return st;
-    if (out_len) CU(cudaMemcpyAsync(out, g->d_tex.get(), bytes, cudaMemcpyDeviceToHost, root->stream.get()));
-    CU(cudaStreamSynchronize(root->stream.get()));
-    if (info) *info = total;
-    return AICB_OK;
+    aicb_layer views[2];
+    LayeredCall c;
+    TRY(group_call(world, ui, backdrop_rgba, no_world_rgba, views, &c));
+    return layers_terminal(c, out, out_len, info);
 }
 
 aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world, const aicb_group_layer *ui,
                                              const float backdrop_rgba[4], const float no_world_rgba[4],
                                              const double depth_transform[16], const uint32_t *pixels, size_t n_pixels,
                                              uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info) {
-    aicb_group *g = nullptr;
-    aicb_status st = group_of(world, ui, &g);
-    if (st != AICB_OK) return st;
-    aicb_layer w0 = replica(world, 0), u0 = replica(ui, 0);
-    const aicb_layer *w = world ? &w0 : nullptr, *u = ui ? &u0 : nullptr, *lead = nullptr;
-    st = aicb_check_layers_texture(w, u, no_world_rgba, depth_transform, pixels, n_pixels, out_rgba16f, out_depth, &lead);
-    if (st != AICB_OK) return st;
-    if (info) std::memset(info, 0, sizeof *info);
-    if (n_pixels == 0) return AICB_OK;
-    GroupLock lock(g);
-    aicb_ctx *root = g->ctx[0];
-    CU(cudaSetDevice(root->device));
-    // device 0: colour texels (8 B), then depth texels (4 B), 256-byte aligned
-    const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
-    TRY(g->d_tex.ensure(off_depth + n_pixels * 4 + 16));
-    char *base = g->d_tex.get<char>();
-    Outputs target;
-    aicb_texture_target(w, u, depth_transform, &target);
-    target.rgba16f = (uint2 *)base;
-    target.tex_depth = (float *)(base + off_depth);
-    std::vector<LayerPart> parts;
-    if (!pixels) {
-        parts = strip_parts(g, world, ui, target);
-    } else {
-        // Contiguous ranges of whole warps (a warp takes 32 consecutive list entries), as even as whole warps allow.
-        // Device i traces its range from its own copy of it and stores at the range's offset: list order is kept.
-        const size_t warps = (n_pixels + 31) / 32;
-        const size_t used = std::min(g->ctx.size(), warps);
-        size_t begin = 0;
-        for (size_t i = 0; i < used; i++) {
-            const size_t count = std::min(32 * (warps / used + (i < warps % used ? 1 : 0)), n_pixels - begin);
-            aicb_ctx *c = g->ctx[i];
-            CU(cudaSetDevice(c->device));
-            TRY(c->d_out.ensure(count * 4 + 16));
-            CU(cudaMemcpy(c->d_out.get(), pixels + begin, count * 4, cudaMemcpyHostToDevice));
-            LayerPart p;
-            p.world = replica(world, i).scene;
-            p.ui = replica(ui, i).scene;
-            p.target = target;
-            p.target.pixel_list = c->d_out.get<const uint32_t>();
-            p.target.n_list = (uint32_t)count;
-            p.target.rgba16f = target.rgba16f + begin;
-            p.target.tex_depth = target.tex_depth + begin;
-            parts.push_back(p);
-            begin += count;
-        }
-    }
-    aicb_render_info total;
-    st = aicb_trace_layers(w, u, backdrop_rgba, no_world_rgba, parts.data(), parts.size(), &total);
-    if (st != AICB_OK) return st;
-    st = join(g, parts.size());
-    if (st != AICB_OK) return st;
-    CU(cudaMemcpyAsync(out_rgba16f, base, n_pixels * 8, cudaMemcpyDeviceToHost, root->stream.get()));
-    CU(cudaMemcpyAsync(out_depth, base + off_depth, n_pixels * 4, cudaMemcpyDeviceToHost, root->stream.get()));
-    CU(cudaStreamSynchronize(root->stream.get()));
-    if (info) *info = total;
-    return AICB_OK;
+    aicb_layer views[2];
+    LayeredCall c;
+    TRY(group_call(world, ui, backdrop_rgba, no_world_rgba, views, &c));
+    return layers_texture(c, depth_transform, pixels, n_pixels, out_rgba16f, out_depth, info);
 }
 
 // ---- light propagation: the single-context calls' arguments, validation and results (light.cu) --------------------
 aicb_status aicb_group_light_fast_evaluate(aicb_group_scene *gs) {
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    GroupLock lock(gs->group);
+    ContextLocks lock(gs->group->ctx);
     LightReplicas r;
     TRY(light_replicas(gs, &r));
     return light_fast_evaluate(r);
@@ -407,7 +411,7 @@ aicb_status aicb_group_light_fast_evaluate(aicb_group_scene *gs) {
 aicb_status aicb_group_light_compute(aicb_group_scene *gs, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
     if (!gs || (n && (!cubes || !out))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n > gs->scene[0]->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
-    GroupLock lock(gs->group);
+    ContextLocks lock(gs->group->ctx);
     LightReplicas r;
     TRY(light_replicas(gs, &r));
     return light_compute(r, cubes, n, out);
@@ -416,7 +420,7 @@ aicb_status aicb_group_light_compute(aicb_group_scene *gs, const int32_t (*cubes
 aicb_status aicb_group_light_evaluate(aicb_group_scene *gs, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                       uint64_t *node_visits) {
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    GroupLock lock(gs->group);
+    ContextLocks lock(gs->group->ctx);
     LightReplicas r;
     TRY(light_replicas(gs, &r));
     return light_evaluate(r, epsilon, updates_done, max_diff, node_visits);
@@ -426,7 +430,7 @@ aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int3
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff) {
     if (!gs || (n_edits && (!cubes || !new_ids))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    GroupLock lock(gs->group);
+    ContextLocks lock(gs->group->ctx);
     LightReplicas r;
     TRY(light_replicas(gs, &r));
     return light_edit_and_propagate(r, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
@@ -435,7 +439,7 @@ aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int3
 aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t (*out)[4], size_t n_texels) {
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (replica < 0 || (size_t)replica >= gs->scene.size()) return aicb_fail(AICB_ERR_INVALID, "no such replica");
-    GroupLock lock(gs->group);
+    ContextLocks lock(gs->group->ctx);
     return light_download(gs->scene[replica], out, n_texels);
 }
 
@@ -443,14 +447,14 @@ aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t
 // indices and texels are every replica's.
 aicb_status aicb_group_light_changes_count(const aicb_group_scene *gs, size_t *n_changed) {
     if (!gs || !n_changed) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    GroupLock lock(gs->group);
+    ContextLocks lock(gs->group->ctx);
     return light_changes_count(gs->scene[0], n_changed);
 }
 
 aicb_status aicb_group_light_take_changes(aicb_group_scene *gs, uint32_t *indices, uint8_t (*texels)[4], size_t capacity,
                                           size_t *n_taken) {
     if (!gs || !n_taken) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    GroupLock lock(gs->group);
+    ContextLocks lock(gs->group->ctx);
     return light_take_changes(gs->scene[0], indices, texels, capacity, n_taken);
 }
 

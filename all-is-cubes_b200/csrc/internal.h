@@ -1,4 +1,4 @@
-// internal.h — objects behind the opaque handles of include/aicb200.h (shared by aicb200.cu and light.cu).
+// internal.h — objects behind the opaque handles of include/aicb200.h (shared by aicb200.cu, group.cu and light.cu).
 #pragma once
 #include <memory>
 #include <mutex>
@@ -141,7 +141,7 @@ struct aicb_ctx {
     int num_sms = 0;
     Stream stream;
     Event ev0, ev1;
-    Event ev_light;              // light propagation on a device group: this context's stream reached a step of a round
+    Event ev_join;               // this context's stream reached a point another context's stream waits for (fan_in)
     Event ev_k[5];               // AICB_PROFILE_KERNELS
     bool profile_kernels = false;
     bool stage_timing = true;    // record the per-kernel events of a frame (aicb_render_info::stage_ms)
@@ -225,50 +225,25 @@ struct aicb_scene {
     uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
 };
 
-// Where a frame's kernels store their outputs, and what the layers hand on between passes (launch_trace).
+// A frame's outputs (launch_trace): `target` is TraceParams::target as the kernels see it, where they store and what
+// the layers hand on between passes; the other fields are the host's choices the kernels do not see in it.
 struct Outputs {
-    bool full_frame = false;
-    uchar4 *srgb8 = nullptr;
-    float4 *colorbuf = nullptr;
-    uint2 *rgba16f = nullptr;
-    double *depth = nullptr;
-    aicb_hit *hit = nullptr;
-    uint32_t *steps = nullptr;
-    int32_t *text = nullptr;
-    // layers (renderer.rs:454-478)
-    const float4 *in_accum = nullptr;
-    float4 *out_accum = nullptr;
-    const float *backdrop = nullptr;    // premultiplied light rgb + transmittance
-    const float *no_world = nullptr;    // ColorBuf (light rgb, transmittance)
-    int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
-    // RaytraceToTexture's targets (aicb_render_layers_texture): the TEX kernels; rgba16f takes the colour texels
-    bool texture = false;
-    const uint32_t *pixel_list = nullptr;   // device: the pixel tasks (y * fb_width + x), or nullptr for every pixel
-    uint32_t n_list = 0;
-    const double *rays = nullptr;           // device: the tasks of a frame without a camera (origin, direction per ray)
+    aicb::TargetParams target{};
+    int kind = aicb::TGT_FRAME;         // the compositing kernels' target: TGT_FRAME, TGT_TEX or TGT_TERM
+    bool full_frame = false;            // outputs at framebuffer positions (TraceParams::out_full_frame)
+    bool aux = false;                   // the marching kernel that also counts steps and blocks (render_aux)
+    const double *rays = nullptr;       // device: the tasks of a frame without a camera (origin, direction per ray)
     uint64_t n_rays = 0;
-    bool aux = false;                       // the marching kernel that also counts steps and blocks (render_aux)
-    float *tex_depth = nullptr;
-    const double *in_depth = nullptr;
-    double *out_task_depth = nullptr;
-    uint32_t tex_layer = aicb::TEX_WORLD;
-    float tex_exposure[2] = {1.0f, 1.0f};
-    double depth_m[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    // the terminal's ColorCharacterBuf (aicb_render_layers_terminal): the TERM kernels; tex_layer names the pass's layer
-    bool terminal = false;
-    aicb_terminal_pixel *term = nullptr;
-    const int2 *in_text = nullptr;
-    int2 *out_task_text = nullptr;
-    int32_t text_start = AICB_TEXT_EMPTY;
+    int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
 };
 
-// One device's share of a layered frame or texture (aicb_trace_layers): that device's scenes of the layers (nullptr for
-// an absent layer; both on one context), its row strips of a whole frame or its range of a pixel list
-// (target.pixel_list), and where it stores its outputs.  A single context draws with one part and no strips.
+// One context's share of a layered frame or texture (aicb_trace_layers): that context's scenes of the layers (nullptr
+// for an absent layer; both on one context), its row strips of a whole frame or its range of a pixel list
+// (out.target.pixel_list), and where it stores its outputs.
 struct LayerPart {
     aicb_scene *world = nullptr, *ui = nullptr;
     aicb_shard shard = {1, 0, 1};
-    Outputs target;
+    Outputs out;
 };
 
 // One context's share of one pass of a frame (aicb_trace_pass): the scene it traces, its row strips, where it stores,
@@ -283,11 +258,11 @@ struct FramePart {
     aicb_render_info info{};
 };
 
-// aicb200.cu: the layer rules shared by aicb_render_layers_* and aicb_group_render_layers_*.  The layers give the
-// cameras and options (their scenes only say which layers exist).  Validation of the arguments of the single-context
-// calls; the texture target's exposures and depth transform; the passes of a frame over every part, and the one loop
-// that re-issues a pass whose hit stream overflowed (aicb_trace_pass); the one merge of aicb_render_info.  The passes
-// need the locks of the parts' contexts.  (C linkage: aicb200.cu defines them among the entry points of the C ABI.)
+// aicb200.cu: the layer rules of the layered calls.  The layers give the cameras and options (their scenes only say
+// which layers exist).  Validation of their arguments; the texture target's exposures and depth transform; the passes
+// of a frame over every part, and the one loop that re-issues a pass whose hit stream overflowed (aicb_trace_pass); the
+// one merge of aicb_render_info.  The passes need the locks of the parts' contexts.  (C linkage: aicb200.cu defines
+// them among the entry points of the C ABI.)
 extern "C" {
 aicb_status aicb_check_render_args(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
                                    const aicb_shard *shard, size_t out_len);
@@ -296,7 +271,7 @@ aicb_status aicb_check_layers(const aicb_layer *world, const aicb_layer *ui, con
 aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba,
                                       const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
                                       const void *out_rgba16f, const float *out_depth, const aicb_layer **lead_out);
-void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *target);
+void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out);
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
                               const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total);
 aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
@@ -306,12 +281,45 @@ void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool sa
 aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
 }
 
-// light.cu: the light calls over the replicas of one scene, device 0's first; a single context is the one-replica case.
-// Validation is against replica 0, before anything changes.  The caller holds every replica's context lock; on a group,
-// device 0 has peer access to every other device and they to device 0, with native atomics.  After every call the
-// replicas' light volumes are identical.
+// ---- calls over several contexts ----------------------------------------------------------------------------------
+// A call that runs on several contexts lists them device 0's first, with a scene's replica on each (a group scene's
+// replicas, in the group's order); a single context is the one-context case and runs as it would alone.  The call
+// holds every listed context's lock throughout, and device 0 is where its results are collected.
+
+// Every listed context's lock, for the whole of a call.
+struct ContextLocks {
+    std::vector<std::unique_lock<std::mutex>> locks;
+    explicit ContextLocks(const std::vector<aicb_ctx *> &ctx) {
+        for (aicb_ctx *c : ctx) locks.emplace_back(c->mu);
+    }
+};
+
+// group.cu: the order between the listed contexts' streams: every other context's stream waits until device 0's has
+// reached this point (fan_out), or device 0's until every other one's has (fan_in, which leaves device 0 current).
+aicb_status fan_out(aicb_ctx *const *ctx, size_t n);
+aicb_status fan_in(aicb_ctx *const *ctx, size_t n);
+
+// group.cu: the layered calls (aicb_render_layers_* and aicb_group_render_layers_*), which validate, lock, trace the
+// layers over one part per context (aicb_trace_layers), collect the parts' outputs on device 0, copy them to the caller
+// and fill info.  `world` and `ui` are the layers as device 0 sees them; world_scenes / ui_scenes each layer's replica
+// on every one of the n contexts (nullptr for an absent layer).
+struct LayeredCall {
+    const aicb_layer *world, *ui;
+    aicb_scene *const *world_scenes, *const *ui_scenes;
+    size_t n;
+    const float *backdrop_rgba, *no_world_rgba;
+};
+aicb_status layers_srgb8(const LayeredCall &c, uint8_t (*out)[4], size_t out_len, aicb_render_info *info);
+aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info);
+aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
+                           uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info);
+
+// light.cu: the light calls over a scene's replicas (ctx[i] is scene[i]'s context).  Validation is against replica 0,
+// before anything changes.  On a group, device 0 has peer access to every other device and they to device 0, with
+// native atomics.  After every call the replicas' light volumes are identical.
 struct LightReplicas {
     aicb_scene *const *scene;
+    aicb_ctx *const *ctx;
     size_t n;
 };
 aicb_status light_fast_evaluate(LightReplicas r);

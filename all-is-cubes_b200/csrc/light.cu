@@ -783,45 +783,14 @@ aicb_status ensure_light_state(aicb_scene *s, bool queue = true) {
     return AICB_OK;
 }
 
-// The order between a group's streams: every other replica's stream waits until device 0's has reached this point
-// (fan_out), or device 0's until every other one's has (fan_in).
-aicb_status fan_out(LightReplicas r) {
-    aicb_ctx *c0 = r.scene[0]->ctx;
-    CU(cudaSetDevice(c0->device));
-    CU(cudaEventRecord(c0->ev_light.get(), c0->stream.get()));
-    for (size_t i = 1; i < r.n; i++) {
-        aicb_ctx *c = r.scene[i]->ctx;
-        CU(cudaSetDevice(c->device));
-        CU(cudaStreamWaitEvent(c->stream.get(), c0->ev_light.get(), 0));
-    }
-    return AICB_OK;
-}
-aicb_status fan_in(LightReplicas r) {
-    for (size_t i = 1; i < r.n; i++) {
-        aicb_ctx *c = r.scene[i]->ctx;
-        CU(cudaSetDevice(c->device));
-        CU(cudaEventRecord(c->ev_light.get(), c->stream.get()));
-    }
-    aicb_ctx *c0 = r.scene[0]->ctx;
-    CU(cudaSetDevice(c0->device));
-    for (size_t i = 1; i < r.n; i++) CU(cudaStreamWaitEvent(c0->stream.get(), r.scene[i]->ctx->ev_light.get(), 0));
-    return AICB_OK;
-}
-
 // Every replica's light state (the queue on replica 0 only) and, on a group, what a round needs beyond one context's:
-// each context's event, replica 0's dirty bits, and the other replicas' light volumes as push targets.
+// replica 0's dirty bits, and the other replicas' light volumes as push targets.
 aicb_status ensure_replicas(LightReplicas r) {
     for (size_t i = 0; i < r.n; i++) {
         CU(cudaSetDevice(r.scene[i]->ctx->device));
         TRY(ensure_light_state(r.scene[i], i == 0));
     }
     if (r.n == 1) return AICB_OK;
-    for (size_t i = 0; i < r.n; i++) {
-        aicb_ctx *c = r.scene[i]->ctx;
-        if (c->ev_light) continue;
-        CU(cudaSetDevice(c->device));
-        TRY(create_event(c->ev_light, cudaEventDisableTiming));
-    }
     aicb_scene *s = r.scene[0];
     CU(cudaSetDevice(s->ctx->device));
     if (!s->d_dirty) {
@@ -837,7 +806,7 @@ aicb_status ensure_replicas(LightReplicas r) {
     TRY(s->d_push_targets.ensure(targets.size() * sizeof(uint32_t *)));
     CU(cudaMemcpy(s->d_push_targets.get(), targets.data(), targets.size() * sizeof(uint32_t *), cudaMemcpyHostToDevice));
     // device 0 writes the other replicas' volumes: after what their streams hold (aicb_scene_update_cubes is queued)
-    return fan_in(r);
+    return fan_in(r.ctx, r.n);
 }
 
 // evaluate_light (space.rs:1496-1527): rounds until the highest queued priority is <= from_difference(epsilon).
@@ -887,18 +856,18 @@ aicb_status propagate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, 
             CU(cudaMemsetAsync(P.scalars + 6, 0, 4 * 4, st));   // ... its count of changed cubes, the two work counters, the overflow count
             k_find_max<<<16, 256, 0, st>>>(P, n_tiles);
             k_gather<<<blocks, 256, 0, st>>>(P, n_tiles);
-            if (group) TRY(fan_out(r));
+            if (group) TRY(fan_out(r.ctx, r.n));
             TRY(walk(false));
-            if (group) TRY(fan_in(r));
+            if (group) TRY(fan_in(r.ctx, r.n));
             if (group) k_apply<true><<<wide, 128, 0, st>>>(P);
             else k_apply<false><<<wide, 128, 0, st>>>(P);
             k_compact_changed<<<blocks, 256, 0, st>>>(P);
             if (group) {
                 k_push<<<blocks, 256, 0, st>>>(P, s->d_push_targets.get<uint32_t *const>(), (uint32_t)(r.n - 1));
-                TRY(fan_out(r));
+                TRY(fan_out(r.ctx, r.n));
             }
             TRY(walk(true));
-            if (group) TRY(fan_in(r));   // (the next round's queue holds every replica's marks)
+            if (group) TRY(fan_in(r.ctx, r.n));   // (the next round's queue holds every replica's marks)
         }
         uint32_t h[8];
         CU(cudaMemcpyAsync(h, P.scalars, 8 * 4, cudaMemcpyDeviceToHost, st));
@@ -1003,7 +972,7 @@ aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, 
     TRY(d_cubes.upload(cubes, n * 12));
     const int32_t *explicit_cubes = d_cubes.get<int32_t>();
     CU(cudaMemsetAsync(P.scalars, 0, 16 * 4, stream));
-    if (group) TRY(fan_out(r));
+    if (group) TRY(fan_out(r.ctx, r.n));
     for (size_t i = 0; i < r.n; i++) {
         aicb_ctx *c = r.scene[i]->ctx;
         cudaStream_t cs = c->stream.get();
@@ -1012,7 +981,7 @@ aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, 
         k_walk_chains<false><<<c->chain_walk_blocks, 128, 0, cs>>>(RP[i], (uint32_t)n, explicit_cubes);
         k_compute_overflow<<<c->num_sms * 8, 128, 0, cs>>>(RP[i], explicit_cubes);
     }
-    if (group) TRY(fan_in(r));
+    if (group) TRY(fan_in(r.ctx, r.n));
     uint32_t h[16];
     CU(cudaMemcpyAsync(out, P.new_light, n * 4, cudaMemcpyDeviceToHost, stream));
     CU(cudaMemcpyAsync(h, P.scalars, sizeof h, cudaMemcpyDeviceToHost, stream));
@@ -1220,28 +1189,28 @@ uint32_t aicb_light_chart(float *weights, uint32_t *children) {
 aicb_status aicb_light_fast_evaluate(aicb_scene *s) {
     if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_fast_evaluate({&s, 1});
+    return light_fast_evaluate({&s, &s->ctx, 1});
 }
 
 aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
     if (!s || (n && (!cubes || !out))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_compute({&s, 1}, cubes, n, out);
+    return light_compute({&s, &s->ctx, 1}, cubes, n, out);
 }
 
 aicb_status aicb_light_evaluate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                 uint64_t *node_visits) {
     if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_evaluate({&s, 1}, epsilon, updates_done, max_diff, node_visits);
+    return light_evaluate({&s, &s->ctx, 1}, epsilon, updates_done, max_diff, node_visits);
 }
 
 aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                           uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
     if (!s || (n_edits && (!cubes || !new_ids))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_edit_and_propagate({&s, 1}, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+    return light_edit_and_propagate({&s, &s->ctx, 1}, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
 }
 
 aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {

@@ -145,6 +145,51 @@ struct __align__(16) TaskOut {
     uint32_t n_hits;     // hit records of this ray (consecutive slots; the last slot of a chunk links to the next chunk)
 };
 
+// Where a frame's kernels store their outputs, and what the layers hand on between passes (TraceParams::target).
+struct TargetParams {
+    uchar4 *out_srgb8;
+    float4 *out_colorbuf;
+    uint2 *out_rgba16f;         // premultiplied RGBA, 4 x f16 (raytrace_to_texture.rs:645-661)
+    double *out_depth;
+    aicb_hit *out_hit;
+    uint32_t *out_steps;
+    int32_t *out_text;          // CharacterBuf (text.rs:52-123) per pixel: block index of the first hit, or AICB_TEXT_*
+    // layers (RtScene::trace_ray_through_layers, renderer.rs:454-478): a ray's accumulator can start from what the
+    // layer in front left in it, and can be handed on instead of becoming a pixel
+    const float4 *in_accum;     // per task (global index): ColorBuf (light, transmittance) to start from, or nullptr
+    float4 *out_accum;          // per task: the ray's ColorBuf goes here and no pixel is produced, or nullptr
+    float backdrop[4];          // Exception::Backdrop hit added after the ray (premultiplied light rgb, transmittance)
+    uint32_t has_backdrop;
+    float no_world[4];          // ColorBuf the accumulator is replaced by if it is not opaque in the end
+    uint32_t has_no_world;
+    // RaytraceToTexture's colour and depth targets (raytrace_to_texture.rs:591-683): read only by the TGT_TEX
+    // instantiations of resolve_kernel / encode_kernel, and (the pixel list) by gen_kernel
+    const uint32_t *pixel_list; // pixel task i is the framebuffer pixel pixel_list[i] = y * fb_width + x, or nullptr
+    uint32_t n_list;
+    uint32_t tex_layer;         // InLayer of this pass's hits: TEX_WORLD or TEX_UI (also the TGT_TERM text's layer)
+    // A frame has one target, so the fields of the other target share the space: the parameter block, and with it
+    // the code of the kernels that read neither, keeps its size.
+    union {
+        struct {
+            float tex_exposure[2];      // exposure of the world and of the UI camera
+            double depth_m[8];          // m13 m23 m33 m43 m14 m24 m34 m44 of the depth transform
+            const double *in_depth;     // per task (global index): DepthBuf the layer in front left, or nullptr
+            double *out_task_depth;     // per task: the ray's DepthBuf, handed on next to out_accum, or nullptr
+            float *out_tex_depth;       // per pixel: the depth texel
+        };
+        // The terminal's ColorCharacterBuf (aicb_render_layers_terminal): read only by the TGT_TERM instantiations.
+        // A CharacterBuf is (text, layer): an AICB_TEXT_* state or block index, and the tex_layer of the pass whose
+        // Space the index belongs to.
+        struct {
+            aicb_terminal_pixel *out_term;  // per pixel: post-processed colour, text, layer
+            const int2 *in_text;            // per task (global index): CharacterBuf the layer in front left, or nullptr
+            int2 *out_task_text;            // per task: the ray's CharacterBuf, handed on next to out_accum, or nullptr
+            int32_t text_start;             // CharacterBuf of a ray without in_text: Empty, or Hit(" ") behind a lone
+                                            // backdrop
+        };
+    };
+};
+
 struct TraceParams {
     DeviceScene scene;
     // camera
@@ -191,48 +236,7 @@ struct TraceParams {
     uint32_t tail_divisor;      // once the ray list is exhausted: leave the loop when (lanes that still have a ray) / this wait
     uint32_t refill_threshold;  // tail mode: once the ray list is exhausted and at most this many lanes of a warp still march,
                                 // they run the lean per-lane loop
-    // outputs
-    uchar4 *out_srgb8;
-    float4 *out_colorbuf;
-    uint2 *out_rgba16f;         // premultiplied RGBA, 4 x f16 (raytrace_to_texture.rs:645-661)
-    double *out_depth;
-    aicb_hit *out_hit;
-    uint32_t *out_steps;
-    int32_t *out_text;          // CharacterBuf (text.rs:52-123) per pixel: block index of the first hit, or AICB_TEXT_*
-    // layers (RtScene::trace_ray_through_layers, renderer.rs:454-478): a ray's accumulator can start from what the
-    // layer in front left in it, and can be handed on instead of becoming a pixel
-    const float4 *in_accum;     // per task (global index): ColorBuf (light, transmittance) to start from, or nullptr
-    float4 *out_accum;          // per task: the ray's ColorBuf goes here and no pixel is produced, or nullptr
-    float backdrop[4];          // Exception::Backdrop hit added after the ray (premultiplied light rgb, transmittance)
-    uint32_t has_backdrop;
-    float no_world[4];          // ColorBuf the accumulator is replaced by if it is not opaque in the end
-    uint32_t has_no_world;
-    // RaytraceToTexture's colour and depth targets (raytrace_to_texture.rs:591-683): read only by the TGT_TEX
-    // instantiations of resolve_kernel / encode_kernel, and (the pixel list) by gen_kernel
-    const uint32_t *pixel_list; // pixel task i is the framebuffer pixel pixel_list[i] = y * fb_width + x, or nullptr
-    uint32_t n_list;
-    uint32_t tex_layer;         // InLayer of this pass's hits: TEX_WORLD or TEX_UI (also the TGT_TERM text's layer)
-    // A frame has one target, so the fields of the other target share the space: the parameter block, and with it
-    // the code of the kernels that read neither, keeps its size.
-    union {
-        struct {
-            float tex_exposure[2];      // exposure of the world and of the UI camera
-            double depth_m[8];          // m13 m23 m33 m43 m14 m24 m34 m44 of the depth transform
-            const double *in_depth;     // per task (global index): DepthBuf the layer in front left, or nullptr
-            double *out_task_depth;     // per task: the ray's DepthBuf, handed on next to out_accum, or nullptr
-            float *out_tex_depth;       // per pixel: the depth texel
-        };
-        // The terminal's ColorCharacterBuf (aicb_render_layers_terminal): read only by the TGT_TERM instantiations.
-        // A CharacterBuf is (text, layer): an AICB_TEXT_* state or block index, and the tex_layer of the pass whose
-        // Space the index belongs to.
-        struct {
-            aicb_terminal_pixel *out_term;  // per pixel: post-processed colour, text, layer
-            const int2 *in_text;            // per task (global index): CharacterBuf the layer in front left, or nullptr
-            int2 *out_task_text;            // per task: the ray's CharacterBuf, handed on next to out_accum, or nullptr
-            int32_t text_start;             // CharacterBuf of a ray without in_text: Empty, or Hit(" ") behind a lone
-                                            // backdrop
-        };
-    };
+    TargetParams target;        // outputs
     // LightingOption::Bounce (surface.rs:113-166): the frame's primary pass and its secondary passes share these
     uint32_t bounce_mode;       // BOUNCE_OFF / BOUNCE_PRIMARY / BOUNCE_SECONDARY
     uint32_t bounce_samples;    // LightingOption::Bounce { samples }
@@ -801,9 +805,9 @@ AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px
         *out_index = pixel_task;
         return pixel_task < P.n_rays;
     }
-    if (LIST && P.pixel_list) {
-        if (pixel_task >= P.n_list) return false;
-        const uint32_t v = __ldg(P.pixel_list + pixel_task);
+    if (LIST && P.target.pixel_list) {
+        if (pixel_task >= P.target.n_list) return false;
+        const uint32_t v = __ldg(P.target.pixel_list + pixel_task);
         *px = v % P.fb_width;
         *py = v / P.fb_width;
         *out_index = pixel_task;
@@ -1252,8 +1256,8 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
                         valid = (rec.flags & 16u) != 0;
                         L = 0.0f;
                         step_limit = 1000u;
-                        if (P.in_accum) {   // the layers in front may have made the ray opaque already
-                            const float t0 = __ldg(&P.in_accum[P.task_base + task].w);
+                        if (P.target.in_accum) {   // the layers in front may have made the ray opaque already
+                            const float t0 = __ldg(&P.target.in_accum[P.task_base + task].w);
                             L = (t0 > 0.0f) ? __log2f(t0) + 1e-3f : F_NEG_INF;
                             step_limit = (L < -8.0f) ? 0u : 1000u;
                         }
@@ -1690,7 +1694,7 @@ static __global__ void __launch_bounds__(128) bounce_select_kernel(const __grid_
     TaskOut o;
     *reinterpret_cast<uint4 *>(&o) = *reinterpret_cast<const uint4 *>(P.task_out + i);
     float T = 1.0f;
-    if (P.in_accum) T = P.in_accum[P.task_base + i].w;
+    if (P.target.in_accum) T = P.target.in_accum[P.task_base + i].w;
     uint32_t hi = o.first_hit, req = HIT_NONE;
     for (uint32_t hk = 0; hk < o.n_hits; hk++) {
         ShadedHit c;
@@ -1866,12 +1870,12 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
         float lr, lg, lb, T;
         uint32_t steps, sample_first;
         chain(k, o, lr, lg, lb, T, steps, sample_first);
-        if (sample_first != 0xffffffffu && (P.out_depth || P.out_hit)) {
+        if (sample_first != 0xffffffffu && (P.target.out_depth || P.target.out_hit)) {
             const HitRecord *hr = P.hits + sample_first;   // Hit::t_distance = last_t / resolution (surface.rs:385-386)
             depth = fmin(depth, hr->last_t * recip_pow2(1 << ((hr->flags >> 4) & 15u)));
             if (first_valid == 0xffffffffu) first_valid = sample_first;
         }
-        if (P.out_text) {
+        if (P.target.out_text) {
             // CharacterBuf::add (text.rs:84-98): the first hit of a block names it; Exception::Incomplete without one
             // is "X"; a ray that counted a step entered the space (sr.rs:628-637)
             int32_t tk = o.steps > 0 ? AICB_TEXT_ENTERED_SPACE : AICB_TEXT_EMPTY;
@@ -1905,47 +1909,47 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
             lr = red; lg = green; lb = ps_clamped(lum * 0.2f);
             T = 0.0f;
         }
-        if (P.has_backdrop) {   // Exception::Backdrop between the UI and the world (renderer.rs:458-466)
-            lr = lr + P.backdrop[0] * T; lg = lg + P.backdrop[1] * T; lb = lb + P.backdrop[2] * T;
-            T = T * P.backdrop[3];
+        if (P.target.has_backdrop) {   // Exception::Backdrop between the UI and the world (renderer.rs:458-466)
+            lr = lr + P.target.backdrop[0] * T; lg = lg + P.target.backdrop[1] * T; lb = lb + P.target.backdrop[2] * T;
+            T = T * P.target.backdrop[3];
         }
         if constexpr (TEX) {
             // DepthBuf::add (accum.rs:275-282): f64::min of the layer in front's depth and this layer's first surface
-            double d = P.in_depth ? P.in_depth[P.task_base + t0 + k] : D_INF;
+            double d = P.target.in_depth ? P.target.in_depth[P.task_base + t0 + k] : D_INF;
             if (sample_first != 0xffffffffu) {
                 const HitRecord *hr = P.hits + sample_first;
                 d = fmin(d, hr->last_t * recip_pow2(1 << ((hr->flags >> 4) & 15u)));
             }
-            const float t_in = P.in_accum ? P.in_accum[P.task_base + t0 + k].w : 1.0f;
-            uint32_t layer = t_in != 1.0f ? TEX_UI : (T != 1.0f ? P.tex_layer : TEX_NONE);
-            if (P.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint: a fresh Split with the paint hit alone
+            const float t_in = P.target.in_accum ? P.target.in_accum[P.task_base + t0 + k].w : 1.0f;
+            uint32_t layer = t_in != 1.0f ? TEX_UI : (T != 1.0f ? P.target.tex_layer : TEX_NONE);
+            if (P.target.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint: a fresh Split with the paint hit alone
                 d = D_INF;
-                layer = P.no_world[3] != 1.0f ? TEX_WORLD : TEX_NONE;
+                layer = P.target.no_world[3] != 1.0f ? TEX_WORLD : TEX_NONE;
             }
-            if (P.out_task_depth) P.out_task_depth[P.task_base + t0 + k] = d;
+            if (P.target.out_task_depth) P.target.out_task_depth[P.task_base + t0 + k] = d;
             tex_depth = fmin(tex_depth, d);
             if (tex_layer == TEX_NONE) tex_layer = layer;
         }
         if constexpr (TERM) {
-            int2 c = P.in_text ? P.in_text[P.task_base + t0 + k] : make_int2(P.text_start, (int)TEX_NONE);
+            int2 c = P.target.in_text ? P.target.in_text[P.task_base + t0 + k] : make_int2(P.target.text_start, (int)TEX_NONE);
             if (!text_is_hit(c.x)) {   // CharacterBuf::add of this layer's hits, then the backdrop's
-                if (sample_first != 0xffffffffu) c = make_int2(hit_block(P, sample_first), (int)P.tex_layer);
+                if (sample_first != 0xffffffffu) c = make_int2(hit_block(P, sample_first), (int)P.target.tex_layer);
                 else if (o.steps > 1000u) c.x = AICB_TEXT_INCOMPLETE;
-                else if (P.debug_pixel_cost || P.has_backdrop) c.x = AICB_TEXT_BLANK;
+                else if (P.debug_pixel_cost || P.target.has_backdrop) c.x = AICB_TEXT_BLANK;
                 else if (o.steps > 0) c.x = AICB_TEXT_ENTERED_SPACE;
             }
-            if (P.has_no_world && !(T < (1.0f / 256.0f))) c = make_int2(AICB_TEXT_BLANK, (int)TEX_NONE);   // P::paint
-            if (P.out_task_text) P.out_task_text[P.task_base + t0 + k] = c;
+            if (P.target.has_no_world && !(T < (1.0f / 256.0f))) c = make_int2(AICB_TEXT_BLANK, (int)TEX_NONE);   // P::paint
+            if (P.target.out_task_text) P.target.out_task_text[P.task_base + t0 + k] = c;
             // CharacterBuf::mean (text.rs:96-108): the first sample that holds a Hit; EnteredSpace only if all entered
             if (k == 0 || (!text_is_hit(term.x) && text_is_hit(c.x))) term = c;
             else if (!text_is_hit(term.x))
                 term.x = (term.x == AICB_TEXT_ENTERED_SPACE && c.x == AICB_TEXT_ENTERED_SPACE) ? AICB_TEXT_ENTERED_SPACE
                                                                                              : AICB_TEXT_EMPTY;
         }
-        if (P.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint(NO_WORLD_TO_SHOW) replaces it (renderer.rs:474-477)
-            lr = P.no_world[0]; lg = P.no_world[1]; lb = P.no_world[2]; T = P.no_world[3];
+        if (P.target.has_no_world && !(T < (1.0f / 256.0f))) {   // P::paint(NO_WORLD_TO_SHOW) replaces it (renderer.rs:474-477)
+            lr = P.target.no_world[0]; lg = P.target.no_world[1]; lb = P.target.no_world[2]; T = P.target.no_world[3];
         }
-        if (P.out_accum) P.out_accum[P.task_base + t0 + k] = make_float4(lr, lg, lb, T);
+        if (P.target.out_accum) P.target.out_accum[P.task_base + t0 + k] = make_float4(lr, lg, lb, T);
         if (P.bounce_mode == BOUNCE_SECONDARY) {
             // Rgba::from(light_accum_buf.inner).to_rgb() added to the surface's multi_ray_accum (surface.rs:158-160)
             if (P.bounce_req[t0 + k] != HIT_NONE) {
@@ -1963,25 +1967,25 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
         steps_total += steps;
         a0 = a0 + lr; a1 = a1 + lg; a2 = a2 + lb; aT = aT + T;
     }
-    if (P.out_text) P.out_text[out_index] = text;
+    if (P.target.out_text) P.target.out_text[out_index] = text;
     float l0 = a0, l1 = a1, l2 = a2, tT = aT;
     if (P.n_samples == 4) { l0 = a0 / 4.0f; l1 = a1 / 4.0f; l2 = a2 / 4.0f; tT = aT / 4.0f; }
-    if (P.out_srgb8) P.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
-    if (P.out_colorbuf) P.out_colorbuf[out_index] = make_float4(l0, l1, l2, tT);
+    if (P.target.out_srgb8) P.target.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
+    if (P.target.out_colorbuf) P.target.out_colorbuf[out_index] = make_float4(l0, l1, l2, tT);
     if constexpr (TERM) {
-        if (P.out_term) {   // ColorCharacterBuf::output (terminal.rs:355-366): post_process_color(Rgba::from(ColorBuf))
+        if (P.target.out_term) {   // ColorCharacterBuf::output (terminal.rs:355-366): post_process_color(Rgba::from(ColorBuf))
             float rgba[4], c[3];
             colorbuf_to_rgba(l0, l1, l2, tT, rgba);
             post_process_color(P, rgba, c);
-            float2 *dst = reinterpret_cast<float2 *>(P.out_term + out_index);   // 24-byte pixels: 8-byte stores
+            float2 *dst = reinterpret_cast<float2 *>(P.target.out_term + out_index);   // 24-byte pixels: 8-byte stores
             dst[0] = make_float2(c[0], c[1]);
             dst[1] = make_float2(c[2], rgba[3]);
             reinterpret_cast<int2 *>(dst)[2] = term;
         }
     }
     if constexpr (TEX) {
-        if (P.out_rgba16f) {   // trace_one's colour (raytrace_to_texture.rs:643-661): the exposure of the pixel's layer
-            const float e = tex_layer == TEX_UI ? P.tex_exposure[1] : (tex_layer == TEX_WORLD ? P.tex_exposure[0] : 1.0f);
+        if (P.target.out_rgba16f) {   // trace_one's colour (raytrace_to_texture.rs:643-661): the exposure of the pixel's layer
+            const float e = tex_layer == TEX_UI ? P.target.tex_exposure[1] : (tex_layer == TEX_WORLD ? P.target.tex_exposure[0] : 1.0f);
             float a = 1.0f - tT;
             a = a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a);
             const __half2 rg = __floats2half2_rn(l0 * e, l1 * e);
@@ -1989,20 +1993,20 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
             uint2 packed;
             packed.x = *reinterpret_cast<const uint32_t *>(&rg);
             packed.y = *reinterpret_cast<const uint32_t *>(&ba);
-            P.out_rgba16f[out_index] = packed;
+            P.target.out_rgba16f[out_index] = packed;
         }
-        if (P.out_tex_depth) {
+        if (P.target.out_tex_depth) {
             // trace_one's depth (:663-674): clamp(0, 1) (NaN passes), depth_transform.transform_point3d_homogeneous
             // (0, 0, d) in euclid's term order, z / w as f32, the layer's sign (World +1, Ui or none -1)
             double d = tex_depth;
             if (d < 0.0) d = 0.0;
             if (d > 1.0) d = 1.0;
-            const double *m = P.depth_m;
+            const double *m = P.target.depth_m;
             const double z = ((0.0 * m[0] + 0.0 * m[1]) + d * m[2]) + m[3];
             const double w = ((0.0 * m[4] + 0.0 * m[5]) + d * m[6]) + m[7];
-            P.out_tex_depth[out_index] = (float)(z / w) * (tex_layer == TEX_WORLD ? 1.0f : -1.0f);
+            P.target.out_tex_depth[out_index] = (float)(z / w) * (tex_layer == TEX_WORLD ? 1.0f : -1.0f);
         }
-    } else if (P.out_rgba16f) {
+    } else if (P.target.out_rgba16f) {
         // ColorBuf::into_premultiplied_rgba (raytracer_components.rs:70-77) scaled by the exposure and rounded to
         // f16 as half::f16::from_f32 does (round to nearest even, overflow to infinity)
         float a = 1.0f - tT;
@@ -2012,11 +2016,11 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
         uint2 packed;
         packed.x = *reinterpret_cast<const uint32_t *>(&rg);
         packed.y = *reinterpret_cast<const uint32_t *>(&ba);
-        P.out_rgba16f[out_index] = packed;
+        P.target.out_rgba16f[out_index] = packed;
     }
-    if (P.out_depth) P.out_depth[out_index] = depth;
-    if (P.out_steps) P.out_steps[out_index] = steps_total;
-    if (P.out_hit) {
+    if (P.target.out_depth) P.target.out_depth[out_index] = depth;
+    if (P.target.out_steps) P.target.out_steps[out_index] = steps_total;
+    if (P.target.out_hit) {
         aicb_hit hh;
         if (first_valid != 0xffffffffu) {
             HitRecord hr;
@@ -2037,7 +2041,7 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
             hh.resolution = -1;
             hh.face = -1;
         }
-        P.out_hit[out_index] = hh;
+        P.target.out_hit[out_index] = hh;
     }
     return steps_total;
 }
@@ -2080,8 +2084,8 @@ __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ Tra
         cubes_traced = finish_pixel<TEX, TERM>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
                                                                float &T, uint32_t &steps, uint32_t &sample_first) {
             lr = 0.f; lg = 0.f; lb = 0.f; T = 1.0f;
-            if (P.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
-                const float4 a = P.in_accum[P.task_base + t0 + k];
+            if (P.target.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
+                const float4 a = P.target.in_accum[P.task_base + t0 + k];
                 lr = a.x; lg = a.y; lb = a.z; T = a.w;
             }
             steps = o.steps;
@@ -2174,8 +2178,8 @@ __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const 
     if (active) {
         TaskOut o;
         *reinterpret_cast<uint4 *>(&o) = *reinterpret_cast<const uint4 *>(P.task_out + t);
-        if (P.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
-            const float4 a = P.in_accum[P.task_base + t];
+        if (P.target.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
+            const float4 a = P.target.in_accum[P.task_base + t];
             lr = a.x; lg = a.y; lb = a.z; T = a.w;
         }
         steps = o.steps;

@@ -8,8 +8,8 @@ import numpy as np
 import pytest
 
 import aicb200
-from aicb200 import (FOG_NONE, LIGHT_FLAT, LIGHT_NONE, TRANSPARENCY_VOLUMETRIC, AicbError, Block, Context,
-                     GraphicsOptions, SpaceRaytracer, abi, scenes)
+from aicb200 import (FOG_NONE, LIGHT_BOUNCE, LIGHT_FLAT, LIGHT_NONE, TRANSPARENCY_VOLUMETRIC, AicbError, Block, Context,
+                     GraphicsOptions, RtRenderer, SpaceRaytracer, abi, scenes)
 from test_gpu_resolve import faint_slab
 
 pytestmark = pytest.mark.gpu
@@ -31,8 +31,11 @@ def spaces():
     return scenes.small_mixed_scene(n=12, seed=7), scenes.small_mixed_scene(n=6, seed=11, lower=(0, 0, 0))
 
 
-def setup(world_space, ui_space, aa, debug=False, w=W, h=H):
-    wopts = GraphicsOptions(view_distance=40.0, antialiasing_always=aa, exposure=1.75, debug_pixel_cost=debug)
+def setup(world_space, ui_space, aa, debug=False, w=W, h=H, bounce=False):
+    # bounce: the world layer with LightingOption::Bounce, whose frames run a secondary pass per sample
+    lighting = dict(lighting_display=LIGHT_BOUNCE, bounce_samples=2) if bounce else {}
+    wopts = GraphicsOptions(view_distance=40.0, antialiasing_always=aa, exposure=1.75, debug_pixel_cost=debug,
+                            **lighting)
     uopts = GraphicsOptions(view_distance=30.0, fog=FOG_NONE, lighting_display=LIGHT_FLAT, exposure=0.625,
                             antialiasing_always=aa)
     wcam = scenes.standard_camera(world_space, wopts, w, h)
@@ -48,10 +51,12 @@ def same_info(a, b):
     return a.cubes_traced == b.cubes_traced and a.rays == b.rays
 
 
-@pytest.mark.parametrize("aa,debug", [(False, False), (True, False), (False, True)])
-def test_layered_frames_equal_the_single_context_frame(spaces, aa, debug):
+@pytest.mark.parametrize("aa,debug,bounce", [(False, False, False), (True, False, False), (False, True, False),
+                                             (False, False, True)],
+                         ids=["False-False", "True-False", "False-True", "bounce"])
+def test_layered_frames_equal_the_single_context_frame(spaces, aa, debug, bounce):
     mixed, ui_space = spaces
-    wopts, uopts, wcam, ucam = setup(mixed, ui_space, aa, debug)
+    wopts, uopts, wcam, ucam = setup(mixed, ui_space, aa, debug, bounce=bounce)
     wrt = SpaceRaytracer(mixed, wopts)
     urt = SpaceRaytracer(ui_space, uopts, wrt.ctx)
     alone = [aicb200.render_layers(*layers(c, (wrt, wcam, wopts), (urt, ucam, uopts)), c["backdrop"], NO_WORLD)
@@ -61,17 +66,22 @@ def test_layered_frames_equal_the_single_context_frame(spaces, aa, debug):
         gw, gu = g.add_scene(mixed), g.add_scene(ui_space)
         for c, ref in zip(CASES, alone):
             got = g.render_layers(*layers(c, (gw, wcam, wopts), (gu, ucam, uopts)), c["backdrop"], NO_WORLD)
-            assert np.array_equal(got.data, ref.data), f"{devices} aa={aa} debug={debug} {c}"
+            assert np.array_equal(got.data, ref.data), f"{devices} aa={aa} debug={debug} bounce={bounce} {c}"
             assert same_info(got.info, ref.info), f"{devices} {c}"
         g.close()
+    if bounce:   # the world alone, no backdrop, no paint: the frame of aicb_render_srgb8 (with the sky)
+        r = RtRenderer(wcam, wrt.ctx)
+        r.update(mixed)
+        assert np.array_equal(aicb200.render_layers((wrt, wcam, wopts)).data, r.draw().data)
+        r.rt.close()
     urt.close()
     wrt.close()
 
 
-@pytest.mark.parametrize("aa", [False, True])
-def test_texture_targets_equal_the_single_context_texels(spaces, aa):
+@pytest.mark.parametrize("aa,bounce", [(False, False), (True, False), (False, True)], ids=["False", "True", "bounce"])
+def test_texture_targets_equal_the_single_context_texels(spaces, aa, bounce):
     mixed, ui_space = spaces
-    wopts, uopts, wcam, ucam = setup(mixed, ui_space, aa)
+    wopts, uopts, wcam, ucam = setup(mixed, ui_space, aa, bounce=bounce)
     wrt = SpaceRaytracer(mixed, wopts)
     urt = SpaceRaytracer(ui_space, uopts, wrt.ctx)
     m = wcam.depth_transform()
@@ -89,7 +99,7 @@ def test_texture_targets_equal_the_single_context_texels(spaces, aa):
         for (c, px), (rgba, depth, info) in zip(runs, alone):
             got = g.render_layers_texture(*layers(c, (gw, wcam, wopts), (gu, ucam, uopts)), c["backdrop"], NO_WORLD, m,
                                           pixels=px)
-            label = f"{devices} aa={aa} {c} {'whole' if px is None else len(px)}"
+            label = f"{devices} aa={aa} bounce={bounce} {c} {'whole' if px is None else len(px)}"
             assert np.array_equal(got[0], rgba), label
             assert np.array_equal(got[1].view(np.uint32), depth.view(np.uint32)), label
             assert same_info(got[2], info), label

@@ -9,8 +9,8 @@ import pytest
 import aicb200
 import orc
 import termorc
-from aicb200 import (FOG_NONE, LIGHT_FLAT, LIGHT_LINEAR, LIGHT_NONE, TRANSPARENCY_VOLUMETRIC, AicbError, Block, Camera,
-                     Context, GraphicsOptions, RtRenderer, Space, SpaceRaytracer, Viewport, abi, scenes)
+from aicb200 import (FOG_NONE, LIGHT_BOUNCE, LIGHT_FLAT, LIGHT_LINEAR, LIGHT_NONE, TRANSPARENCY_VOLUMETRIC, AicbError,
+                     Block, Camera, Context, GraphicsOptions, RtRenderer, Space, SpaceRaytracer, Viewport, abi, scenes)
 from test_gpu_resolve import faint_slab
 
 pytestmark = pytest.mark.gpu
@@ -153,11 +153,15 @@ def test_deep_frame_overflows_then_matches_through_both_compositing_paths(lighti
 DEVICES = ([0], [0, 0], [0, 0, 0])
 
 
-@pytest.mark.parametrize("aa,debug", [(False, False), (True, False), (False, True)])
-def test_group_frames_equal_the_single_context_frame(aa, debug):
+@pytest.mark.parametrize("aa,debug,bounce", [(False, False, False), (True, False, False), (False, True, False),
+                                             (False, False, True)],
+                         ids=["False-False", "True-False", "False-True", "bounce"])
+def test_group_frames_equal_the_single_context_frame(aa, debug, bounce):
     mixed = scenes.small_mixed_scene(n=12, seed=7)
     ui_space = scenes.small_mixed_scene(n=6, seed=11, lower=(0, 0, 0))
     wopts, uopts, wcam, ucam = layer_setup(mixed, ui_space, aa, debug, h=45)   # 45 rows: not a multiple of 16 x n
+    if bounce:   # the world layer with LightingOption::Bounce, whose frames run a secondary pass per sample
+        wopts = GraphicsOptions(view_distance=40.0, exposure=1.75, lighting_display=LIGHT_BOUNCE, bounce_samples=2)
     wrt = SpaceRaytracer(mixed, wopts)
     urt = SpaceRaytracer(ui_space, uopts, wrt.ctx)
     alone = [aicb200.render_layers_terminal(*pick(c, (wrt, wcam, wopts), (urt, ucam, uopts)), c["backdrop"], NO_WORLD)
@@ -167,7 +171,7 @@ def test_group_frames_equal_the_single_context_frame(aa, debug):
         gw, gu = g.add_scene(mixed), g.add_scene(ui_space)
         for c, ref in zip(CASES, alone):
             got = g.render_layers_terminal(*pick(c, (gw, wcam, wopts), (gu, ucam, uopts)), c["backdrop"], NO_WORLD)
-            assert same_frame(got, ref), f"{devices} aa={aa} debug={debug} {c}"
+            assert same_frame(got, ref), f"{devices} aa={aa} debug={debug} bounce={bounce} {c}"
             assert got["info"].cubes_traced == ref["info"].cubes_traced and got["info"].rays == ref["info"].rays
         g.close()
     urt.close()
