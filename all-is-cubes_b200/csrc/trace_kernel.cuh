@@ -117,8 +117,9 @@ struct __align__(16) HitRecord {
     uint32_t cell;          // linear index of the Space cube
     uint32_t vidx;          // inner level: index of the voxel in the brick pool
     uint32_t flags;         // face | inner<<3 | log2(resolution)<<4
-    float thickness;        // Volumetric: length of the span inside the surface's material (world units), written when
-                            // the span is closed; Surface / Threshold: 0; < 0: the surface was never shaded
+    float thickness;        // Volumetric: length of the span inside the surface's material (world units); the record
+                            // is written when the span closes; Surface / Threshold: 0; < 0: an unused slot (the tail of
+                            // a lane's last chunk)
     uint32_t steps;         // the ray's step counter when the surface was shaded (the reference stops at the first
                             // counted step after the hit that brings the transmittance under 1/256; compositing
                             // needs the counter to restore that when the marcher's bound let the ray run on)
@@ -263,7 +264,8 @@ constexpr int N_BINS = 8;            // chord-length classes of the ray list (lo
 constexpr uint32_t HIT_CHUNK = 8;   // hit slots a lane takes from the stream at a time (one atomic per chunk)
 constexpr uint32_t HIT_NONE = 0xffffffffu;
 // Resident marching blocks per SM the register budget is sized for (65536 registers / (128 threads x 5) = 96 registers).
-// For sm_90a the Volumetric kernels then spill a few dozen bytes to L1-resident local memory; 4 blocks (no spills) were
+// The Volumetric kernels fit without spills since their state touched only at surfaces, level switches and refills
+// moved to shared memory.  With that state in registers they spilled a few dozen bytes; 4 blocks (no spills) were then
 // measured on an H100 SXM (700 W) 2.5 % faster on the C2 bench frame but 3-4 % slower on C1 and C3, so 5 stays.
 constexpr int MIN_BLOCKS_PER_SM = 5;
 // The marching loop's exits (TraceParams::event_threshold, tail_divisor, refill_threshold; launch_trace sets them):
@@ -982,17 +984,31 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     // Cold per-ray state lives in shared memory, one column per thread, so that the registers of the marching loop
     // hold only what a DDA step touches; the level switches read what they need into short-lived locals.
     __shared__ double sh_d[13][WARPS_PER_BLOCK * 32];
-    __shared__ uint32_t sh_w[14][WARPS_PER_BLOCK * 32];
+    __shared__ uint32_t sh_w[13][WARPS_PER_BLOCK * 32];
+    // Volumetric: the first 48 bytes of the pending surface's hit record (HitRecord tmx..flags), written when its span
+    // closes
+    __shared__ uint4 sh_stash[VOLUMETRIC ? 3 : 1][WARPS_PER_BLOCK * 32];
     const int tid = threadIdx.x;
 #define COLD_D(k) sh_d[k][tid]
 #define COLD_W(k) sh_w[k][tid]
+#define STASH(k) sh_stash[k][tid]
     // doubles: 0-2 origin, 3-5 direction, 6 half_over_len, 7 t_to_abs, 8-10 outer t_max while inside a block, 11 outer last_t
     // words:   0 outer index (= the Space cube of the entered block), 1-3 outer step counters, 4 outer face, 5 outer valid,
     //          6 record index (HitRecord::task), 7 first hit, 8 sky octant, 9 palette offset of the entered block,
-    //          10 log2(resolution) of it, 11 pending surface's slot, 12 its log2(1 - alpha) bound, 13 task;
+    //          10 log2(resolution) of it, 11 pending surface's log2(1 - alpha) bound, 12 task;
     //          double 12: the pending surface's entry t
-    unsigned long long dbg_t0 = 0, dbg_passes = 0, dbg_rays = 0;
-    if (P.debug_warp_times) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(dbg_t0));
+    // State that the marching loop only touches at a surface, a level switch or a refill lives in shared memory too:
+    // with it in registers the Volumetric variants spill at 96 registers.
+    __shared__ double sh_t_scale[WARPS_PER_BLOCK * 32];
+    __shared__ uint32_t sh_hits[3][WARPS_PER_BLOCK * 32];
+    __shared__ unsigned long long sh_dbg[3][WARPS_PER_BLOCK * 32];
+    unsigned long long &dbg_t0 = sh_dbg[0][tid], &dbg_passes = sh_dbg[1][tid], &dbg_rays = sh_dbg[2][tid];
+    dbg_t0 = dbg_passes = dbg_rays = 0;
+    if (P.debug_warp_times) {
+        unsigned long long t0;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+        dbg_t0 = t0;
+    }
 
     // the ray list: bins in order, longest chords first
     __shared__ uint32_t s_bin_start[N_BINS + 1];
@@ -1009,7 +1025,8 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     int st = ST_IDLE;
     double tmx = 0.0, tmy = 0.0, tmz = 0.0, last_t = 0.0;   // State::t_max, last_t_distance of the active level
     double tdx = 0.0, tdy = 0.0, tdz = 0.0;                 // t_delta (raycast.rs:769)
-    double t_scale = 1.0;                // 1 on the outer level, 1/resolution inside a block (surface.rs:385-386)
+    double &t_scale = sh_t_scale[tid];   // 1 on the outer level, 1/resolution inside a block (surface.rs:385-386)
+    t_scale = 1.0;
     uint32_t idx = 0;                    // linear index of the current cube (cells) / voxel (brick pool)
     int stx = 0, sty = 0, stz = 0;       // signed index strides of the active level
     int cx = 0, cy = 0, cz = 0;          // steps left inside the level along each axis (< 0: outside)
@@ -1024,8 +1041,11 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     // until the bound says "opaque", 0 from then on.
     float L = 0.0f;
     uint32_t steps = 0, step_limit = 1000u;
-    uint32_t n_hits = 0;                 // hit records of the current ray (consecutive slots of this lane's chunks)
-    uint32_t chunk_base = HIT_NONE, chunk_used = HIT_CHUNK;   // this lane's chunk of the hit stream
+    uint32_t &n_hits = sh_hits[0][tid];  // hit records of the current ray (consecutive slots of this lane's chunks)
+    uint32_t &chunk_base = sh_hits[1][tid], &chunk_used = sh_hits[2][tid];   // this lane's chunk of the hit stream
+    n_hits = 0;
+    chunk_base = HIT_NONE;
+    chunk_used = HIT_CHUNK;
     uint32_t ev_word = 0;
     AuxState<AUX> aux{};
     bool list_exhausted = false;         // warp-uniform: the ray list has run out (tail of the frame)
@@ -1077,18 +1097,8 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
         }
     };
 
-    // A visible surface (surface.rs:322-331, 399-409): its hit record goes to the lane's chunk of the hit stream.
-    auto emit_surface = [&](uint32_t word) {
-        uint32_t entry;   // palette entry of the surface, and what the transmittance bound needs of it
-        float2 te;
-        if (inner) {
-            entry = COLD_W(9) + word;
-            te = __ldg(S.pal_tab + entry);
-        } else {
-            const float4 t4 = __ldg(S.blk_tab + word);
-            te = make_float2(t4.x, t4.y);
-            entry = __float_as_uint(t4.z);
-        }
+    // A slot of the lane's chunk of the hit stream for the ray's next record, or HIT_NONE once the stream is full.
+    auto take_slot = [&]() -> uint32_t {
         if (chunk_used == HIT_CHUNK) {   // one atomic per HIT_CHUNK hits of this lane
             const uint32_t nb = atomicAdd(P.hit_counter, HIT_CHUNK);
             if (nb + HIT_CHUNK > P.hit_capacity) {   // (the capacity is a multiple of HIT_CHUNK)
@@ -1105,26 +1115,57 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
         if (chunk_base != HIT_NONE) {
             slot = chunk_base + chunk_used;
             chunk_used++;
-            uint4 *dst = reinterpret_cast<uint4 *>(P.hits + slot);
-            st_stream(dst, make_uint4((uint32_t)__double2loint(tmx), (uint32_t)__double2hiint(tmx),
-                                      (uint32_t)__double2loint(tmy), (uint32_t)__double2hiint(tmy)));
-            st_stream(dst + 1, make_uint4((uint32_t)__double2loint(tmz), (uint32_t)__double2hiint(tmz),
-                                          (uint32_t)__double2loint(last_t), (uint32_t)__double2hiint(last_t)));
-            st_stream(dst + 2, make_uint4(entry, inner ? COLD_W(0) : idx, idx,
-                                          (uint32_t)face | (inner ? (8u | (COLD_W(10) << 4)) : 0u)));
-            st_stream(dst + 3, make_uint4(__float_as_uint(VOLUMETRIC ? -1.0f : 0.0f), steps, COLD_W(6), HIT_NONE));
             if (n_hits == 0) COLD_W(7) = slot;
             n_hits++;
         }
-        if constexpr (VOLUMETRIC) {   // the span is closed by the next step (surface.rs:467-476)
-            COLD_W(11) = slot;
-            COLD_W(12) = __float_as_uint(te.y);
+        return slot;
+    };
+
+    // The whole 64-byte record: the caster state at the surface (q0-q2), the thickness of its span, the step counter.
+    auto store_record = [&](uint32_t slot, uint4 q0, uint4 q1, uint4 q2, float thickness) {
+        uint4 *dst = reinterpret_cast<uint4 *>(P.hits + slot);
+        st_stream(dst, q0);
+        st_stream(dst + 1, q1);
+        st_stream(dst + 2, q2);
+        st_stream(dst + 3, make_uint4(__float_as_uint(thickness), steps, COLD_W(6), HIT_NONE));
+    };
+
+    // A visible surface (surface.rs:322-331, 399-409).  Surface / Threshold: its hit record goes to the lane's chunk of
+    // the hit stream at once.  Volumetric: the record waits in the lane's stash until a later step closes the surface's
+    // span (surface.rs:467-476), possibly on the outer level after the block is left, and is written whole then; a
+    // surface whose ray stops before its span closes is never shaded, and takes no slot.
+    auto emit_surface = [&](uint32_t word) {
+        uint32_t entry;   // palette entry of the surface, and what the transmittance bound needs of it
+        float2 te;
+        if (inner) {
+            entry = COLD_W(9) + word;
+            te = __ldg(S.pal_tab + entry);
+        } else {
+            const float4 t4 = __ldg(S.blk_tab + word);
+            te = make_float2(t4.x, t4.y);
+            entry = __float_as_uint(t4.z);
+        }
+        const uint4 q0 = make_uint4((uint32_t)__double2loint(tmx), (uint32_t)__double2hiint(tmx),
+                                    (uint32_t)__double2loint(tmy), (uint32_t)__double2hiint(tmy));
+        const uint4 q1 = make_uint4((uint32_t)__double2loint(tmz), (uint32_t)__double2hiint(tmz),
+                                    (uint32_t)__double2loint(last_t), (uint32_t)__double2hiint(last_t));
+        const uint4 q2 = make_uint4(entry, inner ? COLD_W(0) : idx, idx,
+                                    (uint32_t)face | (inner ? (8u | (COLD_W(10) << 4)) : 0u));
+        if constexpr (VOLUMETRIC) {
+            STASH(0) = q0;
+            STASH(1) = q1;
+            STASH(2) = q2;
+            COLD_W(11) = __float_as_uint(te.y);
             COLD_D(12) = last_t * t_scale;
             have_pending = true;
-        } else if (P.transparency == AICB_TRANSPARENCY_THRESHOLD) {   // limit_alpha (graphics_options.rs:496-507)
-            if (te.x > P.threshold) L = F_NEG_INF;
         } else {
-            bound_factor(te.y);
+            const uint32_t slot = take_slot();
+            if (slot != HIT_NONE) store_record(slot, q0, q1, q2, 0.0f);
+            if (P.transparency == AICB_TRANSPARENCY_THRESHOLD) {   // limit_alpha (graphics_options.rs:496-507)
+                if (te.x > P.threshold) L = F_NEG_INF;
+            } else {
+                bound_factor(te.y);
+            }
         }
     };
 
@@ -1160,10 +1201,9 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
         if constexpr (VOLUMETRIC) {
             if (have_pending) {   // DepthIter: this step's t ends the pending surface's span (surface.rs:460-490)
                 const float th = fmaxf((float)((last_t * t_scale - COLD_D(12)) * COLD_D(7)), 0.0f);   // sr.rs:720-731
-                const uint32_t pend_slot = COLD_W(11);
-                const float pend_l2a = __uint_as_float(COLD_W(12));
-                if (pend_slot != HIT_NONE)
-                    *reinterpret_cast<uint2 *>(&P.hits[pend_slot].thickness) = make_uint2(__float_as_uint(th), steps);
+                const float pend_l2a = __uint_as_float(COLD_W(11));
+                const uint32_t slot = take_slot();
+                if (slot != HIT_NONE) store_record(slot, STASH(0), STASH(1), STASH(2), th);
                 bound_factor(pend_l2a == F_NEG_INF ? F_NEG_INF : th * pend_l2a);
                 have_pending = false;
             }
@@ -1197,7 +1237,7 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
             o.steps = steps;
             o.flags = COLD_W(8);
             o.n_hits = n_hits;
-            *reinterpret_cast<uint4 *>(P.task_out + COLD_W(13)) = *reinterpret_cast<const uint4 *>(&o);
+            *reinterpret_cast<uint4 *>(P.task_out + COLD_W(12)) = *reinterpret_cast<const uint4 *>(&o);
             if constexpr (AUX) { n_outer += aux.n_outer; n_inner += aux.n_inner; n_blocks += aux.n_blocks; }
             st = ST_IDLE;
         }
@@ -1233,7 +1273,7 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
                         }
                         const uint32_t task = rb.task;
                         COLD_W(6) = ri;
-                        COLD_W(13) = task;
+                        COLD_W(12) = task;
                         COLD_D(0) = rec.ox; COLD_D(1) = rec.oy; COLD_D(2) = rec.oz;
                         COLD_D(3) = rec.dx; COLD_D(4) = rec.dy; COLD_D(5) = rec.dz;
                         COLD_D(6) = rb.half_over_len;
@@ -1369,10 +1409,11 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     if (P.debug_warp_times) {
         unsigned long long t1;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-        for (int off = 16; off > 0; off >>= 1) dbg_rays += __shfl_down_sync(0xffffffffu, dbg_rays, off);
+        unsigned long long rays = dbg_rays;
+        for (int off = 16; off > 0; off >>= 1) rays += __shfl_down_sync(0xffffffffu, rays, off);
         if (lane == 0) {
             unsigned long long *d = P.debug_warp_times + 4 * (size_t)(blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5));
-            d[0] = dbg_t0; d[1] = t1; d[2] = dbg_passes; d[3] = dbg_rays;
+            d[0] = dbg_t0; d[1] = t1; d[2] = dbg_passes; d[3] = rays;
         }
     }
     // the unused rest of this lane's chunk of the hit stream: never shaded
@@ -1394,6 +1435,7 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     }
 #undef COLD_D
 #undef COLD_W
+#undef STASH
 }
 
 // Position of a hit (hit.rs:92-101) from its record: Space cube, voxel, resolution, face, and the palette entry.
@@ -1468,7 +1510,7 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
     out.next = h.next;
     out.steps = h.steps;
     out._pad[0] = out._pad[1] = 0;
-    if (h.thickness < 0.0f) return out;   // never shaded (its ray stopped before the span closed): skipped
+    if (h.thickness < 0.0f) return out;   // an unused slot: skipped
     HitGeom g;
     decode_hit(S, h, g);
     float ca = col.w;
@@ -1601,9 +1643,9 @@ __global__ void __launch_bounds__(128, SHADE_BLOCKS_PER_SM) shade_kernel(const _
     unsigned long long texels = 0;
     auto shade_one = [&](const uint32_t i) { store_shaded(P, i, shade_hit<LC>(P, s_lut, i, nullptr, texels)); };
 
-    // The hit stream holds slots that were never shaded (the unused tail of each lane's last chunk, surfaces whose ray
-    // stopped before their span closed: a quarter of the slots of the bench frame).  Each warp scans its slots 32 at
-    // a time, answers the dead ones on the spot, and queues the live ones until it has 32 of them to shade together.
+    // The hit stream holds slots that are never shaded: the unused tail of each lane's last chunk.  Each warp scans its
+    // slots 32 at a time, passes over the dead ones, and queues the live ones until it has 32 of them to shade
+    // together.
     __shared__ uint32_t s_queue[4][64];
     uint32_t *queue = s_queue[threadIdx.x >> 5];
     const uint32_t lane = threadIdx.x & 31u;
@@ -1614,18 +1656,8 @@ __global__ void __launch_bounds__(128, SHADE_BLOCKS_PER_SM) shade_kernel(const _
             const uint32_t slot = base + lane;
             base += n_warps * 32u;
             bool live = false;
-            if (slot < n) {
-                live = __ldg(&P.hits[slot].thickness) >= 0.0f;
-                if (!live) {   // encode_kernel may still walk over it (the last, never shaded surface of a ray)
-                    ShadedHit out;
-                    out.r = out.g = out.b = 0.0f;
-                    out.factor = -1.0f;
-                    out.next = P.hits[slot].next;
-                    out.steps = 0;
-                    out._pad[0] = out._pad[1] = 0;
-                    store_shaded(P, slot, out);
-                }
-            }
+            // (no ray lists a dead slot, so none is read back: a chunk is full before its link is followed)
+            if (slot < n) live = __ldg(&P.hits[slot].thickness) >= 0.0f;
             const unsigned m = __ballot_sync(0xffffffffu, live);
             if (live) queue[queued + __popc(m & ((1u << lane) - 1u))] = slot;
             queued += __popc(m);
