@@ -409,8 +409,7 @@ aicb_status aicb_group_light_fast_evaluate(aicb_group_scene *gs) {
 }
 
 aicb_status aicb_group_light_compute(aicb_group_scene *gs, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
-    if (!gs || (n && (!cubes || !out))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n > gs->scene[0]->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     ContextLocks lock(gs->group->ctx);
     LightReplicas r;
     TRY(light_replicas(gs, &r));
@@ -429,7 +428,7 @@ aicb_status aicb_group_light_evaluate(aicb_group_scene *gs, uint8_t epsilon, uin
 aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff) {
-    if (!gs || (n_edits && (!cubes || !new_ids))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     ContextLocks lock(gs->group->ctx);
     LightReplicas r;
     TRY(light_replicas(gs, &r));
@@ -446,14 +445,14 @@ aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t
 // The set of changed cubes is device 0's: device 0 applies every round and the push keeps the replicas identical, so its
 // indices and texels are every replica's.
 aicb_status aicb_group_light_changes_count(const aicb_group_scene *gs, size_t *n_changed) {
-    if (!gs || !n_changed) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     ContextLocks lock(gs->group->ctx);
     return light_changes_count(gs->scene[0], n_changed);
 }
 
 aicb_status aicb_group_light_take_changes(aicb_group_scene *gs, uint32_t *indices, uint8_t (*texels)[4], size_t capacity,
                                           size_t *n_taken) {
-    if (!gs || !n_taken) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     ContextLocks lock(gs->group->ctx);
     return light_take_changes(gs->scene[0], indices, texels, capacity, n_taken);
 }

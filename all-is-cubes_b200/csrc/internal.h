@@ -135,6 +135,45 @@ struct ChunkStreams {
     }
 };
 
+// Light propagation's static ray chart (space/light/chart) on a context's device, uploaded on first use (ensure_chart):
+// in depth-first preorder (LightNodePre, the lockstep walk); as chains, the per-node cube offsets and the Euler tour of
+// the chain tree; and the chain walk's term slots, one set per resident warp of its `walk_blocks`.
+struct LightChart {
+    DeviceBuffer pre, chains, node_rel, euler, term_scratch;
+    uint32_t nodes = 0, n_chains = 0, n_euler = 0, walk_blocks = 0;
+};
+
+// A scene's light propagation state (light.cu), in two parts: what every replica's own walks need, and what replica 0
+// alone holds and the other replicas' kernels reach through peer pointers.  Between light calls only the block records,
+// the queue and the set of changed cubes hold anything, so round buffers serve other jobs too (the accessors below).
+struct LightState {
+    DeviceBuffer blocks;   // every replica: LightBlockDev per block, uploaded with the scene (aicb_light_scene_upload)
+    struct Own {
+        DeviceBuffer sky_term;         // per chart node: the sky light its bundle collects (end_of_ray) from this sky
+        DeviceBuffer overflow;         // list positions whose chain walk overflowed (k_compute_overflow's work)
+        DeviceBuffer overflow_count;   // replicas 1..n-1: its length (replica 0's is its LightCounters::overflow)
+    } own;
+    struct Shared {
+        DeviceBuffer pending;          // per cube: queued priority (0 = not queued) — LightUpdateQueue
+        DeviceBuffer tile_max;         // per LIGHT_TILE cubes: upper bound of the queued priorities
+        DeviceBuffer list, new_light, diff;   // one round's cubes, their computed texels, their difference_priority
+        DeviceBuffer counters;         // LightCounters
+        DeviceBuffer changes;          // one bit per cube: the set of changed cubes (SpaceChange::CubeLight)
+        DeviceBuffer dirty, push_targets;     // a group's: the segments written this round, the other replicas' fields
+    } shared;
+
+    // Replica `replica` of `n_replicas`'s part(s) and the scene's light volume, where `s` (this state's scene) has none
+    // yet; the scene changes only if every step succeeds.
+    aicb_status ensure(aicb_scene *s, size_t replica, size_t n_replicas);
+
+    // replica 0's overflow list is also the round's `changed` list: its overflow is computed before k_compact_changed
+    uint32_t *changed() const { return own.overflow.get<uint32_t>(); }
+    // taking the set of changed cubes: the chunks' output positions, then the indices and texels
+    uint32_t *chunk_sums() const { return shared.diff.get<uint32_t>(); }
+    uint32_t *taken_indices() const { return shared.list.get<uint32_t>(); }
+    uint32_t *taken_texels() const { return shared.new_light.get<uint32_t>(); }
+};
+
 // Members are destroyed in reverse order of declaration: the stream and events go after the buffers.
 struct aicb_ctx {
     int device = 0;
@@ -172,15 +211,7 @@ struct aicb_ctx {
     DeviceBuffer d_task_aux;
     DeviceBuffer d_task_depth;   // per task: the UI pass's DepthBuf for the world pass (aicb_render_layers_texture)
     DeviceBuffer d_task_text;    // per task: the UI pass's CharacterBuf for the world pass (aicb_render_layers_terminal)
-    // light propagation: the static ray chart (space/light/chart), built and uploaded on first use
-    DeviceBuffer d_chart_pre;    // LightNodePre: the chart in depth-first preorder (the lockstep walk)
-    uint32_t chart_nodes = 0;
-    DeviceBuffer d_chains;       // the chart as chains, the per-node cube offsets, the Euler tour of the chain tree
-    DeviceBuffer d_node_rel;
-    DeviceBuffer d_euler;
-    uint32_t n_chains = 0, n_euler = 0;
-    DeviceBuffer d_term_scratch; // term slots of the chain walk, one set per resident warp
-    uint32_t chain_walk_blocks = 0;
+    LightChart light_chart;
     std::mutex mu;
 };
 
@@ -207,20 +238,7 @@ struct aicb_scene {
     // ---- light propagation state (light.cu) ----
     std::vector<uint16_t> h_ids;            // host mirror of Space::contents (edits are applied in order on the host)
     std::vector<uint32_t> h_block_light;    // per block: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission
-    DeviceBuffer d_light_blocks;            // LightBlockDev per block
-    DeviceBuffer d_pending;                 // per cube: queued priority (0 = not queued) — LightUpdateQueue
-    DeviceBuffer d_list;                    // work list of one round (cube indices)
-    DeviceBuffer d_new_light;               // computed texels of one round
-    DeviceBuffer d_diff;                    // difference_priority of one round
-    DeviceBuffer d_scalars;                 // [0] list length, [1] max priority, [2] max diff, [3] updates
-    DeviceBuffer d_sky_term;                // per chart node: the sky light its bundle collects (end_of_ray), for this scene's sky
-    DeviceBuffer d_changed;                 // list positions whose cube changed by more than one unit this round
-    DeviceBuffer d_tile_max;                // per LIGHT_TILE cubes: upper bound of the queued priorities
-    DeviceBuffer d_changes;                 // one bit per cube: the set of changed cubes (SpaceChange::CubeLight), kept
-                                            // across calls until the host takes it; replica 0 of a group holds it
-    // replica 0 of a group scene: the light volume's segments written this round, and the other replicas' volumes
-    DeviceBuffer d_dirty;
-    DeviceBuffer d_push_targets;
+    LightState light;
     uint32_t light_max_distance = 0;
     uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
 };
@@ -314,9 +332,9 @@ aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size
 aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
                            uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info);
 
-// light.cu: the light calls over a scene's replicas (ctx[i] is scene[i]'s context).  Validation is against replica 0,
-// before anything changes.  On a group, device 0 has peer access to every other device and they to device 0, with
-// native atomics.  After every call the replicas' light volumes are identical.
+// light.cu: the light calls over a scene's replicas (ctx[i] is scene[i]'s context).  They validate their arguments
+// other than the scenes against replica 0, before anything changes.  On a group, device 0 has peer access to every
+// other device and they to device 0, with native atomics.  After every call the replicas' light volumes are identical.
 struct LightReplicas {
     aicb_scene *const *scene;
     aicb_ctx *const *ctx;

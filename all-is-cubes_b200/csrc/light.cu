@@ -207,30 +207,26 @@ const ChainTables &chain_tables_host() {
 
 // The chart's tables on the context's device; the context takes them once every one is uploaded.
 aicb_status ensure_chart(aicb_ctx *ctx) {
-    if (ctx->d_chart_pre) return AICB_OK;
+    if (ctx->light_chart.pre) return AICB_OK;
     const ChainTables &t = chain_tables_host();
     if (t.chains.size() > (size_t)LIGHT_MAX_CHAINS || t.chains.size() >= 0x8000u)
         return aicb_fail(AICB_ERR_INVALID, "light chart has more chains than the walk's shared arrays hold");
     size_t branches = 0;
     for (const LightChain &c : t.chains) branches += c.n_children ? 1 : 0;
     if (branches > (size_t)LIGHT_MAX_BRANCHES) return aicb_fail(AICB_ERR_INVALID, "light chart has more branching chains than expected");
-    DeviceBuffer chains, node_rel, euler, term_scratch, chart_pre;
-    TRY(chains.upload(t.chains));
-    TRY(node_rel.upload(t.node_rel));
-    TRY(euler.upload(t.euler));
+    LightChart c;
+    TRY(c.chains.upload(t.chains));
+    TRY(c.node_rel.upload(t.node_rel));
+    TRY(c.euler.upload(t.euler));
+    c.walk_blocks = (uint32_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM;
     // one set of term slots per resident warp of the chain walk
-    TRY(term_scratch.ensure((size_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM * 4 * LIGHT_WARP_SCRATCH_F4 * sizeof(float4)));
+    TRY(c.term_scratch.ensure((size_t)c.walk_blocks * 4 * LIGHT_WARP_SCRATCH_F4 * sizeof(float4)));
     const std::vector<LightNodePre> &pre = chart_preorder_host();
-    TRY(chart_pre.upload(pre));
-    ctx->d_chains = std::move(chains);
-    ctx->d_node_rel = std::move(node_rel);
-    ctx->d_euler = std::move(euler);
-    ctx->d_term_scratch = std::move(term_scratch);
-    ctx->d_chart_pre = std::move(chart_pre);
-    ctx->n_chains = (uint32_t)t.chains.size();
-    ctx->n_euler = (uint32_t)t.euler.size();
-    ctx->chain_walk_blocks = (uint32_t)ctx->num_sms * CHAIN_WALK_BLOCKS_PER_SM;
-    ctx->chart_nodes = (uint32_t)pre.size();
+    TRY(c.pre.upload(pre));
+    c.nodes = (uint32_t)pre.size();
+    c.n_chains = (uint32_t)t.chains.size();
+    c.n_euler = (uint32_t)t.euler.size();
+    ctx->light_chart = std::move(c);
     return AICB_OK;
 }
 
@@ -263,18 +259,15 @@ __global__ void k_find_max(const LightParams P, uint32_t n_tiles) {
     uint32_t m = 0;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_tiles; i += gridDim.x * blockDim.x) m = max(m, P.tile_max[i]);
     for (int off = 16; off > 0; off >>= 1) m = max(m, __shfl_down_sync(0xffffffffu, m, off));
-    if ((threadIdx.x & 31) == 0 && m) atomicMax(P.scalars + 1, m);
+    if ((threadIdx.x & 31) == 0 && m) atomicMax(&P.counters->priority, m);
 }
 
-// scalars: [0] cubes gathered this round, [1] highest queued priority this round, [2] largest difference applied
-// (accumulated), [3] cube updates (accumulated), [4..5] chart nodes visited (64-bit, accumulated).
-// A round's kernels read the round's priority and count from device memory, so rounds are queued back to back
-// without a host round trip; a round whose priority is already <= epsilon does nothing.
+// A round whose priority is already <= epsilon does nothing.
 // One block per tile: the cubes of a tile reach the list in index order (block-wide scan), so 32 consecutive list
 // entries are neighbours along z — what the lockstep walk wants.
 __global__ void __launch_bounds__(256) k_gather(const LightParams P, uint32_t n_tiles) {
     __shared__ uint32_t s_part[8], s_max[8], s_base;
-    const uint32_t prio = P.scalars[1];
+    const uint32_t prio = P.counters->priority;
     if (prio <= P.epsilon_priority) return;
     const uint32_t n_words = (P.volume + 3) / 4;
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -318,7 +311,7 @@ __global__ void __launch_bounds__(256) k_gather(const LightParams P, uint32_t n_
         if (threadIdx.x == 0) {
             uint32_t total = 0, m = 0;
             for (int i = 0; i < 8; i++) { const uint32_t c = s_part[i]; s_part[i] = total; total += c; m = max(m, s_max[i]); }
-            s_base = total ? atomicAdd(P.scalars + 0, total) : 0u;
+            s_base = total ? atomicAdd(&P.counters->gathered, total) : 0u;
             P.tile_max[tile] = m;
         }
         __syncthreads();
@@ -346,11 +339,11 @@ __global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(c
     const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     ChainShared &sh = s_sh[wib];
     float4 *terms = P.term_scratch + (size_t)(blockIdx.x * 4 + wib) * LIGHT_WARP_SCRATCH_F4;
-    if (!explicit_cubes) n = MARK ? P.scalars[6] : P.scalars[0];
+    if (!explicit_cubes) n = MARK ? P.counters->changed : P.counters->gathered;
     unsigned long long total_visits = 0;
     for (;;) {
         uint32_t item = 0;
-        if (lane == 0) item = atomicAdd(P.scalars + (MARK ? 8 : 7), 1u);
+        if (lane == 0) item = atomicAdd(MARK ? &P.counters->mark_work : &P.counters->compute_work, 1u);
         item = __shfl_sync(0xffffffffu, item, 0);
         if (item >= n) break;
         const uint32_t i = MARK ? P.changed[item] : item;   // position in the round's list
@@ -367,7 +360,7 @@ __global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(c
         }
         total_visits += visits;
     }
-    if (!MARK && lane == 0 && total_visits) atomicAdd(reinterpret_cast<unsigned long long *>(P.scalars + 4), total_visits);
+    if (!MARK && lane == 0 && total_visits) atomicAdd(&P.counters->node_visits, total_visits);
 }
 
 // 8 CTAs of 4 warps per SM (64 registers; the records requested ahead spill to L1-resident local memory): the walk is
@@ -397,7 +390,7 @@ __global__ void __launch_bounds__(128, LOCKSTEP_MIN_BLOCKS) k_compute_overflow(c
         total_visits += visits;
     }
     for (int off = 16; off > 0; off >>= 1) total_visits += __shfl_down_sync(0xffffffffu, total_visits, off);
-    if (lane == 0 && total_visits) atomicAdd(reinterpret_cast<unsigned long long *>(P.scalars + 4), total_visits);
+    if (lane == 0 && total_visits) atomicAdd(&P.counters->node_visits, total_visits);
 }
 
 // A texel of device 0's light volume was written: its 32-cube segment goes to the other replicas (k_push).
@@ -415,19 +408,19 @@ __device__ __forceinline__ void mark_changed(const LightParams &P, uint32_t idx)
 // GROUP: device 0 of a group also marks every texel it writes dirty.
 template <bool GROUP>
 __global__ void k_apply(const LightParams P) {
-    const uint32_t n = P.scalars[0];
+    const uint32_t n = P.counters->gathered;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint32_t idx = P.list[i];
     uint32_t *light = const_cast<uint32_t *>(P.scene.light);
     const uint32_t old = light[idx], nv = P.new_light[i];
     const int d = difference_priority(nv, old);
     P.diff[i] = (uint8_t)d;
-    atomicAdd(P.scalars + 3, 1u);
+    atomicAdd(&P.counters->updates, 1u);
     if (d > 0) {
         light[idx] = nv;
         mark_changed(P, idx);
         if (GROUP) mark_dirty(P, idx);
-        atomicMax(P.scalars + 2, (uint32_t)d);
+        atomicMax(&P.counters->max_diff, (uint32_t)d);
         int x, y, z;
         cube_of(P.scene, idx, x, y, z);
         const float *lut = P.scene.tables;
@@ -479,7 +472,7 @@ __global__ void __launch_bounds__(256) k_push(const LightParams P, uint32_t *con
 // k_walk_chains<true> walks the chart only for cubes that need it.
 __global__ void __launch_bounds__(256) k_compact_changed(const LightParams P) {
     __shared__ uint32_t s_part[8], s_base;
-    const uint32_t n = P.scalars[0];
+    const uint32_t n = P.counters->gathered;
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     for (uint32_t base = blockIdx.x * 256u; base < n; base += gridDim.x * 256u) {
         const uint32_t i = base + threadIdx.x;
@@ -494,7 +487,7 @@ __global__ void __launch_bounds__(256) k_compact_changed(const LightParams P) {
         if (threadIdx.x == 0) {
             uint32_t total = 0;
             for (int k = 0; k < 8; k++) { const uint32_t c = s_part[k]; s_part[k] = total; total += c; }
-            s_base = total ? atomicAdd(P.scalars + 6, total) : 0u;
+            s_base = total ? atomicAdd(&P.counters->changed, total) : 0u;
         }
         __syncthreads();
         if (keep) P.changed[s_base + s_part[wid] + inc - 1] = i;
@@ -654,160 +647,84 @@ __global__ void __launch_bounds__(256) k_changes_emit(uint32_t *bits, uint32_t n
     }
 }
 
-LightParams make_params(aicb_scene *s) {
+// Replica i's parameters: its own field, blocks, chart, term slots and overflow list with its count; replica 0's queue,
+// round buffers, counters and sets (peer pointers on the other replicas).  Replica 0 takes both parts from itself.
+LightParams light_params(LightReplicas r, size_t i) {
+    const aicb_scene *s = r.scene[i];
+    const LightState::Own &own = s->light.own;
+    const LightState::Shared &root = r.scene[0]->light.shared;
+    const LightChart &chart = r.ctx[i]->light_chart;
     LightParams P;
     std::memset(&P, 0, sizeof P);
     P.scene = s->ds;
-    P.blocks = s->d_light_blocks.get<LightBlockDev>();
-    P.chart_pre = s->ctx->d_chart_pre.get<LightNodePre>();
-    P.sky_term = s->d_sky_term.get<float4>();
-    P.chains = s->ctx->d_chains.get<LightChain>();
-    P.node_rel = s->ctx->d_node_rel.get<uchar4>();
-    P.euler = s->ctx->d_euler.get<uint16_t>();
-    P.n_chains = s->ctx->n_chains;
-    P.n_euler = s->ctx->n_euler;
-    P.term_scratch = s->ctx->d_term_scratch.get<float4>();
-    P.overflow = s->d_changed.get<uint32_t>();   // (k_walk_chains<false>'s overflow list and k_walk_chains<true>'s work list are never live together)
-    P.chart_nodes = s->ctx->chart_nodes;
-    P.tile_max = s->d_tile_max.get<uint32_t>();
-    P.changed = s->d_changed.get<uint32_t>();
-    P.pending = s->d_pending.get<uint8_t>();
-    P.list = s->d_list.get<uint32_t>();
-    P.new_light = s->d_new_light.get<uint32_t>();
-    P.diff = s->d_diff.get<uint8_t>();
-    P.scalars = s->d_scalars.get<uint32_t>();
-    P.overflow_count = P.scalars + 9;
-    P.dirty = s->d_dirty.get<uint32_t>();
-    P.changes = s->d_changes.get<uint32_t>();
+    P.blocks = s->light.blocks.get<LightBlockDev>();
+    P.chart_pre = chart.pre.get<LightNodePre>();
+    P.sky_term = own.sky_term.get<float4>();
+    P.chains = chart.chains.get<LightChain>();
+    P.node_rel = chart.node_rel.get<uchar4>();
+    P.euler = chart.euler.get<uint16_t>();
+    P.n_chains = chart.n_chains;
+    P.n_euler = chart.n_euler;
+    P.term_scratch = chart.term_scratch.get<float4>();
+    P.overflow = own.overflow.get<uint32_t>();
+    P.chart_nodes = chart.nodes;
+    P.tile_max = root.tile_max.get<uint32_t>();
+    P.changed = r.scene[0]->light.changed();
+    P.pending = root.pending.get<uint8_t>();
+    P.list = root.list.get<uint32_t>();
+    P.new_light = root.new_light.get<uint32_t>();
+    P.diff = root.diff.get<uint8_t>();
+    P.counters = root.counters.get<LightCounters>();
+    P.overflow_count = i == 0 ? &P.counters->overflow : own.overflow_count.get<uint32_t>();
+    P.dirty = root.dirty.get<uint32_t>();
+    P.changes = root.changes.get<uint32_t>();
     P.volume = (uint32_t)s->volume;
     P.max_distance = s->light_max_distance;
     return P;
 }
 
-// Every replica's parameters: its own field, blocks, chart, term slots and overflow list; device 0's queue, round list,
-// results and counters (peer pointers).
-std::vector<LightParams> replica_params(LightReplicas r) {
-    std::vector<LightParams> P;
-    for (size_t i = 0; i < r.n; i++) {
-        LightParams p = make_params(r.scene[i]);
-        if (i > 0) {
-            const LightParams &p0 = P[0];
-            p.tile_max = p0.tile_max;
-            p.changed = p0.changed;
-            p.pending = p0.pending;
-            p.list = p0.list;
-            p.new_light = p0.new_light;
-            p.diff = p0.diff;
-            p.scalars = p0.scalars;
-        }
-        P.push_back(p);
-    }
-    return P;
-}
-
-// The scene's light state, built in locals: the scene takes them once every step has succeeded.  `queue`: the
-// priority queue, a round's lists and the set of changed cubes, which only replica 0 of a group holds.
-aicb_status ensure_light_state(aicb_scene *s, bool queue = true) {
-    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
-    TRY(ensure_chart(s->ctx));
-    DeviceBuffer light, sky_term, pending, list, new_light, diff, scalars, tile_max, changed, changes;
-    const size_t change_bytes = (s->volume + 31) / 32 * 4;
-    if (!s->d_light) {  // a scene created without a light volume starts all NO_RAYS (initialize_light, updater.rs:628-656)
-        const std::vector<uint32_t> init(s->volume, TX_NO_RAYS);
-        TRY(light.upload(init.data(), s->volume * 4, 16));
-    }
-    if (!s->d_sky_term) {
-        // end_of_ray (updater.rs:889-924) without the lane's alpha and bundle weight: per chart node, the sky light
-        // its bundle collects — the same f32 operations, in the same order, as the reference evaluates per ray end
-        const std::vector<LightNodePre> &pre = chart_preorder_host();
-        float lut[256];
-        lut[0] = 0.0f;
-        for (int i = 1; i < 256; i++) lut[i] = (float)std::exp2((double)(((float)i - 144.0f) / 10.0f));
-        auto psc = [](float v) { return v > 0.0f ? v : 0.0f; };
-        auto psm = [](float a, float b) { float v = a * b; return (v != v) ? 0.0f : v; };
-        std::vector<float4> sky(pre.size());
-        for (size_t k = 0; k < pre.size(); k++) {
-            const float *cw = pre[k].w;
-            float t[6][3];
-            for (int f = 0; f < 6; f++) {
-                const uint32_t tx = s->ds.sky_faces[f];
-                const float kk = psc(cw[f]);
-                t[f][0] = psm(lut[tx & 255], kk);
-                t[f][1] = psm(lut[(tx >> 8) & 255], kk);
-                t[f][2] = psm(lut[(tx >> 16) & 255], kk);
-            }
-            const float kr = psc(1.0f / ((cw[0] + cw[3]) + (cw[1] + cw[4]) + (cw[2] + cw[5])));
-            float c[3];
-            for (int i = 0; i < 3; i++) c[i] = psm((t[0][i] + t[3][i]) + (t[1][i] + t[4][i]) + (t[2][i] + t[5][i]), kr);
-            sky[k] = make_float4(c[0], c[1], c[2], 0.0f);
-        }
-        TRY(sky_term.upload(sky));
-    }
-    const bool work = queue && !s->d_pending;
-    const bool overflow = !s->d_changed;   // the overflow list and the scalars: every replica's
-    if (work) {
-        TRY(pending.ensure(s->volume + 16));
-        CU(cudaMemset(pending.get(), 0, s->volume + 16));
-        TRY(list.ensure(s->volume * 4 + 16));
-        TRY(new_light.ensure(s->volume * 4 + 16));
-        TRY(diff.ensure(s->volume + 16));
-        TRY(changes.ensure(change_bytes));
-        CU(cudaMemset(changes.get(), 0, change_bytes));
-    }
-    if (overflow) TRY(scalars.ensure(16 * 4));
-    if (work) TRY(tile_max.ensure(((s->volume + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
-    if (overflow) TRY(changed.ensure(s->volume * 4 + 16));
-    if (light) {
-        s->d_light = std::move(light);
-        s->ds.light = s->d_light.get<uint32_t>();
-        s->device_bytes += s->volume * 4;
-    }
-    if (sky_term) {
-        s->d_sky_term = std::move(sky_term);
-        s->device_bytes += chart_preorder_host().size() * sizeof(float4);
-    }
-    if (work) {
-        s->d_pending = std::move(pending);
-        s->d_list = std::move(list);
-        s->d_new_light = std::move(new_light);
-        s->d_diff = std::move(diff);
-        s->d_tile_max = std::move(tile_max);
-        s->d_changes = std::move(changes);
-        s->device_bytes += s->volume * 10 + change_bytes;
-    }
-    if (overflow) {
-        s->d_scalars = std::move(scalars);
-        s->d_changed = std::move(changed);
-        s->device_bytes += s->volume * 4;
-    }
-    return AICB_OK;
-}
-
-// Every replica's light state (the queue on replica 0 only) and, on a group, what a round needs beyond one context's:
-// replica 0's dirty bits, and the other replicas' light volumes as push targets.
+// Every replica's light state and, on a group, replica 0's push targets: the other replicas' light volumes.
 aicb_status ensure_replicas(LightReplicas r) {
     for (size_t i = 0; i < r.n; i++) {
-        CU(cudaSetDevice(r.scene[i]->ctx->device));
-        TRY(ensure_light_state(r.scene[i], i == 0));
+        CU(cudaSetDevice(r.ctx[i]->device));
+        TRY(r.scene[i]->light.ensure(r.scene[i], i, r.n));
     }
     if (r.n == 1) return AICB_OK;
-    aicb_scene *s = r.scene[0];
-    CU(cudaSetDevice(s->ctx->device));
-    if (!s->d_dirty) {
-        const size_t bytes = (s->volume + 1023) / 1024 * 4 + 16;
-        DeviceBuffer dirty;
-        TRY(dirty.ensure(bytes));
-        CU(cudaMemset(dirty.get(), 0, bytes));
-        s->d_dirty = std::move(dirty);
-        s->device_bytes += bytes;
-    }
     std::vector<uint32_t *> targets;
     for (size_t i = 1; i < r.n; i++) targets.push_back(const_cast<uint32_t *>(r.scene[i]->ds.light));
-    TRY(s->d_push_targets.ensure(targets.size() * sizeof(uint32_t *)));
-    CU(cudaMemcpy(s->d_push_targets.get(), targets.data(), targets.size() * sizeof(uint32_t *), cudaMemcpyHostToDevice));
+    CU(cudaSetDevice(r.ctx[0]->device));
+    CU(cudaMemcpy(r.scene[0]->light.shared.push_targets.get(), targets.data(), targets.size() * sizeof(uint32_t *),
+                  cudaMemcpyHostToDevice));
     // device 0 writes the other replicas' volumes: after what their streams hold (aicb_scene_update_cubes is queued)
     return fan_in(r.ctx, r.n);
 }
+
+// Every replica's walk of one form, replica i against its own field on its own context: the compute form (the round's
+// list, or the n `explicit_cubes`) with the lockstep walk of the overflow it met, or the mark form.  On a group the
+// walks start behind device 0's stream, and device 0's stream waits for them.
+aicb_status walk(LightReplicas r, const std::vector<LightParams> &RP, bool mark, uint32_t n = 0,
+                 const int32_t *explicit_cubes = nullptr) {
+    const bool group = r.n > 1;
+    if (group) TRY(fan_out(r.ctx, r.n));
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_ctx *c = r.ctx[i];
+        cudaStream_t cs = c->stream.get();
+        if (group) CU(cudaSetDevice(c->device));
+        if (mark) {
+            k_walk_chains<true><<<c->light_chart.walk_blocks, 128, 0, cs>>>(RP[i], 0, nullptr);
+            continue;
+        }
+        if (i > 0) CU(cudaMemsetAsync(RP[i].overflow_count, 0, 4, cs));   // (replica 0's: with its other counters)
+        k_walk_chains<false><<<c->light_chart.walk_blocks, 128, 0, cs>>>(RP[i], n, explicit_cubes);
+        k_compute_overflow<<<c->num_sms * 8, 128, 0, cs>>>(RP[i], explicit_cubes);
+    }
+    return group ? fan_in(r.ctx, r.n) : AICB_OK;
+}
+
+// A round restarts the counters of its list (gathered, priority) and of its walks (changed .. overflow).
+constexpr size_t ROUND_LIST_COUNTERS = offsetof(LightCounters, max_diff);
+constexpr size_t ROUND_WALK_COUNTERS =
+    offsetof(LightCounters, overflow) + sizeof(uint32_t) - offsetof(LightCounters, changed);
 
 // evaluate_light (space.rs:1496-1527): rounds until the highest queued priority is <= from_difference(epsilon).
 // A round: device 0 gathers the cubes of the round's band from its queue; every replica walks a share of them against
@@ -821,63 +738,45 @@ aicb_status propagate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, 
     aicb_ctx *ctx = s->ctx;
     cudaStream_t st = ctx->stream.get();
     const bool group = r.n > 1;
-    std::vector<LightParams> RP = replica_params(r);
-    for (LightParams &p : RP) p.epsilon_priority = (uint32_t)epsilon / 2 + 1;
+    std::vector<LightParams> RP;
+    for (size_t i = 0; i < r.n; i++) {
+        RP.push_back(light_params(r, i));
+        RP.back().epsilon_priority = (uint32_t)epsilon / 2 + 1;
+    }
     const LightParams &P = RP[0];
     const int blocks = ctx->num_sms * 8;
     const int wide = ctx->num_sms * 8;    // 128-thread blocks of k_compute_overflow and k_apply (grid-stride)
     const uint32_t n_tiles = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
     uint64_t total = 0, visits = 0, rounds = 0;
     uint32_t maxd = 0;
-    // every replica's walk of one form: replica i against its own field, on its own context
-    auto walk = [&](bool mark) -> aicb_status {
-        for (size_t i = 0; i < r.n; i++) {
-            aicb_ctx *c = r.scene[i]->ctx;
-            cudaStream_t cs = c->stream.get();
-            if (group) CU(cudaSetDevice(c->device));
-            if (mark) {
-                k_walk_chains<true><<<c->chain_walk_blocks, 128, 0, cs>>>(RP[i], 0, nullptr);
-                continue;
-            }
-            if (i > 0) CU(cudaMemsetAsync(RP[i].overflow_count, 0, 4, cs));   // (device 0's: with the round's counters)
-            k_walk_chains<false><<<c->chain_walk_blocks, 128, 0, cs>>>(RP[i], 0, nullptr);
-            k_compute_overflow<<<c->num_sms * 8, 128, 0, cs>>>(RP[i], nullptr);
-        }
-        if (group) CU(cudaSetDevice(ctx->device));
-        return AICB_OK;
-    };
     CU(cudaEventRecord(ctx->ev0.get(), st));
-    CU(cudaMemsetAsync(P.scalars, 0, 16 * 4, st));
+    CU(cudaMemsetAsync(P.counters, 0, sizeof(LightCounters), st));
     k_tile_rebuild<<<blocks, 256, 0, st>>>(P, n_tiles);   // (fast_evaluate / edits write the priority bytes directly)
     const int ROUNDS_PER_SYNC = 8;
     for (int batch = 0; batch < 100000; batch++) {
         for (int round = 0; round < ROUNDS_PER_SYNC; round++) {
-            CU(cudaMemsetAsync(P.scalars, 0, 2 * 4, st));   // this round's count and priority
-            CU(cudaMemsetAsync(P.scalars + 6, 0, 4 * 4, st));   // ... its count of changed cubes, the two work counters, the overflow count
+            CU(cudaMemsetAsync(P.counters, 0, ROUND_LIST_COUNTERS, st));
+            CU(cudaMemsetAsync(&P.counters->changed, 0, ROUND_WALK_COUNTERS, st));
             k_find_max<<<16, 256, 0, st>>>(P, n_tiles);
             k_gather<<<blocks, 256, 0, st>>>(P, n_tiles);
-            if (group) TRY(fan_out(r.ctx, r.n));
-            TRY(walk(false));
-            if (group) TRY(fan_in(r.ctx, r.n));
+            TRY(walk(r, RP, false));
             if (group) k_apply<true><<<wide, 128, 0, st>>>(P);
             else k_apply<false><<<wide, 128, 0, st>>>(P);
             k_compact_changed<<<blocks, 256, 0, st>>>(P);
-            if (group) {
-                k_push<<<blocks, 256, 0, st>>>(P, s->d_push_targets.get<uint32_t *const>(), (uint32_t)(r.n - 1));
-                TRY(fan_out(r.ctx, r.n));
-            }
-            TRY(walk(true));
-            if (group) TRY(fan_in(r.ctx, r.n));   // (the next round's queue holds every replica's marks)
+            if (group)
+                k_push<<<blocks, 256, 0, st>>>(P, s->light.shared.push_targets.get<uint32_t *const>(),
+                                               (uint32_t)(r.n - 1));
+            TRY(walk(r, RP, true));   // (on a group, the next round's queue holds every replica's marks)
         }
-        uint32_t h[8];
-        CU(cudaMemcpyAsync(h, P.scalars, 8 * 4, cudaMemcpyDeviceToHost, st));
+        LightCounters h;
+        CU(cudaMemcpyAsync(&h, P.counters, sizeof h, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         CU(cudaGetLastError());
-        total = h[3];
-        visits = (uint64_t)h[4] | ((uint64_t)h[5] << 32);
-        maxd = h[2];
+        total = h.updates;
+        visits = h.node_visits;
+        maxd = h.max_diff;
         rounds += ROUNDS_PER_SYNC;
-        if (h[1] <= P.epsilon_priority) break;   // the batch's last round found nothing above epsilon
+        if (h.priority <= P.epsilon_priority) break;   // the batch's last round found nothing above epsilon
     }
     CU(cudaEventRecord(ctx->ev1.get(), st));
     CU(cudaEventSynchronize(ctx->ev1.get()));
@@ -911,6 +810,84 @@ LightBlockDev light_block(const aicb_block_desc &b) {
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------
+// a scene's light state (internal.h)
+// ---------------------------------------------------------------------------------------------
+aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas) {
+    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    TRY(ensure_chart(s->ctx));
+    const size_t vol = s->volume;
+    const size_t change_bytes = (vol + 31) / 32 * 4, dirty_bytes = (vol + 1023) / 1024 * 4 + 16;
+    const bool add_own = !own.sky_term, add_shared = replica == 0 && !shared.pending, group = n_replicas > 1;
+    DeviceBuffer light;
+    Own o;
+    Shared sh;
+    if (!s->d_light) {  // a scene created without a light volume starts all NO_RAYS (initialize_light, updater.rs:628-656)
+        const std::vector<uint32_t> init(vol, TX_NO_RAYS);
+        TRY(light.upload(init.data(), vol * 4, 16));
+    }
+    if (add_own) {
+        // end_of_ray (updater.rs:889-924) without the lane's alpha and bundle weight: per chart node, the sky light
+        // its bundle collects — the same f32 operations, in the same order, as the reference evaluates per ray end
+        const std::vector<LightNodePre> &pre = chart_preorder_host();
+        float lut[256];
+        lut[0] = 0.0f;
+        for (int i = 1; i < 256; i++) lut[i] = (float)std::exp2((double)(((float)i - 144.0f) / 10.0f));
+        auto psc = [](float v) { return v > 0.0f ? v : 0.0f; };
+        auto psm = [](float a, float b) { float v = a * b; return (v != v) ? 0.0f : v; };
+        std::vector<float4> sky(pre.size());
+        for (size_t k = 0; k < pre.size(); k++) {
+            const float *cw = pre[k].w;
+            float t[6][3];
+            for (int f = 0; f < 6; f++) {
+                const uint32_t tx = s->ds.sky_faces[f];
+                const float kk = psc(cw[f]);
+                t[f][0] = psm(lut[tx & 255], kk);
+                t[f][1] = psm(lut[(tx >> 8) & 255], kk);
+                t[f][2] = psm(lut[(tx >> 16) & 255], kk);
+            }
+            const float kr = psc(1.0f / ((cw[0] + cw[3]) + (cw[1] + cw[4]) + (cw[2] + cw[5])));
+            float c[3];
+            for (int i = 0; i < 3; i++) c[i] = psm((t[0][i] + t[3][i]) + (t[1][i] + t[4][i]) + (t[2][i] + t[5][i]), kr);
+            sky[k] = make_float4(c[0], c[1], c[2], 0.0f);
+        }
+        TRY(o.sky_term.upload(sky));
+        TRY(o.overflow.ensure(vol * 4 + 16));
+        if (replica > 0) TRY(o.overflow_count.ensure(4));
+    }
+    if (add_shared) {
+        TRY(sh.pending.ensure(vol + 16));
+        CU(cudaMemset(sh.pending.get(), 0, vol + 16));
+        TRY(sh.tile_max.ensure(((vol + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
+        TRY(sh.list.ensure(vol * 4 + 16));
+        TRY(sh.new_light.ensure(vol * 4 + 16));
+        TRY(sh.diff.ensure(vol + 16));
+        TRY(sh.counters.ensure(sizeof(LightCounters)));
+        TRY(sh.changes.ensure(change_bytes));
+        CU(cudaMemset(sh.changes.get(), 0, change_bytes));
+        if (group) {
+            TRY(sh.dirty.ensure(dirty_bytes));
+            CU(cudaMemset(sh.dirty.get(), 0, dirty_bytes));
+            TRY(sh.push_targets.ensure((n_replicas - 1) * sizeof(uint32_t *)));
+        }
+    }
+    // (aicb_scene_device_bytes leaves out the tile bounds, the counters, the overflow count and the push targets)
+    if (light) {
+        s->d_light = std::move(light);
+        s->ds.light = s->d_light.get<uint32_t>();
+        s->device_bytes += vol * 4;
+    }
+    if (add_own) {
+        own = std::move(o);
+        s->device_bytes += chart_preorder_host().size() * sizeof(float4) + vol * 4;
+    }
+    if (add_shared) {
+        shared = std::move(sh);
+        s->device_bytes += vol * 10 + change_bytes + (group ? dirty_bytes : 0);
+    }
+    return AICB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // called from aicb200.cu
 // ---------------------------------------------------------------------------------------------
 aicb_status aicb_light_scene_upload(aicb_scene *s, const aicb_scene_desc *d) {
@@ -923,7 +900,7 @@ aicb_status aicb_light_scene_upload(aicb_scene *s, const aicb_scene_desc *d) {
         s->h_block_light[i] = lb[i].flags;
     }
     if (!lb.empty()) {
-        TRY(s->d_light_blocks.upload(lb));
+        TRY(s->light.blocks.upload(lb));
         s->device_bytes += lb.size() * sizeof(LightBlockDev);
     }
     return AICB_OK;
@@ -934,8 +911,8 @@ aicb_status aicb_light_blocks_update(aicb_scene *s, const uint16_t *indices, con
     for (size_t i = 0; i < n; i++) {
         const LightBlockDev o = light_block(descs[i]);
         if (indices[i] < s->h_block_light.size()) s->h_block_light[indices[i]] = o.flags;
-        if (s->d_light_blocks)
-            CU(cudaMemcpy(s->d_light_blocks.get<LightBlockDev>() + indices[i], &o, sizeof o, cudaMemcpyHostToDevice));
+        if (s->light.blocks)
+            CU(cudaMemcpy(s->light.blocks.get<LightBlockDev>() + indices[i], &o, sizeof o, cudaMemcpyHostToDevice));
     }
     return AICB_OK;
 }
@@ -947,7 +924,7 @@ aicb_status light_fast_evaluate(LightReplicas r) {
     TRY(ensure_replicas(r));
     aicb_scene *s = r.scene[0];
     cudaStream_t stream = s->ctx->stream.get();
-    LightParams P = make_params(s);
+    LightParams P = light_params(r, 0);
     const uint32_t cols = (uint32_t)s->ds.size[0] * (uint32_t)s->ds.size[2];
     if (cols) k_fast_evaluate<<<(cols + 127) / 128, 128, 0, stream>>>(P);
     CU(cudaGetLastError());
@@ -961,39 +938,31 @@ aicb_status light_fast_evaluate(LightReplicas r) {
 // The cubes are split across the replicas by device 0's work counter; every replica computes the overflow of its own
 // walks; the outputs are device 0's, in input order.
 aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
+    aicb_scene *s = r.scene[0];
+    if (n && (!cubes || !out)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
     TRY(ensure_replicas(r));
     if (!n) return AICB_OK;
-    aicb_scene *s = r.scene[0];
-    const bool group = r.n > 1;
-    const std::vector<LightParams> RP = replica_params(r);
+    std::vector<LightParams> RP;
+    for (size_t i = 0; i < r.n; i++) RP.push_back(light_params(r, i));
     const LightParams &P = RP[0];
     cudaStream_t stream = s->ctx->stream.get();
     DeviceBuffer d_cubes;   // on device 0; the other replicas read it over peer access
     TRY(d_cubes.upload(cubes, n * 12));
-    const int32_t *explicit_cubes = d_cubes.get<int32_t>();
-    CU(cudaMemsetAsync(P.scalars, 0, 16 * 4, stream));
-    if (group) TRY(fan_out(r.ctx, r.n));
-    for (size_t i = 0; i < r.n; i++) {
-        aicb_ctx *c = r.scene[i]->ctx;
-        cudaStream_t cs = c->stream.get();
-        if (group) CU(cudaSetDevice(c->device));
-        if (i > 0) CU(cudaMemsetAsync(RP[i].overflow_count, 0, 4, cs));
-        k_walk_chains<false><<<c->chain_walk_blocks, 128, 0, cs>>>(RP[i], (uint32_t)n, explicit_cubes);
-        k_compute_overflow<<<c->num_sms * 8, 128, 0, cs>>>(RP[i], explicit_cubes);
-    }
-    if (group) TRY(fan_in(r.ctx, r.n));
-    uint32_t h[16];
+    CU(cudaMemsetAsync(P.counters, 0, sizeof(LightCounters), stream));
+    TRY(walk(r, RP, false, (uint32_t)n, d_cubes.get<int32_t>()));
+    LightCounters h;
     CU(cudaMemcpyAsync(out, P.new_light, n * 4, cudaMemcpyDeviceToHost, stream));
-    CU(cudaMemcpyAsync(h, P.scalars, sizeof h, cudaMemcpyDeviceToHost, stream));
+    CU(cudaMemcpyAsync(&h, P.counters, sizeof h, cudaMemcpyDeviceToHost, stream));
     CU(cudaStreamSynchronize(stream));
-    uint64_t overflowed = h[9];
+    uint64_t overflowed = h.overflow;
     for (size_t i = 1; i < r.n; i++) {   // (every replica's stream is done: device 0's waited for them)
         uint32_t c = 0;
         CU(cudaMemcpy(&c, RP[i].overflow_count, 4, cudaMemcpyDeviceToHost));
         overflowed += c;
     }
     s->light_stats[0] = n;
-    s->light_stats[1] = (uint64_t)h[4] | ((uint64_t)h[5] << 32);
+    s->light_stats[1] = h.node_visits;
     s->light_stats[2] = overflowed;   // cubes that took the lockstep walk (a chain with more terms than its slots)
     s->light_stats[3] = 0;
     return AICB_OK;
@@ -1010,6 +979,7 @@ aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_d
 // mirror's, the cells' and the light's changes; only replica 0 holds the queue.
 aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
+    if (n_edits && (!cubes || !new_ids)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     TRY(ensure_replicas(r));
     aicb_scene *s = r.scene[0];
     const DeviceScene &ds = s->ds;
@@ -1074,7 +1044,7 @@ aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3],
             DeviceBuffer d_ops;
             TRY(d_ops.ensure(flat.size() * sizeof(EditOp)));
             CU(cudaMemcpyAsync(d_ops.get(), flat.data(), flat.size() * sizeof(EditOp), cudaMemcpyHostToDevice, stream));
-            LightParams P = make_params(ri);
+            LightParams P = light_params(r, i);
             k_edits<<<(unsigned)((flat.size() + 127) / 128), 128, 0, stream>>>(P, d_ops.get<EditOp>(), (uint32_t)flat.size(),
                                                                                ds.wide_cells, i == 0);
             CU(cudaStreamSynchronize(stream));
@@ -1095,14 +1065,14 @@ aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     return AICB_OK;
 }
 
-// The size of the set of changed cubes (kernels 1 and 2 of the take), behind everything queued on the context's stream.
-// The chunks' output positions stay in the round's `diff` buffer, which no light call keeps anything in between calls.
+// The size of the set of changed cubes (kernels 1 and 2 of the take), behind everything queued on the context's stream;
+// the chunks' output positions stay in chunk_sums() for k_changes_emit.
 static aicb_status count_changes(const aicb_scene *s, uint32_t *n) {
     const uint32_t n_words = (uint32_t)((s->volume + 31) / 32);
     const uint32_t n_chunks = (n_words + CHANGES_CHUNK_WORDS - 1) / CHANGES_CHUNK_WORDS;
     cudaStream_t st = s->ctx->stream.get();
-    uint32_t *chunk_sums = s->d_diff.get<uint32_t>();   // (n_chunks + 1) * 4 <= volume / 8192 + 8 bytes of its volume + 16
-    k_changes_count<<<n_chunks, 256, 0, st>>>(s->d_changes.get<uint32_t>(), n_words, chunk_sums);
+    uint32_t *chunk_sums = s->light.chunk_sums();   // (n_chunks + 1) * 4 <= volume / 8192 + 8 of diff's volume + 16
+    k_changes_count<<<n_chunks, 256, 0, st>>>(s->light.shared.changes.get<uint32_t>(), n_words, chunk_sums);
     k_changes_scan<<<1, 1024, 0, st>>>(chunk_sums, n_chunks);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(n, chunk_sums + n_chunks, 4, cudaMemcpyDeviceToHost, st));
@@ -1111,9 +1081,10 @@ static aicb_status count_changes(const aicb_scene *s, uint32_t *n) {
 }
 
 aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed) {
+    if (!n_changed) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     *n_changed = 0;
-    if (!s->d_changes) return AICB_OK;   // no light call yet
+    if (!s->light.shared.changes) return AICB_OK;   // no light call yet
     CU(cudaSetDevice(s->ctx->device));
     uint32_t n = 0;
     TRY(count_changes(s, &n));
@@ -1122,13 +1093,13 @@ aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed) {
 }
 
 // Both outputs: the set, in increasing index order, and the texels as they are now, then the set is empty.  Neither:
-// the set is emptied without a copy.  The indices and texels are compacted into the round's `list` and `new_light`
-// buffers (idle between light calls) and copied to the caller behind everything queued on the context's stream.
+// the set is emptied without a copy.  The copy to the caller is queued behind everything on the context's stream.
 aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity, size_t *n_taken) {
+    if (!n_taken) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (!indices != !texels) return aicb_fail(AICB_ERR_INVALID, "give both outputs, or neither to discard the set");
     if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     *n_taken = 0;
-    if (!s->d_changes) return AICB_OK;
+    if (!s->light.shared.changes) return AICB_OK;
     CU(cudaSetDevice(s->ctx->device));
     cudaStream_t st = s->ctx->stream.get();
     uint32_t n = 0;
@@ -1141,12 +1112,13 @@ aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texel
         const uint32_t n_words = (uint32_t)((s->volume + 31) / 32);
         if (indices) {
             const uint32_t n_chunks = (n_words + CHANGES_CHUNK_WORDS - 1) / CHANGES_CHUNK_WORDS;
-            k_changes_emit<<<n_chunks, 256, 0, st>>>(s->d_changes.get<uint32_t>(), n_words, s->d_diff.get<uint32_t>(),
-                                                      s->ds.light, s->d_list.get<uint32_t>(), s->d_new_light.get<uint32_t>());
-            CU(cudaMemcpyAsync(indices, s->d_list.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-            CU(cudaMemcpyAsync(texels, s->d_new_light.get(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+            const LightState &L = s->light;
+            k_changes_emit<<<n_chunks, 256, 0, st>>>(L.shared.changes.get<uint32_t>(), n_words, L.chunk_sums(),
+                                                      s->ds.light, L.taken_indices(), L.taken_texels());
+            CU(cudaMemcpyAsync(indices, L.taken_indices(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(texels, L.taken_texels(), (size_t)n * 4, cudaMemcpyDeviceToHost, st));
         } else {
-            CU(cudaMemsetAsync(s->d_changes.get(), 0, (size_t)n_words * 4, st));
+            CU(cudaMemsetAsync(s->light.shared.changes.get(), 0, (size_t)n_words * 4, st));
         }
         CU(cudaStreamSynchronize(st));
         CU(cudaGetLastError());
@@ -1193,8 +1165,7 @@ aicb_status aicb_light_fast_evaluate(aicb_scene *s) {
 }
 
 aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
-    if (!s || (n && (!cubes || !out))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return light_compute({&s, &s->ctx, 1}, cubes, n, out);
 }
@@ -1208,7 +1179,7 @@ aicb_status aicb_light_evaluate(aicb_scene *s, uint8_t epsilon, uint64_t *update
 
 aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                           uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
-    if (!s || (n_edits && (!cubes || !new_ids))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return light_edit_and_propagate({&s, &s->ctx, 1}, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
 }
@@ -1220,14 +1191,14 @@ aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texel
 }
 
 aicb_status aicb_light_changes_count(const aicb_scene *s, size_t *n_changed) {
-    if (!s || !n_changed) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return light_changes_count(s, n_changed);
 }
 
 aicb_status aicb_light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity,
                                     size_t *n_taken) {
-    if (!s || !n_taken) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return light_take_changes(s, indices, texels, capacity, n_taken);
 }

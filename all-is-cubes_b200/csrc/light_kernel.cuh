@@ -21,6 +21,7 @@
 // The relaxation order differs from the reference's (batch = a priority band), which the reference leaves unspecified
 // (queue.rs:226-246) — parity contract SURVEY §8(a) L4.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 #include <cuda_runtime.h>
 
@@ -79,6 +80,28 @@ constexpr uint32_t TX_OPAQUE = 128u << 24, TX_NO_RAYS = 1u << 24, TX_UNINIT = 0u
 constexpr int PRIO_NEWLY_VISIBLE = 250, PRIO_ESTIMATED = 200;
 constexpr uint32_t LIGHT_TILE = 1024;   // cubes per queue tile (256 words of pending bytes: one 256-thread block)
 
+// A light call's counters in device memory, which the kernels count into and the host reads back.  The kernels of a
+// round read its list length and priority from here, so rounds are queued back to back without a host round trip.
+// A round restarts `gathered` .. `priority` and `changed` .. `overflow`; the totals between them run over the call.
+struct LightCounters {
+    uint32_t gathered;              // cubes in this round's list
+    uint32_t priority;              // highest queued priority this round
+    uint32_t max_diff;              // largest difference applied
+    uint32_t updates;               // cube updates
+    unsigned long long node_visits; // chart nodes visited
+    uint32_t changed;               // entries of this round's `changed` list
+    uint32_t compute_work;          // cubes handed out by the chain walk's compute form this round
+    uint32_t mark_work;             // ... and by its mark form
+    uint32_t overflow;              // entries of replica 0's overflow list
+    uint32_t _pad[6];
+};
+static_assert(offsetof(LightCounters, gathered) == 0 && offsetof(LightCounters, priority) == 4 &&
+              offsetof(LightCounters, max_diff) == 8 && offsetof(LightCounters, updates) == 12 &&
+              offsetof(LightCounters, node_visits) == 16 && offsetof(LightCounters, changed) == 24 &&
+              offsetof(LightCounters, compute_work) == 28 && offsetof(LightCounters, mark_work) == 32 &&
+              offsetof(LightCounters, overflow) == 36 && sizeof(LightCounters) == 64,
+              "LightCounters: the layout the kernels and the round's memsets address");
+
 struct LightParams {
     aicb::DeviceScene scene;        // cells, light, sky faces, tables (LUT)
     const LightBlockDev *blocks;
@@ -89,12 +112,12 @@ struct LightParams {
     uint32_t n_chains, n_euler;
     float4 *term_scratch;           // per resident warp: LIGHT_MAX_CHAINS * LIGHT_CHAIN_SLOTS terms
     uint32_t *overflow;             // list entries whose walk needs more than LIGHT_CHAIN_K terms in one chain
-    uint32_t *overflow_count;       // ... and their count (scalars + 9 of the replica's own scalars: every device of a
-                                    // group computes the overflow of its own walks)
+    uint32_t *overflow_count;       // ... and their count: every device of a group computes the overflow of its own
+                                    // walks (replica 0's is its LightCounters::overflow)
     uint32_t *dirty;                // device 0 of a group: one bit per 32-cube segment of the light volume written this
                                     // round, for the push to the other replicas (nullptr on one context)
-    uint32_t *changes;              // replica 0: one bit per cube whose texel a light call wrote since the host last took
-                                    // the set (SpaceChange::CubeLight, space.rs:1079-1083); nullptr on the others
+    uint32_t *changes;              // replica 0's: one bit per cube whose texel a light call wrote since the host last
+                                    // took the set (SpaceChange::CubeLight, space.rs:1079-1083)
     const float4 *sky_term;         // per preorder node: the sky light its bundle collects at the end of a ray (end_of_ray)
     uint32_t chart_nodes;
     uint32_t *tile_max;             // per LIGHT_TILE cubes: an upper bound of the tile's highest queued priority
@@ -103,13 +126,9 @@ struct LightParams {
     uint32_t *new_light;
     uint8_t *diff;
     uint32_t *changed;              // positions in the round's list whose cube changed by more than one unit (the mark walk's work)
-    uint32_t *scalars;              // [0] list length, [1] max priority, [2] max diff, [3] updates, [4..5] node visits, [6] changed,
-                                    // [7] / [8] cubes handed out by the chain walk's compute / mark form this round,
-                                    // [9] overflow list length.  On a group every replica's kernels use device 0's
-                                    // scalars, except [9], which is each replica's own (overflow_count).
+    LightCounters *counters;        // on a group, every replica's kernels count into device 0's
     uint32_t volume;
     uint32_t max_distance;
-    uint32_t priority;              // the round's priority level
     uint32_t epsilon_priority;
 };
 
