@@ -59,6 +59,7 @@ def load_library() -> C.CDLL:
     lib.aicb_scene_device_bytes.restype = C.c_uint64
     lib.aicb_scene_update_cubes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_shard_pixel_count.argtypes = [C.POINTER(abi.CameraData), C.POINTER(abi.Shard)]
     lib.aicb_shard_pixel_count.restype = C.c_size_t
@@ -123,6 +124,7 @@ def load_library() -> C.CDLL:
                                             C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_group_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_group_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_group_render_layers_srgb8.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_render_layers_texture.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
@@ -543,6 +545,14 @@ def fill_block_desc(bd, b):
     bd.light_emission[:] = b.light_emission
 
 
+def _block_descs(blocks):
+    """Blocks -> an aicb_block_desc array (its arrays stay owned by the blocks)."""
+    arr = (abi.BlockDesc * max(len(blocks), 1))()
+    for i, b in enumerate(blocks):
+        fill_block_desc(arr[i], b)
+    return arr
+
+
 def light_chart():
     """The static light-ray chart (space/light/chart/generator.rs) as (weights [n,6] f32, children [n,6] u32)."""
     lib = load_library()
@@ -689,6 +699,12 @@ class SpaceRaytracer:
         for i, b in enumerate(blocks):
             fill_block_desc(arr[i], b)
         _check(load_library().aicb_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
+
+    def append_blocks(self, blocks):
+        """SpaceChange::BlockIndex for new indices (UpdatingSpaceRaytracer::update, updating.rs:145-151): the blocks
+        become the table's next indices, valid in update_cubes, update_blocks and light_edit_and_propagate."""
+        arr = _block_descs(blocks)
+        _check(load_library().aicb_scene_append_blocks(self.handle, arr, len(blocks)))
 
     # ---- light propagation (space::light; SURVEY 8(a) L1-L4) ----
     def light_fast_evaluate(self):
@@ -940,6 +956,11 @@ class GroupScene:
         for i, b in enumerate(blocks):
             fill_block_desc(arr[i], b)
         _check(load_library().aicb_group_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
+
+    def append_blocks(self, blocks):
+        """SpaceRaytracer.append_blocks on every replica; a rejected call changes none."""
+        arr = _block_descs(blocks)
+        _check(load_library().aicb_group_scene_append_blocks(self.handle, arr, len(blocks)))
 
     def upload_light(self, light: np.ndarray):
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)

@@ -283,6 +283,27 @@ static __global__ void scatter_cubes_kernel(const CubeDelta *ops, uint32_t n, ui
     if (op.has_light) light[op.idx] = op.light;
 }
 
+// A u16 cell word (id | kind << 14) as the u32 cell word of the same cube: cell_word(id, kind, true).
+static __device__ __forceinline__ uint32_t widened_cell(uint32_t w) { return (w & 0x3fffu) | ((w >> 14) << 16); }
+
+// A scene's cells from u16 to u32 words (a block table grown past 16384 ids): one streaming pass, eight cells per
+// thread and step (one 16-byte load, two 16-byte stores, evict-first), the last n % 8 cells one at a time.
+static __global__ void __launch_bounds__(256) widen_cells_kernel(const uint16_t *__restrict__ in, uint32_t *__restrict__ out,
+                                                                 size_t n) {
+    const size_t stride = (size_t)gridDim.x * blockDim.x, first = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t n8 = n / 8;
+    for (size_t i = first; i < n8; i += stride) {
+        const uint4 v = __ldcs(reinterpret_cast<const uint4 *>(in) + i);
+        __stcs(reinterpret_cast<uint4 *>(out) + 2 * i,
+               make_uint4(widened_cell(v.x & 0xffffu), widened_cell(v.x >> 16), widened_cell(v.y & 0xffffu),
+                          widened_cell(v.y >> 16)));
+        __stcs(reinterpret_cast<uint4 *>(out) + 2 * i + 1,
+               make_uint4(widened_cell(v.z & 0xffffu), widened_cell(v.z >> 16), widened_cell(v.w & 0xffffu),
+                          widened_cell(v.w >> 16)));
+    }
+    for (size_t i = n8 * 8 + first; i < n; i += stride) out[i] = widened_cell(in[i]);
+}
+
 static aicb_status validate_options(const aicb_options *o) {
     if (!o) return fail(AICB_ERR_INVALID, "options is NULL");
     if (o->fog > AICB_FOG_PHYSICAL) return fail(AICB_ERR_INVALID, "bad fog option");
@@ -622,6 +643,129 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
         info->flaws = 0;
     }
     sc->pending = false;
+    return AICB_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// growing a scene's block table (aicb_scene_append_blocks, aicb_group_scene_append_blocks)
+// ---------------------------------------------------------------------------------------------
+aicb_status grow_buffer(DeviceBuffer &buf, size_t used, size_t bytes, cudaStream_t stream,
+                        std::vector<DeviceBuffer> *retired) {
+    if (buf.bytes() >= bytes) return AICB_OK;
+    DeviceBuffer b;
+    TRY(b.ensure(std::max(bytes, 2 * buf.bytes())));
+    if (used) CU(cudaMemcpyAsync(b.get(), buf.get(), used, cudaMemcpyDeviceToDevice, stream));
+    retired->push_back(std::move(buf));
+    buf = std::move(b);
+    return AICB_OK;
+}
+
+// The arrays a scene replaced while it grew, freed when the call ends: after the scene's frame in flight (if the
+// context's last frame is one of this scene's) and the copies queued on the context's stream.  Nothing else reads them.
+struct Retired {
+    aicb_scene *s;
+    std::vector<DeviceBuffer> bufs;
+    ~Retired() {
+        if (bufs.empty()) return;
+        aicb_ctx *ctx = s->ctx;
+        if (ctx->last_scene == s && ctx->frame_in_flight) cudaEventSynchronize(ctx->ev1.get());
+        cudaStreamSynchronize(ctx->stream.get());
+    }
+};
+
+aicb_status append_blocks_validate(const aicb_scene *s, const aicb_block_desc *descs, size_t n, BlockAppend *a) {
+    if (n && !descs) return fail(AICB_ERR_INVALID, "NULL argument");
+    if (s->block_kind.size() + n > 65536) return fail(AICB_ERR_INVALID, "more than 65536 blocks");
+    a->recs.resize(n);
+    a->kinds.resize(n);
+    for (size_t i = 0; i < n; i++) TRY(flatten_block(descs[i], a->recs[i], a->kinds[i], a->bricks, a->palette, a->pal_tab));
+    if (s->n_bricks + a->bricks.size() > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
+    return AICB_OK;
+}
+
+// Every copy is queued on the context's stream and ev_delta is recorded behind them, as aicb_scene_update_cubes does:
+// a frame issued later on another stream waits for them (launch_trace).  The new entries go to spare capacity that no
+// cell refers to until a later, stream-ordered cube update, so a frame in flight is not disturbed; an array that has to
+// move is freed only after it (Retired).
+aicb_status append_blocks_apply(aicb_scene *s, const BlockAppend &a, const aicb_block_desc *descs) {
+    const size_t n = a.recs.size();
+    if (n == 0) return AICB_OK;
+    aicb_ctx *ctx = s->ctx;
+    cudaStream_t stream = ctx->stream.get();
+    DeviceScene &ds = s->ds;
+    const size_t count = s->block_kind.size();
+    const uint32_t pal_base = (uint32_t)(s->n_palette / 2);   // palette entries (2 x float4 each)
+    std::vector<BlockRec> recs(a.recs);
+    std::vector<float4> blk_tab(n);
+    for (size_t i = 0; i < n; i++) {   // offsets into the device pools, as aicb_scene_update_blocks patches them
+        BlockRec &r = recs[i];
+        blk_tab[i] = block_entry(a.kinds[i], r.pal_off, a.pal_tab, pal_base);
+        if (a.kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)s->n_bricks;
+        if (a.kinds[i] != KIND_INVISIBLE || !descs[i].is_air) r.pal_off += pal_base;
+    }
+    // ---- room for the new entries; the scene's pointers follow every array that moved, whatever fails later ------
+    Retired retired{s, {}};
+    aicb_status st = AICB_OK;
+    auto room = [&](DeviceBuffer &b, size_t used, size_t add) {
+        if (st == AICB_OK && add) st = grow_buffer(b, used, used + add, stream, &retired.bufs);
+    };
+    room(s->d_blocks, count * sizeof(BlockRec), n * sizeof(BlockRec));
+    room(s->d_blk_tab, count * sizeof(float4), n * sizeof(float4));
+    room(s->d_bricks, s->n_bricks * 2, a.bricks.size() * 2);
+    room(s->d_palette, s->n_palette * sizeof(float4), a.palette.size() * sizeof(float4));
+    room(s->d_pal_tab, (size_t)pal_base * sizeof(float2), a.pal_tab.size() * sizeof(float2));
+    ds.blocks = s->d_blocks.get<BlockRec>();
+    ds.blk_tab = s->d_blk_tab.get<float4>();
+    ds.bricks = s->d_bricks.get<uint16_t>();
+    ds.palette = s->d_palette.get<float4>();
+    ds.pal_tab = s->d_pal_tab.get<float2>();
+    TRY(st);
+    // u16 cells hold ids below 16384 (aicb_scene_create): a table that grows past that takes u32 cells
+    const bool widen = !ds.wide_cells && count + n > 16384;
+    DeviceBuffer wide;
+    if (widen && s->volume) TRY(wide.ensure(s->volume * 4));
+    // ---- the new entries, behind the copies of the arrays that moved ---------------------------------------------
+    CU(cudaMemcpyAsync(s->d_blocks.get<BlockRec>() + count, recs.data(), n * sizeof(BlockRec), cudaMemcpyHostToDevice,
+                       stream));
+    CU(cudaMemcpyAsync(s->d_blk_tab.get<float4>() + count, blk_tab.data(), n * sizeof(float4), cudaMemcpyHostToDevice,
+                       stream));
+    if (!a.bricks.empty())
+        CU(cudaMemcpyAsync(s->d_bricks.get<uint16_t>() + s->n_bricks, a.bricks.data(), a.bricks.size() * 2,
+                           cudaMemcpyHostToDevice, stream));
+    if (!a.palette.empty()) {
+        CU(cudaMemcpyAsync(s->d_palette.get<float4>() + s->n_palette, a.palette.data(), a.palette.size() * sizeof(float4),
+                           cudaMemcpyHostToDevice, stream));
+        CU(cudaMemcpyAsync(s->d_pal_tab.get<float2>() + pal_base, a.pal_tab.data(), a.pal_tab.size() * sizeof(float2),
+                           cudaMemcpyHostToDevice, stream));
+    }
+    if (wide) {   // behind every queued cube update of this context
+        const size_t n8 = s->volume / 8;
+        const size_t want = (std::max<size_t>(n8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
+        widen_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, stream>>>(s->d_cells.get<const uint16_t>(),
+                                                                             wide.get<uint32_t>(), s->volume);
+        CU(cudaGetLastError());
+    }
+    const aicb_status lst = aicb_light_blocks_append(s, descs, n, &retired.bufs);
+    if (lst != AICB_OK) {
+        if (wide) retired.bufs.push_back(std::move(wide));   // (the widening pass may still be writing it)
+        return lst;
+    }
+    // ---- the scene takes the longer table ------------------------------------------------------------------------
+    if (widen) {
+        if (wide) {
+            retired.bufs.push_back(std::move(s->d_cells));
+            s->d_cells = std::move(wide);
+            ds.cells = s->d_cells.get();
+            s->device_bytes += s->volume * 2;
+        }
+        ds.wide_cells = 1;
+    }
+    s->block_kind.insert(s->block_kind.end(), a.kinds.begin(), a.kinds.end());
+    s->n_bricks += a.bricks.size();
+    s->n_palette += a.palette.size();
+    s->device_bytes += n * (sizeof(BlockRec) + sizeof(float4)) + a.bricks.size() * 2 +
+                       a.palette.size() * sizeof(float4) + a.pal_tab.size() * sizeof(float2);
+    CU(cudaEventRecord(ctx->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
     return AICB_OK;
 }
 
@@ -975,6 +1119,18 @@ aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, con
         }
     }
     return aicb_light_blocks_update(s, indices, descs, n);
+}
+
+// == SpaceChange::BlockIndex for indices past the table (palette.rs:207-210; UpdatingSpaceRaytracer::update appends
+// TracingBlock::from_block of each, updating.rs:145-151): the blocks become the table's next indices.
+aicb_status aicb_scene_append_blocks(aicb_scene *s, const aicb_block_desc *descs, size_t n) {
+    if (!s || (n && !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    CU(cudaSetDevice(s->ctx->device));
+    if (n == 0) return AICB_OK;
+    BlockAppend a;
+    TRY(append_blocks_validate(s, descs, n, &a));   // validate and flatten everything before touching any state
+    return append_blocks_apply(s, a, descs);
 }
 
 aicb_status aicb_scene_upload_light(aicb_scene *s, const uint8_t (*light)[4], size_t n_texels) {

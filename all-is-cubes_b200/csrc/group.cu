@@ -361,6 +361,21 @@ aicb_status aicb_group_scene_update_blocks(aicb_group_scene *gs, const uint16_t 
     return AICB_OK;
 }
 
+aicb_status aicb_group_scene_append_blocks(aicb_group_scene *gs, const aicb_block_desc *descs, size_t n) {
+    if (!gs || (n && !descs)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    if (n == 0) return AICB_OK;
+    // the replicas hold the same block table: replica 0's validation is every replica's, and a rejected call changes
+    // none; each replica then appends (and widens its cells, past 16384 blocks) on its own device
+    BlockAppend a;
+    TRY(append_blocks_validate(gs->scene[0], descs, n, &a));
+    for (aicb_scene *s : gs->scene) {
+        CU(cudaSetDevice(s->ctx->device));
+        TRY(append_blocks_apply(s, a, descs));
+    }
+    return AICB_OK;
+}
+
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *gs, const uint8_t (*light)[4], size_t n_texels) {
     if (!gs || !light) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n_texels != gs->scene[0]->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");

@@ -104,6 +104,13 @@ inline aicb_status create_event(Event &e, unsigned int flags) {
     return AICB_OK;
 }
 
+// Room for `bytes` in `buf`, of which the first `used` are kept.  A buffer that is too small is replaced by one of at
+// least twice its size, its `used` bytes copied on `stream`; the replaced buffer goes to `retired`, and the caller
+// frees it once nothing can read it any more (the copy, and any frame in flight).  Appending k elements one call at a
+// time thus reallocates O(log k) times.
+aicb_status grow_buffer(DeviceBuffer &buf, size_t used, size_t bytes, cudaStream_t stream,
+                        std::vector<DeviceBuffer> *retired);
+
 // A cube's cell word: its block id with the block's kind in the top bits (16-bit cells up to 16384 block ids).
 inline uint32_t cell_word(uint32_t id, uint8_t kind, bool wide) { return id | ((uint32_t)kind << (wide ? 16 : 14)); }
 
@@ -228,7 +235,10 @@ struct aicb_scene {
     DeviceBuffer d_palette;
     DeviceBuffer d_pal_tab;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
     DeviceBuffer d_blk_tab;   // per block id: that pair and the palette entry of single-voxel blocks
-    size_t n_bricks = 0, n_palette = 0;   // elements in d_bricks / d_palette (aicb_scene_update_blocks appends)
+    // Elements in use: d_bricks / d_palette (aicb_scene_update_blocks and aicb_scene_append_blocks append) and, per block
+    // id, d_blocks / d_blk_tab / light.blocks (block_kind.size(); aicb_scene_append_blocks appends).  The buffers may
+    // be larger: appends grow them geometrically (grow_buffer).
+    size_t n_bricks = 0, n_palette = 0;
     // state of the last asynchronous render
     bool pending = false;
     uint64_t pending_rays = 0;
@@ -298,6 +308,24 @@ void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool sa
 // aicb_scene_update_blocks' validation alone: AICB_OK if that call would accept the update (changes nothing)
 aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
 }
+
+// aicb200.cu: aicb_scene_append_blocks in two steps, for one scene and for every replica of a group scene (whose block
+// tables are identical).  `append_blocks_validate` flattens the descriptors against `s` and changes nothing: records
+// and palette offsets relative to the appended data alone.  `append_blocks_apply` appends them (the caller holds s's
+// context lock, and s's device is current).
+struct BlockAppend {
+    std::vector<aicb::BlockRec> recs;
+    std::vector<uint8_t> kinds;
+    std::vector<uint16_t> bricks;
+    std::vector<float4> palette;
+    std::vector<float2> pal_tab;
+};
+aicb_status append_blocks_validate(const aicb_scene *s, const aicb_block_desc *descs, size_t n, BlockAppend *out);
+aicb_status append_blocks_apply(aicb_scene *s, const BlockAppend &a, const aicb_block_desc *descs);
+// light.cu: the light-side records of blocks appended to the table (h_block_light, light.blocks); the caller frees the
+// replaced buffer (`retired`) once the context's stream is past the copy.
+aicb_status aicb_light_blocks_append(aicb_scene *s, const aicb_block_desc *descs, size_t n,
+                                     std::vector<DeviceBuffer> *retired);
 
 // ---- calls over several contexts ----------------------------------------------------------------------------------
 // A call that runs on several contexts lists them device 0's first, with a scene's replica on each (a group scene's

@@ -917,6 +917,21 @@ aicb_status aicb_light_blocks_update(aicb_scene *s, const uint16_t *indices, con
     return AICB_OK;
 }
 
+// the light-side records of blocks appended to the table (aicb_scene_append_blocks), queued on the context's stream
+aicb_status aicb_light_blocks_append(aicb_scene *s, const aicb_block_desc *descs, size_t n,
+                                     std::vector<DeviceBuffer> *retired) {
+    const size_t count = s->h_block_light.size();
+    std::vector<LightBlockDev> lb(n);
+    for (size_t i = 0; i < n; i++) lb[i] = light_block(descs[i]);
+    cudaStream_t stream = s->ctx->stream.get();
+    TRY(grow_buffer(s->light.blocks, count * sizeof(LightBlockDev), (count + n) * sizeof(LightBlockDev), stream, retired));
+    CU(cudaMemcpyAsync(s->light.blocks.get<LightBlockDev>() + count, lb.data(), n * sizeof(LightBlockDev),
+                       cudaMemcpyHostToDevice, stream));
+    for (const LightBlockDev &o : lb) s->h_block_light.push_back(o.flags);
+    s->device_bytes += n * sizeof(LightBlockDev);
+    return AICB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // the light calls over a scene's replicas (internal.h): one context's entry points below, a group's in group.cu
 // ---------------------------------------------------------------------------------------------

@@ -5,7 +5,8 @@
 //!
 //! * `update()` = `RtRenderer::update` (renderer.rs:96-161): camera sync, then per layer either a full snapshot
 //!   (`SpaceRaytracer::new`, sr.rs:64-88 → `aicb_scene_create`) or the `SpaceChange` deltas an
-//!   `UpdatingSpaceRaytracer` would apply (updating.rs:107-172 → `aicb_scene_update_blocks` / `_update_cubes`).
+//!   `UpdatingSpaceRaytracer` would apply (updating.rs:107-172 → `aicb_scene_append_blocks` / `_update_blocks` /
+//!   `_update_cubes`).
 //! * `draw()` = `RtRenderer::draw_rgba` (renderer.rs:282-308) with `trace_ray_through_layers` (renderer.rs:454-478)
 //!   → `aicb_render_layers_srgb8`; the info text is drawn here over the returned pixels like renderer.rs:659-683.
 //! * `trace_texture_batch()` = the tracing of `RaytraceToTexture::do_some_tracing` (raytrace_to_texture.rs:591-683)
@@ -133,6 +134,15 @@ impl SceneHandle {
             match self {
                 Self::Single(s) => sys::aicb_scene_update_blocks(s, indices.as_ptr(), descs.as_ptr(), indices.len()),
                 Self::Group(s) => sys::aicb_group_scene_update_blocks(s, indices.as_ptr(), descs.as_ptr(), indices.len()),
+            }
+        })
+    }
+
+    fn append_blocks(self, descs: &[sys::aicb_block_desc]) -> Result<(), B200Error> {
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_scene_append_blocks(s, descs.as_ptr(), descs.len()),
+                Self::Group(s) => sys::aicb_group_scene_append_blocks(s, descs.as_ptr(), descs.len()),
             }
         })
     }
@@ -265,20 +275,26 @@ impl SceneFollower {
             }
             self.chars = space.block_data().iter().map(character_of).collect();
         } else if let Some(scene) = self.scene {
-            // SpaceChange::BlockIndex / BlockEvaluation: re-run TracingBlock::from_block for those indices (updating.rs:128-150);
-            // on a group every replica takes them (aicb_group_scene_update_blocks), no rebuild
-            if !todo.blocks.is_empty() {
-                let idx: Vec<u16> = todo.blocks.iter().copied().collect();
-                let owned: Vec<OwnedBlockDesc> =
-                    idx.iter().map(|&i| block_desc_of(&space.block_data()[usize::from(i)])).collect();
+            // SpaceChange::BlockIndex for indices past the table: append TracingBlock::from_block of every entry the
+            // scene lacks (updating.rs:145-151); on a group every replica takes them (aicb_group_scene_append_blocks)
+            let known = self.chars.len();
+            let data = space.block_data();
+            if data.len() > known {
+                let owned: Vec<OwnedBlockDesc> = data[known..].iter().map(block_desc_of).collect();
+                let descs: Vec<sys::aicb_block_desc> = owned.iter().map(OwnedBlockDesc::as_ffi).collect();
+                scene.append_blocks(&descs).map_err(to_render_error)?;
+                self.chars.extend(data[known..].iter().map(character_of));
+            }
+            // SpaceChange::BlockIndex / BlockEvaluation of indices the scene already had: re-run
+            // TracingBlock::from_block for those (updating.rs:152-157); on a group every replica takes them
+            // (aicb_group_scene_update_blocks), no rebuild
+            let idx: Vec<u16> = todo.blocks.iter().copied().filter(|&i| usize::from(i) < known).collect();
+            if !idx.is_empty() {
+                let owned: Vec<OwnedBlockDesc> = idx.iter().map(|&i| block_desc_of(&data[usize::from(i)])).collect();
                 let descs: Vec<sys::aicb_block_desc> = owned.iter().map(OwnedBlockDesc::as_ffi).collect();
                 scene.update_blocks(&idx, &descs).map_err(to_render_error)?;
                 for &i in &idx {
-                    let i = usize::from(i);
-                    if i >= self.chars.len() {
-                        self.chars.resize(i + 1, String::new());
-                    }
-                    self.chars[i] = character_of(&space.block_data()[i]);
+                    self.chars[usize::from(i)] = character_of(&data[usize::from(i)]);
                 }
             }
             // SpaceChange::CubeBlock / CubeLight (updating.rs:151-166)

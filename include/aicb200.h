@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 7
+#define AICB_ABI_VERSION 8
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -200,10 +200,20 @@ aicb_status aicb_scene_create(aicb_ctx *, const aicb_scene_desc *, aicb_scene **
 aicb_status aicb_scene_update_cubes(aicb_scene *, const int32_t (*cubes)[3], const uint16_t *block_ids,
                                     const uint8_t (*light)[4], size_t n);
 /* SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; updating.rs:128-150): new definitions for EXISTING
- * block indices (an index beyond the table needs a new scene).  Voxel data is appended to the device pools; cubes
+ * block indices (an index beyond the table is rejected: aicb_scene_append_blocks adds new ones).  Voxel data is appended to the device pools; cubes
  * holding a block whose classification (invisible / single voxel / voxel brick) changed are re-encoded.  Light is not
  * re-propagated (call aicb_light_evaluate).  GPU test: tests/test_gpu_parity.py::test_block_definition_update_equals_fresh_snapshot. */
 aicb_status aicb_scene_update_blocks(aicb_scene *, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
+/* SpaceChange::BlockIndex for indices past the table (palette.rs:207-210; UpdatingSpaceRaytracer::update appends them,
+ * updating.rs:145-151): the blocks become indices [count, count + n) of the scene's table, where count is the table's
+ * size before the call.  From then on they are valid everywhere a block id is: aicb_scene_update_cubes,
+ * aicb_scene_update_blocks, aicb_light_edit_and_propagate.  Every output is what a scene created with the longer table
+ * gives.  The copies are queued on the context's stream, ordered like aicb_scene_update_cubes (a frame issued later on
+ * another stream waits for them); a frame in flight is not disturbed.  The device tables grow geometrically; a table
+ * that grows past 16384 blocks re-encodes the cells from 16 to 32 bits on the device.  AICB_ERR_INVALID: NULL with
+ * n > 0, count + n > 65536, or a descriptor that scene creation rejects; a rejected call changes nothing.  n == 0 does
+ * nothing.  GPU test: tests/test_gpu_append_blocks.py. */
+aicb_status aicb_scene_append_blocks(aicb_scene *, const aicb_block_desc *descs, size_t n);
 /* Whole light volume replaced (after light propagation on the host or on another rank). */
 aicb_status aicb_scene_upload_light(aicb_scene *, const uint8_t (*light)[4], size_t n_texels);
 void aicb_scene_destroy(aicb_scene *);
@@ -381,6 +391,10 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *, const aicb_camera *, con
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *, const uint16_t *indices, const aicb_block_desc *descs,
                                            size_t n);
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *, const uint8_t (*light)[4], size_t n_texels);
+/* aicb_scene_append_blocks on every replica, validated against replica 0 before any replica changes: a rejected call
+ * changes no replica.  The call holds every context of the group; a table that grows past 16384 blocks widens every
+ * replica's cells on its own device. */
+aicb_status aicb_group_scene_append_blocks(aicb_group_scene *, const aicb_block_desc *descs, size_t n);
 
 /* == RtScene::trace_ray_through_layers + draw_rgba (renderer.rs:454-478, 282-308) and RaytraceToTexture::do_some_tracing's
  * trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) on the whole group: the arguments, the validation and
