@@ -695,9 +695,7 @@ class SpaceRaytracer:
     def update_blocks(self, indices, blocks):
         """SpaceChange::BlockEvaluation / BlockIndex: new definitions for existing block indices."""
         idx = np.ascontiguousarray(indices, dtype=np.uint16)
-        arr = (abi.BlockDesc * len(blocks))()
-        for i, b in enumerate(blocks):
-            fill_block_desc(arr[i], b)
+        arr = _block_descs(blocks)
         _check(load_library().aicb_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
 
     def append_blocks(self, blocks):
@@ -952,9 +950,7 @@ class GroupScene:
     def update_blocks(self, indices, blocks):
         """SpaceChange::BlockEvaluation / BlockIndex on every replica; a rejected update changes none."""
         idx = np.ascontiguousarray(indices, dtype=np.uint16)
-        arr = (abi.BlockDesc * len(blocks))()
-        for i, b in enumerate(blocks):
-            fill_block_desc(arr[i], b)
+        arr = _block_descs(blocks)
         _check(load_library().aicb_group_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
 
     def append_blocks(self, blocks):

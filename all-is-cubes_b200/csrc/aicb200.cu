@@ -35,10 +35,6 @@ aicb_status aicb_cuda_fail(cudaError_t e, const char *what) {
 static aicb_status fail(aicb_status st, const std::string &msg) { return aicb_fail(st, msg); }
 static aicb_status cuda_fail(cudaError_t e, const char *what) { return aicb_cuda_fail(e, what); }
 
-void aicb_light_scene_init(aicb_scene *s, const aicb_scene_desc *d);   // light.cu
-aicb_status aicb_light_scene_upload(aicb_scene *s, const aicb_scene_desc *d);
-aicb_status aicb_light_blocks_update(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
-
 // PackedLight::some -> scalar_in (light/data.rs:213-217)
 static uint8_t scalar_in(float v) {
     float x = std::round(std::log2(v) * 10.0f + 144.0f);
@@ -144,7 +140,7 @@ static bool voxel_invisible(const aicb_voxel &v) {
 // TracingBlock::from_block (sr.rs:579-587) for one block definition: its 32-byte record, classification, brick words
 // and palette entries (appended to `bricks` / `palette`; the record's offsets are relative to those vectors), plus
 // what the marching kernel needs of each surface: {alpha, an upper bound of log2(1 - alpha)} per palette entry.
-// Shared by aicb_scene_create and aicb_scene_update_blocks.
+// Called by flatten_blocks alone.
 static const aicb_voxel AIR_VOXEL = {{0, 0, 0, 0}, {0, 0, 0}, 0};
 
 static float2 surface_entry(float alpha) {
@@ -647,125 +643,269 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// growing a scene's block table (aicb_scene_append_blocks, aicb_group_scene_append_blocks)
+// a scene's block table (internal.h): flattened once, placed on each replica
 // ---------------------------------------------------------------------------------------------
-aicb_status grow_buffer(DeviceBuffer &buf, size_t used, size_t bytes, cudaStream_t stream,
-                        std::vector<DeviceBuffer> *retired) {
+// Room for `bytes` in `buf`, of which the first `used` are kept.  A buffer that is too small is replaced by one of at
+// least twice its size (exactly `bytes` if it was empty), its `used` bytes copied on `stream`; the replaced buffer goes
+// to `retired`.  Appending k elements one call at a time thus reallocates O(log k) times.
+static aicb_status grow_buffer(DeviceBuffer &buf, size_t used, size_t bytes, cudaStream_t stream,
+                               std::vector<DeviceBuffer> *retired) {
     if (buf.bytes() >= bytes) return AICB_OK;
     DeviceBuffer b;
     TRY(b.ensure(std::max(bytes, 2 * buf.bytes())));
     if (used) CU(cudaMemcpyAsync(b.get(), buf.get(), used, cudaMemcpyDeviceToDevice, stream));
-    retired->push_back(std::move(buf));
+    if (buf) retired->push_back(std::move(buf));
     buf = std::move(b);
     return AICB_OK;
 }
 
-// The arrays a scene replaced while it grew, freed when the call ends: after the scene's frame in flight (if the
-// context's last frame is one of this scene's) and the copies queued on the context's stream.  Nothing else reads them.
-struct Retired {
-    aicb_scene *s;
-    std::vector<DeviceBuffer> bufs;
-    ~Retired() {
-        if (bufs.empty()) return;
-        aicb_ctx *ctx = s->ctx;
-        if (ctx->last_scene == s && ctx->frame_in_flight) cudaEventSynchronize(ctx->ev1.get());
-        cudaStreamSynchronize(ctx->stream.get());
-    }
-};
-
-aicb_status append_blocks_validate(const aicb_scene *s, const aicb_block_desc *descs, size_t n, BlockAppend *a) {
-    if (n && !descs) return fail(AICB_ERR_INVALID, "NULL argument");
-    if (s->block_kind.size() + n > 65536) return fail(AICB_ERR_INVALID, "more than 65536 blocks");
-    a->recs.resize(n);
-    a->kinds.resize(n);
-    for (size_t i = 0; i < n; i++) TRY(flatten_block(descs[i], a->recs[i], a->kinds[i], a->bricks, a->palette, a->pal_tab));
-    if (s->n_bricks + a->bricks.size() > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
+// Returns once nothing on the context can read a scene's arrays: its frame in flight, whichever scene drew it (the
+// context's frames run one after another, launch_trace, so it is behind every earlier one), and the context's stream.
+static aicb_status wait_context(aicb_ctx *ctx) {
+    if (ctx->frame_in_flight) CU(cudaEventSynchronize(ctx->ev1.get()));
+    CU(cudaStreamSynchronize(ctx->stream.get()));
     return AICB_OK;
 }
 
-// Every copy is queued on the context's stream and ev_delta is recorded behind them, as aicb_scene_update_cubes does:
-// a frame issued later on another stream waits for them (launch_trace).  The new entries go to spare capacity that no
-// cell refers to until a later, stream-ordered cube update, so a frame in flight is not disturbed; an array that has to
-// move is freed only after it (Retired).
-aicb_status append_blocks_apply(aicb_scene *s, const BlockAppend &a, const aicb_block_desc *descs) {
-    const size_t n = a.recs.size();
-    if (n == 0) return AICB_OK;
-    aicb_ctx *ctx = s->ctx;
-    cudaStream_t stream = ctx->stream.get();
-    DeviceScene &ds = s->ds;
-    const size_t count = s->block_kind.size();
-    const uint32_t pal_base = (uint32_t)(s->n_palette / 2);   // palette entries (2 x float4 each)
-    std::vector<BlockRec> recs(a.recs);
-    std::vector<float4> blk_tab(n);
-    for (size_t i = 0; i < n; i++) {   // offsets into the device pools, as aicb_scene_update_blocks patches them
-        BlockRec &r = recs[i];
-        blk_tab[i] = block_entry(a.kinds[i], r.pal_off, a.pal_tab, pal_base);
-        if (a.kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)s->n_bricks;
-        if (a.kinds[i] != KIND_INVISIBLE || !descs[i].is_air) r.pal_off += pal_base;
+// The arrays a scene replaced, freed when the call ends, once nothing can read them (wait_context).
+struct Retired {
+    aicb_ctx *ctx;
+    std::vector<DeviceBuffer> bufs;
+    ~Retired() {
+        if (!bufs.empty()) wait_context(ctx);
     }
-    // ---- room for the new entries; the scene's pointers follow every array that moved, whatever fails later ------
-    Retired retired{s, {}};
+};
+
+// Block definitions flattened against a table: per definition its record (brick_off / pal_off already offsets into the
+// table's pools), blk_tab entry, kind and light record; and the voxel data they append to the pools.
+struct FlatBlocks {
+    std::vector<BlockRec> recs;
+    std::vector<float4> blk_tab;
+    std::vector<uint8_t> kinds;
+    std::vector<LightBlockDev> light;
+    std::vector<uint16_t> bricks;
+    std::vector<float4> palette;
+    std::vector<float2> pal_tab;
+};
+
+// Validates and flattens n definitions against `t`, for the next ids (indices == nullptr) or for existing `indices`.
+// Changes nothing.
+static aicb_status flatten_blocks(const BlockTable &t, const aicb_block_desc *descs, size_t n, const uint16_t *indices,
+                                  FlatBlocks *f) {
+    if (!indices && t.block_count() + n > 65536) return fail(AICB_ERR_INVALID, "more than 65536 blocks");
+    const uint32_t pal_base = (uint32_t)(t.n_palette / 2);   // palette entries (2 x float4 each)
+    f->recs.resize(n);
+    f->blk_tab.resize(n);
+    f->kinds.resize(n);
+    f->light.resize(n);
+    for (size_t i = 0; i < n; i++) {
+        if (indices && indices[i] >= t.block_count())
+            return fail(AICB_ERR_INVALID, "block index out of range (new indices need a new scene)");
+        BlockRec &r = f->recs[i];
+        TRY(flatten_block(descs[i], r, f->kinds[i], f->bricks, f->palette, f->pal_tab));
+        f->blk_tab[i] = block_entry(f->kinds[i], r.pal_off, f->pal_tab, pal_base);
+        if (f->kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)t.n_bricks;
+        if (!descs[i].is_air) r.pal_off += pal_base;
+        f->light[i] = light_block(descs[i]);
+    }
+    if (t.n_bricks + f->bricks.size() > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
+    return AICB_OK;
+}
+
+// Places `f` (flattened against s's table) in s's table: the voxel data appended to the pools; the per-id records
+// appended (indices == nullptr) or written at `indices`, where a repeated index keeps its last definition.  Every copy
+// is queued on the context's stream, and the scene's pointers follow every array that moved, whatever fails later.
+static aicb_status place(aicb_scene *s, const FlatBlocks &f, const uint16_t *indices, Retired &retired) {
+    BlockTable &t = s->blocks;
+    cudaStream_t stream = s->ctx->stream.get();
+    const size_t n = f.kinds.size(), count = t.block_count(), added = indices ? 0 : n;
     aicb_status st = AICB_OK;
     auto room = [&](DeviceBuffer &b, size_t used, size_t add) {
         if (st == AICB_OK && add) st = grow_buffer(b, used, used + add, stream, &retired.bufs);
     };
-    room(s->d_blocks, count * sizeof(BlockRec), n * sizeof(BlockRec));
-    room(s->d_blk_tab, count * sizeof(float4), n * sizeof(float4));
-    room(s->d_bricks, s->n_bricks * 2, a.bricks.size() * 2);
-    room(s->d_palette, s->n_palette * sizeof(float4), a.palette.size() * sizeof(float4));
-    room(s->d_pal_tab, (size_t)pal_base * sizeof(float2), a.pal_tab.size() * sizeof(float2));
-    ds.blocks = s->d_blocks.get<BlockRec>();
-    ds.blk_tab = s->d_blk_tab.get<float4>();
-    ds.bricks = s->d_bricks.get<uint16_t>();
-    ds.palette = s->d_palette.get<float4>();
-    ds.pal_tab = s->d_pal_tab.get<float2>();
+    room(t.blocks, count * sizeof(BlockRec), added * sizeof(BlockRec));
+    room(t.bricks, t.n_bricks * 2, f.bricks.size() * 2);
+    room(t.palette, t.n_palette * sizeof(float4), f.palette.size() * sizeof(float4));
+    room(t.pal_tab, t.n_palette / 2 * sizeof(float2), f.pal_tab.size() * sizeof(float2));
+    room(t.blk_tab, count * sizeof(float4), added * sizeof(float4));
+    room(t.light, count * sizeof(LightBlockDev), added * sizeof(LightBlockDev));
+    t.bind(s->ds);
     TRY(st);
-    // u16 cells hold ids below 16384 (aicb_scene_create): a table that grows past that takes u32 cells
-    const bool widen = !ds.wide_cells && count + n > 16384;
-    DeviceBuffer wide;
-    if (widen && s->volume) TRY(wide.ensure(s->volume * 4));
-    // ---- the new entries, behind the copies of the arrays that moved ---------------------------------------------
-    CU(cudaMemcpyAsync(s->d_blocks.get<BlockRec>() + count, recs.data(), n * sizeof(BlockRec), cudaMemcpyHostToDevice,
-                       stream));
-    CU(cudaMemcpyAsync(s->d_blk_tab.get<float4>() + count, blk_tab.data(), n * sizeof(float4), cudaMemcpyHostToDevice,
-                       stream));
-    if (!a.bricks.empty())
-        CU(cudaMemcpyAsync(s->d_bricks.get<uint16_t>() + s->n_bricks, a.bricks.data(), a.bricks.size() * 2,
-                           cudaMemcpyHostToDevice, stream));
-    if (!a.palette.empty()) {
-        CU(cudaMemcpyAsync(s->d_palette.get<float4>() + s->n_palette, a.palette.data(), a.palette.size() * sizeof(float4),
-                           cudaMemcpyHostToDevice, stream));
-        CU(cudaMemcpyAsync(s->d_pal_tab.get<float2>() + pal_base, a.pal_tab.data(), a.pal_tab.size() * sizeof(float2),
-                           cudaMemcpyHostToDevice, stream));
+    auto put = [&](void *dst, const void *src, size_t bytes) {
+        if (bytes) CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
+        return AICB_OK;
+    };
+    TRY(put(t.bricks.get<uint16_t>() + t.n_bricks, f.bricks.data(), f.bricks.size() * 2));
+    TRY(put(t.palette.get<float4>() + t.n_palette, f.palette.data(), f.palette.size() * sizeof(float4)));
+    TRY(put(t.pal_tab.get<float2>() + t.n_palette / 2, f.pal_tab.data(), f.pal_tab.size() * sizeof(float2)));
+    // the per-id records: one run of n at the end of the table, or one record at each index, in order
+    const size_t runs = indices ? n : 1, len = indices ? 1 : n;
+    for (size_t i = 0; i < runs; i++) {
+        const size_t id = indices ? indices[i] : count;
+        TRY(put(t.blocks.get<BlockRec>() + id, f.recs.data() + i, len * sizeof(BlockRec)));
+        TRY(put(t.blk_tab.get<float4>() + id, f.blk_tab.data() + i, len * sizeof(float4)));
+        TRY(put(t.light.get<LightBlockDev>() + id, f.light.data() + i, len * sizeof(LightBlockDev)));
     }
-    if (wide) {   // behind every queued cube update of this context
-        const size_t n8 = s->volume / 8;
-        const size_t want = (std::max<size_t>(n8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
-        widen_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, stream>>>(s->d_cells.get<const uint16_t>(),
-                                                                             wide.get<uint32_t>(), s->volume);
-        CU(cudaGetLastError());
+    t.kind.resize(count + added);
+    t.light_flags.resize(count + added);
+    for (size_t i = 0; i < n; i++) {
+        const size_t id = indices ? indices[i] : count + i;
+        t.kind[id] = f.kinds[i];
+        t.light_flags[id] = f.light[i].flags;
     }
-    const aicb_status lst = aicb_light_blocks_append(s, descs, n, &retired.bufs);
-    if (lst != AICB_OK) {
-        if (wide) retired.bufs.push_back(std::move(wide));   // (the widening pass may still be writing it)
-        return lst;
+    t.n_bricks += f.bricks.size();
+    t.n_palette += f.palette.size();
+    s->device_bytes += added * (sizeof(BlockRec) + sizeof(float4) + sizeof(LightBlockDev)) + f.bricks.size() * 2 +
+                       f.palette.size() * sizeof(float4) + f.pal_tab.size() * sizeof(float2);
+    return AICB_OK;
+}
+
+aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out) {
+    const int64_t LIM = 1 << 30;
+    uint64_t volume = 1;
+    for (int a = 0; a < 3; a++) {
+        int64_t lo = d->bounds.lower[a], hi = lo + (int64_t)d->bounds.size[a];
+        if (lo < -LIM || hi > LIM) return fail(AICB_ERR_INVALID, "space bounds must lie within +-2^30");
+        volume *= d->bounds.size[a];
+        if (volume > (1ull << 31)) return fail(AICB_ERR_INVALID, "space volume exceeds 2^31 cubes");
     }
-    // ---- the scene takes the longer table ------------------------------------------------------------------------
-    if (widen) {
-        if (wide) {
-            retired.bufs.push_back(std::move(s->d_cells));
-            s->d_cells = std::move(wide);
-            ds.cells = s->d_cells.get();
-            s->device_bytes += s->volume * 2;
+    if (volume && !d->block_ids) return fail(AICB_ERR_INVALID, "block_ids is NULL");
+    if (volume && d->n_blocks == 0) return fail(AICB_ERR_INVALID, "non-empty space with an empty block table");
+    if (d->n_blocks && !d->blocks) return fail(AICB_ERR_INVALID, "blocks is NULL");
+    FlatBlocks f;
+    TRY(flatten_blocks(BlockTable(), d->blocks, d->n_blocks, nullptr, &f));
+
+    // ---- cells: block id with its kind in the top bits --------------------------------------------------------------
+    const bool wide = d->n_blocks > 16384;
+    std::vector<uint16_t> cells16(wide ? 0 : volume);
+    std::vector<uint32_t> cells32(wide ? volume : 0);
+    for (size_t i = 0; i < volume; i++) {
+        const uint16_t id = d->block_ids[i];
+        if (id >= d->n_blocks) return fail(AICB_ERR_INVALID, "block id out of range");
+        if (wide) cells32[i] = cell_word(id, f.kinds[id], true);
+        else cells16[i] = (uint16_t)cell_word(id, f.kinds[id], false);
+    }
+    const void *cells = wide ? (const void *)cells32.data() : cells16.data();
+    const size_t cell_bytes = volume * (wide ? 4 : 2);
+
+    // ---- one scene per context, complete when it is returned; until then a failure frees it ------------------------
+    auto create = [&](aicb_ctx *c, aicb_scene **o) {
+        CU(cudaSetDevice(c->device));
+        std::unique_ptr<aicb_scene> s(new aicb_scene());
+        s->ctx = c;
+        s->volume = (size_t)volume;
+        DeviceScene &ds = s->ds;
+        for (int a = 0; a < 3; a++) {
+            ds.lo[a] = d->bounds.lower[a];
+            ds.size[a] = (int32_t)d->bounds.size[a];
         }
-        ds.wide_cells = 1;
+        ds.wide_cells = wide ? 1 : 0;
+        if (volume) {
+            TRY(s->d_cells.upload(cells, cell_bytes));
+            s->device_bytes += cell_bytes;
+            if (d->light) {
+                TRY(s->d_light.upload(d->light, volume * 4));
+                s->device_bytes += volume * 4;
+            }
+            s->h_ids.assign(d->block_ids, d->block_ids + volume);
+        }
+        ds.cells = s->d_cells.get();
+        ds.light = s->d_light.get<uint32_t>();
+        ds.tables = c->d_lut.get<float>();
+        build_block_sky(d->sky, &ds);
+        s->light_max_distance = d->light_max_distance;
+        Retired retired{c, {}};   // (a new table replaces no array)
+        TRY(place(s.get(), f, nullptr, retired));
+        CU(cudaStreamSynchronize(c->stream.get()));
+        *o = s.release();
+        return AICB_OK;
+    };
+    for (size_t i = 0; i < n; i++) {
+        const aicb_status st = create(ctx[i], &out[i]);
+        if (st != AICB_OK) {
+            for (size_t k = 0; k < i; k++) aicb_scene_destroy(out[k]);
+            return st;
+        }
     }
-    s->block_kind.insert(s->block_kind.end(), a.kinds.begin(), a.kinds.end());
-    s->n_bricks += a.bricks.size();
-    s->n_palette += a.palette.size();
-    s->device_bytes += n * (sizeof(BlockRec) + sizeof(float4)) + a.bricks.size() * 2 +
-                       a.palette.size() * sizeof(float4) + a.pal_tab.size() * sizeof(float2);
-    CU(cudaEventRecord(ctx->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
+    return AICB_OK;
+}
+
+aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t *indices, const aicb_block_desc *descs,
+                                 size_t n_blocks) {
+    if (n_blocks == 0) return AICB_OK;
+    const BlockTable &t = s[0]->blocks;
+    FlatBlocks f;
+    TRY(flatten_blocks(t, descs, n_blocks, indices, &f));
+    // cubes that hold a block whose kind changes carry the new kind in their cell words
+    std::vector<uint8_t> kind(t.kind);
+    for (size_t i = 0; i < n_blocks; i++) kind[indices[i]] = f.kinds[i];
+    std::vector<CubeDelta> ops;
+    if (kind != t.kind) {
+        if (s[0]->h_ids.size() != s[0]->volume) return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
+        const bool wide = s[0]->ds.wide_cells;
+        uint32_t idx = 0;
+        for (const uint16_t id : s[0]->h_ids) {
+            if (kind[id] != t.kind[id]) ops.push_back({idx, cell_word(id, kind[id], wide), 0, 0});
+            idx++;
+        }
+    }
+    for (size_t r = 0; r < n; r++) {
+        aicb_ctx *ctx = s[r]->ctx;
+        cudaStream_t stream = ctx->stream.get();
+        CU(cudaSetDevice(ctx->device));
+        TRY(wait_context(ctx));   // the records are written over in place
+        Retired retired{ctx, {}};
+        TRY(place(s[r], f, indices, retired));
+        if (!ops.empty()) {
+            DeviceBuffer d_ops;
+            TRY(d_ops.ensure(ops.size() * sizeof(CubeDelta)));
+            CU(cudaMemcpyAsync(d_ops.get(), ops.data(), ops.size() * sizeof(CubeDelta), cudaMemcpyHostToDevice, stream));
+            scatter_cubes_kernel<<<(unsigned)((ops.size() + 127) / 128), 128, 0, stream>>>(
+                d_ops.get<const CubeDelta>(), (uint32_t)ops.size(), s[r]->ds.wide_cells, s[r]->d_cells.get(),
+                s[r]->d_light.get<uint32_t>());
+            retired.bufs.push_back(std::move(d_ops));
+            CU(cudaGetLastError());
+        }
+        CU(cudaEventRecord(ctx->ev_delta.get(), stream));
+        TRY(wait_context(ctx));   // the call returns once its writes are done
+    }
+    return AICB_OK;
+}
+
+// The copies are queued on the context's stream and ev_delta is recorded behind them, as aicb_scene_update_cubes does:
+// a frame issued later on another stream waits for them (launch_trace).  The new entries go to spare capacity that no
+// cell refers to until a later, stream-ordered cube update, so a frame in flight is not disturbed; an array that has to
+// move is freed only after it (Retired).
+aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks) {
+    if (n_blocks == 0) return AICB_OK;
+    FlatBlocks f;
+    TRY(flatten_blocks(s[0]->blocks, descs, n_blocks, nullptr, &f));
+    for (size_t r = 0; r < n; r++) {
+        aicb_scene *sc = s[r];
+        aicb_ctx *ctx = sc->ctx;
+        cudaStream_t stream = ctx->stream.get();
+        CU(cudaSetDevice(ctx->device));
+        Retired retired{ctx, {}};
+        // u16 cells hold ids below 16384 (scenes_create): a table that grows past that takes u32 cells, re-encoded
+        // behind every queued cube update of this context
+        if (!sc->ds.wide_cells && sc->blocks.block_count() + n_blocks > 16384) {
+            if (sc->volume) {
+                DeviceBuffer wide;
+                TRY(wide.ensure(sc->volume * 4));
+                const size_t want = (std::max<size_t>(sc->volume / 8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
+                widen_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, stream>>>(
+                    sc->d_cells.get<const uint16_t>(), wide.get<uint32_t>(), sc->volume);
+                CU(cudaGetLastError());
+                retired.bufs.push_back(std::move(sc->d_cells));
+                sc->d_cells = std::move(wide);
+                sc->ds.cells = sc->d_cells.get();
+                sc->device_bytes += sc->volume * 2;
+            }
+            sc->ds.wide_cells = 1;
+        }
+        TRY(place(sc, f, nullptr, retired));
+        CU(cudaEventRecord(ctx->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
+    }
     return AICB_OK;
 }
 
@@ -802,6 +942,7 @@ aicb_status aicb_ctx_create(int device_id, aicb_ctx **out) {
     c->stream.reset(stream);
     TRY(create_event(c->ev0, cudaEventDefault));
     TRY(create_event(c->ev1, cudaEventDefault));
+    for (Event &e : c->ev_light) TRY(create_event(e, cudaEventDefault));
     c->profile_kernels = getenv("AICB_PROFILE_KERNELS") != nullptr;
     for (int i = 0; i < 5; i++) TRY(create_event(c->ev_k[i], cudaEventDefault));
     TRY(create_event(c->ev_delta, cudaEventDisableTiming));
@@ -838,104 +979,14 @@ aicb_status aicb_scene_create(aicb_ctx *ctx, const aicb_scene_desc *d, aicb_scen
     if (!ctx || !d || !out) return fail(AICB_ERR_INVALID, "NULL argument");
     *out = nullptr;
     std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    const int64_t LIM = 1 << 30;
-    uint64_t volume = 1;
-    for (int a = 0; a < 3; a++) {
-        int64_t lo = d->bounds.lower[a], hi = lo + (int64_t)d->bounds.size[a];
-        if (lo < -LIM || hi > LIM) return fail(AICB_ERR_INVALID, "space bounds must lie within +-2^30");
-        volume *= d->bounds.size[a];
-        if (volume > (1ull << 31)) return fail(AICB_ERR_INVALID, "space volume exceeds 2^31 cubes");
-    }
-    if (volume && !d->block_ids) return fail(AICB_ERR_INVALID, "block_ids is NULL");
-    if (d->n_blocks > 65536) return fail(AICB_ERR_INVALID, "more than 65536 blocks");
-    if (volume && d->n_blocks == 0) return fail(AICB_ERR_INVALID, "non-empty space with an empty block table");
-
-    // ---- flatten the block table --------------------------------------------------------------
-    if (d->n_blocks && !d->blocks) return fail(AICB_ERR_INVALID, "blocks is NULL");
-    std::vector<BlockRec> recs(d->n_blocks);
-    std::vector<uint8_t> kinds(d->n_blocks);
-    std::vector<uint16_t> bricks;
-    std::vector<float4> palette;
-    std::vector<float2> pal_tab;
-    std::vector<float4> blk_tab(d->n_blocks);
-    for (size_t i = 0; i < d->n_blocks; i++) {
-        aicb_status fst = flatten_block(d->blocks[i], recs[i], kinds[i], bricks, palette, pal_tab);
-        if (fst != AICB_OK) return fst;
-        blk_tab[i] = block_entry(kinds[i], recs[i].pal_off, pal_tab, 0);
-    }
-
-    // the scene is the caller's once every step has succeeded; until then a failure frees what was uploaded
-    std::unique_ptr<aicb_scene> s(new aicb_scene());
-    s->ctx = ctx;
-    s->volume = (size_t)volume;
-    s->block_kind = kinds;
-    DeviceScene &ds = s->ds;
-    for (int a = 0; a < 3; a++) {
-        ds.lo[a] = d->bounds.lower[a];
-        ds.size[a] = (int32_t)d->bounds.size[a];
-    }
-    ds.wide_cells = d->n_blocks > 16384 ? 1 : 0;
-
-    // ---- cells: block id with its kind in the top bits ------------------------------------------
-    if (volume) {
-        for (size_t i = 0; i < volume; i++)
-            if (d->block_ids[i] >= d->n_blocks) return fail(AICB_ERR_INVALID, "block id out of range");
-        if (ds.wide_cells) {
-            std::vector<uint32_t> cells(volume);
-            for (size_t i = 0; i < volume; i++) cells[i] = cell_word(d->block_ids[i], kinds[d->block_ids[i]], true);
-            TRY(s->d_cells.upload(cells));
-            s->device_bytes += volume * 4;
-        } else {
-            std::vector<uint16_t> cells(volume);
-            for (size_t i = 0; i < volume; i++) cells[i] = (uint16_t)cell_word(d->block_ids[i], kinds[d->block_ids[i]], false);
-            TRY(s->d_cells.upload(cells));
-            s->device_bytes += volume * 2;
-        }
-        if (d->light) {
-            TRY(s->d_light.upload(d->light, volume * 4));
-            s->device_bytes += volume * 4;
-        }
-    }
-    if (!recs.empty()) {
-        TRY(s->d_blocks.upload(recs));
-        s->device_bytes += recs.size() * sizeof(BlockRec);
-    }
-    s->n_bricks = bricks.size();
-    s->n_palette = palette.size();
-    if (!bricks.empty()) {
-        TRY(s->d_bricks.upload(bricks));
-        s->device_bytes += bricks.size() * 2;
-    }
-    if (!palette.empty()) {
-        TRY(s->d_palette.upload(palette));
-        s->device_bytes += palette.size() * sizeof(float4);
-        TRY(s->d_pal_tab.upload(pal_tab));
-        s->device_bytes += pal_tab.size() * sizeof(float2);
-    }
-    if (!blk_tab.empty()) {
-        TRY(s->d_blk_tab.upload(blk_tab));
-        s->device_bytes += blk_tab.size() * sizeof(float4);
-    }
-    ds.cells = s->d_cells.get();
-    ds.light = s->d_light.get<uint32_t>();
-    ds.blocks = s->d_blocks.get<BlockRec>();
-    ds.bricks = s->d_bricks.get<uint16_t>();
-    ds.palette = s->d_palette.get<float4>();
-    ds.blk_tab = s->d_blk_tab.get<float4>();
-    ds.pal_tab = s->d_pal_tab.get<float2>();
-    ds.tables = ctx->d_lut.get<float>();
-    build_block_sky(d->sky, &ds);
-    TRY(aicb_light_scene_upload(s.get(), d));
-    *out = s.release();
-    return AICB_OK;
+    return scenes_create(&ctx, 1, d, out);
 }
 
 void aicb_scene_destroy(aicb_scene *s) {
     if (!s) return;
     cudaSetDevice(s->ctx->device);
-    if (s->ctx->last_scene == s) {   // its frame (if any) must be through with the scene's arrays
-        if (s->ctx->frame_in_flight) cudaEventSynchronize(s->ctx->ev1.get());
+    wait_context(s->ctx);
+    if (s->ctx->last_scene == s) {
         s->ctx->last_scene = nullptr;
         s->ctx->frame_in_flight = false;
     }
@@ -958,7 +1009,7 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
                  dz = (uint32_t)(cubes[i][2] - ds.lo[2]);
         if (dx >= (uint32_t)ds.size[0] || dy >= (uint32_t)ds.size[1] || dz >= (uint32_t)ds.size[2])
             return fail(AICB_ERR_INVALID, "cube out of bounds");
-        if (ids[i] >= s->block_kind.size()) return fail(AICB_ERR_INVALID, "block id out of range");
+        if (ids[i] >= s->blocks.block_count()) return fail(AICB_ERR_INVALID, "block id out of range");
     }
     // one pinned staging buffer, one H2D copy, one scatter kernel per batch; a cube named twice keeps its
     // last value (the scatter is parallel, so duplicates are resolved here)
@@ -983,7 +1034,7 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
         if (!s->h_ids.empty()) s->h_ids[idx] = ids[i];
         CubeDelta op;
         op.idx = (uint32_t)idx;
-        op.cell = cell_word(ids[i], s->block_kind[ids[i]], ds.wide_cells);
+        op.cell = cell_word(ids[i], s->blocks.kind[ids[i]], ds.wide_cells);
         op.has_light = (light && s->d_light) ? 1u : 0u;
         op.light = 0;
         if (op.has_light) std::memcpy(&op.light, light[i], 4);
@@ -1003,122 +1054,10 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
 // existing block indices.  New voxel data is appended to the brick pool and the palette (the replaced ranges are
 // reclaimed by the next aicb_scene_create); cubes that hold a block whose classification changed are re-encoded.
 // Does not queue light updates: call aicb_light_evaluate afterwards if the change affects light.
-// Validates and flattens the new definitions of aicb_scene_update_blocks without touching the scene.
-static aicb_status flatten_update(const aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n,
-                                  std::vector<BlockRec> &recs, std::vector<uint8_t> &kinds, std::vector<uint16_t> &bricks,
-                                  std::vector<float4> &palette, std::vector<float2> &pal_tab, bool *any_kind_changed) {
-    const size_t n_blocks = s->block_kind.size();
-    recs.resize(n);
-    kinds.resize(n);
-    for (size_t i = 0; i < n; i++) {
-        if (indices[i] >= n_blocks) return fail(AICB_ERR_INVALID, "block index out of range (new indices need a new scene)");
-        aicb_status fst = flatten_block(descs[i], recs[i], kinds[i], bricks, palette, pal_tab);
-        if (fst != AICB_OK) return fst;
-    }
-    if (s->n_bricks + bricks.size() > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
-    *any_kind_changed = false;
-    for (size_t i = 0; i < n; i++) *any_kind_changed |= s->block_kind[indices[i]] != kinds[i];
-    if (*any_kind_changed && s->h_ids.size() != s->volume)
-        return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
-    return AICB_OK;
-}
-
-aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
-    if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    std::vector<BlockRec> recs;
-    std::vector<uint8_t> kinds;
-    std::vector<uint16_t> bricks;
-    std::vector<float4> palette;
-    std::vector<float2> pal_tab;
-    bool any_kind_changed = false;
-    return flatten_update(s, indices, descs, n, recs, kinds, bricks, palette, pal_tab, &any_kind_changed);
-}
-
-// A new buffer `out`: the first `old_bytes` of `old`, then `add_bytes` from the host.
-static aicb_status appended(DeviceBuffer &out, const DeviceBuffer &old, size_t old_bytes, const void *add, size_t add_bytes) {
-    TRY(out.ensure(old_bytes + add_bytes));
-    if (old_bytes) CU(cudaMemcpy(out.get(), old.get(), old_bytes, cudaMemcpyDeviceToDevice));
-    CU(cudaMemcpy(out.get<char>() + old_bytes, add, add_bytes, cudaMemcpyHostToDevice));
-    return AICB_OK;
-}
-
 aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
     if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
-    aicb_ctx *ctx = s->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    if (n == 0) return AICB_OK;
-    const size_t n_blocks = s->block_kind.size();
-    std::vector<BlockRec> recs;
-    std::vector<uint8_t> kinds;
-    std::vector<uint16_t> bricks;
-    std::vector<float4> palette;
-    std::vector<float2> pal_tab;
-    bool any_kind_changed = false;
-    // validate and flatten everything before touching any state
-    aicb_status vst = flatten_update(s, indices, descs, n, recs, kinds, bricks, palette, pal_tab, &any_kind_changed);
-    if (vst != AICB_OK) return vst;
-    CU(cudaDeviceSynchronize());   // nothing (on any stream) may still be reading the arrays that are replaced
-
-    // ---- grow the pools: the new arrays are complete before any pointer of the scene changes ----------------
-    const size_t n_pal_old = s->n_palette / 2;   // palette entries (2 x float4 each)
-    DeviceBuffer nb, np, nt;
-    if (!bricks.empty()) TRY(appended(nb, s->d_bricks, s->n_bricks * 2, bricks.data(), bricks.size() * 2));
-    if (!palette.empty()) {
-        TRY(appended(np, s->d_palette, s->n_palette * sizeof(float4), palette.data(), palette.size() * sizeof(float4)));
-        TRY(appended(nt, s->d_pal_tab, n_pal_old * sizeof(float2), pal_tab.data(), pal_tab.size() * sizeof(float2)));
-    }
-    if (nb) {
-        s->d_bricks = std::move(nb);
-        s->ds.bricks = s->d_bricks.get<uint16_t>();
-        s->device_bytes += bricks.size() * 2;
-    }
-    if (np) {
-        s->d_palette = std::move(np);
-        s->ds.palette = s->d_palette.get<float4>();
-        s->d_pal_tab = std::move(nt);
-        s->ds.pal_tab = s->d_pal_tab.get<float2>();
-        s->device_bytes += palette.size() * sizeof(float4) + pal_tab.size() * sizeof(float2);
-    }
-    // ---- patch the block table ------------------------------------------------------------------------------
-    std::vector<uint8_t> kind_changed(n_blocks, 0);
-    for (size_t i = 0; i < n; i++) {
-        BlockRec &r = recs[i];
-        const float4 bt = block_entry(kinds[i], r.pal_off, pal_tab, (uint32_t)n_pal_old);
-        if (kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)s->n_bricks;
-        if (kinds[i] != KIND_INVISIBLE || !descs[i].is_air) r.pal_off += (uint32_t)n_pal_old;
-        CU(cudaMemcpy(s->d_blocks.get<BlockRec>() + indices[i], &r, sizeof r, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(s->d_blk_tab.get<float4>() + indices[i], &bt, sizeof bt, cudaMemcpyHostToDevice));
-        if (s->block_kind[indices[i]] != kinds[i]) {
-            kind_changed[indices[i]] = 1;
-            s->block_kind[indices[i]] = kinds[i];
-        }
-    }
-    s->n_bricks += bricks.size();
-    s->n_palette += palette.size();
-    // ---- cubes whose block changed its classification carry the kind in their cell word -------------------
-    if (any_kind_changed) {
-        std::vector<CubeDelta> ops;
-        for (size_t idx = 0; idx < s->volume; idx++) {
-            const uint16_t id = s->h_ids[idx];
-            if (!kind_changed[id]) continue;
-            CubeDelta op;
-            op.idx = (uint32_t)idx;
-            op.cell = cell_word(id, s->block_kind[id], s->ds.wide_cells);
-            op.light = 0;
-            op.has_light = 0;
-            ops.push_back(op);
-        }
-        if (!ops.empty()) {
-            DeviceBuffer d_ops;
-            TRY(d_ops.upload(ops));
-            scatter_cubes_kernel<<<(unsigned)((ops.size() + 127) / 128), 128, 0, ctx->stream.get()>>>(
-                d_ops.get<const CubeDelta>(), (uint32_t)ops.size(), s->ds.wide_cells, s->d_cells.get(), s->d_light.get<uint32_t>());
-            CU(cudaStreamSynchronize(ctx->stream.get()));
-        }
-    }
-    return aicb_light_blocks_update(s, indices, descs, n);
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return scenes_update_blocks(&s, 1, indices, descs, n);
 }
 
 // == SpaceChange::BlockIndex for indices past the table (palette.rs:207-210; UpdatingSpaceRaytracer::update appends
@@ -1126,11 +1065,7 @@ aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, con
 aicb_status aicb_scene_append_blocks(aicb_scene *s, const aicb_block_desc *descs, size_t n) {
     if (!s || (n && !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
-    CU(cudaSetDevice(s->ctx->device));
-    if (n == 0) return AICB_OK;
-    BlockAppend a;
-    TRY(append_blocks_validate(s, descs, n, &a));   // validate and flatten everything before touching any state
-    return append_blocks_apply(s, a, descs);
+    return scenes_append_blocks(&s, 1, descs, n);
 }
 
 aicb_status aicb_scene_upload_light(aicb_scene *s, const uint8_t (*light)[4], size_t n_texels) {

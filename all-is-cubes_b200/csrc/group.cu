@@ -290,18 +290,10 @@ void aicb_group_scene_destroy(aicb_group_scene *gs) {
 aicb_status aicb_group_scene_create(aicb_group *g, const aicb_scene_desc *d, aicb_group_scene **out) {
     if (!g || !d || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     *out = nullptr;
-    aicb_group_scene *gs = new aicb_group_scene();
-    gs->group = g;
-    for (aicb_ctx *c : g->ctx) {   // the scene is replicated (<= ~0.3 GB at 256^3), SURVEY §8(e)
-        aicb_scene *s = nullptr;
-        aicb_status st = aicb_scene_create(c, d, &s);
-        if (st != AICB_OK) {
-            aicb_group_scene_destroy(gs);
-            return st;
-        }
-        gs->scene.push_back(s);
-    }
-    *out = gs;
+    std::vector<aicb_scene *> scene(g->ctx.size());   // the scene is replicated (<= ~0.3 GB at 256^3), SURVEY §8(e)
+    ContextLocks lock(g->ctx);
+    TRY(scenes_create(g->ctx.data(), scene.size(), d, scene.data()));
+    *out = new aicb_group_scene{g, std::move(scene)};
     return AICB_OK;
 }
 
@@ -349,31 +341,15 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
 
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *gs, const uint16_t *indices, const aicb_block_desc *descs,
                                            size_t n) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    // the replicas hold the same block table: what replica 0 accepts every replica accepts, and a rejected update
-    // leaves them all as they were
-    aicb_status st = aicb_scene_check_blocks(gs->scene[0], indices, descs, n);
-    if (st != AICB_OK) return st;
-    for (aicb_scene *s : gs->scene) {
-        st = aicb_scene_update_blocks(s, indices, descs, n);
-        if (st != AICB_OK) return st;
-    }
-    return AICB_OK;
+    if (!gs || (n && (!indices || !descs))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    return scenes_update_blocks(gs->scene.data(), gs->scene.size(), indices, descs, n);
 }
 
 aicb_status aicb_group_scene_append_blocks(aicb_group_scene *gs, const aicb_block_desc *descs, size_t n) {
     if (!gs || (n && !descs)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     ContextLocks lock(gs->group->ctx);
-    if (n == 0) return AICB_OK;
-    // the replicas hold the same block table: replica 0's validation is every replica's, and a rejected call changes
-    // none; each replica then appends (and widens its cells, past 16384 blocks) on its own device
-    BlockAppend a;
-    TRY(append_blocks_validate(gs->scene[0], descs, n, &a));
-    for (aicb_scene *s : gs->scene) {
-        CU(cudaSetDevice(s->ctx->device));
-        TRY(append_blocks_apply(s, a, descs));
-    }
-    return AICB_OK;
+    return scenes_append_blocks(gs->scene.data(), gs->scene.size(), descs, n);
 }
 
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *gs, const uint8_t (*light)[4], size_t n_texels) {

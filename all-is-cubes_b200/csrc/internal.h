@@ -104,13 +104,6 @@ inline aicb_status create_event(Event &e, unsigned int flags) {
     return AICB_OK;
 }
 
-// Room for `bytes` in `buf`, of which the first `used` are kept.  A buffer that is too small is replaced by one of at
-// least twice its size, its `used` bytes copied on `stream`; the replaced buffer goes to `retired`, and the caller
-// frees it once nothing can read it any more (the copy, and any frame in flight).  Appending k elements one call at a
-// time thus reallocates O(log k) times.
-aicb_status grow_buffer(DeviceBuffer &buf, size_t used, size_t bytes, cudaStream_t stream,
-                        std::vector<DeviceBuffer> *retired);
-
 // A cube's cell word: its block id with the block's kind in the top bits (16-bit cells up to 16384 block ids).
 inline uint32_t cell_word(uint32_t id, uint8_t kind, bool wide) { return id | ((uint32_t)kind << (wide ? 16 : 14)); }
 
@@ -151,10 +144,9 @@ struct LightChart {
 };
 
 // A scene's light propagation state (light.cu), in two parts: what every replica's own walks need, and what replica 0
-// alone holds and the other replicas' kernels reach through peer pointers.  Between light calls only the block records,
-// the queue and the set of changed cubes hold anything, so round buffers serve other jobs too (the accessors below).
+// alone holds and the other replicas' kernels reach through peer pointers.  Between light calls only the queue and the
+// set of changed cubes hold anything, so round buffers serve other jobs too (the accessors below).
 struct LightState {
-    DeviceBuffer blocks;   // every replica: LightBlockDev per block, uploaded with the scene (aicb_light_scene_upload)
     struct Own {
         DeviceBuffer sky_term;         // per chart node: the sky light its bundle collects (end_of_ray) from this sky
         DeviceBuffer overflow;         // list positions whose chain walk overflowed (k_compute_overflow's work)
@@ -186,8 +178,9 @@ struct aicb_ctx {
     int device = 0;
     int num_sms = 0;
     Stream stream;
-    Event ev0, ev1;
-    Event ev_join;               // this context's stream reached a point another context's stream waits for (fan_in)
+    Event ev0, ev1;              // the start and end of the context's last frame, and nothing else (wait_context)
+    Event ev_light[2];           // the start and end of the last light propagation (light_stats[3])
+    Event ev_join;              // this context's stream reached a point another context's stream waits for (fan_in)
     Event ev_k[5];               // AICB_PROFILE_KERNELS
     bool profile_kernels = false;
     bool stage_timing = true;    // record the per-kernel events of a frame (aicb_render_info::stage_ms)
@@ -222,23 +215,41 @@ struct aicb_ctx {
     std::mutex mu;
 };
 
+// A scene's block table: everything indexed by block id or by pool offset, on the device and on the host.  It is
+// written in one way (aicb200.cu): definitions are flattened against the table, then placed in it, appended at the
+// next ids or written over existing ones, with their voxel data appended to the pools (a replaced range is not
+// reclaimed).  Elements in use: per block id, block_count(); in the pools, n_bricks and n_palette.  The buffers may be
+// larger: they grow geometrically (grow_buffer).
+struct BlockTable {
+    DeviceBuffer blocks;    // per block id: BlockRec
+    DeviceBuffer blk_tab;   // per block id: the pal_tab pair and the palette entry of single-voxel blocks
+    DeviceBuffer light;     // per block id: LightBlockDev (light propagation)
+    DeviceBuffer bricks;    // u16 voxel words of the recursive blocks
+    DeviceBuffer palette;   // two float4 per palette entry
+    DeviceBuffer pal_tab;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
+    std::vector<uint8_t> kind;           // per block id: its kind, which its cubes' cell words carry
+    std::vector<uint32_t> light_flags;   // per block id: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission
+    size_t n_bricks = 0, n_palette = 0;  // u16 words, float4s
+
+    size_t block_count() const { return kind.size(); }
+    // the scene's pointers into the current buffers (LightParams::blocks is read from `light` by light_params)
+    void bind(aicb::DeviceScene &ds) const {
+        ds.blocks = blocks.get<aicb::BlockRec>();
+        ds.blk_tab = blk_tab.get<float4>();
+        ds.bricks = bricks.get<uint16_t>();
+        ds.palette = palette.get<float4>();
+        ds.pal_tab = pal_tab.get<float2>();
+    }
+};
+
 struct aicb_scene {
     aicb_ctx *ctx = nullptr;
     aicb::DeviceScene ds{};
-    std::vector<uint8_t> block_kind;   // host copy, for update_cubes
     size_t volume = 0;
     uint64_t device_bytes = 0;
     DeviceBuffer d_cells;
     DeviceBuffer d_light;
-    DeviceBuffer d_blocks;
-    DeviceBuffer d_bricks;
-    DeviceBuffer d_palette;
-    DeviceBuffer d_pal_tab;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
-    DeviceBuffer d_blk_tab;   // per block id: that pair and the palette entry of single-voxel blocks
-    // Elements in use: d_bricks / d_palette (aicb_scene_update_blocks and aicb_scene_append_blocks append) and, per block
-    // id, d_blocks / d_blk_tab / light.blocks (block_kind.size(); aicb_scene_append_blocks appends).  The buffers may
-    // be larger: appends grow them geometrically (grow_buffer).
-    size_t n_bricks = 0, n_palette = 0;
+    BlockTable blocks;
     // state of the last asynchronous render
     bool pending = false;
     uint64_t pending_rays = 0;
@@ -247,7 +258,6 @@ struct aicb_scene {
     bool pending_fused = false;    // shading and encode ran as one kernel (resolve_kernel)
     // ---- light propagation state (light.cu) ----
     std::vector<uint16_t> h_ids;            // host mirror of Space::contents (edits are applied in order on the host)
-    std::vector<uint32_t> h_block_light;    // per block: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission
     LightState light;
     uint32_t light_max_distance = 0;
     uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
@@ -305,27 +315,10 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
 aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
                             bool want_info);
 void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part);
-// aicb_scene_update_blocks' validation alone: AICB_OK if that call would accept the update (changes nothing)
-aicb_status aicb_scene_check_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
 }
 
-// aicb200.cu: aicb_scene_append_blocks in two steps, for one scene and for every replica of a group scene (whose block
-// tables are identical).  `append_blocks_validate` flattens the descriptors against `s` and changes nothing: records
-// and palette offsets relative to the appended data alone.  `append_blocks_apply` appends them (the caller holds s's
-// context lock, and s's device is current).
-struct BlockAppend {
-    std::vector<aicb::BlockRec> recs;
-    std::vector<uint8_t> kinds;
-    std::vector<uint16_t> bricks;
-    std::vector<float4> palette;
-    std::vector<float2> pal_tab;
-};
-aicb_status append_blocks_validate(const aicb_scene *s, const aicb_block_desc *descs, size_t n, BlockAppend *out);
-aicb_status append_blocks_apply(aicb_scene *s, const BlockAppend &a, const aicb_block_desc *descs);
-// light.cu: the light-side records of blocks appended to the table (h_block_light, light.blocks); the caller frees the
-// replaced buffer (`retired`) once the context's stream is past the copy.
-aicb_status aicb_light_blocks_append(aicb_scene *s, const aicb_block_desc *descs, size_t n,
-                                     std::vector<DeviceBuffer> *retired);
+// light.cu: the light-side record of a block definition (its flags are BlockTable::light_flags).
+LightBlockDev light_block(const aicb_block_desc &b);
 
 // ---- calls over several contexts ----------------------------------------------------------------------------------
 // A call that runs on several contexts lists them device 0's first, with a scene's replica on each (a group scene's
@@ -339,6 +332,14 @@ struct ContextLocks {
         for (aicb_ctx *c : ctx) locks.emplace_back(c->mu);
     }
 };
+
+// aicb200.cu: creating a scene and changing its block table, on each of n contexts (a group scene's replicas hold
+// identical tables).  The block definitions are validated and flattened once, against replica 0's table, and a new
+// scene's cells are encoded once; only then does each replica place them on its own device.
+aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out);
+aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t *indices, const aicb_block_desc *descs,
+                                 size_t n_blocks);
+aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks);
 
 // group.cu: the order between the listed contexts' streams: every other context's stream waits until device 0's has
 // reached this point (fan_out), or device 0's until every other one's has (fan_in, which leaves device 0 current).

@@ -657,7 +657,7 @@ LightParams light_params(LightReplicas r, size_t i) {
     LightParams P;
     std::memset(&P, 0, sizeof P);
     P.scene = s->ds;
-    P.blocks = s->light.blocks.get<LightBlockDev>();
+    P.blocks = s->blocks.light.get<LightBlockDev>();
     P.chart_pre = chart.pre.get<LightNodePre>();
     P.sky_term = own.sky_term.get<float4>();
     P.chains = chart.chains.get<LightChain>();
@@ -749,7 +749,7 @@ aicb_status propagate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, 
     const uint32_t n_tiles = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
     uint64_t total = 0, visits = 0, rounds = 0;
     uint32_t maxd = 0;
-    CU(cudaEventRecord(ctx->ev0.get(), st));
+    CU(cudaEventRecord(ctx->ev_light[0].get(), st));
     CU(cudaMemsetAsync(P.counters, 0, sizeof(LightCounters), st));
     k_tile_rebuild<<<blocks, 256, 0, st>>>(P, n_tiles);   // (fast_evaluate / edits write the priority bytes directly)
     const int ROUNDS_PER_SYNC = 8;
@@ -778,10 +778,10 @@ aicb_status propagate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, 
         rounds += ROUNDS_PER_SYNC;
         if (h.priority <= P.epsilon_priority) break;   // the batch's last round found nothing above epsilon
     }
-    CU(cudaEventRecord(ctx->ev1.get(), st));
-    CU(cudaEventSynchronize(ctx->ev1.get()));
+    CU(cudaEventRecord(ctx->ev_light[1].get(), st));
+    CU(cudaEventSynchronize(ctx->ev_light[1].get()));
     float ms = 0.0f;
-    CU(cudaEventElapsedTime(&ms, ctx->ev0.get(), ctx->ev1.get()));
+    CU(cudaEventElapsedTime(&ms, ctx->ev_light[0].get(), ctx->ev_light[1].get()));
     s->light_stats[0] = total;
     s->light_stats[1] = visits;
     s->light_stats[2] = rounds;
@@ -792,7 +792,9 @@ aicb_status propagate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, 
     return AICB_OK;
 }
 
-// The light-side record of a block definition: its face colours, emission and flags (which h_block_light mirrors).
+}  // namespace
+
+// The light-side record of a block definition (internal.h): its face colours, emission and flags.
 LightBlockDev light_block(const aicb_block_desc &b) {
     LightBlockDev o;
     std::memset(&o, 0, sizeof o);
@@ -806,8 +808,6 @@ LightBlockDev light_block(const aicb_block_desc &b) {
     o.flags = fl;
     return o;
 }
-
-}  // namespace
 
 // ---------------------------------------------------------------------------------------------
 // a scene's light state (internal.h)
@@ -884,51 +884,6 @@ aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas)
         shared = std::move(sh);
         s->device_bytes += vol * 10 + change_bytes + (group ? dirty_bytes : 0);
     }
-    return AICB_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// called from aicb200.cu
-// ---------------------------------------------------------------------------------------------
-aicb_status aicb_light_scene_upload(aicb_scene *s, const aicb_scene_desc *d) {
-    s->light_max_distance = d->light_max_distance;
-    if (s->volume) s->h_ids.assign(d->block_ids, d->block_ids + s->volume);
-    std::vector<LightBlockDev> lb(d->n_blocks);
-    s->h_block_light.resize(d->n_blocks);
-    for (size_t i = 0; i < d->n_blocks; i++) {
-        lb[i] = light_block(d->blocks[i]);
-        s->h_block_light[i] = lb[i].flags;
-    }
-    if (!lb.empty()) {
-        TRY(s->light.blocks.upload(lb));
-        s->device_bytes += lb.size() * sizeof(LightBlockDev);
-    }
-    return AICB_OK;
-}
-
-// the light-side records of replaced block definitions (aicb_scene_update_blocks)
-aicb_status aicb_light_blocks_update(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
-    for (size_t i = 0; i < n; i++) {
-        const LightBlockDev o = light_block(descs[i]);
-        if (indices[i] < s->h_block_light.size()) s->h_block_light[indices[i]] = o.flags;
-        if (s->light.blocks)
-            CU(cudaMemcpy(s->light.blocks.get<LightBlockDev>() + indices[i], &o, sizeof o, cudaMemcpyHostToDevice));
-    }
-    return AICB_OK;
-}
-
-// the light-side records of blocks appended to the table (aicb_scene_append_blocks), queued on the context's stream
-aicb_status aicb_light_blocks_append(aicb_scene *s, const aicb_block_desc *descs, size_t n,
-                                     std::vector<DeviceBuffer> *retired) {
-    const size_t count = s->h_block_light.size();
-    std::vector<LightBlockDev> lb(n);
-    for (size_t i = 0; i < n; i++) lb[i] = light_block(descs[i]);
-    cudaStream_t stream = s->ctx->stream.get();
-    TRY(grow_buffer(s->light.blocks, count * sizeof(LightBlockDev), (count + n) * sizeof(LightBlockDev), stream, retired));
-    CU(cudaMemcpyAsync(s->light.blocks.get<LightBlockDev>() + count, lb.data(), n * sizeof(LightBlockDev),
-                       cudaMemcpyHostToDevice, stream));
-    for (const LightBlockDev &o : lb) s->h_block_light.push_back(o.flags);
-    s->device_bytes += n * sizeof(LightBlockDev);
     return AICB_OK;
 }
 
@@ -1020,7 +975,7 @@ aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3],
     for (size_t i = 0; i < n_edits; i++) {
         uint32_t idx;
         if (!index_of(cubes[i][0], cubes[i][1], cubes[i][2], &idx)) return aicb_fail(AICB_ERR_INVALID, "cube out of bounds");
-        if (new_ids[i] >= s->h_block_light.size()) return aicb_fail(AICB_ERR_INVALID, "block id out of range");
+        if (new_ids[i] >= s->blocks.light_flags.size()) return aicb_fail(AICB_ERR_INVALID, "block id out of range");
     }
     for (size_t i = 0; i < n_edits; i++) {
         uint32_t idx;
@@ -1028,8 +983,8 @@ aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3],
         if (s->h_ids[idx] == new_ids[i]) continue;  // Mutation::set of the same block changes nothing
         s->h_ids[idx] = new_ids[i];
         EditOp &o = op_of(idx);
-        o.cell = cell_word(new_ids[i], s->block_kind[new_ids[i]], ds.wide_cells);
-        const uint32_t fl = s->h_block_light[new_ids[i]];
+        o.cell = cell_word(new_ids[i], s->blocks.kind[new_ids[i]], ds.wide_cells);
+        const uint32_t fl = s->blocks.light_flags[new_ids[i]];
         if ((fl & LB_ALL_OPAQUE) && !(fl & LB_EMISSIVE)) {  // opaque_for_light_computation
             o.set_opaque = 1;
             o.pending_op = 1;
@@ -1042,7 +997,7 @@ aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3],
             if (!index_of(cubes[i][0] + (a == 0 ? sgn : 0), cubes[i][1] + (a == 1 ? sgn : 0), cubes[i][2] + (a == 2 ? sgn : 0), &nidx))
                 continue;
             const int opp = (f < 3) ? f + 3 : f - 3;
-            if (!((s->h_block_light[s->h_ids[nidx]] >> opp) & 1u)) op_of(nidx).pending_op = 2;
+            if (!((s->blocks.light_flags[s->h_ids[nidx]] >> opp) & 1u)) op_of(nidx).pending_op = 2;
         }
     }
     if (!ops.empty()) {

@@ -42,14 +42,6 @@ struct LightNodePre {
 };
 static_assert(sizeof(LightNodePre) == 32, "LightNodePre must be 32 bytes");
 
-// The EvaluatedBlock members light reads (evaluated.rs:189-272), 128 bytes.
-struct LightBlockDev {
-    float face_color[7][4];  // Within, NX..PZ (face7_color)
-    float emission[3];
-    uint32_t flags;          // bits 0-5 opaque[NX..PZ], 6 all opaque, 7 visible_or_animated, 8 emission != 0
-};
-static_assert(sizeof(LightBlockDev) == 128, "LightBlockDev must be 128 bytes");
-
 // The chart as chains.  99 % of the chart's nodes have exactly one child, with bit-identical weights (they carry the
 // same rays): the tree is 1043 chains (maximal single-child paths; 602 of them end in leaves) joined at 441 branching
 // nodes, 8 chain levels deep.  A chain's nodes are consecutive in preorder.  One record per chain, numbered breadth

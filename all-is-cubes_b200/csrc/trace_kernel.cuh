@@ -43,6 +43,15 @@
 #include <cuda_fp16.h>
 #endif
 
+// The EvaluatedBlock members light reads (evaluated.rs:189-272), 128 bytes: light propagation's per-block record
+// (light_kernel.cuh), here so that the host code that builds a scene's block table sees it too.
+struct LightBlockDev {
+    float face_color[7][4];  // Within, NX..PZ (face7_color)
+    float emission[3];
+    uint32_t flags;          // bits 0-5 opaque[NX..PZ], 6 all opaque, 7 visible_or_animated, 8 emission != 0
+};
+static_assert(sizeof(LightBlockDev) == 128, "LightBlockDev must be 128 bytes");
+
 namespace aicb {
 
 // ---- device-side scene -------------------------------------------------------------------------

@@ -202,7 +202,9 @@ aicb_status aicb_scene_update_cubes(aicb_scene *, const int32_t (*cubes)[3], con
 /* SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; updating.rs:128-150): new definitions for EXISTING
  * block indices (an index beyond the table is rejected: aicb_scene_append_blocks adds new ones).  Voxel data is appended to the device pools; cubes
  * holding a block whose classification (invisible / single voxel / voxel brick) changed are re-encoded.  Light is not
- * re-propagated (call aicb_light_evaluate).  GPU test: tests/test_gpu_parity.py::test_block_definition_update_equals_fresh_snapshot. */
+ * re-propagated (call aicb_light_evaluate).  The call first waits for the context's frame in flight and the work queued
+ * on the context's stream, and returns once its own device writes are done; it does not wait for other contexts, or
+ * for other work on the caller's streams.  GPU test: tests/test_gpu_parity.py::test_block_definition_update_equals_fresh_snapshot. */
 aicb_status aicb_scene_update_blocks(aicb_scene *, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
 /* SpaceChange::BlockIndex for indices past the table (palette.rs:207-210; UpdatingSpaceRaytracer::update appends them,
  * updating.rs:145-151): the blocks become indices [count, count + n) of the scene's table, where count is the table's
