@@ -100,6 +100,9 @@ def load_library() -> C.CDLL:
     lib.aicb_light_edit_and_propagate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8,
                                                   C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
     lib.aicb_light_download.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    for prefix in ("aicb_light", "aicb_group_light"):
+        getattr(lib, prefix + "_relight_blocks").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8,
+                                                             C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
     lib.aicb_light_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     lib.aicb_render_text.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p, C.c_size_t,
                                      C.POINTER(abi.RenderInfo)]
@@ -693,7 +696,8 @@ class SpaceRaytracer:
                                                       lt.ctypes.data if lt is not None else None, c.shape[0]))
 
     def update_blocks(self, indices, blocks):
-        """SpaceChange::BlockEvaluation / BlockIndex: new definitions for existing block indices."""
+        """SpaceChange::BlockEvaluation / BlockIndex: new definitions for existing block indices.  Light is not touched:
+        light_relight_blocks(indices) follows it on a lit scene."""
         idx = np.ascontiguousarray(indices, dtype=np.uint16)
         arr = _block_descs(blocks)
         _check(load_library().aicb_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
@@ -731,6 +735,12 @@ class SpaceRaytracer:
                                                             C.byref(n), C.byref(md)))
         return int(n.value), int(md.value)
 
+    def light_relight_blocks(self, indices, epsilon: int = 0):
+        """The light side of SpaceChange::BlockEvaluation: after update_blocks(indices, ...), Mutation::set's light rule
+        (modified_cube_needs_update) for every cube holding one of the indices, then evaluate_light(epsilon)
+        -> (updates, max_difference)"""
+        return _light_relight_blocks(load_library().aicb_light_relight_blocks, self.handle, indices, epsilon)
+
     def light_stats(self) -> dict:
         """Counters of the last propagation: cube updates, chart node visits, rounds, device seconds."""
         out = (C.c_uint64 * 4)()
@@ -757,6 +767,13 @@ class SpaceRaytracer:
     def upload_light(self, light: np.ndarray):
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
         _check(load_library().aicb_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
+
+
+def _light_relight_blocks(fn, handle, indices, epsilon):
+    idx = np.ascontiguousarray(indices, dtype=np.uint16).reshape(-1)
+    n, md = C.c_uint64(0), C.c_uint8(0)
+    _check(fn(handle, idx.ctypes.data, idx.size, epsilon, C.byref(n), C.byref(md)))
+    return int(n.value), int(md.value)
 
 
 def _light_changes_count(count_fn, handle) -> int:
@@ -989,6 +1006,11 @@ class GroupScene:
         _check(load_library().aicb_group_light_edit_and_propagate(self.handle, c.ctypes.data, ids.ctypes.data, c.shape[0],
                                                                   epsilon, C.byref(n), C.byref(md)))
         return int(n.value), int(md.value)
+
+    def light_relight_blocks(self, indices, epsilon: int = 0):
+        """SpaceRaytracer.light_relight_blocks on the group: every replica finds the cubes in its own cells; device 0
+        queues them -> (updates, max_difference)"""
+        return _light_relight_blocks(load_library().aicb_group_light_relight_blocks, self.handle, indices, epsilon)
 
     def light_stats(self) -> dict:
         """Counters of the last light call, summed over the devices; device seconds are device 0's (it waits for every

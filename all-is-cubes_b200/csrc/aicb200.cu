@@ -1053,7 +1053,7 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
 // updating.rs:128-150 by re-running TracingBlock::from_block for the changed indices): replace the definition of
 // existing block indices.  New voxel data is appended to the brick pool and the palette (the replaced ranges are
 // reclaimed by the next aicb_scene_create); cubes that hold a block whose classification changed are re-encoded.
-// Does not queue light updates: call aicb_light_evaluate afterwards if the change affects light.
+// Does not touch light: aicb_light_relight_blocks with the same indices applies the light side of the change.
 aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
     if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);

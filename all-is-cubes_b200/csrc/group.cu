@@ -426,6 +426,15 @@ aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int3
     return light_edit_and_propagate(r, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
 }
 
+aicb_status aicb_group_light_relight_blocks(aicb_group_scene *gs, const uint16_t *indices, size_t n, uint8_t epsilon,
+                                            uint64_t *updates_done, uint8_t *max_diff) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    LightReplicas r;
+    TRY(light_replicas(gs, &r));
+    return light_relight_blocks(r, indices, n, epsilon, updates_done, max_diff);
+}
+
 aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t (*out)[4], size_t n_texels) {
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (replica < 0 || (size_t)replica >= gs->scene.size()) return aicb_fail(AICB_ERR_INVALID, "no such replica");

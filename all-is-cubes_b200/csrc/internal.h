@@ -375,6 +375,8 @@ aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_d
                            uint64_t *node_visits);
 aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
+aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
+                                 uint64_t *updates_done, uint8_t *max_diff);
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels);
 // The set of changed cubes of replica 0 (the other replicas' texels are identical); the caller holds the locks.
 aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed);

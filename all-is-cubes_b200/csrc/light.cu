@@ -560,6 +560,64 @@ __global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint
     else if (op.pending_op == 2) P.pending[op.idx] = PRIO_NEWLY_VISIBLE;
 }
 
+// modified_cube_needs_update (updater.rs:135-173) for a cube that holds block `id`, if `id` is one of the redefined
+// indices (`s_mask`, one bit per block index): k_edits' writes for that block, then the face neighbours whose own face
+// toward the cube is not opaque are queued.  Only `queue` (device 0 of a group) touches the queue and the set.
+// No two threads write one pending byte with different values: a cube opaque for light is opaque on every face, so no
+// neighbour queues it.
+__device__ __forceinline__ void relight_cube(const LightParams &P, const uint32_t *s_mask, uint32_t idx, uint32_t id,
+                                             uint32_t queue) {
+    if (!((s_mask[id >> 5] >> (id & 31u)) & 1u)) return;
+    const uint32_t fl = __ldg(&P.blocks[id].flags);
+    if ((fl & LB_ALL_OPAQUE) && !(fl & LB_EMISSIVE)) {   // opaque_for_light_computation
+        const_cast<uint32_t *>(P.scene.light)[idx] = TX_OPAQUE;
+        if (!queue) return;
+        mark_changed(P, idx);
+        P.pending[idx] = 0;
+    } else {
+        if (!queue) return;
+        P.pending[idx] = PRIO_NEWLY_VISIBLE;
+    }
+    int x, y, z;
+    cube_of(P.scene, idx, x, y, z);
+#pragma unroll
+    for (int f = 0; f < 6; f++) {
+        const int s = (f < 3) ? -1 : 1, a = f % 3, opp = (f < 3) ? f + 3 : f - 3;
+        uint32_t nidx;
+        if (!cube_index(P.scene, x + (a == 0 ? s : 0), y + (a == 1 ? s : 0), z + (a == 2 ? s : 0), &nidx)) continue;
+        if (!((__ldg(&P.blocks[block_id_at(P.scene, nidx)].flags) >> opp) & 1u)) P.pending[nidx] = PRIO_NEWLY_VISIBLE;
+    }
+}
+
+// The scan of aicb_light_relight_blocks: every cell of the scene, 16 bytes per load (8 u16 cells or 4 u32 cells,
+// decoded as block_id_at does), against the redefined indices in shared memory (65 536 bits).  Grid-stride; the cells
+// past the last whole vector are read one by one.
+constexpr uint32_t RELIGHT_MASK_WORDS = 65536 / 32;
+__global__ void __launch_bounds__(256) k_relight_blocks(const LightParams P, const uint32_t *mask, uint32_t queue) {
+    __shared__ uint32_t s_mask[RELIGHT_MASK_WORDS];
+    for (uint32_t i = threadIdx.x; i < RELIGHT_MASK_WORDS; i += blockDim.x) s_mask[i] = mask[i];
+    __syncthreads();
+    const DeviceScene &S = P.scene;
+    const uint32_t t0 = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+    const uint4 *cells = (const uint4 *)S.cells;
+    const uint32_t per = S.wide_cells ? 4u : 8u, n_vec = P.volume / per;
+    for (uint32_t v = t0; v < n_vec; v += stride) {
+        const uint4 c = __ldg(cells + v);
+        const uint32_t w[4] = {c.x, c.y, c.z, c.w}, base = v * per;
+        if (S.wide_cells) {
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++) relight_cube(P, s_mask, base + k, w[k] & 0xffffu, queue);
+        } else {
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++) {
+                relight_cube(P, s_mask, base + 2 * k, w[k] & 0x3fffu, queue);
+                relight_cube(P, s_mask, base + 2 * k + 1, (w[k] >> 16) & 0x3fffu, queue);
+            }
+        }
+    }
+    for (uint32_t idx = n_vec * per + t0; idx < P.volume; idx += stride) relight_cube(P, s_mask, idx, block_id_at(S, idx), queue);
+}
+
 // Taking the set of changed cubes: an ordered stream compaction of the bitmap.  A chunk is the CHANGES_CHUNK_WORDS
 // words of bits (32 768 cubes) one 256-thread block reads, four consecutive words per thread.
 constexpr uint32_t CHANGES_CHUNK_WORDS = 1024;
@@ -1024,6 +1082,40 @@ aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3],
     return propagate(r, epsilon, updates_done, max_diff, nullptr);
 }
 
+// modified_cube_needs_update (updater.rs:135-173) for every cube that holds one of the indices, with the block's current
+// definition, then evaluate_light(epsilon).  The cubes are found on the device (k_relight_blocks), on every replica
+// against its own cells, ordered on each replica's stream behind the cube updates queued there; only replica 0 holds
+// the queue and the set of changed cubes.
+aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
+                                 uint64_t *updates_done, uint8_t *max_diff) {
+    if (n && !indices) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    aicb_scene *s = r.scene[0];
+    std::vector<uint32_t> mask(RELIGHT_MASK_WORDS, 0u);
+    for (size_t i = 0; i < n; i++) {
+        if (indices[i] >= s->blocks.block_count()) return aicb_fail(AICB_ERR_INVALID, "block index out of range");
+        mask[indices[i] >> 5] |= 1u << (indices[i] & 31u);
+    }
+    TRY(ensure_replicas(r));
+    if (n) {
+        std::vector<DeviceBuffer> d_mask(r.n);
+        for (size_t i = 0; i < r.n; i++) {
+            aicb_ctx *c = r.ctx[i];
+            cudaStream_t stream = c->stream.get();
+            CU(cudaSetDevice(c->device));
+            TRY(d_mask[i].ensure(mask.size() * 4));
+            CU(cudaMemcpyAsync(d_mask[i].get(), mask.data(), mask.size() * 4, cudaMemcpyHostToDevice, stream));
+            k_relight_blocks<<<c->num_sms * 8, 256, 0, stream>>>(light_params(r, i), d_mask[i].get<uint32_t>(), i == 0);
+            CU(cudaGetLastError());
+        }
+        for (size_t i = 0; i < r.n; i++) {
+            CU(cudaSetDevice(r.ctx[i]->device));
+            CU(cudaStreamSynchronize(r.ctx[i]->stream.get()));
+        }
+        CU(cudaSetDevice(s->ctx->device));
+    }
+    return propagate(r, epsilon, updates_done, max_diff, nullptr);
+}
+
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     if (!s || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n_texels != s->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
@@ -1152,6 +1244,13 @@ aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[
     if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return light_edit_and_propagate({&s, &s->ctx, 1}, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+}
+
+aicb_status aicb_light_relight_blocks(aicb_scene *s, const uint16_t *indices, size_t n, uint8_t epsilon,
+                                      uint64_t *updates_done, uint8_t *max_diff) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_relight_blocks({&s, &s->ctx, 1}, indices, n, epsilon, updates_done, max_diff);
 }
 
 aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 8 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 9 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -292,6 +292,8 @@ unsafe extern "C" {
                                chart_node_visits: *mut u64) -> aicb_status;
     pub fn aicb_light_edit_and_propagate(s: *mut aicb_scene, cubes: *const [i32; 3], new_ids: *const u16, n_edits: usize,
                                          epsilon: u8, updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
+    pub fn aicb_light_relight_blocks(s: *mut aicb_scene, indices: *const u16, n: usize, epsilon: u8, updates_done: *mut u64,
+                                     max_diff: *mut u8) -> aicb_status;
     pub fn aicb_light_download(s: *mut aicb_scene, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_light_stats(s: *const aicb_scene, out: *mut [u64; 4]) -> aicb_status;
     pub fn aicb_light_changes_count(s: *const aicb_scene, n_changed: *mut usize) -> aicb_status;
@@ -305,6 +307,8 @@ unsafe extern "C" {
     pub fn aicb_group_light_edit_and_propagate(gs: *mut aicb_group_scene, cubes: *const [i32; 3], new_ids: *const u16,
                                                n_edits: usize, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8)
                                                -> aicb_status;
+    pub fn aicb_group_light_relight_blocks(gs: *mut aicb_group_scene, indices: *const u16, n: usize, epsilon: u8,
+                                           updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
     pub fn aicb_group_light_download(gs: *mut aicb_group_scene, replica: c_int, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_group_light_stats(gs: *const aicb_group_scene, out: *mut [u64; 4]) -> aicb_status;
     pub fn aicb_group_light_changes_count(gs: *const aicb_group_scene, n_changed: *mut usize) -> aicb_status;

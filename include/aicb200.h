@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 8
+#define AICB_ABI_VERSION 9
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -202,7 +202,7 @@ aicb_status aicb_scene_update_cubes(aicb_scene *, const int32_t (*cubes)[3], con
 /* SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; updating.rs:128-150): new definitions for EXISTING
  * block indices (an index beyond the table is rejected: aicb_scene_append_blocks adds new ones).  Voxel data is appended to the device pools; cubes
  * holding a block whose classification (invisible / single voxel / voxel brick) changed are re-encoded.  Light is not
- * re-propagated (call aicb_light_evaluate).  The call first waits for the context's frame in flight and the work queued
+ * touched: call aicb_light_relight_blocks with the same indices afterwards to bring the light up to date.  The call first waits for the context's frame in flight and the work queued
  * on the context's stream, and returns once its own device writes are done; it does not wait for other contexts, or
  * for other work on the caller's streams.  GPU test: tests/test_gpu_parity.py::test_block_definition_update_equals_fresh_snapshot. */
 aicb_status aicb_scene_update_blocks(aicb_scene *, const uint16_t *indices, const aicb_block_desc *descs, size_t n);
@@ -389,7 +389,8 @@ aicb_status aicb_group_scene_update_cubes(aicb_group_scene *, const int32_t (*cu
 aicb_status aicb_group_render_srgb8(aicb_group_scene *, const aicb_camera *, const aicb_options *,
                                     uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
 /* aicb_scene_update_blocks (SpaceChange::BlockEvaluation / BlockIndex, updating.rs:128-150) and aicb_scene_upload_light
- * on every replica.  The update is validated against replica 0 first: a rejected call changes no replica. */
+ * on every replica.  The update is validated against replica 0 first: a rejected call changes no replica.  The update
+ * does not touch light: aicb_group_light_relight_blocks follows it. */
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *, const uint16_t *indices, const aicb_block_desc *descs,
                                            size_t n);
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *, const uint8_t (*light)[4], size_t n_texels);
@@ -481,10 +482,26 @@ aicb_status aicb_light_evaluate(aicb_scene *, uint8_t epsilon, uint64_t *updates
 aicb_status aicb_light_edit_and_propagate(aicb_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                           size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                           uint8_t *max_diff);
+/* The light side of SpaceChange::BlockEvaluation: after aicb_scene_update_blocks gave `indices` new definitions, apply
+ * Mutation::set's light rule (side_effects_of_set -> modified_cube_needs_update, space.rs:499-531,
+ * space/light/updater.rs:135-173) to every cube that holds one of them, with the block's current definition, then
+ * evaluate_light(epsilon) as aicb_light_edit_and_propagate does.  The same-block skip of Mutation::set does not apply:
+ *   - a block opaque for light (every face opaque, no emission): its cubes' texels become OPAQUE, even over OPAQUE,
+ *     their queued updates are cancelled and they enter the set of changed cubes;
+ *   - any other block: its cubes are queued at Priority::NEWLY_VISIBLE;
+ *   - either way, every in-bounds face neighbour of the cube whose own face toward it is not opaque is queued at
+ *     NEWLY_VISIBLE.
+ * The cubes are found on the device by a scan of the cells (2 or 4 bytes per cube), ordered behind the cube updates
+ * queued on the context.  Duplicates are allowed; an index no cube holds adds nothing; n == 0 only relaxes.
+ * AICB_ERR_INVALID, with nothing changed: NULL with n > 0, an index >= the table's size, or LightPhysics::None.
+ * The counters of aicb_light_stats are the propagation's (the scan is not in its device time).  aicb_scene_update_blocks
+ * itself does not touch light.  GPU test: tests/test_gpu_light_relight.py. */
+aicb_status aicb_light_relight_blocks(aicb_scene *, const uint16_t *indices, size_t n, uint8_t epsilon,
+                                      uint64_t *updates_done, uint8_t *max_diff);
 aicb_status aicb_light_download(aicb_scene *, uint8_t (*out)[4], size_t n_texels);
-/* Counters of the last propagation (aicb_light_evaluate / aicb_light_edit_and_propagate) on this scene:
- * out[0] cube updates (compute_light calls, updater.rs:368), out[1] chart nodes visited by them, out[2] relaxation
- * rounds queued, out[3] device time of the propagation in microseconds (CUDA events on the context's stream).
+/* Counters of the last propagation (aicb_light_evaluate / aicb_light_edit_and_propagate / aicb_light_relight_blocks)
+ * on this scene: out[0] cube updates (compute_light calls, updater.rs:368), out[1] chart nodes visited by them,
+ * out[2] relaxation rounds queued, out[3] device time of the propagation in microseconds (CUDA events on the context's stream).
  * After aicb_light_compute: out[0] cubes computed, out[1] chart nodes visited, out[2] cubes whose walk needed more
  * term slots than the chain walk holds and took the lockstep walk instead, out[3] 0. */
 aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
@@ -492,6 +509,7 @@ aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
  * it when
  *   - aicb_light_edit_and_propagate sets it to a different block that is opaque for light, which stores OPAQUE even
  *     over OPAQUE (modified_cube_needs_update, space/light/updater.rs:153-161);
+ *   - aicb_light_relight_blocks finds it holding a redefined block that is opaque for light (OPAQUE even over OPAQUE);
  *   - a relaxation round stores a value with difference_priority > 0 (apply_light_update, updater.rs:313-317);
  *   - a round writes a guess into an Uninitialized neighbour (updater.rs:335-338);
  *   - aicb_light_fast_evaluate changes its texel.  The reference announces nothing there (fast_evaluate_light has a
@@ -529,6 +547,10 @@ aicb_status aicb_group_light_evaluate(aicb_group_scene *, uint8_t epsilon, uint6
 aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff);
+/* aicb_light_relight_blocks on the group: the indices are checked against replica 0's table; every replica scans its
+ * own cells and writes its own OPAQUE texels; device 0 alone queues and records the changed cubes. */
+aicb_status aicb_group_light_relight_blocks(aicb_group_scene *, const uint16_t *indices, size_t n, uint8_t epsilon,
+                                            uint64_t *updates_done, uint8_t *max_diff);
 /* Replica `replica` (0 .. group size - 1) of the light volume. */
 aicb_status aicb_group_light_download(aicb_group_scene *, int replica, uint8_t (*out)[4], size_t n_texels);
 /* aicb_light_stats of the group's last light call: counters summed over the devices; out[3] is device 0's device time

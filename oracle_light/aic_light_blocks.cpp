@@ -1,0 +1,81 @@
+// ORACLE — TEST INFRASTRUCTURE ONLY (see ../oracle/aic_oracle.hpp).
+//
+// The light oracle (../oracle/aic_light.cpp, compiled into this library a second time, with the raytracer oracle it
+// builds its sky from) with a live block table: definitions replaced or appended after creation, and the light side of
+// a redefinition.  It changes nothing there.
+//
+// The reference leaves the light side of SpaceChange::BlockEvaluation as a TODO (space/palette.rs:862-863).  What it
+// defines is what placing a block in a cube does to light: Mutation::set -> side_effects_of_set ->
+// modified_cube_needs_update (space.rs:499-531, space/light/updater.rs:135-173).  orc_light_relight_blocks applies that
+// rule, without Mutation::set's same-block skip, to every cube that holds a redefined block, in increasing linear index
+// order.
+//
+// Build: g++ -O2 -std=c++17 -ffp-contract=off -fno-fast-math (Rust never contracts to FMA).
+#include "../oracle/aic_oracle.cpp"
+#include "../oracle/aic_light.cpp"
+
+namespace orc_blocks {
+using namespace orc;
+
+// the EvaluatedBlock members light reads, from a block descriptor (as orc_light_create converts them)
+static LBlock light_block_of(const aicb_block_desc &bd) {
+    LBlock b;
+    std::memset(&b, 0, sizeof b);
+    b.all_opaque = true;
+    for (int f = 0; f < 6; f++) {
+        b.opaque[f] = (bd.light_opaque_faces >> f) & 1;
+        b.all_opaque = b.all_opaque && b.opaque[f];
+        std::memcpy(b.face_color[f + 1], bd.light_face_colors[f], 16);
+    }
+    std::memcpy(b.face_color[0], bd.light_color, 16);
+    std::memcpy(b.emission, bd.light_emission, 12);
+    b.has_emission = !(b.emission[0] == 0.0f && b.emission[1] == 0.0f && b.emission[2] == 0.0f);
+    b.visible = bd.light_visible != 0;
+    return b;
+}
+
+// modified_cube_needs_update (updater.rs:135-173) for the cube at linear index `idx`, with the block it holds now
+static void modified_cube_needs_update(orc_light &L, size_t idx) {
+    int32_t c[3];
+    l_cube_of(L, idx, c);
+    if (opaque_for_light(L.blocks[L.ids[idx]])) {
+        L.light[idx] = L_OPAQUE;
+        q_remove(L, idx);
+    } else {
+        light_needs_update(L, c, PRIO_NEWLY_VISIBLE);
+    }
+    for (int f = 0; f < 6; f++) {
+        int32_t nc[3] = {c[0], c[1], c[2]};
+        nc[f % 3] += (f < 3) ? -1 : 1;
+        const int opp = (f < 3) ? f + 3 : f - 3;
+        if (!get_evaluated(L, nc).opaque[opp]) light_needs_update(L, nc, PRIO_NEWLY_VISIBLE);
+    }
+}
+
+}  // namespace orc_blocks
+
+using namespace orc_blocks;
+
+extern "C" {
+
+// SpaceChange::BlockEvaluation: new definitions for existing indices (light is not touched)
+void orc_light_update_blocks(orc_light *L, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
+    for (size_t i = 0; i < n; i++) L->blocks.at(indices[i]) = light_block_of(descs[i]);
+}
+
+// SpaceChange::BlockIndex past the table: the blocks become the next indices
+void orc_light_append_blocks(orc_light *L, const aicb_block_desc *descs, size_t n) {
+    for (size_t i = 0; i < n; i++) L->blocks.push_back(light_block_of(descs[i]));
+}
+
+// The light side of a redefinition: modified_cube_needs_update for every cube holding one of the indices, in increasing
+// linear index order (no relaxation: orc_light_evaluate follows)
+void orc_light_relight_blocks(orc_light *L, const uint16_t *indices, size_t n) {
+    if (L->max_distance == 0 || n == 0) return;
+    std::vector<char> redefined(L->blocks.size(), 0);
+    for (size_t i = 0; i < n; i++) redefined.at(indices[i]) = 1;
+    for (size_t idx = 0; idx < L->ids.size(); idx++)
+        if (redefined[L->ids[idx]]) modified_cube_needs_update(*L, idx);
+}
+
+}
