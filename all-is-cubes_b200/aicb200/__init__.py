@@ -61,6 +61,7 @@ def load_library() -> C.CDLL:
     lib.aicb_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_scene_set_physics.argtypes = [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8]
     lib.aicb_shard_pixel_count.argtypes = [C.POINTER(abi.CameraData), C.POINTER(abi.Shard)]
     lib.aicb_shard_pixel_count.restype = C.c_size_t
     lib.aicb_render_srgb8.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options),
@@ -127,6 +128,7 @@ def load_library() -> C.CDLL:
                                             C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_group_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_group_scene_set_physics.argtypes = [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8]
     lib.aicb_group_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_group_render_layers_srgb8.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
@@ -499,8 +501,7 @@ class Space:
         if sky_colors is None:
             # Sky::DEFAULT = Uniform(DAY_SKY_COLOR = srgb[243 243 255]) (sky.rs:24, palette.rs:63)
             sky_colors = [srgb8_to_linear((243, 243, 255))]
-        self.sky_colors = np.asarray(sky_colors, dtype=np.float32).reshape(-1, 3)
-        assert self.sky_colors.shape[0] in (1, 8)
+        self.sky_colors = _sky_colors(sky_colors)
         self.light_max_distance = int(light_max_distance)
 
     def to_desc(self):
@@ -517,13 +518,27 @@ class Space:
             keep.append(b)
         d.blocks = arr
         d.n_blocks = len(self.blocks)
-        d.sky.kind = 0 if self.sky_colors.shape[0] == 1 else 1
-        for k in range(self.sky_colors.shape[0]):
-            d.sky.colors[k][:] = [float(v) for v in self.sky_colors[k]]
+        d.sky = _sky(self.sky_colors)
         d.light_max_distance = self.light_max_distance
         keep.append(arr)
         keep.append(self)
         return d, keep
+
+
+def _sky_colors(sky_colors) -> np.ndarray:
+    """One row: Sky::Uniform; eight rows: Sky::Octants (index (x>=0)<<2 | (y>=0)<<1 | (z>=0))."""
+    c = np.asarray(sky_colors, dtype=np.float32).reshape(-1, 3)
+    assert c.shape[0] in (1, 8)
+    return c
+
+
+def _sky(sky_colors) -> abi.Sky:
+    c = _sky_colors(sky_colors)
+    sky = abi.Sky()
+    sky.kind = 0 if c.shape[0] == 1 else 1
+    for k in range(c.shape[0]):
+        sky.colors[k][:] = [float(v) for v in c[k]]
+    return sky
 
 
 def fill_block_desc(bd, b):
@@ -768,6 +783,12 @@ class SpaceRaytracer:
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
         _check(load_library().aicb_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
 
+    def set_physics(self, sky_colors, light_max_distance: int):
+        """SpaceChange::Physics (Space::set_physics): a new sky (Space's sky_colors: 1 row Uniform, 8 rows Octants) and
+        LightPhysics (0 = None, d = Rays { maximum_distance: d }).  A new sky alone leaves the light as it is; a new
+        distance reinitialises it (fast_evaluate_light, every cube changed); None frees it."""
+        _check(load_library().aicb_scene_set_physics(self.handle, C.byref(_sky(sky_colors)), light_max_distance))
+
 
 def _light_relight_blocks(fn, handle, indices, epsilon):
     idx = np.ascontiguousarray(indices, dtype=np.uint16).reshape(-1)
@@ -978,6 +999,10 @@ class GroupScene:
     def upload_light(self, light: np.ndarray):
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
         _check(load_library().aicb_group_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
+
+    def set_physics(self, sky_colors, light_max_distance: int):
+        """SpaceRaytracer.set_physics on every replica; a reinitialisation is device 0's, copied to the others."""
+        _check(load_library().aicb_group_scene_set_physics(self.handle, C.byref(_sky(sky_colors)), light_max_distance))
 
     # ---- light propagation on every device of the group (SpaceRaytracer's light_* methods, same results) ----
     def light_fast_evaluate(self):

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -133,6 +133,7 @@ EXPORTED_SYMBOLS = [
     "aicb_scene_upload_light",
     "aicb_scene_destroy",
     "aicb_scene_device_bytes",
+    "aicb_scene_set_physics",
     "aicb_shard_pixel_count",
     "aicb_render_srgb8",
     "aicb_render_rgba16f",
@@ -180,6 +181,7 @@ EXPORTED_SYMBOLS = [
     "aicb_group_render_srgb8",
     "aicb_group_scene_update_blocks",
     "aicb_group_scene_upload_light",
+    "aicb_group_scene_set_physics",
     "aicb_group_scene_append_blocks",
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",

@@ -909,6 +909,26 @@ aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_bloc
     return AICB_OK;
 }
 
+// Space::set_physics (space.rs:609-630) on a scene's replicas: the sky tables once (Sky::for_blocks, Sky::mean), then, if
+// the sky or the LightPhysics differs, each replica's context is waited for (an issued frame may still read the light
+// volume a change to None frees) and light.cu applies the change.  The sky is read as aicb_scene_create reads it.
+aicb_status scenes_set_physics(LightReplicas r, const aicb_sky &sky, uint8_t light_max_distance) {
+    const DeviceScene &cur = r.scene[0]->ds;
+    DeviceScene next = cur;
+    build_block_sky(sky, &next);
+    bool same_sky = next.sky_kind == cur.sky_kind;
+    for (int k = 0; k < (next.sky_kind ? 8 : 1); k++)   // Uniform's colour, or the eight octants'
+        for (int i = 0; i < 3; i++) same_sky = same_sky && next.sky_colors[k][i] == cur.sky_colors[k][i];
+    if (same_sky && light_max_distance == r.scene[0]->light_max_distance) return AICB_OK;   // no SpaceChange::Physics
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.ctx[i]->device));
+        TRY(wait_context(r.ctx[i]));
+    }
+    const aicb_status st = light_set_physics(r, next, light_max_distance);
+    cudaSetDevice(r.ctx[0]->device);
+    return st;
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
@@ -994,6 +1014,12 @@ void aicb_scene_destroy(aicb_scene *s) {
 }
 
 uint64_t aicb_scene_device_bytes(const aicb_scene *s) { return s ? s->device_bytes : 0; }
+
+aicb_status aicb_scene_set_physics(aicb_scene *s, const aicb_sky *sky, uint8_t light_max_distance) {
+    if (!s || !sky) return fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return scenes_set_physics({&s, &s->ctx, 1}, *sky, light_max_distance);
+}
 
 aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *ids,
                                     const uint8_t (*light)[4], size_t n) {

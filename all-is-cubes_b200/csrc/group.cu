@@ -352,6 +352,14 @@ aicb_status aicb_group_scene_append_blocks(aicb_group_scene *gs, const aicb_bloc
     return scenes_append_blocks(gs->scene.data(), gs->scene.size(), descs, n);
 }
 
+aicb_status aicb_group_scene_set_physics(aicb_group_scene *gs, const aicb_sky *sky, uint8_t light_max_distance) {
+    if (!gs || !sky) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    // a reinitialisation runs as aicb_group_light_fast_evaluate does, over the light calls' peers
+    if (light_max_distance && light_max_distance != gs->scene[0]->light_max_distance) TRY(ensure_light_peers(gs->group));
+    return scenes_set_physics({gs->scene.data(), gs->group->ctx.data(), gs->scene.size()}, *sky, light_max_distance);
+}
+
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *gs, const uint8_t (*light)[4], size_t n_texels) {
     if (!gs || !light) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n_texels != gs->scene[0]->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");

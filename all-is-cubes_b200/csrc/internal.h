@@ -162,8 +162,9 @@ struct LightState {
     } shared;
 
     // Replica `replica` of `n_replicas`'s part(s) and the scene's light volume, where `s` (this state's scene) has none
-    // yet; the scene changes only if every step succeeds.
-    aicb_status ensure(aicb_scene *s, size_t replica, size_t n_replicas);
+    // yet; the scene changes only if every step succeeds.  A new own part takes `terms` as its sky_term (nullptr: the
+    // scene's sky, tabulated here).
+    aicb_status ensure(aicb_scene *s, size_t replica, size_t n_replicas, const std::vector<float4> *terms);
 
     // replica 0's overflow list is also the round's `changed` list: its overflow is computed before k_compact_changed
     uint32_t *changed() const { return own.overflow.get<uint32_t>(); }
@@ -369,6 +370,8 @@ struct LightReplicas {
     aicb_ctx *const *ctx;
     size_t n;
 };
+// aicb200.cu: aicb_scene_set_physics / aicb_group_scene_set_physics over a scene's replicas (the caller holds the locks).
+aicb_status scenes_set_physics(LightReplicas r, const aicb_sky &sky, uint8_t light_max_distance);
 aicb_status light_fast_evaluate(LightReplicas r);
 aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]);
 aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
@@ -377,6 +380,9 @@ aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3],
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
 aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
                                  uint64_t *updates_done, uint8_t *max_diff);
+// Space::set_physics on the replicas' light side, once nothing on their contexts reads their arrays: `sky` holds the
+// new sky in a DeviceScene's sky fields, which every replica takes; `max_distance` is the new LightPhysics (0 = None).
+aicb_status light_set_physics(LightReplicas r, const aicb::DeviceScene &sky, uint32_t max_distance);
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels);
 // The set of changed cubes of replica 0 (the other replicas' texels are identical); the caller holds the locks.
 aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed);

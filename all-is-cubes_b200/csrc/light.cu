@@ -741,11 +741,46 @@ LightParams light_params(LightReplicas r, size_t i) {
     return P;
 }
 
-// Every replica's light state and, on a group, replica 0's push targets: the other replicas' light volumes.
-aicb_status ensure_replicas(LightReplicas r) {
+// end_of_ray (updater.rs:889-924) without the lane's alpha and bundle weight: per chart node, the sky light its bundle
+// collects from a BlockSky with these faces (texels NX..PZ) — the same f32 operations, in the same order, as the
+// reference evaluates per ray end.  LightState::Own::sky_term.
+std::vector<float4> sky_terms(const uint32_t sky_faces[6]) {
+    const std::vector<LightNodePre> &pre = chart_preorder_host();
+    float lut[256];
+    lut[0] = 0.0f;
+    for (int i = 1; i < 256; i++) lut[i] = (float)std::exp2((double)(((float)i - 144.0f) / 10.0f));
+    auto psc = [](float v) { return v > 0.0f ? v : 0.0f; };
+    auto psm = [](float a, float b) { float v = a * b; return (v != v) ? 0.0f : v; };
+    std::vector<float4> sky(pre.size());
+    for (size_t k = 0; k < pre.size(); k++) {
+        const float *cw = pre[k].w;
+        float t[6][3];
+        for (int f = 0; f < 6; f++) {
+            const uint32_t tx = sky_faces[f];
+            const float kk = psc(cw[f]);
+            t[f][0] = psm(lut[tx & 255], kk);
+            t[f][1] = psm(lut[(tx >> 8) & 255], kk);
+            t[f][2] = psm(lut[(tx >> 16) & 255], kk);
+        }
+        const float kr = psc(1.0f / ((cw[0] + cw[3]) + (cw[1] + cw[4]) + (cw[2] + cw[5])));
+        float c[3];
+        for (int i = 0; i < 3; i++) c[i] = psm((t[0][i] + t[3][i]) + (t[1][i] + t[4][i]) + (t[2][i] + t[5][i]), kr);
+        sky[k] = make_float4(c[0], c[1], c[2], 0.0f);
+    }
+    return sky;
+}
+
+// Every replica's light state and, on a group, replica 0's push targets: the other replicas' light volumes.  A replica
+// that has no own part yet takes `terms` as its sky_term, or the scene's sky tabulated once for every such replica.
+aicb_status ensure_replicas(LightReplicas r, const std::vector<float4> *terms = nullptr) {
+    std::vector<float4> tabulated;
     for (size_t i = 0; i < r.n; i++) {
+        if (!terms && !r.scene[i]->light.own.sky_term) {
+            tabulated = sky_terms(r.scene[0]->ds.sky_faces);
+            terms = &tabulated;
+        }
         CU(cudaSetDevice(r.ctx[i]->device));
-        TRY(r.scene[i]->light.ensure(r.scene[i], i, r.n));
+        TRY(r.scene[i]->light.ensure(r.scene[i], i, r.n, terms));
     }
     if (r.n == 1) return AICB_OK;
     std::vector<uint32_t *> targets;
@@ -870,11 +905,17 @@ LightBlockDev light_block(const aicb_block_desc &b) {
 // ---------------------------------------------------------------------------------------------
 // a scene's light state (internal.h)
 // ---------------------------------------------------------------------------------------------
-aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas) {
+// What aicb_scene_device_bytes counts of a light state's parts (it leaves out the tile bounds, the counters, the overflow
+// count and the push targets).
+static size_t change_bytes(size_t vol) { return (vol + 31) / 32 * 4; }
+static size_t dirty_bytes(size_t vol) { return (vol + 1023) / 1024 * 4 + 16; }
+static uint64_t own_bytes(size_t vol) { return chart_preorder_host().size() * sizeof(float4) + vol * 4; }
+static uint64_t shared_bytes(size_t vol, bool group) { return vol * 10 + change_bytes(vol) + (group ? dirty_bytes(vol) : 0); }
+
+aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas, const std::vector<float4> *terms) {
     if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     TRY(ensure_chart(s->ctx));
     const size_t vol = s->volume;
-    const size_t change_bytes = (vol + 31) / 32 * 4, dirty_bytes = (vol + 1023) / 1024 * 4 + 16;
     const bool add_own = !own.sky_term, add_shared = replica == 0 && !shared.pending, group = n_replicas > 1;
     DeviceBuffer light;
     Own o;
@@ -884,31 +925,7 @@ aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas)
         TRY(light.upload(init.data(), vol * 4, 16));
     }
     if (add_own) {
-        // end_of_ray (updater.rs:889-924) without the lane's alpha and bundle weight: per chart node, the sky light
-        // its bundle collects — the same f32 operations, in the same order, as the reference evaluates per ray end
-        const std::vector<LightNodePre> &pre = chart_preorder_host();
-        float lut[256];
-        lut[0] = 0.0f;
-        for (int i = 1; i < 256; i++) lut[i] = (float)std::exp2((double)(((float)i - 144.0f) / 10.0f));
-        auto psc = [](float v) { return v > 0.0f ? v : 0.0f; };
-        auto psm = [](float a, float b) { float v = a * b; return (v != v) ? 0.0f : v; };
-        std::vector<float4> sky(pre.size());
-        for (size_t k = 0; k < pre.size(); k++) {
-            const float *cw = pre[k].w;
-            float t[6][3];
-            for (int f = 0; f < 6; f++) {
-                const uint32_t tx = s->ds.sky_faces[f];
-                const float kk = psc(cw[f]);
-                t[f][0] = psm(lut[tx & 255], kk);
-                t[f][1] = psm(lut[(tx >> 8) & 255], kk);
-                t[f][2] = psm(lut[(tx >> 16) & 255], kk);
-            }
-            const float kr = psc(1.0f / ((cw[0] + cw[3]) + (cw[1] + cw[4]) + (cw[2] + cw[5])));
-            float c[3];
-            for (int i = 0; i < 3; i++) c[i] = psm((t[0][i] + t[3][i]) + (t[1][i] + t[4][i]) + (t[2][i] + t[5][i]), kr);
-            sky[k] = make_float4(c[0], c[1], c[2], 0.0f);
-        }
-        TRY(o.sky_term.upload(sky));
+        TRY(o.sky_term.upload(terms ? *terms : sky_terms(s->ds.sky_faces)));
         TRY(o.overflow.ensure(vol * 4 + 16));
         if (replica > 0) TRY(o.overflow_count.ensure(4));
     }
@@ -920,15 +937,14 @@ aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas)
         TRY(sh.new_light.ensure(vol * 4 + 16));
         TRY(sh.diff.ensure(vol + 16));
         TRY(sh.counters.ensure(sizeof(LightCounters)));
-        TRY(sh.changes.ensure(change_bytes));
-        CU(cudaMemset(sh.changes.get(), 0, change_bytes));
+        TRY(sh.changes.ensure(change_bytes(vol)));
+        CU(cudaMemset(sh.changes.get(), 0, change_bytes(vol)));
         if (group) {
-            TRY(sh.dirty.ensure(dirty_bytes));
-            CU(cudaMemset(sh.dirty.get(), 0, dirty_bytes));
+            TRY(sh.dirty.ensure(dirty_bytes(vol)));
+            CU(cudaMemset(sh.dirty.get(), 0, dirty_bytes(vol)));
             TRY(sh.push_targets.ensure((n_replicas - 1) * sizeof(uint32_t *)));
         }
     }
-    // (aicb_scene_device_bytes leaves out the tile bounds, the counters, the overflow count and the push targets)
     if (light) {
         s->d_light = std::move(light);
         s->ds.light = s->d_light.get<uint32_t>();
@@ -936,11 +952,11 @@ aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas)
     }
     if (add_own) {
         own = std::move(o);
-        s->device_bytes += chart_preorder_host().size() * sizeof(float4) + vol * 4;
+        s->device_bytes += own_bytes(vol);
     }
     if (add_shared) {
         shared = std::move(sh);
-        s->device_bytes += vol * 10 + change_bytes + (group ? dirty_bytes : 0);
+        s->device_bytes += shared_bytes(vol, group);
     }
     return AICB_OK;
 }
@@ -1114,6 +1130,89 @@ aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_
         CU(cudaSetDevice(s->ctx->device));
     }
     return propagate(r, epsilon, updates_done, max_diff, nullptr);
+}
+
+// LightStorage::maybe_reinitialize_for_physics_change (space/light/updater.rs:80-113):
+//   - the sky: every replica takes it, and a replica's sky_term is re-tabulated (once per call) where the BlockSky's
+//     faces changed.  Nothing else changes for the sky alone (the reference's "TODO: if only sky color is different").
+//   - Rays of another distance: every replica's state, allocated where it has none (LightState::ensure), then
+//     fast_evaluate_light with the new sky on device 0, copied to the others.  It writes every texel and every queue
+//     entry, so initialize_light's uniform fill is never observable and is not made.  Every cube enters the set of
+//     changed cubes: the whole volume was replaced.
+//   - None: every replica's light volume and state are freed (frames read PackedLight::ONE; the set goes with them).
+// The allocation comes first and is the only step that can fail for want of memory: a failure frees what it allocated
+// and leaves every replica as it was.
+aicb_status light_set_physics(LightReplicas r, const DeviceScene &sky, uint32_t max_distance) {
+    aicb_scene *s0 = r.scene[0];
+    const bool relight = max_distance != s0->light_max_distance;
+    const bool new_faces = std::memcmp(sky.sky_faces, s0->ds.sky_faces, sizeof sky.sky_faces) != 0;
+    std::vector<float4> terms;
+    if (new_faces || (relight && max_distance)) terms = sky_terms(sky.sky_faces);
+    if (relight && max_distance) {
+        struct Before {
+            bool light, own, shared;
+            uint32_t max_distance;
+            uint64_t device_bytes;
+        };
+        std::vector<Before> before;
+        for (size_t i = 0; i < r.n; i++) {
+            aicb_scene *s = r.scene[i];
+            before.push_back({(bool)s->d_light, (bool)s->light.own.sky_term, (bool)s->light.shared.pending,
+                              s->light_max_distance, s->device_bytes});
+            s->light_max_distance = max_distance;
+        }
+        const aicb_status st = ensure_replicas(r, &terms);
+        if (st != AICB_OK) {
+            for (size_t i = 0; i < r.n; i++) {
+                aicb_scene *s = r.scene[i];
+                cudaSetDevice(r.ctx[i]->device);
+                if (!before[i].light) {
+                    s->d_light.reset();
+                    s->ds.light = nullptr;
+                }
+                if (!before[i].own) s->light.own = LightState::Own();
+                if (!before[i].shared) s->light.shared = LightState::Shared();
+                s->light_max_distance = before[i].max_distance;
+                s->device_bytes = before[i].device_bytes;
+            }
+            cudaSetDevice(s0->ctx->device);
+            return st;
+        }
+    }
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_scene *s = r.scene[i];
+        DeviceScene &ds = s->ds;
+        CU(cudaSetDevice(r.ctx[i]->device));
+        std::memcpy(ds.sky_faces, sky.sky_faces, sizeof ds.sky_faces);
+        ds.sky_mean = sky.sky_mean;
+        ds.sky_kind = sky.sky_kind;
+        std::memcpy(ds.sky_colors, sky.sky_colors, sizeof ds.sky_colors);
+        if (new_faces && s->light.own.sky_term)
+            CU(cudaMemcpy(s->light.own.sky_term.get(), terms.data(), terms.size() * sizeof(float4), cudaMemcpyHostToDevice));
+        if (relight && !max_distance) {
+            const size_t vol = s->volume;
+            if (s->d_light) s->device_bytes -= vol * 4;
+            if (s->light.own.sky_term) s->device_bytes -= own_bytes(vol);
+            if (s->light.shared.pending) s->device_bytes -= shared_bytes(vol, (bool)s->light.shared.dirty);
+            s->light.own = LightState::Own();
+            s->light.shared = LightState::Shared();
+            s->d_light.reset();
+            ds.light = nullptr;
+            s->light_max_distance = 0;
+        }
+    }
+    CU(cudaSetDevice(s0->ctx->device));
+    if (!relight || !max_distance) return AICB_OK;
+    TRY(light_fast_evaluate(r));
+    // every cube is changed: whole words of the bitmap, then the cubes of a last, partial word
+    uint32_t *changes = s0->light.shared.changes.get<uint32_t>();
+    cudaStream_t stream = s0->ctx->stream.get();
+    const size_t whole = s0->volume / 32;
+    const uint32_t tail = (1u << (s0->volume % 32)) - 1u;
+    CU(cudaMemsetAsync(changes, 0xff, whole * 4, stream));
+    if (tail) CU(cudaMemcpyAsync(changes + whole, &tail, 4, cudaMemcpyHostToDevice, stream));
+    CU(cudaStreamSynchronize(stream));
+    return AICB_OK;
 }
 
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 9 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 10 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -200,6 +200,7 @@ unsafe extern "C" {
     pub fn aicb_scene_upload_light(s: *mut aicb_scene, light: *const [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_scene_destroy(s: *mut aicb_scene);
     pub fn aicb_scene_device_bytes(s: *const aicb_scene) -> u64;
+    pub fn aicb_scene_set_physics(s: *mut aicb_scene, sky: *const aicb_sky, light_max_distance: u8) -> aicb_status;
 
     pub fn aicb_shard_pixel_count(cam: *const aicb_camera, shard: *const aicb_shard) -> usize;
     pub fn aicb_render_srgb8(s: *mut aicb_scene, cam: *const aicb_camera, opt: *const aicb_options, shard: *const aicb_shard,
@@ -255,6 +256,8 @@ unsafe extern "C" {
     pub fn aicb_group_scene_update_blocks(gs: *mut aicb_group_scene, indices: *const u16, descs: *const aicb_block_desc,
                                           n: usize) -> aicb_status;
     pub fn aicb_group_scene_upload_light(gs: *mut aicb_group_scene, light: *const [u8; 4], n_texels: usize) -> aicb_status;
+    pub fn aicb_group_scene_set_physics(gs: *mut aicb_group_scene, sky: *const aicb_sky, light_max_distance: u8)
+                                        -> aicb_status;
     // every replica; validated against replica 0 first, so a rejected call changes none
     pub fn aicb_group_scene_append_blocks(gs: *mut aicb_group_scene, descs: *const aicb_block_desc, n: usize) -> aicb_status;
     // aicb_render_layers_* on a group: both layers must be scenes of the same group

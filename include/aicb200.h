@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 9
+#define AICB_ABI_VERSION 10
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -220,6 +220,24 @@ aicb_status aicb_scene_append_blocks(aicb_scene *, const aicb_block_desc *descs,
 aicb_status aicb_scene_upload_light(aicb_scene *, const uint8_t (*light)[4], size_t n_texels);
 void aicb_scene_destroy(aicb_scene *);
 uint64_t aicb_scene_device_bytes(const aicb_scene *);
+/* SpaceChange::Physics: Space::set_physics (space.rs:609-630) and, on the light side,
+ * LightStorage::maybe_reinitialize_for_physics_change (space/light/updater.rs:80-113).  `sky` is read as
+ * aicb_scene_desc::sky is (kind != 0 is Octants); `light_max_distance` means what aicb_scene_desc's does: 0 = None.
+ *   - Same sky and same distance: nothing happens (the reference sends no SpaceChange::Physics).
+ *   - A new sky: frames use it from then on (Sky::sample, the fog blend, BlockSky::light_outside beyond the bounds) and
+ *     so do later light calls.  The light volume, the queue and the set of changed cubes are left as they are, as the
+ *     reference leaves them; a host that wants the new sky's light calls aicb_light_fast_evaluate + aicb_light_evaluate.
+ *   - Another distance d > 0 (from None or from another d): the light is reinitialised.  The volume is allocated if the
+ *     scene has none, fast_evaluate_light runs with the new sky (every texel and every queue entry is written), and every
+ *     cube enters the set of changed cubes.  Later light calls use the new maximum_distance.
+ *   - None: the light volume and the light state are freed (aicb_scene_device_bytes drops by them), frames read
+ *     PackedLight::ONE, the set of changed cubes goes with the state, and light calls are AICB_ERR_INVALID.
+ * Afterwards every output equals that of a scene created with the same cells and block table, the new sky, the new
+ * light_max_distance and the volume aicb_light_download returns as its light (NULL under None).  The call first waits
+ * for the context's frame in flight and the work queued on its stream.  AICB_ERR_INVALID: a NULL scene or sky.
+ * AICB_ERR_OOM: the volume or the state could not be allocated.  A failed call changes nothing.
+ * GPU test: tests/test_gpu_physics.py. */
+aicb_status aicb_scene_set_physics(aicb_scene *, const aicb_sky *sky, uint8_t light_max_distance);
 
 /* ---------------------------------------------------------------------------------------------
  * draw(): replaces RtRenderer::draw_rgba / RtRenderer::draw::<ColorBuf> and the Rayon pixel
@@ -394,6 +412,11 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *, const aicb_camera *, con
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *, const uint16_t *indices, const aicb_block_desc *descs,
                                            size_t n);
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *, const uint8_t (*light)[4], size_t n_texels);
+/* aicb_scene_set_physics on every replica, holding every context of the group.  It is decided against replica 0 before
+ * any replica changes, and every replica takes the sky.  A reinitialisation runs as aicb_group_light_fast_evaluate does
+ * (device 0 computes, the others take peer copies; the set of changed cubes and the queue are device 0's), so the
+ * replicas stay identical.  A failed call changes no replica. */
+aicb_status aicb_group_scene_set_physics(aicb_group_scene *, const aicb_sky *sky, uint8_t light_max_distance);
 /* aicb_scene_append_blocks on every replica, validated against replica 0 before any replica changes: a rejected call
  * changes no replica.  The call holds every context of the group; a table that grows past 16384 blocks widens every
  * replica's cells on its own device. */
@@ -513,7 +536,8 @@ aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
  *   - a relaxation round stores a value with difference_priority > 0 (apply_light_update, updater.rs:313-317);
  *   - a round writes a guess into an Uninitialized neighbour (updater.rs:335-338);
  *   - aicb_light_fast_evaluate changes its texel.  The reference announces nothing there (fast_evaluate_light has a
- *     TODO for EveryBlock); a host following the light needs the cubes all the same.
+ *     TODO for EveryBlock); a host following the light needs the cubes all the same;
+ *   - aicb_scene_set_physics reinitialises the light (every cube).
  * Nothing else adds to it: not aicb_light_compute, aicb_scene_update_cubes, aicb_scene_upload_light (texels the host
  * supplied), frames, or a rejected call.  The set accumulates across calls until it is taken; a scene with no light
  * call yet has none.  LightPhysics::None is AICB_ERR_INVALID.

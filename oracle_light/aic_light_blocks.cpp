@@ -78,4 +78,26 @@ void orc_light_relight_blocks(orc_light *L, const uint16_t *indices, size_t n) {
         if (redefined[L->ids[idx]]) modified_cube_needs_update(*L, idx);
 }
 
+// SpaceChange::Physics on the light side: LightStorage::maybe_reinitialize_for_physics_change (updater.rs:80-113).  The
+// BlockSky is replaced (Sky::for_blocks through the raytracer oracle's construction; light reads nothing else of the
+// sky, so Space::set_physics's early return for an unchanged physics, space.rs:609-612, changes nothing here).  A
+// different LightPhysics reinitialises the light: an empty volume and queue under None, else fast_evaluate_light over
+// the whole volume (initialize_light's uniform fill is overwritten there, texel by texel).
+void orc_light_set_physics(orc_light *L, const aicb_sky *sky, uint8_t light_max_distance) {
+    orc_scene s;
+    s.sky = *sky;
+    build_block_sky(&s);
+    for (int f = 0; f < 6; f++) L->sky_faces[f] = PL{s.sky_faces[f].r, s.sky_faces[f].g, s.sky_faces[f].b, s.sky_faces[f].status};
+    if (light_max_distance == L->max_distance) return;   // "TODO: if only sky color is different, trigger light updates"
+    L->max_distance = light_max_distance;
+    L->by_priority.clear();
+    L->by_cube.clear();
+    if (light_max_distance == 0) {
+        L->light.clear();
+        return;
+    }
+    L->light.assign(L->ids.size(), L_UNINIT);
+    orc_light_fast_evaluate(L);
+}
+
 }
