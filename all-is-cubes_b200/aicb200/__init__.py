@@ -104,6 +104,10 @@ def load_library() -> C.CDLL:
     for prefix in ("aicb_light", "aicb_group_light"):
         getattr(lib, prefix + "_relight_blocks").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8,
                                                              C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
+    for prefix in ("aicb_light", "aicb_group_light"):
+        getattr(lib, prefix + "_queue_uninitialized").argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
+        getattr(lib, prefix + "_queue_region").argtypes = [C.c_void_p, C.POINTER(abi.Aab), C.c_uint8]
+        getattr(lib, prefix + "_download_queue").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.aicb_light_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     lib.aicb_render_text.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p, C.c_size_t,
                                      C.POINTER(abi.RenderInfo)]
@@ -779,6 +783,21 @@ class SpaceRaytracer:
         return _light_take_changes(load_library().aicb_light_changes_count, load_library().aicb_light_take_changes,
                                    self.handle, discard)
 
+    def light_queue_uninitialized(self) -> int:
+        """The load rule of Space::new_from_builder (space.rs:290-313): every cube whose texel is Uninitialized (status
+        byte 0) enters the light update queue at Priority::UNINIT (210), raise-only.  Returns how many such cubes there
+        are.  Nothing propagates: light_evaluate follows."""
+        return _light_queue_uninitialized(load_library().aicb_light_queue_uninitialized, self.handle)
+
+    def light_queue_region(self, lower, size, priority: int):
+        """LightStorage::light_needs_update_in_region (updater.rs:122-133): every cube of the box (lower, size) within the
+        bounds enters the queue at `priority` (1..255), raise-only."""
+        _light_queue_region(load_library().aicb_light_queue_region, self.handle, lower, size, priority)
+
+    def light_download_queue(self) -> np.ndarray:
+        """Each cube's queued priority (0 = not queued), uint8 shaped like the volume."""
+        return _light_download_queue(load_library().aicb_light_download_queue, self.handle, self.space.size)
+
     def upload_light(self, light: np.ndarray):
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
         _check(load_library().aicb_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
@@ -795,6 +814,25 @@ def _light_relight_blocks(fn, handle, indices, epsilon):
     n, md = C.c_uint64(0), C.c_uint8(0)
     _check(fn(handle, idx.ctypes.data, idx.size, epsilon, C.byref(n), C.byref(md)))
     return int(n.value), int(md.value)
+
+
+def _light_queue_uninitialized(fn, handle) -> int:
+    n = C.c_size_t(0)
+    _check(fn(handle, C.byref(n)))
+    return int(n.value)
+
+
+def _light_queue_region(fn, handle, lower, size, priority):
+    region = abi.Aab()
+    region.lower[:] = [int(v) for v in lower]
+    region.size[:] = [int(v) for v in size]
+    _check(fn(handle, C.byref(region), priority))
+
+
+def _light_download_queue(fn, handle, shape) -> np.ndarray:
+    out = np.zeros(shape, dtype=np.uint8)
+    _check(fn(handle, out.ctypes.data, out.size, None))
+    return out
 
 
 def _light_changes_count(count_fn, handle) -> int:
@@ -1050,6 +1088,18 @@ class GroupScene:
         out = np.zeros(self.space.size + (4,), dtype=np.uint8)
         _check(load_library().aicb_group_light_download(self.handle, replica, out.ctypes.data, out.size // 4))
         return out
+
+    def light_queue_uninitialized(self) -> int:
+        """SpaceRaytracer.light_queue_uninitialized on the group: replica 0's volume, device 0's queue."""
+        return _light_queue_uninitialized(load_library().aicb_group_light_queue_uninitialized, self.handle)
+
+    def light_queue_region(self, lower, size, priority: int):
+        """SpaceRaytracer.light_queue_region on the group's queue (device 0's)."""
+        _light_queue_region(load_library().aicb_group_light_queue_region, self.handle, lower, size, priority)
+
+    def light_download_queue(self) -> np.ndarray:
+        """SpaceRaytracer.light_download_queue of the group's queue (device 0's)."""
+        return _light_download_queue(load_library().aicb_group_light_download_queue, self.handle, self.space.size)
 
     def light_changes_count(self) -> int:
         """SpaceRaytracer.light_changes_count of the group: the set is device 0's, and every replica's texels are

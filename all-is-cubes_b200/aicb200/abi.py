@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -169,6 +169,9 @@ EXPORTED_SYMBOLS = [
     "aicb_light_edit_and_propagate",
     "aicb_light_relight_blocks",
     "aicb_light_download",
+    "aicb_light_queue_uninitialized",
+    "aicb_light_queue_region",
+    "aicb_light_download_queue",
     "aicb_light_stats",
     "aicb_light_changes_count",
     "aicb_light_take_changes",
@@ -192,6 +195,9 @@ EXPORTED_SYMBOLS = [
     "aicb_group_light_edit_and_propagate",
     "aicb_group_light_relight_blocks",
     "aicb_group_light_download",
+    "aicb_group_light_queue_uninitialized",
+    "aicb_group_light_queue_region",
+    "aicb_group_light_download_queue",
     "aicb_group_light_stats",
     "aicb_group_light_changes_count",
     "aicb_group_light_take_changes",

@@ -31,6 +31,7 @@ from . import Block, Space
 
 # LightStatusSerV1 (schema.rs:491-498) -> the status byte of PackedLight::as_texel (light/data.rs:31-46, 162)
 _STATUS_TEXEL = {0: 0, 1: 1, 2: 128, 3: 255}
+_TEXEL_STATUS = {t: s for s, t in _STATUS_TEXEL.items()}
 _IGNORED_MODIFIERS = {"DisplayNameV1", "TagV1", "QuoteV1", "SelectableV1", "BlockInventoryV1", "InventoryConfigV1",
                       "RotationRuleV1", "PlacementActionV1", "TickActionV1", "ActivationActionV1", "AnimationHintV1"}
 
@@ -100,6 +101,39 @@ def _block_of(block_ser, resolve_space):
     raise UnsupportedBlock(f"primitive {kind} needs the reference's block evaluator")
 
 
+def light_from_value(value, size) -> np.ndarray:
+    """A `GzSerde` `LightSerV1` volume -> PackedLight texels shaped `size + (4,)`."""
+    raw = np.frombuffer(gz_decode(value), dtype=np.uint8).reshape(-1, 4)
+    if raw.shape[0] != size[0] * size[1] * size[2]:
+        raise ValueError("light volume size mismatch")
+    light = raw.copy()
+    light[:, 3] = np.vectorize(_STATUS_TEXEL.__getitem__, otypes=[np.uint8])(raw[:, 3])
+    return light.reshape(tuple(size) + (4,))
+
+
+def light_to_value(texels, queue=None):
+    """PackedLight texels (and the light update queue: one priority per cube, 0 = not queued, as
+    light_download_queue returns it) -> the `GzSerde` `LightSerV1` value of a `SpaceV1`, the inverse of what
+    space_from_value reads.  As Serialize for space::Read writes it (save/conversion.rs:773-785), a queued cube's status
+    is Uninitialized and its r, g, b are kept, so a Space loaded from it resumes the queued work
+    (SpaceRaytracer.light_queue_uninitialized)."""
+    t = np.ascontiguousarray(texels, dtype=np.uint8).reshape(-1, 4)
+    status = t[:, 3]
+    known = np.isin(status, list(_TEXEL_STATUS))
+    if not known.all():
+        raise ValueError(f"texel status byte {int(status[~known][0])} has no LightStatusSerV1")
+    out = t.copy()
+    lut = np.zeros(256, dtype=np.uint8)
+    lut[list(_TEXEL_STATUS)] = list(_TEXEL_STATUS.values())
+    out[:, 3] = lut[status]
+    if queue is not None:
+        q = np.asarray(queue, dtype=np.uint8).reshape(-1)
+        if q.size != t.shape[0]:
+            raise ValueError("queue size mismatch")
+        out[q > 0, 3] = 0
+    return gz_encode(out.tobytes())
+
+
 def space_from_value(v, resolve_space=None) -> Space:
     """A `SpaceV1` value (the parsed JSON object) -> Space."""
     if v.get("type") != "SpaceV1":
@@ -126,12 +160,7 @@ def space_from_value(v, resolve_space=None) -> Space:
     max_distance = int(lp["maximum_distance"]) if lp["type"] == "RaysV1" else 0
     light = None
     if v.get("light") is not None and max_distance:
-        raw = np.frombuffer(gz_decode(v["light"]), dtype=np.uint8).reshape(-1, 4)
-        if raw.shape[0] != n:
-            raise ValueError("light volume size mismatch")
-        light = raw.copy()
-        light[:, 3] = np.vectorize(_STATUS_TEXEL.__getitem__, otypes=[np.uint8])(raw[:, 3])
-        light = light.reshape(size + (4,))
+        light = light_from_value(v["light"], size)
     return Space(tuple(lower), ids.astype(np.uint16).reshape(size), blocks, light=light, sky_colors=sky_colors,
                  light_max_distance=max_distance)
 

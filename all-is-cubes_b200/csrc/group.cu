@@ -443,6 +443,29 @@ aicb_status aicb_group_light_relight_blocks(aicb_group_scene *gs, const uint16_t
     return light_relight_blocks(r, indices, n, epsilon, updates_done, max_diff);
 }
 
+// The queue is device 0's and the scan reads replica 0's volume (the replicas' are identical).
+aicb_status aicb_group_light_queue_uninitialized(aicb_group_scene *gs, size_t *n_queued) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    LightReplicas r;
+    TRY(light_replicas(gs, &r));
+    return light_queue_uninitialized(r, n_queued);
+}
+
+aicb_status aicb_group_light_queue_region(aicb_group_scene *gs, const aicb_aab *region, uint8_t priority) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    LightReplicas r;
+    TRY(light_replicas(gs, &r));
+    return light_queue_region(r, region, priority);
+}
+
+aicb_status aicb_group_light_download_queue(aicb_group_scene *gs, uint8_t *priorities, size_t n_texels, size_t *n_queued) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    return light_download_queue(gs->scene[0], priorities, n_texels, n_queued);
+}
+
 aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t (*out)[4], size_t n_texels) {
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (replica < 0 || (size_t)replica >= gs->scene.size()) return aicb_fail(AICB_ERR_INVALID, "no such replica");

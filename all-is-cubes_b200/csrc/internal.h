@@ -383,6 +383,11 @@ aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_
 // Space::set_physics on the replicas' light side, once nothing on their contexts reads their arrays: `sky` holds the
 // new sky in a DeviceScene's sky fields, which every replica takes; `max_distance` is the new LightPhysics (0 = None).
 aicb_status light_set_physics(LightReplicas r, const aicb::DeviceScene &sky, uint32_t max_distance);
+// The light update queue: the load rule of Space::new_from_builder and light_needs_update_in_region over replica 0's
+// volume and device 0's queue, and a copy of the queue's bytes.
+aicb_status light_queue_uninitialized(LightReplicas r, size_t *n_queued);
+aicb_status light_queue_region(LightReplicas r, const aicb_aab *region, uint8_t priority);
+aicb_status light_download_queue(aicb_scene *s, uint8_t *priorities, size_t n_texels, size_t *n_queued);
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels);
 // The set of changed cubes of replica 0 (the other replicas' texels are identical); the caller holds the locks.
 aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed);

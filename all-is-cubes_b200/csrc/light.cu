@@ -2,6 +2,7 @@
 // (space/light/chart/generator.rs), the per-block derived table, and the batched relaxation driver
 // replacing LightStorage::update_light_from_queue / apply_light_update / fast_evaluate_light /
 // modified_cube_needs_update (space/light/updater.rs) and Mutation::evaluate_light (space.rs:1496-1527).
+#include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -618,6 +619,77 @@ __global__ void __launch_bounds__(256) k_relight_blocks(const LightParams P, con
     for (uint32_t idx = n_vec * per + t0; idx < P.volume; idx += stride) relight_cube(P, s_mask, idx, block_id_at(S, idx), queue);
 }
 
+// A box of cubes as offsets from the scene's lower corner (hi exclusive), already clipped to the bounds.
+struct QueueBox {
+    uint32_t lo[3], hi[3];
+};
+
+// LightUpdateQueue::insert (queue.rs:107-133) at one priority, raise-only, for a set of cubes: those whose texel is
+// Uninitialized (UNINIT: the load rule of Space::new_from_builder, space.rs:290-313) or those in `box`
+// (light_needs_update_in_region, updater.rs:122-133).  One 256-thread block per queue tile, grid-stride over the tiles
+// [tile0, tile1); a thread owns 4 consecutive cubes: one word of pending bytes and, for UNINIT, one 16-byte load of
+// their texels.  No other thread writes the word, so no CAS.  A tile with a selected cube has its bound raised to
+// `prio`, which k_gather reads; the selected cubes are counted into counters->queued.
+template <bool UNINIT>
+__global__ void __launch_bounds__(256) k_queue_cubes(const LightParams P, uint32_t tile0, uint32_t tile1, QueueBox box,
+                                                     uint32_t prio) {
+    __shared__ uint32_t s_n[8];
+    const DeviceScene &S = P.scene;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint32_t total = 0;   // (thread 0) the block's selected cubes
+    for (uint32_t tile = tile0 + blockIdx.x; tile < tile1; tile += gridDim.x) {
+        const uint32_t w = tile * (LIGHT_TILE / 4) + threadIdx.x, base = w * 4;
+        uint32_t sel = 0;
+        if (base < P.volume) {
+            if (UNINIT) {
+                uint32_t t[4];
+                if (base + 4 <= P.volume) {
+                    const uint4 v = __ldg((const uint4 *)S.light + w);
+                    t[0] = v.x; t[1] = v.y; t[2] = v.z; t[3] = v.w;
+                } else {
+#pragma unroll
+                    for (uint32_t k = 0; k < 4; k++) t[k] = base + k < P.volume ? S.light[base + k] : TX_NO_RAYS;
+                }
+#pragma unroll
+                for (uint32_t k = 0; k < 4; k++) sel |= ((t[k] >> 24) == 0 ? 1u : 0u) << k;   // LightStatus::Uninitialized
+            } else {
+                const uint32_t sy = (uint32_t)S.size[1], sz = (uint32_t)S.size[2];
+                uint32_t z = base % sz, y = (base / sz) % sy, x = base / sz / sy;
+#pragma unroll
+                for (uint32_t k = 0; k < 4; k++) {
+                    const bool in = base + k < P.volume && x >= box.lo[0] && x < box.hi[0] && y >= box.lo[1] &&
+                                    y < box.hi[1] && z >= box.lo[2] && z < box.hi[2];
+                    sel |= (in ? 1u : 0u) << k;
+                    if (++z == sz) {
+                        z = 0;
+                        if (++y == sy) { y = 0; x++; }
+                    }
+                }
+            }
+            if (sel) {
+                uint32_t *wp = (uint32_t *)P.pending + w;
+                const uint32_t old = *wp;
+                uint32_t nv = old;
+#pragma unroll
+                for (uint32_t k = 0; k < 4; k++)
+                    if (((sel >> k) & 1u) && ((old >> (8 * k)) & 255u) < prio) nv = (nv & ~(255u << (8 * k))) | (prio << (8 * k));
+                if (nv != old) *wp = nv;
+            }
+        }
+        const uint32_t n = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(sel));
+        if (lane == 0) s_n[wid] = n;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t c = 0;
+            for (int i = 0; i < 8; i++) c += s_n[i];
+            if (c && P.tile_max[tile] < prio) P.tile_max[tile] = prio;
+            total += c;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0 && total) atomicAdd(&P.counters->queued, total);
+}
+
 // Taking the set of changed cubes: an ordered stream compaction of the bitmap.  A chunk is the CHANGES_CHUNK_WORDS
 // words of bits (32 768 cubes) one 256-thread block reads, four consecutive words per thread.
 constexpr uint32_t CHANGES_CHUNK_WORDS = 1024;
@@ -1215,6 +1287,76 @@ aicb_status light_set_physics(LightReplicas r, const DeviceScene &sky, uint32_t 
     return AICB_OK;
 }
 
+// k_queue_cubes on replica 0 (its texels, its queue), behind the work queued on its context: the cube updates and
+// uploads whose texels the load rule reads.  *n_queued: the cubes selected.
+static aicb_status queue_cubes(LightReplicas r, bool uninit, const QueueBox &box, uint8_t priority, size_t *n_queued) {
+    aicb_scene *s = r.scene[0];
+    const LightParams P = light_params(r, 0);
+    cudaStream_t st = s->ctx->stream.get();
+    uint32_t tile0 = 0, tile1 = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
+    if (!uninit) {   // the tiles from the box's first cube to its last
+        const uint32_t sy = (uint32_t)s->ds.size[1], sz = (uint32_t)s->ds.size[2];
+        tile0 = ((box.lo[0] * sy + box.lo[1]) * sz + box.lo[2]) / LIGHT_TILE;
+        tile1 = (((box.hi[0] - 1) * sy + box.hi[1] - 1) * sz + box.hi[2] - 1) / LIGHT_TILE + 1;
+    }
+    const uint32_t blocks = std::min(tile1 - tile0, (uint32_t)s->ctx->num_sms * 32u);
+    CU(cudaMemsetAsync(&P.counters->queued, 0, 4, st));
+    if (uninit) k_queue_cubes<true><<<blocks, 256, 0, st>>>(P, tile0, tile1, box, priority);
+    else k_queue_cubes<false><<<blocks, 256, 0, st>>>(P, tile0, tile1, box, priority);
+    CU(cudaGetLastError());
+    uint32_t n = 0;
+    CU(cudaMemcpyAsync(&n, &P.counters->queued, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (n_queued) *n_queued = n;
+    return AICB_OK;
+}
+
+// Space::new_from_builder's load rule (space.rs:290-313): every cube of replica 0's volume whose texel is
+// Uninitialized enters the queue at Priority::UNINIT.  No texel is written and nothing propagates.
+aicb_status light_queue_uninitialized(LightReplicas r, size_t *n_queued) {
+    TRY(ensure_replicas(r));
+    return queue_cubes(r, true, QueueBox{}, PRIO_UNINIT, n_queued);
+}
+
+// LightStorage::light_needs_update_in_region (updater.rs:122-133): every cube of region ∩ bounds at `priority`.  Its
+// sweep branch (more than 400 cubes) queues the same cubes at the same priority.
+aicb_status light_queue_region(LightReplicas r, const aicb_aab *region, uint8_t priority) {
+    if (!region) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (priority == 0) return aicb_fail(AICB_ERR_INVALID, "priority 0 (Priority::MIN) never enters the queue");
+    TRY(ensure_replicas(r));
+    const DeviceScene &ds = r.scene[0]->ds;
+    QueueBox box;
+    for (int a = 0; a < 3; a++) {
+        const int64_t lo = std::max<int64_t>(region->lower[a], ds.lo[a]);
+        const int64_t hi = std::min<int64_t>((int64_t)region->lower[a] + region->size[a], (int64_t)ds.lo[a] + ds.size[a]);
+        if (hi <= lo) return AICB_OK;   // an empty intersection
+        box.lo[a] = (uint32_t)(lo - ds.lo[a]);
+        box.hi[a] = (uint32_t)(hi - ds.lo[a]);
+    }
+    return queue_cubes(r, false, box, priority, nullptr);
+}
+
+// The pending bytes are the whole queue between light calls; a scene with no light call yet has an empty queue.
+aicb_status light_download_queue(aicb_scene *s, uint8_t *priorities, size_t n_texels, size_t *n_queued) {
+    if (!priorities) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n_texels != s->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
+    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    if (s->light.shared.pending) {
+        CU(cudaSetDevice(s->ctx->device));
+        cudaStream_t st = s->ctx->stream.get();
+        CU(cudaMemcpyAsync(priorities, s->light.shared.pending.get(), s->volume, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+    } else {
+        std::memset(priorities, 0, s->volume);
+    }
+    if (n_queued) {
+        size_t n = 0;
+        for (size_t i = 0; i < s->volume; i++) n += priorities[i] != 0;
+        *n_queued = n;
+    }
+    return AICB_OK;
+}
+
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     if (!s || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n_texels != s->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
@@ -1350,6 +1492,24 @@ aicb_status aicb_light_relight_blocks(aicb_scene *s, const uint16_t *indices, si
     if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return light_relight_blocks({&s, &s->ctx, 1}, indices, n, epsilon, updates_done, max_diff);
+}
+
+aicb_status aicb_light_queue_uninitialized(aicb_scene *s, size_t *n_queued) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_queue_uninitialized({&s, &s->ctx, 1}, n_queued);
+}
+
+aicb_status aicb_light_queue_region(aicb_scene *s, const aicb_aab *region, uint8_t priority) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_queue_region({&s, &s->ctx, 1}, region, priority);
+}
+
+aicb_status aicb_light_download_queue(aicb_scene *s, uint8_t *priorities, size_t n_texels, size_t *n_queued) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return light_download_queue(s, priorities, n_texels, n_queued);
 }
 
 aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {

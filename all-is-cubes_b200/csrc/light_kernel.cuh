@@ -69,7 +69,7 @@ constexpr uint32_t LB_ALL_OPAQUE = 1u << 6, LB_VISIBLE = 1u << 7, LB_EMISSIVE = 
 constexpr int LIGHT_MAX_DEPTH = 224;  // longest chart path is 219 (rays end at t = 127, generator.rs:101)
 
 constexpr uint32_t TX_OPAQUE = 128u << 24, TX_NO_RAYS = 1u << 24, TX_UNINIT = 0u;
-constexpr int PRIO_NEWLY_VISIBLE = 250, PRIO_ESTIMATED = 200;
+constexpr int PRIO_NEWLY_VISIBLE = 250, PRIO_UNINIT = 210, PRIO_ESTIMATED = 200;   // Priority (queue.rs)
 constexpr uint32_t LIGHT_TILE = 1024;   // cubes per queue tile (256 words of pending bytes: one 256-thread block)
 
 // A light call's counters in device memory, which the kernels count into and the host reads back.  The kernels of a
@@ -85,13 +85,14 @@ struct LightCounters {
     uint32_t compute_work;          // cubes handed out by the chain walk's compute form this round
     uint32_t mark_work;             // ... and by its mark form
     uint32_t overflow;              // entries of replica 0's overflow list
-    uint32_t _pad[6];
+    uint32_t queued;                // cubes the last queue scan (k_queue_cubes) selected
+    uint32_t _pad[5];
 };
 static_assert(offsetof(LightCounters, gathered) == 0 && offsetof(LightCounters, priority) == 4 &&
               offsetof(LightCounters, max_diff) == 8 && offsetof(LightCounters, updates) == 12 &&
               offsetof(LightCounters, node_visits) == 16 && offsetof(LightCounters, changed) == 24 &&
               offsetof(LightCounters, compute_work) == 28 && offsetof(LightCounters, mark_work) == 32 &&
-              offsetof(LightCounters, overflow) == 36 && sizeof(LightCounters) == 64,
+              offsetof(LightCounters, overflow) == 36 && offsetof(LightCounters, queued) == 40 && sizeof(LightCounters) == 64,
               "LightCounters: the layout the kernels and the round's memsets address");
 
 struct LightParams {

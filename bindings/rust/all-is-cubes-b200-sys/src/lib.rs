@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 10 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 11 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -298,6 +298,11 @@ unsafe extern "C" {
     pub fn aicb_light_relight_blocks(s: *mut aicb_scene, indices: *const u16, n: usize, epsilon: u8, updates_done: *mut u64,
                                      max_diff: *mut u8) -> aicb_status;
     pub fn aicb_light_download(s: *mut aicb_scene, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
+    // the light update queue across save and load (all-is-cubes space.rs:290-313, save/conversion.rs:773-785)
+    pub fn aicb_light_queue_uninitialized(s: *mut aicb_scene, n_queued_or_null: *mut usize) -> aicb_status;
+    pub fn aicb_light_queue_region(s: *mut aicb_scene, region: *const aicb_aab, priority: u8) -> aicb_status;
+    pub fn aicb_light_download_queue(s: *mut aicb_scene, priorities: *mut u8, n_texels: usize, n_queued_or_null: *mut usize)
+                                     -> aicb_status;
     pub fn aicb_light_stats(s: *const aicb_scene, out: *mut [u64; 4]) -> aicb_status;
     pub fn aicb_light_changes_count(s: *const aicb_scene, n_changed: *mut usize) -> aicb_status;
     pub fn aicb_light_take_changes(s: *mut aicb_scene, indices: *mut u32, texels: *mut [u8; 4], capacity: usize,
@@ -312,6 +317,11 @@ unsafe extern "C" {
                                                -> aicb_status;
     pub fn aicb_group_light_relight_blocks(gs: *mut aicb_group_scene, indices: *const u16, n: usize, epsilon: u8,
                                            updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
+    // the queue is device 0's; the scan reads replica 0's volume
+    pub fn aicb_group_light_queue_uninitialized(gs: *mut aicb_group_scene, n_queued_or_null: *mut usize) -> aicb_status;
+    pub fn aicb_group_light_queue_region(gs: *mut aicb_group_scene, region: *const aicb_aab, priority: u8) -> aicb_status;
+    pub fn aicb_group_light_download_queue(gs: *mut aicb_group_scene, priorities: *mut u8, n_texels: usize,
+                                           n_queued_or_null: *mut usize) -> aicb_status;
     pub fn aicb_group_light_download(gs: *mut aicb_group_scene, replica: c_int, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_group_light_stats(gs: *const aicb_group_scene, out: *mut [u64; 4]) -> aicb_status;
     pub fn aicb_group_light_changes_count(gs: *const aicb_group_scene, n_changed: *mut usize) -> aicb_status;

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 10
+#define AICB_ABI_VERSION 11
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -522,6 +522,30 @@ aicb_status aicb_light_edit_and_propagate(aicb_scene *, const int32_t (*cubes)[3
 aicb_status aicb_light_relight_blocks(aicb_scene *, const uint16_t *indices, size_t n, uint8_t epsilon,
                                       uint64_t *updates_done, uint8_t *max_diff);
 aicb_status aicb_light_download(aicb_scene *, uint8_t (*out)[4], size_t n_texels);
+/* The light update queue across save and load.  The queue holds one priority per cube (0: not queued); an insert raises
+ * a cube's priority and never lowers it (LightUpdateQueue::insert, space/light/queue.rs).  None of these calls writes a
+ * texel, adds to the set of changed cubes or propagates: aicb_light_evaluate follows, as the reference's step does.
+ * LightPhysics::None is AICB_ERR_INVALID, and a rejected call changes nothing.
+ *   - aicb_light_queue_uninitialized: the load rule of Space::new_from_builder (space.rs:290-313).  Every cube whose
+ *     texel's status byte is 0 (LightStatus::Uninitialized) is inserted at Priority::UNINIT (210), and
+ *     *n_queued_or_null is the number of such cubes.  A scene created without a light volume holds only NO_RAYS, so it
+ *     queues none.  A host calls it once after aicb_scene_create from a saved Space that has light (aicb_scene_create
+ *     and aicb_scene_upload_light leave the queue as it is).  The scan of the volume is ordered behind the cube updates
+ *     and uploads queued on the context.
+ *   - aicb_light_queue_region: LightStorage::light_needs_update_in_region (space/light/updater.rs:122-133).  Every cube
+ *     of region ∩ bounds is inserted at `priority`; an empty intersection does nothing.  The reference's sweep branch
+ *     (more than 400 cubes) queues the same cubes at the same priority.  After SpaceChange::EveryBlock (fill_uniform
+ *     over the whole Space, space.rs:1461-1474) a host rebuilds the scene and calls it with the bounds and 210.
+ *     AICB_ERR_INVALID: a NULL region or priority 0 (Priority::MIN never enters the queue).
+ *   - aicb_light_download_queue: each cube's queued priority, Z-major (aicb_light_download's order), 0 where it is not
+ *     queued; *n_queued_or_null is the number of queued cubes.  The copy is ordered behind all work on the context.
+ *     AICB_ERR_INVALID: a NULL output or n_texels other than the volume.  The save form of a Space
+ *     (Serialize for space::Read, save/conversion.rs:773-785) is aicb_light_download's texels with the status byte set
+ *     to 0 (Uninitialized) wherever the priority is > 0, and r, g, b kept.
+ * GPU test: tests/test_gpu_light_resume.py. */
+aicb_status aicb_light_queue_uninitialized(aicb_scene *, size_t *n_queued_or_null);
+aicb_status aicb_light_queue_region(aicb_scene *, const aicb_aab *region, uint8_t priority);
+aicb_status aicb_light_download_queue(aicb_scene *, uint8_t *priorities, size_t n_texels, size_t *n_queued_or_null);
 /* Counters of the last propagation (aicb_light_evaluate / aicb_light_edit_and_propagate / aicb_light_relight_blocks)
  * on this scene: out[0] cube updates (compute_light calls, updater.rs:368), out[1] chart nodes visited by them,
  * out[2] relaxation rounds queued, out[3] device time of the propagation in microseconds (CUDA events on the context's stream).
@@ -575,6 +599,13 @@ aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *, const int32_
  * own cells and writes its own OPAQUE texels; device 0 alone queues and records the changed cubes. */
 aicb_status aicb_group_light_relight_blocks(aicb_group_scene *, const uint16_t *indices, size_t n, uint8_t epsilon,
                                             uint64_t *updates_done, uint8_t *max_diff);
+/* The queue calls on the group: the queue is device 0's, and aicb_group_light_queue_uninitialized scans replica 0's
+ * volume (the replicas' are identical).  Validation is against replica 0 before anything changes, and each call holds
+ * every context of the group. */
+aicb_status aicb_group_light_queue_uninitialized(aicb_group_scene *, size_t *n_queued_or_null);
+aicb_status aicb_group_light_queue_region(aicb_group_scene *, const aicb_aab *region, uint8_t priority);
+aicb_status aicb_group_light_download_queue(aicb_group_scene *, uint8_t *priorities, size_t n_texels,
+                                            size_t *n_queued_or_null);
 /* Replica `replica` (0 .. group size - 1) of the light volume. */
 aicb_status aicb_group_light_download(aicb_group_scene *, int replica, uint8_t (*out)[4], size_t n_texels);
 /* aicb_light_stats of the group's last light call: counters summed over the devices; out[3] is device 0's device time

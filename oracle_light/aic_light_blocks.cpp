@@ -100,4 +100,45 @@ void orc_light_set_physics(orc_light *L, const aicb_sky *sky, uint8_t light_max_
     orc_light_fast_evaluate(L);
 }
 
+// The load rule of Space::new_from_builder (space.rs:290-313): every cube whose light is LightStatus::Uninitialized is
+// inserted in the queue at Priority::UNINIT, in increasing linear index order.  Returns the number of such cubes (0
+// under LightPhysics::None, which has no light storage).
+size_t orc_light_queue_uninitialized(orc_light *L) {
+    if (L->max_distance == 0) return 0;
+    size_t n = 0;
+    for (size_t idx = 0; idx < L->light.size(); idx++)
+        if (L->light[idx].s == 0) {
+            q_insert(*L, idx, PRIO_UNINIT);
+            n++;
+        }
+    return n;
+}
+
+// LightStorage::light_needs_update_in_region (updater.rs:122-133): every cube of region ∩ bounds is inserted at
+// `priority`.  The sweep branch (more than 400 cubes) queues the same set at the same priority.  Priority::MIN (0)
+// never enters the queue: -1 and nothing changes.
+int orc_light_queue_region(orc_light *L, const aicb_aab *region, uint8_t priority) {
+    if (priority == 0) return -1;
+    if (L->max_distance == 0) return 0;
+    int64_t lo[3], hi[3];
+    for (int a = 0; a < 3; a++) {
+        lo[a] = std::max<int64_t>(region->lower[a], L->bounds.lo[a]);
+        hi[a] = std::min<int64_t>((int64_t)region->lower[a] + region->size[a], L->bounds.hi[a]);
+        if (hi[a] <= lo[a]) return 0;
+    }
+    for (int64_t x = lo[0]; x < hi[0]; x++)
+        for (int64_t y = lo[1]; y < hi[1]; y++)
+            for (int64_t z = lo[2]; z < hi[2]; z++) {
+                const int32_t c[3] = {(int32_t)x, (int32_t)y, (int32_t)z};
+                light_needs_update(*L, c, priority);
+            }
+    return 0;
+}
+
+// Each cube's queued priority, Z-major, 0 where it is not queued
+void orc_light_get_queue(const orc_light *L, uint8_t *out) {
+    std::memset(out, 0, L->ids.size());
+    for (const auto &kv : L->by_cube) out[kv.first] = (uint8_t)kv.second;
+}
+
 }
