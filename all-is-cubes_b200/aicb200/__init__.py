@@ -60,6 +60,7 @@ def load_library() -> C.CDLL:
     lib.aicb_scene_update_cubes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_scene_fill_uniform.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_scene_set_physics.argtypes = [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8]
     lib.aicb_shard_pixel_count.argtypes = [C.POINTER(abi.CameraData), C.POINTER(abi.Shard)]
@@ -134,6 +135,7 @@ def load_library() -> C.CDLL:
     lib.aicb_group_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_group_scene_set_physics.argtypes = [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8]
     lib.aicb_group_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.aicb_group_scene_fill_uniform.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_group_render_layers_srgb8.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_render_layers_texture.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
@@ -727,6 +729,12 @@ class SpaceRaytracer:
         arr = _block_descs(blocks)
         _check(load_library().aicb_scene_append_blocks(self.handle, arr, len(blocks)))
 
+    def fill_uniform(self, block):
+        """SpaceChange::EveryBlock (Mutation::fill_uniform over the whole Space): the table becomes [block] and every
+        cube holds id 0.  Light is not touched: on a lit scene, light_queue_region(bounds, 210) follows."""
+        arr = _block_descs([block])
+        _check(load_library().aicb_scene_fill_uniform(self.handle, arr))
+
     # ---- light propagation (space::light; SURVEY 8(a) L1-L4) ----
     def light_fast_evaluate(self):
         """LightStorage::fast_evaluate_light (updater.rs:537-582)"""
@@ -1033,6 +1041,11 @@ class GroupScene:
         """SpaceRaytracer.append_blocks on every replica; a rejected call changes none."""
         arr = _block_descs(blocks)
         _check(load_library().aicb_group_scene_append_blocks(self.handle, arr, len(blocks)))
+
+    def fill_uniform(self, block):
+        """SpaceRaytracer.fill_uniform on every replica; a rejected call changes none."""
+        arr = _block_descs([block])
+        _check(load_library().aicb_group_scene_fill_uniform(self.handle, arr))
 
     def upload_light(self, light: np.ndarray):
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -130,6 +130,7 @@ EXPORTED_SYMBOLS = [
     "aicb_scene_update_cubes",
     "aicb_scene_update_blocks",
     "aicb_scene_append_blocks",
+    "aicb_scene_fill_uniform",
     "aicb_scene_upload_light",
     "aicb_scene_destroy",
     "aicb_scene_device_bytes",
@@ -186,6 +187,7 @@ EXPORTED_SYMBOLS = [
     "aicb_group_scene_upload_light",
     "aicb_group_scene_set_physics",
     "aicb_group_scene_append_blocks",
+    "aicb_group_scene_fill_uniform",
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",
     "aicb_group_render_layers_terminal",

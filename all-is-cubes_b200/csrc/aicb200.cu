@@ -4,10 +4,12 @@
 // No CPU fallback lives here: every compute entry point needs a CUDA device and fails with
 // AICB_ERR_CUDA otherwise.
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <unordered_map>
@@ -15,6 +17,7 @@
 
 #include <cuda_runtime.h>
 
+#include "brick_room.h"
 #include "internal.h"
 
 using namespace aicb;
@@ -298,6 +301,75 @@ static __global__ void __launch_bounds__(256) widen_cells_kernel(const uint16_t 
                           widened_cell(v.w >> 16)));
     }
     for (size_t i = n8 * 8 + first; i < n; i += stride) out[i] = widened_cell(in[i]);
+}
+
+// Every u16 cell of a scene set to one word (Mutation::fill_uniform over the whole Space): one 16-byte streaming store
+// per eight cells, the last n % 8 cells one at a time.
+static __global__ void __launch_bounds__(256) fill_cells_kernel(uint16_t *__restrict__ cells, size_t n, uint32_t word) {
+    const size_t stride = (size_t)gridDim.x * blockDim.x, first = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t pair = word | word << 16;
+    const size_t n8 = n / 8;
+    for (size_t i = first; i < n8; i += stride) __stcs(reinterpret_cast<uint4 *>(cells) + i, make_uint4(pair, pair, pair, pair));
+    for (size_t i = n8 * 8 + first; i < n; i += stride) cells[i] = (uint16_t)word;
+}
+
+// One run of a pool compaction (compact_pools): `bytes` bytes from byte `src` of the old pool to byte `dst` of the new
+// one.  Offsets and lengths are even (a u16 brick word is a pool's smallest element).
+struct PoolSegment {
+    uint64_t src, dst, bytes;
+};
+
+// Gathers a pool's live runs into a new buffer: blocks take segments in a grid-stride loop.  Within a segment, every
+// 16-byte chunk of the destination that it covers whole is one coalesced 16-byte store, assembled from the one or two
+// aligned 16-byte source chunks that hold its bytes (a funnel shift when the run moves by other than a multiple of 16
+// bytes).  The at most seven u16 words at either end, whose chunk a neighbouring segment shares, are stored one at a
+// time.  Both buffers are multiples of 16 bytes (grow_buffer, compact_pools), so an aligned source chunk that holds one
+// byte of a run lies inside the old buffer.
+static __global__ void __launch_bounds__(256) compact_pool_kernel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst,
+                                                                  const PoolSegment *__restrict__ segs, uint32_t n_segs) {
+    for (uint32_t k = blockIdx.x; k < n_segs; k += gridDim.x) {
+        const PoolSegment g = segs[k];
+        const uint64_t shift = g.src - g.dst;   // modulo 2^64: dst + shift is the source of a destination byte
+        const uint64_t c0 = (g.dst + 15) / 16, c1 = (g.dst + g.bytes) / 16;   // the chunks the segment covers whole
+        const uint32_t s = (uint32_t)(shift & 15), b = (s & 3) * 8;
+        for (uint64_t c = c0 + threadIdx.x; c < c1; c += blockDim.x) {
+            const uint4 *p = reinterpret_cast<const uint4 *>(src + ((c * 16 + shift) & ~15ull));
+            const uint4 lo = p[0];
+            uint4 out = lo;
+            if (s) {
+                const uint4 hi = p[1];
+                const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+#define FS(i) __funnelshift_r(w[i], w[(i) + 1], b)
+                switch (s >> 2) {
+                    case 0: out = make_uint4(FS(0), FS(1), FS(2), FS(3)); break;
+                    case 1: out = make_uint4(FS(1), FS(2), FS(3), FS(4)); break;
+                    case 2: out = make_uint4(FS(2), FS(3), FS(4), FS(5)); break;
+                    default: out = make_uint4(FS(3), FS(4), FS(5), FS(6)); break;
+                }
+#undef FS
+            }
+            reinterpret_cast<uint4 *>(dst)[c] = out;
+        }
+        // the words before the first whole chunk (threads 0-7) and after the last (threads 8-15)
+        const uint64_t end = g.dst + g.bytes, head_end = min(c0 * 16, end), tail = max(c1 * 16, head_end);
+        if (threadIdx.x < 16) {
+            const uint64_t x = threadIdx.x < 8 ? g.dst + 2 * threadIdx.x : tail + 2 * (threadIdx.x - 8);
+            if (x < (threadIdx.x < 8 ? head_end : end))
+                reinterpret_cast<uint16_t *>(dst)[x / 2] = reinterpret_cast<const uint16_t *>(src)[(x + shift) / 2];
+        }
+    }
+}
+
+// After a compaction, each id's record takes its extents' new offsets ({brick word, palette entry} per id); a single
+// voxel's blk_tab entry carries its absolute palette entry (block_entry).
+static __global__ void rebase_blocks_kernel(BlockRec *blocks, float4 *blk_tab, const uint2 *__restrict__ off, uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    BlockRec r = blocks[i];
+    r.brick_off = off[i].x;
+    r.pal_off = off[i].y;
+    blocks[i] = r;
+    if ((r.kind_res & 0xffu) == KIND_SINGLE) blk_tab[i].z = __uint_as_float(off[i].y);
 }
 
 static aicb_status validate_options(const aicb_options *o) {
@@ -645,14 +717,16 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
 // ---------------------------------------------------------------------------------------------
 // a scene's block table (internal.h): flattened once, placed on each replica
 // ---------------------------------------------------------------------------------------------
+static size_t round16(size_t bytes) { return (bytes + 15) & ~(size_t)15; }
+
 // Room for `bytes` in `buf`, of which the first `used` are kept.  A buffer that is too small is replaced by one of at
-// least twice its size (exactly `bytes` if it was empty), its `used` bytes copied on `stream`; the replaced buffer goes
-// to `retired`.  Appending k elements one call at a time thus reallocates O(log k) times.
+// least twice its size (`bytes` rounded up to 16 if it was empty), its `used` bytes copied on `stream`; the replaced
+// buffer goes to `retired`.  Appending k elements one call at a time thus reallocates O(log k) times.
 static aicb_status grow_buffer(DeviceBuffer &buf, size_t used, size_t bytes, cudaStream_t stream,
                                std::vector<DeviceBuffer> *retired) {
     if (buf.bytes() >= bytes) return AICB_OK;
     DeviceBuffer b;
-    TRY(b.ensure(std::max(bytes, 2 * buf.bytes())));
+    TRY(b.ensure(std::max(round16(bytes), 2 * buf.bytes())));
     if (used) CU(cudaMemcpyAsync(b.get(), buf.get(), used, cudaMemcpyDeviceToDevice, stream));
     if (buf) retired->push_back(std::move(buf));
     buf = std::move(b);
@@ -677,9 +751,10 @@ struct Retired {
 };
 
 // Block definitions flattened against a table: per definition its record (brick_off / pal_off already offsets into the
-// table's pools), blk_tab entry, kind and light record; and the voxel data they append to the pools.
+// table's pools) and extents, blk_tab entry, kind and light record; and the voxel data they append to the pools.
 struct FlatBlocks {
     std::vector<BlockRec> recs;
+    std::vector<BlockTable::Extent> extents;
     std::vector<float4> blk_tab;
     std::vector<uint8_t> kinds;
     std::vector<LightBlockDev> light;
@@ -695,6 +770,7 @@ static aicb_status flatten_blocks(const BlockTable &t, const aicb_block_desc *de
     if (!indices && t.block_count() + n > 65536) return fail(AICB_ERR_INVALID, "more than 65536 blocks");
     const uint32_t pal_base = (uint32_t)(t.n_palette / 2);   // palette entries (2 x float4 each)
     f->recs.resize(n);
+    f->extents.resize(n);
     f->blk_tab.resize(n);
     f->kinds.resize(n);
     f->light.resize(n);
@@ -702,13 +778,19 @@ static aicb_status flatten_blocks(const BlockTable &t, const aicb_block_desc *de
         if (indices && indices[i] >= t.block_count())
             return fail(AICB_ERR_INVALID, "block index out of range (new indices need a new scene)");
         BlockRec &r = f->recs[i];
+        const size_t bricks_before = f->bricks.size(), pal_before = f->pal_tab.size();
         TRY(flatten_block(descs[i], r, f->kinds[i], f->bricks, f->palette, f->pal_tab));
         f->blk_tab[i] = block_entry(f->kinds[i], r.pal_off, f->pal_tab, pal_base);
         if (f->kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)t.n_bricks;
         if (!descs[i].is_air) r.pal_off += pal_base;
+        f->extents[i] = {r.brick_off, (uint32_t)(f->bricks.size() - bricks_before), r.pal_off,
+                         (uint32_t)(f->pal_tab.size() - pal_before)};
         f->light[i] = light_block(descs[i]);
     }
-    if (t.n_bricks + f->bricks.size() > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
+    // live data only: the dead part of the pool is compacted away before it could push positions past 2^32
+    // (flatten_placeable)
+    if (brick_room(t.n_bricks, t.dead_bricks, f->bricks.size()) == BrickRoom::too_big)
+        return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
     return AICB_OK;
 }
 
@@ -748,15 +830,108 @@ static aicb_status place(aicb_scene *s, const FlatBlocks &f, const uint16_t *ind
     }
     t.kind.resize(count + added);
     t.light_flags.resize(count + added);
+    t.extent.resize(count + added);
     for (size_t i = 0; i < n; i++) {
         const size_t id = indices ? indices[i] : count + i;
+        if (indices) {   // the extents written over, an earlier definition of this call included, are dead
+            t.dead_bricks += t.extent[id].n_bricks;
+            t.dead_pal += t.extent[id].n_pal;
+        }
         t.kind[id] = f.kinds[i];
         t.light_flags[id] = f.light[i].flags;
+        t.extent[id] = f.extents[i];
     }
     t.n_bricks += f.bricks.size();
     t.n_palette += f.palette.size();
-    s->device_bytes += added * (sizeof(BlockRec) + sizeof(float4) + sizeof(LightBlockDev)) + f.bricks.size() * 2 +
-                       f.palette.size() * sizeof(float4) + f.pal_tab.size() * sizeof(float2);
+    return AICB_OK;
+}
+
+// Compacts s's brick pool and/or palette pool (palette and pal_tab): each pool's live extents, in pool order, are
+// gathered to the front of a new buffer of the live size by compact_pool_kernel, and each id's extent, record and
+// blk_tab entry follow them.  The old buffers go to `retired`.  Queued on the context's stream; the caller has waited
+// for the context (wait_context), since a frame's hit records hold absolute pool positions.  Every allocation comes
+// first: a failure changes nothing.
+static aicb_status compact_pools(aicb_scene *s, bool bricks, bool palette, Retired &retired) {
+    BlockTable &t = s->blocks;
+    aicb_ctx *ctx = s->ctx;
+    cudaStream_t stream = ctx->stream.get();
+    const size_t count = t.block_count();
+    std::vector<BlockTable::Extent> ext = t.extent;
+    // one pool's plan: its live extents in pool order, gathered to the front; the ids' new offsets go to `ext`.  Each
+    // run (neighbouring extents merged) of `elem`-byte elements becomes segments of at most 16 KiB of `segs`.
+    std::vector<PoolSegment> segs;
+    auto plan = [&](uint32_t BlockTable::Extent::*off, uint32_t BlockTable::Extent::*len, std::initializer_list<size_t> elems,
+                    std::vector<std::pair<size_t, size_t>> *seg_ranges) {
+        std::vector<uint32_t> order;
+        for (uint32_t id = 0; id < count; id++)
+            if (ext[id].*len) order.push_back(id);
+        std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return ext[a].*off < ext[b].*off; });
+        std::vector<std::array<size_t, 3>> runs;   // src, dst, elements
+        size_t live = 0;
+        for (const uint32_t id : order) {
+            BlockTable::Extent &e = ext[id];
+            if (!runs.empty() && runs.back()[0] + runs.back()[2] == e.*off) runs.back()[2] += e.*len;
+            else runs.push_back({e.*off, live, e.*len});
+            e.*off = (uint32_t)live;
+            live += e.*len;
+        }
+        const size_t SEG = 16384;
+        for (const size_t elem : elems) {
+            const size_t first = segs.size();
+            for (const auto &r : runs)
+                for (size_t k = 0; k < r[2] * elem; k += SEG)
+                    segs.push_back({r[0] * elem + k, r[1] * elem + k, std::min(SEG, r[2] * elem - k)});
+            seg_ranges->push_back({first, segs.size() - first});
+        }
+        return live;
+    };
+    std::vector<std::pair<size_t, size_t>> ranges;   // per buffer gathered: its segments in `segs`
+    const size_t live_bricks = bricks ? plan(&BlockTable::Extent::brick_off, &BlockTable::Extent::n_bricks, {2}, &ranges) : 0;
+    const size_t live_pal = palette ? plan(&BlockTable::Extent::pal_off, &BlockTable::Extent::n_pal,
+                                           {2 * sizeof(float4), sizeof(float2)}, &ranges) : 0;
+    DeviceBuffer new_bricks, new_palette, new_pal_tab, d_segs, d_off;
+    if (bricks) TRY(new_bricks.ensure(round16(live_bricks * 2)));
+    if (palette) {
+        TRY(new_palette.ensure(live_pal * 2 * sizeof(float4)));
+        TRY(new_pal_tab.ensure(round16(live_pal * sizeof(float2))));
+    }
+    TRY(d_segs.ensure(segs.size() * sizeof(PoolSegment)));
+    TRY(d_off.ensure(count * sizeof(uint2)));
+    std::vector<uint2> off(count);
+    for (size_t id = 0; id < count; id++) off[id] = make_uint2(ext[id].brick_off, ext[id].pal_off);
+    if (!segs.empty())
+        CU(cudaMemcpyAsync(d_segs.get(), segs.data(), segs.size() * sizeof(PoolSegment), cudaMemcpyHostToDevice, stream));
+    if (count) CU(cudaMemcpyAsync(d_off.get(), off.data(), count * sizeof(uint2), cudaMemcpyHostToDevice, stream));
+    size_t next = 0;
+    auto gather = [&](DeviceBuffer &buf, DeviceBuffer &to) {
+        const auto [first, n] = ranges[next++];
+        if (n) {
+            const unsigned grid = (unsigned)std::min(n, (size_t)ctx->num_sms * 8);
+            compact_pool_kernel<<<grid, 256, 0, stream>>>(buf.get<const uint8_t>(), to.get<uint8_t>(),
+                                                          d_segs.get<const PoolSegment>() + first, (uint32_t)n);
+        }
+        if (buf) retired.bufs.push_back(std::move(buf));
+        buf = std::move(to);
+    };
+    if (bricks) {
+        gather(t.bricks, new_bricks);
+        t.n_bricks = live_bricks;
+        t.dead_bricks = 0;
+    }
+    if (palette) {
+        gather(t.palette, new_palette);
+        gather(t.pal_tab, new_pal_tab);
+        t.n_palette = live_pal * 2;
+        t.dead_pal = 0;
+    }
+    t.extent = std::move(ext);
+    t.bind(s->ds);
+    if (count)
+        rebase_blocks_kernel<<<(unsigned)((count + 127) / 128), 128, 0, stream>>>(
+            t.blocks.get<BlockRec>(), t.blk_tab.get<float4>(), d_off.get<const uint2>(), (uint32_t)count);
+    retired.bufs.push_back(std::move(d_segs));
+    retired.bufs.push_back(std::move(d_off));
+    CU(cudaGetLastError());
     return AICB_OK;
 }
 
@@ -830,12 +1005,32 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
     return AICB_OK;
 }
 
+// flatten_blocks against replica 0's table, for an update (`indices`) or an append (nullptr) of the scene's replicas,
+// such that the result can be placed: brick positions are u32, so when the live data fits but the pool's words in use
+// plus the new ones would not (brick_room), every replica's brick pool is compacted first and the definitions are
+// flattened again against the compacted table.  A compaction moves the pools, so each replica's context is waited
+// for first (wait_context).
+static aicb_status flatten_placeable(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks,
+                                     const uint16_t *indices, FlatBlocks *f) {
+    const BlockTable &t = s[0]->blocks;
+    TRY(flatten_blocks(t, descs, n_blocks, indices, f));
+    if (brick_room(t.n_bricks, t.dead_bricks, f->bricks.size()) != BrickRoom::compact_first) return AICB_OK;
+    for (size_t r = 0; r < n; r++) {
+        CU(cudaSetDevice(s[r]->ctx->device));
+        TRY(wait_context(s[r]->ctx));
+        Retired retired{s[r]->ctx, {}};
+        TRY(compact_pools(s[r], true, false, retired));
+    }
+    *f = FlatBlocks();
+    return flatten_blocks(t, descs, n_blocks, indices, f);
+}
+
 aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t *indices, const aicb_block_desc *descs,
                                  size_t n_blocks) {
     if (n_blocks == 0) return AICB_OK;
     const BlockTable &t = s[0]->blocks;
     FlatBlocks f;
-    TRY(flatten_blocks(t, descs, n_blocks, indices, &f));
+    TRY(flatten_placeable(s, n, descs, n_blocks, indices, &f));
     // cubes that hold a block whose kind changes carry the new kind in their cell words
     std::vector<uint8_t> kind(t.kind);
     for (size_t i = 0; i < n_blocks; i++) kind[indices[i]] = f.kinds[i];
@@ -849,13 +1044,20 @@ aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t 
             idx++;
         }
     }
+    bool compact_bricks = false, compact_palette = false;   // replica 0's decision, which every replica takes
     for (size_t r = 0; r < n; r++) {
         aicb_ctx *ctx = s[r]->ctx;
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
-        TRY(wait_context(ctx));   // the records are written over in place
+        TRY(wait_context(ctx));   // the records are written over in place, and compaction moves the pools
         Retired retired{ctx, {}};
         TRY(place(s[r], f, indices, retired));
+        if (r == 0) {
+            const BlockTable &t0 = s[0]->blocks;
+            compact_bricks = t0.dead_bricks > t0.n_bricks - t0.dead_bricks;
+            compact_palette = t0.dead_pal > t0.n_palette / 2 - t0.dead_pal;
+        }
+        if (compact_bricks || compact_palette) TRY(compact_pools(s[r], compact_bricks, compact_palette, retired));
         if (!ops.empty()) {
             DeviceBuffer d_ops;
             TRY(d_ops.ensure(ops.size() * sizeof(CubeDelta)));
@@ -879,7 +1081,7 @@ aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t 
 aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks) {
     if (n_blocks == 0) return AICB_OK;
     FlatBlocks f;
-    TRY(flatten_blocks(s[0]->blocks, descs, n_blocks, nullptr, &f));
+    TRY(flatten_placeable(s, n, descs, n_blocks, nullptr, &f));
     for (size_t r = 0; r < n; r++) {
         aicb_scene *sc = s[r];
         aicb_ctx *ctx = sc->ctx;
@@ -905,6 +1107,54 @@ aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_bloc
         }
         TRY(place(sc, f, nullptr, retired));
         CU(cudaEventRecord(ctx->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
+    }
+    return AICB_OK;
+}
+
+// Mutation::fill_uniform over the whole Space (space.rs:1461-1474), the source of SpaceChange::EveryBlock: the table
+// becomes [block] in exact-size buffers, as a new scene's, and every cell id 0 with its kind, written on the device
+// (u32 cells go back to u16: a one-block table fits them).  Light is not touched.  Each replica's context is waited for
+// first, since the table and the cells are replaced, and the call returns once its writes are done.  On each replica
+// the allocations come before any change, so a failure leaves that replica as it was.
+aicb_status scenes_fill_uniform(aicb_scene *const *s, size_t n, const aicb_block_desc *block) {
+    FlatBlocks f;
+    TRY(flatten_blocks(BlockTable(), block, 1, nullptr, &f));
+    const uint32_t word = cell_word(0, f.kinds[0], false);
+    for (size_t r = 0; r < n; r++) {
+        aicb_scene *sc = s[r];
+        aicb_ctx *ctx = sc->ctx;
+        cudaStream_t stream = ctx->stream.get();
+        CU(cudaSetDevice(ctx->device));
+        TRY(wait_context(ctx));
+        Retired retired{ctx, {}};
+        DeviceBuffer narrow;
+        if (sc->ds.wide_cells && sc->volume) TRY(narrow.ensure(sc->volume * 2));
+        BlockTable old = std::move(sc->blocks);
+        sc->blocks = BlockTable();
+        const aicb_status st = place(sc, f, nullptr, retired);
+        if (st != AICB_OK) {
+            sc->blocks = std::move(old);
+            sc->blocks.bind(sc->ds);
+            return st;
+        }
+        for (DeviceBuffer *b : {&old.blocks, &old.blk_tab, &old.light, &old.bricks, &old.palette, &old.pal_tab})
+            if (*b) retired.bufs.push_back(std::move(*b));
+        if (narrow) {
+            retired.bufs.push_back(std::move(sc->d_cells));
+            sc->d_cells = std::move(narrow);
+            sc->ds.cells = sc->d_cells.get();
+            sc->device_bytes -= sc->volume * 2;
+        }
+        sc->ds.wide_cells = 0;
+        if (sc->volume) {
+            const size_t want = (std::max<size_t>(sc->volume / 8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
+            fill_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, stream>>>(sc->d_cells.get<uint16_t>(), sc->volume,
+                                                                                  word);
+            CU(cudaGetLastError());
+        }
+        sc->h_ids.assign(sc->volume, 0);
+        CU(cudaEventRecord(ctx->ev_delta.get(), stream));
+        TRY(wait_context(ctx));   // the call returns once its writes are done
     }
     return AICB_OK;
 }
@@ -1013,7 +1263,7 @@ void aicb_scene_destroy(aicb_scene *s) {
     delete s;
 }
 
-uint64_t aicb_scene_device_bytes(const aicb_scene *s) { return s ? s->device_bytes : 0; }
+uint64_t aicb_scene_device_bytes(const aicb_scene *s) { return s ? s->device_bytes + s->blocks.bytes() : 0; }
 
 aicb_status aicb_scene_set_physics(aicb_scene *s, const aicb_sky *sky, uint8_t light_max_distance) {
     if (!s || !sky) return fail(AICB_ERR_INVALID, "NULL argument");
@@ -1077,8 +1327,8 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
 
 // == SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; UpdatingSpaceRaytracer::update handles them in
 // updating.rs:128-150 by re-running TracingBlock::from_block for the changed indices): replace the definition of
-// existing block indices.  New voxel data is appended to the brick pool and the palette (the replaced ranges are
-// reclaimed by the next aicb_scene_create); cubes that hold a block whose classification changed are re-encoded.
+// existing block indices.  New voxel data is appended to the brick pool and the palette, and the replaced ranges are
+// reclaimed by compaction (BlockTable); cubes that hold a block whose classification changed are re-encoded.
 // Does not touch light: aicb_light_relight_blocks with the same indices applies the light side of the change.
 aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
     if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
@@ -1092,6 +1342,13 @@ aicb_status aicb_scene_append_blocks(aicb_scene *s, const aicb_block_desc *descs
     if (!s || (n && !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     return scenes_append_blocks(&s, 1, descs, n);
+}
+
+// == SpaceChange::EveryBlock (Mutation::fill_uniform over the whole bounds, space.rs:1461-1474).
+aicb_status aicb_scene_fill_uniform(aicb_scene *s, const aicb_block_desc *block) {
+    if (!s || !block) return fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return scenes_fill_uniform(&s, 1, block);
 }
 
 aicb_status aicb_scene_upload_light(aicb_scene *s, const uint8_t (*light)[4], size_t n_texels) {

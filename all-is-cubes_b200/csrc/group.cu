@@ -352,6 +352,12 @@ aicb_status aicb_group_scene_append_blocks(aicb_group_scene *gs, const aicb_bloc
     return scenes_append_blocks(gs->scene.data(), gs->scene.size(), descs, n);
 }
 
+aicb_status aicb_group_scene_fill_uniform(aicb_group_scene *gs, const aicb_block_desc *block) {
+    if (!gs || !block) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    return scenes_fill_uniform(gs->scene.data(), gs->scene.size(), block);
+}
+
 aicb_status aicb_group_scene_set_physics(aicb_group_scene *gs, const aicb_sky *sky, uint8_t light_max_distance) {
     if (!gs || !sky) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     ContextLocks lock(gs->group->ctx);

@@ -218,10 +218,22 @@ struct aicb_ctx {
 
 // A scene's block table: everything indexed by block id or by pool offset, on the device and on the host.  It is
 // written in one way (aicb200.cu): definitions are flattened against the table, then placed in it, appended at the
-// next ids or written over existing ones, with their voxel data appended to the pools (a replaced range is not
-// reclaimed).  Elements in use: per block id, block_count(); in the pools, n_bricks and n_palette.  The buffers may be
-// larger: they grow geometrically (grow_buffer).
+// next ids or written over existing ones, with their voxel data appended to the pools.  Elements in use: per block id,
+// block_count(); in the pools, n_bricks and n_palette.  The buffers may be larger: they grow geometrically
+// (grow_buffer), to multiples of 16 bytes.
+//
+// Each id's extent in both pools is recorded.  A definition written over an id makes its old extents dead; once a
+// pool's dead part exceeds its live part, the pool is compacted (compact_pools): its live extents are gathered on the
+// device into a buffer of the live size, and every id's records follow them.  A pool thus holds at most twice its live
+// data after every call, and each dead element is copied O(1) times, amortised.  A frame's hit records hold absolute
+// pool positions, so a compaction runs only once nothing on the context can read the pools (wait_context), as
+// aicb_scene_update_blocks waits anyway.
 struct BlockTable {
+    struct Extent {
+        uint32_t brick_off, n_bricks;   // u16 words of the brick pool
+        uint32_t pal_off, n_pal;        // palette entries (two float4 each, and one pal_tab pair)
+    };
+
     DeviceBuffer blocks;    // per block id: BlockRec
     DeviceBuffer blk_tab;   // per block id: the pal_tab pair and the palette entry of single-voxel blocks
     DeviceBuffer light;     // per block id: LightBlockDev (light propagation)
@@ -230,9 +242,16 @@ struct BlockTable {
     DeviceBuffer pal_tab;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
     std::vector<uint8_t> kind;           // per block id: its kind, which its cubes' cell words carry
     std::vector<uint32_t> light_flags;   // per block id: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission
+    std::vector<Extent> extent;          // per block id: its voxel data in the pools
     size_t n_bricks = 0, n_palette = 0;  // u16 words, float4s
+    size_t dead_bricks = 0, dead_pal = 0;   // of those, u16 words and palette entries no id's extent holds
 
     size_t block_count() const { return kind.size(); }
+    // what aicb_scene_device_bytes counts of the table: the per-id records and the pools' elements in use, live or dead
+    size_t bytes() const {
+        return block_count() * (sizeof(aicb::BlockRec) + sizeof(float4) + sizeof(LightBlockDev)) + n_bricks * 2 +
+               n_palette * sizeof(float4) + n_palette / 2 * sizeof(float2);
+    }
     // the scene's pointers into the current buffers (LightParams::blocks is read from `light` by light_params)
     void bind(aicb::DeviceScene &ds) const {
         ds.blocks = blocks.get<aicb::BlockRec>();
@@ -247,7 +266,7 @@ struct aicb_scene {
     aicb_ctx *ctx = nullptr;
     aicb::DeviceScene ds{};
     size_t volume = 0;
-    uint64_t device_bytes = 0;
+    uint64_t device_bytes = 0;   // every array but the block table's (aicb_scene_device_bytes adds BlockTable::bytes)
     DeviceBuffer d_cells;
     DeviceBuffer d_light;
     BlockTable blocks;
@@ -341,6 +360,7 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
 aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t *indices, const aicb_block_desc *descs,
                                  size_t n_blocks);
 aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks);
+aicb_status scenes_fill_uniform(aicb_scene *const *s, size_t n, const aicb_block_desc *block);
 
 // group.cu: the order between the listed contexts' streams: every other context's stream waits until device 0's has
 // reached this point (fan_out), or device 0's until every other one's has (fan_in, which leaves device 0 current).

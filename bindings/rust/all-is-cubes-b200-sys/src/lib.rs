@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 11 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 12 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -197,6 +197,8 @@ unsafe extern "C" {
     pub fn aicb_scene_update_blocks(s: *mut aicb_scene, indices: *const u16, descs: *const aicb_block_desc, n: usize) -> aicb_status;
     // SpaceChange::BlockIndex for indices past the table: the blocks become the table's next indices
     pub fn aicb_scene_append_blocks(s: *mut aicb_scene, descs: *const aicb_block_desc, n: usize) -> aicb_status;
+    // SpaceChange::EveryBlock: the table becomes [block] and every cube holds id 0; light is not touched
+    pub fn aicb_scene_fill_uniform(s: *mut aicb_scene, block: *const aicb_block_desc) -> aicb_status;
     pub fn aicb_scene_upload_light(s: *mut aicb_scene, light: *const [u8; 4], n_texels: usize) -> aicb_status;
     pub fn aicb_scene_destroy(s: *mut aicb_scene);
     pub fn aicb_scene_device_bytes(s: *const aicb_scene) -> u64;
@@ -260,6 +262,8 @@ unsafe extern "C" {
                                         -> aicb_status;
     // every replica; validated against replica 0 first, so a rejected call changes none
     pub fn aicb_group_scene_append_blocks(gs: *mut aicb_group_scene, descs: *const aicb_block_desc, n: usize) -> aicb_status;
+    // every replica; validated once, so a rejected call changes none
+    pub fn aicb_group_scene_fill_uniform(gs: *mut aicb_group_scene, block: *const aicb_block_desc) -> aicb_status;
     // aicb_render_layers_* on a group: both layers must be scenes of the same group
     pub fn aicb_group_render_layers_srgb8(world: *const aicb_group_layer, ui: *const aicb_group_layer,
                                           backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],

@@ -147,6 +147,24 @@ impl SceneHandle {
         })
     }
 
+    fn fill_uniform(self, block: &sys::aicb_block_desc) -> Result<(), B200Error> {
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_scene_fill_uniform(s, block),
+                Self::Group(s) => sys::aicb_group_scene_fill_uniform(s, block),
+            }
+        })
+    }
+
+    fn light_queue_region(self, region: &sys::aicb_aab, priority: u8) -> Result<(), B200Error> {
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_light_queue_region(s, region, priority),
+                Self::Group(s) => sys::aicb_group_light_queue_region(s, region, priority),
+            }
+        })
+    }
+
     fn update_cubes(self, cubes: &[[i32; 3]], ids: &[u16], light: &[[u8; 4]]) -> Result<(), B200Error> {
         check(unsafe {
             match self {
@@ -249,7 +267,7 @@ impl SceneFollower {
         if todo.listener {
             space.listen(self.todo.listener());
         }
-        if self.scene.is_none() || todo.everything {
+        if self.scene.is_none() {
             // SpaceRaytracer::new (sr.rs:64-88): bounds, extract() of (block index, light texel), block_data(), sky
             let bounds = space.bounds();
             let cubes = space.extract(bounds, |e| (e.block_index(), e.light().as_texel())); // space.rs:740-761, Z-major
@@ -275,6 +293,19 @@ impl SceneFollower {
             }
             self.chars = space.block_data().iter().map(character_of).collect();
         } else if let Some(scene) = self.scene {
+            // SpaceChange::EveryBlock: Mutation::fill_uniform over the whole bounds (space.rs:1461-1474), the one
+            // source of it, left every cube holding palette index 0.  The scene takes the fill in place (the table
+            // becomes [data[0]]) and, if the Space is lit, queues every cube at Priority::UNINIT as the reference
+            // does; the light texels stay as they are.  The changes that came after it follow below.
+            if todo.everything {
+                let data = space.block_data();
+                let block = block_desc_of(&data[0]);
+                scene.fill_uniform(&block.as_ffi()).map_err(to_render_error)?;
+                if !matches!(space.physics().light, space::LightPhysics::None) {
+                    scene.light_queue_region(&convert::aab_of(space.bounds()), 210).map_err(to_render_error)?;
+                }
+                self.chars = vec![character_of(&data[0])];
+            }
             // SpaceChange::BlockIndex for indices past the table: append TracingBlock::from_block of every entry the
             // scene lacks (updating.rs:145-151); on a group every replica takes them (aicb_group_scene_append_blocks)
             let known = self.chars.len();

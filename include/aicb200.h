@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 11
+#define AICB_ABI_VERSION 12
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -200,7 +200,11 @@ aicb_status aicb_scene_create(aicb_ctx *, const aicb_scene_desc *, aicb_scene **
 aicb_status aicb_scene_update_cubes(aicb_scene *, const int32_t (*cubes)[3], const uint16_t *block_ids,
                                     const uint8_t (*light)[4], size_t n);
 /* SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; updating.rs:128-150): new definitions for EXISTING
- * block indices (an index beyond the table is rejected: aicb_scene_append_blocks adds new ones).  Voxel data is appended to the device pools; cubes
+ * block indices (an index beyond the table is rejected: aicb_scene_append_blocks adds new ones).  Voxel data is appended to the device pools, and the
+ * replaced definitions' voxel data is reclaimed: once a pool's replaced part exceeds its live part, the call compacts
+ * that pool on the device (after the wait below, since a frame's hit records hold absolute pool positions).  A pool
+ * thus holds at most twice its live data, and aicb_scene_device_bytes counts live and not yet compacted data alike.
+ * The 2^32-voxel limit of the brick pool applies to live data.  Cubes
  * holding a block whose classification (invisible / single voxel / voxel brick) changed are re-encoded.  Light is not
  * touched: call aicb_light_relight_blocks with the same indices afterwards to bring the light up to date.  The call first waits for the context's frame in flight and the work queued
  * on the context's stream, and returns once its own device writes are done; it does not wait for other contexts, or
@@ -216,6 +220,16 @@ aicb_status aicb_scene_update_blocks(aicb_scene *, const uint16_t *indices, cons
  * n > 0, count + n > 65536, or a descriptor that scene creation rejects; a rejected call changes nothing.  n == 0 does
  * nothing.  GPU test: tests/test_gpu_append_blocks.py. */
 aicb_status aicb_scene_append_blocks(aicb_scene *, const aicb_block_desc *descs, size_t n);
+/* SpaceChange::EveryBlock: Mutation::fill_uniform over the whole bounds (space.rs:1461-1474).  The block table becomes
+ * exactly [block] and every cube holds id 0; device buffers larger than a new one-block scene needs are freed, and a
+ * scene with 32-bit cells goes back to 16-bit cells.  The cells are written on the device.  Light is not touched: the
+ * volume, the queue and the set of changed cubes stay as they are, as the reference leaves them; a lit scene's host
+ * follows with aicb_light_queue_region(scene, &bounds, 210) and, when it wants the light to move, aicb_light_evaluate.
+ * Afterwards every output, and aicb_scene_device_bytes, is what a scene created from the filled Space with
+ * aicb_light_download's light gives.  Waiting and ordering are aicb_scene_update_blocks': a frame issued earlier on a
+ * caller's stream is the old scene's frame.  AICB_ERR_INVALID: a NULL argument or a descriptor that aicb_scene_create
+ * rejects; a rejected call changes nothing.  GPU test: tests/test_gpu_fill_uniform.py. */
+aicb_status aicb_scene_fill_uniform(aicb_scene *, const aicb_block_desc *block);
 /* Whole light volume replaced (after light propagation on the host or on another rank). */
 aicb_status aicb_scene_upload_light(aicb_scene *, const uint8_t (*light)[4], size_t n_texels);
 void aicb_scene_destroy(aicb_scene *);
@@ -407,8 +421,12 @@ aicb_status aicb_group_scene_update_cubes(aicb_group_scene *, const int32_t (*cu
 aicb_status aicb_group_render_srgb8(aicb_group_scene *, const aicb_camera *, const aicb_options *,
                                     uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
 /* aicb_scene_update_blocks (SpaceChange::BlockEvaluation / BlockIndex, updating.rs:128-150) and aicb_scene_upload_light
- * on every replica.  The update is validated against replica 0 first: a rejected call changes no replica.  The update
- * does not touch light: aicb_group_light_relight_blocks follows it. */
+ * on every replica.  The update is validated against replica 0 first: a rejected call changes no replica.  Whether a
+ * pool is compacted is decided from replica 0's table, and every replica compacts, so the tables stay identical.  The
+ * update does not touch light: aicb_group_light_relight_blocks follows it.  A call that fails after validation, for want
+ * of device memory on a replica other than the first (placing the definitions, or compacting a pool, there or in
+ * aicb_group_scene_append_blocks), may leave the replicas' tables different: destroy the group scene and create it
+ * again. */
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *, const uint16_t *indices, const aicb_block_desc *descs,
                                            size_t n);
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *, const uint8_t (*light)[4], size_t n_texels);
@@ -421,6 +439,9 @@ aicb_status aicb_group_scene_set_physics(aicb_group_scene *, const aicb_sky *sky
  * changes no replica.  The call holds every context of the group; a table that grows past 16384 blocks widens every
  * replica's cells on its own device. */
 aicb_status aicb_group_scene_append_blocks(aicb_group_scene *, const aicb_block_desc *descs, size_t n);
+/* aicb_scene_fill_uniform on every replica, holding every context of the group: the block is validated and flattened
+ * once, so a rejected call changes no replica, then every replica is filled on its own device. */
+aicb_status aicb_group_scene_fill_uniform(aicb_group_scene *, const aicb_block_desc *block);
 
 /* == RtScene::trace_ray_through_layers + draw_rgba (renderer.rs:454-478, 282-308) and RaytraceToTexture::do_some_tracing's
  * trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) on the whole group: the arguments, the validation and
@@ -535,7 +556,7 @@ aicb_status aicb_light_download(aicb_scene *, uint8_t (*out)[4], size_t n_texels
  *   - aicb_light_queue_region: LightStorage::light_needs_update_in_region (space/light/updater.rs:122-133).  Every cube
  *     of region ∩ bounds is inserted at `priority`; an empty intersection does nothing.  The reference's sweep branch
  *     (more than 400 cubes) queues the same cubes at the same priority.  After SpaceChange::EveryBlock (fill_uniform
- *     over the whole Space, space.rs:1461-1474) a host rebuilds the scene and calls it with the bounds and 210.
+ *     over the whole Space, space.rs:1461-1474) a host calls aicb_scene_fill_uniform, then this with the bounds and 210.
  *     AICB_ERR_INVALID: a NULL region or priority 0 (Priority::MIN never enters the queue).
  *   - aicb_light_download_queue: each cube's queued priority, Z-major (aicb_light_download's order), 0 where it is not
  *     queued; *n_queued_or_null is the number of queued cubes.  The copy is ordered behind all work on the context.
