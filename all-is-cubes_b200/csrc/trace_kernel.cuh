@@ -382,7 +382,9 @@ AICB_DEV bool tmax_valid(const Caster &c, const Ray &r) {  // valid_for_stepping
 // Raycaster::new(...).within(bounds, true) (raycast.rs:196-230, 513-545, 632-704) followed by the
 // FirstLast::Beginning part of next() (raycast.rs:255-263): advance until the first in-bounds
 // cube.  Returns false when the iterator produces nothing.  *valid = valid_for_stepping().
-AICB_NOINLINE bool caster_begin(Caster &c, const Ray &r, double ox, double oy, double oz, const Level lv, bool *valid) {
+// Inlined: as a call, its Ray and Caster went through a 160-byte stack frame per thread (100 KB of local memory per SM
+// in trace_kernel, competing with the cell, brick and ray loads for L1) and every field was a local load or store.
+AICB_DEV bool caster_begin(Caster &c, const Ray &r, double ox, double oy, double oz, const Level lv, bool *valid) {
     *valid = false;
     if (!(in_i32_range(ox) & in_i32_range(oy) & in_i32_range(oz))) return false;  // Cube::containing -> EMPTY
     {
