@@ -57,12 +57,6 @@ def load_library() -> C.CDLL:
     lib.aicb_scene_destroy.argtypes = [C.c_void_p]
     lib.aicb_scene_device_bytes.argtypes = [C.c_void_p]
     lib.aicb_scene_device_bytes.restype = C.c_uint64
-    lib.aicb_scene_update_cubes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_scene_fill_uniform.argtypes = [C.c_void_p, C.c_void_p]
-    lib.aicb_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_scene_set_physics.argtypes = [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8]
     lib.aicb_shard_pixel_count.argtypes = [C.POINTER(abi.CameraData), C.POINTER(abi.Shard)]
     lib.aicb_shard_pixel_count.restype = C.c_size_t
     lib.aicb_render_srgb8.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options),
@@ -99,17 +93,7 @@ def load_library() -> C.CDLL:
     lib.aicb_camera_project_ndc.argtypes = [C.POINTER(abi.CameraData), C.c_double, C.c_double,
                                             C.POINTER(C.c_double)]
     lib.aicb_camera_project_ndc.restype = None
-    lib.aicb_light_edit_and_propagate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8,
-                                                  C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
     lib.aicb_light_download.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    for prefix in ("aicb_light", "aicb_group_light"):
-        getattr(lib, prefix + "_relight_blocks").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8,
-                                                             C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
-    for prefix in ("aicb_light", "aicb_group_light"):
-        getattr(lib, prefix + "_queue_uninitialized").argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
-        getattr(lib, prefix + "_queue_region").argtypes = [C.c_void_p, C.POINTER(abi.Aab), C.c_uint8]
-        getattr(lib, prefix + "_download_queue").argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
-    lib.aicb_light_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
     lib.aicb_render_text.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p, C.c_size_t,
                                      C.POINTER(abi.RenderInfo)]
     lib.aicb_render_layers_srgb8.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p, C.c_void_p,
@@ -128,14 +112,8 @@ def load_library() -> C.CDLL:
     lib.aicb_group_scene_create.argtypes = [C.c_void_p, C.POINTER(abi.SceneDesc), C.POINTER(C.c_void_p)]
     lib.aicb_group_scene_destroy.argtypes = [C.c_void_p]
     lib.aicb_group_scene_destroy.restype = None
-    lib.aicb_group_scene_update_cubes.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_group_render_srgb8.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p,
                                             C.c_size_t, C.POINTER(abi.RenderInfo)]
-    lib.aicb_group_scene_update_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_group_scene_upload_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_group_scene_set_physics.argtypes = [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8]
-    lib.aicb_group_scene_append_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_group_scene_fill_uniform.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_group_render_layers_srgb8.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_render_layers_texture.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
@@ -145,22 +123,30 @@ def load_library() -> C.CDLL:
                                                       C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_light_chart.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_light_chart.restype = C.c_uint32
-    lib.aicb_light_fast_evaluate.argtypes = [C.c_void_p]
-    lib.aicb_light_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.aicb_light_evaluate.argtypes = [C.c_void_p, C.c_uint8, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
-                                        C.POINTER(C.c_uint64)]
-    lib.aicb_group_light_fast_evaluate.argtypes = [C.c_void_p]
-    lib.aicb_group_light_compute.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.aicb_group_light_evaluate.argtypes = [C.c_void_p, C.c_uint8, C.POINTER(C.c_uint64), C.POINTER(C.c_uint8),
-                                              C.POINTER(C.c_uint64)]
-    lib.aicb_group_light_edit_and_propagate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8,
-                                                        C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
     lib.aicb_group_light_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
-    lib.aicb_group_light_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
-    for prefix in ("aicb_light", "aicb_group_light"):
-        getattr(lib, prefix + "_changes_count").argtypes = [C.c_void_p, C.POINTER(C.c_size_t)]
-        getattr(lib, prefix + "_take_changes").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
-                                                           C.POINTER(C.c_size_t)]
+    # the calls of _Scene: a group scene's form of aicb_<name> is aicb_group_<name>, with the same arguments
+    u64, u8, size = C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_size_t)
+    for name, argtypes in {
+        "scene_update_cubes": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t],
+        "scene_update_blocks": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t],
+        "scene_append_blocks": [C.c_void_p, C.c_void_p, C.c_size_t],
+        "scene_fill_uniform": [C.c_void_p, C.c_void_p],
+        "scene_upload_light": [C.c_void_p, C.c_void_p, C.c_size_t],
+        "scene_set_physics": [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8],
+        "light_fast_evaluate": [C.c_void_p],
+        "light_compute": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
+        "light_evaluate": [C.c_void_p, C.c_uint8, u64, u8, u64],
+        "light_edit_and_propagate": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
+        "light_relight_blocks": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
+        "light_stats": [C.c_void_p, u64],
+        "light_queue_uninitialized": [C.c_void_p, size],
+        "light_queue_region": [C.c_void_p, C.POINTER(abi.Aab), C.c_uint8],
+        "light_download_queue": [C.c_void_p, C.c_void_p, C.c_size_t, size],
+        "light_changes_count": [C.c_void_p, size],
+        "light_take_changes": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, size],
+    }.items():
+        for prefix in ("aicb_", "aicb_group_"):
+            getattr(lib, prefix + name).argtypes = argtypes
     if lib.aicb_abi_version() != abi.ABI_VERSION:
         raise RuntimeError("libaicb200.so ABI version mismatch")
     _lib = lib
@@ -665,7 +651,149 @@ class Rendering:
     info: RenderInfo
 
 
-class SpaceRaytracer:
+class _Scene:
+    """The calls SpaceRaytracer and GroupScene share: updates of the scene and light propagation.  Each calls the C
+    function aicb_<name> through `_prefix` ("aicb_" on one context, "aicb_group_" on a group)."""
+
+    _prefix = "aicb_"
+
+    def _fn(self, name: str):
+        """This kind of scene's form of the C function aicb_<name> (on a group, aicb_group_<name>)."""
+        return getattr(load_library(), self._prefix + name)
+
+    def close(self):
+        if self.handle:
+            self._fn("scene_destroy")(self.handle)
+            self.handle = C.c_void_p()
+
+    def update_cubes(self, cubes: np.ndarray, block_ids: np.ndarray, light: Optional[np.ndarray] = None):
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
+        lt = None if light is None else np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
+        _check(self._fn("scene_update_cubes")(self.handle, c.ctypes.data, ids.ctypes.data,
+                                              lt.ctypes.data if lt is not None else None, c.shape[0]))
+
+    def update_blocks(self, indices, blocks):
+        """SpaceChange::BlockEvaluation / BlockIndex: new definitions for existing block indices.  Light is not touched:
+        light_relight_blocks(indices) follows it on a lit scene."""
+        idx = np.ascontiguousarray(indices, dtype=np.uint16)
+        arr = _block_descs(blocks)
+        _check(self._fn("scene_update_blocks")(self.handle, idx.ctypes.data, arr, len(blocks)))
+
+    def append_blocks(self, blocks):
+        """SpaceChange::BlockIndex for new indices (UpdatingSpaceRaytracer::update, updating.rs:145-151): the blocks
+        become the table's next indices, valid in update_cubes, update_blocks and light_edit_and_propagate."""
+        arr = _block_descs(blocks)
+        _check(self._fn("scene_append_blocks")(self.handle, arr, len(blocks)))
+
+    def fill_uniform(self, block):
+        """SpaceChange::EveryBlock (Mutation::fill_uniform over the whole Space): the table becomes [block] and every
+        cube holds id 0.  Light is not touched: on a lit scene, light_queue_region(bounds, 210) follows."""
+        arr = _block_descs([block])
+        _check(self._fn("scene_fill_uniform")(self.handle, arr))
+
+    def upload_light(self, light: np.ndarray):
+        lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
+        _check(self._fn("scene_upload_light")(self.handle, lt.ctypes.data, lt.shape[0]))
+
+    def set_physics(self, sky_colors, light_max_distance: int):
+        """SpaceChange::Physics (Space::set_physics): a new sky (Space's sky_colors: 1 row Uniform, 8 rows Octants) and
+        LightPhysics (0 = None, d = Rays { maximum_distance: d }).  A new sky alone leaves the light as it is; a new
+        distance reinitialises it (fast_evaluate_light, every cube changed); None frees it."""
+        _check(self._fn("scene_set_physics")(self.handle, C.byref(_sky(sky_colors)), light_max_distance))
+
+    # ---- light propagation (space::light; SURVEY 8(a) L1-L4) ----
+    def light_fast_evaluate(self):
+        """LightStorage::fast_evaluate_light (updater.rs:537-582)"""
+        _check(self._fn("light_fast_evaluate")(self.handle))
+
+    def light_compute(self, cubes: np.ndarray) -> np.ndarray:
+        """LightStorage::compute_light (updater.rs:368-418) for explicit cubes; returns texels [n,4] in input order."""
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        out = np.zeros((c.shape[0], 4), dtype=np.uint8)
+        _check(self._fn("light_compute")(self.handle, c.ctypes.data, c.shape[0], out.ctypes.data))
+        return out
+
+    def light_evaluate(self, epsilon: int = 0):
+        """Mutation::evaluate_light (space.rs:1496-1527) -> (updates, max_difference, chart_node_visits)"""
+        n, md, nv = C.c_uint64(0), C.c_uint8(0), C.c_uint64(0)
+        _check(self._fn("light_evaluate")(self.handle, epsilon, C.byref(n), C.byref(md), C.byref(nv)))
+        return int(n.value), int(md.value), int(nv.value)
+
+    def light_edit_and_propagate(self, cubes: np.ndarray, block_ids: np.ndarray, epsilon: int = 0):
+        """Mutation::set x n + evaluate_light(epsilon) -> (updates, max_difference)"""
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
+        n, md = C.c_uint64(0), C.c_uint8(0)
+        _check(self._fn("light_edit_and_propagate")(self.handle, c.ctypes.data, ids.ctypes.data, c.shape[0], epsilon,
+                                                    C.byref(n), C.byref(md)))
+        return int(n.value), int(md.value)
+
+    def light_relight_blocks(self, indices, epsilon: int = 0):
+        """The light side of SpaceChange::BlockEvaluation: after update_blocks(indices, ...), Mutation::set's light rule
+        (modified_cube_needs_update) for every cube holding one of the indices, then evaluate_light(epsilon)
+        -> (updates, max_difference)"""
+        idx = np.ascontiguousarray(indices, dtype=np.uint16).reshape(-1)
+        n, md = C.c_uint64(0), C.c_uint8(0)
+        _check(self._fn("light_relight_blocks")(self.handle, idx.ctypes.data, idx.size, epsilon, C.byref(n),
+                                                C.byref(md)))
+        return int(n.value), int(md.value)
+
+    def light_stats(self) -> dict:
+        """Counters of the last propagation: cube updates, chart node visits, rounds, device seconds."""
+        out = (C.c_uint64 * 4)()
+        _check(self._fn("light_stats")(self.handle, out))
+        return {"cube_updates": int(out[0]), "chart_node_visits": int(out[1]), "rounds": int(out[2]),
+                "device_seconds": int(out[3]) * 1e-6}
+
+    def light_changes_count(self) -> int:
+        """The number of cubes whose light texel the light calls wrote since the set was last taken
+        (SpaceChange::CubeLight, space.rs:1079-1083)."""
+        n = C.c_size_t(0)
+        _check(self._fn("light_changes_count")(self.handle, C.byref(n)))
+        return int(n.value)
+
+    def light_take_changes(self, discard: bool = False):
+        """Take the set of changed cubes -> (indices uint32[n], texels uint8[n, 4]): Z-major linear indices in increasing
+        order and each cube's texel as it is now.  discard=True empties the set without copying (both arrays empty)."""
+        indices = np.zeros(0, dtype=np.uint32)
+        texels = np.zeros((0, 4), dtype=np.uint8)
+        got = C.c_size_t(0)
+        take = self._fn("light_take_changes")
+        if discard:
+            _check(take(self.handle, None, None, 0, C.byref(got)))
+            return indices, texels
+        n = self.light_changes_count()
+        if n:
+            indices = np.zeros(n, dtype=np.uint32)
+            texels = np.zeros((n, 4), dtype=np.uint8)
+            _check(take(self.handle, indices.ctypes.data, texels.ctypes.data, n, C.byref(got)))
+        return indices, texels
+
+    def light_queue_uninitialized(self) -> int:
+        """The load rule of Space::new_from_builder (space.rs:290-313): every cube whose texel is Uninitialized (status
+        byte 0) enters the light update queue at Priority::UNINIT (210), raise-only.  Returns how many such cubes there
+        are.  Nothing propagates: light_evaluate follows."""
+        n = C.c_size_t(0)
+        _check(self._fn("light_queue_uninitialized")(self.handle, C.byref(n)))
+        return int(n.value)
+
+    def light_queue_region(self, lower, size, priority: int):
+        """LightStorage::light_needs_update_in_region (updater.rs:122-133): every cube of the box (lower, size) within the
+        bounds enters the queue at `priority` (1..255), raise-only."""
+        region = abi.Aab()
+        region.lower[:] = [int(v) for v in lower]
+        region.size[:] = [int(v) for v in size]
+        _check(self._fn("light_queue_region")(self.handle, C.byref(region), priority))
+
+    def light_download_queue(self) -> np.ndarray:
+        """Each cube's queued priority (0 = not queued), uint8 shaped like the volume."""
+        out = np.zeros(self.space.size, dtype=np.uint8)
+        _check(self._fn("light_download_queue")(self.handle, out.ctypes.data, out.size, None))
+        return out
+
+
+class SpaceRaytracer(_Scene):
     """SpaceRaytracer<()> (sr.rs:51): device-resident snapshot of a Space + graphics options."""
 
     def __init__(self, space: Space, graphics_options: GraphicsOptions, ctx: Optional[Context] = None):
@@ -676,11 +804,6 @@ class SpaceRaytracer:
         self.handle = C.c_void_p()
         _check(load_library().aicb_scene_create(self.ctx.handle, C.byref(desc), C.byref(self.handle)))
         del keep
-
-    def close(self):
-        if self.handle:
-            load_library().aicb_scene_destroy(self.handle)
-            self.handle = C.c_void_p()
 
     def __del__(self):
         try:
@@ -709,159 +832,10 @@ class SpaceRaytracer:
                                               steps.ctypes.data if want_steps else None, C.byref(info)))
         return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
 
-    def update_cubes(self, cubes: np.ndarray, block_ids: np.ndarray, light: Optional[np.ndarray] = None):
-        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
-        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
-        lt = None if light is None else np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
-        _check(load_library().aicb_scene_update_cubes(self.handle, c.ctypes.data, ids.ctypes.data,
-                                                      lt.ctypes.data if lt is not None else None, c.shape[0]))
-
-    def update_blocks(self, indices, blocks):
-        """SpaceChange::BlockEvaluation / BlockIndex: new definitions for existing block indices.  Light is not touched:
-        light_relight_blocks(indices) follows it on a lit scene."""
-        idx = np.ascontiguousarray(indices, dtype=np.uint16)
-        arr = _block_descs(blocks)
-        _check(load_library().aicb_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
-
-    def append_blocks(self, blocks):
-        """SpaceChange::BlockIndex for new indices (UpdatingSpaceRaytracer::update, updating.rs:145-151): the blocks
-        become the table's next indices, valid in update_cubes, update_blocks and light_edit_and_propagate."""
-        arr = _block_descs(blocks)
-        _check(load_library().aicb_scene_append_blocks(self.handle, arr, len(blocks)))
-
-    def fill_uniform(self, block):
-        """SpaceChange::EveryBlock (Mutation::fill_uniform over the whole Space): the table becomes [block] and every
-        cube holds id 0.  Light is not touched: on a lit scene, light_queue_region(bounds, 210) follows."""
-        arr = _block_descs([block])
-        _check(load_library().aicb_scene_fill_uniform(self.handle, arr))
-
-    # ---- light propagation (space::light; SURVEY 8(a) L1-L4) ----
-    def light_fast_evaluate(self):
-        """LightStorage::fast_evaluate_light (updater.rs:537-582)"""
-        _check(load_library().aicb_light_fast_evaluate(self.handle))
-
-    def light_compute(self, cubes: np.ndarray) -> np.ndarray:
-        """LightStorage::compute_light (updater.rs:368-418) for explicit cubes; returns texels [n,4]."""
-        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
-        out = np.zeros((c.shape[0], 4), dtype=np.uint8)
-        _check(load_library().aicb_light_compute(self.handle, c.ctypes.data, c.shape[0], out.ctypes.data))
-        return out
-
-    def light_evaluate(self, epsilon: int = 0):
-        """Mutation::evaluate_light (space.rs:1496-1527) -> (updates, max_difference, chart_node_visits)"""
-        n, md, nv = C.c_uint64(0), C.c_uint8(0), C.c_uint64(0)
-        _check(load_library().aicb_light_evaluate(self.handle, epsilon, C.byref(n), C.byref(md), C.byref(nv)))
-        return int(n.value), int(md.value), int(nv.value)
-
-    def light_edit_and_propagate(self, cubes: np.ndarray, block_ids: np.ndarray, epsilon: int = 0):
-        """Mutation::set x n + evaluate_light(epsilon) -> (updates, max_difference)"""
-        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
-        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
-        n, md = C.c_uint64(0), C.c_uint8(0)
-        _check(load_library().aicb_light_edit_and_propagate(self.handle, c.ctypes.data, ids.ctypes.data, c.shape[0], epsilon,
-                                                            C.byref(n), C.byref(md)))
-        return int(n.value), int(md.value)
-
-    def light_relight_blocks(self, indices, epsilon: int = 0):
-        """The light side of SpaceChange::BlockEvaluation: after update_blocks(indices, ...), Mutation::set's light rule
-        (modified_cube_needs_update) for every cube holding one of the indices, then evaluate_light(epsilon)
-        -> (updates, max_difference)"""
-        return _light_relight_blocks(load_library().aicb_light_relight_blocks, self.handle, indices, epsilon)
-
-    def light_stats(self) -> dict:
-        """Counters of the last propagation: cube updates, chart node visits, rounds, device seconds."""
-        out = (C.c_uint64 * 4)()
-        _check(load_library().aicb_light_stats(self.handle, out))
-        return {"cube_updates": int(out[0]), "chart_node_visits": int(out[1]), "rounds": int(out[2]),
-                "device_seconds": int(out[3]) * 1e-6}
-
     def light_download(self) -> np.ndarray:
         out = np.zeros(self.space.size + (4,), dtype=np.uint8)
         _check(load_library().aicb_light_download(self.handle, out.ctypes.data, out.size // 4))
         return out
-
-    def light_changes_count(self) -> int:
-        """The number of cubes whose light texel the light calls wrote since the set was last taken
-        (SpaceChange::CubeLight, space.rs:1079-1083)."""
-        return _light_changes_count(load_library().aicb_light_changes_count, self.handle)
-
-    def light_take_changes(self, discard: bool = False):
-        """Take the set of changed cubes -> (indices uint32[n], texels uint8[n, 4]): Z-major linear indices in increasing
-        order and each cube's texel as it is now.  discard=True empties the set without copying (both arrays empty)."""
-        return _light_take_changes(load_library().aicb_light_changes_count, load_library().aicb_light_take_changes,
-                                   self.handle, discard)
-
-    def light_queue_uninitialized(self) -> int:
-        """The load rule of Space::new_from_builder (space.rs:290-313): every cube whose texel is Uninitialized (status
-        byte 0) enters the light update queue at Priority::UNINIT (210), raise-only.  Returns how many such cubes there
-        are.  Nothing propagates: light_evaluate follows."""
-        return _light_queue_uninitialized(load_library().aicb_light_queue_uninitialized, self.handle)
-
-    def light_queue_region(self, lower, size, priority: int):
-        """LightStorage::light_needs_update_in_region (updater.rs:122-133): every cube of the box (lower, size) within the
-        bounds enters the queue at `priority` (1..255), raise-only."""
-        _light_queue_region(load_library().aicb_light_queue_region, self.handle, lower, size, priority)
-
-    def light_download_queue(self) -> np.ndarray:
-        """Each cube's queued priority (0 = not queued), uint8 shaped like the volume."""
-        return _light_download_queue(load_library().aicb_light_download_queue, self.handle, self.space.size)
-
-    def upload_light(self, light: np.ndarray):
-        lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
-        _check(load_library().aicb_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
-
-    def set_physics(self, sky_colors, light_max_distance: int):
-        """SpaceChange::Physics (Space::set_physics): a new sky (Space's sky_colors: 1 row Uniform, 8 rows Octants) and
-        LightPhysics (0 = None, d = Rays { maximum_distance: d }).  A new sky alone leaves the light as it is; a new
-        distance reinitialises it (fast_evaluate_light, every cube changed); None frees it."""
-        _check(load_library().aicb_scene_set_physics(self.handle, C.byref(_sky(sky_colors)), light_max_distance))
-
-
-def _light_relight_blocks(fn, handle, indices, epsilon):
-    idx = np.ascontiguousarray(indices, dtype=np.uint16).reshape(-1)
-    n, md = C.c_uint64(0), C.c_uint8(0)
-    _check(fn(handle, idx.ctypes.data, idx.size, epsilon, C.byref(n), C.byref(md)))
-    return int(n.value), int(md.value)
-
-
-def _light_queue_uninitialized(fn, handle) -> int:
-    n = C.c_size_t(0)
-    _check(fn(handle, C.byref(n)))
-    return int(n.value)
-
-
-def _light_queue_region(fn, handle, lower, size, priority):
-    region = abi.Aab()
-    region.lower[:] = [int(v) for v in lower]
-    region.size[:] = [int(v) for v in size]
-    _check(fn(handle, C.byref(region), priority))
-
-
-def _light_download_queue(fn, handle, shape) -> np.ndarray:
-    out = np.zeros(shape, dtype=np.uint8)
-    _check(fn(handle, out.ctypes.data, out.size, None))
-    return out
-
-
-def _light_changes_count(count_fn, handle) -> int:
-    n = C.c_size_t(0)
-    _check(count_fn(handle, C.byref(n)))
-    return int(n.value)
-
-
-def _light_take_changes(count_fn, take_fn, handle, discard: bool):
-    indices = np.zeros(0, dtype=np.uint32)
-    texels = np.zeros((0, 4), dtype=np.uint8)
-    got = C.c_size_t(0)
-    if discard:
-        _check(take_fn(handle, None, None, 0, C.byref(got)))
-        return indices, texels
-    n = _light_changes_count(count_fn, handle)
-    if n:
-        indices = np.zeros(n, dtype=np.uint32)
-        texels = np.zeros((n, 4), dtype=np.uint8)
-        _check(take_fn(handle, indices.ctypes.data, texels.ctypes.data, n, C.byref(got)))
-    return indices, texels
 
 
 NO_WORLD_TO_SHOW_SRGB8 = (0xBC, 0xBC, 0xBC, 0xFF)   # content/palette.rs:76
@@ -1011,10 +985,21 @@ def print_space(space: "Space", direction, block_chars: dict, rt: "SpaceRaytrace
     return ["".join(special[v] if v < 0 else block_chars[int(v)] for v in out[r * 80:(r + 1) * 80]) for r in range(40)]
 
 
-class GroupScene:
+class GroupScene(_Scene):
     """A Space replicated on every device of a DeviceGroup (aicb_group_scene): what a SpaceRaytracer is to one context,
     kept current by the same updates, applied to every replica, and lit by the same light calls, whose rounds every
-    device shares."""
+    device shares.  Its methods are SpaceRaytracer's, with the same results:
+
+    - Every update and set_physics is validated against replica 0 first: a rejected call changes no replica.
+    - light_fast_evaluate, and a set_physics that reinitialises the light, run on device 0; the other replicas take
+      copies.  light_compute splits the cubes across the devices.  light_relight_blocks finds the cubes in every
+      replica's own cells.
+    - The light update queue and the set of changed cubes are device 0's, and the queue calls scan replica 0's volume;
+      every replica's texels are identical after every light call.
+    - light_stats: the counters of the last light call, summed over the devices; device seconds are device 0's (it
+      waits for every device in every round)."""
+
+    _prefix = "aicb_group_"
 
     def __init__(self, group: "DeviceGroup", space: "Space"):
         self.group = group
@@ -1024,110 +1009,11 @@ class GroupScene:
         _check(load_library().aicb_group_scene_create(group.handle, C.byref(desc), C.byref(self.handle)))
         del keep
 
-    def update_cubes(self, cubes: np.ndarray, block_ids: np.ndarray, light: Optional[np.ndarray] = None):
-        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
-        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
-        lt = None if light is None else np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
-        _check(load_library().aicb_group_scene_update_cubes(self.handle, c.ctypes.data, ids.ctypes.data,
-                                                            lt.ctypes.data if lt is not None else None, c.shape[0]))
-
-    def update_blocks(self, indices, blocks):
-        """SpaceChange::BlockEvaluation / BlockIndex on every replica; a rejected update changes none."""
-        idx = np.ascontiguousarray(indices, dtype=np.uint16)
-        arr = _block_descs(blocks)
-        _check(load_library().aicb_group_scene_update_blocks(self.handle, idx.ctypes.data, arr, len(blocks)))
-
-    def append_blocks(self, blocks):
-        """SpaceRaytracer.append_blocks on every replica; a rejected call changes none."""
-        arr = _block_descs(blocks)
-        _check(load_library().aicb_group_scene_append_blocks(self.handle, arr, len(blocks)))
-
-    def fill_uniform(self, block):
-        """SpaceRaytracer.fill_uniform on every replica; a rejected call changes none."""
-        arr = _block_descs([block])
-        _check(load_library().aicb_group_scene_fill_uniform(self.handle, arr))
-
-    def upload_light(self, light: np.ndarray):
-        lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
-        _check(load_library().aicb_group_scene_upload_light(self.handle, lt.ctypes.data, lt.shape[0]))
-
-    def set_physics(self, sky_colors, light_max_distance: int):
-        """SpaceRaytracer.set_physics on every replica; a reinitialisation is device 0's, copied to the others."""
-        _check(load_library().aicb_group_scene_set_physics(self.handle, C.byref(_sky(sky_colors)), light_max_distance))
-
-    # ---- light propagation on every device of the group (SpaceRaytracer's light_* methods, same results) ----
-    def light_fast_evaluate(self):
-        """LightStorage::fast_evaluate_light (updater.rs:537-582) on device 0, copied to every replica"""
-        _check(load_library().aicb_group_light_fast_evaluate(self.handle))
-
-    def light_compute(self, cubes: np.ndarray) -> np.ndarray:
-        """LightStorage::compute_light (updater.rs:368-418) for explicit cubes, split across the devices; returns
-        texels [n,4] in input order."""
-        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
-        out = np.zeros((c.shape[0], 4), dtype=np.uint8)
-        _check(load_library().aicb_group_light_compute(self.handle, c.ctypes.data, c.shape[0], out.ctypes.data))
-        return out
-
-    def light_evaluate(self, epsilon: int = 0):
-        """Mutation::evaluate_light (space.rs:1496-1527) -> (updates, max_difference, chart_node_visits)"""
-        n, md, nv = C.c_uint64(0), C.c_uint8(0), C.c_uint64(0)
-        _check(load_library().aicb_group_light_evaluate(self.handle, epsilon, C.byref(n), C.byref(md), C.byref(nv)))
-        return int(n.value), int(md.value), int(nv.value)
-
-    def light_edit_and_propagate(self, cubes: np.ndarray, block_ids: np.ndarray, epsilon: int = 0):
-        """Mutation::set x n + evaluate_light(epsilon) -> (updates, max_difference)"""
-        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
-        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
-        n, md = C.c_uint64(0), C.c_uint8(0)
-        _check(load_library().aicb_group_light_edit_and_propagate(self.handle, c.ctypes.data, ids.ctypes.data, c.shape[0],
-                                                                  epsilon, C.byref(n), C.byref(md)))
-        return int(n.value), int(md.value)
-
-    def light_relight_blocks(self, indices, epsilon: int = 0):
-        """SpaceRaytracer.light_relight_blocks on the group: every replica finds the cubes in its own cells; device 0
-        queues them -> (updates, max_difference)"""
-        return _light_relight_blocks(load_library().aicb_group_light_relight_blocks, self.handle, indices, epsilon)
-
-    def light_stats(self) -> dict:
-        """Counters of the last light call, summed over the devices; device seconds are device 0's (it waits for every
-        device in every round)."""
-        out = (C.c_uint64 * 4)()
-        _check(load_library().aicb_group_light_stats(self.handle, out))
-        return {"cube_updates": int(out[0]), "chart_node_visits": int(out[1]), "rounds": int(out[2]),
-                "device_seconds": int(out[3]) * 1e-6}
-
     def light_download(self, replica: int = 0) -> np.ndarray:
         """The light volume of one replica (they are identical after every light call)."""
         out = np.zeros(self.space.size + (4,), dtype=np.uint8)
         _check(load_library().aicb_group_light_download(self.handle, replica, out.ctypes.data, out.size // 4))
         return out
-
-    def light_queue_uninitialized(self) -> int:
-        """SpaceRaytracer.light_queue_uninitialized on the group: replica 0's volume, device 0's queue."""
-        return _light_queue_uninitialized(load_library().aicb_group_light_queue_uninitialized, self.handle)
-
-    def light_queue_region(self, lower, size, priority: int):
-        """SpaceRaytracer.light_queue_region on the group's queue (device 0's)."""
-        _light_queue_region(load_library().aicb_group_light_queue_region, self.handle, lower, size, priority)
-
-    def light_download_queue(self) -> np.ndarray:
-        """SpaceRaytracer.light_download_queue of the group's queue (device 0's)."""
-        return _light_download_queue(load_library().aicb_group_light_download_queue, self.handle, self.space.size)
-
-    def light_changes_count(self) -> int:
-        """SpaceRaytracer.light_changes_count of the group: the set is device 0's, and every replica's texels are
-        identical."""
-        return _light_changes_count(load_library().aicb_group_light_changes_count, self.handle)
-
-    def light_take_changes(self, discard: bool = False):
-        """SpaceRaytracer.light_take_changes of the group -> (indices uint32[n], texels uint8[n, 4])."""
-        return _light_take_changes(load_library().aicb_group_light_changes_count,
-                                   load_library().aicb_group_light_take_changes, self.handle, discard)
-
-    def close(self):
-        if self.handle:
-            load_library().aicb_group_scene_destroy(self.handle)
-            self.handle = C.c_void_p()
 
 
 class DeviceGroup:

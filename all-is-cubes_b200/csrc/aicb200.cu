@@ -1010,61 +1010,123 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
 // plus the new ones would not (brick_room), every replica's brick pool is compacted first and the definitions are
 // flattened again against the compacted table.  A compaction moves the pools, so each replica's context is waited
 // for first (wait_context).
-static aicb_status flatten_placeable(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks,
-                                     const uint16_t *indices, FlatBlocks *f) {
-    const BlockTable &t = s[0]->blocks;
+static aicb_status flatten_placeable(Replicas r, const aicb_block_desc *descs, size_t n_blocks, const uint16_t *indices,
+                                     FlatBlocks *f) {
+    const BlockTable &t = r.scene[0]->blocks;
     TRY(flatten_blocks(t, descs, n_blocks, indices, f));
     if (brick_room(t.n_bricks, t.dead_bricks, f->bricks.size()) != BrickRoom::compact_first) return AICB_OK;
-    for (size_t r = 0; r < n; r++) {
-        CU(cudaSetDevice(s[r]->ctx->device));
-        TRY(wait_context(s[r]->ctx));
-        Retired retired{s[r]->ctx, {}};
-        TRY(compact_pools(s[r], true, false, retired));
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.ctx[i]->device));
+        TRY(wait_context(r.ctx[i]));
+        Retired retired{r.ctx[i], {}};
+        TRY(compact_pools(r.scene[i], true, false, retired));
     }
     *f = FlatBlocks();
     return flatten_blocks(t, descs, n_blocks, indices, f);
 }
 
-aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t *indices, const aicb_block_desc *descs,
-                                 size_t n_blocks) {
+// One pinned staging buffer, one H2D copy and one scatter kernel per batch and replica, stream-ordered before any later
+// render of the context.  The batch is validated and built once: a cube named twice keeps its last value (the scatter
+// is parallel, so duplicates are resolved here).
+aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uint16_t *ids, const uint8_t (*light)[4],
+                                size_t n) {
+    if (n && (!cubes || !ids)) return fail(AICB_ERR_INVALID, "NULL argument");
+    CU(cudaSetDevice(r.ctx[0]->device));
+    if (n == 0) return AICB_OK;
+    const aicb_scene *s0 = r.scene[0];
+    const DeviceScene &ds = s0->ds;
+    // validate and build the whole batch before touching any state
+    std::vector<uint32_t> idx(n);
+    std::vector<CubeDelta> ops;
+    ops.reserve(n);
+    std::unordered_map<uint32_t, uint32_t> seen;
+    seen.reserve(n * 2);
+    for (size_t i = 0; i < n; i++) {
+        const uint32_t dx = (uint32_t)(cubes[i][0] - ds.lo[0]), dy = (uint32_t)(cubes[i][1] - ds.lo[1]),
+                       dz = (uint32_t)(cubes[i][2] - ds.lo[2]);
+        if (dx >= (uint32_t)ds.size[0] || dy >= (uint32_t)ds.size[1] || dz >= (uint32_t)ds.size[2])
+            return fail(AICB_ERR_INVALID, "cube out of bounds");
+        if (ids[i] >= s0->blocks.block_count()) return fail(AICB_ERR_INVALID, "block id out of range");
+        idx[i] = (uint32_t)(((size_t)dx * ds.size[1] + dy) * ds.size[2] + dz);
+        CubeDelta op;
+        op.idx = idx[i];
+        op.cell = cell_word(ids[i], s0->blocks.kind[ids[i]], ds.wide_cells);
+        op.has_light = (light && s0->d_light) ? 1u : 0u;
+        op.light = 0;
+        if (op.has_light) std::memcpy(&op.light, light[i], 4);
+        const auto [at, first] = seen.emplace(op.idx, (uint32_t)ops.size());
+        if (first) ops.push_back(op); else ops[at->second] = op;
+    }
+    const uint32_t m = (uint32_t)ops.size();
+    const size_t bytes = (size_t)m * sizeof(CubeDelta);
+    for (size_t k = 0; k < r.n; k++) {
+        aicb_scene *s = r.scene[k];
+        aicb_ctx *ctx = r.ctx[k];
+        cudaStream_t stream = ctx->stream.get();
+        CU(cudaSetDevice(ctx->device));
+        if (!s->h_ids.empty())
+            for (size_t i = 0; i < n; i++) s->h_ids[idx[i]] = ids[i];
+        if (std::min(ctx->h_delta.bytes(), ctx->d_delta.bytes()) < bytes) {
+            if (ctx->h_delta) cudaEventSynchronize(ctx->ev_delta.get());   // the previous batch's copy may still read it
+            ctx->h_delta.reset();
+            ctx->d_delta.reset();
+            const size_t cap = bytes < 65536 ? 65536 : bytes * 2;
+            TRY(ctx->h_delta.ensure(cap));
+            TRY(ctx->d_delta.ensure(cap));
+        }
+        CU(cudaEventSynchronize(ctx->ev_delta.get()));  // the previous batch has left the staging buffer
+        std::memcpy(ctx->h_delta.get(), ops.data(), bytes);
+        CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
+        scatter_cubes_kernel<<<(m + 127) / 128, 128, 0, stream>>>(ctx->d_delta.get<const CubeDelta>(), m, s->ds.wide_cells,
+                                                                  s->d_cells.get(), s->d_light.get<uint32_t>());
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(ctx->ev_delta.get(), stream));  // renders on other streams wait for it (launch_trace)
+    }
+    return AICB_OK;
+}
+
+aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks) {
+    if (n_blocks && (!indices || !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
     if (n_blocks == 0) return AICB_OK;
-    const BlockTable &t = s[0]->blocks;
+    aicb_scene *s0 = r.scene[0];
+    const BlockTable &t = s0->blocks;
     FlatBlocks f;
-    TRY(flatten_placeable(s, n, descs, n_blocks, indices, &f));
+    TRY(flatten_placeable(r, descs, n_blocks, indices, &f));
     // cubes that hold a block whose kind changes carry the new kind in their cell words
     std::vector<uint8_t> kind(t.kind);
     for (size_t i = 0; i < n_blocks; i++) kind[indices[i]] = f.kinds[i];
     std::vector<CubeDelta> ops;
     if (kind != t.kind) {
-        if (s[0]->h_ids.size() != s[0]->volume) return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
-        const bool wide = s[0]->ds.wide_cells;
+        if (s0->h_ids.size() != s0->volume) return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
+        const bool wide = s0->ds.wide_cells;
         uint32_t idx = 0;
-        for (const uint16_t id : s[0]->h_ids) {
+        for (const uint16_t id : s0->h_ids) {
             if (kind[id] != t.kind[id]) ops.push_back({idx, cell_word(id, kind[id], wide), 0, 0});
             idx++;
         }
     }
     bool compact_bricks = false, compact_palette = false;   // replica 0's decision, which every replica takes
-    for (size_t r = 0; r < n; r++) {
-        aicb_ctx *ctx = s[r]->ctx;
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_scene *sc = r.scene[i];
+        aicb_ctx *ctx = r.ctx[i];
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
         TRY(wait_context(ctx));   // the records are written over in place, and compaction moves the pools
         Retired retired{ctx, {}};
-        TRY(place(s[r], f, indices, retired));
-        if (r == 0) {
-            const BlockTable &t0 = s[0]->blocks;
+        TRY(place(sc, f, indices, retired));
+        if (i == 0) {
+            const BlockTable &t0 = s0->blocks;
             compact_bricks = t0.dead_bricks > t0.n_bricks - t0.dead_bricks;
             compact_palette = t0.dead_pal > t0.n_palette / 2 - t0.dead_pal;
         }
-        if (compact_bricks || compact_palette) TRY(compact_pools(s[r], compact_bricks, compact_palette, retired));
+        if (compact_bricks || compact_palette) TRY(compact_pools(sc, compact_bricks, compact_palette, retired));
         if (!ops.empty()) {
             DeviceBuffer d_ops;
             TRY(d_ops.ensure(ops.size() * sizeof(CubeDelta)));
             CU(cudaMemcpyAsync(d_ops.get(), ops.data(), ops.size() * sizeof(CubeDelta), cudaMemcpyHostToDevice, stream));
             scatter_cubes_kernel<<<(unsigned)((ops.size() + 127) / 128), 128, 0, stream>>>(
-                d_ops.get<const CubeDelta>(), (uint32_t)ops.size(), s[r]->ds.wide_cells, s[r]->d_cells.get(),
-                s[r]->d_light.get<uint32_t>());
+                d_ops.get<const CubeDelta>(), (uint32_t)ops.size(), sc->ds.wide_cells, sc->d_cells.get(),
+                sc->d_light.get<uint32_t>());
             retired.bufs.push_back(std::move(d_ops));
             CU(cudaGetLastError());
         }
@@ -1078,13 +1140,14 @@ aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t 
 // a frame issued later on another stream waits for them (launch_trace).  The new entries go to spare capacity that no
 // cell refers to until a later, stream-ordered cube update, so a frame in flight is not disturbed; an array that has to
 // move is freed only after it (Retired).
-aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks) {
+aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks) {
+    if (n_blocks && !descs) return fail(AICB_ERR_INVALID, "NULL argument");
     if (n_blocks == 0) return AICB_OK;
     FlatBlocks f;
-    TRY(flatten_placeable(s, n, descs, n_blocks, nullptr, &f));
-    for (size_t r = 0; r < n; r++) {
-        aicb_scene *sc = s[r];
-        aicb_ctx *ctx = sc->ctx;
+    TRY(flatten_placeable(r, descs, n_blocks, nullptr, &f));
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_scene *sc = r.scene[i];
+        aicb_ctx *ctx = r.ctx[i];
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
         Retired retired{ctx, {}};
@@ -1116,13 +1179,14 @@ aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_bloc
 // (u32 cells go back to u16: a one-block table fits them).  Light is not touched.  Each replica's context is waited for
 // first, since the table and the cells are replaced, and the call returns once its writes are done.  On each replica
 // the allocations come before any change, so a failure leaves that replica as it was.
-aicb_status scenes_fill_uniform(aicb_scene *const *s, size_t n, const aicb_block_desc *block) {
+aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block) {
+    if (!block) return fail(AICB_ERR_INVALID, "NULL argument");
     FlatBlocks f;
     TRY(flatten_blocks(BlockTable(), block, 1, nullptr, &f));
     const uint32_t word = cell_word(0, f.kinds[0], false);
-    for (size_t r = 0; r < n; r++) {
-        aicb_scene *sc = s[r];
-        aicb_ctx *ctx = sc->ctx;
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_scene *sc = r.scene[i];
+        aicb_ctx *ctx = r.ctx[i];
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
         TRY(wait_context(ctx));
@@ -1162,10 +1226,11 @@ aicb_status scenes_fill_uniform(aicb_scene *const *s, size_t n, const aicb_block
 // Space::set_physics (space.rs:609-630) on a scene's replicas: the sky tables once (Sky::for_blocks, Sky::mean), then, if
 // the sky or the LightPhysics differs, each replica's context is waited for (an issued frame may still read the light
 // volume a change to None frees) and light.cu applies the change.  The sky is read as aicb_scene_create reads it.
-aicb_status scenes_set_physics(LightReplicas r, const aicb_sky &sky, uint8_t light_max_distance) {
+aicb_status scenes_set_physics(Replicas r, const aicb_sky *sky, uint8_t light_max_distance) {
+    if (!sky) return fail(AICB_ERR_INVALID, "NULL argument");
     const DeviceScene &cur = r.scene[0]->ds;
     DeviceScene next = cur;
-    build_block_sky(sky, &next);
+    build_block_sky(*sky, &next);
     bool same_sky = next.sky_kind == cur.sky_kind;
     for (int k = 0; k < (next.sky_kind ? 8 : 1); k++)   // Uniform's colour, or the eight octants'
         for (int i = 0; i < 3; i++) same_sky = same_sky && next.sky_colors[k][i] == cur.sky_colors[k][i];
@@ -1177,6 +1242,29 @@ aicb_status scenes_set_physics(LightReplicas r, const aicb_sky &sky, uint8_t lig
     const aicb_status st = light_set_physics(r, next, light_max_distance);
     cudaSetDevice(r.ctx[0]->device);
     return st;
+}
+
+// Every replica takes the texels, ordered behind its queued cube updates; renders on other streams wait for ev_delta
+// (launch_trace).  A replica with no light volume gets one.
+aicb_status scenes_upload_light(Replicas r, const uint8_t (*light)[4], size_t n_texels) {
+    if (!light) return fail(AICB_ERR_INVALID, "NULL argument");
+    if (n_texels != r.scene[0]->volume) return fail(AICB_ERR_INVALID, "light volume size mismatch");
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_scene *s = r.scene[i];
+        cudaStream_t stream = r.ctx[i]->stream.get();
+        CU(cudaSetDevice(r.ctx[i]->device));
+        if (!s->d_light && s->volume) {
+            TRY(s->d_light.ensure(s->volume * 4));
+            s->device_bytes += s->volume * 4;
+            s->ds.light = s->d_light.get<uint32_t>();
+        }
+        if (s->volume) {
+            CU(cudaMemcpyAsync(s->d_light.get(), light, s->volume * 4, cudaMemcpyHostToDevice, stream));
+            CU(cudaEventRecord(r.ctx[i]->ev_delta.get(), stream));
+            CU(cudaStreamSynchronize(stream));
+        }
+    }
+    return AICB_OK;
 }
 
 
@@ -1266,63 +1354,12 @@ void aicb_scene_destroy(aicb_scene *s) {
 uint64_t aicb_scene_device_bytes(const aicb_scene *s) { return s ? s->device_bytes + s->blocks.bytes() : 0; }
 
 aicb_status aicb_scene_set_physics(aicb_scene *s, const aicb_sky *sky, uint8_t light_max_distance) {
-    if (!s || !sky) return fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return scenes_set_physics({&s, &s->ctx, 1}, *sky, light_max_distance);
+    return on_scene(s, [&](Replicas r) { return scenes_set_physics(r, sky, light_max_distance); });
 }
 
 aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *ids,
                                     const uint8_t (*light)[4], size_t n) {
-    if (!s || (n && (!cubes || !ids))) return fail(AICB_ERR_INVALID, "NULL argument");
-    aicb_ctx *ctx = s->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    if (n == 0) return AICB_OK;
-    const DeviceScene &ds = s->ds;
-    // validate everything before touching any state
-    for (size_t i = 0; i < n; i++) {
-        uint32_t dx = (uint32_t)(cubes[i][0] - ds.lo[0]), dy = (uint32_t)(cubes[i][1] - ds.lo[1]),
-                 dz = (uint32_t)(cubes[i][2] - ds.lo[2]);
-        if (dx >= (uint32_t)ds.size[0] || dy >= (uint32_t)ds.size[1] || dz >= (uint32_t)ds.size[2])
-            return fail(AICB_ERR_INVALID, "cube out of bounds");
-        if (ids[i] >= s->blocks.block_count()) return fail(AICB_ERR_INVALID, "block id out of range");
-    }
-    // one pinned staging buffer, one H2D copy, one scatter kernel per batch; a cube named twice keeps its
-    // last value (the scatter is parallel, so duplicates are resolved here)
-    const size_t need = n * sizeof(CubeDelta);
-    if (std::min(ctx->h_delta.bytes(), ctx->d_delta.bytes()) < need) {
-        if (ctx->h_delta) cudaEventSynchronize(ctx->ev_delta.get());   // the previous batch's copy may still read it
-        ctx->h_delta.reset();
-        ctx->d_delta.reset();
-        const size_t cap = need < 65536 ? 65536 : need * 2;
-        TRY(ctx->h_delta.ensure(cap));
-        TRY(ctx->d_delta.ensure(cap));
-    }
-    CU(cudaEventSynchronize(ctx->ev_delta.get()));  // the previous batch has left the staging buffer
-    CubeDelta *ops = ctx->h_delta.get<CubeDelta>();
-    std::unordered_map<uint32_t, uint32_t> seen;
-    seen.reserve(n * 2);
-    uint32_t m = 0;
-    for (size_t i = 0; i < n; i++) {
-        const uint32_t dx = (uint32_t)(cubes[i][0] - ds.lo[0]), dy = (uint32_t)(cubes[i][1] - ds.lo[1]),
-                       dz = (uint32_t)(cubes[i][2] - ds.lo[2]);
-        const size_t idx = ((size_t)dx * ds.size[1] + dy) * ds.size[2] + dz;
-        if (!s->h_ids.empty()) s->h_ids[idx] = ids[i];
-        CubeDelta op;
-        op.idx = (uint32_t)idx;
-        op.cell = cell_word(ids[i], s->blocks.kind[ids[i]], ds.wide_cells);
-        op.has_light = (light && s->d_light) ? 1u : 0u;
-        op.light = 0;
-        if (op.has_light) std::memcpy(&op.light, light[i], 4);
-        auto it = seen.find(op.idx);
-        if (it == seen.end()) { seen.emplace(op.idx, m); ops[m++] = op; } else { ops[it->second] = op; }
-    }
-    CU(cudaMemcpyAsync(ctx->d_delta.get(), ops, (size_t)m * sizeof(CubeDelta), cudaMemcpyHostToDevice, ctx->stream.get()));
-    scatter_cubes_kernel<<<(m + 127) / 128, 128, 0, ctx->stream.get()>>>(ctx->d_delta.get<const CubeDelta>(), m, ds.wide_cells,
-                                                                         s->d_cells.get(), s->d_light.get<uint32_t>());
-    CU(cudaGetLastError());
-    CU(cudaEventRecord(ctx->ev_delta.get(), ctx->stream.get()));  // renders on other streams wait for it (launch_trace)
-    return AICB_OK;  // stream-ordered before any later render of this context
+    return on_scene(s, [&](Replicas r) { return scenes_update_cubes(r, cubes, ids, light, n); });
 }
 
 // == SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; UpdatingSpaceRaytracer::update handles them in
@@ -1331,42 +1368,22 @@ aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], co
 // reclaimed by compaction (BlockTable); cubes that hold a block whose classification changed are re-encoded.
 // Does not touch light: aicb_light_relight_blocks with the same indices applies the light side of the change.
 aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
-    if (!s || (n && (!indices || !descs))) return fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return scenes_update_blocks(&s, 1, indices, descs, n);
+    return on_scene(s, [&](Replicas r) { return scenes_update_blocks(r, indices, descs, n); });
 }
 
 // == SpaceChange::BlockIndex for indices past the table (palette.rs:207-210; UpdatingSpaceRaytracer::update appends
 // TracingBlock::from_block of each, updating.rs:145-151): the blocks become the table's next indices.
 aicb_status aicb_scene_append_blocks(aicb_scene *s, const aicb_block_desc *descs, size_t n) {
-    if (!s || (n && !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return scenes_append_blocks(&s, 1, descs, n);
+    return on_scene(s, [&](Replicas r) { return scenes_append_blocks(r, descs, n); });
 }
 
 // == SpaceChange::EveryBlock (Mutation::fill_uniform over the whole bounds, space.rs:1461-1474).
 aicb_status aicb_scene_fill_uniform(aicb_scene *s, const aicb_block_desc *block) {
-    if (!s || !block) return fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return scenes_fill_uniform(&s, 1, block);
+    return on_scene(s, [&](Replicas r) { return scenes_fill_uniform(r, block); });
 }
 
 aicb_status aicb_scene_upload_light(aicb_scene *s, const uint8_t (*light)[4], size_t n_texels) {
-    if (!s || !light) return fail(AICB_ERR_INVALID, "NULL argument");
-    if (n_texels != s->volume) return fail(AICB_ERR_INVALID, "light volume size mismatch");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    CU(cudaSetDevice(s->ctx->device));
-    if (!s->d_light && s->volume) {
-        TRY(s->d_light.ensure(s->volume * 4));
-        s->device_bytes += s->volume * 4;
-        s->ds.light = s->d_light.get<uint32_t>();
-    }
-    if (s->volume) {   // ordered behind queued cube deltas; renders on other streams wait for ev_delta (launch_trace)
-        CU(cudaMemcpyAsync(s->d_light.get(), light, s->volume * 4, cudaMemcpyHostToDevice, s->ctx->stream.get()));
-        CU(cudaEventRecord(s->ctx->ev_delta.get(), s->ctx->stream.get()));
-        CU(cudaStreamSynchronize(s->ctx->stream.get()));
-    }
-    return AICB_OK;
+    return on_scene(s, [&](Replicas r) { return scenes_upload_light(r, light, n_texels); });
 }
 
 size_t aicb_shard_pixel_count(const aicb_camera *cam, const aicb_shard *shard) {

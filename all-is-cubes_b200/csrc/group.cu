@@ -232,11 +232,14 @@ static aicb_status ensure_light_peers(aicb_group *g) {
     return AICB_OK;
 }
 
-// The group's replicas for light.cu, after the group's locks are held and its peers are ready.
-static aicb_status light_replicas(aicb_group_scene *gs, LightReplicas *r) {
-    TRY(ensure_light_peers(gs->group));
-    *r = {gs->scene.data(), gs->group->ctx.data(), gs->scene.size()};
-    return AICB_OK;
+// The body of a group entry point: the handle checked, every context's lock held, with `peers` the light calls' peer
+// access ready, `call` run on the group scene's replicas.
+template <typename Call>
+static aicb_status on_group(const aicb_group_scene *gs, bool peers, Call call) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    ContextLocks lock(gs->group->ctx);
+    if (peers) TRY(ensure_light_peers(gs->group));
+    return call(Replicas{gs->scene.data(), gs->group->ctx.data(), gs->scene.size()});
 }
 
 extern "C" {
@@ -299,12 +302,7 @@ aicb_status aicb_group_scene_create(aicb_group *g, const aicb_scene_desc *d, aic
 
 aicb_status aicb_group_scene_update_cubes(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *ids,
                                           const uint8_t (*light)[4], size_t n) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    for (aicb_scene *s : gs->scene) {
-        aicb_status st = aicb_scene_update_cubes(s, cubes, ids, light, n);
-        if (st != AICB_OK) return st;
-    }
-    return AICB_OK;
+    return on_group(gs, false, [&](Replicas r) { return scenes_update_cubes(r, cubes, ids, light, n); });
 }
 
 aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt,
@@ -341,39 +339,28 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
 
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *gs, const uint16_t *indices, const aicb_block_desc *descs,
                                            size_t n) {
-    if (!gs || (n && (!indices || !descs))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    return scenes_update_blocks(gs->scene.data(), gs->scene.size(), indices, descs, n);
+    return on_group(gs, false, [&](Replicas r) { return scenes_update_blocks(r, indices, descs, n); });
 }
 
 aicb_status aicb_group_scene_append_blocks(aicb_group_scene *gs, const aicb_block_desc *descs, size_t n) {
-    if (!gs || (n && !descs)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    return scenes_append_blocks(gs->scene.data(), gs->scene.size(), descs, n);
+    return on_group(gs, false, [&](Replicas r) { return scenes_append_blocks(r, descs, n); });
 }
 
 aicb_status aicb_group_scene_fill_uniform(aicb_group_scene *gs, const aicb_block_desc *block) {
-    if (!gs || !block) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    return scenes_fill_uniform(gs->scene.data(), gs->scene.size(), block);
+    return on_group(gs, false, [&](Replicas r) { return scenes_fill_uniform(r, block); });
 }
 
 aicb_status aicb_group_scene_set_physics(aicb_group_scene *gs, const aicb_sky *sky, uint8_t light_max_distance) {
-    if (!gs || !sky) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    // a reinitialisation runs as aicb_group_light_fast_evaluate does, over the light calls' peers
-    if (light_max_distance && light_max_distance != gs->scene[0]->light_max_distance) TRY(ensure_light_peers(gs->group));
-    return scenes_set_physics({gs->scene.data(), gs->group->ctx.data(), gs->scene.size()}, *sky, light_max_distance);
+    return on_group(gs, false, [&](Replicas r) {
+        // a reinitialisation runs as aicb_group_light_fast_evaluate does, over the light calls' peers
+        if (light_max_distance && light_max_distance != r.scene[0]->light_max_distance)
+            TRY(ensure_light_peers(gs->group));
+        return scenes_set_physics(r, sky, light_max_distance);
+    });
 }
 
 aicb_status aicb_group_scene_upload_light(aicb_group_scene *gs, const uint8_t (*light)[4], size_t n_texels) {
-    if (!gs || !light) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n_texels != gs->scene[0]->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
-    for (aicb_scene *s : gs->scene) {
-        aicb_status st = aicb_scene_upload_light(s, light, n_texels);
-        if (st != AICB_OK) return st;
-    }
-    return AICB_OK;
+    return on_group(gs, false, [&](Replicas r) { return scenes_upload_light(r, light, n_texels); });
 }
 
 aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world, const aicb_group_layer *ui,
@@ -406,97 +393,73 @@ aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world, cons
 
 // ---- light propagation: the single-context calls' arguments, validation and results (light.cu) --------------------
 aicb_status aicb_group_light_fast_evaluate(aicb_group_scene *gs) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    LightReplicas r;
-    TRY(light_replicas(gs, &r));
-    return light_fast_evaluate(r);
+    return on_group(gs, true, [&](Replicas r) { return light_fast_evaluate(r); });
 }
 
 aicb_status aicb_group_light_compute(aicb_group_scene *gs, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    LightReplicas r;
-    TRY(light_replicas(gs, &r));
-    return light_compute(r, cubes, n, out);
+    return on_group(gs, true, [&](Replicas r) { return light_compute(r, cubes, n, out); });
 }
 
 aicb_status aicb_group_light_evaluate(aicb_group_scene *gs, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                       uint64_t *node_visits) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    LightReplicas r;
-    TRY(light_replicas(gs, &r));
-    return light_evaluate(r, epsilon, updates_done, max_diff, node_visits);
+    return on_group(gs, true, [&](Replicas r) {
+        return light_evaluate(r, epsilon, updates_done, max_diff, node_visits);
+    });
 }
 
 aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    LightReplicas r;
-    TRY(light_replicas(gs, &r));
-    return light_edit_and_propagate(r, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+    return on_group(gs, true, [&](Replicas r) {
+        return light_edit_and_propagate(r, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+    });
 }
 
 aicb_status aicb_group_light_relight_blocks(aicb_group_scene *gs, const uint16_t *indices, size_t n, uint8_t epsilon,
                                             uint64_t *updates_done, uint8_t *max_diff) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    LightReplicas r;
-    TRY(light_replicas(gs, &r));
-    return light_relight_blocks(r, indices, n, epsilon, updates_done, max_diff);
+    return on_group(gs, true, [&](Replicas r) {
+        return light_relight_blocks(r, indices, n, epsilon, updates_done, max_diff);
+    });
 }
 
 // The queue is device 0's and the scan reads replica 0's volume (the replicas' are identical).
 aicb_status aicb_group_light_queue_uninitialized(aicb_group_scene *gs, size_t *n_queued) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    LightReplicas r;
-    TRY(light_replicas(gs, &r));
-    return light_queue_uninitialized(r, n_queued);
+    return on_group(gs, true, [&](Replicas r) { return light_queue_uninitialized(r, n_queued); });
 }
 
 aicb_status aicb_group_light_queue_region(aicb_group_scene *gs, const aicb_aab *region, uint8_t priority) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    LightReplicas r;
-    TRY(light_replicas(gs, &r));
-    return light_queue_region(r, region, priority);
+    return on_group(gs, true, [&](Replicas r) { return light_queue_region(r, region, priority); });
 }
 
 aicb_status aicb_group_light_download_queue(aicb_group_scene *gs, uint8_t *priorities, size_t n_texels, size_t *n_queued) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    return light_download_queue(gs->scene[0], priorities, n_texels, n_queued);
+    return on_group(gs, false, [&](Replicas r) {
+        return light_download_queue(r.scene[0], priorities, n_texels, n_queued);
+    });
 }
 
 aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t (*out)[4], size_t n_texels) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (replica < 0 || (size_t)replica >= gs->scene.size()) return aicb_fail(AICB_ERR_INVALID, "no such replica");
-    ContextLocks lock(gs->group->ctx);
-    return light_download(gs->scene[replica], out, n_texels);
+    return on_group(gs, false, [&](Replicas r) {
+        if (replica < 0 || (size_t)replica >= r.n) return aicb_fail(AICB_ERR_INVALID, "no such replica");
+        return light_download(r.scene[replica], out, n_texels);
+    });
 }
 
 // The set of changed cubes is device 0's: device 0 applies every round and the push keeps the replicas identical, so its
 // indices and texels are every replica's.
 aicb_status aicb_group_light_changes_count(const aicb_group_scene *gs, size_t *n_changed) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    return light_changes_count(gs->scene[0], n_changed);
+    return on_group(gs, false, [&](Replicas r) { return light_changes_count(r.scene[0], n_changed); });
 }
 
 aicb_status aicb_group_light_take_changes(aicb_group_scene *gs, uint32_t *indices, uint8_t (*texels)[4], size_t capacity,
                                           size_t *n_taken) {
-    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    ContextLocks lock(gs->group->ctx);
-    return light_take_changes(gs->scene[0], indices, texels, capacity, n_taken);
+    return on_group(gs, false, [&](Replicas r) {
+        return light_take_changes(r.scene[0], indices, texels, capacity, n_taken);
+    });
 }
 
 aicb_status aicb_group_light_stats(const aicb_group_scene *gs, uint64_t out[4]) {
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    return aicb_light_stats(gs->scene[0], out);   // device 0's counters are the group's (light.cu)
+    return light_stats(gs->scene[0], out);   // device 0's counters are the group's (light.cu)
 }
 
 }  // extern "C"

@@ -353,14 +353,38 @@ struct ContextLocks {
     }
 };
 
-// aicb200.cu: creating a scene and changing its block table, on each of n contexts (a group scene's replicas hold
-// identical tables).  The block definitions are validated and flattened once, against replica 0's table, and a new
-// scene's cells are encoded once; only then does each replica place them on its own device.
+// A scene's replicas, one per listed context (ctx[i] is scene[i]'s context), device 0's first.  Every call that acts on
+// a scene runs once over them: the one-context entry points (on_scene) and the group's (group.cu) only check the handle,
+// take the locks and build the list.  The shared function validates its other arguments against replica 0 before
+// anything changes, so a rejected call changes no replica.
+struct Replicas {
+    aicb_scene *const *scene;
+    aicb_ctx *const *ctx;
+    size_t n;
+};
+
+// The body of a one-context entry point: the handle checked, the context's lock held, `call` run on the scene as a
+// list of one.
+template <typename Call>
+aicb_status on_scene(aicb_scene *s, Call call) {
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    return call(Replicas{&s, &s->ctx, 1});
+}
+
+// aicb200.cu: creating a scene and changing it, on each of n contexts (a group scene's replicas hold identical tables,
+// cells and light).  The block definitions are validated and flattened once, against replica 0's table, a new scene's
+// cells are encoded once and a batch of cubes is deduplicated once; only then does each replica place them on its own
+// device.
 aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out);
-aicb_status scenes_update_blocks(aicb_scene *const *s, size_t n, const uint16_t *indices, const aicb_block_desc *descs,
-                                 size_t n_blocks);
-aicb_status scenes_append_blocks(aicb_scene *const *s, size_t n, const aicb_block_desc *descs, size_t n_blocks);
-aicb_status scenes_fill_uniform(aicb_scene *const *s, size_t n, const aicb_block_desc *block);
+aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uint16_t *ids, const uint8_t (*light)[4],
+                                size_t n);
+aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks);
+aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks);
+aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block);
+aicb_status scenes_upload_light(Replicas r, const uint8_t (*light)[4], size_t n_texels);
+// Space::set_physics over the replicas.
+aicb_status scenes_set_physics(Replicas r, const aicb_sky *sky, uint8_t light_max_distance);
 
 // group.cu: the order between the listed contexts' streams: every other context's stream waits until device 0's has
 // reached this point (fan_out), or device 0's until every other one's has (fan_in, which leaves device 0 current).
@@ -382,33 +406,27 @@ aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size
 aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
                            uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info);
 
-// light.cu: the light calls over a scene's replicas (ctx[i] is scene[i]'s context).  They validate their arguments
-// other than the scenes against replica 0, before anything changes.  On a group, device 0 has peer access to every
-// other device and they to device 0, with native atomics.  After every call the replicas' light volumes are identical.
-struct LightReplicas {
-    aicb_scene *const *scene;
-    aicb_ctx *const *ctx;
-    size_t n;
-};
-// aicb200.cu: aicb_scene_set_physics / aicb_group_scene_set_physics over a scene's replicas (the caller holds the locks).
-aicb_status scenes_set_physics(LightReplicas r, const aicb_sky &sky, uint8_t light_max_distance);
-aicb_status light_fast_evaluate(LightReplicas r);
-aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]);
-aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
+// light.cu: the light calls over a scene's replicas.  On a group, device 0 has peer access to every other device and
+// they to device 0, with native atomics.  After every call the replicas' light volumes are identical.
+aicb_status light_fast_evaluate(Replicas r);
+aicb_status light_compute(Replicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]);
+aicb_status light_evaluate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                            uint64_t *node_visits);
-aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
+aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
-aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
+aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
                                  uint64_t *updates_done, uint8_t *max_diff);
 // Space::set_physics on the replicas' light side, once nothing on their contexts reads their arrays: `sky` holds the
 // new sky in a DeviceScene's sky fields, which every replica takes; `max_distance` is the new LightPhysics (0 = None).
-aicb_status light_set_physics(LightReplicas r, const aicb::DeviceScene &sky, uint32_t max_distance);
+aicb_status light_set_physics(Replicas r, const aicb::DeviceScene &sky, uint32_t max_distance);
 // The light update queue: the load rule of Space::new_from_builder and light_needs_update_in_region over replica 0's
 // volume and device 0's queue, and a copy of the queue's bytes.
-aicb_status light_queue_uninitialized(LightReplicas r, size_t *n_queued);
-aicb_status light_queue_region(LightReplicas r, const aicb_aab *region, uint8_t priority);
+aicb_status light_queue_uninitialized(Replicas r, size_t *n_queued);
+aicb_status light_queue_region(Replicas r, const aicb_aab *region, uint8_t priority);
 aicb_status light_download_queue(aicb_scene *s, uint8_t *priorities, size_t n_texels, size_t *n_queued);
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels);
 // The set of changed cubes of replica 0 (the other replicas' texels are identical); the caller holds the locks.
 aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed);
 aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity, size_t *n_taken);
+// The counters of replica 0's last light call, which are the group's.
+aicb_status light_stats(const aicb_scene *s, uint64_t out[4]);

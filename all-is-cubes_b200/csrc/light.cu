@@ -779,7 +779,7 @@ __global__ void __launch_bounds__(256) k_changes_emit(uint32_t *bits, uint32_t n
 
 // Replica i's parameters: its own field, blocks, chart, term slots and overflow list with its count; replica 0's queue,
 // round buffers, counters and sets (peer pointers on the other replicas).  Replica 0 takes both parts from itself.
-LightParams light_params(LightReplicas r, size_t i) {
+LightParams light_params(Replicas r, size_t i) {
     const aicb_scene *s = r.scene[i];
     const LightState::Own &own = s->light.own;
     const LightState::Shared &root = r.scene[0]->light.shared;
@@ -844,7 +844,7 @@ std::vector<float4> sky_terms(const uint32_t sky_faces[6]) {
 
 // Every replica's light state and, on a group, replica 0's push targets: the other replicas' light volumes.  A replica
 // that has no own part yet takes `terms` as its sky_term, or the scene's sky tabulated once for every such replica.
-aicb_status ensure_replicas(LightReplicas r, const std::vector<float4> *terms = nullptr) {
+aicb_status ensure_replicas(Replicas r, const std::vector<float4> *terms = nullptr) {
     std::vector<float4> tabulated;
     for (size_t i = 0; i < r.n; i++) {
         if (!terms && !r.scene[i]->light.own.sky_term) {
@@ -867,7 +867,7 @@ aicb_status ensure_replicas(LightReplicas r, const std::vector<float4> *terms = 
 // Every replica's walk of one form, replica i against its own field on its own context: the compute form (the round's
 // list, or the n `explicit_cubes`) with the lockstep walk of the overflow it met, or the mark form.  On a group the
 // walks start behind device 0's stream, and device 0's stream waits for them.
-aicb_status walk(LightReplicas r, const std::vector<LightParams> &RP, bool mark, uint32_t n = 0,
+aicb_status walk(Replicas r, const std::vector<LightParams> &RP, bool mark, uint32_t n = 0,
                  const int32_t *explicit_cubes = nullptr) {
     const bool group = r.n > 1;
     if (group) TRY(fan_out(r.ctx, r.n));
@@ -898,7 +898,7 @@ constexpr size_t ROUND_WALK_COUNTERS =
 // then walks a share of the changed cubes (mark form), raising priorities in device 0's queue.  Compute is Jacobi
 // within a round and marks merge by max, so a group performs one context's operations.  One context issues no event
 // and no push.
-aicb_status propagate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits) {
+aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits) {
     aicb_scene *s = r.scene[0];
     aicb_ctx *ctx = s->ctx;
     cudaStream_t st = ctx->stream.get();
@@ -1036,7 +1036,7 @@ aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas,
 // ---------------------------------------------------------------------------------------------
 // the light calls over a scene's replicas (internal.h): one context's entry points below, a group's in group.cu
 // ---------------------------------------------------------------------------------------------
-aicb_status light_fast_evaluate(LightReplicas r) {
+aicb_status light_fast_evaluate(Replicas r) {
     TRY(ensure_replicas(r));
     aicb_scene *s = r.scene[0];
     cudaStream_t stream = s->ctx->stream.get();
@@ -1053,7 +1053,7 @@ aicb_status light_fast_evaluate(LightReplicas r) {
 
 // The cubes are split across the replicas by device 0's work counter; every replica computes the overflow of its own
 // walks; the outputs are device 0's, in input order.
-aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
+aicb_status light_compute(Replicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
     aicb_scene *s = r.scene[0];
     if (n && (!cubes || !out)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
@@ -1084,7 +1084,7 @@ aicb_status light_compute(LightReplicas r, const int32_t (*cubes)[3], size_t n, 
     return AICB_OK;
 }
 
-aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
+aicb_status light_evaluate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                            uint64_t *node_visits) {
     TRY(ensure_replicas(r));
     return propagate(r, epsilon, updates_done, max_diff, node_visits);
@@ -1093,7 +1093,7 @@ aicb_status light_evaluate(LightReplicas r, uint8_t epsilon, uint64_t *updates_d
 // Mutation::set x n (space.rs:1346-1352 -> side_effects_of_set -> modified_cube_needs_update,
 // updater.rs:135-173) applied in order on the host mirror, then evaluate_light(epsilon).  Every replica takes the
 // mirror's, the cells' and the light's changes; only replica 0 holds the queue.
-aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
+aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
     if (n_edits && (!cubes || !new_ids)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     TRY(ensure_replicas(r));
@@ -1174,7 +1174,7 @@ aicb_status light_edit_and_propagate(LightReplicas r, const int32_t (*cubes)[3],
 // definition, then evaluate_light(epsilon).  The cubes are found on the device (k_relight_blocks), on every replica
 // against its own cells, ordered on each replica's stream behind the cube updates queued there; only replica 0 holds
 // the queue and the set of changed cubes.
-aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
+aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
                                  uint64_t *updates_done, uint8_t *max_diff) {
     if (n && !indices) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     aicb_scene *s = r.scene[0];
@@ -1214,7 +1214,7 @@ aicb_status light_relight_blocks(LightReplicas r, const uint16_t *indices, size_
 //   - None: every replica's light volume and state are freed (frames read PackedLight::ONE; the set goes with them).
 // The allocation comes first and is the only step that can fail for want of memory: a failure frees what it allocated
 // and leaves every replica as it was.
-aicb_status light_set_physics(LightReplicas r, const DeviceScene &sky, uint32_t max_distance) {
+aicb_status light_set_physics(Replicas r, const DeviceScene &sky, uint32_t max_distance) {
     aicb_scene *s0 = r.scene[0];
     const bool relight = max_distance != s0->light_max_distance;
     const bool new_faces = std::memcmp(sky.sky_faces, s0->ds.sky_faces, sizeof sky.sky_faces) != 0;
@@ -1289,7 +1289,7 @@ aicb_status light_set_physics(LightReplicas r, const DeviceScene &sky, uint32_t 
 
 // k_queue_cubes on replica 0 (its texels, its queue), behind the work queued on its context: the cube updates and
 // uploads whose texels the load rule reads.  *n_queued: the cubes selected.
-static aicb_status queue_cubes(LightReplicas r, bool uninit, const QueueBox &box, uint8_t priority, size_t *n_queued) {
+static aicb_status queue_cubes(Replicas r, bool uninit, const QueueBox &box, uint8_t priority, size_t *n_queued) {
     aicb_scene *s = r.scene[0];
     const LightParams P = light_params(r, 0);
     cudaStream_t st = s->ctx->stream.get();
@@ -1313,14 +1313,14 @@ static aicb_status queue_cubes(LightReplicas r, bool uninit, const QueueBox &box
 
 // Space::new_from_builder's load rule (space.rs:290-313): every cube of replica 0's volume whose texel is
 // Uninitialized enters the queue at Priority::UNINIT.  No texel is written and nothing propagates.
-aicb_status light_queue_uninitialized(LightReplicas r, size_t *n_queued) {
+aicb_status light_queue_uninitialized(Replicas r, size_t *n_queued) {
     TRY(ensure_replicas(r));
     return queue_cubes(r, true, QueueBox{}, PRIO_UNINIT, n_queued);
 }
 
 // LightStorage::light_needs_update_in_region (updater.rs:122-133): every cube of region ∩ bounds at `priority`.  Its
 // sweep branch (more than 400 cubes) queues the same cubes at the same priority.
-aicb_status light_queue_region(LightReplicas r, const aicb_aab *region, uint8_t priority) {
+aicb_status light_queue_region(Replicas r, const aicb_aab *region, uint8_t priority) {
     if (!region) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (priority == 0) return aicb_fail(AICB_ERR_INVALID, "priority 0 (Priority::MIN) never enters the queue");
     TRY(ensure_replicas(r));
@@ -1430,6 +1430,12 @@ aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texel
     return AICB_OK;
 }
 
+aicb_status light_stats(const aicb_scene *s, uint64_t out[4]) {
+    if (!out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    for (int i = 0; i < 4; i++) out[i] = s->light_stats[i];
+    return AICB_OK;
+}
+
 // ---------------------------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------------------------
@@ -1462,60 +1468,46 @@ uint32_t aicb_light_chart(float *weights, uint32_t *children) {
 }
 
 aicb_status aicb_light_fast_evaluate(aicb_scene *s) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_fast_evaluate({&s, &s->ctx, 1});
+    return on_scene(s, [&](Replicas r) { return light_fast_evaluate(r); });
 }
 
 aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_compute({&s, &s->ctx, 1}, cubes, n, out);
+    return on_scene(s, [&](Replicas r) { return light_compute(r, cubes, n, out); });
 }
 
 aicb_status aicb_light_evaluate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                 uint64_t *node_visits) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_evaluate({&s, &s->ctx, 1}, epsilon, updates_done, max_diff, node_visits);
+    return on_scene(s, [&](Replicas r) { return light_evaluate(r, epsilon, updates_done, max_diff, node_visits); });
 }
 
 aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                           uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_edit_and_propagate({&s, &s->ctx, 1}, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+    return on_scene(s, [&](Replicas r) {
+        return light_edit_and_propagate(r, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
+    });
 }
 
 aicb_status aicb_light_relight_blocks(aicb_scene *s, const uint16_t *indices, size_t n, uint8_t epsilon,
                                       uint64_t *updates_done, uint8_t *max_diff) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_relight_blocks({&s, &s->ctx, 1}, indices, n, epsilon, updates_done, max_diff);
+    return on_scene(s, [&](Replicas r) {
+        return light_relight_blocks(r, indices, n, epsilon, updates_done, max_diff);
+    });
 }
 
 aicb_status aicb_light_queue_uninitialized(aicb_scene *s, size_t *n_queued) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_queue_uninitialized({&s, &s->ctx, 1}, n_queued);
+    return on_scene(s, [&](Replicas r) { return light_queue_uninitialized(r, n_queued); });
 }
 
 aicb_status aicb_light_queue_region(aicb_scene *s, const aicb_aab *region, uint8_t priority) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_queue_region({&s, &s->ctx, 1}, region, priority);
+    return on_scene(s, [&](Replicas r) { return light_queue_region(r, region, priority); });
 }
 
 aicb_status aicb_light_download_queue(aicb_scene *s, uint8_t *priorities, size_t n_texels, size_t *n_queued) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_download_queue(s, priorities, n_texels, n_queued);
+    return on_scene(s, [&](Replicas r) { return light_download_queue(r.scene[0], priorities, n_texels, n_queued); });
 }
 
 aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_download(s, out, n_texels);
+    return on_scene(s, [&](Replicas r) { return light_download(r.scene[0], out, n_texels); });
 }
 
 aicb_status aicb_light_changes_count(const aicb_scene *s, size_t *n_changed) {
@@ -1526,14 +1518,11 @@ aicb_status aicb_light_changes_count(const aicb_scene *s, size_t *n_changed) {
 
 aicb_status aicb_light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity,
                                     size_t *n_taken) {
-    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    return light_take_changes(s, indices, texels, capacity, n_taken);
+    return on_scene(s, [&](Replicas r) { return light_take_changes(r.scene[0], indices, texels, capacity, n_taken); });
 }
 
 aicb_status aicb_light_stats(const aicb_scene *s, uint64_t out[4]) {
-    if (!s || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    for (int i = 0; i < 4; i++) out[i] = s->light_stats[i];
-    return AICB_OK;
+    if (!s) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    return light_stats(s, out);
 }
 }

@@ -421,7 +421,8 @@ aicb_status aicb_group_scene_update_cubes(aicb_group_scene *, const int32_t (*cu
 aicb_status aicb_group_render_srgb8(aicb_group_scene *, const aicb_camera *, const aicb_options *,
                                     uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
 /* aicb_scene_update_blocks (SpaceChange::BlockEvaluation / BlockIndex, updating.rs:128-150) and aicb_scene_upload_light
- * on every replica.  The update is validated against replica 0 first: a rejected call changes no replica.  Whether a
+ * on every replica.  These calls and aicb_group_scene_update_cubes hold every context of the group until they return.
+ * The update is validated against replica 0 first: a rejected call changes no replica.  Whether a
  * pool is compacted is decided from replica 0's table, and every replica compacts, so the tables stay identical.  The
  * update does not touch light: aicb_group_light_relight_blocks follows it.  A call that fails after validation, for want
  * of device memory on a replica other than the first (placing the definitions, or compacting a pool, there or in

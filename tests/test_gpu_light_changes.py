@@ -45,10 +45,7 @@ class Lit:
         return self.group.render_layers((self.scene, cam, opts)).data
 
     def abi_calls(self):
-        lib = aicb200.load_library()
-        if self.group is None:
-            return lib.aicb_light_changes_count, lib.aicb_light_take_changes, self.scene.handle
-        return lib.aicb_group_light_changes_count, lib.aicb_group_light_take_changes, self.scene.handle
+        return self.scene._fn("light_changes_count"), self.scene._fn("light_take_changes"), self.scene.handle
 
     def close(self):
         (self.scene if self.group is None else self.group).close()

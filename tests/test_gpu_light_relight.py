@@ -186,8 +186,7 @@ def test_rejected_relights_change_nothing(devices):
     opts = GraphicsOptions(lighting_display=aicb200.LIGHT_LINEAR)
     cam = scenes.standard_camera(space, opts, 64, 48)
     field, frame = lit.field(), lit.frame(cam, opts)
-    lib = aicb200.load_library()
-    fn = lib.aicb_light_relight_blocks if devices is None else lib.aicb_group_light_relight_blocks
+    fn = lit.scene._fn("light_relight_blocks")
     calls = [lambda: aicb200._check(fn(lit.scene.handle, None, 2, 0, None, None)),
              lambda: lit.light_relight_blocks([3, len(space.blocks)], 0),
              lambda: lit.light_relight_blocks([65535], 0)]

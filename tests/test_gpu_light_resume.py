@@ -24,10 +24,8 @@ OPTS = GraphicsOptions(lighting_display=aicb200.LIGHT_LINEAR, fog=aicb200.FOG_AB
 
 
 def abi_queue_calls(lit):
-    lib = aicb200.load_library()
-    p = "aicb_light" if lit.group is None else "aicb_group_light"
-    return (getattr(lib, p + "_queue_uninitialized"), getattr(lib, p + "_queue_region"),
-            getattr(lib, p + "_download_queue"))
+    return (lit.scene._fn("light_queue_uninitialized"), lit.scene._fn("light_queue_region"),
+            lit.scene._fn("light_download_queue"))
 
 
 def download_queue_counted(lit):

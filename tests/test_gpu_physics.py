@@ -209,8 +209,7 @@ def test_rejected_calls_change_nothing(devices):
     cam = scenes.standard_camera(space, OPTS, 64, 48)
     field, frames = lit.field(), outputs(lit, cam)
     bytes_before = lit.device_bytes if devices is None else None
-    lib = aicb200.load_library()
-    fn = lib.aicb_scene_set_physics if devices is None else lib.aicb_group_scene_set_physics
+    fn = lit.scene._fn("scene_set_physics")
     sky = aicb200._sky(UNIFORM_SKY)
     for handle, sky_arg in ((lit.scene.handle, None), (None, C.byref(sky))):
         for distance in (0, 6, 12):
