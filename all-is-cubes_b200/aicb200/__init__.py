@@ -128,6 +128,7 @@ def load_library() -> C.CDLL:
     u64, u8, size = C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_size_t)
     for name, argtypes in {
         "scene_update_cubes": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t],
+        "scene_update_region": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, C.c_void_p],
         "scene_update_blocks": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t],
         "scene_append_blocks": [C.c_void_p, C.c_void_p, C.c_size_t],
         "scene_fill_uniform": [C.c_void_p, C.c_void_p],
@@ -137,6 +138,7 @@ def load_library() -> C.CDLL:
         "light_compute": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
         "light_evaluate": [C.c_void_p, C.c_uint8, u64, u8, u64],
         "light_edit_and_propagate": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
+        "light_edit_region": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, size],
         "light_relight_blocks": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
         "light_stats": [C.c_void_p, u64],
         "light_queue_uninitialized": [C.c_void_p, size],
@@ -673,6 +675,29 @@ class _Scene:
         _check(self._fn("scene_update_cubes")(self.handle, c.ctypes.data, ids.ctypes.data,
                                               lt.ctypes.data if lt is not None else None, c.shape[0]))
 
+    @staticmethod
+    def _region(lower, size, block_ids):
+        """A box call's arguments: the region, the dense id array of shape `size` or None, and the uniform id."""
+        region = abi.Aab()
+        region.lower[:] = [int(v) for v in lower]
+        region.size[:] = [int(v) for v in size]
+        if np.ndim(block_ids) == 0:
+            return region, None, int(block_ids)
+        ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
+        if ids.shape != tuple(region.size):
+            raise ValueError(f"block_ids has shape {ids.shape}, the region {tuple(region.size)}")
+        return region, ids, 0
+
+    def update_region(self, lower, size, block_ids, light: Optional[np.ndarray] = None):
+        """SpaceChange::CubeBlock (and CubeLight) for every cube of the box (lower, size): update_cubes' box form.
+        block_ids: one id for every cube, or an array of shape `size`; light: texels of shape size + (4,), or None."""
+        region, ids, uniform = self._region(lower, size, block_ids)
+        lt = None if light is None else np.ascontiguousarray(light, dtype=np.uint8)
+        if lt is not None and lt.shape != tuple(region.size) + (4,):
+            raise ValueError(f"light has shape {lt.shape}, the region {tuple(region.size) + (4,)}")
+        _check(self._fn("scene_update_region")(self.handle, C.byref(region), None if ids is None else ids.ctypes.data,
+                                               uniform, None if lt is None else lt.ctypes.data))
+
     def update_blocks(self, indices, blocks):
         """SpaceChange::BlockEvaluation / BlockIndex: new definitions for existing block indices.  Light is not touched:
         light_relight_blocks(indices) follows it on a lit scene."""
@@ -728,6 +753,16 @@ class _Scene:
         _check(self._fn("light_edit_and_propagate")(self.handle, c.ctypes.data, ids.ctypes.data, c.shape[0], epsilon,
                                                     C.byref(n), C.byref(md)))
         return int(n.value), int(md.value)
+
+    def light_edit_region(self, lower, size, block_ids) -> int:
+        """Mutation::fill / fill_uniform over the box (lower, size): Mutation::set for every cube, without propagation
+        (light_evaluate follows).  block_ids: one id, or an array of shape `size` (a cube the fill leaves alone gets the
+        id it holds).  Returns the number of cubes whose block changed."""
+        region, ids, uniform = self._region(lower, size, block_ids)
+        n = C.c_size_t(0)
+        _check(self._fn("light_edit_region")(self.handle, C.byref(region), None if ids is None else ids.ctypes.data,
+                                             uniform, C.byref(n)))
+        return int(n.value)
 
     def light_relight_blocks(self, indices, epsilon: int = 0):
         """The light side of SpaceChange::BlockEvaluation: after update_blocks(indices, ...), Mutation::set's light rule

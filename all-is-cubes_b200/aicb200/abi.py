@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -128,6 +128,7 @@ EXPORTED_SYMBOLS = [
     "aicb_last_error",
     "aicb_scene_create",
     "aicb_scene_update_cubes",
+    "aicb_scene_update_region",
     "aicb_scene_update_blocks",
     "aicb_scene_append_blocks",
     "aicb_scene_fill_uniform",
@@ -168,6 +169,7 @@ EXPORTED_SYMBOLS = [
     "aicb_light_compute",
     "aicb_light_evaluate",
     "aicb_light_edit_and_propagate",
+    "aicb_light_edit_region",
     "aicb_light_relight_blocks",
     "aicb_light_download",
     "aicb_light_queue_uninitialized",
@@ -182,6 +184,7 @@ EXPORTED_SYMBOLS = [
     "aicb_group_scene_create",
     "aicb_group_scene_destroy",
     "aicb_group_scene_update_cubes",
+    "aicb_group_scene_update_region",
     "aicb_group_render_srgb8",
     "aicb_group_scene_update_blocks",
     "aicb_group_scene_upload_light",
@@ -195,6 +198,7 @@ EXPORTED_SYMBOLS = [
     "aicb_group_light_compute",
     "aicb_group_light_evaluate",
     "aicb_group_light_edit_and_propagate",
+    "aicb_group_light_edit_region",
     "aicb_group_light_relight_blocks",
     "aicb_group_light_download",
     "aicb_group_light_queue_uninitialized",

@@ -313,6 +313,117 @@ static __global__ void __launch_bounds__(256) fill_cells_kernel(uint16_t *__rest
     for (size_t i = n8 * 8 + first; i < n; i += stride) cells[i] = (uint16_t)word;
 }
 
+// One work item of a box update: a 16-byte-aligned chunk of PER elements of the scene's array, or the part of it that
+// one row of the box covers.  A box is size[0] x size[1] rows of size[2] consecutive elements (the arrays are Z-major);
+// a row touches at most `chunks_per_row` chunks, so item = row * chunks_per_row + k.  False: chunk k lies past the row.
+struct RowChunk {
+    uint32_t at;    // the first element's linear index in the scene
+    uint32_t pos;   // ... and its position in the box, Z-major (the index into the caller's dense arrays)
+    uint32_t n;     // elements: PER for a whole chunk, fewer at a row's unaligned head and tail
+};
+template <uint32_t PER>
+static __device__ __forceinline__ bool row_chunk(const DeviceScene &S, const RegionBox &box, uint32_t item,
+                                                 uint32_t chunks_per_row, RowChunk *c) {
+    const uint32_t row = item / chunks_per_row, k = item - row * chunks_per_row;
+    const uint32_t rx = row / box.size[1], ry = row - rx * box.size[1];
+    const uint32_t first = ((box.lo[0] + rx) * (uint32_t)S.size[1] + box.lo[1] + ry) * (uint32_t)S.size[2] + box.lo[2];
+    const uint32_t end = first + box.size[2], chunk = (first / PER + k) * PER;
+    if (chunk >= end) return false;
+    c->at = max(chunk, first);
+    c->n = min(chunk + PER, end) - c->at;
+    c->pos = row * box.size[2] + (c->at - first);
+    return true;
+}
+
+// The cells of a box (aicb_scene_update_region, aicb_light_edit_region): each gets cell_word(id, kind of id), the kind
+// from the block table's records on the device.  The ids are the caller's dense array (Z-major within the box), or with
+// UNIFORM one id.  A whole chunk is one 16-byte store (and one 16-byte load of the ids where their address allows it);
+// a row's head and tail are written one cell at a time.  MASK: the old cells are read first (one 16-byte load per whole
+// chunk), bit `pos` of `mask` (zeroed by the caller) is set for every cube whose block id changes, and the changed
+// cubes are counted into *n_changed if it is given.
+template <bool WIDE, bool UNIFORM, bool MASK>
+static __global__ void __launch_bounds__(256) k_region_cells(const DeviceScene S, const RegionBox box,
+                                                             const uint16_t *__restrict__ ids, uint32_t uniform_id,
+                                                             uint32_t chunks_per_row, uint32_t n_items,
+                                                             uint32_t *__restrict__ mask, uint32_t *n_changed) {
+    using Cell = typename std::conditional<WIDE, uint32_t, uint16_t>::type;
+    constexpr uint32_t PER = 16 / sizeof(Cell), KIND_SHIFT = WIDE ? 16 : 14, ID_MASK = WIDE ? 0xffffu : 0x3fffu;
+    Cell *cells = (Cell *)S.cells;
+    const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t changed = 0;
+    RowChunk c;
+    if (item < n_items && row_chunk<PER>(S, box, item, chunks_per_row, &c)) {
+        const bool whole = c.n == PER;
+        uint32_t id[PER], word[PER];
+        if (UNIFORM) {
+#pragma unroll
+            for (uint32_t k = 0; k < PER; k++) id[k] = uniform_id;
+        } else if (whole && ((uintptr_t)(ids + c.pos) & (2 * PER - 1)) == 0) {
+            __align__(16) uint32_t w[PER / 2];
+            if constexpr (WIDE) *(uint2 *)w = __ldg((const uint2 *)(ids + c.pos));
+            else *(uint4 *)w = __ldg((const uint4 *)(ids + c.pos));
+#pragma unroll
+            for (uint32_t k = 0; k < PER; k++) id[k] = (w[k / 2] >> (16 * (k & 1))) & 0xffffu;
+        } else {
+#pragma unroll
+            for (uint32_t k = 0; k < PER; k++) id[k] = k < c.n ? (uint32_t)__ldg(ids + c.pos + k) : 0u;
+        }
+        if (MASK) {
+            __align__(16) Cell old[PER];
+            if (whole) {
+                *(uint4 *)old = *(const uint4 *)(cells + c.at);
+            } else {
+#pragma unroll
+                for (uint32_t k = 0; k < PER; k++) old[k] = k < c.n ? cells[c.at + k] : (Cell)0;
+            }
+#pragma unroll
+            for (uint32_t k = 0; k < PER; k++) changed |= (k < c.n && ((uint32_t)old[k] & ID_MASK) != id[k] ? 1u : 0u) << k;
+        }
+        if (UNIFORM) {
+            const uint32_t w = uniform_id | (__ldg(&S.blocks[uniform_id].kind_res) & 0xffu) << KIND_SHIFT;
+#pragma unroll
+            for (uint32_t k = 0; k < PER; k++) word[k] = w;
+        } else {
+#pragma unroll
+            for (uint32_t k = 0; k < PER; k++) word[k] = id[k] | (__ldg(&S.blocks[id[k]].kind_res) & 0xffu) << KIND_SHIFT;
+        }
+        if (whole) {
+            uint4 v;
+            if constexpr (WIDE) v = make_uint4(word[0], word[1], word[2], word[3]);
+            else v = make_uint4(word[0] | word[1] << 16, word[2] | word[3] << 16, word[4] | word[5] << 16, word[6] | word[7] << 16);
+            *(uint4 *)(cells + c.at) = v;
+        } else {
+#pragma unroll
+            for (uint32_t k = 0; k < PER; k++)
+                if (k < c.n) cells[c.at + k] = (Cell)word[k];
+        }
+        if (MASK && changed) {
+            const uint32_t shift = c.pos & 31u;
+            atomicOr(mask + (c.pos >> 5), changed << shift);
+            if (shift + c.n > 32u) atomicOr(mask + (c.pos >> 5) + 1, changed >> (32u - shift));
+        }
+    }
+    if (MASK) {
+        const uint32_t total = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(changed));
+        if ((threadIdx.x & 31u) == 0 && total && n_changed) atomicAdd(n_changed, total);
+    }
+}
+
+// The texels of a box (aicb_scene_update_region's dense light): 4 texels per chunk, one 16-byte store per whole chunk
+// (and one 16-byte load where the caller's array allows it), a row's head and tail one texel at a time.
+static __global__ void __launch_bounds__(256) k_region_texels(const DeviceScene S, const RegionBox box,
+                                                              const uint32_t *__restrict__ texels, uint32_t chunks_per_row,
+                                                              uint32_t n_items, uint32_t *__restrict__ light) {
+    const uint32_t item = blockIdx.x * blockDim.x + threadIdx.x;
+    RowChunk c;
+    if (item >= n_items || !row_chunk<4>(S, box, item, chunks_per_row, &c)) return;
+    if (c.n == 4 && ((uintptr_t)(texels + c.pos) & 15u) == 0) {
+        *(uint4 *)(light + c.at) = __ldg((const uint4 *)(texels + c.pos));
+    } else {
+        for (uint32_t k = 0; k < c.n; k++) light[c.at + k] = __ldg(texels + c.pos + k);
+    }
+}
+
 // One run of a pool compaction (compact_pools): `bytes` bytes from byte `src` of the old pool to byte `dst` of the new
 // one.  Offsets and lengths are even (a u16 brick word is a pool's smallest element).
 struct PoolSegment {
@@ -1025,6 +1136,20 @@ static aicb_status flatten_placeable(Replicas r, const aicb_block_desc *descs, s
     return flatten_blocks(t, descs, n_blocks, indices, f);
 }
 
+// The context's staging (h_delta / d_delta) with room for a batch of `bytes`, once the previous batch has left it.
+static aicb_status delta_room(aicb_ctx *ctx, size_t bytes) {
+    if (std::min(ctx->h_delta.bytes(), ctx->d_delta.bytes()) < bytes) {
+        if (ctx->h_delta) cudaEventSynchronize(ctx->ev_delta.get());   // the previous batch's copy may still read it
+        ctx->h_delta.reset();
+        ctx->d_delta.reset();
+        const size_t cap = bytes < 65536 ? 65536 : bytes * 2;
+        TRY(ctx->h_delta.ensure(cap));
+        TRY(ctx->d_delta.ensure(cap));
+    }
+    CU(cudaEventSynchronize(ctx->ev_delta.get()));  // the previous batch has left the staging buffer
+    return AICB_OK;
+}
+
 // One pinned staging buffer, one H2D copy and one scatter kernel per batch and replica, stream-ordered before any later
 // render of the context.  The batch is validated and built once: a cube named twice keeps its last value (the scatter
 // is parallel, so duplicates are resolved here).
@@ -1066,21 +1191,101 @@ aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uin
         CU(cudaSetDevice(ctx->device));
         if (!s->h_ids.empty())
             for (size_t i = 0; i < n; i++) s->h_ids[idx[i]] = ids[i];
-        if (std::min(ctx->h_delta.bytes(), ctx->d_delta.bytes()) < bytes) {
-            if (ctx->h_delta) cudaEventSynchronize(ctx->ev_delta.get());   // the previous batch's copy may still read it
-            ctx->h_delta.reset();
-            ctx->d_delta.reset();
-            const size_t cap = bytes < 65536 ? 65536 : bytes * 2;
-            TRY(ctx->h_delta.ensure(cap));
-            TRY(ctx->d_delta.ensure(cap));
-        }
-        CU(cudaEventSynchronize(ctx->ev_delta.get()));  // the previous batch has left the staging buffer
+        TRY(delta_room(ctx, bytes));
         std::memcpy(ctx->h_delta.get(), ops.data(), bytes);
         CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
         scatter_cubes_kernel<<<(m + 127) / 128, 128, 0, stream>>>(ctx->d_delta.get<const CubeDelta>(), m, s->ds.wide_cells,
                                                                   s->d_cells.get(), s->d_light.get<uint32_t>());
         CU(cudaGetLastError());
         CU(cudaEventRecord(ctx->ev_delta.get(), stream));  // renders on other streams wait for it (launch_trace)
+    }
+    return AICB_OK;
+}
+
+aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                         RegionBox *box) {
+    if (!region) return fail(AICB_ERR_INVALID, "NULL argument");
+    for (int a = 0; a < 3; a++) {
+        const int64_t lo = (int64_t)region->lower[a] - s->ds.lo[a];
+        if (lo < 0 || lo + (int64_t)region->size[a] > (int64_t)s->ds.size[a])
+            return fail(AICB_ERR_INVALID, "region is not inside the bounds");
+        box->lo[a] = (uint32_t)lo;
+        box->size[a] = region->size[a];
+    }
+    // the kernels' work items, at most size[2] / 4 + 2 per row, are counted in 32 bits
+    if ((uint64_t)box->size[0] * box->size[1] * (box->size[2] / 4 + 2) > 0xffffffffull)
+        return fail(AICB_ERR_INVALID, "region too large");
+    const size_t count = s->blocks.block_count();
+    if (!ids) {
+        if (uniform_id >= count) return fail(AICB_ERR_INVALID, "block id out of range");
+        return AICB_OK;
+    }
+    uint16_t highest = 0;
+    for (size_t i = 0, n = box->volume(); i < n; i++) highest = std::max(highest, ids[i]);
+    if (box->volume() && highest >= count) return fail(AICB_ERR_INVALID, "block id out of range");
+    return AICB_OK;
+}
+
+aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *ids, uint16_t uniform_id,
+                         const uint8_t (*light)[4], uint32_t *d_mask, uint32_t *d_n_changed) {
+    aicb_ctx *ctx = s->ctx;
+    cudaStream_t stream = ctx->stream.get();
+    const size_t vol = box.volume(), rows = (size_t)box.size[0] * box.size[1], sz = box.size[2];
+    if (!s->h_ids.empty())
+        for (size_t row = 0; row < rows; row++) {
+            uint16_t *dst = s->h_ids.data() + ((size_t)(box.lo[0] + row / box.size[1]) * s->ds.size[1] + box.lo[1] +
+                                               row % box.size[1]) * s->ds.size[2] + box.lo[2];
+            if (ids) std::memcpy(dst, ids + row * sz, sz * 2);
+            else std::fill(dst, dst + sz, uniform_id);
+        }
+    if (!s->d_light) light = nullptr;
+    // the ids, then (16-byte aligned) the texels
+    const size_t id_bytes = ids ? (vol * 2 + 15) / 16 * 16 : 0, bytes = id_bytes + (light ? vol * 4 : 0);
+    if (bytes) {
+        TRY(delta_room(ctx, bytes));
+        if (ids) std::memcpy(ctx->h_delta.get(), ids, vol * 2);
+        if (light) std::memcpy(ctx->h_delta.get<char>() + id_bytes, light, vol * 4);
+        CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
+    }
+    if (d_mask) CU(cudaMemsetAsync(d_mask, 0, (vol + 31) / 32 * 4, stream));
+    const bool wide = s->ds.wide_cells;
+    const uint32_t per = wide ? 4u : 8u, chunks_per_row = (uint32_t)((sz + per - 1) / per + 1);
+    const uint32_t n_items = (uint32_t)(rows * chunks_per_row);
+    const uint16_t *d_ids = ids ? ctx->d_delta.get<const uint16_t>() : nullptr;
+    auto launch = [&](auto kernel) {
+        kernel<<<(n_items + 255) / 256, 256, 0, stream>>>(s->ds, box, d_ids, uniform_id, chunks_per_row, n_items, d_mask,
+                                                          d_n_changed);
+    };
+    switch ((wide ? 4 : 0) | (ids ? 0 : 2) | (d_mask ? 1 : 0)) {
+    case 0: launch(k_region_cells<false, false, false>); break;
+    case 1: launch(k_region_cells<false, false, true>); break;
+    case 2: launch(k_region_cells<false, true, false>); break;
+    case 3: launch(k_region_cells<false, true, true>); break;
+    case 4: launch(k_region_cells<true, false, false>); break;
+    case 5: launch(k_region_cells<true, false, true>); break;
+    case 6: launch(k_region_cells<true, true, false>); break;
+    default: launch(k_region_cells<true, true, true>); break;
+    }
+    if (light) {
+        const uint32_t cpr = (uint32_t)((sz + 3) / 4 + 1), n = (uint32_t)(rows * cpr);
+        k_region_texels<<<(n + 255) / 256, 256, 0, stream>>>(
+            s->ds, box, (const uint32_t *)(ctx->d_delta.get<const char>() + id_bytes), cpr, n, s->d_light.get<uint32_t>());
+    }
+    CU(cudaGetLastError());
+    return AICB_OK;
+}
+
+// The box form of scenes_update_cubes: nothing is built per cube on the host.  Every replica stages the caller's dense
+// arrays in its own context and writes its own cells and texels, stream-ordered like a cube update.
+aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                 const uint8_t (*light)[4]) {
+    RegionBox box;
+    TRY(check_region(r.scene[0], region, ids, uniform_id, &box));
+    if (box.volume() == 0) return AICB_OK;
+    for (size_t k = 0; k < r.n; k++) {
+        CU(cudaSetDevice(r.ctx[k]->device));
+        TRY(region_cells(r.scene[k], box, ids, uniform_id, light, nullptr, nullptr));
+        CU(cudaEventRecord(r.ctx[k]->ev_delta.get(), r.ctx[k]->stream.get()));  // renders on other streams wait for it
     }
     return AICB_OK;
 }
@@ -1360,6 +1565,11 @@ aicb_status aicb_scene_set_physics(aicb_scene *s, const aicb_sky *sky, uint8_t l
 aicb_status aicb_scene_update_cubes(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *ids,
                                     const uint8_t (*light)[4], size_t n) {
     return on_scene(s, [&](Replicas r) { return scenes_update_cubes(r, cubes, ids, light, n); });
+}
+
+aicb_status aicb_scene_update_region(aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                     const uint8_t (*light)[4]) {
+    return on_scene(s, [&](Replicas r) { return scenes_update_region(r, region, ids, uniform_id, light); });
 }
 
 // == SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; UpdatingSpaceRaytracer::update handles them in

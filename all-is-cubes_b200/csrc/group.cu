@@ -305,6 +305,11 @@ aicb_status aicb_group_scene_update_cubes(aicb_group_scene *gs, const int32_t (*
     return on_group(gs, false, [&](Replicas r) { return scenes_update_cubes(r, cubes, ids, light, n); });
 }
 
+aicb_status aicb_group_scene_update_region(aicb_group_scene *gs, const aicb_aab *region, const uint16_t *ids,
+                                           uint16_t uniform_id, const uint8_t (*light)[4]) {
+    return on_group(gs, false, [&](Replicas r) { return scenes_update_region(r, region, ids, uniform_id, light); });
+}
+
 aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt,
                                     uint8_t (*out)[4], size_t out_len, aicb_render_info *info) {
     if (!gs || !cam || !opt) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
@@ -420,6 +425,11 @@ aicb_status aicb_group_light_relight_blocks(aicb_group_scene *gs, const uint16_t
     return on_group(gs, true, [&](Replicas r) {
         return light_relight_blocks(r, indices, n, epsilon, updates_done, max_diff);
     });
+}
+
+aicb_status aicb_group_light_edit_region(aicb_group_scene *gs, const aicb_aab *region, const uint16_t *ids,
+                                         uint16_t uniform_id, size_t *n_changed) {
+    return on_group(gs, true, [&](Replicas r) { return light_edit_region(r, region, ids, uniform_id, n_changed); });
 }
 
 // The queue is device 0's and the scan reads replica 0's volume (the replicas' are identical).

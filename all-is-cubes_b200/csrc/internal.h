@@ -379,6 +379,26 @@ aicb_status on_scene(aicb_scene *s, Call call) {
 aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out);
 aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uint16_t *ids, const uint8_t (*light)[4],
                                 size_t n);
+// A box of cubes inside a scene's bounds: its lower corner as offsets from the scene's, and its size.
+struct RegionBox {
+    uint32_t lo[3], size[3];
+    size_t volume() const { return (size_t)size[0] * size[1] * size[2]; }
+};
+// The arguments of the box calls (aicb_scene_update_region, aicb_light_edit_region) against a scene: AICB_ERR_INVALID
+// for a NULL region, a region not inside the bounds, or an id (every entry of `ids`, or with ids == nullptr
+// `uniform_id`) past the table.
+aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                         RegionBox *box);
+// One replica's share of a box call, on its context's device and stream: the host mirror takes the ids row by row, the
+// ids (2 bytes per cube; none if uniform) and `light` (if given and the scene has a light volume) go through the
+// context's staging, and k_region_cells / k_region_texels write them.  With d_mask (ceil(volume / 32) words) the cubes
+// whose block id changes are marked there and counted into *d_n_changed (if given).  The caller records
+// aicb_ctx::ev_delta behind its last kernel.
+aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *ids, uint16_t uniform_id,
+                         const uint8_t (*light)[4], uint32_t *d_mask, uint32_t *d_n_changed);
+// SpaceChange::CubeBlock / CubeLight for every cube of a box.
+aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                 const uint8_t (*light)[4]);
 aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks);
 aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks);
 aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block);
@@ -416,6 +436,9 @@ aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], cons
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
 aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, uint8_t epsilon,
                                  uint64_t *updates_done, uint8_t *max_diff);
+// Mutation::fill / fill_uniform(region): Mutation::set for every cube of a box, without propagation.
+aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                              size_t *n_changed);
 // Space::set_physics on the replicas' light side, once nothing on their contexts reads their arrays: `sky` holds the
 // new sky in a DeviceScene's sky fields, which every replica takes; `max_distance` is the new LightPhysics (0 = None).
 aicb_status light_set_physics(Replicas r, const aicb::DeviceScene &sky, uint32_t max_distance);

@@ -561,14 +561,12 @@ __global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint
     else if (op.pending_op == 2) P.pending[op.idx] = PRIO_NEWLY_VISIBLE;
 }
 
-// modified_cube_needs_update (updater.rs:135-173) for a cube that holds block `id`, if `id` is one of the redefined
-// indices (`s_mask`, one bit per block index): k_edits' writes for that block, then the face neighbours whose own face
-// toward the cube is not opaque are queued.  Only `queue` (device 0 of a group) touches the queue and the set.
-// No two threads write one pending byte with different values: a cube opaque for light is opaque on every face, so no
-// neighbour queues it.
-__device__ __forceinline__ void relight_cube(const LightParams &P, const uint32_t *s_mask, uint32_t idx, uint32_t id,
-                                             uint32_t queue) {
-    if (!((s_mask[id >> 5] >> (id & 31u)) & 1u)) return;
+// modified_cube_needs_update (updater.rs:135-173) for a cube that holds block `id`: k_edits' writes for that block, then
+// the face neighbours whose own face toward the cube is not opaque are queued.  Only `queue` (device 0 of a group)
+// touches the queue and the set.  Threads may apply it to any set of cubes at once, reading the cells as they are after
+// every edit: no two threads write one pending byte with different values, since a cube opaque for light is opaque on
+// every face, so no neighbour queues it, and every other write stores NEWLY_VISIBLE.
+__device__ __forceinline__ void modified_cube(const LightParams &P, uint32_t idx, uint32_t id, uint32_t queue) {
     const uint32_t fl = __ldg(&P.blocks[id].flags);
     if ((fl & LB_ALL_OPAQUE) && !(fl & LB_EMISSIVE)) {   // opaque_for_light_computation
         const_cast<uint32_t *>(P.scene.light)[idx] = TX_OPAQUE;
@@ -588,6 +586,30 @@ __device__ __forceinline__ void relight_cube(const LightParams &P, const uint32_
         if (!cube_index(P.scene, x + (a == 0 ? s : 0), y + (a == 1 ? s : 0), z + (a == 2 ? s : 0), &nidx)) continue;
         if (!((__ldg(&P.blocks[block_id_at(P.scene, nidx)].flags) >> opp) & 1u)) P.pending[nidx] = PRIO_NEWLY_VISIBLE;
     }
+}
+
+// modified_cube for a cube that holds block `id`, if `id` is one of the redefined indices (`s_mask`, one bit per block
+// index).
+__device__ __forceinline__ void relight_cube(const LightParams &P, const uint32_t *s_mask, uint32_t idx, uint32_t id,
+                                             uint32_t queue) {
+    if ((s_mask[id >> 5] >> (id & 31u)) & 1u) modified_cube(P, idx, id, queue);
+}
+
+// The light rule of aicb_light_edit_region, after k_region_cells wrote the box's cells and marked in `mask` the cubes
+// whose block changed: modified_cube for each of those, one cube of the box per thread (consecutive threads take
+// consecutive cubes of a row, so their cell, flag and pending accesses coalesce).  Mutation::set applies the rule cube by
+// cube, each reading the neighbours' blocks of that moment; run against the final cells it leaves the same queue and
+// texels.  A changed cube ends OPAQUE and unqueued, or queued at NEWLY_VISIBLE, whatever its neighbours did.  An unchanged
+// or not yet edited neighbour shows the rule its final block; a neighbour edited later is queued by its own edit unless
+// it becomes opaque for light, and then it is opaque on every face, so the rule on its final block does not queue it.
+__global__ void __launch_bounds__(256) k_region_light(const LightParams P, const RegionBox box, const uint32_t *mask,
+                                                      uint32_t volume, uint32_t queue) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= volume || !((__ldg(mask + (p >> 5)) >> (p & 31u)) & 1u)) return;
+    const uint32_t row = p / box.size[2], rx = row / box.size[1], ry = row - rx * box.size[1];
+    const uint32_t idx = ((box.lo[0] + rx) * (uint32_t)P.scene.size[1] + box.lo[1] + ry) * (uint32_t)P.scene.size[2] +
+                         box.lo[2] + (p - row * box.size[2]);
+    modified_cube(P, idx, block_id_at(P.scene, idx), queue);
 }
 
 // The scan of aicb_light_relight_blocks: every cell of the scene, 16 bytes per load (8 u16 cells or 4 u32 cells,
@@ -1204,6 +1226,41 @@ aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, 
     return propagate(r, epsilon, updates_done, max_diff, nullptr);
 }
 
+// Mutation::fill / fill_uniform(region) (space.rs:1392-1412, 1455-1479): Mutation::set for every cube of the box.  On
+// every replica, behind the cube updates queued on its stream: the host mirror and the cells (region_cells), the changed
+// cubes marked in the replica's overflow list (a round buffer, empty between light calls: one bit per cube of the box),
+// then the light rule on the device (k_region_light).  Replica 0 alone counts the changed cubes and touches the queue
+// and the set.  Nothing propagates; the tile bounds are rebuilt from the pending bytes by the next propagation.
+aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                              size_t *n_changed) {
+    RegionBox box;
+    TRY(check_region(r.scene[0], region, ids, uniform_id, &box));
+    TRY(ensure_replicas(r));
+    if (n_changed) *n_changed = 0;
+    const size_t vol = box.volume();
+    if (vol == 0) return AICB_OK;
+    uint32_t edited = 0;
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_ctx *c = r.ctx[i];
+        cudaStream_t stream = c->stream.get();
+        CU(cudaSetDevice(c->device));
+        const LightParams P = light_params(r, i);
+        if (i == 0) CU(cudaMemsetAsync(&P.counters->edited, 0, 4, stream));
+        TRY(region_cells(r.scene[i], box, ids, uniform_id, nullptr, P.overflow, i == 0 ? &P.counters->edited : nullptr));
+        k_region_light<<<(unsigned)((vol + 255) / 256), 256, 0, stream>>>(P, box, P.overflow, (uint32_t)vol, i == 0);
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(c->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
+        if (i == 0) CU(cudaMemcpyAsync(&edited, &P.counters->edited, 4, cudaMemcpyDeviceToHost, stream));
+    }
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.ctx[i]->device));
+        CU(cudaStreamSynchronize(r.ctx[i]->stream.get()));
+    }
+    CU(cudaSetDevice(r.ctx[0]->device));
+    if (n_changed) *n_changed = edited;
+    return AICB_OK;
+}
+
 // LightStorage::maybe_reinitialize_for_physics_change (space/light/updater.rs:80-113):
 //   - the sky: every replica takes it, and a replica's sky_term is re-tabulated (once per call) where the BlockSky's
 //     faces changed.  Nothing else changes for the sky alone (the reference's "TODO: if only sky color is different").
@@ -1492,6 +1549,11 @@ aicb_status aicb_light_relight_blocks(aicb_scene *s, const uint16_t *indices, si
     return on_scene(s, [&](Replicas r) {
         return light_relight_blocks(r, indices, n, epsilon, updates_done, max_diff);
     });
+}
+
+aicb_status aicb_light_edit_region(aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                   size_t *n_changed) {
+    return on_scene(s, [&](Replicas r) { return light_edit_region(r, region, ids, uniform_id, n_changed); });
 }
 
 aicb_status aicb_light_queue_uninitialized(aicb_scene *s, size_t *n_queued) {

@@ -86,7 +86,8 @@ struct LightCounters {
     uint32_t mark_work;             // ... and by its mark form
     uint32_t overflow;              // entries of replica 0's overflow list
     uint32_t queued;                // cubes the last queue scan (k_queue_cubes) selected
-    uint32_t _pad[5];
+    uint32_t edited;                // cubes whose block the last box edit (k_region_cells) changed
+    uint32_t _pad[4];
 };
 static_assert(offsetof(LightCounters, gathered) == 0 && offsetof(LightCounters, priority) == 4 &&
               offsetof(LightCounters, max_diff) == 8 && offsetof(LightCounters, updates) == 12 &&

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 12 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 13 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -194,6 +194,9 @@ unsafe extern "C" {
 
     pub fn aicb_scene_create(ctx: *mut aicb_ctx, desc: *const aicb_scene_desc, out: *mut *mut aicb_scene) -> aicb_status;
     pub fn aicb_scene_update_cubes(s: *mut aicb_scene, cubes: *const [i32; 3], block_ids: *const u16, light: *const [u8; 4], n: usize) -> aicb_status;
+    // SpaceChange::CubeBlock / CubeLight for every cube of a box: dense Z-major arrays, or one id (block_ids NULL)
+    pub fn aicb_scene_update_region(s: *mut aicb_scene, region: *const aicb_aab, block_ids: *const u16, uniform_id: u16,
+                                    light: *const [u8; 4]) -> aicb_status;
     pub fn aicb_scene_update_blocks(s: *mut aicb_scene, indices: *const u16, descs: *const aicb_block_desc, n: usize) -> aicb_status;
     // SpaceChange::BlockIndex for indices past the table: the blocks become the table's next indices
     pub fn aicb_scene_append_blocks(s: *mut aicb_scene, descs: *const aicb_block_desc, n: usize) -> aicb_status;
@@ -252,6 +255,8 @@ unsafe extern "C" {
     pub fn aicb_group_scene_destroy(gs: *mut aicb_group_scene);
     pub fn aicb_group_scene_update_cubes(gs: *mut aicb_group_scene, cubes: *const [i32; 3], block_ids: *const u16,
                                          light: *const [u8; 4], n: usize) -> aicb_status;
+    pub fn aicb_group_scene_update_region(gs: *mut aicb_group_scene, region: *const aicb_aab, block_ids: *const u16,
+                                          uniform_id: u16, light: *const [u8; 4]) -> aicb_status;
     pub fn aicb_group_render_srgb8(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
                                    out: *mut [u8; 4], out_len: usize, info: *mut aicb_render_info) -> aicb_status;
     // every replica; validated against replica 0 first, so a rejected call changes none
@@ -299,6 +304,9 @@ unsafe extern "C" {
                                chart_node_visits: *mut u64) -> aicb_status;
     pub fn aicb_light_edit_and_propagate(s: *mut aicb_scene, cubes: *const [i32; 3], new_ids: *const u16, n_edits: usize,
                                          epsilon: u8, updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
+    // Mutation::fill / fill_uniform(region): Mutation::set for every cube of a box, without propagation
+    pub fn aicb_light_edit_region(s: *mut aicb_scene, region: *const aicb_aab, block_ids: *const u16, uniform_id: u16,
+                                  n_changed_or_null: *mut usize) -> aicb_status;
     pub fn aicb_light_relight_blocks(s: *mut aicb_scene, indices: *const u16, n: usize, epsilon: u8, updates_done: *mut u64,
                                      max_diff: *mut u8) -> aicb_status;
     pub fn aicb_light_download(s: *mut aicb_scene, out: *mut [u8; 4], n_texels: usize) -> aicb_status;
@@ -319,6 +327,8 @@ unsafe extern "C" {
     pub fn aicb_group_light_edit_and_propagate(gs: *mut aicb_group_scene, cubes: *const [i32; 3], new_ids: *const u16,
                                                n_edits: usize, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8)
                                                -> aicb_status;
+    pub fn aicb_group_light_edit_region(gs: *mut aicb_group_scene, region: *const aicb_aab, block_ids: *const u16,
+                                        uniform_id: u16, n_changed_or_null: *mut usize) -> aicb_status;
     pub fn aicb_group_light_relight_blocks(gs: *mut aicb_group_scene, indices: *const u16, n: usize, epsilon: u8,
                                            updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
     // the queue is device 0's; the scan reads replica 0's volume

@@ -28,7 +28,7 @@ use std::sync::{Arc, Mutex};
 use all_is_cubes::character::Cursor;
 use all_is_cubes::content::palette;
 use all_is_cubes::listen::{self, Listen as _};
-use all_is_cubes::math::{Cube, Rgba, ZeroOne};
+use all_is_cubes::math::{Cube, GridAab, Rgba, ZeroOne};
 use all_is_cubes::space::{self, Space, SpaceChange};
 use all_is_cubes::universe::{Handle, ReadTicket};
 use all_is_cubes::util::maybe_sync::BoxFuture;
@@ -176,6 +176,29 @@ impl SceneHandle {
         })
     }
 
+    fn update_region(self, region: &sys::aicb_aab, fill: RegionFill<'_>, light: Option<&[[u8; 4]]>) -> Result<(), B200Error> {
+        let (ids, uniform) = fill.as_ffi();
+        let light = light.map_or(core::ptr::null(), <[[u8; 4]]>::as_ptr);
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_scene_update_region(s, region, ids, uniform, light),
+                Self::Group(s) => sys::aicb_group_scene_update_region(s, region, ids, uniform, light),
+            }
+        })
+    }
+
+    fn light_edit_region(self, region: &sys::aicb_aab, fill: RegionFill<'_>) -> Result<usize, B200Error> {
+        let (ids, uniform) = fill.as_ffi();
+        let mut changed = 0usize;
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_light_edit_region(s, region, ids, uniform, &mut changed),
+                Self::Group(s) => sys::aicb_group_light_edit_region(s, region, ids, uniform, &mut changed),
+            }
+        })?;
+        Ok(changed)
+    }
+
     fn destroy(self) {
         match self {
             Self::Single(s) => unsafe { sys::aicb_scene_destroy(s) },
@@ -194,6 +217,27 @@ impl SceneHandle {
         match self {
             Self::Group(s) => s,
             Self::Single(_) => unreachable!("a single-context scene on a group renderer"),
+        }
+    }
+}
+
+/// What a box of cubes is filled with: one block index, or one per cube, Z-major within the box (`Vol`'s order).
+#[derive(Clone, Copy, Debug)]
+pub enum RegionFill<'a> {
+    Uniform(space::BlockIndex),
+    Each(&'a [space::BlockIndex]),
+}
+impl RegionFill<'_> {
+    fn as_ffi(self) -> (*const u16, u16) {
+        match self {
+            Self::Uniform(id) => (core::ptr::null(), id),
+            Self::Each(ids) => (ids.as_ptr(), 0),
+        }
+    }
+    fn fits(self, region: GridAab) -> bool {
+        match self {
+            Self::Uniform(_) => true,
+            Self::Each(ids) => ids.len() == region.volume().unwrap_or(usize::MAX),
         }
     }
 }
@@ -389,6 +433,33 @@ impl B200Renderer {
 
     fn with_backend(backend: Backend, cameras: StandardCameras) -> Self {
         Self { backend, cameras, layers: Layers { world: None, ui: None }, had_cursor: false }
+    }
+
+    /// The world layer's scene, once `update()` has created it.
+    fn world_scene(&self) -> Result<SceneHandle, B200Error> {
+        self.layers.world.as_ref().and_then(|f| f.scene).ok_or_else(|| B200Error {
+            status: sys::AICB_ERR_INVALID,
+            message: "no world scene yet: call update() first".into(),
+        })
+    }
+
+    /// For a host that fills a box of the world Space itself (`Space::fill`, `fill_uniform` over a region,
+    /// `SpaceTransaction::filling`) and sends the box instead of waiting for one `SpaceChange::CubeBlock` per cube:
+    /// the box's new block indices, and its light texels if given, Z-major within `region`
+    /// (`aicb_scene_update_region`).  The follower still applies the per-cube changes the Space announces, to the
+    /// same values.
+    pub fn update_world_region(&self, region: GridAab, fill: RegionFill<'_>, light: Option<&[[u8; 4]]>) -> Result<(), B200Error> {
+        assert!(fill.fits(region) && light.map_or(true, |l| l.len() == region.volume().unwrap_or(usize::MAX)),
+                "array length is not the region's volume");
+        self.world_scene()?.update_region(&convert::aab_of(region), fill, light)
+    }
+
+    /// The same fill on a world scene whose light the library computes: `Mutation::set`'s light rule for every cube of
+    /// `region` whose block changes, on the device (`aicb_light_edit_region`).  Returns the number of changed cubes;
+    /// nothing propagates until the host asks for it (`aicb_light_evaluate`).
+    pub fn light_edit_world_region(&self, region: GridAab, fill: RegionFill<'_>) -> Result<usize, B200Error> {
+        assert!(fill.fits(region), "array length is not the region's volume");
+        self.world_scene()?.light_edit_region(&convert::aab_of(region), fill)
     }
 
     /// Calls `single` with the layers this renderer holds as `aicb_layer`s, or on a group `group` with them as

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 12
+#define AICB_ABI_VERSION 13
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -199,6 +199,17 @@ aicb_status aicb_scene_create(aicb_ctx *, const aicb_scene_desc *, aicb_scene **
 /* SpaceChange::CubeBlock / CubeLight (space.rs:1062-1100): light may be NULL to leave light alone. */
 aicb_status aicb_scene_update_cubes(aicb_scene *, const int32_t (*cubes)[3], const uint16_t *block_ids,
                                     const uint8_t (*light)[4], size_t n);
+/* SpaceChange::CubeBlock (and CubeLight) for every cube of `region`: the box form of aicb_scene_update_cubes, for a host
+ * that filled a box (Space::fill, fill_uniform over a region, SpaceTransaction::filling).  block_ids: Z-major within
+ * `region` (as Vol and interior_iter order them: z fastest), one entry per cube; NULL: every cube takes `uniform_id`.
+ * light: Z-major within `region`, or NULL to leave the texels alone (ignored on a scene without a light volume, as
+ * aicb_scene_update_cubes ignores it).  Nothing is built per cube on the host: the arrays go to the device as they are
+ * (2 + 4 bytes per cube; a uniform fill uploads no ids) and the cells are encoded there, 16 bytes per store.  The light
+ * update queue and the set of changed cubes are not touched.  Queued on the context's stream and ordered like
+ * aicb_scene_update_cubes.  AICB_ERR_INVALID, with nothing changed: a NULL region, a region not inside the bounds, or an
+ * id past the block table.  A region of volume 0 does nothing.  GPU test: tests/test_gpu_region.py. */
+aicb_status aicb_scene_update_region(aicb_scene *, const aicb_aab *region, const uint16_t *block_ids_or_null,
+                                     uint16_t uniform_id, const uint8_t (*light_or_null)[4]);
 /* SpaceChange::BlockEvaluation / BlockIndex (space.rs:1062-1100; updating.rs:128-150): new definitions for EXISTING
  * block indices (an index beyond the table is rejected: aicb_scene_append_blocks adds new ones).  Voxel data is appended to the device pools, and the
  * replaced definitions' voxel data is reclaimed: once a pool's replaced part exceeds its live part, the call compacts
@@ -415,6 +426,10 @@ aicb_status aicb_group_scene_create(aicb_group *, const aicb_scene_desc *, aicb_
 void aicb_group_scene_destroy(aicb_group_scene *);
 aicb_status aicb_group_scene_update_cubes(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *block_ids,
                                           const uint8_t (*light)[4], size_t n);
+/* aicb_scene_update_region on every replica, holding every context of the group: validated against replica 0, then
+ * every replica stages the arrays in its own context and writes its own cells and texels. */
+aicb_status aicb_group_scene_update_region(aicb_group_scene *, const aicb_aab *region, const uint16_t *block_ids_or_null,
+                                           uint16_t uniform_id, const uint8_t (*light_or_null)[4]);
 /* == draw_rgba on the whole group: out_len must be fb_width * fb_height; the options apply as given (include_sky too).
  * The frame is issued on every device before any is waited for; a device whose hit stream overflowed is re-issued
  * alone.  The call holds every context of the group until it returns. */
@@ -544,6 +559,21 @@ aicb_status aicb_light_edit_and_propagate(aicb_scene *, const int32_t (*cubes)[3
 aicb_status aicb_light_relight_blocks(aicb_scene *, const uint16_t *indices, size_t n, uint8_t epsilon,
                                       uint64_t *updates_done, uint8_t *max_diff);
 aicb_status aicb_light_download(aicb_scene *, uint8_t (*out)[4], size_t n_texels);
+/* Mutation::fill / fill_uniform over a region smaller than the bounds (space.rs:1392-1412, 1455-1479) on a scene whose
+ * light the library computes: Mutation::set for every cube of `region` in interior_iter order.  The arguments are
+ * aicb_scene_update_region's; a cube the fill leaves alone is passed the id it already holds (Mutation::set of the same
+ * block changes nothing).  The cells and the host mirror take the ids, and every cube whose block changes gets
+ * Mutation::set's light rule (modified_cube_needs_update, space/light/updater.rs:135-173) as
+ * aicb_light_edit_and_propagate applies it: a block opaque for light stores OPAQUE, cancels the cube's queued update and
+ * puts the cube into the set of changed cubes; any other block queues the cube at Priority::NEWLY_VISIBLE; every
+ * in-bounds face neighbour whose own face toward the cube is not opaque is queued at NEWLY_VISIBLE.  The rule runs on
+ * the device against the box's final cells, which leaves the queue and the texels the cube-by-cube order leaves.
+ * Nothing propagates: aicb_light_evaluate follows when the host wants the light to move, as after
+ * aicb_light_queue_region.  *n_changed_or_null: the cubes whose block changed.  The call returns once its writes are
+ * done.  AICB_ERR_INVALID, with nothing changed: as aicb_scene_update_region, or LightPhysics::None.
+ * GPU test: tests/test_gpu_region.py. */
+aicb_status aicb_light_edit_region(aicb_scene *, const aicb_aab *region, const uint16_t *block_ids_or_null,
+                                   uint16_t uniform_id, size_t *n_changed_or_null);
 /* The light update queue across save and load.  The queue holds one priority per cube (0: not queued); an insert raises
  * a cube's priority and never lowers it (LightUpdateQueue::insert, space/light/queue.rs).  None of these calls writes a
  * texel, adds to the set of changed cubes or propagates: aicb_light_evaluate follows, as the reference's step does.
@@ -579,14 +609,15 @@ aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
  *   - aicb_light_edit_and_propagate sets it to a different block that is opaque for light, which stores OPAQUE even
  *     over OPAQUE (modified_cube_needs_update, space/light/updater.rs:153-161);
  *   - aicb_light_relight_blocks finds it holding a redefined block that is opaque for light (OPAQUE even over OPAQUE);
+ *   - aicb_light_edit_region sets it to a different block that is opaque for light;
  *   - a relaxation round stores a value with difference_priority > 0 (apply_light_update, updater.rs:313-317);
  *   - a round writes a guess into an Uninitialized neighbour (updater.rs:335-338);
  *   - aicb_light_fast_evaluate changes its texel.  The reference announces nothing there (fast_evaluate_light has a
  *     TODO for EveryBlock); a host following the light needs the cubes all the same;
  *   - aicb_scene_set_physics reinitialises the light (every cube).
- * Nothing else adds to it: not aicb_light_compute, aicb_scene_update_cubes, aicb_scene_upload_light (texels the host
- * supplied), frames, or a rejected call.  The set accumulates across calls until it is taken; a scene with no light
- * call yet has none.  LightPhysics::None is AICB_ERR_INVALID.
+ * Nothing else adds to it: not aicb_light_compute, aicb_scene_update_cubes, aicb_scene_update_region,
+ * aicb_scene_upload_light (texels the host supplied), frames, or a rejected call.  The set accumulates across calls until
+ * it is taken; a scene with no light call yet has none.  LightPhysics::None is AICB_ERR_INVALID.
  * aicb_light_take_changes with both outputs and capacity >= the set's size writes each cube once, as its Z-major
  * linear index (the index into aicb_scene_desc::block_ids and light), in increasing order, with its texel as it is now
  * (aicb_light_download's format), empties the set and sets *n_taken to its size.  With both outputs NULL it empties
@@ -621,6 +652,10 @@ aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *, const int32_
  * own cells and writes its own OPAQUE texels; device 0 alone queues and records the changed cubes. */
 aicb_status aicb_group_light_relight_blocks(aicb_group_scene *, const uint16_t *indices, size_t n, uint8_t epsilon,
                                             uint64_t *updates_done, uint8_t *max_diff);
+/* aicb_light_edit_region on the group: validated against replica 0; every replica writes its own cells and its own
+ * OPAQUE texels; device 0 alone counts the changed cubes, queues and records the set. */
+aicb_status aicb_group_light_edit_region(aicb_group_scene *, const aicb_aab *region, const uint16_t *block_ids_or_null,
+                                         uint16_t uniform_id, size_t *n_changed_or_null);
 /* The queue calls on the group: the queue is device 0's, and aicb_group_light_queue_uninitialized scans replica 0's
  * volume (the replicas' are identical).  Validation is against replica 0 before anything changes, and each call holds
  * every context of the group. */
