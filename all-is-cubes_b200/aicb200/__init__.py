@@ -27,6 +27,7 @@ from .abi import (FOG_ABRUPT, FOG_COMPROMISE, FOG_NONE, FOG_PHYSICAL, LIGHT_BOUN
 
 PKG_DIR = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB_PATH = os.environ.get("AICB200_LIB") or os.path.join(PKG_DIR, "libaicb200.so")  # override: kernel experiments only
+LIGHT_RAY_DTYPE = np.dtype(abi.LightRay)   # aicb_light_ray: one ray of light_compute_debug
 
 
 class AicbError(RuntimeError):
@@ -136,6 +137,8 @@ def load_library() -> C.CDLL:
         "scene_set_physics": [C.c_void_p, C.POINTER(abi.Sky), C.c_uint8],
         "light_fast_evaluate": [C.c_void_p],
         "light_compute": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
+        "light_compute_debug": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                size],
         "light_evaluate": [C.c_void_p, C.c_uint8, u64, u8, u64],
         "light_edit_and_propagate": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
         "light_edit_region": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, size],
@@ -738,6 +741,26 @@ class _Scene:
         out = np.zeros((c.shape[0], 4), dtype=np.uint8)
         _check(self._fn("light_compute")(self.handle, c.ctypes.data, c.shape[0], out.ctypes.data))
         return out
+
+    def light_compute_debug(self, cubes: np.ndarray):
+        """Space::compute_light::<LightUpdateCubeInfo> (space.rs:810, space/light/debug.rs) for explicit cubes ->
+        (texels [n,4] uint8, rays): light_compute's texels, and per cube an array of LIGHT_RAY_DTYPE (LightUpdateRayInfo:
+        trigger_cube, value_cube, value, light_from_struck_face) holding the rays that ended on a face opaque for light, in
+        the reference's order.  Nothing is stored."""
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        n = c.shape[0]
+        texels = np.zeros((n, 4), dtype=np.uint8)
+        counts = np.zeros(n, dtype=np.uint32)
+        rays = np.zeros(0, dtype=LIGHT_RAY_DTYPE)
+        total = C.c_size_t(0)
+        fn = self._fn("light_compute_debug")
+        status = fn(self.handle, c.ctypes.data, n, texels.ctypes.data, None, 0, counts.ctypes.data, C.byref(total))
+        if status == abi.ERR_INVALID and total.value > 0:   # the first call sized the rays
+            rays = np.zeros(total.value, dtype=LIGHT_RAY_DTYPE)
+            status = fn(self.handle, c.ctypes.data, n, texels.ctypes.data, rays.ctypes.data, rays.size,
+                        counts.ctypes.data, C.byref(total))
+        _check(status)
+        return texels, np.split(rays, np.cumsum(counts.astype(np.int64))[:-1]) if n else []
 
     def light_evaluate(self, epsilon: int = 0):
         """Mutation::evaluate_light (space.rs:1496-1527) -> (updates, max_difference, chart_node_visits)"""

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -103,6 +103,11 @@ class Hit(C.Structure):
     _fields_ = [("cube", C.c_int32 * 3), ("voxel", C.c_int32 * 3), ("resolution", C.c_int32), ("face", C.c_int32)]
 
 
+class LightRay(C.Structure):
+    _fields_ = [("trigger_cube", C.c_int32 * 3), ("value_cube", C.c_int32 * 3), ("value", C.c_uint8 * 4),
+                ("light_from_struck_face", C.c_float * 3), ("_pad", C.c_uint32)]
+
+
 # Every symbol include/aicb200.h declares (tests check the built library exports all of them).
 class Layer(C.Structure):
     _fields_ = [("scene", C.c_void_p), ("camera", C.POINTER(CameraData)), ("options", C.POINTER(Options))]
@@ -167,6 +172,7 @@ EXPORTED_SYMBOLS = [
     "aicb_light_chart_chains",
     "aicb_light_fast_evaluate",
     "aicb_light_compute",
+    "aicb_light_compute_debug",
     "aicb_light_evaluate",
     "aicb_light_edit_and_propagate",
     "aicb_light_edit_region",
@@ -196,6 +202,7 @@ EXPORTED_SYMBOLS = [
     "aicb_group_render_layers_terminal",
     "aicb_group_light_fast_evaluate",
     "aicb_group_light_compute",
+    "aicb_group_light_compute_debug",
     "aicb_group_light_evaluate",
     "aicb_group_light_edit_and_propagate",
     "aicb_group_light_edit_region",

@@ -405,6 +405,14 @@ aicb_status aicb_group_light_compute(aicb_group_scene *gs, const int32_t (*cubes
     return on_group(gs, true, [&](Replicas r) { return light_compute(r, cubes, n, out); });
 }
 
+aicb_status aicb_group_light_compute_debug(aicb_group_scene *gs, const int32_t (*cubes)[3], size_t n,
+                                           uint8_t (*out_texels)[4], aicb_light_ray *rays, size_t ray_capacity,
+                                           uint32_t *ray_counts, size_t *n_rays_total) {
+    return on_group(gs, true, [&](Replicas r) {
+        return light_compute_debug(r, cubes, n, out_texels, rays, ray_capacity, ray_counts, n_rays_total);
+    });
+}
+
 aicb_status aicb_group_light_evaluate(aicb_group_scene *gs, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                       uint64_t *node_visits) {
     return on_group(gs, true, [&](Replicas r) {

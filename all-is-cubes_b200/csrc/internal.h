@@ -430,6 +430,9 @@ aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, 
 // they to device 0, with native atomics.  After every call the replicas' light volumes are identical.
 aicb_status light_fast_evaluate(Replicas r);
 aicb_status light_compute(Replicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]);
+// compute_light::<LightUpdateCubeInfo>: light_compute's texels on replica 0 alone, with each cube's rays.
+aicb_status light_compute_debug(Replicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4], aicb_light_ray *rays,
+                                size_t capacity, uint32_t *ray_counts, size_t *n_rays_total);
 aicb_status light_evaluate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                            uint64_t *node_visits);
 aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,

@@ -331,8 +331,11 @@ __global__ void __launch_bounds__(256) k_gather(const LightParams P, uint32_t n_
 // cube, cubes handed out by a counter.  k_walk_chains<false> writes new_light for the round's list (or explicit
 // cubes); a cube one of whose chains needs more than LIGHT_CHAIN_K terms goes to the overflow list and is computed by
 // the lockstep walk (k_compute_overflow).  k_walk_chains<true> re-queues the dependencies of the entries of `changed`.
-template <bool MARK>
-__global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(const LightParams P, uint32_t n, const int32_t *explicit_cubes) {
+// RECORD (k_walk_chains_record): the compute form for explicit cubes that also logs every cube's rays and which cubes
+// overflowed.
+template <bool MARK, bool RECORD>
+__device__ __forceinline__ void walk_chains(const LightParams &P, uint32_t n, const int32_t *explicit_cubes,
+                                            const LightRayLog &log) {
     __shared__ float s_lut[256];
     __shared__ ChainShared s_sh[4];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lut[i] = P.scene.tables[i];
@@ -354,22 +357,34 @@ __global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(c
         const uint32_t prio = MARK ? (uint32_t)P.diff[i] / 2u + 1u : 0u;
         uint32_t visits = 0;
         bool overflowed = false;
-        const uint32_t nv = compute_light_chains<MARK>(P, s_lut, sh, terms, x, y, z, prio, &visits, &overflowed);
+        const uint32_t nv = compute_light_chains<MARK, RECORD>(P, s_lut, sh, terms, x, y, z, prio, &visits, &overflowed,
+                                                               log, i);
         if (!MARK && lane == 0) {
             if (overflowed) P.overflow[atomicAdd(P.overflow_count, 1u)] = i;
             else P.new_light[i] = nv;
+            if (RECORD) log.lockstep[i] = overflowed ? 1 : 0;
         }
         total_visits += visits;
     }
     if (!MARK && lane == 0 && total_visits) atomicAdd(&P.counters->node_visits, total_visits);
+}
+template <bool MARK>
+__global__ void __launch_bounds__(128, CHAIN_WALK_BLOCKS_PER_SM) k_walk_chains(const LightParams P, uint32_t n, const int32_t *explicit_cubes) {
+    walk_chains<MARK, false>(P, n, explicit_cubes, LightRayLog());
+}
+__global__ void __launch_bounds__(128) k_walk_chains_record(const LightParams P, uint32_t n, const int32_t *explicit_cubes,
+                                                            const LightRayLog log) {
+    walk_chains<false, true>(P, n, explicit_cubes, log);
 }
 
 // 8 CTAs of 4 warps per SM (64 registers; the records requested ahead spill to L1-resident local memory): the walk is
 // latency bound, so 32 resident warps serve it better than the 20 that 94 registers would allow.
 constexpr int LOCKSTEP_MIN_BLOCKS = 8;
 
-// the cubes the chain walk could not hold (*overflow_count entries of `overflow`), by the lockstep walk
-__global__ void __launch_bounds__(128, LOCKSTEP_MIN_BLOCKS) k_compute_overflow(const LightParams P, const int32_t *explicit_cubes) {
+// the cubes the chain walk could not hold (*overflow_count entries of `overflow`), by the lockstep walk; RECORD
+// (k_compute_overflow_record) also logs their rays
+template <bool RECORD>
+__device__ __forceinline__ void compute_overflow(const LightParams &P, const int32_t *explicit_cubes, const LightRayLog &log) {
     __shared__ float s_lut[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lut[i] = P.scene.tables[i];
     __syncthreads();
@@ -386,12 +401,19 @@ __global__ void __launch_bounds__(128, LOCKSTEP_MIN_BLOCKS) k_compute_overflow(c
             else cube_of(P.scene, P.list[i], x, y, z);
         }
         uint32_t visits = 0;
-        const uint32_t nv = compute_light_lockstep(P, s_lut, active, x, y, z, &visits);
+        const uint32_t nv = compute_light_lockstep<RECORD>(P, s_lut, active, x, y, z, &visits, log, i);
         if (active) P.new_light[i] = nv;
         total_visits += visits;
     }
     for (int off = 16; off > 0; off >>= 1) total_visits += __shfl_down_sync(0xffffffffu, total_visits, off);
     if (lane == 0 && total_visits) atomicAdd(&P.counters->node_visits, total_visits);
+}
+__global__ void __launch_bounds__(128, LOCKSTEP_MIN_BLOCKS) k_compute_overflow(const LightParams P, const int32_t *explicit_cubes) {
+    compute_overflow<false>(P, explicit_cubes, LightRayLog());
+}
+__global__ void __launch_bounds__(128) k_compute_overflow_record(const LightParams P, const int32_t *explicit_cubes,
+                                                                 const LightRayLog log) {
+    compute_overflow<true>(P, explicit_cubes, log);
 }
 
 // A texel of device 0's light volume was written: its 32-cube segment goes to the other replicas (k_push).
@@ -799,6 +821,45 @@ __global__ void __launch_bounds__(256) k_changes_emit(uint32_t *bits, uint32_t n
     }
 }
 
+// Packing the rays of aicb_light_compute_debug.  A cube's rays are the records of the walk that computed its texel:
+// the chain walk's, or the lockstep walk's where the chain walk overflowed.
+__device__ __forceinline__ bool ray_counts_for_its_cube(const LightRayRecord &r, const uint8_t *lockstep) {
+    return ((r.item & LIGHT_RAY_LOCKSTEP) != 0) == (lockstep[r.item & ~LIGHT_RAY_LOCKSTEP] != 0);
+}
+
+// 1. each cube's number of rays (k_changes_scan then turns the counts into each cube's first output position)
+__global__ void __launch_bounds__(256) k_rays_count(const LightRayRecord *recs, uint32_t n_recs, const uint8_t *lockstep,
+                                                    uint32_t *counts) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n_recs; j += gridDim.x * blockDim.x)
+        if (ray_counts_for_its_cube(recs[j], lockstep)) atomicAdd(counts + (recs[j].item & ~LIGHT_RAY_LOCKSTEP), 1u);
+}
+
+// 2. every counted record into its cube's range, in any order
+__global__ void __launch_bounds__(256) k_rays_place(const LightRayRecord *recs, uint32_t n_recs, const uint8_t *lockstep,
+                                                    const uint32_t *starts, uint32_t *fill, LightRayRecord *placed) {
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n_recs; j += gridDim.x * blockDim.x) {
+        const LightRayRecord r = recs[j];
+        if (!ray_counts_for_its_cube(r, lockstep)) continue;
+        const uint32_t c = r.item & ~LIGHT_RAY_LOCKSTEP;
+        placed[starts[c] + atomicAdd(fill + c, 1u)] = r;
+    }
+}
+
+// 3. one warp per cube: each ray goes to its rank by chart node within the cube's range (nodes are distinct per cube)
+__global__ void __launch_bounds__(256) k_rays_order(const LightRayRecord *placed, const uint32_t *starts, uint32_t n_cubes,
+                                                    aicb_light_ray *out) {
+    const uint32_t lane = threadIdx.x & 31;
+    for (uint32_t c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < n_cubes; c += (gridDim.x * blockDim.x) >> 5) {
+        const uint32_t s = starts[c], m = starts[c + 1] - s;
+        for (uint32_t j = lane; j < m; j += 32) {
+            const uint32_t node = placed[s + j].node;
+            uint32_t rank = 0;
+            for (uint32_t k = 0; k < m; k++) rank += placed[s + k].node < node ? 1u : 0u;
+            out[s + rank] = placed[s + j].ray;
+        }
+    }
+}
+
 // Replica i's parameters: its own field, blocks, chart, term slots and overflow list with its count; replica 0's queue,
 // round buffers, counters and sets (peer pointers on the other replicas).  Replica 0 takes both parts from itself.
 LightParams light_params(Replicas r, size_t i) {
@@ -1102,6 +1163,95 @@ aicb_status light_compute(Replicas r, const int32_t (*cubes)[3], size_t n, uint8
     s->light_stats[0] = n;
     s->light_stats[1] = h.node_visits;
     s->light_stats[2] = overflowed;   // cubes that took the lockstep walk (a chain with more terms than its slots)
+    s->light_stats[3] = 0;
+    return AICB_OK;
+}
+
+// Replica 0 walks every cube with the recording walks, then the rays are counted, scanned, placed and put in chart
+// order on the device.  The log starts with room for 256 rays a cube; a call that finds more runs the walks again with
+// room for all of them (the walks are deterministic).  Nothing is copied to the caller before the capacity check.
+aicb_status light_compute_debug(Replicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4], aicb_light_ray *rays,
+                                size_t capacity, uint32_t *ray_counts, size_t *n_rays_total) {
+    aicb_scene *s = r.scene[0];
+    if (!n_rays_total || (n && (!cubes || !out || !ray_counts))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
+    for (size_t i = 0; i < n; i++)
+        for (int a = 0; a < 3; a++)
+            if ((uint32_t)(cubes[i][a] - s->ds.lo[a]) >= (uint32_t)s->ds.size[a])
+                return aicb_fail(AICB_ERR_INVALID, "cube out of the Space's bounds");
+    TRY(ensure_replicas(r));
+    if (!rays) capacity = 0;
+    if (!n) {
+        *n_rays_total = 0;
+        return AICB_OK;
+    }
+    const Replicas r0{r.scene, r.ctx, 1};
+    const LightParams P = light_params(r0, 0);
+    aicb_ctx *ctx = s->ctx;
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream.get();
+    DeviceBuffer d_cubes, d_lockstep, d_count, d_recs;
+    TRY(d_cubes.upload(cubes, n * 12));
+    TRY(d_lockstep.ensure(n));
+    TRY(d_count.ensure(4));
+    uint32_t n_recs = (uint32_t)std::min<size_t>(n * 256, (size_t)1 << 22);
+    LightCounters h;
+    for (;;) {
+        TRY(d_recs.ensure((size_t)n_recs * sizeof(LightRayRecord)));
+        const LightRayLog log{d_recs.get<LightRayRecord>(), d_count.get<uint32_t>(), d_lockstep.get<uint8_t>(), n_recs};
+        CU(cudaMemsetAsync(P.counters, 0, sizeof(LightCounters), st));
+        CU(cudaMemsetAsync(log.count, 0, 4, st));
+        k_walk_chains_record<<<ctx->light_chart.walk_blocks, 128, 0, st>>>(P, (uint32_t)n, d_cubes.get<int32_t>(), log);
+        k_compute_overflow_record<<<ctx->num_sms * 8, 128, 0, st>>>(P, d_cubes.get<int32_t>(), log);
+        CU(cudaGetLastError());
+        uint32_t logged = 0;
+        CU(cudaMemcpyAsync(&logged, log.count, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(&h, P.counters, sizeof h, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (logged <= n_recs) {
+            n_recs = logged;
+            break;
+        }
+        n_recs = logged;
+    }
+    // k_changes_scan scans any array of counts: starts[c] = the first ray of cube c, starts[n] = the total
+    DeviceBuffer d_starts, d_fill;
+    TRY(d_starts.ensure((n + 1) * 4));
+    TRY(d_fill.ensure(n * 4));
+    CU(cudaMemsetAsync(d_starts.get(), 0, (n + 1) * 4, st));
+    const int wide = ctx->num_sms * 8;
+    const uint8_t *lockstep = d_lockstep.get<uint8_t>();
+    if (n_recs) k_rays_count<<<wide, 256, 0, st>>>(d_recs.get<LightRayRecord>(), n_recs, lockstep, d_starts.get<uint32_t>());
+    k_changes_scan<<<1, 1024, 0, st>>>(d_starts.get<uint32_t>(), (uint32_t)n);
+    CU(cudaGetLastError());
+    std::vector<uint32_t> starts(n + 1);
+    std::vector<uint32_t> texels(n);
+    CU(cudaMemcpyAsync(starts.data(), d_starts.get(), (n + 1) * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(texels.data(), P.new_light, n * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const size_t total = starts[n];
+    *n_rays_total = total;
+    if (capacity < total)
+        return aicb_fail(AICB_ERR_INVALID, "ray_capacity is smaller than the number of rays (*n_rays_total)");
+    if (total) {
+        DeviceBuffer d_placed, d_rays;
+        TRY(d_placed.ensure(total * sizeof(LightRayRecord)));
+        TRY(d_rays.ensure(total * sizeof(aicb_light_ray)));
+        CU(cudaMemsetAsync(d_fill.get(), 0, n * 4, st));
+        k_rays_place<<<wide, 256, 0, st>>>(d_recs.get<LightRayRecord>(), n_recs, lockstep, d_starts.get<uint32_t>(),
+                                           d_fill.get<uint32_t>(), d_placed.get<LightRayRecord>());
+        k_rays_order<<<wide, 256, 0, st>>>(d_placed.get<LightRayRecord>(), d_starts.get<uint32_t>(), (uint32_t)n,
+                                           d_rays.get<aicb_light_ray>());
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(rays, d_rays.get(), total * sizeof(aicb_light_ray), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+    }
+    std::memcpy(out, texels.data(), n * 4);
+    for (size_t i = 0; i < n; i++) ray_counts[i] = starts[i + 1] - starts[i];
+    // aicb_light_compute's counters: the walks' are the same on one context or a group
+    s->light_stats[0] = n;
+    s->light_stats[1] = h.node_visits;
+    s->light_stats[2] = h.overflow;
     s->light_stats[3] = 0;
     return AICB_OK;
 }
@@ -1530,6 +1680,14 @@ aicb_status aicb_light_fast_evaluate(aicb_scene *s) {
 
 aicb_status aicb_light_compute(aicb_scene *s, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
     return on_scene(s, [&](Replicas r) { return light_compute(r, cubes, n, out); });
+}
+
+aicb_status aicb_light_compute_debug(aicb_scene *s, const int32_t (*cubes)[3], size_t n, uint8_t (*out_texels)[4],
+                                     aicb_light_ray *rays, size_t ray_capacity, uint32_t *ray_counts,
+                                     size_t *n_rays_total) {
+    return on_scene(s, [&](Replicas r) {
+        return light_compute_debug(r, cubes, n, out_texels, rays, ray_capacity, ray_counts, n_rays_total);
+    });
 }
 
 aicb_status aicb_light_evaluate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,

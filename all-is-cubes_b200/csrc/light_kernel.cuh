@@ -126,6 +126,23 @@ struct LightParams {
     uint32_t epsilon_priority;
 };
 
+// compute_light::<LightUpdateCubeInfo>'s rays (aicb_light_compute_debug).  The recording walks append one record per
+// ray that ends on a face opaque for light (LightBuffer::traverse, updater.rs:838-853), tagged with the cube's position
+// in the call's list and the chart node it was struck at; light.cu then sorts each cube's records by node.  A walk
+// enters each node at most once per cube, so preorder is walk_ray_tree's depth-first order.
+constexpr uint32_t LIGHT_RAY_LOCKSTEP = 1u << 31;   // LightRayRecord::item: recorded by the lockstep walk
+struct LightRayRecord {
+    uint32_t item;          // position in the list | LIGHT_RAY_LOCKSTEP
+    uint32_t node;          // preorder index of the node whose cube was struck
+    aicb_light_ray ray;
+};
+struct LightRayLog {
+    LightRayRecord *recs;
+    uint32_t *count;        // records appended; those past `capacity` are counted, not stored
+    uint8_t *lockstep;      // per list position: 1 if the chain walk overflowed, so the lockstep walk's records count
+    uint32_t capacity;
+};
+
 #ifdef __CUDACC__
 
 namespace aicb_light {
@@ -215,6 +232,23 @@ struct Accum {
     float in0, in1, in2, total;
 };
 
+// LightUpdateRayInfo (debug.rs) of a ray that ended on the struck face of cube t, lit from cube v
+__device__ __forceinline__ void record_ray(const LightRayLog &log, uint32_t item, uint32_t node, int tx, int ty, int tz,
+                                           int vx, int vy, int vz, uint32_t stored, const float lf[3]) {
+    const uint32_t at = atomicAdd(log.count, 1u);
+    if (at >= log.capacity) return;
+    LightRayRecord &r = log.recs[at];
+    r.item = item;
+    r.node = node;
+    r.ray.trigger_cube[0] = tx; r.ray.trigger_cube[1] = ty; r.ray.trigger_cube[2] = tz;
+    r.ray.value_cube[0] = vx; r.ray.value_cube[1] = vy; r.ray.value_cube[2] = vz;
+#pragma unroll
+    for (int k = 0; k < 4; k++) r.ray.value[k] = (uint8_t)(stored >> (8 * k));
+#pragma unroll
+    for (int k = 0; k < 3; k++) r.ray.light_from_struck_face[k] = lf[k];
+    r.ray._pad = 0;
+}
+
 // end_of_ray (updater.rs:889-924) + add_weighted_light (:926-929).  The sky light a chart node's bundle collects —
 // sum over the six faces of sky_face * max(weight, 0), times 1 / sum(weights) — depends on the node and the sky
 // only; it is tabulated per scene (`sky`, see light.cu) and a lane only applies its own alpha and bundle weight.
@@ -235,8 +269,11 @@ __device__ __forceinline__ void end_of_ray(Accum &a, float alpha, float bundle, 
 // deepest live frame (-1: only the call of the root is pending; -2: the lane does not walk), and its frames (alpha
 // after traverse(), ray_bundle_weight, the children's weight so far, light_ahead_cache) indexed by depth — the depth is
 // warp-uniform, so these local-memory accesses are coalesced.
+// RECORD: the lane's rays go to `log` as list position `item` (recorded by the lockstep walk).
+template <bool RECORD = false>
 __device__ uint32_t compute_light_lockstep(const LightParams &P, const float *lut, bool active, int ox,
-                                           int oy, int oz, uint32_t *visits_out) {
+                                           int oy, int oz, uint32_t *visits_out, const LightRayLog &log = LightRayLog(),
+                                           uint32_t item = 0) {
     const DeviceScene &S = P.scene;
     Accum acc = {0.f, 0.f, 0.f, 0.f};
     uint32_t oidx;
@@ -378,6 +415,8 @@ __device__ uint32_t compute_light_lockstep(const LightParams &P, const float *lu
                                     acc.in0 = acc.in0 + ps_mul(ps_mul(lf[0], ka), kw);
                                     acc.in1 = acc.in1 + ps_mul(ps_mul(lf[1], ka), kw);
                                     acc.in2 = acc.in2 + ps_mul(ps_mul(lf[2], ka), kw);
+                                    if (RECORD && hit_opaque_face)
+                                        record_ray(log, item | LIGHT_RAY_LOCKSTEP, n, e_x, e_y, e_z, lx, ly, lz, stored, lf);
                                     if (hit_opaque_face) alpha = 0.0f; else alpha *= 1.0f - hit_alpha;
                                 }
                                 if (hit_alpha < 1.0f) {
@@ -476,11 +515,12 @@ struct ChainShared {
     uint8_t cnt_pop[LIGHT_MAX_CHAINS];
 };
 
-// returns the new PackedLight texel (every lane); *overflowed: some chain had more terms than its slots hold
-template <bool MARK>
+// returns the new PackedLight texel (every lane); *overflowed: some chain had more terms than its slots hold.
+// RECORD (compute form only): the cube's rays go to `log` as list position `item`, overflowed or not.
+template <bool MARK, bool RECORD = false>
 __device__ uint32_t compute_light_chains(const LightParams &P, const float *lut, ChainShared &sh, float4 *terms,
                                          int ox, int oy, int oz, uint32_t mark_priority, uint32_t *visits_out,
-                                         bool *overflowed) {
+                                         bool *overflowed, const LightRayLog &log = LightRayLog(), uint32_t item = 0) {
     const DeviceScene &S = P.scene;
     const unsigned lane = threadIdx.x & 31u;
     const unsigned lt_mask = (1u << lane) - 1u;
@@ -671,6 +711,7 @@ __device__ uint32_t compute_light_chains(const LightParams &P, const float *lut,
                                     terms[cur * LIGHT_CHAIN_SLOTS + tcount] = make_float4(ps_mul(ps_mul(lf[0], ka), kw), ps_mul(ps_mul(lf[1], ka), kw), ps_mul(ps_mul(lf[2], ka), kw), 0.0f);
                                 else over = true;
                                 tcount++;
+                                if (RECORD && hit_opaque_face) record_ray(log, item, node, e_x, e_y, e_z, lx, ly, lz, stored, lf);
                             }
                             if (hit_opaque_face) alpha = 0.0f; else alpha *= 1.0f - hit_alpha;
                         }

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 13 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 14 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -140,6 +140,17 @@ pub struct aicb_hit {
     pub voxel: [i32; 3],
     pub resolution: i32,
     pub face: i32,
+}
+
+/// one ray of `Space::compute_light::<LightUpdateCubeInfo>`: `LightUpdateRayInfo` (all-is-cubes/src/space/light/debug.rs)
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_light_ray {
+    pub trigger_cube: [i32; 3],
+    pub value_cube: [i32; 3],
+    pub value: [u8; 4],
+    pub light_from_struck_face: [f32; 3],
+    pub _pad: u32,
 }
 
 /// one pixel of the terminal's frame: `ColorCharacterBuf::output` (all-is-cubes-desktop/src/terminal.rs:355-366)
@@ -319,6 +330,10 @@ unsafe extern "C" {
     pub fn aicb_light_changes_count(s: *const aicb_scene, n_changed: *mut usize) -> aicb_status;
     pub fn aicb_light_take_changes(s: *mut aicb_scene, indices: *mut u32, texels: *mut [u8; 4], capacity: usize,
                                    n_taken: *mut usize) -> aicb_status;
+    // Space::compute_light::<LightUpdateCubeInfo>: aicb_light_compute's texels with each cube's rays
+    pub fn aicb_light_compute_debug(s: *mut aicb_scene, cubes: *const [i32; 3], n: usize, out_texels: *mut [u8; 4],
+                                    rays_or_null: *mut aicb_light_ray, ray_capacity: usize, ray_counts: *mut u32,
+                                    n_rays_total: *mut usize) -> aicb_status;
 
     pub fn aicb_group_light_fast_evaluate(gs: *mut aicb_group_scene) -> aicb_status;
     pub fn aicb_group_light_compute(gs: *mut aicb_group_scene, cubes: *const [i32; 3], n: usize, out: *mut [u8; 4]) -> aicb_status;
@@ -341,4 +356,7 @@ unsafe extern "C" {
     pub fn aicb_group_light_changes_count(gs: *const aicb_group_scene, n_changed: *mut usize) -> aicb_status;
     pub fn aicb_group_light_take_changes(gs: *mut aicb_group_scene, indices: *mut u32, texels: *mut [u8; 4],
                                          capacity: usize, n_taken: *mut usize) -> aicb_status;
+    pub fn aicb_group_light_compute_debug(gs: *mut aicb_group_scene, cubes: *const [i32; 3], n: usize,
+                                          out_texels: *mut [u8; 4], rays_or_null: *mut aicb_light_ray, ray_capacity: usize,
+                                          ray_counts: *mut u32, n_rays_total: *mut usize) -> aicb_status;
 }

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 13
+#define AICB_ABI_VERSION 14
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -628,6 +628,32 @@ aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
 aicb_status aicb_light_changes_count(const aicb_scene *, size_t *n_changed);
 aicb_status aicb_light_take_changes(aicb_scene *, uint32_t *indices_or_null, uint8_t (*texels_or_null)[4],
                                     size_t capacity, size_t *n_taken);
+/* One ray of Space::compute_light::<LightUpdateCubeInfo> (space/light/debug.rs: LightUpdateRayInfo): a ray that ended
+ * on a face opaque for light (LightBuffer::traverse, space/light/updater.rs:838-853).  trigger_cube is the cube struck,
+ * value_cube the cube the ray came from, whose stored light the face reflects; value is that stored light
+ * (PackedLight::as_texel, aicb_light_download's format); light_from_struck_face = the struck block's emission + its
+ * face colour (clamped) * value * the colour's alpha, in f32 as the reference computes it. */
+typedef struct aicb_light_ray {
+    int32_t trigger_cube[3];
+    int32_t value_cube[3];
+    uint8_t value[4];
+    float light_from_struck_face[3];
+    uint32_t _pad;
+} aicb_light_ray;
+/* Space::compute_light::<LightUpdateCubeInfo> (space.rs:810, space/light/debug.rs) for explicit cubes against the
+ * current field: aicb_light_compute with the rays that produced each result, for a host that draws them
+ * (GraphicsOptions::debug_light_rays_at_cursor).  out_texels[i] is what aicb_light_compute gives for cubes[i], and
+ * ray_counts[i] the number of its rays.  The rays of all cubes are packed cube after cube in list order, each cube's
+ * in the reference's order (walk_ray_tree's depth-first order); an opaque cube has none.  *n_rays_total is their sum.
+ * Nothing is stored: the light volume, the queue and the set of changed cubes stay as they are, and aicb_light_stats
+ * reads as after aicb_light_compute on the same cubes.
+ * AICB_ERR_INVALID, with nothing written but *n_rays_total: ray_capacity < the total (*n_rays_total = the total; a
+ * NULL `rays` counts as capacity 0, so a first call with NULL sizes the buffer).  AICB_ERR_INVALID with nothing
+ * written: NULL cubes, out_texels or ray_counts with n > 0, NULL n_rays_total, n > the volume, a cube out of bounds,
+ * or LightPhysics::None.  GPU test: tests/test_gpu_light_debug.py. */
+aicb_status aicb_light_compute_debug(aicb_scene *, const int32_t (*cubes)[3], size_t n, uint8_t (*out_texels)[4],
+                                     aicb_light_ray *rays_or_null, size_t ray_capacity, uint32_t *ray_counts,
+                                     size_t *n_rays_total);
 
 /* The light calls above on a device group (csrc/group.cu, csrc/light.cu), with their arguments, validation, errors and
  * results: LightStorage::fast_evaluate_light / compute_light / Mutation::set x n + evaluate_light
@@ -674,6 +700,11 @@ aicb_status aicb_group_light_stats(const aicb_group_scene *, uint64_t out[4]);
 aicb_status aicb_group_light_changes_count(const aicb_group_scene *, size_t *n_changed);
 aicb_status aicb_group_light_take_changes(aicb_group_scene *, uint32_t *indices_or_null, uint8_t (*texels_or_null)[4],
                                           size_t capacity, size_t *n_taken);
+/* aicb_light_compute_debug on the group: replica 0 walks every cube against its own field (the replicas' are
+ * identical), with the same arguments, results and errors. */
+aicb_status aicb_group_light_compute_debug(aicb_group_scene *, const int32_t (*cubes)[3], size_t n,
+                                           uint8_t (*out_texels)[4], aicb_light_ray *rays_or_null, size_t ray_capacity,
+                                           uint32_t *ray_counts, size_t *n_rays_total);
 
 #ifdef __cplusplus
 }

@@ -10,6 +10,9 @@
 // rule, without Mutation::set's same-block skip, to every cube that holds a redefined block, in increasing linear index
 // order.
 //
+// orc_light_compute_debug is Space::compute_light::<LightUpdateCubeInfo>: compute_light with the rays that ended on a
+// face opaque for light, recorded where the reference records them (space/light/debug.rs, updater.rs:838-853).
+//
 // Build: g++ -O2 -std=c++17 -ffp-contract=off -fno-fast-math (Rust never contracts to FMA).
 #include "../oracle/aic_oracle.cpp"
 #include "../oracle/aic_light.cpp"
@@ -50,6 +53,117 @@ static void modified_cube_needs_update(orc_light &L, size_t idx) {
         const int opp = (f < 3) ? f + 3 : f - 3;
         if (!get_evaluated(L, nc).opaque[opp]) light_needs_update(L, nc, PRIO_NEWLY_VISIBLE);
     }
+}
+
+// ---- Space::compute_light::<LightUpdateCubeInfo> (space.rs:810, space/light/debug.rs) ------------------------------
+// The preorder index of every node of the chart: walk_ray_tree's depth-first order, children NX..PZ (updater.rs:500).
+static const std::vector<uint32_t> &preorder_of() {
+    static const std::vector<uint32_t> pre = [] {
+        const std::vector<FlatNode> &ch = chart();
+        std::vector<uint32_t> p(ch.size(), 0);
+        std::vector<uint32_t> stack{0};
+        uint32_t next = 0;
+        while (!stack.empty()) {
+            const uint32_t i = stack.back();
+            stack.pop_back();
+            p[i] = next++;
+            for (int f = 5; f >= 0; f--)
+                if (ch[i].children[f]) stack.push_back(ch[i].children[f]);
+        }
+        return p;
+    }();
+    return pre;
+}
+
+struct RayRecord {
+    uint32_t node;   // preorder index of the node whose cube was struck
+    aicb_light_ray ray;
+};
+
+// walk_ray_tree (updater.rs:427-529), as walk() in ../oracle/aic_light.cpp, with D = LightUpdateCubeInfo: after
+// LightBuffer::traverse, a ray that ended on a face opaque for light is pushed as traverse pushes it (updater.rs:816-853:
+// a face other than Within, opaque, with alpha > 0).
+static float walk_debug(orc_light &L, LightBuffer &b, std::vector<RayRecord> &rays, const int32_t origin[3],
+                        const int32_t cube[3], int face7, uint32_t node_index, bool have_prev, PL prev, RayState rs) {
+    const FlatNode &node = chart()[node_index];
+    b.visits++;
+    float prod[6];
+    for (int f = 0; f < 6; f++) prod[f] = node.weight[f] * rs.dw[f];
+    const float bundle = fm_sum(prod);
+    if (bundle <= 0.0f) return bundle;
+    const double dx = ((double)cube[0] + 0.5) - ((double)origin[0] + 0.5),
+                 dy = ((double)cube[1] + 0.5) - ((double)origin[1] + 0.5),
+                 dz = ((double)cube[2] + 0.5) - ((double)origin[2] + 0.5);
+    size_t idx;
+    if (dx * dx + dy * dy + dz * dz > b.max_dist_sq || !l_index(L, cube, &idx)) {
+        end_of_ray(L, b, rs, bundle, node.weight);
+        return bundle;
+    }
+    const LBlock &ev = L.blocks[L.ids[idx]];
+    bool have_ahead = false;
+    PL ahead = L_UNINIT;
+    traverse(L, b, rs, cube, face7, ev, &have_ahead, &ahead, have_prev, prev, node.weight);
+    const float hit_alpha = face7 ? ev.face_color[face7][3] : 0.0f;
+    if (ev.visible && face7 != 0 && ev.opaque[face7 - 1] && hit_alpha > 0.0f) {
+        RayRecord r;
+        std::memset(&r, 0, sizeof r);
+        r.node = preorder_of()[node_index];
+        int32_t lc[3] = {cube[0], cube[1], cube[2]};   // hit.adjacent()
+        lc[(face7 - 1) % 3] += (face7 >= 4) ? 1 : -1;
+        const PL stored = have_prev ? prev : light_get(L, lc);
+        const float sv[3] = {lut(stored.r), lut(stored.g), lut(stored.b)};
+        for (int i = 0; i < 3; i++) {
+            r.ray.trigger_cube[i] = cube[i];
+            r.ray.value_cube[i] = lc[i];
+            const float col = ev.face_color[face7][i] > 1.0f ? 1.0f : ev.face_color[face7][i];   // Rgba::clamp
+            r.ray.light_from_struck_face[i] = ev.emission[i] + ps_mul_l(ps_mul_l(col, sv[i]), hit_alpha);
+        }
+        r.ray.value[0] = stored.r; r.ray.value[1] = stored.g; r.ray.value[2] = stored.b; r.ray.value[3] = stored.s;
+        rays.push_back(r);
+    }
+    if (!(rs.alpha > 0.0f)) {
+        end_of_ray(L, b, rs, bundle, node.weight);
+        return bundle;
+    }
+    float child_sum = 0.0f;
+    for (int f = 0; f < 6; f++) {
+        if (node.children[f]) {
+            int32_t nc[3] = {cube[0], cube[1], cube[2]};
+            nc[f % 3] += (f < 3) ? -1 : 1;
+            const int opp = (f < 3) ? f + 3 : f - 3;
+            child_sum += walk_debug(L, b, rays, origin, nc, opp + 1, node.children[f], have_ahead, ahead, rs);
+        }
+    }
+    end_of_ray(L, b, rs, std::fmax(bundle - child_sum, 0.0f), node.weight);
+    return bundle;
+}
+
+// compute_light (updater.rs:368-418) + finish (:932-944), as compute_light() in ../oracle/aic_light.cpp, with its rays
+static PL compute_light_debug(orc_light &L, const int32_t cube[3], std::vector<RayRecord> &rays) {
+    LightBuffer b;
+    b.max_dist_sq = (double)L.max_distance * (double)L.max_distance;
+    const LBlock &ev = get_evaluated(L, cube);
+    const bool origin_opaque = ev.all_opaque;
+    if (origin_opaque) {
+        if (!opaque_for_light(ev)) add_weighted_light(b, ev.emission, 1.0f);
+    } else {
+        RayState rs;
+        rs.alpha = 1.0f;
+        for (int f = 0; f < 6; f++) {   // directions_to_seek_light (updater.rs:669-690)
+            const int opp = (f < 3) ? f + 3 : f - 3;
+            int32_t nf[3] = {cube[0], cube[1], cube[2]}, no[3] = {cube[0], cube[1], cube[2]};
+            nf[f % 3] += (f < 3) ? -1 : 1;
+            no[opp % 3] += (opp < 3) ? -1 : 1;
+            rs.dw[f] = (ev.visible || get_evaluated(L, no).visible || get_evaluated(L, nf).has_emission) ? 1.0f : 0.0f;
+        }
+        walk_debug(L, b, rays, cube, cube, 0, 0, false, L_UNINIT, rs);
+    }
+    L.node_visits.fetch_add(b.visits, std::memory_order_relaxed);
+    const float scale = ps_clamped_l(1.0f / std::fmax(b.total_weight, 1.0f));
+    if (b.total_weight > 0.0f)
+        return PL{scalar_in_l(ps_mul_l(b.incoming[0], scale)), scalar_in_l(ps_mul_l(b.incoming[1], scale)),
+                  scalar_in_l(ps_mul_l(b.incoming[2], scale)), 255};
+    return origin_opaque ? L_OPAQUE : L_NO_RAYS;
 }
 
 }  // namespace orc_blocks
@@ -139,6 +253,28 @@ int orc_light_queue_region(orc_light *L, const aicb_aab *region, uint8_t priorit
 void orc_light_get_queue(const orc_light *L, uint8_t *out) {
     std::memset(out, 0, L->ids.size());
     for (const auto &kv : L->by_cube) out[kv.first] = (uint8_t)kv.second;
+}
+
+// Space::compute_light::<LightUpdateCubeInfo> for explicit cubes, against the current field: each cube's texel (what
+// orc_light_compute gives), its number of rays, and the rays packed cube after cube in the order the walk pushes them,
+// with the preorder index of the node each was struck at.  Returns the total; the rays and nodes are written only if
+// `capacity` holds them all.
+size_t orc_light_compute_debug(orc_light *L, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4],
+                               aicb_light_ray *rays_or_null, uint32_t *nodes_or_null, size_t capacity,
+                               uint32_t *ray_counts) {
+    std::vector<RayRecord> all;
+    for (size_t i = 0; i < n; i++) {
+        const size_t before = all.size();
+        const PL p = compute_light_debug(*L, cubes[i], all);
+        out[i][0] = p.r; out[i][1] = p.g; out[i][2] = p.b; out[i][3] = p.s;
+        ray_counts[i] = (uint32_t)(all.size() - before);
+    }
+    if (all.size() <= capacity)
+        for (size_t k = 0; k < all.size(); k++) {
+            if (rays_or_null) rays_or_null[k] = all[k].ray;
+            if (nodes_or_null) nodes_or_null[k] = all[k].node;
+        }
+    return all.size();
 }
 
 }
