@@ -140,6 +140,7 @@ def load_library() -> C.CDLL:
         "light_compute_debug": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
                                 size],
         "light_evaluate": [C.c_void_p, C.c_uint8, u64, u8, u64],
+        "light_update_from_queue": [C.c_void_p, C.c_uint64, C.POINTER(abi.LightUpdatesInfo)],
         "light_edit_and_propagate": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
         "light_edit_region": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, size],
         "light_relight_blocks": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
@@ -767,6 +768,17 @@ class _Scene:
         n, md, nv = C.c_uint64(0), C.c_uint8(0), C.c_uint64(0)
         _check(self._fn("light_evaluate")(self.handle, epsilon, C.byref(n), C.byref(md), C.byref(nv)))
         return int(n.value), int(md.value), int(nv.value)
+
+    def light_update_from_queue(self, max_updates=None) -> dict:
+        """LightStorage::update_light_from_queue (updater.rs:180-290): relaxation rounds until `max_updates` cube updates
+        are made or the queue is empty (None: no budget).  Every queued priority >= 1 is eligible; a round that does not
+        fit takes the highest priorities first, then the lowest indices.  Returns LightUpdatesInfo (updater.rs:970-984):
+        update_count, max_update_difference, queue_count, max_queue_priority."""
+        info = abi.LightUpdatesInfo()
+        budget = 2**64 - 1 if max_updates is None else int(max_updates)
+        _check(self._fn("light_update_from_queue")(self.handle, budget, C.byref(info)))
+        return {"update_count": int(info.update_count), "max_update_difference": int(info.max_update_difference),
+                "queue_count": int(info.queue_count), "max_queue_priority": int(info.max_queue_priority)}
 
     def light_edit_and_propagate(self, cubes: np.ndarray, block_ids: np.ndarray, epsilon: int = 0):
         """Mutation::set x n + evaluate_light(epsilon) -> (updates, max_difference)"""

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -108,6 +108,12 @@ class LightRay(C.Structure):
                 ("light_from_struck_face", C.c_float * 3), ("_pad", C.c_uint32)]
 
 
+class LightUpdatesInfo(C.Structure):
+    """aicb_light_updates_info: LightUpdatesInfo (space/light/updater.rs:970-984) of one light step."""
+    _fields_ = [("update_count", C.c_uint64), ("queue_count", C.c_uint64), ("max_update_difference", C.c_uint8),
+                ("max_queue_priority", C.c_uint8), ("_pad", C.c_uint8 * 6)]
+
+
 # Every symbol include/aicb200.h declares (tests check the built library exports all of them).
 class Layer(C.Structure):
     _fields_ = [("scene", C.c_void_p), ("camera", C.POINTER(CameraData)), ("options", C.POINTER(Options))]
@@ -174,6 +180,7 @@ EXPORTED_SYMBOLS = [
     "aicb_light_compute",
     "aicb_light_compute_debug",
     "aicb_light_evaluate",
+    "aicb_light_update_from_queue",
     "aicb_light_edit_and_propagate",
     "aicb_light_edit_region",
     "aicb_light_relight_blocks",
@@ -204,6 +211,7 @@ EXPORTED_SYMBOLS = [
     "aicb_group_light_compute",
     "aicb_group_light_compute_debug",
     "aicb_group_light_evaluate",
+    "aicb_group_light_update_from_queue",
     "aicb_group_light_edit_and_propagate",
     "aicb_group_light_edit_region",
     "aicb_group_light_relight_blocks",

@@ -420,6 +420,10 @@ aicb_status aicb_group_light_evaluate(aicb_group_scene *gs, uint8_t epsilon, uin
     });
 }
 
+aicb_status aicb_group_light_update_from_queue(aicb_group_scene *gs, uint64_t max_updates, aicb_light_updates_info *info) {
+    return on_group(gs, true, [&](Replicas r) { return light_update_from_queue(r, max_updates, info); });
+}
+
 aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff) {

@@ -155,6 +155,7 @@ struct LightState {
     struct Shared {
         DeviceBuffer pending;          // per cube: queued priority (0 = not queued) — LightUpdateQueue
         DeviceBuffer tile_max;         // per LIGHT_TILE cubes: upper bound of the queued priorities
+        DeviceBuffer step;             // a budgeted round's cut (light.cu: LightStepCut), then per tile: its rank base
         DeviceBuffer list, new_light, diff;   // one round's cubes, their computed texels, their difference_priority
         DeviceBuffer counters;         // LightCounters
         DeviceBuffer changes;          // one bit per cube: the set of changed cubes (SpaceChange::CubeLight)
@@ -435,6 +436,8 @@ aicb_status light_compute_debug(Replicas r, const int32_t (*cubes)[3], size_t n,
                                 size_t capacity, uint32_t *ray_counts, size_t *n_rays_total);
 aicb_status light_evaluate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                            uint64_t *node_visits);
+// update_light_from_queue: relaxation rounds until max_updates cube updates are made or the queue is empty.
+aicb_status light_update_from_queue(Replicas r, uint64_t max_updates, aicb_light_updates_info *info);
 aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
 aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, uint8_t epsilon,

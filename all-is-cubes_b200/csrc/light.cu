@@ -266,24 +266,27 @@ __global__ void k_find_max(const LightParams P, uint32_t n_tiles) {
 // A round whose priority is already <= epsilon does nothing.
 // One block per tile: the cubes of a tile reach the list in index order (block-wide scan), so 32 consecutive list
 // entries are neighbours along z — what the lockstep walk wants.
+// Thread -> word of the tile whose cubes a gathering thread lists.  With a power-of-two z extent the tile is a few whole
+// z-rows, and the threads are laid out so that 8 consecutive threads (32 cubes: one warp of the lockstep walk) cover a
+// 4 x 8 patch of (y, z) instead of 32 cubes in a line: neighbours in two directions share more of their chart walk.
+__device__ __forceinline__ uint32_t list_word_of_thread(const LightParams &P) {
+    uint32_t wl = threadIdx.x;
+    const uint32_t nz = (uint32_t)P.scene.size[2];
+    if (nz >= 8 && nz <= 256 && (nz & (nz - 1)) == 0) {
+        const uint32_t wpr = nz / 4, q = threadIdx.x >> 3, within = threadIdx.x & 7;
+        const uint32_t row_group = q / (wpr / 2), pz = q % (wpr / 2);
+        wl = (row_group * 4 + (within >> 1)) * wpr + pz * 2 + (within & 1);
+    }
+    return wl;
+}
+
 __global__ void __launch_bounds__(256) k_gather(const LightParams P, uint32_t n_tiles) {
     __shared__ uint32_t s_part[8], s_max[8], s_base;
     const uint32_t prio = P.counters->priority;
     if (prio <= P.epsilon_priority) return;
     const uint32_t n_words = (P.volume + 3) / 4;
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    // Thread -> word of the tile.  With a power-of-two z extent the tile is a few whole z-rows, and the threads are
-    // laid out so that 8 consecutive threads (32 cubes: one warp of the lockstep walk) cover a 4 x 8 patch of (y, z)
-    // instead of 32 cubes in a line: neighbours in two directions share more of their chart walk.
-    uint32_t wl = threadIdx.x;
-    {
-        const uint32_t nz = (uint32_t)P.scene.size[2];
-        if (nz >= 8 && nz <= 256 && (nz & (nz - 1)) == 0) {
-            const uint32_t wpr = nz / 4, q = threadIdx.x >> 3, within = threadIdx.x & 7;
-            const uint32_t row_group = q / (wpr / 2), pz = q % (wpr / 2);
-            wl = (row_group * 4 + (within >> 1)) * wpr + pz * 2 + (within & 1);
-        }
-    }
+    const uint32_t wl = list_word_of_thread(P);
     for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const uint32_t tm = P.tile_max[tile];
         if (tm <= P.epsilon_priority || tm + PRIORITY_BAND < prio) continue;   // (block-uniform)
@@ -821,6 +824,204 @@ __global__ void __launch_bounds__(256) k_changes_emit(uint32_t *bits, uint32_t n
     }
 }
 
+// The rounds of a budgeted step (aicb_light_update_from_queue) gather with these kernels in place of k_gather.  A round
+// whose band (the cubes k_gather would take) fits in the budget left takes the band.  A round that does not fit takes the
+// budget's worth of it: by priority, highest first, and within the priority where the budget ends (the cut level),
+// lowest index first.  Which cubes a round takes thus depends on the queue alone, never on the order blocks run in.
+// Everything stays on the device, behind the round's k_find_max:
+//   1. k_step_band: the band's cubes per priority, over the tiles k_gather would read;
+//   2. k_step_cut (one thread): the whole band, or the cut level and how many of its cubes to take; the round's list
+//      length, taken from the budget;
+//   3. only when a round may cut: k_step_level counts each tile's cubes at the cut level, and k_changes_scan turns the
+//      counts into the rank of each tile's first such cube;
+//   4. k_step_emit: the taken cubes into the list, their pending bytes cleared, each tile's bound lowered to what stays,
+//      as k_gather does.
+// A round that starts with no budget left or nothing above epsilon gathers nothing and leaves the bounds alone.
+struct LightStepCut {
+    uint32_t hist[PRIORITY_BAND + 1];   // the band's cubes at priority `priority - k` (k_step_cut clears it)
+    uint32_t active;                    // this round gathers
+    uint32_t level;                     // the cut level; 0 when the round takes its whole band
+    uint32_t take;                      // cubes of the cut level the round takes
+    uint32_t emitted;                   // list entries k_step_emit has placed
+};
+
+// the tiles k_gather reads in a round of priority `prio`, and the cubes it takes from them (block-uniform / per cube)
+__device__ __forceinline__ bool band_tile(const LightParams &P, uint32_t tile, uint32_t prio) {
+    const uint32_t tm = P.tile_max[tile];
+    return tm > P.epsilon_priority && tm + PRIORITY_BAND >= prio;
+}
+__device__ __forceinline__ bool in_band(const LightParams &P, uint32_t p, uint32_t prio) {
+    return p > P.epsilon_priority && p <= prio && p + PRIORITY_BAND >= prio;
+}
+
+__global__ void __launch_bounds__(256) k_step_band(const LightParams P, uint32_t n_tiles, LightStepCut *cut) {
+    __shared__ uint32_t s_hist[PRIORITY_BAND + 1];
+    const uint32_t prio = P.counters->priority;
+    if (P.counters->budget == 0 || prio <= P.epsilon_priority) return;
+    for (uint32_t i = threadIdx.x; i <= PRIORITY_BAND; i += blockDim.x) s_hist[i] = 0;
+    __syncthreads();
+    const uint32_t n_words = (P.volume + 3) / 4;
+    for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        if (!band_tile(P, tile, prio)) continue;   // (block-uniform)
+        const uint32_t w = tile * (LIGHT_TILE / 4) + threadIdx.x;
+        const uint32_t v = w < n_words ? ((const uint32_t *)P.pending)[w] : 0u;
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) {
+            const uint32_t p = (v >> (8 * k)) & 255u;
+            const bool in = in_band(P, p, prio) && w * 4 + k < P.volume;
+            // one shared atomic per distinct level of the warp
+            const uint32_t key = in ? prio - p : 0xffu;
+            const uint32_t same = __match_any_sync(0xffffffffu, key);
+            if (in && (threadIdx.x & 31) == (uint32_t)(__ffs(same) - 1)) atomicAdd(&s_hist[key], (uint32_t)__popc(same));
+        }
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i <= PRIORITY_BAND; i += blockDim.x)
+        if (s_hist[i]) atomicAdd(&cut->hist[i], s_hist[i]);
+}
+
+__global__ void k_step_cut(const LightParams P, LightStepCut *cut) {
+    const uint32_t prio = P.counters->priority;
+    unsigned long long left = P.counters->budget;
+    const bool active = left != 0 && prio > P.epsilon_priority;
+    uint32_t level = 0, take = 0, taken = 0;
+    for (uint32_t k = 0; k <= PRIORITY_BAND; k++) {
+        const uint32_t h = cut->hist[k];
+        cut->hist[k] = 0u;
+        if (!active || level) continue;
+        if (h > left) {   // the budget ends inside this level
+            level = prio - k;
+            take = (uint32_t)left;
+        } else {
+            left -= h;
+        }
+        taken += level ? take : h;
+    }
+    cut->active = active ? 1u : 0u;
+    cut->level = level;
+    cut->take = take;
+    cut->emitted = 0u;
+    if (!active) return;
+    P.counters->gathered = taken;
+    P.counters->budget = level ? 0ull : left;
+}
+
+__global__ void __launch_bounds__(256) k_step_level(const LightParams P, uint32_t n_tiles, const LightStepCut *cut,
+                                                    uint32_t *counts) {
+    if (!cut->active || !cut->level) return;
+    const uint32_t prio = P.counters->priority, level = cut->level;
+    const uint32_t n_words = (P.volume + 3) / 4;
+    for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        uint32_t c = 0;
+        if (band_tile(P, tile, prio)) {
+            const uint32_t w = tile * (LIGHT_TILE / 4) + threadIdx.x;
+            const uint32_t v = w < n_words ? ((const uint32_t *)P.pending)[w] : 0u;
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++) c += (((v >> (8 * k)) & 255u) == level && w * 4 + k < P.volume) ? 1u : 0u;
+        }
+        uint32_t total;
+        block_exclusive_scan(c, &total);
+        if (threadIdx.x == 0) counts[tile] = total;
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(256) k_step_emit(const LightParams P, uint32_t n_tiles, LightStepCut *cut,
+                                                   const uint32_t *level_starts) {
+    __shared__ uint8_t s_sel[LIGHT_TILE / 4];
+    __shared__ uint32_t s_max[8], s_base;
+    if (!cut->active) return;
+    const uint32_t prio = P.counters->priority, level = cut->level, take = cut->take;
+    const uint32_t n_words = (P.volume + 3) / 4;
+    const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const uint32_t wl = list_word_of_thread(P);
+    uint32_t *pending = (uint32_t *)P.pending;
+    for (uint32_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        if (!band_tile(P, tile, prio)) continue;   // (block-uniform)
+        // which cubes of the tile the round takes: one word per thread in index order, for the rank in the cut level
+        {
+            const uint32_t w = tile * (LIGHT_TILE / 4) + threadIdx.x;
+            const uint32_t v = w < n_words ? pending[w] : 0u;
+            uint32_t sel = 0, at_level = 0;
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++) {
+                const uint32_t p = (v >> (8 * k)) & 255u;
+                if (!in_band(P, p, prio) || w * 4 + k >= P.volume) continue;
+                if (p > level) sel |= 1u << k;
+                else if (p == level) at_level |= 1u << k;
+            }
+            if (level) {   // (block-uniform)
+                uint32_t total;
+                uint32_t rank = level_starts[tile] + block_exclusive_scan((uint32_t)__popc(at_level), &total);
+#pragma unroll
+                for (uint32_t k = 0; k < 4; k++)
+                    if (at_level & (1u << k)) {
+                        if (rank < take) sel |= 1u << k;
+                        rank++;
+                    }
+            }
+            s_sel[threadIdx.x] = (uint8_t)sel;
+        }
+        __syncthreads();
+        // the list, in k_gather's thread layout
+        const uint32_t w = tile * (LIGHT_TILE / 4) + wl;
+        uint32_t v = w < n_words ? pending[w] : 0u;
+        const uint32_t sel = s_sel[wl], cnt = (uint32_t)__popc(sel);
+        uint32_t total;
+        const uint32_t before = block_exclusive_scan(cnt, &total);
+        uint32_t rest = 0;
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) if (!(sel & (1u << k))) rest = max(rest, (v >> (8 * k)) & 255u);
+        rest = __reduce_max_sync(0xffffffffu, rest);
+        if (lane == 0) s_max[wid] = rest;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t m = 0;
+            for (int i = 0; i < 8; i++) m = max(m, s_max[i]);
+            s_base = total ? atomicAdd(&cut->emitted, total) : 0u;
+            P.tile_max[tile] = m;
+        }
+        __syncthreads();
+        if (cnt) {
+            uint32_t at = s_base + before;
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++)
+                if (sel & (1u << k)) { P.list[at++] = w * 4 + k; v &= ~(255u << (8 * k)); }
+            pending[w] = v;
+        }
+        __syncthreads();
+    }
+}
+
+// The queue as a budgeted step leaves it: the queued cubes and their highest priority, exact (the tile bounds are upper
+// bounds only), from the pending bytes, 16 per load.
+__global__ void __launch_bounds__(256) k_queue_summary(const LightParams P) {
+    uint32_t n = 0, m = 0;
+    const uint32_t t0 = blockIdx.x * blockDim.x + threadIdx.x, stride = gridDim.x * blockDim.x;
+    const uint32_t n_vec = P.volume / 16;
+    for (uint32_t i = t0; i < n_vec; i += stride) {
+        const uint4 q = ((const uint4 *)P.pending)[i];
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (uint32_t k = 0; k < 4; k++) {
+            n += (uint32_t)__popc(__vcmpne4(w[k], 0u)) / 8u;   // (0xff per byte that differs)
+            const uint32_t h = __vmaxu4(w[k], w[k] >> 16);
+            m = max(m, max(h & 255u, (h >> 8) & 255u));
+        }
+    }
+    for (uint32_t idx = n_vec * 16 + t0; idx < P.volume; idx += stride) {
+        const uint32_t p = P.pending[idx];
+        n += p ? 1u : 0u;
+        m = max(m, p);
+    }
+    n = __reduce_add_sync(0xffffffffu, n);
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0) {
+        if (n) atomicAdd(&P.counters->queue_len, n);
+        if (m) atomicMax(&P.counters->queue_max, m);
+    }
+}
+
 // Packing the rays of aicb_light_compute_debug.  A cube's rays are the records of the walk that computed its texel:
 // the chain walk's, or the lockstep walk's where the chain walk overflowed.
 __device__ __forceinline__ bool ray_counts_for_its_cube(const LightRayRecord &r, const uint8_t *lockstep) {
@@ -981,7 +1182,12 @@ constexpr size_t ROUND_WALK_COUNTERS =
 // then walks a share of the changed cubes (mark form), raising priorities in device 0's queue.  Compute is Jacobi
 // within a round and marks merge by max, so a group performs one context's operations.  One context issues no event
 // and no push.
-aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits) {
+// `budget` (a budgeted step, light_update_from_queue): every queued priority is eligible, the rounds gather with the
+// k_step_* kernels, and they stop once *budget cube updates are made or the queue is empty.  The budget left lives in
+// the device counters, so a batch's rounds stay queued back to back; a round after it runs out gathers nothing.
+// nullptr: evaluate_light(epsilon)'s rounds.
+aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff, uint64_t *node_visits,
+                      const uint64_t *budget = nullptr) {
     aicb_scene *s = r.scene[0];
     aicb_ctx *ctx = s->ctx;
     cudaStream_t st = ctx->stream.get();
@@ -989,24 +1195,43 @@ aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8
     std::vector<LightParams> RP;
     for (size_t i = 0; i < r.n; i++) {
         RP.push_back(light_params(r, i));
-        RP.back().epsilon_priority = (uint32_t)epsilon / 2 + 1;
+        RP.back().epsilon_priority = budget ? 0u : (uint32_t)epsilon / 2 + 1;
     }
     const LightParams &P = RP[0];
     const int blocks = ctx->num_sms * 8;
     const int wide = ctx->num_sms * 8;    // 128-thread blocks of k_compute_overflow and k_apply (grid-stride)
     const uint32_t n_tiles = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
+    LightStepCut *cut = s->light.shared.step.get<LightStepCut>();
+    uint32_t *level_starts = (uint32_t *)(cut + 1);
     uint64_t total = 0, visits = 0, rounds = 0;
     uint32_t maxd = 0;
     CU(cudaEventRecord(ctx->ev_light[0].get(), st));
     CU(cudaMemsetAsync(P.counters, 0, sizeof(LightCounters), st));
+    if (budget) {
+        CU(cudaMemcpyAsync(&P.counters->budget, budget, sizeof *budget, cudaMemcpyHostToDevice, st));
+        CU(cudaMemsetAsync(cut, 0, sizeof(LightStepCut), st));
+    }
     k_tile_rebuild<<<blocks, 256, 0, st>>>(P, n_tiles);   // (fast_evaluate / edits write the priority bytes directly)
     const int ROUNDS_PER_SYNC = 8;
-    for (int batch = 0; batch < 100000; batch++) {
+    uint64_t left = budget ? *budget : 1;   // (the budget left at the last synchronisation)
+    for (int batch = 0; batch < 100000 && left; batch++) {
+        // a round takes at most the volume, so with this much left no round of the batch can cut
+        const bool may_cut = left < (uint64_t)ROUNDS_PER_SYNC * s->volume;
         for (int round = 0; round < ROUNDS_PER_SYNC; round++) {
             CU(cudaMemsetAsync(P.counters, 0, ROUND_LIST_COUNTERS, st));
             CU(cudaMemsetAsync(&P.counters->changed, 0, ROUND_WALK_COUNTERS, st));
             k_find_max<<<16, 256, 0, st>>>(P, n_tiles);
-            k_gather<<<blocks, 256, 0, st>>>(P, n_tiles);
+            if (!budget) {
+                k_gather<<<blocks, 256, 0, st>>>(P, n_tiles);
+            } else {
+                k_step_band<<<blocks, 256, 0, st>>>(P, n_tiles, cut);
+                k_step_cut<<<1, 1, 0, st>>>(P, cut);
+                if (may_cut) {
+                    k_step_level<<<blocks, 256, 0, st>>>(P, n_tiles, cut, level_starts);
+                    k_changes_scan<<<1, 1024, 0, st>>>(level_starts, n_tiles);
+                }
+                k_step_emit<<<blocks, 256, 0, st>>>(P, n_tiles, cut, level_starts);
+            }
             TRY(walk(r, RP, false));
             if (group) k_apply<true><<<wide, 128, 0, st>>>(P);
             else k_apply<false><<<wide, 128, 0, st>>>(P);
@@ -1024,6 +1249,7 @@ aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8
         visits = h.node_visits;
         maxd = h.max_diff;
         rounds += ROUNDS_PER_SYNC;
+        if (budget) left = h.budget;
         if (h.priority <= P.epsilon_priority) break;   // the batch's last round found nothing above epsilon
     }
     CU(cudaEventRecord(ctx->ev_light[1].get(), st));
@@ -1060,8 +1286,8 @@ LightBlockDev light_block(const aicb_block_desc &b) {
 // ---------------------------------------------------------------------------------------------
 // a scene's light state (internal.h)
 // ---------------------------------------------------------------------------------------------
-// What aicb_scene_device_bytes counts of a light state's parts (it leaves out the tile bounds, the counters, the overflow
-// count and the push targets).
+// What aicb_scene_device_bytes counts of a light state's parts (it leaves out the tile bounds, the step's cut, the
+// counters, the overflow count and the push targets).
 static size_t change_bytes(size_t vol) { return (vol + 31) / 32 * 4; }
 static size_t dirty_bytes(size_t vol) { return (vol + 1023) / 1024 * 4 + 16; }
 static uint64_t own_bytes(size_t vol) { return chart_preorder_host().size() * sizeof(float4) + vol * 4; }
@@ -1088,6 +1314,7 @@ aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas,
         TRY(sh.pending.ensure(vol + 16));
         CU(cudaMemset(sh.pending.get(), 0, vol + 16));
         TRY(sh.tile_max.ensure(((vol + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
+        TRY(sh.step.ensure(sizeof(LightStepCut) + ((vol + LIGHT_TILE - 1) / LIGHT_TILE + 1) * 4));
         TRY(sh.list.ensure(vol * 4 + 16));
         TRY(sh.new_light.ensure(vol * 4 + 16));
         TRY(sh.diff.ensure(vol + 16));
@@ -1260,6 +1487,32 @@ aicb_status light_evaluate(Replicas r, uint8_t epsilon, uint64_t *updates_done, 
                            uint64_t *node_visits) {
     TRY(ensure_replicas(r));
     return propagate(r, epsilon, updates_done, max_diff, node_visits);
+}
+
+// update_light_from_queue (updater.rs:180-290) with a count budget: propagate's budgeted rounds, then the queue as they
+// left it, counted on the device (k_queue_summary).  A zero budget runs no round.
+aicb_status light_update_from_queue(Replicas r, uint64_t max_updates, aicb_light_updates_info *info) {
+    TRY(ensure_replicas(r));
+    uint64_t updates = 0;
+    uint8_t maxd = 0;
+    TRY(propagate(r, 0, &updates, &maxd, nullptr, &max_updates));
+    aicb_scene *s = r.scene[0];
+    cudaStream_t st = s->ctx->stream.get();
+    const LightParams P = light_params(r, 0);
+    CU(cudaMemsetAsync(&P.counters->queue_len, 0, 2 * sizeof(uint32_t), st));
+    k_queue_summary<<<s->ctx->num_sms * 4, 256, 0, st>>>(P);
+    CU(cudaGetLastError());
+    uint32_t q[2] = {0, 0};
+    CU(cudaMemcpyAsync(q, &P.counters->queue_len, sizeof q, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (info) {
+        std::memset(info, 0, sizeof *info);
+        info->update_count = updates;
+        info->queue_count = q[0];
+        info->max_update_difference = maxd;
+        info->max_queue_priority = (uint8_t)q[1];
+    }
+    return AICB_OK;
 }
 
 // Mutation::set x n (space.rs:1346-1352 -> side_effects_of_set -> modified_cube_needs_update,
@@ -1693,6 +1946,10 @@ aicb_status aicb_light_compute_debug(aicb_scene *s, const int32_t (*cubes)[3], s
 aicb_status aicb_light_evaluate(aicb_scene *s, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                 uint64_t *node_visits) {
     return on_scene(s, [&](Replicas r) { return light_evaluate(r, epsilon, updates_done, max_diff, node_visits); });
+}
+
+aicb_status aicb_light_update_from_queue(aicb_scene *s, uint64_t max_updates, aicb_light_updates_info *info) {
+    return on_scene(s, [&](Replicas r) { return light_update_from_queue(r, max_updates, info); });
 }
 
 aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,

@@ -87,13 +87,18 @@ struct LightCounters {
     uint32_t overflow;              // entries of replica 0's overflow list
     uint32_t queued;                // cubes the last queue scan (k_queue_cubes) selected
     uint32_t edited;                // cubes whose block the last box edit (k_region_cells) changed
-    uint32_t _pad[4];
+    unsigned long long budget;      // a budgeted step's cube updates left (k_step_cut takes each round's from it)
+    uint32_t queue_len;             // the queue after a step (k_queue_summary): queued cubes ...
+    uint32_t queue_max;             // ... and their highest priority
 };
 static_assert(offsetof(LightCounters, gathered) == 0 && offsetof(LightCounters, priority) == 4 &&
               offsetof(LightCounters, max_diff) == 8 && offsetof(LightCounters, updates) == 12 &&
               offsetof(LightCounters, node_visits) == 16 && offsetof(LightCounters, changed) == 24 &&
               offsetof(LightCounters, compute_work) == 28 && offsetof(LightCounters, mark_work) == 32 &&
-              offsetof(LightCounters, overflow) == 36 && offsetof(LightCounters, queued) == 40 && sizeof(LightCounters) == 64,
+              offsetof(LightCounters, overflow) == 36 && offsetof(LightCounters, queued) == 40 &&
+              offsetof(LightCounters, edited) == 44 && offsetof(LightCounters, budget) == 48 &&
+              offsetof(LightCounters, queue_len) == 56 && offsetof(LightCounters, queue_max) == 60 &&
+              sizeof(LightCounters) == 64,
               "LightCounters: the layout the kernels and the round's memsets address");
 
 struct LightParams {

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 14 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 15 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -151,6 +151,17 @@ pub struct aicb_light_ray {
     pub value: [u8; 4],
     pub light_from_struck_face: [f32; 3],
     pub _pad: u32,
+}
+
+/// `LightUpdatesInfo` (all-is-cubes/src/space/light/updater.rs:970-984) of one light step
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_light_updates_info {
+    pub update_count: u64,
+    pub queue_count: u64,
+    pub max_update_difference: u8,
+    pub max_queue_priority: u8,
+    pub _pad: [u8; 6],
 }
 
 /// one pixel of the terminal's frame: `ColorCharacterBuf::output` (all-is-cubes-desktop/src/terminal.rs:355-366)
@@ -313,6 +324,9 @@ unsafe extern "C" {
     pub fn aicb_light_compute(s: *mut aicb_scene, cubes: *const [i32; 3], n: usize, out: *mut [u8; 4]) -> aicb_status;
     pub fn aicb_light_evaluate(s: *mut aicb_scene, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8,
                                chart_node_visits: *mut u64) -> aicb_status;
+    // LightStorage::update_light_from_queue with a budget of cube updates: the light step of a tick
+    pub fn aicb_light_update_from_queue(s: *mut aicb_scene, max_updates: u64, info_or_null: *mut aicb_light_updates_info)
+                                        -> aicb_status;
     pub fn aicb_light_edit_and_propagate(s: *mut aicb_scene, cubes: *const [i32; 3], new_ids: *const u16, n_edits: usize,
                                          epsilon: u8, updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
     // Mutation::fill / fill_uniform(region): Mutation::set for every cube of a box, without propagation
@@ -339,6 +353,8 @@ unsafe extern "C" {
     pub fn aicb_group_light_compute(gs: *mut aicb_group_scene, cubes: *const [i32; 3], n: usize, out: *mut [u8; 4]) -> aicb_status;
     pub fn aicb_group_light_evaluate(gs: *mut aicb_group_scene, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8,
                                      chart_node_visits: *mut u64) -> aicb_status;
+    pub fn aicb_group_light_update_from_queue(gs: *mut aicb_group_scene, max_updates: u64,
+                                              info_or_null: *mut aicb_light_updates_info) -> aicb_status;
     pub fn aicb_group_light_edit_and_propagate(gs: *mut aicb_group_scene, cubes: *const [i32; 3], new_ids: *const u16,
                                                n_edits: usize, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8)
                                                -> aicb_status;

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 14
+#define AICB_ABI_VERSION 15
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -539,6 +539,34 @@ aicb_status aicb_light_compute(aicb_scene *, const int32_t (*cubes)[3], size_t n
  * <= Priority::from_difference(epsilon). */
 aicb_status aicb_light_evaluate(aicb_scene *, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                 uint64_t *chart_node_visits_or_null);
+/* LightUpdatesInfo (space/light/updater.rs:970-984) of one step. */
+typedef struct aicb_light_updates_info {
+    uint64_t update_count;          /* compute_light + apply_light_update calls this step */
+    uint64_t queue_count;           /* cubes queued after the step */
+    uint8_t max_update_difference;  /* largest difference_priority applied this step */
+    uint8_t max_queue_priority;     /* highest queued Priority after the step; 0 (Priority::MIN) when empty */
+    uint8_t _pad[6];
+} aicb_light_updates_info;
+/* LightStorage::update_light_from_queue (space/light/updater.rs:180-290) with a budget of cube updates: the light step
+ * of a tick (update_light_system, space/step.rs:341-369).  A host edits with aicb_light_edit_region (or the queue calls
+ * below), calls this with the tick's budget, then takes the changed cubes; light converges over several ticks and no
+ * tick stalls.  The call is synchronous and deterministic, and the library keeps no clock: a host with a time budget
+ * turns it into a count, e.g. from aicb_light_stats' out[3] / out[0] of earlier steps.
+ *   - Work: relaxation rounds on the queue, as aicb_light_evaluate runs them, until max_updates cube updates are made
+ *     or the queue is empty.  info->update_count = min(max_updates, the updates the queue offered); a cube re-queued
+ *     and updated again counts twice.  Every queued priority >= 1 is eligible (aicb_light_evaluate(0) leaves
+ *     priority-1 entries, which only a host's aicb_light_queue_region(..., 1) creates).  max_updates == 0 runs no round
+ *     and fills info; UINT64_MAX is the reference's `budget: None`.
+ *   - Which cubes: a round whose band (the cubes within 16 priority levels of the round's highest) fits in the budget
+ *     left is aicb_light_evaluate's round.  A round that does not fit takes the budget's worth of the band: by
+ *     priority, highest first, and within the priority where the budget ends, lowest Z-major index first.  So the set
+ *     of cubes a step updates depends only on the queue.
+ *   - A round stays whole: its cubes' results are stored, the set of changed cubes updated and their dependencies
+ *     re-queued (on a group, the replicas updated) before the call returns.
+ *   - info_or_null: queue_count and max_queue_priority are exact, as aicb_light_download_queue would report them.
+ *     aicb_light_stats reads as after aicb_light_evaluate, with out[0] == update_count.
+ * AICB_ERR_INVALID, with nothing changed: a NULL scene or LightPhysics::None.  GPU test: tests/test_gpu_light_step.py. */
+aicb_status aicb_light_update_from_queue(aicb_scene *, uint64_t max_updates, aicb_light_updates_info *info_or_null);
 aicb_status aicb_light_edit_and_propagate(aicb_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                           size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                           uint8_t *max_diff);
@@ -671,6 +699,10 @@ aicb_status aicb_group_light_fast_evaluate(aicb_group_scene *);
 aicb_status aicb_group_light_compute(aicb_group_scene *, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]);
 aicb_status aicb_group_light_evaluate(aicb_group_scene *, uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff,
                                       uint64_t *chart_node_visits_or_null);
+/* aicb_light_update_from_queue on the group: validated against replica 0; the replicas are identical after it, and the
+ * result is one context's. */
+aicb_status aicb_group_light_update_from_queue(aicb_group_scene *, uint64_t max_updates,
+                                               aicb_light_updates_info *info_or_null);
 aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff);
