@@ -141,6 +141,7 @@ def load_library() -> C.CDLL:
                                 size],
         "light_evaluate": [C.c_void_p, C.c_uint8, u64, u8, u64],
         "light_update_from_queue": [C.c_void_p, C.c_uint64, C.POINTER(abi.LightUpdatesInfo)],
+        "light_edit_cubes": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, size],
         "light_edit_and_propagate": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
         "light_edit_region": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, size],
         "light_relight_blocks": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, u64, u8],
@@ -779,6 +780,18 @@ class _Scene:
         _check(self._fn("light_update_from_queue")(self.handle, budget, C.byref(info)))
         return {"update_count": int(info.update_count), "max_update_difference": int(info.max_update_difference),
                 "queue_count": int(info.queue_count), "max_queue_priority": int(info.max_queue_priority)}
+
+    def light_edit_cubes(self, cubes: np.ndarray, block_ids: np.ndarray) -> int:
+        """Mutation::set(cubes[i], block_ids[i]) in list order, without propagation (light_evaluate or
+        light_update_from_queue follows).  A cube may be named more than once.  Returns the number of entries whose id
+        differs from the block their cube holds at that point of the list."""
+        c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
+        ids = np.ascontiguousarray(block_ids, dtype=np.uint16).reshape(-1)
+        if ids.shape[0] != c.shape[0]:
+            raise ValueError(f"{c.shape[0]} cubes but {ids.shape[0]} block ids")
+        n = C.c_size_t(0)
+        _check(self._fn("light_edit_cubes")(self.handle, c.ctypes.data, ids.ctypes.data, c.shape[0], C.byref(n)))
+        return int(n.value)
 
     def light_edit_and_propagate(self, cubes: np.ndarray, block_ids: np.ndarray, epsilon: int = 0):
         """Mutation::set x n + evaluate_light(epsilon) -> (updates, max_difference)"""

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -181,6 +181,7 @@ EXPORTED_SYMBOLS = [
     "aicb_light_compute_debug",
     "aicb_light_evaluate",
     "aicb_light_update_from_queue",
+    "aicb_light_edit_cubes",
     "aicb_light_edit_and_propagate",
     "aicb_light_edit_region",
     "aicb_light_relight_blocks",
@@ -213,6 +214,7 @@ EXPORTED_SYMBOLS = [
     "aicb_group_light_evaluate",
     "aicb_group_light_update_from_queue",
     "aicb_group_light_edit_and_propagate",
+    "aicb_group_light_edit_cubes",
     "aicb_group_light_edit_region",
     "aicb_group_light_relight_blocks",
     "aicb_group_light_download",

@@ -1137,7 +1137,7 @@ static aicb_status flatten_placeable(Replicas r, const aicb_block_desc *descs, s
 }
 
 // The context's staging (h_delta / d_delta) with room for a batch of `bytes`, once the previous batch has left it.
-static aicb_status delta_room(aicb_ctx *ctx, size_t bytes) {
+aicb_status delta_room(aicb_ctx *ctx, size_t bytes) {
     if (std::min(ctx->h_delta.bytes(), ctx->d_delta.bytes()) < bytes) {
         if (ctx->h_delta) cudaEventSynchronize(ctx->ev_delta.get());   // the previous batch's copy may still read it
         ctx->h_delta.reset();

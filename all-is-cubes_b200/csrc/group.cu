@@ -432,6 +432,11 @@ aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *gs, const int3
     });
 }
 
+aicb_status aicb_group_light_edit_cubes(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *new_ids,
+                                        size_t n, size_t *n_changed) {
+    return on_group(gs, true, [&](Replicas r) { return light_edit_cubes(r, cubes, new_ids, n, n_changed); });
+}
+
 aicb_status aicb_group_light_relight_blocks(aicb_group_scene *gs, const uint16_t *indices, size_t n, uint8_t epsilon,
                                             uint64_t *updates_done, uint8_t *max_diff) {
     return on_group(gs, true, [&](Replicas r) {

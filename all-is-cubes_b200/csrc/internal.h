@@ -186,7 +186,7 @@ struct aicb_ctx {
     Event ev_k[5];               // AICB_PROFILE_KERNELS
     bool profile_kernels = false;
     bool stage_timing = true;    // record the per-kernel events of a frame (aicb_render_info::stage_ms)
-    PinnedBuffer h_delta;        // staging of aicb_scene_update_cubes batches (pinned / device)
+    PinnedBuffer h_delta;        // staging of cube and box updates and edit lists (pinned / device)
     DeviceBuffer d_delta;
     Event ev_delta;
     DeviceBuffer d_debug;
@@ -380,6 +380,9 @@ aicb_status on_scene(aicb_scene *s, Call call) {
 aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out);
 aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uint16_t *ids, const uint8_t (*light)[4],
                                 size_t n);
+// The context's pinned staging (h_delta) and its device side (d_delta) with room for a batch of `bytes`, once the
+// previous batch (the copy ordered before aicb_ctx::ev_delta) has left it.
+aicb_status delta_room(aicb_ctx *ctx, size_t bytes);
 // A box of cubes inside a scene's bounds: its lower corner as offsets from the scene's, and its size.
 struct RegionBox {
     uint32_t lo[3], size[3];
@@ -438,6 +441,10 @@ aicb_status light_evaluate(Replicas r, uint8_t epsilon, uint64_t *updates_done, 
                            uint64_t *node_visits);
 // update_light_from_queue: relaxation rounds until max_updates cube updates are made or the queue is empty.
 aicb_status light_update_from_queue(Replicas r, uint64_t max_updates, aicb_light_updates_info *info);
+// Mutation::set x n in list order, without propagation; *n_changed (if given): the entries whose id differs from the
+// block their cube holds at that point of the list.
+aicb_status light_edit_cubes(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n, size_t *n_changed);
+// light_edit_cubes, then evaluate_light(epsilon).
 aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
                                      uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff);
 aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, uint8_t epsilon,

@@ -6,7 +6,6 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <unordered_map>
 
 #include "internal.h"
 #include "light_kernel.cuh"
@@ -558,39 +557,13 @@ __global__ void k_fast_evaluate(const LightParams P) {
     }
 }
 
-struct EditOp {
-    uint32_t idx;
-    uint32_t cell;        // new cell word, or 0xffffffff = leave
-    uint8_t set_opaque;   // light := OPAQUE
-    uint8_t pending_op;   // 0 none, 1 remove, 2 raise to NEWLY_VISIBLE
-    uint8_t _pad[2];
-};
-
-// queue: apply the pending_op too and mark the cubes set to OPAQUE changed (device 0 of a group holds the queue and the
-// set, the other replicas take cells and light only).  A cube set to OPAQUE is changed even if it already was
-// (modified_cube_needs_update, updater.rs:153-161).
-__global__ void k_edits(const LightParams P, const EditOp *ops, uint32_t n, uint32_t wide, uint32_t queue) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const EditOp op = ops[i];
-    if (op.cell != 0xffffffffu) {
-        if (wide) ((uint32_t *)P.scene.cells)[op.idx] = op.cell;
-        else ((uint16_t *)P.scene.cells)[op.idx] = (uint16_t)op.cell;
-    }
-    if (op.set_opaque) {
-        const_cast<uint32_t *>(P.scene.light)[op.idx] = TX_OPAQUE;
-        if (queue) mark_changed(P, op.idx);
-    }
-    if (!queue) return;
-    if (op.pending_op == 1) P.pending[op.idx] = 0;
-    else if (op.pending_op == 2) P.pending[op.idx] = PRIO_NEWLY_VISIBLE;
-}
-
-// modified_cube_needs_update (updater.rs:135-173) for a cube that holds block `id`: k_edits' writes for that block, then
-// the face neighbours whose own face toward the cube is not opaque are queued.  Only `queue` (device 0 of a group)
-// touches the queue and the set.  Threads may apply it to any set of cubes at once, reading the cells as they are after
-// every edit: no two threads write one pending byte with different values, since a cube opaque for light is opaque on
-// every face, so no neighbour queues it, and every other write stores NEWLY_VISIBLE.
+// modified_cube_needs_update (updater.rs:135-173) for a cube that holds block `id`: a block opaque for light stores
+// OPAQUE (a changed cube even if it already was, updater.rs:153-161) and cancels the cube's queued update, any other
+// block queues the cube at NEWLY_VISIBLE; then the face neighbours whose own face toward the cube is not opaque are
+// queued.  Only `queue` (device 0 of a group) touches the queue and the set.  Threads may apply it to any set of cubes
+// at once, reading the cells as they are after every edit: no two threads write one pending byte with different
+// values, since a cube opaque for light is opaque on every face, so no neighbour queues it, and every other write
+// stores NEWLY_VISIBLE.
 __device__ __forceinline__ void modified_cube(const LightParams &P, uint32_t idx, uint32_t id, uint32_t queue) {
     const uint32_t fl = __ldg(&P.blocks[id].flags);
     if ((fl & LB_ALL_OPAQUE) && !(fl & LB_EMISSIVE)) {   // opaque_for_light_computation
@@ -635,6 +608,46 @@ __global__ void __launch_bounds__(256) k_region_light(const LightParams P, const
     const uint32_t idx = ((box.lo[0] + rx) * (uint32_t)P.scene.size[1] + box.lo[1] + ry) * (uint32_t)P.scene.size[2] +
                          box.lo[2] + (p - row * box.size[2]);
     modified_cube(P, idx, block_id_at(P.scene, idx), queue);
+}
+
+// One changing entry of an aicb_light_edit_cubes list (its id differs from the block its cube holds at that point of
+// the list), as staged: the cube's Z-major index, the entry's id, and the block the cube holds after the whole list.
+struct __align__(8) EditEntry {
+    uint32_t idx;
+    uint16_t id;
+    uint16_t final_id;
+};
+static_assert(sizeof(EditEntry) == 8, "an EditEntry is staged as 8 bytes");
+
+// The cells of a list of sets: every changing entry stores its cube's final cell word, the kind from the block table's
+// records on the device.  A cube named by several entries has them all store the same word.
+template <bool WIDE>
+__global__ void __launch_bounds__(256) k_edit_cells(const DeviceScene S, const EditEntry *entries, uint32_t n) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const EditEntry e = entries[i];
+    const uint32_t word = e.final_id | (__ldg(&S.blocks[e.final_id].kind_res) & 0xffu) << (WIDE ? 16 : 14);
+    if (WIDE) ((uint32_t *)S.cells)[e.idx] = word;
+    else ((uint16_t *)S.cells)[e.idx] = (uint16_t)word;
+}
+
+// The light rule of aicb_light_edit_cubes, after k_edit_cells wrote the final cells: one changing entry per thread.
+// A cube's own queue entry, and its neighbours', are k_region_light's argument: its last changing entry decides them and
+// sets its final block, so modified_cube against the final cells is exact.  The texels are not a function of the final
+// cells: every changing entry whose own block is opaque for light stores OPAQUE and enters the set, as the reference's
+// set does even when a later entry makes the cube non-opaque again (A -> B -> A keeps an OPAQUE texel).  Every write
+// stores OPAQUE, 0 or NEWLY_VISIBLE where no other thread stores a different value.
+__global__ void __launch_bounds__(256) k_edit_light(const LightParams P, const EditEntry *entries, uint32_t n,
+                                                    uint32_t queue) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const EditEntry e = entries[i];
+    const uint32_t fl = __ldg(&P.blocks[e.id].flags);
+    if ((fl & LB_ALL_OPAQUE) && !(fl & LB_EMISSIVE)) {   // opaque_for_light_computation
+        const_cast<uint32_t *>(P.scene.light)[e.idx] = TX_OPAQUE;
+        if (queue) mark_changed(P, e.idx);
+    }
+    modified_cube(P, e.idx, block_id_at(P.scene, e.idx), queue);
 }
 
 // The scan of aicb_light_relight_blocks: every cell of the scene, 16 bytes per load (8 u16 cells or 4 u32 cells,
@@ -1515,83 +1528,75 @@ aicb_status light_update_from_queue(Replicas r, uint64_t max_updates, aicb_light
     return AICB_OK;
 }
 
-// Mutation::set x n (space.rs:1346-1352 -> side_effects_of_set -> modified_cube_needs_update,
-// updater.rs:135-173) applied in order on the host mirror, then evaluate_light(epsilon).  Every replica takes the
-// mirror's, the cells' and the light's changes; only replica 0 holds the queue.
-aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
-                                     uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
-    if (n_edits && (!cubes || !new_ids)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    TRY(ensure_replicas(r));
+// Mutation::set x n (space.rs:1346-1352 -> side_effects_of_set -> modified_cube_needs_update, updater.rs:135-173)
+// without propagation.  The list is validated and indexed before anything changes.  One pass in list order over
+// replica 0's host mirror finds the changing entries (the same-block skip) and writes the mirror, which
+// aicb_scene_update_blocks re-encodes cells from; a second pass gives each its cube's final block.  They are staged,
+// 8 bytes each, in every replica's context, behind the cube updates queued there: k_edit_cells writes the final cells
+// and k_edit_light applies the rule (DESIGN.md §4b).  Replica 0 alone touches the queue and the set.
+aicb_status light_edit_cubes(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n,
+                             size_t *n_changed) {
+    if (n && (!cubes || !new_ids)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "more than 2^32 - 1 edits");
     aicb_scene *s = r.scene[0];
     const DeviceScene &ds = s->ds;
-    auto index_of = [&](int x, int y, int z, uint32_t *idx) {
-        uint32_t dx = (uint32_t)(x - ds.lo[0]), dy = (uint32_t)(y - ds.lo[1]), dz = (uint32_t)(z - ds.lo[2]);
-        if (dx >= (uint32_t)ds.size[0] || dy >= (uint32_t)ds.size[1] || dz >= (uint32_t)ds.size[2]) return false;
-        *idx = (dx * (uint32_t)ds.size[1] + dy) * (uint32_t)ds.size[2] + dz;
-        return true;
-    };
-    std::unordered_map<uint32_t, EditOp> ops;
-    auto op_of = [&](uint32_t idx) -> EditOp & {
-        auto it = ops.find(idx);
-        if (it == ops.end()) {
-            EditOp o;
-            std::memset(&o, 0, sizeof o);
-            o.idx = idx;
-            o.cell = 0xffffffffu;
-            it = ops.emplace(idx, o).first;
-        }
-        return it->second;
-    };
-    // validate everything before the host mirror (or anything else) changes
-    for (size_t i = 0; i < n_edits; i++) {
-        uint32_t idx;
-        if (!index_of(cubes[i][0], cubes[i][1], cubes[i][2], &idx)) return aicb_fail(AICB_ERR_INVALID, "cube out of bounds");
-        if (new_ids[i] >= s->blocks.light_flags.size()) return aicb_fail(AICB_ERR_INVALID, "block id out of range");
+    std::vector<uint32_t> idx(n);
+    for (size_t i = 0; i < n; i++) {
+        const uint32_t dx = (uint32_t)(cubes[i][0] - ds.lo[0]), dy = (uint32_t)(cubes[i][1] - ds.lo[1]),
+                       dz = (uint32_t)(cubes[i][2] - ds.lo[2]);
+        if (dx >= (uint32_t)ds.size[0] || dy >= (uint32_t)ds.size[1] || dz >= (uint32_t)ds.size[2])
+            return aicb_fail(AICB_ERR_INVALID, "cube out of bounds");
+        if (new_ids[i] >= s->blocks.block_count()) return aicb_fail(AICB_ERR_INVALID, "block id out of range");
+        idx[i] = (dx * (uint32_t)ds.size[1] + dy) * (uint32_t)ds.size[2] + dz;
     }
-    for (size_t i = 0; i < n_edits; i++) {
-        uint32_t idx;
-        index_of(cubes[i][0], cubes[i][1], cubes[i][2], &idx);
-        if (s->h_ids[idx] == new_ids[i]) continue;  // Mutation::set of the same block changes nothing
-        s->h_ids[idx] = new_ids[i];
-        EditOp &o = op_of(idx);
-        o.cell = cell_word(new_ids[i], s->blocks.kind[new_ids[i]], ds.wide_cells);
-        const uint32_t fl = s->blocks.light_flags[new_ids[i]];
-        if ((fl & LB_ALL_OPAQUE) && !(fl & LB_EMISSIVE)) {  // opaque_for_light_computation
-            o.set_opaque = 1;
-            o.pending_op = 1;
-        } else {
-            o.pending_op = 2;
-        }
-        for (int f = 0; f < 6; f++) {
-            const int sgn = (f < 3) ? -1 : 1, a = f % 3;
-            uint32_t nidx;
-            if (!index_of(cubes[i][0] + (a == 0 ? sgn : 0), cubes[i][1] + (a == 1 ? sgn : 0), cubes[i][2] + (a == 2 ? sgn : 0), &nidx))
-                continue;
-            const int opp = (f < 3) ? f + 3 : f - 3;
-            if (!((s->blocks.light_flags[s->h_ids[nidx]] >> opp) & 1u)) op_of(nidx).pending_op = 2;
-        }
+    TRY(ensure_replicas(r));
+    if (n_changed) *n_changed = 0;
+    if (n == 0) return AICB_OK;
+    const size_t room = n * sizeof(EditEntry);
+    for (size_t k = 0; k < r.n; k++) {   // every replica's staging is free before any mirror changes
+        CU(cudaSetDevice(r.ctx[k]->device));
+        TRY(delta_room(r.ctx[k], room));
     }
-    if (!ops.empty()) {
-        std::vector<EditOp> flat;
-        flat.reserve(ops.size());
-        for (auto &kv : ops) flat.push_back(kv.second);
-        for (size_t i = 0; i < r.n; i++) {
-            aicb_scene *ri = r.scene[i];
-            if (i > 0)
-                for (const EditOp &o : flat)
-                    if (o.cell != 0xffffffffu) ri->h_ids[o.idx] = s->h_ids[o.idx];
-            CU(cudaSetDevice(ri->ctx->device));
-            cudaStream_t stream = ri->ctx->stream.get();
-            DeviceBuffer d_ops;
-            TRY(d_ops.ensure(flat.size() * sizeof(EditOp)));
-            CU(cudaMemcpyAsync(d_ops.get(), flat.data(), flat.size() * sizeof(EditOp), cudaMemcpyHostToDevice, stream));
-            LightParams P = light_params(r, i);
-            k_edits<<<(unsigned)((flat.size() + 127) / 128), 128, 0, stream>>>(P, d_ops.get<EditOp>(), (uint32_t)flat.size(),
-                                                                               ds.wide_cells, i == 0);
-            CU(cudaStreamSynchronize(stream));
-        }
-        CU(cudaSetDevice(s->ctx->device));
+    EditEntry *staged = r.ctx[0]->h_delta.get<EditEntry>();
+    uint32_t m = 0;
+    for (size_t i = 0; i < n; i++) {
+        if (s->h_ids[idx[i]] == new_ids[i]) continue;   // Mutation::set of the same block changes nothing
+        s->h_ids[idx[i]] = new_ids[i];
+        staged[m++] = EditEntry{idx[i], new_ids[i], 0};
     }
+    for (uint32_t k = 0; k < m; k++) staged[k].final_id = s->h_ids[staged[k].idx];
+    const size_t bytes = (size_t)m * sizeof(EditEntry);
+    for (size_t k = 0; m && k < r.n; k++) {
+        aicb_scene *sk = r.scene[k];
+        aicb_ctx *c = r.ctx[k];
+        cudaStream_t stream = c->stream.get();
+        CU(cudaSetDevice(c->device));
+        if (k > 0) {
+            std::memcpy(c->h_delta.get(), staged, bytes);
+            for (uint32_t e = 0; e < m; e++) sk->h_ids[staged[e].idx] = staged[e].final_id;
+        }
+        const EditEntry *d_entries = c->d_delta.get<const EditEntry>();
+        CU(cudaMemcpyAsync(c->d_delta.get(), c->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
+        const unsigned blocks = (m + 255) / 256;
+        if (sk->ds.wide_cells) k_edit_cells<true><<<blocks, 256, 0, stream>>>(sk->ds, d_entries, m);
+        else k_edit_cells<false><<<blocks, 256, 0, stream>>>(sk->ds, d_entries, m);
+        k_edit_light<<<blocks, 256, 0, stream>>>(light_params(r, k), d_entries, m, k == 0);
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(c->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
+    }
+    for (size_t k = 0; m && k < r.n; k++) {
+        CU(cudaSetDevice(r.ctx[k]->device));
+        CU(cudaStreamSynchronize(r.ctx[k]->stream.get()));
+    }
+    CU(cudaSetDevice(r.ctx[0]->device));
+    if (n_changed) *n_changed = m;
+    return AICB_OK;
+}
+
+// light_edit_cubes, then evaluate_light(epsilon).
+aicb_status light_edit_and_propagate(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n_edits,
+                                     uint8_t epsilon, uint64_t *updates_done, uint8_t *max_diff) {
+    TRY(light_edit_cubes(r, cubes, new_ids, n_edits, nullptr));
     return propagate(r, epsilon, updates_done, max_diff, nullptr);
 }
 
@@ -1957,6 +1962,11 @@ aicb_status aicb_light_edit_and_propagate(aicb_scene *s, const int32_t (*cubes)[
     return on_scene(s, [&](Replicas r) {
         return light_edit_and_propagate(r, cubes, new_ids, n_edits, epsilon, updates_done, max_diff);
     });
+}
+
+aicb_status aicb_light_edit_cubes(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n,
+                                  size_t *n_changed) {
+    return on_scene(s, [&](Replicas r) { return light_edit_cubes(r, cubes, new_ids, n, n_changed); });
 }
 
 aicb_status aicb_light_relight_blocks(aicb_scene *s, const uint16_t *indices, size_t n, uint8_t epsilon,

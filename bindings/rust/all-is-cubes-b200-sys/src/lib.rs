@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 15 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 16 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -327,6 +327,9 @@ unsafe extern "C" {
     // LightStorage::update_light_from_queue with a budget of cube updates: the light step of a tick
     pub fn aicb_light_update_from_queue(s: *mut aicb_scene, max_updates: u64, info_or_null: *mut aicb_light_updates_info)
                                         -> aicb_status;
+    // Mutation::set x n in list order, without propagation: a tick's SpaceChange::CubeBlock batch
+    pub fn aicb_light_edit_cubes(s: *mut aicb_scene, cubes: *const [i32; 3], new_ids: *const u16, n: usize,
+                                 n_changed_or_null: *mut usize) -> aicb_status;
     pub fn aicb_light_edit_and_propagate(s: *mut aicb_scene, cubes: *const [i32; 3], new_ids: *const u16, n_edits: usize,
                                          epsilon: u8, updates_done: *mut u64, max_diff: *mut u8) -> aicb_status;
     // Mutation::fill / fill_uniform(region): Mutation::set for every cube of a box, without propagation
@@ -358,6 +361,8 @@ unsafe extern "C" {
     pub fn aicb_group_light_edit_and_propagate(gs: *mut aicb_group_scene, cubes: *const [i32; 3], new_ids: *const u16,
                                                n_edits: usize, epsilon: u8, updates_done: *mut u64, max_diff: *mut u8)
                                                -> aicb_status;
+    pub fn aicb_group_light_edit_cubes(gs: *mut aicb_group_scene, cubes: *const [i32; 3], new_ids: *const u16, n: usize,
+                                       n_changed_or_null: *mut usize) -> aicb_status;
     pub fn aicb_group_light_edit_region(gs: *mut aicb_group_scene, region: *const aicb_aab, block_ids: *const u16,
                                         uniform_id: u16, n_changed_or_null: *mut usize) -> aicb_status;
     pub fn aicb_group_light_relight_blocks(gs: *mut aicb_group_scene, indices: *const u16, n: usize, epsilon: u8,

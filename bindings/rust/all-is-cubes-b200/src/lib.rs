@@ -199,6 +199,17 @@ impl SceneHandle {
         Ok(changed)
     }
 
+    fn light_edit_cubes(self, cubes: &[[i32; 3]], ids: &[u16]) -> Result<usize, B200Error> {
+        let mut changed = 0usize;
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_light_edit_cubes(s, cubes.as_ptr(), ids.as_ptr(), cubes.len(), &mut changed),
+                Self::Group(s) => sys::aicb_group_light_edit_cubes(s, cubes.as_ptr(), ids.as_ptr(), cubes.len(), &mut changed),
+            }
+        })?;
+        Ok(changed)
+    }
+
     fn destroy(self) {
         match self {
             Self::Single(s) => unsafe { sys::aicb_scene_destroy(s) },
@@ -460,6 +471,17 @@ impl B200Renderer {
     pub fn light_edit_world_region(&self, region: GridAab, fill: RegionFill<'_>) -> Result<usize, B200Error> {
         assert!(fill.fits(region), "array length is not the region's volume");
         self.world_scene()?.light_edit_region(&convert::aab_of(region), fill)
+    }
+
+    /// A tick's scattered `Mutation::set`s on a world scene whose light the library computes: `cubes[i]` takes block
+    /// index `ids[i]`, in list order, with `Mutation::set`'s light rule on the device and no propagation
+    /// (`aicb_light_edit_cubes`).  A cube may be named more than once.  Returns the number of entries that changed a
+    /// block, the `SpaceChange::CubeBlock`s the Space sends for the list; the light moves when the host asks for it
+    /// (`aicb_light_update_from_queue`).
+    pub fn light_edit_world_cubes(&self, cubes: &[Cube], ids: &[u16]) -> Result<usize, B200Error> {
+        assert_eq!(cubes.len(), ids.len(), "one block index per cube");
+        let cubes: Vec<[i32; 3]> = cubes.iter().map(|c| [c.x, c.y, c.z]).collect();
+        self.world_scene()?.light_edit_cubes(&cubes, ids)
     }
 
     /// Calls `single` with the layers this renderer holds as `aicb_layer`s, or on a group `group` with them as

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 15
+#define AICB_ABI_VERSION 16
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -548,9 +548,9 @@ typedef struct aicb_light_updates_info {
     uint8_t _pad[6];
 } aicb_light_updates_info;
 /* LightStorage::update_light_from_queue (space/light/updater.rs:180-290) with a budget of cube updates: the light step
- * of a tick (update_light_system, space/step.rs:341-369).  A host edits with aicb_light_edit_region (or the queue calls
- * below), calls this with the tick's budget, then takes the changed cubes; light converges over several ticks and no
- * tick stalls.  The call is synchronous and deterministic, and the library keeps no clock: a host with a time budget
+ * of a tick (update_light_system, space/step.rs:341-369).  A host edits with aicb_light_edit_cubes and
+ * aicb_light_edit_region (or the queue calls below), calls this with the tick's budget, then takes the changed cubes;
+ * light converges over several ticks and no tick stalls.  The call is synchronous and deterministic, and the library keeps no clock: a host with a time budget
  * turns it into a count, e.g. from aicb_light_stats' out[3] / out[0] of earlier steps.
  *   - Work: relaxation rounds on the queue, as aicb_light_evaluate runs them, until max_updates cube updates are made
  *     or the queue is empty.  info->update_count = min(max_updates, the updates the queue offered); a cube re-queued
@@ -567,6 +567,27 @@ typedef struct aicb_light_updates_info {
  *     aicb_light_stats reads as after aicb_light_evaluate, with out[0] == update_count.
  * AICB_ERR_INVALID, with nothing changed: a NULL scene or LightPhysics::None.  GPU test: tests/test_gpu_light_step.py. */
 aicb_status aicb_light_update_from_queue(aicb_scene *, uint64_t max_updates, aicb_light_updates_info *info_or_null);
+/* Mutation::set(cubes[i], new_ids[i]) for i = 0 .. n-1, in list order (space.rs:1346-1352 -> side_effects_of_set ->
+ * modified_cube_needs_update, space/light/updater.rs:135-173), on a scene whose light the library computes: the
+ * SpaceChange::CubeBlock batch of a tick.
+ *   - An entry is changing if its id differs from the block its cube holds at that point of the list (Mutation::set of
+ *     the same block changes nothing); a cube may be named any number of times.  The cells, the host mirror, the
+ *     texels, the queue and the set of changed cubes end byte for byte as the entries applied one by one leave them.
+ *   - Each changing entry applies the light rule: a block opaque for light stores OPAQUE, cancels the cube's queued
+ *     update and puts the cube into the set of changed cubes; any other block queues the cube at
+ *     Priority::NEWLY_VISIBLE; every in-bounds face neighbour whose own face toward the cube is not opaque is queued at
+ *     NEWLY_VISIBLE.  A cube set to an opaque block and back keeps its OPAQUE texel and is queued, as in the reference.
+ *   - *n_changed_or_null: the number of changing entries, the SpaceChange::CubeBlock the reference sends for the list.
+ *   - Nothing propagates: aicb_light_evaluate or aicb_light_update_from_queue follows when the host wants the light to
+ *     move.  aicb_light_stats is left as it was.
+ *   - The call is ordered like aicb_light_edit_region: behind the cube updates queued on the context, before any later
+ *     render, and it returns once its writes are done.  The rule runs on the device against the final cells.
+ * n == 0 changes nothing and reports 0.  AICB_ERR_INVALID, with nothing changed: NULL cubes or new_ids with n > 0, any
+ * cube out of bounds, an id >= the table's size, n >= 2^32, or LightPhysics::None.
+ * GPU test: tests/test_gpu_light_edit_cubes.py. */
+aicb_status aicb_light_edit_cubes(aicb_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n,
+                                  size_t *n_changed_or_null);
+/* aicb_light_edit_cubes, then Mutation::evaluate_light(epsilon) as aicb_light_evaluate runs it. */
 aicb_status aicb_light_edit_and_propagate(aicb_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                           size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                           uint8_t *max_diff);
@@ -634,8 +655,8 @@ aicb_status aicb_light_download_queue(aicb_scene *, uint8_t *priorities, size_t 
 aicb_status aicb_light_stats(const aicb_scene *, uint64_t out[4]);
 /* SpaceChange::CubeLight (space.rs:1079-1083): the set of cubes whose light texel the light calls wrote.  A cube enters
  * it when
- *   - aicb_light_edit_and_propagate sets it to a different block that is opaque for light, which stores OPAQUE even
- *     over OPAQUE (modified_cube_needs_update, space/light/updater.rs:153-161);
+ *   - aicb_light_edit_cubes (or aicb_light_edit_and_propagate) sets it to a different block that is opaque for light,
+ *     which stores OPAQUE even over OPAQUE (modified_cube_needs_update, space/light/updater.rs:153-161);
  *   - aicb_light_relight_blocks finds it holding a redefined block that is opaque for light (OPAQUE even over OPAQUE);
  *   - aicb_light_edit_region sets it to a different block that is opaque for light;
  *   - a relaxation round stores a value with difference_priority > 0 (apply_light_update, updater.rs:313-317);
@@ -706,6 +727,10 @@ aicb_status aicb_group_light_update_from_queue(aicb_group_scene *, uint64_t max_
 aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff);
+/* aicb_light_edit_cubes on the group: validated against replica 0 before any replica changes; every replica writes its
+ * own cells, its own host mirror and its own OPAQUE texels; device 0 alone queues and records the set. */
+aicb_status aicb_group_light_edit_cubes(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
+                                        size_t n, size_t *n_changed_or_null);
 /* aicb_light_relight_blocks on the group: the indices are checked against replica 0's table; every replica scans its
  * own cells and writes its own OPAQUE texels; device 0 alone queues and records the changed cubes. */
 aicb_status aicb_group_light_relight_blocks(aicb_group_scene *, const uint16_t *indices, size_t n, uint8_t epsilon,
