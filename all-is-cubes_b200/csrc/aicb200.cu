@@ -717,7 +717,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
                 switch (lc) {
                     case LC_NONE: CU(launch_after(overlap, shade_kernel<LC_NONE>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
                     case LC_FLAT: CU(launch_after(overlap, shade_kernel<LC_FLAT>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
-                    default: CU(launch_after(overlap, shade_kernel<LC_INTERP>, ctx->num_sms * SHADE_BLOCKS_PER_SM, 128, stream, P)); break;
+                    default: CU(launch_after(overlap, shade_kernel<LC_INTERP>, ctx->num_sms * SHADE_BLOCKS_PER_SM_INTERP, 128, stream, P)); break;
                 }
                 if (stage) cudaEventRecord(ctx->ev_k[3].get(), stream);
                 const uint32_t n_pixels = n / P.n_samples;
@@ -1531,6 +1531,17 @@ aicb_status aicb_ctx_stage_timing(aicb_ctx *c, int enable) {
     c->stage_timing = enable != 0;
     return AICB_OK;
 }
+
+#ifdef AICB_SHADE_PHASES
+// tools/shade_phases.py only (not in the header): copy the phase cycle sums of shade_hit<LC_INTERP> on the current
+// device to out[10], then zero them.
+int aicb_debug_shade_phases(unsigned long long *out) {
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (cudaMemcpyFromSymbol(out, aicb::g_shade_phase, sizeof(aicb::g_shade_phase)) != cudaSuccess) return -1;
+    const unsigned long long zero[10] = {};
+    return cudaMemcpyToSymbol(aicb::g_shade_phase, zero, sizeof zero) == cudaSuccess ? 0 : -1;
+}
+#endif
 
 void aicb_ctx_destroy(aicb_ctx *c) {
     if (!c) return;

@@ -41,6 +41,7 @@
 
 #ifdef __CUDACC__
 #include <cuda_fp16.h>
+#include "exact_math.cuh"
 #endif
 
 // The EvaluatedBlock members light reads (evaluated.rs:189-272), 128 bytes: light propagation's per-block record
@@ -368,11 +369,6 @@ AICB_DEV float zo_clamped(float v) {
     return 1.0f;
 }
 
-// f32 transcendentals: evaluate in f64, round once (<= 1 ULP from glibc's powf/expf). Out of line:
-// one copy of the f64 pow/exp code in the kernel.
-AICB_NOINLINE float powf_exact(float x, float y) { return (float)pow((double)x, (double)y); }
-AICB_NOINLINE float expf_exact(float x) { return (float)exp((double)x); }
-
 AICB_DEV bool tmax_valid(const Caster &c, const Ray &r) {  // valid_for_stepping (raycast.rs:563-570)
     const bool any_nan = (c.tmx != c.tmx) | (c.tmy != c.tmy) | (c.tmz != c.tmz);
     const bool any_fin = isfinite(c.tmx) | isfinite(c.tmy) | isfinite(c.tmz);
@@ -475,29 +471,6 @@ AICB_DEV bool caster_step(Caster &c, const Ray &r, int nx, int ny, int nz) {
     const int pos = ax ? c.rx : (ay ? c.ry : c.rz);
     const int lim = ax ? nx : (ay ? ny : nz);
     return (uint32_t)pos >= (uint32_t)lim;
-}
-
-// RaycastStep::intersection_point (raycast.rs:409-439) for the caster's current (un-stepped)
-// state (cube given in absolute coordinates of its level), against that level's ray origin.
-AICB_DEV void intersection_point(const Caster &c, const Ray &r, int cx, int cy, int cz, double ox, double oy, double oz,
-                                 double ip[3]) {
-    // select-based (the face axis differs between the lanes of the shading kernel)
-    const bool within = c.face == AICB_FACE_WITHIN;
-    const int fa = within ? -1 : (c.face - 1) % 3;
-    const double tm[3] = {c.tmx, c.tmy, c.tmz};
-    const double d[3] = {r.dx, r.dy, r.dz};
-    const double o[3] = {ox, oy, oz};
-    const int s[3] = {r.sx, r.sy, r.sz};
-    const int cu[3] = {cx, cy, cz};
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-        const double base = (double)cu[a];
-        const double off = (tm[a] - c.last_t) * d[a];
-        const double p_face = s[a] < 0 ? base + 1.0 : base;
-        const double p_other = base + ((s[a] > 0) ? (1.0 - rclamp01(off)) : rclamp01(-off));
-        const double p = (a == fa) ? p_face : (s[a] == 0 ? o[a] : p_other);
-        ip[a] = within ? o[a] : p;
-    }
 }
 
 // ---- light ---------------------------------------------------------------------------------------
@@ -1484,6 +1457,42 @@ AICB_DEV void decode_hit(const DeviceScene &S, const HitRecord &h, HitGeom &g) {
     g.pal = h.pal;
 }
 
+// RaycastStep::intersection_point (raycast.rs:409-439) of a hit, brought to Space coordinates (surface.rs:406-407):
+// axis `a`, from the caster state the record holds, against the ray of the level the surface is on (the ray scaled
+// into the block's voxel grid for an inner hit).  `ray` is the ray's origin and direction (RayRecordA's first six
+// doubles).  One axis at a time, so that one axis of the ray is live at a time; select-based, as the face axis differs
+// between the lanes of the shading kernel.
+AICB_DEV double hit_point_axis(const HitRecord &h, const HitGeom &g, const double *ray, uint32_t rflags, int a) {
+    const bool inner = (h.flags & 8u) != 0;
+    const double cube = (double)g.cube[a];
+    const double o = inner ? (__ldg(ray + a) - cube) * (double)g.res : __ldg(ray + a);
+    const double base = (double)(inner ? g.voxel[a] : g.cube[a]);
+    const double tm = a == 0 ? h.tmx : (a == 1 ? h.tmy : h.tmz);
+    const double off = (tm - h.last_t) * __ldg(ray + 3 + a);
+    const int s = (int)((rflags >> (6 + 2 * a)) & 3u) - 1;
+    const double p_face = s < 0 ? base + 1.0 : base;
+    const double p_other = base + ((s > 0) ? (1.0 - rclamp01(off)) : rclamp01(-off));
+    const bool within = g.face == AICB_FACE_WITHIN;
+    const double p = within ? o : (((g.face - 1) % 3 == a) ? p_face : (s == 0 ? o : p_other));
+    return inner ? p * recip_pow2(g.res) + cube : p;
+}
+
+#ifdef AICB_SHADE_PHASES
+// tools/shade_phases.py builds the library with this defined: clock64 cycles of the phases of shade_hit<LC_INTERP>,
+// summed over a frame's hits (SHADE_PHASE_NAMES there).  The build the library ships has no trace of it.
+__device__ unsigned long long g_shade_phase[10];
+#define SHADE_PHASE(k)                                                                                                 \
+    do {                                                                                                               \
+        if constexpr (LC == LC_INTERP) {                                                                               \
+            const long long t_ = clock64();                                                                            \
+            ph_[k] = t_ - t0_;                                                                                         \
+            t0_ = t_;                                                                                                  \
+        }                                                                                                              \
+    } while (0)
+#else
+#define SHADE_PHASE(k) do {} while (0)
+#endif
+
 // One hit record -> its ShadedHit (returned, not stored: resolve_kernel keeps it in shared memory, shade_kernel and
 // bounce_resolve_kernel store it).  `illum_override` (LC_BOUNCE only): the illumination gathered by the hit's
 // secondary rays; without it a Bounce frame lights the surface like Flat (surface.rs:171-176) and marks fully opaque
@@ -1495,6 +1504,15 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
     const bool volumetric = P.transparency == AICB_TRANSPARENCY_VOLUMETRIC;
     const bool have_fog = (P.fog != AICB_FOG_NONE) && P.include_sky;
     const float fog_blend = (P.fog == AICB_FOG_ABRUPT) ? 1.0f : (P.fog == AICB_FOG_COMPROMISE ? 0.5f : 0.0f);
+#ifdef AICB_SHADE_PHASES
+    long long ph_[7] = {0, 0, 0, 0, 0, 0, 0}, t0_ = clock64();
+    struct Flush {
+        long long *ph;
+        __device__ ~Flush() {
+            for (int k = 0; k < 7; k++) atomicAdd(&g_shade_phase[k], (unsigned long long)ph[k]);
+        }
+    } flush_{ph_};
+#endif
     HitRecord h;
     {
         const uint4 *src = reinterpret_cast<const uint4 *>(P.hits + i);
@@ -1508,13 +1526,6 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
     const float4 emi = __ldg(S.palette + 2 * (size_t)h.pal + 1);
     const uint2 rmeta = __ldg(reinterpret_cast<const uint2 *>(&rp->t_to_view));   // t_to_view, flags
     const uint32_t rflags = rmeta.y;
-    Ray rr;
-    rr.ox = rr.oy = rr.oz = rr.dx = rr.dy = rr.dz = 0.0;
-    if constexpr (LC == LC_INTERP) {
-        const double2 *q = reinterpret_cast<const double2 *>(rp);
-        const double2 q0 = __ldg(q), q1 = __ldg(q + 1), q2 = __ldg(q + 2);
-        rr.ox = q0.x; rr.oy = q0.y; rr.oz = q1.x; rr.dx = q1.y; rr.dy = q2.x; rr.dz = q2.y;
-    }
     ShadedHit out;
     out.r = out.g = out.b = 0.0f;
     out.factor = -1.0f;
@@ -1522,8 +1533,10 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
     out.steps = h.steps;
     out._pad[0] = out._pad[1] = 0;
     if (h.thickness < 0.0f) return out;   // an unused slot: skipped
+    SHADE_PHASE(0);
     HitGeom g;
     decode_hit(S, h, g);
+    SHADE_PHASE(1);
     float ca = col.w;
     float coeff = 1.0f;
     bool zeroed = false;
@@ -1538,12 +1551,15 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
             ca = 0.0f; coeff = thickness;   // 1^thickness == 1 exactly
         } else {
             const float unit_t = 1.0f - col.w;
-            const float depth_t = powf_exact(unit_t, thickness);
+            // the short path pays where the kernel's occupancy is its register count (LC_INTERP); resolve_kernel's
+            // None / Flat frames measured 1.3 % slower with it inlined, so they keep the call
+            const float depth_t = LC == LC_INTERP ? powf_exact(unit_t, thickness) : powf_libm(unit_t, thickness);
             ca = zo_clamped(1.0f - depth_t);
             const float k = (unit_t == 1.0f) ? thickness : (depth_t - 1.0f) / (unit_t - 1.0f);
             coeff = fmaxf(k, 0.0f);
         }
     }
+    SHADE_PHASE(2);
     const float kc = ps_clamped(coeff);
     const float er = volumetric ? ps_mul(emi.x, kc) : emi.x, eg = volumetric ? ps_mul(emi.y, kc) : emi.y,
                 eb = volumetric ? ps_mul(emi.z, kc) : emi.z;
@@ -1557,12 +1573,13 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
     if (have_fog) {  // distance_fog (sr.rs:745-768)
         float rel = (float)(h.last_t * t_scale) * __uint_as_float(rmeta.x);
         rel = rel < 0.0f ? 0.0f : (rel > 1.0f ? 1.0f : rel);
-        const float fog_exponential = 1.0f - expf_exact(-1.6f * rel);
+        const float fog_exponential = 1.0f - (LC == LC_INTERP ? expf_exact(-1.6f * rel) : expf_libm(-1.6f * rel));
         const float fudged = fog_exponential / 0.79810348f;
         const float p4 = (rel * rel) * (rel * rel);
         fa = zo_clamped(fudged * (1.0f - fog_blend) + p4 * fog_blend);
         tr = tr * (1.0f - fa);
     }
+    SHADE_PHASE(3);
     const float cr = zeroed ? 0.0f : col.x, cg = zeroed ? 0.0f : col.y, cb = zeroed ? 0.0f : col.z;
     float i0 = 1.0f, i1 = 1.0f, i2 = 1.0f;
     const int face = g.face;
@@ -1584,26 +1601,17 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
         texels += tx;
         i0 = s_lut[t & 255]; i1 = s_lut[(t >> 8) & 255]; i2 = s_lut[(t >> 16) & 255];
     } else if constexpr (LC == LC_INTERP) {
-        // RaycastStep::intersection_point (raycast.rs:409-439) of the level the surface is on, brought to
-        // Space coordinates (surface.rs:406-407)
-        rr.sx = (int)((rflags >> 6) & 3u) - 1; rr.sy = (int)((rflags >> 8) & 3u) - 1; rr.sz = (int)((rflags >> 10) & 3u) - 1;
-        Caster c;
-        c.tmx = h.tmx; c.tmy = h.tmy; c.tmz = h.tmz; c.last_t = h.last_t;
-        c.face = face;
+        // the ray's origin and direction are read here, not with the record: loaded up front they stayed live
+        // through the transmittance and fog and cost the kernel its occupancy
+        const double *ray = reinterpret_cast<const double *>(rp);
         double ip[3];
-        if (!(h.flags & 8u)) {
-            intersection_point(c, rr, g.cube[0], g.cube[1], g.cube[2], rr.ox, rr.oy, rr.oz, ip);
-        } else {
-            const double fres = (double)g.res;
-            intersection_point(c, rr, g.voxel[0], g.voxel[1], g.voxel[2], (rr.ox - (double)g.cube[0]) * fres,
-                               (rr.oy - (double)g.cube[1]) * fres, (rr.oz - (double)g.cube[2]) * fres, ip);
-            ip[0] = ip[0] * t_scale + (double)g.cube[0];
-            ip[1] = ip[1] * t_scale + (double)g.cube[1];
-            ip[2] = ip[2] * t_scale + (double)g.cube[2];
-        }
+#pragma unroll
+        for (int a = 0; a < 3; a++) ip[a] = hit_point_axis(h, g, ray, rflags, a);
+        SHADE_PHASE(4);
         uint32_t tx = 0;
         float il[3];
         interpolated_light(S, s_lut, P.lighting, g.cube[0], g.cube[1], g.cube[2], face, ip[0], ip[1], ip[2], il, &tx);
+        SHADE_PHASE(5);
         i0 = il[0]; i1 = il[1]; i2 = il[2];
         texels += tx;
     }
@@ -1618,6 +1626,7 @@ AICB_DEV ShadedHit shade_hit(const TraceParams &P, const float *s_lut, const uin
         ob = ps_mul(ob, comp) + ps_mul(S.sky_colors[k][2], fa);
     }
     out.r = orr; out.g = og; out.b = ob; out.factor = tr;
+    SHADE_PHASE(6);
     return out;
 }
 
@@ -1642,8 +1651,10 @@ AICB_DEV void store_shaded(const TraceParams &P, const uint32_t i, const ShadedH
 // power limit): 0.236 ms against 0.27 ms for 8 blocks per SM at 90 registers, of which 5 were resident and 3 ran as a
 // second wave.
 constexpr int SHADE_BLOCKS_PER_SM = 6;
+constexpr int SHADE_BLOCKS_PER_SM_INTERP = 8;
+template <int LC> constexpr int shade_blocks_per_sm() { return LC == LC_INTERP ? SHADE_BLOCKS_PER_SM_INTERP : SHADE_BLOCKS_PER_SM; }
 template <int LC>
-__global__ void __launch_bounds__(128, SHADE_BLOCKS_PER_SM) shade_kernel(const __grid_constant__ TraceParams P) {
+__global__ void __launch_bounds__(128, shade_blocks_per_sm<LC>()) shade_kernel(const __grid_constant__ TraceParams P) {
     __shared__ float s_lut[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_lut[i] = P.scene.tables[i];
     grid_dependency_sync();
@@ -1652,7 +1663,22 @@ __global__ void __launch_bounds__(128, SHADE_BLOCKS_PER_SM) shade_kernel(const _
     uint32_t n = *P.hit_counter;
     if (n > P.hit_capacity) n = P.hit_capacity;
     unsigned long long texels = 0;
+#ifdef AICB_SHADE_PHASES
+    auto shade_one = [&](const uint32_t i) {
+        const long long t0 = clock64();
+        const ShadedHit sh = shade_hit<LC>(P, s_lut, i, nullptr, texels);
+        const long long t1 = clock64();
+        store_shaded(P, i, sh);
+        const long long t2 = clock64();
+        if (LC == LC_INTERP) {
+            atomicAdd(&g_shade_phase[7], (unsigned long long)(t2 - t1));
+            atomicAdd(&g_shade_phase[8], (unsigned long long)(t2 - t0));
+            atomicAdd(&g_shade_phase[9], 1ull);
+        }
+    };
+#else
     auto shade_one = [&](const uint32_t i) { store_shaded(P, i, shade_hit<LC>(P, s_lut, i, nullptr, texels)); };
+#endif
 
     // The hit stream holds slots that are never shaded: the unused tail of each lane's last chunk.  Each warp scans its
     // slots 32 at a time, passes over the dead ones, and queues the live ones until it has 32 of them to shade
@@ -1785,26 +1811,11 @@ static __global__ void __launch_bounds__(128) bounce_gen_kernel(const __grid_con
         for (int k = 0; k < 4; k++) dst[k] = src[k];
     }
     const RayRecordA *rp = P.rays_a + P.ray_index[i];
-    Ray rr;
-    rr.ox = rp->ox; rr.oy = rp->oy; rr.oz = rp->oz; rr.dx = rp->dx; rr.dy = rp->dy; rr.dz = rp->dz;
-    const uint32_t rflags = rp->flags;
-    rr.sx = (int)((rflags >> 6) & 3u) - 1; rr.sy = (int)((rflags >> 8) & 3u) - 1; rr.sz = (int)((rflags >> 10) & 3u) - 1;
     HitGeom g;
     decode_hit(S, h, g);
-    Caster c;
-    c.tmx = h.tmx; c.tmy = h.tmy; c.tmz = h.tmz; c.last_t = h.last_t;
-    c.face = g.face;
     double ip[3];
-    if (!(h.flags & 8u)) {
-        intersection_point(c, rr, g.cube[0], g.cube[1], g.cube[2], rr.ox, rr.oy, rr.oz, ip);
-    } else {
-        const double fres = (double)g.res, t_scale = recip_pow2(g.res);
-        intersection_point(c, rr, g.voxel[0], g.voxel[1], g.voxel[2], (rr.ox - (double)g.cube[0]) * fres,
-                           (rr.oy - (double)g.cube[1]) * fres, (rr.oz - (double)g.cube[2]) * fres, ip);
-        ip[0] = ip[0] * t_scale + (double)g.cube[0];
-        ip[1] = ip[1] * t_scale + (double)g.cube[1];
-        ip[2] = ip[2] * t_scale + (double)g.cube[2];
-    }
+#pragma unroll
+    for (int a = 0; a < 3; a++) ip[a] = hit_point_axis(h, g, reinterpret_cast<const double *>(rp), rp->flags, a);
     double nrm[3] = {0.0, 0.0, 0.0};
     if (g.face != AICB_FACE_WITHIN) nrm[(g.face - 1) % 3] = g.face >= AICB_FACE_PX ? 1.0 : -1.0;
     unsigned long long st[4];
