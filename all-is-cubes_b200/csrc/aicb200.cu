@@ -141,8 +141,9 @@ static bool voxel_invisible(const aicb_voxel &v) {
 }
 
 // TracingBlock::from_block (sr.rs:579-587) for one block definition: its 32-byte record, classification, brick words
-// and palette entries (appended to `bricks` / `palette`; the record's offsets are relative to those vectors), plus
-// what the marching kernel needs of each surface: {alpha, an upper bound of log2(1 - alpha)} per palette entry.
+// in the wide form (trace_kernel.cuh) and palette entries (appended to `bricks` / `palette`; the record's offsets are
+// relative to those vectors), plus what the marching kernel needs of each surface: {alpha, an upper bound of
+// log2(1 - alpha)} per palette entry.
 // Called by flatten_blocks alone.
 static const aicb_voxel AIR_VOXEL = {{0, 0, 0, 0}, {0, 0, 0}, 0};
 
@@ -169,7 +170,7 @@ static float4 block_entry(uint8_t kind, uint32_t pal_off, const std::vector<floa
     return make_float4(e.x, e.y, palf, 0.0f);
 }
 
-static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t &kind, std::vector<uint16_t> &bricks,
+static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t &kind, std::vector<uint32_t> &bricks,
                                  std::vector<float4> &palette, std::vector<float2> &pal_tab) {
     std::memset(&r, 0, sizeof r);
     const uint32_t res = b.resolution;
@@ -215,7 +216,9 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
         r.vsize[0] = r.vsize[1] = r.vsize[2] = 1;
         push_voxel(sv);
     } else {
-        if (b.n_palette > 32768) return fail(AICB_ERR_UNSUPPORTED, "block palettes above 32768 entries are not supported");
+        if (b.n_palette > 65536)
+            return fail(AICB_ERR_UNSUPPORTED, "block palettes above 65536 entries are not supported: a voxel's palette "
+                                              "index (VoxelIndex) is 16 bits");
         kind = KIND_RECURSIVE;
         r.kind_res = KIND_RECURSIVE | (res << 8);
         for (int a = 0; a < 3; a++) {
@@ -226,8 +229,8 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
         r.brick_off = (uint32_t)bricks.size();
         r.pal_off = (uint32_t)(palette.size() / 2);
         for (size_t k = 0; k < b.n_indices; k++) {
-            uint16_t v = b.indices[k];
-            bricks.push_back((uint16_t)(v | (voxel_invisible(b.palette[v]) ? 0x8000u : 0u)));
+            const uint32_t v = b.indices[k];
+            bricks.push_back(v << 16 | (voxel_invisible(b.palette[v]) ? 0x8000u : 0u));
         }
         for (size_t k = 0; k < b.n_palette; k++) push_voxel(b.palette[k]);
     }
@@ -239,15 +242,20 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
 // ---------------------------------------------------------------------------------------------
 typedef void (*kernel_fn)(const TraceParams, uint32_t);
 
-template <bool V, bool W, bool AUX>
+template <bool V, bool W, bool AUX, bool B>
 static kernel_fn kernel_of() {
-    return trace_kernel<V, W, AUX>;
+    return trace_kernel<V, W, AUX, B>;
 }
 
-static kernel_fn select_kernel(bool volumetric, bool wide, bool aux) {
-#define PICK(V, W, A) if (volumetric == V && wide == W && aux == A) return kernel_of<V, W, A>();
-    PICK(false, false, false) PICK(false, false, true) PICK(false, true, false) PICK(false, true, true)
-    PICK(true, false, false) PICK(true, false, true) PICK(true, true, false) PICK(true, true, true)
+// The marching kernel of a frame: Volumetric transparency, u32 cells, the step counters (render_aux), u32 brick words.
+static kernel_fn select_kernel(bool volumetric, bool wide, bool aux, bool wide_bricks) {
+#define PICK(V, W, A, B) if (volumetric == V && wide == W && aux == A && wide_bricks == B) return kernel_of<V, W, A, B>();
+    PICK(false, false, false, false) PICK(false, false, true, false) PICK(false, true, false, false)
+    PICK(false, true, true, false) PICK(true, false, false, false) PICK(true, false, true, false)
+    PICK(true, true, false, false) PICK(true, true, true, false)
+    PICK(false, false, false, true) PICK(false, false, true, true) PICK(false, true, false, true)
+    PICK(false, true, true, true) PICK(true, false, false, true) PICK(true, false, true, true)
+    PICK(true, true, false, true) PICK(true, true, true, true)
 #undef PICK
     return nullptr;
 }
@@ -301,6 +309,27 @@ static __global__ void __launch_bounds__(256) widen_cells_kernel(const uint16_t 
                           widened_cell(v.w >> 16)));
     }
     for (size_t i = n8 * 8 + first; i < n; i += stride) out[i] = widened_cell(in[i]);
+}
+
+// A narrow brick word (index | invisible << 15) in the wide form (index << 16 | invisible << 15).
+static __device__ __forceinline__ uint32_t widened_brick(uint32_t w) { return (w & 0x7fffu) << 16 | (w & 0x8000u); }
+
+// A scene's brick pool from u16 to u32 words (a block with more than 32768 palette entries placed): one streaming
+// pass, as widen_cells_kernel.
+static __global__ void __launch_bounds__(256) widen_bricks_kernel(const uint16_t *__restrict__ in,
+                                                                  uint32_t *__restrict__ out, size_t n) {
+    const size_t stride = (size_t)gridDim.x * blockDim.x, first = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t n8 = n / 8;
+    for (size_t i = first; i < n8; i += stride) {
+        const uint4 v = __ldcs(reinterpret_cast<const uint4 *>(in) + i);
+        __stcs(reinterpret_cast<uint4 *>(out) + 2 * i,
+               make_uint4(widened_brick(v.x & 0xffffu), widened_brick(v.x >> 16), widened_brick(v.y & 0xffffu),
+                          widened_brick(v.y >> 16)));
+        __stcs(reinterpret_cast<uint4 *>(out) + 2 * i + 1,
+               make_uint4(widened_brick(v.z & 0xffffu), widened_brick(v.z >> 16), widened_brick(v.w & 0xffffu),
+                          widened_brick(v.w >> 16)));
+    }
+    for (size_t i = n8 * 8 + first; i < n; i += stride) out[i] = widened_brick(in[i]);
 }
 
 // Every u16 cell of a scene set to one word (Mutation::fill_uniform over the whole Space): one 16-byte streaming store
@@ -425,7 +454,8 @@ static __global__ void __launch_bounds__(256) k_region_texels(const DeviceScene 
 }
 
 // One run of a pool compaction (compact_pools): `bytes` bytes from byte `src` of the old pool to byte `dst` of the new
-// one.  Offsets and lengths are even (a u16 brick word is a pool's smallest element).
+// one.  Offsets and lengths are even (a u16 brick word is a pool's smallest element; u32 brick words, float2 and
+// float4 are multiples of it).
 struct PoolSegment {
     uint64_t src, dst, bytes;
 };
@@ -433,8 +463,8 @@ struct PoolSegment {
 // Gathers a pool's live runs into a new buffer: blocks take segments in a grid-stride loop.  Within a segment, every
 // 16-byte chunk of the destination that it covers whole is one coalesced 16-byte store, assembled from the one or two
 // aligned 16-byte source chunks that hold its bytes (a funnel shift when the run moves by other than a multiple of 16
-// bytes).  The at most seven u16 words at either end, whose chunk a neighbouring segment shares, are stored one at a
-// time.  Both buffers are multiples of 16 bytes (grow_buffer, compact_pools), so an aligned source chunk that holds one
+// bytes).  The at most seven u16 halves of words at either end, whose chunk a neighbouring segment shares, are stored
+// one at a time, whatever the pool's element size.  Both buffers are multiples of 16 bytes (grow_buffer, compact_pools), so an aligned source chunk that holds one
 // byte of a run lies inside the old buffer.
 static __global__ void __launch_bounds__(256) compact_pool_kernel(const uint8_t *__restrict__ src, uint8_t *__restrict__ dst,
                                                                   const PoolSegment *__restrict__ segs, uint32_t n_segs) {
@@ -682,7 +712,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.bin_count = Q.task_counter + 4;
             Q.debug_warp_times = nullptr;
         }
-        kernel_fn k = select_kernel(volumetric, sc->ds.wide_cells != 0, out.aux);
+        kernel_fn k = select_kernel(volumetric, sc->ds.wide_cells != 0, out.aux, sc->blocks.wide_bricks);
         int blocks_per_sm = 0;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k, WARPS_PER_BLOCK * 32, 0));
         if (blocks_per_sm < 1) blocks_per_sm = 1;
@@ -862,14 +892,20 @@ struct Retired {
 };
 
 // Block definitions flattened against a table: per definition its record (brick_off / pal_off already offsets into the
-// table's pools) and extents, blk_tab entry, kind and light record; and the voxel data they append to the pools.
+// table's pools) and extents, blk_tab entry, kind and light record; and the voxel data they append to the pools.  The
+// brick words are in the form the table's pool has once they are placed: wide if it is wide already or if a palette
+// has more than 32768 entries.
 struct FlatBlocks {
     std::vector<BlockRec> recs;
     std::vector<BlockTable::Extent> extents;
     std::vector<float4> blk_tab;
     std::vector<uint8_t> kinds;
     std::vector<LightBlockDev> light;
-    std::vector<uint16_t> bricks;
+    bool wide_bricks = false;
+    std::vector<uint32_t> bricks;      // the words in the wide form (flatten_block); their count in either form
+    std::vector<uint16_t> narrow;      // the words in the narrow form, unless wide_bricks
+    size_t brick_word_bytes() const { return wide_bricks ? 4 : 2; }
+    const void *brick_words() const { return wide_bricks ? (const void *)bricks.data() : narrow.data(); }
     std::vector<float4> palette;
     std::vector<float2> pal_tab;
 };
@@ -897,6 +933,12 @@ static aicb_status flatten_blocks(const BlockTable &t, const aicb_block_desc *de
         f->extents[i] = {r.brick_off, (uint32_t)(f->bricks.size() - bricks_before), r.pal_off,
                          (uint32_t)(f->pal_tab.size() - pal_before)};
         f->light[i] = light_block(descs[i]);
+        if (f->kinds[i] == KIND_RECURSIVE && descs[i].n_palette > 32768) f->wide_bricks = true;
+    }
+    if (t.wide_bricks) f->wide_bricks = true;
+    if (!f->wide_bricks) {
+        f->narrow.resize(f->bricks.size());
+        for (size_t k = 0; k < f->bricks.size(); k++) f->narrow[k] = (uint16_t)(f->bricks[k] >> 16 | (f->bricks[k] & 0x8000u));
     }
     // live data only: the dead part of the pool is compacted away before it could push positions past 2^32
     // (flatten_placeable)
@@ -905,19 +947,40 @@ static aicb_status flatten_blocks(const BlockTable &t, const aicb_block_desc *de
     return AICB_OK;
 }
 
-// Places `f` (flattened against s's table) in s's table: the voxel data appended to the pools; the per-id records
-// appended (indices == nullptr) or written at `indices`, where a repeated index keeps its last definition.  Every copy
-// is queued on the context's stream, and the scene's pointers follow every array that moved, whatever fails later.
+// A narrow brick pool as a wide one, with room for `add` more words: its words re-encoded on the device into a new
+// buffer (grow_buffer's size rule, in words), queued on the context's stream; the old buffer goes to `retired`.
+static aicb_status widen_bricks(aicb_scene *s, size_t add, Retired &retired) {
+    BlockTable &t = s->blocks;
+    DeviceBuffer wide;
+    TRY(wide.ensure(std::max(round16((t.n_bricks + add) * 4), 2 * t.bricks.bytes())));
+    if (t.n_bricks) {
+        const size_t want = (std::max<size_t>(t.n_bricks / 8, 1) + 255) / 256, cap = (size_t)s->ctx->num_sms * 16;
+        widen_bricks_kernel<<<(unsigned)std::min(want, cap), 256, 0, s->ctx->stream.get()>>>(
+            t.bricks.get<const uint16_t>(), wide.get<uint32_t>(), t.n_bricks);
+        CU(cudaGetLastError());
+    }
+    if (t.bricks) retired.bufs.push_back(std::move(t.bricks));
+    t.bricks = std::move(wide);
+    t.wide_bricks = true;
+    return AICB_OK;
+}
+
+// Places `f` (flattened against s's table) in s's table: a narrow brick pool widened first if `f` is wide; the voxel
+// data appended to the pools; the per-id records appended (indices == nullptr) or written at `indices`, where a
+// repeated index keeps its last definition.  Every copy is queued on the context's stream, and the scene's pointers
+// follow every array that moved, whatever fails later.
 static aicb_status place(aicb_scene *s, const FlatBlocks &f, const uint16_t *indices, Retired &retired) {
     BlockTable &t = s->blocks;
     cudaStream_t stream = s->ctx->stream.get();
     const size_t n = f.kinds.size(), count = t.block_count(), added = indices ? 0 : n;
     aicb_status st = AICB_OK;
+    if (f.wide_bricks && !t.wide_bricks) st = widen_bricks(s, f.bricks.size(), retired);
+    const size_t wb = t.brick_word_bytes();
     auto room = [&](DeviceBuffer &b, size_t used, size_t add) {
         if (st == AICB_OK && add) st = grow_buffer(b, used, used + add, stream, &retired.bufs);
     };
     room(t.blocks, count * sizeof(BlockRec), added * sizeof(BlockRec));
-    room(t.bricks, t.n_bricks * 2, f.bricks.size() * 2);
+    room(t.bricks, t.n_bricks * wb, f.bricks.size() * wb);
     room(t.palette, t.n_palette * sizeof(float4), f.palette.size() * sizeof(float4));
     room(t.pal_tab, t.n_palette / 2 * sizeof(float2), f.pal_tab.size() * sizeof(float2));
     room(t.blk_tab, count * sizeof(float4), added * sizeof(float4));
@@ -928,7 +991,7 @@ static aicb_status place(aicb_scene *s, const FlatBlocks &f, const uint16_t *ind
         if (bytes) CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
         return AICB_OK;
     };
-    TRY(put(t.bricks.get<uint16_t>() + t.n_bricks, f.bricks.data(), f.bricks.size() * 2));
+    TRY(put(t.bricks.get<char>() + t.n_bricks * wb, f.brick_words(), f.bricks.size() * wb));
     TRY(put(t.palette.get<float4>() + t.n_palette, f.palette.data(), f.palette.size() * sizeof(float4)));
     TRY(put(t.pal_tab.get<float2>() + t.n_palette / 2, f.pal_tab.data(), f.pal_tab.size() * sizeof(float2)));
     // the per-id records: one run of n at the end of the table, or one record at each index, in order
@@ -997,11 +1060,12 @@ static aicb_status compact_pools(aicb_scene *s, bool bricks, bool palette, Retir
         return live;
     };
     std::vector<std::pair<size_t, size_t>> ranges;   // per buffer gathered: its segments in `segs`
-    const size_t live_bricks = bricks ? plan(&BlockTable::Extent::brick_off, &BlockTable::Extent::n_bricks, {2}, &ranges) : 0;
+    const size_t wb = t.brick_word_bytes();
+    const size_t live_bricks = bricks ? plan(&BlockTable::Extent::brick_off, &BlockTable::Extent::n_bricks, {wb}, &ranges) : 0;
     const size_t live_pal = palette ? plan(&BlockTable::Extent::pal_off, &BlockTable::Extent::n_pal,
                                            {2 * sizeof(float4), sizeof(float2)}, &ranges) : 0;
     DeviceBuffer new_bricks, new_palette, new_pal_tab, d_segs, d_off;
-    if (bricks) TRY(new_bricks.ensure(round16(live_bricks * 2)));
+    if (bricks) TRY(new_bricks.ensure(round16(live_bricks * wb)));
     if (palette) {
         TRY(new_palette.ensure(live_pal * 2 * sizeof(float4)));
         TRY(new_pal_tab.ensure(round16(live_pal * sizeof(float2))));

@@ -229,29 +229,36 @@ struct aicb_ctx {
 // data after every call, and each dead element is copied O(1) times, amortised.  A frame's hit records hold absolute
 // pool positions, so a compaction runs only once nothing on the context can read the pools (wait_context), as
 // aicb_scene_update_blocks waits anyway.
+//
+// The brick pool holds one word per voxel in one of two forms (trace_kernel.cuh, BRICK_WIDE): u16 words while every
+// block's palette has at most 32768 entries, u32 words once a block with more is placed (wide_bricks).  A pool widens
+// in place (widen_bricks_kernel) and stays wide until fill_uniform replaces the table.  Positions and lengths in the
+// pool are counted in words of either form.
 struct BlockTable {
     struct Extent {
-        uint32_t brick_off, n_bricks;   // u16 words of the brick pool
+        uint32_t brick_off, n_bricks;   // words of the brick pool
         uint32_t pal_off, n_pal;        // palette entries (two float4 each, and one pal_tab pair)
     };
 
     DeviceBuffer blocks;    // per block id: BlockRec
     DeviceBuffer blk_tab;   // per block id: the pal_tab pair and the palette entry of single-voxel blocks
     DeviceBuffer light;     // per block id: LightBlockDev (light propagation)
-    DeviceBuffer bricks;    // u16 voxel words of the recursive blocks
+    DeviceBuffer bricks;    // voxel words of the recursive blocks: u16, or u32 if wide_bricks
     DeviceBuffer palette;   // two float4 per palette entry
     DeviceBuffer pal_tab;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
     std::vector<uint8_t> kind;           // per block id: its kind, which its cubes' cell words carry
     std::vector<uint32_t> light_flags;   // per block id: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission
     std::vector<Extent> extent;          // per block id: its voxel data in the pools
-    size_t n_bricks = 0, n_palette = 0;  // u16 words, float4s
-    size_t dead_bricks = 0, dead_pal = 0;   // of those, u16 words and palette entries no id's extent holds
+    size_t n_bricks = 0, n_palette = 0;  // brick words, float4s
+    size_t dead_bricks = 0, dead_pal = 0;   // of those, brick words and palette entries no id's extent holds
+    bool wide_bricks = false;
 
     size_t block_count() const { return kind.size(); }
+    size_t brick_word_bytes() const { return wide_bricks ? 4 : 2; }
     // what aicb_scene_device_bytes counts of the table: the per-id records and the pools' elements in use, live or dead
     size_t bytes() const {
-        return block_count() * (sizeof(aicb::BlockRec) + sizeof(float4) + sizeof(LightBlockDev)) + n_bricks * 2 +
-               n_palette * sizeof(float4) + n_palette / 2 * sizeof(float2);
+        return block_count() * (sizeof(aicb::BlockRec) + sizeof(float4) + sizeof(LightBlockDev)) +
+               n_bricks * brick_word_bytes() + n_palette * sizeof(float4) + n_palette / 2 * sizeof(float2);
     }
     // the scene's pointers into the current buffers (LightParams::blocks is read from `light` by light_params)
     void bind(aicb::DeviceScene &ds) const {

@@ -58,6 +58,9 @@ namespace aicb {
 // ---- device-side scene -------------------------------------------------------------------------
 // The kind sits in the top two bits of a u16 cell so that bit 15 means "nothing to see here" on both levels
 // (brick words carry the same flag): the marching loop tests one bit.
+// A brick word is a voxel's palette index (from its block's pal_off) with that flag, in one of two forms per scene:
+// narrow, u16 = index | invisible<<15, while every palette has at most 32768 entries; wide, u32 = index<<16 |
+// invisible<<15, for palettes of up to 65536 entries (VoxelIndex is u16).  trace_kernel's BRICK_WIDE reads the wide form.
 constexpr uint32_t KIND_SINGLE = 0;     // Evoxels::One, visible
 constexpr uint32_t KIND_RECURSIVE = 1;  // paletted brick
 constexpr uint32_t KIND_INVISIBLE = 2;  // AIR, or a single voxel that is fully transparent + non-emissive
@@ -79,7 +82,7 @@ struct DeviceScene {
     const void *cells;          // u16 (id | kind<<14) or u32 (id | kind<<16), Z-major
     const uint32_t *light;      // PackedLight texels r|g<<8|b<<16|status<<24, or nullptr (== ONE)
     const BlockRec *blocks;
-    const uint16_t *bricks;     // palette index | invisible<<15
+    const uint16_t *bricks;     // brick words: palette index | invisible<<15, or (wide pool) u32 index<<16 | invisible<<15
     const float4 *palette;      // 2 x float4 per entry: rgba, emission
     const float4 *blk_tab;      // per block id (single-voxel blocks): {alpha, upper bound of log2(1 - alpha), palette entry (bits), -}
     const float2 *pal_tab;      // per palette entry: {alpha, log2 bound} (what the marching kernel needs of a surface)
@@ -947,14 +950,15 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
 // One iteration of the hot loop is, for every marching lane (no divergent branch up to the surface case):
 //   State::step (raycast.rs:577-626)           select the axis with the smallest t_max, add t_delta, move the index
 //   bounds (raycast.rs:265-274)                per-axis counters of the steps left inside the level: one sign test
-//   SurfaceIter / VoxelSurfaceIter lookup      one dependent 2-byte load; bit 15 = nothing to see
+//   SurfaceIter / VoxelSurfaceIter lookup      one dependent 2-byte load (4 bytes in a wide brick pool); bit 15 = nothing to see
 //   count_step_should_stop (sr.rs:625-656)     step counter, log-domain upper bound of the transmittance
 //   DepthIter span end (surface.rs:460-490)    Volumetric: thickness of the pending surface's span -> its hit record
 //   visible surface (surface.rs:322-331,399)   a 64-byte hit record into the lane's chunk of the hit stream
 // A lane parks when it has to change level (EnterBlock: Raycaster::within on the brick, raycast.rs:458-476; leaving
 // the brick) or when its ray is finished; parked lanes are served together once `event_threshold` lanes wait.
+// WIDE: u32 cells; BRICK_WIDE: u32 brick words (a wide brick pool).
 // ======================================================================================================
-template <bool VOLUMETRIC, bool WIDE, bool AUX>
+template <bool VOLUMETRIC, bool WIDE, bool AUX, bool BRICK_WIDE>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32, AUX ? 1 : MIN_BLOCKS_PER_SM)
 trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
     grid_dependency_sync();
@@ -1172,10 +1176,12 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
                     w = (cell & 0x3fffu) | ((cell >> 2) & 0xc000u);                  // only ids < 16384 keep their bits here
                     ev_word = cell & 0xffffu;
                 } else {
-                    w = __ldg(S.bricks + idx);
+                    if constexpr (BRICK_WIDE) w = __ldg((const uint32_t *)S.bricks + idx);
+                    else w = __ldg(S.bricks + idx);
                 }
             } else {
-                w = __ldg((inner ? S.bricks : (const uint16_t *)S.cells) + idx);
+                if constexpr (BRICK_WIDE) w = inner ? __ldg((const uint32_t *)S.bricks + idx) : __ldg((const uint16_t *)S.cells + idx);
+                else w = __ldg((inner ? S.bricks : (const uint16_t *)S.cells) + idx);
             }
             if constexpr (AUX) { if (inner) aux.n_inner++; else aux.n_outer++; }
         }
@@ -1207,8 +1213,9 @@ trace_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
             st = ST_ENTER;
             return;
         }
-        if constexpr (WIDE) emit_surface(inner ? w : ev_word);
-        else emit_surface(inner ? w : (w & 0x3fffu));
+        const uint32_t voxel = BRICK_WIDE ? w >> 16 : w;   // a brick word's palette index
+        if constexpr (WIDE) emit_surface(inner ? voxel : ev_word);
+        else emit_surface(inner ? voxel : (w & 0x3fffu));
     };
 
     for (;;) {

@@ -64,6 +64,10 @@ enum { AICB_FACE_WITHIN = 0, AICB_FACE_NX = 1, AICB_FACE_NY = 2, AICB_FACE_NZ = 
  * (vol.rs:1013-1018: ((x-lx)*size_y + (y-ly))*size_z + (z-lz)); voxel_bounds may be smaller
  * than resolution^3 (voxel_storage.rs:176-178) but must lie inside [0,resolution)^3.
  * `is_air` is TracingCubeData::always_invisible (sr.rs:547).
+ * A palette may have up to 65536 entries (VoxelIndex is u16, voxel_storage.rs:32), duplicates and
+ * unused entries included; more is AICB_ERR_UNSUPPORTED.  A scene whose blocks all have at most
+ * 32768 entries keeps 2 bytes per voxel on the device; the first block with more makes it keep 4
+ * (aicb_scene_device_bytes), until aicb_scene_fill_uniform replaces its table.
  * The `light_*` members are EvaluatedBlock derived data (block/eval/derived.rs:33-80) read
  * only by the light-propagation path (space/light/updater.rs:760-884). */
 typedef struct aicb_block_desc {
