@@ -712,7 +712,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             Q.bin_count = Q.task_counter + 4;
             Q.debug_warp_times = nullptr;
         }
-        kernel_fn k = select_kernel(volumetric, sc->ds.wide_cells != 0, out.aux, sc->blocks.wide_bricks);
+        kernel_fn k = select_kernel(volumetric, sc->ds.wide_cells != 0, out.aux, sc->host->wide_bricks);
         int blocks_per_sm = 0;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, k, WARPS_PER_BLOCK * 32, 0));
         if (blocks_per_sm < 1) blocks_per_sm = 1;
@@ -891,10 +891,20 @@ struct Retired {
     }
 };
 
-// Block definitions flattened against a table: per definition its record (brick_off / pal_off already offsets into the
-// table's pools) and extents, blk_tab entry, kind and light record; and the voxel data they append to the pools.  The
-// brick words are in the form the table's pool has once they are placed: wide if it is wide already or if a palette
-// has more than 32768 entries.
+// What a call allocated for each replica before changing any, freed on each replica's device once an allocation fails.
+template <typename T>
+static aicb_status free_each(Replicas r, std::vector<T> &per_replica, aicb_status st) {
+    for (size_t i = 0; i < per_replica.size(); i++) {
+        cudaSetDevice(r.ctx[i]->device);
+        per_replica[i] = T();
+    }
+    return st;
+}
+
+// Block definitions flattened against a table's bookkeeping: per definition its record (brick_off / pal_off already
+// offsets into the table's pools) and extents, blk_tab entry, kind and light record; and the voxel data they append to
+// the pools.  The brick words are in the form the table's pool has once they are placed: wide if it is wide already or
+// if a palette has more than 32768 entries.
 struct FlatBlocks {
     std::vector<BlockRec> recs;
     std::vector<BlockTable::Extent> extents;
@@ -910,127 +920,164 @@ struct FlatBlocks {
     std::vector<float2> pal_tab;
 };
 
-// Validates and flattens n definitions against `t`, for the next ids (indices == nullptr) or for existing `indices`.
+// Validates and flattens n definitions against `h`, for the next ids (indices == nullptr) or for existing `indices`.
 // Changes nothing.
-static aicb_status flatten_blocks(const BlockTable &t, const aicb_block_desc *descs, size_t n, const uint16_t *indices,
+static aicb_status flatten_blocks(const SpaceHost &h, const aicb_block_desc *descs, size_t n, const uint16_t *indices,
                                   FlatBlocks *f) {
-    if (!indices && t.block_count() + n > 65536) return fail(AICB_ERR_INVALID, "more than 65536 blocks");
-    const uint32_t pal_base = (uint32_t)(t.n_palette / 2);   // palette entries (2 x float4 each)
+    if (!indices && h.block_count() + n > 65536) return fail(AICB_ERR_INVALID, "more than 65536 blocks");
+    const uint32_t pal_base = (uint32_t)(h.n_palette / 2);   // palette entries (2 x float4 each)
     f->recs.resize(n);
     f->extents.resize(n);
     f->blk_tab.resize(n);
     f->kinds.resize(n);
     f->light.resize(n);
     for (size_t i = 0; i < n; i++) {
-        if (indices && indices[i] >= t.block_count())
+        if (indices && indices[i] >= h.block_count())
             return fail(AICB_ERR_INVALID, "block index out of range (new indices need a new scene)");
         BlockRec &r = f->recs[i];
         const size_t bricks_before = f->bricks.size(), pal_before = f->pal_tab.size();
         TRY(flatten_block(descs[i], r, f->kinds[i], f->bricks, f->palette, f->pal_tab));
         f->blk_tab[i] = block_entry(f->kinds[i], r.pal_off, f->pal_tab, pal_base);
-        if (f->kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)t.n_bricks;
+        if (f->kinds[i] == KIND_RECURSIVE) r.brick_off += (uint32_t)h.n_bricks;
         if (!descs[i].is_air) r.pal_off += pal_base;
         f->extents[i] = {r.brick_off, (uint32_t)(f->bricks.size() - bricks_before), r.pal_off,
                          (uint32_t)(f->pal_tab.size() - pal_before)};
         f->light[i] = light_block(descs[i]);
         if (f->kinds[i] == KIND_RECURSIVE && descs[i].n_palette > 32768) f->wide_bricks = true;
     }
-    if (t.wide_bricks) f->wide_bricks = true;
+    if (h.wide_bricks) f->wide_bricks = true;
     if (!f->wide_bricks) {
         f->narrow.resize(f->bricks.size());
         for (size_t k = 0; k < f->bricks.size(); k++) f->narrow[k] = (uint16_t)(f->bricks[k] >> 16 | (f->bricks[k] & 0x8000u));
     }
     // live data only: the dead part of the pool is compacted away before it could push positions past 2^32
     // (flatten_placeable)
-    if (brick_room(t.n_bricks, t.dead_bricks, f->bricks.size()) == BrickRoom::too_big)
+    if (brick_room(h.n_bricks, h.dead_bricks, f->bricks.size()) == BrickRoom::too_big)
         return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
     return AICB_OK;
 }
 
-// A narrow brick pool as a wide one, with room for `add` more words: its words re-encoded on the device into a new
-// buffer (grow_buffer's size rule, in words), queued on the context's stream; the old buffer goes to `retired`.
-static aicb_status widen_bricks(aicb_scene *s, size_t add, Retired &retired) {
-    BlockTable &t = s->blocks;
-    DeviceBuffer wide;
-    TRY(wide.ensure(std::max(round16((t.n_bricks + add) * 4), 2 * t.bricks.bytes())));
-    if (t.n_bricks) {
-        const size_t want = (std::max<size_t>(t.n_bricks / 8, 1) + 255) / 256, cap = (size_t)s->ctx->num_sms * 16;
-        widen_bricks_kernel<<<(unsigned)std::min(want, cap), 256, 0, s->ctx->stream.get()>>>(
-            t.bricks.get<const uint16_t>(), wide.get<uint32_t>(), t.n_bricks);
-        CU(cudaGetLastError());
+// Every replica's narrow brick pool as a wide one, with room for `add` more words: once every replica's new buffer is
+// allocated (grow_buffer's size rule, in words), each replica's words are re-encoded into it on the device, queued on
+// its context's stream, and the old buffer is retired.
+static aicb_status widen_bricks(Replicas r, size_t add) {
+    SpaceHost &h = *r.scene[0]->host;
+    std::vector<DeviceBuffer> wide(r.n);
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.ctx[i]->device));
+        const size_t bytes = std::max(round16((h.n_bricks + add) * 4), 2 * r.scene[i]->blocks.bricks.bytes());
+        const aicb_status st = wide[i].ensure(bytes);
+        if (st != AICB_OK) return free_each(r, wide, st);
     }
-    if (t.bricks) retired.bufs.push_back(std::move(t.bricks));
-    t.bricks = std::move(wide);
-    t.wide_bricks = true;
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_ctx *ctx = r.ctx[i];
+        BlockTable &t = r.scene[i]->blocks;
+        const size_t want = (std::max<size_t>(h.n_bricks / 8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
+        CU(cudaSetDevice(ctx->device));
+        if (h.n_bricks)
+            widen_bricks_kernel<<<(unsigned)std::min(want, cap), 256, 0, ctx->stream.get()>>>(
+                t.bricks.get<const uint16_t>(), wide[i].get<uint32_t>(), h.n_bricks);
+        CU(cudaGetLastError());
+        Retired retired{ctx, {}};
+        if (t.bricks) retired.bufs.push_back(std::move(t.bricks));
+        t.bricks = std::move(wide[i]);
+        t.bind(r.scene[i]->ds);
+    }
+    h.wide_bricks = true;
     return AICB_OK;
 }
 
-// Places `f` (flattened against s's table) in s's table: a narrow brick pool widened first if `f` is wide; the voxel
-// data appended to the pools; the per-id records appended (indices == nullptr) or written at `indices`, where a
-// repeated index keeps its last definition.  Every copy is queued on the context's stream, and the scene's pointers
-// follow every array that moved, whatever fails later.
-static aicb_status place(aicb_scene *s, const FlatBlocks &f, const uint16_t *indices, Retired &retired) {
-    BlockTable &t = s->blocks;
-    cudaStream_t stream = s->ctx->stream.get();
-    const size_t n = f.kinds.size(), count = t.block_count(), added = indices ? 0 : n;
-    aicb_status st = AICB_OK;
-    if (f.wide_bricks && !t.wide_bricks) st = widen_bricks(s, f.bricks.size(), retired);
-    const size_t wb = t.brick_word_bytes();
-    auto room = [&](DeviceBuffer &b, size_t used, size_t add) {
-        if (st == AICB_OK && add) st = grow_buffer(b, used, used + add, stream, &retired.bufs);
+// Placing `f` (flattened against `h`, with the pool in f's form) takes three steps.  room: on each replica, every
+// buffer of table `t` grown to hold h's elements in use and f's (grow_buffer; the caller binds t, whatever fails).
+// copy: on each replica, f queued on `stream` at the positions h gives: the voxel data after the pools' elements in
+// use, the per-id records appended (indices == nullptr) or written at `indices`, in order, so a repeated index keeps
+// its last definition.  book: f in the bookkeeping, once.
+static aicb_status room(BlockTable &t, const SpaceHost &h, const FlatBlocks &f, const uint16_t *indices,
+                        cudaStream_t stream, Retired &retired) {
+    const size_t count = h.block_count(), added = indices ? 0 : f.kinds.size(), wb = f.brick_word_bytes();
+    auto grow = [&](DeviceBuffer &b, size_t used, size_t add) {
+        return add ? grow_buffer(b, used, used + add, stream, &retired.bufs) : AICB_OK;
     };
-    room(t.blocks, count * sizeof(BlockRec), added * sizeof(BlockRec));
-    room(t.bricks, t.n_bricks * wb, f.bricks.size() * wb);
-    room(t.palette, t.n_palette * sizeof(float4), f.palette.size() * sizeof(float4));
-    room(t.pal_tab, t.n_palette / 2 * sizeof(float2), f.pal_tab.size() * sizeof(float2));
-    room(t.blk_tab, count * sizeof(float4), added * sizeof(float4));
-    room(t.light, count * sizeof(LightBlockDev), added * sizeof(LightBlockDev));
-    t.bind(s->ds);
-    TRY(st);
+    TRY(grow(t.blocks, count * sizeof(BlockRec), added * sizeof(BlockRec)));
+    TRY(grow(t.bricks, h.n_bricks * wb, f.bricks.size() * wb));
+    TRY(grow(t.palette, h.n_palette * sizeof(float4), f.palette.size() * sizeof(float4)));
+    TRY(grow(t.pal_tab, h.n_palette / 2 * sizeof(float2), f.pal_tab.size() * sizeof(float2)));
+    TRY(grow(t.blk_tab, count * sizeof(float4), added * sizeof(float4)));
+    return grow(t.light, count * sizeof(LightBlockDev), added * sizeof(LightBlockDev));
+}
+
+static aicb_status copy(const BlockTable &t, const SpaceHost &h, const FlatBlocks &f, const uint16_t *indices,
+                        cudaStream_t stream) {
     auto put = [&](void *dst, const void *src, size_t bytes) {
         if (bytes) CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
         return AICB_OK;
     };
-    TRY(put(t.bricks.get<char>() + t.n_bricks * wb, f.brick_words(), f.bricks.size() * wb));
-    TRY(put(t.palette.get<float4>() + t.n_palette, f.palette.data(), f.palette.size() * sizeof(float4)));
-    TRY(put(t.pal_tab.get<float2>() + t.n_palette / 2, f.pal_tab.data(), f.pal_tab.size() * sizeof(float2)));
-    // the per-id records: one run of n at the end of the table, or one record at each index, in order
-    const size_t runs = indices ? n : 1, len = indices ? 1 : n;
+    const size_t wb = f.brick_word_bytes();
+    TRY(put(t.bricks.get<char>() + h.n_bricks * wb, f.brick_words(), f.bricks.size() * wb));
+    TRY(put(t.palette.get<float4>() + h.n_palette, f.palette.data(), f.palette.size() * sizeof(float4)));
+    TRY(put(t.pal_tab.get<float2>() + h.n_palette / 2, f.pal_tab.data(), f.pal_tab.size() * sizeof(float2)));
+    // the per-id records: one run of n at the end of the table, or one record at each index
+    const size_t n = f.kinds.size(), runs = indices ? n : 1, len = indices ? 1 : n;
     for (size_t i = 0; i < runs; i++) {
-        const size_t id = indices ? indices[i] : count;
+        const size_t id = indices ? indices[i] : h.block_count();
         TRY(put(t.blocks.get<BlockRec>() + id, f.recs.data() + i, len * sizeof(BlockRec)));
         TRY(put(t.blk_tab.get<float4>() + id, f.blk_tab.data() + i, len * sizeof(float4)));
         TRY(put(t.light.get<LightBlockDev>() + id, f.light.data() + i, len * sizeof(LightBlockDev)));
     }
-    t.kind.resize(count + added);
-    t.light_flags.resize(count + added);
-    t.extent.resize(count + added);
-    for (size_t i = 0; i < n; i++) {
-        const size_t id = indices ? indices[i] : count + i;
-        if (indices) {   // the extents written over, an earlier definition of this call included, are dead
-            t.dead_bricks += t.extent[id].n_bricks;
-            t.dead_pal += t.extent[id].n_pal;
-        }
-        t.kind[id] = f.kinds[i];
-        t.light_flags[id] = f.light[i].flags;
-        t.extent[id] = f.extents[i];
-    }
-    t.n_bricks += f.bricks.size();
-    t.n_palette += f.palette.size();
     return AICB_OK;
 }
 
-// Compacts s's brick pool and/or palette pool (palette and pal_tab): each pool's live extents, in pool order, are
-// gathered to the front of a new buffer of the live size by compact_pool_kernel, and each id's extent, record and
-// blk_tab entry follow them.  The old buffers go to `retired`.  Queued on the context's stream; the caller has waited
-// for the context (wait_context), since a frame's hit records hold absolute pool positions.  Every allocation comes
-// first: a failure changes nothing.
-static aicb_status compact_pools(aicb_scene *s, bool bricks, bool palette, Retired &retired) {
-    BlockTable &t = s->blocks;
-    aicb_ctx *ctx = s->ctx;
-    cudaStream_t stream = ctx->stream.get();
-    const size_t count = t.block_count();
-    std::vector<BlockTable::Extent> ext = t.extent;
+static void book(SpaceHost &h, const FlatBlocks &f, const uint16_t *indices) {
+    const size_t n = f.kinds.size(), count = h.block_count(), added = indices ? 0 : n;
+    h.kind.resize(count + added);
+    h.extent.resize(count + added);
+    for (size_t i = 0; i < n; i++) {
+        const size_t id = indices ? indices[i] : count + i;
+        if (indices) {   // the extents written over, an earlier definition of this call included, are dead
+            h.dead_bricks += h.extent[id].n_bricks;
+            h.dead_pal += h.extent[id].n_pal;
+        }
+        h.kind[id] = f.kinds[i];
+        h.extent[id] = f.extents[i];
+    }
+    h.n_bricks += f.bricks.size();
+    h.n_palette += f.palette.size();
+    h.wide_bricks = f.wide_bricks;
+}
+
+// f (flatten_placeable) placed in every replica's table: room in each, then the copies, recorded in ev_delta (renders
+// on other streams wait for it, launch_trace), and the bookkeeping.  Records are written over in place (`indices`)
+// only once every replica has room and its context has been waited for (wait_context).
+static aicb_status place(Replicas r, const FlatBlocks &f, const uint16_t *indices) {
+    SpaceHost &h = *r.scene[0]->host;
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_scene *s = r.scene[i];
+        CU(cudaSetDevice(r.ctx[i]->device));
+        if (indices) TRY(wait_context(r.ctx[i]));
+        Retired retired{r.ctx[i], {}};
+        const aicb_status st = room(s->blocks, h, f, indices, r.ctx[i]->stream.get(), retired);
+        s->blocks.bind(s->ds);
+        TRY(st);
+    }
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.ctx[i]->device));
+        TRY(copy(r.scene[i]->blocks, h, f, indices, r.ctx[i]->stream.get()));
+        CU(cudaEventRecord(r.ctx[i]->ev_delta.get(), r.ctx[i]->stream.get()));
+    }
+    book(h, f, indices);
+    return AICB_OK;
+}
+
+// Compacts every replica's brick pool and/or palette pool (palette and pal_tab), planned once from the bookkeeping:
+// each pool's live extents, in pool order, go to the front of a new buffer of the live size, and each id's extent
+// follows them.  Once every replica's new buffers are allocated, compact_pool_kernel gathers each replica's pools and
+// rebase_blocks_kernel moves its records and blk_tab entries, queued on its context's stream, and the old buffers are
+// retired.  The caller has waited for every context (wait_context), since a frame's hit records hold absolute pool
+// positions.
+static aicb_status compact_pools(Replicas r, bool bricks, bool palette) {
+    SpaceHost &h = *r.scene[0]->host;
+    const size_t count = h.block_count();
+    std::vector<BlockTable::Extent> ext = h.extent;
     // one pool's plan: its live extents in pool order, gathered to the front; the ids' new offsets go to `ext`.  Each
     // run (neighbouring extents merged) of `elem`-byte elements becomes segments of at most 16 KiB of `segs`.
     std::vector<PoolSegment> segs;
@@ -1060,53 +1107,70 @@ static aicb_status compact_pools(aicb_scene *s, bool bricks, bool palette, Retir
         return live;
     };
     std::vector<std::pair<size_t, size_t>> ranges;   // per buffer gathered: its segments in `segs`
-    const size_t wb = t.brick_word_bytes();
+    const size_t wb = h.brick_word_bytes();
     const size_t live_bricks = bricks ? plan(&BlockTable::Extent::brick_off, &BlockTable::Extent::n_bricks, {wb}, &ranges) : 0;
     const size_t live_pal = palette ? plan(&BlockTable::Extent::pal_off, &BlockTable::Extent::n_pal,
                                            {2 * sizeof(float4), sizeof(float2)}, &ranges) : 0;
-    DeviceBuffer new_bricks, new_palette, new_pal_tab, d_segs, d_off;
-    if (bricks) TRY(new_bricks.ensure(round16(live_bricks * wb)));
-    if (palette) {
-        TRY(new_palette.ensure(live_pal * 2 * sizeof(float4)));
-        TRY(new_pal_tab.ensure(round16(live_pal * sizeof(float2))));
-    }
-    TRY(d_segs.ensure(segs.size() * sizeof(PoolSegment)));
-    TRY(d_off.ensure(count * sizeof(uint2)));
     std::vector<uint2> off(count);
     for (size_t id = 0; id < count; id++) off[id] = make_uint2(ext[id].brick_off, ext[id].pal_off);
-    if (!segs.empty())
-        CU(cudaMemcpyAsync(d_segs.get(), segs.data(), segs.size() * sizeof(PoolSegment), cudaMemcpyHostToDevice, stream));
-    if (count) CU(cudaMemcpyAsync(d_off.get(), off.data(), count * sizeof(uint2), cudaMemcpyHostToDevice, stream));
-    size_t next = 0;
-    auto gather = [&](DeviceBuffer &buf, DeviceBuffer &to) {
-        const auto [first, n] = ranges[next++];
-        if (n) {
-            const unsigned grid = (unsigned)std::min(n, (size_t)ctx->num_sms * 8);
-            compact_pool_kernel<<<grid, 256, 0, stream>>>(buf.get<const uint8_t>(), to.get<uint8_t>(),
-                                                          d_segs.get<const PoolSegment>() + first, (uint32_t)n);
-        }
-        if (buf) retired.bufs.push_back(std::move(buf));
-        buf = std::move(to);
+    struct NewPools {
+        DeviceBuffer bricks, palette, pal_tab, segs, off;
     };
+    std::vector<NewPools> to(r.n);
+    for (size_t i = 0; i < r.n; i++) {
+        NewPools &p = to[i];
+        CU(cudaSetDevice(r.ctx[i]->device));
+        aicb_status st = p.segs.ensure(segs.size() * sizeof(PoolSegment));
+        if (st == AICB_OK) st = p.off.ensure(count * sizeof(uint2));
+        if (st == AICB_OK && bricks) st = p.bricks.ensure(round16(live_bricks * wb));
+        if (st == AICB_OK && palette) st = p.palette.ensure(live_pal * 2 * sizeof(float4));
+        if (st == AICB_OK && palette) st = p.pal_tab.ensure(round16(live_pal * sizeof(float2)));
+        if (st != AICB_OK) return free_each(r, to, st);
+    }
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_ctx *ctx = r.ctx[i];
+        cudaStream_t stream = ctx->stream.get();
+        BlockTable &t = r.scene[i]->blocks;
+        NewPools &p = to[i];
+        CU(cudaSetDevice(ctx->device));
+        if (!segs.empty())
+            CU(cudaMemcpyAsync(p.segs.get(), segs.data(), segs.size() * sizeof(PoolSegment), cudaMemcpyHostToDevice,
+                               stream));
+        if (count) CU(cudaMemcpyAsync(p.off.get(), off.data(), count * sizeof(uint2), cudaMemcpyHostToDevice, stream));
+        Retired retired{ctx, {}};
+        size_t next = 0;
+        auto gather = [&](DeviceBuffer &buf, DeviceBuffer &into) {
+            const auto [first, n] = ranges[next++];
+            if (n) {
+                const unsigned grid = (unsigned)std::min(n, (size_t)ctx->num_sms * 8);
+                compact_pool_kernel<<<grid, 256, 0, stream>>>(buf.get<const uint8_t>(), into.get<uint8_t>(),
+                                                              p.segs.get<const PoolSegment>() + first, (uint32_t)n);
+            }
+            if (buf) retired.bufs.push_back(std::move(buf));
+            buf = std::move(into);
+        };
+        if (bricks) gather(t.bricks, p.bricks);
+        if (palette) {
+            gather(t.palette, p.palette);
+            gather(t.pal_tab, p.pal_tab);
+        }
+        t.bind(r.scene[i]->ds);
+        if (count)
+            rebase_blocks_kernel<<<(unsigned)((count + 127) / 128), 128, 0, stream>>>(
+                t.blocks.get<BlockRec>(), t.blk_tab.get<float4>(), p.off.get<const uint2>(), (uint32_t)count);
+        retired.bufs.push_back(std::move(p.segs));
+        retired.bufs.push_back(std::move(p.off));
+        CU(cudaGetLastError());
+    }
     if (bricks) {
-        gather(t.bricks, new_bricks);
-        t.n_bricks = live_bricks;
-        t.dead_bricks = 0;
+        h.n_bricks = live_bricks;
+        h.dead_bricks = 0;
     }
     if (palette) {
-        gather(t.palette, new_palette);
-        gather(t.pal_tab, new_pal_tab);
-        t.n_palette = live_pal * 2;
-        t.dead_pal = 0;
+        h.n_palette = live_pal * 2;
+        h.dead_pal = 0;
     }
-    t.extent = std::move(ext);
-    t.bind(s->ds);
-    if (count)
-        rebase_blocks_kernel<<<(unsigned)((count + 127) / 128), 128, 0, stream>>>(
-            t.blocks.get<BlockRec>(), t.blk_tab.get<float4>(), d_off.get<const uint2>(), (uint32_t)count);
-    retired.bufs.push_back(std::move(d_segs));
-    retired.bufs.push_back(std::move(d_off));
-    CU(cudaGetLastError());
+    h.extent = std::move(ext);
     return AICB_OK;
 }
 
@@ -1122,8 +1186,9 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
     if (volume && !d->block_ids) return fail(AICB_ERR_INVALID, "block_ids is NULL");
     if (volume && d->n_blocks == 0) return fail(AICB_ERR_INVALID, "non-empty space with an empty block table");
     if (d->n_blocks && !d->blocks) return fail(AICB_ERR_INVALID, "blocks is NULL");
+    auto host = std::make_unique<SpaceHost>();   // empty until every replica holds the table
     FlatBlocks f;
-    TRY(flatten_blocks(BlockTable(), d->blocks, d->n_blocks, nullptr, &f));
+    TRY(flatten_blocks(*host, d->blocks, d->n_blocks, nullptr, &f));
 
     // ---- cells: block id with its kind in the top bits --------------------------------------------------------------
     const bool wide = d->n_blocks > 16384;
@@ -1143,7 +1208,7 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
         CU(cudaSetDevice(c->device));
         std::unique_ptr<aicb_scene> s(new aicb_scene());
         s->ctx = c;
-        s->volume = (size_t)volume;
+        s->host = host.get();
         DeviceScene &ds = s->ds;
         for (int a = 0; a < 3; a++) {
             ds.lo[a] = d->bounds.lower[a];
@@ -1157,15 +1222,15 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
                 TRY(s->d_light.upload(d->light, volume * 4));
                 s->device_bytes += volume * 4;
             }
-            s->h_ids.assign(d->block_ids, d->block_ids + volume);
         }
         ds.cells = s->d_cells.get();
         ds.light = s->d_light.get<uint32_t>();
         ds.tables = c->d_lut.get<float>();
         build_block_sky(d->sky, &ds);
-        s->light_max_distance = d->light_max_distance;
         Retired retired{c, {}};   // (a new table replaces no array)
-        TRY(place(s.get(), f, nullptr, retired));
+        TRY(room(s->blocks, *host, f, nullptr, c->stream.get(), retired));
+        s->blocks.bind(ds);
+        TRY(copy(s->blocks, *host, f, nullptr, c->stream.get()));
         CU(cudaStreamSynchronize(c->stream.get()));
         *o = s.release();
         return AICB_OK;
@@ -1173,31 +1238,37 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
     for (size_t i = 0; i < n; i++) {
         const aicb_status st = create(ctx[i], &out[i]);
         if (st != AICB_OK) {
-            for (size_t k = 0; k < i; k++) aicb_scene_destroy(out[k]);
+            for (size_t k = i; k-- > 0;) aicb_scene_destroy(out[k]);
             return st;
         }
     }
+    host->volume = (size_t)volume;
+    host->h_ids.assign(d->block_ids, d->block_ids + volume);
+    host->light_max_distance = d->light_max_distance;
+    book(*host, f, nullptr);
+    out[0]->own_host = std::move(host);
     return AICB_OK;
 }
 
-// flatten_blocks against replica 0's table, for an update (`indices`) or an append (nullptr) of the scene's replicas,
+// flatten_blocks against the scene's table, for an update (`indices`) or an append (nullptr) of the scene's replicas,
 // such that the result can be placed: brick positions are u32, so when the live data fits but the pool's words in use
 // plus the new ones would not (brick_room), every replica's brick pool is compacted first and the definitions are
 // flattened again against the compacted table.  A compaction moves the pools, so each replica's context is waited
-// for first (wait_context).
+// for first (wait_context).  Wide definitions for a narrow pool widen every replica's pool first.
 static aicb_status flatten_placeable(Replicas r, const aicb_block_desc *descs, size_t n_blocks, const uint16_t *indices,
                                      FlatBlocks *f) {
-    const BlockTable &t = r.scene[0]->blocks;
-    TRY(flatten_blocks(t, descs, n_blocks, indices, f));
-    if (brick_room(t.n_bricks, t.dead_bricks, f->bricks.size()) != BrickRoom::compact_first) return AICB_OK;
-    for (size_t i = 0; i < r.n; i++) {
-        CU(cudaSetDevice(r.ctx[i]->device));
-        TRY(wait_context(r.ctx[i]));
-        Retired retired{r.ctx[i], {}};
-        TRY(compact_pools(r.scene[i], true, false, retired));
+    const SpaceHost &h = *r.scene[0]->host;
+    TRY(flatten_blocks(h, descs, n_blocks, indices, f));
+    if (brick_room(h.n_bricks, h.dead_bricks, f->bricks.size()) == BrickRoom::compact_first) {
+        for (size_t i = 0; i < r.n; i++) {
+            CU(cudaSetDevice(r.ctx[i]->device));
+            TRY(wait_context(r.ctx[i]));
+        }
+        TRY(compact_pools(r, true, false));
+        *f = FlatBlocks();
+        TRY(flatten_blocks(h, descs, n_blocks, indices, f));
     }
-    *f = FlatBlocks();
-    return flatten_blocks(t, descs, n_blocks, indices, f);
+    return f->wide_bricks && !h.wide_bricks ? widen_bricks(r, f->bricks.size()) : AICB_OK;
 }
 
 // The context's staging (h_delta / d_delta) with room for a batch of `bytes`, once the previous batch has left it.
@@ -1222,8 +1293,8 @@ aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uin
     if (n && (!cubes || !ids)) return fail(AICB_ERR_INVALID, "NULL argument");
     CU(cudaSetDevice(r.ctx[0]->device));
     if (n == 0) return AICB_OK;
-    const aicb_scene *s0 = r.scene[0];
-    const DeviceScene &ds = s0->ds;
+    SpaceHost &h = *r.scene[0]->host;
+    const DeviceScene &ds = r.scene[0]->ds;
     // validate and build the whole batch before touching any state
     std::vector<uint32_t> idx(n);
     std::vector<CubeDelta> ops;
@@ -1235,12 +1306,12 @@ aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uin
                        dz = (uint32_t)(cubes[i][2] - ds.lo[2]);
         if (dx >= (uint32_t)ds.size[0] || dy >= (uint32_t)ds.size[1] || dz >= (uint32_t)ds.size[2])
             return fail(AICB_ERR_INVALID, "cube out of bounds");
-        if (ids[i] >= s0->blocks.block_count()) return fail(AICB_ERR_INVALID, "block id out of range");
+        if (ids[i] >= h.block_count()) return fail(AICB_ERR_INVALID, "block id out of range");
         idx[i] = (uint32_t)(((size_t)dx * ds.size[1] + dy) * ds.size[2] + dz);
         CubeDelta op;
         op.idx = idx[i];
-        op.cell = cell_word(ids[i], s0->blocks.kind[ids[i]], ds.wide_cells);
-        op.has_light = (light && s0->d_light) ? 1u : 0u;
+        op.cell = cell_word(ids[i], h.kind[ids[i]], ds.wide_cells);
+        op.has_light = (light && r.scene[0]->d_light) ? 1u : 0u;
         op.light = 0;
         if (op.has_light) std::memcpy(&op.light, light[i], 4);
         const auto [at, first] = seen.emplace(op.idx, (uint32_t)ops.size());
@@ -1253,8 +1324,6 @@ aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uin
         aicb_ctx *ctx = r.ctx[k];
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
-        if (!s->h_ids.empty())
-            for (size_t i = 0; i < n; i++) s->h_ids[idx[i]] = ids[i];
         TRY(delta_room(ctx, bytes));
         std::memcpy(ctx->h_delta.get(), ops.data(), bytes);
         CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
@@ -1263,6 +1332,8 @@ aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uin
         CU(cudaGetLastError());
         CU(cudaEventRecord(ctx->ev_delta.get(), stream));  // renders on other streams wait for it (launch_trace)
     }
+    if (!h.h_ids.empty())
+        for (size_t i = 0; i < n; i++) h.h_ids[idx[i]] = ids[i];
     return AICB_OK;
 }
 
@@ -1279,7 +1350,7 @@ aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint
     // the kernels' work items, at most size[2] / 4 + 2 per row, are counted in 32 bits
     if ((uint64_t)box->size[0] * box->size[1] * (box->size[2] / 4 + 2) > 0xffffffffull)
         return fail(AICB_ERR_INVALID, "region too large");
-    const size_t count = s->blocks.block_count();
+    const size_t count = s->host->block_count();
     if (!ids) {
         if (uniform_id >= count) return fail(AICB_ERR_INVALID, "block id out of range");
         return AICB_OK;
@@ -1290,18 +1361,23 @@ aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint
     return AICB_OK;
 }
 
+void mirror_region(SpaceHost &h, const DeviceScene &ds, const RegionBox &box, const uint16_t *ids,
+                   uint16_t uniform_id) {
+    if (h.h_ids.empty()) return;
+    const size_t rows = (size_t)box.size[0] * box.size[1], sz = box.size[2];
+    for (size_t row = 0; row < rows; row++) {
+        uint16_t *dst = h.h_ids.data() + ((size_t)(box.lo[0] + row / box.size[1]) * ds.size[1] + box.lo[1] +
+                                          row % box.size[1]) * ds.size[2] + box.lo[2];
+        if (ids) std::memcpy(dst, ids + row * sz, sz * 2);
+        else std::fill(dst, dst + sz, uniform_id);
+    }
+}
+
 aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *ids, uint16_t uniform_id,
                          const uint8_t (*light)[4], uint32_t *d_mask, uint32_t *d_n_changed) {
     aicb_ctx *ctx = s->ctx;
     cudaStream_t stream = ctx->stream.get();
     const size_t vol = box.volume(), rows = (size_t)box.size[0] * box.size[1], sz = box.size[2];
-    if (!s->h_ids.empty())
-        for (size_t row = 0; row < rows; row++) {
-            uint16_t *dst = s->h_ids.data() + ((size_t)(box.lo[0] + row / box.size[1]) * s->ds.size[1] + box.lo[1] +
-                                               row % box.size[1]) * s->ds.size[2] + box.lo[2];
-            if (ids) std::memcpy(dst, ids + row * sz, sz * 2);
-            else std::fill(dst, dst + sz, uniform_id);
-        }
     if (!s->d_light) light = nullptr;
     // the ids, then (16-byte aligned) the texels
     const size_t id_bytes = ids ? (vol * 2 + 15) / 16 * 16 : 0, bytes = id_bytes + (light ? vol * 4 : 0);
@@ -1351,44 +1427,39 @@ aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint1
         TRY(region_cells(r.scene[k], box, ids, uniform_id, light, nullptr, nullptr));
         CU(cudaEventRecord(r.ctx[k]->ev_delta.get(), r.ctx[k]->stream.get()));  // renders on other streams wait for it
     }
+    mirror_region(*r.scene[0]->host, r.scene[0]->ds, box, ids, uniform_id);
     return AICB_OK;
 }
 
 aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks) {
     if (n_blocks && (!indices || !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
     if (n_blocks == 0) return AICB_OK;
-    aicb_scene *s0 = r.scene[0];
-    const BlockTable &t = s0->blocks;
+    const SpaceHost &h = *r.scene[0]->host;
     FlatBlocks f;
     TRY(flatten_placeable(r, descs, n_blocks, indices, &f));
     // cubes that hold a block whose kind changes carry the new kind in their cell words
-    std::vector<uint8_t> kind(t.kind);
+    std::vector<uint8_t> kind(h.kind);
     for (size_t i = 0; i < n_blocks; i++) kind[indices[i]] = f.kinds[i];
     std::vector<CubeDelta> ops;
-    if (kind != t.kind) {
-        if (s0->h_ids.size() != s0->volume) return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
-        const bool wide = s0->ds.wide_cells;
+    if (kind != h.kind) {
+        if (h.h_ids.size() != h.volume) return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
+        const bool wide = r.scene[0]->ds.wide_cells;
         uint32_t idx = 0;
-        for (const uint16_t id : s0->h_ids) {
-            if (kind[id] != t.kind[id]) ops.push_back({idx, cell_word(id, kind[id], wide), 0, 0});
+        for (const uint16_t id : h.h_ids) {
+            if (kind[id] != h.kind[id]) ops.push_back({idx, cell_word(id, kind[id], wide), 0, 0});
             idx++;
         }
     }
-    bool compact_bricks = false, compact_palette = false;   // replica 0's decision, which every replica takes
+    TRY(place(r, f, indices));   // (which waits for every context: compaction moves the pools)
+    const bool compact_bricks = h.dead_bricks > h.n_bricks - h.dead_bricks;
+    const bool compact_palette = h.dead_pal > h.n_palette / 2 - h.dead_pal;
+    if (compact_bricks || compact_palette) TRY(compact_pools(r, compact_bricks, compact_palette));
     for (size_t i = 0; i < r.n; i++) {
         aicb_scene *sc = r.scene[i];
         aicb_ctx *ctx = r.ctx[i];
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
-        TRY(wait_context(ctx));   // the records are written over in place, and compaction moves the pools
         Retired retired{ctx, {}};
-        TRY(place(sc, f, indices, retired));
-        if (i == 0) {
-            const BlockTable &t0 = s0->blocks;
-            compact_bricks = t0.dead_bricks > t0.n_bricks - t0.dead_bricks;
-            compact_palette = t0.dead_pal > t0.n_palette / 2 - t0.dead_pal;
-        }
-        if (compact_bricks || compact_palette) TRY(compact_pools(sc, compact_bricks, compact_palette, retired));
         if (!ops.empty()) {
             DeviceBuffer d_ops;
             TRY(d_ops.ensure(ops.size() * sizeof(CubeDelta)));
@@ -1412,83 +1483,93 @@ aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb
 aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks) {
     if (n_blocks && !descs) return fail(AICB_ERR_INVALID, "NULL argument");
     if (n_blocks == 0) return AICB_OK;
+    const SpaceHost &h = *r.scene[0]->host;
     FlatBlocks f;
     TRY(flatten_placeable(r, descs, n_blocks, nullptr, &f));
+    // u16 cells hold ids below 16384 (scenes_create): a table that grows past that takes u32 cells, re-encoded behind
+    // every queued cube update of each context
     for (size_t i = 0; i < r.n; i++) {
         aicb_scene *sc = r.scene[i];
         aicb_ctx *ctx = r.ctx[i];
-        cudaStream_t stream = ctx->stream.get();
+        if (sc->ds.wide_cells || h.block_count() + n_blocks <= 16384) continue;
         CU(cudaSetDevice(ctx->device));
-        Retired retired{ctx, {}};
-        // u16 cells hold ids below 16384 (scenes_create): a table that grows past that takes u32 cells, re-encoded
-        // behind every queued cube update of this context
-        if (!sc->ds.wide_cells && sc->blocks.block_count() + n_blocks > 16384) {
-            if (sc->volume) {
-                DeviceBuffer wide;
-                TRY(wide.ensure(sc->volume * 4));
-                const size_t want = (std::max<size_t>(sc->volume / 8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
-                widen_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, stream>>>(
-                    sc->d_cells.get<const uint16_t>(), wide.get<uint32_t>(), sc->volume);
-                CU(cudaGetLastError());
-                retired.bufs.push_back(std::move(sc->d_cells));
-                sc->d_cells = std::move(wide);
-                sc->ds.cells = sc->d_cells.get();
-                sc->device_bytes += sc->volume * 2;
-            }
-            sc->ds.wide_cells = 1;
+        if (h.volume) {
+            Retired retired{ctx, {}};
+            DeviceBuffer wide;
+            TRY(wide.ensure(h.volume * 4));
+            const size_t want = (std::max<size_t>(h.volume / 8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
+            widen_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, ctx->stream.get()>>>(
+                sc->d_cells.get<const uint16_t>(), wide.get<uint32_t>(), h.volume);
+            CU(cudaGetLastError());
+            retired.bufs.push_back(std::move(sc->d_cells));
+            sc->d_cells = std::move(wide);
+            sc->ds.cells = sc->d_cells.get();
+            sc->device_bytes += h.volume * 2;
         }
-        TRY(place(sc, f, nullptr, retired));
-        CU(cudaEventRecord(ctx->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
+        sc->ds.wide_cells = 1;
     }
-    return AICB_OK;
+    return place(r, f, nullptr);
 }
 
 // Mutation::fill_uniform over the whole Space (space.rs:1461-1474), the source of SpaceChange::EveryBlock: the table
 // becomes [block] in exact-size buffers, as a new scene's, and every cell id 0 with its kind, written on the device
 // (u32 cells go back to u16: a one-block table fits them).  Light is not touched.  Each replica's context is waited for
-// first, since the table and the cells are replaced, and the call returns once its writes are done.  On each replica
-// the allocations come before any change, so a failure leaves that replica as it was.
+// first, since the table and the cells are replaced, and the call returns once its writes are done.  Every replica's
+// new arrays are allocated before any replica changes, so a failure leaves the scene as it was.
 aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block) {
     if (!block) return fail(AICB_ERR_INVALID, "NULL argument");
+    const SpaceHost empty;   // an empty table's bookkeeping, which the new tables are placed against
     FlatBlocks f;
-    TRY(flatten_blocks(BlockTable(), block, 1, nullptr, &f));
+    TRY(flatten_blocks(empty, block, 1, nullptr, &f));
     const uint32_t word = cell_word(0, f.kinds[0], false);
+    SpaceHost &h = *r.scene[0]->host;
+    struct Fresh {
+        BlockTable table;
+        DeviceBuffer narrow;   // the u16 cells of a replica that has u32 cells
+    };
+    std::vector<Fresh> fresh(r.n);
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.ctx[i]->device));
+        TRY(wait_context(r.ctx[i]));
+        Retired retired{r.ctx[i], {}};   // (a new table replaces no array)
+        aicb_status st = AICB_OK;
+        if (r.scene[i]->ds.wide_cells && h.volume) st = fresh[i].narrow.ensure(h.volume * 2);
+        if (st == AICB_OK) st = room(fresh[i].table, empty, f, nullptr, r.ctx[i]->stream.get(), retired);
+        if (st != AICB_OK) return free_each(r, fresh, st);
+    }
     for (size_t i = 0; i < r.n; i++) {
         aicb_scene *sc = r.scene[i];
         aicb_ctx *ctx = r.ctx[i];
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
-        TRY(wait_context(ctx));
         Retired retired{ctx, {}};
-        DeviceBuffer narrow;
-        if (sc->ds.wide_cells && sc->volume) TRY(narrow.ensure(sc->volume * 2));
-        BlockTable old = std::move(sc->blocks);
-        sc->blocks = BlockTable();
-        const aicb_status st = place(sc, f, nullptr, retired);
-        if (st != AICB_OK) {
-            sc->blocks = std::move(old);
-            sc->blocks.bind(sc->ds);
-            return st;
-        }
+        BlockTable &old = sc->blocks;
         for (DeviceBuffer *b : {&old.blocks, &old.blk_tab, &old.light, &old.bricks, &old.palette, &old.pal_tab})
             if (*b) retired.bufs.push_back(std::move(*b));
-        if (narrow) {
+        sc->blocks = std::move(fresh[i].table);
+        sc->blocks.bind(sc->ds);
+        TRY(copy(sc->blocks, empty, f, nullptr, stream));
+        if (fresh[i].narrow) {
             retired.bufs.push_back(std::move(sc->d_cells));
-            sc->d_cells = std::move(narrow);
+            sc->d_cells = std::move(fresh[i].narrow);
             sc->ds.cells = sc->d_cells.get();
-            sc->device_bytes -= sc->volume * 2;
+            sc->device_bytes -= h.volume * 2;
         }
         sc->ds.wide_cells = 0;
-        if (sc->volume) {
-            const size_t want = (std::max<size_t>(sc->volume / 8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
-            fill_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, stream>>>(sc->d_cells.get<uint16_t>(), sc->volume,
+        if (h.volume) {
+            const size_t want = (std::max<size_t>(h.volume / 8, 1) + 255) / 256, cap = (size_t)ctx->num_sms * 16;
+            fill_cells_kernel<<<(unsigned)std::min(want, cap), 256, 0, stream>>>(sc->d_cells.get<uint16_t>(), h.volume,
                                                                                   word);
             CU(cudaGetLastError());
         }
-        sc->h_ids.assign(sc->volume, 0);
         CU(cudaEventRecord(ctx->ev_delta.get(), stream));
         TRY(wait_context(ctx));   // the call returns once its writes are done
     }
+    h.kind.clear();
+    h.extent.clear();
+    h.n_bricks = h.n_palette = h.dead_bricks = h.dead_pal = 0;
+    book(h, f, nullptr);
+    h.h_ids.assign(h.volume, 0);
     return AICB_OK;
 }
 
@@ -1503,7 +1584,8 @@ aicb_status scenes_set_physics(Replicas r, const aicb_sky *sky, uint8_t light_ma
     bool same_sky = next.sky_kind == cur.sky_kind;
     for (int k = 0; k < (next.sky_kind ? 8 : 1); k++)   // Uniform's colour, or the eight octants'
         for (int i = 0; i < 3; i++) same_sky = same_sky && next.sky_colors[k][i] == cur.sky_colors[k][i];
-    if (same_sky && light_max_distance == r.scene[0]->light_max_distance) return AICB_OK;   // no SpaceChange::Physics
+    if (same_sky && light_max_distance == r.scene[0]->host->light_max_distance)
+        return AICB_OK;   // no SpaceChange::Physics
     for (size_t i = 0; i < r.n; i++) {
         CU(cudaSetDevice(r.ctx[i]->device));
         TRY(wait_context(r.ctx[i]));
@@ -1517,18 +1599,19 @@ aicb_status scenes_set_physics(Replicas r, const aicb_sky *sky, uint8_t light_ma
 // (launch_trace).  A replica with no light volume gets one.
 aicb_status scenes_upload_light(Replicas r, const uint8_t (*light)[4], size_t n_texels) {
     if (!light) return fail(AICB_ERR_INVALID, "NULL argument");
-    if (n_texels != r.scene[0]->volume) return fail(AICB_ERR_INVALID, "light volume size mismatch");
+    const size_t volume = r.scene[0]->host->volume;
+    if (n_texels != volume) return fail(AICB_ERR_INVALID, "light volume size mismatch");
     for (size_t i = 0; i < r.n; i++) {
         aicb_scene *s = r.scene[i];
         cudaStream_t stream = r.ctx[i]->stream.get();
         CU(cudaSetDevice(r.ctx[i]->device));
-        if (!s->d_light && s->volume) {
-            TRY(s->d_light.ensure(s->volume * 4));
-            s->device_bytes += s->volume * 4;
+        if (!s->d_light && volume) {
+            TRY(s->d_light.ensure(volume * 4));
+            s->device_bytes += volume * 4;
             s->ds.light = s->d_light.get<uint32_t>();
         }
-        if (s->volume) {
-            CU(cudaMemcpyAsync(s->d_light.get(), light, s->volume * 4, cudaMemcpyHostToDevice, stream));
+        if (volume) {
+            CU(cudaMemcpyAsync(s->d_light.get(), light, volume * 4, cudaMemcpyHostToDevice, stream));
             CU(cudaEventRecord(r.ctx[i]->ev_delta.get(), stream));
             CU(cudaStreamSynchronize(stream));
         }
@@ -1631,7 +1714,7 @@ void aicb_scene_destroy(aicb_scene *s) {
     delete s;
 }
 
-uint64_t aicb_scene_device_bytes(const aicb_scene *s) { return s ? s->device_bytes + s->blocks.bytes() : 0; }
+uint64_t aicb_scene_device_bytes(const aicb_scene *s) { return s ? s->device_bytes + s->host->table_bytes() : 0; }
 
 aicb_status aicb_scene_set_physics(aicb_scene *s, const aicb_sky *sky, uint8_t light_max_distance) {
     return on_scene(s, [&](Replicas r) { return scenes_set_physics(r, sky, light_max_distance); });

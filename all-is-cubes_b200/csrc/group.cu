@@ -286,7 +286,7 @@ int aicb_group_size(const aicb_group *g) { return g ? (int)g->ctx.size() : 0; }
 
 void aicb_group_scene_destroy(aicb_group_scene *gs) {
     if (!gs) return;
-    for (aicb_scene *s : gs->scene) aicb_scene_destroy(s);
+    for (size_t i = gs->scene.size(); i-- > 0;) aicb_scene_destroy(gs->scene[i]);   // replica 0, the owner, last
     delete gs;
 }
 
@@ -358,7 +358,7 @@ aicb_status aicb_group_scene_fill_uniform(aicb_group_scene *gs, const aicb_block
 aicb_status aicb_group_scene_set_physics(aicb_group_scene *gs, const aicb_sky *sky, uint8_t light_max_distance) {
     return on_group(gs, false, [&](Replicas r) {
         // a reinitialisation runs as aicb_group_light_fast_evaluate does, over the light calls' peers
-        if (light_max_distance && light_max_distance != r.scene[0]->light_max_distance)
+        if (light_max_distance && light_max_distance != r.scene[0]->host->light_max_distance)
             TRY(ensure_light_peers(gs->group));
         return scenes_set_physics(r, sky, light_max_distance);
     });

@@ -217,11 +217,11 @@ struct aicb_ctx {
     std::mutex mu;
 };
 
-// A scene's block table: everything indexed by block id or by pool offset, on the device and on the host.  It is
-// written in one way (aicb200.cu): definitions are flattened against the table, then placed in it, appended at the
-// next ids or written over existing ones, with their voxel data appended to the pools.  Elements in use: per block id,
-// block_count(); in the pools, n_bricks and n_palette.  The buffers may be larger: they grow geometrically
-// (grow_buffer), to multiples of 16 bytes.
+// A scene's block table: everything indexed by block id or by pool offset, on the device.  It is written in one way
+// (aicb200.cu): definitions are flattened against the table's bookkeeping (SpaceHost), then placed in it, appended at
+// the next ids or written over existing ones, with their voxel data appended to the pools.  Elements in use: per block
+// id, SpaceHost::block_count(); in the pools, SpaceHost::n_bricks and n_palette.  The buffers may be larger: they grow
+// geometrically (grow_buffer), to multiples of 16 bytes.
 //
 // Each id's extent in both pools is recorded.  A definition written over an id makes its old extents dead; once a
 // pool's dead part exceeds its live part, the pool is compacted (compact_pools): its live extents are gathered on the
@@ -231,9 +231,9 @@ struct aicb_ctx {
 // aicb_scene_update_blocks waits anyway.
 //
 // The brick pool holds one word per voxel in one of two forms (trace_kernel.cuh, BRICK_WIDE): u16 words while every
-// block's palette has at most 32768 entries, u32 words once a block with more is placed (wide_bricks).  A pool widens
-// in place (widen_bricks_kernel) and stays wide until fill_uniform replaces the table.  Positions and lengths in the
-// pool are counted in words of either form.
+// block's palette has at most 32768 entries, u32 words once a block with more is placed (SpaceHost::wide_bricks).  A
+// pool widens in place (widen_bricks_kernel) and stays wide until fill_uniform replaces the table.  Positions and
+// lengths in the pool are counted in words of either form.
 struct BlockTable {
     struct Extent {
         uint32_t brick_off, n_bricks;   // words of the brick pool
@@ -243,23 +243,10 @@ struct BlockTable {
     DeviceBuffer blocks;    // per block id: BlockRec
     DeviceBuffer blk_tab;   // per block id: the pal_tab pair and the palette entry of single-voxel blocks
     DeviceBuffer light;     // per block id: LightBlockDev (light propagation)
-    DeviceBuffer bricks;    // voxel words of the recursive blocks: u16, or u32 if wide_bricks
+    DeviceBuffer bricks;    // voxel words of the recursive blocks: u16, or u32 if wide
     DeviceBuffer palette;   // two float4 per palette entry
     DeviceBuffer pal_tab;   // per palette entry: {alpha, log2(1 - alpha) bound} (marching kernel)
-    std::vector<uint8_t> kind;           // per block id: its kind, which its cubes' cell words carry
-    std::vector<uint32_t> light_flags;   // per block id: bits 0-5 opaque faces, 6 all-opaque, 7 visible, 8 has emission
-    std::vector<Extent> extent;          // per block id: its voxel data in the pools
-    size_t n_bricks = 0, n_palette = 0;  // brick words, float4s
-    size_t dead_bricks = 0, dead_pal = 0;   // of those, brick words and palette entries no id's extent holds
-    bool wide_bricks = false;
 
-    size_t block_count() const { return kind.size(); }
-    size_t brick_word_bytes() const { return wide_bricks ? 4 : 2; }
-    // what aicb_scene_device_bytes counts of the table: the per-id records and the pools' elements in use, live or dead
-    size_t bytes() const {
-        return block_count() * (sizeof(aicb::BlockRec) + sizeof(float4) + sizeof(LightBlockDev)) +
-               n_bricks * brick_word_bytes() + n_palette * sizeof(float4) + n_palette / 2 * sizeof(float2);
-    }
     // the scene's pointers into the current buffers (LightParams::blocks is read from `light` by light_params)
     void bind(aicb::DeviceScene &ds) const {
         ds.blocks = blocks.get<aicb::BlockRec>();
@@ -270,11 +257,38 @@ struct BlockTable {
     }
 };
 
+// What a scene keeps on the host: the Space's size and block ids, the block table's bookkeeping and the light
+// settings.  It is the same for every replica of a group scene, so it exists once: a one-context scene owns its own,
+// and a group's replica 0 owns the group's, which the other replicas point to (aicb_group_scene_destroy destroys
+// replica 0 last).  A call changes it once, after every replica's allocations for the call have succeeded, so a failed
+// call never leaves it describing data that a replica's arrays lack.
+struct SpaceHost {
+    size_t volume = 0;
+    std::vector<uint16_t> h_ids;           // mirror of Space::contents (edits are applied in order on the host)
+    std::vector<uint8_t> kind;             // per block id: its kind, which its cubes' cell words carry
+    std::vector<BlockTable::Extent> extent;   // per block id: its voxel data in the pools
+    size_t n_bricks = 0, n_palette = 0;    // brick words, float4s
+    size_t dead_bricks = 0, dead_pal = 0;  // of those, brick words and palette entries no id's extent holds
+    bool wide_bricks = false;
+    uint32_t light_max_distance = 0;
+    uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
+
+    size_t block_count() const { return kind.size(); }
+    size_t brick_word_bytes() const { return wide_bricks ? 4 : 2; }
+    // what aicb_scene_device_bytes counts of a replica's table: the per-id records and the pools' elements in use,
+    // live or dead
+    size_t table_bytes() const {
+        return block_count() * (sizeof(aicb::BlockRec) + sizeof(float4) + sizeof(LightBlockDev)) +
+               n_bricks * brick_word_bytes() + n_palette * sizeof(float4) + n_palette / 2 * sizeof(float2);
+    }
+};
+
 struct aicb_scene {
     aicb_ctx *ctx = nullptr;
     aicb::DeviceScene ds{};
-    size_t volume = 0;
-    uint64_t device_bytes = 0;   // every array but the block table's (aicb_scene_device_bytes adds BlockTable::bytes)
+    std::unique_ptr<SpaceHost> own_host;   // a one-context scene's and a group's replica 0's; nullptr on the others
+    SpaceHost *host = nullptr;             // own_host, or replica 0's
+    uint64_t device_bytes = 0;   // every array but the block table's (aicb_scene_device_bytes adds table_bytes)
     DeviceBuffer d_cells;
     DeviceBuffer d_light;
     BlockTable blocks;
@@ -284,11 +298,7 @@ struct aicb_scene {
     uint64_t pending_pixels = 0;
     uint32_t pending_out_bytes_per_pixel = 0;
     bool pending_fused = false;    // shading and encode ran as one kernel (resolve_kernel)
-    // ---- light propagation state (light.cu) ----
-    std::vector<uint16_t> h_ids;            // host mirror of Space::contents (edits are applied in order on the host)
-    LightState light;
-    uint32_t light_max_distance = 0;
-    uint64_t light_stats[4] = {0, 0, 0, 0};  // last propagation: cube updates, chart node visits, rounds queued, device microseconds
+    LightState light;              // light propagation state (light.cu)
 };
 
 // A frame's outputs (launch_trace): `target` is TraceParams::target as the kernels see it, where they store and what
@@ -345,7 +355,7 @@ aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera 
 void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part);
 }
 
-// light.cu: the light-side record of a block definition (its flags are BlockTable::light_flags).
+// light.cu: the light-side record of a block definition.
 LightBlockDev light_block(const aicb_block_desc &b);
 
 // ---- calls over several contexts ----------------------------------------------------------------------------------
@@ -363,8 +373,9 @@ struct ContextLocks {
 
 // A scene's replicas, one per listed context (ctx[i] is scene[i]'s context), device 0's first.  Every call that acts on
 // a scene runs once over them: the one-context entry points (on_scene) and the group's (group.cu) only check the handle,
-// take the locks and build the list.  The shared function validates its other arguments against replica 0 before
-// anything changes, so a rejected call changes no replica.
+// take the locks and build the list.  The shared function validates its other arguments against the scene's host part
+// (SpaceHost) before anything changes, so a rejected call changes no replica; it changes the host part once, and its
+// loops over the replicas do device work only.
 struct Replicas {
     aicb_scene *const *scene;
     aicb_ctx *const *ctx;
@@ -381,9 +392,9 @@ aicb_status on_scene(aicb_scene *s, Call call) {
 }
 
 // aicb200.cu: creating a scene and changing it, on each of n contexts (a group scene's replicas hold identical tables,
-// cells and light).  The block definitions are validated and flattened once, against replica 0's table, a new scene's
-// cells are encoded once and a batch of cubes is deduplicated once; only then does each replica place them on its own
-// device.
+// cells and light).  The block definitions are validated and flattened once, against the table's bookkeeping, a new
+// scene's cells are encoded once and a batch of cubes is deduplicated once; only then does each replica place them on
+// its own device.
 aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out);
 aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uint16_t *ids, const uint8_t (*light)[4],
                                 size_t n);
@@ -400,13 +411,16 @@ struct RegionBox {
 // `uniform_id`) past the table.
 aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
                          RegionBox *box);
-// One replica's share of a box call, on its context's device and stream: the host mirror takes the ids row by row, the
-// ids (2 bytes per cube; none if uniform) and `light` (if given and the scene has a light volume) go through the
-// context's staging, and k_region_cells / k_region_texels write them.  With d_mask (ceil(volume / 32) words) the cubes
-// whose block id changes are marked there and counted into *d_n_changed (if given).  The caller records
-// aicb_ctx::ev_delta behind its last kernel.
+// One replica's share of a box call, on its context's device and stream: the ids (2 bytes per cube; none if uniform)
+// and `light` (if given and the scene has a light volume) go through the context's staging, and k_region_cells /
+// k_region_texels write them.  With d_mask (ceil(volume / 32) words) the cubes whose block id changes are marked there
+// and counted into *d_n_changed (if given).  The caller records aicb_ctx::ev_delta behind its last kernel, and writes
+// the host mirror once (mirror_region).
 aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *ids, uint16_t uniform_id,
                          const uint8_t (*light)[4], uint32_t *d_mask, uint32_t *d_n_changed);
+// The host mirror takes a box call's ids row by row.
+void mirror_region(SpaceHost &h, const aicb::DeviceScene &ds, const RegionBox &box, const uint16_t *ids,
+                   uint16_t uniform_id);
 // SpaceChange::CubeBlock / CubeLight for every cube of a box.
 aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
                                  const uint8_t (*light)[4]);

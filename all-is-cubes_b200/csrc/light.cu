@@ -1105,8 +1105,8 @@ LightParams light_params(Replicas r, size_t i) {
     P.overflow_count = i == 0 ? &P.counters->overflow : own.overflow_count.get<uint32_t>();
     P.dirty = root.dirty.get<uint32_t>();
     P.changes = root.changes.get<uint32_t>();
-    P.volume = (uint32_t)s->volume;
-    P.max_distance = s->light_max_distance;
+    P.volume = (uint32_t)s->host->volume;
+    P.max_distance = s->host->light_max_distance;
     return P;
 }
 
@@ -1213,7 +1213,7 @@ aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8
     const LightParams &P = RP[0];
     const int blocks = ctx->num_sms * 8;
     const int wide = ctx->num_sms * 8;    // 128-thread blocks of k_compute_overflow and k_apply (grid-stride)
-    const uint32_t n_tiles = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
+    const uint32_t n_tiles = (uint32_t)((s->host->volume + LIGHT_TILE - 1) / LIGHT_TILE);
     LightStepCut *cut = s->light.shared.step.get<LightStepCut>();
     uint32_t *level_starts = (uint32_t *)(cut + 1);
     uint64_t total = 0, visits = 0, rounds = 0;
@@ -1229,7 +1229,7 @@ aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8
     uint64_t left = budget ? *budget : 1;   // (the budget left at the last synchronisation)
     for (int batch = 0; batch < 100000 && left; batch++) {
         // a round takes at most the volume, so with this much left no round of the batch can cut
-        const bool may_cut = left < (uint64_t)ROUNDS_PER_SYNC * s->volume;
+        const bool may_cut = left < (uint64_t)ROUNDS_PER_SYNC * s->host->volume;
         for (int round = 0; round < ROUNDS_PER_SYNC; round++) {
             CU(cudaMemsetAsync(P.counters, 0, ROUND_LIST_COUNTERS, st));
             CU(cudaMemsetAsync(&P.counters->changed, 0, ROUND_WALK_COUNTERS, st));
@@ -1269,10 +1269,10 @@ aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8
     CU(cudaEventSynchronize(ctx->ev_light[1].get()));
     float ms = 0.0f;
     CU(cudaEventElapsedTime(&ms, ctx->ev_light[0].get(), ctx->ev_light[1].get()));
-    s->light_stats[0] = total;
-    s->light_stats[1] = visits;
-    s->light_stats[2] = rounds;
-    s->light_stats[3] = (uint64_t)(ms * 1000.0f);   // device time of the propagation in microseconds
+    s->host->light_stats[0] = total;
+    s->host->light_stats[1] = visits;
+    s->host->light_stats[2] = rounds;
+    s->host->light_stats[3] = (uint64_t)(ms * 1000.0f);   // device time of the propagation in microseconds
     if (updates_done) *updates_done = total;
     if (max_diff) *max_diff = (uint8_t)maxd;
     if (node_visits) *node_visits = visits;
@@ -1307,9 +1307,9 @@ static uint64_t own_bytes(size_t vol) { return chart_preorder_host().size() * si
 static uint64_t shared_bytes(size_t vol, bool group) { return vol * 10 + change_bytes(vol) + (group ? dirty_bytes(vol) : 0); }
 
 aicb_status LightState::ensure(aicb_scene *s, size_t replica, size_t n_replicas, const std::vector<float4> *terms) {
-    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    if (s->host->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     TRY(ensure_chart(s->ctx));
-    const size_t vol = s->volume;
+    const size_t vol = s->host->volume;
     const bool add_own = !own.sky_term, add_shared = replica == 0 && !shared.pending, group = n_replicas > 1;
     DeviceBuffer light;
     Own o;
@@ -1369,7 +1369,7 @@ aicb_status light_fast_evaluate(Replicas r) {
     CU(cudaGetLastError());
     // the other replicas take the whole volume once (peer copies)
     for (size_t i = 1; i < r.n; i++)
-        CU(cudaMemcpyAsync(r.scene[i]->d_light.get(), s->d_light.get(), s->volume * 4, cudaMemcpyDefault, stream));
+        CU(cudaMemcpyAsync(r.scene[i]->d_light.get(), s->d_light.get(), s->host->volume * 4, cudaMemcpyDefault, stream));
     CU(cudaStreamSynchronize(stream));
     return AICB_OK;
 }
@@ -1379,7 +1379,7 @@ aicb_status light_fast_evaluate(Replicas r) {
 aicb_status light_compute(Replicas r, const int32_t (*cubes)[3], size_t n, uint8_t (*out)[4]) {
     aicb_scene *s = r.scene[0];
     if (n && (!cubes || !out)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
+    if (n > s->host->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
     TRY(ensure_replicas(r));
     if (!n) return AICB_OK;
     std::vector<LightParams> RP;
@@ -1400,10 +1400,10 @@ aicb_status light_compute(Replicas r, const int32_t (*cubes)[3], size_t n, uint8
         CU(cudaMemcpy(&c, RP[i].overflow_count, 4, cudaMemcpyDeviceToHost));
         overflowed += c;
     }
-    s->light_stats[0] = n;
-    s->light_stats[1] = h.node_visits;
-    s->light_stats[2] = overflowed;   // cubes that took the lockstep walk (a chain with more terms than its slots)
-    s->light_stats[3] = 0;
+    s->host->light_stats[0] = n;
+    s->host->light_stats[1] = h.node_visits;
+    s->host->light_stats[2] = overflowed;   // cubes that took the lockstep walk (a chain with more terms than its slots)
+    s->host->light_stats[3] = 0;
     return AICB_OK;
 }
 
@@ -1414,7 +1414,7 @@ aicb_status light_compute_debug(Replicas r, const int32_t (*cubes)[3], size_t n,
                                 size_t capacity, uint32_t *ray_counts, size_t *n_rays_total) {
     aicb_scene *s = r.scene[0];
     if (!n_rays_total || (n && (!cubes || !out || !ray_counts))) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n > s->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
+    if (n > s->host->volume) return aicb_fail(AICB_ERR_INVALID, "more cubes than the Space holds");
     for (size_t i = 0; i < n; i++)
         for (int a = 0; a < 3; a++)
             if ((uint32_t)(cubes[i][a] - s->ds.lo[a]) >= (uint32_t)s->ds.size[a])
@@ -1489,10 +1489,10 @@ aicb_status light_compute_debug(Replicas r, const int32_t (*cubes)[3], size_t n,
     std::memcpy(out, texels.data(), n * 4);
     for (size_t i = 0; i < n; i++) ray_counts[i] = starts[i + 1] - starts[i];
     // aicb_light_compute's counters: the walks' are the same on one context or a group
-    s->light_stats[0] = n;
-    s->light_stats[1] = h.node_visits;
-    s->light_stats[2] = h.overflow;
-    s->light_stats[3] = 0;
+    s->host->light_stats[0] = n;
+    s->host->light_stats[1] = h.node_visits;
+    s->host->light_stats[2] = h.overflow;
+    s->host->light_stats[3] = 0;
     return AICB_OK;
 }
 
@@ -1529,8 +1529,8 @@ aicb_status light_update_from_queue(Replicas r, uint64_t max_updates, aicb_light
 }
 
 // Mutation::set x n (space.rs:1346-1352 -> side_effects_of_set -> modified_cube_needs_update, updater.rs:135-173)
-// without propagation.  The list is validated and indexed before anything changes.  One pass in list order over
-// replica 0's host mirror finds the changing entries (the same-block skip) and writes the mirror, which
+// without propagation.  The list is validated and indexed before anything changes.  One pass in list order over the
+// host mirror finds the changing entries (the same-block skip) and writes the mirror, which
 // aicb_scene_update_blocks re-encodes cells from; a second pass gives each its cube's final block.  They are staged,
 // 8 bytes each, in every replica's context, behind the cube updates queued there: k_edit_cells writes the final cells
 // and k_edit_light applies the rule (DESIGN.md §4b).  Replica 0 alone touches the queue and the set.
@@ -1538,15 +1538,15 @@ aicb_status light_edit_cubes(Replicas r, const int32_t (*cubes)[3], const uint16
                              size_t *n_changed) {
     if (n && (!cubes || !new_ids)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "more than 2^32 - 1 edits");
-    aicb_scene *s = r.scene[0];
-    const DeviceScene &ds = s->ds;
+    SpaceHost &h = *r.scene[0]->host;
+    const DeviceScene &ds = r.scene[0]->ds;
     std::vector<uint32_t> idx(n);
     for (size_t i = 0; i < n; i++) {
         const uint32_t dx = (uint32_t)(cubes[i][0] - ds.lo[0]), dy = (uint32_t)(cubes[i][1] - ds.lo[1]),
                        dz = (uint32_t)(cubes[i][2] - ds.lo[2]);
         if (dx >= (uint32_t)ds.size[0] || dy >= (uint32_t)ds.size[1] || dz >= (uint32_t)ds.size[2])
             return aicb_fail(AICB_ERR_INVALID, "cube out of bounds");
-        if (new_ids[i] >= s->blocks.block_count()) return aicb_fail(AICB_ERR_INVALID, "block id out of range");
+        if (new_ids[i] >= h.block_count()) return aicb_fail(AICB_ERR_INVALID, "block id out of range");
         idx[i] = (dx * (uint32_t)ds.size[1] + dy) * (uint32_t)ds.size[2] + dz;
     }
     TRY(ensure_replicas(r));
@@ -1560,21 +1560,18 @@ aicb_status light_edit_cubes(Replicas r, const int32_t (*cubes)[3], const uint16
     EditEntry *staged = r.ctx[0]->h_delta.get<EditEntry>();
     uint32_t m = 0;
     for (size_t i = 0; i < n; i++) {
-        if (s->h_ids[idx[i]] == new_ids[i]) continue;   // Mutation::set of the same block changes nothing
-        s->h_ids[idx[i]] = new_ids[i];
+        if (h.h_ids[idx[i]] == new_ids[i]) continue;   // Mutation::set of the same block changes nothing
+        h.h_ids[idx[i]] = new_ids[i];
         staged[m++] = EditEntry{idx[i], new_ids[i], 0};
     }
-    for (uint32_t k = 0; k < m; k++) staged[k].final_id = s->h_ids[staged[k].idx];
+    for (uint32_t k = 0; k < m; k++) staged[k].final_id = h.h_ids[staged[k].idx];
     const size_t bytes = (size_t)m * sizeof(EditEntry);
     for (size_t k = 0; m && k < r.n; k++) {
         aicb_scene *sk = r.scene[k];
         aicb_ctx *c = r.ctx[k];
         cudaStream_t stream = c->stream.get();
         CU(cudaSetDevice(c->device));
-        if (k > 0) {
-            std::memcpy(c->h_delta.get(), staged, bytes);
-            for (uint32_t e = 0; e < m; e++) sk->h_ids[staged[e].idx] = staged[e].final_id;
-        }
+        if (k > 0) std::memcpy(c->h_delta.get(), staged, bytes);
         const EditEntry *d_entries = c->d_delta.get<const EditEntry>();
         CU(cudaMemcpyAsync(c->d_delta.get(), c->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
         const unsigned blocks = (m + 255) / 256;
@@ -1610,7 +1607,7 @@ aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, 
     aicb_scene *s = r.scene[0];
     std::vector<uint32_t> mask(RELIGHT_MASK_WORDS, 0u);
     for (size_t i = 0; i < n; i++) {
-        if (indices[i] >= s->blocks.block_count()) return aicb_fail(AICB_ERR_INVALID, "block index out of range");
+        if (indices[i] >= s->host->block_count()) return aicb_fail(AICB_ERR_INVALID, "block index out of range");
         mask[indices[i] >> 5] |= 1u << (indices[i] & 31u);
     }
     TRY(ensure_replicas(r));
@@ -1635,10 +1632,11 @@ aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, 
 }
 
 // Mutation::fill / fill_uniform(region) (space.rs:1392-1412, 1455-1479): Mutation::set for every cube of the box.  On
-// every replica, behind the cube updates queued on its stream: the host mirror and the cells (region_cells), the changed
-// cubes marked in the replica's overflow list (a round buffer, empty between light calls: one bit per cube of the box),
-// then the light rule on the device (k_region_light).  Replica 0 alone counts the changed cubes and touches the queue
-// and the set.  Nothing propagates; the tile bounds are rebuilt from the pending bytes by the next propagation.
+// every replica, behind the cube updates queued on its stream: the cells (region_cells), the changed cubes marked in
+// the replica's overflow list (a round buffer, empty between light calls: one bit per cube of the box), then the light
+// rule on the device (k_region_light).  Replica 0 alone counts the changed cubes and touches the queue and the set; the
+// host mirror takes the ids once.  Nothing propagates; the tile bounds are rebuilt from the pending bytes by the next
+// propagation.
 aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
                               size_t *n_changed) {
     RegionBox box;
@@ -1660,6 +1658,7 @@ aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t
         CU(cudaEventRecord(c->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
         if (i == 0) CU(cudaMemcpyAsync(&edited, &P.counters->edited, 4, cudaMemcpyDeviceToHost, stream));
     }
+    mirror_region(*r.scene[0]->host, r.scene[0]->ds, box, ids, uniform_id);
     for (size_t i = 0; i < r.n; i++) {
         CU(cudaSetDevice(r.ctx[i]->device));
         CU(cudaStreamSynchronize(r.ctx[i]->stream.get()));
@@ -1681,23 +1680,24 @@ aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t
 // and leaves every replica as it was.
 aicb_status light_set_physics(Replicas r, const DeviceScene &sky, uint32_t max_distance) {
     aicb_scene *s0 = r.scene[0];
-    const bool relight = max_distance != s0->light_max_distance;
+    SpaceHost &h = *s0->host;
+    const bool relight = max_distance != h.light_max_distance;
     const bool new_faces = std::memcmp(sky.sky_faces, s0->ds.sky_faces, sizeof sky.sky_faces) != 0;
     std::vector<float4> terms;
     if (new_faces || (relight && max_distance)) terms = sky_terms(sky.sky_faces);
     if (relight && max_distance) {
         struct Before {
             bool light, own, shared;
-            uint32_t max_distance;
             uint64_t device_bytes;
         };
         std::vector<Before> before;
         for (size_t i = 0; i < r.n; i++) {
             aicb_scene *s = r.scene[i];
             before.push_back({(bool)s->d_light, (bool)s->light.own.sky_term, (bool)s->light.shared.pending,
-                              s->light_max_distance, s->device_bytes});
-            s->light_max_distance = max_distance;
+                              s->device_bytes});
         }
+        const uint32_t before_max = h.light_max_distance;
+        h.light_max_distance = max_distance;
         const aicb_status st = ensure_replicas(r, &terms);
         if (st != AICB_OK) {
             for (size_t i = 0; i < r.n; i++) {
@@ -1709,9 +1709,9 @@ aicb_status light_set_physics(Replicas r, const DeviceScene &sky, uint32_t max_d
                 }
                 if (!before[i].own) s->light.own = LightState::Own();
                 if (!before[i].shared) s->light.shared = LightState::Shared();
-                s->light_max_distance = before[i].max_distance;
                 s->device_bytes = before[i].device_bytes;
             }
+            h.light_max_distance = before_max;
             cudaSetDevice(s0->ctx->device);
             return st;
         }
@@ -1727,7 +1727,7 @@ aicb_status light_set_physics(Replicas r, const DeviceScene &sky, uint32_t max_d
         if (new_faces && s->light.own.sky_term)
             CU(cudaMemcpy(s->light.own.sky_term.get(), terms.data(), terms.size() * sizeof(float4), cudaMemcpyHostToDevice));
         if (relight && !max_distance) {
-            const size_t vol = s->volume;
+            const size_t vol = h.volume;
             if (s->d_light) s->device_bytes -= vol * 4;
             if (s->light.own.sky_term) s->device_bytes -= own_bytes(vol);
             if (s->light.shared.pending) s->device_bytes -= shared_bytes(vol, (bool)s->light.shared.dirty);
@@ -1735,17 +1735,17 @@ aicb_status light_set_physics(Replicas r, const DeviceScene &sky, uint32_t max_d
             s->light.shared = LightState::Shared();
             s->d_light.reset();
             ds.light = nullptr;
-            s->light_max_distance = 0;
         }
     }
+    h.light_max_distance = max_distance;
     CU(cudaSetDevice(s0->ctx->device));
     if (!relight || !max_distance) return AICB_OK;
     TRY(light_fast_evaluate(r));
     // every cube is changed: whole words of the bitmap, then the cubes of a last, partial word
     uint32_t *changes = s0->light.shared.changes.get<uint32_t>();
     cudaStream_t stream = s0->ctx->stream.get();
-    const size_t whole = s0->volume / 32;
-    const uint32_t tail = (1u << (s0->volume % 32)) - 1u;
+    const size_t whole = h.volume / 32;
+    const uint32_t tail = (1u << (h.volume % 32)) - 1u;
     CU(cudaMemsetAsync(changes, 0xff, whole * 4, stream));
     if (tail) CU(cudaMemcpyAsync(changes + whole, &tail, 4, cudaMemcpyHostToDevice, stream));
     CU(cudaStreamSynchronize(stream));
@@ -1758,7 +1758,7 @@ static aicb_status queue_cubes(Replicas r, bool uninit, const QueueBox &box, uin
     aicb_scene *s = r.scene[0];
     const LightParams P = light_params(r, 0);
     cudaStream_t st = s->ctx->stream.get();
-    uint32_t tile0 = 0, tile1 = (uint32_t)((s->volume + LIGHT_TILE - 1) / LIGHT_TILE);
+    uint32_t tile0 = 0, tile1 = (uint32_t)((s->host->volume + LIGHT_TILE - 1) / LIGHT_TILE);
     if (!uninit) {   // the tiles from the box's first cube to its last
         const uint32_t sy = (uint32_t)s->ds.size[1], sz = (uint32_t)s->ds.size[2];
         tile0 = ((box.lo[0] * sy + box.lo[1]) * sz + box.lo[2]) / LIGHT_TILE;
@@ -1804,19 +1804,19 @@ aicb_status light_queue_region(Replicas r, const aicb_aab *region, uint8_t prior
 // The pending bytes are the whole queue between light calls; a scene with no light call yet has an empty queue.
 aicb_status light_download_queue(aicb_scene *s, uint8_t *priorities, size_t n_texels, size_t *n_queued) {
     if (!priorities) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n_texels != s->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
-    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    if (n_texels != s->host->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
+    if (s->host->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     if (s->light.shared.pending) {
         CU(cudaSetDevice(s->ctx->device));
         cudaStream_t st = s->ctx->stream.get();
-        CU(cudaMemcpyAsync(priorities, s->light.shared.pending.get(), s->volume, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(priorities, s->light.shared.pending.get(), s->host->volume, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
     } else {
-        std::memset(priorities, 0, s->volume);
+        std::memset(priorities, 0, s->host->volume);
     }
     if (n_queued) {
         size_t n = 0;
-        for (size_t i = 0; i < s->volume; i++) n += priorities[i] != 0;
+        for (size_t i = 0; i < s->host->volume; i++) n += priorities[i] != 0;
         *n_queued = n;
     }
     return AICB_OK;
@@ -1824,11 +1824,11 @@ aicb_status light_download_queue(aicb_scene *s, uint8_t *priorities, size_t n_te
 
 aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     if (!s || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (n_texels != s->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
+    if (n_texels != s->host->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
     if (!s->d_light) return aicb_fail(AICB_ERR_INVALID, "scene has no light volume (LightPhysics::None)");
     CU(cudaSetDevice(s->ctx->device));
     // ordered behind everything queued on the context's stream (cube deltas, propagation)
-    CU(cudaMemcpyAsync(out, s->d_light.get(), s->volume * 4, cudaMemcpyDeviceToHost, s->ctx->stream.get()));
+    CU(cudaMemcpyAsync(out, s->d_light.get(), s->host->volume * 4, cudaMemcpyDeviceToHost, s->ctx->stream.get()));
     CU(cudaStreamSynchronize(s->ctx->stream.get()));
     return AICB_OK;
 }
@@ -1836,7 +1836,7 @@ aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
 // The size of the set of changed cubes (kernels 1 and 2 of the take), behind everything queued on the context's stream;
 // the chunks' output positions stay in chunk_sums() for k_changes_emit.
 static aicb_status count_changes(const aicb_scene *s, uint32_t *n) {
-    const uint32_t n_words = (uint32_t)((s->volume + 31) / 32);
+    const uint32_t n_words = (uint32_t)((s->host->volume + 31) / 32);
     const uint32_t n_chunks = (n_words + CHANGES_CHUNK_WORDS - 1) / CHANGES_CHUNK_WORDS;
     cudaStream_t st = s->ctx->stream.get();
     uint32_t *chunk_sums = s->light.chunk_sums();   // (n_chunks + 1) * 4 <= volume / 8192 + 8 of diff's volume + 16
@@ -1850,7 +1850,7 @@ static aicb_status count_changes(const aicb_scene *s, uint32_t *n) {
 
 aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed) {
     if (!n_changed) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    if (s->host->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     *n_changed = 0;
     if (!s->light.shared.changes) return AICB_OK;   // no light call yet
     CU(cudaSetDevice(s->ctx->device));
@@ -1865,7 +1865,7 @@ aicb_status light_changes_count(const aicb_scene *s, size_t *n_changed) {
 aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texels)[4], size_t capacity, size_t *n_taken) {
     if (!n_taken) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     if (!indices != !texels) return aicb_fail(AICB_ERR_INVALID, "give both outputs, or neither to discard the set");
-    if (s->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
+    if (s->host->light_max_distance == 0) return aicb_fail(AICB_ERR_INVALID, "scene has LightPhysics::None (light_max_distance == 0)");
     *n_taken = 0;
     if (!s->light.shared.changes) return AICB_OK;
     CU(cudaSetDevice(s->ctx->device));
@@ -1877,7 +1877,7 @@ aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texel
         return aicb_fail(AICB_ERR_INVALID, "capacity is smaller than the set of changed cubes (aicb_light_changes_count)");
     }
     if (n) {
-        const uint32_t n_words = (uint32_t)((s->volume + 31) / 32);
+        const uint32_t n_words = (uint32_t)((s->host->volume + 31) / 32);
         if (indices) {
             const uint32_t n_chunks = (n_words + CHANGES_CHUNK_WORDS - 1) / CHANGES_CHUNK_WORDS;
             const LightState &L = s->light;
@@ -1897,7 +1897,7 @@ aicb_status light_take_changes(aicb_scene *s, uint32_t *indices, uint8_t (*texel
 
 aicb_status light_stats(const aicb_scene *s, uint64_t out[4]) {
     if (!out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    for (int i = 0; i < 4; i++) out[i] = s->light_stats[i];
+    for (int i = 0; i < 4; i++) out[i] = s->host->light_stats[i];
     return AICB_OK;
 }
 

@@ -732,7 +732,8 @@ aicb_status aicb_group_light_edit_and_propagate(aicb_group_scene *, const int32_
                                                 size_t n_edits, uint8_t epsilon, uint64_t *updates_done,
                                                 uint8_t *max_diff);
 /* aicb_light_edit_cubes on the group: validated against replica 0 before any replica changes; every replica writes its
- * own cells, its own host mirror and its own OPAQUE texels; device 0 alone queues and records the set. */
+ * own cells and its own OPAQUE texels, and the scene's one host mirror is written once; device 0 alone queues and
+ * records the set. */
 aicb_status aicb_group_light_edit_cubes(aicb_group_scene *, const int32_t (*cubes)[3], const uint16_t *new_ids,
                                         size_t n, size_t *n_changed_or_null);
 /* aicb_light_relight_blocks on the group: the indices are checked against replica 0's table; every replica scans its
