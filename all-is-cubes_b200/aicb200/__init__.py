@@ -81,8 +81,6 @@ def load_library() -> C.CDLL:
     lib.aicb_frame_wait_consumed.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
     lib.aicb_frame_timed_out.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_uint32)]
     lib.aicb_render_finish.argtypes = [C.c_void_p, C.POINTER(abi.RenderInfo)]
-    lib.aicb_trace_rays.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.Options), C.c_void_p,
-                                    C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(abi.RenderInfo)]
     lib.aicb_camera_look_at.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double, C.c_double,
                                         C.c_double, C.c_double, C.c_uint32, C.c_uint32, C.c_float,
                                         C.POINTER(abi.CameraData)]
@@ -95,8 +93,6 @@ def load_library() -> C.CDLL:
                                             C.POINTER(C.c_double)]
     lib.aicb_camera_project_ndc.restype = None
     lib.aicb_light_download.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
-    lib.aicb_render_text.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p, C.c_size_t,
-                                     C.POINTER(abi.RenderInfo)]
     lib.aicb_render_layers_srgb8.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_render_layers_texture.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p,
@@ -104,8 +100,6 @@ def load_library() -> C.CDLL:
                                                C.POINTER(abi.RenderInfo)]
     lib.aicb_render_layers_terminal.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p,
                                                 C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
-    lib.aicb_ortho_image_size.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
-    lib.aicb_render_orthographic.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_create.argtypes = [C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_void_p)]
     lib.aicb_group_destroy.argtypes = [C.c_void_p]
     lib.aicb_group_destroy.restype = None
@@ -122,12 +116,23 @@ def load_library() -> C.CDLL:
                                                      C.c_void_p, C.c_void_p, C.POINTER(abi.RenderInfo)]
     lib.aicb_group_render_layers_terminal.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
                                                       C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.RenderInfo)]
+    lib.aicb_group_render_colorbuf.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options),
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                               C.POINTER(abi.RenderInfo)]
+    lib.aicb_group_render_rgba16f.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p,
+                                              C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_light_chart.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_light_chart.restype = C.c_uint32
     lib.aicb_group_light_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
     # the calls of _Scene: a group scene's form of aicb_<name> is aicb_group_<name>, with the same arguments
     u64, u8, size = C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_size_t)
+    info = C.POINTER(abi.RenderInfo)
     for name, argtypes in {
+        "trace_rays": [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.Options), C.c_void_p, C.c_void_p, C.c_void_p,
+                       C.c_void_p, info],
+        "render_text": [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p, C.c_size_t, info],
+        "ortho_image_size": [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)],
+        "render_orthographic": [C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, info],
         "scene_update_cubes": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t],
         "scene_update_region": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, C.c_void_p],
         "scene_update_blocks": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t],
@@ -901,24 +906,27 @@ class SpaceRaytracer(_Scene):
     def trace_rays(self, origin_dir: np.ndarray, include_sky: bool = True, want_depth=False, want_hit=False,
                    want_steps=False):
         """SpaceRaytracer::trace_ray (sr.rs:113-120) over a batch: returns dict of arrays."""
-        od = np.ascontiguousarray(origin_dir, dtype=np.float64).reshape(-1, 6)
-        n = od.shape[0]
-        cb = np.empty((n, 4), dtype=np.float32)
-        depth = np.empty(n, dtype=np.float64) if want_depth else None
-        hit = np.empty((n, 8), dtype=np.int32) if want_hit else None
-        steps = np.empty(n, dtype=np.uint32) if want_steps else None
-        info = abi.RenderInfo()
-        opt = self.graphics_options.to_abi(include_sky)
-        _check(load_library().aicb_trace_rays(self.handle, od.ctypes.data, n, C.byref(opt), cb.ctypes.data,
-                                              depth.ctypes.data if want_depth else None,
-                                              hit.ctypes.data if want_hit else None,
-                                              steps.ctypes.data if want_steps else None, C.byref(info)))
-        return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
+        return _trace_rays(self, origin_dir, self.graphics_options.to_abi(include_sky), want_depth, want_hit, want_steps)
 
     def light_download(self) -> np.ndarray:
         out = np.zeros(self.space.size + (4,), dtype=np.uint8)
         _check(load_library().aicb_light_download(self.handle, out.ctypes.data, out.size // 4))
         return out
+
+
+def _trace_rays(scene, origin_dir, opt, want_depth, want_hit, want_steps) -> dict:
+    """aicb_trace_rays on a SpaceRaytracer, aicb_group_trace_rays on a GroupScene."""
+    od = np.ascontiguousarray(origin_dir, dtype=np.float64).reshape(-1, 6)
+    n = od.shape[0]
+    cb = np.empty((n, 4), dtype=np.float32)
+    depth = np.empty(n, dtype=np.float64) if want_depth else None
+    hit = np.empty((n, 8), dtype=np.int32) if want_hit else None
+    steps = np.empty(n, dtype=np.uint32) if want_steps else None
+    info = abi.RenderInfo()
+    _check(scene._fn("trace_rays")(scene.handle, od.ctypes.data, n, C.byref(opt), cb.ctypes.data,
+                                   depth.ctypes.data if want_depth else None, hit.ctypes.data if want_hit else None,
+                                   steps.ctypes.data if want_steps else None, C.byref(info)))
+    return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
 
 
 NO_WORLD_TO_SHOW_SRGB8 = (0xBC, 0xBC, 0xBC, 0xFF)   # content/palette.rs:76
@@ -1043,19 +1051,21 @@ def pixel_picker_order(width: int, height: int, count: Optional[int] = None) -> 
     return sorted_pixels[lin].astype(np.uint32)
 
 
-def render_orthographic(rt: "SpaceRaytracer", resolution: int = 32) -> "Rendering":
-    """raytracer::ortho::render_orthographic (ortho.rs:30-84): the five-view pixel-perfect image of the whole Space."""
+def render_orthographic(rt, resolution: int = 32) -> "Rendering":
+    """raytracer::ortho::render_orthographic (ortho.rs:30-84): the five-view pixel-perfect image of the whole Space.
+    `rt`: a SpaceRaytracer, or a GroupScene (its devices share the views' pixels; the same image)."""
     w, h = C.c_uint32(0), C.c_uint32(0)
-    _check(load_library().aicb_ortho_image_size(rt.handle, resolution, C.byref(w), C.byref(h)))
+    _check(rt._fn("ortho_image_size")(rt.handle, resolution, C.byref(w), C.byref(h)))
     out = np.zeros((h.value, w.value, 4), dtype=np.uint8)
     info = abi.RenderInfo()
-    _check(load_library().aicb_render_orthographic(rt.handle, resolution, out.ctypes.data, w.value * h.value, C.byref(info)))
+    _check(rt._fn("render_orthographic")(rt.handle, resolution, out.ctypes.data, w.value * h.value, C.byref(info)))
     return Rendering((w.value, h.value), out, int(info.flaws), RenderInfo.from_abi(info))
 
 
-def print_space(space: "Space", direction, block_chars: dict, rt: "SpaceRaytracer" = None) -> list:
+def print_space(space: "Space", direction, block_chars: dict, rt=None) -> list:
     """raytracer::print_space (text.rs:139-180): the 80 x 40 character image of a Space seen from `direction`, one
-    string per row.  `block_chars` maps a block index to its character (what D::from_block gives each block)."""
+    string per row.  `block_chars` maps a block index to its character (what D::from_block gives each block).
+    `rt`: a SpaceRaytracer or a GroupScene of `space` (None: a new SpaceRaytracer)."""
     opts = GraphicsOptions()
     cam = Camera(opts, Viewport((40.0, 40.0), (80, 40)))
     center = [space.lower[a] + space.size[a] / 2.0 for a in range(3)]
@@ -1063,7 +1073,7 @@ def print_space(space: "Space", direction, block_chars: dict, rt: "SpaceRaytrace
     rt = rt or SpaceRaytracer(space, opts)
     o = opts.to_abi(True)
     out = np.zeros(80 * 40, dtype=np.int32)
-    _check(load_library().aicb_render_text(rt.handle, C.byref(cam.data), C.byref(o), out.ctypes.data, out.size, None))
+    _check(rt._fn("render_text")(rt.handle, C.byref(cam.data), C.byref(o), out.ctypes.data, out.size, None))
     special = {abi.TEXT_ENTERED_SPACE: " ", abi.TEXT_EMPTY: ".", abi.TEXT_INCOMPLETE: "X"}
     return ["".join(special[v] if v < 0 else block_chars[int(v)] for v in out[r * 80:(r + 1) * 80]) for r in range(40)]
 
@@ -1103,7 +1113,8 @@ class DeviceGroup:
     """Several GPUs driven from this one process through the C ABI (csrc/group.cu): scene replicated, frame cut into
     interleaved row strips, pixels stored straight into device 0's frame over NVLink.
 
-    update() / draw(): one world-only scene.  add_scene() / render_layers() / render_layers_texture() /
+    update() / draw(): one world-only scene, which draw_colorbuf() / draw_rgba16f() / trace_rays() / render_text() /
+    render_orthographic() also draw, with RtRenderer's and SpaceRaytracer's results.  add_scene() / render_layers() / render_layers_texture() /
     render_layers_terminal(): any number of replicated scenes (GroupScene) drawn through the layers as the module's
     functions of the same names draw them on one context."""
 
@@ -1150,6 +1161,57 @@ class DeviceGroup:
         _check(load_library().aicb_group_render_srgb8(self.scene.handle if self.scene else None, C.byref(camera.data),
                                                      C.byref(o), out.ctypes.data, w * h, C.byref(info)))
         return Rendering((w, h), out, int(info.flaws), RenderInfo.from_abi(info))
+
+    def _handle(self):
+        return self.scene.handle if self.scene else None
+
+    def draw_colorbuf(self, camera: "Camera", options: "GraphicsOptions", want_depth=True, want_hit=True,
+                      want_steps=True) -> dict:
+        """RtRenderer.draw_colorbuf of the whole frame on the group (same dict)."""
+        n = camera.data.fb_width * camera.data.fb_height
+        cb = np.empty((n, 4), dtype=np.float32)
+        depth = np.empty(n, dtype=np.float64) if want_depth else None
+        hit = np.empty((n, 8), dtype=np.int32) if want_hit else None
+        steps = np.empty(n, dtype=np.uint32) if want_steps else None
+        info = abi.RenderInfo()
+        o = options.to_abi(True)
+        _check(load_library().aicb_group_render_colorbuf(self._handle(), C.byref(camera.data), C.byref(o),
+                                                         cb.ctypes.data, depth.ctypes.data if want_depth else None,
+                                                         hit.ctypes.data if want_hit else None,
+                                                         steps.ctypes.data if want_steps else None, n, C.byref(info)))
+        return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
+
+    def draw_rgba16f(self, camera: "Camera", options: "GraphicsOptions") -> np.ndarray:
+        """RtRenderer.draw_rgba16f of the whole frame on the group: float16 [h, w, 4]."""
+        w, h = camera.data.fb_width, camera.data.fb_height
+        out = np.empty((h, w, 4), dtype=np.float16)
+        o = options.to_abi(True)
+        _check(load_library().aicb_group_render_rgba16f(self._handle(), C.byref(camera.data), C.byref(o),
+                                                        out.ctypes.data, w * h, None))
+        return out
+
+    def trace_rays(self, origin_dir: np.ndarray, options: "GraphicsOptions", include_sky: bool = True, want_depth=False,
+                   want_hit=False, want_steps=False) -> dict:
+        """SpaceRaytracer.trace_rays on the group: the batch is cut into ranges of whole warps, one per device."""
+        if not self.scene:
+            raise AicbError(abi.ERR_INVALID, "trace_rays() before update()")
+        return _trace_rays(self.scene, origin_dir, options.to_abi(include_sky), want_depth, want_hit,
+                           want_steps)
+
+    def render_text(self, camera: "Camera", options: "GraphicsOptions") -> np.ndarray:
+        """aicb_group_render_text: per pixel the CharacterBuf state (block index or abi.TEXT_*), int32 [h, w]."""
+        w, h = camera.data.fb_width, camera.data.fb_height
+        out = np.zeros((h, w), dtype=np.int32)
+        o = options.to_abi(True)
+        _check(load_library().aicb_group_render_text(self._handle(), C.byref(camera.data), C.byref(o), out.ctypes.data,
+                                                     w * h, None))
+        return out
+
+    def render_orthographic(self, resolution: int = 32) -> "Rendering":
+        """render_orthographic of the group's scene."""
+        if not self.scene:
+            raise AicbError(abi.ERR_INVALID, "render_orthographic() before update()")
+        return render_orthographic(self.scene, resolution)
 
     def close(self):
         for s in self.scenes:

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -208,6 +208,12 @@ EXPORTED_SYMBOLS = [
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",
     "aicb_group_render_layers_terminal",
+    "aicb_group_render_colorbuf",
+    "aicb_group_render_rgba16f",
+    "aicb_group_trace_rays",
+    "aicb_group_render_text",
+    "aicb_group_ortho_image_size",
+    "aicb_group_render_orthographic",
     "aicb_group_light_fast_evaluate",
     "aicb_group_light_compute",
     "aicb_group_light_compute_debug",

@@ -247,7 +247,7 @@ static kernel_fn kernel_of() {
     return trace_kernel<V, W, AUX, B>;
 }
 
-// The marching kernel of a frame: Volumetric transparency, u32 cells, the step counters (render_aux), u32 brick words.
+// The marching kernel of a frame: Volumetric transparency, u32 cells, the step counters (AuxOutputs), u32 brick words.
 static kernel_fn select_kernel(bool volumetric, bool wide, bool aux, bool wide_bricks) {
 #define PICK(V, W, A, B) if (volumetric == V && wide == W && aux == A && wide_bricks == B) return kernel_of<V, W, A, B>();
     PICK(false, false, false, false) PICK(false, false, true, false) PICK(false, true, false, false)
@@ -513,7 +513,7 @@ static __global__ void rebase_blocks_kernel(BlockRec *blocks, float4 *blk_tab, c
     if ((r.kind_res & 0xffu) == KIND_SINGLE) blk_tab[i].z = __uint_as_float(off[i].y);
 }
 
-static aicb_status validate_options(const aicb_options *o) {
+aicb_status validate_options(const aicb_options *o) {
     if (!o) return fail(AICB_ERR_INVALID, "options is NULL");
     if (o->fog > AICB_FOG_PHYSICAL) return fail(AICB_ERR_INVALID, "bad fog option");
     if (o->lighting_display > AICB_LIGHT_BOUNCE) return fail(AICB_ERR_INVALID, "bad lighting option");
@@ -1822,45 +1822,14 @@ aicb_status aicb_render_rgba16f(aicb_scene *s, const aicb_camera *cam, const aic
     return AICB_OK;
 }
 
-static aicb_status render_aux(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
-                              const double *d_rays, uint64_t n_rays, float (*out_cb)[4], double *depth, aicb_hit *hit,
-                              uint32_t *steps, size_t n, aicb_render_info *info) {
-    aicb_ctx *ctx = s->ctx;
-    // layout of the aux staging buffer: colorbuf | depth | hit | steps
-    size_t off_cb = 0, off_depth = off_cb + n * 16, off_hit = off_depth + n * 8, off_steps = off_hit + n * sizeof(aicb_hit);
-    size_t total = off_steps + n * 4 + 16;
-    TRY(ctx->d_aux.ensure(total));
-    char *base = ctx->d_aux.get<char>();
-    FramePart part{s, shard};
-    Outputs &o = part.out;
-    o.target.out_colorbuf = (float4 *)(base + off_cb);
-    o.target.out_depth = (double *)(base + off_depth);
-    o.target.out_hit = (aicb_hit *)(base + off_hit);
-    o.target.out_steps = (uint32_t *)(base + off_steps);
-    o.rays = d_rays;
-    o.n_rays = n_rays;
-    o.aux = true;
-    TRY(aicb_trace_pass(&part, 1, cam, opt, info != nullptr));
-    if (info) *info = part.info;
-    if (n) {
-        const TargetParams &t = o.target;
-        if (out_cb) CU(cudaMemcpyAsync(out_cb, t.out_colorbuf, n * 16, cudaMemcpyDeviceToHost, ctx->stream.get()));
-        if (depth) CU(cudaMemcpyAsync(depth, t.out_depth, n * 8, cudaMemcpyDeviceToHost, ctx->stream.get()));
-        if (hit) CU(cudaMemcpyAsync(hit, t.out_hit, n * sizeof(aicb_hit), cudaMemcpyDeviceToHost, ctx->stream.get()));
-        if (steps) CU(cudaMemcpyAsync(steps, t.out_steps, n * 4, cudaMemcpyDeviceToHost, ctx->stream.get()));
-    }
-    CU(cudaStreamSynchronize(ctx->stream.get()));
-    return AICB_OK;
-}
-
 aicb_status aicb_render_colorbuf(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
                                  const aicb_shard *shard, float (*out_cb)[4], double *depth, aicb_hit *hit,
                                  uint32_t *steps, size_t out_len, aicb_render_info *info) {
     aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
-    std::lock_guard<std::mutex> lock(s->ctx->mu);
-    CU(cudaSetDevice(s->ctx->device));
-    return render_aux(s, cam, opt, shard, nullptr, 0, out_cb, depth, hit, steps, out_len, info);
+    return on_scene(s, [&](Replicas r) {
+        return frame_colorbuf(r, cam, opt, shard, {out_cb, depth, hit, steps}, out_len, info);
+    });
 }
 
 aicb_status aicb_render_srgb8_device(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
@@ -2036,17 +2005,7 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
     aicb_status st = aicb_check_render_args(s, cam, opt, nullptr, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
-    aicb_ctx *ctx = s->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    TRY(ctx->d_aux.ensure(out_len * 4 + 16));
-    FramePart part{s};
-    part.out.target.out_text = ctx->d_aux.get<int32_t>();
-    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
-    if (st != AICB_OK) return st;
-    if (info) *info = part.info;
-    if (out_len) CU(cudaMemcpy(out, ctx->d_aux.get(), out_len * 4, cudaMemcpyDeviceToHost));
-    return AICB_OK;
+    return on_scene(s, [&](Replicas r) { return frame_text(r, cam, opt, out, out_len, info); });
 }
 
 // Arguments shared by the layered entry points: at least one layer (or the paint colour), complete layers, one context
@@ -2361,48 +2320,111 @@ aicb_status aicb_ortho_image_size(const aicb_scene *s, uint32_t resolution, uint
     return AICB_OK;
 }
 
-aicb_status aicb_render_orthographic(aicb_scene *s, uint32_t resolution, uint8_t (*out)[4], size_t out_len,
-                                     aicb_render_info *info) {
+}  // extern "C"
+
+// The five views of an orthographic image for its kernels: view v's pixel (px, py) is number first[v] + py * vw[v] + px
+// of the views' pixels, and lands at (oy[v] + py) * W + ox[v] + px of the image.
+struct OrthoViews {
+    uint32_t vw[5], vh[5], ox[5], oy[5];
+    uint64_t first[6];
+    uint32_t W;
+    double inv, lb[3], ub[3];
+};
+
+static __device__ __forceinline__ uint32_t ortho_view_of(const OrthoViews &V, uint64_t k) {
+    uint32_t v = 0;
+    while (k >= V.first[v + 1]) v++;
+    return v;
+}
+
+// Ray k of the views' pixels, for k in [begin, begin + n): the pixel centre, y flipped, scaled to cubes
+// (ortho.rs:278-283), then the view's rotation and corner.  Every sum and product is rounded on its own, as the
+// reference rounds them: contracted into an FMA, lb + (px + 0.5) * inv could round differently.  (The library is
+// built with -fmad=false; the explicit roundings keep this kernel exact without it.)
+static __global__ void __launch_bounds__(256) ortho_rays_kernel(const OrthoViews V, uint64_t begin, uint32_t n,
+                                                                double *__restrict__ rays) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t k = begin + i;
+    const uint32_t v = ortho_view_of(V, k);
+    const uint64_t local = k - V.first[v];
+    const uint32_t px = (uint32_t)(local % V.vw[v]), py = (uint32_t)(local / V.vw[v]);
+    const double u = __dmul_rn(__dadd_rn((double)px, 0.5), V.inv), w = -__dmul_rn(__dadd_rn((double)py, 0.5), V.inv);
+    auto add = [](double a, double b) { return __dadd_rn(a, b); };
+    auto sub = [](double a, double b) { return __dsub_rn(a, b); };
+    const double *lb = V.lb, *ub = V.ub;
+    double o[3], d[3] = {0.0, 0.0, 0.0};
+    switch (v) {
+        case 0: o[0] = add(lb[0], u); o[1] = ub[1]; o[2] = sub(lb[2], w); d[1] = -1.0; break;   // top: Face::PY
+        case 1: o[0] = lb[0]; o[1] = add(ub[1], w); o[2] = add(lb[2], u); d[0] = 1.0; break;    // left: Face::NX
+        case 2: o[0] = add(lb[0], u); o[1] = add(ub[1], w); o[2] = ub[2]; d[2] = -1.0; break;   // front: Face::PZ
+        case 3: o[0] = ub[0]; o[1] = add(ub[1], w); o[2] = sub(ub[2], u); d[0] = -1.0; break;   // right: Face::PX
+        default: o[0] = add(lb[0], u); o[1] = lb[1]; o[2] = add(ub[2], w); d[1] = 1.0; break;   // bottom: Face::NY
+    }
+    double *r = rays + 6 * (size_t)i;
+    for (int a = 0; a < 3; a++) {
+        r[a] = o[a];
+        r[3 + a] = d[a];
+    }
+}
+
+// The traced pixels, in the rays' order, to their places in the image.
+static __global__ void __launch_bounds__(256) ortho_place_kernel(const OrthoViews V, const uchar4 *__restrict__ traced,
+                                                                 uint64_t n, uchar4 *__restrict__ image) {
+    const uint64_t k = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const uint32_t v = ortho_view_of(V, k);
+    const uint64_t local = k - V.first[v];
+    const uint32_t px = (uint32_t)(local % V.vw[v]), py = (uint32_t)(local / V.vw[v]);
+    image[(size_t)(V.oy[v] + py) * V.W + V.ox[v] + px] = traced[k];
+}
+
+// The views' rays are built on the device, each context building its range of whole warps of them into its d_aux, and
+// go through the explicit-ray path; every context stores its pixels in ray order at its range's offset in device 0's
+// d_out.  Device 0 clears the image to Rgba::TRANSPARENT first and places the pixels once every context is done.
+aicb_status ortho_srgb8(Replicas r, uint32_t resolution, uint8_t (*out)[4], size_t out_len, aicb_render_info *info) {
+    aicb_scene *s = r.scene[0];
     uint32_t W = 0, H = 0;
     aicb_status st = aicb_ortho_image_size(s, resolution, &W, &H);
     if (st != AICB_OK) return st;
     if (out_len != (size_t)W * H) return fail(AICB_ERR_INVALID, "Viewport size does not match output buffer length");
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
-    aicb_ctx *ctx = s->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
     const DeviceScene &ds = s->ds;
-    uint32_t vw[5], vh[5], ox[5], oy[5];
-    ortho_views(ds, resolution, vw, vh, ox, oy, &W, &H);
-    const double inv = 1.0 / (double)resolution;   // (a power of two: exact)
-    const double lb[3] = {(double)ds.lo[0], (double)ds.lo[1], (double)ds.lo[2]};
-    const double ub[3] = {(double)ds.lo[0] + ds.size[0], (double)ds.lo[1] + ds.size[1], (double)ds.lo[2] + ds.size[2]};
-    std::vector<double> rays;
-    std::vector<uint32_t> where;
-    for (int v = 0; v < 5; v++) {
-        for (uint32_t py = 0; py < vh[v]; py++)
-            for (uint32_t px = 0; px < vw[v]; px++) {
-                // pixel centre, y flipped, scaled to cubes (ortho.rs:278-283); then the view's rotation and corner
-                const double u = ((double)px + 0.5) * inv, w = -(((double)py + 0.5) * inv);
-                double o[3], d[3] = {0, 0, 0};
-                switch (v) {
-                    case 0: o[0] = lb[0] + u; o[1] = ub[1]; o[2] = lb[2] - w; d[1] = -1.0; break;   // top: Face::PY
-                    case 1: o[0] = lb[0]; o[1] = ub[1] + w; o[2] = lb[2] + u; d[0] = 1.0; break;    // left: Face::NX
-                    case 2: o[0] = lb[0] + u; o[1] = ub[1] + w; o[2] = ub[2]; d[2] = -1.0; break;   // front: Face::PZ
-                    case 3: o[0] = ub[0]; o[1] = ub[1] + w; o[2] = ub[2] - u; d[0] = -1.0; break;   // right: Face::PX
-                    default: o[0] = lb[0] + u; o[1] = lb[1]; o[2] = ub[2] + w; d[1] = 1.0; break;   // bottom: Face::NY
-                }
-                for (int a = 0; a < 3; a++) rays.push_back(o[a]);
-                for (int a = 0; a < 3; a++) rays.push_back(d[a]);
-                where.push_back((oy[v] + py) * W + (ox[v] + px));
-            }
+    OrthoViews V;
+    ortho_views(ds, resolution, V.vw, V.vh, V.ox, V.oy, &V.W, &H);
+    V.inv = 1.0 / (double)resolution;   // (a power of two: exact)
+    for (int a = 0; a < 3; a++) {
+        V.lb[a] = (double)ds.lo[a];
+        V.ub[a] = (double)ds.lo[a] + ds.size[a];
     }
-    const size_t n = where.size();
-    std::vector<uchar4> px(n);
+    V.first[0] = 0;
+    for (int v = 0; v < 5; v++) V.first[v + 1] = V.first[v] + (uint64_t)V.vw[v] * V.vh[v];
+    const uint64_t n = V.first[5];
+    if (info) std::memset(info, 0, sizeof *info);
+    aicb_ctx *root = r.ctx[0];
+    CU(cudaSetDevice(root->device));
+    const size_t off_traced = (out_len * 4 + 255) & ~(size_t)255;   // d_out: the image, then the traced pixels
+    TRY(root->d_out.ensure(off_traced + n * 4 + 16));
+    uchar4 *image = root->d_out.get<uchar4>(), *traced = (uchar4 *)(root->d_out.get<char>() + off_traced);
+    CU(cudaMemsetAsync(image, 0, out_len * 4, root->stream.get()));
+    std::vector<FramePart> parts;
     if (n) {
-        DeviceBuffer d_rays;
-        TRY(d_rays.upload(rays.data(), n * 48, 16));
-        TRY(ctx->d_out.ensure(n * 4 + 16));
+        const std::vector<WarpRange> ranges = warp_ranges(n, r.n);
+        for (size_t i = 0; i < ranges.size(); i++) {
+            if (ranges[i].count > 0xffffffffull) return fail(AICB_ERR_INVALID, "too many rays");
+            aicb_ctx *ctx = r.ctx[i];
+            const uint32_t count = (uint32_t)ranges[i].count;
+            CU(cudaSetDevice(ctx->device));
+            TRY(ctx->d_aux.ensure((size_t)count * 48 + 16));
+            ortho_rays_kernel<<<(count + 255) / 256, 256, 0, ctx->stream.get()>>>(V, ranges[i].begin, count,
+                                                                                  ctx->d_aux.get<double>());
+            CU(cudaGetLastError());
+            FramePart p{r.scene[i]};
+            p.out.target.out_srgb8 = traced + ranges[i].begin;
+            p.out.rays = ctx->d_aux.get<double>();
+            p.out.n_rays = count;
+            parts.push_back(p);
+        }
         aicb_options opt;   // GraphicsOptions::UNALTERED_COLORS (graphics_options.rs:168)
         std::memset(&opt, 0, sizeof opt);
         opt.fog = AICB_FOG_NONE;
@@ -2412,17 +2434,21 @@ aicb_status aicb_render_orthographic(aicb_scene *s, uint32_t resolution, uint8_t
         opt.maximum_intensity = INFINITY;
         opt.view_distance = 200.0;
         opt.include_sky = 1;
-        FramePart part{s};
-        part.out.target.out_srgb8 = ctx->d_out.get<uchar4>();
-        part.out.rays = d_rays.get<double>();
-        part.out.n_rays = n;
-        TRY(aicb_trace_pass(&part, 1, nullptr, &opt, info != nullptr));
-        if (info) *info = part.info;
-        CU(cudaMemcpy(px.data(), ctx->d_out.get(), n * 4, cudaMemcpyDeviceToHost));
+        TRY(aicb_trace_pass(parts.data(), parts.size(), nullptr, &opt, info != nullptr));
+        TRY(fan_in(r.ctx, parts.size()));
+        ortho_place_kernel<<<(unsigned)((n + 255) / 256), 256, 0, root->stream.get()>>>(V, traced, n, image);
+        CU(cudaGetLastError());
+        if (info)
+            for (const FramePart &p : parts) aicb_merge_info(info, &p.info, false);
     }
-    std::memset(out, 0, out_len * 4);   // Rgba::TRANSPARENT between the views
-    for (size_t i = 0; i < n; i++) std::memcpy(out[where[i]], &px[i], 4);
-    return AICB_OK;
+    return deliver(r.ctx, 1, {{out, image, out_len * 4}});   // (the other contexts are waited for above)
+}
+
+extern "C" {
+
+aicb_status aicb_render_orthographic(aicb_scene *s, uint32_t resolution, uint8_t (*out)[4], size_t out_len,
+                                     aicb_render_info *info) {
+    return on_scene(s, [&](Replicas r) { return ortho_srgb8(r, resolution, out, out_len, info); });
 }
 
 aicb_status aicb_render_finish(aicb_scene *s, aicb_render_info *info) {
@@ -2438,12 +2464,7 @@ aicb_status aicb_trace_rays(aicb_scene *s, const double (*origin_dir)[6], size_t
     if (!s || (n && !origin_dir)) return fail(AICB_ERR_INVALID, "NULL argument");
     aicb_status st = validate_options(opt);
     if (st != AICB_OK) return st;
-    aicb_ctx *ctx = s->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    DeviceBuffer d_rays;
-    TRY(d_rays.upload(origin_dir, n * 48, 16));
-    return render_aux(s, nullptr, opt, nullptr, d_rays.get<double>(), n, out_cb, depth, hit, steps, n, info);
+    return on_scene(s, [&](Replicas r) { return rays_colorbuf(r, origin_dir, n, opt, {out_cb, depth, hit, steps}, info); });
 }
 
 }

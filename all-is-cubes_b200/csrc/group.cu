@@ -75,11 +75,9 @@ static aicb_status layer_parts(const LayeredCall &c, aicb_ctx *const *ctx, const
         }
         return AICB_OK;
     }
-    const size_t warps = (n_pixels + 31) / 32;
-    const size_t used = std::min(c.n, warps);
-    size_t begin = 0;
-    for (size_t i = 0; i < used; i++) {
-        const size_t count = std::min(32 * (warps / used + (i < warps % used ? 1 : 0)), n_pixels - begin);
+    const std::vector<WarpRange> ranges = warp_ranges(n_pixels, c.n);
+    for (size_t i = 0; i < ranges.size(); i++) {
+        const size_t begin = ranges[i].begin, count = ranges[i].count;
         CU(cudaSetDevice(ctx[i]->device));
         TRY(ctx[i]->d_aux.ensure(count * 4 + 16));
         CU(cudaMemcpy(ctx[i]->d_aux.get(), pixels + begin, count * 4, cudaMemcpyHostToDevice));
@@ -89,20 +87,24 @@ static aicb_status layer_parts(const LayeredCall &c, aicb_ctx *const *ctx, const
         p.out.target.out_rgba16f = target.target.out_rgba16f + begin;
         p.out.target.out_tex_depth = target.target.out_tex_depth + begin;
         parts->push_back(p);
-        begin += count;
     }
     return AICB_OK;
 }
 
-// A copy of device 0's outputs to the caller.
-struct Delivery {
-    void *to;
-    const void *from;
-    size_t bytes;
-};
+std::vector<WarpRange> warp_ranges(size_t n_items, size_t n_ctx) {
+    const size_t warps = (n_items + 31) / 32;
+    const size_t used = std::max<size_t>(1, std::min(n_ctx, warps));
+    std::vector<WarpRange> ranges;
+    size_t begin = 0;
+    for (size_t i = 0; i < used; i++) {
+        const size_t count = std::min(32 * (warps / used + (i < warps % used ? 1 : 0)), n_items - begin);
+        ranges.push_back({begin, count});
+        begin += count;
+    }
+    return ranges;
+}
 
-// Device 0's stream waits for the streams of the contexts that drew a part, then copies the outputs to the caller.
-static aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, std::initializer_list<Delivery> copies) {
+aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies) {
     TRY(fan_in(ctx, n_parts));
     cudaStream_t stream = ctx[0]->stream.get();
     for (const Delivery &d : copies)
@@ -121,7 +123,7 @@ static std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *
 
 // The rest of a layered call once device 0's outputs are in `target`: the parts, the layers, the delivery.
 static aicb_status draw_layers(const LayeredCall &c, const std::vector<aicb_ctx *> &ctx, const Outputs &target,
-                               const uint32_t *pixels, size_t n_pixels, std::initializer_list<Delivery> copies,
+                               const uint32_t *pixels, size_t n_pixels, const std::vector<Delivery> &copies,
                                aicb_render_info *info) {
     std::vector<LayerPart> parts;
     TRY(layer_parts(c, ctx.data(), target, pixels, n_pixels, &parts));
@@ -183,6 +185,124 @@ aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, 
     target.target.out_tex_depth = (float *)(base + off_depth);
     return draw_layers(c, ctx, target, pixels, n_pixels,
                        {{out_rgba16f, base, n_pixels * 8}, {out_depth, base + off_depth, n_pixels * 4}}, info);
+}
+
+// ---- world-only frames and ray batches of one scene -------------------------------------------------------------------
+// The parts' info summed: counters add up, times are the slowest part's.
+static void sum_info(const std::vector<FramePart> &parts, aicb_render_info *info) {
+    if (!info) return;
+    std::memset(info, 0, sizeof *info);
+    for (const FramePart &p : parts) aicb_merge_info(info, &p.info, false);
+}
+
+// A frame of the replicas' scene with the caller's options as given: interleaved 16-row strips as
+// aicb_group_render_srgb8 cuts them, each part storing at framebuffer positions in device 0's outputs (`target`); with
+// `shard` (one context), that shard's rows, packed.  Then the delivery of device 0's outputs.
+static aicb_status draw_frame(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
+                              Outputs target, const std::vector<Delivery> &copies, aicb_render_info *info) {
+    std::vector<LayerPart> strips;   // (the parts' shards)
+    std::vector<FramePart> parts;
+    if (shard) {
+        parts.push_back({r.scene[0], shard, target});
+    } else {
+        target.full_frame = true;
+        const aicb_layer w0 = {r.scene[0], cam, opt};
+        const LayeredCall world = {&w0, nullptr, r.scene, nullptr, r.n, nullptr, nullptr};
+        TRY(layer_parts(world, r.ctx, target, nullptr, 0, &strips));
+        for (const LayerPart &p : strips) parts.push_back({p.world, &p.shard, p.out});
+    }
+    TRY(aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr));
+    TRY(deliver(r.ctx, parts.size(), copies));
+    sum_info(parts, info);
+    return AICB_OK;
+}
+
+// draw::<ColorBuf> and its companions' outputs for n pixels or rays in device 0's d_out: colorbuf, then the wanted
+// ones of depth, hit and steps; an output the caller does not want is neither allocated, stored nor copied.
+static aicb_status aux_target(aicb_ctx *root, size_t n, const AuxOutputs &want, Outputs *o) {
+    size_t bytes = n * 16;
+    auto take = [&](bool wanted, size_t size) -> size_t {
+        const size_t off = bytes;
+        if (wanted) bytes += n * size;
+        return off;
+    };
+    const size_t off_depth = take(want.depth, 8), off_hit = take(want.hit, sizeof(aicb_hit));
+    const size_t off_steps = take(want.steps, 4);
+    CU(cudaSetDevice(root->device));
+    TRY(root->d_out.ensure(bytes + 16));
+    char *base = root->d_out.get<char>();
+    o->aux = true;
+    o->target.out_colorbuf = (float4 *)base;
+    o->target.out_depth = want.depth ? (double *)(base + off_depth) : nullptr;
+    o->target.out_hit = want.hit ? (aicb_hit *)(base + off_hit) : nullptr;
+    o->target.out_steps = want.steps ? (uint32_t *)(base + off_steps) : nullptr;
+    return AICB_OK;
+}
+
+static std::vector<Delivery> aux_copies(const Outputs &o, const AuxOutputs &want, size_t n) {
+    const aicb::TargetParams &t = o.target;
+    return {{want.colorbuf, t.out_colorbuf, want.colorbuf ? n * 16 : 0},
+            {want.depth, t.out_depth, want.depth ? n * 8 : 0},
+            {want.hit, t.out_hit, want.hit ? n * sizeof(aicb_hit) : 0},
+            {want.steps, t.out_steps, want.steps ? n * 4 : 0}};
+}
+
+aicb_status frame_colorbuf(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
+                           AuxOutputs out, size_t out_len, aicb_render_info *info) {
+    Outputs target;
+    TRY(aux_target(r.ctx[0], out_len, out, &target));
+    return draw_frame(r, cam, opt, shard, target, aux_copies(target, out, out_len), info);
+}
+
+aicb_status frame_rgba16f(Replicas r, const aicb_camera *cam, const aicb_options *opt, uint16_t (*out)[4],
+                          size_t out_len, aicb_render_info *info) {
+    aicb_ctx *root = r.ctx[0];
+    CU(cudaSetDevice(root->device));
+    TRY(root->d_out.ensure(out_len * 8 + 16));
+    Outputs target;
+    target.target.out_rgba16f = root->d_out.get<uint2>();
+    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 8}}, info);
+}
+
+aicb_status frame_text(Replicas r, const aicb_camera *cam, const aicb_options *opt, int32_t *out, size_t out_len,
+                       aicb_render_info *info) {
+    aicb_ctx *root = r.ctx[0];
+    CU(cudaSetDevice(root->device));
+    TRY(root->d_out.ensure(out_len * 4 + 16));
+    Outputs target;
+    target.target.out_text = root->d_out.get<int32_t>();
+    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 4}}, info);
+}
+
+// Context i uploads its range of the batch to its own d_aux and stores at the range's offset in device 0's outputs.
+aicb_status rays_colorbuf(Replicas r, const double (*origin_dir)[6], size_t n, const aicb_options *opt, AuxOutputs out,
+                          aicb_render_info *info) {
+    if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "too many rays");
+    Outputs target;
+    TRY(aux_target(r.ctx[0], n, out, &target));
+    const std::vector<WarpRange> ranges = warp_ranges(n, r.n);
+    std::vector<FramePart> parts;
+    for (size_t i = 0; i < ranges.size(); i++) {
+        const size_t begin = ranges[i].begin, count = ranges[i].count;
+        aicb_ctx *ctx = r.ctx[i];
+        CU(cudaSetDevice(ctx->device));
+        TRY(ctx->d_aux.ensure(count * 48 + 16));
+        if (count) CU(cudaMemcpy(ctx->d_aux.get(), origin_dir + begin, count * 48, cudaMemcpyHostToDevice));
+        FramePart p{r.scene[i]};
+        p.out = target;
+        aicb::TargetParams &t = p.out.target;
+        t.out_colorbuf += begin;
+        if (t.out_depth) t.out_depth += begin;
+        if (t.out_hit) t.out_hit += begin;
+        if (t.out_steps) t.out_steps += begin;
+        p.out.rays = ctx->d_aux.get<double>();
+        p.out.n_rays = count;
+        parts.push_back(p);
+    }
+    TRY(aicb_trace_pass(parts.data(), parts.size(), nullptr, opt, info != nullptr));
+    TRY(deliver(r.ctx, parts.size(), aux_copies(target, out, n)));
+    sum_info(parts, info);
+    return AICB_OK;
 }
 
 // The layers of a group call as device 0 sees them (its replicas, the cameras and options), and every replica of each.
@@ -313,33 +433,70 @@ aicb_status aicb_group_scene_update_region(aicb_group_scene *gs, const aicb_aab 
 aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt,
                                     uint8_t (*out)[4], size_t out_len, aicb_render_info *info) {
     if (!gs || !cam || !opt) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
-    aicb_group *g = gs->group;
     const size_t pixels = (size_t)cam->fb_width * cam->fb_height;
     if (out_len != pixels) return aicb_fail(AICB_ERR_INVALID, "Viewport size does not match output buffer length");
     if (pixels && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
     aicb_status st = aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len);
     if (st != AICB_OK) return st;
-    ContextLocks lock(g->ctx);
-    aicb_ctx *root = g->ctx[0];
-    CU(cudaSetDevice(root->device));
-    TRY(root->d_out.ensure(pixels * 4 + 16));
-    Outputs target;
-    target.full_frame = true;
-    target.target.out_srgb8 = root->d_out.get<uchar4>();
-    // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
-    const aicb_layer w0 = {gs->scene[0], cam, opt};
-    const LayeredCall world = {&w0, nullptr, gs->scene.data(), nullptr, g->ctx.size(), nullptr, nullptr};
-    std::vector<LayerPart> strips;
-    TRY(layer_parts(world, g->ctx.data(), target, nullptr, 0, &strips));
-    std::vector<FramePart> parts;
-    for (const LayerPart &p : strips) parts.push_back({p.world, &p.shard, p.out});
-    TRY(aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr));
-    TRY(deliver(g->ctx.data(), parts.size(), {{out, root->d_out.get(), pixels * 4}}));
-    if (info) {
-        std::memset(info, 0, sizeof *info);
-        for (const FramePart &p : parts) aicb_merge_info(info, &p.info, false);
-    }
-    return AICB_OK;
+    return on_group(gs, false, [&](Replicas r) {
+        aicb_ctx *root = r.ctx[0];
+        CU(cudaSetDevice(root->device));
+        TRY(root->d_out.ensure(pixels * 4 + 16));
+        Outputs target;
+        target.target.out_srgb8 = root->d_out.get<uchar4>();
+        // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
+        return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), pixels * 4}}, info);
+    });
+}
+
+// The world-only outputs of one context on the group, with the single-context calls' validation against replica 0.
+aicb_status aicb_group_render_colorbuf(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt,
+                                       float (*out_colorbuf)[4], double *depth, aicb_hit *hit, uint32_t *steps,
+                                       size_t out_len, aicb_render_info *info) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len));
+    if (out_len && !out_colorbuf) return aicb_fail(AICB_ERR_INVALID, "out_colorbuf is NULL");
+    return on_group(gs, false, [&](Replicas r) {
+        return frame_colorbuf(r, cam, opt, nullptr, {out_colorbuf, depth, hit, steps}, out_len, info);
+    });
+}
+
+aicb_status aicb_group_render_rgba16f(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt,
+                                      uint16_t (*out)[4], size_t out_len, aicb_render_info *info) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len));
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    return on_group(gs, false, [&](Replicas r) { return frame_rgba16f(r, cam, opt, out, out_len, info); });
+}
+
+aicb_status aicb_group_trace_rays(aicb_group_scene *gs, const double (*origin_dir)[6], size_t n, const aicb_options *opt,
+                                  float (*out_colorbuf)[4], double *depth, aicb_hit *hit, uint32_t *steps,
+                                  aicb_render_info *info) {
+    if (!gs || (n && !origin_dir)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(validate_options(opt));
+    if (n && !out_colorbuf) return aicb_fail(AICB_ERR_INVALID, "out_colorbuf is NULL");
+    return on_group(gs, false, [&](Replicas r) {
+        return rays_colorbuf(r, origin_dir, n, opt, {out_colorbuf, depth, hit, steps}, info);
+    });
+}
+
+aicb_status aicb_group_render_text(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt, int32_t *out,
+                                   size_t out_len, aicb_render_info *info) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len));
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    return on_group(gs, false, [&](Replicas r) { return frame_text(r, cam, opt, out, out_len, info); });
+}
+
+aicb_status aicb_group_ortho_image_size(const aicb_group_scene *gs, uint32_t resolution, uint32_t *width,
+                                        uint32_t *height) {
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    return aicb_ortho_image_size(gs->scene[0], resolution, width, height);
+}
+
+aicb_status aicb_group_render_orthographic(aicb_group_scene *gs, uint32_t resolution, uint8_t (*out)[4], size_t out_len,
+                                           aicb_render_info *info) {
+    return on_group(gs, false, [&](Replicas r) { return ortho_srgb8(r, resolution, out, out_len, info); });
 }
 
 aicb_status aicb_group_scene_update_blocks(aicb_group_scene *gs, const uint16_t *indices, const aicb_block_desc *descs,

@@ -307,7 +307,7 @@ struct Outputs {
     aicb::TargetParams target{};
     int kind = aicb::TGT_FRAME;         // the compositing kernels' target: TGT_FRAME, TGT_TEX or TGT_TERM
     bool full_frame = false;            // outputs at framebuffer positions (TraceParams::out_full_frame)
-    bool aux = false;                   // the marching kernel that also counts steps and blocks (render_aux)
+    bool aux = false;                   // the marching kernel that also counts steps and blocks (AuxOutputs)
     const double *rays = nullptr;       // device: the tasks of a frame without a camera (origin, direction per ray)
     uint64_t n_rays = 0;
     int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
@@ -450,6 +450,45 @@ aicb_status layers_srgb8(const LayeredCall &c, uint8_t (*out)[4], size_t out_len
 aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info);
 aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
                            uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info);
+
+// group.cu: one scene's world-only outputs over its replicas (aicb_render_* on one context, aicb_group_render_* and
+// aicb_group_trace_rays on a group).  The caller has validated the arguments and holds every context's lock.  A frame
+// is cut into interleaved 16-row strips (with `shard`, one context only: that shard's rows, packed); a ray batch into
+// contiguous ranges of whole warps (warp_ranges).  Every part stores into device 0's buffers, and device 0 copies the
+// outputs the caller asked for (non-null pointers) to the caller.
+struct AuxOutputs {
+    float (*colorbuf)[4];
+    double *depth;
+    aicb_hit *hit;
+    uint32_t *steps;
+};
+aicb_status frame_colorbuf(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
+                           AuxOutputs out, size_t out_len, aicb_render_info *info);
+aicb_status frame_rgba16f(Replicas r, const aicb_camera *cam, const aicb_options *opt, uint16_t (*out)[4],
+                          size_t out_len, aicb_render_info *info);
+aicb_status frame_text(Replicas r, const aicb_camera *cam, const aicb_options *opt, int32_t *out, size_t out_len,
+                       aicb_render_info *info);
+aicb_status rays_colorbuf(Replicas r, const double (*origin_dir)[6], size_t n, const aicb_options *opt, AuxOutputs out,
+                          aicb_render_info *info);
+// aicb200.cu: render_orthographic over the replicas, validated against replica 0 (the caller holds the locks).
+aicb_status ortho_srgb8(Replicas r, uint32_t resolution, uint8_t (*out)[4], size_t out_len, aicb_render_info *info);
+
+// group.cu: n items cut into contiguous ranges of whole 32-item warps, one per context, as even as whole warps allow:
+// min(n_ctx, warps) ranges, device 0's first (one empty range for n_items == 0).
+struct WarpRange {
+    size_t begin, count;
+};
+std::vector<WarpRange> warp_ranges(size_t n_items, size_t n_ctx);
+// A copy of device 0's outputs to the caller (none if bytes == 0).
+struct Delivery {
+    void *to;
+    const void *from;
+    size_t bytes;
+};
+// Device 0's stream waits for the streams of the first n_parts contexts, then copies the outputs to the caller.
+aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies);
+// aicb200.cu: GraphicsOptions as every frame call accepts them (AICB_ERR_INVALID otherwise).
+aicb_status validate_options(const aicb_options *o);
 
 // light.cu: the light calls over a scene's replicas.  On a group, device 0 has peer access to every other device and
 // they to device 0, with native atomics.  After every call the replicas' light volumes are identical.

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 16 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 17 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -304,6 +304,21 @@ unsafe extern "C" {
                                              backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],
                                              out: *mut aicb_terminal_pixel, out_len: usize,
                                              info: *mut aicb_render_info) -> aicb_status;
+    // the world-only single-context outputs on a group: whole frames, ray batches cut into warp ranges
+    pub fn aicb_group_render_colorbuf(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
+                                      out_colorbuf: *mut [f32; 4], depth: *mut f64, hit: *mut aicb_hit, steps: *mut u32,
+                                      out_len: usize, info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_rgba16f(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
+                                     out: *mut [u16; 4], out_len: usize, info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_trace_rays(gs: *mut aicb_group_scene, origin_dir: *const [f64; 6], n: usize,
+                                 opt: *const aicb_options, out_colorbuf: *mut [f32; 4], depth: *mut f64,
+                                 hit: *mut aicb_hit, steps: *mut u32, info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_text(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
+                                  out: *mut i32, out_len: usize, info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_ortho_image_size(gs: *const aicb_group_scene, resolution: u32, width: *mut u32, height: *mut u32)
+                                       -> aicb_status;
+    pub fn aicb_group_render_orthographic(gs: *mut aicb_group_scene, resolution: u32, out: *mut [u8; 4], out_len: usize,
+                                          info: *mut aicb_render_info) -> aicb_status;
 
     pub fn aicb_trace_rays(s: *mut aicb_scene, origin_dir: *const [f64; 6], n: usize, opt: *const aicb_options,
                            out_colorbuf: *mut [f32; 4], depth: *mut f64, hit: *mut aicb_hit, steps: *mut u32,

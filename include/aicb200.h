@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 16
+#define AICB_ABI_VERSION 17
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -493,6 +493,31 @@ aicb_status aicb_group_render_layers_texture(const aicb_group_layer *world_or_nu
 aicb_status aicb_group_render_layers_terminal(const aicb_group_layer *world_or_null, const aicb_group_layer *ui_or_null,
                                               const float backdrop_rgba[4], const float no_world_rgba[4],
                                               aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info_or_null);
+
+/* The world-only outputs of one context on the whole group: the arguments, the validation (against replica 0, before
+ * any device is touched) and the outputs of aicb_render_colorbuf / _rgba16f / _text / _orthographic /
+ * aicb_ortho_image_size and aicb_trace_rays, bit for bit, with a group scene in place of a scene.  Frames are whole
+ * frames (out_len = fb_width * fb_height, no shard): each is cut into interleaved 16-row strips as
+ * aicb_group_render_srgb8 cuts it.  A ray batch is cut into contiguous ranges of whole 32-ray warps, one per device, as
+ * even as whole warps allow (a batch of fewer than 32 x devices rays uses fewer devices); each device uploads only its
+ * own range.  The orthographic image's five views are built on the devices and their pixels cut the same way.  Every
+ * device stores its outputs straight into device 0's buffers, in framebuffer or batch order, and device 0 copies the
+ * outputs the caller asked for (the non-NULL ones) to the caller.  Unlike the single-context calls, out_colorbuf may
+ * not be NULL when there are pixels or rays (AICB_ERR_INVALID).  A device whose hit stream overflowed is re-issued
+ * alone.  aicb_render_info: counters summed over the devices, times = the slowest device's. */
+aicb_status aicb_group_render_colorbuf(aicb_group_scene *, const aicb_camera *, const aicb_options *,
+                                       float (*out_colorbuf)[4], double *depth_or_null, aicb_hit *hit_or_null,
+                                       uint32_t *steps_or_null, size_t out_len, aicb_render_info *info_or_null);
+aicb_status aicb_group_render_rgba16f(aicb_group_scene *, const aicb_camera *, const aicb_options *,
+                                      uint16_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
+aicb_status aicb_group_trace_rays(aicb_group_scene *, const double (*origin_dir)[6], size_t n, const aicb_options *,
+                                  float (*out_colorbuf)[4], double *depth_or_null, aicb_hit *hit_or_null,
+                                  uint32_t *steps_or_null, aicb_render_info *info_or_null);
+aicb_status aicb_group_render_text(aicb_group_scene *, const aicb_camera *, const aicb_options *,
+                                   int32_t *out, size_t out_len, aicb_render_info *info_or_null);
+aicb_status aicb_group_ortho_image_size(const aicb_group_scene *, uint32_t resolution, uint32_t *width, uint32_t *height);
+aicb_status aicb_group_render_orthographic(aicb_group_scene *, uint32_t resolution, uint8_t (*out)[4],
+                                           size_t out_len, aicb_render_info *info_or_null);
 
 /* == SpaceRaytracer::trace_ray (sr.rs:113-120) for a batch of explicit rays:
  * origin_dir[i] = {ox,oy,oz,dx,dy,dz}. Output as aicb_render_colorbuf. */
