@@ -54,6 +54,7 @@ def load_library() -> C.CDLL:
     lib.aicb_ctx_create.argtypes = [C.c_int, C.POINTER(C.c_void_p)]
     lib.aicb_ctx_destroy.argtypes = [C.c_void_p]
     lib.aicb_ctx_stage_timing.argtypes = [C.c_void_p, C.c_int]
+    lib.aicb_ctx_device.argtypes = [C.c_void_p]
     lib.aicb_scene_create.argtypes = [C.c_void_p, C.POINTER(abi.SceneDesc), C.POINTER(C.c_void_p)]
     lib.aicb_scene_destroy.argtypes = [C.c_void_p]
     lib.aicb_scene_device_bytes.argtypes = [C.c_void_p]
@@ -123,6 +124,20 @@ def load_library() -> C.CDLL:
                                               C.c_size_t, C.POINTER(abi.RenderInfo)]
     lib.aicb_light_chart.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_light_chart.restype = C.c_uint32
+    outs = C.POINTER(abi.DeviceOutputs)
+    lib.aicb_render_device.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options),
+                                       C.POINTER(abi.Shard), outs, C.c_void_p]
+    lib.aicb_trace_rays_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.Options), outs,
+                                           C.c_void_p]
+    lib.aicb_render_layers_device.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_size_t, outs, C.c_void_p]
+    lib.aicb_group_render_device.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), outs,
+                                             C.c_void_p, C.POINTER(abi.RenderInfo)]
+    lib.aicb_group_trace_rays_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.Options), outs,
+                                                 C.c_void_p, C.POINTER(abi.RenderInfo)]
+    lib.aicb_group_render_layers_device.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, outs, C.c_void_p,
+                                                    C.POINTER(abi.RenderInfo)]
     lib.aicb_group_light_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
     # the calls of _Scene: a group scene's form of aicb_<name> is aicb_group_<name>, with the same arguments
     u64, u8, size = C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_size_t)
@@ -623,6 +638,14 @@ class Context:
         lib = load_library()
         self.handle = C.c_void_p()
         _check(lib.aicb_ctx_create(device_id, C.byref(self.handle)))
+        self.device_id = lib.aicb_ctx_device(self.handle)   # -1 resolved to the device current at creation
+        self._pending = None   # the DeviceRendering issued last and not finished yet
+
+    def settle(self):
+        """Finish the asynchronous call issued last on this context, if it is not finished yet: the context tracks one
+        frame, so its next render call, or a change of one of its scenes, must come after that call's finish."""
+        if self._pending is not None:
+            self._pending.result()
 
     @classmethod
     def default(cls) -> "Context":
@@ -663,6 +686,111 @@ class Rendering:
     info: RenderInfo
 
 
+# ------------------------------------------------------------------------------------------------
+# outputs in device memory (aicb_device_outputs): torch tensors, issued on torch.cuda.current_stream()
+# ------------------------------------------------------------------------------------------------
+def _torch():
+    import torch
+    return torch
+
+
+def _ctx_device(ctx: "Context"):
+    return _torch().device("cuda", ctx.device_id)
+
+
+def _device_outputs(out, device, spec) -> dict:
+    """The output tensors of a device call: spec maps a name to (shape, dtype); `out` (a tensor for a call of one output,
+    or a dict of them) supplies the caller's own tensors, checked for shape, dtype, device and contiguity; the others
+    are allocated with torch's caching allocator."""
+    torch = _torch()
+    given = out if isinstance(out, dict) else ({next(iter(spec)): out} if out is not None else {})
+    unknown = set(given) - set(spec)
+    if unknown:
+        raise ValueError(f"out= names outputs this call does not make: {sorted(unknown)}")
+    tensors = {}
+    for name, (shape, dtype) in spec.items():
+        t = given.get(name)
+        if t is None:
+            t = torch.empty(shape, dtype=dtype, device=device)
+        elif tuple(t.shape) != tuple(shape) or t.dtype != dtype or t.device != device or not t.is_contiguous():
+            raise ValueError(f"out[{name!r}] must be a contiguous {dtype} tensor of shape {tuple(shape)} on {device}, "
+                             f"not {t.dtype} {tuple(t.shape)} on {t.device}")
+        tensors[name] = t
+    return tensors
+
+
+def _outs_abi(n: int, tensors: dict) -> abi.DeviceOutputs:
+    o = abi.DeviceOutputs()
+    for name, t in tensors.items():
+        setattr(o, name, t.data_ptr())
+    o.len = n
+    return o
+
+
+def _stream(device) -> int:
+    """The current torch stream of `device` as a cudaStream_t.  torch's default stream is the legacy default stream:
+    it goes as cudaStreamLegacy (1), since NULL names the context's own stream."""
+    return _torch().cuda.current_stream(device).cuda_stream or 1
+
+
+class DeviceRendering:
+    """A device-output call issued on one context (device=True): its outputs are torch tensors on the scene's device,
+    written in the order of the stream that was current when it was issued; nothing has synchronised.  result()
+    finishes the call (aicb_render_finish: the host waits for the frame), re-issues it into the same tensors on the same
+    stream when its hit stream overflowed, and returns what the host call returns, with tensors in place of arrays;
+    `info` is then the call's RenderInfo.  The context tracks one frame: the next call on the context (a render, an
+    update of one of its scenes, a light call) finishes this one first (Context.settle)."""
+
+    def __init__(self, scene, issue, build):
+        self._scene = scene      # the scene that aicb_render_finish finishes (kept alive until then)
+        self._issue = issue
+        self._build = build
+        self._result = None
+        self.info = None
+        scene.ctx.settle()
+        _check(issue())
+        scene.ctx._pending = self
+
+    def result(self):
+        if self.info is None:
+            ctx = self._scene.ctx
+            if ctx._pending is self:
+                ctx._pending = None
+            lib = load_library()
+            info = abi.RenderInfo()
+            status = lib.aicb_render_finish(self._scene.handle, C.byref(info))
+            while status == abi.ERR_RETRY:   # the capacity has been raised: the same call again
+                _check(self._issue())
+                status = lib.aicb_render_finish(self._scene.handle, C.byref(info))
+            _check(status)
+            self.info = RenderInfo.from_abi(info)
+            self._result = self._build(self.info)
+        return self._result
+
+
+def _colorbuf_spec(n, want_depth, want_hit, want_steps) -> dict:
+    torch = _torch()
+    spec = {"colorbuf": ((n, 4), torch.float32)}
+    if want_depth:
+        spec["depth"] = ((n,), torch.float64)
+    if want_hit:
+        spec["hit"] = ((n, 8), torch.int32)
+    if want_steps:
+        spec["steps"] = ((n,), torch.uint32)
+    return spec
+
+
+def _colorbuf_result(t: dict, info) -> dict:
+    return {"colorbuf": t["colorbuf"], "depth": t.get("depth"), "hit": t.get("hit"), "steps": t.get("steps"),
+            "info": info}
+
+
+def _terminal_result(t: dict, info) -> dict:
+    """aicb_terminal_pixel as int32 [H, W, 6]: rgba (f32 bits), text, layer."""
+    px = t["terminal"]
+    return {"text": px[..., 4], "layer": px[..., 5], "rgba": px[..., :4].view(_torch().float32), "info": info}
+
+
 class _Scene:
     """The calls SpaceRaytracer and GroupScene share: updates of the scene and light propagation.  Each calls the C
     function aicb_<name> through `_prefix` ("aicb_" on one context, "aicb_group_" on a group)."""
@@ -670,7 +798,10 @@ class _Scene:
     _prefix = "aicb_"
 
     def _fn(self, name: str):
-        """This kind of scene's form of the C function aicb_<name> (on a group, aicb_group_<name>)."""
+        """This kind of scene's form of the C function aicb_<name> (on a group, aicb_group_<name>), once the context's
+        asynchronous call issued last is finished."""
+        if hasattr(self, "ctx"):
+            self.ctx.settle()
         return getattr(load_library(), self._prefix + name)
 
     def close(self):
@@ -903,9 +1034,14 @@ class SpaceRaytracer(_Scene):
     def device_bytes(self) -> int:
         return int(load_library().aicb_scene_device_bytes(self.handle))
 
-    def trace_rays(self, origin_dir: np.ndarray, include_sky: bool = True, want_depth=False, want_hit=False,
-                   want_steps=False):
-        """SpaceRaytracer::trace_ray (sr.rs:113-120) over a batch: returns dict of arrays."""
+    def trace_rays(self, origin_dir, include_sky: bool = True, want_depth=False, want_hit=False, want_steps=False,
+                   out=None):
+        """SpaceRaytracer::trace_ray (sr.rs:113-120) over a batch: returns dict of arrays.  With origin_dir a CUDA tensor
+        [n, 6] of float64 on the scene's device, the batch is read where it is and the call returns a DeviceRendering
+        whose result() is the same dict of tensors (out=: a dict of the caller's own)."""
+        if _is_cuda_tensor(origin_dir):
+            return _trace_rays_device(self, origin_dir, self.graphics_options.to_abi(include_sky), want_depth, want_hit,
+                                      want_steps, out, _ctx_device(self.ctx), None)
         return _trace_rays(self, origin_dir, self.graphics_options.to_abi(include_sky), want_depth, want_hit, want_steps)
 
     def light_download(self) -> np.ndarray:
@@ -929,6 +1065,71 @@ def _trace_rays(scene, origin_dir, opt, want_depth, want_hit, want_steps) -> dic
     return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
 
 
+def _is_cuda_tensor(x) -> bool:
+    return type(x).__module__.startswith("torch") and getattr(x, "is_cuda", False)
+
+
+def _trace_rays_device(scene, origin_dir, opt, want_depth, want_hit, want_steps, out, device, group):
+    """aicb_trace_rays_device on a SpaceRaytracer (a DeviceRendering), aicb_group_trace_rays_device on a group's scene
+    (`group`: the dict of tensors)."""
+    torch = _torch()
+    od = origin_dir.reshape(-1, 6)
+    if od.dtype != torch.float64 or od.device != device or not od.is_contiguous():
+        raise ValueError(f"origin_dir must be a contiguous float64 tensor [n, 6] on {device}")
+    n = od.shape[0]
+    t = _device_outputs(out, device, _colorbuf_spec(n, want_depth, want_hit, want_steps))
+    o = _outs_abi(n, t)
+    lib = load_library()
+    stream = _stream(device)
+    if group is None:
+        return DeviceRendering(scene, lambda: lib.aicb_trace_rays_device(scene.handle, od.data_ptr(), n, C.byref(opt),
+                                                                         C.byref(o), stream),
+                               lambda info: _colorbuf_result(t, info))
+    info = abi.RenderInfo()
+    _check(lib.aicb_group_trace_rays_device(scene.handle, od.data_ptr(), n, C.byref(opt), C.byref(o), stream,
+                                            C.byref(info)))
+    return _colorbuf_result(t, RenderInfo.from_abi(info))
+
+
+def _layers_device(group, world, ui, backdrop, no_world, spec, out, n, build, depth_transform=None, pixels=None):
+    """aicb_render_layers_device (a DeviceRendering) or, with `group` (a DeviceGroup), aicb_group_render_layers_device
+    (the result): the outputs of `spec`, n pixels or listed pixels."""
+    torch = _torch()
+    lead = world if world else ui
+    device = torch.device("cuda", group.device_ids[0]) if group is not None else _ctx_device(lead[0].ctx)
+    t = _device_outputs(out, device, spec)
+    o = _outs_abi(n, t)
+    keep = []
+    cls = abi.GroupLayer if group is not None else abi.Layer
+    w_arg, u_arg = _layer_arg(world, keep, cls), _layer_arg(ui, keep, cls)
+    b = np.array(backdrop, dtype=np.float32) if backdrop is not None else None
+    nw = np.array(no_world, dtype=np.float32) if no_world is not None else None
+    m = np.ascontiguousarray(depth_transform, dtype=np.float64).reshape(16) if depth_transform is not None else None
+    plist = None
+    if pixels is not None:   # u32 indices: an int32 or uint32 tensor as it is, anything else converted
+        if not _is_cuda_tensor(pixels):   # a list on the host is checked as the host call checks it
+            host_px = np.asarray(pixels, dtype=np.int64)
+            cam = lead[1].data
+            if host_px.size and (host_px.min() < 0 or host_px.max() >= cam.fb_width * cam.fb_height):
+                raise AicbError(abi.ERR_INVALID, "pixel index >= fb_width * fb_height")
+        plist = pixels if _is_cuda_tensor(pixels) else torch.as_tensor(host_px)
+        if plist.dtype not in (torch.int32, torch.uint32):
+            plist = plist.to(dtype=torch.int32)
+        plist = plist.reshape(-1).to(device=device).contiguous()
+    args = (w_arg, u_arg, b.ctypes.data if b is not None else None, nw.ctypes.data if nw is not None else None,
+            m.ctypes.data if m is not None else None, plist.data_ptr() if plist is not None else None,
+            n if m is not None else 0, C.byref(o))   # the texture's pixels (listed or every one); 0 for frames
+    lib = load_library()
+    stream = _stream(device)
+    if group is None:
+        def issue(held=(keep, plist, b, nw, m)):   # what `args` points to stays alive for a re-issue
+            return lib.aicb_render_layers_device(*args, stream)
+        return DeviceRendering(lead[0], issue, lambda info: build(t, info))
+    info = abi.RenderInfo()
+    _check(lib.aicb_group_render_layers_device(*args, stream, C.byref(info)))
+    return build(t, RenderInfo.from_abi(info))
+
+
 NO_WORLD_TO_SHOW_SRGB8 = (0xBC, 0xBC, 0xBC, 0xFF)   # content/palette.rs:76
 
 
@@ -937,6 +1138,8 @@ def _layer_arg(l, keep, cls):
     `keep`."""
     if not l:
         return None
+    if hasattr(l[0], "ctx"):
+        l[0].ctx.settle()
     o = l[2].to_abi(True)
     s = cls(l[0].handle, C.pointer(l[1].data), C.pointer(o))
     keep += [o, s]
@@ -957,19 +1160,53 @@ def _layers_srgb8(fn, cls, world, ui, backdrop, no_world) -> "Rendering":
     return Rendering((w, h), out, int(info.flaws), RenderInfo.from_abi(info))
 
 
-def render_layers(world=None, ui=None, backdrop=None, no_world=None) -> "Rendering":
+def render_layers(world=None, ui=None, backdrop=None, no_world=None, device=False, out=None):
     """RtRenderer::draw_rgba through every layer (renderer.rs:282-308, 454-478).
-    world / ui = (SpaceRaytracer, Camera, GraphicsOptions) or None; backdrop / no_world = linear RGBA or None."""
+    world / ui = (SpaceRaytracer, Camera, GraphicsOptions) or None; backdrop / no_world = linear RGBA or None.
+    device=True: a DeviceRendering whose result() is the Rendering with a uint8 CUDA tensor [H, W, 4] (out=: the
+    caller's own)."""
+    if device:
+        return _layers_srgb8_device(None, world, ui, backdrop, no_world, out)
     return _layers_srgb8(load_library().aicb_render_layers_srgb8, abi.Layer, world, ui, backdrop, no_world)
 
 
-def render_layers_texture(world=None, ui=None, backdrop=None, no_world=None, depth_transform=None, pixels=None):
+def _layers_srgb8_device(group, world, ui, backdrop, no_world, out):
+    cam = (world if world else ui)[1]
+    w, h = cam.data.fb_width, cam.data.fb_height
+    return _layers_device(group, world, ui, backdrop, no_world, {"srgb8": ((h, w, 4), _torch().uint8)}, out, w * h,
+                          lambda t, info: Rendering((w, h), t["srgb8"], int(info.flaws), info))
+
+
+def _layers_texture_device(group, world, ui, backdrop, no_world, depth_transform, pixels, out):
+    torch = _torch()
+    cam = (world if world else ui)[1]
+    if pixels is None:
+        n = cam.data.fb_width * cam.data.fb_height
+    else:
+        n = pixels.numel() if _is_cuda_tensor(pixels) else np.asarray(pixels).size
+    spec = {"texel_rgba16f": ((n, 4), torch.uint16), "texel_depth": ((n,), torch.float32)}
+    return _layers_device(group, world, ui, backdrop, no_world, spec, out, n,
+                          lambda t, info: (t["texel_rgba16f"], t["texel_depth"], info), depth_transform, pixels)
+
+
+def _layers_terminal_device(group, world, ui, backdrop, no_world, out):
+    cam = (world if world else ui)[1]
+    w, h = cam.data.fb_width, cam.data.fb_height
+    return _layers_device(group, world, ui, backdrop, no_world, {"terminal": ((h, w, 6), _torch().int32)}, out, w * h,
+                          _terminal_result)
+
+
+def render_layers_texture(world=None, ui=None, backdrop=None, no_world=None, depth_transform=None, pixels=None,
+                          device=False, out=None):
     """RaytraceToTexture::do_some_tracing's trace_one (raytrace_to_texture.rs:591-683) for a batch of pixels, through
     every layer as render_layers traces them.  world / ui = (SpaceRaytracer, Camera, GraphicsOptions) or None;
     depth_transform: [4, 4] (Camera.depth_transform() of the world camera); pixels: linear framebuffer indices
     y * width + x (any order, repeats allowed) or None for the whole texture in row-major order.
     Returns (rgba16f bits uint16 [n, 4], depth float32 [n], RenderInfo); the depth's sign is the pixel's layer (+ world,
-    - UI or neither)."""
+    - UI or neither).  device=True: a DeviceRendering whose result() is that triple with CUDA tensors (out=: a dict
+    with texel_rgba16f / texel_depth); pixels may then be a CUDA tensor, which is read where it is, unchecked."""
+    if device:
+        return _layers_texture_device(None, world, ui, backdrop, no_world, depth_transform, pixels, out)
     return _layers_texture(load_library().aicb_render_layers_texture, abi.Layer, world, ui, backdrop, no_world,
                            depth_transform, pixels)
 
@@ -996,12 +1233,15 @@ def _layers_texture(fn, cls, world, ui, backdrop, no_world, depth_transform, pix
     return rgba, depth, RenderInfo.from_abi(info)
 
 
-def render_layers_terminal(world=None, ui=None, backdrop=None, no_world=None) -> dict:
+def render_layers_terminal(world=None, ui=None, backdrop=None, no_world=None, device=False, out=None):
     """The desktop app's terminal frame (all-is-cubes-desktop/src/terminal.rs:114-142): draw::<ColorCharacterBuf>
     through every layer as render_layers traces them, and ColorCharacterBuf::output per pixel.  Same arguments as
     render_layers.  Returns a dict: text (int32 [H, W]: block index, or abi.TEXT_*), layer (int32 [H, W]: the layer
     whose Space a block index belongs to, abi.LAYER_*), rgba (float32 [H, W, 4]: post_process_color(Rgba::from(ColorBuf)),
-    linear) and info (RenderInfo)."""
+    linear) and info (RenderInfo).  device=True: a DeviceRendering whose result() is that dict of views of one int32
+    CUDA tensor [H, W, 6] (aicb_terminal_pixel; out=: the caller's own)."""
+    if device:
+        return _layers_terminal_device(None, world, ui, backdrop, no_world, out)
     return _layers_terminal(load_library().aicb_render_layers_terminal, abi.Layer, world, ui, backdrop, no_world)
 
 
@@ -1123,6 +1363,7 @@ class DeviceGroup:
         h = C.c_void_p()
         _check(load_library().aicb_group_create(ids, len(device_ids), C.byref(h)))
         self.handle = h
+        self.device_ids = [int(d) for d in device_ids]
         self.scene = None
         self.scenes = []
 
@@ -1131,19 +1372,31 @@ class DeviceGroup:
         self.scenes.append(s)
         return s
 
-    def render_layers(self, world=None, ui=None, backdrop=None, no_world=None) -> "Rendering":
-        """render_layers with GroupScenes of this group: world / ui = (GroupScene, Camera, GraphicsOptions) or None."""
+    def _device(self):
+        return _torch().device("cuda", self.device_ids[0])
+
+    def render_layers(self, world=None, ui=None, backdrop=None, no_world=None, device=False, out=None) -> "Rendering":
+        """render_layers with GroupScenes of this group: world / ui = (GroupScene, Camera, GraphicsOptions) or None.
+        device=True (here and in the other calls): the outputs are CUDA tensors on device 0 (out=: the caller's own),
+        ordered before the work queued afterwards on device 0's current torch stream; the call returns once they are
+        final."""
+        if device:
+            return _layers_srgb8_device(self, world, ui, backdrop, no_world, out)
         return _layers_srgb8(load_library().aicb_group_render_layers_srgb8, abi.GroupLayer, world, ui, backdrop,
                              no_world)
 
     def render_layers_texture(self, world=None, ui=None, backdrop=None, no_world=None, depth_transform=None,
-                              pixels=None):
+                              pixels=None, device=False, out=None):
         """render_layers_texture with GroupScenes of this group (same arguments and results)."""
+        if device:
+            return _layers_texture_device(self, world, ui, backdrop, no_world, depth_transform, pixels, out)
         return _layers_texture(load_library().aicb_group_render_layers_texture, abi.GroupLayer, world, ui, backdrop,
                                no_world, depth_transform, pixels)
 
-    def render_layers_terminal(self, world=None, ui=None, backdrop=None, no_world=None) -> dict:
+    def render_layers_terminal(self, world=None, ui=None, backdrop=None, no_world=None, device=False, out=None) -> dict:
         """render_layers_terminal with GroupScenes of this group (same arguments and results)."""
+        if device:
+            return _layers_terminal_device(self, world, ui, backdrop, no_world, out)
         return _layers_terminal(load_library().aicb_group_render_layers_terminal, abi.GroupLayer, world, ui, backdrop,
                                 no_world)
 
@@ -1153,8 +1406,22 @@ class DeviceGroup:
             self.scenes.remove(self.scene)
         self.scene = self.add_scene(space)
 
-    def draw(self, camera: "Camera", options: "GraphicsOptions") -> "Rendering":
+    def _render_device(self, camera, options, spec, out, build):
+        """aicb_group_render_device: the outputs of `spec` for the whole frame, on device 0."""
+        device = self._device()
+        t = _device_outputs(out, device, spec)
+        o = _outs_abi(camera.data.fb_width * camera.data.fb_height, t)
+        info = abi.RenderInfo()
+        opt = options.to_abi(True)
+        _check(load_library().aicb_group_render_device(self._handle(), C.byref(camera.data), C.byref(opt), C.byref(o),
+                                                      _stream(device), C.byref(info)))
+        return build(t, RenderInfo.from_abi(info))
+
+    def draw(self, camera: "Camera", options: "GraphicsOptions", device=False, out=None) -> "Rendering":
         w, h = camera.data.fb_width, camera.data.fb_height
+        if device:
+            return self._render_device(camera, options, {"srgb8": ((h, w, 4), _torch().uint8)}, out,
+                                       lambda t, info: Rendering((w, h), t["srgb8"], int(info.flaws), info))
         out = np.zeros((h, w, 4), dtype=np.uint8)
         info = abi.RenderInfo()
         o = options.to_abi(True)
@@ -1166,9 +1433,12 @@ class DeviceGroup:
         return self.scene.handle if self.scene else None
 
     def draw_colorbuf(self, camera: "Camera", options: "GraphicsOptions", want_depth=True, want_hit=True,
-                      want_steps=True) -> dict:
+                      want_steps=True, device=False, out=None) -> dict:
         """RtRenderer.draw_colorbuf of the whole frame on the group (same dict)."""
         n = camera.data.fb_width * camera.data.fb_height
+        if device:
+            return self._render_device(camera, options, _colorbuf_spec(n, want_depth, want_hit, want_steps), out,
+                                       _colorbuf_result)
         cb = np.empty((n, 4), dtype=np.float32)
         depth = np.empty(n, dtype=np.float64) if want_depth else None
         hit = np.empty((n, 8), dtype=np.int32) if want_hit else None
@@ -1181,26 +1451,36 @@ class DeviceGroup:
                                                          steps.ctypes.data if want_steps else None, n, C.byref(info)))
         return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
 
-    def draw_rgba16f(self, camera: "Camera", options: "GraphicsOptions") -> np.ndarray:
+    def draw_rgba16f(self, camera: "Camera", options: "GraphicsOptions", device=False, out=None) -> np.ndarray:
         """RtRenderer.draw_rgba16f of the whole frame on the group: float16 [h, w, 4]."""
         w, h = camera.data.fb_width, camera.data.fb_height
+        if device:
+            return self._render_device(camera, options, {"rgba16f": ((h, w, 4), _torch().float16)}, out,
+                                       lambda t, info: t["rgba16f"])
         out = np.empty((h, w, 4), dtype=np.float16)
         o = options.to_abi(True)
         _check(load_library().aicb_group_render_rgba16f(self._handle(), C.byref(camera.data), C.byref(o),
                                                         out.ctypes.data, w * h, None))
         return out
 
-    def trace_rays(self, origin_dir: np.ndarray, options: "GraphicsOptions", include_sky: bool = True, want_depth=False,
-                   want_hit=False, want_steps=False) -> dict:
-        """SpaceRaytracer.trace_rays on the group: the batch is cut into ranges of whole warps, one per device."""
+    def trace_rays(self, origin_dir, options: "GraphicsOptions", include_sky: bool = True, want_depth=False,
+                   want_hit=False, want_steps=False, out=None) -> dict:
+        """SpaceRaytracer.trace_rays on the group: the batch is cut into ranges of whole warps, one per device.  A CUDA
+        tensor batch on device 0 is read where it is, by every device, and the outputs are tensors on device 0."""
         if not self.scene:
             raise AicbError(abi.ERR_INVALID, "trace_rays() before update()")
+        if _is_cuda_tensor(origin_dir):
+            return _trace_rays_device(self.scene, origin_dir, options.to_abi(include_sky), want_depth, want_hit,
+                                      want_steps, out, self._device(), self)
         return _trace_rays(self.scene, origin_dir, options.to_abi(include_sky), want_depth, want_hit,
                            want_steps)
 
-    def render_text(self, camera: "Camera", options: "GraphicsOptions") -> np.ndarray:
+    def render_text(self, camera: "Camera", options: "GraphicsOptions", device=False, out=None) -> np.ndarray:
         """aicb_group_render_text: per pixel the CharacterBuf state (block index or abi.TEXT_*), int32 [h, w]."""
         w, h = camera.data.fb_width, camera.data.fb_height
+        if device:
+            return self._render_device(camera, options, {"text": ((h, w), _torch().int32)}, out,
+                                       lambda t, info: t["text"])
         out = np.zeros((h, w), dtype=np.int32)
         o = options.to_abi(True)
         _check(load_library().aicb_group_render_text(self._handle(), C.byref(camera.data), C.byref(o), out.ctypes.data,
@@ -1256,13 +1536,39 @@ class RtRenderer:
     def _require(self) -> SpaceRaytracer:
         if self.rt is None:
             raise AicbError(abi.ERR_INVALID, "draw() before update()")
+        self.rt.ctx.settle()
         return self.rt
 
     def pixel_count(self, shard=None) -> int:
         s = _shard_abi(shard)
         return int(load_library().aicb_shard_pixel_count(C.byref(self.camera.data), C.byref(s) if s else None))
 
-    def draw(self, info_text: str = "", shard=None) -> Rendering:
+    def _render_device(self, shard, spec, out, build) -> DeviceRendering:
+        """aicb_render_device on the current torch stream: the outputs of `spec` for the shard's pixels."""
+        rt = self._require()
+        device = _ctx_device(rt.ctx)
+        t = _device_outputs(out, device, spec)
+        o = _outs_abi(self.pixel_count(shard), t)
+        opt = rt.graphics_options.to_abi(True)
+        s = _shard_abi(shard)
+        stream = _stream(device)
+        lib = load_library()
+        return DeviceRendering(rt, lambda: lib.aicb_render_device(rt.handle, C.byref(self.camera.data), C.byref(opt),
+                                                                  C.byref(s) if s else None, C.byref(o), stream),
+                               lambda info: build(t, info))
+
+    def _rows(self, shard):
+        n, w = self.pixel_count(shard), self.camera.data.fb_width
+        return (n // w if w else 0), w
+
+    def draw(self, info_text: str = "", shard=None, device=False, out=None):
+        """draw_rgba.  device=True: a DeviceRendering whose result() is the Rendering with a uint8 CUDA tensor
+        [h, w, 4] on the scene's device (out=: the caller's own), issued on the current torch stream; the same holds
+        for device=True in draw_rgba16f, draw_colorbuf (out=: a dict) and render_text."""
+        if device:
+            h, w = self._rows(shard)
+            return self._render_device(shard, {"srgb8": ((h, w, 4), _torch().uint8)}, out,
+                                       lambda t, info: Rendering((w, h), t["srgb8"], int(info.flaws), info))
         rt = self._require()
         n = self.pixel_count(shard)
         w = self.camera.data.fb_width
@@ -1278,9 +1584,12 @@ class RtRenderer:
 
     draw_rgba = draw
 
-    def draw_rgba16f(self, shard=None):
+    def draw_rgba16f(self, shard=None, device=False, out=None):
         """The per-pixel colour raytrace_to_texture uploads (raytrace_to_texture.rs:645-661): premultiplied RGBA,
         exposure applied, as float16 [h, w, 4]."""
+        if device:
+            h, w = self._rows(shard)
+            return self._render_device(shard, {"rgba16f": ((h, w, 4), _torch().float16)}, out, lambda t, info: t["rgba16f"])
         rt = self._require()
         n = self.pixel_count(shard)
         w = self.camera.data.fb_width
@@ -1293,8 +1602,11 @@ class RtRenderer:
         h = n // w if w else 0
         return out.reshape(h, w, 4) if w else out.reshape(0, 0, 4)
 
-    def draw_colorbuf(self, shard=None, want_depth=True, want_hit=True, want_steps=True):
+    def draw_colorbuf(self, shard=None, want_depth=True, want_hit=True, want_steps=True, device=False, out=None):
         """RtRenderer::draw::<ColorBuf> (+DepthBuf, +Position) (renderer.rs:183-220)."""
+        if device:
+            return self._render_device(shard, _colorbuf_spec(self.pixel_count(shard), want_depth, want_hit, want_steps),
+                                       out, _colorbuf_result)
         rt = self._require()
         n = self.pixel_count(shard)
         cb = np.empty((n, 4), dtype=np.float32)
@@ -1310,6 +1622,19 @@ class RtRenderer:
                                                    hit.ctypes.data if want_hit else None,
                                                    steps.ctypes.data if want_steps else None, n, C.byref(info)))
         return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
+
+    def render_text(self, device=False, out=None):
+        """aicb_render_text of the whole frame: per pixel the CharacterBuf state (block index or abi.TEXT_*), int32
+        [h, w]."""
+        w, h = self.camera.data.fb_width, self.camera.data.fb_height
+        if device:
+            return self._render_device(None, {"text": ((h, w), _torch().int32)}, out, lambda t, info: t["text"])
+        rt = self._require()
+        text = np.zeros((h, w), dtype=np.int32)
+        o = rt.graphics_options.to_abi(True)
+        _check(load_library().aicb_render_text(rt.handle, C.byref(self.camera.data), C.byref(o), text.ctypes.data, w * h,
+                                               None))
+        return text
 
 
 HeadlessRenderer = RtRenderer

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 17
+ABI_VERSION = 18
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -131,11 +131,20 @@ class TerminalPixel(C.Structure):
     _fields_ = [("rgba", C.c_float * 4), ("text", C.c_int32), ("layer", C.c_int32)]
 
 
+class DeviceOutputs(C.Structure):
+    """aicb_device_outputs: nullable device pointers of the device-output calls, their length and full_frame."""
+    _fields_ = [("srgb8", C.c_void_p), ("rgba16f", C.c_void_p), ("colorbuf", C.c_void_p), ("depth", C.c_void_p),
+                ("hit", C.c_void_p), ("steps", C.c_void_p), ("text", C.c_void_p), ("texel_rgba16f", C.c_void_p),
+                ("texel_depth", C.c_void_p), ("terminal", C.c_void_p), ("len", C.c_size_t), ("full_frame", C.c_uint32),
+                ("_pad", C.c_uint32)]
+
+
 EXPORTED_SYMBOLS = [
     "aicb_abi_version",
     "aicb_ctx_create",
     "aicb_ctx_destroy",
     "aicb_ctx_stage_timing",
+    "aicb_ctx_device",
     "aicb_last_error",
     "aicb_scene_create",
     "aicb_scene_update_cubes",
@@ -160,6 +169,9 @@ EXPORTED_SYMBOLS = [
     "aicb_render_srgb8_device",
     "aicb_render_srgb8_device_frame",
     "aicb_render_finish",
+    "aicb_render_device",
+    "aicb_trace_rays_device",
+    "aicb_render_layers_device",
     "aicb_frame_create",
     "aicb_frame_open",
     "aicb_frame_close",
@@ -214,6 +226,9 @@ EXPORTED_SYMBOLS = [
     "aicb_group_render_text",
     "aicb_group_ortho_image_size",
     "aicb_group_render_orthographic",
+    "aicb_group_render_device",
+    "aicb_group_trace_rays_device",
+    "aicb_group_render_layers_device",
     "aicb_group_light_fast_evaluate",
     "aicb_group_light_compute",
     "aicb_group_light_compute_debug",

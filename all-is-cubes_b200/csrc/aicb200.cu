@@ -539,6 +539,12 @@ static uint32_t shard_rows(uint32_t fb_height, const aicb_shard *sh) {
     return rows;
 }
 
+// A layered frame's accumulators before its world pass, where a backdrop but no UI layer lies in front of the world.
+static __global__ void __launch_bounds__(256) fill_accum_kernel(float4 *__restrict__ accum, size_t n, float4 v) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) accum[i] = v;
+}
+
 // The compositing kernels of a frame's target (TGT_*): resolve_kernel with None / Flat lighting, encode_kernel after
 // shade_kernel.
 static kernel_fn resolve_for(int lc, int tgt) {
@@ -552,9 +558,13 @@ static kernel_fn encode_for(int tgt) {
     return tgt == TGT_TEX ? encode_kernel<TGT_TEX> : (tgt == TGT_TERM ? encode_kernel<TGT_TERM> : encode_kernel<TGT_FRAME>);
 }
 
-// Launches the trace kernel on `stream`. Camera rays when cam != NULL, the explicit rays of `out` otherwise.
+// Launches the trace kernel on `stream`. Camera rays when cam != NULL, the explicit rays of `out` otherwise.  With
+// `continues`, the pass continues the context's frame in flight on the same stream (the world pass of a layered frame
+// behind its UI pass, aicb_render_layers_device): the frame counters, the overflow flag and the start event carry on,
+// so finish reports both passes, and the frame is finished on `sc`.
 static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const aicb_options *opt,
-                                const aicb_shard *shard, const Outputs &out, cudaStream_t stream) {
+                                const aicb_shard *shard, const Outputs &out, cudaStream_t stream,
+                                bool continues = false) {
     aicb_ctx *ctx = sc->ctx;
     TraceParams P;
     std::memset(&P, 0, sizeof P);
@@ -620,11 +630,20 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     P.tail_divisor = TAIL_DIVISOR;
     P.event_threshold = EVENT_THRESHOLD;
 
+    uint64_t frame_pixels = pixels, frame_rays = pixels * (P.antialias ? 4 : 1);
+    uint64_t out_bytes =
+        (P.target.out_srgb8 ? 4 : (tgt == TGT_TEX ? 12 : (tgt == TGT_TERM ? 24 : (P.target.out_rgba16f ? 8 : 16)))) * pixels;
+    if (continues && ctx->last_scene) {
+        aicb_scene *prev = ctx->last_scene;
+        frame_pixels += prev->pending_pixels;
+        frame_rays += prev->pending_rays;
+        out_bytes += prev->pending_out_bytes;
+        prev->pending = false;
+    }
     sc->pending = true;
-    sc->pending_pixels = pixels;
-    sc->pending_rays = pixels * (P.antialias ? 4 : 1);
-    sc->pending_out_bytes_per_pixel =
-        P.target.out_srgb8 ? 4 : (tgt == TGT_TEX ? 12 : (tgt == TGT_TERM ? 24 : (P.target.out_rgba16f ? 8 : 16)));
+    sc->pending_pixels = frame_pixels;
+    sc->pending_rays = frame_rays;
+    sc->pending_out_bytes = out_bytes;
 
     // ---- the kernels of a frame, chunked so the per-frame streams stay bounded ----------------------------------
     P.n_samples = P.antialias ? 4 : 1;
@@ -669,8 +688,12 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     ctx->frame_in_flight = true;
     ctx->last_stream = stream;
     ctx->last_scene = sc;
-    CU(cudaMemsetAsync(P.counters, 0, 8 * sizeof(unsigned long long) + 2 * (4 + N_BINS) * sizeof(unsigned int), stream));
-    CU(cudaEventRecord(ctx->ev0.get(), stream));
+    if (continues) {
+        CU(cudaMemsetAsync(ctx->d_tile_counter, 0, 2 * (4 + N_BINS) * sizeof(unsigned int), stream));
+    } else {
+        CU(cudaMemsetAsync(P.counters, 0, 8 * sizeof(unsigned long long) + 2 * (4 + N_BINS) * sizeof(unsigned int), stream));
+        CU(cudaEventRecord(ctx->ev0.get(), stream));
+    }
     if (total_tasks > 0) {
         const bool volumetric = opt->transparency == AICB_TRANSPARENCY_VOLUMETRIC;
         const int lc = opt->lighting_display == AICB_LIGHT_NONE ? LC_NONE
@@ -847,11 +870,83 @@ static aicb_status finish(aicb_scene *sc, aicb_render_info *info) {
         info->counters[5] = sc->pending_pixels;
         // SURVEY 8(d): 2 B per outer/inner step, 32 B per surface hit, 4 B per light texel,
         // 32 B per recursive block entered (our BlockRec), + output bytes per pixel
-        info->algorithmic_bytes = 2 * c[1] + 2 * c[2] + 32 * c[3] + 4 * c[4] + 32 * c[5] +
-                                  (uint64_t)sc->pending_out_bytes_per_pixel * sc->pending_pixels;
+        info->algorithmic_bytes = 2 * c[1] + 2 * c[2] + 32 * c[3] + 4 * c[4] + 32 * c[5] + sc->pending_out_bytes;
         info->flaws = 0;
     }
     sc->pending = false;
+    return AICB_OK;
+}
+
+// ---- outputs in the caller's device memory (aicb_device_outputs) --------------------------------------------------
+aicb_status issue_empty_frame(aicb_scene *s, const aicb_options *opt, cudaStream_t stream) {
+    return launch_trace(s, nullptr, opt, nullptr, Outputs{}, stream);
+}
+
+// A caller's device buffer: memory of `device`, or with peer_ok of a device it reaches as a peer (a frame of another
+// rank mapped into this process, aicb_render_srgb8_device_frame), aligned to `align` bytes, the width of the kernels'
+// stores to it or loads from it (a misaligned vector access would fault the context).
+aicb_status check_device_pointer(const void *p, int device, bool peer_ok, size_t align, const char *what) {
+    if ((uintptr_t)p % align)
+        return fail(AICB_ERR_INVALID, std::string(what) + " is not aligned to " + std::to_string(align) + " bytes");
+    cudaPointerAttributes a;
+    const cudaError_t e = cudaPointerGetAttributes(&a, p);
+    if (e != cudaSuccess) cudaGetLastError();
+    if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged))
+        return fail(AICB_ERR_INVALID, std::string(what) + " is not device memory");
+    if (a.device == device) return AICB_OK;
+    int can = 0;
+    if (peer_ok && cudaDeviceCanAccessPeer(&can, device, a.device) == cudaSuccess && can) return AICB_OK;
+    return fail(AICB_ERR_INVALID, std::string(what) + " is memory of another device");
+}
+
+aicb_status device_target(const aicb_device_outputs *d, int device, DeviceCall call, bool need_colorbuf, bool peer_ok,
+                          Outputs *o) {
+    if (!d) return fail(AICB_ERR_INVALID, "outs is NULL");
+    const void *const ptr[10] = {d->srgb8, d->rgba16f, d->colorbuf, d->depth, d->hit,
+                                 d->steps, d->text,    d->texel_rgba16f, d->texel_depth, d->terminal};
+    static const char *const name[10] = {"srgb8", "rgba16f", "colorbuf", "depth", "hit",
+                                         "steps", "text",    "texel_rgba16f", "texel_depth", "terminal"};
+    // the width of each output's stores (uchar4, uint2, float4, double, aicb_hit, u32, i32, uint2, float, 2 x float2)
+    static const size_t align[10] = {4, 8, 16, 8, 4, 4, 4, 8, 4, 8};
+    unsigned set = 0;
+    for (int i = 0; i < 10; i++)
+        if (ptr[i]) set |= 1u << i;
+    // the sets of outputs one host call gives: sRGB8, rgba16f, ColorBuf and its companions, text; layered: sRGB8,
+    // the terminal's pixels, the texture's two texels
+    const unsigned SRGB8 = 1, RGBA16F = 2, AUX = 4 | 8 | 16 | 32, TEXT = 64, TEXELS = 128 | 256, TERMINAL = 512;
+    const bool aux = set && !(set & ~AUX);
+    bool ok = false;
+    switch (call) {
+        case DEV_FRAME: ok = set == SRGB8 || set == RGBA16F || aux || set == TEXT; break;
+        case DEV_RAYS: ok = aux; break;
+        case DEV_LAYERS: ok = set == SRGB8 || set == TERMINAL || set == TEXELS; break;
+    }
+    if (set == 0 && d->len == 0) ok = true;
+    if (!ok) return fail(AICB_ERR_INVALID, "the outputs are not a set that this call gives (aicb_device_outputs)");
+    if (aux && need_colorbuf && d->len && !d->colorbuf) return fail(AICB_ERR_INVALID, "colorbuf is NULL");
+    for (int i = 0; i < 10; i++)
+        if (ptr[i]) TRY(check_device_pointer(ptr[i], device, peer_ok, align[i], name[i]));
+    TargetParams &t = o->target;
+    t.out_srgb8 = (uchar4 *)d->srgb8;
+    t.out_text = d->text;
+    o->aux = aux;
+    if (aux) {
+        t.out_colorbuf = (float4 *)d->colorbuf;
+        t.out_depth = d->depth;
+        t.out_hit = d->hit;
+        t.out_steps = d->steps;
+    }
+    if (set == RGBA16F) t.out_rgba16f = (uint2 *)d->rgba16f;
+    if (set == TEXELS) {
+        o->kind = TGT_TEX;
+        t.out_rgba16f = (uint2 *)d->texel_rgba16f;
+        t.out_tex_depth = d->texel_depth;
+    }
+    if (set == TERMINAL) {
+        o->kind = TGT_TERM;
+        t.out_term = d->terminal;
+        t.text_start = AICB_TEXT_EMPTY;
+    }
     return AICB_OK;
 }
 
@@ -1690,6 +1785,8 @@ int aicb_debug_shade_phases(unsigned long long *out) {
 }
 #endif
 
+int aicb_ctx_device(const aicb_ctx *c) { return c ? c->device : -1; }
+
 void aicb_ctx_destroy(aicb_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
@@ -1832,32 +1929,53 @@ aicb_status aicb_render_colorbuf(aicb_scene *s, const aicb_camera *cam, const ai
     });
 }
 
-aicb_status aicb_render_srgb8_device(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
-                                     const aicb_shard *shard, void *d_out, size_t out_len, void *stream) {
-    aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
-    if (st != AICB_OK) return st;
-    if (out_len && !d_out) return fail(AICB_ERR_INVALID, "d_out is NULL");
+aicb_status aicb_render_device(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
+                               const aicb_device_outputs *outs, void *stream) {
+    if (!s || !cam || !outs) return fail(AICB_ERR_INVALID, "NULL argument");
+    const bool full = outs->full_frame != 0;
+    TRY(aicb_check_render_args(s, cam, opt, shard, full ? aicb_shard_pixel_count(cam, shard) : outs->len));
+    if (full && outs->len != (size_t)cam->fb_width * cam->fb_height)
+        return fail(AICB_ERR_INVALID, "Viewport size does not match frame buffer length");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     Outputs o;
-    o.target.out_srgb8 = (uchar4 *)d_out;
+    TRY(device_target(outs, s->ctx->device, DEV_FRAME, false, full, &o));
+    o.full_frame = full;
     return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream.get());
+}
+
+aicb_status aicb_render_srgb8_device(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
+                                     const aicb_shard *shard, void *d_out, size_t out_len, void *stream) {
+    aicb_device_outputs o{};
+    o.srgb8 = (uint8_t(*)[4])d_out;
+    o.len = out_len;
+    return aicb_render_device(s, cam, opt, shard, &o, stream);
 }
 
 aicb_status aicb_render_srgb8_device_frame(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
                                            const aicb_shard *shard, void *d_frame, size_t frame_len, void *stream) {
-    if (!s || !cam) return fail(AICB_ERR_INVALID, "NULL argument");
-    aicb_status st = aicb_check_render_args(s, cam, opt, shard, aicb_shard_pixel_count(cam, shard));
-    if (st != AICB_OK) return st;
-    if (frame_len != (size_t)cam->fb_width * cam->fb_height)
-        return fail(AICB_ERR_INVALID, "Viewport size does not match frame buffer length");
-    if (frame_len && !d_frame) return fail(AICB_ERR_INVALID, "d_frame is NULL");
+    aicb_device_outputs o{};
+    o.srgb8 = (uint8_t(*)[4])d_frame;
+    o.len = frame_len;
+    o.full_frame = 1;
+    return aicb_render_device(s, cam, opt, shard, &o, stream);
+}
+
+aicb_status aicb_trace_rays_device(aicb_scene *s, const double (*d_origin_dir)[6], size_t n, const aicb_options *opt,
+                                   const aicb_device_outputs *outs, void *stream) {
+    if (!s || !outs || (n && !d_origin_dir)) return fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(validate_options(opt));
+    if (outs->full_frame) return fail(AICB_ERR_INVALID, "full_frame is for camera frames");
+    if (outs->len != n) return fail(AICB_ERR_INVALID, "outs->len must equal the number of rays");
+    if (n > 0xffffffffull) return fail(AICB_ERR_INVALID, "too many rays");
     std::lock_guard<std::mutex> lock(s->ctx->mu);
     CU(cudaSetDevice(s->ctx->device));
     Outputs o;
-    o.full_frame = true;
-    o.target.out_srgb8 = (uchar4 *)d_frame;
-    return launch_trace(s, cam, opt, shard, o, stream ? (cudaStream_t)stream : s->ctx->stream.get());
+    TRY(device_target(outs, s->ctx->device, DEV_RAYS, false, false, &o));
+    if (n) TRY(check_device_pointer(d_origin_dir, s->ctx->device, false, 8, "the ray batch"));
+    o.rays = (const double *)d_origin_dir;   // gen_kernel reads the caller's batch in place
+    o.n_rays = n;
+    return launch_trace(s, nullptr, opt, nullptr, o, stream ? (cudaStream_t)stream : s->ctx->stream.get());
 }
 
 // ---- full-frame buffers shared between ranks (CUDA IPC) ------------------------------------------
@@ -2085,10 +2203,13 @@ aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera 
 // accumulator (its rays start opaque where the UI covered the pixel), and a pixel that is not opaque in the end — there
 // is no world — is painted NO_WORLD_TO_SHOW.  The last pass writes each part's target; with texture targets the UI pass
 // hands its DepthBuf on next to its ColorBuf, with terminal targets its CharacterBuf.  Each pass runs on every part
-// through aicb_trace_pass (a re-issued world pass starts from the same accumulator).  The caller holds the parts'
+// through aicb_trace_pass (a re-issued world pass starts from the same accumulator).  With `async` (one part), the
+// passes are issued back to back on that stream instead, the world pass continuing the UI pass's frame, and
+// aicb_render_finish on the last pass's scene finishes them (total is not filled).  The caller holds the parts'
 // contexts' locks.
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
-                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total) {
+                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total,
+                              cudaStream_t async) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
     const aicb_layer *lead = have_world ? world : ui;
     aicb_status st = AICB_OK;
@@ -2125,6 +2246,7 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
     // one pass of the frame on every part: `layer` picks the part's scene, `outputs(part, ctx)` its Outputs; each
     // part's info sums its passes
     std::vector<FramePart> pass_parts(n_parts);
+    bool first_pass = true;
     auto pass = [&](aicb_scene *LayerPart::*layer, const aicb_camera *cam, const aicb_options *opt,
                     auto outputs) -> aicb_status {
         for (size_t i = 0; i < n_parts; i++) {
@@ -2132,7 +2254,11 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
             pass_parts[i].shard = &parts[i].shard;
             pass_parts[i].out = outputs(parts[i], pass_parts[i].scene->ctx);
         }
-        return aicb_trace_pass(pass_parts.data(), n_parts, cam, opt, true);
+        if (!async) return aicb_trace_pass(pass_parts.data(), n_parts, cam, opt, true);
+        const FramePart &p = pass_parts[0];
+        const bool continues = !first_pass;
+        first_pass = false;
+        return launch_trace(p.scene, cam, opt, p.shard, p.out, async, continues);
     };
     if (have_ui && have_world) {
         for (size_t i = 0; i < n_parts; i++) {
@@ -2188,8 +2314,12 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
                 const size_t n = n_tasks(parts[i]);
                 CU(cudaSetDevice(ctx->device));
                 TRY(ctx->d_task_aux.ensure(n * sizeof(float4) + 16));
-                std::vector<float4> init(n, make_float4(backdrop[0] * 1.0f, backdrop[1] * 1.0f, backdrop[2] * 1.0f, 1.0f * backdrop[3]));
-                CU(cudaMemcpy(ctx->d_task_aux.get(), init.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
+                // stream-ordered: behind the context's last frame, which may still read the accumulators
+                const cudaStream_t stream = async ? async : ctx->stream.get();
+                if (ctx->frame_in_flight && ctx->last_stream != stream) CU(cudaStreamWaitEvent(stream, ctx->ev1.get(), 0));
+                fill_accum_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
+                    ctx->d_task_aux.get<float4>(), n, make_float4(backdrop[0], backdrop[1], backdrop[2], backdrop[3]));
+                CU(cudaGetLastError());
             }
         }
         st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
@@ -2213,15 +2343,16 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
             return o;
         });
     }
-    if (st != AICB_OK) return st;
+    if (st != AICB_OK || async) return st;
     std::memset(total, 0, sizeof *total);
     for (const FramePart &p : pass_parts) aicb_merge_info(total, &p.info, false);
     return AICB_OK;
 }
 
 aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba,
-                                      const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
-                                      const void *out_rgba16f, const float *out_depth, const aicb_layer **lead_out) {
+                                      const double *depth_transform, const uint32_t *pixels, bool pixels_on_device,
+                                      size_t n_pixels, const void *out_rgba16f, const float *out_depth,
+                                      const aicb_layer **lead_out) {
     const bool have_world = world && world->scene;
     const aicb_layer *lead0 = have_world ? world : ui;
     if (!lead0 || !lead0->camera) return fail(AICB_ERR_INVALID, "a layer needs its camera and options");
@@ -2233,7 +2364,7 @@ aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer 
         return fail(AICB_ERR_INVALID, "without a pixel list n_pixels must be fb_width * fb_height");
     if (n_pixels > 0xffffffffull / 4) return fail(AICB_ERR_INVALID, "too many pixels");
     if (n_pixels && (!out_rgba16f || !out_depth)) return fail(AICB_ERR_INVALID, "an output is NULL");
-    if (pixels)
+    if (pixels && !pixels_on_device)   // (a device list is read as it is)
         for (size_t i = 0; i < n_pixels; i++)
             if (pixels[i] >= fb_pixels) return fail(AICB_ERR_INVALID, "pixel index >= fb_width * fb_height");
     return AICB_OK;
@@ -2280,6 +2411,15 @@ aicb_status aicb_render_layers_texture(const aicb_layer *world, const aicb_layer
                                        float *out_depth, aicb_render_info *info) {
     return layers_texture(one_context(world, ui, backdrop_rgba, no_world_rgba), depth_transform, pixels, n_pixels,
                           out_rgba16f, out_depth, info);
+}
+
+// The three layered calls into the caller's device memory, issued on its stream and finished by aicb_render_finish.
+aicb_status aicb_render_layers_device(const aicb_layer *world, const aicb_layer *ui, const float backdrop_rgba[4],
+                                      const float no_world_rgba[4], const double depth_transform[16],
+                                      const uint32_t *d_pixels, size_t n_pixels, const aicb_device_outputs *outs,
+                                      void *stream) {
+    return layers_device(one_context(world, ui, backdrop_rgba, no_world_rgba), depth_transform, d_pixels, n_pixels,
+                         outs, (cudaStream_t)stream, true, nullptr);
 }
 
 // == render_orthographic (raytracer/ortho.rs:30-84) with MultiOrthoCamera (:143-199) / OrthoCamera (:209-297): five

@@ -57,10 +57,11 @@ aicb_status fan_in(aicb_ctx *const *ctx, size_t n) {
 // Every context's part of a layered call.  A whole frame or texture: interleaved 16-row strips, outputs at their
 // framebuffer positions in device 0's buffers (`target`).  A pixel list: contiguous ranges of whole warps (a warp
 // takes 32 consecutive list entries), as even as whole warps allow; context i traces its range from its own copy of
-// it (its d_aux) and stores at the range's offset, so list order is kept.  One context: one part, every row or the
-// whole list.
+// it (its d_aux), or of a list in device 0's memory (pixels_on_device) in place, and stores at the range's offset, so
+// list order is kept.  One context: one part, every row or the whole list.
 static aicb_status layer_parts(const LayeredCall &c, aicb_ctx *const *ctx, const Outputs &target,
-                               const uint32_t *pixels, size_t n_pixels, std::vector<LayerPart> *parts) {
+                               const uint32_t *pixels, bool pixels_on_device, size_t n_pixels,
+                               std::vector<LayerPart> *parts) {
     auto part = [&](size_t i) {
         LayerPart p;
         p.world = c.world_scenes ? c.world_scenes[i] : nullptr;
@@ -78,11 +79,15 @@ static aicb_status layer_parts(const LayeredCall &c, aicb_ctx *const *ctx, const
     const std::vector<WarpRange> ranges = warp_ranges(n_pixels, c.n);
     for (size_t i = 0; i < ranges.size(); i++) {
         const size_t begin = ranges[i].begin, count = ranges[i].count;
-        CU(cudaSetDevice(ctx[i]->device));
-        TRY(ctx[i]->d_aux.ensure(count * 4 + 16));
-        CU(cudaMemcpy(ctx[i]->d_aux.get(), pixels + begin, count * 4, cudaMemcpyHostToDevice));
         LayerPart p = part(i);
-        p.out.target.pixel_list = ctx[i]->d_aux.get<const uint32_t>();
+        if (pixels_on_device) {
+            p.out.target.pixel_list = pixels + begin;
+        } else {
+            CU(cudaSetDevice(ctx[i]->device));
+            TRY(ctx[i]->d_aux.ensure(count * 4 + 16));
+            CU(cudaMemcpy(ctx[i]->d_aux.get(), pixels + begin, count * 4, cudaMemcpyHostToDevice));
+            p.out.target.pixel_list = ctx[i]->d_aux.get<const uint32_t>();
+        }
         p.out.target.n_list = (uint32_t)count;
         p.out.target.out_rgba16f = target.target.out_rgba16f + begin;
         p.out.target.out_tex_depth = target.target.out_tex_depth + begin;
@@ -104,12 +109,29 @@ std::vector<WarpRange> warp_ranges(size_t n_items, size_t n_ctx) {
     return ranges;
 }
 
-aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies) {
+aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies, cudaStream_t caller) {
     TRY(fan_in(ctx, n_parts));
     cudaStream_t stream = ctx[0]->stream.get();
     for (const Delivery &d : copies)
         if (d.bytes) CU(cudaMemcpyAsync(d.to, d.from, d.bytes, cudaMemcpyDeviceToHost, stream));
+    if (caller) {
+        CU(cudaEventRecord(ctx[0]->ev_join.get(), stream));
+        CU(cudaStreamWaitEvent(caller, ctx[0]->ev_join.get(), 0));
+    }
     CU(cudaStreamSynchronize(stream));
+    return AICB_OK;
+}
+
+// Every listed context's stream waits for the work queued on the caller's stream (device 0's; none if NULL) so far,
+// which may be writing the call's inputs or still using its output buffers' memory.
+static aicb_status after_caller(aicb_ctx *const *ctx, size_t n, cudaStream_t caller) {
+    if (!caller) return AICB_OK;
+    CU(cudaSetDevice(ctx[0]->device));
+    CU(cudaEventRecord(ctx[0]->ev_join.get(), caller));
+    for (size_t i = 0; i < n; i++) {
+        CU(cudaSetDevice(ctx[i]->device));
+        CU(cudaStreamWaitEvent(ctx[i]->stream.get(), ctx[0]->ev_join.get(), 0));
+    }
     return AICB_OK;
 }
 
@@ -123,13 +145,14 @@ static std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *
 
 // The rest of a layered call once device 0's outputs are in `target`: the parts, the layers, the delivery.
 static aicb_status draw_layers(const LayeredCall &c, const std::vector<aicb_ctx *> &ctx, const Outputs &target,
-                               const uint32_t *pixels, size_t n_pixels, const std::vector<Delivery> &copies,
-                               aicb_render_info *info) {
+                               const uint32_t *pixels, bool pixels_on_device, size_t n_pixels,
+                               const std::vector<Delivery> &copies, cudaStream_t caller, aicb_render_info *info) {
     std::vector<LayerPart> parts;
-    TRY(layer_parts(c, ctx.data(), target, pixels, n_pixels, &parts));
+    TRY(layer_parts(c, ctx.data(), target, pixels, pixels_on_device, n_pixels, &parts));
     aicb_render_info total;
-    TRY(aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), &total));
-    TRY(deliver(ctx.data(), parts.size(), copies));
+    TRY(aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), &total,
+                          nullptr));
+    TRY(deliver(ctx.data(), parts.size(), copies, caller));
     if (info) *info = total;
     return AICB_OK;
 }
@@ -145,7 +168,7 @@ aicb_status layers_srgb8(const LayeredCall &c, uint8_t (*out)[4], size_t out_len
     Outputs target;
     target.full_frame = true;
     target.target.out_srgb8 = ctx[0]->d_out.get<uchar4>();
-    return draw_layers(c, ctx, target, nullptr, 0, {{out, ctx[0]->d_out.get(), out_len * 4}}, info);
+    return draw_layers(c, ctx, target, nullptr, false, 0, {{out, ctx[0]->d_out.get(), out_len * 4}}, nullptr, info);
 }
 
 aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info) {
@@ -162,13 +185,13 @@ aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size
     target.kind = aicb::TGT_TERM;
     target.target.out_term = ctx[0]->d_out.get<aicb_terminal_pixel>();
     target.target.text_start = AICB_TEXT_EMPTY;
-    return draw_layers(c, ctx, target, nullptr, 0, {{out, ctx[0]->d_out.get(), bytes}}, info);
+    return draw_layers(c, ctx, target, nullptr, false, 0, {{out, ctx[0]->d_out.get(), bytes}}, nullptr, info);
 }
 
 aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
                            uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info) {
     const aicb_layer *lead = nullptr;
-    TRY(aicb_check_layers_texture(c.world, c.ui, c.no_world_rgba, depth_transform, pixels, n_pixels, out_rgba16f,
+    TRY(aicb_check_layers_texture(c.world, c.ui, c.no_world_rgba, depth_transform, pixels, false, n_pixels, out_rgba16f,
                                   out_depth, &lead));
     if (info) std::memset(info, 0, sizeof *info);
     if (n_pixels == 0) return AICB_OK;
@@ -183,8 +206,44 @@ aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, 
     aicb_texture_target(c.world, c.ui, depth_transform, &target);
     target.target.out_rgba16f = (uint2 *)base;
     target.target.out_tex_depth = (float *)(base + off_depth);
-    return draw_layers(c, ctx, target, pixels, n_pixels,
-                       {{out_rgba16f, base, n_pixels * 8}, {out_depth, base + off_depth, n_pixels * 4}}, info);
+    return draw_layers(c, ctx, target, pixels, false, n_pixels,
+                       {{out_rgba16f, base, n_pixels * 8}, {out_depth, base + off_depth, n_pixels * 4}}, nullptr, info);
+}
+
+aicb_status layers_device(const LayeredCall &c, const double *depth_transform, const uint32_t *d_pixels, size_t n_pixels,
+                          const aicb_device_outputs *outs, cudaStream_t stream, bool async, aicb_render_info *info) {
+    if (!outs) return aicb_fail(AICB_ERR_INVALID, "outs is NULL");
+    if (outs->full_frame) return aicb_fail(AICB_ERR_INVALID, "full_frame is for aicb_render_device");
+    const aicb_layer *lead = nullptr;
+    const bool texels = outs->texel_rgba16f || outs->texel_depth;
+    if (texels) {
+        TRY(aicb_check_layers_texture(c.world, c.ui, c.no_world_rgba, depth_transform, d_pixels, true, n_pixels,
+                                      outs->texel_rgba16f, outs->texel_depth, &lead));
+        if (outs->len != n_pixels) return aicb_fail(AICB_ERR_INVALID, "outs->len must equal n_pixels");
+    } else {
+        TRY(aicb_check_layers(c.world, c.ui, c.no_world_rgba, outs->len, &lead));
+        if (d_pixels || n_pixels) return aicb_fail(AICB_ERR_INVALID, "a pixel list is for the texture's texels");
+    }
+    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
+    ContextLocks lock(ctx);
+    CU(cudaSetDevice(ctx[0]->device));
+    Outputs target;
+    TRY(device_target(outs, ctx[0]->device, DEV_LAYERS, false, false, &target));
+    if (d_pixels && n_pixels) TRY(check_device_pointer(d_pixels, ctx[0]->device, false, 4, "the pixel list"));
+    if (target.kind == aicb::TGT_TEX) aicb_texture_target(c.world, c.ui, depth_transform, &target);
+    target.full_frame = true;
+    if (info) std::memset(info, 0, sizeof *info);
+    if (async) {
+        if (!stream) stream = ctx[0]->stream.get();
+        if (texels && n_pixels == 0) return issue_empty_frame(lead->scene, lead->options, stream);
+        std::vector<LayerPart> parts;
+        TRY(layer_parts(c, ctx.data(), target, d_pixels, true, n_pixels, &parts));
+        return aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), nullptr,
+                                 stream);
+    }
+    if (texels && n_pixels == 0) return AICB_OK;
+    TRY(after_caller(ctx.data(), c.n, stream));
+    return draw_layers(c, ctx, target, d_pixels, true, n_pixels, {}, stream, info);
 }
 
 // ---- world-only frames and ray batches of one scene -------------------------------------------------------------------
@@ -197,9 +256,11 @@ static void sum_info(const std::vector<FramePart> &parts, aicb_render_info *info
 
 // A frame of the replicas' scene with the caller's options as given: interleaved 16-row strips as
 // aicb_group_render_srgb8 cuts them, each part storing at framebuffer positions in device 0's outputs (`target`); with
-// `shard` (one context), that shard's rows, packed.  Then the delivery of device 0's outputs.
+// `shard` (one context), that shard's rows, packed.  Then the delivery of device 0's outputs; a caller's stream
+// (`caller`, or NULL) goes first and waits for them.
 static aicb_status draw_frame(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
-                              Outputs target, const std::vector<Delivery> &copies, aicb_render_info *info) {
+                              Outputs target, const std::vector<Delivery> &copies, cudaStream_t caller,
+                              aicb_render_info *info) {
     std::vector<LayerPart> strips;   // (the parts' shards)
     std::vector<FramePart> parts;
     if (shard) {
@@ -208,11 +269,12 @@ static aicb_status draw_frame(Replicas r, const aicb_camera *cam, const aicb_opt
         target.full_frame = true;
         const aicb_layer w0 = {r.scene[0], cam, opt};
         const LayeredCall world = {&w0, nullptr, r.scene, nullptr, r.n, nullptr, nullptr};
-        TRY(layer_parts(world, r.ctx, target, nullptr, 0, &strips));
+        TRY(layer_parts(world, r.ctx, target, nullptr, false, 0, &strips));
         for (const LayerPart &p : strips) parts.push_back({p.world, &p.shard, p.out});
     }
+    TRY(after_caller(r.ctx, parts.size(), caller));
     TRY(aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr));
-    TRY(deliver(r.ctx, parts.size(), copies));
+    TRY(deliver(r.ctx, parts.size(), copies, caller));
     sum_info(parts, info);
     return AICB_OK;
 }
@@ -251,7 +313,7 @@ aicb_status frame_colorbuf(Replicas r, const aicb_camera *cam, const aicb_option
                            AuxOutputs out, size_t out_len, aicb_render_info *info) {
     Outputs target;
     TRY(aux_target(r.ctx[0], out_len, out, &target));
-    return draw_frame(r, cam, opt, shard, target, aux_copies(target, out, out_len), info);
+    return draw_frame(r, cam, opt, shard, target, aux_copies(target, out, out_len), nullptr, info);
 }
 
 aicb_status frame_rgba16f(Replicas r, const aicb_camera *cam, const aicb_options *opt, uint16_t (*out)[4],
@@ -261,7 +323,7 @@ aicb_status frame_rgba16f(Replicas r, const aicb_camera *cam, const aicb_options
     TRY(root->d_out.ensure(out_len * 8 + 16));
     Outputs target;
     target.target.out_rgba16f = root->d_out.get<uint2>();
-    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 8}}, info);
+    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 8}}, nullptr, info);
 }
 
 aicb_status frame_text(Replicas r, const aicb_camera *cam, const aicb_options *opt, int32_t *out, size_t out_len,
@@ -271,23 +333,27 @@ aicb_status frame_text(Replicas r, const aicb_camera *cam, const aicb_options *o
     TRY(root->d_out.ensure(out_len * 4 + 16));
     Outputs target;
     target.target.out_text = root->d_out.get<int32_t>();
-    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 4}}, info);
+    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 4}}, nullptr, info);
 }
 
-// Context i uploads its range of the batch to its own d_aux and stores at the range's offset in device 0's outputs.
-aicb_status rays_colorbuf(Replicas r, const double (*origin_dir)[6], size_t n, const aicb_options *opt, AuxOutputs out,
-                          aicb_render_info *info) {
-    if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "too many rays");
-    Outputs target;
-    TRY(aux_target(r.ctx[0], n, out, &target));
+// Context i uploads its range of the batch to its own d_aux (or with rays_on_device reads it in place from device 0's
+// memory) and stores at the range's offset in device 0's outputs.
+static aicb_status draw_rays(Replicas r, const double (*origin_dir)[6], bool rays_on_device, size_t n,
+                             const aicb_options *opt, const Outputs &target, const std::vector<Delivery> &copies,
+                             cudaStream_t caller, aicb_render_info *info) {
     const std::vector<WarpRange> ranges = warp_ranges(n, r.n);
     std::vector<FramePart> parts;
+    TRY(after_caller(r.ctx, ranges.size(), caller));
     for (size_t i = 0; i < ranges.size(); i++) {
         const size_t begin = ranges[i].begin, count = ranges[i].count;
         aicb_ctx *ctx = r.ctx[i];
         CU(cudaSetDevice(ctx->device));
-        TRY(ctx->d_aux.ensure(count * 48 + 16));
-        if (count) CU(cudaMemcpy(ctx->d_aux.get(), origin_dir + begin, count * 48, cudaMemcpyHostToDevice));
+        const double *rays = (const double *)(origin_dir + begin);
+        if (!rays_on_device) {
+            TRY(ctx->d_aux.ensure(count * 48 + 16));
+            if (count) CU(cudaMemcpy(ctx->d_aux.get(), origin_dir + begin, count * 48, cudaMemcpyHostToDevice));
+            rays = ctx->d_aux.get<double>();
+        }
         FramePart p{r.scene[i]};
         p.out = target;
         aicb::TargetParams &t = p.out.target;
@@ -295,14 +361,22 @@ aicb_status rays_colorbuf(Replicas r, const double (*origin_dir)[6], size_t n, c
         if (t.out_depth) t.out_depth += begin;
         if (t.out_hit) t.out_hit += begin;
         if (t.out_steps) t.out_steps += begin;
-        p.out.rays = ctx->d_aux.get<double>();
+        p.out.rays = rays;
         p.out.n_rays = count;
         parts.push_back(p);
     }
     TRY(aicb_trace_pass(parts.data(), parts.size(), nullptr, opt, info != nullptr));
-    TRY(deliver(r.ctx, parts.size(), aux_copies(target, out, n)));
+    TRY(deliver(r.ctx, parts.size(), copies, caller));
     sum_info(parts, info);
     return AICB_OK;
+}
+
+aicb_status rays_colorbuf(Replicas r, const double (*origin_dir)[6], size_t n, const aicb_options *opt, AuxOutputs out,
+                          aicb_render_info *info) {
+    if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "too many rays");
+    Outputs target;
+    TRY(aux_target(r.ctx[0], n, out, &target));
+    return draw_rays(r, origin_dir, false, n, opt, target, aux_copies(target, out, n), nullptr, info);
 }
 
 // The layers of a group call as device 0 sees them (its replicas, the cameras and options), and every replica of each.
@@ -445,7 +519,7 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
         Outputs target;
         target.target.out_srgb8 = root->d_out.get<uchar4>();
         // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
-        return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), pixels * 4}}, info);
+        return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), pixels * 4}}, nullptr, info);
     });
 }
 
@@ -532,6 +606,48 @@ aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world, const 
     LayeredCall c;
     TRY(group_call(world, ui, backdrop_rgba, no_world_rgba, views, &c));
     return layers_srgb8(c, out, out_len, info);
+}
+
+// The device-output calls on the group: every device stores into the caller's device-0 buffers; blocking.
+aicb_status aicb_group_render_device(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt,
+                                     const aicb_device_outputs *outs, void *stream, aicb_render_info *info) {
+    if (!gs || !outs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (outs->full_frame) return aicb_fail(AICB_ERR_INVALID, "full_frame is for aicb_render_device");
+    TRY(aicb_check_render_args(gs->scene[0], cam, opt, nullptr, outs->len));
+    return on_group(gs, false, [&](Replicas r) {
+        CU(cudaSetDevice(r.ctx[0]->device));
+        Outputs target;
+        TRY(device_target(outs, r.ctx[0]->device, DEV_FRAME, true, false, &target));
+        return draw_frame(r, cam, opt, nullptr, target, {}, (cudaStream_t)stream, info);
+    });
+}
+
+aicb_status aicb_group_trace_rays_device(aicb_group_scene *gs, const double (*d_origin_dir)[6], size_t n,
+                                         const aicb_options *opt, const aicb_device_outputs *outs, void *stream,
+                                         aicb_render_info *info) {
+    if (!gs || !outs || (n && !d_origin_dir)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(validate_options(opt));
+    if (outs->full_frame) return aicb_fail(AICB_ERR_INVALID, "full_frame is for aicb_render_device");
+    if (outs->len != n) return aicb_fail(AICB_ERR_INVALID, "outs->len must equal the number of rays");
+    if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "too many rays");
+    return on_group(gs, false, [&](Replicas r) {
+        CU(cudaSetDevice(r.ctx[0]->device));
+        Outputs target;
+        TRY(device_target(outs, r.ctx[0]->device, DEV_RAYS, true, false, &target));
+        if (n) TRY(check_device_pointer(d_origin_dir, r.ctx[0]->device, false, 8, "the ray batch"));
+        return draw_rays(r, d_origin_dir, true, n, opt, target, {}, (cudaStream_t)stream, info);
+    });
+}
+
+aicb_status aicb_group_render_layers_device(const aicb_group_layer *world, const aicb_group_layer *ui,
+                                            const float backdrop_rgba[4], const float no_world_rgba[4],
+                                            const double depth_transform[16], const uint32_t *d_pixels,
+                                            size_t n_pixels, const aicb_device_outputs *outs, void *stream,
+                                            aicb_render_info *info) {
+    aicb_layer views[2];
+    LayeredCall c;
+    TRY(group_call(world, ui, backdrop_rgba, no_world_rgba, views, &c));
+    return layers_device(c, depth_transform, d_pixels, n_pixels, outs, (cudaStream_t)stream, false, info);
 }
 
 aicb_status aicb_group_render_layers_terminal(const aicb_group_layer *world, const aicb_group_layer *ui,

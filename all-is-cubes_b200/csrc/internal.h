@@ -296,7 +296,7 @@ struct aicb_scene {
     bool pending = false;
     uint64_t pending_rays = 0;
     uint64_t pending_pixels = 0;
-    uint32_t pending_out_bytes_per_pixel = 0;
+    uint64_t pending_out_bytes = 0;   // the frame's output bytes (aicb_render_info::algorithmic_bytes)
     bool pending_fused = false;    // shading and encode ran as one kernel (resolve_kernel)
     LightState light;              // light propagation state (light.cu)
 };
@@ -345,11 +345,13 @@ aicb_status aicb_check_render_args(aicb_scene *s, const aicb_camera *cam, const 
 aicb_status aicb_check_layers(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba, size_t out_len,
                               const aicb_layer **lead_out);
 aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer *ui, const float *no_world_rgba,
-                                      const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
-                                      const void *out_rgba16f, const float *out_depth, const aicb_layer **lead_out);
+                                      const double *depth_transform, const uint32_t *pixels, bool pixels_on_device,
+                                      size_t n_pixels, const void *out_rgba16f, const float *out_depth,
+                                      const aicb_layer **lead_out);
 void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out);
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
-                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total);
+                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total,
+                              cudaStream_t async);
 aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
                             bool want_info);
 void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part);
@@ -450,6 +452,12 @@ aicb_status layers_srgb8(const LayeredCall &c, uint8_t (*out)[4], size_t out_len
 aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info);
 aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
                            uint16_t (*out_rgba16f)[4], float *out_depth, aicb_render_info *info);
+// The layered calls into the caller's device memory (aicb_render_layers_device, aicb_group_render_layers_device): the
+// output set chooses the call (sRGB8, terminal or texture).  With `async` (one context) both passes are issued on
+// `stream` (NULL: the context's) and aicb_render_finish finishes them; otherwise the call blocks as the host calls do,
+// behind the work queued on `stream` before it, and `stream` waits for the outputs.
+aicb_status layers_device(const LayeredCall &c, const double *depth_transform, const uint32_t *d_pixels, size_t n_pixels,
+                          const aicb_device_outputs *outs, cudaStream_t stream, bool async, aicb_render_info *info);
 
 // group.cu: one scene's world-only outputs over its replicas (aicb_render_* on one context, aicb_group_render_* and
 // aicb_group_trace_rays on a group).  The caller has validated the arguments and holds every context's lock.  A frame
@@ -479,14 +487,28 @@ struct WarpRange {
     size_t begin, count;
 };
 std::vector<WarpRange> warp_ranges(size_t n_items, size_t n_ctx);
+// aicb200.cu: the outputs of a device-output call (aicb_device_outputs) as a frame's target, validated before anything
+// is issued: the set of one host call of `call`'s kind (with need_colorbuf, a ColorBuf set must hold colorbuf, as on a
+// group), every pointer memory of `device` and aligned to its stores' width (check_device_pointer).
+enum DeviceCall { DEV_FRAME, DEV_RAYS, DEV_LAYERS };
+aicb_status device_target(const aicb_device_outputs *d, int device, DeviceCall call, bool need_colorbuf, bool peer_ok,
+                          Outputs *o);
+// aicb200.cu: a frame of no rays on `stream`, for aicb_render_finish to finish (an asynchronous call with nothing to
+// trace).
+aicb_status issue_empty_frame(aicb_scene *s, const aicb_options *opt, cudaStream_t stream);
+// A caller's device buffer: memory of `device`, or with peer_ok of a device it reaches as a peer, aligned to `align`
+// bytes (AICB_ERR_INVALID).
+aicb_status check_device_pointer(const void *p, int device, bool peer_ok, size_t align, const char *what);
 // A copy of device 0's outputs to the caller (none if bytes == 0).
 struct Delivery {
     void *to;
     const void *from;
     size_t bytes;
 };
-// Device 0's stream waits for the streams of the first n_parts contexts, then copies the outputs to the caller.
-aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies);
+// Device 0's stream waits for the streams of the first n_parts contexts, then copies the outputs to the caller; a
+// caller's stream (`caller`, device 0's; or NULL) waits for device 0's.
+aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies,
+                    cudaStream_t caller = nullptr);
 // aicb200.cu: GraphicsOptions as every frame call accepts them (AICB_ERR_INVALID otherwise).
 aicb_status validate_options(const aicb_options *o);
 

@@ -208,6 +208,25 @@ pub struct aicb_group_layer {
     pub options: *const aicb_options,
 }
 
+/// every output in the caller's device memory: nullable device pointers of the call's device (device 0 on a group)
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct aicb_device_outputs {
+    pub srgb8: *mut [u8; 4],
+    pub rgba16f: *mut [u16; 4],
+    pub colorbuf: *mut [f32; 4],
+    pub depth: *mut f64,
+    pub hit: *mut aicb_hit,
+    pub steps: *mut u32,
+    pub text: *mut i32,
+    pub texel_rgba16f: *mut [u16; 4],
+    pub texel_depth: *mut f32,
+    pub terminal: *mut aicb_terminal_pixel,
+    pub len: usize,
+    pub full_frame: u32,
+    pub _pad: u32,
+}
+
 unsafe extern "C" {
     pub fn aicb_abi_version() -> u32;
     pub fn aicb_ctx_create(device_id: c_int, out: *mut *mut aicb_ctx) -> aicb_status;
@@ -258,6 +277,15 @@ unsafe extern "C" {
                                           shard: *const aicb_shard, d_frame: *mut c_void, frame_len: usize,
                                           stream: *mut c_void) -> aicb_status;
     pub fn aicb_render_finish(s: *mut aicb_scene, info: *mut aicb_render_info) -> aicb_status;
+    // asynchronous, on `stream` (a cudaStream_t, NULL = the context's); aicb_render_finish completes them
+    pub fn aicb_render_device(s: *mut aicb_scene, cam: *const aicb_camera, opt: *const aicb_options, shard: *const aicb_shard,
+                              outs: *const aicb_device_outputs, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_trace_rays_device(s: *mut aicb_scene, d_origin_dir: *const [f64; 6], n: usize, opt: *const aicb_options,
+                                  outs: *const aicb_device_outputs, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_render_layers_device(world: *const aicb_layer, ui: *const aicb_layer, backdrop_rgba: *const [f32; 4],
+                                     no_world_rgba: *const [f32; 4], depth_transform: *const [f64; 16],
+                                     d_pixels: *const u32, n_pixels: usize, outs: *const aicb_device_outputs,
+                                     stream: *mut c_void) -> aicb_status;
     pub fn aicb_frame_create(ctx: *mut aicb_ctx, n_pixels: usize, d_frame: *mut *mut c_void, handle_out: *mut [u8; 64]) -> aicb_status;
     pub fn aicb_frame_open(ctx: *mut aicb_ctx, handle: *const [u8; 64], d_frame: *mut *mut c_void) -> aicb_status;
     pub fn aicb_frame_close(ctx: *mut aicb_ctx, d_frame: *mut c_void, opened: c_int) -> aicb_status;
@@ -269,6 +297,7 @@ unsafe extern "C" {
     pub fn aicb_frame_wait_consumed(ctx: *mut aicb_ctx, d_frame: *mut c_void, n_pixels: usize, frame_id: u32, stream: *mut c_void) -> aicb_status;
     pub fn aicb_frame_timed_out(ctx: *mut aicb_ctx, d_frame: *mut c_void, n_pixels: usize, out: *mut u32) -> aicb_status;
     pub fn aicb_ctx_stage_timing(ctx: *mut aicb_ctx, enable: c_int) -> aicb_status;
+    pub fn aicb_ctx_device(ctx: *const aicb_ctx) -> c_int;
 
     pub fn aicb_group_create(device_ids: *const c_int, n_devices: c_int, out: *mut *mut aicb_group) -> aicb_status;
     pub fn aicb_group_destroy(g: *mut aicb_group);
@@ -313,6 +342,18 @@ unsafe extern "C" {
     pub fn aicb_group_trace_rays(gs: *mut aicb_group_scene, origin_dir: *const [f64; 6], n: usize,
                                  opt: *const aicb_options, out_colorbuf: *mut [f32; 4], depth: *mut f64,
                                  hit: *mut aicb_hit, steps: *mut u32, info: *mut aicb_render_info) -> aicb_status;
+    // the device-output calls on a group: device-0 buffers, blocking; `stream` waits for the outputs
+    pub fn aicb_group_render_device(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
+                                    outs: *const aicb_device_outputs, stream: *mut c_void,
+                                    info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_trace_rays_device(gs: *mut aicb_group_scene, d_origin_dir: *const [f64; 6], n: usize,
+                                        opt: *const aicb_options, outs: *const aicb_device_outputs, stream: *mut c_void,
+                                        info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_layers_device(world: *const aicb_group_layer, ui: *const aicb_group_layer,
+                                           backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],
+                                           depth_transform: *const [f64; 16], d_pixels: *const u32, n_pixels: usize,
+                                           outs: *const aicb_device_outputs, stream: *mut c_void,
+                                           info: *mut aicb_render_info) -> aicb_status;
     pub fn aicb_group_render_text(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
                                   out: *mut i32, out_len: usize, info: *mut aicb_render_info) -> aicb_status;
     pub fn aicb_group_ortho_image_size(gs: *const aicb_group_scene, resolution: u32, width: *mut u32, height: *mut u32)

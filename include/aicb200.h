@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 17
+#define AICB_ABI_VERSION 18
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -192,6 +192,8 @@ aicb_status aicb_ctx_create(int device_id, aicb_ctx **out);
 void aicb_ctx_destroy(aicb_ctx *);
 /* aicb_render_info::stage_ms needs up to five event records per frame; on by default, off for callers that only want frames. */
 aicb_status aicb_ctx_stage_timing(aicb_ctx *, int enable);
+/* The CUDA device the context was created on (a device_id of -1 resolved to the device current then); -1 for NULL. */
+int aicb_ctx_device(const aicb_ctx *);
 /* Thread-local message for the last failing call on this thread. Never NULL. */
 const char *aicb_last_error(void);
 
@@ -390,6 +392,62 @@ aicb_status aicb_render_srgb8_device_frame(aicb_scene *, const aicb_camera *, co
                                            void *d_frame, size_t frame_len, void *stream);
 aicb_status aicb_render_finish(aicb_scene *, aicb_render_info *info_or_null);
 
+/* Every output in the caller's device memory: the outputs of a call are stored where these pointers say, by the
+ * kernels that compute them, and nothing is copied to the host.  Each pointer is NULL or device memory of the call's
+ * device (the scene's; device 0 on a group), checked with cudaPointerGetAttributes before anything is issued: host
+ * memory or another device's memory is AICB_ERR_INVALID.  Element types and layouts are the host calls':
+ *   world frames and ray batches: srgb8, rgba16f, colorbuf + depth + hit + steps, text;
+ *   layered frames: srgb8, terminal; texture targets: texel_rgba16f + texel_depth.
+ * A call accepts the outputs of one host call, and only those: {srgb8}, {rgba16f}, a non-empty subset of
+ * {colorbuf, depth, hit, steps} (the group calls need colorbuf, as aicb_group_render_colorbuf does), {text}; layered:
+ * {srgb8}, {terminal}, {texel_rgba16f and texel_depth}.  Any other combination, or a pointer the call cannot fill, is
+ * AICB_ERR_INVALID.  `len` is the host call's out_len (pixels, rays or listed pixels).  `full_frame` (aicb_render_device
+ * only, 0 elsewhere) has aicb_render_srgb8_device_frame's meaning: len = fb_width * fb_height and the shard's pixels are
+ * stored at their framebuffer positions. */
+typedef struct aicb_device_outputs {
+    uint8_t (*srgb8)[4];
+    uint16_t (*rgba16f)[4];
+    float (*colorbuf)[4];
+    double *depth;
+    aicb_hit *hit;
+    uint32_t *steps;
+    int32_t *text;
+    uint16_t (*texel_rgba16f)[4];
+    float *texel_depth;
+    aicb_terminal_pixel *terminal;
+    size_t len;
+    uint32_t full_frame;
+    uint32_t _pad;
+} aicb_device_outputs;
+
+/* Asynchronous calls on one context, issued on `stream` (a cudaStream_t of the scene's device; NULL = the context's
+ * stream), which nothing synchronises: aicb_render_finish on the scene completes the call (for a layered call, the
+ * world layer's scene, or the UI layer's without a world), fills info and returns AICB_ERR_RETRY after a hit-stream
+ * overflow, after which the caller issues the same call again.  The outputs are final once the stream has passed the
+ * call's work; the inputs (rays, pixel list) must stay valid until then.  A frame on a caller's stream waits for the
+ * context's previous frame and for the scene updates queued before it; the scene must not change again before the
+ * frame is finished.  A context tracks one frame: any render call on it (another asynchronous call, a host call, on
+ * any of its scenes) starts a new frame whose counters and overflow flag replace this one's, so aicb_render_finish
+ * would report that frame and could miss this one's overflow.  Finish each asynchronous call before the context's next
+ * render call.  Outputs, info and validation are those of the host calls, bit for bit.  Every pointer must be aligned
+ * to its elements' stores (16 bytes for colorbuf; 8 for rgba16f, depth, texel_rgba16f, terminal and the ray batch; 4
+ * for the others), AICB_ERR_INVALID otherwise.
+ *   aicb_render_device: the world-only frames of aicb_render_srgb8 / _rgba16f / _colorbuf / _text.
+ *   aicb_trace_rays_device: aicb_trace_rays with the batch read from device memory of the scene's device.
+ *   aicb_render_layers_device: aicb_render_layers_srgb8 (outs->srgb8), _terminal (outs->terminal) or _texture
+ *     (outs->texel_rgba16f and texel_depth, with depth_transform and the pixel list; n_pixels is 0 otherwise).  The UI
+ *     pass and the world pass are issued back to back; an overflow in either surfaces as AICB_ERR_RETRY.  The pixel list
+ *     is device memory of the scene's device and is read as it is: unlike the host call's, its indices are not checked
+ *     (an index >= fb_width * fb_height traces a ray outside the viewport into its own list position). */
+aicb_status aicb_render_device(aicb_scene *, const aicb_camera *, const aicb_options *, const aicb_shard *shard_or_null,
+                               const aicb_device_outputs *outs, void *stream);
+aicb_status aicb_trace_rays_device(aicb_scene *, const double (*d_origin_dir)[6], size_t n, const aicb_options *,
+                                   const aicb_device_outputs *outs, void *stream);
+aicb_status aicb_render_layers_device(const aicb_layer *world_or_null, const aicb_layer *ui_or_null,
+                                      const float backdrop_rgba[4], const float no_world_rgba[4],
+                                      const double depth_transform_or_null[16], const uint32_t *d_pixels_or_null,
+                                      size_t n_pixels, const aicb_device_outputs *outs, void *stream);
+
 /* Full-frame buffers shared between the ranks of one node (one process per GPU): the root creates
  * the frame on its GPU and publishes a 64-byte CUDA IPC handle; the other ranks open it on THEIR
  * device (peer access over NVLink is enabled lazily) and pass the mapped pointer to
@@ -518,6 +576,26 @@ aicb_status aicb_group_render_text(aicb_group_scene *, const aicb_camera *, cons
 aicb_status aicb_group_ortho_image_size(const aicb_group_scene *, uint32_t resolution, uint32_t *width, uint32_t *height);
 aicb_status aicb_group_render_orthographic(aicb_group_scene *, uint32_t resolution, uint8_t (*out)[4],
                                            size_t out_len, aicb_render_info *info_or_null);
+
+/* aicb_render_device, aicb_trace_rays_device and aicb_render_layers_device on the whole group: the group calls above
+ * with their cuts, validation and outputs, bit for bit, every device storing straight into the caller's device-0
+ * buffers (aicb_device_outputs), and no copy to the host.  The ray batch and the pixel list are device-0 memory, which
+ * every device reads over peer access.  Unlike the single-context calls these block, as the other group calls do: a
+ * device whose hit stream overflowed is re-issued alone, and the call returns once device 0's buffers are final, with
+ * info filled.  `stream` (a cudaStream_t of device 0, or NULL): every device's work starts after the work queued on it
+ * before the call (which may be writing the inputs), and it waits for the call's completion events, so work queued
+ * on it afterwards is ordered behind the outputs without the host.  A fully asynchronous group call is not offered. */
+aicb_status aicb_group_render_device(aicb_group_scene *, const aicb_camera *, const aicb_options *,
+                                     const aicb_device_outputs *outs, void *stream, aicb_render_info *info_or_null);
+aicb_status aicb_group_trace_rays_device(aicb_group_scene *, const double (*d_origin_dir)[6], size_t n,
+                                         const aicb_options *, const aicb_device_outputs *outs, void *stream,
+                                         aicb_render_info *info_or_null);
+aicb_status aicb_group_render_layers_device(const aicb_group_layer *world_or_null, const aicb_group_layer *ui_or_null,
+                                            const float backdrop_rgba[4], const float no_world_rgba[4],
+                                            const double depth_transform_or_null[16],
+                                            const uint32_t *d_pixels_or_null, size_t n_pixels,
+                                            const aicb_device_outputs *outs, void *stream,
+                                            aicb_render_info *info_or_null);
 
 /* == SpaceRaytracer::trace_ray (sr.rs:113-120) for a batch of explicit rays:
  * origin_dir[i] = {ox,oy,oz,dx,dy,dz}. Output as aicb_render_colorbuf. */
