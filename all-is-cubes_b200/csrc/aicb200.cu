@@ -247,7 +247,7 @@ static kernel_fn kernel_of() {
     return trace_kernel<V, W, AUX, B>;
 }
 
-// The marching kernel of a frame: Volumetric transparency, u32 cells, the step counters (AuxOutputs), u32 brick words.
+// The marching kernel of a frame: Volumetric transparency, u32 cells, the step counters (ColorBuf), u32 brick words.
 static kernel_fn select_kernel(bool volumetric, bool wide, bool aux, bool wide_bricks) {
 #define PICK(V, W, A, B) if (volumetric == V && wide == W && aux == A && wide_bricks == B) return kernel_of<V, W, A, B>();
     PICK(false, false, false, false) PICK(false, false, true, false) PICK(false, true, false, false)
@@ -899,15 +899,10 @@ aicb_status check_device_pointer(const void *p, int device, bool peer_ok, size_t
     return fail(AICB_ERR_INVALID, std::string(what) + " is memory of another device");
 }
 
-aicb_status device_target(const aicb_device_outputs *d, int device, DeviceCall call, bool need_colorbuf, bool peer_ok,
-                          Outputs *o) {
+aicb_status output_target(const aicb_device_outputs *d, DeviceCall call, bool need_colorbuf, Outputs *o) {
     if (!d) return fail(AICB_ERR_INVALID, "outs is NULL");
     const void *const ptr[10] = {d->srgb8, d->rgba16f, d->colorbuf, d->depth, d->hit,
                                  d->steps, d->text,    d->texel_rgba16f, d->texel_depth, d->terminal};
-    static const char *const name[10] = {"srgb8", "rgba16f", "colorbuf", "depth", "hit",
-                                         "steps", "text",    "texel_rgba16f", "texel_depth", "terminal"};
-    // the width of each output's stores (uchar4, uint2, float4, double, aicb_hit, u32, i32, uint2, float, 2 x float2)
-    static const size_t align[10] = {4, 8, 16, 8, 4, 4, 4, 8, 4, 8};
     unsigned set = 0;
     for (int i = 0; i < 10; i++)
         if (ptr[i]) set |= 1u << i;
@@ -924,8 +919,6 @@ aicb_status device_target(const aicb_device_outputs *d, int device, DeviceCall c
     if (set == 0 && d->len == 0) ok = true;
     if (!ok) return fail(AICB_ERR_INVALID, "the outputs are not a set that this call gives (aicb_device_outputs)");
     if (aux && need_colorbuf && d->len && !d->colorbuf) return fail(AICB_ERR_INVALID, "colorbuf is NULL");
-    for (int i = 0; i < 10; i++)
-        if (ptr[i]) TRY(check_device_pointer(ptr[i], device, peer_ok, align[i], name[i]));
     TargetParams &t = o->target;
     t.out_srgb8 = (uchar4 *)d->srgb8;
     t.out_text = d->text;
@@ -947,6 +940,20 @@ aicb_status device_target(const aicb_device_outputs *d, int device, DeviceCall c
         t.out_term = d->terminal;
         t.text_start = AICB_TEXT_EMPTY;
     }
+    return AICB_OK;
+}
+
+aicb_status device_target(const aicb_device_outputs *d, int device, DeviceCall call, bool need_colorbuf, bool peer_ok,
+                          Outputs *o) {
+    TRY(output_target(d, call, need_colorbuf, o));
+    const void *const ptr[10] = {d->srgb8, d->rgba16f, d->colorbuf, d->depth, d->hit,
+                                 d->steps, d->text,    d->texel_rgba16f, d->texel_depth, d->terminal};
+    static const char *const name[10] = {"srgb8", "rgba16f", "colorbuf", "depth", "hit",
+                                         "steps", "text",    "texel_rgba16f", "texel_depth", "terminal"};
+    // the width of each output's stores (uchar4, uint2, float4, double, aicb_hit, u32, i32, uint2, float, 2 x float2)
+    static const size_t align[10] = {4, 8, 16, 8, 4, 4, 4, 8, 4, 8};
+    for (int i = 0; i < 10; i++)
+        if (ptr[i]) TRY(check_device_pointer(ptr[i], device, peer_ok, align[i], name[i]));
     return AICB_OK;
 }
 
@@ -1872,31 +1879,8 @@ aicb_status aicb_render_srgb8(aicb_scene *s, const aicb_camera *cam, const aicb_
     aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
-    aicb_ctx *ctx = s->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    TRY(ctx->d_out.ensure(out_len * 4 + 16));
-    FramePart part{s, shard};
-    part.out.target.out_srgb8 = ctx->d_out.get<uchar4>();
-    // A pageable destination (a Rust Vec<[u8; 4]>, a numpy array) cannot take an asynchronous DMA: the frame goes to a
-    // pinned staging buffer of the library's and is copied out by the host.  Pinned / registered memory is written directly.
-    bool staged = false;
-    if (out_len) {
-        cudaPointerAttributes attr;
-        const cudaError_t pe = cudaPointerGetAttributes(&attr, out);
-        if (pe != cudaSuccess) cudaGetLastError();
-        staged = pe != cudaSuccess || attr.type == cudaMemoryTypeUnregistered;
-        if (staged) TRY(ctx->h_stage.ensure(out_len * 4));
-    }
-    // the copy is queued behind the frame: one host synchronisation per call
-    part.copy_to = staged ? ctx->h_stage.get() : (void *)out;
-    part.copy_from = ctx->d_out.get();
-    part.copy_bytes = out_len * 4;
-    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
-    if (st != AICB_OK) return st;
-    if (staged && out_len) std::memcpy(out, ctx->h_stage.get(), out_len * 4);
-    if (info) *info = part.info;
-    return AICB_OK;
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::srgb8, out, out_len);
+    return on_scene(s, [&](Replicas r) { return frame_host(r, cam, opt, shard, o, STAGE_PINNED, info); });
 }
 
 aicb_status aicb_render_rgba16f(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
@@ -1904,19 +1888,8 @@ aicb_status aicb_render_rgba16f(aicb_scene *s, const aicb_camera *cam, const aic
     aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
-    aicb_ctx *ctx = s->ctx;
-    std::lock_guard<std::mutex> lock(ctx->mu);
-    CU(cudaSetDevice(ctx->device));
-    TRY(ctx->d_out.ensure(out_len * 8 + 16));
-    FramePart part{s, shard};
-    part.out.target.out_rgba16f = ctx->d_out.get<uint2>();
-    part.copy_to = out;
-    part.copy_from = ctx->d_out.get();
-    part.copy_bytes = out_len * 8;
-    st = aicb_trace_pass(&part, 1, cam, opt, info != nullptr);
-    if (st != AICB_OK) return st;
-    if (info) *info = part.info;
-    return AICB_OK;
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::rgba16f, out, out_len);
+    return on_scene(s, [&](Replicas r) { return frame_host(r, cam, opt, shard, o, STAGE_GIVEN, info); });
 }
 
 aicb_status aicb_render_colorbuf(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
@@ -1924,9 +1897,8 @@ aicb_status aicb_render_colorbuf(aicb_scene *s, const aicb_camera *cam, const ai
                                  uint32_t *steps, size_t out_len, aicb_render_info *info) {
     aicb_status st = aicb_check_render_args(s, cam, opt, shard, out_len);
     if (st != AICB_OK) return st;
-    return on_scene(s, [&](Replicas r) {
-        return frame_colorbuf(r, cam, opt, shard, {out_cb, depth, hit, steps}, out_len, info);
-    });
+    const aicb_device_outputs o = colorbuf_outputs(out_cb, depth, hit, steps, out_len);
+    return on_scene(s, [&](Replicas r) { return frame_host(r, cam, opt, shard, o, STAGE_COLORBUF, info); });
 }
 
 aicb_status aicb_render_device(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
@@ -2123,7 +2095,8 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
     aicb_status st = aicb_check_render_args(s, cam, opt, nullptr, out_len);
     if (st != AICB_OK) return st;
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
-    return on_scene(s, [&](Replicas r) { return frame_text(r, cam, opt, out, out_len, info); });
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::text, out, out_len);
+    return on_scene(s, [&](Replicas r) { return frame_host(r, cam, opt, nullptr, o, STAGE_GIVEN, info); });
 }
 
 // Arguments shared by the layered entry points: at least one layer (or the paint colour), complete layers, one context
@@ -2167,21 +2140,24 @@ void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool sa
 // tracks one frame (finish), so its next pass waits until this one is finished.  finish decides whether a part's hit
 // stream overflowed and raises that context's capacity (x4 per retry, AICB_ERR_OOM at the cap); such a part is
 // re-issued alone.  With want_info, each finished pass is added to its part's info; without, finish skips its event
-// queries, as a caller that passes no aicb_render_info expects.  The caller holds the parts' contexts' locks.
+// queries, as a caller that passes no aicb_render_info expects.  Every round delivers `copies` (deliver): device 0
+// (parts[0]'s context) copies behind that round's parts, before the host waits for them, so a frame and its copy
+// cost one host synchronisation.  The caller holds the parts' contexts' locks.
 aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
-                            bool want_info) {
+                            bool want_info, const std::vector<Delivery> &copies) {
     std::vector<size_t> todo(n_parts), again;
     for (size_t i = 0; i < n_parts; i++) todo[i] = i;
     while (!todo.empty()) {
+        std::vector<aicb_ctx *> round = {parts[0].scene->ctx};   // device 0, then the other contexts of the round
         for (size_t i : todo) {
             const FramePart &p = parts[i];
             aicb_ctx *ctx = p.scene->ctx;
             CU(cudaSetDevice(ctx->device));
             aicb_status r = launch_trace(p.scene, cam, opt, p.shard, p.out, ctx->stream.get());
             if (r != AICB_OK) return r;
-            if (p.copy_bytes)
-                CU(cudaMemcpyAsync(p.copy_to, p.copy_from, p.copy_bytes, cudaMemcpyDeviceToHost, ctx->stream.get()));
+            if (i) round.push_back(ctx);
         }
+        if (!copies.empty()) TRY(deliver(round.data(), round.size(), copies));
         again.clear();
         for (size_t i : todo) {
             aicb_scene *sc = parts[i].scene;
@@ -2203,13 +2179,13 @@ aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera 
 // accumulator (its rays start opaque where the UI covered the pixel), and a pixel that is not opaque in the end — there
 // is no world — is painted NO_WORLD_TO_SHOW.  The last pass writes each part's target; with texture targets the UI pass
 // hands its DepthBuf on next to its ColorBuf, with terminal targets its CharacterBuf.  Each pass runs on every part
-// through aicb_trace_pass (a re-issued world pass starts from the same accumulator).  With `async` (one part), the
-// passes are issued back to back on that stream instead, the world pass continuing the UI pass's frame, and
-// aicb_render_finish on the last pass's scene finishes them (total is not filled).  The caller holds the parts'
-// contexts' locks.
+// through aicb_trace_pass (a re-issued world pass starts from the same accumulator), and the last pass delivers
+// `copies`.  With `async` (one part), the passes are issued back to back on that stream instead, the world pass
+// continuing the UI pass's frame, and aicb_render_finish on the last pass's scene finishes them (total is not filled).
+// The caller holds the parts' contexts' locks.
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
-                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total,
-                              cudaStream_t async) {
+                              const float *no_world_rgba, LayerPart *parts, size_t n_parts,
+                              const std::vector<Delivery> &copies, aicb_render_info *total, cudaStream_t async) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
     const aicb_layer *lead = have_world ? world : ui;
     aicb_status st = AICB_OK;
@@ -2243,18 +2219,18 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         std::memcpy(o.target.no_world, no_world, 16);
         o.target.has_no_world = 1;
     };
-    // one pass of the frame on every part: `layer` picks the part's scene, `outputs(part, ctx)` its Outputs; each
-    // part's info sums its passes
+    // one pass of the frame on every part: `layer` picks the part's scene, `outputs(part, ctx)` its Outputs, and the
+    // pass delivers `pass_copies`; each part's info sums its passes
     std::vector<FramePart> pass_parts(n_parts);
     bool first_pass = true;
     auto pass = [&](aicb_scene *LayerPart::*layer, const aicb_camera *cam, const aicb_options *opt,
-                    auto outputs) -> aicb_status {
+                    const std::vector<Delivery> &pass_copies, auto outputs) -> aicb_status {
         for (size_t i = 0; i < n_parts; i++) {
             pass_parts[i].scene = parts[i].*layer;
             pass_parts[i].shard = &parts[i].shard;
             pass_parts[i].out = outputs(parts[i], pass_parts[i].scene->ctx);
         }
-        if (!async) return aicb_trace_pass(pass_parts.data(), n_parts, cam, opt, true);
+        if (!async) return aicb_trace_pass(pass_parts.data(), n_parts, cam, opt, true, pass_copies);
         const FramePart &p = pass_parts[0];
         const bool continues = !first_pass;
         first_pass = false;
@@ -2274,7 +2250,7 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         }
         aicb_options ui_opt = *ui->options;
         ui_opt.include_sky = 0;   // ui.trace_ray(.., false)
-        st = pass(&LayerPart::ui, ui->camera, &ui_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
+        st = pass(&LayerPart::ui, ui->camera, &ui_opt, {}, [&](const LayerPart &p, aicb_ctx *ctx) {
             // the pass that writes no pixel keeps the task layout and the target kind only
             Outputs o;
             o.kind = p.out.kind;
@@ -2294,7 +2270,7 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
         if (st != AICB_OK) return st;
         aicb_options w_opt = *world->options;
         w_opt.include_sky = 1;    // world.trace_ray(.., true)
-        st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
+        st = pass(&LayerPart::world, world->camera, &w_opt, copies, [&](const LayerPart &p, aicb_ctx *ctx) {
             Outputs o = p.out;
             // a re-issued world pass starts from the same accumulator
             o.target.in_accum = ctx->d_task_aux.get<const float4>();
@@ -2322,7 +2298,7 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
                 CU(cudaGetLastError());
             }
         }
-        st = pass(&LayerPart::world, world->camera, &w_opt, [&](const LayerPart &p, aicb_ctx *ctx) {
+        st = pass(&LayerPart::world, world->camera, &w_opt, copies, [&](const LayerPart &p, aicb_ctx *ctx) {
             Outputs o = p.out;
             o.target.tex_layer = TEX_WORLD;
             if (have_backdrop) {
@@ -2335,7 +2311,7 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
     } else {
         aicb_options ui_opt = *ui->options;
         ui_opt.include_sky = 0;
-        st = pass(&LayerPart::ui, ui->camera, &ui_opt, [&](const LayerPart &p, aicb_ctx *) {
+        st = pass(&LayerPart::ui, ui->camera, &ui_opt, copies, [&](const LayerPart &p, aicb_ctx *) {
             Outputs o = p.out;
             o.target.tex_layer = TEX_UI;
             add_backdrop(o);
@@ -2574,7 +2550,7 @@ aicb_status ortho_srgb8(Replicas r, uint32_t resolution, uint8_t (*out)[4], size
         opt.maximum_intensity = INFINITY;
         opt.view_distance = 200.0;
         opt.include_sky = 1;
-        TRY(aicb_trace_pass(parts.data(), parts.size(), nullptr, &opt, info != nullptr));
+        TRY(aicb_trace_pass(parts.data(), parts.size(), nullptr, &opt, info != nullptr, {}));
         TRY(fan_in(r.ctx, parts.size()));
         ortho_place_kernel<<<(unsigned)((n + 255) / 256), 256, 0, root->stream.get()>>>(V, traced, n, image);
         CU(cudaGetLastError());
@@ -2604,7 +2580,8 @@ aicb_status aicb_trace_rays(aicb_scene *s, const double (*origin_dir)[6], size_t
     if (!s || (n && !origin_dir)) return fail(AICB_ERR_INVALID, "NULL argument");
     aicb_status st = validate_options(opt);
     if (st != AICB_OK) return st;
-    return on_scene(s, [&](Replicas r) { return rays_colorbuf(r, origin_dir, n, opt, {out_cb, depth, hit, steps}, info); });
+    const aicb_device_outputs o = colorbuf_outputs(out_cb, depth, hit, steps, n);
+    return on_scene(s, [&](Replicas r) { return rays_host(r, origin_dir, opt, o, info); });
 }
 
 }

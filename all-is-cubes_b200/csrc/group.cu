@@ -10,6 +10,8 @@
 // aicb_render_layers_* on one context and aicb_group_render_layers_* on a group) cut the work the same way, or a pixel
 // list into ranges of whole warps, and hand the parts to aicb_trace_layers (aicb200.cu).  Every call issues a pass on
 // every device before it waits for any, and re-issues it on a device whose hit stream overflowed (aicb_trace_pass).
+// A host call draws as its blocking device-output twin does, into regions of device 0's staging buffer that stand for
+// the caller's pointers (stage_outputs); the last pass copies them to the caller (deliver).
 // Light propagation (aicb_group_light_*) hands the replicas to light.cu, which runs one context's rounds over them.
 #include <algorithm>
 #include <cstring>
@@ -109,16 +111,14 @@ std::vector<WarpRange> warp_ranges(size_t n_items, size_t n_ctx) {
     return ranges;
 }
 
-aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies, cudaStream_t caller) {
-    TRY(fan_in(ctx, n_parts));
+aicb_status deliver(aicb_ctx *const *ctx, size_t n, const std::vector<Delivery> &copies) {
+    TRY(fan_in(ctx, n));
     cudaStream_t stream = ctx[0]->stream.get();
     for (const Delivery &d : copies)
         if (d.bytes) CU(cudaMemcpyAsync(d.to, d.from, d.bytes, cudaMemcpyDeviceToHost, stream));
-    if (caller) {
-        CU(cudaEventRecord(ctx[0]->ev_join.get(), stream));
-        CU(cudaStreamWaitEvent(caller, ctx[0]->ev_join.get(), 0));
-    }
     CU(cudaStreamSynchronize(stream));
+    for (const Delivery &d : copies)
+        if (d.then && d.bytes) std::memcpy(d.then, d.to, d.bytes);
     return AICB_OK;
 }
 
@@ -135,6 +135,68 @@ static aicb_status after_caller(aicb_ctx *const *ctx, size_t n, cudaStream_t cal
     return AICB_OK;
 }
 
+// The caller's stream (device 0's; none if NULL) waits for the call's work on the first n listed contexts.
+static aicb_status before_caller(aicb_ctx *const *ctx, size_t n, cudaStream_t caller) {
+    if (!caller) return AICB_OK;
+    TRY(fan_in(ctx, n));
+    CU(cudaEventRecord(ctx[0]->ev_join.get(), ctx[0]->stream.get()));
+    CU(cudaStreamWaitEvent(caller, ctx[0]->ev_join.get(), 0));
+    return AICB_OK;
+}
+
+// A host call's outputs (`how`) each in a region of device 0's d_out at a 256-byte aligned offset, mapped to a frame's
+// target as a device call's are (output_target); `copies` takes the regions to the caller's non-NULL pointers.
+static aicb_status stage_outputs(aicb_ctx *root, const aicb_device_outputs &host, Staging how, DeviceCall call,
+                                 Outputs *target, std::vector<Delivery> *copies) {
+    const size_t n = host.len;
+    aicb_device_outputs staged{};
+    staged.len = n;
+    size_t bytes = 0;
+    char *base = nullptr;
+    // one output's region: counted on the first walk over the outputs, placed and listed on the second (base set)
+    auto take = [&](auto *given, auto *&region, size_t size, bool stored = false) {
+        if (!given && !stored) return;
+        if (base) {
+            region = (std::remove_reference_t<decltype(region)>)(base + bytes);
+            if (given) copies->push_back({given, region, n * size});
+        }
+        bytes += (n * size + 255) & ~(size_t)255;
+    };
+    auto walk = [&] {
+        take(host.srgb8, staged.srgb8, 4);
+        take(host.rgba16f, staged.rgba16f, 8);
+        take(host.colorbuf, staged.colorbuf, 16, how == STAGE_COLORBUF);
+        take(host.depth, staged.depth, 8);
+        take(host.hit, staged.hit, sizeof(aicb_hit));
+        take(host.steps, staged.steps, 4);
+        take(host.text, staged.text, 4);
+        take(host.texel_rgba16f, staged.texel_rgba16f, 8);
+        take(host.texel_depth, staged.texel_depth, 4);
+        take(host.terminal, staged.terminal, sizeof(aicb_terminal_pixel));
+    };
+    walk();
+    CU(cudaSetDevice(root->device));
+    TRY(root->d_out.ensure(bytes + 16));
+    base = root->d_out.get<char>();
+    bytes = 0;
+    walk();
+    // A pageable destination (a Rust Vec<[u8; 4]>, a numpy array) cannot take an asynchronous DMA: the frame goes to a
+    // pinned staging buffer of the library's and is copied out by the host.  Pinned / registered memory is written
+    // directly.
+    if (how == STAGE_PINNED && n) {
+        cudaPointerAttributes attr;
+        const cudaError_t pe = cudaPointerGetAttributes(&attr, host.srgb8);
+        if (pe != cudaSuccess) cudaGetLastError();
+        if (pe != cudaSuccess || attr.type == cudaMemoryTypeUnregistered) {
+            TRY(root->h_stage.ensure(n * 4));
+            Delivery &d = copies->front();
+            d.then = d.to;
+            d.to = root->h_stage.get();
+        }
+    }
+    return output_target(&staged, call, false, target);
+}
+
 // The contexts of a validated layered call: those of its lead layer's replicas.
 static std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *lead) {
     aicb_scene *const *scenes = lead == c.world ? c.world_scenes : c.ui_scenes;
@@ -143,49 +205,48 @@ static std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *
     return ctx;
 }
 
-// The rest of a layered call once device 0's outputs are in `target`: the parts, the layers, the delivery.
+// The rest of a layered call once device 0's outputs are in `target`: the parts, the layers and the delivery of
+// `copies`, then the caller's stream.
 static aicb_status draw_layers(const LayeredCall &c, const std::vector<aicb_ctx *> &ctx, const Outputs &target,
                                const uint32_t *pixels, bool pixels_on_device, size_t n_pixels,
                                const std::vector<Delivery> &copies, cudaStream_t caller, aicb_render_info *info) {
     std::vector<LayerPart> parts;
     TRY(layer_parts(c, ctx.data(), target, pixels, pixels_on_device, n_pixels, &parts));
     aicb_render_info total;
-    TRY(aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), &total,
+    TRY(aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), copies, &total,
                           nullptr));
-    TRY(deliver(ctx.data(), parts.size(), copies, caller));
+    TRY(before_caller(ctx.data(), parts.size(), caller));
     if (info) *info = total;
     return AICB_OK;
+}
+
+// A validated layered host call: its outputs staged in device 0's d_out.
+static aicb_status layers_host(const LayeredCall &c, const aicb_layer *lead, const double *depth_transform,
+                               const uint32_t *pixels, const aicb_device_outputs &host, aicb_render_info *info) {
+    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
+    ContextLocks lock(ctx);
+    Outputs target;
+    std::vector<Delivery> copies;
+    TRY(stage_outputs(ctx[0], host, STAGE_GIVEN, DEV_LAYERS, &target, &copies));
+    if (target.kind == aicb::TGT_TEX) aicb_texture_target(c.world, c.ui, depth_transform, &target);
+    target.full_frame = true;
+    return draw_layers(c, ctx, target, pixels, false, host.len, copies, nullptr, info);
 }
 
 aicb_status layers_srgb8(const LayeredCall &c, uint8_t (*out)[4], size_t out_len, aicb_render_info *info) {
     const aicb_layer *lead = nullptr;
     TRY(aicb_check_layers(c.world, c.ui, c.no_world_rgba, out_len, &lead));
     if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
-    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
-    ContextLocks lock(ctx);
-    CU(cudaSetDevice(ctx[0]->device));
-    TRY(ctx[0]->d_out.ensure(out_len * 4 + 16));
-    Outputs target;
-    target.full_frame = true;
-    target.target.out_srgb8 = ctx[0]->d_out.get<uchar4>();
-    return draw_layers(c, ctx, target, nullptr, false, 0, {{out, ctx[0]->d_out.get(), out_len * 4}}, nullptr, info);
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::srgb8, out, out_len);
+    return layers_host(c, lead, nullptr, nullptr, o, info);
 }
 
 aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info) {
     const aicb_layer *lead = nullptr;
     TRY(aicb_check_layers(c.world, c.ui, c.no_world_rgba, out_len, &lead));
     if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
-    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
-    ContextLocks lock(ctx);
-    CU(cudaSetDevice(ctx[0]->device));
-    const size_t bytes = out_len * sizeof(aicb_terminal_pixel);
-    TRY(ctx[0]->d_out.ensure(bytes + 16));
-    Outputs target;
-    target.full_frame = true;
-    target.kind = aicb::TGT_TERM;
-    target.target.out_term = ctx[0]->d_out.get<aicb_terminal_pixel>();
-    target.target.text_start = AICB_TEXT_EMPTY;
-    return draw_layers(c, ctx, target, nullptr, false, 0, {{out, ctx[0]->d_out.get(), bytes}}, nullptr, info);
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::terminal, out, out_len);
+    return layers_host(c, lead, nullptr, nullptr, o, info);
 }
 
 aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,
@@ -195,19 +256,11 @@ aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, 
                                   out_depth, &lead));
     if (info) std::memset(info, 0, sizeof *info);
     if (n_pixels == 0) return AICB_OK;
-    const std::vector<aicb_ctx *> ctx = contexts(c, lead);
-    ContextLocks lock(ctx);
-    CU(cudaSetDevice(ctx[0]->device));
-    // device 0's d_out: colour texels (8 B), then depth texels (4 B), 256-byte aligned
-    const size_t off_depth = (n_pixels * 8 + 255) & ~(size_t)255;
-    TRY(ctx[0]->d_out.ensure(off_depth + n_pixels * 4 + 16));
-    char *base = ctx[0]->d_out.get<char>();
-    Outputs target;
-    aicb_texture_target(c.world, c.ui, depth_transform, &target);
-    target.target.out_rgba16f = (uint2 *)base;
-    target.target.out_tex_depth = (float *)(base + off_depth);
-    return draw_layers(c, ctx, target, pixels, false, n_pixels,
-                       {{out_rgba16f, base, n_pixels * 8}, {out_depth, base + off_depth, n_pixels * 4}}, nullptr, info);
+    aicb_device_outputs o{};
+    o.texel_rgba16f = out_rgba16f;
+    o.texel_depth = out_depth;
+    o.len = n_pixels;
+    return layers_host(c, lead, depth_transform, pixels, o, info);
 }
 
 aicb_status layers_device(const LayeredCall &c, const double *depth_transform, const uint32_t *d_pixels, size_t n_pixels,
@@ -238,8 +291,8 @@ aicb_status layers_device(const LayeredCall &c, const double *depth_transform, c
         if (texels && n_pixels == 0) return issue_empty_frame(lead->scene, lead->options, stream);
         std::vector<LayerPart> parts;
         TRY(layer_parts(c, ctx.data(), target, d_pixels, true, n_pixels, &parts));
-        return aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), nullptr,
-                                 stream);
+        return aicb_trace_layers(c.world, c.ui, c.backdrop_rgba, c.no_world_rgba, parts.data(), parts.size(), {},
+                                 nullptr, stream);
     }
     if (texels && n_pixels == 0) return AICB_OK;
     TRY(after_caller(ctx.data(), c.n, stream));
@@ -256,8 +309,8 @@ static void sum_info(const std::vector<FramePart> &parts, aicb_render_info *info
 
 // A frame of the replicas' scene with the caller's options as given: interleaved 16-row strips as
 // aicb_group_render_srgb8 cuts them, each part storing at framebuffer positions in device 0's outputs (`target`); with
-// `shard` (one context), that shard's rows, packed.  Then the delivery of device 0's outputs; a caller's stream
-// (`caller`, or NULL) goes first and waits for them.
+// `shard` (one context), that shard's rows, packed.  A caller's stream (`caller`, or NULL) goes first, the delivery of
+// `copies` follows the frame, and then the caller's stream waits for it.
 static aicb_status draw_frame(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
                               Outputs target, const std::vector<Delivery> &copies, cudaStream_t caller,
                               aicb_render_info *info) {
@@ -273,67 +326,18 @@ static aicb_status draw_frame(Replicas r, const aicb_camera *cam, const aicb_opt
         for (const LayerPart &p : strips) parts.push_back({p.world, &p.shard, p.out});
     }
     TRY(after_caller(r.ctx, parts.size(), caller));
-    TRY(aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr));
-    TRY(deliver(r.ctx, parts.size(), copies, caller));
+    TRY(aicb_trace_pass(parts.data(), parts.size(), cam, opt, info != nullptr, copies));
+    TRY(before_caller(r.ctx, parts.size(), caller));
     sum_info(parts, info);
     return AICB_OK;
 }
 
-// draw::<ColorBuf> and its companions' outputs for n pixels or rays in device 0's d_out: colorbuf, then the wanted
-// ones of depth, hit and steps; an output the caller does not want is neither allocated, stored nor copied.
-static aicb_status aux_target(aicb_ctx *root, size_t n, const AuxOutputs &want, Outputs *o) {
-    size_t bytes = n * 16;
-    auto take = [&](bool wanted, size_t size) -> size_t {
-        const size_t off = bytes;
-        if (wanted) bytes += n * size;
-        return off;
-    };
-    const size_t off_depth = take(want.depth, 8), off_hit = take(want.hit, sizeof(aicb_hit));
-    const size_t off_steps = take(want.steps, 4);
-    CU(cudaSetDevice(root->device));
-    TRY(root->d_out.ensure(bytes + 16));
-    char *base = root->d_out.get<char>();
-    o->aux = true;
-    o->target.out_colorbuf = (float4 *)base;
-    o->target.out_depth = want.depth ? (double *)(base + off_depth) : nullptr;
-    o->target.out_hit = want.hit ? (aicb_hit *)(base + off_hit) : nullptr;
-    o->target.out_steps = want.steps ? (uint32_t *)(base + off_steps) : nullptr;
-    return AICB_OK;
-}
-
-static std::vector<Delivery> aux_copies(const Outputs &o, const AuxOutputs &want, size_t n) {
-    const aicb::TargetParams &t = o.target;
-    return {{want.colorbuf, t.out_colorbuf, want.colorbuf ? n * 16 : 0},
-            {want.depth, t.out_depth, want.depth ? n * 8 : 0},
-            {want.hit, t.out_hit, want.hit ? n * sizeof(aicb_hit) : 0},
-            {want.steps, t.out_steps, want.steps ? n * 4 : 0}};
-}
-
-aicb_status frame_colorbuf(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
-                           AuxOutputs out, size_t out_len, aicb_render_info *info) {
+aicb_status frame_host(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
+                       const aicb_device_outputs &host, Staging how, aicb_render_info *info) {
     Outputs target;
-    TRY(aux_target(r.ctx[0], out_len, out, &target));
-    return draw_frame(r, cam, opt, shard, target, aux_copies(target, out, out_len), nullptr, info);
-}
-
-aicb_status frame_rgba16f(Replicas r, const aicb_camera *cam, const aicb_options *opt, uint16_t (*out)[4],
-                          size_t out_len, aicb_render_info *info) {
-    aicb_ctx *root = r.ctx[0];
-    CU(cudaSetDevice(root->device));
-    TRY(root->d_out.ensure(out_len * 8 + 16));
-    Outputs target;
-    target.target.out_rgba16f = root->d_out.get<uint2>();
-    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 8}}, nullptr, info);
-}
-
-aicb_status frame_text(Replicas r, const aicb_camera *cam, const aicb_options *opt, int32_t *out, size_t out_len,
-                       aicb_render_info *info) {
-    aicb_ctx *root = r.ctx[0];
-    CU(cudaSetDevice(root->device));
-    TRY(root->d_out.ensure(out_len * 4 + 16));
-    Outputs target;
-    target.target.out_text = root->d_out.get<int32_t>();
-    return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), out_len * 4}}, nullptr, info);
+    std::vector<Delivery> copies;
+    TRY(stage_outputs(r.ctx[0], host, how, DEV_FRAME, &target, &copies));
+    return draw_frame(r, cam, opt, shard, target, copies, nullptr, info);
 }
 
 // Context i uploads its range of the batch to its own d_aux (or with rays_on_device reads it in place from device 0's
@@ -365,18 +369,19 @@ static aicb_status draw_rays(Replicas r, const double (*origin_dir)[6], bool ray
         p.out.n_rays = count;
         parts.push_back(p);
     }
-    TRY(aicb_trace_pass(parts.data(), parts.size(), nullptr, opt, info != nullptr));
-    TRY(deliver(r.ctx, parts.size(), copies, caller));
+    TRY(aicb_trace_pass(parts.data(), parts.size(), nullptr, opt, info != nullptr, copies));
+    TRY(before_caller(r.ctx, parts.size(), caller));
     sum_info(parts, info);
     return AICB_OK;
 }
 
-aicb_status rays_colorbuf(Replicas r, const double (*origin_dir)[6], size_t n, const aicb_options *opt, AuxOutputs out,
-                          aicb_render_info *info) {
-    if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "too many rays");
+aicb_status rays_host(Replicas r, const double (*origin_dir)[6], const aicb_options *opt,
+                      const aicb_device_outputs &host, aicb_render_info *info) {
+    if (host.len > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "too many rays");
     Outputs target;
-    TRY(aux_target(r.ctx[0], n, out, &target));
-    return draw_rays(r, origin_dir, false, n, opt, target, aux_copies(target, out, n), nullptr, info);
+    std::vector<Delivery> copies;
+    TRY(stage_outputs(r.ctx[0], host, STAGE_COLORBUF, DEV_RAYS, &target, &copies));
+    return draw_rays(r, origin_dir, false, host.len, opt, target, copies, nullptr, info);
 }
 
 // The layers of a group call as device 0 sees them (its replicas, the cameras and options), and every replica of each.
@@ -512,15 +517,9 @@ aicb_status aicb_group_render_srgb8(aicb_group_scene *gs, const aicb_camera *cam
     if (pixels && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
     aicb_status st = aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len);
     if (st != AICB_OK) return st;
-    return on_group(gs, false, [&](Replicas r) {
-        aicb_ctx *root = r.ctx[0];
-        CU(cudaSetDevice(root->device));
-        TRY(root->d_out.ensure(pixels * 4 + 16));
-        Outputs target;
-        target.target.out_srgb8 = root->d_out.get<uchar4>();
-        // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
-        return draw_frame(r, cam, opt, nullptr, target, {{out, root->d_out.get(), pixels * 4}}, nullptr, info);
-    });
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::srgb8, out, out_len);
+    // the caller's options as given (a world-only frame of aicb_trace_layers would force include_sky)
+    return on_group(gs, false, [&](Replicas r) { return frame_host(r, cam, opt, nullptr, o, STAGE_GIVEN, info); });
 }
 
 // The world-only outputs of one context on the group, with the single-context calls' validation against replica 0.
@@ -530,9 +529,8 @@ aicb_status aicb_group_render_colorbuf(aicb_group_scene *gs, const aicb_camera *
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     TRY(aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len));
     if (out_len && !out_colorbuf) return aicb_fail(AICB_ERR_INVALID, "out_colorbuf is NULL");
-    return on_group(gs, false, [&](Replicas r) {
-        return frame_colorbuf(r, cam, opt, nullptr, {out_colorbuf, depth, hit, steps}, out_len, info);
-    });
+    const aicb_device_outputs o = colorbuf_outputs(out_colorbuf, depth, hit, steps, out_len);
+    return on_group(gs, false, [&](Replicas r) { return frame_host(r, cam, opt, nullptr, o, STAGE_COLORBUF, info); });
 }
 
 aicb_status aicb_group_render_rgba16f(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt,
@@ -540,7 +538,8 @@ aicb_status aicb_group_render_rgba16f(aicb_group_scene *gs, const aicb_camera *c
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     TRY(aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len));
     if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
-    return on_group(gs, false, [&](Replicas r) { return frame_rgba16f(r, cam, opt, out, out_len, info); });
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::rgba16f, out, out_len);
+    return on_group(gs, false, [&](Replicas r) { return frame_host(r, cam, opt, nullptr, o, STAGE_GIVEN, info); });
 }
 
 aicb_status aicb_group_trace_rays(aicb_group_scene *gs, const double (*origin_dir)[6], size_t n, const aicb_options *opt,
@@ -549,9 +548,8 @@ aicb_status aicb_group_trace_rays(aicb_group_scene *gs, const double (*origin_di
     if (!gs || (n && !origin_dir)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     TRY(validate_options(opt));
     if (n && !out_colorbuf) return aicb_fail(AICB_ERR_INVALID, "out_colorbuf is NULL");
-    return on_group(gs, false, [&](Replicas r) {
-        return rays_colorbuf(r, origin_dir, n, opt, {out_colorbuf, depth, hit, steps}, info);
-    });
+    const aicb_device_outputs o = colorbuf_outputs(out_colorbuf, depth, hit, steps, n);
+    return on_group(gs, false, [&](Replicas r) { return rays_host(r, origin_dir, opt, o, info); });
 }
 
 aicb_status aicb_group_render_text(aicb_group_scene *gs, const aicb_camera *cam, const aicb_options *opt, int32_t *out,
@@ -559,7 +557,8 @@ aicb_status aicb_group_render_text(aicb_group_scene *gs, const aicb_camera *cam,
     if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
     TRY(aicb_check_render_args(gs->scene[0], cam, opt, nullptr, out_len));
     if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
-    return on_group(gs, false, [&](Replicas r) { return frame_text(r, cam, opt, out, out_len, info); });
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::text, out, out_len);
+    return on_group(gs, false, [&](Replicas r) { return frame_host(r, cam, opt, nullptr, o, STAGE_GIVEN, info); });
 }
 
 aicb_status aicb_group_ortho_image_size(const aicb_group_scene *gs, uint32_t resolution, uint32_t *width,

@@ -307,7 +307,7 @@ struct Outputs {
     aicb::TargetParams target{};
     int kind = aicb::TGT_FRAME;         // the compositing kernels' target: TGT_FRAME, TGT_TEX or TGT_TERM
     bool full_frame = false;            // outputs at framebuffer positions (TraceParams::out_full_frame)
-    bool aux = false;                   // the marching kernel that also counts steps and blocks (AuxOutputs)
+    bool aux = false;                   // the marching kernel that also counts steps and blocks (a ColorBuf set)
     const double *rays = nullptr;       // device: the tasks of a frame without a camera (origin, direction per ray)
     uint64_t n_rays = 0;
     int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
@@ -323,22 +323,28 @@ struct LayerPart {
 };
 
 // One context's share of one pass of a frame (aicb_trace_pass): the scene it traces, its row strips, where it stores,
-// a device-to-host copy queued behind every issue (if copy_bytes), and its finished passes' info, summed.
+// and its finished passes' info, summed.
 struct FramePart {
     aicb_scene *scene = nullptr;
     const aicb_shard *shard = nullptr;   // nullptr: every row
     Outputs out;
-    void *copy_to = nullptr;
-    const void *copy_from = nullptr;
-    size_t copy_bytes = 0;
     aicb_render_info info{};
+};
+
+// A copy of device 0's outputs to the caller (none if bytes == 0).  With `then`, `to` is the context's pinned staging
+// (aicb_ctx::h_stage) and the host copies it on to `then` once the device's copy is done.
+struct Delivery {
+    void *to;
+    const void *from;
+    size_t bytes;
+    void *then = nullptr;
 };
 
 // aicb200.cu: the layer rules of the layered calls.  The layers give the cameras and options (their scenes only say
 // which layers exist).  Validation of their arguments; the texture target's exposures and depth transform; the passes
-// of a frame over every part, and the one loop that re-issues a pass whose hit stream overflowed (aicb_trace_pass); the
-// one merge of aicb_render_info.  The passes need the locks of the parts' contexts.  (C linkage: aicb200.cu defines
-// them among the entry points of the C ABI.)
+// of a frame over every part, and the one loop that re-issues a pass whose hit stream overflowed and delivers its
+// outputs (aicb_trace_pass); the one merge of aicb_render_info.  The passes need the locks of the parts' contexts.
+// (C linkage: aicb200.cu defines them among the entry points of the C ABI.)
 extern "C" {
 aicb_status aicb_check_render_args(aicb_scene *s, const aicb_camera *cam, const aicb_options *opt,
                                    const aicb_shard *shard, size_t out_len);
@@ -350,10 +356,10 @@ aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer 
                                       const aicb_layer **lead_out);
 void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out);
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
-                              const float *no_world_rgba, LayerPart *parts, size_t n_parts, aicb_render_info *total,
-                              cudaStream_t async);
+                              const float *no_world_rgba, LayerPart *parts, size_t n_parts,
+                              const std::vector<Delivery> &copies, aicb_render_info *total, cudaStream_t async);
 aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera *cam, const aicb_options *opt,
-                            bool want_info);
+                            bool want_info, const std::vector<Delivery> &copies);
 void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part);
 }
 
@@ -439,9 +445,10 @@ aicb_status fan_out(aicb_ctx *const *ctx, size_t n);
 aicb_status fan_in(aicb_ctx *const *ctx, size_t n);
 
 // group.cu: the layered calls (aicb_render_layers_* and aicb_group_render_layers_*), which validate, lock, trace the
-// layers over one part per context (aicb_trace_layers), collect the parts' outputs on device 0, copy them to the caller
-// and fill info.  `world` and `ui` are the layers as device 0 sees them; world_scenes / ui_scenes each layer's replica
-// on every one of the n contexts (nullptr for an absent layer).
+// layers over one part per context (aicb_trace_layers), collect the parts' outputs on device 0 (a host call's in its
+// staging buffer, as the world-only host calls below do), copy them to the caller and fill info.  `world` and `ui`
+// are the layers as device 0 sees them; world_scenes / ui_scenes each layer's replica on every one of the n contexts
+// (nullptr for an absent layer).
 struct LayeredCall {
     const aicb_layer *world, *ui;
     aicb_scene *const *world_scenes, *const *ui_scenes;
@@ -462,22 +469,35 @@ aicb_status layers_device(const LayeredCall &c, const double *depth_transform, c
 // group.cu: one scene's world-only outputs over its replicas (aicb_render_* on one context, aicb_group_render_* and
 // aicb_group_trace_rays on a group).  The caller has validated the arguments and holds every context's lock.  A frame
 // is cut into interleaved 16-row strips (with `shard`, one context only: that shard's rows, packed); a ray batch into
-// contiguous ranges of whole warps (warp_ranges).  Every part stores into device 0's buffers, and device 0 copies the
-// outputs the caller asked for (non-null pointers) to the caller.
-struct AuxOutputs {
-    float (*colorbuf)[4];
-    double *depth;
-    aicb_hit *hit;
-    uint32_t *steps;
-};
-aicb_status frame_colorbuf(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
-                           AuxOutputs out, size_t out_len, aicb_render_info *info);
-aicb_status frame_rgba16f(Replicas r, const aicb_camera *cam, const aicb_options *opt, uint16_t (*out)[4],
-                          size_t out_len, aicb_render_info *info);
-aicb_status frame_text(Replicas r, const aicb_camera *cam, const aicb_options *opt, int32_t *out, size_t out_len,
-                       aicb_render_info *info);
-aicb_status rays_colorbuf(Replicas r, const double (*origin_dir)[6], size_t n, const aicb_options *opt, AuxOutputs out,
-                          aicb_render_info *info);
+// contiguous ranges of whole warps (warp_ranges).  Every part stores into device 0's buffers.
+//
+// A host call draws as a blocking device call does, its outputs (aicb_device_outputs of the caller's host pointers)
+// staged in device 0's d_out and copied to the caller (stage_outputs).  `how`: the outputs given; a ColorBuf set, whose
+// colorbuf is stored whether or not the caller wants it; an sRGB8 frame that takes a pageable destination through
+// the context's pinned staging (the one-context aicb_render_srgb8 only).
+enum Staging { STAGE_GIVEN, STAGE_COLORBUF, STAGE_PINNED };
+aicb_status frame_host(Replicas r, const aicb_camera *cam, const aicb_options *opt, const aicb_shard *shard,
+                       const aicb_device_outputs &host, Staging how, aicb_render_info *info);
+aicb_status rays_host(Replicas r, const double (*origin_dir)[6], const aicb_options *opt,
+                      const aicb_device_outputs &host, aicb_render_info *info);
+// The outputs of a host call of one output (`field`, at `p`) or of the ColorBuf set, n elements each.
+template <typename T>
+aicb_device_outputs one_output(T aicb_device_outputs::*field, T p, size_t n) {
+    aicb_device_outputs o{};
+    o.*field = p;
+    o.len = n;
+    return o;
+}
+inline aicb_device_outputs colorbuf_outputs(float (*colorbuf)[4], double *depth, aicb_hit *hit, uint32_t *steps,
+                                            size_t n) {
+    aicb_device_outputs o{};
+    o.colorbuf = colorbuf;
+    o.depth = depth;
+    o.hit = hit;
+    o.steps = steps;
+    o.len = n;
+    return o;
+}
 // aicb200.cu: render_orthographic over the replicas, validated against replica 0 (the caller holds the locks).
 aicb_status ortho_srgb8(Replicas r, uint32_t resolution, uint8_t (*out)[4], size_t out_len, aicb_render_info *info);
 
@@ -489,8 +509,10 @@ struct WarpRange {
 std::vector<WarpRange> warp_ranges(size_t n_items, size_t n_ctx);
 // aicb200.cu: the outputs of a device-output call (aicb_device_outputs) as a frame's target, validated before anything
 // is issued: the set of one host call of `call`'s kind (with need_colorbuf, a ColorBuf set must hold colorbuf, as on a
-// group), every pointer memory of `device` and aligned to its stores' width (check_device_pointer).
+// group; output_target), and for a caller's pointers (device_target) every pointer memory of `device` and aligned to
+// its stores' width (check_device_pointer).
 enum DeviceCall { DEV_FRAME, DEV_RAYS, DEV_LAYERS };
+aicb_status output_target(const aicb_device_outputs *d, DeviceCall call, bool need_colorbuf, Outputs *o);
 aicb_status device_target(const aicb_device_outputs *d, int device, DeviceCall call, bool need_colorbuf, bool peer_ok,
                           Outputs *o);
 // aicb200.cu: a frame of no rays on `stream`, for aicb_render_finish to finish (an asynchronous call with nothing to
@@ -499,16 +521,9 @@ aicb_status issue_empty_frame(aicb_scene *s, const aicb_options *opt, cudaStream
 // A caller's device buffer: memory of `device`, or with peer_ok of a device it reaches as a peer, aligned to `align`
 // bytes (AICB_ERR_INVALID).
 aicb_status check_device_pointer(const void *p, int device, bool peer_ok, size_t align, const char *what);
-// A copy of device 0's outputs to the caller (none if bytes == 0).
-struct Delivery {
-    void *to;
-    const void *from;
-    size_t bytes;
-};
-// Device 0's stream waits for the streams of the first n_parts contexts, then copies the outputs to the caller; a
-// caller's stream (`caller`, device 0's; or NULL) waits for device 0's.
-aicb_status deliver(aicb_ctx *const *ctx, size_t n_parts, const std::vector<Delivery> &copies,
-                    cudaStream_t caller = nullptr);
+// Device 0's stream waits for the streams of the n listed contexts, then copies the outputs to the caller, and the host
+// waits for the copies.
+aicb_status deliver(aicb_ctx *const *ctx, size_t n, const std::vector<Delivery> &copies);
 // aicb200.cu: GraphicsOptions as every frame call accepts them (AICB_ERR_INVALID otherwise).
 aicb_status validate_options(const aicb_options *o);
 
