@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include "brick_room.h"
+#include "host_tables.h"
 #include "internal.h"
 
 using namespace aicb;
@@ -38,13 +39,6 @@ aicb_status aicb_cuda_fail(cudaError_t e, const char *what) {
 static aicb_status fail(aicb_status st, const std::string &msg) { return aicb_fail(st, msg); }
 static aicb_status cuda_fail(cudaError_t e, const char *what) { return aicb_cuda_fail(e, what); }
 
-// PackedLight::some -> scalar_in (light/data.rs:213-217)
-static uint8_t scalar_in(float v) {
-    float x = std::round(std::log2(v) * 10.0f + 144.0f);
-    if (!(x > 0.0f)) return 0;
-    if (x >= 255.0f) return 255;
-    return (uint8_t)x;
-}
 static uint32_t texel_some(const float rgb[3]) {
     return (uint32_t)scalar_in(rgb[0]) | ((uint32_t)scalar_in(rgb[1]) << 8) | ((uint32_t)scalar_in(rgb[2]) << 16) |
            (255u << 24);
@@ -93,47 +87,6 @@ static void build_block_sky(const aicb_sky &sky, DeviceScene *ds) {
     float q[3];
     for (int i = 0; i < 3; i++) q[i] = ps_mul_h(sum[i], 1.0f / 8.0f);
     ds->sky_mean = texel_some(q);
-}
-
-// component_to_srgb8 (math/color.rs:1038-1054) evaluated with the platform powf — exactly what the
-// reference computes on this host — and inverted into thresholds: thr[k] = the smallest non-negative
-// f32 whose encoding is >= k.  The device encodes by searching this table.
-static uint8_t srgb8_host(float c) {
-    float s = (c <= 0.0031308f) ? c * (323.0f / 25.0f) : (211.0f * std::pow(c, 5.0f / 12.0f) - 11.0f) / 200.0f;
-    float v = std::round(s * 255.0f);
-    if (!(v > 0.0f)) return 0;
-    if (v >= 255.0f) return 255;
-    return (uint8_t)v;
-}
-static void build_srgb_thresholds(float *thr) {
-    thr[0] = 0.0f;
-    for (int k = 1; k < 256; k++) {
-        // bisection over the bit patterns of non-negative floats (monotone in value)
-        uint32_t lo = 0, hi = 0x7f800000u;  // +0 .. +inf
-        while (lo < hi) {
-            uint32_t mid = lo + (hi - lo) / 2;
-            float f;
-            std::memcpy(&f, &mid, 4);
-            if (srgb8_host(f) >= k) hi = mid; else lo = mid + 1;
-        }
-        std::memcpy(&thr[k], &lo, 4);
-    }
-}
-
-// PackedLight::scalar_in (light/data.rs:213-217) inverted into thresholds with the platform log2f
-// (see light_kernel.cuh scalar_in_t): thr[k] = the smallest non-negative f32 whose quantised value is >= k.
-static void build_light_thresholds(float *thr) {
-    thr[0] = 0.0f;
-    for (int k = 1; k < 256; k++) {
-        uint32_t lo = 0, hi = 0x7f800000u;
-        while (lo < hi) {
-            uint32_t mid = lo + (hi - lo) / 2;
-            float f;
-            std::memcpy(&f, &mid, 4);
-            if (scalar_in(f) >= k) hi = mid; else lo = mid + 1;
-        }
-        std::memcpy(&thr[k], &lo, 4);
-    }
 }
 
 static bool voxel_invisible(const aicb_voxel &v) {

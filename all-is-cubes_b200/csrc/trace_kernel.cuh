@@ -332,10 +332,17 @@ AICB_DEV int signum_101(double x) { return (x == 0.0 || x != x) ? 0 : (x < 0.0 ?
 // correctly rounded reciprocal and a faithful quotient, q + (a - b q) rb rounds to RN(a / b)).  The ray's t_delta IS
 // RN(1 / |direction|) (raycast.rs:769), so the divisions by the direction in Raycaster::within / fast_forward /
 // scale_to_integer_step cost five FP64 instructions instead of a division routine.  Outside a generous exponent
-// window (where an intermediate could leave the normal range) the real division is used.
+// window (where an intermediate could leave the normal range) the real division is used.  The window bounds |a| from
+// below as well: with 2^-600 <= |a| the quotient is at least 2^-1001 and the remainders are multiples of 2^-705, so
+// all stay normal and exact; a quotient near the subnormal range would not be correctly rounded.  Zeros take the
+// division too (the corrections would turn -0 / b into +0).  Of the callers, pixel_ray's numerators are integers
+// (0 among them) and scale_to_integer_step's are >= 2^-53; caster_begin's and project_ndc's can be zero, and can be
+// tiny only for a ray origin within 2^-600 of a grid plane or a degenerate camera matrix.
+// tests/test_gpu_scalar_math.py checks it against IEEE division on every pixel quotient x / W with W <= 16384, on
+// random pairs with |b| from 2^-420 to 2^420 and |a| from 2^-1074 to 2^210, and on project_ndc's three quotients.
 AICB_DEV double div_known_recip(double a, double b, double rb) {
-    const double ab = fabs(b);
-    if (!((ab >= 0x1p-400) & (ab <= 0x1p400) & (fabs(a) <= 0x1p200))) return a / b;
+    const double ab = fabs(b), aa = fabs(a);
+    if (!((ab >= 0x1p-400) & (ab <= 0x1p400) & (aa <= 0x1p200) & (aa >= 0x1p-600))) return a / b;
     const double q0 = a * rb;
     const double r0 = fma(-b, q0, a);
     const double q1 = fma(r0, rb, q0);
@@ -515,8 +522,11 @@ AICB_DEV void texel_value_ao(const float *lut, uint32_t t, float out[4]) {  // d
     out[3] = (st == 255) ? 1.0f : (st == 128 ? 0.25f : 0.0f);
 }
 
+// f64::rem_euclid(1.0): r = x % 1.0 (fmod: exact, with x's sign, so -0 for a negative integer or -0), + 1 if r < 0.
+// x - trunc(x) is that remainder exactly except for its zeros, which it makes +0; copysign restores fmod's -0.
+// tests/test_gpu_scalar_math.py checks it against fmod around the integers, 2^52 .. 2^53 and beyond, both signs.
 AICB_DEV double rem_euclid1(double x) {
-    double r = x - trunc(x);
+    const double r = copysign(x - trunc(x), x);
     return r < 0.0 ? r + 1.0 : r;
 }
 
@@ -654,6 +664,13 @@ AICB_DEV void colorbuf_to_rgba(float l0, float l1, float l2, float tr, float out
     out[3] = (alpha > 0.0f && alpha <= 1.0f) ? alpha : (alpha == 0.0f ? 0.0f : 1.0f);
 }
 
+// Two f16 texel channels as one word, lo in the low half: half::f16::from_f32 of each (round to nearest even, overflow
+// to infinity, subnormals kept).  tests/test_gpu_scalar_math.py checks it on every f32 bit pattern.
+AICB_DEV uint32_t f16x2_texel(float lo, float hi) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t *>(&h);
+}
+
 AICB_DEV unsigned char sat_u8(float v) {  // `as u8`: saturating, NaN -> 0
     if (!(v > 0.0f)) return 0;
     if (v >= 255.0f) return 255;
@@ -715,7 +732,7 @@ AICB_DEV void project_ndc(const TraceParams &P, double x, double y, double z, do
 
 // viewport.rs:104-113 + renderer.rs:424-451,489-491.  The four quotients by the framebuffer size are correctly rounded
 // from the host's RN(1 / W) and RN(1 / H) (pixel coordinates and sizes are integers < 2^32, well inside
-// div_known_recip's exponent window), so they equal the divisions bit for bit.
+// div_known_recip's exponent window, or 0, which it divides), so they equal the divisions bit for bit.
 AICB_DEV void pixel_ray(const TraceParams &P, uint32_t xch, uint32_t ych, int sample, double o[3], double d[3]) {
     const double W = (double)P.fb_width, H = (double)P.fb_height;
     const double x0 = div_known_recip((double)xch, W, P.inv_width) * 2.0 - 1.0;
@@ -2049,11 +2066,9 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
             const float e = tex_layer == TEX_UI ? P.target.tex_exposure[1] : (tex_layer == TEX_WORLD ? P.target.tex_exposure[0] : 1.0f);
             float a = 1.0f - tT;
             a = a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a);
-            const __half2 rg = __floats2half2_rn(l0 * e, l1 * e);
-            const __half2 ba = __floats2half2_rn(l2 * e, a);
             uint2 packed;
-            packed.x = *reinterpret_cast<const uint32_t *>(&rg);
-            packed.y = *reinterpret_cast<const uint32_t *>(&ba);
+            packed.x = f16x2_texel(l0 * e, l1 * e);
+            packed.y = f16x2_texel(l2 * e, a);
             P.target.out_rgba16f[out_index] = packed;
         }
         if (P.target.out_tex_depth) {
@@ -2072,11 +2087,9 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
         // f16 as half::f16::from_f32 does (round to nearest even, overflow to infinity)
         float a = 1.0f - tT;
         a = a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a);   // clamp(0, 1): NaN passes through
-        const __half2 rg = __floats2half2_rn(l0 * P.exposure, l1 * P.exposure);
-        const __half2 ba = __floats2half2_rn(l2 * P.exposure, a);
         uint2 packed;
-        packed.x = *reinterpret_cast<const uint32_t *>(&rg);
-        packed.y = *reinterpret_cast<const uint32_t *>(&ba);
+        packed.x = f16x2_texel(l0 * P.exposure, l1 * P.exposure);
+        packed.y = f16x2_texel(l2 * P.exposure, a);
         P.target.out_rgba16f[out_index] = packed;
     }
     if (P.target.out_depth) P.target.out_depth[out_index] = depth;

@@ -5,6 +5,7 @@
 // operation: f64 for ray geometry, f32 for colour, no FMA contraction, Rust semantics for
 // min/max/clamp/round/saturating casts (SURVEY.md Appendix B).
 #include "aic_oracle.hpp"
+#include "../all-is-cubes_b200/csrc/exact_math.cuh"   // LIBM_CR: the correctly rounded powf / expf
 
 #include <atomic>
 #include <cmath>
@@ -741,11 +742,11 @@ struct ColorBuf {
 };
 
 // The two f32 transcendentals of the per-ray path: f32::powf (raytracer_components.rs:233) and f32::exp (sr.rs:751).
-// Rust's std calls the platform libm; mode 0 does the same (glibc powf / expf).  Mode 1 ("cr") evaluates in f64 and
-// rounds once, which is what the CUDA path does: it is the correctly rounded result except when the f64 value lies
-// within an f64 ULP or two of an f32 rounding boundary (probability ~1e-8 per call).  The parity tests compare the
-// GPU with mode 1 exactly (0 ULP) and bound mode 0 against mode 1 per call (<= 1 ULP), so that a libm difference
-// cannot hide a kernel difference.  Selected by orc_set_libm() / ORC_LIBM=cr.
+// Rust's std calls the platform libm; mode 0 does the same (glibc powf / expf).  Mode 1 ("cr") is the correctly
+// rounded f32, computed by the CUDA path's own header (exact_math.cuh) compiled as host code, so that the oracle and
+// the device do not depend on two f64 libms agreeing (libdevice's and glibc's f64 pow, rounded to f32, do not always).
+// The parity tests compare the GPU with mode 1 exactly (0 ULP) and bound mode 0 against mode 1 per call (<= 1 ULP),
+// so that a libm difference cannot hide a kernel difference.  Selected by orc_set_libm() / ORC_LIBM=cr.
 static std::atomic<int> g_libm_mode{-1};
 static int libm_mode() {
     int m = g_libm_mode.load(std::memory_order_relaxed);
@@ -756,10 +757,8 @@ static int libm_mode() {
     }
     return m;
 }
-static inline float orc_powf_mode(float x, float y) {
-    return libm_mode() ? (float)std::pow((double)x, (double)y) : std::pow(x, y);
-}
-static inline float orc_expf_mode(float x) { return libm_mode() ? (float)std::exp((double)x) : std::exp(x); }
+static inline float orc_powf_mode(float x, float y) { return libm_mode() ? aicb::powf_exact(x, y) : std::pow(x, y); }
+static inline float orc_expf_mode(float x) { return libm_mode() ? aicb::expf_exact(x) : std::exp(x); }
 
 // apply_transmittance (raytracer_components.rs:215-258)
 static void apply_transmittance(const float color[4], float thickness_in, float out_color[4], float *coeff) {
@@ -1828,11 +1827,11 @@ void orc_scene_block_sky(const orc_scene *s, uint8_t out[7][4]) {
     out[6][0] = s->sky_mean.r; out[6][1] = s->sky_mean.g; out[6][2] = s->sky_mean.b; out[6][3] = s->sky_mean.status;
 }
 
-// libm mode of the two per-ray transcendentals: 0 = platform powf/expf (what Rust's std calls), 1 = f64 + one rounding.
+// libm mode of the two per-ray transcendentals: 0 = platform powf/expf (what Rust's std calls), 1 = correctly rounded.
 void orc_set_libm(int mode) { g_libm_mode.store(mode ? 1 : 0, std::memory_order_relaxed); }
 int orc_get_libm(void) { return libm_mode(); }
-float orc_powf(float x, float y, int mode) { return mode ? (float)std::pow((double)x, (double)y) : std::pow(x, y); }
-float orc_expf(float x, int mode) { return mode ? (float)std::exp((double)x) : std::exp(x); }
+float orc_powf(float x, float y, int mode) { return mode ? aicb::powf_exact(x, y) : std::pow(x, y); }
+float orc_expf(float x, int mode) { return mode ? aicb::expf_exact(x) : std::exp(x); }
 
 int orc_hardware_threads(void) {
     unsigned n = std::thread::hardware_concurrency();

@@ -105,7 +105,7 @@ LIBM_PLATFORM, LIBM_CR = 0, 1
 
 def set_libm(mode):
     """How the oracle evaluates f32::powf (raytracer_components.rs:233) and f32::exp (sr.rs:751): LIBM_PLATFORM = glibc
-    powf / expf (what Rust's std calls on this host), LIBM_CR = in f64, rounded once (what the CUDA path does)."""
+    powf / expf (what Rust's std calls on this host), LIBM_CR = correctly rounded (what the CUDA path does)."""
     lib().orc_set_libm(int(mode))
 
 

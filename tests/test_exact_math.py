@@ -1,6 +1,7 @@
 """The shading path's f32 transcendentals (csrc/exact_math.cuh): powf_exact and expf_exact are a short f64 polynomial
-and Ziv's rounding test, with the libm call as the fallback, and must give (float)pow((double)x, (double)y) and
-(float)exp((double)x) bit for bit.  The header is compiled here as host code with the project's -fmad=false and
+and Ziv's rounding test, with a correctly rounded double-double evaluation as the fallback, and must give glibc's
+(float)pow((double)x, (double)y) and (float)exp((double)x) bit for bit on these arguments, where that is correctly
+rounded (tests/test_gpu_scalar_math.py checks the device against the host and every glibc disagreement).  The header is compiled here as host code with the project's -fmad=false and
 -ffp-contract=off contract; its short paths use only correctly rounded operations, so they compute on the host the
 f64 values the device computes.  Each check also measures the short path's f64 error against x87 long double powl /
 expl, which must stay well inside the bound the rounding test assumes (EXACT_MATH_BOUND = 2^-40)."""

@@ -4,7 +4,7 @@ against the oracle on identical Space / Camera / options.
 Bar (BASELINE.json north_star: +-1 ULP per f32 channel, hit indices bit-exact).  What is asserted here is
 stronger and leaves no slack for an ordering bug to hide in: hit indices, step counts, depths, **every ColorBuf
 channel and every sRGB8 byte are bit-identical (0 ULP)** to the oracle evaluating f32::powf / f32::exp the way
-the device does (in f64, rounded once: `orc.LIBM_CR`).  The only other difference between that oracle and the
+the device does (correctly rounded: `orc.LIBM_CR`).  The only other difference between that oracle and the
 reference on this host is glibc's powf / expf, which tests/test_oracle_libm.py bounds per call (<= 1 ULP, the
 two modes agree on ~99 % of calls) and per image."""
 import itertools

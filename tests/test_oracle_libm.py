@@ -1,12 +1,12 @@
 """The oracle's two libm modes (tests/orc.py: LIBM_PLATFORM = glibc powf / expf, what Rust's std calls on this host;
-LIBM_CR = evaluated in f64 and rounded once, what the CUDA path does).
+LIBM_CR = correctly rounded, computed by the CUDA path's exact_math.cuh as host code, what the CUDA path does).
 
 The GPU parity tests hold the CUDA path to the LIBM_CR oracle bit for bit; this module bounds the only remaining
 difference to the reference on this platform — the libm — per call and per image, so that the two statements
 together give the north_star's +-1 ULP per transcendental call without a tolerance window a kernel bug could hide in:
   * f32::powf in apply_transmittance (raytracer_components.rs:233) and f32::exp in distance_fog (sr.rs:751) are the
     only transcendental calls of the per-ray path (the sRGB encode uses the platform powf on both sides);
-  * per call, glibc's result is within 1 ULP of the round-once result, and equal to it on almost all inputs;
+  * per call, glibc's result is within 1 ULP of the correctly rounded result, and equal to it on almost all inputs;
   * per image, the two modes give identical hits, steps and depths, and ColorBuf channels whose difference is
     bounded by (calls on the ray) x 1 ULP of the factors involved.
 """
@@ -27,14 +27,14 @@ def test_powf_expf_per_call_within_one_ulp():
     a = np.array([L.orc_powf(float(x[i]), float(y[i]), 0) for i in range(n)], dtype=np.float32)
     b = np.array([L.orc_powf(float(x[i]), float(y[i]), 1) for i in range(n)], dtype=np.float32)
     d = orc.ulp_diff(a, b)
-    assert d.max() <= 1, f"powf: glibc differs from the round-once value by {d.max()} ULP"
+    assert d.max() <= 1, f"powf: glibc differs from the correctly rounded value by {d.max()} ULP"
     assert (d == 0).mean() > 0.95
     # fog: exp(-1.6 * rel), rel in [0, 1]
     e = (-1.6 * rng.uniform(0.0, 1.0, n)).astype(np.float32)
     a = np.array([L.orc_expf(float(v), 0) for v in e], dtype=np.float32)
     b = np.array([L.orc_expf(float(v), 1) for v in e], dtype=np.float32)
     d = orc.ulp_diff(a, b)
-    assert d.max() <= 1, f"expf: glibc differs from the round-once value by {d.max()} ULP"
+    assert d.max() <= 1, f"expf: glibc differs from the correctly rounded value by {d.max()} ULP"
     assert (d == 0).mean() > 0.95
 
 
