@@ -174,6 +174,25 @@ def load_library() -> C.CDLL:
     }.items():
         for prefix in ("aicb_", "aicb_group_"):
             getattr(lib, prefix + name).argtypes = argtypes
+    # the texture targets: aicb_texture_target_<name> and aicb_group_texture_target_<name>, the layers aside
+    for name, argtypes in {
+        "create": [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.POINTER(C.c_void_p)],
+        "destroy": [C.c_void_p],
+        "resize": [C.c_void_p, C.c_uint32, C.c_uint32],
+        "mark_dirty": [C.c_void_p],
+        "state": [C.c_void_p, C.POINTER(abi.TextureTargetInfo)],
+        "picks": [C.c_void_p, C.c_uint64, C.c_size_t, C.c_void_p],
+        "buffers": [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)],
+        "read": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t],
+    }.items():
+        for prefix in ("aicb_texture_target_", "aicb_group_texture_target_"):
+            getattr(lib, prefix + name).argtypes = argtypes
+    lib.aicb_texture_target_destroy.restype = None
+    lib.aicb_group_texture_target_destroy.restype = None
+    for prefix, layer in (("aicb_", abi.Layer), ("aicb_group_", abi.GroupLayer)):
+        getattr(lib, prefix + "texture_target_trace").argtypes = [
+            C.c_void_p, C.POINTER(layer), C.POINTER(layer), C.c_void_p, C.c_void_p, C.POINTER(C.c_double), C.c_size_t,
+            size, info]
     if lib.aicb_abi_version() != abi.ABI_VERSION:
         raise RuntimeError("libaicb200.so ABI version mismatch")
     _lib = lib
@@ -1291,6 +1310,129 @@ def pixel_picker_order(width: int, height: int, count: Optional[int] = None) -> 
     return sorted_pixels[lin].astype(np.uint32)
 
 
+def consistent_picks(width: int, height: int, start: int, count: int) -> np.ndarray:
+    """The pixels UpdateStrategy::Consistent traces from `next` = start (raytrace_to_texture.rs:704-727): picks
+    start .. start + count - 1 through point_from_pixel_index (:912-918), which wraps with rem_euclid / div_euclid, as
+    linear indices y * width + x."""
+    i = np.uint64(start) + np.arange(count, dtype=np.uint64)
+    w, h = np.uint64(width), np.uint64(height)
+    return (i % w + (i // w) % h * w).astype(np.uint32)
+
+
+TEXTURE_INCREMENTAL, TEXTURE_CONSISTENT = abi.TEXTURE_INCREMENTAL, abi.TEXTURE_CONSISTENT
+
+
+class _DeviceArray:
+    """A device buffer the library owns, as __cuda_array_interface__ for torch.as_tensor (no copy); it keeps its owner
+    alive as long as a tensor of it lives."""
+
+    def __init__(self, owner, ptr: int, shape, typestr: str):
+        self._owner = owner
+        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (ptr, False),
+                                         "strides": None, "version": 2}
+
+
+class TextureTarget:
+    """RaytraceToTexture's state on the device (raytrace_to_texture.rs): the update strategy and its pick position,
+    dirty_pixels, and the colour and depth render targets of RaytraceToTexture::Inner, without the RtRenderer (the
+    layers are passed to each trace).  aicb_texture_target_* on a Context, aicb_group_texture_target_* on a DeviceGroup
+    (DeviceGroup.texture_target), with the same results.  strategy: TEXTURE_INCREMENTAL (PixelPicker, the reference's)
+    or TEXTURE_CONSISTENT (row-major `next`).  rays_per_frame and its time budget stay with the caller, which passes a
+    batch size to trace() and times it."""
+
+    def __init__(self, width: int, height: int, strategy: int = TEXTURE_INCREMENTAL, ctx: Optional["Context"] = None,
+                 group: Optional["DeviceGroup"] = None):
+        self.group = group
+        self.ctx = None if group is not None else (ctx or Context.default())
+        self._prefix = "aicb_group_texture_target_" if group is not None else "aicb_texture_target_"
+        self.handle = C.c_void_p()
+        owner = group.handle if group is not None else self.ctx.handle
+        _check(self._fn("create")(owner, int(width), int(height), int(strategy), C.byref(self.handle)))
+
+    def _fn(self, name: str):
+        if self.ctx is not None:
+            self.ctx.settle()
+        return getattr(load_library(), self._prefix + name)
+
+    def _device(self):
+        return _torch().device("cuda", self.group.device_ids[0] if self.group is not None else self.ctx.device_id)
+
+    def close(self):
+        """Destroys the target; a target whose Context was closed first holds nothing that can still be freed."""
+        if self.handle and (self.ctx is None or self.ctx.handle):
+            self._fn("destroy")(self.handle)
+        self.handle = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def resize(self, width: int, height: int):
+        """UpdateStrategy::resize: the same size does nothing; another makes cleared targets and, for Incremental, a
+        new order from pick 0.  dirty_pixels is left as it is."""
+        _check(self._fn("resize")(self.handle, int(width), int(height)))
+
+    def mark_dirty(self):
+        """RaytraceToTexture::dirty: dirty_pixels = cycle_length."""
+        _check(self._fn("mark_dirty")(self.handle))
+
+    def trace(self, world=None, ui=None, backdrop=None, no_world=None, depth_transform=None, n: int = 0):
+        """One do_some_tracing batch of n picks: world / ui = (scene, Camera, GraphicsOptions) or None, as
+        render_layers_texture takes them (SpaceRaytracers on a Context, GroupScenes on a group).  Returns
+        (n_traced, RenderInfo); n_traced is 0 when dirty_pixels was 0, n otherwise."""
+        keep = []
+        cls = abi.GroupLayer if self.group is not None else abi.Layer
+        fn = self._fn("trace")
+        w_arg, u_arg = _layer_arg(world, keep, cls), _layer_arg(ui, keep, cls)
+        b = np.array(backdrop, dtype=np.float32) if backdrop is not None else None
+        nw = np.array(no_world, dtype=np.float32) if no_world is not None else None
+        m = np.ascontiguousarray(depth_transform, dtype=np.float64).reshape(16) if depth_transform is not None else None
+        traced = C.c_size_t(0)
+        info = abi.RenderInfo()
+        _check(fn(self.handle, w_arg, u_arg, b.ctypes.data if b is not None else None,
+                  nw.ctypes.data if nw is not None else None,
+                  m.ctypes.data_as(C.POINTER(C.c_double)) if m is not None else None, int(n), C.byref(traced),
+                  C.byref(info)))
+        return int(traced.value), RenderInfo.from_abi(info)
+
+    @property
+    def state(self) -> dict:
+        """width, height, strategy, dirty_pixels, next_pick (the pick position) and cycle_length."""
+        s = abi.TextureTargetInfo()
+        _check(self._fn("state")(self.handle, C.byref(s)))
+        return {"width": s.width, "height": s.height, "strategy": s.strategy, "dirty_pixels": s.dirty_pixels,
+                "next_pick": s.next_pick, "cycle_length": s.cycle_length}
+
+    def picks(self, start: int, n: int) -> np.ndarray:
+        """The linear pixel indices y * width + x of picks start .. start + n - 1, from the device code that feeds a
+        batch."""
+        out = np.zeros(int(n), dtype=np.uint32)
+        _check(self._fn("picks")(self.handle, int(start), int(n), out.ctypes.data))
+        return out
+
+    def read(self):
+        """Copies of the targets: (rgba16f bits uint16 [h, w, 4], depth float32 [h, w])."""
+        s = self.state
+        rgba = np.zeros((s["height"], s["width"], 4), dtype=np.uint16)
+        depth = np.zeros((s["height"], s["width"]), dtype=np.float32)
+        _check(self._fn("read")(self.handle, rgba.ctypes.data, depth.ctypes.data, s["width"] * s["height"]))
+        return rgba, depth
+
+    def tensors(self):
+        """The targets in place, as CUDA tensors on the target's device (device 0 of a group): (uint16 [h, w, 4],
+        float32 [h, w]).  They stay valid until the next resize() or close(); a later trace() writes into them."""
+        torch = _torch()
+        s = self.state
+        rgba, depth = C.c_void_p(), C.c_void_p()
+        _check(self._fn("buffers")(self.handle, C.byref(rgba), C.byref(depth)))
+        h, w = s["height"], s["width"]
+        dev = self._device()
+        return (torch.as_tensor(_DeviceArray(self, rgba.value, (h, w, 4), "<u2"), device=dev),
+                torch.as_tensor(_DeviceArray(self, depth.value, (h, w), "<f4"), device=dev))
+
+
 def render_orthographic(rt, resolution: int = 32) -> "Rendering":
     """raytracer::ortho::render_orthographic (ortho.rs:30-84): the five-view pixel-perfect image of the whole Space.
     `rt`: a SpaceRaytracer, or a GroupScene (its devices share the views' pixels; the same image)."""
@@ -1366,6 +1508,7 @@ class DeviceGroup:
         self.device_ids = [int(d) for d in device_ids]
         self.scene = None
         self.scenes = []
+        self.targets = []
 
     def add_scene(self, space: "Space") -> GroupScene:
         s = GroupScene(self, space)
@@ -1399,6 +1542,13 @@ class DeviceGroup:
             return _layers_terminal_device(self, world, ui, backdrop, no_world, out)
         return _layers_terminal(load_library().aicb_group_render_layers_terminal, abi.GroupLayer, world, ui, backdrop,
                                 no_world)
+
+    def texture_target(self, width: int, height: int, strategy: int = TEXTURE_INCREMENTAL) -> "TextureTarget":
+        """A TextureTarget on this group: its targets are device 0's, and a batch is cut across the devices as
+        render_layers_texture cuts a pixel list.  Close it before the group."""
+        t = TextureTarget(width, height, strategy, group=self)
+        self.targets.append(t)
+        return t
 
     def update(self, space: "Space"):
         if self.scene:
@@ -1494,6 +1644,9 @@ class DeviceGroup:
         return render_orthographic(self.scene, resolution)
 
     def close(self):
+        for t in self.targets:
+            t.close()
+        self.targets = []
         for s in self.scenes:
             s.close()
         self.scenes = []

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 18
+ABI_VERSION = 19
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -139,6 +139,15 @@ class DeviceOutputs(C.Structure):
                 ("_pad", C.c_uint32)]
 
 
+TEXTURE_INCREMENTAL, TEXTURE_CONSISTENT = 1, 2
+
+
+class TextureTargetInfo(C.Structure):
+    """aicb_texture_target_info: a texture target's size, strategy, dirty_pixels, pick position and cycle_length."""
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("strategy", C.c_uint32), ("_pad", C.c_uint32),
+                ("dirty_pixels", C.c_uint64), ("next_pick", C.c_uint64), ("cycle_length", C.c_uint64)]
+
+
 EXPORTED_SYMBOLS = [
     "aicb_abi_version",
     "aicb_ctx_create",
@@ -229,6 +238,24 @@ EXPORTED_SYMBOLS = [
     "aicb_group_render_device",
     "aicb_group_trace_rays_device",
     "aicb_group_render_layers_device",
+    "aicb_texture_target_create",
+    "aicb_texture_target_destroy",
+    "aicb_texture_target_resize",
+    "aicb_texture_target_mark_dirty",
+    "aicb_texture_target_trace",
+    "aicb_texture_target_state",
+    "aicb_texture_target_picks",
+    "aicb_texture_target_buffers",
+    "aicb_texture_target_read",
+    "aicb_group_texture_target_create",
+    "aicb_group_texture_target_destroy",
+    "aicb_group_texture_target_resize",
+    "aicb_group_texture_target_mark_dirty",
+    "aicb_group_texture_target_trace",
+    "aicb_group_texture_target_state",
+    "aicb_group_texture_target_picks",
+    "aicb_group_texture_target_buffers",
+    "aicb_group_texture_target_read",
     "aicb_group_light_fast_evaluate",
     "aicb_group_light_compute",
     "aicb_group_light_compute_debug",

@@ -545,7 +545,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
         if ((uint64_t)P.tiles_x * P.tiles_y * 32 > 0xffffffffull) return fail(AICB_ERR_INVALID, "frame too large");
         P.n_tasks = P.tiles_x * P.tiles_y * 32;
         pixels = (uint64_t)P.fb_width * P.local_rows;
-        if (out.target.pixel_list) {   // one pixel task per listed pixel, 32 consecutive entries per warp
+        if (listed(out.target)) {   // one pixel task per listed pixel, 32 consecutive entries per warp
             P.tiles_x = (out.target.n_list + 31) / 32;
             P.tiles_y = 1;
             P.n_tasks = out.target.n_list;
@@ -2145,7 +2145,7 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
     const int aa = lead->options->antialiasing_always ? 1 : 0;
     // per-task buffers between the passes: one entry per ray of the part's task layout (launch_trace)
     auto n_tasks = [&](const LayerPart &p) -> size_t {
-        return (p.out.target.pixel_list ? (size_t)p.out.target.n_list
+        return (listed(p.out.target) ? (size_t)p.out.target.n_list
                                         : (((size_t)lead->camera->fb_width + TILE_W - 1) / TILE_W) *
                                               ((shard_rows(lead->camera->fb_height, &p.shard) + TILE_H - 1) / TILE_H) * 32) *
                (aa ? 4 : 1);
@@ -2209,6 +2209,9 @@ aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, con
             o.kind = p.out.kind;
             o.target.pixel_list = p.out.target.pixel_list;
             o.target.n_list = p.out.target.n_list;
+            o.target.picks = p.out.target.picks;
+            o.target.pick_central = p.out.target.pick_central;
+            o.target.pick_base = p.out.target.pick_base;
             o.target.tex_layer = TEX_UI;
             if (o.kind == TGT_TEX) o.target.out_task_depth = ctx->d_task_depth.get<double>();
             if (o.kind == TGT_TERM) {
@@ -2299,7 +2302,7 @@ aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer 
     return AICB_OK;
 }
 
-void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out) {
+void aicb_texture_outputs(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out) {
     out->full_frame = true;
     out->kind = TGT_TEX;
     // the exposure of each layer's camera (:603-605); a missing layer's is never used

@@ -20,19 +20,6 @@
 
 #include "internal.h"
 
-struct aicb_group {
-    std::vector<aicb_ctx *> ctx;
-    bool light_peers = false;  // device 0 reaches every device too, and the devices have native peer atomics
-    ~aicb_group() {
-        for (aicb_ctx *c : ctx) aicb_ctx_destroy(c);
-    }
-};
-
-struct aicb_group_scene {
-    aicb_group *group = nullptr;
-    std::vector<aicb_scene *> scene;
-};
-
 static const uint32_t GROUP_STRIP_ROWS = 16;
 
 aicb_status fan_out(aicb_ctx *const *ctx, size_t n) {
@@ -198,7 +185,7 @@ static aicb_status stage_outputs(aicb_ctx *root, const aicb_device_outputs &host
 }
 
 // The contexts of a validated layered call: those of its lead layer's replicas.
-static std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *lead) {
+std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *lead) {
     aicb_scene *const *scenes = lead == c.world ? c.world_scenes : c.ui_scenes;
     std::vector<aicb_ctx *> ctx;
     for (size_t i = 0; i < c.n; i++) ctx.push_back(scenes[i]->ctx);
@@ -228,7 +215,7 @@ static aicb_status layers_host(const LayeredCall &c, const aicb_layer *lead, con
     Outputs target;
     std::vector<Delivery> copies;
     TRY(stage_outputs(ctx[0], host, STAGE_GIVEN, DEV_LAYERS, &target, &copies));
-    if (target.kind == aicb::TGT_TEX) aicb_texture_target(c.world, c.ui, depth_transform, &target);
+    if (target.kind == aicb::TGT_TEX) aicb_texture_outputs(c.world, c.ui, depth_transform, &target);
     target.full_frame = true;
     return draw_layers(c, ctx, target, pixels, false, host.len, copies, nullptr, info);
 }
@@ -283,7 +270,7 @@ aicb_status layers_device(const LayeredCall &c, const double *depth_transform, c
     Outputs target;
     TRY(device_target(outs, ctx[0]->device, DEV_LAYERS, false, false, &target));
     if (d_pixels && n_pixels) TRY(check_device_pointer(d_pixels, ctx[0]->device, false, 4, "the pixel list"));
-    if (target.kind == aicb::TGT_TEX) aicb_texture_target(c.world, c.ui, depth_transform, &target);
+    if (target.kind == aicb::TGT_TEX) aicb_texture_outputs(c.world, c.ui, depth_transform, &target);
     target.full_frame = true;
     if (info) std::memset(info, 0, sizeof *info);
     if (async) {
@@ -393,7 +380,7 @@ static aicb_layer on_device0(const aicb_group_layer *l) {
     return r;
 }
 
-static aicb_status group_call(const aicb_group_layer *world, const aicb_group_layer *ui, const float *backdrop_rgba,
+aicb_status group_call(const aicb_group_layer *world, const aicb_group_layer *ui, const float *backdrop_rgba,
                               const float *no_world_rgba, aicb_layer views[2], LayeredCall *c) {
     const bool have_world = world && world->scene, have_ui = ui && ui->scene;
     if (have_world && have_ui && world->scene->group != ui->scene->group)

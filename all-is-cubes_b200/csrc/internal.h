@@ -313,6 +313,10 @@ struct Outputs {
     int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
 };
 
+// A frame whose pixel tasks are listed: a pixel list, or a texture target's picks (one task per entry, 32 per warp).
+// task_pixel recognises one by its n_list, which is never 0 for these (a call with no pixel or pick returns first).
+inline bool listed(const aicb::TargetParams &t) { return t.pixel_list || t.picks != aicb::PICK_LIST; }
+
 // One context's share of a layered frame or texture (aicb_trace_layers): that context's scenes of the layers (nullptr
 // for an absent layer; both on one context), its row strips of a whole frame or its range of a pixel list
 // (out.target.pixel_list), and where it stores its outputs.
@@ -354,7 +358,7 @@ aicb_status aicb_check_layers_texture(const aicb_layer *world, const aicb_layer 
                                       const double *depth_transform, const uint32_t *pixels, bool pixels_on_device,
                                       size_t n_pixels, const void *out_rgba16f, const float *out_depth,
                                       const aicb_layer **lead_out);
-void aicb_texture_target(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out);
+void aicb_texture_outputs(const aicb_layer *world, const aicb_layer *ui, const double *depth_transform, Outputs *out);
 aicb_status aicb_trace_layers(const aicb_layer *world, const aicb_layer *ui, const float *backdrop_rgba,
                               const float *no_world_rgba, LayerPart *parts, size_t n_parts,
                               const std::vector<Delivery> &copies, aicb_render_info *total, cudaStream_t async);
@@ -367,6 +371,21 @@ void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool sa
 LightBlockDev light_block(const aicb_block_desc &b);
 
 // ---- calls over several contexts ----------------------------------------------------------------------------------
+// A device group (group.cu): one context per listed device, device 0's first; every other device reaches device 0's
+// memory as a peer.  A group scene: a scene's replica on each of them.
+struct aicb_group {
+    std::vector<aicb_ctx *> ctx;
+    bool light_peers = false;  // device 0 reaches every device too, and the devices have native peer atomics
+    ~aicb_group() {
+        for (aicb_ctx *c : ctx) aicb_ctx_destroy(c);
+    }
+};
+
+struct aicb_group_scene {
+    aicb_group *group = nullptr;
+    std::vector<aicb_scene *> scene;
+};
+
 // A call that runs on several contexts lists them device 0's first, with a scene's replica on each (a group scene's
 // replicas, in the group's order); a single context is the one-context case and runs as it would alone.  The call
 // holds every listed context's lock throughout, and device 0 is where its results are collected.
@@ -455,6 +474,12 @@ struct LayeredCall {
     size_t n;
     const float *backdrop_rgba, *no_world_rgba;
 };
+// A group call's layers as device 0 sees them (`views`, filled here) and each layer's replicas; AICB_ERR_INVALID for
+// scenes of two groups.
+aicb_status group_call(const aicb_group_layer *world, const aicb_group_layer *ui, const float *backdrop_rgba,
+                       const float *no_world_rgba, aicb_layer views[2], LayeredCall *c);
+// The contexts of a validated layered call: those of its lead layer's replicas, device 0's first.
+std::vector<aicb_ctx *> contexts(const LayeredCall &c, const aicb_layer *lead);
 aicb_status layers_srgb8(const LayeredCall &c, uint8_t (*out)[4], size_t out_len, aicb_render_info *info);
 aicb_status layers_terminal(const LayeredCall &c, aicb_terminal_pixel *out, size_t out_len, aicb_render_info *info);
 aicb_status layers_texture(const LayeredCall &c, const double *depth_transform, const uint32_t *pixels, size_t n_pixels,

@@ -181,6 +181,12 @@ struct TargetParams {
     const uint32_t *pixel_list; // pixel task i is the framebuffer pixel pixel_list[i] = y * fb_width + x, or nullptr
     uint32_t n_list;
     uint32_t tex_layer;         // InLayer of this pass's hits: TEX_WORLD or TEX_UI (also the TGT_TERM text's layer)
+    // A texture target's batch (aicb_texture_target_trace) instead of a pixel list: pixel task i is pick pick_base + i
+    // of the target's UpdateStrategy (pick_pixel; pixel_list is then the target's order, or nullptr for Consistent),
+    // and its texels are stored at the pixel's framebuffer position.
+    uint32_t picks;             // PICK_LIST (a pixel list, or none), PICK_INCREMENTAL or PICK_CONSISTENT
+    uint32_t pick_central;      // PixelPicker's central_pixel_count
+    uint64_t pick_base;
     // A frame has one target, so the fields of the other target share the space: the parameter block, and with it
     // the code of the kernels that read neither, keeps its size.
     union {
@@ -800,10 +806,30 @@ struct AuxState<true> {
 // A lane is marching, parked (waiting for the warp to serve its level switch / to take its result), or has no ray.
 enum LaneState : int { ST_IDLE = 0, ST_MARCH = 1, ST_ENTER = 2, ST_POP = 3, ST_DONE = 4, ST_EXHAUSTED = 5 };
 
+// A texture target's pick k (raytrace_to_texture.rs:700-727, 835-918), as a linear index y * width + x of a w x h
+// viewport.  Consistent: point_from_pixel_index(k) (:912-918), which wraps with rem_euclid / div_euclid.  Incremental:
+// PixelPicker::next, sorted_pixels[Interleave(Cycle(0..central), Cycle(central..n))] with `order` = sorted_pixels.
+// itertools' Interleave takes from its first iterator when its flag (toggled before every item) is set, from the second
+// otherwise, and from the other one whenever the one in turn is exhausted; a Cycle of an empty range is exhausted for
+// ever, so with central == 0 (n < 4) every pick comes from the rest, in turn.  The rest is never empty.
+// Out of line: its 64-bit divisions stay out of the code of gen_kernel, which every frame runs.
+constexpr uint32_t PICK_LIST = 0, PICK_INCREMENTAL = 1, PICK_CONSISTENT = 2;
+static __device__ __noinline__ uint32_t pick_pixel(uint32_t picks, const uint32_t *order, uint32_t central, uint32_t w,
+                                                   uint32_t h, uint64_t k) {
+    if (picks == PICK_CONSISTENT) return (uint32_t)(k % w + (k / w) % h * w);
+    const uint64_t n = (uint64_t)w * h;
+    uint64_t lin;
+    if (central == 0) lin = k % n;
+    else if (k & 1) lin = central + (k >> 1) % (n - central);
+    else lin = (k >> 1) % central;
+    return __ldg(order + lin);
+}
+
 // task -> pixel mapping shared by the three kernels: pixel tasks are tile-ordered (32 consecutive
 // pixel tasks = one 8x4 tile); returns false for the padding pixels of edge tiles.  With a pixel list (LIST
 // instantiations only, so that the kernels of other frames do not carry the branch) pixel task i is the listed pixel
-// and its outputs go to position i; a warp then takes 32 consecutive list entries.
+// and its outputs go to position i; a warp then takes 32 consecutive list entries.  A texture target's batch lists its
+// picks the same way, and its outputs go to the pixel's framebuffer position.
 template <bool LIST>
 AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px, uint32_t *py, size_t *out_index) {
     if (P.rays) {
@@ -811,12 +837,15 @@ AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px
         *out_index = pixel_task;
         return pixel_task < P.n_rays;
     }
-    if (LIST && P.target.pixel_list) {
+    if (LIST && P.target.n_list) {   // (a listed frame has entries: a pixel list or picks; no other frame has any)
         if (pixel_task >= P.target.n_list) return false;
-        const uint32_t v = __ldg(P.target.pixel_list + pixel_task);
+        const bool picked = P.target.picks != PICK_LIST;
+        const uint32_t v = picked ? pick_pixel(P.target.picks, P.target.pixel_list, P.target.pick_central, P.fb_width,
+                                               P.fb_height, P.target.pick_base + pixel_task)
+                                  : __ldg(P.target.pixel_list + pixel_task);
         *px = v % P.fb_width;
         *py = v / P.fb_width;
-        *out_index = pixel_task;
+        *out_index = picked ? v : pixel_task;
         return true;
     }
     const uint32_t tile = pixel_task >> 5, in_tile = pixel_task & 31;

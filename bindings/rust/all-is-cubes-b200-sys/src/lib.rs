@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 17 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 19 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -189,6 +189,31 @@ pub struct aicb_group {
 pub struct aicb_group_scene {
     _opaque: [u8; 0],
 }
+#[repr(C)]
+pub struct aicb_texture_target {
+    _opaque: [u8; 0],
+}
+#[repr(C)]
+pub struct aicb_group_texture_target {
+    _opaque: [u8; 0],
+}
+
+/// `UpdateStrategy` of a texture target (all-is-cubes-gpu/src/raytrace_to_texture.rs:704-727, 835-918)
+pub const AICB_TEXTURE_INCREMENTAL: c_int = 1;
+pub const AICB_TEXTURE_CONSISTENT: c_int = 2;
+
+/// a texture target's size, strategy, `dirty_pixels`, pick position and cycle length
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_texture_target_info {
+    pub width: u32,
+    pub height: u32,
+    pub strategy: u32,
+    pub _pad: u32,
+    pub dirty_pixels: u64,
+    pub next_pick: u64,
+    pub cycle_length: u64,
+}
 
 /// one layer of `RtScene::trace_ray_through_layers` (renderer.rs:454-478)
 #[repr(C)]
@@ -360,6 +385,41 @@ unsafe extern "C" {
                                        -> aicb_status;
     pub fn aicb_group_render_orthographic(gs: *mut aicb_group_scene, resolution: u32, out: *mut [u8; 4], out_len: usize,
                                           info: *mut aicb_render_info) -> aicb_status;
+
+    // RaytraceToTexture's state on the device: the strategy, dirty_pixels and both render targets (blocking calls)
+    pub fn aicb_texture_target_create(ctx: *mut aicb_ctx, width: u32, height: u32, strategy: c_int,
+                                      out: *mut *mut aicb_texture_target) -> aicb_status;
+    pub fn aicb_texture_target_destroy(t: *mut aicb_texture_target);
+    pub fn aicb_texture_target_resize(t: *mut aicb_texture_target, width: u32, height: u32) -> aicb_status;
+    pub fn aicb_texture_target_mark_dirty(t: *mut aicb_texture_target) -> aicb_status;
+    pub fn aicb_texture_target_trace(t: *mut aicb_texture_target, world: *const aicb_layer, ui: *const aicb_layer,
+                                     backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],
+                                     depth_transform: *const [f64; 16], n: usize, n_traced: *mut usize,
+                                     info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_texture_target_state(t: *const aicb_texture_target, out: *mut aicb_texture_target_info) -> aicb_status;
+    pub fn aicb_texture_target_picks(t: *mut aicb_texture_target, start: u64, n: usize, out: *mut u32) -> aicb_status;
+    pub fn aicb_texture_target_buffers(t: *mut aicb_texture_target, d_rgba16f: *mut *mut c_void,
+                                       d_depth: *mut *mut c_void) -> aicb_status;
+    pub fn aicb_texture_target_read(t: *mut aicb_texture_target, rgba16f: *mut [u16; 4], depth: *mut f32, n: usize)
+                                    -> aicb_status;
+    // the same on a device group: the targets are device 0's, a batch is cut into warp ranges across the devices
+    pub fn aicb_group_texture_target_create(g: *mut aicb_group, width: u32, height: u32, strategy: c_int,
+                                            out: *mut *mut aicb_group_texture_target) -> aicb_status;
+    pub fn aicb_group_texture_target_destroy(t: *mut aicb_group_texture_target);
+    pub fn aicb_group_texture_target_resize(t: *mut aicb_group_texture_target, width: u32, height: u32) -> aicb_status;
+    pub fn aicb_group_texture_target_mark_dirty(t: *mut aicb_group_texture_target) -> aicb_status;
+    pub fn aicb_group_texture_target_trace(t: *mut aicb_group_texture_target, world: *const aicb_group_layer,
+                                           ui: *const aicb_group_layer, backdrop_rgba: *const [f32; 4],
+                                           no_world_rgba: *const [f32; 4], depth_transform: *const [f64; 16], n: usize,
+                                           n_traced: *mut usize, info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_texture_target_state(t: *const aicb_group_texture_target, out: *mut aicb_texture_target_info)
+                                           -> aicb_status;
+    pub fn aicb_group_texture_target_picks(t: *mut aicb_group_texture_target, start: u64, n: usize, out: *mut u32)
+                                           -> aicb_status;
+    pub fn aicb_group_texture_target_buffers(t: *mut aicb_group_texture_target, d_rgba16f: *mut *mut c_void,
+                                             d_depth: *mut *mut c_void) -> aicb_status;
+    pub fn aicb_group_texture_target_read(t: *mut aicb_group_texture_target, rgba16f: *mut [u16; 4], depth: *mut f32,
+                                          n: usize) -> aicb_status;
 
     pub fn aicb_trace_rays(s: *mut aicb_scene, origin_dir: *const [f64; 6], n: usize, opt: *const aicb_options,
                            out_colorbuf: *mut [f32; 4], depth: *mut f64, hit: *mut aicb_hit, steps: *mut u32,

@@ -11,6 +11,8 @@
 //!   → `aicb_render_layers_srgb8`; the info text is drawn here over the returned pixels like renderer.rs:659-683.
 //! * `trace_texture_batch()` = the tracing of `RaytraceToTexture::do_some_tracing` (raytrace_to_texture.rs:591-683)
 //!   for a batch of pixels → `aicb_render_layers_texture`.
+//! * `trace_texture_target()` = a whole `do_some_tracing` call on a `B200TextureTarget`: the pick order,
+//!   `dirty_pixels` and both render targets stay on the device (`aicb_texture_target_trace`).
 //! * `draw_terminal()` = the desktop terminal's `RtRenderer<CharacterRtData>::draw::<ColorCharacterBuf>`
 //!   (all-is-cubes-desktop/src/terminal.rs:114-142, 341-394) → `aicb_render_layers_terminal`; the block indices it
 //!   returns are mapped to `CharacterRtData` strings from one table per layer, kept current with the scenes.
@@ -96,6 +98,124 @@ impl B200Group {
 impl Drop for B200Group {
     fn drop(&mut self) {
         unsafe { sys::aicb_group_destroy(self.0) }
+    }
+}
+
+/// The depth transform of `RaytraceToTexture::do_some_tracing` (raytrace_to_texture.rs:613-618), composed by euclid
+/// exactly as the reference composes it.
+fn depth_transform_of(camera: &Camera) -> [f64; 16] {
+    let depth_scale = -(camera.view_distance().into_inner() - camera.near_plane_distance().into_inner());
+    let depth_bias = -camera.near_plane_distance().into_inner();
+    camera
+        .projection_matrix()
+        .pre_translate(euclid::vec3(0., 0., depth_bias))
+        .pre_scale(0., 0., depth_scale)
+        .to_array()
+}
+
+#[derive(Clone, Copy, Debug)]
+enum TargetHandle {
+    Single(*mut sys::aicb_texture_target),
+    Group(*mut sys::aicb_group_texture_target),
+}
+
+/// The state `RaytraceToTexture::Inner` keeps around its tracing (all-is-cubes-gpu/src/raytrace_to_texture.rs), on the
+/// device (`aicb_texture_target_*`): the update strategy (`PixelPicker`'s order and position, or `Consistent`'s
+/// `next`), `dirty_pixels`, and the `Rgba16Float` and `R32Float` render targets.  With it `do_some_tracing` becomes
+/// `mark_dirty()` when `RtRenderer::update` reports a change, one `B200Renderer::trace_texture_target` per frame with
+/// the caller's `rays_per_frame` rule, and an upload of the texels from `buffers()` (device memory) or `read()`.
+#[derive(Debug)]
+pub struct B200TextureTarget {
+    handle: TargetHandle,
+    _backend: Backend, // the context or group the target's buffers live on, kept alive as long as the target
+}
+// SAFETY: the library holds the target's context locks in every call.
+unsafe impl Send for B200TextureTarget {}
+unsafe impl Sync for B200TextureTarget {}
+
+impl B200TextureTarget {
+    fn new(backend: &Backend, width: u32, height: u32, incremental: bool) -> Result<Self, B200Error> {
+        let strategy = if incremental { sys::AICB_TEXTURE_INCREMENTAL } else { sys::AICB_TEXTURE_CONSISTENT };
+        let handle = match backend {
+            Backend::Context(ctx) => {
+                let mut t = core::ptr::null_mut();
+                check(unsafe { sys::aicb_texture_target_create(ctx.0, width, height, strategy, &mut t) })?;
+                TargetHandle::Single(t)
+            }
+            Backend::Group(g) => {
+                let mut t = core::ptr::null_mut();
+                check(unsafe { sys::aicb_group_texture_target_create(g.0, width, height, strategy, &mut t) })?;
+                TargetHandle::Group(t)
+            }
+        };
+        Ok(Self { handle, _backend: backend.clone() })
+    }
+
+    /// `UpdateStrategy::resize` and the textures' resize (:311-324): nothing for the same size.
+    pub fn resize(&self, width: u32, height: u32) -> Result<(), B200Error> {
+        check(match self.handle {
+            TargetHandle::Single(t) => unsafe { sys::aicb_texture_target_resize(t, width, height) },
+            TargetHandle::Group(t) => unsafe { sys::aicb_group_texture_target_resize(t, width, height) },
+        })
+    }
+
+    /// `RaytraceToTexture::dirty` (:587-589).
+    pub fn mark_dirty(&self) -> Result<(), B200Error> {
+        check(match self.handle {
+            TargetHandle::Single(t) => unsafe { sys::aicb_texture_target_mark_dirty(t) },
+            TargetHandle::Group(t) => unsafe { sys::aicb_group_texture_target_mark_dirty(t) },
+        })
+    }
+
+    pub fn state(&self) -> Result<sys::aicb_texture_target_info, B200Error> {
+        let mut out = sys::aicb_texture_target_info::default();
+        check(match self.handle {
+            TargetHandle::Single(t) => unsafe { sys::aicb_texture_target_state(t, &mut out) },
+            TargetHandle::Group(t) => unsafe { sys::aicb_group_texture_target_state(t, &mut out) },
+        })?;
+        Ok(out)
+    }
+
+    /// The linear pixel indices of picks `start .. start + out.len()`: the texels a batch changed.
+    pub fn picks(&self, start: u64, out: &mut [u32]) -> Result<(), B200Error> {
+        check(match self.handle {
+            TargetHandle::Single(t) => unsafe { sys::aicb_texture_target_picks(t, start, out.len(), out.as_mut_ptr()) },
+            TargetHandle::Group(t) => unsafe {
+                sys::aicb_group_texture_target_picks(t, start, out.len(), out.as_mut_ptr())
+            },
+        })
+    }
+
+    /// Device pointers (the context's device, or the group's device 0) to the colour and depth texels, row-major;
+    /// valid until the next `resize` or the target's drop.
+    pub fn buffers(&self) -> Result<(*mut core::ffi::c_void, *mut core::ffi::c_void), B200Error> {
+        let (mut color, mut depth) = (core::ptr::null_mut(), core::ptr::null_mut());
+        check(match self.handle {
+            TargetHandle::Single(t) => unsafe { sys::aicb_texture_target_buffers(t, &mut color, &mut depth) },
+            TargetHandle::Group(t) => unsafe { sys::aicb_group_texture_target_buffers(t, &mut color, &mut depth) },
+        })?;
+        Ok((color, depth))
+    }
+
+    /// Copies of both render targets (`width * height` texels each, row-major).
+    pub fn read(&self, color: &mut [[u16; 4]], depth: &mut [f32]) -> Result<(), B200Error> {
+        assert_eq!(color.len(), depth.len(), "one depth texel per colour texel");
+        check(match self.handle {
+            TargetHandle::Single(t) => unsafe {
+                sys::aicb_texture_target_read(t, color.as_mut_ptr(), depth.as_mut_ptr(), color.len())
+            },
+            TargetHandle::Group(t) => unsafe {
+                sys::aicb_group_texture_target_read(t, color.as_mut_ptr(), depth.as_mut_ptr(), color.len())
+            },
+        })
+    }
+}
+impl Drop for B200TextureTarget {
+    fn drop(&mut self) {
+        match self.handle {
+            TargetHandle::Single(t) => unsafe { sys::aicb_texture_target_destroy(t) },
+            TargetHandle::Group(t) => unsafe { sys::aicb_group_texture_target_destroy(t) },
+        }
     }
 }
 
@@ -525,15 +645,7 @@ impl B200Renderer {
         color: &mut [[u16; 4]],
         depth: &mut [f32],
     ) -> Result<sys::aicb_render_info, B200Error> {
-        let camera = &cams.world;
-        // :613-618, composed by euclid exactly as the reference composes it
-        let depth_scale = -(camera.view_distance().into_inner() - camera.near_plane_distance().into_inner());
-        let depth_bias = -camera.near_plane_distance().into_inner();
-        let depth_transform = camera
-            .projection_matrix()
-            .pre_translate(euclid::vec3(0., 0., depth_bias))
-            .pre_scale(0., 0., depth_scale)
-            .to_array();
+        let depth_transform = depth_transform_of(&cams.world);
 
         let backdrop: Rgba = self.cameras.ui_view_state().backdrop;
         let backdrop_arr: [f32; 4] = backdrop.into();
@@ -558,6 +670,50 @@ impl B200Renderer {
             },
         ))?;
         Ok(info)
+    }
+
+    /// One `RaytraceToTexture::do_some_tracing` batch into a `B200TextureTarget` of this renderer's backend:
+    /// `rays_per_frame` picks from the target's update strategy, traced through the layers this renderer holds and
+    /// stored into the target's render targets on the device (`aicb_texture_target_trace`).  Returns the picks traced
+    /// (0 once `dirty_pixels` is 0) and the batch's info; the caller times the call for its `rays_per_frame` rule.
+    pub fn trace_texture_target(
+        &self,
+        target: &B200TextureTarget,
+        cams: &Layers<Camera>,
+        rays_per_frame: usize,
+    ) -> Result<(usize, sys::aicb_render_info), B200Error> {
+        let depth_transform = depth_transform_of(&cams.world);
+        let backdrop: Rgba = self.cameras.ui_view_state().backdrop;
+        let backdrop_arr: [f32; 4] = backdrop.into();
+        let backdrop_ptr: *const [f32; 4] = if backdrop == Rgba::TRANSPARENT { core::ptr::null() } else { &backdrop_arr };
+        let no_world: [f32; 4] = palette::NO_WORLD_TO_SHOW.into();
+        let mut info = sys::aicb_render_info::default();
+        let info_ptr: *mut sys::aicb_render_info = &mut info;
+        let mut traced = 0usize;
+        let traced_ptr: *mut usize = &mut traced;
+        check(self.with_layers(
+            cams,
+            |world, ui| match target.handle {
+                TargetHandle::Single(t) => unsafe {
+                    sys::aicb_texture_target_trace(t, world, ui, backdrop_ptr, &no_world, &depth_transform,
+                                                   rays_per_frame, traced_ptr, info_ptr)
+                },
+                TargetHandle::Group(_) => sys::AICB_ERR_INVALID,
+            },
+            |world, ui| match target.handle {
+                TargetHandle::Group(t) => unsafe {
+                    sys::aicb_group_texture_target_trace(t, world, ui, backdrop_ptr, &no_world, &depth_transform,
+                                                         rays_per_frame, traced_ptr, info_ptr)
+                },
+                TargetHandle::Single(_) => sys::AICB_ERR_INVALID,
+            },
+        ))?;
+        Ok((traced, info))
+    }
+
+    /// A `B200TextureTarget` on this renderer's context or group.
+    pub fn texture_target(&self, width: u32, height: u32, incremental: bool) -> Result<B200TextureTarget, B200Error> {
+        B200TextureTarget::new(&self.backend, width, height, incremental)
     }
 
     /// The desktop terminal's frame (all-is-cubes-desktop/src/terminal.rs:114-142), in place of

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 18
+#define AICB_ABI_VERSION 19
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -596,6 +596,86 @@ aicb_status aicb_group_render_layers_device(const aicb_group_layer *world_or_nul
                                             const uint32_t *d_pixels_or_null, size_t n_pixels,
                                             const aicb_device_outputs *outs, void *stream,
                                             aicb_render_info *info_or_null);
+
+/* ---------------------------------------------------------------------------------------------
+ * Texture targets: the state RaytraceToTexture::Inner keeps around trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs),
+ * on the device: the update strategy and its position, dirty_pixels, and the colour and depth render targets.  The
+ * RtRenderer is not part of it: the layers are passed to each trace, as aicb_render_layers_texture takes them.
+ * rays_per_frame and its 2 ms budget rule (:733-744) stay with the caller, which passes the batch size and times the
+ * call with its own clock.  Reprojection (UpdateStrategy::want_reprojection) is not offered: the reference never
+ * takes it (:140).
+ *   create: a w x h render viewport (w, h >= 1 and w * h <= 2^30 - 1; AICB_ERR_INVALID otherwise) with
+ *     AICB_TEXTURE_INCREMENTAL (PixelPicker, :835-918: the pixels stably sorted by their Chebyshev distance from the
+ *     centre plus a dither, the order built and kept on the device, 4 bytes per pixel) or AICB_TEXTURE_CONSISTENT
+ *     (`next`, :704-727; point_from_pixel_index wraps, :912-918).  Both targets hold zero bits (a new DrawableTexture),
+ *     the pick position is 0 and dirty_pixels = cycle_length (:188).
+ *   cycle_length: Incremental 2 * max(central, w * h - central) with central = min(60000, w * h / 4) (:877-886);
+ *     Consistent w * h.
+ *   mark_dirty: dirty_pixels = cycle_length (RaytraceToTexture::dirty, :587-589), for a host whose RtRenderer::update
+ *     reported a change.
+ *   resize (:311-324): the same size does nothing.  Another size makes new targets of zero bits and, for Incremental,
+ *     a new order whose pick position is 0 (PixelPicker::new); Consistent keeps its position.  dirty_pixels is left as
+ *     it is, as the reference leaves it.  A failed resize changes nothing.
+ *   trace (do_some_tracing, :591-745): with dirty_pixels == 0 nothing is traced and *n_traced = 0.  Otherwise picks
+ *     p .. p + n - 1 (p the pick position) are traced as aicb_render_layers_texture traces a pixel list, each pick's two
+ *     texels are stored at its framebuffer position in the targets (store_one, :685-690; a pixel picked twice in a
+ *     batch gets the same bits twice), p += n, dirty_pixels -= min(n, dirty_pixels), and *n_traced = n.  The picks are
+ *     computed by the kernel that lists the batch's rays: no pixel list and no texel crosses to or from the host.
+ *     AICB_ERR_INVALID: what aicb_render_layers_texture rejects, a camera whose framebuffer size is not the target's,
+ *     layers whose scenes are not on the target's context (of the target's group), or n > 2^30 - 1.
+ *   state: the size, the strategy, dirty_pixels, the pick position and cycle_length.
+ *   picks: the linear indices y * w + x of picks start .. start + n - 1, from the device code that feeds a batch.
+ *   buffers: device pointers, on the context's device, to the w * h texels of each target, row-major: the colour texels
+ *     as aicb_render_layers_texture's out_rgba16f (4 x f16 bits), the depth texels as its out_depth (f32); valid until
+ *     the next resize or destroy.  read: a copy of them (n must be w * h; either pointer may be NULL).
+ * Every call is blocking: it holds the target's context locks, issues on the context's stream and returns once its
+ * device work is done (a trace retries its hit stream inside).  Destroy a target before its context or group.
+ * GPU test: tests/test_gpu_texture_target.py. */
+enum { AICB_TEXTURE_INCREMENTAL = 1, AICB_TEXTURE_CONSISTENT = 2 };
+typedef struct aicb_texture_target aicb_texture_target;
+typedef struct aicb_texture_target_info {
+    uint32_t width, height;
+    uint32_t strategy;             /* AICB_TEXTURE_INCREMENTAL or AICB_TEXTURE_CONSISTENT */
+    uint32_t _pad;
+    uint64_t dirty_pixels;
+    uint64_t next_pick;            /* the pick position: PixelPicker's count of picks, or Consistent's `next` */
+    uint64_t cycle_length;
+} aicb_texture_target_info;
+aicb_status aicb_texture_target_create(aicb_ctx *, uint32_t width, uint32_t height, int strategy,
+                                       aicb_texture_target **out);
+void aicb_texture_target_destroy(aicb_texture_target *);
+aicb_status aicb_texture_target_resize(aicb_texture_target *, uint32_t width, uint32_t height);
+aicb_status aicb_texture_target_mark_dirty(aicb_texture_target *);
+aicb_status aicb_texture_target_trace(aicb_texture_target *, const aicb_layer *world_or_null,
+                                      const aicb_layer *ui_or_null, const float backdrop_rgba[4],
+                                      const float no_world_rgba[4], const double depth_transform[16], size_t n,
+                                      size_t *n_traced_or_null, aicb_render_info *info_or_null);
+aicb_status aicb_texture_target_state(const aicb_texture_target *, aicb_texture_target_info *out);
+aicb_status aicb_texture_target_picks(aicb_texture_target *, uint64_t start, size_t n, uint32_t *out);
+aicb_status aicb_texture_target_buffers(aicb_texture_target *, void **d_rgba16f, void **d_depth);
+aicb_status aicb_texture_target_read(aicb_texture_target *, uint16_t (*rgba16f_or_null)[4], float *depth_or_null,
+                                     size_t n);
+
+/* The texture target on a device group, with the same semantics, state and results: the order and both targets live
+ * on device 0; a batch is cut into contiguous ranges of whole 32-pick warps, one per device, as
+ * aicb_group_render_layers_texture cuts a pixel list, every device computes its own picks (reading device 0's order
+ * over peer access) and stores its texels straight into device 0's targets.  The layers must be scenes of the target's
+ * group.  Every call holds every context of the group. */
+typedef struct aicb_group_texture_target aicb_group_texture_target;
+aicb_status aicb_group_texture_target_create(aicb_group *, uint32_t width, uint32_t height, int strategy,
+                                             aicb_group_texture_target **out);
+void aicb_group_texture_target_destroy(aicb_group_texture_target *);
+aicb_status aicb_group_texture_target_resize(aicb_group_texture_target *, uint32_t width, uint32_t height);
+aicb_status aicb_group_texture_target_mark_dirty(aicb_group_texture_target *);
+aicb_status aicb_group_texture_target_trace(aicb_group_texture_target *, const aicb_group_layer *world_or_null,
+                                            const aicb_group_layer *ui_or_null, const float backdrop_rgba[4],
+                                            const float no_world_rgba[4], const double depth_transform[16], size_t n,
+                                            size_t *n_traced_or_null, aicb_render_info *info_or_null);
+aicb_status aicb_group_texture_target_state(const aicb_group_texture_target *, aicb_texture_target_info *out);
+aicb_status aicb_group_texture_target_picks(aicb_group_texture_target *, uint64_t start, size_t n, uint32_t *out);
+aicb_status aicb_group_texture_target_buffers(aicb_group_texture_target *, void **d_rgba16f, void **d_depth);
+aicb_status aicb_group_texture_target_read(aicb_group_texture_target *, uint16_t (*rgba16f_or_null)[4],
+                                           float *depth_or_null, size_t n);
 
 /* == SpaceRaytracer::trace_ray (sr.rs:113-120) for a batch of explicit rays:
  * origin_dir[i] = {ox,oy,oz,dx,dy,dz}. Output as aicb_render_colorbuf. */
