@@ -139,6 +139,7 @@ def load_library() -> C.CDLL:
                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, outs, C.c_void_p,
                                                     C.POINTER(abi.RenderInfo)]
     lib.aicb_group_light_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
+    lib.aicb_derive_block_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     # the calls of _Scene: a group scene's form of aicb_<name> is aicb_group_<name>, with the same arguments
     u64, u8, size = C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_size_t)
     info = C.POINTER(abi.RenderInfo)
@@ -516,9 +517,33 @@ class Block:
         self.light_emission = tuple(float(v) for v in (all_em / surface)) if count else (0.0, 0.0, 0.0)
         self.light_visible = bool((vox[..., 3] != 0).any() or (vox[..., 4:7] != 0).any())
 
+    def set_light_data(self, bl: "BlockLight"):
+        """Take compute_derived's light fields (Context.derive_block_light) in place of the numpy restatement."""
+        self.light_face_colors = list(bl.face_colors)
+        self.light_color = bl.color
+        self.light_emission = bl.emission
+        self.light_opaque_faces = bl.opaque_faces
+        self.light_visible = bl.visible
+
     @staticmethod
     def air() -> "Block":
         return Block(is_air=True)
+
+
+@dataclasses.dataclass(frozen=True)
+class BlockLight:
+    """compute_derived's light fields of one block (block/eval/derived.rs:80-216): the face colours NX..PZ, colour and
+    emission, the faces opaque to light (bit face - 1) and Derived::visible."""
+    face_colors: tuple
+    color: tuple
+    emission: tuple
+    opaque_faces: int
+    visible: bool
+
+    @staticmethod
+    def from_abi(o: abi.BlockLight) -> "BlockLight":
+        return BlockLight(face_colors=tuple(tuple(o.face_colors[f][:]) for f in range(6)), color=tuple(o.color[:]),
+                          emission=tuple(o.emission[:]), opaque_faces=int(o.opaque_faces), visible=bool(o.visible))
 
 
 class Space:
@@ -671,6 +696,17 @@ class Context:
         if cls._default is None:
             cls._default = Context(-1)
         return cls._default
+
+    def derive_block_light(self, blocks: Sequence[Block]) -> list:
+        """compute_derived's light fields of every block on this context's device (aicb_derive_block_light), one
+        BlockLight per block.  Raises AicbError (ERR_INVALID) for a block scene creation rejects, or where the
+        reference's colour or emission sum is NaN and it panics."""
+        if not blocks:
+            return []
+        descs = _block_descs(blocks)
+        out = (abi.BlockLight * len(blocks))()
+        _check(load_library().aicb_derive_block_light(self.handle, descs, len(blocks), out))
+        return [BlockLight.from_abi(o) for o in out]
 
     def close(self):
         if self.handle:

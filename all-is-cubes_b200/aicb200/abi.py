@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 19
+ABI_VERSION = 20
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -36,6 +36,18 @@ class BlockDesc(C.Structure):
         ("light_color", C.c_float * 4),
         ("light_emission", C.c_float * 3),
         ("_pad", C.c_float),
+    ]
+
+
+class BlockLight(C.Structure):
+    """aicb_block_light: compute_derived's light fields of one block, as aicb_block_desc's light_* members take them."""
+    _fields_ = [
+        ("face_colors", (C.c_float * 4) * 6),
+        ("color", C.c_float * 4),
+        ("emission", C.c_float * 3),
+        ("opaque_faces", C.c_uint8),
+        ("visible", C.c_uint8),
+        ("_pad", C.c_uint8 * 2),
     ]
 
 
@@ -155,6 +167,7 @@ EXPORTED_SYMBOLS = [
     "aicb_ctx_stage_timing",
     "aicb_ctx_device",
     "aicb_last_error",
+    "aicb_derive_block_light",
     "aicb_scene_create",
     "aicb_scene_update_cubes",
     "aicb_scene_update_region",

@@ -134,8 +134,10 @@ def light_to_value(texels, queue=None):
     return gz_encode(out.tobytes())
 
 
-def space_from_value(v, resolve_space=None) -> Space:
-    """A `SpaceV1` value (the parsed JSON object) -> Space."""
+def space_from_value(v, resolve_space=None, ctx=None) -> Space:
+    """A `SpaceV1` value (the parsed JSON object) -> Space.  With a Context `ctx`, the light data of its recursive
+    blocks is compute_derived's, computed on that context's device (Context.derive_block_light), instead of the
+    numpy restatement Block computes."""
     if v.get("type") != "SpaceV1":
         raise ValueError(f"not a SpaceV1 value: {v.get('type')}")
     lower = [int(c) for c in v["bounds"]["lower"]]
@@ -148,6 +150,10 @@ def space_from_value(v, resolve_space=None) -> Space:
     blocks = [_block_of(b, resolve_space) for b in v["blocks"]]
     if ids.size and int(ids.max()) >= len(blocks):
         raise ValueError("block index out of range")   # (save/tests.rs:749-785 space_de_invalid_index)
+    if ctx is not None:
+        recursive = [b for b in blocks if b.indices is not None]
+        for b, bl in zip(recursive, ctx.derive_block_light(recursive)):
+            b.set_light_data(bl)
     physics = v["physics"]
     sky = physics["sky"]
     if sky["type"] == "UniformV1":
@@ -165,8 +171,9 @@ def space_from_value(v, resolve_space=None) -> Space:
                  light_max_distance=max_distance)
 
 
-def spaces_from_universe(u) -> dict:
-    """A `UniverseV1` value -> {name key: Space} for every Space member that can be ingested (voxel Spaces first)."""
+def spaces_from_universe(u, ctx=None) -> dict:
+    """A `UniverseV1` value -> {name key: Space} for every Space member that can be ingested (voxel Spaces first);
+    `ctx` as space_from_value takes it."""
     if u.get("type") != "UniverseV1":
         raise ValueError(f"not a UniverseV1 value: {u.get('type')}")
     raw = {name_key(m["name"]): m["value"] for m in u["members"] if m.get("member_type") == "Space"}
@@ -179,7 +186,7 @@ def spaces_from_universe(u) -> dict:
         if key in in_progress or key not in raw:
             raise UnsupportedBlock(f"Space {key} is missing or refers to itself")
         in_progress.add(key)
-        done[key] = space_from_value(raw[key], resolve)
+        done[key] = space_from_value(raw[key], resolve, ctx)
         in_progress.discard(key)
         return done[key]
 
@@ -192,9 +199,9 @@ def spaces_from_universe(u) -> dict:
     return out
 
 
-def load_universe(path) -> dict:
+def load_universe(path, ctx=None) -> dict:
     with open(path, "rb") as f:
         data = f.read()
     if data[:2] == b"\x1f\x8b":
         data = gzip.decompress(data)
-    return spaces_from_universe(json.loads(data))
+    return spaces_from_universe(json.loads(data), ctx)

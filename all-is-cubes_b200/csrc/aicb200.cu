@@ -123,42 +123,48 @@ static float4 block_entry(uint8_t kind, uint32_t pal_off, const std::vector<floa
     return make_float4(e.x, e.y, palf, 0.0f);
 }
 
+aicb_status check_block_desc(const aicb_block_desc &b) {
+    const uint32_t res = b.resolution;
+    if (res == 0 || (res & (res - 1)) || res > 128) return fail(AICB_ERR_INVALID, "block resolution must be 1..128, power of 2");
+    if (b.indices == nullptr) {
+        if (b.n_palette && !b.palette) return fail(AICB_ERR_INVALID, "palette is NULL");
+        return AICB_OK;
+    }
+    const uint64_t nvox = (uint64_t)b.voxel_bounds.size[0] * b.voxel_bounds.size[1] * b.voxel_bounds.size[2];
+    if (nvox != b.n_indices) return fail(AICB_ERR_INVALID, "n_indices does not match voxel_bounds");
+    for (int a = 0; a < 3; a++) {
+        int64_t lo = b.voxel_bounds.lower[a], hi = lo + (int64_t)b.voxel_bounds.size[a];
+        if (lo < 0 || hi > (int64_t)res) return fail(AICB_ERR_INVALID, "voxel_bounds must lie within [0, resolution)^3");
+    }
+    if (!b.palette && b.n_palette) return fail(AICB_ERR_INVALID, "palette is NULL");
+    for (size_t k = 0; k < b.n_indices; k++)
+        if (b.indices[k] >= b.n_palette) return fail(AICB_ERR_INVALID, "voxel index out of palette range");
+    if (!b.is_air && res != 1 && b.n_palette > 65536)
+        return fail(AICB_ERR_UNSUPPORTED, "block palettes above 65536 entries are not supported: a voxel's palette "
+                                          "index (VoxelIndex) is 16 bits");
+    return AICB_OK;
+}
+
+aicb_voxel single_voxel_of(const aicb_block_desc &b) {
+    if (b.indices == nullptr) return b.n_palette ? b.palette[0] : AIR_VOXEL;
+    // single_voxel_or_palette (voxel_storage.rs:371-383)
+    const bool at_origin = b.n_indices == 1 && b.voxel_bounds.lower[0] == 0 && b.voxel_bounds.lower[1] == 0 &&
+                           b.voxel_bounds.lower[2] == 0;
+    return at_origin ? b.palette[b.indices[0]] : AIR_VOXEL;
+}
+
 static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t &kind, std::vector<uint32_t> &bricks,
                                  std::vector<float4> &palette, std::vector<float2> &pal_tab) {
     std::memset(&r, 0, sizeof r);
+    TRY(check_block_desc(b));
     const uint32_t res = b.resolution;
-    if (res == 0 || (res & (res - 1)) || res > 128) return fail(AICB_ERR_INVALID, "block resolution must be 1..128, power of 2");
     auto push_voxel = [&](const aicb_voxel &v) {
         palette.push_back(make_float4(v.rgba[0], v.rgba[1], v.rgba[2], v.rgba[3]));
         palette.push_back(make_float4(v.emission[0], v.emission[1], v.emission[2], 0.0f));
         pal_tab.push_back(surface_entry(v.rgba[3]));
     };
-    bool single = false;
-    aicb_voxel sv = AIR_VOXEL;
-    if (b.indices == nullptr) {
-        single = true;
-        if (b.n_palette) {
-            if (!b.palette) return fail(AICB_ERR_INVALID, "palette is NULL");
-            sv = b.palette[0];
-        }
-    } else {
-        const uint64_t nvox = (uint64_t)b.voxel_bounds.size[0] * b.voxel_bounds.size[1] * b.voxel_bounds.size[2];
-        if (nvox != b.n_indices) return fail(AICB_ERR_INVALID, "n_indices does not match voxel_bounds");
-        for (int a = 0; a < 3; a++) {
-            int64_t lo = b.voxel_bounds.lower[a], hi = lo + (int64_t)b.voxel_bounds.size[a];
-            if (lo < 0 || hi > (int64_t)res) return fail(AICB_ERR_INVALID, "voxel_bounds must lie within [0, resolution)^3");
-        }
-        if (!b.palette && b.n_palette) return fail(AICB_ERR_INVALID, "palette is NULL");
-        for (size_t k = 0; k < b.n_indices; k++)
-            if (b.indices[k] >= b.n_palette) return fail(AICB_ERR_INVALID, "voxel index out of palette range");
-        if (res == 1) {
-            // single_voxel_or_palette (voxel_storage.rs:371-383)
-            single = true;
-            sv = (nvox == 1 && b.voxel_bounds.lower[0] == 0 && b.voxel_bounds.lower[1] == 0 && b.voxel_bounds.lower[2] == 0)
-                     ? b.palette[b.indices[0]]
-                     : AIR_VOXEL;
-        }
-    }
+    const bool single = is_single_voxel(b);
+    const aicb_voxel sv = single ? single_voxel_of(b) : AIR_VOXEL;
     if (b.is_air) {
         kind = KIND_INVISIBLE;
         r.kind_res = KIND_INVISIBLE | (1u << 8);
@@ -169,9 +175,6 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
         r.vsize[0] = r.vsize[1] = r.vsize[2] = 1;
         push_voxel(sv);
     } else {
-        if (b.n_palette > 65536)
-            return fail(AICB_ERR_UNSUPPORTED, "block palettes above 65536 entries are not supported: a voxel's palette "
-                                              "index (VoxelIndex) is 16 bits");
         kind = KIND_RECURSIVE;
         r.kind_res = KIND_RECURSIVE | (res << 8);
         for (int a = 0; a < 3; a++) {

@@ -214,6 +214,7 @@ struct aicb_ctx {
     DeviceBuffer d_task_depth;   // per task: the UI pass's DepthBuf for the world pass (aicb_render_layers_texture)
     DeviceBuffer d_task_text;    // per task: the UI pass's CharacterBuf for the world pass (aicb_render_layers_terminal)
     LightChart light_chart;
+    DeviceBuffer d_derive;       // aicb_derive_block_light's per-palette-entry and per-ray terms and its results
     std::mutex mu;
 };
 
@@ -366,6 +367,13 @@ aicb_status aicb_trace_pass(FramePart *parts, size_t n_parts, const aicb_camera 
                             bool want_info, const std::vector<Delivery> &copies);
 void aicb_merge_info(aicb_render_info *sum, const aicb_render_info *one, bool same_part);
 }
+
+// aicb200.cu: a block definition as scene creation accepts it (AICB_ERR_INVALID, or AICB_ERR_UNSUPPORTED for a palette
+// the brick pool cannot index); and, for a valid one, whether its voxels are Evoxels::single_voxel (voxel_storage.rs:364)
+// and that voxel.
+aicb_status check_block_desc(const aicb_block_desc &b);
+inline bool is_single_voxel(const aicb_block_desc &b) { return b.indices == nullptr || b.resolution == 1; }
+aicb_voxel single_voxel_of(const aicb_block_desc &b);
 
 // light.cu: the light-side record of a block definition.
 LightBlockDev light_block(const aicb_block_desc &b);

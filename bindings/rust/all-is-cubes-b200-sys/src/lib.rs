@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 19 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 20 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -58,6 +58,19 @@ pub struct aicb_block_desc {
     pub light_color: [f32; 4],
     pub light_emission: [f32; 3],
     pub _pad: f32,
+}
+
+/// `compute_derived`'s light fields of one block (block/eval/derived.rs:80-216), as `aicb_block_desc`'s `light_*`
+/// members take them; `opaque_faces` has bit (face - 1) per face NX..PZ.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_block_light {
+    pub face_colors: [[f32; 4]; 6],
+    pub color: [f32; 4],
+    pub emission: [f32; 3],
+    pub opaque_faces: u8,
+    pub visible: u8,
+    pub _pad: [u8; 2],
 }
 
 /// `Sky` (space/sky.rs:16-21): kind 0 = Uniform(colors[0]), 1 = Octants
@@ -323,6 +336,9 @@ unsafe extern "C" {
     pub fn aicb_frame_timed_out(ctx: *mut aicb_ctx, d_frame: *mut c_void, n_pixels: usize, out: *mut u32) -> aicb_status;
     pub fn aicb_ctx_stage_timing(ctx: *mut aicb_ctx, enable: c_int) -> aicb_status;
     pub fn aicb_ctx_device(ctx: *const aicb_ctx) -> c_int;
+    // compute_derived's light fields of n blocks (blocking; writes `out` only on success)
+    pub fn aicb_derive_block_light(ctx: *mut aicb_ctx, descs: *const aicb_block_desc, n: usize,
+                                   out: *mut aicb_block_light) -> aicb_status;
 
     pub fn aicb_group_create(device_ids: *const c_int, n_devices: c_int, out: *mut *mut aicb_group) -> aicb_status;
     pub fn aicb_group_destroy(g: *mut aicb_group);

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 19
+#define AICB_ABI_VERSION 20
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -196,6 +196,30 @@ aicb_status aicb_ctx_stage_timing(aicb_ctx *, int enable);
 int aicb_ctx_device(const aicb_ctx *);
 /* Thread-local message for the last failing call on this thread. Never NULL. */
 const char *aicb_last_error(void);
+
+/* ---------------------------------------------------------------------------------------------
+ * Block evaluation: the light fields of EvaluatedBlock's derived data
+ * ------------------------------------------------------------------------------------------- */
+/* compute_derived (block/eval/derived.rs:80-216) of one block's voxels, the fields aicb_block_desc::light_* take. */
+typedef struct aicb_block_light {
+    float face_colors[6][4];   /* NX..PZ, what aicb_block_desc::light_face_colors takes */
+    float color[4];
+    float emission[3];
+    uint8_t opaque_faces;      /* bit (face-1), as light_opaque_faces */
+    uint8_t visible;
+    uint8_t _pad[2];
+} aicb_block_light;
+/* == compute_derived (block/eval/derived.rs:80-216) for the light fields; reads only the voxel fields of descs.
+ * A single voxel (indices == NULL, or resolution 1) gives its own colour and emission.  Any other block is traced on the
+ * context's device: trace_for_eval (raytracer_components.rs:174-200) from every voxel face of the data bounds' six
+ * sides, summed per face in iproduct!'s order, with the reference's f32 arithmetic (no contraction, the correctly
+ * rounded powf).  `visible` is Derived::visible; EvaluatedBlock::visible_or_animated, which light_visible is, also
+ * holds for blocks with an animation hint, which the caller ORs in.  is_air plays no part.
+ * Blocks, runs on the context's stream after its queued work, and writes `out` only if it succeeds.  n == 0 does
+ * nothing.  AICB_ERR_INVALID: a NULL pointer with n > 0, a block scene creation rejects (its status, so also
+ * AICB_ERR_UNSUPPORTED for a palette over 65536 entries), or a colour or emission sum that is NaN (or negative) where
+ * the reference's Rgb::try_from(..).expect(..) panics, with the block's position in aicb_last_error. */
+aicb_status aicb_derive_block_light(aicb_ctx *, const aicb_block_desc *descs, size_t n, aicb_block_light *out);
 
 /* ---------------------------------------------------------------------------------------------
  * update(): replaces SpaceRaytracer::new / UpdatingSpaceRaytracer::update
