@@ -172,6 +172,13 @@ def load_library() -> C.CDLL:
         "light_download_queue": [C.c_void_p, C.c_void_p, C.c_size_t, size],
         "light_changes_count": [C.c_void_p, size],
         "light_take_changes": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, size],
+        "scene_update_cubes_device": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
+        "scene_update_region_device": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, C.c_void_p, C.c_void_p],
+        "scene_upload_light_device": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
+        "scene_download_ids_device": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
+        "light_edit_cubes_device": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, size, C.c_void_p],
+        "light_edit_region_device": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, size, C.c_void_p],
+        "light_download_device": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
     }.items():
         for prefix in ("aicb_", "aicb_group_"):
             getattr(lib, prefix + name).argtypes = argtypes
@@ -864,7 +871,62 @@ class _Scene:
             self._fn("scene_destroy")(self.handle)
             self.handle = C.c_void_p()
 
+    # ---- arrays in device memory: a CUDA tensor where a numpy array goes, read on the device (aicb_*_device) ----
+    def _tensor(self, x, dtype, shape, name):
+        """x as a device call takes it: a contiguous tensor of `dtype` and `shape` on the scene's device (device 0 of a
+        group); ValueError otherwise."""
+        device = self._device()
+        if (not _is_cuda_tensor(x) or x.dtype != dtype or x.device != device or not x.is_contiguous()
+                or tuple(x.shape) != tuple(shape)):
+            kind = str(dtype).replace("torch.", "")
+            raise ValueError(f"{name} must be a contiguous {kind} tensor {list(shape)} on {device}")
+        return x
+
+    def _cube_list(self, cubes, block_ids, light=None):
+        """A device call's cube list: int32 [n, 3] cubes, uint16 [n] ids, uint8 [n, 4] light or None."""
+        torch = _torch()
+        n = cubes.shape[0] if _is_cuda_tensor(cubes) and cubes.dim() == 2 else -1
+        c = self._tensor(cubes, torch.int32, (n, 3), "cubes")
+        ids = self._tensor(block_ids, torch.uint16, (n,), "block_ids")
+        lt = None if light is None else self._tensor(light, torch.uint8, (n, 4), "light")
+        return c, ids, lt, n
+
+    def _region_device(self, lower, size, block_ids):
+        """_region with the ids a uint16 tensor of shape `size` on the scene's device, or one id."""
+        region = abi.Aab()
+        region.lower[:] = [int(v) for v in lower]
+        region.size[:] = [int(v) for v in size]
+        if not _is_cuda_tensor(block_ids) and np.ndim(block_ids) == 0:
+            return region, None, int(block_ids)
+        return region, self._tensor(block_ids, _torch().uint16, tuple(region.size), "block_ids"), 0
+
+    def block_ids(self, device: bool = False):
+        """Each cube's block id, shaped like the Space, decoded from the scene's cells: a numpy uint16 array, or with
+        device=True a uint16 tensor on the scene's device (device 0 of a group), ordered before the work queued
+        afterwards on its current torch stream."""
+        torch = _torch()
+        dev = self._device()
+        out = torch.empty(self.space.size, dtype=torch.uint16 if device else torch.int16, device=dev)
+        _check(self._fn("scene_download_ids_device")(self.handle, out.data_ptr(), out.numel(), _stream(dev)))
+        return out if device else out.cpu().numpy().view(np.uint16)
+
+    def _light_download_device(self):
+        torch = _torch()
+        dev = self._device()
+        out = torch.empty(self.space.size + (4,), dtype=torch.uint8, device=dev)
+        _check(self._fn("light_download_device")(self.handle, out.data_ptr(), out.numel() // 4, _stream(dev)))
+        return out
+
     def update_cubes(self, cubes: np.ndarray, block_ids: np.ndarray, light: Optional[np.ndarray] = None):
+        """SpaceChange::CubeBlock / CubeLight for a list of cubes; the last entry for a cube wins.  CUDA tensors (int32
+        [n, 3], uint16 [n], uint8 [n, 4]) on the scene's device are read where they are, after the work queued on its
+        current torch stream."""
+        if _is_cuda_tensor(cubes):
+            c, ids, lt, n = self._cube_list(cubes, block_ids, light)
+            _check(self._fn("scene_update_cubes_device")(self.handle, c.data_ptr(), ids.data_ptr(),
+                                                         lt.data_ptr() if lt is not None else None, n,
+                                                         _stream(self._device())))
+            return
         c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
         ids = np.ascontiguousarray(block_ids, dtype=np.uint16)
         lt = None if light is None else np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
@@ -886,7 +948,16 @@ class _Scene:
 
     def update_region(self, lower, size, block_ids, light: Optional[np.ndarray] = None):
         """SpaceChange::CubeBlock (and CubeLight) for every cube of the box (lower, size): update_cubes' box form.
-        block_ids: one id for every cube, or an array of shape `size`; light: texels of shape size + (4,), or None."""
+        block_ids: one id for every cube, or an array of shape `size`; light: texels of shape size + (4,), or None.
+        Either array may be a CUDA tensor on the scene's device (uint16, uint8), then both are."""
+        if _is_cuda_tensor(block_ids) or _is_cuda_tensor(light):
+            region, ids, uniform = self._region_device(lower, size, block_ids)
+            lt = None if light is None else self._tensor(light, _torch().uint8, tuple(region.size) + (4,), "light")
+            _check(self._fn("scene_update_region_device")(self.handle, C.byref(region),
+                                                          None if ids is None else ids.data_ptr(), uniform,
+                                                          None if lt is None else lt.data_ptr(),
+                                                          _stream(self._device())))
+            return
         region, ids, uniform = self._region(lower, size, block_ids)
         lt = None if light is None else np.ascontiguousarray(light, dtype=np.uint8)
         if lt is not None and lt.shape != tuple(region.size) + (4,):
@@ -914,6 +985,13 @@ class _Scene:
         _check(self._fn("scene_fill_uniform")(self.handle, arr))
 
     def upload_light(self, light: np.ndarray):
+        """The whole light volume replaced; a CUDA tensor (uint8, Z-major texels) on the scene's device is copied on the
+        device."""
+        if _is_cuda_tensor(light):
+            lt = self._tensor(light, _torch().uint8, tuple(light.shape), "light")
+            _check(self._fn("scene_upload_light_device")(self.handle, lt.data_ptr(), lt.numel() // 4,
+                                                         _stream(self._device())))
+            return
         lt = np.ascontiguousarray(light, dtype=np.uint8).reshape(-1, 4)
         _check(self._fn("scene_upload_light")(self.handle, lt.ctypes.data, lt.shape[0]))
 
@@ -975,7 +1053,14 @@ class _Scene:
     def light_edit_cubes(self, cubes: np.ndarray, block_ids: np.ndarray) -> int:
         """Mutation::set(cubes[i], block_ids[i]) in list order, without propagation (light_evaluate or
         light_update_from_queue follows).  A cube may be named more than once.  Returns the number of entries whose id
-        differs from the block their cube holds at that point of the list."""
+        differs from the block their cube holds at that point of the list.  CUDA tensors (int32 [n, 3], uint16 [n]) on
+        the scene's device are checked and staged on the device."""
+        if _is_cuda_tensor(cubes):
+            c, ids, _, n = self._cube_list(cubes, block_ids)
+            m = C.c_size_t(0)
+            _check(self._fn("light_edit_cubes_device")(self.handle, c.data_ptr(), ids.data_ptr(), n, C.byref(m),
+                                                       _stream(self._device())))
+            return int(m.value)
         c = np.ascontiguousarray(cubes, dtype=np.int32).reshape(-1, 3)
         ids = np.ascontiguousarray(block_ids, dtype=np.uint16).reshape(-1)
         if ids.shape[0] != c.shape[0]:
@@ -996,7 +1081,14 @@ class _Scene:
     def light_edit_region(self, lower, size, block_ids) -> int:
         """Mutation::fill / fill_uniform over the box (lower, size): Mutation::set for every cube, without propagation
         (light_evaluate follows).  block_ids: one id, or an array of shape `size` (a cube the fill leaves alone gets the
-        id it holds).  Returns the number of cubes whose block changed."""
+        id it holds; a CUDA uint16 tensor on the scene's device is read there).  Returns the number of cubes whose block
+        changed."""
+        if _is_cuda_tensor(block_ids):
+            region, ids, uniform = self._region_device(lower, size, block_ids)
+            n = C.c_size_t(0)
+            _check(self._fn("light_edit_region_device")(self.handle, C.byref(region), ids.data_ptr(), uniform, C.byref(n),
+                                                        _stream(self._device())))
+            return int(n.value)
         region, ids, uniform = self._region(lower, size, block_ids)
         n = C.c_size_t(0)
         _check(self._fn("light_edit_region")(self.handle, C.byref(region), None if ids is None else ids.ctypes.data,
@@ -1099,7 +1191,14 @@ class SpaceRaytracer(_Scene):
                                       want_steps, out, _ctx_device(self.ctx), None)
         return _trace_rays(self, origin_dir, self.graphics_options.to_abi(include_sky), want_depth, want_hit, want_steps)
 
-    def light_download(self) -> np.ndarray:
+    def _device(self):
+        return _ctx_device(self.ctx)
+
+    def light_download(self, device: bool = False):
+        """The light volume, shaped like the Space + (4,): numpy, or with device=True a uint8 tensor on the scene's
+        device, ordered before the work queued afterwards on its current torch stream."""
+        if device:
+            return self._light_download_device()
         out = np.zeros(self.space.size + (4,), dtype=np.uint8)
         _check(load_library().aicb_light_download(self.handle, out.ctypes.data, out.size // 4))
         return out
@@ -1520,8 +1619,16 @@ class GroupScene(_Scene):
         _check(load_library().aicb_group_scene_create(group.handle, C.byref(desc), C.byref(self.handle)))
         del keep
 
-    def light_download(self, replica: int = 0) -> np.ndarray:
-        """The light volume of one replica (they are identical after every light call)."""
+    def _device(self):
+        return self.group._device()
+
+    def light_download(self, replica: int = 0, device: bool = False):
+        """The light volume of one replica (they are identical after every light call); device=True: replica 0's, as
+        a tensor on device 0."""
+        if device:
+            if replica != 0:
+                raise ValueError("device=True downloads replica 0")
+            return self._light_download_device()
         out = np.zeros(self.space.size + (4,), dtype=np.uint8)
         _check(load_library().aicb_group_light_download(self.handle, replica, out.ctypes.data, out.size // 4))
         return out

@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 20
+ABI_VERSION = 21
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -178,6 +178,13 @@ EXPORTED_SYMBOLS = [
     "aicb_scene_destroy",
     "aicb_scene_device_bytes",
     "aicb_scene_set_physics",
+    "aicb_scene_update_cubes_device",
+    "aicb_scene_update_region_device",
+    "aicb_scene_upload_light_device",
+    "aicb_scene_download_ids_device",
+    "aicb_light_edit_cubes_device",
+    "aicb_light_edit_region_device",
+    "aicb_light_download_device",
     "aicb_shard_pixel_count",
     "aicb_render_srgb8",
     "aicb_render_rgba16f",
@@ -239,6 +246,13 @@ EXPORTED_SYMBOLS = [
     "aicb_group_scene_set_physics",
     "aicb_group_scene_append_blocks",
     "aicb_group_scene_fill_uniform",
+    "aicb_group_scene_update_cubes_device",
+    "aicb_group_scene_update_region_device",
+    "aicb_group_scene_upload_light_device",
+    "aicb_group_scene_download_ids_device",
+    "aicb_group_light_edit_cubes_device",
+    "aicb_group_light_edit_region_device",
+    "aicb_group_light_download_device",
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",
     "aicb_group_render_layers_terminal",

@@ -16,6 +16,7 @@
 #include <vector>
 
 #include <cuda_runtime.h>
+#include <cub/device/device_radix_sort.cuh>
 
 #include "brick_room.h"
 #include "host_tables.h"
@@ -1375,6 +1376,7 @@ aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uin
         const auto [at, first] = seen.emplace(op.idx, (uint32_t)ops.size());
         if (first) ops.push_back(op); else ops[at->second] = op;
     }
+    TRY(refresh_mirror(r.scene[0]));   // (the mirror is written below)
     const uint32_t m = (uint32_t)ops.size();
     const size_t bytes = (size_t)m * sizeof(CubeDelta);
     for (size_t k = 0; k < r.n; k++) {
@@ -1395,8 +1397,7 @@ aicb_status scenes_update_cubes(Replicas r, const int32_t (*cubes)[3], const uin
     return AICB_OK;
 }
 
-aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
-                         RegionBox *box) {
+aicb_status check_box(const aicb_scene *s, const aicb_aab *region, RegionBox *box) {
     if (!region) return fail(AICB_ERR_INVALID, "NULL argument");
     for (int a = 0; a < 3; a++) {
         const int64_t lo = (int64_t)region->lower[a] - s->ds.lo[a];
@@ -1408,6 +1409,12 @@ aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint
     // the kernels' work items, at most size[2] / 4 + 2 per row, are counted in 32 bits
     if ((uint64_t)box->size[0] * box->size[1] * (box->size[2] / 4 + 2) > 0xffffffffull)
         return fail(AICB_ERR_INVALID, "region too large");
+    return AICB_OK;
+}
+
+aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                         RegionBox *box) {
+    TRY(check_box(s, region, box));
     const size_t count = s->host->block_count();
     if (!ids) {
         if (uniform_id >= count) return fail(AICB_ERR_INVALID, "block id out of range");
@@ -1432,14 +1439,14 @@ void mirror_region(SpaceHost &h, const DeviceScene &ds, const RegionBox &box, co
 }
 
 aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *ids, uint16_t uniform_id,
-                         const uint8_t (*light)[4], uint32_t *d_mask, uint32_t *d_n_changed) {
+                         const uint8_t (*light)[4], bool on_device, uint32_t *d_mask, uint32_t *d_n_changed) {
     aicb_ctx *ctx = s->ctx;
     cudaStream_t stream = ctx->stream.get();
     const size_t vol = box.volume(), rows = (size_t)box.size[0] * box.size[1], sz = box.size[2];
     if (!s->d_light) light = nullptr;
     // the ids, then (16-byte aligned) the texels
     const size_t id_bytes = ids ? (vol * 2 + 15) / 16 * 16 : 0, bytes = id_bytes + (light ? vol * 4 : 0);
-    if (bytes) {
+    if (bytes && !on_device) {
         TRY(delta_room(ctx, bytes));
         if (ids) std::memcpy(ctx->h_delta.get(), ids, vol * 2);
         if (light) std::memcpy(ctx->h_delta.get<char>() + id_bytes, light, vol * 4);
@@ -1449,7 +1456,7 @@ aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *id
     const bool wide = s->ds.wide_cells;
     const uint32_t per = wide ? 4u : 8u, chunks_per_row = (uint32_t)((sz + per - 1) / per + 1);
     const uint32_t n_items = (uint32_t)(rows * chunks_per_row);
-    const uint16_t *d_ids = ids ? ctx->d_delta.get<const uint16_t>() : nullptr;
+    const uint16_t *d_ids = on_device ? ids : ids ? ctx->d_delta.get<const uint16_t>() : nullptr;
     auto launch = [&](auto kernel) {
         kernel<<<(n_items + 255) / 256, 256, 0, stream>>>(s->ds, box, d_ids, uniform_id, chunks_per_row, n_items, d_mask,
                                                           d_n_changed);
@@ -1466,8 +1473,9 @@ aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *id
     }
     if (light) {
         const uint32_t cpr = (uint32_t)((sz + 3) / 4 + 1), n = (uint32_t)(rows * cpr);
-        k_region_texels<<<(n + 255) / 256, 256, 0, stream>>>(
-            s->ds, box, (const uint32_t *)(ctx->d_delta.get<const char>() + id_bytes), cpr, n, s->d_light.get<uint32_t>());
+        const uint32_t *texels = on_device ? (const uint32_t *)light
+                                           : (const uint32_t *)(ctx->d_delta.get<const char>() + id_bytes);
+        k_region_texels<<<(n + 255) / 256, 256, 0, stream>>>(s->ds, box, texels, cpr, n, s->d_light.get<uint32_t>());
     }
     CU(cudaGetLastError());
     return AICB_OK;
@@ -1480,9 +1488,10 @@ aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint1
     RegionBox box;
     TRY(check_region(r.scene[0], region, ids, uniform_id, &box));
     if (box.volume() == 0) return AICB_OK;
+    TRY(refresh_mirror(r.scene[0]));
     for (size_t k = 0; k < r.n; k++) {
         CU(cudaSetDevice(r.ctx[k]->device));
-        TRY(region_cells(r.scene[k], box, ids, uniform_id, light, nullptr, nullptr));
+        TRY(region_cells(r.scene[k], box, ids, uniform_id, light, false, nullptr, nullptr));
         CU(cudaEventRecord(r.ctx[k]->ev_delta.get(), r.ctx[k]->stream.get()));  // renders on other streams wait for it
     }
     mirror_region(*r.scene[0]->host, r.scene[0]->ds, box, ids, uniform_id);
@@ -1500,6 +1509,7 @@ aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb
     for (size_t i = 0; i < n_blocks; i++) kind[indices[i]] = f.kinds[i];
     std::vector<CubeDelta> ops;
     if (kind != h.kind) {
+        TRY(refresh_mirror(r.scene[0]));
         if (h.h_ids.size() != h.volume) return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
         const bool wide = r.scene[0]->ds.wide_cells;
         uint32_t idx = 0;
@@ -1628,6 +1638,7 @@ aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block) {
     h.n_bricks = h.n_palette = h.dead_bricks = h.dead_pal = 0;
     book(h, f, nullptr);
     h.h_ids.assign(h.volume, 0);
+    h.ids_stale = false;
     return AICB_OK;
 }
 
@@ -1675,6 +1686,305 @@ aicb_status scenes_upload_light(Replicas r, const uint8_t (*light)[4], size_t n_
         }
     }
     return AICB_OK;
+}
+
+
+// ---------------------------------------------------------------------------------------------
+// scene inputs in device memory (internal.h): validated on the device, one verdict read back
+// ---------------------------------------------------------------------------------------------
+aicb_status join_caller(aicb_ctx *const *ctx, size_t n, cudaStream_t caller) {
+    if (!caller) return AICB_OK;
+    CU(cudaSetDevice(ctx[0]->device));
+    CU(cudaEventRecord(ctx[0]->ev_join.get(), caller));
+    for (size_t i = 0; i < n; i++) {
+        if (ctx[i]->stream.get() == caller) continue;
+        CU(cudaSetDevice(ctx[i]->device));
+        CU(cudaStreamWaitEvent(ctx[i]->stream.get(), ctx[0]->ev_join.get(), 0));
+    }
+    CU(cudaSetDevice(ctx[0]->device));
+    return AICB_OK;
+}
+
+aicb_status release_caller(aicb_ctx *ctx, cudaStream_t caller) {
+    if (!caller || caller == ctx->stream.get()) return AICB_OK;
+    CU(cudaSetDevice(ctx->device));
+    CU(cudaEventRecord(ctx->ev_join.get(), ctx->stream.get()));
+    CU(cudaStreamWaitEvent(caller, ctx->ev_join.get(), 0));
+    return AICB_OK;
+}
+
+// Every replica's stream has finished the call's work (the group calls return once their writes are done).
+static aicb_status settle_replicas(Replicas r) {
+    if (r.n == 1) return AICB_OK;
+    for (size_t i = 0; i < r.n; i++) {
+        CU(cudaSetDevice(r.ctx[i]->device));
+        CU(cudaStreamSynchronize(r.ctx[i]->stream.get()));
+    }
+    CU(cudaSetDevice(r.ctx[0]->device));
+    return AICB_OK;
+}
+
+// At least `bytes` of the context's d_inputs, once its stream no longer uses the smaller buffer.
+static aicb_status inputs_room(aicb_ctx *ctx, size_t bytes) {
+    if (ctx->d_inputs.bytes() >= bytes) return AICB_OK;
+    CU(cudaStreamSynchronize(ctx->stream.get()));
+    return ctx->d_inputs.ensure(bytes);
+}
+
+static size_t align256(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
+
+// One entry of a cube list per thread: its Z-major index (0 for a cube out of bounds) and its list position, and the
+// list's first bad entry (the host loop's first failing check) by atomicMin.
+static __global__ void __launch_bounds__(256) k_check_cubes(const int32_t *__restrict__ cubes, const uint16_t *__restrict__ ids,
+                                                            uint32_t n, int3 lo, int3 size, uint32_t n_blocks,
+                                                            uint32_t *__restrict__ idx, uint32_t *__restrict__ pos,
+                                                            InputVerdict *v) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t dx = (uint32_t)(cubes[3 * i] - lo.x), dy = (uint32_t)(cubes[3 * i + 1] - lo.y),
+                   dz = (uint32_t)(cubes[3 * i + 2] - lo.z);
+    const bool inside = dx < (uint32_t)size.x && dy < (uint32_t)size.y && dz < (uint32_t)size.z;
+    idx[i] = inside ? (dx * (uint32_t)size.y + dy) * (uint32_t)size.z + dz : 0u;
+    pos[i] = i;
+    if (!inside) atomicMin(&v->first_bad, 2ull * i);
+    else if (ids[i] >= n_blocks) atomicMin(&v->first_bad, 2ull * i + 1);
+}
+
+// Whether any id of a dense array is past the table (first_bad = 1); grid-stride.
+static __global__ void __launch_bounds__(256) k_check_ids(const uint16_t *__restrict__ ids, size_t n, uint32_t n_blocks,
+                                                          InputVerdict *v) {
+    bool bad = false;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        bad |= ids[i] >= n_blocks;
+    if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31u) == 0) atomicMin(&v->first_bad, 1ull);
+}
+
+// aicb_scene_update_cubes' batch from a sorted cube list: the last entry for each cube (the last of its run, the sort
+// being stable) gives its CubeDelta, the kind from the block table's records; the deltas go to `ops` in any order
+// (their cubes are distinct) and are counted in v->count.  An entry with an id past the table is skipped: its call is
+// rejected.
+static __global__ void __launch_bounds__(256) k_cube_deltas(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
+                                                            uint32_t n, const uint16_t *__restrict__ ids,
+                                                            const uint32_t *__restrict__ light, const BlockRec *blocks,
+                                                            uint32_t n_blocks, uint32_t wide, CubeDelta *ops, InputVerdict *v) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n || (p + 1 < n && keys[p + 1] == keys[p])) return;
+    const uint32_t i = vals[p], id = ids[i];
+    if (id >= n_blocks) return;
+    CubeDelta op;
+    op.idx = keys[p];
+    op.cell = id | (__ldg(&blocks[id].kind_res) & 0xffu) << (wide ? 16 : 14);
+    op.light = light ? light[i] : 0u;
+    op.has_light = light ? 1u : 0u;
+    ops[atomicAdd(&v->count, 1u)] = op;
+}
+
+// Each cube's block id from its cell word (16-bit cells: id | kind << 14; 32-bit: id | kind << 16); grid-stride.
+static __global__ void __launch_bounds__(256) k_decode_ids(const void *__restrict__ cells, uint32_t wide, size_t n,
+                                                           uint16_t *__restrict__ out) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        out[i] = wide ? (uint16_t)(((const uint32_t *)cells)[i] & 0xffffu) : (uint16_t)(((const uint16_t *)cells)[i] & 0x3fffu);
+}
+
+static unsigned stride_grid(const aicb_ctx *ctx, size_t n) {
+    return (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)ctx->num_sms * 16));
+}
+
+static aicb_status reset_verdict(InputVerdict *v, cudaStream_t stream) {
+    CU(cudaMemsetAsync(&v->first_bad, 0xff, sizeof v->first_bad, stream));
+    CU(cudaMemsetAsync(&v->count, 0, sizeof v->count, stream));
+    return AICB_OK;
+}
+
+aicb_status stage_cube_list(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *ids, uint32_t n,
+                            size_t extra_bytes, size_t temp_bytes, CubeList *l) {
+    aicb_ctx *ctx = s->ctx;
+    cudaStream_t stream = ctx->stream.get();
+    int end_bit = 1;
+    while (end_bit < 32 && ((uint64_t)1 << end_bit) < s->host->volume) end_bit++;
+    size_t sort_bytes = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr,
+                                       (const uint32_t *)nullptr, (uint32_t *)nullptr, n, 0, end_bit, stream));
+    l->temp_bytes = std::max(sort_bytes, temp_bytes);
+    const size_t a = align256((size_t)n * 4);
+    TRY(inputs_room(ctx, 256 + 4 * a + align256(extra_bytes) + l->temp_bytes));
+    char *p = ctx->d_inputs.get<char>();
+    l->verdict = (InputVerdict *)p;
+    l->idx = (uint32_t *)(p + 256);
+    uint32_t *pos = (uint32_t *)(p + 256 + a);
+    l->keys = (uint32_t *)(p + 256 + 2 * a);
+    l->vals = (uint32_t *)(p + 256 + 3 * a);
+    l->extra = p + 256 + 4 * a;
+    l->temp = p + 256 + 4 * a + align256(extra_bytes);
+    const DeviceScene &ds = s->ds;
+    TRY(reset_verdict(l->verdict, stream));
+    k_check_cubes<<<(n + 255) / 256, 256, 0, stream>>>(&cubes[0][0], ids, n, make_int3(ds.lo[0], ds.lo[1], ds.lo[2]),
+                                                       make_int3(ds.size[0], ds.size[1], ds.size[2]),
+                                                       (uint32_t)s->host->block_count(), l->idx, pos, l->verdict);
+    CU(cudaGetLastError());
+    size_t tb = l->temp_bytes;
+    CU(cub::DeviceRadixSort::SortPairs(l->temp, tb, l->idx, l->keys, pos, l->vals, n, 0, end_bit, stream));
+    return AICB_OK;
+}
+
+aicb_status read_verdict(aicb_ctx *ctx, const InputVerdict *d_verdict, uint32_t *count) {
+    InputVerdict v;
+    CU(cudaMemcpyAsync(&v, d_verdict, sizeof v, cudaMemcpyDeviceToHost, ctx->stream.get()));
+    CU(cudaStreamSynchronize(ctx->stream.get()));
+    if (v.first_bad != ~0ull) return fail(AICB_ERR_INVALID, v.first_bad & 1 ? "block id out of range" : "cube out of bounds");
+    *count = v.count;
+    return AICB_OK;
+}
+
+aicb_status check_region_device(Replicas r, const aicb_aab *region, const uint16_t *d_ids, uint16_t uniform_id,
+                                const uint8_t (*d_light)[4], cudaStream_t caller, RegionBox *box) {
+    aicb_scene *s = r.scene[0];
+    aicb_ctx *ctx = r.ctx[0];
+    TRY(check_box(s, region, box));
+    CU(cudaSetDevice(ctx->device));
+    const size_t count = s->host->block_count(), vol = box->volume();
+    if (!d_ids && uniform_id >= count) return fail(AICB_ERR_INVALID, "block id out of range");
+    if (vol == 0) return AICB_OK;
+    if (d_ids) TRY(check_device_pointer(d_ids, ctx->device, false, 2, "block_ids"));
+    if (d_light) TRY(check_device_pointer(d_light, ctx->device, false, 4, "light"));
+    TRY(join_caller(r.ctx, r.n, caller));
+    if (!d_ids) return AICB_OK;
+    TRY(inputs_room(ctx, 256));
+    InputVerdict *v = ctx->d_inputs.get<InputVerdict>();
+    TRY(reset_verdict(v, ctx->stream.get()));
+    k_check_ids<<<stride_grid(ctx, vol), 256, 0, ctx->stream.get()>>>(d_ids, vol, (uint32_t)count, v);
+    CU(cudaGetLastError());
+    uint32_t unused;
+    return read_verdict(ctx, v, &unused);
+}
+
+aicb_status copy_to_replica(Replicas r, size_t k, const void *from, size_t bytes, void **to) {
+    aicb_ctx *c = r.ctx[k];
+    CU(cudaSetDevice(c->device));
+    TRY(inputs_room(c, bytes));
+    CU(cudaMemcpyPeerAsync(c->d_inputs.get(), c->device, from, r.ctx[0]->device, bytes, c->stream.get()));
+    *to = c->d_inputs.get();
+    return AICB_OK;
+}
+
+aicb_status refresh_mirror(aicb_scene *s0) {
+    SpaceHost &h = *s0->host;
+    if (!h.ids_stale) return AICB_OK;
+    if (h.volume) {
+        aicb_ctx *ctx = s0->ctx;
+        cudaStream_t stream = ctx->stream.get();
+        CU(cudaSetDevice(ctx->device));
+        DeviceBuffer ids;
+        TRY(ids.ensure(h.volume * 2));
+        k_decode_ids<<<stride_grid(ctx, h.volume), 256, 0, stream>>>(s0->d_cells.get(), s0->ds.wide_cells, h.volume,
+                                                                      ids.get<uint16_t>());
+        CU(cudaGetLastError());
+        h.h_ids.resize(h.volume);
+        CU(cudaMemcpyAsync(h.h_ids.data(), ids.get(), h.volume * 2, cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+    }
+    h.ids_stale = false;
+    return AICB_OK;
+}
+
+// The batch is checked and de-duplicated on replica 0's device (k_check_cubes, a stable radix sort by cube, the last
+// entry of each run: k_cube_deltas), and only the verdict and the number of distinct cubes come back.  Every replica
+// then scatters the same deltas (scatter_cubes_kernel), the others from a peer copy of replica 0's.
+aicb_status scenes_update_cubes_device(Replicas r, const int32_t (*cubes)[3], const uint16_t *ids,
+                                       const uint8_t (*light)[4], size_t n, cudaStream_t caller) {
+    if (n && (!cubes || !ids)) return fail(AICB_ERR_INVALID, "NULL argument");
+    aicb_scene *s0 = r.scene[0];
+    aicb_ctx *c0 = r.ctx[0];
+    CU(cudaSetDevice(c0->device));
+    if (n == 0) return AICB_OK;
+    if (n > 0xffffffffull) return fail(AICB_ERR_INVALID, "more than 2^32 - 1 cubes");
+    TRY(check_device_pointer(cubes, c0->device, false, 4, "cubes"));
+    TRY(check_device_pointer(ids, c0->device, false, 2, "block_ids"));
+    if (light) TRY(check_device_pointer(light, c0->device, false, 4, "light"));
+    TRY(join_caller(r.ctx, 1, caller));
+    const uint32_t nn = (uint32_t)n;
+    CubeList l;
+    TRY(stage_cube_list(s0, cubes, ids, nn, n * sizeof(CubeDelta), 0, &l));
+    CubeDelta *ops = (CubeDelta *)l.extra;
+    const bool lit = light && s0->d_light;
+    k_cube_deltas<<<(nn + 255) / 256, 256, 0, c0->stream.get()>>>(l.keys, l.vals, nn, ids,
+                                                                  lit ? (const uint32_t *)light : nullptr, s0->ds.blocks,
+                                                                  (uint32_t)s0->host->block_count(), s0->ds.wide_cells,
+                                                                  ops, l.verdict);
+    CU(cudaGetLastError());
+    uint32_t m = 0;
+    TRY(read_verdict(c0, l.verdict, &m));
+    for (size_t k = 0; k < r.n; k++) {
+        aicb_scene *s = r.scene[k];
+        aicb_ctx *ctx = r.ctx[k];
+        CU(cudaSetDevice(ctx->device));
+        void *from = ops;
+        if (k > 0) TRY(copy_to_replica(r, k, ops, (size_t)m * sizeof(CubeDelta), &from));
+        scatter_cubes_kernel<<<(m + 127) / 128, 128, 0, ctx->stream.get()>>>((const CubeDelta *)from, m, s->ds.wide_cells,
+                                                                            s->d_cells.get(), s->d_light.get<uint32_t>());
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(ctx->ev_delta.get(), ctx->stream.get()));   // renders on other streams wait for it
+    }
+    s0->host->ids_stale = true;
+    TRY(settle_replicas(r));
+    return release_caller(c0, caller);
+}
+
+// The box form: the ids are checked on the device (check_region_device), then every replica's k_region_cells and
+// k_region_texels read the caller's arrays where they are (peer memory for the other replicas).
+aicb_status scenes_update_region_device(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                        const uint8_t (*light)[4], cudaStream_t caller) {
+    RegionBox box;
+    TRY(check_region_device(r, region, ids, uniform_id, light, caller, &box));
+    if (box.volume() == 0) return AICB_OK;
+    for (size_t k = 0; k < r.n; k++) {
+        CU(cudaSetDevice(r.ctx[k]->device));
+        TRY(region_cells(r.scene[k], box, ids, uniform_id, light, true, nullptr, nullptr));
+        CU(cudaEventRecord(r.ctx[k]->ev_delta.get(), r.ctx[k]->stream.get()));   // renders on other streams wait for it
+    }
+    r.scene[0]->host->ids_stale = true;
+    TRY(settle_replicas(r));
+    return release_caller(r.ctx[0], caller);
+}
+
+aicb_status scenes_upload_light_device(Replicas r, const uint8_t (*light)[4], size_t n_texels, cudaStream_t caller) {
+    if (!light) return fail(AICB_ERR_INVALID, "NULL argument");
+    const size_t volume = r.scene[0]->host->volume;
+    if (n_texels != volume) return fail(AICB_ERR_INVALID, "light volume size mismatch");
+    aicb_ctx *c0 = r.ctx[0];
+    CU(cudaSetDevice(c0->device));
+    if (volume == 0) return AICB_OK;
+    TRY(check_device_pointer(light, c0->device, false, 4, "light"));
+    TRY(join_caller(r.ctx, r.n, caller));
+    for (size_t i = 0; i < r.n; i++) {
+        aicb_scene *s = r.scene[i];
+        cudaStream_t stream = r.ctx[i]->stream.get();
+        CU(cudaSetDevice(r.ctx[i]->device));
+        if (!s->d_light) {
+            TRY(s->d_light.ensure(volume * 4));
+            s->device_bytes += volume * 4;
+            s->ds.light = s->d_light.get<uint32_t>();
+        }
+        CU(cudaMemcpyPeerAsync(s->d_light.get(), r.ctx[i]->device, light, c0->device, volume * 4, stream));
+        CU(cudaEventRecord(r.ctx[i]->ev_delta.get(), stream));
+    }
+    TRY(settle_replicas(r));
+    return release_caller(c0, caller);
+}
+
+aicb_status scene_download_ids_device(Replicas r, uint16_t *out, size_t n, cudaStream_t caller) {
+    aicb_scene *s = r.scene[0];
+    aicb_ctx *ctx = r.ctx[0];
+    if (!out) return fail(AICB_ERR_INVALID, "NULL argument");
+    if (n != s->host->volume) return fail(AICB_ERR_INVALID, "block id volume size mismatch");
+    CU(cudaSetDevice(ctx->device));
+    if (n == 0) return AICB_OK;
+    TRY(check_device_pointer(out, ctx->device, false, 2, "out"));
+    TRY(join_caller(r.ctx, 1, caller));
+    k_decode_ids<<<stride_grid(ctx, n), 256, 0, ctx->stream.get()>>>(s->d_cells.get(), s->ds.wide_cells, n, out);
+    CU(cudaGetLastError());
+    if (r.n > 1) CU(cudaStreamSynchronize(ctx->stream.get()));   // a group call returns with its output final
+    return release_caller(ctx, caller);
 }
 
 
@@ -1812,6 +2122,26 @@ aicb_status aicb_scene_fill_uniform(aicb_scene *s, const aicb_block_desc *block)
 
 aicb_status aicb_scene_upload_light(aicb_scene *s, const uint8_t (*light)[4], size_t n_texels) {
     return on_scene(s, [&](Replicas r) { return scenes_upload_light(r, light, n_texels); });
+}
+
+aicb_status aicb_scene_update_cubes_device(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *ids,
+                                           const uint8_t (*light)[4], size_t n, void *stream) {
+    return on_scene(s, [&](Replicas r) { return scenes_update_cubes_device(r, cubes, ids, light, n, (cudaStream_t)stream); });
+}
+
+aicb_status aicb_scene_update_region_device(aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                            const uint8_t (*light)[4], void *stream) {
+    return on_scene(s, [&](Replicas r) {
+        return scenes_update_region_device(r, region, ids, uniform_id, light, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_scene_upload_light_device(aicb_scene *s, const uint8_t (*light)[4], size_t n_texels, void *stream) {
+    return on_scene(s, [&](Replicas r) { return scenes_upload_light_device(r, light, n_texels, (cudaStream_t)stream); });
+}
+
+aicb_status aicb_scene_download_ids_device(aicb_scene *s, uint16_t *out, size_t n, void *stream) {
+    return on_scene(s, [&](Replicas r) { return scene_download_ids_device(r, out, n, (cudaStream_t)stream); });
 }
 
 size_t aicb_shard_pixel_count(const aicb_camera *cam, const aicb_shard *shard) {

@@ -723,6 +723,51 @@ aicb_status aicb_group_light_download_queue(aicb_group_scene *gs, uint8_t *prior
     });
 }
 
+// The calls with inputs or outputs in device memory: device 0's, which every replica reads over peer access (a group
+// enables it at creation); each returns once every replica's writes are done.
+aicb_status aicb_group_scene_update_cubes_device(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *ids,
+                                                 const uint8_t (*light)[4], size_t n, void *stream) {
+    return on_group(gs, false, [&](Replicas r) {
+        return scenes_update_cubes_device(r, cubes, ids, light, n, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_group_scene_update_region_device(aicb_group_scene *gs, const aicb_aab *region, const uint16_t *ids,
+                                                  uint16_t uniform_id, const uint8_t (*light)[4], void *stream) {
+    return on_group(gs, false, [&](Replicas r) {
+        return scenes_update_region_device(r, region, ids, uniform_id, light, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_group_scene_upload_light_device(aicb_group_scene *gs, const uint8_t (*light)[4], size_t n_texels,
+                                                 void *stream) {
+    return on_group(gs, false, [&](Replicas r) {
+        return scenes_upload_light_device(r, light, n_texels, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_group_scene_download_ids_device(aicb_group_scene *gs, uint16_t *out, size_t n, void *stream) {
+    return on_group(gs, false, [&](Replicas r) { return scene_download_ids_device(r, out, n, (cudaStream_t)stream); });
+}
+
+aicb_status aicb_group_light_edit_cubes_device(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *new_ids,
+                                               size_t n, size_t *n_changed, void *stream) {
+    return on_group(gs, true, [&](Replicas r) {
+        return light_edit_cubes_device(r, cubes, new_ids, n, n_changed, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_group_light_edit_region_device(aicb_group_scene *gs, const aicb_aab *region, const uint16_t *ids,
+                                                uint16_t uniform_id, size_t *n_changed, void *stream) {
+    return on_group(gs, true, [&](Replicas r) {
+        return light_edit_region_device(r, region, ids, uniform_id, n_changed, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_group_light_download_device(aicb_group_scene *gs, uint8_t (*out)[4], size_t n_texels, void *stream) {
+    return on_group(gs, false, [&](Replicas r) { return light_download_device(r, out, n_texels, (cudaStream_t)stream); });
+}
+
 aicb_status aicb_group_light_download(aicb_group_scene *gs, int replica, uint8_t (*out)[4], size_t n_texels) {
     return on_group(gs, false, [&](Replicas r) {
         if (replica < 0 || (size_t)replica >= r.n) return aicb_fail(AICB_ERR_INVALID, "no such replica");

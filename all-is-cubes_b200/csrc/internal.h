@@ -215,6 +215,7 @@ struct aicb_ctx {
     DeviceBuffer d_task_text;    // per task: the UI pass's CharacterBuf for the world pass (aicb_render_layers_terminal)
     LightChart light_chart;
     DeviceBuffer d_derive;       // aicb_derive_block_light's per-palette-entry and per-ray terms and its results
+    DeviceBuffer d_inputs;       // the device-input calls' scratch: verdict, sorted cube lists, staged entries
     std::mutex mu;
 };
 
@@ -266,6 +267,8 @@ struct BlockTable {
 struct SpaceHost {
     size_t volume = 0;
     std::vector<uint16_t> h_ids;           // mirror of Space::contents (edits are applied in order on the host)
+    bool ids_stale = false;                // a device-input call changed the cells since h_ids was last written;
+                                           // the first host reader rebuilds it from replica 0's cells (refresh_mirror)
     std::vector<uint8_t> kind;             // per block id: its kind, which its cubes' cell words carry
     std::vector<BlockTable::Extent> extent;   // per block id: its voxel data in the pools
     size_t n_bricks = 0, n_palette = 0;    // brick words, float4s
@@ -446,19 +449,69 @@ struct RegionBox {
 // `uniform_id`) past the table.
 aicb_status check_region(const aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
                          RegionBox *box);
+// check_region's first part: the region alone, as a box (AICB_ERR_INVALID: NULL, not inside the bounds, too large).
+aicb_status check_box(const aicb_scene *s, const aicb_aab *region, RegionBox *box);
 // One replica's share of a box call, on its context's device and stream: the ids (2 bytes per cube; none if uniform)
-// and `light` (if given and the scene has a light volume) go through the context's staging, and k_region_cells /
-// k_region_texels write them.  With d_mask (ceil(volume / 32) words) the cubes whose block id changes are marked there
+// and `light` (if given and the scene has a light volume) go through the context's staging, or with on_device are
+// read where they are (device memory the replica's device reaches), and k_region_cells / k_region_texels write them.  With d_mask (ceil(volume / 32) words) the cubes whose block id changes are marked there
 // and counted into *d_n_changed (if given).  The caller records aicb_ctx::ev_delta behind its last kernel, and writes
 // the host mirror once (mirror_region).
 aicb_status region_cells(aicb_scene *s, const RegionBox &box, const uint16_t *ids, uint16_t uniform_id,
-                         const uint8_t (*light)[4], uint32_t *d_mask, uint32_t *d_n_changed);
+                         const uint8_t (*light)[4], bool on_device, uint32_t *d_mask, uint32_t *d_n_changed);
 // The host mirror takes a box call's ids row by row.
 void mirror_region(SpaceHost &h, const aicb::DeviceScene &ds, const RegionBox &box, const uint16_t *ids,
                    uint16_t uniform_id);
 // SpaceChange::CubeBlock / CubeLight for every cube of a box.
 aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
                                  const uint8_t (*light)[4]);
+
+// ---- scene inputs in device memory (aicb200.cu: the scene calls; light.cu: the light edits) -----------------------
+// Inputs are device memory of replica 0's device.  Each call makes replica 0's stream wait for the caller's (`caller`,
+// NULL: none) before reading them, and the caller's stream wait for replica 0's before returning, so the caller may
+// reuse the buffers for work it queues afterwards.  Validation runs on the device and reduces the inputs to an
+// InputVerdict, the only bytes read back before the call decides; on a group the call returns once every replica's
+// writes are done.
+struct InputVerdict {
+    unsigned long long first_bad;   // 2 * i + 0: entry i's cube out of bounds; + 1: its id past the table; ~0: none
+    uint32_t count;                 // the entries the call applies: distinct cubes, or changing entries
+    uint32_t _pad;
+};
+// The first n listed contexts' streams wait for the caller's (join_caller); the caller's waits for replica 0's
+// (release_caller).
+aicb_status join_caller(aicb_ctx *const *ctx, size_t n, cudaStream_t caller);
+aicb_status release_caller(aicb_ctx *ctx, cudaStream_t caller);
+// A cube list (int32[n][3] cubes, u16[n] ids) checked and sorted on replica 0's stream, in its context's d_inputs:
+// verdict (first_bad over the list; count 0), each entry's Z-major index in list order (idx), and (keys, vals) the
+// indices sorted stably with each entry's list position; `extra` bytes follow for the caller.  The scratch is 256-byte
+// aligned piece by piece.  Nothing is read back.
+struct CubeList {
+    InputVerdict *verdict;
+    uint32_t *idx, *keys, *vals;
+    void *extra;
+    void *temp;              // CUB's scratch, temp_bytes
+    size_t temp_bytes;
+};
+aicb_status stage_cube_list(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *ids, uint32_t n,
+                            size_t extra_bytes, size_t temp_bytes, CubeList *l);
+// The verdict read back (replica 0's stream synchronised): AICB_ERR_INVALID with the host twin's message for a bad
+// entry, else *count.
+aicb_status read_verdict(aicb_ctx *ctx, const InputVerdict *d_verdict, uint32_t *count);
+// A box call's region (check_box), its arrays' pointers, and its ids (every id < the table's size, checked on the
+// device; or uniform_id) against replica 0.  For a non-empty box every replica's stream then waits for the caller's.
+aicb_status check_region_device(Replicas r, const aicb_aab *region, const uint16_t *d_ids, uint16_t uniform_id,
+                                const uint8_t (*d_light)[4], cudaStream_t caller, RegionBox *box);
+// `bytes` of replica 0's d_inputs scratch at `from` copied to replica k's (k > 0), which grows to hold them; the copy
+// is queued on replica k's stream.  Returns the copy's address.
+aicb_status copy_to_replica(Replicas r, size_t k, const void *from, size_t bytes, void **to);
+// Rebuilds the host mirror from replica 0's cells if a device-input call left it stale (one device-to-host copy of
+// 2 bytes per cube).
+aicb_status refresh_mirror(aicb_scene *s0);
+aicb_status scenes_update_cubes_device(Replicas r, const int32_t (*cubes)[3], const uint16_t *ids,
+                                       const uint8_t (*light)[4], size_t n, cudaStream_t caller);
+aicb_status scenes_update_region_device(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                        const uint8_t (*light)[4], cudaStream_t caller);
+aicb_status scenes_upload_light_device(Replicas r, const uint8_t (*light)[4], size_t n_texels, cudaStream_t caller);
+aicb_status scene_download_ids_device(Replicas r, uint16_t *out, size_t n, cudaStream_t caller);
 aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks);
 aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks);
 aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block);
@@ -582,6 +635,12 @@ aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, 
 // Mutation::fill / fill_uniform(region): Mutation::set for every cube of a box, without propagation.
 aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
                               size_t *n_changed);
+// The light edits with their lists in device memory (see the device-input calls above).
+aicb_status light_edit_cubes_device(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n,
+                                    size_t *n_changed, cudaStream_t caller);
+aicb_status light_edit_region_device(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                     size_t *n_changed, cudaStream_t caller);
+aicb_status light_download_device(Replicas r, uint8_t (*out)[4], size_t n_texels, cudaStream_t caller);
 // Space::set_physics on the replicas' light side, once nothing on their contexts reads their arrays: `sky` holds the
 // new sky in a DeviceScene's sky fields, which every replica takes; `max_distance` is the new LightPhysics (0 = None).
 aicb_status light_set_physics(Replicas r, const aicb::DeviceScene &sky, uint32_t max_distance);

@@ -7,6 +7,8 @@
 #include <cstdlib>
 #include <cstring>
 
+#include <cub/device/device_scan.cuh>
+
 #include "internal.h"
 #include "light_kernel.cuh"
 
@@ -648,6 +650,49 @@ __global__ void __launch_bounds__(256) k_edit_light(const LightParams P, const E
         if (queue) mark_changed(P, e.idx);
     }
     modified_cube(P, e.idx, block_id_at(P.scene, e.idx), queue);
+}
+
+// The staging of a device edit list (light_edit_cubes_device) over the list sorted stably by cube (stage_cube_list):
+// (keys, vals) = (cube, list position) in sorted order, so a cube's entries form a run in list order.  What the host
+// loop of light_edit_cubes finds, as three passes and two scans:
+//   - k_stage_changing: an entry changes iff its id differs from the one before it in its run, or for a run's first
+//     entry from its cube's cell (the host mirror's value then); `head` marks the runs' first entries.
+//   - k_stage_final: the last entry of each run (run = the inclusive sum of head) gives its cube's final id.
+//   - k_stage_entries: each changing entry at its rank among the changing entries in list order (pos, the exclusive
+//     sum of `changing`), as the host loop stages it; v->count is their number.
+// A cube out of bounds sorts as cube 0 and is never applied (its call is rejected).
+__global__ void __launch_bounds__(256) k_stage_changing(const DeviceScene S, const uint32_t *__restrict__ keys,
+                                                        const uint32_t *__restrict__ vals, const uint16_t *__restrict__ ids,
+                                                        uint32_t n, uint32_t volume, uint32_t *__restrict__ head,
+                                                        uint32_t *__restrict__ changing) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    const uint32_t key = keys[p], i = vals[p];
+    const bool first = p == 0 || keys[p - 1] != key;
+    const uint32_t before = !first ? (uint32_t)ids[vals[p - 1]] : key < volume ? block_id_at(S, key) : 0u;
+    head[p] = first ? 1u : 0u;
+    changing[i] = ids[i] != before ? 1u : 0u;
+}
+
+__global__ void __launch_bounds__(256) k_stage_final(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
+                                                     const uint16_t *__restrict__ ids, const uint32_t *__restrict__ run,
+                                                     uint32_t n, uint16_t *__restrict__ run_final) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n || (p + 1 < n && keys[p + 1] == keys[p])) return;
+    run_final[run[p] - 1] = ids[vals[p]];
+}
+
+__global__ void __launch_bounds__(256) k_stage_entries(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
+                                                       const uint16_t *__restrict__ ids, const uint32_t *__restrict__ run,
+                                                       const uint16_t *__restrict__ run_final,
+                                                       const uint32_t *__restrict__ changing,
+                                                       const uint32_t *__restrict__ pos, uint32_t n,
+                                                       EditEntry *__restrict__ entries, InputVerdict *v) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n) return;
+    if (p == 0) v->count = pos[n - 1] + changing[n - 1];
+    const uint32_t i = vals[p];
+    if (changing[i]) entries[pos[i]] = EditEntry{keys[p], ids[i], run_final[run[p] - 1]};
 }
 
 // The scan of aicb_light_relight_blocks: every cell of the scene, 16 bytes per load (8 u16 cells or 4 u32 cells,
@@ -1557,6 +1602,7 @@ aicb_status light_edit_cubes(Replicas r, const int32_t (*cubes)[3], const uint16
         CU(cudaSetDevice(r.ctx[k]->device));
         TRY(delta_room(r.ctx[k], room));
     }
+    TRY(refresh_mirror(r.scene[0]));
     EditEntry *staged = r.ctx[0]->h_delta.get<EditEntry>();
     uint32_t m = 0;
     for (size_t i = 0; i < n; i++) {
@@ -1588,6 +1634,79 @@ aicb_status light_edit_cubes(Replicas r, const int32_t (*cubes)[3], const uint16
     CU(cudaSetDevice(r.ctx[0]->device));
     if (n_changed) *n_changed = m;
     return AICB_OK;
+}
+
+// light_edit_cubes with the list in device memory: checked and staged on replica 0's device (stage_cube_list, then
+// k_stage_*), so that the EditEntry list is the host loop's; only the verdict and its length come back.  Every replica
+// then applies it as light_edit_cubes does, the others from a peer copy of replica 0's list.  The host mirror is left
+// stale.
+aicb_status light_edit_cubes_device(Replicas r, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n,
+                                    size_t *n_changed, cudaStream_t caller) {
+    if (n && (!cubes || !new_ids)) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n > 0xffffffffull) return aicb_fail(AICB_ERR_INVALID, "more than 2^32 - 1 edits");
+    aicb_scene *s0 = r.scene[0];
+    aicb_ctx *c0 = r.ctx[0];
+    CU(cudaSetDevice(c0->device));
+    uint32_t m = 0;
+    const EditEntry *d_entries = nullptr;
+    if (n) {
+        TRY(check_device_pointer(cubes, c0->device, false, 4, "cubes"));
+        TRY(check_device_pointer(new_ids, c0->device, false, 2, "new_ids"));
+        TRY(join_caller(r.ctx, 1, caller));
+        const uint32_t nn = (uint32_t)n;
+        cudaStream_t stream = c0->stream.get();
+        size_t scan_in = 0, scan_ex = 0;
+        CU(cub::DeviceScan::InclusiveSum(nullptr, scan_in, (uint32_t *)nullptr, (uint32_t *)nullptr, nn, stream));
+        CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_ex, (uint32_t *)nullptr, (uint32_t *)nullptr, nn, stream));
+        const size_t a = ((size_t)nn * 4 + 255) & ~(size_t)255, b = ((size_t)nn * 2 + 255) & ~(size_t)255;
+        CubeList l;
+        TRY(stage_cube_list(s0, cubes, new_ids, nn, 4 * a + b + (size_t)nn * sizeof(EditEntry),
+                            std::max(scan_in, scan_ex), &l));
+        char *x = (char *)l.extra;
+        uint32_t *head = (uint32_t *)x, *run = (uint32_t *)(x + a), *changing = (uint32_t *)(x + 2 * a),
+                 *pos = (uint32_t *)(x + 3 * a);
+        uint16_t *run_final = (uint16_t *)(x + 4 * a);
+        EditEntry *entries = (EditEntry *)(x + 4 * a + b);
+        const unsigned blocks = (nn + 255) / 256;
+        k_stage_changing<<<blocks, 256, 0, stream>>>(s0->ds, l.keys, l.vals, new_ids, nn, (uint32_t)s0->host->volume,
+                                                     head, changing);
+        size_t tb = l.temp_bytes;
+        CU(cub::DeviceScan::InclusiveSum(l.temp, tb, head, run, nn, stream));
+        k_stage_final<<<blocks, 256, 0, stream>>>(l.keys, l.vals, new_ids, run, nn, run_final);
+        tb = l.temp_bytes;
+        CU(cub::DeviceScan::ExclusiveSum(l.temp, tb, changing, pos, nn, stream));
+        k_stage_entries<<<blocks, 256, 0, stream>>>(l.keys, l.vals, new_ids, run, run_final, changing, pos, nn, entries,
+                                                    l.verdict);
+        CU(cudaGetLastError());
+        TRY(read_verdict(c0, l.verdict, &m));
+        d_entries = entries;
+    }
+    TRY(ensure_replicas(r));
+    if (n_changed) *n_changed = 0;
+    if (n == 0) return AICB_OK;
+    for (size_t k = 0; m && k < r.n; k++) {
+        aicb_scene *sk = r.scene[k];
+        aicb_ctx *c = r.ctx[k];
+        cudaStream_t stream = c->stream.get();
+        CU(cudaSetDevice(c->device));
+        void *from = const_cast<EditEntry *>(d_entries);
+        if (k > 0) TRY(copy_to_replica(r, k, d_entries, (size_t)m * sizeof(EditEntry), &from));
+        const EditEntry *e = (const EditEntry *)from;
+        const unsigned blocks = (m + 255) / 256;
+        if (sk->ds.wide_cells) k_edit_cells<true><<<blocks, 256, 0, stream>>>(sk->ds, e, m);
+        else k_edit_cells<false><<<blocks, 256, 0, stream>>>(sk->ds, e, m);
+        k_edit_light<<<blocks, 256, 0, stream>>>(light_params(r, k), e, m, k == 0);
+        CU(cudaGetLastError());
+        CU(cudaEventRecord(c->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
+    }
+    for (size_t k = 0; m && k < r.n; k++) {
+        CU(cudaSetDevice(r.ctx[k]->device));
+        CU(cudaStreamSynchronize(r.ctx[k]->stream.get()));
+    }
+    if (m) s0->host->ids_stale = true;
+    CU(cudaSetDevice(c0->device));
+    if (n_changed) *n_changed = m;
+    return release_caller(c0, caller);
 }
 
 // light_edit_cubes, then evaluate_light(epsilon).
@@ -1636,15 +1755,16 @@ aicb_status light_relight_blocks(Replicas r, const uint16_t *indices, size_t n, 
 // the replica's overflow list (a round buffer, empty between light calls: one bit per cube of the box), then the light
 // rule on the device (k_region_light).  Replica 0 alone counts the changed cubes and touches the queue and the set; the
 // host mirror takes the ids once.  Nothing propagates; the tile bounds are rebuilt from the pending bytes by the next
-// propagation.
-aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
-                              size_t *n_changed) {
-    RegionBox box;
-    TRY(check_region(r.scene[0], region, ids, uniform_id, &box));
+// propagation.  This is the body of the host and the device form, after validation: the ids are a host array (staged,
+// and the host mirror takes them) or, with on_device, device memory every replica reads where it is (the mirror is then
+// marked stale).
+static aicb_status edit_region(Replicas r, const RegionBox &box, const uint16_t *ids, uint16_t uniform_id, bool on_device,
+                               size_t *n_changed) {
     TRY(ensure_replicas(r));
     if (n_changed) *n_changed = 0;
     const size_t vol = box.volume();
     if (vol == 0) return AICB_OK;
+    if (!on_device) TRY(refresh_mirror(r.scene[0]));
     uint32_t edited = 0;
     for (size_t i = 0; i < r.n; i++) {
         aicb_ctx *c = r.ctx[i];
@@ -1652,13 +1772,15 @@ aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t
         CU(cudaSetDevice(c->device));
         const LightParams P = light_params(r, i);
         if (i == 0) CU(cudaMemsetAsync(&P.counters->edited, 0, 4, stream));
-        TRY(region_cells(r.scene[i], box, ids, uniform_id, nullptr, P.overflow, i == 0 ? &P.counters->edited : nullptr));
+        TRY(region_cells(r.scene[i], box, ids, uniform_id, nullptr, on_device, P.overflow,
+                         i == 0 ? &P.counters->edited : nullptr));
         k_region_light<<<(unsigned)((vol + 255) / 256), 256, 0, stream>>>(P, box, P.overflow, (uint32_t)vol, i == 0);
         CU(cudaGetLastError());
         CU(cudaEventRecord(c->ev_delta.get(), stream));   // renders on other streams wait for it (launch_trace)
         if (i == 0) CU(cudaMemcpyAsync(&edited, &P.counters->edited, 4, cudaMemcpyDeviceToHost, stream));
     }
-    mirror_region(*r.scene[0]->host, r.scene[0]->ds, box, ids, uniform_id);
+    if (on_device) r.scene[0]->host->ids_stale = true;
+    else mirror_region(*r.scene[0]->host, r.scene[0]->ds, box, ids, uniform_id);
     for (size_t i = 0; i < r.n; i++) {
         CU(cudaSetDevice(r.ctx[i]->device));
         CU(cudaStreamSynchronize(r.ctx[i]->stream.get()));
@@ -1666,6 +1788,21 @@ aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t
     CU(cudaSetDevice(r.ctx[0]->device));
     if (n_changed) *n_changed = edited;
     return AICB_OK;
+}
+
+aicb_status light_edit_region(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                              size_t *n_changed) {
+    RegionBox box;
+    TRY(check_region(r.scene[0], region, ids, uniform_id, &box));
+    return edit_region(r, box, ids, uniform_id, false, n_changed);
+}
+
+aicb_status light_edit_region_device(Replicas r, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                     size_t *n_changed, cudaStream_t caller) {
+    RegionBox box;
+    TRY(check_region_device(r, region, ids, uniform_id, nullptr, caller, &box));
+    TRY(edit_region(r, box, ids, uniform_id, ids != nullptr, n_changed));
+    return release_caller(r.ctx[0], caller);
 }
 
 // LightStorage::maybe_reinitialize_for_physics_change (space/light/updater.rs:80-113):
@@ -1833,6 +1970,23 @@ aicb_status light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     return AICB_OK;
 }
 
+// aicb_light_download into device memory of replica 0's device: one device-to-device copy on replica 0's stream,
+// behind the caller's work and everything queued on the context.
+aicb_status light_download_device(Replicas r, uint8_t (*out)[4], size_t n_texels, cudaStream_t caller) {
+    aicb_scene *s = r.scene[0];
+    if (!out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (n_texels != s->host->volume) return aicb_fail(AICB_ERR_INVALID, "light volume size mismatch");
+    if (!s->d_light) return aicb_fail(AICB_ERR_INVALID, "scene has no light volume (LightPhysics::None)");
+    CU(cudaSetDevice(s->ctx->device));
+    if (n_texels == 0) return AICB_OK;
+    TRY(check_device_pointer(out, s->ctx->device, false, 4, "out"));
+    TRY(join_caller(r.ctx, 1, caller));
+    cudaStream_t st = s->ctx->stream.get();
+    CU(cudaMemcpyAsync(out, s->d_light.get(), n_texels * 4, cudaMemcpyDeviceToDevice, st));
+    if (r.n > 1) CU(cudaStreamSynchronize(st));   // a group call returns with its output final
+    return release_caller(s->ctx, caller);
+}
+
 // The size of the set of changed cubes (kernels 1 and 2 of the take), behind everything queued on the context's stream;
 // the chunks' output positions stay in chunk_sums() for k_changes_emit.
 static aicb_status count_changes(const aicb_scene *s, uint32_t *n) {
@@ -1995,6 +2149,24 @@ aicb_status aicb_light_download_queue(aicb_scene *s, uint8_t *priorities, size_t
 
 aicb_status aicb_light_download(aicb_scene *s, uint8_t (*out)[4], size_t n_texels) {
     return on_scene(s, [&](Replicas r) { return light_download(r.scene[0], out, n_texels); });
+}
+
+aicb_status aicb_light_edit_cubes_device(aicb_scene *s, const int32_t (*cubes)[3], const uint16_t *new_ids, size_t n,
+                                         size_t *n_changed, void *stream) {
+    return on_scene(s, [&](Replicas r) {
+        return light_edit_cubes_device(r, cubes, new_ids, n, n_changed, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_light_edit_region_device(aicb_scene *s, const aicb_aab *region, const uint16_t *ids, uint16_t uniform_id,
+                                          size_t *n_changed, void *stream) {
+    return on_scene(s, [&](Replicas r) {
+        return light_edit_region_device(r, region, ids, uniform_id, n_changed, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_light_download_device(aicb_scene *s, uint8_t (*out)[4], size_t n_texels, void *stream) {
+    return on_scene(s, [&](Replicas r) { return light_download_device(r, out, n_texels, (cudaStream_t)stream); });
 }
 
 aicb_status aicb_light_changes_count(const aicb_scene *s, size_t *n_changed) {

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 20 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 21 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -285,6 +285,23 @@ unsafe extern "C" {
     pub fn aicb_scene_destroy(s: *mut aicb_scene);
     pub fn aicb_scene_device_bytes(s: *const aicb_scene) -> u64;
     pub fn aicb_scene_set_physics(s: *mut aicb_scene, sky: *const aicb_sky, light_max_distance: u8) -> aicb_status;
+    // a scene fed from device memory: arrays in CUDA buffers of the scene's device, ordered on `stream` (a cudaStream_t,
+    // NULL = the context's); validated on the device
+    pub fn aicb_scene_update_cubes_device(s: *mut aicb_scene, d_cubes: *const [i32; 3], d_ids: *const u16,
+                                          d_light_or_null: *const [u8; 4], n: usize, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_scene_update_region_device(s: *mut aicb_scene, region: *const aicb_aab, d_ids_or_null: *const u16,
+                                           uniform_id: u16, d_light_or_null: *const [u8; 4],
+                                           stream: *mut c_void) -> aicb_status;
+    pub fn aicb_scene_upload_light_device(s: *mut aicb_scene, d_light: *const [u8; 4], n_texels: usize,
+                                          stream: *mut c_void) -> aicb_status;
+    pub fn aicb_scene_download_ids_device(s: *mut aicb_scene, d_out: *mut u16, n: usize, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_light_edit_cubes_device(s: *mut aicb_scene, d_cubes: *const [i32; 3], d_ids: *const u16, n: usize,
+                                        n_changed_or_null: *mut usize, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_light_edit_region_device(s: *mut aicb_scene, region: *const aicb_aab, d_ids_or_null: *const u16,
+                                         uniform_id: u16, n_changed_or_null: *mut usize,
+                                         stream: *mut c_void) -> aicb_status;
+    pub fn aicb_light_download_device(s: *mut aicb_scene, d_out: *mut [u8; 4], n_texels: usize,
+                                      stream: *mut c_void) -> aicb_status;
 
     pub fn aicb_shard_pixel_count(cam: *const aicb_camera, shard: *const aicb_shard) -> usize;
     pub fn aicb_render_srgb8(s: *mut aicb_scene, cam: *const aicb_camera, opt: *const aicb_options, shard: *const aicb_shard,
@@ -361,6 +378,24 @@ unsafe extern "C" {
     pub fn aicb_group_scene_append_blocks(gs: *mut aicb_group_scene, descs: *const aicb_block_desc, n: usize) -> aicb_status;
     // every replica; validated once, so a rejected call changes none
     pub fn aicb_group_scene_fill_uniform(gs: *mut aicb_group_scene, block: *const aicb_block_desc) -> aicb_status;
+    pub fn aicb_group_scene_update_cubes_device(gs: *mut aicb_group_scene, d_cubes: *const [i32; 3], d_ids: *const u16,
+                                                d_light_or_null: *const [u8; 4], n: usize,
+                                                stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_scene_update_region_device(gs: *mut aicb_group_scene, region: *const aicb_aab,
+                                                 d_ids_or_null: *const u16, uniform_id: u16,
+                                                 d_light_or_null: *const [u8; 4], stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_scene_upload_light_device(gs: *mut aicb_group_scene, d_light: *const [u8; 4], n_texels: usize,
+                                                stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_scene_download_ids_device(gs: *mut aicb_group_scene, d_out: *mut u16, n: usize,
+                                                stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_light_edit_cubes_device(gs: *mut aicb_group_scene, d_cubes: *const [i32; 3], d_ids: *const u16,
+                                              n: usize, n_changed_or_null: *mut usize,
+                                              stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_light_edit_region_device(gs: *mut aicb_group_scene, region: *const aicb_aab,
+                                               d_ids_or_null: *const u16, uniform_id: u16,
+                                               n_changed_or_null: *mut usize, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_light_download_device(gs: *mut aicb_group_scene, d_out: *mut [u8; 4], n_texels: usize,
+                                            stream: *mut c_void) -> aicb_status;
     // aicb_render_layers_* on a group: both layers must be scenes of the same group
     pub fn aicb_group_render_layers_srgb8(world: *const aicb_group_layer, ui: *const aicb_group_layer,
                                           backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 20
+#define AICB_ABI_VERSION 21
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -295,6 +295,57 @@ uint64_t aicb_scene_device_bytes(const aicb_scene *);
 aicb_status aicb_scene_set_physics(aicb_scene *, const aicb_sky *sky, uint8_t light_max_distance);
 
 /* ---------------------------------------------------------------------------------------------
+ * A scene fed from device memory: the update, light-edit and download calls with their arrays in CUDA buffers of the
+ * scene's device (device 0 on a group), for a host whose world changes on the GPU.  Each call leaves the scene, its
+ * light, queue and set of changed cubes byte for byte as its host twin does with the same data, with the same errors
+ * and messages.
+ *   - Pointers: each array is device memory of the scene's device, aligned to its element (4 bytes for cubes and
+ *     texels, 2 for ids), checked with cudaPointerGetAttributes before anything is issued: host memory, another
+ *     device's memory or a misaligned pointer is AICB_ERR_INVALID.
+ *   - Stream: `stream` is a cudaStream_t of the scene's device, or NULL for the context's stream.  The call's kernels
+ *     run after the work queued on it before the call (ids a producer kernel wrote there are read correctly), and work
+ *     queued on it afterwards runs after the call has read its inputs and written its outputs.  Frames issued later on
+ *     any stream see the update, as they see host updates.
+ *   - Validation stays on the device: the checks of the host twin (cube in bounds, id < the table's size, region
+ *     inside the bounds, LightPhysics::None for the light calls) are reduced by a kernel to a verdict of a few bytes,
+ *     the only thing read back before the call decides.  So the calls with ids synchronise with the stream up to their
+ *     validation; then they issue their writes, or return AICB_ERR_INVALID with nothing changed.
+ *   - Duplicates: a list is sorted stably by cube on the device (CUB radix sort), so update_cubes keeps the last entry
+ *     for a cube and light_edit_cubes counts and applies exactly the entries the host loop finds changing.
+ *   - The host mirror of the block ids (which aicb_light_edit_cubes, aicb_light_edit_region, aicb_scene_update_blocks
+ *     and the host updates use) is not copied back per call: a device update marks it stale, and the first host call
+ *     that needs it rebuilds it from the cells with one device-to-host copy of 2 bytes per cube (33.5 MB at 256^3).
+ *     aicb_scene_fill_uniform resets it.
+ *   - Groups: inputs and outputs are device 0's memory; every replica reads them over peer access or takes a peer copy
+ *     of device 0's staged list, and ends identical to the others.  The group calls return once every replica's writes
+ *     are done, as the group calls do.
+ * The single-context update calls return once their writes are issued; the light edits once their writes are done.
+ * GPU test: tests/test_gpu_device_inputs.py. */
+/* aicb_scene_update_cubes: int32[n][3] cubes, u16[n] ids, u8[n][4] light or NULL.  n == 0 does nothing. */
+aicb_status aicb_scene_update_cubes_device(aicb_scene *, const int32_t (*d_cubes)[3], const uint16_t *d_ids,
+                                           const uint8_t (*d_light_or_null)[4], size_t n, void *stream);
+/* aicb_scene_update_region: ids Z-major within `region` (NULL: uniform_id), light Z-major within it or NULL.  Every
+ * replica's kernels read the arrays where they are.  A uniform fill without light reads nothing and does not wait. */
+aicb_status aicb_scene_update_region_device(aicb_scene *, const aicb_aab *region, const uint16_t *d_ids_or_null,
+                                            uint16_t uniform_id, const uint8_t (*d_light_or_null)[4], void *stream);
+/* aicb_scene_upload_light: one device-to-device copy per replica; nothing to validate on the device, so it does not
+ * synchronise. */
+aicb_status aicb_scene_upload_light_device(aicb_scene *, const uint8_t (*d_light)[4], size_t n_texels, void *stream);
+/* Each cube's block id, Z-major (aicb_scene_desc::block_ids' order), decoded on the device from its cell word (16- or
+ * 32-bit cells) into u16[volume] at d_out.  n must be the volume.  Ordered behind the updates queued on the context;
+ * does not synchronise on one context. */
+aicb_status aicb_scene_download_ids_device(aicb_scene *, uint16_t *d_out, size_t n, void *stream);
+/* aicb_light_edit_cubes: the list as above; *n_changed_or_null the changing entries.  Returns once its writes are
+ * done. */
+aicb_status aicb_light_edit_cubes_device(aicb_scene *, const int32_t (*d_cubes)[3], const uint16_t *d_ids, size_t n,
+                                         size_t *n_changed_or_null, void *stream);
+/* aicb_light_edit_region: ids Z-major within `region` or NULL for uniform_id.  Returns once its writes are done. */
+aicb_status aicb_light_edit_region_device(aicb_scene *, const aicb_aab *region, const uint16_t *d_ids_or_null,
+                                          uint16_t uniform_id, size_t *n_changed_or_null, void *stream);
+/* aicb_light_download into u8[volume][4] at d_out: a device-to-device copy; does not synchronise on one context. */
+aicb_status aicb_light_download_device(aicb_scene *, uint8_t (*d_out)[4], size_t n_texels, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * draw(): replaces RtRenderer::draw_rgba / RtRenderer::draw::<ColorBuf> and the Rayon pixel
  * dispatch trace_scene_to_image_impl (renderer.rs:183-220, 282-308, 516-556).
  * Host-buffer variants copy device->host inside the call (blocking, like draw_rgba).
@@ -544,6 +595,24 @@ aicb_status aicb_group_scene_append_blocks(aicb_group_scene *, const aicb_block_
 /* aicb_scene_fill_uniform on every replica, holding every context of the group: the block is validated and flattened
  * once, so a rejected call changes no replica, then every replica is filled on its own device. */
 aicb_status aicb_group_scene_fill_uniform(aicb_group_scene *, const aicb_block_desc *block);
+/* The device-input calls (aicb_scene_update_cubes_device ..) on the group: arrays in device 0's memory, validated on
+ * device 0 before any replica changes; every replica ends identical; each call returns once every replica's writes
+ * are done (for the downloads, once device 0's output is final).  aicb_group_scene_download_ids_device and
+ * aicb_group_light_download_device read replica 0. */
+aicb_status aicb_group_scene_update_cubes_device(aicb_group_scene *, const int32_t (*d_cubes)[3], const uint16_t *d_ids,
+                                                 const uint8_t (*d_light_or_null)[4], size_t n, void *stream);
+aicb_status aicb_group_scene_update_region_device(aicb_group_scene *, const aicb_aab *region,
+                                                  const uint16_t *d_ids_or_null, uint16_t uniform_id,
+                                                  const uint8_t (*d_light_or_null)[4], void *stream);
+aicb_status aicb_group_scene_upload_light_device(aicb_group_scene *, const uint8_t (*d_light)[4], size_t n_texels,
+                                                 void *stream);
+aicb_status aicb_group_scene_download_ids_device(aicb_group_scene *, uint16_t *d_out, size_t n, void *stream);
+aicb_status aicb_group_light_edit_cubes_device(aicb_group_scene *, const int32_t (*d_cubes)[3], const uint16_t *d_ids,
+                                               size_t n, size_t *n_changed_or_null, void *stream);
+aicb_status aicb_group_light_edit_region_device(aicb_group_scene *, const aicb_aab *region,
+                                                const uint16_t *d_ids_or_null, uint16_t uniform_id,
+                                                size_t *n_changed_or_null, void *stream);
+aicb_status aicb_group_light_download_device(aicb_group_scene *, uint8_t (*d_out)[4], size_t n_texels, void *stream);
 
 /* == RtScene::trace_ray_through_layers + draw_rgba (renderer.rs:454-478, 282-308) and RaytraceToTexture::do_some_tracing's
  * trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) on the whole group: the arguments, the validation and
