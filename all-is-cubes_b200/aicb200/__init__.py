@@ -179,6 +179,8 @@ def load_library() -> C.CDLL:
         "light_edit_cubes_device": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, size, C.c_void_p],
         "light_edit_region_device": [C.c_void_p, C.POINTER(abi.Aab), C.c_void_p, C.c_uint16, size, C.c_void_p],
         "light_download_device": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
+        "scene_update_blocks_device": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p],
+        "scene_append_blocks_device": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p],
     }.items():
         for prefix in ("aicb_", "aicb_group_"):
             getattr(lib, prefix + name).argtypes = argtypes
@@ -551,6 +553,57 @@ class BlockLight:
     def from_abi(o: abi.BlockLight) -> "BlockLight":
         return BlockLight(face_colors=tuple(tuple(o.face_colors[f][:]) for f in range(6)), color=tuple(o.color[:]),
                           emission=tuple(o.emission[:]), opaque_faces=int(o.opaque_faces), visible=bool(o.visible))
+
+
+class DeviceBlock:
+    """A block definition whose voxels are CUDA tensors on the scene's device (device 0 of a group), for
+    update_blocks / append_blocks (aicb_scene_*_blocks_device): `indices` a uint16 tensor of the data bounds' shape
+    (Z-major), or None for a single voxel, palette[0]; `palette` a float32 [n, 8] tensor (rgba, emission, pad).
+    `light` is the block's BlockLight, or None to derive it on the device (AICB_BLOCKS_DERIVE_LIGHT); `visible`
+    ORs an animation hint into a derived Derived::visible."""
+
+    def __init__(self, resolution, voxel_lower, indices, palette, is_air=False, light: Optional["BlockLight"] = None,
+                 visible: bool = False):
+        self.resolution = int(resolution)
+        self.voxel_lower = tuple(int(v) for v in (voxel_lower or (0, 0, 0)))
+        self.indices = indices
+        self.palette = palette
+        self.is_air = bool(is_air)
+        self.light = light
+        self.visible = bool(visible)
+
+    def _check(self, device):
+        torch = _torch()
+        for name, t, dtype in (("indices", self.indices, torch.uint16), ("palette", self.palette, torch.float32)):
+            if t is None and name == "indices":
+                continue
+            if not _is_cuda_tensor(t) or t.dtype != dtype or t.device != device or not t.is_contiguous():
+                raise ValueError(f"DeviceBlock.{name} must be a contiguous {dtype} tensor on {device}")
+        if self.palette.dim() != 2 or self.palette.shape[1] != 8:
+            raise ValueError("DeviceBlock.palette must have shape [n, 8]")
+        if self.indices is not None and self.indices.dim() != 3:
+            raise ValueError("DeviceBlock.indices must have 3 dimensions (the data bounds)")
+
+    def fill_desc(self, bd):
+        """DeviceBlock -> aicb_block_desc with device pointers (the tensors stay owned by the block)."""
+        bd.resolution = 1 if self.indices is None else self.resolution
+        bd.is_air = 1 if self.is_air else 0
+        bd.voxel_bounds.lower[:] = (0, 0, 0) if self.indices is None else self.voxel_lower
+        bd.voxel_bounds.size[:] = (1, 1, 1) if self.indices is None else tuple(self.indices.shape)
+        bd.indices = None if self.indices is None else self.indices.data_ptr()
+        bd.n_indices = 0 if self.indices is None else self.indices.numel()
+        bd.palette = self.palette.data_ptr() if self.palette.shape[0] else None
+        bd.n_palette = self.palette.shape[0]
+        bl = self.light
+        if bl is None:
+            bd.light_visible = 1 if self.visible else 0
+            return
+        bd.light_opaque_faces = bl.opaque_faces
+        bd.light_visible = 1 if bl.visible else 0
+        for f in range(6):
+            bd.light_face_colors[f][:] = bl.face_colors[f]
+        bd.light_color[:] = bl.color
+        bd.light_emission[:] = bl.emission
 
 
 class Space:
@@ -965,16 +1018,45 @@ class _Scene:
         _check(self._fn("scene_update_region")(self.handle, C.byref(region), None if ids is None else ids.ctypes.data,
                                                uniform, None if lt is None else lt.ctypes.data))
 
+    def _device_blocks(self, blocks):
+        """The aicb_block_desc array and flags of a device call, or None for Blocks; ValueError for a mix."""
+        on_device = [isinstance(b, DeviceBlock) for b in blocks]
+        if not any(on_device):
+            return None
+        if not all(on_device):
+            raise ValueError("one call takes Blocks or DeviceBlocks, not both")
+        device = self._device()
+        derive = [b.light is None for b in blocks]
+        if any(derive) and not all(derive):
+            raise ValueError("one call derives the light of every DeviceBlock (light=None) or of none")
+        arr = (abi.BlockDesc * len(blocks))()
+        for i, b in enumerate(blocks):
+            b._check(device)
+            b.fill_desc(arr[i])
+        return arr, abi.BLOCKS_DERIVE_LIGHT if derive[0] else 0
+
     def update_blocks(self, indices, blocks):
         """SpaceChange::BlockEvaluation / BlockIndex: new definitions for existing block indices.  Light is not touched:
-        light_relight_blocks(indices) follows it on a lit scene."""
+        light_relight_blocks(indices) follows it on a lit scene.  DeviceBlocks are read on the device, after the work
+        queued on the scene device's current torch stream."""
         idx = np.ascontiguousarray(indices, dtype=np.uint16)
+        dev = self._device_blocks(blocks)
+        if dev is not None:
+            _check(self._fn("scene_update_blocks_device")(self.handle, idx.ctypes.data, dev[0], len(blocks), dev[1],
+                                                          _stream(self._device())))
+            return
         arr = _block_descs(blocks)
         _check(self._fn("scene_update_blocks")(self.handle, idx.ctypes.data, arr, len(blocks)))
 
     def append_blocks(self, blocks):
         """SpaceChange::BlockIndex for new indices (UpdatingSpaceRaytracer::update, updating.rs:145-151): the blocks
-        become the table's next indices, valid in update_cubes, update_blocks and light_edit_and_propagate."""
+        become the table's next indices, valid in update_cubes, update_blocks and light_edit_and_propagate.
+        DeviceBlocks as in update_blocks."""
+        dev = self._device_blocks(blocks)
+        if dev is not None:
+            _check(self._fn("scene_append_blocks_device")(self.handle, dev[0], len(blocks), dev[1],
+                                                          _stream(self._device())))
+            return
         arr = _block_descs(blocks)
         _check(self._fn("scene_append_blocks")(self.handle, arr, len(blocks)))
 

@@ -1,7 +1,9 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 21
+ABI_VERSION = 22
+
+BLOCKS_DERIVE_LIGHT = 1
 
 OK, ERR_INVALID, ERR_OOM, ERR_CUDA, ERR_UNSUPPORTED, ERR_BUSY, ERR_RETRY = range(7)
 STATUS_NAMES = {0: "OK", 1: "ERR_INVALID", 2: "ERR_OOM", 3: "ERR_CUDA", 4: "ERR_UNSUPPORTED", 5: "ERR_BUSY", 6: "ERR_RETRY"}
@@ -185,6 +187,8 @@ EXPORTED_SYMBOLS = [
     "aicb_light_edit_cubes_device",
     "aicb_light_edit_region_device",
     "aicb_light_download_device",
+    "aicb_scene_update_blocks_device",
+    "aicb_scene_append_blocks_device",
     "aicb_shard_pixel_count",
     "aicb_render_srgb8",
     "aicb_render_rgba16f",
@@ -253,6 +257,8 @@ EXPORTED_SYMBOLS = [
     "aicb_group_light_edit_cubes_device",
     "aicb_group_light_edit_region_device",
     "aicb_group_light_download_device",
+    "aicb_group_scene_update_blocks_device",
+    "aicb_group_scene_append_blocks_device",
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",
     "aicb_group_render_layers_terminal",

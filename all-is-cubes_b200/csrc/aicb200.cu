@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 
+#include "block_words.cuh"
 #include "brick_room.h"
 #include "host_tables.h"
 #include "internal.h"
@@ -90,28 +91,13 @@ static void build_block_sky(const aicb_sky &sky, DeviceScene *ds) {
     ds->sky_mean = texel_some(q);
 }
 
-static bool voxel_invisible(const aicb_voxel &v) {
-    return v.rgba[3] == 0.0f && v.emission[0] == 0.0f && v.emission[1] == 0.0f && v.emission[2] == 0.0f;
-}
-
 // TracingBlock::from_block (sr.rs:579-587) for one block definition: its 32-byte record, classification, brick words
 // in the wide form (trace_kernel.cuh) and palette entries (appended to `bricks` / `palette`; the record's offsets are
 // relative to those vectors), plus what the marching kernel needs of each surface: {alpha, an upper bound of
 // log2(1 - alpha)} per palette entry.
 // Called by flatten_blocks alone.
+static const char *const BRICKS_PAST_2_32 = "brick pool exceeds 2^32 voxels";
 static const aicb_voxel AIR_VOXEL = {{0, 0, 0, 0}, {0, 0, 0}, 0};
-
-static float2 surface_entry(float alpha) {
-    float l2a;
-    if (alpha >= 1.0f) l2a = -INFINITY;
-    else if (!(alpha > 0.0f)) l2a = 0.0f;
-    else {
-        const float unit_t = 1.0f - alpha;   // the f32 value apply_transmittance raises to the span's thickness
-        l2a = std::nextafterf((float)std::log2((double)unit_t), INFINITY);
-        if (l2a > 0.0f) l2a = 0.0f;
-    }
-    return make_float2(alpha, l2a);
-}
 
 // blk_tab entry of a block: what the marching kernel needs of a single-voxel surface on the Space level.
 // `pal_off` indexes `pal_tab`; `pal_base` is added to it for the device-wide palette index.
@@ -124,7 +110,7 @@ static float4 block_entry(uint8_t kind, uint32_t pal_off, const std::vector<floa
     return make_float4(e.x, e.y, palf, 0.0f);
 }
 
-aicb_status check_block_desc(const aicb_block_desc &b) {
+aicb_status check_block_scalars(const aicb_block_desc &b) {
     const uint32_t res = b.resolution;
     if (res == 0 || (res & (res - 1)) || res > 128) return fail(AICB_ERR_INVALID, "block resolution must be 1..128, power of 2");
     if (b.indices == nullptr) {
@@ -138,12 +124,23 @@ aicb_status check_block_desc(const aicb_block_desc &b) {
         if (lo < 0 || hi > (int64_t)res) return fail(AICB_ERR_INVALID, "voxel_bounds must lie within [0, resolution)^3");
     }
     if (!b.palette && b.n_palette) return fail(AICB_ERR_INVALID, "palette is NULL");
-    for (size_t k = 0; k < b.n_indices; k++)
-        if (b.indices[k] >= b.n_palette) return fail(AICB_ERR_INVALID, "voxel index out of palette range");
-    if (!b.is_air && res != 1 && b.n_palette > 65536)
+    return AICB_OK;
+}
+
+aicb_status check_block_palette(const aicb_block_desc &b) {
+    if (b.indices && !b.is_air && b.resolution != 1 && b.n_palette > 65536)
         return fail(AICB_ERR_UNSUPPORTED, "block palettes above 65536 entries are not supported: a voxel's palette "
                                           "index (VoxelIndex) is 16 bits");
     return AICB_OK;
+}
+
+static const char *const BAD_VOXEL_INDEX = "voxel index out of palette range";
+
+aicb_status check_block_desc(const aicb_block_desc &b) {
+    TRY(check_block_scalars(b));
+    for (size_t k = 0; b.indices && k < b.n_indices; k++)
+        if (b.indices[k] >= b.n_palette) return fail(AICB_ERR_INVALID, BAD_VOXEL_INDEX);
+    return check_block_palette(b);
 }
 
 aicb_voxel single_voxel_of(const aicb_block_desc &b) {
@@ -154,11 +151,33 @@ aicb_voxel single_voxel_of(const aicb_block_desc &b) {
     return at_origin ? b.palette[b.indices[0]] : AIR_VOXEL;
 }
 
+// The record of a definition of kind `kind` (an air block's is KIND_INVISIBLE) whose voxel data starts at brick word
+// `brick_off` and palette entry `pal_off`.
+static BlockRec block_rec(const aicb_block_desc &b, uint8_t kind, uint32_t brick_off, uint32_t pal_off) {
+    BlockRec r;
+    std::memset(&r, 0, sizeof r);
+    if (b.is_air) {
+        r.kind_res = KIND_INVISIBLE | (1u << 8);
+    } else if (kind != KIND_RECURSIVE) {
+        r.kind_res = kind | (1u << 8);
+        r.pal_off = pal_off;
+        r.vsize[0] = r.vsize[1] = r.vsize[2] = 1;
+    } else {
+        r.kind_res = KIND_RECURSIVE | ((uint32_t)b.resolution << 8);
+        for (int a = 0; a < 3; a++) {
+            r.vlo[a] = (int16_t)b.voxel_bounds.lower[a];
+            r.vsize[a] = (uint16_t)b.voxel_bounds.size[a];
+        }
+        r.brick_off = brick_off;
+        r.pal_off = pal_off;
+    }
+    return r;
+}
+
 static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t &kind, std::vector<uint32_t> &bricks,
                                  std::vector<float4> &palette, std::vector<float2> &pal_tab) {
     std::memset(&r, 0, sizeof r);
     TRY(check_block_desc(b));
-    const uint32_t res = b.resolution;
     auto push_voxel = [&](const aicb_voxel &v) {
         palette.push_back(make_float4(v.rgba[0], v.rgba[1], v.rgba[2], v.rgba[3]));
         palette.push_back(make_float4(v.emission[0], v.emission[1], v.emission[2], 0.0f));
@@ -168,23 +187,15 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
     const aicb_voxel sv = single ? single_voxel_of(b) : AIR_VOXEL;
     if (b.is_air) {
         kind = KIND_INVISIBLE;
-        r.kind_res = KIND_INVISIBLE | (1u << 8);
+        r = block_rec(b, kind, 0, 0);
     } else if (single) {
         kind = voxel_invisible(sv) ? KIND_INVISIBLE : KIND_SINGLE;
-        r.kind_res = kind | (1u << 8);
-        r.pal_off = (uint32_t)(palette.size() / 2);
-        r.vsize[0] = r.vsize[1] = r.vsize[2] = 1;
+        r = block_rec(b, kind, 0, (uint32_t)(palette.size() / 2));
         push_voxel(sv);
     } else {
         kind = KIND_RECURSIVE;
-        r.kind_res = KIND_RECURSIVE | (res << 8);
-        for (int a = 0; a < 3; a++) {
-            r.vlo[a] = (int16_t)b.voxel_bounds.lower[a];
-            r.vsize[a] = (uint16_t)b.voxel_bounds.size[a];
-        }
-        if (bricks.size() + b.n_indices > 0xffffffffull) return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
-        r.brick_off = (uint32_t)bricks.size();
-        r.pal_off = (uint32_t)(palette.size() / 2);
+        if (bricks.size() + b.n_indices > 0xffffffffull) return fail(AICB_ERR_INVALID, BRICKS_PAST_2_32);
+        r = block_rec(b, kind, (uint32_t)bricks.size(), (uint32_t)(palette.size() / 2));
         for (size_t k = 0; k < b.n_indices; k++) {
             const uint32_t v = b.indices[k];
             bricks.push_back(v << 16 | (voxel_invisible(b.palette[v]) ? 0x8000u : 0u));
@@ -977,6 +988,7 @@ struct FlatBlocks {
     const void *brick_words() const { return wide_bricks ? (const void *)bricks.data() : narrow.data(); }
     std::vector<float4> palette;
     std::vector<float2> pal_tab;
+    size_t words = 0, entries = 0;   // brick words and palette entries added (the vectors' sizes, if on the host)
 };
 
 // Validates and flattens n definitions against `h`, for the next ids (indices == nullptr) or for existing `indices`.
@@ -1009,11 +1021,49 @@ static aicb_status flatten_blocks(const SpaceHost &h, const aicb_block_desc *des
         f->narrow.resize(f->bricks.size());
         for (size_t k = 0; k < f->bricks.size(); k++) f->narrow[k] = (uint16_t)(f->bricks[k] >> 16 | (f->bricks[k] & 0x8000u));
     }
+    f->words = f->bricks.size();
+    f->entries = f->pal_tab.size();
     // live data only: the dead part of the pool is compacted away before it could push positions past 2^32
     // (flatten_placeable)
-    if (brick_room(h.n_bricks, h.dead_bricks, f->bricks.size()) == BrickRoom::too_big)
-        return fail(AICB_ERR_INVALID, "brick pool exceeds 2^32 voxels");
+    if (brick_room(h.n_bricks, h.dead_bricks, f->words) == BrickRoom::too_big) return fail(AICB_ERR_INVALID, BRICKS_PAST_2_32);
     return AICB_OK;
+}
+
+// single_voxel_of's source (DeviceBlockJob::single) for a definition whose voxels the host does not read.
+static uint32_t single_source(const aicb_block_desc &b) {
+    if (!is_single_voxel(b)) return SINGLE_NONE;
+    if (b.indices == nullptr) return b.n_palette ? SINGLE_FIRST : SINGLE_AIR;
+    const bool at_origin = b.n_indices == 1 && b.voxel_bounds.lower[0] == 0 && b.voxel_bounds.lower[1] == 0 &&
+                           b.voxel_bounds.lower[2] == 0;
+    return at_origin ? SINGLE_INDEXED : SINGLE_AIR;
+}
+
+// flatten_blocks for n validated definitions whose voxels are in device memory: the kind of each single voxel is
+// `kinds`' (read back from the device), everything else comes from the descriptors' sizes.  The voxel data, the
+// blk_tab entries and, with `derive`, the light records are left to the device (DeviceDefs).
+static void flatten_device(const SpaceHost &h, const aicb_block_desc *descs, size_t n, const std::vector<uint8_t> &kinds,
+                           bool derive, FlatBlocks *f) {
+    const size_t pal_base = h.n_palette / 2;
+    f->recs.resize(n);
+    f->extents.resize(n);
+    f->blk_tab.assign(n, make_float4(0.0f, 0.0f, 0.0f, 0.0f));
+    f->kinds.resize(n);
+    f->light.assign(n, LightBlockDev{});
+    for (size_t i = 0; i < n; i++) {
+        const aicb_block_desc &b = descs[i];
+        const bool single = is_single_voxel(b);
+        const uint8_t kind = b.is_air ? KIND_INVISIBLE : single ? kinds[i] : KIND_RECURSIVE;
+        const size_t words = kind == KIND_RECURSIVE ? b.n_indices : 0, entries = b.is_air ? 0 : single ? 1 : b.n_palette;
+        const BlockRec r = block_rec(b, kind, (uint32_t)(h.n_bricks + f->words), (uint32_t)(pal_base + f->entries));
+        f->recs[i] = r;
+        f->extents[i] = {r.brick_off, (uint32_t)words, r.pal_off, (uint32_t)entries};
+        f->kinds[i] = kind;
+        if (!derive) f->light[i] = light_block(b);
+        if (kind == KIND_RECURSIVE && b.n_palette > 32768) f->wide_bricks = true;
+        f->words += words;
+        f->entries += entries;
+    }
+    if (h.wide_bricks) f->wide_bricks = true;
 }
 
 // Every replica's narrow brick pool as a wide one, with room for `add` more words: once every replica's new buffer is
@@ -1058,9 +1108,9 @@ static aicb_status room(BlockTable &t, const SpaceHost &h, const FlatBlocks &f, 
         return add ? grow_buffer(b, used, used + add, stream, &retired.bufs) : AICB_OK;
     };
     TRY(grow(t.blocks, count * sizeof(BlockRec), added * sizeof(BlockRec)));
-    TRY(grow(t.bricks, h.n_bricks * wb, f.bricks.size() * wb));
-    TRY(grow(t.palette, h.n_palette * sizeof(float4), f.palette.size() * sizeof(float4)));
-    TRY(grow(t.pal_tab, h.n_palette / 2 * sizeof(float2), f.pal_tab.size() * sizeof(float2)));
+    TRY(grow(t.bricks, h.n_bricks * wb, f.words * wb));
+    TRY(grow(t.palette, h.n_palette * sizeof(float4), 2 * f.entries * sizeof(float4)));
+    TRY(grow(t.pal_tab, h.n_palette / 2 * sizeof(float2), f.entries * sizeof(float2)));
     TRY(grow(t.blk_tab, count * sizeof(float4), added * sizeof(float4)));
     return grow(t.light, count * sizeof(LightBlockDev), added * sizeof(LightBlockDev));
 }
@@ -1099,15 +1149,63 @@ static void book(SpaceHost &h, const FlatBlocks &f, const uint16_t *indices) {
         h.kind[id] = f.kinds[i];
         h.extent[id] = f.extents[i];
     }
-    h.n_bricks += f.bricks.size();
-    h.n_palette += f.palette.size();
+    h.n_bricks += f.words;
+    h.n_palette += 2 * f.entries;
     h.wide_bricks = f.wide_bricks;
 }
 
 // f (flatten_placeable) placed in every replica's table: room in each, then the copies, recorded in ev_delta (renders
 // on other streams wait for it, launch_trace), and the bookkeeping.  Records are written over in place (`indices`)
 // only once every replica has room and its context has been waited for (wait_context).
-static aicb_status place(Replicas r, const FlatBlocks &f, const uint16_t *indices) {
+// Definitions in device memory (scenes_blocks_device): what the device read back (each single voxel's kind), the light
+// records derive made on device 0, and per replica the jobs its kernels place (built by flatten_device).
+struct DeviceDefs {
+    std::vector<uint8_t> kinds;
+    bool derive = false;
+    std::vector<int32_t> derived;            // per definition: derive's record, or LIGHT_SINGLE
+    const aicb_block_light *d_derived = nullptr;
+    std::vector<DeviceBlockJob> jobs;
+    uint64_t most_words = 0, most_entries = 0;
+};
+
+// The jobs of `f` (flattened against h) for `dev`: the caller's pointers and each definition's pool positions, and the
+// per-id records of each id's last definition.
+static void device_jobs(const SpaceHost &h, const aicb_block_desc *descs, const FlatBlocks &f, const uint16_t *indices,
+                        DeviceDefs &dev) {
+    const size_t n = f.kinds.size();
+    dev.jobs.assign(n, DeviceBlockJob{});
+    dev.most_words = dev.most_entries = 0;
+    std::unordered_map<uint32_t, size_t> last;
+    for (size_t i = 0; i < n; i++) {
+        const aicb_block_desc &b = descs[i];
+        DeviceBlockJob &J = dev.jobs[i];
+        J.indices = b.indices;
+        J.palette = b.palette;
+        J.n_indices = b.n_indices;
+        J.n_palette = (uint32_t)b.n_palette;
+        J.single = single_source(b);
+        J.kind = f.kinds[i];
+        J.brick_off = f.extents[i].brick_off;
+        J.pal_off = f.extents[i].pal_off;
+        J.n_entries = f.extents[i].n_pal;
+        J.id = (uint32_t)(indices ? indices[i] : h.block_count() + i);
+        J.derived = dev.derive ? dev.derived[i] : LIGHT_GIVEN;
+        J.light_visible = b.light_visible;
+        J.rec = f.recs[i];
+        J.light = f.light[i];
+        dev.most_words = std::max<uint64_t>(dev.most_words, f.extents[i].n_bricks);
+        dev.most_entries = std::max<uint64_t>(dev.most_entries, J.n_entries);
+        if (indices) {
+            const auto [at, first] = last.emplace(J.id, i);
+            if (!first) {
+                dev.jobs[at->second].id = NO_ID;
+                at->second = i;
+            }
+        }
+    }
+}
+
+static aicb_status place(Replicas r, const FlatBlocks &f, const uint16_t *indices, const DeviceDefs *dev) {
     SpaceHost &h = *r.scene[0]->host;
     for (size_t i = 0; i < r.n; i++) {
         aicb_scene *s = r.scene[i];
@@ -1119,9 +1217,20 @@ static aicb_status place(Replicas r, const FlatBlocks &f, const uint16_t *indice
         TRY(st);
     }
     for (size_t i = 0; i < r.n; i++) {
-        CU(cudaSetDevice(r.ctx[i]->device));
-        TRY(copy(r.scene[i]->blocks, h, f, indices, r.ctx[i]->stream.get()));
-        CU(cudaEventRecord(r.ctx[i]->ev_delta.get(), r.ctx[i]->stream.get()));
+        aicb_ctx *ctx = r.ctx[i];
+        cudaStream_t stream = ctx->stream.get();
+        CU(cudaSetDevice(ctx->device));
+        if (!dev) {
+            TRY(copy(r.scene[i]->blocks, h, f, indices, stream));
+        } else {   // each replica's kernels read the caller's buffers on device 0 (as a peer on the others)
+            const size_t bytes = dev->jobs.size() * sizeof(DeviceBlockJob);
+            TRY(delta_room(ctx, bytes));
+            std::memcpy(ctx->h_delta.get(), dev->jobs.data(), bytes);
+            CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
+            TRY(issue_block_data(stream, ctx->d_delta.get<const DeviceBlockJob>(), (uint32_t)dev->jobs.size(),
+                                 dev->most_words, dev->most_entries, f.wide_bricks, r.scene[i]->blocks, dev->d_derived));
+        }
+        CU(cudaEventRecord(ctx->ev_delta.get(), stream));
     }
     book(h, f, indices);
     return AICB_OK;
@@ -1315,19 +1424,25 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
 // flattened again against the compacted table.  A compaction moves the pools, so each replica's context is waited
 // for first (wait_context).  Wide definitions for a narrow pool widen every replica's pool first.
 static aicb_status flatten_placeable(Replicas r, const aicb_block_desc *descs, size_t n_blocks, const uint16_t *indices,
-                                     FlatBlocks *f) {
+                                     DeviceDefs *dev, FlatBlocks *f) {
     const SpaceHost &h = *r.scene[0]->host;
-    TRY(flatten_blocks(h, descs, n_blocks, indices, f));
-    if (brick_room(h.n_bricks, h.dead_bricks, f->bricks.size()) == BrickRoom::compact_first) {
+    auto flatten = [&]() {
+        if (!dev) return flatten_blocks(h, descs, n_blocks, indices, f);
+        flatten_device(h, descs, n_blocks, dev->kinds, dev->derive, f);
+        return AICB_OK;
+    };
+    TRY(flatten());
+    if (brick_room(h.n_bricks, h.dead_bricks, f->words) == BrickRoom::compact_first) {
         for (size_t i = 0; i < r.n; i++) {
             CU(cudaSetDevice(r.ctx[i]->device));
             TRY(wait_context(r.ctx[i]));
         }
         TRY(compact_pools(r, true, false));
         *f = FlatBlocks();
-        TRY(flatten_blocks(h, descs, n_blocks, indices, f));
+        TRY(flatten());
     }
-    return f->wide_bricks && !h.wide_bricks ? widen_bricks(r, f->bricks.size()) : AICB_OK;
+    if (dev) device_jobs(h, descs, *f, indices, *dev);
+    return f->wide_bricks && !h.wide_bricks ? widen_bricks(r, f->words) : AICB_OK;
 }
 
 // The context's staging (h_delta / d_delta) with room for a batch of `bytes`, once the previous batch has left it.
@@ -1498,27 +1613,34 @@ aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint1
     return AICB_OK;
 }
 
-aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks) {
-    if (n_blocks && (!indices || !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
-    if (n_blocks == 0) return AICB_OK;
+// The body of aicb_scene_update_blocks and its device form (dev: the definitions' voxels are in device memory).  The
+// host form finds the cubes whose block changes kind in the host mirror and scatters their new words; the device form
+// re-encodes them in one pass over every replica's cells against a per-id table of new words, so it needs no mirror.
+static aicb_status update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks,
+                                 DeviceDefs *dev) {
     const SpaceHost &h = *r.scene[0]->host;
     FlatBlocks f;
-    TRY(flatten_placeable(r, descs, n_blocks, indices, &f));
+    TRY(flatten_placeable(r, descs, n_blocks, indices, dev, &f));
     // cubes that hold a block whose kind changes carry the new kind in their cell words
     std::vector<uint8_t> kind(h.kind);
     for (size_t i = 0; i < n_blocks; i++) kind[indices[i]] = f.kinds[i];
+    const bool wide = r.scene[0]->ds.wide_cells;
     std::vector<CubeDelta> ops;
-    if (kind != h.kind) {
+    std::vector<uint32_t> word;   // the device form's table: per id its new cell word, or NO_WORD
+    if (kind != h.kind && dev) {
+        word.assign(kind.size(), NO_WORD);
+        for (size_t id = 0; id < kind.size(); id++)
+            if (kind[id] != h.kind[id]) word[id] = cell_word((uint32_t)id, kind[id], wide);
+    } else if (kind != h.kind) {
         TRY(refresh_mirror(r.scene[0]));
         if (h.h_ids.size() != h.volume) return fail(AICB_ERR_INVALID, "scene has no host mirror of its block ids");
-        const bool wide = r.scene[0]->ds.wide_cells;
         uint32_t idx = 0;
         for (const uint16_t id : h.h_ids) {
             if (kind[id] != h.kind[id]) ops.push_back({idx, cell_word(id, kind[id], wide), 0, 0});
             idx++;
         }
     }
-    TRY(place(r, f, indices));   // (which waits for every context: compaction moves the pools)
+    TRY(place(r, f, indices, dev));   // (which waits for every context: compaction moves the pools)
     const bool compact_bricks = h.dead_bricks > h.n_bricks - h.dead_bricks;
     const bool compact_palette = h.dead_pal > h.n_palette / 2 - h.dead_pal;
     if (compact_bricks || compact_palette) TRY(compact_pools(r, compact_bricks, compact_palette));
@@ -1538,22 +1660,32 @@ aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb
             retired.bufs.push_back(std::move(d_ops));
             CU(cudaGetLastError());
         }
+        if (!word.empty() && h.volume) {
+            DeviceBuffer d_word;
+            TRY(d_word.upload(word.data(), word.size() * 4));
+            TRY(issue_rekind_cells(ctx, sc->d_cells.get(), wide, h.volume, d_word.get<const uint32_t>()));
+            retired.bufs.push_back(std::move(d_word));
+        }
         CU(cudaEventRecord(ctx->ev_delta.get(), stream));
         TRY(wait_context(ctx));   // the call returns once its writes are done
     }
     return AICB_OK;
 }
 
+aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks) {
+    if (n_blocks && (!indices || !descs)) return fail(AICB_ERR_INVALID, "NULL argument");
+    if (n_blocks == 0) return AICB_OK;
+    return update_blocks(r, indices, descs, n_blocks, nullptr);
+}
+
 // The copies are queued on the context's stream and ev_delta is recorded behind them, as aicb_scene_update_cubes does:
 // a frame issued later on another stream waits for them (launch_trace).  The new entries go to spare capacity that no
 // cell refers to until a later, stream-ordered cube update, so a frame in flight is not disturbed; an array that has to
 // move is freed only after it (Retired).
-aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks) {
-    if (n_blocks && !descs) return fail(AICB_ERR_INVALID, "NULL argument");
-    if (n_blocks == 0) return AICB_OK;
+static aicb_status append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks, DeviceDefs *dev) {
     const SpaceHost &h = *r.scene[0]->host;
     FlatBlocks f;
-    TRY(flatten_placeable(r, descs, n_blocks, nullptr, &f));
+    TRY(flatten_placeable(r, descs, n_blocks, nullptr, dev, &f));
     // u16 cells hold ids below 16384 (scenes_create): a table that grows past that takes u32 cells, re-encoded behind
     // every queued cube update of each context
     for (size_t i = 0; i < r.n; i++) {
@@ -1576,7 +1708,13 @@ aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_
         }
         sc->ds.wide_cells = 1;
     }
-    return place(r, f, nullptr);
+    return place(r, f, nullptr, dev);
+}
+
+aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks) {
+    if (n_blocks && !descs) return fail(AICB_ERR_INVALID, "NULL argument");
+    if (n_blocks == 0) return AICB_OK;
+    return append_blocks(r, descs, n_blocks, nullptr);
 }
 
 // Mutation::fill_uniform over the whole Space (space.rs:1461-1474), the source of SpaceChange::EveryBlock: the table
@@ -1987,6 +2125,108 @@ aicb_status scene_download_ids_device(Replicas r, uint16_t *out, size_t n, cudaS
     return release_caller(ctx, caller);
 }
 
+// The first failure of the host twin that the descriptors' scalars decide (flatten_blocks' checks without the index
+// scan): at definition `at` before its scan, or after it (`after_scan`); at == n for the brick pool's room, which is
+// checked after every definition.  at == SIZE_MAX: none.
+struct HostVerdict {
+    size_t at = SIZE_MAX;
+    bool after_scan = false;
+    aicb_status st = AICB_OK;
+    std::string msg;
+};
+
+static HostVerdict host_checks(const SpaceHost &h, const uint16_t *indices, const aicb_block_desc *descs, size_t n) {
+    HostVerdict v;
+    auto failed = [&](size_t at, bool after, aicb_status st) {
+        v.at = at;
+        v.after_scan = after;
+        v.st = st;
+        v.msg = aicb_last_error();
+        return v;
+    };
+    if (!indices && h.block_count() + n > 65536) return failed(0, false, fail(AICB_ERR_INVALID, "more than 65536 blocks"));
+    size_t words = 0;
+    for (size_t i = 0; i < n; i++) {
+        const aicb_block_desc &b = descs[i];
+        if (indices && indices[i] >= h.block_count())
+            return failed(i, false, fail(AICB_ERR_INVALID, "block index out of range (new indices need a new scene)"));
+        aicb_status st = check_block_scalars(b);
+        if (st != AICB_OK) return failed(i, false, st);
+        if ((st = check_block_palette(b)) != AICB_OK) return failed(i, true, st);
+        if (b.is_air || is_single_voxel(b)) continue;
+        if (words + b.n_indices > 0xffffffffull) return failed(i, true, fail(AICB_ERR_INVALID, BRICKS_PAST_2_32));
+        words += b.n_indices;
+    }
+    if (brick_room(h.n_bricks, h.dead_bricks, words) == BrickRoom::too_big)
+        return failed(n, false, fail(AICB_ERR_INVALID, BRICKS_PAST_2_32));
+    return v;
+}
+
+// aicb_scene_update_blocks_device / append_blocks_device over the replicas.  The host
+// checks what the scalars decide; one kernel scans the voxel indices of the definitions before the first host-side
+// failure and reads the kind of each single voxel, and those bytes are all that comes back before the call decides.
+// With AICB_BLOCKS_DERIVE_LIGHT, derive's kernels then run on device 0 on the caller's voxels and their error words
+// come back too.  Then the call is the host twin's body (update_blocks, append_blocks) with the voxel data placed by
+// blocks.cu's kernels on every replica, which read device 0's buffers (as a peer on other devices).
+aicb_status scenes_blocks_device(Replicas r, bool append, const uint16_t *indices, const aicb_block_desc *descs, size_t n,
+                                 uint32_t flags, cudaStream_t caller) {
+    if (n && (!descs || (!append && !indices))) return fail(AICB_ERR_INVALID, "NULL argument");
+    aicb_ctx *c0 = r.ctx[0];
+    CU(cudaSetDevice(c0->device));
+    if (n == 0) return AICB_OK;
+    if (append) indices = nullptr;
+    if (flags & ~AICB_BLOCKS_DERIVE_LIGHT) return fail(AICB_ERR_INVALID, "unknown flags");
+    for (size_t i = 0; i < n; i++) {
+        const aicb_block_desc &b = descs[i];
+        const std::string name = "block " + std::to_string(i) + "'s ";
+        if (b.indices && b.n_indices) TRY(check_device_pointer(b.indices, c0->device, false, 2, (name + "indices").c_str()));
+        if (b.palette && b.n_palette) TRY(check_device_pointer(b.palette, c0->device, false, 4, (name + "palette").c_str()));
+    }
+    const SpaceHost &h = *r.scene[0]->host;
+    const HostVerdict hv = host_checks(h, indices, descs, n);
+    const size_t n_scan = std::min(n, hv.at == SIZE_MAX ? n : hv.at + (hv.after_scan ? 1 : 0));
+    TRY(join_caller(r.ctx, r.n, caller));
+    DeviceDefs dev;
+    dev.kinds.assign(n, KIND_INVISIBLE);
+    unsigned long long bad = ~0ull;
+    if (n_scan) {   // verdict (16 bytes) and the kinds, read back together; then the jobs
+        std::vector<DeviceBlockJob> jobs(n_scan, DeviceBlockJob{});
+        uint64_t most = 0;
+        for (size_t i = 0; i < n_scan; i++) {
+            jobs[i].indices = descs[i].indices;
+            jobs[i].palette = descs[i].palette;
+            jobs[i].n_indices = descs[i].indices ? descs[i].n_indices : 0;
+            jobs[i].n_palette = (uint32_t)std::min<size_t>(descs[i].n_palette, 0xffffffffu);
+            jobs[i].single = single_source(descs[i]);
+            most = std::max(most, jobs[i].n_indices);
+        }
+        const size_t head = align256(sizeof(InputVerdict) + n_scan), job_bytes = n_scan * sizeof(DeviceBlockJob);
+        cudaStream_t stream = c0->stream.get();
+        TRY(inputs_room(c0, head + job_bytes));
+        char *p = c0->d_inputs.get<char>();
+        InputVerdict *v = (InputVerdict *)p;
+        DeviceBlockJob *d_jobs = (DeviceBlockJob *)(p + head);
+        CU(cudaMemcpyAsync(d_jobs, jobs.data(), job_bytes, cudaMemcpyHostToDevice, stream));
+        TRY(reset_verdict(v, stream));
+        TRY(issue_block_verdict(stream, d_jobs, (uint32_t)n_scan, most, v, (uint8_t *)(v + 1)));
+        std::vector<char> back(sizeof(InputVerdict) + n_scan);
+        CU(cudaMemcpyAsync(back.data(), p, back.size(), cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+        bad = ((const InputVerdict *)back.data())->first_bad;
+        std::memcpy(dev.kinds.data(), back.data() + sizeof(InputVerdict), n_scan);
+    }
+    // the host twin's first failure: block order, and within a block the scalars, the scan, the palette's size
+    if (bad != ~0ull && (bad < hv.at || (bad == hv.at && hv.after_scan))) return fail(AICB_ERR_INVALID, BAD_VOXEL_INDEX);
+    if (hv.at != SIZE_MAX) return fail(hv.st, hv.msg);
+    if (flags & AICB_BLOCKS_DERIVE_LIGHT) {
+        dev.derive = true;
+        TRY(derive_on_device(c0, descs, n, &dev.derived, &dev.d_derived));
+    }
+    TRY(indices ? update_blocks(r, indices, descs, n, &dev) : append_blocks(r, descs, n, &dev));
+    TRY(settle_replicas(r));
+    return release_caller(c0, caller);
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // C ABI
@@ -2113,6 +2353,16 @@ aicb_status aicb_scene_update_blocks(aicb_scene *s, const uint16_t *indices, con
 // TracingBlock::from_block of each, updating.rs:145-151): the blocks become the table's next indices.
 aicb_status aicb_scene_append_blocks(aicb_scene *s, const aicb_block_desc *descs, size_t n) {
     return on_scene(s, [&](Replicas r) { return scenes_append_blocks(r, descs, n); });
+}
+
+aicb_status aicb_scene_update_blocks_device(aicb_scene *s, const uint16_t *indices, const aicb_block_desc *descs,
+                                            size_t n, uint32_t flags, void *stream) {
+    return on_scene(s, [&](Replicas r) { return scenes_blocks_device(r, false, indices, descs, n, flags, (cudaStream_t)stream); });
+}
+
+aicb_status aicb_scene_append_blocks_device(aicb_scene *s, const aicb_block_desc *descs, size_t n, uint32_t flags,
+                                            void *stream) {
+    return on_scene(s, [&](Replicas r) { return scenes_blocks_device(r, true, nullptr, descs, n, flags, (cudaStream_t)stream); });
 }
 
 // == SpaceChange::EveryBlock (Mutation::fill_uniform over the whole bounds, space.rs:1461-1474).

@@ -1,0 +1,36 @@
+// block_words.cuh — what one palette entry of a block definition becomes in a scene's block table: its invisible flag
+// (the brick words' bit 15) and what the marching kernel needs of its surface, {alpha, an upper bound of
+// log2(1 - alpha)} (pal_tab).  __host__ __device__, so that the host flattening (aicb200.cu: flatten_block) and the
+// kernels that flatten definitions held in device memory (blocks.cu) evaluate one expression each, and their tables
+// are the same bytes.  tests/test_gpu_block_words.py checks surface_entry on the device against the host on every f32
+// bit pattern of alpha.
+#pragma once
+#include <cmath>
+
+#include <cuda_runtime.h>
+
+#include "../../include/aicb200.h"
+
+namespace aicb {
+
+// A voxel the marching kernel steps over (bit 15 of its brick word): fully transparent and not emissive.
+__host__ __device__ inline bool voxel_invisible(const aicb_voxel &v) {
+    return v.rgba[3] == 0.0f && v.emission[0] == 0.0f && v.emission[1] == 0.0f && v.emission[2] == 0.0f;
+}
+
+// {alpha, l2a}: l2a >= log2(1 - alpha) (the f32 value apply_transmittance raises to a span's thickness), so the
+// marching kernel's log-domain transmittance stays an upper bound.  log2 is evaluated in f64 (glibc's on the host,
+// libdevice's on the device), rounded to f32 and stepped up by one ulp.
+__host__ __device__ inline float2 surface_entry(float alpha) {
+    float l2a;
+    if (alpha >= 1.0f) l2a = -INFINITY;
+    else if (!(alpha > 0.0f)) l2a = 0.0f;
+    else {
+        const float unit_t = 1.0f - alpha;
+        l2a = nextafterf((float)log2((double)unit_t), INFINITY);
+        if (l2a > 0.0f) l2a = 0.0f;
+    }
+    return make_float2(alpha, l2a);
+}
+
+}  // namespace aicb

@@ -309,8 +309,13 @@ aicb_block_light single_light(const aicb_voxel &v) {
     return o;
 }
 
-aicb_status derive(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, aicb_block_light *out) {
-    std::vector<aicb_block_light> result(n);
+// compute_derived of n validated blocks: into `out` (host memory), or with on_device (the blocks' voxels in the
+// context's device memory, copied device to device into the kernels' inputs) left in d_derive, each block's record
+// in *rec (LIGHT_SINGLE: a single voxel, which the caller derives from its voxel) and the records at *d_out.
+aicb_status derive(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, aicb_block_light *out, bool on_device = false,
+                   std::vector<int32_t> *rec = nullptr, const aicb_block_light **d_out_ptr = nullptr) {
+    std::vector<aicb_block_light> result(on_device ? 0 : n);
+    if (on_device) rec->assign(n, LIGHT_SINGLE);
     std::vector<DeriveRec> recs;
     std::vector<size_t> rec_block;   // per record: its position in descs
     uint64_t n_vox = 0, n_rays = 0;
@@ -318,9 +323,10 @@ aicb_status derive(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, aicb_b
     for (size_t i = 0; i < n; i++) {
         const aicb_block_desc &b = descs[i];
         if (is_single_voxel(b)) {
-            result[i] = single_light(single_voxel_of(b));
+            if (!on_device) result[i] = single_light(single_voxel_of(b));
             continue;
         }
+        if (on_device) (*rec)[i] = (int32_t)recs.size();
         DeriveRec R;
         std::memset(&R, 0, sizeof R);
         R.vox_off = n_vox;
@@ -360,11 +366,21 @@ aicb_status derive(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, aicb_b
         for (uint32_t r = 0; r < n_recs; r++) {
             const aicb_block_desc &b = descs[rec_block[r]];
             std::fill(h_pal_rec + recs[r].pal_off, h_pal_rec + recs[r].pal_off + b.n_palette, r);
+            if (on_device) continue;
             if (b.n_palette) std::memcpy(h + up_pal + recs[r].pal_off * sizeof(aicb_voxel), b.palette, b.n_palette * sizeof(aicb_voxel));
             if (b.n_indices) std::memcpy(h + up_idx + recs[r].vox_off * 2, b.indices, b.n_indices * 2);
         }
         char *d = ctx->d_delta.get<char>();
-        CU(cudaMemcpyAsync(d, h, up_bytes, cudaMemcpyHostToDevice, stream));
+        CU(cudaMemcpyAsync(d, h, on_device ? up_pal : up_bytes, cudaMemcpyHostToDevice, stream));
+        for (uint32_t r = 0; on_device && r < n_recs; r++) {
+            const aicb_block_desc &b = descs[rec_block[r]];
+            if (b.n_palette)
+                CU(cudaMemcpyAsync(d + up_pal + recs[r].pal_off * sizeof(aicb_voxel), b.palette,
+                                   b.n_palette * sizeof(aicb_voxel), cudaMemcpyDeviceToDevice, stream));
+            if (b.n_indices)
+                CU(cudaMemcpyAsync(d + up_idx + recs[r].vox_off * 2, b.indices, b.n_indices * 2,
+                                   cudaMemcpyDeviceToDevice, stream));
+        }
         CU(cudaEventRecord(ctx->ev_delta.get(), stream));
         // scratch: palette terms, ray terms, per-record flags and errors, results
         const size_t s_pal = 0, s_rays = align16((size_t)n_pal * 32), s_flags = s_rays + n_rays * 32;
@@ -395,9 +411,10 @@ aicb_status derive(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, aicb_b
         k_derive_reduce<<<(n_recs + REDUCE_BLOCKS - 1) / REDUCE_BLOCKS, REDUCE_BLOCKS * 6, 0, stream>>>(
             d_recs, n_recs, ray_terms, flags, d_out, err);
         CU(cudaGetLastError());
-        std::vector<aicb_block_light> lights(n_recs);
+        std::vector<aicb_block_light> lights(on_device ? 0 : n_recs);
         std::vector<uint32_t> errs(n_recs);
-        CU(cudaMemcpyAsync(lights.data(), d_out, n_recs * sizeof(aicb_block_light), cudaMemcpyDeviceToHost, stream));
+        if (on_device) *d_out_ptr = d_out;
+        else CU(cudaMemcpyAsync(lights.data(), d_out, n_recs * sizeof(aicb_block_light), cudaMemcpyDeviceToHost, stream));
         CU(cudaMemcpyAsync(errs.data(), err, n_recs * 4, cudaMemcpyDeviceToHost, stream));
         CU(cudaStreamSynchronize(stream));
         for (uint32_t r = 0; r < n_recs; r++) {
@@ -405,14 +422,20 @@ aicb_status derive(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, aicb_b
                 return aicb_fail(AICB_ERR_INVALID, "block " + std::to_string(rec_block[r]) +
                                                        ": its colour or emission sum is NaN or negative, where "
                                                        "compute_derived's Rgb::try_from(..).expect(..) panics");
-            result[rec_block[r]] = lights[r];
+            if (!on_device) result[rec_block[r]] = lights[r];
         }
     }
-    std::memcpy(out, result.data(), n * sizeof(aicb_block_light));
+    if (!on_device) std::memcpy(out, result.data(), n * sizeof(aicb_block_light));
     return AICB_OK;
 }
 
 }  // namespace
+
+aicb_status derive_on_device(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, std::vector<int32_t> *rec,
+                             const aicb_block_light **out) {
+    *out = nullptr;
+    return derive(ctx, descs, n, nullptr, true, rec, out);
+}
 
 extern "C" aicb_status aicb_derive_block_light(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n,
                                                aicb_block_light *out) {

@@ -568,6 +568,20 @@ aicb_status aicb_group_scene_append_blocks(aicb_group_scene *gs, const aicb_bloc
     return on_group(gs, false, [&](Replicas r) { return scenes_append_blocks(r, descs, n); });
 }
 
+aicb_status aicb_group_scene_update_blocks_device(aicb_group_scene *gs, const uint16_t *indices,
+                                                  const aicb_block_desc *descs, size_t n, uint32_t flags, void *stream) {
+    return on_group(gs, false, [&](Replicas r) {
+        return scenes_blocks_device(r, false, indices, descs, n, flags, (cudaStream_t)stream);
+    });
+}
+
+aicb_status aicb_group_scene_append_blocks_device(aicb_group_scene *gs, const aicb_block_desc *descs, size_t n,
+                                                  uint32_t flags, void *stream) {
+    return on_group(gs, false, [&](Replicas r) {
+        return scenes_blocks_device(r, true, nullptr, descs, n, flags, (cudaStream_t)stream);
+    });
+}
+
 aicb_status aicb_group_scene_fill_uniform(aicb_group_scene *gs, const aicb_block_desc *block) {
     return on_group(gs, false, [&](Replicas r) { return scenes_fill_uniform(r, block); });
 }

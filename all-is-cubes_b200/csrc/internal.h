@@ -378,8 +378,13 @@ aicb_status check_block_desc(const aicb_block_desc &b);
 inline bool is_single_voxel(const aicb_block_desc &b) { return b.indices == nullptr || b.resolution == 1; }
 aicb_voxel single_voxel_of(const aicb_block_desc &b);
 
-// light.cu: the light-side record of a block definition.
-LightBlockDev light_block(const aicb_block_desc &b);
+// The check_block_desc checks that read no voxel, in its order: those before its index scan (resolution, n_indices
+// against voxel_bounds, the bounds, NULL palettes) and the one after it (a palette over 65536 entries).
+aicb_status check_block_scalars(const aicb_block_desc &b);
+aicb_status check_block_palette(const aicb_block_desc &b);
+
+// blocks.cu: the light-side record of a block definition.
+__host__ __device__ LightBlockDev light_block(const aicb_block_desc &b);
 
 // ---- calls over several contexts ----------------------------------------------------------------------------------
 // A device group (group.cu): one context per listed device, device 0's first; every other device reaches device 0's
@@ -473,6 +478,7 @@ aicb_status scenes_update_region(Replicas r, const aicb_aab *region, const uint1
 // writes are done.
 struct InputVerdict {
     unsigned long long first_bad;   // 2 * i + 0: entry i's cube out of bounds; + 1: its id past the table; ~0: none
+                                    // (block definitions, k_block_verdict: i, the first with a bad voxel index)
     uint32_t count;                 // the entries the call applies: distinct cubes, or changing entries
     uint32_t _pad;
 };
@@ -514,6 +520,49 @@ aicb_status scenes_upload_light_device(Replicas r, const uint8_t (*light)[4], si
 aicb_status scene_download_ids_device(Replicas r, uint16_t *out, size_t n, cudaStream_t caller);
 aicb_status scenes_update_blocks(Replicas r, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks);
 aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_t n_blocks);
+// The same with each definition's indices and palette in device 0's memory (aicb_scene_update_blocks_device and
+// aicb_scene_append_blocks_device).  `flags`: AICB_BLOCKS_*.
+aicb_status scenes_blocks_device(Replicas r, bool append, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks,
+                                 uint32_t flags, cudaStream_t caller);
+
+// blocks.cu: one definition whose voxel data is in device memory, as its kernels read it.  aicb200.cu fills it from the
+// descriptor and the table's bookkeeping; the kernels take the caller's pointers as they are.
+enum : uint32_t { SINGLE_NONE = 0, SINGLE_AIR = 1, SINGLE_FIRST = 2, SINGLE_INDEXED = 3 };   // single_voxel_of
+constexpr uint32_t NO_ID = ~0u, NO_WORD = ~0u;
+constexpr int32_t LIGHT_GIVEN = -1, LIGHT_SINGLE = -2;
+struct DeviceBlockJob {
+    const uint16_t *indices;     // the caller's, Z-major (nullptr: none)
+    const aicb_voxel *palette;   // the caller's
+    uint64_t n_indices;
+    uint32_t n_palette;
+    uint32_t single;             // SINGLE_*: a single-voxel block's voxel (SINGLE_NONE: not a single voxel)
+    uint32_t kind;               // KIND_*
+    uint32_t brick_off;          // its brick words' first pool position (recursive)
+    uint32_t pal_off;            // its palette entries' first pool position
+    uint32_t n_entries;          // palette entries it adds: 0 (air), 1 (single voxel) or n_palette
+    uint32_t id;                 // the id whose records it writes; NO_ID: a later definition of the call writes them
+    int32_t derived;             // its light record: LIGHT_GIVEN (`light`), LIGHT_SINGLE (its voxel's) or derive's record
+    uint32_t light_visible;      // ORed into Derived::visible
+    uint32_t _pad;
+    aicb::BlockRec rec;
+    LightBlockDev light;
+};
+// k_block_verdict over jobs [0, n) on `stream`: v->first_bad = the first job with a voxel index past its palette
+// (v reset by the caller), kinds[i] = the kind of job i's single voxel.
+aicb_status issue_block_verdict(cudaStream_t stream, const DeviceBlockJob *jobs, uint32_t n, uint64_t most_indices,
+                                InputVerdict *v, uint8_t *kinds);
+// The jobs' brick words, palette entries and per-id records into table `t` (room made, positions in the jobs);
+// `derived`: derive's records (device 0's memory), or nullptr.
+aicb_status issue_block_data(cudaStream_t stream, const DeviceBlockJob *jobs, uint32_t n, uint64_t most_words,
+                             uint64_t most_entries, bool wide_bricks, const BlockTable &t,
+                             const aicb_block_light *derived);
+// Every cell whose id has word[id] != NO_WORD takes that word, on the context's stream.
+aicb_status issue_rekind_cells(const aicb_ctx *ctx, void *cells, bool wide, size_t n, const uint32_t *word);
+// derive.cu: aicb_derive_block_light's kernels on definitions whose voxel data is in the context's device memory,
+// the per-block error words read back.  For each block, rec[i] is its record in *out (device memory, valid until the
+// context's next derive), or LIGHT_SINGLE for a single voxel, which is its own derived data.
+aicb_status derive_on_device(aicb_ctx *ctx, const aicb_block_desc *descs, size_t n, std::vector<int32_t> *rec,
+                             const aicb_block_light **out);
 aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block);
 aicb_status scenes_upload_light(Replicas r, const uint8_t (*light)[4], size_t n_texels);
 // Space::set_physics over the replicas.

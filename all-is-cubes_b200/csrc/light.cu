@@ -1326,21 +1326,6 @@ aicb_status propagate(Replicas r, uint8_t epsilon, uint64_t *updates_done, uint8
 
 }  // namespace
 
-// The light-side record of a block definition (internal.h): its face colours, emission and flags.
-LightBlockDev light_block(const aicb_block_desc &b) {
-    LightBlockDev o;
-    std::memset(&o, 0, sizeof o);
-    std::memcpy(o.face_color[0], b.light_color, 16);
-    for (int f = 0; f < 6; f++) std::memcpy(o.face_color[f + 1], b.light_face_colors[f], 16);
-    std::memcpy(o.emission, b.light_emission, 12);
-    uint32_t fl = b.light_opaque_faces & 0x3f;
-    if (fl == 0x3f) fl |= LB_ALL_OPAQUE;
-    if (b.light_visible) fl |= LB_VISIBLE;
-    if (!(b.light_emission[0] == 0.0f && b.light_emission[1] == 0.0f && b.light_emission[2] == 0.0f)) fl |= LB_EMISSIVE;
-    o.flags = fl;
-    return o;
-}
-
 // ---------------------------------------------------------------------------------------------
 // a scene's light state (internal.h)
 // ---------------------------------------------------------------------------------------------

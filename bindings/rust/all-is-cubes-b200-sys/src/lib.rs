@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 21 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 22 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -13,6 +13,9 @@ pub const AICB_ERR_CUDA: aicb_status = 3;
 pub const AICB_ERR_UNSUPPORTED: aicb_status = 4;
 pub const AICB_ERR_BUSY: aicb_status = 5;
 pub const AICB_ERR_RETRY: aicb_status = 6;
+
+/// aicb_scene_*_blocks_device flags: light_* come from compute_derived on the device.
+pub const AICB_BLOCKS_DERIVE_LIGHT: u32 = 1;
 
 pub const AICB_TEXT_ENTERED_SPACE: i32 = -1;
 pub const AICB_TEXT_EMPTY: i32 = -2;
@@ -302,6 +305,11 @@ unsafe extern "C" {
                                          stream: *mut c_void) -> aicb_status;
     pub fn aicb_light_download_device(s: *mut aicb_scene, d_out: *mut [u8; 4], n_texels: usize,
                                       stream: *mut c_void) -> aicb_status;
+    // descs[i].indices and descs[i].palette in the scene's device memory; `indices` and the descriptors on the host
+    pub fn aicb_scene_update_blocks_device(s: *mut aicb_scene, indices: *const u16, descs: *const aicb_block_desc,
+                                           n: usize, flags: u32, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_scene_append_blocks_device(s: *mut aicb_scene, descs: *const aicb_block_desc, n: usize, flags: u32,
+                                           stream: *mut c_void) -> aicb_status;
 
     pub fn aicb_shard_pixel_count(cam: *const aicb_camera, shard: *const aicb_shard) -> usize;
     pub fn aicb_render_srgb8(s: *mut aicb_scene, cam: *const aicb_camera, opt: *const aicb_options, shard: *const aicb_shard,
@@ -396,6 +404,11 @@ unsafe extern "C" {
                                                n_changed_or_null: *mut usize, stream: *mut c_void) -> aicb_status;
     pub fn aicb_group_light_download_device(gs: *mut aicb_group_scene, d_out: *mut [u8; 4], n_texels: usize,
                                             stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_scene_update_blocks_device(gs: *mut aicb_group_scene, indices: *const u16,
+                                                 descs: *const aicb_block_desc, n: usize, flags: u32,
+                                                 stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_scene_append_blocks_device(gs: *mut aicb_group_scene, descs: *const aicb_block_desc, n: usize,
+                                                 flags: u32, stream: *mut c_void) -> aicb_status;
     // aicb_render_layers_* on a group: both layers must be scenes of the same group
     pub fn aicb_group_render_layers_srgb8(world: *const aicb_group_layer, ui: *const aicb_group_layer,
                                           backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 21
+#define AICB_ABI_VERSION 22
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -344,6 +344,25 @@ aicb_status aicb_light_edit_region_device(aicb_scene *, const aicb_aab *region, 
                                           uint16_t uniform_id, size_t *n_changed_or_null, void *stream);
 /* aicb_light_download into u8[volume][4] at d_out: a device-to-device copy; does not synchronise on one context. */
 aicb_status aicb_light_download_device(aicb_scene *, uint8_t (*d_out)[4], size_t n_texels, void *stream);
+/* aicb_scene_update_blocks and aicb_scene_append_blocks with each descriptor's `indices` (u16, Z-major, 2-byte aligned)
+ * and `palette` (4-byte aligned) in the scene's device memory; `indices`, the descriptor array and every scalar field
+ * stay on the host.  The scene ends as the host twin leaves it with the same data: frames, aicb_scene_device_bytes,
+ * light records, cells, compaction, widening.  The host checks what the scalars decide; a kernel checks every voxel
+ * index and reads each single voxel's kind, and those bytes are all that is read back before anything is placed
+ * (with AICB_BLOCKS_DERIVE_LIGHT, derive's error words are read back after them).  The
+ * status and message are the host twin's first; a rejected call changes nothing.  The voxel data is written into the
+ * pools on the device, and the cubes of a block whose kind changes are re-encoded on the device, without the host
+ * mirror of the block ids.  Ordering is the device calls'; an update also waits for the frame in flight, as
+ * aicb_scene_update_blocks does, and both return once their writes are done.  Light is not touched.
+ * flags: AICB_BLOCKS_DERIVE_LIGHT ignores the descriptors' light_face_colors, light_color, light_emission and
+ * light_opaque_faces and takes them from aicb_derive_block_light's kernels run on the same buffers; light_visible becomes
+ * Derived::visible OR the descriptor's light_visible (an animation hint).  A NaN or negative sum fails as
+ * aicb_derive_block_light does, naming the block, and changes nothing.  GPU test: tests/test_gpu_device_blocks.py. */
+#define AICB_BLOCKS_DERIVE_LIGHT 1u
+aicb_status aicb_scene_update_blocks_device(aicb_scene *, const uint16_t *indices, const aicb_block_desc *descs,
+                                            size_t n, uint32_t flags, void *stream);
+aicb_status aicb_scene_append_blocks_device(aicb_scene *, const aicb_block_desc *descs, size_t n, uint32_t flags,
+                                            void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * draw(): replaces RtRenderer::draw_rgba / RtRenderer::draw::<ColorBuf> and the Rayon pixel
@@ -613,6 +632,12 @@ aicb_status aicb_group_light_edit_region_device(aicb_group_scene *, const aicb_a
                                                 const uint16_t *d_ids_or_null, uint16_t uniform_id,
                                                 size_t *n_changed_or_null, void *stream);
 aicb_status aicb_group_light_download_device(aicb_group_scene *, uint8_t (*d_out)[4], size_t n_texels, void *stream);
+/* The block definitions' voxels are device 0's memory, checked once there; every replica's kernels read them over
+ * peer access and every replica's table ends identical.  Returns once every replica's writes are done. */
+aicb_status aicb_group_scene_update_blocks_device(aicb_group_scene *, const uint16_t *indices,
+                                                  const aicb_block_desc *descs, size_t n, uint32_t flags, void *stream);
+aicb_status aicb_group_scene_append_blocks_device(aicb_group_scene *, const aicb_block_desc *descs, size_t n,
+                                                  uint32_t flags, void *stream);
 
 /* == RtScene::trace_ray_through_layers + draw_rgba (renderer.rs:454-478, 282-308) and RaytraceToTexture::do_some_tracing's
  * trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) on the whole group: the arguments, the validation and
