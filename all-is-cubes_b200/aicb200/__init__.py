@@ -106,6 +106,9 @@ def load_library() -> C.CDLL:
     lib.aicb_group_destroy.restype = None
     lib.aicb_group_size.argtypes = [C.c_void_p]
     lib.aicb_group_scene_create.argtypes = [C.c_void_p, C.POINTER(abi.SceneDesc), C.POINTER(C.c_void_p)]
+    for name in ("aicb_scene_create_device", "aicb_group_scene_create_device"):
+        getattr(lib, name).argtypes = [C.c_void_p, C.POINTER(abi.SceneDesc), C.c_uint32, C.c_void_p,
+                                       C.POINTER(C.c_void_p)]
     lib.aicb_group_scene_destroy.argtypes = [C.c_void_p]
     lib.aicb_group_scene_destroy.restype = None
     lib.aicb_group_render_srgb8.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p,
@@ -181,6 +184,7 @@ def load_library() -> C.CDLL:
         "light_download_device": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p],
         "scene_update_blocks_device": [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p],
         "scene_append_blocks_device": [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p],
+        "scene_fill_uniform_device": [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p],
     }.items():
         for prefix in ("aicb_", "aicb_group_"):
             getattr(lib, prefix + name).argtypes = argtypes
@@ -648,6 +652,76 @@ class Space:
         return d, keep
 
 
+class DeviceSpace:
+    """Space's device twin, as DeviceBlock is Block's, for a world that lives on the GPU: SpaceRaytracer, GroupScene,
+    DeviceGroup.add_scene / update and RtRenderer.update create the scene from it on the device
+    (aicb_scene_create_device), on the device's current torch stream.  `block_ids` is a contiguous uint16 CUDA tensor
+    [X, Y, Z] (Z-major); `light` a contiguous uint8 tensor [X, Y, Z, 4] on the same device, or None; `blocks` are
+    DeviceBlocks whose light is given for all of them, or derived on the device for all (light=None).  The tensors
+    must stay unchanged until the scene is created; the scene does not keep them."""
+
+    def __init__(self, lower, block_ids, blocks: Sequence["DeviceBlock"], light=None, sky_colors=None,
+                 light_max_distance: int = 0):
+        torch = _torch()
+        if (not _is_cuda_tensor(block_ids) or block_ids.dtype != torch.uint16 or block_ids.dim() != 3
+                or not block_ids.is_contiguous()):
+            raise ValueError("DeviceSpace.block_ids must be a contiguous uint16 CUDA tensor [X, Y, Z]")
+        self.device = block_ids.device
+        self.lower = tuple(int(v) for v in lower)
+        self.block_ids = block_ids
+        self.size = tuple(int(v) for v in block_ids.shape)
+        if light is not None and (not _is_cuda_tensor(light) or light.dtype != torch.uint8 or light.device != self.device
+                                  or tuple(light.shape) != self.size + (4,) or not light.is_contiguous()):
+            raise ValueError(f"DeviceSpace.light must be a contiguous uint8 tensor {list(self.size) + [4]} on "
+                             f"{self.device}, or None")
+        self.light = light
+        self.blocks = list(blocks)
+        if not all(isinstance(b, DeviceBlock) for b in self.blocks):
+            raise ValueError("DeviceSpace.blocks must all be DeviceBlocks")
+        derive = [b.light is None for b in self.blocks]
+        if any(derive) and not all(derive):
+            raise ValueError("a DeviceSpace derives the light of every block (light=None) or of none")
+        for b in self.blocks:
+            b._check(self.device)
+        self.flags = abi.BLOCKS_DERIVE_LIGHT if any(derive) else 0
+        if sky_colors is None:
+            sky_colors = [srgb8_to_linear((243, 243, 255))]
+        self.sky_colors = _sky_colors(sky_colors)
+        self.light_max_distance = int(light_max_distance)
+
+    def to_desc(self, device):
+        """Returns (abi.SceneDesc with device pointers, keepalive list); ValueError unless the tensors are on
+        `device`."""
+        if self.device != device:
+            raise ValueError(f"the DeviceSpace's tensors are on {self.device}, the scene's device is {device}")
+        d = abi.SceneDesc()
+        d.bounds.lower[:] = self.lower
+        d.bounds.size[:] = self.size
+        d.block_ids = self.block_ids.data_ptr()
+        d.light = self.light.data_ptr() if self.light is not None else None
+        arr = (abi.BlockDesc * max(len(self.blocks), 1))()
+        for i, b in enumerate(self.blocks):
+            b.fill_desc(arr[i])
+        d.blocks = arr
+        d.n_blocks = len(self.blocks)
+        d.sky = _sky(self.sky_colors)
+        d.light_max_distance = self.light_max_distance
+        return d, [arr, self]
+
+
+def _create_scene(fn, owner, space, device, out):
+    """aicb_scene_create or aicb_group_scene_create (`fn`) on `owner`; a DeviceSpace through their device form on the
+    device's current torch stream."""
+    lib = load_library()
+    if isinstance(space, DeviceSpace):
+        desc, keep = space.to_desc(device)
+        _check(getattr(lib, fn + "_device")(owner, C.byref(desc), space.flags, _stream(device), C.byref(out)))
+    else:
+        desc, keep = space.to_desc()
+        _check(getattr(lib, fn)(owner, C.byref(desc), C.byref(out)))
+    del keep
+
+
 def _sky_colors(sky_colors) -> np.ndarray:
     """One row: Sky::Uniform; eight rows: Sky::Octants (index (x>=0)<<2 | (y>=0)<<1 | (z>=0))."""
     c = np.asarray(sky_colors, dtype=np.float32).reshape(-1, 3)
@@ -1062,7 +1136,12 @@ class _Scene:
 
     def fill_uniform(self, block):
         """SpaceChange::EveryBlock (Mutation::fill_uniform over the whole Space): the table becomes [block] and every
-        cube holds id 0.  Light is not touched: on a lit scene, light_queue_region(bounds, 210) follows."""
+        cube holds id 0.  Light is not touched: on a lit scene, light_queue_region(bounds, 210) follows.  A DeviceBlock
+        is read on the device, as in update_blocks."""
+        dev = self._device_blocks([block])
+        if dev is not None:
+            _check(self._fn("scene_fill_uniform_device")(self.handle, dev[0], dev[1], _stream(self._device())))
+            return
         arr = _block_descs([block])
         _check(self._fn("scene_fill_uniform")(self.handle, arr))
 
@@ -1248,10 +1327,8 @@ class SpaceRaytracer(_Scene):
         self.ctx = ctx or Context.default()
         self.graphics_options = graphics_options.repair()
         self.space = space
-        desc, keep = space.to_desc()
         self.handle = C.c_void_p()
-        _check(load_library().aicb_scene_create(self.ctx.handle, C.byref(desc), C.byref(self.handle)))
-        del keep
+        _create_scene("aicb_scene_create", self.ctx.handle, space, _ctx_device(self.ctx), self.handle)
 
     def __del__(self):
         try:
@@ -1696,10 +1773,8 @@ class GroupScene(_Scene):
     def __init__(self, group: "DeviceGroup", space: "Space"):
         self.group = group
         self.space = space
-        desc, keep = space.to_desc()
         self.handle = C.c_void_p()
-        _check(load_library().aicb_group_scene_create(group.handle, C.byref(desc), C.byref(self.handle)))
-        del keep
+        _create_scene("aicb_group_scene_create", group.handle, space, group._device(), self.handle)
 
     def _device(self):
         return self.group._device()

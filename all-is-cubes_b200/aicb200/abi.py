@@ -1,7 +1,7 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 22
+ABI_VERSION = 23
 
 BLOCKS_DERIVE_LIGHT = 1
 
@@ -189,6 +189,8 @@ EXPORTED_SYMBOLS = [
     "aicb_light_download_device",
     "aicb_scene_update_blocks_device",
     "aicb_scene_append_blocks_device",
+    "aicb_scene_create_device",
+    "aicb_scene_fill_uniform_device",
     "aicb_shard_pixel_count",
     "aicb_render_srgb8",
     "aicb_render_rgba16f",
@@ -259,6 +261,8 @@ EXPORTED_SYMBOLS = [
     "aicb_group_light_download_device",
     "aicb_group_scene_update_blocks_device",
     "aicb_group_scene_append_blocks_device",
+    "aicb_group_scene_create_device",
+    "aicb_group_scene_fill_uniform_device",
     "aicb_group_render_layers_srgb8",
     "aicb_group_render_layers_texture",
     "aicb_group_render_layers_terminal",

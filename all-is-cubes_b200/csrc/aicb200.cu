@@ -1205,6 +1205,18 @@ static void device_jobs(const SpaceHost &h, const aicb_block_desc *descs, const 
     }
 }
 
+// copy's device form: the jobs go up through the context's staging and blocks.cu's kernels write table `t` on the
+// context's stream, reading the caller's buffers on device 0 (as a peer on the other devices).
+static aicb_status copy_device(aicb_ctx *ctx, const BlockTable &t, const FlatBlocks &f, const DeviceDefs &dev) {
+    cudaStream_t stream = ctx->stream.get();
+    const size_t bytes = dev.jobs.size() * sizeof(DeviceBlockJob);
+    TRY(delta_room(ctx, bytes));
+    std::memcpy(ctx->h_delta.get(), dev.jobs.data(), bytes);
+    CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
+    return issue_block_data(stream, ctx->d_delta.get<const DeviceBlockJob>(), (uint32_t)dev.jobs.size(),
+                            dev.most_words, dev.most_entries, f.wide_bricks, t, dev.d_derived);
+}
+
 static aicb_status place(Replicas r, const FlatBlocks &f, const uint16_t *indices, const DeviceDefs *dev) {
     SpaceHost &h = *r.scene[0]->host;
     for (size_t i = 0; i < r.n; i++) {
@@ -1220,16 +1232,8 @@ static aicb_status place(Replicas r, const FlatBlocks &f, const uint16_t *indice
         aicb_ctx *ctx = r.ctx[i];
         cudaStream_t stream = ctx->stream.get();
         CU(cudaSetDevice(ctx->device));
-        if (!dev) {
-            TRY(copy(r.scene[i]->blocks, h, f, indices, stream));
-        } else {   // each replica's kernels read the caller's buffers on device 0 (as a peer on the others)
-            const size_t bytes = dev->jobs.size() * sizeof(DeviceBlockJob);
-            TRY(delta_room(ctx, bytes));
-            std::memcpy(ctx->h_delta.get(), dev->jobs.data(), bytes);
-            CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
-            TRY(issue_block_data(stream, ctx->d_delta.get<const DeviceBlockJob>(), (uint32_t)dev->jobs.size(),
-                                 dev->most_words, dev->most_entries, f.wide_bricks, r.scene[i]->blocks, dev->d_derived));
-        }
+        if (!dev) TRY(copy(r.scene[i]->blocks, h, f, indices, stream));
+        else TRY(copy_device(ctx, r.scene[i]->blocks, f, *dev));
         CU(cudaEventRecord(ctx->ev_delta.get(), stream));
     }
     book(h, f, indices);
@@ -1342,36 +1346,49 @@ static aicb_status compact_pools(Replicas r, bool bricks, bool palette) {
     return AICB_OK;
 }
 
-aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out) {
+// Scene creation's checks before it reads a block, in order: the bounds, then the NULLs.  *volume: the bounds' cubes.
+static aicb_status check_scene_desc(const aicb_scene_desc *d, uint64_t *volume) {
     const int64_t LIM = 1 << 30;
-    uint64_t volume = 1;
+    *volume = 1;
     for (int a = 0; a < 3; a++) {
         int64_t lo = d->bounds.lower[a], hi = lo + (int64_t)d->bounds.size[a];
         if (lo < -LIM || hi > LIM) return fail(AICB_ERR_INVALID, "space bounds must lie within +-2^30");
-        volume *= d->bounds.size[a];
-        if (volume > (1ull << 31)) return fail(AICB_ERR_INVALID, "space volume exceeds 2^31 cubes");
+        *volume *= d->bounds.size[a];
+        if (*volume > (1ull << 31)) return fail(AICB_ERR_INVALID, "space volume exceeds 2^31 cubes");
     }
-    if (volume && !d->block_ids) return fail(AICB_ERR_INVALID, "block_ids is NULL");
-    if (volume && d->n_blocks == 0) return fail(AICB_ERR_INVALID, "non-empty space with an empty block table");
+    if (*volume && !d->block_ids) return fail(AICB_ERR_INVALID, "block_ids is NULL");
+    if (*volume && d->n_blocks == 0) return fail(AICB_ERR_INVALID, "non-empty space with an empty block table");
     if (d->n_blocks && !d->blocks) return fail(AICB_ERR_INVALID, "blocks is NULL");
+    return AICB_OK;
+}
+
+// A new scene's cells from the caller's ids (Z-major over the bounds, device memory the scene's device reaches):
+// region_cells over boxes of whole x layers, or of one layer's whole rows, small enough that their work items (at
+// most 2^30) are counted in 32 bits.  Each box's ids are one contiguous run of the caller's array.
+static aicb_status device_cells(aicb_scene *s, const uint16_t *ids) {
+    const uint32_t sx = (uint32_t)s->ds.size[0], sy = (uint32_t)s->ds.size[1], sz = (uint32_t)s->ds.size[2];
+    const uint64_t LIMIT = 1ull << 30, row_items = (sz + (s->ds.wide_cells ? 3 : 7)) / (s->ds.wide_cells ? 4 : 8) + 1;
+    const uint32_t ny = (uint32_t)std::min<uint64_t>(sy, std::max<uint64_t>(1, LIMIT / row_items));
+    const uint32_t nx = ny < sy ? 1 : (uint32_t)std::min<uint64_t>(sx, std::max<uint64_t>(1, LIMIT / (row_items * sy)));
+    for (uint32_t x = 0; x < sx; x += nx)
+        for (uint32_t y = 0; y < sy; y += ny) {
+            const RegionBox box = {{x, y, 0}, {std::min(nx, sx - x), std::min(ny, sy - y), sz}};
+            TRY(region_cells(s, box, ids + ((size_t)x * sy + y) * sz, 0, nullptr, true, nullptr, nullptr));
+        }
+    return AICB_OK;
+}
+
+// The body of scene creation, host and device form, once the definitions are flattened (f, against an empty table):
+// one scene per context, complete when it is returned (until then a failure frees every scene made), and then the
+// host part, once.  The host form (dev == nullptr) uploads `cells`, encoded on the host, and the light.  The device
+// form writes each replica's table with blocks.cu's kernels, encodes its cells from the caller's ids with
+// k_region_cells (the kinds from the records just written) and copies the light, each replica reading device 0's
+// buffers (as a peer on the other devices); its host mirror of the ids starts stale (refresh_mirror).
+static aicb_status create_scenes(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, uint64_t volume,
+                                 const FlatBlocks &f, const void *cells, const DeviceDefs *dev, aicb_scene **out) {
     auto host = std::make_unique<SpaceHost>();   // empty until every replica holds the table
-    FlatBlocks f;
-    TRY(flatten_blocks(*host, d->blocks, d->n_blocks, nullptr, &f));
-
-    // ---- cells: block id with its kind in the top bits --------------------------------------------------------------
     const bool wide = d->n_blocks > 16384;
-    std::vector<uint16_t> cells16(wide ? 0 : volume);
-    std::vector<uint32_t> cells32(wide ? volume : 0);
-    for (size_t i = 0; i < volume; i++) {
-        const uint16_t id = d->block_ids[i];
-        if (id >= d->n_blocks) return fail(AICB_ERR_INVALID, "block id out of range");
-        if (wide) cells32[i] = cell_word(id, f.kinds[id], true);
-        else cells16[i] = (uint16_t)cell_word(id, f.kinds[id], false);
-    }
-    const void *cells = wide ? (const void *)cells32.data() : cells16.data();
     const size_t cell_bytes = volume * (wide ? 4 : 2);
-
-    // ---- one scene per context, complete when it is returned; until then a failure frees it ------------------------
     auto create = [&](aicb_ctx *c, aicb_scene **o) {
         CU(cudaSetDevice(c->device));
         std::unique_ptr<aicb_scene> s(new aicb_scene());
@@ -1384,10 +1401,17 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
         }
         ds.wide_cells = wide ? 1 : 0;
         if (volume) {
-            TRY(s->d_cells.upload(cells, cell_bytes));
+            if (dev) TRY(s->d_cells.ensure(cell_bytes));
+            else TRY(s->d_cells.upload(cells, cell_bytes));
             s->device_bytes += cell_bytes;
             if (d->light) {
-                TRY(s->d_light.upload(d->light, volume * 4));
+                if (dev) {
+                    TRY(s->d_light.ensure(volume * 4));
+                    CU(cudaMemcpyPeerAsync(s->d_light.get(), c->device, d->light, ctx[0]->device, volume * 4,
+                                           c->stream.get()));
+                } else {
+                    TRY(s->d_light.upload(d->light, volume * 4));
+                }
                 s->device_bytes += volume * 4;
             }
         }
@@ -1398,7 +1422,13 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
         Retired retired{c, {}};   // (a new table replaces no array)
         TRY(room(s->blocks, *host, f, nullptr, c->stream.get(), retired));
         s->blocks.bind(ds);
-        TRY(copy(s->blocks, *host, f, nullptr, c->stream.get()));
+        if (dev) {
+            TRY(copy_device(c, s->blocks, f, *dev));
+            if (volume) TRY(device_cells(s.get(), d->block_ids));
+            CU(cudaEventRecord(c->ev_delta.get(), c->stream.get()));
+        } else {
+            TRY(copy(s->blocks, *host, f, nullptr, c->stream.get()));
+        }
         CU(cudaStreamSynchronize(c->stream.get()));
         *o = s.release();
         return AICB_OK;
@@ -1411,11 +1441,32 @@ aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc 
         }
     }
     host->volume = (size_t)volume;
-    host->h_ids.assign(d->block_ids, d->block_ids + volume);
+    if (dev) host->ids_stale = true;
+    else host->h_ids.assign(d->block_ids, d->block_ids + volume);
     host->light_max_distance = d->light_max_distance;
     book(*host, f, nullptr);
     out[0]->own_host = std::move(host);
     return AICB_OK;
+}
+
+aicb_status scenes_create(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, aicb_scene **out) {
+    uint64_t volume;
+    TRY(check_scene_desc(d, &volume));
+    const SpaceHost empty;
+    FlatBlocks f;
+    TRY(flatten_blocks(empty, d->blocks, d->n_blocks, nullptr, &f));
+
+    // ---- cells: block id with its kind in the top bits --------------------------------------------------------------
+    const bool wide = d->n_blocks > 16384;
+    std::vector<uint16_t> cells16(wide ? 0 : volume);
+    std::vector<uint32_t> cells32(wide ? volume : 0);
+    for (size_t i = 0; i < volume; i++) {
+        const uint16_t id = d->block_ids[i];
+        if (id >= d->n_blocks) return fail(AICB_ERR_INVALID, "block id out of range");
+        if (wide) cells32[i] = cell_word(id, f.kinds[id], true);
+        else cells16[i] = (uint16_t)cell_word(id, f.kinds[id], false);
+    }
+    return create_scenes(ctx, n, d, volume, f, wide ? (const void *)cells32.data() : cells16.data(), nullptr, out);
 }
 
 // flatten_blocks against the scene's table, for an update (`indices`) or an append (nullptr) of the scene's replicas,
@@ -1721,12 +1772,9 @@ aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_
 // becomes [block] in exact-size buffers, as a new scene's, and every cell id 0 with its kind, written on the device
 // (u32 cells go back to u16: a one-block table fits them).  Light is not touched.  Each replica's context is waited for
 // first, since the table and the cells are replaced, and the call returns once its writes are done.  Every replica's
-// new arrays are allocated before any replica changes, so a failure leaves the scene as it was.
-aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block) {
-    if (!block) return fail(AICB_ERR_INVALID, "NULL argument");
-    const SpaceHost empty;   // an empty table's bookkeeping, which the new tables are placed against
-    FlatBlocks f;
-    TRY(flatten_blocks(empty, block, 1, nullptr, &f));
+// new arrays are allocated before any replica changes, so a failure leaves the scene as it was.  `f` is the block
+// flattened against `empty`, an empty table's bookkeeping; with `dev` its voxels are in device memory (copy_device).
+static aicb_status fill_uniform(Replicas r, const SpaceHost &empty, const FlatBlocks &f, const DeviceDefs *dev) {
     const uint32_t word = cell_word(0, f.kinds[0], false);
     SpaceHost &h = *r.scene[0]->host;
     struct Fresh {
@@ -1754,7 +1802,8 @@ aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block) {
             if (*b) retired.bufs.push_back(std::move(*b));
         sc->blocks = std::move(fresh[i].table);
         sc->blocks.bind(sc->ds);
-        TRY(copy(sc->blocks, empty, f, nullptr, stream));
+        if (dev) TRY(copy_device(ctx, sc->blocks, f, *dev));
+        else TRY(copy(sc->blocks, empty, f, nullptr, stream));
         if (fresh[i].narrow) {
             retired.bufs.push_back(std::move(sc->d_cells));
             sc->d_cells = std::move(fresh[i].narrow);
@@ -1778,6 +1827,14 @@ aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block) {
     h.h_ids.assign(h.volume, 0);
     h.ids_stale = false;
     return AICB_OK;
+}
+
+aicb_status scenes_fill_uniform(Replicas r, const aicb_block_desc *block) {
+    if (!block) return fail(AICB_ERR_INVALID, "NULL argument");
+    const SpaceHost empty;
+    FlatBlocks f;
+    TRY(flatten_blocks(empty, block, 1, nullptr, &f));
+    return fill_uniform(r, empty, f, nullptr);
 }
 
 // Space::set_physics (space.rs:609-630) on a scene's replicas: the sky tables once (Sky::for_blocks, Sky::mean), then, if
@@ -2162,34 +2219,35 @@ static HostVerdict host_checks(const SpaceHost &h, const uint16_t *indices, cons
     return v;
 }
 
-// aicb_scene_update_blocks_device / append_blocks_device over the replicas.  The host
-// checks what the scalars decide; one kernel scans the voxel indices of the definitions before the first host-side
-// failure and reads the kind of each single voxel, and those bytes are all that comes back before the call decides.
-// With AICB_BLOCKS_DERIVE_LIGHT, derive's kernels then run on device 0 on the caller's voxels and their error words
-// come back too.  Then the call is the host twin's body (update_blocks, append_blocks) with the voxel data placed by
-// blocks.cu's kernels on every replica, which read device 0's buffers (as a peer on other devices).
-aicb_status scenes_blocks_device(Replicas r, bool append, const uint16_t *indices, const aicb_block_desc *descs, size_t n,
-                                 uint32_t flags, cudaStream_t caller) {
-    if (n && (!descs || (!append && !indices))) return fail(AICB_ERR_INVALID, "NULL argument");
-    aicb_ctx *c0 = r.ctx[0];
-    CU(cudaSetDevice(c0->device));
-    if (n == 0) return AICB_OK;
-    if (append) indices = nullptr;
-    if (flags & ~AICB_BLOCKS_DERIVE_LIGHT) return fail(AICB_ERR_INVALID, "unknown flags");
+// Each definition's voxel pointers: device memory of device 0, aligned to their elements.
+static aicb_status check_def_pointers(const aicb_ctx *c0, const aicb_block_desc *descs, size_t n) {
     for (size_t i = 0; i < n; i++) {
         const aicb_block_desc &b = descs[i];
         const std::string name = "block " + std::to_string(i) + "'s ";
         if (b.indices && b.n_indices) TRY(check_device_pointer(b.indices, c0->device, false, 2, (name + "indices").c_str()));
         if (b.palette && b.n_palette) TRY(check_device_pointer(b.palette, c0->device, false, 4, (name + "palette").c_str()));
     }
-    const SpaceHost &h = *r.scene[0]->host;
+    return AICB_OK;
+}
+
+// n definitions whose voxels are in device 0's memory, checked against `h` (for `indices`, or appended) once the first
+// n_ctx contexts' streams wait for the caller's.  The host checks what the scalars decide; one pass on device 0 scans
+// the voxel indices of the definitions before the first host-side failure and reads the kind of each single voxel,
+// and with `ids` checks those `volume` block ids against the n definitions (k_check_ids; the host twin checks them
+// after every definition, scene creation's "block id out of range").  Those bytes are all that comes back before the
+// call decides, and the status and message are the host twin's first failure.  With AICB_BLOCKS_DERIVE_LIGHT,
+// derive's kernels then run on device 0 on the caller's voxels and their error words come back too.
+static aicb_status check_device_defs(aicb_ctx *const *ctx, size_t n_ctx, const SpaceHost &h, const uint16_t *indices,
+                                     const aicb_block_desc *descs, size_t n, uint32_t flags, cudaStream_t caller,
+                                     const uint16_t *ids, size_t volume, DeviceDefs *dev) {
+    aicb_ctx *c0 = ctx[0];
     const HostVerdict hv = host_checks(h, indices, descs, n);
     const size_t n_scan = std::min(n, hv.at == SIZE_MAX ? n : hv.at + (hv.after_scan ? 1 : 0));
-    TRY(join_caller(r.ctx, r.n, caller));
-    DeviceDefs dev;
-    dev.kinds.assign(n, KIND_INVISIBLE);
+    TRY(join_caller(ctx, n_ctx, caller));
+    dev->kinds.assign(n, KIND_INVISIBLE);
     unsigned long long bad = ~0ull;
-    if (n_scan) {   // verdict (16 bytes) and the kinds, read back together; then the jobs
+    bool bad_id = false;
+    if (n_scan) {   // the verdicts (16 bytes each: the definitions', the ids') and the kinds, read back together
         std::vector<DeviceBlockJob> jobs(n_scan, DeviceBlockJob{});
         uint64_t most = 0;
         for (size_t i = 0; i < n_scan; i++) {
@@ -2200,7 +2258,8 @@ aicb_status scenes_blocks_device(Replicas r, bool append, const uint16_t *indice
             jobs[i].single = single_source(descs[i]);
             most = std::max(most, jobs[i].n_indices);
         }
-        const size_t head = align256(sizeof(InputVerdict) + n_scan), job_bytes = n_scan * sizeof(DeviceBlockJob);
+        const size_t verdicts = 2 * sizeof(InputVerdict);
+        const size_t head = align256(verdicts + n_scan), job_bytes = n_scan * sizeof(DeviceBlockJob);
         cudaStream_t stream = c0->stream.get();
         TRY(inputs_room(c0, head + job_bytes));
         char *p = c0->d_inputs.get<char>();
@@ -2208,22 +2267,95 @@ aicb_status scenes_blocks_device(Replicas r, bool append, const uint16_t *indice
         DeviceBlockJob *d_jobs = (DeviceBlockJob *)(p + head);
         CU(cudaMemcpyAsync(d_jobs, jobs.data(), job_bytes, cudaMemcpyHostToDevice, stream));
         TRY(reset_verdict(v, stream));
-        TRY(issue_block_verdict(stream, d_jobs, (uint32_t)n_scan, most, v, (uint8_t *)(v + 1)));
-        std::vector<char> back(sizeof(InputVerdict) + n_scan);
+        TRY(reset_verdict(v + 1, stream));
+        TRY(issue_block_verdict(stream, d_jobs, (uint32_t)n_scan, most, v, (uint8_t *)p + verdicts));
+        if (ids && volume) {
+            k_check_ids<<<stride_grid(c0, volume), 256, 0, stream>>>(ids, volume, (uint32_t)n, v + 1);
+            CU(cudaGetLastError());
+        }
+        std::vector<char> back(verdicts + n_scan);
         CU(cudaMemcpyAsync(back.data(), p, back.size(), cudaMemcpyDeviceToHost, stream));
         CU(cudaStreamSynchronize(stream));
-        bad = ((const InputVerdict *)back.data())->first_bad;
-        std::memcpy(dev.kinds.data(), back.data() + sizeof(InputVerdict), n_scan);
+        bad = ((const InputVerdict *)back.data())[0].first_bad;
+        bad_id = ((const InputVerdict *)back.data())[1].first_bad != ~0ull;
+        std::memcpy(dev->kinds.data(), back.data() + verdicts, n_scan);
     }
-    // the host twin's first failure: block order, and within a block the scalars, the scan, the palette's size
+    // the host twin's first failure: block order, and within a block the scalars, the scan, the palette's size; then
+    // the ids
     if (bad != ~0ull && (bad < hv.at || (bad == hv.at && hv.after_scan))) return fail(AICB_ERR_INVALID, BAD_VOXEL_INDEX);
     if (hv.at != SIZE_MAX) return fail(hv.st, hv.msg);
+    if (bad_id) return fail(AICB_ERR_INVALID, "block id out of range");
     if (flags & AICB_BLOCKS_DERIVE_LIGHT) {
-        dev.derive = true;
-        TRY(derive_on_device(c0, descs, n, &dev.derived, &dev.d_derived));
+        dev->derive = true;
+        TRY(derive_on_device(c0, descs, n, &dev->derived, &dev->d_derived));
     }
+    return AICB_OK;
+}
+
+// aicb_scene_update_blocks_device / append_blocks_device over the replicas: the definitions checked on device 0
+// (check_device_defs), then the host twin's body (update_blocks, append_blocks) with the voxel data placed by
+// blocks.cu's kernels on every replica, which read device 0's buffers (as a peer on other devices).
+aicb_status scenes_blocks_device(Replicas r, bool append, const uint16_t *indices, const aicb_block_desc *descs, size_t n,
+                                 uint32_t flags, cudaStream_t caller) {
+    if (n && (!descs || (!append && !indices))) return fail(AICB_ERR_INVALID, "NULL argument");
+    aicb_ctx *c0 = r.ctx[0];
+    CU(cudaSetDevice(c0->device));
+    if (n == 0) return AICB_OK;
+    if (append) indices = nullptr;
+    if (flags & ~AICB_BLOCKS_DERIVE_LIGHT) return fail(AICB_ERR_INVALID, "unknown flags");
+    TRY(check_def_pointers(c0, descs, n));
+    DeviceDefs dev;
+    TRY(check_device_defs(r.ctx, r.n, *r.scene[0]->host, indices, descs, n, flags, caller, nullptr, 0, &dev));
     TRY(indices ? update_blocks(r, indices, descs, n, &dev) : append_blocks(r, descs, n, &dev));
     TRY(settle_replicas(r));
+    return release_caller(c0, caller);
+}
+
+// The jobs of n checked definitions whose voxels are in device memory, flattened against `empty` (a new table).
+static void flatten_new_table(const SpaceHost &empty, const aicb_block_desc *descs, size_t n, DeviceDefs &dev,
+                              FlatBlocks *f) {
+    flatten_device(empty, descs, n, dev.kinds, dev.derive, f);
+    device_jobs(empty, descs, *f, nullptr, dev);
+}
+
+// aicb_scene_create_device over n contexts: the pointers, then scene creation's checks in the host form's order, the
+// definitions' and the ids' verdicts read back once (check_device_defs), and the body both forms share.  The light is
+// a device-to-device copy per replica.
+aicb_status scenes_create_device(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, uint32_t flags,
+                                 cudaStream_t caller, aicb_scene **out) {
+    aicb_ctx *c0 = ctx[0];
+    CU(cudaSetDevice(c0->device));
+    if (flags & ~AICB_BLOCKS_DERIVE_LIGHT) return fail(AICB_ERR_INVALID, "unknown flags");
+    const bool cubes = d->bounds.size[0] && d->bounds.size[1] && d->bounds.size[2];
+    if (cubes && d->block_ids) TRY(check_device_pointer(d->block_ids, c0->device, false, 2, "block_ids"));
+    if (cubes && d->light) TRY(check_device_pointer(d->light, c0->device, false, 4, "light"));
+    if (d->blocks) TRY(check_def_pointers(c0, d->blocks, d->n_blocks));
+    uint64_t volume;
+    TRY(check_scene_desc(d, &volume));
+    const SpaceHost empty;
+    DeviceDefs dev;
+    TRY(check_device_defs(ctx, n, empty, nullptr, d->blocks, d->n_blocks, flags, caller, d->block_ids, volume, &dev));
+    FlatBlocks f;
+    flatten_new_table(empty, d->blocks, d->n_blocks, dev, &f);
+    TRY(create_scenes(ctx, n, d, volume, f, nullptr, &dev, out));
+    return release_caller(c0, caller);
+}
+
+// aicb_scene_fill_uniform_device over the replicas: the block checked on device 0 (check_device_defs), then
+// fill_uniform with its voxel data placed by blocks.cu's kernels.
+aicb_status scenes_fill_uniform_device(Replicas r, const aicb_block_desc *block, uint32_t flags, cudaStream_t caller) {
+    if (!block) return fail(AICB_ERR_INVALID, "NULL argument");
+    aicb_ctx *c0 = r.ctx[0];
+    CU(cudaSetDevice(c0->device));
+    if (flags & ~AICB_BLOCKS_DERIVE_LIGHT) return fail(AICB_ERR_INVALID, "unknown flags");
+    TRY(check_def_pointers(c0, block, 1));
+    const SpaceHost empty;
+    DeviceDefs dev;
+    TRY(check_device_defs(r.ctx, r.n, empty, nullptr, block, 1, flags, caller, nullptr, 0, &dev));
+    FlatBlocks f;
+    flatten_new_table(empty, block, 1, dev, &f);
+    TRY(fill_uniform(r, empty, f, &dev));   // (which returns once every replica's writes are done)
+    cudaSetDevice(c0->device);
     return release_caller(c0, caller);
 }
 
@@ -2313,6 +2445,14 @@ aicb_status aicb_scene_create(aicb_ctx *ctx, const aicb_scene_desc *d, aicb_scen
     return scenes_create(&ctx, 1, d, out);
 }
 
+aicb_status aicb_scene_create_device(aicb_ctx *ctx, const aicb_scene_desc *d, uint32_t flags, void *stream,
+                                     aicb_scene **out) {
+    if (!ctx || !d || !out) return fail(AICB_ERR_INVALID, "NULL argument");
+    *out = nullptr;
+    std::lock_guard<std::mutex> lock(ctx->mu);
+    return scenes_create_device(&ctx, 1, d, flags, (cudaStream_t)stream, out);
+}
+
 void aicb_scene_destroy(aicb_scene *s) {
     if (!s) return;
     cudaSetDevice(s->ctx->device);
@@ -2368,6 +2508,10 @@ aicb_status aicb_scene_append_blocks_device(aicb_scene *s, const aicb_block_desc
 // == SpaceChange::EveryBlock (Mutation::fill_uniform over the whole bounds, space.rs:1461-1474).
 aicb_status aicb_scene_fill_uniform(aicb_scene *s, const aicb_block_desc *block) {
     return on_scene(s, [&](Replicas r) { return scenes_fill_uniform(r, block); });
+}
+
+aicb_status aicb_scene_fill_uniform_device(aicb_scene *s, const aicb_block_desc *block, uint32_t flags, void *stream) {
+    return on_scene(s, [&](Replicas r) { return scenes_fill_uniform_device(r, block, flags, (cudaStream_t)stream); });
 }
 
 aicb_status aicb_scene_upload_light(aicb_scene *s, const uint8_t (*light)[4], size_t n_texels) {

@@ -486,6 +486,17 @@ aicb_status aicb_group_scene_create(aicb_group *g, const aicb_scene_desc *d, aic
     return AICB_OK;
 }
 
+aicb_status aicb_group_scene_create_device(aicb_group *g, const aicb_scene_desc *d, uint32_t flags, void *stream,
+                                           aicb_group_scene **out) {
+    if (!g || !d || !out) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    *out = nullptr;
+    std::vector<aicb_scene *> scene(g->ctx.size());
+    ContextLocks lock(g->ctx);
+    TRY(scenes_create_device(g->ctx.data(), scene.size(), d, flags, (cudaStream_t)stream, scene.data()));
+    *out = new aicb_group_scene{g, std::move(scene)};
+    return AICB_OK;
+}
+
 aicb_status aicb_group_scene_update_cubes(aicb_group_scene *gs, const int32_t (*cubes)[3], const uint16_t *ids,
                                           const uint8_t (*light)[4], size_t n) {
     return on_group(gs, false, [&](Replicas r) { return scenes_update_cubes(r, cubes, ids, light, n); });
@@ -584,6 +595,13 @@ aicb_status aicb_group_scene_append_blocks_device(aicb_group_scene *gs, const ai
 
 aicb_status aicb_group_scene_fill_uniform(aicb_group_scene *gs, const aicb_block_desc *block) {
     return on_group(gs, false, [&](Replicas r) { return scenes_fill_uniform(r, block); });
+}
+
+aicb_status aicb_group_scene_fill_uniform_device(aicb_group_scene *gs, const aicb_block_desc *block, uint32_t flags,
+                                                 void *stream) {
+    return on_group(gs, false, [&](Replicas r) {
+        return scenes_fill_uniform_device(r, block, flags, (cudaStream_t)stream);
+    });
 }
 
 aicb_status aicb_group_scene_set_physics(aicb_group_scene *gs, const aicb_sky *sky, uint8_t light_max_distance) {

@@ -524,6 +524,11 @@ aicb_status scenes_append_blocks(Replicas r, const aicb_block_desc *descs, size_
 // aicb_scene_append_blocks_device).  `flags`: AICB_BLOCKS_*.
 aicb_status scenes_blocks_device(Replicas r, bool append, const uint16_t *indices, const aicb_block_desc *descs, size_t n_blocks,
                                  uint32_t flags, cudaStream_t caller);
+// scenes_create and scenes_fill_uniform with the block ids, the light and each definition's voxels in device 0's
+// memory (aicb_scene_create_device, aicb_scene_fill_uniform_device).  Both return once every replica is complete.
+aicb_status scenes_create_device(aicb_ctx *const *ctx, size_t n, const aicb_scene_desc *d, uint32_t flags,
+                                 cudaStream_t caller, aicb_scene **out);
+aicb_status scenes_fill_uniform_device(Replicas r, const aicb_block_desc *block, uint32_t flags, cudaStream_t caller);
 
 // blocks.cu: one definition whose voxel data is in device memory, as its kernels read it.  aicb200.cu fills it from the
 // descriptor and the table's bookkeeping; the kernels take the caller's pointers as they are.

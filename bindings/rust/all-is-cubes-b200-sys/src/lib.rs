@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 22 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 23 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -310,6 +310,11 @@ unsafe extern "C" {
                                            n: usize, flags: u32, stream: *mut c_void) -> aicb_status;
     pub fn aicb_scene_append_blocks_device(s: *mut aicb_scene, descs: *const aicb_block_desc, n: usize, flags: u32,
                                            stream: *mut c_void) -> aicb_status;
+    // the Space in the context's device memory: desc.block_ids, desc.light and every descriptor's indices and palette
+    pub fn aicb_scene_create_device(ctx: *mut aicb_ctx, desc: *const aicb_scene_desc, flags: u32, stream: *mut c_void,
+                                    out: *mut *mut aicb_scene) -> aicb_status;
+    pub fn aicb_scene_fill_uniform_device(s: *mut aicb_scene, block: *const aicb_block_desc, flags: u32,
+                                          stream: *mut c_void) -> aicb_status;
 
     pub fn aicb_shard_pixel_count(cam: *const aicb_camera, shard: *const aicb_shard) -> usize;
     pub fn aicb_render_srgb8(s: *mut aicb_scene, cam: *const aicb_camera, opt: *const aicb_options, shard: *const aicb_shard,
@@ -409,6 +414,10 @@ unsafe extern "C" {
                                                  stream: *mut c_void) -> aicb_status;
     pub fn aicb_group_scene_append_blocks_device(gs: *mut aicb_group_scene, descs: *const aicb_block_desc, n: usize,
                                                  flags: u32, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_scene_create_device(g: *mut aicb_group, desc: *const aicb_scene_desc, flags: u32,
+                                          stream: *mut c_void, out: *mut *mut aicb_group_scene) -> aicb_status;
+    pub fn aicb_group_scene_fill_uniform_device(gs: *mut aicb_group_scene, block: *const aicb_block_desc, flags: u32,
+                                                stream: *mut c_void) -> aicb_status;
     // aicb_render_layers_* on a group: both layers must be scenes of the same group
     pub fn aicb_group_render_layers_srgb8(world: *const aicb_group_layer, ui: *const aicb_group_layer,
                                           backdrop_rgba: *const [f32; 4], no_world_rgba: *const [f32; 4],

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 22
+#define AICB_ABI_VERSION 23
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -363,6 +363,24 @@ aicb_status aicb_scene_update_blocks_device(aicb_scene *, const uint16_t *indice
                                             size_t n, uint32_t flags, void *stream);
 aicb_status aicb_scene_append_blocks_device(aicb_scene *, const aicb_block_desc *descs, size_t n, uint32_t flags,
                                             void *stream);
+/* aicb_scene_create with the Space in device memory of the context's device: block_ids (u16, Z-major, 2-byte aligned),
+ * light (4-byte aligned, or NULL) and each descriptor's indices and palette, as for aicb_scene_append_blocks_device.
+ * The aicb_scene_desc itself, the blocks array, its scalar fields, sky and light_max_distance stay on the host.  The
+ * new scene is byte for byte the one aicb_scene_create builds from the same data (cells, block table, light,
+ * aicb_scene_device_bytes), and a rejected call fails with aicb_scene_create's status and message, leaves *out NULL
+ * and frees what it allocated.  Pointers are checked first; then the bounds, the NULLs and the definitions in
+ * aicb_scene_create's order, and "block id out of range" last.  One readback decides: a kernel checks every voxel
+ * index and every block id and reads each single voxel's kind.  The cells are encoded on the device from the table's
+ * records, and the light is a device-to-device copy.  The scene's host mirror of the block ids starts stale, as
+ * after a device update.  flags: AICB_BLOCKS_DERIVE_LIGHT, as for the block calls.  Ordering is the device calls';
+ * the call returns once the scene is complete, so the caller may then reuse its buffers.
+ * GPU test: tests/test_gpu_device_create.py. */
+aicb_status aicb_scene_create_device(aicb_ctx *, const aicb_scene_desc *, uint32_t flags, void *stream,
+                                     aicb_scene **out);
+/* aicb_scene_fill_uniform with the block's indices and palette in the scene's device memory, checked and placed as
+ * aicb_scene_append_blocks_device checks and places them; flags as there.  The scene ends as the host twin leaves it,
+ * its host mirror of the block ids reset; a rejected call changes nothing.  Returns once its writes are done. */
+aicb_status aicb_scene_fill_uniform_device(aicb_scene *, const aicb_block_desc *block, uint32_t flags, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * draw(): replaces RtRenderer::draw_rgba / RtRenderer::draw::<ColorBuf> and the Rayon pixel
@@ -638,6 +656,14 @@ aicb_status aicb_group_scene_update_blocks_device(aicb_group_scene *, const uint
                                                   const aicb_block_desc *descs, size_t n, uint32_t flags, void *stream);
 aicb_status aicb_group_scene_append_blocks_device(aicb_group_scene *, const aicb_block_desc *descs, size_t n,
                                                   uint32_t flags, void *stream);
+/* aicb_scene_create_device and aicb_scene_fill_uniform_device on the group: the inputs are device 0's memory, checked
+ * once there.  Every replica's table is written by its own kernels, and every replica encodes its own cells from
+ * device 0's ids, read over peer access; the light is a peer copy per replica.  Each returns once every replica is
+ * complete. */
+aicb_status aicb_group_scene_create_device(aicb_group *, const aicb_scene_desc *, uint32_t flags, void *stream,
+                                           aicb_group_scene **out);
+aicb_status aicb_group_scene_fill_uniform_device(aicb_group_scene *, const aicb_block_desc *block, uint32_t flags,
+                                                 void *stream);
 
 /* == RtScene::trace_ray_through_layers + draw_rgba (renderer.rs:454-478, 282-308) and RaytraceToTexture::do_some_tracing's
  * trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs:591-683) on the whole group: the arguments, the validation and
