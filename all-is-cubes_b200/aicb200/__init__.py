@@ -143,6 +143,14 @@ def load_library() -> C.CDLL:
                                                     C.POINTER(abi.RenderInfo)]
     lib.aicb_group_light_download.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t]
     lib.aicb_derive_block_light.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    for prefix in ("aicb_", "aicb_group_"):
+        getattr(lib, prefix + "cursor_raycast").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+        getattr(lib, prefix + "cursor_raycast_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                                  C.c_void_p, C.c_void_p]
+    lib.aicb_project_cursor.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_size_t,
+                                        C.c_double, C.c_void_p]
+    lib.aicb_group_project_cursor.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
+                                              C.c_size_t, C.c_double, C.c_void_p]
     # the calls of _Scene: a group scene's form of aicb_<name> is aicb_group_<name>, with the same arguments
     u64, u8, size = C.POINTER(C.c_uint64), C.POINTER(C.c_uint8), C.POINTER(C.c_size_t)
     info = C.POINTER(abi.RenderInfo)
@@ -413,8 +421,13 @@ class Block:
     """One Space palette entry as the raytracer sees it (TracingBlock, sr.rs:569-587)."""
 
     def __init__(self, *, color=None, emission=(0.0, 0.0, 0.0), is_air=False, resolution=1, voxel_lower=None,
-                 indices: Optional[np.ndarray] = None, palette: Optional[np.ndarray] = None):
+                 indices: Optional[np.ndarray] = None, palette: Optional[np.ndarray] = None, selectable=True,
+                 voxel_selectable=None):
+        """selectable: BlockAttributes::selectable (AICB_BLOCK_NOT_SELECTABLE when false; an air block is never
+        selectable).  voxel_selectable: each palette entry's Evoxel::selectable (a bool or a bool per entry), written
+        into the palette's column 7 as AICB_VOXEL_NOT_SELECTABLE; None keeps the column as given (zero: selectable)."""
         self.is_air = bool(is_air)
+        self.selectable = bool(selectable) and not self.is_air
         self.resolution = int(resolution)
         if indices is None:
             c = (0.0, 0.0, 0.0, 0.0) if color is None else tuple(color)
@@ -432,6 +445,11 @@ class Block:
             assert self.palette.ndim == 2 and self.palette.shape[1] == 8
             self.voxel_lower = tuple(int(v) for v in (voxel_lower or (0, 0, 0)))
             self.voxel_size = tuple(int(v) for v in indices.shape)
+        if voxel_selectable is not None:
+            if self.indices is not None and palette is not None and np.shares_memory(self.palette, palette):
+                self.palette = self.palette.copy()
+            sel = np.broadcast_to(np.asarray(voxel_selectable, dtype=bool), (self.palette.shape[0],))
+            self.palette.view(np.uint32)[:, 7] = np.where(sel, 0, abi.VOXEL_NOT_SELECTABLE).astype(np.uint32)
         self._derive_for_light()
 
     def _derive_for_light(self):
@@ -564,10 +582,12 @@ class DeviceBlock:
     update_blocks / append_blocks (aicb_scene_*_blocks_device): `indices` a uint16 tensor of the data bounds' shape
     (Z-major), or None for a single voxel, palette[0]; `palette` a float32 [n, 8] tensor (rgba, emission, pad).
     `light` is the block's BlockLight, or None to derive it on the device (AICB_BLOCKS_DERIVE_LIGHT); `visible`
-    ORs an animation hint into a derived Derived::visible."""
+    ORs an animation hint into a derived Derived::visible.  Column 7 of the palette holds each voxel's flags as the
+    bits of the float32 (AICB_VOXEL_NOT_SELECTABLE); `selectable` is BlockAttributes::selectable."""
 
     def __init__(self, resolution, voxel_lower, indices, palette, is_air=False, light: Optional["BlockLight"] = None,
-                 visible: bool = False):
+                 visible: bool = False, selectable: bool = True):
+        self.selectable = bool(selectable)
         self.resolution = int(resolution)
         self.voxel_lower = tuple(int(v) for v in (voxel_lower or (0, 0, 0)))
         self.indices = indices
@@ -598,6 +618,7 @@ class DeviceBlock:
         bd.n_indices = 0 if self.indices is None else self.indices.numel()
         bd.palette = self.palette.data_ptr() if self.palette.shape[0] else None
         bd.n_palette = self.palette.shape[0]
+        bd.flags = 0 if self.selectable else abi.BLOCK_NOT_SELECTABLE
         bl = self.light
         if bl is None:
             bd.light_visible = 1 if self.visible else 0
@@ -758,6 +779,7 @@ def fill_block_desc(bd, b):
         bd.light_face_colors[f][:] = b.light_face_colors[f]
     bd.light_color[:] = b.light_color
     bd.light_emission[:] = b.light_emission
+    bd.flags = 0 if getattr(b, "selectable", True) else abi.BLOCK_NOT_SELECTABLE
 
 
 def _block_descs(blocks):
@@ -1036,6 +1058,36 @@ class _Scene:
         out = torch.empty(self.space.size, dtype=torch.uint16 if device else torch.int16, device=dev)
         _check(self._fn("scene_download_ids_device")(self.handle, out.data_ptr(), out.numel(), _stream(dev)))
         return out if device else out.cpu().numpy().view(np.uint16)
+
+    def cursor_raycast(self, origin_dir, max_distance=None, device: bool = False):
+        """cursor_raycast (cursor.rs:26-107) for a batch of rays [n, 6] (origin, direction): a numpy array of
+        abi.CURSOR_DTYPE, block_id abi.CURSOR_NONE where nothing was selected.  max_distance: None (f64::INFINITY), a
+        number or one per ray.  device=True: origin_dir (and max_distance, if an array) are float64 tensors on the
+        scene's device (device 0 of a group), the call is issued on its current torch stream, and the result is a
+        uint8 tensor [n, 80] (view it with .cpu().numpy().view(abi.CURSOR_DTYPE))."""
+        if device:
+            torch = _torch()
+            dev = self._device()
+            od = origin_dir.reshape(-1, 6)
+            n = od.shape[0]
+            od = self._tensor(od, torch.float64, (n, 6), "origin_dir")
+            md = None
+            if max_distance is not None:
+                md = max_distance if _is_cuda_tensor(max_distance) else torch.full((n,), float(max_distance),
+                                                                                   dtype=torch.float64, device=dev)
+                md = self._tensor(md, torch.float64, (n,), "max_distance")
+            out = torch.empty((n, 80), dtype=torch.uint8, device=dev)
+            _check(self._fn("cursor_raycast_device")(self.handle, od.data_ptr(), None if md is None else md.data_ptr(),
+                                                      n, out.data_ptr(), _stream(dev)))
+            return out
+        od = np.ascontiguousarray(origin_dir, dtype=np.float64).reshape(-1, 6)
+        n = od.shape[0]
+        md = None if max_distance is None else np.ascontiguousarray(np.broadcast_to(
+            np.asarray(max_distance, dtype=np.float64), (n,)))
+        out = np.zeros(n, dtype=abi.CURSOR_DTYPE)
+        _check(self._fn("cursor_raycast")(self.handle, od.ctypes.data, None if md is None else md.ctypes.data, n,
+                                          out.ctypes.data))
+        return out
 
     def _light_download_device(self):
         torch = _torch()
@@ -1443,6 +1495,32 @@ def _layers_device(group, world, ui, backdrop, no_world, spec, out, n, build, de
     return build(t, RenderInfo.from_abi(info))
 
 
+def _project_cursor(fn, cls, world, ui, ndc, world_max_distance):
+    keep = []
+
+    def layer(l):
+        if not l:
+            return None
+        if hasattr(l[0], "ctx"):
+            l[0].ctx.settle()
+        s = cls(l[0].handle, C.pointer(l[1].data), None)
+        keep.append(s)
+        return C.byref(s)
+
+    p = np.ascontiguousarray(ndc, dtype=np.float64).reshape(-1, 2)
+    out = np.zeros(p.shape[0], dtype=abi.CURSOR_DTYPE)
+    _check(fn(layer(world), layer(ui), p.ctypes.data, p.shape[0], float(world_max_distance), out.ctypes.data))
+    return out
+
+
+def project_cursor(world=None, ui=None, ndc=None, world_max_distance: float = 6.0):
+    """StandardCameras::project_cursor (stdcam.rs:357-389) for a batch of NDC points [n, 2]: world / ui =
+    (SpaceRaytracer, Camera) or None.  Per point the UI layer with f64::INFINITY, then the world layer with
+    world_max_distance (the reference hard-codes 6.0); returns an abi.CURSOR_DTYPE array whose `layer` is 1 (UI),
+    2 (world) or 0 (nothing)."""
+    return _project_cursor(load_library().aicb_project_cursor, abi.Layer, world, ui, ndc, world_max_distance)
+
+
 NO_WORLD_TO_SHOW_SRGB8 = (0xBC, 0xBC, 0xBC, 0xFF)   # content/palette.rs:76
 
 
@@ -1817,6 +1895,11 @@ class DeviceGroup:
 
     def _device(self):
         return _torch().device("cuda", self.device_ids[0])
+
+    def project_cursor(self, world=None, ui=None, ndc=None, world_max_distance: float = 6.0):
+        """project_cursor with GroupScenes of this group: world / ui = (GroupScene, Camera) or None."""
+        return _project_cursor(load_library().aicb_group_project_cursor, abi.GroupLayer, world, ui, ndc,
+                               world_max_distance)
 
     def render_layers(self, world=None, ui=None, backdrop=None, no_world=None, device=False, out=None) -> "Rendering":
         """render_layers with GroupScenes of this group: world / ui = (GroupScene, Camera, GraphicsOptions) or None.

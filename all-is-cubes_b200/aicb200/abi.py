@@ -1,7 +1,9 @@
 """ctypes mirror of include/aicb200.h (plain data only; no compute)."""
 import ctypes as C
 
-ABI_VERSION = 23
+import numpy as np
+
+ABI_VERSION = 24
 
 BLOCKS_DERIVE_LIGHT = 1
 
@@ -20,7 +22,7 @@ class Aab(C.Structure):
 
 
 class Voxel(C.Structure):
-    _fields_ = [("rgba", C.c_float * 4), ("emission", C.c_float * 3), ("_pad", C.c_float)]
+    _fields_ = [("rgba", C.c_float * 4), ("emission", C.c_float * 3), ("flags", C.c_uint32)]
 
 
 class BlockDesc(C.Structure):
@@ -37,7 +39,7 @@ class BlockDesc(C.Structure):
         ("light_face_colors", (C.c_float * 4) * 6),
         ("light_color", C.c_float * 4),
         ("light_emission", C.c_float * 3),
-        ("_pad", C.c_float),
+        ("flags", C.c_uint32),
     ]
 
 
@@ -162,6 +164,28 @@ class TextureTargetInfo(C.Structure):
                 ("dirty_pixels", C.c_uint64), ("next_pick", C.c_uint64), ("cycle_length", C.c_uint64)]
 
 
+VOXEL_NOT_SELECTABLE = 1   # aicb_voxel::flags
+BLOCK_NOT_SELECTABLE = 1   # aicb_block_desc::flags
+CURSOR_NONE = 0xFFFFFFFF
+CURSOR_OUTSIDE = 0xFFFFFFFE
+
+
+class Cursor(C.Structure):
+    """aicb_cursor: Cursor + its CubeSnapshots (cursor.rs:111-149), 80 bytes."""
+    _fields_ = [("point_entered", C.c_double * 3), ("distance", C.c_double), ("cube", C.c_int32 * 3),
+                ("preceding_cube", C.c_int32 * 3), ("block_id", C.c_uint32), ("preceding_block_id", C.c_uint32),
+                ("light", C.c_uint8 * 4), ("preceding_light", C.c_uint8 * 4), ("face_entered", C.c_uint8),
+                ("face_selected", C.c_uint8), ("layer", C.c_uint8), ("_pad", C.c_uint8 * 5)]
+
+
+# aicb_cursor as a numpy structured dtype (the arrays the cursor calls return)
+CURSOR_DTYPE = np.dtype([("point_entered", "<f8", (3,)), ("distance", "<f8"), ("cube", "<i4", (3,)),
+                         ("preceding_cube", "<i4", (3,)), ("block_id", "<u4"), ("preceding_block_id", "<u4"),
+                         ("light", "u1", (4,)), ("preceding_light", "u1", (4,)), ("face_entered", "u1"),
+                         ("face_selected", "u1"), ("layer", "u1"), ("_pad", "u1", (5,))])
+assert CURSOR_DTYPE.itemsize == 80
+
+
 EXPORTED_SYMBOLS = [
     "aicb_abi_version",
     "aicb_ctx_create",
@@ -221,6 +245,12 @@ EXPORTED_SYMBOLS = [
     "aicb_camera_from_view",
     "aicb_eye_for_look_at",
     "aicb_camera_project_ndc",
+    "aicb_cursor_raycast",
+    "aicb_cursor_raycast_device",
+    "aicb_project_cursor",
+    "aicb_group_cursor_raycast",
+    "aicb_group_cursor_raycast_device",
+    "aicb_group_project_cursor",
     "aicb_light_chart",
     "aicb_light_chart_chains",
     "aicb_light_fast_evaluate",

@@ -11,7 +11,10 @@ What is read:
     resolution}` (schema.rs:84-98) whose voxel Space consists of `AirV1` / `AtomV1` blocks — the cases whose evaluation
     is a table lookup (block/eval: an atom's Evoxel is its colour and emission; a Recur block's Evoxels are its
     Space's blocks over `offset .. offset + resolution`, clipped to the Space's bounds).
-  * modifiers that do not change what is drawn (`DisplayNameV1`, `TagV1`, `QuoteV1`, selectable / inventory / action
+  * `SelectableV1{selectable}` sets the block's BlockAttributes::selectable (attributes.rs:389), and through
+    Evoxel::from_block (voxel_storage.rs:76-100) the selectable of each voxel a `RecurV1` block takes from it; an
+    `AirV1` block, and so an `AirV1` voxel, is never selectable (AIR_ATTRIBUTES);
+  * modifiers that do not change what is drawn or picked (`DisplayNameV1`, `TagV1`, `QuoteV1`, inventory / action
     attributes) are ignored; `RotateV1`, `CompositeV1`, `ZoomV1`, `Move`, `IndirectV1` and `TextPrimitiveV1` need the
     reference's block evaluator (out of scope, SURVEY §2) and raise `UnsupportedBlock`.
   * universes: `UniverseV1{members: [{name, member_type, value}]}` (schema.rs:548-600).
@@ -32,7 +35,7 @@ from . import Block, Space
 # LightStatusSerV1 (schema.rs:491-498) -> the status byte of PackedLight::as_texel (light/data.rs:31-46, 162)
 _STATUS_TEXEL = {0: 0, 1: 1, 2: 128, 3: 255}
 _TEXEL_STATUS = {t: s for s, t in _STATUS_TEXEL.items()}
-_IGNORED_MODIFIERS = {"DisplayNameV1", "TagV1", "QuoteV1", "SelectableV1", "BlockInventoryV1", "InventoryConfigV1",
+_IGNORED_MODIFIERS = {"DisplayNameV1", "TagV1", "QuoteV1", "BlockInventoryV1", "InventoryConfigV1",
                       "RotationRuleV1", "PlacementActionV1", "TickActionV1", "ActivationActionV1", "AnimationHintV1"}
 
 
@@ -69,8 +72,11 @@ def _atom(prim):
 def _block_of(block_ser, resolve_space):
     if block_ser.get("type") != "BlockV1":
         raise UnsupportedBlock(f"block type {block_ser.get('type')}")
+    selectable = True
     for m in block_ser.get("modifiers", []):
-        if m.get("type") not in _IGNORED_MODIFIERS:
+        if m.get("type") == "SelectableV1":
+            selectable = bool(m["selectable"])
+        elif m.get("type") not in _IGNORED_MODIFIERS:
             raise UnsupportedBlock(f"modifier {m.get('type')} needs the reference's block evaluator")
     prim = block_ser["primitive"]
     kind = prim["type"]
@@ -78,7 +84,7 @@ def _block_of(block_ser, resolve_space):
         return Block.air()
     if kind == "AtomV1":
         c, e = _atom(prim)
-        return Block(color=tuple(c), emission=tuple(e))
+        return Block(color=tuple(c), emission=tuple(e), selectable=selectable)
     if kind == "RecurV1":
         if resolve_space is None:
             raise UnsupportedBlock("RecurV1 needs the universe the Space handle points into")
@@ -89,7 +95,7 @@ def _block_of(block_ser, resolve_space):
         lo = [max(off[a], vs.lower[a]) for a in range(3)]
         hi = [min(off[a] + res, vs.lower[a] + vs.size[a]) for a in range(3)]
         if any(hi[a] <= lo[a] for a in range(3)):
-            return Block(color=(0.0, 0.0, 0.0, 0.0))
+            return Block(color=(0.0, 0.0, 0.0, 0.0), selectable=selectable)
         sl = tuple(slice(lo[a] - vs.lower[a], hi[a] - vs.lower[a]) for a in range(3))
         ids = vs.block_ids[sl]
         pal = np.zeros((len(vs.blocks), 8), dtype=np.float32)
@@ -97,7 +103,8 @@ def _block_of(block_ser, resolve_space):
             if b.indices is not None:
                 raise UnsupportedBlock("a voxel Space made of recursive blocks needs the reference's block evaluator")
             pal[i] = b.palette[0]
-        return Block(resolution=res, voxel_lower=[lo[a] - off[a] for a in range(3)], indices=ids.astype(np.uint16), palette=pal)
+        return Block(resolution=res, voxel_lower=[lo[a] - off[a] for a in range(3)], indices=ids.astype(np.uint16),
+                     palette=pal, selectable=selectable, voxel_selectable=[b.selectable for b in vs.blocks])
     raise UnsupportedBlock(f"primitive {kind} needs the reference's block evaluator")
 
 

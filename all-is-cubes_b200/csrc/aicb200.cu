@@ -97,7 +97,7 @@ static void build_block_sky(const aicb_sky &sky, DeviceScene *ds) {
 // log2(1 - alpha)} per palette entry.
 // Called by flatten_blocks alone.
 static const char *const BRICKS_PAST_2_32 = "brick pool exceeds 2^32 voxels";
-static const aicb_voxel AIR_VOXEL = {{0, 0, 0, 0}, {0, 0, 0}, 0};
+static const aicb_voxel AIR_VOXEL = {{0, 0, 0, 0}, {0, 0, 0}, AICB_VOXEL_NOT_SELECTABLE};   // Evoxel::AIR
 
 // blk_tab entry of a block: what the marching kernel needs of a single-voxel surface on the Space level.
 // `pal_off` indexes `pal_tab`; `pal_base` is added to it for the device-wide palette index.
@@ -156,6 +156,7 @@ aicb_voxel single_voxel_of(const aicb_block_desc &b) {
 static BlockRec block_rec(const aicb_block_desc &b, uint8_t kind, uint32_t brick_off, uint32_t pal_off) {
     BlockRec r;
     std::memset(&r, 0, sizeof r);
+    r.flags = (b.is_air || (b.flags & AICB_BLOCK_NOT_SELECTABLE)) ? AICB_BLOCK_NOT_SELECTABLE : 0u;
     if (b.is_air) {
         r.kind_res = KIND_INVISIBLE | (1u << 8);
     } else if (kind != KIND_RECURSIVE) {
@@ -180,7 +181,7 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
     TRY(check_block_desc(b));
     auto push_voxel = [&](const aicb_voxel &v) {
         palette.push_back(make_float4(v.rgba[0], v.rgba[1], v.rgba[2], v.rgba[3]));
-        palette.push_back(make_float4(v.emission[0], v.emission[1], v.emission[2], 0.0f));
+        palette.push_back(make_float4(v.emission[0], v.emission[1], v.emission[2], voxel_flags(v)));
         pal_tab.push_back(surface_entry(v.rgba[3]));
     };
     const bool single = is_single_voxel(b);

@@ -6,6 +6,7 @@
 // bit pattern of alpha.
 #pragma once
 #include <cmath>
+#include <cstring>
 
 #include <cuda_runtime.h>
 
@@ -16,6 +17,15 @@ namespace aicb {
 // A voxel the marching kernel steps over (bit 15 of its brick word): fully transparent and not emissive.
 __host__ __device__ inline bool voxel_invisible(const aicb_voxel &v) {
     return v.rgba[3] == 0.0f && v.emission[0] == 0.0f && v.emission[1] == 0.0f && v.emission[2] == 0.0f;
+}
+
+// The .w lane of a palette entry's second float4 (its emission): the voxel's AICB_VOXEL_NOT_SELECTABLE bit, which only
+// the cursor reads.  The other bits of aicb_voxel::flags are not kept.
+__host__ __device__ inline float voxel_flags(const aicb_voxel &v) {
+    const uint32_t f = v.flags & AICB_VOXEL_NOT_SELECTABLE;
+    float w;
+    memcpy(&w, &f, 4);
+    return w;
 }
 
 // {alpha, l2a}: l2a >= log2(1 - alpha) (the f32 value apply_transmittance raises to a span's thickness), so the

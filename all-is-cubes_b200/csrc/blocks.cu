@@ -42,6 +42,7 @@ const unsigned THREADS = 256;
 __device__ aicb_voxel single_voxel(const DeviceBlockJob &J) {
     aicb_voxel v;
     memset(&v, 0, sizeof v);
+    v.flags = AICB_VOXEL_NOT_SELECTABLE;   // Evoxel::AIR
     if (J.single == SINGLE_FIRST) v = J.palette[0];
     else if (J.single == SINGLE_INDEXED) {
         const uint32_t k = J.indices[0];
@@ -104,7 +105,7 @@ __global__ void __launch_bounds__(THREADS) k_block_palette(const DeviceBlockJob 
         const aicb_voxel v = J.kind == KIND_RECURSIVE ? J.palette[e] : single_voxel(J);
         const size_t at = (size_t)J.pal_off + e;
         palette[2 * at] = make_float4(v.rgba[0], v.rgba[1], v.rgba[2], v.rgba[3]);
-        palette[2 * at + 1] = make_float4(v.emission[0], v.emission[1], v.emission[2], 0.0f);
+        palette[2 * at + 1] = make_float4(v.emission[0], v.emission[1], v.emission[2], voxel_flags(v));
         pal_tab[at] = surface_entry(v.rgba[3]);
     }
 }

@@ -216,6 +216,7 @@ struct aicb_ctx {
     LightChart light_chart;
     DeviceBuffer d_derive;       // aicb_derive_block_light's per-palette-entry and per-ray terms and its results
     DeviceBuffer d_inputs;       // the device-input calls' scratch: verdict, sorted cube lists, staged entries
+    DeviceBuffer d_cursor;       // the host cursor calls' queries and results (cursor.cu), apart from a frame's buffers
     std::mutex mu;
 };
 

@@ -72,7 +72,8 @@ struct BlockRec {
     uint16_t vsize[3];     // voxel_bounds size
     uint32_t brick_off;    // first u16 of this block's brick in the pool
     uint32_t pal_off;      // first palette entry (single: the voxel)
-    uint32_t _pad[2];
+    uint32_t flags;        // AICB_BLOCK_NOT_SELECTABLE (set for an is_air block); read by the cursor alone
+    uint32_t _pad;
 };
 static_assert(sizeof(BlockRec) == 32, "BlockRec must be 32 bytes");
 

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 23 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 24 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -34,13 +34,40 @@ pub struct aicb_aab {
     pub size: [u32; 3],
 }
 
-/// colour part of `Evoxel` (block/eval/voxel_storage.rs:41-53)
+/// `Evoxel` without its collision (block/eval/voxel_storage.rs:41-60); `flags`: `AICB_VOXEL_*`
 #[repr(C)]
 #[derive(Clone, Copy, Debug, Default)]
 pub struct aicb_voxel {
     pub rgba: [f32; 4],
     pub emission: [f32; 3],
-    pub _pad: f32,
+    pub flags: u32,
+}
+
+/// `Evoxel::selectable == false`
+pub const AICB_VOXEL_NOT_SELECTABLE: u32 = 1;
+/// `BlockAttributes::selectable == false` (an `is_air` block is never selectable)
+pub const AICB_BLOCK_NOT_SELECTABLE: u32 = 1;
+/// `aicb_cursor::block_id` of a query that selected nothing; `preceding_block_id` of a ray that started in the cube
+pub const AICB_CURSOR_NONE: u32 = 0xFFFF_FFFF;
+/// `aicb_cursor::preceding_block_id` of a preceding cube outside the bounds
+pub const AICB_CURSOR_OUTSIDE: u32 = 0xFFFF_FFFE;
+
+/// `Cursor` + its `CubeSnapshot`s (character/cursor.rs:111-149)
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_cursor {
+    pub point_entered: [f64; 3],
+    pub distance: f64,
+    pub cube: [i32; 3],
+    pub preceding_cube: [i32; 3],
+    pub block_id: u32,
+    pub preceding_block_id: u32,
+    pub light: [u8; 4],
+    pub preceding_light: [u8; 4],
+    pub face_entered: u8,
+    pub face_selected: u8,
+    pub layer: u8,
+    pub _pad: [u8; 5],
 }
 
 /// one entry of `Space::block_data()` as `TracingBlock::from_block` sees it (sr.rs:569-587) plus the
@@ -60,7 +87,7 @@ pub struct aicb_block_desc {
     pub light_face_colors: [[f32; 4]; 6],
     pub light_color: [f32; 4],
     pub light_emission: [f32; 3],
-    pub _pad: f32,
+    pub flags: u32,
 }
 
 /// `compute_derived`'s light fields of one block (block/eval/derived.rs:80-216), as `aicb_block_desc`'s `light_*`
@@ -506,6 +533,23 @@ unsafe extern "C" {
                                  fb_height: u32, exposure: f32, out: *mut aicb_camera) -> aicb_status;
     pub fn aicb_eye_for_look_at(bounds: *const aicb_aab, direction: *const [f64; 3], out_eye: *mut [f64; 3]);
     pub fn aicb_camera_project_ndc(cam: *const aicb_camera, ndc_x: f64, ndc_y: f64, out_origin_dir: *mut [f64; 6]);
+
+    pub fn aicb_cursor_raycast(s: *mut aicb_scene, origin_dir: *const [f64; 6], max_distance_or_null: *const f64,
+                               n: usize, out: *mut aicb_cursor) -> aicb_status;
+    pub fn aicb_cursor_raycast_device(s: *mut aicb_scene, d_origin_dir: *const [f64; 6],
+                                      d_max_distance_or_null: *const f64, n: usize, d_out: *mut aicb_cursor,
+                                      stream: *mut c_void) -> aicb_status;
+    pub fn aicb_project_cursor(world_or_null: *const aicb_layer, ui_or_null: *const aicb_layer, ndc: *const [f64; 2],
+                               n: usize, world_max_distance: f64, out: *mut aicb_cursor) -> aicb_status;
+    pub fn aicb_group_cursor_raycast(gs: *mut aicb_group_scene, origin_dir: *const [f64; 6],
+                                     max_distance_or_null: *const f64, n: usize, out: *mut aicb_cursor)
+                                     -> aicb_status;
+    pub fn aicb_group_cursor_raycast_device(gs: *mut aicb_group_scene, d_origin_dir: *const [f64; 6],
+                                            d_max_distance_or_null: *const f64, n: usize, d_out: *mut aicb_cursor,
+                                            stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_project_cursor(world_or_null: *const aicb_group_layer, ui_or_null: *const aicb_group_layer,
+                                     ndc: *const [f64; 2], n: usize, world_max_distance: f64, out: *mut aicb_cursor)
+                                     -> aicb_status;
 
     pub fn aicb_light_chart(weights: *mut f32, children: *mut u32) -> u32;
     pub fn aicb_light_chart_chains(preorder: *mut u32, chains: *mut [u32; 6], euler: *mut u16) -> u32;

@@ -57,7 +57,8 @@ pub fn block_desc_of(data: &space::SpaceBlockData) -> OwnedBlockDesc {
     let voxel = |v: &all_is_cubes::block::Evoxel| {
         let c: [f32; 4] = v.color.into();
         let e: [f32; 3] = v.emission.into();
-        sys::aicb_voxel { rgba: c, emission: e, _pad: 0.0 }
+        let flags = if v.selectable { 0 } else { sys::AICB_VOXEL_NOT_SELECTABLE };
+        sys::aicb_voxel { rgba: c, emission: e, flags }
     };
     let (indices, palette, bounds, resolution) = match ev.voxels() {
         // Evoxels::One: indices == NULL (include/aicb200.h, aicb_block_desc)
@@ -73,7 +74,7 @@ pub fn block_desc_of(data: &space::SpaceBlockData) -> OwnedBlockDesc {
                 .as_linear()
                 .iter()
                 .map(|v| {
-                    *lookup.entry((v.color.to_bits(), v.emission.to_bits())).or_insert_with(|| {
+                    *lookup.entry((v.color.to_bits(), v.emission.to_bits(), v.selectable)).or_insert_with(|| {
                         palette.push(voxel(v));
                         (palette.len() - 1) as u16
                     })
@@ -108,7 +109,7 @@ pub fn block_desc_of(data: &space::SpaceBlockData) -> OwnedBlockDesc {
             light_face_colors: face_colors,
             light_color: color.into(),
             light_emission: ev.light_emission().into(),
-            _pad: 0.0,
+            flags: if ev.attributes().selectable { 0 } else { sys::AICB_BLOCK_NOT_SELECTABLE },
         },
     }
 }

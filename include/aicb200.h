@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 23
+#define AICB_ABI_VERSION 24
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -46,13 +46,15 @@ typedef struct aicb_aab {
     uint32_t size[3];
 } aicb_aab;
 
-/* Colour part of Evoxel (all-is-cubes/src/block/eval/voxel_storage.rs:41-53):
- * non-premultiplied linear RGBA reflectance + RGB emission. 32 bytes. */
+/* Evoxel (all-is-cubes/src/block/eval/voxel_storage.rs:41-60) without its collision:
+ * non-premultiplied linear RGBA reflectance + RGB emission, and `flags`. 32 bytes. */
 typedef struct aicb_voxel {
     float rgba[4];
     float emission[3];
-    float _pad;
+    uint32_t flags;                /* AICB_VOXEL_*; other bits are ignored */
 } aicb_voxel;
+/* Evoxel::selectable == false (voxel_storage.rs:57).  Zero, the default, is selectable.  Only the cursor reads it. */
+#define AICB_VOXEL_NOT_SELECTABLE 1u
 
 /* Face7 (all-is-cubes-base/src/math/face.rs:105). */
 enum { AICB_FACE_WITHIN = 0, AICB_FACE_NX = 1, AICB_FACE_NY = 2, AICB_FACE_NZ = 3,
@@ -83,8 +85,11 @@ typedef struct aicb_block_desc {
     float light_face_colors[6][4]; /* EvaluatedBlock::face7_color(face), NX..PZ */
     float light_color[4];          /* EvaluatedBlock::color() */
     float light_emission[3];       /* EvaluatedBlock::light_emission() */
-    float _pad;
+    uint32_t flags;                /* AICB_BLOCK_*; other bits are ignored */
 } aicb_block_desc;
+/* BlockAttributes::selectable == false (attributes.rs:389).  Zero, the default, is selectable; an is_air block is never
+ * selectable, whatever its flags (AIR_ATTRIBUTES, block/eval/evaluated.rs:419-421).  Only the cursor reads it. */
+#define AICB_BLOCK_NOT_SELECTABLE 1u
 
 /* Sky (all-is-cubes/src/space/sky.rs:16-21). kind 0 = Uniform(colors[0]), 1 = Octants.
  * Octant index = (x>=0)<<2 | (y>=0)<<1 | (z>=0)  (sky.rs:36-39). */
@@ -844,6 +849,66 @@ aicb_status aicb_camera_from_view(const double rotation_ijkr[4], const double tr
 void aicb_eye_for_look_at(const aicb_aab *bounds, const double direction[3], double out_eye[3]);
 /* Camera::project_ndc_into_world for one NDC point (host, for tests): out = origin xyz, dir xyz. */
 void aicb_camera_project_ndc(const aicb_camera *, double ndc_x, double ndc_y, double out_origin_dir[6]);
+
+/* ---------------------------------------------------------------------------------------------
+ * The cursor: cursor_raycast (all-is-cubes/src/character/cursor.rs:26-107) and StandardCameras::project_cursor
+ * (all-is-cubes-render/src/camera/stdcam.rs:357-389) over a scene's cells on the device, for a batch of queries.
+ * One query finds the first cube of Raycaster::new(origin, normalize(direction)).within(bounds, false) whose block is
+ * selectable (AICB_BLOCK_NOT_SELECTABLE clear, not is_air) and whose voxels let the ray select it: a single voxel
+ * (Evoxels::One, or a resolution-1 block, whose voxel outside its bounds is Evoxel::AIR) by its AICB_VOXEL_* flag;
+ * otherwise the first voxel of recursive_raycast(...).within(voxel_bounds, true) that is selectable, face_selected
+ * being the face of that cast's first step.  The walk stops at the first step with t_distance > maximum_distance.
+ * Nothing of the scene changes: not the host mirror of the block ids (no call here rebuilds it), the light, the
+ * queue, the set of changed cubes, nor an asynchronous frame in flight (aicb_render_finish reports it unchanged).
+ * ------------------------------------------------------------------------------------------- */
+#define AICB_CURSOR_NONE 0xFFFFFFFFu      /* block_id of a query that selected nothing; preceding_block_id of WITHIN */
+#define AICB_CURSOR_OUTSIDE 0xFFFFFFFEu   /* preceding_block_id of a preceding cube outside the bounds (AIR there) */
+/* Cursor + its CubeSnapshots (cursor.rs:111-149), 80 bytes.  A query that selects nothing has block_id and
+ * preceding_block_id AICB_CURSOR_NONE and every other byte 0. */
+typedef struct aicb_cursor {
+    double point_entered[3];       /* step.intersection_point(ray), the ray's direction normalised */
+    double distance;               /* PositiveSign::new_clamped(step.t_distance()) */
+    int32_t cube[3];               /* the selected cube */
+    int32_t preceding_cube[3];     /* step.cube_behind(); = cube when face_entered is AICB_FACE_WITHIN */
+    uint32_t block_id;             /* the Space's block id at `cube` */
+    uint32_t preceding_block_id;   /* its id; AICB_CURSOR_OUTSIDE outside the bounds; AICB_CURSOR_NONE when WITHIN */
+    uint8_t light[4];              /* Space::get_light(cube), aicb_light_download's format (PackedLight::ONE under
+                                      LightPhysics::None) */
+    uint8_t preceding_light[4];    /* get_light(preceding_cube): BlockSky::light_outside beyond the bounds; 0 when
+                                      WITHIN */
+    uint8_t face_entered, face_selected;   /* Face7 (AICB_FACE_*) */
+    uint8_t layer;                 /* aicb_project_cursor: 0 nothing, 1 the UI layer, 2 the world layer; else 0 */
+    uint8_t _pad[5];
+} aicb_cursor;
+/* cursor_raycast for n rays {ox,oy,oz,dx,dy,dz}, with maximum_distance max_distance_or_null[i] (NULL: every ray
+ * f64::INFINITY; NaN sets no limit, as `t_distance > NaN` never holds).  Returns once `out` is written.
+ * AICB_ERR_INVALID with nothing written: NULL rays or out with n > 0.  n == 0 does nothing. */
+aicb_status aicb_cursor_raycast(aicb_scene *, const double (*origin_dir)[6], const double *max_distance_or_null,
+                                size_t n, aicb_cursor *out);
+/* The same with the rays (8-byte aligned), the distances and `out` (8-byte aligned) in device memory of the scene's
+ * device, issued on `stream` (NULL: the context's) with the device calls' ordering (aicb_scene_update_cubes_device):
+ * it reads the rays after the work queued there before it, and work queued there afterwards sees `out`.  It does not
+ * synchronise on one context.  Pointers are checked as those calls check them (AICB_ERR_INVALID). */
+aicb_status aicb_cursor_raycast_device(aicb_scene *, const double (*d_origin_dir)[6], const double *d_max_distance_or_null,
+                                       size_t n, aicb_cursor *d_out, void *stream);
+/* project_cursor for n NDC points: per point, the UI layer's cursor_raycast with f64::INFINITY, then if it selected
+ * nothing the world layer's with world_max_distance (the reference hard-codes 6.0); each layer's ray is
+ * Camera::project_ndc_into_world(ndc) of its camera (aicb_camera_project_ndc, as frames compute it), and `layer` says
+ * which answered.  Only the layers' scenes and cameras are read.  Either layer may be NULL.  AICB_ERR_INVALID with
+ * nothing written: NULL ndc or out with n > 0, a layer without a scene or camera, or layers on two contexts. */
+aicb_status aicb_project_cursor(const aicb_layer *world_or_null, const aicb_layer *ui_or_null, const double (*ndc)[2],
+                                size_t n, double world_max_distance, aicb_cursor *out);
+/* The group forms: outputs bit-identical to one context's.  The batch is cut into ranges of whole warps, one per
+ * replica, as aicb_group_trace_rays cuts its rays; each replica walks its own cells and stores into device 0.  The
+ * device form's buffers are device 0's memory; a group call returns once every replica's part is done.
+ * GPU test: tests/test_gpu_cursor.py. */
+aicb_status aicb_group_cursor_raycast(aicb_group_scene *, const double (*origin_dir)[6],
+                                      const double *max_distance_or_null, size_t n, aicb_cursor *out);
+aicb_status aicb_group_cursor_raycast_device(aicb_group_scene *, const double (*d_origin_dir)[6],
+                                             const double *d_max_distance_or_null, size_t n, aicb_cursor *d_out,
+                                             void *stream);
+aicb_status aicb_group_project_cursor(const aicb_group_layer *world_or_null, const aicb_group_layer *ui_or_null,
+                                      const double (*ndc)[2], size_t n, double world_max_distance, aicb_cursor *out);
 
 /* ---------------------------------------------------------------------------------------------
  * Light propagation (secondary path): replaces Mutation::set x n + evaluate_light(epsilon)
