@@ -147,6 +147,12 @@ def load_library() -> C.CDLL:
         getattr(lib, prefix + "cursor_raycast").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
         getattr(lib, prefix + "cursor_raycast_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                                                   C.c_void_p, C.c_void_p]
+    for prefix in ("aicb_", "aicb_group_"):
+        getattr(lib, prefix + "step_bodies").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double,
+                                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
+        getattr(lib, prefix + "step_bodies_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                               C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                               C.c_uint32, C.c_void_p]
     lib.aicb_project_cursor.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_size_t,
                                         C.c_double, C.c_void_p]
     lib.aicb_group_project_cursor.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
@@ -422,10 +428,15 @@ class Block:
 
     def __init__(self, *, color=None, emission=(0.0, 0.0, 0.0), is_air=False, resolution=1, voxel_lower=None,
                  indices: Optional[np.ndarray] = None, palette: Optional[np.ndarray] = None, selectable=True,
-                 voxel_selectable=None):
+                 voxel_selectable=None, collision=True, voxel_collision=None):
         """selectable: BlockAttributes::selectable (AICB_BLOCK_NOT_SELECTABLE when false; an air block is never
         selectable).  voxel_selectable: each palette entry's Evoxel::selectable (a bool or a bool per entry), written
-        into the palette's column 7 as AICB_VOXEL_NOT_SELECTABLE; None keeps the column as given (zero: selectable)."""
+        into the palette's column 7 as AICB_VOXEL_NOT_SELECTABLE; None keeps the column as given (zero: selectable).
+        collision: a single voxel's Evoxel::collision, True for BlockCollision::Hard, False for None.  voxel_collision:
+        each palette entry's, a bool or a bool per entry.  Both are kept beside the palette (voxel_no_collision) and
+        add AICB_VOXEL_NO_COLLISION to the flags of column 7 when the block is described to the library, so column 7
+        keeps what the caller wrote there (a caller may also set the bit in it directly).  The block's own collision is
+        derived from its voxels when it is placed."""
         self.is_air = bool(is_air)
         self.selectable = bool(selectable) and not self.is_air
         self.resolution = int(resolution)
@@ -450,7 +461,22 @@ class Block:
                 self.palette = self.palette.copy()
             sel = np.broadcast_to(np.asarray(voxel_selectable, dtype=bool), (self.palette.shape[0],))
             self.palette.view(np.uint32)[:, 7] = np.where(sel, 0, abi.VOXEL_NOT_SELECTABLE).astype(np.uint32)
+        if self.indices is None and not collision:
+            voxel_collision = False
+        self.voxel_no_collision = None if voxel_collision is None else ~np.broadcast_to(
+            np.asarray(voxel_collision, dtype=bool), (self.palette.shape[0],)).copy()
         self._derive_for_light()
+
+    def desc_palette(self) -> np.ndarray:
+        """The palette as the library reads it: column 7 with AICB_VOXEL_NO_COLLISION added where voxel_no_collision
+        says so (the palette itself when it says nothing)."""
+        mask = getattr(self, "voxel_no_collision", None)
+        if mask is None or not mask.any():
+            return self.palette
+        pal = np.array(self.palette, dtype=np.float32, copy=True)
+        col = pal.view(np.uint32)[:, 7]
+        col[mask] |= np.uint32(abi.VOXEL_NO_COLLISION)
+        return pal
 
     def _derive_for_light(self):
         """EvaluatedBlock derived data read by light propagation (block/eval/derived.rs:80-104 for single voxels,
@@ -631,6 +657,23 @@ class DeviceBlock:
         bd.light_emission[:] = bl.emission
 
 
+def bodies(n, position=(0.0, 0.0, 0.0), collision_box=(-0.5, -0.5, -0.5, 0.5, 0.5, 0.5), velocity=(0.0, 0.0, 0.0),
+           flying=False, noclip=False):
+    """n bodies as Body::new_minimal makes them (occupying: the box at the position), an abi.BODY_DTYPE array.  Each
+    argument is one value or one per body."""
+    b = np.zeros(n, dtype=abi.BODY_DTYPE)
+    p = np.broadcast_to(np.asarray(position, dtype=np.float64), (n, 3))
+    box = np.broadcast_to(np.asarray(collision_box, dtype=np.float64), (n, 6))
+    b["position"] = p
+    b["velocity"] = np.broadcast_to(np.asarray(velocity, dtype=np.float64), (n, 3))
+    b["collision_box"] = box
+    b["occupying"][:, :3] = box[:, :3] + p
+    b["occupying"][:, 3:] = box[:, 3:] + p
+    b["flying"] = flying
+    b["noclip"] = noclip
+    return b
+
+
 class Space:
     """What SpaceRaytracer::new reads from space::Read (sr.rs:64-88): bounds, per-cube block
     index (shape [X,Y,Z], C order == Vol Z-major, vol.rs:1013-1018), optional PackedLight texels
@@ -771,8 +814,10 @@ def fill_block_desc(bd, b):
     else:
         bd.indices = None
         bd.n_indices = 0
-    bd.palette = b.palette.ctypes.data
-    bd.n_palette = b.palette.shape[0]
+    pal = b.desc_palette() if hasattr(b, "desc_palette") else b.palette
+    b._desc_palette = pal   # kept alive with the block, which the caller keeps
+    bd.palette = pal.ctypes.data
+    bd.n_palette = pal.shape[0]
     bd.light_opaque_faces = b.light_opaque_faces
     bd.light_visible = 1 if b.light_visible else 0
     for f in range(6):
@@ -1088,6 +1133,41 @@ class _Scene:
         _check(self._fn("cursor_raycast")(self.handle, od.ctypes.data, None if md is None else md.ctypes.data, n,
                                           out.ctypes.data))
         return out
+
+    def step_bodies(self, bodies, dt, gravity, external_delta_v=None, max_contacts: int = 16, device: bool = False):
+        """step_one_body (physics/step.rs:316-590) against this scene for a batch of bodies: (bodies, info, contacts).
+        bodies: an abi.BODY_DTYPE array (see aicb200.bodies); info: abi.BODY_STEP_INFO_DTYPE; contacts:
+        abi.CONTACT_DTYPE [n, max_contacts], each body's ContactSet in first-insertion order (info["n_contacts"] of
+        them, at most max_contacts).  gravity: SpacePhysics::gravity; dt: Tick::delta_t in seconds, in (0, 1];
+        external_delta_v: None or [n, 3].  device=True: bodies is a uint8 CUDA tensor [n, 152] on the scene's device
+        (device 0 of a group), stepped in place on its current torch stream; external_delta_v a float64 tensor [n, 3]
+        or None; info and contacts are returned as uint8 tensors [n, 312] and [n, max_contacts, 28] (view them with
+        .cpu().numpy().view(abi.BODY_STEP_INFO_DTYPE) etc.)."""
+        g = np.ascontiguousarray(gravity, dtype=np.float64).reshape(3)
+        if device:
+            torch = _torch()
+            dev = self._device()
+            n = bodies.shape[0]
+            b = self._tensor(bodies, torch.uint8, (n, abi.BODY_DTYPE.itemsize), "bodies")
+            edv = None if external_delta_v is None else self._tensor(external_delta_v, torch.float64, (n, 3),
+                                                                      "external_delta_v")
+            info = torch.empty((n, abi.BODY_STEP_INFO_DTYPE.itemsize), dtype=torch.uint8, device=dev)
+            contacts = torch.zeros((n, max_contacts, abi.CONTACT_DTYPE.itemsize), dtype=torch.uint8, device=dev)
+            _check(self._fn("step_bodies_device")(self.handle, b.data_ptr(), None if edv is None else edv.data_ptr(),
+                                                   n, float(dt), g.ctypes.data, info.data_ptr(),
+                                                   contacts.data_ptr() if max_contacts else None, max_contacts,
+                                                   _stream(dev)))
+            return b, info, contacts
+        b = np.ascontiguousarray(bodies, dtype=abi.BODY_DTYPE).copy()
+        n = b.shape[0]
+        edv = None if external_delta_v is None else np.ascontiguousarray(
+            np.broadcast_to(np.asarray(external_delta_v, dtype=np.float64), (n, 3)))
+        info = np.zeros(n, dtype=abi.BODY_STEP_INFO_DTYPE)
+        contacts = np.zeros((n, max_contacts), dtype=abi.CONTACT_DTYPE)
+        _check(self._fn("step_bodies")(self.handle, b.ctypes.data, None if edv is None else edv.ctypes.data, n,
+                                       float(dt), g.ctypes.data, info.ctypes.data,
+                                       contacts.ctypes.data if max_contacts else None, max_contacts))
+        return b, info, contacts
 
     def _light_download_device(self):
         torch = _torch()

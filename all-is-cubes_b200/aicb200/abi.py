@@ -3,7 +3,7 @@ import ctypes as C
 
 import numpy as np
 
-ABI_VERSION = 24
+ABI_VERSION = 25
 
 BLOCKS_DERIVE_LIGHT = 1
 
@@ -165,6 +165,7 @@ class TextureTargetInfo(C.Structure):
 
 
 VOXEL_NOT_SELECTABLE = 1   # aicb_voxel::flags
+VOXEL_NO_COLLISION = 2     # aicb_voxel::flags
 BLOCK_NOT_SELECTABLE = 1   # aicb_block_desc::flags
 CURSOR_NONE = 0xFFFFFFFF
 CURSOR_OUTSIDE = 0xFFFFFFFE
@@ -184,6 +185,32 @@ CURSOR_DTYPE = np.dtype([("point_entered", "<f8", (3,)), ("distance", "<f8"), ("
                          ("light", "u1", (4,)), ("preceding_light", "u1", (4,)), ("face_entered", "u1"),
                          ("face_selected", "u1"), ("layer", "u1"), ("_pad", "u1", (5,))])
 assert CURSOR_DTYPE.itemsize == 80
+
+
+CONTACT_NONE, CONTACT_BLOCK, CONTACT_VOXEL = 0, 1, 2
+UNCRUSH_NOT_NEEDED, UNCRUSH_NOT_POSSIBLE, UNCRUSH_COMPLETE, UNCRUSH_PARTIAL = 0, 1, 2, 3
+AXIS_NONE = 0xFF
+BODY_INVALID = 1
+BODY_CONTACTS_TRUNCATED = 2
+BODY_NO_PENETRATION = 4
+BODY_SLIDING_UNFINISHED = 8
+BODY_CRUSH_UNFINISHED = 16
+
+# aicb_body, aicb_contact and aicb_body_step_info as numpy structured dtypes (what step_bodies takes and returns)
+BODY_DTYPE = np.dtype([("position", "<f8", (3,)), ("velocity", "<f8", (3,)), ("collision_box", "<f8", (6,)),
+                       ("occupying", "<f8", (6,)), ("flying", "u1"), ("noclip", "u1"), ("_pad", "u1", (6,))])
+assert BODY_DTYPE.itemsize == 152
+CONTACT_DTYPE = np.dtype([("cube", "<i4", (3,)), ("voxel", "<i4", (3,)), ("kind", "u1"), ("face", "u1"),
+                          ("resolution", "u1"), ("_pad", "u1")])
+assert CONTACT_DTYPE.itemsize == 28
+MOVE_SEGMENT_DTYPE = np.dtype([("delta_position", "<f8", (3,)), ("stopped_by", CONTACT_DTYPE), ("_pad", "<u4")])
+assert MOVE_SEGMENT_DTYPE.itemsize == 56
+BODY_STEP_INFO_DTYPE = np.dtype([("move_segments", MOVE_SEGMENT_DTYPE, (3,)), ("push_out", "<f8", (3,)),
+                                 ("initial_crush", "<f8", (6,)), ("delta_v", "<f8", (3,)),
+                                 ("already_colliding", CONTACT_DTYPE), ("n_contacts", "<u4"), ("status", "<u4"),
+                                 ("quiescent", "u1"), ("has_push_out", "u1"), ("uncrush", "u1"),
+                                 ("uncrush_axes", "u1", (3,)), ("_pad", "u1", (6,))])
+assert BODY_STEP_INFO_DTYPE.itemsize == 312
 
 
 EXPORTED_SYMBOLS = [
@@ -251,6 +278,10 @@ EXPORTED_SYMBOLS = [
     "aicb_group_cursor_raycast",
     "aicb_group_cursor_raycast_device",
     "aicb_group_project_cursor",
+    "aicb_step_bodies",
+    "aicb_step_bodies_device",
+    "aicb_group_step_bodies",
+    "aicb_group_step_bodies_device",
     "aicb_light_chart",
     "aicb_light_chart_chains",
     "aicb_light_fast_evaluate",

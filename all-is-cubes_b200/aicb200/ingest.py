@@ -7,13 +7,16 @@ What is read:
     (save/compress.rs:20-130: `{"Base64Gzip": "<standard base64 without padding of a gzip stream>"}`; contents are
     little-endian u16 block indices in Z-major order, light is `LightSerV1` = r, g, b, status with the status byte
     0 Uninitialized / 1 NoRays / 2 Opaque / 3 Visible, schema.rs:486-498 — NOT the PackedLight texel's status byte);
-  * `blocks`: `BlockV1` with the primitives `AirV1`, `AtomV1{color, light_emission}` and `RecurV1{space, offset,
+  * `blocks`: `BlockV1` with the primitives `AirV1`, `AtomV1{color, light_emission, collision}` and `RecurV1{space, offset,
     resolution}` (schema.rs:84-98) whose voxel Space consists of `AirV1` / `AtomV1` blocks — the cases whose evaluation
     is a table lookup (block/eval: an atom's Evoxel is its colour and emission; a Recur block's Evoxels are its
     Space's blocks over `offset .. offset + resolution`, clipped to the Space's bounds).
   * `SelectableV1{selectable}` sets the block's BlockAttributes::selectable (attributes.rs:389), and through
     Evoxel::from_block (voxel_storage.rs:76-100) the selectable of each voxel a `RecurV1` block takes from it; an
     `AirV1` block, and so an `AirV1` voxel, is never selectable (AIR_ATTRIBUTES);
+  * `AtomV1.collision` (`HardV1`, the default, or `NoneV1`; schema.rs:86-114) is the atom's voxel's collision, and a
+    `RecurV1` voxel takes its block's uniform collision (Evoxel::from_block: `uniform_collision().unwrap_or(Hard)`);
+    an `AirV1` block and an empty `RecurV1` region collide as BlockCollision::None;
   * modifiers that do not change what is drawn or picked (`DisplayNameV1`, `TagV1`, `QuoteV1`, inventory / action
     attributes) are ignored; `RotateV1`, `CompositeV1`, `ZoomV1`, `Move`, `IndirectV1` and `TextPrimitiveV1` need the
     reference's block evaluator (out of scope, SURVEY §2) and raise `UnsupportedBlock`.
@@ -66,7 +69,20 @@ def name_key(name) -> str:
 def _atom(prim):
     c = [float(v) for v in prim["color"]]
     e = [float(v) for v in prim.get("light_emission", (0.0, 0.0, 0.0))]
-    return c, e
+    coll = prim.get("collision", "HardV1")
+    if isinstance(coll, dict):
+        coll = coll.get("type")
+    if coll not in ("HardV1", "NoneV1"):
+        raise UnsupportedBlock(f"collision {coll!r}")
+    return c, e, coll == "HardV1"
+
+
+def _collides(block):
+    """Evoxel::from_block's collision for a voxel Space's block: an air block's is None, an atom's its own."""
+    if block.is_air:
+        return False
+    mask = block.voxel_no_collision
+    return mask is None or not bool(mask[0])
 
 
 def _block_of(block_ser, resolve_space):
@@ -83,8 +99,8 @@ def _block_of(block_ser, resolve_space):
     if kind == "AirV1":
         return Block.air()
     if kind == "AtomV1":
-        c, e = _atom(prim)
-        return Block(color=tuple(c), emission=tuple(e), selectable=selectable)
+        c, e, hard = _atom(prim)
+        return Block(color=tuple(c), emission=tuple(e), selectable=selectable, collision=hard)
     if kind == "RecurV1":
         if resolve_space is None:
             raise UnsupportedBlock("RecurV1 needs the universe the Space handle points into")
@@ -95,7 +111,7 @@ def _block_of(block_ser, resolve_space):
         lo = [max(off[a], vs.lower[a]) for a in range(3)]
         hi = [min(off[a] + res, vs.lower[a] + vs.size[a]) for a in range(3)]
         if any(hi[a] <= lo[a] for a in range(3)):
-            return Block(color=(0.0, 0.0, 0.0, 0.0), selectable=selectable)
+            return Block(color=(0.0, 0.0, 0.0, 0.0), selectable=selectable, collision=False)
         sl = tuple(slice(lo[a] - vs.lower[a], hi[a] - vs.lower[a]) for a in range(3))
         ids = vs.block_ids[sl]
         pal = np.zeros((len(vs.blocks), 8), dtype=np.float32)
@@ -104,7 +120,8 @@ def _block_of(block_ser, resolve_space):
                 raise UnsupportedBlock("a voxel Space made of recursive blocks needs the reference's block evaluator")
             pal[i] = b.palette[0]
         return Block(resolution=res, voxel_lower=[lo[a] - off[a] for a in range(3)], indices=ids.astype(np.uint16),
-                     palette=pal, selectable=selectable, voxel_selectable=[b.selectable for b in vs.blocks])
+                     palette=pal, selectable=selectable, voxel_selectable=[b.selectable for b in vs.blocks],
+                     voxel_collision=[_collides(b) for b in vs.blocks])
     raise UnsupportedBlock(f"primitive {kind} needs the reference's block evaluator")
 
 

@@ -97,7 +97,7 @@ static void build_block_sky(const aicb_sky &sky, DeviceScene *ds) {
 // log2(1 - alpha)} per palette entry.
 // Called by flatten_blocks alone.
 static const char *const BRICKS_PAST_2_32 = "brick pool exceeds 2^32 voxels";
-static const aicb_voxel AIR_VOXEL = {{0, 0, 0, 0}, {0, 0, 0}, AICB_VOXEL_NOT_SELECTABLE};   // Evoxel::AIR
+static const aicb_voxel AIR_VOXEL = {{0, 0, 0, 0}, {0, 0, 0}, AICB_VOXEL_NOT_SELECTABLE | AICB_VOXEL_NO_COLLISION};   // Evoxel::AIR
 
 // blk_tab entry of a block: what the marching kernel needs of a single-voxel surface on the Space level.
 // `pal_off` indexes `pal_tab`; `pal_base` is added to it for the device-wide palette index.
@@ -152,11 +152,13 @@ aicb_voxel single_voxel_of(const aicb_block_desc &b) {
 }
 
 // The record of a definition of kind `kind` (an air block's is KIND_INVISIBLE) whose voxel data starts at brick word
-// `brick_off` and palette entry `pal_off`.
+// `brick_off` and palette entry `pal_off`.  Of its collision bits only an air block's are here: the others come from
+// the voxels, which flatten_block reads on the host and k_block_records on the device.
 static BlockRec block_rec(const aicb_block_desc &b, uint8_t kind, uint32_t brick_off, uint32_t pal_off) {
     BlockRec r;
     std::memset(&r, 0, sizeof r);
     r.flags = (b.is_air || (b.flags & AICB_BLOCK_NOT_SELECTABLE)) ? AICB_BLOCK_NOT_SELECTABLE : 0u;
+    if (b.is_air) r.flags |= BLOCK_COLLISION_NONE;   // AIR_EVALUATED
     if (b.is_air) {
         r.kind_res = KIND_INVISIBLE | (1u << 8);
     } else if (kind != KIND_RECURSIVE) {
@@ -192,6 +194,7 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
     } else if (single) {
         kind = voxel_invisible(sv) ? KIND_INVISIBLE : KIND_SINGLE;
         r = block_rec(b, kind, 0, (uint32_t)(palette.size() / 2));
+        if (sv.flags & AICB_VOXEL_NO_COLLISION) r.flags |= BLOCK_COLLISION_NONE;
         push_voxel(sv);
     } else {
         kind = KIND_RECURSIVE;
@@ -202,6 +205,12 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
             bricks.push_back(v << 16 | (voxel_invisible(b.palette[v]) ? 0x8000u : 0u));
         }
         for (size_t k = 0; k < b.n_palette; k++) push_voxel(b.palette[k]);
+        const bool less = less_than_full(r);
+        uint32_t pal_mask = 0, used_mask = 0;
+        for (size_t k = 0; k < b.n_palette; k++) pal_mask |= collision_mask(b.palette[k].flags);
+        if ((pal_mask | (less ? 2u : 0u)) == 3u)   // the palette disagrees: the entries in use decide
+            for (size_t k = 0; k < b.n_indices && used_mask != 3u; k++) used_mask |= collision_mask(b.palette[b.indices[k]].flags);
+        r.flags |= block_collision(pal_mask, used_mask, less);
     }
     return AICB_OK;
 }
@@ -1214,7 +1223,7 @@ static aicb_status copy_device(aicb_ctx *ctx, const BlockTable &t, const FlatBlo
     TRY(delta_room(ctx, bytes));
     std::memcpy(ctx->h_delta.get(), dev.jobs.data(), bytes);
     CU(cudaMemcpyAsync(ctx->d_delta.get(), ctx->h_delta.get(), bytes, cudaMemcpyHostToDevice, stream));
-    return issue_block_data(stream, ctx->d_delta.get<const DeviceBlockJob>(), (uint32_t)dev.jobs.size(),
+    return issue_block_data(stream, ctx->d_delta.get<DeviceBlockJob>(), (uint32_t)dev.jobs.size(),
                             dev.most_words, dev.most_entries, f.wide_bricks, t, dev.d_derived);
 }
 

@@ -20,12 +20,29 @@ __host__ __device__ inline bool voxel_invisible(const aicb_voxel &v) {
 }
 
 // The .w lane of a palette entry's second float4 (its emission): the voxel's AICB_VOXEL_NOT_SELECTABLE bit, which only
-// the cursor reads.  The other bits of aicb_voxel::flags are not kept.
+// the cursor reads, and its AICB_VOXEL_NO_COLLISION bit, which only the body step reads.  The other bits of
+// aicb_voxel::flags are not kept.
 __host__ __device__ inline float voxel_flags(const aicb_voxel &v) {
-    const uint32_t f = v.flags & AICB_VOXEL_NOT_SELECTABLE;
+    const uint32_t f = v.flags & (AICB_VOXEL_NOT_SELECTABLE | AICB_VOXEL_NO_COLLISION);
     float w;
     memcpy(&w, &f, 4);
     return w;
+}
+
+// A voxel's collision as a bit of a collision mask: 1 some voxel is Hard, 2 some voxel is None.
+__host__ __device__ inline uint32_t collision_mask(uint32_t voxel_flags_word) {
+    return (voxel_flags_word & AICB_VOXEL_NO_COLLISION) ? 2u : 1u;
+}
+
+// A recursive block's BlockRec collision bits (trace_kernel.cuh: BLOCK_COLLISION_*) from the collision masks of its
+// palette and of the palette entries its voxels use, as compute_derived's uniform_collision (derived.rs:159-190): the
+// implicit air outside voxel bounds smaller than the block counts as None; then the palette, if all its entries agree;
+// then the entries in use; else mixed.  An empty sequence agrees on nothing.
+__host__ __device__ inline uint32_t block_collision(uint32_t palette_mask, uint32_t used_mask, bool less_than_full) {
+    const uint32_t outside = less_than_full ? 2u : 0u, p = palette_mask | outside, u = used_mask | outside;
+    if (p == 1u || u == 1u) return 0u;
+    if (p == 2u || u == 2u) return 2u;   // BLOCK_COLLISION_NONE
+    return 4u;                           // BLOCK_COLLISION_MIXED
 }
 
 // {alpha, l2a}: l2a >= log2(1 - alpha) (the f32 value apply_transmittance raises to a span's thickness), so the

@@ -42,7 +42,7 @@ const unsigned THREADS = 256;
 __device__ aicb_voxel single_voxel(const DeviceBlockJob &J) {
     aicb_voxel v;
     memset(&v, 0, sizeof v);
-    v.flags = AICB_VOXEL_NOT_SELECTABLE;   // Evoxel::AIR
+    v.flags = AICB_VOXEL_NOT_SELECTABLE | AICB_VOXEL_NO_COLLISION;   // Evoxel::AIR
     if (J.single == SINGLE_FIRST) v = J.palette[0];
     else if (J.single == SINGLE_INDEXED) {
         const uint32_t k = J.indices[0];
@@ -68,14 +68,22 @@ __global__ void __launch_bounds__(THREADS) k_block_verdict(const DeviceBlockJob 
         kinds[blockIdx.x] = (uint8_t)(voxel_invisible(single_voxel(J)) ? KIND_INVISIBLE : KIND_SINGLE);
 }
 
+// A warp's OR of `mask` into a job's collision word.
+__device__ __forceinline__ void or_collision(DeviceBlockJob &J, uint32_t mask) {
+    mask = __reduce_or_sync(0xffffffffu, mask);
+    if ((threadIdx.x & 31) == 0 && mask) atomicOr(&J.collision, mask);
+}
+
 // Brick words of the recursive jobs at pool positions [brick_off, brick_off + n_indices), in groups of 16 bytes of
-// the pool: a whole group is one store, a group cut by the range's ends is stored word by word.
+// the pool: a whole group is one store, a group cut by the range's ends is stored word by word.  The collision masks of
+// the entries the voxels use go into the job's collision word (bits 2-3).
 template <bool WIDE>
-__global__ void __launch_bounds__(THREADS) k_block_bricks(const DeviceBlockJob *jobs, void *pool) {
+__global__ void __launch_bounds__(THREADS) k_block_bricks(DeviceBlockJob *jobs, void *pool) {
     using Word = typename std::conditional<WIDE, uint32_t, uint16_t>::type;
     constexpr uint32_t G = 16 / sizeof(Word);
-    const DeviceBlockJob &J = jobs[blockIdx.x];
+    DeviceBlockJob &J = jobs[blockIdx.x];
     if (J.kind != KIND_RECURSIVE) return;
+    uint32_t used = 0;
     const uint64_t lo = J.brick_off, hi = lo + J.n_indices;
     Word *out = static_cast<Word *>(pool);
     for (uint64_t g = lo / G + (uint64_t)blockIdx.y * THREADS + threadIdx.x; g * G < hi; g += (uint64_t)gridDim.y * THREADS) {
@@ -89,6 +97,7 @@ __global__ void __launch_bounds__(THREADS) k_block_bricks(const DeviceBlockJob *
             if (p < lo || p >= hi) continue;
             const uint32_t k = __ldg(J.indices + (p - lo));
             const uint32_t inv = invisible_at(J.palette, k) ? 0x8000u : 0u;
+            used |= collision_mask(__ldg(&J.palette[k].flags));
             u.w[j] = (Word)(WIDE ? k << 16 | inv : k | inv);
         }
         if (g * G >= lo && g * G + G <= hi) reinterpret_cast<uint4 *>(out)[g] = u.v;
@@ -96,18 +105,23 @@ __global__ void __launch_bounds__(THREADS) k_block_bricks(const DeviceBlockJob *
             for (uint32_t j = 0; j < G; j++)
                 if (g * G + j >= lo && g * G + j < hi) out[g * G + j] = u.w[j];
     }
+    or_collision(J, used << 2);
 }
 
-// Palette entries: a recursive job's palette, a single voxel's one entry; air has none.
-__global__ void __launch_bounds__(THREADS) k_block_palette(const DeviceBlockJob *jobs, float4 *palette, float2 *pal_tab) {
-    const DeviceBlockJob &J = jobs[blockIdx.x];
+// Palette entries: a recursive job's palette, a single voxel's one entry; air has none.  A recursive job's palette's
+// collision mask goes into its collision word (bits 0-1).
+__global__ void __launch_bounds__(THREADS) k_block_palette(DeviceBlockJob *jobs, float4 *palette, float2 *pal_tab) {
+    DeviceBlockJob &J = jobs[blockIdx.x];
+    uint32_t mask = 0;
     for (uint32_t e = blockIdx.y * THREADS + threadIdx.x; e < J.n_entries; e += gridDim.y * THREADS) {
         const aicb_voxel v = J.kind == KIND_RECURSIVE ? J.palette[e] : single_voxel(J);
         const size_t at = (size_t)J.pal_off + e;
         palette[2 * at] = make_float4(v.rgba[0], v.rgba[1], v.rgba[2], v.rgba[3]);
         palette[2 * at + 1] = make_float4(v.emission[0], v.emission[1], v.emission[2], voxel_flags(v));
         pal_tab[at] = surface_entry(v.rgba[3]);
+        mask |= collision_mask(v.flags);
     }
+    if (J.kind == KIND_RECURSIVE) or_collision(J, mask);
 }
 
 // compute_derived of a single voxel (derived.rs:84-104), as derive.cu's single_light.
@@ -124,6 +138,7 @@ __device__ aicb_block_light single_light(const aicb_voxel &v) {
 }
 
 // One thread per job that writes its id's records (a repeated id: its last definition of the call).
+// A recursive job's collision bits come from the masks k_block_palette and k_block_bricks left in its collision word.
 __global__ void __launch_bounds__(THREADS) k_block_records(const DeviceBlockJob *jobs, uint32_t n, BlockRec *blocks,
                                                            float4 *blk_tab, LightBlockDev *light,
                                                            const aicb_block_light *derived) {
@@ -131,7 +146,14 @@ __global__ void __launch_bounds__(THREADS) k_block_records(const DeviceBlockJob 
     if (i >= n) return;
     const DeviceBlockJob &J = jobs[i];
     if (J.id == NO_ID) return;
-    blocks[J.id] = J.rec;
+    BlockRec rec = J.rec;   // an air block's collision bits are in it already (block_rec)
+    if (!(rec.flags & BLOCK_COLLISION_NONE)) {
+        if (J.kind == KIND_RECURSIVE)
+            rec.flags |= block_collision(J.collision & 3u, (J.collision >> 2) & 3u, less_than_full(rec));
+        else if (single_voxel(J).flags & AICB_VOXEL_NO_COLLISION)
+            rec.flags |= BLOCK_COLLISION_NONE;
+    }
+    blocks[J.id] = rec;
     float4 e = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     if (J.kind == KIND_SINGLE) {
         const float2 s = surface_entry(single_voxel(J).rgba[3]);
@@ -200,7 +222,7 @@ aicb_status issue_block_verdict(cudaStream_t stream, const DeviceBlockJob *jobs,
     return AICB_OK;
 }
 
-aicb_status issue_block_data(cudaStream_t stream, const DeviceBlockJob *jobs, uint32_t n, uint64_t most_words,
+aicb_status issue_block_data(cudaStream_t stream, DeviceBlockJob *jobs, uint32_t n, uint64_t most_words,
                              uint64_t most_entries, bool wide_bricks, const BlockTable &t,
                              const aicb_block_light *derived) {
     if (n == 0) return AICB_OK;

@@ -217,6 +217,7 @@ struct aicb_ctx {
     DeviceBuffer d_derive;       // aicb_derive_block_light's per-palette-entry and per-ray terms and its results
     DeviceBuffer d_inputs;       // the device-input calls' scratch: verdict, sorted cube lists, staged entries
     DeviceBuffer d_cursor;       // the host cursor calls' queries and results (cursor.cu), apart from a frame's buffers
+    DeviceBuffer d_bodies;       // the host body steps' bodies and results (body.cu)
     std::mutex mu;
 };
 
@@ -549,7 +550,8 @@ struct DeviceBlockJob {
     uint32_t id;                 // the id whose records it writes; NO_ID: a later definition of the call writes them
     int32_t derived;             // its light record: LIGHT_GIVEN (`light`), LIGHT_SINGLE (its voxel's) or derive's record
     uint32_t light_visible;      // ORed into Derived::visible
-    uint32_t _pad;
+    uint32_t collision;          // collision masks (block_words.cuh) of a recursive job's palette (bits 0-1) and of the
+                                 // entries its voxels use (bits 2-3), ORed in by k_block_palette and k_block_bricks
     aicb::BlockRec rec;
     LightBlockDev light;
 };
@@ -559,7 +561,7 @@ aicb_status issue_block_verdict(cudaStream_t stream, const DeviceBlockJob *jobs,
                                 InputVerdict *v, uint8_t *kinds);
 // The jobs' brick words, palette entries and per-id records into table `t` (room made, positions in the jobs);
 // `derived`: derive's records (device 0's memory), or nullptr.
-aicb_status issue_block_data(cudaStream_t stream, const DeviceBlockJob *jobs, uint32_t n, uint64_t most_words,
+aicb_status issue_block_data(cudaStream_t stream, DeviceBlockJob *jobs, uint32_t n, uint64_t most_words,
                              uint64_t most_entries, bool wide_bricks, const BlockTable &t,
                              const aicb_block_light *derived);
 // Every cell whose id has word[id] != NO_WORD takes that word, on the context's stream.

@@ -72,10 +72,21 @@ struct BlockRec {
     uint16_t vsize[3];     // voxel_bounds size
     uint32_t brick_off;    // first u16 of this block's brick in the pool
     uint32_t pal_off;      // first palette entry (single: the voxel)
-    uint32_t flags;        // AICB_BLOCK_NOT_SELECTABLE (set for an is_air block); read by the cursor alone
+    uint32_t flags;        // AICB_BLOCK_NOT_SELECTABLE (set for an is_air block), read by the cursor; BLOCK_COLLISION_*,
+                           // read by the body step
     uint32_t _pad;
 };
 static_assert(sizeof(BlockRec) == 32, "BlockRec must be 32 bytes");
+// BlockRec::flags: the block's uniform_collision (derived.rs:159-190), derived when the block is placed
+// (block_words.cuh: block_collision).  Neither bit: Some(Hard).
+constexpr uint32_t BLOCK_COLLISION_NONE = 2u;    // Some(BlockCollision::None); every is_air block
+constexpr uint32_t BLOCK_COLLISION_MIXED = 4u;   // None: the voxels' AICB_VOXEL_NO_COLLISION bits decide
+
+// A recursive block's voxel bounds are smaller than the block (derived.rs:112: full_block_bounds != data_bounds).
+__host__ __device__ inline bool less_than_full(const BlockRec &r) {
+    const uint32_t res = r.kind_res >> 8;
+    return r.vlo[0] != 0 || r.vlo[1] != 0 || r.vlo[2] != 0 || r.vsize[0] != res || r.vsize[1] != res || r.vsize[2] != res;
+}
 
 struct DeviceScene {
     int32_t lo[3];

@@ -45,6 +45,8 @@ pub struct aicb_voxel {
 
 /// `Evoxel::selectable == false`
 pub const AICB_VOXEL_NOT_SELECTABLE: u32 = 1;
+/// `Evoxel::collision == BlockCollision::None` (zero: `Hard`)
+pub const AICB_VOXEL_NO_COLLISION: u32 = 2;
 /// `BlockAttributes::selectable == false` (an `is_air` block is never selectable)
 pub const AICB_BLOCK_NOT_SELECTABLE: u32 = 1;
 /// `aicb_cursor::block_id` of a query that selected nothing; `preceding_block_id` of a ray that started in the cube
@@ -68,6 +70,73 @@ pub struct aicb_cursor {
     pub face_selected: u8,
     pub layer: u8,
     pub _pad: [u8; 5],
+}
+
+/// `Body` (physics/body.rs:38-90) without its look direction; boxes are `[lower xyz, upper xyz]`
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_body {
+    pub position: [f64; 3],
+    pub velocity: [f64; 3],
+    pub collision_box: [f64; 6],
+    pub occupying: [f64; 6],
+    pub flying: u8,
+    pub noclip: u8,
+    pub _pad: [u8; 6],
+}
+
+pub const AICB_CONTACT_NONE: u8 = 0;
+pub const AICB_CONTACT_BLOCK: u8 = 1;
+pub const AICB_CONTACT_VOXEL: u8 = 2;
+
+/// `Contact` (physics/contact.rs:31-48), or `AICB_CONTACT_NONE` for an absent one
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default, PartialEq, Eq, Hash)]
+pub struct aicb_contact {
+    pub cube: [i32; 3],
+    pub voxel: [i32; 3],
+    pub kind: u8,
+    pub face: u8,
+    pub resolution: u8,
+    pub _pad: u8,
+}
+
+/// `MoveSegment` (physics/step.rs:231-241)
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_move_segment {
+    pub delta_position: [f64; 3],
+    pub stopped_by: aicb_contact,
+    pub _pad: u32,
+}
+
+pub const AICB_UNCRUSH_NOT_NEEDED: u8 = 0;
+pub const AICB_UNCRUSH_NOT_POSSIBLE: u8 = 1;
+pub const AICB_UNCRUSH_COMPLETE: u8 = 2;
+pub const AICB_UNCRUSH_PARTIAL: u8 = 3;
+pub const AICB_AXIS_NONE: u8 = 0xFF;
+pub const AICB_BODY_INVALID: u32 = 1;
+pub const AICB_BODY_CONTACTS_TRUNCATED: u32 = 2;
+pub const AICB_BODY_NO_PENETRATION: u32 = 4;
+pub const AICB_BODY_SLIDING_UNFINISHED: u32 = 8;
+pub const AICB_BODY_CRUSH_UNFINISHED: u32 = 16;
+
+/// `BodyStepDetails` (physics/step.rs:160-215) and the size of the body's `ContactSet`
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_body_step_info {
+    pub move_segments: [aicb_move_segment; 3],
+    pub push_out: [f64; 3],
+    pub initial_crush: [f64; 6],
+    pub delta_v: [f64; 3],
+    pub already_colliding: aicb_contact,
+    pub n_contacts: u32,
+    pub status: u32,
+    pub quiescent: u8,
+    pub has_push_out: u8,
+    pub uncrush: u8,
+    pub uncrush_axes: [u8; 3],
+    pub _pad: [u8; 6],
 }
 
 /// one entry of `Space::block_data()` as `TracingBlock::from_block` sees it (sr.rs:569-587) plus the
@@ -550,6 +619,24 @@ unsafe extern "C" {
     pub fn aicb_group_project_cursor(world_or_null: *const aicb_group_layer, ui_or_null: *const aicb_group_layer,
                                      ndc: *const [f64; 2], n: usize, world_max_distance: f64, out: *mut aicb_cursor)
                                      -> aicb_status;
+
+    pub fn aicb_step_bodies(s: *mut aicb_scene, bodies: *mut aicb_body, external_delta_v_or_null: *const [f64; 3],
+                            n: usize, dt: f64, gravity: *const f64, info_or_null: *mut aicb_body_step_info,
+                            contacts_or_null: *mut aicb_contact, max_contacts: u32) -> aicb_status;
+    pub fn aicb_step_bodies_device(s: *mut aicb_scene, d_bodies: *mut aicb_body,
+                                   d_external_delta_v_or_null: *const [f64; 3], n: usize, dt: f64,
+                                   gravity: *const f64, d_info_or_null: *mut aicb_body_step_info,
+                                   d_contacts_or_null: *mut aicb_contact, max_contacts: u32, stream: *mut c_void)
+                                   -> aicb_status;
+    pub fn aicb_group_step_bodies(gs: *mut aicb_group_scene, bodies: *mut aicb_body,
+                                  external_delta_v_or_null: *const [f64; 3], n: usize, dt: f64, gravity: *const f64,
+                                  info_or_null: *mut aicb_body_step_info, contacts_or_null: *mut aicb_contact,
+                                  max_contacts: u32) -> aicb_status;
+    pub fn aicb_group_step_bodies_device(gs: *mut aicb_group_scene, d_bodies: *mut aicb_body,
+                                         d_external_delta_v_or_null: *const [f64; 3], n: usize, dt: f64,
+                                         gravity: *const f64, d_info_or_null: *mut aicb_body_step_info,
+                                         d_contacts_or_null: *mut aicb_contact, max_contacts: u32,
+                                         stream: *mut c_void) -> aicb_status;
 
     pub fn aicb_light_chart(weights: *mut f32, children: *mut u32) -> u32;
     pub fn aicb_light_chart_chains(preorder: *mut u32, chains: *mut [u32; 6], euler: *mut u16) -> u32;

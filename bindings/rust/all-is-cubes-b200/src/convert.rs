@@ -57,7 +57,10 @@ pub fn block_desc_of(data: &space::SpaceBlockData) -> OwnedBlockDesc {
     let voxel = |v: &all_is_cubes::block::Evoxel| {
         let c: [f32; 4] = v.color.into();
         let e: [f32; 3] = v.emission.into();
-        let flags = if v.selectable { 0 } else { sys::AICB_VOXEL_NOT_SELECTABLE };
+        let mut flags = if v.selectable { 0 } else { sys::AICB_VOXEL_NOT_SELECTABLE };
+        if v.collision == all_is_cubes::block::BlockCollision::None {
+            flags |= sys::AICB_VOXEL_NO_COLLISION;
+        }
         sys::aicb_voxel { rgba: c, emission: e, flags }
     };
     let (indices, palette, bounds, resolution) = match ev.voxels() {
@@ -74,7 +77,7 @@ pub fn block_desc_of(data: &space::SpaceBlockData) -> OwnedBlockDesc {
                 .as_linear()
                 .iter()
                 .map(|v| {
-                    *lookup.entry((v.color.to_bits(), v.emission.to_bits(), v.selectable)).or_insert_with(|| {
+                    *lookup.entry((v.color.to_bits(), v.emission.to_bits(), v.selectable, v.collision == all_is_cubes::block::BlockCollision::None)).or_insert_with(|| {
                         palette.push(voxel(v));
                         (palette.len() - 1) as u16
                     })
@@ -115,6 +118,36 @@ pub fn block_desc_of(data: &space::SpaceBlockData) -> OwnedBlockDesc {
 }
 
 /// What `Camera::project_ndc_into_world` / `post_process_color` need (camera_struct.rs:238-257, 376-382).
+/// A `Body` as `aicb_step_bodies` takes it (physics/body.rs: every field through the public accessors;
+/// `collision_box_abs()` is `occupying`).
+pub fn body_of(body: &all_is_cubes::physics::Body) -> sys::aicb_body {
+    let aab = |a: all_is_cubes::math::Aab| {
+        let (l, u) = (a.lower_bounds_p(), a.upper_bounds_p());
+        [l.x, l.y, l.z, u.x, u.y, u.z]
+    };
+    let p = body.position();
+    let v = body.velocity();
+    sys::aicb_body {
+        position: [p.x, p.y, p.z],
+        velocity: [v.x, v.y, v.z],
+        collision_box: aab(body.collision_box_rel()),
+        occupying: aab(body.collision_box_abs()),
+        flying: u8::from(body.flying),
+        noclip: u8::from(body.noclip),
+        _pad: [0; 6],
+    }
+}
+
+/// A stepped `aicb_body` back into `body`: its position and velocity.  `Body::set_position` resets `occupying` to the
+/// uncrushed box, which is what the next step's `uncrush` would restore where there is room; the crushed box itself
+/// cannot be written from outside the reference's physics module.
+pub fn apply_stepped_body(body: &mut all_is_cubes::physics::Body, stepped: &sys::aicb_body) {
+    let [x, y, z] = stepped.position;
+    body.set_position(all_is_cubes::math::FreePoint::new(x, y, z));
+    let [vx, vy, vz] = stepped.velocity;
+    body.set_velocity(euclid::vec3(vx, vy, vz));
+}
+
 pub fn camera_of(camera: &Camera) -> sys::aicb_camera {
     let size = camera.viewport().framebuffer_size;
     sys::aicb_camera {

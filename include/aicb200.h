@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 24
+#define AICB_ABI_VERSION 25
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -46,8 +46,8 @@ typedef struct aicb_aab {
     uint32_t size[3];
 } aicb_aab;
 
-/* Evoxel (all-is-cubes/src/block/eval/voxel_storage.rs:41-60) without its collision:
- * non-premultiplied linear RGBA reflectance + RGB emission, and `flags`. 32 bytes. */
+/* Evoxel (all-is-cubes/src/block/eval/voxel_storage.rs:41-60): non-premultiplied linear RGBA reflectance + RGB
+ * emission, and `flags` (selectable, collision). 32 bytes. */
 typedef struct aicb_voxel {
     float rgba[4];
     float emission[3];
@@ -55,6 +55,9 @@ typedef struct aicb_voxel {
 } aicb_voxel;
 /* Evoxel::selectable == false (voxel_storage.rs:57).  Zero, the default, is selectable.  Only the cursor reads it. */
 #define AICB_VOXEL_NOT_SELECTABLE 1u
+/* Evoxel::collision == BlockCollision::None (voxel_storage.rs:60).  Zero, the default, is BlockCollision::Hard
+ * (DEFAULT_FOR_FROM_COLOR, attributes.rs:527).  Only aicb_step_bodies reads it. */
+#define AICB_VOXEL_NO_COLLISION 2u
 
 /* Face7 (all-is-cubes-base/src/math/face.rs:105). */
 enum { AICB_FACE_WITHIN = 0, AICB_FACE_NX = 1, AICB_FACE_NY = 2, AICB_FACE_NZ = 3,
@@ -909,6 +912,103 @@ aicb_status aicb_group_cursor_raycast_device(aicb_group_scene *, const double (*
                                              void *stream);
 aicb_status aicb_group_project_cursor(const aicb_group_layer *world_or_null, const aicb_group_layer *ui_or_null,
                                       const double (*ndc)[2], size_t n, double world_max_distance, aicb_cursor *out);
+
+/* ---------------------------------------------------------------------------------------------
+ * Bodies: step_one_body (all-is-cubes/src/physics/step.rs:316-590) against a scene's cells on the device, for a batch
+ * of bodies, with the collision functions of physics/collision.rs:100-249.  A block's collision is derived when it is
+ * placed, as compute_derived derives uniform_collision (block/eval/derived.rs:85-104, 159-190): Hard, None, or mixed,
+ * in which case its voxels' AICB_VOXEL_NO_COLLISION flags decide; an is_air block is None.  Arithmetic is f64 without
+ * contraction, as the reference's.  Nothing of the scene changes (as the cursor calls: no host mirror rebuild, no light
+ * state, no frame in flight).
+ * ------------------------------------------------------------------------------------------- */
+/* Body (physics/body.rs:38-90) without its look direction, 152 bytes.  Boxes are {lower xyz, upper xyz}.  `occupying`
+ * should contain `position` (Body's invariant), but a crush can leave it not containing it, as the reference's
+ * crush_if_colliding can ("TODO: stop if we would lose the occupying-contains-position property"), so a body a step
+ * returns is always a body a step takes. */
+typedef struct aicb_body {
+    double position[3];
+    double velocity[3];
+    double collision_box[6];       /* relative to position */
+    double occupying[6];           /* absolute; should contain position (see above), need not */
+    uint8_t flying, noclip;
+    uint8_t _pad[6];
+} aicb_body;
+enum { AICB_CONTACT_NONE = 0, AICB_CONTACT_BLOCK = 1, AICB_CONTACT_VOXEL = 2 };
+/* Contact (physics/contact.rs:31-48), 28 bytes: Block(CubeFace { cube, face }) or Voxel { cube, resolution,
+ * voxel: CubeFace }; AICB_CONTACT_NONE stands for Option::None where a contact is optional.  `voxel` and
+ * `resolution` are 0 unless kind is AICB_CONTACT_VOXEL. */
+typedef struct aicb_contact {
+    int32_t cube[3];
+    int32_t voxel[3];
+    uint8_t kind;                  /* AICB_CONTACT_* */
+    uint8_t face;                  /* Face7 (AICB_FACE_*) */
+    uint8_t resolution;
+    uint8_t _pad;
+} aicb_contact;
+/* MoveSegment (step.rs:231-241), 56 bytes. */
+typedef struct aicb_move_segment {
+    double delta_position[3];
+    aicb_contact stopped_by;       /* kind AICB_CONTACT_NONE: not stopped */
+    uint32_t _pad;
+} aicb_move_segment;
+/* UncrushInfo (step.rs:281-295) */
+enum { AICB_UNCRUSH_NOT_NEEDED = 0, AICB_UNCRUSH_NOT_POSSIBLE = 1, AICB_UNCRUSH_COMPLETE = 2,
+       AICB_UNCRUSH_PARTIAL = 3 };
+#define AICB_AXIS_NONE 0xFFu
+/* aicb_body_step_info::status bits.  INVALID: the body could not be a Body (a non-finite position, velocity or
+ * external delta-v, a non-finite, empty or inverted collision_box, or a non-finite or inverted occupying); the body is unchanged and the rest of its info is zero.  NO_PENETRATION and SLIDING_UNFINISHED
+ * are the reference's panics "collision but found no penetration" and "sliding collision loop did not finish";
+ * CRUSH_UNFINISHED is a crush where the reference would not return: a shrink that leaves the box as it was (the
+ * same box meets the same contact forever), or more shrinks than a finishing crush can take (four per plane of
+ * resolution 128 that each face of the box could cross, plus 64).  With
+ * any of the three the body is unchanged and its info holds only the status.  CONTACTS_TRUNCATED: the contact set
+ * held more than max_contacts contacts; the step is unaffected. */
+#define AICB_BODY_INVALID 1u
+#define AICB_BODY_CONTACTS_TRUNCATED 2u
+#define AICB_BODY_NO_PENETRATION 4u
+#define AICB_BODY_SLIDING_UNFINISHED 8u
+#define AICB_BODY_CRUSH_UNFINISHED 16u
+/* BodyStepDetails (step.rs:160-215) and the size of the body's ContactSet, 312 bytes. */
+typedef struct aicb_body_step_info {
+    aicb_move_segment move_segments[3];
+    double push_out[3];            /* valid if has_push_out */
+    double initial_crush[6];       /* CrushInfo, a FaceMap: NX, NY, NZ, PX, PY, PZ */
+    double delta_v[3];
+    aicb_contact already_colliding;   /* the last Within contact of the move, or kind AICB_CONTACT_NONE */
+    uint32_t n_contacts;           /* the ContactSet's true size */
+    uint32_t status;               /* AICB_BODY_* bits */
+    uint8_t quiescent;
+    uint8_t has_push_out;
+    uint8_t uncrush;               /* AICB_UNCRUSH_* */
+    uint8_t uncrush_axes[3];       /* PARTIAL: first, second, third (0 X, 1 Y, 2 Z, AICB_AXIS_NONE: absent) */
+    uint8_t _pad[6];
+} aicb_body_step_info;
+/* step_one_body(body, tick, external_delta_v, Some(space)) for n bodies, in place: what the reference leaves in each
+ * body, its BodyStepDetails in info_or_null[i], and its ContactSet, each contact once in first-insertion order, in
+ * contacts_or_null[i * max_contacts ...] (n_contacts of them, at most max_contacts).  external_delta_v_or_null: NULL is
+ * zero.  gravity: SpacePhysics::gravity.  dt: Tick::delta_t in seconds, finite and in (0, 1] (a paused tick is not
+ * a step).  A body with noclip moves without collision and without gravity, as the reference's.
+ * AICB_ERR_INVALID with nothing written: a NULL bodies with n > 0, a non-finite gravity, a dt out of range, or any
+ * body the reference could not hold (see AICB_BODY_INVALID).  Returns once the bodies and outputs are written. */
+aicb_status aicb_step_bodies(aicb_scene *, aicb_body *bodies, const double (*external_delta_v_or_null)[3], size_t n,
+                             double dt, const double gravity[3], aicb_body_step_info *info_or_null,
+                             aicb_contact *contacts_or_null, uint32_t max_contacts);
+/* The same with bodies, external_delta_v, info and contacts (8-byte aligned) in device memory of the scene's device,
+ * and gravity on the host, issued on `stream` (NULL: the context's) with the device calls' ordering
+ * (aicb_cursor_raycast_device).  It does not synchronise on one context.  The scalar arguments are checked as the host
+ * form checks them; a body the reference could not hold gets AICB_BODY_INVALID in its info and is left unchanged. */
+aicb_status aicb_step_bodies_device(aicb_scene *, aicb_body *d_bodies, const double (*d_external_delta_v_or_null)[3],
+                                    size_t n, double dt, const double gravity[3], aicb_body_step_info *d_info_or_null,
+                                    aicb_contact *d_contacts_or_null, uint32_t max_contacts, void *stream);
+/* The group forms: outputs bit-identical to one context's; the batch is cut into whole warps, one range per replica,
+ * each replica walking its own cells and storing into device 0's buffers.  GPU test: tests/test_gpu_body_step.py. */
+aicb_status aicb_group_step_bodies(aicb_group_scene *, aicb_body *bodies, const double (*external_delta_v_or_null)[3],
+                                   size_t n, double dt, const double gravity[3], aicb_body_step_info *info_or_null,
+                                   aicb_contact *contacts_or_null, uint32_t max_contacts);
+aicb_status aicb_group_step_bodies_device(aicb_group_scene *, aicb_body *d_bodies,
+                                          const double (*d_external_delta_v_or_null)[3], size_t n, double dt,
+                                          const double gravity[3], aicb_body_step_info *d_info_or_null,
+                                          aicb_contact *d_contacts_or_null, uint32_t max_contacts, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Light propagation (secondary path): replaces Mutation::set x n + evaluate_light(epsilon)
