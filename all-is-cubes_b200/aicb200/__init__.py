@@ -93,6 +93,8 @@ def load_library() -> C.CDLL:
     lib.aicb_camera_project_ndc.argtypes = [C.POINTER(abi.CameraData), C.c_double, C.c_double,
                                             C.POINTER(C.c_double)]
     lib.aicb_camera_project_ndc.restype = None
+    lib.aicb_view_transform_matrix.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]
+    lib.aicb_view_transform_matrix.restype = None
     lib.aicb_light_download.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.aicb_render_layers_srgb8.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_void_p, C.c_void_p,
                                              C.c_size_t, C.POINTER(abi.RenderInfo)]
@@ -153,6 +155,11 @@ def load_library() -> C.CDLL:
         getattr(lib, prefix + "step_bodies_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                                                C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                                                C.c_uint32, C.c_void_p]
+    for prefix in ("aicb_", "aicb_group_"):
+        getattr(lib, prefix + "step_exposure").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_double,
+                                                          C.c_void_p]
+        getattr(lib, prefix + "step_exposure_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                                 C.c_double, C.c_void_p, C.c_void_p]
     lib.aicb_project_cursor.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_size_t,
                                         C.c_double, C.c_void_p]
     lib.aicb_group_project_cursor.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
@@ -272,6 +279,9 @@ def _check(status: int):
 # ------------------------------------------------------------------------------------------------
 # GraphicsOptions / Viewport / Camera
 # ------------------------------------------------------------------------------------------------
+EXPOSURE_AUTOMATIC = "automatic"   # GraphicsOptions.exposure = ExposureOption::Automatic (graphics_options.rs:380-407)
+
+
 @dataclasses.dataclass
 class GraphicsOptions:
     """The pixel-affecting subset of GraphicsOptions (graphics_options.rs:28-150).
@@ -280,7 +290,7 @@ class GraphicsOptions:
     fov_y: float = 90.0
     tone_mapping: int = TONE_CLAMP
     maximum_intensity: float = math.inf
-    exposure: float = 1.0  # ExposureOption::Fixed(1)
+    exposure: float = 1.0  # ExposureOption::Fixed(1); or EXPOSURE_AUTOMATIC (see Camera.set_measured_exposure)
     view_distance: float = 200.0
     lighting_display: int = LIGHT_LINEAR
     transparency: int = TRANSPARENCY_VOLUMETRIC
@@ -336,6 +346,8 @@ class Camera:
         self.viewport = viewport
         self._rotation = (0.0, 0.0, 0.0, 1.0)
         self._translation = (0.0, 0.0, 0.0)
+        # Camera::exposure_value: ExposureOption::initial(), 1 under Automatic
+        self.exposure_value = 1.0 if self.options.exposure == EXPOSURE_AUTOMATIC else self.options.exposure
         self.data = abi.CameraData()
         self._compute()
 
@@ -345,7 +357,7 @@ class Camera:
         _check_cam(_cam("camera_from_view")(q, t, self.options.fov_y, self.options.view_distance,
                                          float(self.viewport.nominal_size[0]), float(self.viewport.nominal_size[1]),
                                          self.viewport.framebuffer_size[0], self.viewport.framebuffer_size[1],
-                                         self.options.exposure, C.byref(self.data)))
+                                         self.exposure_value, C.byref(self.data)))
 
     def set_view_transform(self, rotation_ijkr: Sequence[float], translation: Sequence[float]):
         self._rotation = tuple(float(v) for v in rotation_ijkr)
@@ -359,7 +371,17 @@ class Camera:
         _check_cam(_cam("camera_look_at")(e, t, self.options.fov_y, self.options.view_distance,
                                        float(self.viewport.nominal_size[0]), float(self.viewport.nominal_size[1]),
                                        self.viewport.framebuffer_size[0], self.viewport.framebuffer_size[1],
-                                       self.options.exposure, C.byref(self.data)))
+                                       self.exposure_value, C.byref(self.data)))
+
+    def set_measured_exposure(self, value: float):
+        """Camera::set_measured_exposure (camera_struct.rs:169-181): with EXPOSURE_AUTOMATIC the camera's exposure
+        becomes `value` (1 under LIGHT_NONE), if it is a non-negative, non-NaN f32 (PositiveSign::try_from, a zero
+        of either sign being +0); a Fixed exposure ignores it.  Typically a step_exposure result."""
+        v = float(np.float32(value))
+        if math.isnan(v) or v < 0.0 or self.options.exposure != EXPOSURE_AUTOMATIC:
+            return
+        self.exposure_value = 1.0 if self.options.lighting_display == LIGHT_NONE else abs(v)
+        self.data.exposure = self.exposure_value
 
     def project_ndc_into_world(self, x: float, y: float) -> np.ndarray:
         """camera_struct.rs:238-257 -> [ox,oy,oz,dx,dy,dz]"""
@@ -655,6 +677,24 @@ class DeviceBlock:
             bd.light_face_colors[f][:] = bl.face_colors[f]
         bd.light_color[:] = bl.color
         bd.light_emission[:] = bl.emission
+
+
+def exposure_states(n):
+    """n default exposure::State values (exposure.rs:50-58): every sample 1.0, index 0, log 0; an
+    abi.EXPOSURE_STATE_DTYPE array."""
+    st = np.zeros(n, dtype=abi.EXPOSURE_STATE_DTYPE)
+    st["luminance_samples"] = 1.0
+    return st
+
+
+def view_transform_matrix(rotation_ijkr, translation) -> np.ndarray:
+    """ViewTransform::to_transform of an eye's view transform (aicb_view_transform_matrix): the eye-to-world matrix
+    step_exposure takes, m11..m44 as 16 float64 in the row-vector convention of Camera."""
+    q = (C.c_double * 4)(*[float(v) for v in rotation_ijkr])
+    t = (C.c_double * 3)(*[float(v) for v in translation])
+    out = (C.c_double * 16)()
+    load_library().aicb_view_transform_matrix(q, t, out)
+    return np.array(out[:], dtype=np.float64)
 
 
 def bodies(n, position=(0.0, 0.0, 0.0), collision_box=(-0.5, -0.5, -0.5, 0.5, 0.5, 0.5), velocity=(0.0, 0.0, 0.0),
@@ -1168,6 +1208,30 @@ class _Scene:
                                        float(dt), g.ctypes.data, info.ctypes.data,
                                        contacts.ctypes.data if max_contacts else None, max_contacts))
         return b, info, contacts
+
+    def step_exposure(self, states, eye_to_world, dt, device: bool = False):
+        """exposure::State::step (character/exposure.rs:67-136) against this scene for a batch of eyes: (states,
+        exposures).  states: an abi.EXPOSURE_STATE_DTYPE array (see aicb200.exposure_states), stepped by one tick;
+        exposures: State::exposure() afterwards, float32 [n].  eye_to_world: [n, 16] float64 (view_transform_matrix per
+        eye); dt: Tick::delta_t in seconds, finite and >= 0.  device=True: states is a uint8 CUDA tensor [n, 408] on the
+        scene's device (device 0 of a group), stepped in place on its current torch stream, eye_to_world a float64
+        tensor [n, 16], and the exposures a float32 tensor."""
+        if device:
+            torch = _torch()
+            dev = self._device()
+            n = states.shape[0]
+            st = self._tensor(states, torch.uint8, (n, abi.EXPOSURE_STATE_DTYPE.itemsize), "states")
+            m = self._tensor(eye_to_world, torch.float64, (n, 16), "eye_to_world")
+            out = torch.empty(n, dtype=torch.float32, device=dev)
+            _check(self._fn("step_exposure_device")(self.handle, st.data_ptr(), m.data_ptr(), n, float(dt),
+                                                     out.data_ptr(), _stream(dev)))
+            return st, out
+        st = np.ascontiguousarray(states, dtype=abi.EXPOSURE_STATE_DTYPE).copy()
+        n = st.shape[0]
+        m = np.ascontiguousarray(eye_to_world, dtype=np.float64).reshape(n, 16)
+        out = np.zeros(n, dtype=np.float32)
+        _check(self._fn("step_exposure")(self.handle, st.ctypes.data, m.ctypes.data, n, float(dt), out.ctypes.data))
+        return st, out
 
     def _light_download_device(self):
         torch = _torch()

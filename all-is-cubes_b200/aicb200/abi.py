@@ -3,7 +3,7 @@ import ctypes as C
 
 import numpy as np
 
-ABI_VERSION = 25
+ABI_VERSION = 26
 
 BLOCKS_DERIVE_LIGHT = 1
 
@@ -212,6 +212,11 @@ BODY_STEP_INFO_DTYPE = np.dtype([("move_segments", MOVE_SEGMENT_DTYPE, (3,)), ("
                                  ("uncrush_axes", "u1", (3,)), ("_pad", "u1", (6,))])
 assert BODY_STEP_INFO_DTYPE.itemsize == 312
 
+# aicb_exposure_state as a numpy structured dtype (what step_exposure takes and returns)
+EXPOSURE_STATE_DTYPE = np.dtype([("luminance_samples", "<f4", (100,)), ("luminance_sample_index", "<u4"),
+                                 ("exposure_log", "<f4")])
+assert EXPOSURE_STATE_DTYPE.itemsize == 408
+
 
 EXPORTED_SYMBOLS = [
     "aicb_abi_version",
@@ -272,6 +277,7 @@ EXPORTED_SYMBOLS = [
     "aicb_camera_from_view",
     "aicb_eye_for_look_at",
     "aicb_camera_project_ndc",
+    "aicb_view_transform_matrix",
     "aicb_cursor_raycast",
     "aicb_cursor_raycast_device",
     "aicb_project_cursor",
@@ -282,6 +288,10 @@ EXPORTED_SYMBOLS = [
     "aicb_step_bodies_device",
     "aicb_group_step_bodies",
     "aicb_group_step_bodies_device",
+    "aicb_step_exposure",
+    "aicb_step_exposure_device",
+    "aicb_group_step_exposure",
+    "aicb_group_step_exposure_device",
     "aicb_light_chart",
     "aicb_light_chart_chains",
     "aicb_light_fast_evaluate",

@@ -153,12 +153,14 @@ aicb_voxel single_voxel_of(const aicb_block_desc &b) {
 
 // The record of a definition of kind `kind` (an air block's is KIND_INVISIBLE) whose voxel data starts at brick word
 // `brick_off` and palette entry `pal_off`.  Of its collision bits only an air block's are here: the others come from
-// the voxels, which flatten_block reads on the host and k_block_records on the device.
+// the voxels, which flatten_block reads on the host and k_block_records on the device.  So is a recursive block's
+// BLOCK_VISIBLE; a single voxel's is its kind's.
 static BlockRec block_rec(const aicb_block_desc &b, uint8_t kind, uint32_t brick_off, uint32_t pal_off) {
     BlockRec r;
     std::memset(&r, 0, sizeof r);
     r.flags = (b.is_air || (b.flags & AICB_BLOCK_NOT_SELECTABLE)) ? AICB_BLOCK_NOT_SELECTABLE : 0u;
     if (b.is_air) r.flags |= BLOCK_COLLISION_NONE;   // AIR_EVALUATED
+    if (!b.is_air && kind == KIND_SINGLE) r.flags |= BLOCK_VISIBLE;
     if (b.is_air) {
         r.kind_res = KIND_INVISIBLE | (1u << 8);
     } else if (kind != KIND_RECURSIVE) {
@@ -200,10 +202,14 @@ static aicb_status flatten_block(const aicb_block_desc &b, BlockRec &r, uint8_t 
         kind = KIND_RECURSIVE;
         if (bricks.size() + b.n_indices > 0xffffffffull) return fail(AICB_ERR_INVALID, BRICKS_PAST_2_32);
         r = block_rec(b, kind, (uint32_t)bricks.size(), (uint32_t)(palette.size() / 2));
+        bool visible = false;
         for (size_t k = 0; k < b.n_indices; k++) {
             const uint32_t v = b.indices[k];
-            bricks.push_back(v << 16 | (voxel_invisible(b.palette[v]) ? 0x8000u : 0u));
+            const bool inv = voxel_invisible(b.palette[v]);
+            visible |= !inv;
+            bricks.push_back(v << 16 | (inv ? 0x8000u : 0u));
         }
+        if (visible) r.flags |= BLOCK_VISIBLE;
         for (size_t k = 0; k < b.n_palette; k++) push_voxel(b.palette[k]);
         const bool less = less_than_full(r);
         uint32_t pal_mask = 0, used_mask = 0;

@@ -68,15 +68,15 @@ __global__ void __launch_bounds__(THREADS) k_block_verdict(const DeviceBlockJob 
         kinds[blockIdx.x] = (uint8_t)(voxel_invisible(single_voxel(J)) ? KIND_INVISIBLE : KIND_SINGLE);
 }
 
-// A warp's OR of `mask` into a job's collision word.
-__device__ __forceinline__ void or_collision(DeviceBlockJob &J, uint32_t mask) {
+// A warp's OR of `mask` into a job's mask word.
+__device__ __forceinline__ void or_masks(DeviceBlockJob &J, uint32_t mask) {
     mask = __reduce_or_sync(0xffffffffu, mask);
-    if ((threadIdx.x & 31) == 0 && mask) atomicOr(&J.collision, mask);
+    if ((threadIdx.x & 31) == 0 && mask) atomicOr(&J.masks, mask);
 }
 
 // Brick words of the recursive jobs at pool positions [brick_off, brick_off + n_indices), in groups of 16 bytes of
 // the pool: a whole group is one store, a group cut by the range's ends is stored word by word.  The collision masks of
-// the entries the voxels use go into the job's collision word (bits 2-3).
+// the entries the voxels use go into the job's mask word (bits 2-3), and bit 4 if one of them is visible.
 template <bool WIDE>
 __global__ void __launch_bounds__(THREADS) k_block_bricks(DeviceBlockJob *jobs, void *pool) {
     using Word = typename std::conditional<WIDE, uint32_t, uint16_t>::type;
@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(THREADS) k_block_bricks(DeviceBlockJob *jobs, 
             if (p < lo || p >= hi) continue;
             const uint32_t k = __ldg(J.indices + (p - lo));
             const uint32_t inv = invisible_at(J.palette, k) ? 0x8000u : 0u;
-            used |= collision_mask(__ldg(&J.palette[k].flags));
+            used |= collision_mask(__ldg(&J.palette[k].flags)) | (inv ? 0u : 4u);
             u.w[j] = (Word)(WIDE ? k << 16 | inv : k | inv);
         }
         if (g * G >= lo && g * G + G <= hi) reinterpret_cast<uint4 *>(out)[g] = u.v;
@@ -105,11 +105,11 @@ __global__ void __launch_bounds__(THREADS) k_block_bricks(DeviceBlockJob *jobs, 
             for (uint32_t j = 0; j < G; j++)
                 if (g * G + j >= lo && g * G + j < hi) out[g * G + j] = u.w[j];
     }
-    or_collision(J, used << 2);
+    or_masks(J, used << 2);
 }
 
 // Palette entries: a recursive job's palette, a single voxel's one entry; air has none.  A recursive job's palette's
-// collision mask goes into its collision word (bits 0-1).
+// collision mask goes into its mask word (bits 0-1).
 __global__ void __launch_bounds__(THREADS) k_block_palette(DeviceBlockJob *jobs, float4 *palette, float2 *pal_tab) {
     DeviceBlockJob &J = jobs[blockIdx.x];
     uint32_t mask = 0;
@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(THREADS) k_block_palette(DeviceBlockJob *jobs,
         pal_tab[at] = surface_entry(v.rgba[3]);
         mask |= collision_mask(v.flags);
     }
-    if (J.kind == KIND_RECURSIVE) or_collision(J, mask);
+    if (J.kind == KIND_RECURSIVE) or_masks(J, mask);
 }
 
 // compute_derived of a single voxel (derived.rs:84-104), as derive.cu's single_light.
@@ -138,7 +138,8 @@ __device__ aicb_block_light single_light(const aicb_voxel &v) {
 }
 
 // One thread per job that writes its id's records (a repeated id: its last definition of the call).
-// A recursive job's collision bits come from the masks k_block_palette and k_block_bricks left in its collision word.
+// A recursive job's collision and visible bits come from the masks k_block_palette and k_block_bricks left in its mask
+// word.
 __global__ void __launch_bounds__(THREADS) k_block_records(const DeviceBlockJob *jobs, uint32_t n, BlockRec *blocks,
                                                            float4 *blk_tab, LightBlockDev *light,
                                                            const aicb_block_light *derived) {
@@ -146,10 +147,11 @@ __global__ void __launch_bounds__(THREADS) k_block_records(const DeviceBlockJob 
     if (i >= n) return;
     const DeviceBlockJob &J = jobs[i];
     if (J.id == NO_ID) return;
-    BlockRec rec = J.rec;   // an air block's collision bits are in it already (block_rec)
+    BlockRec rec = J.rec;   // an air block's collision bits and a single voxel's visible bit are in it already (block_rec)
+    if (J.kind == KIND_RECURSIVE && (J.masks & 16u)) rec.flags |= BLOCK_VISIBLE;
     if (!(rec.flags & BLOCK_COLLISION_NONE)) {
         if (J.kind == KIND_RECURSIVE)
-            rec.flags |= block_collision(J.collision & 3u, (J.collision >> 2) & 3u, less_than_full(rec));
+            rec.flags |= block_collision(J.masks & 3u, (J.masks >> 2) & 3u, less_than_full(rec));
         else if (single_voxel(J).flags & AICB_VOXEL_NO_COLLISION)
             rec.flags |= BLOCK_COLLISION_NONE;
     }

@@ -332,6 +332,22 @@ AICB_HD_INLINE float powf_exact(float x, float y) {
     return powf_libm_call(x, y);
 }
 
+// ln x correctly rounded to f32 (f32::ln, glibc's logf), for every f32 x.  Short path: x a normal f32, where log_core's
+// value is within 2^-50 relative and Ziv's test at EXACT_MATH_BOUND decides; the rest of it, and the subnormals, take
+// log_dd (2^-102) rounded by round_cr.  ln 1 is +0 exactly (log_core's s is 0 there).  The special cases are glibc's:
+// ln +-0 = -inf, ln +inf = +inf, NaN for a negative x, and a NaN passes through.
+static AICB_HD_NOINLINE float log_dd_f32(float x) { return exact_math::round_cr(exact_math::log_dd(x)); }
+AICB_HD_INLINE float logf_exact(float x) {
+    if ((x >= 0x1p-126f) & (x <= 3.4028235e38f)) {
+        float out;
+        if (exact_math::round_certain(exact_math::log_core(x), out)) return out;
+        return log_dd_f32(x);
+    }
+    if (x > 0.0f) return x == INFINITY ? x : log_dd_f32(x);
+    if (x == 0.0f) return -INFINITY;
+    return x != x ? x : NAN;
+}
+
 // e^x correctly rounded.  Short path: x in [-1.6, 0] (distance_fog's exponent), where it is exhaustively
 // checked.
 AICB_HD_INLINE float expf_exact(float x) {

@@ -218,6 +218,7 @@ struct aicb_ctx {
     DeviceBuffer d_inputs;       // the device-input calls' scratch: verdict, sorted cube lists, staged entries
     DeviceBuffer d_cursor;       // the host cursor calls' queries and results (cursor.cu), apart from a frame's buffers
     DeviceBuffer d_bodies;       // the host body steps' bodies and results (body.cu)
+    DeviceBuffer d_exposure;     // the host exposure steps' states, matrices and exposures (exposure.cu)
     std::mutex mu;
 };
 
@@ -550,8 +551,9 @@ struct DeviceBlockJob {
     uint32_t id;                 // the id whose records it writes; NO_ID: a later definition of the call writes them
     int32_t derived;             // its light record: LIGHT_GIVEN (`light`), LIGHT_SINGLE (its voxel's) or derive's record
     uint32_t light_visible;      // ORed into Derived::visible
-    uint32_t collision;          // collision masks (block_words.cuh) of a recursive job's palette (bits 0-1) and of the
-                                 // entries its voxels use (bits 2-3), ORed in by k_block_palette and k_block_bricks
+    uint32_t masks;              // collision masks (block_words.cuh) of a recursive job's palette (bits 0-1) and of the
+                                 // entries its voxels use (bits 2-3), and bit 4 if one of those entries is visible,
+                                 // ORed in by k_block_palette and k_block_bricks
     aicb::BlockRec rec;
     LightBlockDev light;
 };

@@ -73,7 +73,7 @@ struct BlockRec {
     uint32_t brick_off;    // first u16 of this block's brick in the pool
     uint32_t pal_off;      // first palette entry (single: the voxel)
     uint32_t flags;        // AICB_BLOCK_NOT_SELECTABLE (set for an is_air block), read by the cursor; BLOCK_COLLISION_*,
-                           // read by the body step
+                           // read by the body step; BLOCK_VISIBLE, read by the exposure step
     uint32_t _pad;
 };
 static_assert(sizeof(BlockRec) == 32, "BlockRec must be 32 bytes");
@@ -81,6 +81,10 @@ static_assert(sizeof(BlockRec) == 32, "BlockRec must be 32 bytes");
 // (block_words.cuh: block_collision).  Neither bit: Some(Hard).
 constexpr uint32_t BLOCK_COLLISION_NONE = 2u;    // Some(BlockCollision::None); every is_air block
 constexpr uint32_t BLOCK_COLLISION_MIXED = 4u;   // None: the voxels' AICB_VOXEL_NO_COLLISION bits decide
+// BlockRec::flags: Derived::visible (derived.rs:214, 393-399), derived when the block is placed: some voxel the block
+// uses inside its voxel bounds is visible (a KIND_SINGLE block; a recursive block by its brick words).  Never set for an
+// is_air block.  Unlike LightBlockDev's LB_VISIBLE it carries no animation hint.
+constexpr uint32_t BLOCK_VISIBLE = 8u;
 
 // A recursive block's voxel bounds are smaller than the block (derived.rs:112: full_block_bounds != data_bounds).
 __host__ __device__ inline bool less_than_full(const BlockRec &r) {

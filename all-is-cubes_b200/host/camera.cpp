@@ -209,6 +209,13 @@ aicb_status aicb_camera_look_at(const double eye[3], const double target[3], dou
                                  fb_height, exposure, out);
 }
 
+// ViewTransform::to_transform (RigidTransform3D::to_transform): rotation.to_transform().then(translation.to_transform())
+void aicb_view_transform_matrix(const double q[4], const double translation_[3], double out[16]) {
+    const Mat4 t = then(q_to_transform(Quat{q[0], q[1], q[2], q[3]}), translation(translation_));
+    for (int i = 0; i < 4; i++)
+        for (int j = 0; j < 4; j++) out[i * 4 + j] = t.m[i][j];
+}
+
 // eye_for_look_at (all-is-cubes/src/camera.rs:34-40)
 void aicb_eye_for_look_at(const aicb_aab *bounds, const double direction[3], double out_eye[3]) {
     double radius = 0.0;

@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 24 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 26 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -70,6 +70,22 @@ pub struct aicb_cursor {
     pub face_selected: u8,
     pub layer: u8,
     pub _pad: [u8; 5],
+}
+
+/// `character::exposure::State` (character/exposure.rs:37-58), 408 bytes; the default state is every sample 1.0,
+/// index 0 and log 0
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct aicb_exposure_state {
+    pub luminance_samples: [f32; 100],
+    pub luminance_sample_index: u32,
+    pub exposure_log: f32,
+}
+
+impl Default for aicb_exposure_state {
+    fn default() -> Self {
+        Self { luminance_samples: [1.0; 100], luminance_sample_index: 0, exposure_log: 0.0 }
+    }
 }
 
 /// `Body` (physics/body.rs:38-90) without its look direction; boxes are `[lower xyz, upper xyz]`
@@ -602,6 +618,7 @@ unsafe extern "C" {
                                  fb_height: u32, exposure: f32, out: *mut aicb_camera) -> aicb_status;
     pub fn aicb_eye_for_look_at(bounds: *const aicb_aab, direction: *const [f64; 3], out_eye: *mut [f64; 3]);
     pub fn aicb_camera_project_ndc(cam: *const aicb_camera, ndc_x: f64, ndc_y: f64, out_origin_dir: *mut [f64; 6]);
+    pub fn aicb_view_transform_matrix(rotation_ijkr: *const [f64; 4], translation: *const [f64; 3], out: *mut [f64; 16]);
 
     pub fn aicb_cursor_raycast(s: *mut aicb_scene, origin_dir: *const [f64; 6], max_distance_or_null: *const f64,
                                n: usize, out: *mut aicb_cursor) -> aicb_status;
@@ -637,6 +654,18 @@ unsafe extern "C" {
                                          gravity: *const f64, d_info_or_null: *mut aicb_body_step_info,
                                          d_contacts_or_null: *mut aicb_contact, max_contacts: u32,
                                          stream: *mut c_void) -> aicb_status;
+
+    pub fn aicb_step_exposure(s: *mut aicb_scene, states: *mut aicb_exposure_state, eye_to_world: *const [f64; 16],
+                              n: usize, dt: f64, exposure_out_or_null: *mut f32) -> aicb_status;
+    pub fn aicb_step_exposure_device(s: *mut aicb_scene, d_states: *mut aicb_exposure_state,
+                                     d_eye_to_world: *const [f64; 16], n: usize, dt: f64,
+                                     d_exposure_out_or_null: *mut f32, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_step_exposure(gs: *mut aicb_group_scene, states: *mut aicb_exposure_state,
+                                    eye_to_world: *const [f64; 16], n: usize, dt: f64, exposure_out_or_null: *mut f32)
+                                    -> aicb_status;
+    pub fn aicb_group_step_exposure_device(gs: *mut aicb_group_scene, d_states: *mut aicb_exposure_state,
+                                           d_eye_to_world: *const [f64; 16], n: usize, dt: f64,
+                                           d_exposure_out_or_null: *mut f32, stream: *mut c_void) -> aicb_status;
 
     pub fn aicb_light_chart(weights: *mut f32, children: *mut u32) -> u32;
     pub fn aicb_light_chart_chains(preorder: *mut u32, chains: *mut [u32; 6], euler: *mut u16) -> u32;

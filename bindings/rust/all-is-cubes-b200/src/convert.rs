@@ -148,6 +148,13 @@ pub fn apply_stepped_body(body: &mut all_is_cubes::physics::Body, stepped: &sys:
     body.set_velocity(euclid::vec3(vx, vy, vz));
 }
 
+/// An eye's `ViewTransform` (its eye-to-world transform) as `aicb_step_exposure` takes it: `to_transform()` as m11..m44,
+/// row-major (euclid `Transform3D::to_array`), what `aicb_view_transform_matrix` computes from its rotation and
+/// translation.
+pub fn view_transform_of(vt: &all_is_cubes::camera::ViewTransform) -> [f64; 16] {
+    vt.to_transform().to_array()
+}
+
 pub fn camera_of(camera: &Camera) -> sys::aicb_camera {
     let size = camera.viewport().framebuffer_size;
     sys::aicb_camera {

@@ -330,6 +330,18 @@ impl SceneHandle {
         Ok(changed)
     }
 
+    fn step_exposure(self, states: &mut [sys::aicb_exposure_state], eye_to_world: &[[f64; 16]], dt: f64,
+                     exposures: &mut [f32]) -> Result<(), B200Error> {
+        check(unsafe {
+            match self {
+                Self::Single(s) => sys::aicb_step_exposure(s, states.as_mut_ptr(), eye_to_world.as_ptr(), states.len(),
+                                                           dt, exposures.as_mut_ptr()),
+                Self::Group(s) => sys::aicb_group_step_exposure(s, states.as_mut_ptr(), eye_to_world.as_ptr(),
+                                                                states.len(), dt, exposures.as_mut_ptr()),
+            }
+        })
+    }
+
     fn destroy(self) {
         match self {
             Self::Single(s) => unsafe { sys::aicb_scene_destroy(s) },
@@ -602,6 +614,17 @@ impl B200Renderer {
         assert_eq!(cubes.len(), ids.len(), "one block index per cube");
         let cubes: Vec<[i32; 3]> = cubes.iter().map(|c| [c.x, c.y, c.z]).collect();
         self.world_scene()?.light_edit_cubes(&cubes, ids)
+    }
+
+    /// `character::exposure::State::step` (character/exposure.rs:67-136) for a world that lives on the GPU, where no
+    /// reference `Character` steps its own exposure: each of `states` by one tick of `dt` seconds against the world
+    /// scene, from the eye whose view transform is `eye_to_world[i]` (`convert::view_transform_of`);
+    /// `exposures[i]` receives `State::exposure()`, which the host hands to `Camera::set_measured_exposure`
+    /// (`aicb_step_exposure`).  A Space kept in Rust needs none of this: `StandardCameras` applies its character's own.
+    pub fn step_world_exposure(&self, states: &mut [sys::aicb_exposure_state], eye_to_world: &[[f64; 16]], dt: f64,
+                               exposures: &mut [f32]) -> Result<(), B200Error> {
+        assert!(eye_to_world.len() == states.len() && exposures.len() == states.len(), "one matrix and one exposure per state");
+        self.world_scene()?.step_exposure(states, eye_to_world, dt, exposures)
     }
 
     /// Calls `single` with the layers this renderer holds as `aicb_layer`s, or on a group `group` with them as

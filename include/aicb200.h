@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 25
+#define AICB_ABI_VERSION 26
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -852,6 +852,10 @@ aicb_status aicb_camera_from_view(const double rotation_ijkr[4], const double tr
 void aicb_eye_for_look_at(const aicb_aab *bounds, const double direction[3], double out_eye[3]);
 /* Camera::project_ndc_into_world for one NDC point (host, for tests): out = origin xyz, dir xyz. */
 void aicb_camera_project_ndc(const aicb_camera *, double ndc_x, double ndc_y, double out_origin_dir[6]);
+/* ViewTransform::to_transform (RigidTransform3D::to_transform: rotation.to_transform().then(translation.to_transform()))
+ * of an eye's view transform {rotation (i, j, k, r), translation}: m11..m44 in the row-vector convention of
+ * aicb_camera, the eye-to-world matrix aicb_step_exposure takes.  Host only. */
+void aicb_view_transform_matrix(const double rotation_ijkr[4], const double translation[3], double out[16]);
 
 /* ---------------------------------------------------------------------------------------------
  * The cursor: cursor_raycast (all-is-cubes/src/character/cursor.rs:26-107) and StandardCameras::project_cursor
@@ -1009,6 +1013,44 @@ aicb_status aicb_group_step_bodies_device(aicb_group_scene *, aicb_body *d_bodie
                                           const double (*d_external_delta_v_or_null)[3], size_t n, double dt,
                                           const double gravity[3], aicb_body_step_info *d_info_or_null,
                                           aicb_contact *d_contacts_or_null, uint32_t max_contacts, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Automatic exposure: character::exposure::State::step (all-is-cubes/src/character/exposure.rs:67-136) over a scene's
+ * cells and light on the device, for a batch of eyes.  Per tick each eye casts 10 rays from its eye-to-world transform's
+ * origin through the Space (Raycaster::new(origin, direction).within(bounds, false), at most 2 * maximum_distance
+ * steps, none under LightPhysics::None); a ray's sample is the luminance of get_light(cube_behind) at the first visible
+ * block (Derived::visible, derived when the block is placed) whose light there is Visible, else of the sky in the ray's
+ * direction.  The moving average of 100 samples sets the target exposure, and exposure_log moves towards its ln.  The
+ * f32 ln and exp are correctly rounded (glibc's logf and expf where those are).  Nothing of the scene changes (as the
+ * cursor calls: no host mirror rebuild, no light state, no frame in flight).
+ * ------------------------------------------------------------------------------------------- */
+/* exposure::State (exposure.rs:37-58), 408 bytes.  The default state is every sample 1.0f, index 0 and log 0. */
+typedef struct aicb_exposure_state {
+    float luminance_samples[100];
+    uint32_t luminance_sample_index;   /* the last sample written; advanced as a 64-bit usize, (index + 1) % 100 */
+    float exposure_log;                /* ln of the exposure */
+} aicb_exposure_state;
+/* State::step(space, view_transform, dt) for n eyes, in place; exposure_out_or_null[i] = State::exposure() afterwards
+ * (exp(exposure_log), correctly rounded).  eye_to_world[i]: aicb_view_transform_matrix of the eye's view transform,
+ * or any matrix: an origin whose w is not > 0 leaves the state unchanged, as transform_point3d's None does.
+ * dt: Tick::delta_t in seconds, finite and >= 0; dt == 0 leaves every state unchanged (the reference returns early).
+ * AICB_ERR_INVALID with nothing written: NULL states or eye_to_world with n > 0, or a dt out of range.  Returns once the
+ * states and exposures are written. */
+aicb_status aicb_step_exposure(aicb_scene *, aicb_exposure_state *states, const double (*eye_to_world)[16], size_t n,
+                               double dt, float *exposure_out_or_null);
+/* The same with states (4-byte aligned), matrices (8-byte aligned) and exposures (4-byte aligned) in device memory of
+ * the scene's device, issued on `stream` (NULL: the context's) with the device calls' ordering
+ * (aicb_cursor_raycast_device).  It does not synchronise on one context.  Pointers and dt are checked as the host
+ * form checks them (AICB_ERR_INVALID). */
+aicb_status aicb_step_exposure_device(aicb_scene *, aicb_exposure_state *d_states, const double (*d_eye_to_world)[16],
+                                      size_t n, double dt, float *d_exposure_out_or_null, void *stream);
+/* The group forms: outputs bit-identical to one context's.  The eyes are cut into ranges, one per replica; each replica
+ * walks its own cells and stores into device 0's buffers.  GPU test: tests/test_gpu_exposure.py. */
+aicb_status aicb_group_step_exposure(aicb_group_scene *, aicb_exposure_state *states, const double (*eye_to_world)[16],
+                                     size_t n, double dt, float *exposure_out_or_null);
+aicb_status aicb_group_step_exposure_device(aicb_group_scene *, aicb_exposure_state *d_states,
+                                            const double (*d_eye_to_world)[16], size_t n, double dt,
+                                            float *d_exposure_out_or_null, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Light propagation (secondary path): replaces Mutation::set x n + evaluate_light(epsilon)
