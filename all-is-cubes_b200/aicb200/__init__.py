@@ -127,6 +127,19 @@ def load_library() -> C.CDLL:
                                                C.POINTER(abi.RenderInfo)]
     lib.aicb_group_render_rgba16f.argtypes = [C.c_void_p, C.POINTER(abi.CameraData), C.POINTER(abi.Options), C.c_void_p,
                                               C.c_size_t, C.POINTER(abi.RenderInfo)]
+    for prefix in ("aicb_", "aicb_group_"):
+        for kind in ("srgb8", "rgba16f", "text"):
+            getattr(lib, prefix + "render_views_" + kind).argtypes = [
+                C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.Options), C.c_void_p, C.c_size_t,
+                C.POINTER(abi.RenderInfo)]
+        getattr(lib, prefix + "render_views_colorbuf").argtypes = [
+            C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(abi.Options), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+            C.c_size_t, C.POINTER(abi.RenderInfo)]
+    lib.aicb_render_views_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32,
+                                             C.POINTER(abi.Options), C.POINTER(abi.DeviceOutputs), C.c_void_p]
+    lib.aicb_group_render_views_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32,
+                                                   C.POINTER(abi.Options), C.POINTER(abi.DeviceOutputs), C.c_void_p,
+                                                   C.POINTER(abi.RenderInfo)]
     lib.aicb_light_chart.argtypes = [C.c_void_p, C.c_void_p]
     lib.aicb_light_chart.restype = C.c_uint32
     outs = C.POINTER(abi.DeviceOutputs)
@@ -1516,7 +1529,123 @@ class _Scene:
         return out
 
 
-class SpaceRaytracer(_Scene):
+
+# ------------------------------------------------------------------------------------------------
+# batches of views of one scene (aicb_render_views_* / aicb_group_render_views_*)
+# ------------------------------------------------------------------------------------------------
+def camera_table(cameras) -> np.ndarray:
+    """The aicb_camera records of a list of Camera, as an abi.CAMERA_DTYPE array."""
+    table = np.zeros(len(cameras), dtype=abi.CAMERA_DTYPE)
+    for v, cam in enumerate(cameras):
+        table[v:v + 1].view(np.uint8)[:] = np.frombuffer(bytes(cam.data), dtype=np.uint8)
+    return table
+
+
+def _views_spec(kind, v, h, w, want_depth=False, want_hit=False, want_steps=False) -> dict:
+    torch = _torch()
+    if kind == "srgb8":
+        return {"srgb8": ((v, h, w, 4), torch.uint8)}
+    if kind == "rgba16f":
+        return {"rgba16f": ((v, h, w, 4), torch.float16)}
+    if kind == "text":
+        return {"text": ((v, h, w), torch.int32)}
+    spec = {"colorbuf": ((v, h * w, 4), torch.float32)}
+    if want_depth:
+        spec["depth"] = ((v, h * w), torch.float64)
+    if want_hit:
+        spec["hit"] = ((v, h * w, 8), torch.int32)
+    if want_steps:
+        spec["steps"] = ((v, h * w), torch.uint32)
+    return spec
+
+
+def _draw_views(scene, group, cameras, options, kind, device, out, size, want_depth=False, want_hit=False,
+                want_steps=False):
+    """One batch of views on a SpaceRaytracer (group None) or on a DeviceGroup's scene.  kind: srgb8, rgba16f,
+    colorbuf or text.  Host: numpy arrays; device: the tensors of _views_spec (a DeviceRendering on one context)."""
+    lib = load_library()
+    prefix = "aicb_group_" if group is not None else "aicb_"
+    opt = options.to_abi(True)
+    if device:
+        torch = _torch()
+        dev = group._device() if group is not None else _ctx_device(scene.ctx)
+        if _is_cuda_tensor(cameras):
+            if size is None:
+                raise ValueError("a camera table tensor needs size=(fb_width, fb_height)")
+            w, h = size
+            v = cameras.shape[0]
+            if (cameras.dtype != torch.uint8 or cameras.device != dev or not cameras.is_contiguous()
+                    or tuple(cameras.shape) != (v, abi.CAMERA_DTYPE.itemsize)):
+                raise ValueError(f"cameras must be a contiguous uint8 tensor [n, {abi.CAMERA_DTYPE.itemsize}] on {dev}")
+            table = cameras
+        else:
+            v = len(cameras)
+            w, h = (cameras[0].data.fb_width, cameras[0].data.fb_height) if v else (0, 0) if size is None else size
+            table = torch.from_numpy(camera_table(cameras).view(np.uint8).reshape(v, abi.CAMERA_DTYPE.itemsize)).to(dev)
+        t = _device_outputs(out, dev, _views_spec(kind, v, h, w, want_depth, want_hit, want_steps))
+        o = _outs_abi(v * w * h, t)
+        stream = _stream(dev)
+        build = (lambda t, info: _colorbuf_result(t, info)) if kind == "colorbuf" else (lambda t, info: t[kind])
+        if group is None:
+            return DeviceRendering(scene, lambda held=table: lib.aicb_render_views_device(
+                scene.handle, held.data_ptr(), v, w, h, C.byref(opt), C.byref(o), stream), lambda info: build(t, info))
+        info = abi.RenderInfo()
+        _check(lib.aicb_group_render_views_device(scene.handle if scene else None, table.data_ptr(), v, w, h, C.byref(opt), C.byref(o),
+                                                  stream, C.byref(info)))
+        return build(t, RenderInfo.from_abi(info))
+    table = camera_table(cameras)
+    v = len(cameras)
+    w, h = (int(table["fb_width"][0]), int(table["fb_height"][0])) if v else (0, 0)
+    n = v * w * h
+    info = abi.RenderInfo()
+    fn = getattr(lib, prefix + "render_views_" + kind)
+    handle = scene.handle if scene is not None else None
+    if kind == "colorbuf":
+        cb = np.empty((v, h * w, 4), dtype=np.float32)
+        depth = np.empty((v, h * w), dtype=np.float64) if want_depth else None
+        hit = np.empty((v, h * w, 8), dtype=np.int32) if want_hit else None
+        steps = np.empty((v, h * w), dtype=np.uint32) if want_steps else None
+        _check(fn(handle, table.ctypes.data, v, C.byref(opt), cb.ctypes.data, depth.ctypes.data if want_depth else None,
+                  hit.ctypes.data if want_hit else None, steps.ctypes.data if want_steps else None, n, C.byref(info)))
+        return {"colorbuf": cb, "depth": depth, "hit": hit, "steps": steps, "info": RenderInfo.from_abi(info)}
+    shape, dtype = {"srgb8": ((v, h, w, 4), np.uint8), "rgba16f": ((v, h, w, 4), np.float16),
+                    "text": ((v, h, w), np.int32)}[kind]
+    arr = np.empty(shape, dtype=dtype)
+    _check(fn(handle, table.ctypes.data, v, C.byref(opt), arr.ctypes.data, n, C.byref(info)))
+    return arr
+
+
+class _Views:
+    """draw_views and its siblings: a batch of cameras of one scene, sharing one GraphicsOptions and one framebuffer
+    size, drawn as one frame; view v of the result is the single-camera call's output for cameras[v], bit for bit.
+    cameras: a list of Camera, or with device=True a uint8 CUDA tensor [n, 144] of aicb_camera records
+    (abi.CAMERA_DTYPE, see camera_table) with size=(fb_width, fb_height).  device=True: the outputs are CUDA tensors
+    (out=: the caller's own), as for the other device=True calls."""
+
+    def _views(self, cameras, options, kind, device, out, size, **want):
+        raise NotImplementedError
+
+    def draw_views(self, cameras, options, device=False, out=None, size=None):
+        """draw_rgba of every camera: uint8 [V, H, W, 4]."""
+        return self._views(cameras, options, "srgb8", device, out, size)
+
+    def draw_views_rgba16f(self, cameras, options, device=False, out=None, size=None):
+        """draw_rgba16f of every camera: float16 [V, H, W, 4]."""
+        return self._views(cameras, options, "rgba16f", device, out, size)
+
+    def draw_views_colorbuf(self, cameras, options, want_depth=True, want_hit=True, want_steps=True, device=False,
+                            out=None, size=None):
+        """draw_colorbuf of every camera: a dict of colorbuf [V, H * W, 4], depth, hit and steps, and the batch's
+        info (counters summed over the views)."""
+        return self._views(cameras, options, "colorbuf", device, out, size, want_depth=want_depth, want_hit=want_hit,
+                           want_steps=want_steps)
+
+    def render_views_text(self, cameras, options, device=False, out=None, size=None):
+        """render_text of every camera: int32 [V, H, W]."""
+        return self._views(cameras, options, "text", device, out, size)
+
+
+class SpaceRaytracer(_Scene, _Views):
     """SpaceRaytracer<()> (sr.rs:51): device-resident snapshot of a Space + graphics options."""
 
     def __init__(self, space: Space, graphics_options: GraphicsOptions, ctx: Optional[Context] = None):
@@ -1548,6 +1677,10 @@ class SpaceRaytracer(_Scene):
 
     def _device(self):
         return _ctx_device(self.ctx)
+
+    def _views(self, cameras, options, kind, device, out, size, **want):
+        self.ctx.settle()
+        return _draw_views(self, None, cameras, options, kind, device, out, size, **want)
 
     def light_download(self, device: bool = False):
         """The light volume, shaped like the Space + (4,): numpy, or with device=True a uint8 tensor on the scene's
@@ -2013,7 +2146,7 @@ class GroupScene(_Scene):
         return out
 
 
-class DeviceGroup:
+class DeviceGroup(_Views):
     """Several GPUs driven from this one process through the C ABI (csrc/group.cu): scene replicated, frame cut into
     interleaved row strips, pixels stored straight into device 0's frame over NVLink.
 
@@ -2108,6 +2241,10 @@ class DeviceGroup:
 
     def _handle(self):
         return self.scene.handle if self.scene else None
+
+    def _views(self, cameras, options, kind, device, out, size, **want):
+        """The batch on the group's scene: view v drawn by device v mod N."""
+        return _draw_views(self.scene, self, cameras, options, kind, device, out, size, **want)
 
     def draw_colorbuf(self, camera: "Camera", options: "GraphicsOptions", want_depth=True, want_hit=True,
                       want_steps=True, device=False, out=None) -> dict:

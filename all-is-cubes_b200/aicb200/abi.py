@@ -3,7 +3,7 @@ import ctypes as C
 
 import numpy as np
 
-ABI_VERSION = 26
+ABI_VERSION = 27
 
 BLOCKS_DERIVE_LIGHT = 1
 
@@ -80,6 +80,12 @@ class CameraData(C.Structure):
         ("exposure", C.c_float),
         ("_pad", C.c_uint32),
     ]
+
+
+# aicb_camera as a numpy structured dtype: the camera table of a batch of views (draw_views with device=True)
+CAMERA_DTYPE = np.dtype([("inverse_projection_view", "<f8", (16,)), ("fb_width", "<u4"), ("fb_height", "<u4"),
+                         ("exposure", "<f4"), ("_pad", "<u4")])
+assert CAMERA_DTYPE.itemsize == C.sizeof(CameraData) == 144
 
 
 class Options(C.Structure):
@@ -263,6 +269,11 @@ EXPORTED_SYMBOLS = [
     "aicb_render_device",
     "aicb_trace_rays_device",
     "aicb_render_layers_device",
+    "aicb_render_views_srgb8",
+    "aicb_render_views_rgba16f",
+    "aicb_render_views_colorbuf",
+    "aicb_render_views_text",
+    "aicb_render_views_device",
     "aicb_frame_create",
     "aicb_frame_open",
     "aicb_frame_close",
@@ -346,6 +357,11 @@ EXPORTED_SYMBOLS = [
     "aicb_group_render_device",
     "aicb_group_trace_rays_device",
     "aicb_group_render_layers_device",
+    "aicb_group_render_views_srgb8",
+    "aicb_group_render_views_rgba16f",
+    "aicb_group_render_views_colorbuf",
+    "aicb_group_render_views_text",
+    "aicb_group_render_views_device",
     "aicb_texture_target_create",
     "aicb_texture_target_destroy",
     "aicb_texture_target_resize",

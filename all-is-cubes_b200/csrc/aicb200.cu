@@ -535,14 +535,22 @@ static kernel_fn resolve_for(int lc, int tgt) {
     switch (tgt) {
         case TGT_TEX: return lc == LC_NONE ? resolve_kernel<LC_NONE, TGT_TEX> : resolve_kernel<LC_FLAT, TGT_TEX>;
         case TGT_TERM: return lc == LC_NONE ? resolve_kernel<LC_NONE, TGT_TERM> : resolve_kernel<LC_FLAT, TGT_TERM>;
+        case TGT_VIEWS: return lc == LC_NONE ? resolve_kernel<LC_NONE, TGT_VIEWS> : resolve_kernel<LC_FLAT, TGT_VIEWS>;
         default: return lc == LC_NONE ? resolve_kernel<LC_NONE, TGT_FRAME> : resolve_kernel<LC_FLAT, TGT_FRAME>;
     }
 }
 static kernel_fn encode_for(int tgt) {
-    return tgt == TGT_TEX ? encode_kernel<TGT_TEX> : (tgt == TGT_TERM ? encode_kernel<TGT_TERM> : encode_kernel<TGT_FRAME>);
+    switch (tgt) {
+        case TGT_TEX: return encode_kernel<TGT_TEX>;
+        case TGT_TERM: return encode_kernel<TGT_TERM>;
+        case TGT_VIEWS: return encode_kernel<TGT_VIEWS>;
+        default: return encode_kernel<TGT_FRAME>;
+    }
 }
 
-// Launches the trace kernel on `stream`. Camera rays when cam != NULL, the explicit rays of `out` otherwise.  With
+// Launches the trace kernel on `stream`. Camera rays when cam != NULL, the explicit rays of `out` otherwise; with a
+// TGT_VIEWS target, cam gives only the framebuffer size and the rays of out.n_views views come from the target's
+// camera table (the caller has checked that the batch's tasks fit in 32 bits).  With
 // `continues`, the pass continues the context's frame in flight on the same stream (the world pass of a layered frame
 // behind its UI pass, aicb_render_layers_device): the frame counters, the overflow flag and the start event carry on,
 // so finish reports both passes, and the frame is finished on `sc`.
@@ -582,6 +590,10 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             P.n_tasks = out.target.n_list;
             pixels = out.target.n_list;
         }
+        if (out.kind == TGT_VIEWS) {   // the views' tile-ordered tasks end to end
+            P.n_tasks = P.tiles_x * P.tiles_y * 32 * out.n_views;
+            pixels *= out.n_views;
+        }
     } else {
         P.exposure = 1.0f;
         P.rays = out.rays;
@@ -608,6 +620,7 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
     P.out_full_frame = out.full_frame ? 1 : 0;
     P.target = out.target;
     const int tgt = out.kind;
+    if (tgt == TGT_VIEWS) P.target.view_tiles = P.tiles_x * P.tiles_y;
     P.counters = ctx->d_counters.get<unsigned long long>();
     P.task_counter = ctx->d_tile_counter;
     P.refill_threshold = REFILL_THRESHOLD;
@@ -731,7 +744,8 @@ static aicb_status launch_trace(aicb_scene *sc, const aicb_camera *cam, const ai
             const bool prof = ctx->profile_kernels && first;
             const bool stage = first && ctx->stage_timing;
             if (stage) cudaEventRecord(ctx->ev_k[0].get(), stream);
-            gen_kernel<<<(n + 127) / 128, 128, 0, stream>>>(P, n);
+            if (tgt == TGT_VIEWS) gen_views_kernel<<<(n + 127) / 128, 128, 0, stream>>>(P, n);
+            else gen_kernel<<<(n + 127) / 128, 128, 0, stream>>>(P, n);
             if (stage) cudaEventRecord(ctx->ev_k[1].get(), stream);
             uint64_t want = ((uint64_t)n + WARPS_PER_BLOCK * 32 - 1) / (WARPS_PER_BLOCK * 32);
             uint64_t grid = (uint64_t)ctx->num_sms * blocks_per_sm;  // persistent: a multiple of the SM count
@@ -2379,6 +2393,30 @@ aicb_status scenes_fill_uniform_device(Replicas r, const aicb_block_desc *block,
 // ---------------------------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------------------------
+aicb_status check_views(const aicb_camera *cameras, bool host_cameras, size_t n_views, uint32_t *width,
+                        uint32_t *height, const aicb_options *opt, size_t out_len) {
+    TRY(validate_options(opt));
+    if (n_views && !cameras) return fail(AICB_ERR_INVALID, "cameras is NULL");
+    if (host_cameras) {
+        *width = n_views ? cameras[0].fb_width : 0;
+        *height = n_views ? cameras[0].fb_height : 0;
+        for (size_t v = 1; v < n_views; v++)
+            if (cameras[v].fb_width != *width || cameras[v].fb_height != *height)
+                return fail(AICB_ERR_INVALID, "the views' cameras must share the framebuffer size");
+    }
+    const uint64_t per_view = (uint64_t)*width * *height;
+    if (per_view && n_views > SIZE_MAX / per_view) return fail(AICB_ERR_INVALID, "batch too large");
+    if (out_len != n_views * per_view)
+        return fail(AICB_ERR_INVALID, "output length must be n_views * fb_width * fb_height");
+    if (per_view && n_views) {   // n_views * tiles * 32 * samples < 2^32
+        const uint64_t tasks = ((uint64_t)*width + TILE_W - 1) / TILE_W * (((uint64_t)*height + TILE_H - 1) / TILE_H) *
+                               32 * (opt->antialiasing_always ? 4 : 1);   // (< 2^63: width, height < 2^32)
+        if (tasks > 0xffffffffull || n_views > 0xffffffffull / tasks)
+            return fail(AICB_ERR_INVALID, "batch too large: its tasks reach 2^32");
+    }
+    return AICB_OK;
+}
+
 extern "C" {
 
 uint32_t aicb_abi_version(void) { return AICB_ABI_VERSION; }
@@ -2793,6 +2831,66 @@ aicb_status aicb_render_text(aicb_scene *s, const aicb_camera *cam, const aicb_o
     if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
     const aicb_device_outputs o = one_output(&aicb_device_outputs::text, out, out_len);
     return on_scene(s, [&](Replicas r) { return frame_host(r, cam, opt, nullptr, o, STAGE_GIVEN, info); });
+}
+
+// A batch of views of one scene (internal.h: check_views, views_host): the single-camera calls' outputs, view-major.
+aicb_status aicb_render_views_srgb8(aicb_scene *s, const aicb_camera *cameras, size_t n_views, const aicb_options *opt,
+                                    uint8_t (*out)[4], size_t out_len, aicb_render_info *info) {
+    uint32_t w, h;
+    if (!s) return fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::srgb8, out, out_len);
+    return on_scene(s, [&](Replicas r) { return views_host(r, cameras, n_views, opt, o, STAGE_PINNED, info); });
+}
+
+aicb_status aicb_render_views_rgba16f(aicb_scene *s, const aicb_camera *cameras, size_t n_views, const aicb_options *opt,
+                                      uint16_t (*out)[4], size_t out_len, aicb_render_info *info) {
+    uint32_t w, h;
+    if (!s) return fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::rgba16f, out, out_len);
+    return on_scene(s, [&](Replicas r) { return views_host(r, cameras, n_views, opt, o, STAGE_GIVEN, info); });
+}
+
+aicb_status aicb_render_views_colorbuf(aicb_scene *s, const aicb_camera *cameras, size_t n_views,
+                                       const aicb_options *opt, float (*out_cb)[4], double *depth, aicb_hit *hit,
+                                       uint32_t *steps, size_t out_len, aicb_render_info *info) {
+    uint32_t w, h;
+    if (!s) return fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    const aicb_device_outputs o = colorbuf_outputs(out_cb, depth, hit, steps, out_len);
+    return on_scene(s, [&](Replicas r) { return views_host(r, cameras, n_views, opt, o, STAGE_COLORBUF, info); });
+}
+
+aicb_status aicb_render_views_text(aicb_scene *s, const aicb_camera *cameras, size_t n_views, const aicb_options *opt,
+                                   int32_t *out, size_t out_len, aicb_render_info *info) {
+    uint32_t w, h;
+    if (!s) return fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    if (out_len && !out) return fail(AICB_ERR_INVALID, "out is NULL");
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::text, out, out_len);
+    return on_scene(s, [&](Replicas r) { return views_host(r, cameras, n_views, opt, o, STAGE_GIVEN, info); });
+}
+
+// The batch as one frame on `stream`, reading the caller's camera table where it is; aicb_render_finish finishes it.
+aicb_status aicb_render_views_device(aicb_scene *s, const aicb_camera *d_cameras, size_t n_views, uint32_t fb_width,
+                                     uint32_t fb_height, const aicb_options *opt, const aicb_device_outputs *outs,
+                                     void *stream) {
+    if (!s || !outs) return fail(AICB_ERR_INVALID, "NULL argument");
+    if (outs->full_frame) return fail(AICB_ERR_INVALID, "full_frame is for aicb_render_device");
+    TRY(check_views(d_cameras, false, n_views, &fb_width, &fb_height, opt, outs->len));
+    std::lock_guard<std::mutex> lock(s->ctx->mu);
+    CU(cudaSetDevice(s->ctx->device));
+    Outputs o;
+    TRY(device_target(outs, s->ctx->device, DEV_FRAME, false, false, &o));
+    if (n_views) TRY(check_device_pointer(d_cameras, s->ctx->device, false, 8, "the camera table"));
+    cudaStream_t st = stream ? (cudaStream_t)stream : s->ctx->stream.get();
+    if (outs->len == 0) return issue_empty_frame(s, opt, st);
+    views_part(&o, d_cameras, n_views, 0, 1);
+    const aicb_camera size = views_frame_camera(fb_width, fb_height);
+    return launch_trace(s, &size, opt, nullptr, o, st);
 }
 
 // Arguments shared by the layered entry points: at least one layer (or the paint colour), complete layers, one context

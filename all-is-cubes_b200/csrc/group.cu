@@ -371,6 +371,63 @@ aicb_status rays_host(Replicas r, const double (*origin_dir)[6], const aicb_opti
     return draw_rays(r, origin_dir, false, host.len, opt, target, copies, nullptr, info);
 }
 
+// ---- batches of views of one scene -------------------------------------------------------------------------------
+// View v is drawn by replica v mod n, interleaved as row strips are, since views differ in cost.  Every replica traces
+// its views as one frame (TGT_VIEWS) and stores them at their view-major positions in device 0's outputs (`target`);
+// with `d_cameras` every replica reads device 0's camera table, otherwise each takes its own copy of the caller's
+// (through its pinned h_views, on its stream).  A caller's stream, the delivery of `copies` and the info are
+// draw_frame's.
+static aicb_status draw_views(Replicas r, const aicb_camera *cameras, bool on_device, size_t n_views, uint32_t width,
+                              uint32_t height, const aicb_options *opt, const Outputs &target,
+                              const std::vector<Delivery> &copies, cudaStream_t caller, aicb_render_info *info) {
+    if (info) std::memset(info, 0, sizeof *info);
+    if (n_views == 0 || (uint64_t)width * height == 0) return AICB_OK;
+    const size_t used = std::min(r.n, n_views);
+    std::vector<FramePart> parts;
+    TRY(after_caller(r.ctx, used, caller));
+    for (size_t i = 0; i < used; i++) {
+        const aicb_camera *table = cameras;
+        if (!on_device) {
+            aicb_ctx *ctx = r.ctx[i];
+            const size_t bytes = n_views * sizeof(aicb_camera);
+            CU(cudaSetDevice(ctx->device));
+            TRY(ctx->h_views.ensure(bytes));
+            TRY(ctx->d_views.ensure(bytes));
+            std::memcpy(ctx->h_views.get(), cameras, bytes);
+            CU(cudaMemcpyAsync(ctx->d_views.get(), ctx->h_views.get(), bytes, cudaMemcpyHostToDevice, ctx->stream.get()));
+            table = ctx->d_views.get<const aicb_camera>();
+        }
+        FramePart p{r.scene[i]};
+        p.out = target;
+        views_part(&p.out, table, n_views, i, r.n);
+        parts.push_back(p);
+    }
+    const aicb_camera size = views_frame_camera(width, height);
+    TRY(aicb_trace_pass(parts.data(), parts.size(), &size, opt, info != nullptr, copies));
+    TRY(before_caller(r.ctx, parts.size(), caller));
+    sum_info(parts, info);
+    return AICB_OK;
+}
+
+aicb_status views_host(Replicas r, const aicb_camera *cameras, size_t n_views, const aicb_options *opt,
+                       const aicb_device_outputs &host, Staging how, aicb_render_info *info) {
+    Outputs target;
+    std::vector<Delivery> copies;
+    TRY(stage_outputs(r.ctx[0], host, how, DEV_FRAME, &target, &copies));
+    const uint32_t width = n_views ? cameras[0].fb_width : 0, height = n_views ? cameras[0].fb_height : 0;
+    return draw_views(r, cameras, false, n_views, width, height, opt, target, copies, nullptr, info);
+}
+
+aicb_status views_device(Replicas r, const aicb_camera *d_cameras, size_t n_views, uint32_t width, uint32_t height,
+                         const aicb_options *opt, const aicb_device_outputs *outs, cudaStream_t caller,
+                         aicb_render_info *info) {
+    CU(cudaSetDevice(r.ctx[0]->device));
+    Outputs target;
+    TRY(device_target(outs, r.ctx[0]->device, DEV_FRAME, true, false, &target));
+    if (n_views) TRY(check_device_pointer(d_cameras, r.ctx[0]->device, false, 8, "the camera table"));
+    return draw_views(r, d_cameras, true, n_views, width, height, opt, target, {}, caller, info);
+}
+
 // The layers of a group call as device 0 sees them (its replicas, the cameras and options), and every replica of each.
 static aicb_layer on_device0(const aicb_group_layer *l) {
     aicb_layer r;
@@ -624,6 +681,63 @@ aicb_status aicb_group_render_layers_srgb8(const aicb_group_layer *world, const 
     LayeredCall c;
     TRY(group_call(world, ui, backdrop_rgba, no_world_rgba, views, &c));
     return layers_srgb8(c, out, out_len, info);
+}
+
+// A batch of views on the group, validated as one context's (check_views) before any device is touched.
+aicb_status aicb_group_render_views_srgb8(aicb_group_scene *gs, const aicb_camera *cameras, size_t n_views,
+                                          const aicb_options *opt, uint8_t (*out)[4], size_t out_len,
+                                          aicb_render_info *info) {
+    uint32_t w, h;
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::srgb8, out, out_len);
+    return on_group(gs, false, [&](Replicas r) { return views_host(r, cameras, n_views, opt, o, STAGE_PINNED, info); });
+}
+
+aicb_status aicb_group_render_views_rgba16f(aicb_group_scene *gs, const aicb_camera *cameras, size_t n_views,
+                                            const aicb_options *opt, uint16_t (*out)[4], size_t out_len,
+                                            aicb_render_info *info) {
+    uint32_t w, h;
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::rgba16f, out, out_len);
+    return on_group(gs, false, [&](Replicas r) { return views_host(r, cameras, n_views, opt, o, STAGE_GIVEN, info); });
+}
+
+aicb_status aicb_group_render_views_colorbuf(aicb_group_scene *gs, const aicb_camera *cameras, size_t n_views,
+                                             const aicb_options *opt, float (*out_colorbuf)[4], double *depth,
+                                             aicb_hit *hit, uint32_t *steps, size_t out_len, aicb_render_info *info) {
+    uint32_t w, h;
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    if (out_len && !out_colorbuf) return aicb_fail(AICB_ERR_INVALID, "out_colorbuf is NULL");
+    const aicb_device_outputs o = colorbuf_outputs(out_colorbuf, depth, hit, steps, out_len);
+    return on_group(gs, false, [&](Replicas r) {
+        return views_host(r, cameras, n_views, opt, o, STAGE_COLORBUF, info);
+    });
+}
+
+aicb_status aicb_group_render_views_text(aicb_group_scene *gs, const aicb_camera *cameras, size_t n_views,
+                                         const aicb_options *opt, int32_t *out, size_t out_len, aicb_render_info *info) {
+    uint32_t w, h;
+    if (!gs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    TRY(check_views(cameras, true, n_views, &w, &h, opt, out_len));
+    if (out_len && !out) return aicb_fail(AICB_ERR_INVALID, "out is NULL");
+    const aicb_device_outputs o = one_output(&aicb_device_outputs::text, out, out_len);
+    return on_group(gs, false, [&](Replicas r) { return views_host(r, cameras, n_views, opt, o, STAGE_GIVEN, info); });
+}
+
+aicb_status aicb_group_render_views_device(aicb_group_scene *gs, const aicb_camera *d_cameras, size_t n_views,
+                                           uint32_t fb_width, uint32_t fb_height, const aicb_options *opt,
+                                           const aicb_device_outputs *outs, void *stream, aicb_render_info *info) {
+    if (!gs || !outs) return aicb_fail(AICB_ERR_INVALID, "NULL argument");
+    if (outs->full_frame) return aicb_fail(AICB_ERR_INVALID, "full_frame is for aicb_render_device");
+    TRY(check_views(d_cameras, false, n_views, &fb_width, &fb_height, opt, outs->len));
+    return on_group(gs, false, [&](Replicas r) {
+        return views_device(r, d_cameras, n_views, fb_width, fb_height, opt, outs, (cudaStream_t)stream, info);
+    });
 }
 
 // The device-output calls on the group: every device stores into the caller's device-0 buffers; blocking.

@@ -219,6 +219,8 @@ struct aicb_ctx {
     DeviceBuffer d_cursor;       // the host cursor calls' queries and results (cursor.cu), apart from a frame's buffers
     DeviceBuffer d_bodies;       // the host body steps' bodies and results (body.cu)
     DeviceBuffer d_exposure;     // the host exposure steps' states, matrices and exposures (exposure.cu)
+    PinnedBuffer h_views;        // the host view batches' camera table, staged (pinned) and on the device
+    DeviceBuffer d_views;
     std::mutex mu;
 };
 
@@ -312,12 +314,13 @@ struct aicb_scene {
 // the layers hand on between passes; the other fields are the host's choices the kernels do not see in it.
 struct Outputs {
     aicb::TargetParams target{};
-    int kind = aicb::TGT_FRAME;         // the compositing kernels' target: TGT_FRAME, TGT_TEX or TGT_TERM
+    int kind = aicb::TGT_FRAME;         // the compositing kernels' target: TGT_FRAME, TGT_TEX, TGT_TERM or TGT_VIEWS
     bool full_frame = false;            // outputs at framebuffer positions (TraceParams::out_full_frame)
     bool aux = false;                   // the marching kernel that also counts steps and blocks (a ColorBuf set)
     const double *rays = nullptr;       // device: the tasks of a frame without a camera (origin, direction per ray)
     uint64_t n_rays = 0;
     int force_antialias = -1;           // the world layer's antialiasing option governs every layer's sample points
+    uint32_t n_views = 0;               // TGT_VIEWS: the views this frame traces (target.cameras, view_first, view_step)
 };
 
 // A frame whose pixel tasks are listed: a pixel list, or a texture target's picks (one task per entry, 32 per warp).
@@ -643,6 +646,40 @@ inline aicb_device_outputs colorbuf_outputs(float (*colorbuf)[4], double *depth,
     o.len = n;
     return o;
 }
+// A batch of views (aicb_render_views_* and aicb_group_render_views_*): n_views cameras of one framebuffer size and
+// one set of options, their outputs view-major (view v's pixel (x, y) at v * W * H + y * W + x).
+// aicb200.cu: the batch's arguments, before anything is issued (AICB_ERR_INVALID): the options, a camera table for
+// n_views > 0, out_len == n_views * W * H, and fewer than 2^32 tasks (task_base is 32-bit).  With `host_cameras`
+// the size is the first camera's and every camera must have it (*width / *height are set); otherwise the call gives it.
+aicb_status check_views(const aicb_camera *cameras, bool host_cameras, size_t n_views, uint32_t *width,
+                        uint32_t *height, const aicb_options *opt, size_t out_len);
+// group.cu: a validated batch over the replicas: view v is drawn by replica v mod n, which traces its views' tiles end
+// to end as one frame and stores them in device 0's outputs.  The host form stages the caller's outputs (as frame_host
+// does) and each replica's copy of the camera table (through its context's pinned h_views into d_views); the device
+// form reads a camera table in device 0's memory, and its outputs there, as aicb_group_render_device does.
+aicb_status views_host(Replicas r, const aicb_camera *cameras, size_t n_views, const aicb_options *opt,
+                       const aicb_device_outputs &host, Staging how, aicb_render_info *info);
+aicb_status views_device(Replicas r, const aicb_camera *d_cameras, size_t n_views, uint32_t width, uint32_t height,
+                         const aicb_options *opt, const aicb_device_outputs *outs, cudaStream_t caller,
+                         aicb_render_info *info);
+// The camera a batch's frames are launched with (launch_trace): the framebuffer size alone.
+inline aicb_camera views_frame_camera(uint32_t width, uint32_t height) {
+    aicb_camera c{};
+    c.fb_width = width;
+    c.fb_height = height;
+    c.exposure = 1.0f;
+    return c;
+}
+// One replica's views of a batch as a frame's outputs: the views r, r + n, ... of the camera table.
+inline void views_part(Outputs *o, const aicb_camera *cameras, size_t n_views, size_t replica, size_t n_replicas) {
+    o->kind = aicb::TGT_VIEWS;
+    o->full_frame = false;
+    o->n_views = (uint32_t)((n_views - replica + n_replicas - 1) / n_replicas);
+    o->target.cameras = cameras;
+    o->target.view_first = (uint32_t)replica;
+    o->target.view_step = (uint32_t)n_replicas;
+}
+
 // aicb200.cu: render_orthographic over the replicas, validated against replica 0 (the caller holds the locks).
 aicb_status ortho_srgb8(Replicas r, uint32_t resolution, uint8_t (*out)[4], size_t out_len, aicb_render_info *info);
 

@@ -223,6 +223,14 @@ struct TargetParams {
             int32_t text_start;             // CharacterBuf of a ray without in_text: Empty, or Hit(" ") behind a lone
                                             // backdrop
         };
+        // A batch of views (aicb_render_views_*): read only by the VIEWS / TGT_VIEWS instantiations.  The views'
+        // tile-ordered tasks lie end to end; local view j is the batch's view view_first + j * view_step, whose camera
+        // gives its rays and exposure and whose pixels are stored from view * fb_width * fb_height on.
+        struct {
+            const aicb_camera *cameras;     // the batch's camera table (inverse_projection_view and exposure are read)
+            uint32_t view_tiles;            // tiles of one view: tiles_x * tiles_y
+            uint32_t view_first, view_step;
+        };
     };
 };
 
@@ -727,6 +735,23 @@ AICB_DEV void post_process_color(const TraceParams &P, const float rgba[4], floa
     }
 }
 
+// post_process_color with a view's exposure in place of P.exposure (a batch of views).  A copy rather than a parameter:
+// the frames' kernels keep the code they have.
+AICB_DEV void post_process_view_color(const TraceParams &P, const float exposure, const float rgba[4], float c[3]) {
+    c[0] = ps_mul(rgba[0], exposure); c[1] = ps_mul(rgba[1], exposure); c[2] = ps_mul(rgba[2], exposure);
+    if (isfinite(P.maximum_intensity)) {
+        if (P.tone_mapping == AICB_TONE_CLAMP) {
+#pragma unroll
+            for (int i = 0; i < 3; i++) c[i] = c[i] > P.maximum_intensity ? P.maximum_intensity : c[i];
+        } else {
+            float lum = c[1] * 0.7152f + (c[0] * 0.2126f + c[2] * 0.0722f);
+            float s = ps_clamped(1.0f / (1.0f + lum / P.maximum_intensity));
+#pragma unroll
+            for (int i = 0; i < 3; i++) c[i] = ps_mul(c[i], s);
+        }
+    }
+}
+
 // Camera::post_process_color + to_srgb8 (camera_struct.rs:376-382, color.rs:669-676)
 AICB_DEV uchar4 encode_srgb8(const TraceParams &P, const float *thr, float l0, float l1, float l2, float tr) {
     float rgba[4];
@@ -737,9 +762,20 @@ AICB_DEV uchar4 encode_srgb8(const TraceParams &P, const float *thr, float l0, f
                        sat_u8(roundf(rgba[3] * 255.0f)));
 }
 
-// Camera::project_ndc_into_world (camera_struct.rs:238-257); euclid transform_point3d
-AICB_DEV void project_ndc(const TraceParams &P, double x, double y, double z, double out[3]) {
-    const double *m = P.m;
+// encode_srgb8 with a view's exposure
+AICB_DEV uchar4 encode_view_srgb8(const TraceParams &P, const float *thr, const float exposure, float l0, float l1,
+                                  float l2, float tr) {
+    float rgba[4];
+    colorbuf_to_rgba(l0, l1, l2, tr, rgba);
+    float c[3];
+    post_process_view_color(P, exposure, rgba, c);
+    return make_uchar4(component_to_srgb8(thr, c[0]), component_to_srgb8(thr, c[1]), component_to_srgb8(thr, c[2]),
+                       sat_u8(roundf(rgba[3] * 255.0f)));
+}
+
+// Camera::project_ndc_into_world (camera_struct.rs:238-257); euclid transform_point3d.  m: the camera's
+// inverse_projection_view (P.m, or a view's).
+AICB_DEV void project_ndc(const double *m, double x, double y, double z, double out[3]) {
     double hx = x * m[0] + y * m[4] + z * m[8] + m[12];
     double hy = x * m[1] + y * m[5] + z * m[9] + m[13];
     double hz = x * m[2] + y * m[6] + z * m[10] + m[14];
@@ -755,7 +791,8 @@ AICB_DEV void project_ndc(const TraceParams &P, double x, double y, double z, do
 // viewport.rs:104-113 + renderer.rs:424-451,489-491.  The four quotients by the framebuffer size are correctly rounded
 // from the host's RN(1 / W) and RN(1 / H) (pixel coordinates and sizes are integers < 2^32, well inside
 // div_known_recip's exponent window, or 0, which it divides), so they equal the divisions bit for bit.
-AICB_DEV void pixel_ray(const TraceParams &P, uint32_t xch, uint32_t ych, int sample, double o[3], double d[3]) {
+AICB_DEV void pixel_ray(const TraceParams &P, const double *m, uint32_t xch, uint32_t ych, int sample, double o[3],
+                        double d[3]) {
     const double W = (double)P.fb_width, H = (double)P.fb_height;
     const double x0 = div_known_recip((double)xch, W, P.inv_width) * 2.0 - 1.0;
     const double x1 = div_known_recip((double)(xch + 1), W, P.inv_width) * 2.0 - 1.0;
@@ -772,8 +809,8 @@ AICB_DEV void pixel_ray(const TraceParams &P, uint32_t xch, uint32_t ych, int sa
         py = y0 + (y1 - y0) * v;
     }
     double nearp[3], farp[3];
-    project_ndc(P, px, py, 0.0, nearp);
-    project_ndc(P, px, py, 1.0, farp);
+    project_ndc(m, px, py, 0.0, nearp);
+    project_ndc(m, px, py, 1.0, farp);
     o[0] = nearp[0]; o[1] = nearp[1]; o[2] = nearp[2];
     d[0] = farp[0] - nearp[0]; d[1] = farp[1] - nearp[1]; d[2] = farp[2] - nearp[2];
 }
@@ -845,10 +882,15 @@ static __device__ __noinline__ uint32_t pick_pixel(uint32_t picks, const uint32_
 // pixel tasks = one 8x4 tile); returns false for the padding pixels of edge tiles.  With a pixel list (LIST
 // instantiations only, so that the kernels of other frames do not carry the branch) pixel task i is the listed pixel
 // and its outputs go to position i; a warp then takes 32 consecutive list entries.  A texture target's batch lists its
-// picks the same way, and its outputs go to the pixel's framebuffer position.
-template <bool LIST>
+// picks the same way, and its outputs go to the pixel's framebuffer position.  A batch of views (VIEWS instantiations
+// only) lays its views' tiles end to end: a pixel task is in the tile of its view (task_view) that its rank there
+// gives, and its outputs are view-major.
+AICB_DEV uint32_t task_view(const TraceParams &P, uint32_t pixel_task) {
+    return P.target.view_first + (pixel_task >> 5) / P.target.view_tiles * P.target.view_step;
+}
+template <bool LIST, bool VIEWS = false>
 AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px, uint32_t *py, size_t *out_index) {
-    if (P.rays) {
+    if (!VIEWS && P.rays) {
         *px = *py = 0;
         *out_index = pixel_task;
         return pixel_task < P.n_rays;
@@ -864,7 +906,7 @@ AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px
         *out_index = picked ? v : pixel_task;
         return true;
     }
-    const uint32_t tile = pixel_task >> 5, in_tile = pixel_task & 31;
+    const uint32_t tile = VIEWS ? (pixel_task >> 5) % P.target.view_tiles : pixel_task >> 5, in_tile = pixel_task & 31;
     const uint32_t tx = tile % P.tiles_x, ty = tile / P.tiles_x;
     const uint32_t x = tx * TILE_W + (in_tile & (TILE_W - 1));
     const uint32_t ly = ty * TILE_H + (in_tile / TILE_W);
@@ -875,7 +917,8 @@ AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px
     }
     *px = x;
     *py = y;
-    *out_index = P.out_full_frame ? (size_t)y * P.fb_width + x : (size_t)ly * P.fb_width + x;
+    *out_index = VIEWS ? ((size_t)task_view(P, pixel_task) * P.fb_height + y) * P.fb_width + x
+                       : (P.out_full_frame ? (size_t)y * P.fb_width + x : (size_t)ly * P.fb_width + x);
     return x < P.fb_width && ly < P.local_rows;
 }
 
@@ -883,8 +926,11 @@ AICB_DEV bool task_pixel(const TraceParams &P, uint32_t pixel_task, uint32_t *px
 // Kernel 1 — ray generation: pixel -> NDC patch -> world ray (viewport.rs:104-113, renderer.rs:424-451,
 // camera_struct.rs:238-257), trace_ray_impl's prologue (sr.rs:135-180) and the outer
 // Raycaster::new().within(space bounds) (raycast.rs:196-230, 632-704).  One thread per ray, fully convergent.
+// VIEWS (gen_views_kernel): a batch of views, each pixel's ray from its view's camera; a warp's 32 tasks are one tile
+// of one view, so the camera's matrix is a warp-uniform load.
 // ======================================================================================================
-static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
+template <bool VIEWS>
+AICB_DEV void gen_rays(const TraceParams &P, uint32_t n_chunk_tasks) {
     grid_dependency_sync();
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const bool in_range = i < n_chunk_tasks;
@@ -894,7 +940,7 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
     RayRecordB rb;
     uint32_t px, py;
     size_t out_index;
-    bool active = in_range && task_pixel<true>(P, pixel_task, &px, &py, &out_index);
+    bool active = in_range && task_pixel<!VIEWS, VIEWS>(P, pixel_task, &px, &py, &out_index);
     if (P.bounce_mode == BOUNCE_SECONDARY && active) active = P.bounce_req[i] != HIT_NONE;   // no surface to light
     rec.flags = 0;
     bool running = false;
@@ -907,7 +953,8 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
             const double *rp = P.rays + 6 * (size_t)pixel_task;
             o[0] = rp[0]; o[1] = rp[1]; o[2] = rp[2]; d[0] = rp[3]; d[1] = rp[4]; d[2] = rp[5];
         } else {
-            pixel_ray(P, px, py, P.n_samples == 4 ? (int)sample : -1, o, d);
+            const double *m = VIEWS ? P.target.cameras[task_view(P, pixel_task)].inverse_projection_view : P.m;
+            pixel_ray(P, m, px, py, P.n_samples == 4 ? (int)sample : -1, o, d);
         }
         // Sky::sample octant (sky.rs:32-41) and the t conversions (sr.rs:146-151) use the original direction
         octant = ((d[0] >= 0.0) << 2) + ((d[1] >= 0.0) << 1) + (d[2] >= 0.0);
@@ -1003,6 +1050,13 @@ static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__
         o.n_hits = 0;
         *reinterpret_cast<uint4 *>(P.task_out + i) = *reinterpret_cast<const uint4 *>(&o);
     }
+}
+static __global__ void __launch_bounds__(128) gen_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
+    gen_rays<false>(P, n_chunk_tasks);
+}
+static __global__ void __launch_bounds__(128) gen_views_kernel(const __grid_constant__ TraceParams P,
+                                                               uint32_t n_chunk_tasks) {
+    gen_rays<true>(P, n_chunk_tasks);
 }
 
 // ======================================================================================================
@@ -1937,7 +1991,7 @@ static __global__ void __launch_bounds__(128) bounce_resolve_kernel(const __grid
 // encoder of draw_rgba (renderer.rs:287-291) and the stores.  `chain(k, o, lr, lg, lb, T, steps, sample_first)`
 // yields sample k's accumulator after its hits (add_color_internal, raytracer_components.rs:87-92, with
 // count_step_should_stop's opacity cut, sr.rs:648-652), its step count and the slot of its first visible surface.
-// Returns the pixel's cubes_traced.
+// Returns the pixel's cubes_traced.  VIEWS: a batch of views, whose pixels take their view's exposure.
 //
 // TEX: the accumulator is RaytraceToTexture's Split (raytrace_to_texture.rs:922-977): ColorBuf, DepthBuf and the
 // layer the pixel belongs to, stored as the colour and depth texels of trace_one (:622-683).  Split::add sets the layer
@@ -1959,8 +2013,9 @@ static __global__ void __launch_bounds__(128) bounce_resolve_kernel(const __grid
 // UI pass hands the CharacterBuf on next to the ColorBuf (out_task_text); CharacterBuf::mean reduces the samples.
 // ======================================================================================================
 constexpr uint32_t TEX_NONE = 0, TEX_WORLD = 1, TEX_UI = 2;
-// the target of a pixel-writing kernel (template): frames, aicb_render_layers_texture's texels, the terminal's pixels
-constexpr int TGT_FRAME = 0, TGT_TEX = 1, TGT_TERM = 2;
+// the target of a pixel-writing kernel (template): frames, aicb_render_layers_texture's texels, the terminal's pixels,
+// a batch of views (a frame's outputs, view-major, each view with its own camera's exposure)
+constexpr int TGT_FRAME = 0, TGT_TEX = 1, TGT_TERM = 2, TGT_VIEWS = 3;
 
 // the Space block index of the cube a hit is in (the cell word's block field)
 AICB_DEV int32_t hit_block(const TraceParams &P, uint32_t slot) {
@@ -1972,7 +2027,7 @@ AICB_DEV int32_t hit_block(const TraceParams &P, uint32_t slot) {
 
 AICB_DEV bool text_is_hit(int32_t t) { return t >= 0 || t <= AICB_TEXT_INCOMPLETE; }   // CharacterBuf State::Hit
 
-template <bool TEX, bool TERM, class Chain>
+template <bool TEX, bool TERM, bool VIEWS = false, class Chain>
 AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const uint32_t i, const size_t out_index,
                                Chain &&chain) {
     const DeviceScene &S = P.scene;
@@ -2093,7 +2148,12 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
     if (P.target.out_text) P.target.out_text[out_index] = text;
     float l0 = a0, l1 = a1, l2 = a2, tT = aT;
     if (P.n_samples == 4) { l0 = a0 / 4.0f; l1 = a1 / 4.0f; l2 = a2 / 4.0f; tT = aT / 4.0f; }
-    if (P.target.out_srgb8) P.target.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
+    float view_exposure;
+    if constexpr (VIEWS) view_exposure = P.target.cameras[task_view(P, P.task_base / P.n_samples + i)].exposure;
+    if (P.target.out_srgb8) {
+        if constexpr (VIEWS) P.target.out_srgb8[out_index] = encode_view_srgb8(P, s_thr, view_exposure, l0, l1, l2, tT);
+        else P.target.out_srgb8[out_index] = encode_srgb8(P, s_thr, l0, l1, l2, tT);
+    }
     if (P.target.out_colorbuf) P.target.out_colorbuf[out_index] = make_float4(l0, l1, l2, tT);
     if constexpr (TERM) {
         if (P.target.out_term) {   // ColorCharacterBuf::output (terminal.rs:355-366): post_process_color(Rgba::from(ColorBuf))
@@ -2133,8 +2193,13 @@ AICB_DEV uint32_t finish_pixel(const TraceParams &P, const float *s_thr, const u
         float a = 1.0f - tT;
         a = a < 0.0f ? 0.0f : (a > 1.0f ? 1.0f : a);   // clamp(0, 1): NaN passes through
         uint2 packed;
-        packed.x = f16x2_texel(l0 * P.exposure, l1 * P.exposure);
-        packed.y = f16x2_texel(l2 * P.exposure, a);
+        if constexpr (VIEWS) {
+            packed.x = f16x2_texel(l0 * view_exposure, l1 * view_exposure);
+            packed.y = f16x2_texel(l2 * view_exposure, a);
+        } else {
+            packed.x = f16x2_texel(l0 * P.exposure, l1 * P.exposure);
+            packed.y = f16x2_texel(l2 * P.exposure, a);
+        }
         P.target.out_rgba16f[out_index] = packed;
     }
     if (P.target.out_depth) P.target.out_depth[out_index] = depth;
@@ -2183,11 +2248,11 @@ AICB_DEV void count_pixels(const TraceParams &P, unsigned long long cubes_traced
 // that shade_kernel left, then finish_pixel.
 // ======================================================================================================
 // TGT: the texture targets of aicb_render_layers_texture or the terminal pixels of aicb_render_layers_terminal
-// (finish_pixel); the instantiation other frames use (TGT_FRAME) carries neither.
+// (finish_pixel), or a batch of views; the instantiation other frames use (TGT_FRAME) carries none of them.
 constexpr uint32_t ENCODE_RUN = 4;
 template <int TGT>
 __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ TraceParams P, uint32_t n_chunk_tasks) {
-    constexpr bool TEX = TGT == TGT_TEX, TERM = TGT == TGT_TERM;
+    constexpr bool TEX = TGT == TGT_TEX, TERM = TGT == TGT_TERM, VIEWS = TGT == TGT_VIEWS;
     __shared__ float s_thr[256];
     for (int i = threadIdx.x; i < 256; i += blockDim.x) s_thr[i] = P.scene.tables[256 + i];
     grid_dependency_sync();
@@ -2196,11 +2261,11 @@ __global__ void __launch_bounds__(128) encode_kernel(const __grid_constant__ Tra
     const uint32_t n_pixels = n_chunk_tasks / P.n_samples;
     uint32_t px = 0, py = 0;
     size_t out_index = 0;
-    const bool active = i < n_pixels && task_pixel<TEX>(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
+    const bool active = i < n_pixels && task_pixel<TEX, VIEWS>(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
     unsigned long long cubes_traced = 0, n_hits = 0;
     if (active) {
         const uint32_t t0 = i * P.n_samples;
-        cubes_traced = finish_pixel<TEX, TERM>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
+        cubes_traced = finish_pixel<TEX, TERM, VIEWS>(P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &o, float &lr, float &lg, float &lb,
                                                                float &T, uint32_t &steps, uint32_t &sample_first) {
             lr = 0.f; lg = 0.f; lb = 0.f; T = 1.0f;
             if (P.target.in_accum) {   // what the layer in front left in the accumulator (renderer.rs:454-471)
@@ -2291,7 +2356,8 @@ __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const 
     uint32_t px = 0, py = 0;
     size_t out_index = 0;
     const bool active = t < n_chunk_tasks &&
-                        task_pixel<TGT == TGT_TEX>(P, P.task_base / P.n_samples + i, &px, &py, &out_index);
+                        task_pixel<TGT == TGT_TEX, TGT == TGT_VIEWS>(P, P.task_base / P.n_samples + i, &px, &py,
+                                                                     &out_index);
     float lr = 0.f, lg = 0.f, lb = 0.f, T = 1.0f;
     uint32_t steps = 0, sample_first = 0xffffffffu, hi = HIT_NONE, left = 0;
     if (active) {
@@ -2372,7 +2438,7 @@ __global__ void __launch_bounds__(128, RESOLVE_MIN_BLOCKS) resolve_kernel(const 
     __syncwarp();
     unsigned long long cubes_traced = 0;
     if (active && t % P.n_samples == 0u) {
-        cubes_traced = finish_pixel<TGT == TGT_TEX, TGT == TGT_TERM>(
+        cubes_traced = finish_pixel<TGT == TGT_TEX, TGT == TGT_TERM, TGT == TGT_VIEWS>(
             P, s_thr, i, out_index, [&](uint32_t k, const TaskOut &, float &r, float &g, float &b, float &tr,
                                         uint32_t &st, uint32_t &sf) {
             const float4 a = shaded[lane + k];

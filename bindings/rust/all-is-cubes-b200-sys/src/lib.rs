@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 26 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 27 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -460,6 +460,22 @@ unsafe extern "C" {
     // asynchronous, on `stream` (a cudaStream_t, NULL = the context's); aicb_render_finish completes them
     pub fn aicb_render_device(s: *mut aicb_scene, cam: *const aicb_camera, opt: *const aicb_options, shard: *const aicb_shard,
                               outs: *const aicb_device_outputs, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_render_views_srgb8(s: *mut aicb_scene, cameras: *const aicb_camera, n_views: usize,
+                                   opt: *const aicb_options, out: *mut [u8; 4], out_len: usize,
+                                   info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_render_views_rgba16f(s: *mut aicb_scene, cameras: *const aicb_camera, n_views: usize,
+                                     opt: *const aicb_options, out: *mut [u16; 4], out_len: usize,
+                                     info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_render_views_colorbuf(s: *mut aicb_scene, cameras: *const aicb_camera, n_views: usize,
+                                      opt: *const aicb_options, out_colorbuf: *mut [f32; 4], depth: *mut f64,
+                                      hit: *mut aicb_hit, steps: *mut u32, out_len: usize,
+                                      info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_render_views_text(s: *mut aicb_scene, cameras: *const aicb_camera, n_views: usize,
+                                  opt: *const aicb_options, out: *mut i32, out_len: usize,
+                                  info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_render_views_device(s: *mut aicb_scene, d_cameras: *const aicb_camera, n_views: usize, fb_width: u32,
+                                    fb_height: u32, opt: *const aicb_options, outs: *const aicb_device_outputs,
+                                    stream: *mut c_void) -> aicb_status;
     pub fn aicb_trace_rays_device(s: *mut aicb_scene, d_origin_dir: *const [f64; 6], n: usize, opt: *const aicb_options,
                                   outs: *const aicb_device_outputs, stream: *mut c_void) -> aicb_status;
     pub fn aicb_render_layers_device(world: *const aicb_layer, ui: *const aicb_layer, backdrop_rgba: *const [f32; 4],
@@ -556,6 +572,23 @@ unsafe extern "C" {
     pub fn aicb_group_render_device(gs: *mut aicb_group_scene, cam: *const aicb_camera, opt: *const aicb_options,
                                     outs: *const aicb_device_outputs, stream: *mut c_void,
                                     info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_views_srgb8(gs: *mut aicb_group_scene, cameras: *const aicb_camera, n_views: usize,
+                                         opt: *const aicb_options, out: *mut [u8; 4], out_len: usize,
+                                         info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_views_rgba16f(gs: *mut aicb_group_scene, cameras: *const aicb_camera, n_views: usize,
+                                           opt: *const aicb_options, out: *mut [u16; 4], out_len: usize,
+                                           info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_views_colorbuf(gs: *mut aicb_group_scene, cameras: *const aicb_camera, n_views: usize,
+                                            opt: *const aicb_options, out_colorbuf: *mut [f32; 4], depth: *mut f64,
+                                            hit: *mut aicb_hit, steps: *mut u32, out_len: usize,
+                                            info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_views_text(gs: *mut aicb_group_scene, cameras: *const aicb_camera, n_views: usize,
+                                        opt: *const aicb_options, out: *mut i32, out_len: usize,
+                                        info: *mut aicb_render_info) -> aicb_status;
+    pub fn aicb_group_render_views_device(gs: *mut aicb_group_scene, d_cameras: *const aicb_camera, n_views: usize,
+                                          fb_width: u32, fb_height: u32, opt: *const aicb_options,
+                                          outs: *const aicb_device_outputs, stream: *mut c_void,
+                                          info: *mut aicb_render_info) -> aicb_status;
     pub fn aicb_group_trace_rays_device(gs: *mut aicb_group_scene, d_origin_dir: *const [f64; 6], n: usize,
                                         opt: *const aicb_options, outs: *const aicb_device_outputs, stream: *mut c_void,
                                         info: *mut aicb_render_info) -> aicb_status;

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 26
+#define AICB_ABI_VERSION 27
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -568,6 +568,39 @@ aicb_status aicb_render_layers_device(const aicb_layer *world_or_null, const aic
                                       const double depth_transform_or_null[16], const uint32_t *d_pixels_or_null,
                                       size_t n_pixels, const aicb_device_outputs *outs, void *stream);
 
+/* A batch of views of one scene drawn as one frame: n_views cameras (a world for many characters, sensors, split
+ * screens), each view RtRenderer::draw for its camera, bit for bit the single-camera call's output.  The host forms take
+ * the arguments and give the outputs of aicb_render_srgb8 / _rgba16f / _colorbuf / _text, with the camera table and
+ * n_views in place of the one camera, and no shard:
+ *   - outputs are view-major: view v's pixel (x, y) is element v * W * H + y * W + x, and out_len must be
+ *     n_views * W * H;
+ *   - each view uses its own camera's inverse_projection_view and exposure; everything in aicb_options is shared;
+ *   - every camera must have the same fb_width x fb_height (W x H), AICB_ERR_INVALID otherwise;
+ *   - info covers the batch: cubes_traced, rays and counters are the sums of the single calls', flaws are ORed, and
+ *     kernel_ms is the batch's time;
+ *   - n_views == 0 or W * H == 0 does nothing;
+ *   - AICB_ERR_INVALID also for NULL cameras with n_views > 0, and for a batch whose task count
+ *     (n_views * ceil(W / 8) * ceil(H / 4) * 32 * samples, 4 samples with antialiasing) reaches 2^32.
+ * Every argument is checked before anything is issued: a rejected call writes nothing.  The calls block, and re-issue
+ * the batch after a hit-stream overflow as the single-camera host calls do. */
+aicb_status aicb_render_views_srgb8(aicb_scene *, const aicb_camera *cameras, size_t n_views, const aicb_options *,
+                                    uint8_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
+aicb_status aicb_render_views_rgba16f(aicb_scene *, const aicb_camera *cameras, size_t n_views, const aicb_options *,
+                                      uint16_t (*out)[4], size_t out_len, aicb_render_info *info_or_null);
+aicb_status aicb_render_views_colorbuf(aicb_scene *, const aicb_camera *cameras, size_t n_views, const aicb_options *,
+                                       float (*out_colorbuf)[4], double *depth_or_null, aicb_hit *hit_or_null,
+                                       uint32_t *steps_or_null, size_t out_len, aicb_render_info *info_or_null);
+aicb_status aicb_render_views_text(aicb_scene *, const aicb_camera *cameras, size_t n_views, const aicb_options *,
+                                   int32_t *out, size_t out_len, aicb_render_info *info_or_null);
+/* The batch with the camera table (8-byte aligned) and the outputs in device memory of the scene's device.  The
+ * framebuffer size is the call's: only inverse_projection_view and exposure are read from each camera, whose own size
+ * fields are not checked.  The outputs are the world-frame sets aicb_render_device accepts, with full_frame 0 and len
+ * n_views * fb_width * fb_height.  Otherwise aicb_render_device's contract: issued on `stream`, completed by
+ * aicb_render_finish, AICB_ERR_RETRY after an overflow. */
+aicb_status aicb_render_views_device(aicb_scene *, const aicb_camera *d_cameras, size_t n_views, uint32_t fb_width,
+                                     uint32_t fb_height, const aicb_options *, const aicb_device_outputs *outs,
+                                     void *stream);
+
 /* Full-frame buffers shared between the ranks of one node (one process per GPU): the root creates
  * the frame on its GPU and publishes a 64-byte CUDA IPC handle; the other ranks open it on THEIR
  * device (peer access over NVLink is enabled lazily) and pass the mapped pointer to
@@ -748,6 +781,28 @@ aicb_status aicb_group_render_layers_device(const aicb_group_layer *world_or_nul
                                             const uint32_t *d_pixels_or_null, size_t n_pixels,
                                             const aicb_device_outputs *outs, void *stream,
                                             aicb_render_info *info_or_null);
+
+/* The batches of views (aicb_render_views_*) on the whole group, bit for bit one context's: view v is drawn by device
+ * v mod N (views differ in cost, as row strips do), and every device stores its views into device 0's buffers.  The
+ * device form blocks and orders `stream` as aicb_group_render_device does; its camera table is device-0 memory, which
+ * every device reads over peer access. */
+aicb_status aicb_group_render_views_srgb8(aicb_group_scene *, const aicb_camera *cameras, size_t n_views,
+                                          const aicb_options *, uint8_t (*out)[4], size_t out_len,
+                                          aicb_render_info *info_or_null);
+aicb_status aicb_group_render_views_rgba16f(aicb_group_scene *, const aicb_camera *cameras, size_t n_views,
+                                            const aicb_options *, uint16_t (*out)[4], size_t out_len,
+                                            aicb_render_info *info_or_null);
+aicb_status aicb_group_render_views_colorbuf(aicb_group_scene *, const aicb_camera *cameras, size_t n_views,
+                                             const aicb_options *, float (*out_colorbuf)[4], double *depth_or_null,
+                                             aicb_hit *hit_or_null, uint32_t *steps_or_null, size_t out_len,
+                                             aicb_render_info *info_or_null);
+aicb_status aicb_group_render_views_text(aicb_group_scene *, const aicb_camera *cameras, size_t n_views,
+                                         const aicb_options *, int32_t *out, size_t out_len,
+                                         aicb_render_info *info_or_null);
+aicb_status aicb_group_render_views_device(aicb_group_scene *, const aicb_camera *d_cameras, size_t n_views,
+                                           uint32_t fb_width, uint32_t fb_height, const aicb_options *,
+                                           const aicb_device_outputs *outs, void *stream,
+                                           aicb_render_info *info_or_null);
 
 /* ---------------------------------------------------------------------------------------------
  * Texture targets: the state RaytraceToTexture::Inner keeps around trace_one (all-is-cubes-gpu/src/raytrace_to_texture.rs),
