@@ -979,11 +979,14 @@ class RenderInfo:
     # first chunk: ray generation, marching, shading, encode; where shading and encode ran as one kernel
     # (resolve_kernel: None / Flat lighting, most frames) [2] is its time and [3] is 0
     stage_ms: tuple = (0.0, 0.0, 0.0, 0.0)
+    # 1: the rays were taken in order of their tiles' steps in the context's previous frame of the same view and layout;
+    # 0: by chord
+    ray_order: int = 0
 
     @staticmethod
     def from_abi(i: abi.RenderInfo) -> "RenderInfo":
         return RenderInfo(int(i.cubes_traced), int(i.rays), int(i.algorithmic_bytes), tuple(int(c) for c in i.counters),
-                          float(i.kernel_ms), int(i.flaws), tuple(float(v) for v in i.stage_ms))
+                          float(i.kernel_ms), int(i.flaws), tuple(float(v) for v in i.stage_ms), int(i.ray_order))
 
 
 @dataclasses.dataclass

@@ -116,7 +116,7 @@ class RenderInfo(C.Structure):
         ("counters", C.c_uint64 * 6),
         ("kernel_ms", C.c_float),
         ("flaws", C.c_uint16),
-        ("_pad", C.c_uint16),
+        ("ray_order", C.c_uint16),
         ("stage_ms", C.c_float * 4),
     ]
 

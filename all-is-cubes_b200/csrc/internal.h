@@ -1,5 +1,6 @@
 // internal.h — objects behind the opaque handles of include/aicb200.h (shared by aicb200.cu, group.cu and light.cu).
 #pragma once
+#include <cstring>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -110,7 +111,7 @@ inline uint32_t cell_word(uint32_t id, uint8_t kind, bool wide) { return id | ((
 // One chunk's streams between the kernels of a frame (trace_kernel.cuh): the listed rays' records (array A, then
 // array B), a TaskOut per task, the HitRecord stream (march -> resolve, or march -> shade -> encode), a ShadedHit per
 // hit (shade -> encode: not used by frames that run resolve_kernel) and the task ids of the rays that enter the space,
-// per chord-length bin.
+// per cost bin (longest first).
 struct ChunkStreams {
     DeviceBuffer rays, task_out, hits, shaded, bin_list;
 
@@ -132,6 +133,20 @@ struct ChunkStreams {
     void release_hits() {
         hits.reset();
         shaded.reset();
+    }
+};
+
+// The view and task layout of a frame whose TaskOut stream primary.task_out holds: a frame with the same key finds each
+// task's steps of that frame at its own index, and lists its rays by them (launch_trace).  The zero key holds nothing.
+struct RayOrderKey {
+    const aicb_scene *scene = nullptr;
+    double view[16] = {};   // the camera's inverse_projection_view
+    uint32_t fb_width = 0, fb_height = 0, n_samples = 0;
+    uint32_t strip_rows = 0, shard_index = 0, shard_count = 0;
+    bool operator==(const RayOrderKey &o) const {
+        return scene == o.scene && std::memcmp(view, o.view, sizeof view) == 0 && fb_width == o.fb_width &&
+               fb_height == o.fb_height && n_samples == o.n_samples && strip_rows == o.strip_rows &&
+               shard_index == o.shard_index && shard_count == o.shard_count;
     }
 };
 
@@ -205,6 +220,8 @@ struct aicb_ctx {
     uint32_t hits_per_task = 8;  // capacity of the hit stream per ray; raised x4 when a frame overflows it,
     uint32_t shallow_frames = 0; //   lowered again after 16 frames in a row that needed a small fraction of it
     bool deep_frames = false;    // the last frame met >= 3/4 visible surfaces per ray: no resolve_kernel (launch_trace)
+    RayOrderKey order_key;       // the frame whose steps primary.task_out holds
+    bool ray_ordered = false;    // the frame in flight listed its rays by the previous frame's steps (ray_order)
     PinnedBuffer h_stage;        // pinned staging of frames whose destination is pageable host memory
     // the frame whose per-frame scratch (streams, counters, events) is in use
     bool frame_in_flight = false;

@@ -256,7 +256,7 @@ pub struct aicb_render_info {
     pub counters: [u64; 6],
     pub kernel_ms: f32,
     pub flaws: u16,
-    pub _pad: u16,
+    pub ray_order: u16,
     pub stage_ms: [f32; 4],
 }
 

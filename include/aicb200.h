@@ -165,7 +165,10 @@ typedef struct aicb_render_info {
     uint64_t counters[6];          /* outer steps, inner steps, surface hits, light texels, blocks entered, pixels */
     float kernel_ms;               /* CUDA-event duration of the whole frame (all kernels) on its stream */
     uint16_t flaws;                /* Flaws bits (flaws.rs:20-91) */
-    uint16_t _pad;
+    uint16_t ray_order;            /* 1: the marching kernel took the frame's rays in order of the steps their tiles took
+                                      in the context's previous frame, of the same scene, camera view, size, samples and
+                                      shard (a scheduling choice only: the outputs are the same either way); 0: in order
+                                      of their chords through the Space */
     float stage_ms[4];             /* the frame's kernels (first chunk): ray generation, marching, shading, encode;
                                       where shading and encode ran as one kernel (LightingOption::None / Flat, most
                                       frames) [2] is its time and [3] is 0 */
