@@ -173,6 +173,15 @@ def load_library() -> C.CDLL:
                                                           C.c_void_p]
         getattr(lib, prefix + "step_exposure_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                                                                  C.c_double, C.c_void_p, C.c_void_p]
+    lib.aicb_look_rotation.argtypes = [C.c_double, C.c_double, C.c_void_p]
+    lib.aicb_look_rotation.restype = None
+    for prefix in ("aicb_", "aicb_group_"):
+        getattr(lib, prefix + "step_eyes_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                             C.c_double, C.c_void_p]
+        getattr(lib, prefix + "eye_views_device").argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                             C.c_void_p, C.c_size_t, C.POINTER(abi.EyeViewParams),
+                                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                             C.c_void_p]
     lib.aicb_project_cursor.argtypes = [C.POINTER(abi.Layer), C.POINTER(abi.Layer), C.c_void_p, C.c_size_t,
                                         C.c_double, C.c_void_p]
     lib.aicb_group_project_cursor.argtypes = [C.POINTER(abi.GroupLayer), C.POINTER(abi.GroupLayer), C.c_void_p,
@@ -708,6 +717,42 @@ def view_transform_matrix(rotation_ijkr, translation) -> np.ndarray:
     out = (C.c_double * 16)()
     load_library().aicb_view_transform_matrix(q, t, out)
     return np.array(out[:], dtype=np.float64)
+
+
+def eyes(n):
+    """n CharacterEye::default() values with no previous velocity: an abi.EYE_DTYPE array of zeros."""
+    return np.zeros(n, dtype=abi.EYE_DTYPE)
+
+
+def look_rotation(yaw_degrees: float, pitch_degrees: float) -> np.ndarray:
+    """Body::look_rotation (physics/body.rs:285-292) of a yaw and a pitch in degrees: the eye-to-world rotation
+    (i, j, k, r) as float64 [4], what eye_views takes per eye."""
+    out = (C.c_double * 4)()
+    load_library().aicb_look_rotation(float(yaw_degrees), float(pitch_degrees), out)
+    return np.array(out[:], dtype=np.float64)
+
+
+def eye_view_params(options: "GraphicsOptions", viewport: "Viewport") -> abi.EyeViewParams:
+    """The aicb_eye_view_params of a batch of eyes whose world cameras have these options and this viewport."""
+    o = options.repair()
+    p = abi.EyeViewParams()
+    p.fov_y_degrees = o.fov_y
+    p.view_distance = o.view_distance
+    p.nominal_width = float(viewport.nominal_size[0])
+    p.nominal_height = float(viewport.nominal_size[1])
+    p.fb_width, p.fb_height = (int(v) for v in viewport.framebuffer_size)
+    automatic = o.exposure == EXPOSURE_AUTOMATIC
+    p.fixed_exposure = 1.0 if automatic else float(o.exposure)
+    p.automatic_exposure = 1 if automatic else 0
+    p.lighting_display = o.lighting_display
+    return p
+
+
+def eye_cameras(n, options: "GraphicsOptions", viewport: "Viewport") -> np.ndarray:
+    """A camera table of n world cameras as Camera::new leaves them (identity view transform, exposure
+    ExposureOption::initial()): the abi.CAMERA_DTYPE array eye_views updates in place."""
+    cam = Camera(options, viewport)
+    return np.repeat(np.frombuffer(bytes(cam.data), dtype=abi.CAMERA_DTYPE), n)
 
 
 def bodies(n, position=(0.0, 0.0, 0.0), collision_box=(-0.5, -0.5, -0.5, 0.5, 0.5, 0.5), velocity=(0.0, 0.0, 0.0),
@@ -1248,6 +1293,44 @@ class _Scene:
         out = np.zeros(n, dtype=np.float32)
         _check(self._fn("step_exposure")(self.handle, st.ctypes.data, m.ctypes.data, n, float(dt), out.ctypes.data))
         return st, out
+
+    def step_eyes(self, eyes, bodies, dt):
+        """step_eye_position (character/eye.rs:90-121) for a batch of eyes after one stepped tick of their bodies, in
+        place on the current torch stream.  eyes: a uint8 CUDA tensor [n, 72] of abi.EYE_DTYPE records (see
+        aicb200.eyes) on the scene's device (device 0 of a group); bodies: a uint8 tensor [n, 152] of the stepped
+        bodies; dt: Tick::delta_t in seconds, in (0, 1].  previous_body_velocity becomes each body's velocity."""
+        torch = _torch()
+        n = eyes.shape[0]
+        e = self._tensor(eyes, torch.uint8, (n, abi.EYE_DTYPE.itemsize), "eyes")
+        b = self._tensor(bodies, torch.uint8, (n, abi.BODY_DTYPE.itemsize), "bodies")
+        _check(self._fn("step_eyes_device")(self.handle, e.data_ptr(), b.data_ptr(), n, float(dt),
+                                             _stream(self._device())))
+        return e
+
+    def eye_views(self, eyes, bodies, rotations, exposures, camera_params, eye_to_world=None, cameras=None,
+                  look_rays=None, status=None):
+        """compute_view_transform (character/eye.rs:187-203) and the world camera's update for a batch of eyes, on the
+        current torch stream: each output given is written (None: not written).  eyes and bodies as step_eyes takes
+        them; rotations: float64 [n, 4] (look_rotation per eye); exposures: float32 [n] (step_exposure's, device=True)
+        or None; camera_params: aicb200.eye_view_params(options, viewport).  Outputs: eye_to_world float64 [n, 16]
+        (the next tick's step_exposure input), cameras a uint8 tensor [n, 144] of abi.CAMERA_DTYPE records updated in
+        place (see eye_cameras), look_rays float64 [n, 6] (origin, direction at the screen centre) and status int32
+        [n] (0, or abi.EYE_NOT_INVERTIBLE).  Returns (eye_to_world, cameras, look_rays, status)."""
+        torch = _torch()
+        n = eyes.shape[0]
+        e = self._tensor(eyes, torch.uint8, (n, abi.EYE_DTYPE.itemsize), "eyes")
+        b = self._tensor(bodies, torch.uint8, (n, abi.BODY_DTYPE.itemsize), "bodies")
+        r = self._tensor(rotations, torch.float64, (n, 4), "rotations")
+        x = None if exposures is None else self._tensor(exposures, torch.float32, (n,), "exposures")
+        m = None if eye_to_world is None else self._tensor(eye_to_world, torch.float64, (n, 16), "eye_to_world")
+        c = None if cameras is None else self._tensor(cameras, torch.uint8, (n, abi.CAMERA_DTYPE.itemsize), "cameras")
+        lr = None if look_rays is None else self._tensor(look_rays, torch.float64, (n, 6), "look_rays")
+        st = None if status is None else self._tensor(status, torch.int32, (n,), "status")
+        ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
+        _check(self._fn("eye_views_device")(self.handle, e.data_ptr(), b.data_ptr(), r.data_ptr(), ptr(x), n,
+                                             C.byref(camera_params), ptr(m), ptr(c), ptr(lr), ptr(st),
+                                             _stream(self._device())))
+        return m, c, lr, st
 
     def _light_download_device(self):
         torch = _torch()

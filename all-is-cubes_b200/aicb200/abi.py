@@ -3,7 +3,7 @@ import ctypes as C
 
 import numpy as np
 
-ABI_VERSION = 27
+ABI_VERSION = 28
 
 BLOCKS_DERIVE_LIGHT = 1
 
@@ -223,6 +223,24 @@ EXPOSURE_STATE_DTYPE = np.dtype([("luminance_samples", "<f4", (100,)), ("luminan
                                  ("exposure_log", "<f4")])
 assert EXPOSURE_STATE_DTYPE.itemsize == 408
 
+# aicb_eye as a numpy structured dtype (what step_eyes and eye_views take): CharacterEye + PreviousBodyVelocity
+EYE_DTYPE = np.dtype([("displacement_pos", "<f8", (3,)), ("displacement_vel", "<f8", (3,)),
+                      ("previous_body_velocity", "<f8", (3,))])
+assert EYE_DTYPE.itemsize == 72
+
+
+class EyeViewParams(C.Structure):
+    """aicb_eye_view_params: what the world camera of a batch of eyes takes from GraphicsOptions and the Viewport."""
+    _fields_ = [("fov_y_degrees", C.c_double), ("view_distance", C.c_double), ("nominal_width", C.c_double),
+                ("nominal_height", C.c_double), ("fb_width", C.c_uint32), ("fb_height", C.c_uint32),
+                ("fixed_exposure", C.c_float), ("automatic_exposure", C.c_uint8), ("lighting_display", C.c_uint8),
+                ("_pad", C.c_uint8 * 2)]
+
+
+EYE_VIEW_PARAMS = EyeViewParams
+assert C.sizeof(EYE_VIEW_PARAMS) == 48
+EYE_NOT_INVERTIBLE = 1   # aicb_eye_views_device status
+
 
 EXPORTED_SYMBOLS = [
     "aicb_abi_version",
@@ -303,6 +321,11 @@ EXPORTED_SYMBOLS = [
     "aicb_step_exposure_device",
     "aicb_group_step_exposure",
     "aicb_group_step_exposure_device",
+    "aicb_look_rotation",
+    "aicb_step_eyes_device",
+    "aicb_eye_views_device",
+    "aicb_group_step_eyes_device",
+    "aicb_group_eye_views_device",
     "aicb_light_chart",
     "aicb_light_chart_chains",
     "aicb_light_fast_evaluate",

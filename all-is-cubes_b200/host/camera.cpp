@@ -7,10 +7,7 @@
 // (eye_for_look_at); graphics_options.rs:194-198 (repair).
 //
 // The matrix/quaternion algebra is euclid 0.22.14 (Transform3D / Rotation3D /
-// RigidTransform3D), which is a crates.io dependency NOT vendored in the reference tree; it is
-// restated here from its published definitions (row-vector convention, m11..m44) and pinned by
-// the reference's own camera tests (camera/tests.rs:78-109 exact frustum corners, :198-222) and
-// the text.rs ASCII golden images — see tests/test_camera.py.
+// RigidTransform3D), restated once for the host and the device in ../csrc/camera_math.cuh.
 //
 // Compiled with -ffp-contract=off / -fmad=false semantics (host code; nvcc passes it to g++).
 #include <cmath>
@@ -18,82 +15,12 @@
 #include <limits>
 
 #include "../../include/aicb200.h"
+#include "../csrc/camera_math.cuh"
 
 namespace {
 
-struct Mat4 {
-    // m[r][c] = m{r+1}{c+1}
-    double m[4][4];
-};
+using namespace aicb::camera_math;
 
-// Transform3D::then: row-vector convention, result = self * other
-Mat4 then(const Mat4 &a, const Mat4 &b) {
-    Mat4 r;
-    for (int i = 0; i < 4; i++)
-        for (int j = 0; j < 4; j++)
-            r.m[i][j] = a.m[i][0] * b.m[0][j] + a.m[i][1] * b.m[1][j] + a.m[i][2] * b.m[2][j] + a.m[i][3] * b.m[3][j];
-    return r;
-}
-
-// Transform3D::determinant
-double determinant(const Mat4 &t) {
-    const double m11 = t.m[0][0], m12 = t.m[0][1], m13 = t.m[0][2], m14 = t.m[0][3];
-    const double m21 = t.m[1][0], m22 = t.m[1][1], m23 = t.m[1][2], m24 = t.m[1][3];
-    const double m31 = t.m[2][0], m32 = t.m[2][1], m33 = t.m[2][2], m34 = t.m[2][3];
-    const double m41 = t.m[3][0], m42 = t.m[3][1], m43 = t.m[3][2], m44 = t.m[3][3];
-    return m14 * m23 * m32 * m41 - m13 * m24 * m32 * m41 - m14 * m22 * m33 * m41 + m12 * m24 * m33 * m41 +
-           m13 * m22 * m34 * m41 - m12 * m23 * m34 * m41 - m14 * m23 * m31 * m42 + m13 * m24 * m31 * m42 +
-           m14 * m21 * m33 * m42 - m11 * m24 * m33 * m42 - m13 * m21 * m34 * m42 + m11 * m23 * m34 * m42 +
-           m14 * m22 * m31 * m43 - m12 * m24 * m31 * m43 - m14 * m21 * m32 * m43 + m11 * m24 * m32 * m43 +
-           m12 * m21 * m34 * m43 - m11 * m22 * m34 * m43 - m13 * m22 * m31 * m44 + m12 * m23 * m31 * m44 +
-           m13 * m21 * m32 * m44 - m11 * m23 * m32 * m44 - m12 * m21 * m33 * m44 + m11 * m22 * m33 * m44;
-}
-
-// Transform3D::inverse: adjugate scaled by 1/det
-bool inverse(const Mat4 &t, Mat4 *out) {
-    const double det = determinant(t);
-    if (det == 0.0) return false;
-    const double m11 = t.m[0][0], m12 = t.m[0][1], m13 = t.m[0][2], m14 = t.m[0][3];
-    const double m21 = t.m[1][0], m22 = t.m[1][1], m23 = t.m[1][2], m24 = t.m[1][3];
-    const double m31 = t.m[2][0], m32 = t.m[2][1], m33 = t.m[2][2], m34 = t.m[2][3];
-    const double m41 = t.m[3][0], m42 = t.m[3][1], m43 = t.m[3][2], m44 = t.m[3][3];
-    Mat4 a;
-    a.m[0][0] = m23 * m34 * m42 - m24 * m33 * m42 + m24 * m32 * m43 - m22 * m34 * m43 - m23 * m32 * m44 + m22 * m33 * m44;
-    a.m[0][1] = m14 * m33 * m42 - m13 * m34 * m42 - m14 * m32 * m43 + m12 * m34 * m43 + m13 * m32 * m44 - m12 * m33 * m44;
-    a.m[0][2] = m13 * m24 * m42 - m14 * m23 * m42 + m14 * m22 * m43 - m12 * m24 * m43 - m13 * m22 * m44 + m12 * m23 * m44;
-    a.m[0][3] = m14 * m23 * m32 - m13 * m24 * m32 - m14 * m22 * m33 + m12 * m24 * m33 + m13 * m22 * m34 - m12 * m23 * m34;
-    a.m[1][0] = m24 * m33 * m41 - m23 * m34 * m41 - m24 * m31 * m43 + m21 * m34 * m43 + m23 * m31 * m44 - m21 * m33 * m44;
-    a.m[1][1] = m13 * m34 * m41 - m14 * m33 * m41 + m14 * m31 * m43 - m11 * m34 * m43 - m13 * m31 * m44 + m11 * m33 * m44;
-    a.m[1][2] = m14 * m23 * m41 - m13 * m24 * m41 - m14 * m21 * m43 + m11 * m24 * m43 + m13 * m21 * m44 - m11 * m23 * m44;
-    a.m[1][3] = m13 * m24 * m31 - m14 * m23 * m31 + m14 * m21 * m33 - m11 * m24 * m33 - m13 * m21 * m34 + m11 * m23 * m34;
-    a.m[2][0] = m22 * m34 * m41 - m24 * m32 * m41 + m24 * m31 * m42 - m21 * m34 * m42 - m22 * m31 * m44 + m21 * m32 * m44;
-    a.m[2][1] = m14 * m32 * m41 - m12 * m34 * m41 - m14 * m31 * m42 + m11 * m34 * m42 + m12 * m31 * m44 - m11 * m32 * m44;
-    a.m[2][2] = m12 * m24 * m41 - m14 * m22 * m41 + m14 * m21 * m42 - m11 * m24 * m42 - m12 * m21 * m44 + m11 * m22 * m44;
-    a.m[2][3] = m14 * m22 * m31 - m12 * m24 * m31 - m14 * m21 * m32 + m11 * m24 * m32 + m12 * m21 * m34 - m11 * m22 * m34;
-    a.m[3][0] = m23 * m32 * m41 - m22 * m33 * m41 - m23 * m31 * m42 + m21 * m33 * m42 + m22 * m31 * m43 - m21 * m32 * m43;
-    a.m[3][1] = m12 * m33 * m41 - m13 * m32 * m41 + m13 * m31 * m42 - m11 * m33 * m42 - m12 * m31 * m43 + m11 * m32 * m43;
-    a.m[3][2] = m13 * m22 * m41 - m12 * m23 * m41 - m13 * m21 * m42 + m11 * m23 * m42 + m12 * m21 * m43 - m11 * m22 * m43;
-    a.m[3][3] = m12 * m23 * m31 - m13 * m22 * m31 + m13 * m21 * m32 - m11 * m23 * m32 - m12 * m21 * m33 + m11 * m22 * m33;
-    const double s = 1.0 / det;
-    for (int i = 0; i < 4; i++)
-        for (int j = 0; j < 4; j++) out->m[i][j] = a.m[i][j] * s;
-    return true;
-}
-
-struct Quat {
-    double i, j, k, r;
-};
-
-// Rotation3D::then (Hamilton product, other applied after self)
-Quat q_then(const Quat &s, const Quat &o) {
-    return Quat{
-        o.i * s.r + o.r * s.i + o.j * s.k - o.k * s.j,
-        o.j * s.r + o.r * s.j + o.k * s.i - o.i * s.k,
-        o.k * s.r + o.r * s.k + o.i * s.j - o.j * s.i,
-        o.r * s.r - o.i * s.i - o.j * s.j - o.k * s.k,
-    };
-}
-Quat q_inverse(const Quat &q) { return Quat{-q.i, -q.j, -q.k, q.r}; }
 Quat around_x(double radians) {
     double h = radians / 2.0;
     return Quat{std::sin(h), 0.0, 0.0, std::cos(h)};
@@ -102,79 +29,13 @@ Quat around_y(double radians) {
     double h = radians / 2.0;
     return Quat{0.0, std::sin(h), 0.0, std::cos(h)};
 }
-// Rotation3D::transform_vector3d
-void q_transform(const Quat &q, const double v[3], double out[3]) {
-    // cross = vector_part x v * 2
-    double cx = (q.j * v[2] - q.k * v[1]) * 2.0;
-    double cy = (q.k * v[0] - q.i * v[2]) * 2.0;
-    double cz = (q.i * v[1] - q.j * v[0]) * 2.0;
-    out[0] = v[0] + q.r * cx + q.j * cz - q.k * cy;
-    out[1] = v[1] + q.r * cy + q.k * cx - q.i * cz;
-    out[2] = v[2] + q.r * cz + q.i * cy - q.j * cx;
-}
-// Rotation3D::to_transform
-Mat4 q_to_transform(const Quat &q) {
-    double i2 = q.i + q.i, j2 = q.j + q.j, k2 = q.k + q.k;
-    double ii = q.i * i2, ij = q.i * j2, ik = q.i * k2;
-    double jj = q.j * j2, jk = q.j * k2, kk = q.k * k2;
-    double ri = q.r * i2, rj = q.r * j2, rk = q.r * k2;
-    Mat4 t;
-    std::memset(&t, 0, sizeof t);
-    t.m[0][0] = 1.0 - (jj + kk);
-    t.m[0][1] = ij + rk;
-    t.m[0][2] = ik - rj;
-    t.m[1][0] = ij - rk;
-    t.m[1][1] = 1.0 - (ii + kk);
-    t.m[1][2] = jk + ri;
-    t.m[2][0] = ik + rj;
-    t.m[2][1] = jk - ri;
-    t.m[2][2] = 1.0 - (ii + jj);
-    t.m[3][3] = 1.0;
-    return t;
-}
-Mat4 translation(const double v[3]) {
-    Mat4 t;
-    std::memset(&t, 0, sizeof t);
-    t.m[0][0] = t.m[1][1] = t.m[2][2] = t.m[3][3] = 1.0;
-    t.m[3][0] = v[0];
-    t.m[3][1] = v[1];
-    t.m[3][2] = v[2];
-    return t;
-}
-
-double repair(double v, double lo, double hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
 // Camera::compute_matrices (camera_struct.rs:387-416)
 bool compute(const Quat &rotation, const double trans[3], double fov_y_degrees, double view_distance,
              double nominal_w, double nominal_h, aicb_camera *out) {
-    double fov_y = repair(fov_y_degrees, 1.0, 189.0);       // graphics_options.rs:195
-    double far = repair(view_distance, 1.0, 10000.0);       // graphics_options.rs:196
-    double fov_cot = 1.0 / std::tan((fov_y / 2.0) * (M_PI / 180.0));  // f64::to_radians = x * (PI/180)
-    double aspect = nominal_w / nominal_h;                  // viewport.rs:80-83
-    if (!std::isfinite(aspect)) aspect = 1.0;
-    double near = 1.0 / 32.0;                               // camera_struct.rs:202-205
-
-    Mat4 proj;
-    std::memset(&proj, 0, sizeof proj);
-    proj.m[0][0] = fov_cot / aspect;
-    proj.m[1][1] = fov_cot;
-    proj.m[2][2] = far / (near - far);
-    proj.m[2][3] = -1.0;
-    proj.m[3][2] = (far * near) / (near - far);
-
-    // RigidTransform3D::inverse: rotation^-1, translation = rotation^-1 * (-translation);
-    // to_transform: rotation.to_transform().then(translation.to_transform())
-    Quat rinv = q_inverse(rotation);
-    double neg[3] = {-trans[0], -trans[1], -trans[2]};
-    double tinv[3];
-    q_transform(rinv, neg, tinv);
-    Mat4 world_to_eye = then(q_to_transform(rinv), translation(tinv));
-
-    Mat4 inv;
-    if (!inverse(then(world_to_eye, proj), &inv)) return false;
-    for (int i = 0; i < 4; i++)
-        for (int j = 0; j < 4; j++) out->inverse_projection_view[i * 4 + j] = inv.m[i][j];
-    return true;
+    double fov_cot, aspect, far;
+    projection_terms(fov_y_degrees, view_distance, nominal_w, nominal_h, &fov_cot, &aspect, &far);
+    return projection_view_inverse(rotation, trans, fov_cot, aspect, far, out->inverse_projection_view);
 }
 
 }  // namespace
@@ -211,9 +72,17 @@ aicb_status aicb_camera_look_at(const double eye[3], const double target[3], dou
 
 // ViewTransform::to_transform (RigidTransform3D::to_transform): rotation.to_transform().then(translation.to_transform())
 void aicb_view_transform_matrix(const double q[4], const double translation_[3], double out[16]) {
-    const Mat4 t = then(q_to_transform(Quat{q[0], q[1], q[2], q[3]}), translation(translation_));
-    for (int i = 0; i < 4; i++)
-        for (int j = 0; j < 4; j++) out[i * 4 + j] = t.m[i][j];
+    view_transform_matrix(Quat{q[0], q[1], q[2], q[3]}, translation_, out);
+}
+
+// Body::look_rotation (physics/body.rs:285-292): around_x(-pitch.to_radians()).then(around_y(-yaw.to_radians())),
+// f64::to_radians being x * (PI / 180)
+void aicb_look_rotation(double yaw_degrees, double pitch_degrees, double out[4]) {
+    const Quat q = q_then(around_x(-(pitch_degrees * (M_PI / 180.0))), around_y(-(yaw_degrees * (M_PI / 180.0))));
+    out[0] = q.i;
+    out[1] = q.j;
+    out[2] = q.k;
+    out[3] = q.r;
 }
 
 // eye_for_look_at (all-is-cubes/src/camera.rs:34-40)

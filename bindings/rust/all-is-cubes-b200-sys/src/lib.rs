@@ -1,4 +1,4 @@
-//! `include/aicb200.h`, item for item.  ABI version 27 (`aicb_abi_version()`).
+//! `include/aicb200.h`, item for item.  ABI version 28 (`aicb_abi_version()`).
 //! Layouts are checked against the C header by `tests/test_abi.py` on the Python mirror; keep the three in step.
 #![allow(non_camel_case_types)]
 #![no_std]
@@ -87,6 +87,37 @@ impl Default for aicb_exposure_state {
         Self { luminance_samples: [1.0; 100], luminance_sample_index: 0, exposure_log: 0.0 }
     }
 }
+
+/// `CharacterEye` and `PreviousBodyVelocity` (character/eye.rs:38-57), 72 bytes; all zeros is
+/// `CharacterEye::default()`.  A host that changes a body's velocity outside the body step also writes
+/// `previous_body_velocity`.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_eye {
+    pub displacement_pos: [f64; 3],
+    pub displacement_vel: [f64; 3],
+    pub previous_body_velocity: [f64; 3],
+}
+
+/// What a batch of eyes' world cameras take from `GraphicsOptions` and the `Viewport`, 48 bytes;
+/// `automatic_exposure == 0` is `ExposureOption::Fixed(fixed_exposure)`.
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct aicb_eye_view_params {
+    pub fov_y_degrees: f64,
+    pub view_distance: f64,
+    pub nominal_width: f64,
+    pub nominal_height: f64,
+    pub fb_width: u32,
+    pub fb_height: u32,
+    pub fixed_exposure: f32,
+    pub automatic_exposure: u8,
+    pub lighting_display: u8,
+    pub _pad: [u8; 2],
+}
+
+/// `aicb_eye_views_device` status: the projection-view matrix has no inverse; nothing else of the eye is written.
+pub const AICB_EYE_NOT_INVERTIBLE: u32 = 1;
 
 /// `Body` (physics/body.rs:38-90) without its look direction; boxes are `[lower xyz, upper xyz]`
 #[repr(C)]
@@ -699,6 +730,24 @@ unsafe extern "C" {
     pub fn aicb_group_step_exposure_device(gs: *mut aicb_group_scene, d_states: *mut aicb_exposure_state,
                                            d_eye_to_world: *const [f64; 16], n: usize, dt: f64,
                                            d_exposure_out_or_null: *mut f32, stream: *mut c_void) -> aicb_status;
+
+    pub fn aicb_look_rotation(yaw_degrees: f64, pitch_degrees: f64, out_ijkr: *mut [f64; 4]);
+    pub fn aicb_step_eyes_device(s: *mut aicb_scene, d_eyes: *mut aicb_eye, d_bodies: *const aicb_body, n: usize,
+                                 dt: f64, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_eye_views_device(s: *mut aicb_scene, d_eyes: *const aicb_eye, d_bodies: *const aicb_body,
+                                 d_rotations: *const [f64; 4], d_exposures_or_null: *const f32, n: usize,
+                                 params: *const aicb_eye_view_params, d_eye_to_world_or_null: *mut [f64; 16],
+                                 d_cameras_or_null: *mut aicb_camera, d_look_rays_or_null: *mut [f64; 6],
+                                 d_status_or_null: *mut u32, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_step_eyes_device(gs: *mut aicb_group_scene, d_eyes: *mut aicb_eye, d_bodies: *const aicb_body,
+                                       n: usize, dt: f64, stream: *mut c_void) -> aicb_status;
+    pub fn aicb_group_eye_views_device(gs: *mut aicb_group_scene, d_eyes: *const aicb_eye,
+                                       d_bodies: *const aicb_body, d_rotations: *const [f64; 4],
+                                       d_exposures_or_null: *const f32, n: usize,
+                                       params: *const aicb_eye_view_params,
+                                       d_eye_to_world_or_null: *mut [f64; 16], d_cameras_or_null: *mut aicb_camera,
+                                       d_look_rays_or_null: *mut [f64; 6], d_status_or_null: *mut u32,
+                                       stream: *mut c_void) -> aicb_status;
 
     pub fn aicb_light_chart(weights: *mut f32, children: *mut u32) -> u32;
     pub fn aicb_light_chart_chains(preorder: *mut u32, chains: *mut [u32; 6], euler: *mut u16) -> u32;

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define AICB_ABI_VERSION 27
+#define AICB_ABI_VERSION 28
 
 typedef enum aicb_status {
     AICB_OK = 0,
@@ -1109,6 +1109,89 @@ aicb_status aicb_group_step_exposure(aicb_group_scene *, aicb_exposure_state *st
 aicb_status aicb_group_step_exposure_device(aicb_group_scene *, aicb_exposure_state *d_states,
                                             const double (*d_eye_to_world)[16], size_t n, double dt,
                                             float *d_exposure_out_or_null, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Characters' eyes on the device: step_eye_position (all-is-cubes/src/character/eye.rs:90-121), compute_view_transform
+ * (eye.rs:187-203) and the world camera StandardCameras::update builds from it (stdcam.rs:237-256: set_view_transform,
+ * compute_matrices, set_measured_exposure), for a batch of eyes.  With aicb_step_bodies_device and
+ * aicb_step_exposure_device, a tick of many characters is one stream of device calls with no host wait:
+ *   bodies, then exposure, then eyes, then eye views, then cursor and frames (INTEGRATION §2p).
+ * The body's look rotation comes in as a quaternion (aicb_look_rotation on the host): yaw and pitch come from input,
+ * and their sine and cosine are glibc's, which the device could not reproduce bit for bit.  Nothing of the scene is
+ * read or changed (no host mirror rebuild, no light state, no frame in flight); the scene fixes the device and the
+ * context's stream.
+ * ------------------------------------------------------------------------------------------- */
+/* CharacterEye and PreviousBodyVelocity (eye.rs:38-57), 72 bytes.  All zeros is CharacterEye::default().
+ * previous_body_velocity is the body's velocity before this tick's body step: aicb_step_eyes_device stores the body's
+ * velocity there after each step, which is what the next tick's record_previous_velocity (eye.rs:83-87) reads as long
+ * as nothing else changes the body between ticks.  A host that changes a velocity outside the body step (a teleport,
+ * a jump added on a paused tick) writes previous_body_velocity too. */
+typedef struct aicb_eye {
+    double displacement_pos[3];
+    double displacement_vel[3];
+    double previous_body_velocity[3];
+} aicb_eye;
+/* What the world camera takes from GraphicsOptions and the Viewport, shared by a batch, 48 bytes.  fov_y_degrees and
+ * view_distance are repaired as aicb_camera_from_view repairs them.  The exposure rule (set_measured_exposure,
+ * camera_struct.rs:169-181): automatic_exposure == 0 is ExposureOption::Fixed(fixed_exposure); lighting_display is an
+ * AICB_LIGHT_* value. */
+typedef struct aicb_eye_view_params {
+    double fov_y_degrees;
+    double view_distance;
+    double nominal_width;
+    double nominal_height;
+    uint32_t fb_width, fb_height;
+    float fixed_exposure;
+    uint8_t automatic_exposure;
+    uint8_t lighting_display;
+    uint8_t _pad[2];
+} aicb_eye_view_params;
+/* aicb_eye_views_device status: the projection-view matrix has no inverse (the reference panics,
+ * camera_struct.rs:416); nothing else of that eye is written. */
+#define AICB_EYE_NOT_INVERTIBLE 1u
+/* Body::look_rotation (physics/body.rs:285-292): around_x(-pitch in radians).then(around_y(-yaw in radians)), with
+ * glibc's sin and cos, as (i, j, k, r).  Host only. */
+void aicb_look_rotation(double yaw_degrees, double pitch_degrees, double out_ijkr[4]);
+/* step_eye_position for one stepped tick, eye i against body i, in place: the displacement spring moves by the
+ * change of the body's velocity since previous_body_velocity, in uncontracted f64, with 1e21^dt and 1e-9^dt computed
+ * once by the host's pow; then previous_body_velocity = the body's velocity.  A paused tick is no step: do not call
+ * it then.  dt: finite and in (0, 1], as aicb_step_bodies takes it.  Eyes and bodies (8-byte aligned) are device
+ * memory of the scene's device; the call is issued on `stream` (NULL: the context's) with the device calls' ordering
+ * (aicb_cursor_raycast_device) and does not synchronise.  AICB_ERR_INVALID with nothing issued: NULL eyes or bodies
+ * with n > 0, a pointer that is not the scene's device memory or is misaligned, or a dt out of range. */
+aicb_status aicb_step_eyes_device(aicb_scene *, aicb_eye *d_eyes, const aicb_body *d_bodies, size_t n, double dt,
+                                  void *stream);
+/* compute_view_transform and the world camera's update for eye i, every tick (paused or not), after the exposure
+ * step.  Rotation i is d_rotations[i] (i, j, k, r); the translation is body i's position + eye i's displacement.
+ * Writes, for each output that is not NULL:
+ *   eye_to_world[i]: aicb_view_transform_matrix of {rotation, translation}, the matrix the next tick's
+ *     aicb_step_exposure_device takes (a fresh eye's all-zero matrix leaves its first exposure step a no-op, as
+ *     view_transform: None does);
+ *   cameras[i]: the whole record, inverse_projection_view as aicb_camera_from_view gives it for the same rotation,
+ *     translation and params, fb_width and fb_height from params, _pad 0, and the exposure of set_measured_exposure:
+ *     under Fixed the fixed value; under automatic exposure d_exposures[i] (the aicb_step_exposure_device output)
+ *     when it is not NaN and not negative (-0 as +0), or 1 for it under AICB_LIGHT_NONE; an invalid measurement or
+ *     NULL d_exposures keeps the entry's exposure;
+ *   look_rays[i]: {origin xyz, direction xyz} of the new camera at the screen centre, aicb_camera_project_ndc at
+ *     (0, 0): with aicb_cursor_raycast_device and a distance of 6, what the character is looking at;
+ *   status[i]: 0, or AICB_EYE_NOT_INVERTIBLE with nothing else of the eye written.
+ * Rotations, eyes, bodies, matrices, cameras and rays are 8-byte aligned, exposures and statuses 4-byte aligned,
+ * device memory of the scene's device; the call is issued as aicb_step_eyes_device is.  AICB_ERR_INVALID with nothing
+ * issued: a NULL params, NULL eyes, bodies or rotations with n > 0, or a pointer the device calls reject. */
+aicb_status aicb_eye_views_device(aicb_scene *, const aicb_eye *d_eyes, const aicb_body *d_bodies,
+                                  const double (*d_rotations)[4], const float *d_exposures_or_null, size_t n,
+                                  const aicb_eye_view_params *params, double (*d_eye_to_world_or_null)[16],
+                                  aicb_camera *d_cameras_or_null, double (*d_look_rays_or_null)[6],
+                                  uint32_t *d_status_or_null, void *stream);
+/* The group forms run on device 0 with device 0's buffers, and their outputs are one context's bytes.  They do not
+ * synchronise either.  GPU test: tests/test_gpu_eyes.py. */
+aicb_status aicb_group_step_eyes_device(aicb_group_scene *, aicb_eye *d_eyes, const aicb_body *d_bodies, size_t n,
+                                        double dt, void *stream);
+aicb_status aicb_group_eye_views_device(aicb_group_scene *, const aicb_eye *d_eyes, const aicb_body *d_bodies,
+                                        const double (*d_rotations)[4], const float *d_exposures_or_null, size_t n,
+                                        const aicb_eye_view_params *params, double (*d_eye_to_world_or_null)[16],
+                                        aicb_camera *d_cameras_or_null, double (*d_look_rays_or_null)[6],
+                                        uint32_t *d_status_or_null, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Light propagation (secondary path): replaces Mutation::set x n + evaluate_light(epsilon)
